@@ -299,6 +299,14 @@ struct NumTab {
 __device__ __forceinline__ double num_of(const NumTab& nt, u32 id) { return id < nt.n_ids ? __ldg(nt.num_or0 + id) : 0.0; }
 __device__ __forceinline__ bool isnum_of(const NumTab& nt, u32 id) { return id < nt.n_ids ? __ldg(nt.is_num + id) != 0 : false; }
 
+// Seed of an aggregate accumulator: the identity of its fold, so that a slot no row (or only some rows) reached gives what folding
+// the group's rows from its first value gives (execute_query.rs:1198-1201). MIN / MAX: a quiet NaN — fmin / fmax and
+// atomic_min_f64 / atomic_max_f64 replace it by any non-NaN value, and a group whose values are all NaN stays NaN (f64::min(NaN, NaN)).
+// SUM / AVG: -0.0, the only identity of IEEE addition (+0.0 + -0.0 = +0.0 would turn an all-(-0.0) group positive).
+__device__ __forceinline__ double agg_identity(u32 kind) {
+    return (kind == KB_AGG_MIN || kind == KB_AGG_MAX) ? __longlong_as_double(0x7FF8000000000000ll) : -0.0;
+}
+
 __device__ __forceinline__ bool cmp_num(u32 cmp, double a, double b) {
     switch (cmp) {  // types.rs:133-148 — only the four ordering operators reach the numeric path
         case KB_CMP_GT: return a > b;

@@ -1291,7 +1291,7 @@ __global__ void __launch_bounds__(PROBEF_THREADS, KB_PI_MINB) probe_index_kernel
         for (int i = tid; i < PI_GROUP_SMEM; i += PROBEF_THREADS) {
             a_key[i] = EMPTY32;
             a_cnt[i] = 0u;
-            a_val[i] = P.akind == KB_AGG_MIN ? CUDART_INF : (P.akind == KB_AGG_MAX ? -CUDART_INF : 0.0);
+            a_val[i] = agg_identity(P.akind);
         }
     }
     __shared__ u32 s_tcnt[2];  // rows in the staged tile
@@ -2341,8 +2341,7 @@ __global__ void group_init_kernel(const GroupParams P) {
     for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < P.n_slots; i += stride) {
         P.gstate[i] = 0u;
         P.gcnt[i] = 0ull;
-        for (u32 a = 0; a < P.n_aggs; a++)
-            P.gval[(u64)i * 8 + a] = P.akind[a] == KB_AGG_MIN ? CUDART_INF : (P.akind[a] == KB_AGG_MAX ? -CUDART_INF : 0.0);
+        for (u32 a = 0; a < P.n_aggs; a++) P.gval[(u64)i * 8 + a] = agg_identity(P.akind[a]);
     }
 }
 void launch_group_init(const GroupParams& p, cudaStream_t st) {
@@ -2497,7 +2496,7 @@ __global__ void __launch_bounds__(256) group_kernel(const __grid_constant__ Grou
     for (int i = threadIdx.x; i < GROUP_SMEM; i += blockDim.x) {
         sstate[i] = 0u;
         scnt[i] = 0ull;
-        for (u32 a = 0; a < 8; a++) sval[i][a] = (a < P.n_aggs && P.akind[a] == KB_AGG_MIN) ? CUDART_INF : ((a < P.n_aggs && P.akind[a] == KB_AGG_MAX) ? -CUDART_INF : 0.0);
+        for (u32 a = 0; a < 8; a++) sval[i][a] = agg_identity(a < P.n_aggs ? P.akind[a] : (u32)KB_AGG_COUNT);
     }
     __syncthreads();
     const int lane = threadIdx.x & 31;
@@ -2514,7 +2513,10 @@ __global__ void __launch_bounds__(256) group_kernel(const __grid_constant__ Grou
         unsigned peers = __match_any_sync(act, h);
         int leader = __ffs(peers) - 1;
         bool same = true;
-        for (u32 c = 0; c < P.n_gcols; c++) same = same && (__shfl_sync(peers, k[c], leader) == k[c]);
+        for (u32 c = 0; c < P.n_gcols; c++) {  // every lane of `peers` must reach every shuffle: no short-circuit around it
+            const u32 lk = __shfl_sync(peers, k[c], leader);
+            same = same && lk == k[c];
+        }
         const unsigned agree = __ballot_sync(act, same);
         peers = same ? (peers & agree) : (1u << lane);  // rare hash collision inside a warp: the odd lanes go alone
         leader = __ffs(peers) - 1;
@@ -2586,7 +2588,7 @@ __global__ void __launch_bounds__(256) group1_kernel(const __grid_constant__ Gro
     for (int i = threadIdx.x; i < GROUP_SMEM; i += blockDim.x) {
         sk[i] = EMPTY32;
         scnt[i] = 0u;
-        sval[i] = AGG == KB_AGG_MIN ? CUDART_INF : (AGG == KB_AGG_MAX ? -CUDART_INF : 0.0);
+        sval[i] = agg_identity((u32)AGG);
     }
     __syncthreads();
     const int lane = threadIdx.x & 31;

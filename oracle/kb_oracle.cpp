@@ -620,8 +620,8 @@ Groups group_aggregate(const Rel& in, const NumTable& nt, const u32* gslots, u32
             if (fresh) { acc = v; continue; }                          // :1198-1201 first row initialises
             switch (aggs[i].kind) {
                 case KB_AGG_SUM: case KB_AGG_AVG: acc += v; break;
-                case KB_AGG_MIN: acc = std::min(acc, v); break;        // f64::min
-                case KB_AGG_MAX: acc = std::max(acc, v); break;
+                case KB_AGG_MIN: acc = std::fmin(acc, v); break;       // f64::min: a NaN operand is ignored
+                case KB_AGG_MAX: acc = std::fmax(acc, v); break;       // f64::max
                 default: break;
             }
         }

@@ -12,16 +12,17 @@ from tests import helpers as H
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRC = os.path.join(ROOT, "tests", "cpp", "host_only.cpp")
-BIN = os.path.join(ROOT, "tests", "cpp", "host_only")
 LIBDIR = os.path.join(ROOT, "kolibrie_b200")
 
 
-def run(strings):
-    cmd = ["/usr/bin/g++", "-std=c++17", "-O1", "-Wall", "-o", BIN, SRC, f"-L{LIBDIR}", "-lkolibrie_b200", f"-Wl,-rpath,{LIBDIR}"]
+def run(strings, out_dir):
+    """builds the host-only program into out_dir (the repository tree may be read-only) and feeds it `strings`"""
+    exe = os.path.join(str(out_dir), "host_only")
+    cmd = ["/usr/bin/g++", "-std=c++17", "-O1", "-Wall", "-o", exe, SRC, f"-L{LIBDIR}", "-lkolibrie_b200", f"-Wl,-rpath,{LIBDIR}"]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     assert r.returncode == 0, r.stdout
     inp = "".join(s.encode("utf-8").hex() + "\n" for s in strings)
-    r = subprocess.run([BIN], input=inp, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=120)
+    r = subprocess.run([exe], input=inp, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=120)
     assert r.returncode == 0, r.stdout
     lines = r.stdout.splitlines()
     progs = [tuple(x.split()[1:]) for x in lines if x.startswith("F ")]
@@ -39,14 +40,14 @@ def same(a, b):
     return (math.isnan(a) and math.isnan(b)) or a == b
 
 
-def test_cpp_mirror_parses_f64_like_rust_and_like_the_python_mirror():
+def test_cpp_mirror_parses_f64_like_rust_and_like_the_python_mirror(tmp_path):
     table = H.load("rust_parse_f64.json")
     rng = np.random.default_rng(12)
     alphabet = list("0123456789+-.eEinfINFatyN x_\n\t") + ["١", "é"]
     fuzz = ["".join(rng.choice(alphabet, size=int(rng.integers(0, 9)))) for _ in range(4000)]
     fuzz = [s for s in fuzz if "\x00" not in s]
     strings = list(table["accept"]) + list(table["reject"]) + fuzz
-    parsed, ids, n_ids, n_num, progs = run(strings)
+    parsed, ids, n_ids, n_num, progs = run(strings, tmp_path)
     for s, v in zip(strings[: len(table["accept"])], parsed):
         assert v is not None, f"C++ mirror rejects {s!r}, Rust accepts it"
     for s, v in zip(table["reject"], parsed[len(table["accept"]):]):

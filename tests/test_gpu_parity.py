@@ -8,6 +8,7 @@ import pytest
 from kolibrie_b200 import capi as c
 from kolibrie_b200 import datagen
 from kolibrie_b200.engine import Dictionary
+from tests import agg_reference as AR
 from tests import helpers as H
 from tests import oracle_api as O
 
@@ -288,9 +289,8 @@ def test_group_aggregate_vs_oracle(ctx, emp):
         gk, gc, gv = table(g)
         wk, wc, wv = table(w)
         assert np.array_equal(gk, wk) and np.array_equal(gc, wc)
-        for a, b in zip(gv, wv):
-            # salaries are integers: sums stay exact in f64 (< 2^53), so equality is exact; AVG within 1 ulp-ish
-            assert np.allclose(a, b, rtol=1e-12, atol=0)
+        sl = sorted(orel.slots)
+        AR.assert_groups_match_slots(g, orel.to_numpy(sl), sl, d.num_or0, gslots, aggs, f"{gslots} {aggs}")
 
 
 def test_star_join_aggregate_fused_vs_oracle(ctx, emp):
@@ -314,8 +314,8 @@ def test_star_join_aggregate_fused_vs_oracle(ctx, emp):
         wk, wc, wv = table(w)
         assert n_rows == len(orel.to_numpy(sorted(orel.slots))), what
         assert np.array_equal(gk, wk) and np.array_equal(gc, wc), what
-        for a, b in zip(gv, wv):
-            assert np.allclose(a, b, rtol=1e-12, atol=0), what
+        sl = sorted(orel.slots)
+        AR.assert_groups_match_slots(g, orel.to_numpy(sl), sl, d.num_or0, gslots, aggs, what)
 
     one = [[(c.AGG_COUNT, 0)], [(c.AGG_SUM, 2)], [(c.AGG_MIN, 2)], [(c.AGG_MAX, 2)], [(c.AGG_AVG, 2)], []]
     for indexed in (True, False):

@@ -5,6 +5,7 @@ import pytest
 
 from kolibrie_b200 import capi as c
 from kolibrie_b200 import datagen
+from tests import agg_reference as AR
 from tests import helpers as H
 from tests import oracle_api as O
 
@@ -69,15 +70,16 @@ def test_prepared_group_by_equals_oracle(ctx, emp):
         assert plan.grouped
         orel = db.bgp(pp, ff)
         w = db.group(orel, [gslot], aggs)
+        osl = sorted(orel.slots)
+        orows = orel.to_numpy(osl)
         for rep in range(3):
             t = plan.submit()
             g, n_rows = plan.collect_groups(t)
             assert n_rows == orel.n_rows
-            gk, gc, gv = table(g)
-            wk, wc, wv = table(w)
+            gk, gc, _ = table(g)
+            wk, wc, _ = table(w)
             assert np.array_equal(gk, wk) and np.array_equal(gc, wc)
-            for a, b in zip(gv, wv):
-                assert np.allclose(a, b, rtol=1e-12, atol=0)
+            AR.assert_groups_match_slots(g, orows, osl, d.num_or0, [gslot], aggs, f"{aggs} rep {rep}")
         plan.free()
     # a GROUP BY with thousands of groups does not fit the plan's fixed table: reported at collect, not silently truncated
     plan = ctx.prepare_star_join(js, pats, None, group_slots=[2], aggs=[(c.AGG_COUNT, 0)], ring=1)
@@ -142,14 +144,15 @@ def test_groups_merge_of_shard_partials_equals_global_group_by(ctx, n_parts):
             if i == 0:
                 rows += n_rows
     assert rows == orel.n_rows
+    osl = sorted(orel.slots)
+    orows = orel.to_numpy(osl)
     for i, (gs, aggs) in enumerate(cases):
         g = ctx.groups_merge(parts[i])
         w = db.group(orel, gs, aggs)
-        gk, gc, gv = table(g)
-        wk, wc, wv = table(w)
+        gk, gc, _ = table(g)
+        wk, wc, _ = table(w)
         assert np.array_equal(gk, wk) and np.array_equal(gc, wc), (gs, aggs)
-        for a, b in zip(gv, wv):
-            assert np.allclose(a, b, rtol=1e-12, atol=0), (gs, aggs)
+        AR.assert_groups_match_slots(g, orows, osl, d.num_or0, gs, aggs, f"{gs} {aggs}")
     # merging a single partial is the identity; garbage is rejected
     g1 = ctx.groups_merge([parts[0][0]])
     assert int(g1["counts"].sum()) > 0
@@ -225,6 +228,8 @@ def test_peer_merged_group_plan_world_of_one(ctx):
     db = O.Db(d.s, d.p, d.o, d.num_or0, d.is_num)
     js, pats, _ = datagen.employee_queries(d)["cfg3"]
     orel = db.bgp(pats)
+    osl = sorted(orel.slots)
+    orows = orel.to_numpy(osl)
     ctx.store_load(d.s, d.p, d.o)
     ctx.dict_numeric_load(d.num_or0, d.is_num)
     ctx.build_index()
@@ -237,17 +242,16 @@ def test_peer_merged_group_plan_world_of_one(ctx):
         torch.cuda.synchronize()
         plan.attach_peers(0, 1, [scratch.data_ptr()], keep=scratch)
         w = db.group(orel, [1], aggs)
-        wk, wc, wv = table(w)
+        wk, wc, _ = table(w)
         tickets = []
         for rep in range(5):  # more queries than ring slots: the slots and the barrier epochs are reused
             tickets.append(plan.submit())
             if len(tickets) == 2:
                 g, n_rows = plan.collect_groups(tickets.pop(0))
                 assert n_rows == orel.n_rows
-                gk, gc, gv = table(g)
+                gk, gc, _ = table(g)
                 assert np.array_equal(gk, wk) and np.array_equal(gc, wc), (aggs, rep)
-                for a, b in zip(gv, wv):
-                    assert np.allclose(a, b, rtol=1e-12, atol=0), (aggs, rep)
+                AR.assert_groups_match_slots(g, orows, osl, d.num_or0, [1], aggs, f"{aggs} rep {rep}")
         plan.collect_groups(tickets.pop(0))
         plan.free()
     # a row plan has nothing to merge; a ring of one cannot be attached
