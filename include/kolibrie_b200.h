@@ -332,6 +332,46 @@ KB_API kb_status kb_datalog_fixpoint(kb_ctx* ctx, const kb_rule* rules, uint32_t
 KB_API kb_status kb_datalog_fixpoint_seed(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rules, uint32_t strategy, const kb_rel* seed,
                                           kb_rel** out, uint64_t* n_seed_new, kb_fixpoint_stats* stats);
 
+/* Sliding-window maintenance of the closure by delete-and-rederive: what a window firing with rules reaches by evicting the previous
+ * window, adding the current one and materialising from scratch (rsp_engine.rs:94-109, simple_r2r.rs:103-128), reached from the slide.
+ *   B  = the distinct triples of every segment whose tag is not KB_TAG_INFERRED, I = the triples of the KB_TAG_INFERRED segments,
+ *   B' = the segments left after the `evict_tags` segments are dropped, plus `add` (all taken as sets).
+ * Precondition: I = closure(B) \ B under the same rules and closure semantics. The context records a "closed" token (store version,
+ * numeric-table version, the rules byte for byte, a hash-join strategy) when kb_datalog_fixpoint (on a store without inferred segments,
+ * strategy other than KB_SEMI_NAIVE_PARALLEL) or kb_datalog_maintain returns KB_OK; any other store mutation, other rules or
+ * kb_datalog_fixpoint_seed (its seed facts are stored as KB_TAG_INFERRED) void it -> KB_E_INVALID ("store not closed under these
+ * rules: run kb_datalog_fixpoint"). kb_dict_numeric_load voids it only when a rule filter compares numbers (a constant right-hand side,
+ * or a variable no premise binds): other rules have the same closure whatever the numeric table holds.
+ * Postcondition: the evicted segments are gone; `add` (nullable; 3 columns, slots 0,1,2 = s,p,o) is ONE new segment tagged add_tag,
+ * stored as kb_store_append_device stores it; the KB_TAG_INFERRED segments are replaced by one segment holding closure(B') \ B', each
+ * fact once (none when that set is empty; an unchanged single segment is kept). *inferred_removed = I \ I', *inferred_added = I' \ I
+ * (nullable; 3 columns, every fact once). A base fact that is still derivable after it left the base moves into I'; a fact of `add` that
+ * was inferred moves to the base; a fact that an evicted segment and a surviving segment (or `add`) both hold does not move.
+ * KB_SEMI_NAIVE, KB_SEMI_NAIVE_OLD_DELTA and KB_NAIVE share one closure (hash-join premises, quirks Q6/Q7); KB_SEMI_NAIVE_PARALLEL ->
+ * KB_E_UNSUPPORTED; rule shapes kb_datalog_fixpoint refuses are refused. n_evict = 0 and add = NULL: no-op, empty outputs.
+ * Errors before anything changes (the store is untouched): unknown tag -> KB_E_NOT_FOUND; KB_TAG_INFERRED in evict_tags or as add_tag,
+ * a bad `add`, a stale token -> KB_E_INVALID. A CUDA / out-of-memory error while the result is computed leaves the store as it was
+ * (still closed); one while the store is rewritten leaves exactly the B' segments, no inferred segment and no token: run
+ * kb_datalog_fixpoint to restore the precondition. A valid store index stays valid (maintained in place, as by kb_store_evict /
+ * kb_store_append_device). The base counts (base_removed, base_added) cover the predicates the rules mention: the facts of other
+ * predicates take no part in the closure. */
+typedef struct kb_maintain_stats {
+    uint64_t base_removed;      /* distinct facts that left the base set */
+    uint64_t base_added;        /* distinct facts of `add` that were not base facts before the call */
+    uint64_t overdeleted;       /* facts removed by the over-deletion phase, not counting the base_removed facts themselves */
+    uint64_t rederived;         /* over-deleted or removed facts that the rederivation phase found still derivable */
+    uint64_t inferred_removed;  /* rows of *inferred_removed */
+    uint64_t inferred_added;    /* rows of *inferred_added */
+    uint64_t derivations;       /* candidate head instances over all phases (compare kb_fixpoint_stats.derivations of a closure from scratch) */
+    uint32_t overdelete_rounds, insert_rounds;
+    double device_ms;
+} kb_maintain_stats;
+KB_API kb_status kb_datalog_maintain(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rules, uint32_t strategy,
+                                     const uint64_t* evict_tags, uint32_t n_evict,
+                                     const kb_rel* add /* nullable; 3 columns, slots 0,1,2 = s,p,o */, uint64_t add_tag,
+                                     kb_rel** inferred_removed /* nullable */, kb_rel** inferred_added /* nullable */,
+                                     kb_maintain_stats* stats /* nullable */);
+
 /* ------------------------------------------------------------------ multi-GPU helpers (one process per GPU; the host layer
  * runs the NCCL all-to-all between kb_partition and kb_rel_from_device) */
 /* Shard function (host and device agree): block-cyclic on the dictionary id, (key >> KB_SHARD_BLOCK_BITS) % n_shards. Dictionary ids

@@ -66,6 +66,12 @@ class KbFixpointStats(C.Structure):
     _fields_ = [("rounds", C.c_uint32), ("inferred", C.c_uint64), ("derivations", C.c_uint64), ("round_new", C.c_uint64 * 64), ("device_ms", C.c_double)]
 
 
+class KbMaintainStats(C.Structure):
+    """kb_maintain_stats: what one kb_datalog_maintain call moved"""
+    _fields_ = [(n, C.c_uint64) for n in ("base_removed", "base_added", "overdeleted", "rederived", "inferred_removed", "inferred_added", "derivations")] + [
+        ("overdelete_rounds", C.c_uint32), ("insert_rounds", C.c_uint32), ("device_ms", C.c_double)]
+
+
 class KbStats(C.Structure):
     _fields_ = [(n, C.c_double) for n in ("scan_ms", "build_ms", "probe_ms", "filter_ms", "group_ms", "other_ms", "total_ms")] + [
         (n, C.c_uint64)
@@ -200,6 +206,7 @@ def lib() -> C.CDLL:
         "kb_star_join_aggregate": (i32, [vp, u32, P(KbPattern), u32, P(KbFilterOp), u32, P(u32), u32, P(KbAgg), u32, P(vp), P(u64)]),
         "kb_datalog_fixpoint": (i32, [vp, P(KbRule), u32, u32, P(vp), P(KbFixpointStats)]),
         "kb_datalog_fixpoint_seed": (i32, [vp, P(KbRule), u32, u32, vp, P(vp), P(u64), P(KbFixpointStats)]),
+        "kb_datalog_maintain": (i32, [vp, P(KbRule), u32, u32, P(u64), u32, vp, u64, P(vp), P(vp), P(KbMaintainStats)]),
         "kb_shard_of": (u32, [u32, u32]),
         "kb_set_sharding": (i32, [vp, u32, u32]),
         "kb_partition": (i32, [vp, vp, u32, u32, P(vp), P(u64)]),
@@ -230,7 +237,7 @@ EXPORTED_SYMBOLS = [
     "kb_rel_from_device", "kb_rel_free", "kb_scan", "kb_filter", "kb_project", "kb_hash_join", "kb_bind_join", "kb_star_join", "kb_bgp_execute",
     "kb_group_aggregate", "kb_groups_info", "kb_groups_keys", "kb_groups_values", "kb_groups_counts", "kb_groups_free", "kb_groups_pack", "kb_groups_merge", "kb_star_join_aggregate",
     "kb_star_join_prepare", "kb_plan_submit", "kb_plan_collect", "kb_plan_info", "kb_plan_free", "kb_plan_peer_scratch_bytes", "kb_plan_attach_peers",
-    "kb_datalog_fixpoint", "kb_datalog_fixpoint_seed", "kb_shard_of", "kb_set_sharding", "kb_partition", "kb_partition_counts", "kb_segment_write", "kb_segment_info", "kb_segment_save", "kb_store_append_file", "kb_shuffle_scatter", "kb_shuffle_push", "kb_rel_wrap_device", "kb_star_join_host", "kb_star_join_host_into", "perform_hash_join_cuda",
+    "kb_datalog_fixpoint", "kb_datalog_fixpoint_seed", "kb_datalog_maintain", "kb_shard_of", "kb_set_sharding", "kb_partition", "kb_partition_counts", "kb_segment_write", "kb_segment_info", "kb_segment_save", "kb_store_append_file", "kb_shuffle_scatter", "kb_shuffle_push", "kb_rel_wrap_device", "kb_star_join_host", "kb_star_join_host_into", "perform_hash_join_cuda",
 ]
 
 
@@ -625,6 +632,24 @@ class Context:
         st = KbFixpointStats()
         self._check(lib().kb_datalog_fixpoint_seed(self.h, arr, len(rules), strategy, seed.h, C.byref(out), C.byref(n_new), C.byref(st)))
         return Relation(self, out), int(n_new.value), st
+
+    def datalog_maintain(self, rules: Sequence[dict], evict_tags: Sequence[int] = (), add=None, add_tag: int = 0, strategy: int = SEMI_NAIVE):
+        """kb_datalog_maintain: the store is closed under `rules` (an earlier datalog_fixpoint or datalog_maintain with the same rules and
+        nothing changed since); the segments tagged `evict_tags` leave, `add` (a Relation with slots 0,1,2 = s,p,o, or an (n,3) uint32
+        array; None: nothing added) becomes one segment tagged `add_tag`, and the inferred segment becomes the closure of the new base.
+        Returns (inferred_removed, inferred_added, stats): the inferred facts that left and the ones that arrived (3-column relations)."""
+        arr, keep = make_rules(rules)
+        tags = (C.c_uint64 * max(len(evict_tags), 1))(*[int(t) for t in evict_tags])
+        if add is not None and not isinstance(add, Relation):
+            a = np.asarray(add, dtype=np.uint32)
+            if a.ndim != 2:
+                raise ValueError("add must be an (n, 3) array of (s, p, o)")
+            add = self.rel_from_host(list(range(a.shape[1])), [a[:, j] for j in range(a.shape[1])])
+        rem, new = C.c_void_p(), C.c_void_p()
+        st = KbMaintainStats()
+        self._check(lib().kb_datalog_maintain(self.h, arr, len(rules), strategy, tags, len(evict_tags), add.h if add is not None else None, add_tag,
+                                              C.byref(rem), C.byref(new), C.byref(st)))
+        return Relation(self, rem), Relation(self, new), st
 
     def partition(self, rel: Relation, key_slot: int, n_parts: int):
         out = C.c_void_p()

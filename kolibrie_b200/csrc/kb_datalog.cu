@@ -9,10 +9,14 @@
 // known_facts (infer_generic.rs:30) is a device hash set of 96-bit (s,p,o) keys; a derived fact is new iff its insert wins.
 // Round structure is the reference's: every rule of a round sees the same snapshot; new facts become visible (and become the
 // next delta) only after the round (infer_generic.rs:42-48) — so round counts and per-round fact counts match the oracle.
+//
+// kb_datalog_maintain keeps a closed store closed across a window slide by delete-and-rederive (DRed) over the same per-predicate
+// relations and known-fact sets, kept in the context between calls, plus a base multiplicity table per predicate (see maintain_impl).
 #include <algorithm>
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
+#include <functional>
 
 #include "kb_internal.hpp"
 
@@ -81,6 +85,28 @@ struct FixState {
     u64 version = 0;  // ctx->store_version the state belongs to
     std::map<u32, PredRel> rels;
 };
+
+// base multiplicity of one predicate's facts: how many live base segments hold each (s,o) (kb_datalog_maintain)
+struct BaseCount {
+    Buf keys, cnt;     // 64-bit (s,o) keys, u32 count per slot
+    u32 slots = 0;
+    u64 occupied = 0;  // keys that hold a slot (a key whose count fell to 0 keeps its slot until the next rehash)
+    u64 live = 0;      // keys with a positive count: the distinct base facts of the predicate
+};
+
+// The "closed" token: kb_datalog_fixpoint (hash-join strategies, on a store without inferred segments) or kb_datalog_maintain returned
+// OK, so the store holds closure(B) \ B as its KB_TAG_INFERRED segments, for these rules, at these store / numeric-table versions.
+// kb_datalog_maintain also leaves its working state here: the per-predicate relations of B ∪ I with their known-fact sets and the base
+// multiplicities, so that the next slide reads nothing but its own delta. KOLIBRIE_FIX_STATE=0: that state is rebuilt from the store.
+struct Closed {
+    std::string sig;
+    u64 store_version = 0, num_version = 0;
+    bool numeric = false;  // a rule filter compares numbers: the closure depends on the numeric side table (num_version counts)
+    bool has_state = false;
+    std::map<u32, PredRel> rels;
+    std::map<u32, BaseCount> base;
+};
+
 std::string rules_signature(const kb_rule* rules, u32 n_rules) {
     std::string s;
     auto put = [&](const void* p, size_t n) { s.append(static_cast<const char*>(p), n); };
@@ -104,6 +130,28 @@ std::string rules_signature(const kb_rule* rules, u32 n_rules) {
     return s;
 }
 
+// whether the closure reads the numeric side table: a rule filter that takes the numeric branch of evaluate_filters (rules.rs:148-160) —
+// a constant right-hand side, or a variable no premise binds. Rules without one have the same closure whatever kb_dict_numeric_load holds.
+bool rules_read_numbers(const kb_rule* rules, u32 n_rules) {
+    for (u32 r = 0; r < n_rules; r++) {
+        const kb_rule& k = rules[r];
+        for (u32 f = 0; f < k.n_filters; f++) {
+            const kb_rule_filter& fl = k.filters[f];
+            if (fl.cmp == 0) continue;
+            if (!fl.rhs_is_var) return true;
+            bool bound = false;
+            for (u32 i = 0; i < k.n_premise; i++) {
+                const kb_pattern& p = k.premise[i];
+                if ((p.s.is_var && p.s.value == fl.rhs_slot) || (p.p.is_var && p.p.value == fl.rhs_slot) || (p.o.is_var && p.o.value == fl.rhs_slot)) bound = true;
+            }
+            if (!bound) return true;
+        }
+    }
+    return false;
+}
+
+bool state_disabled() { return getenv("KOLIBRIE_FIX_STATE") && getenv("KOLIBRIE_FIX_STATE")[0] == '0'; }  // (read per call: a test flips it)
+
 kb_status grow_rel(kb_ctx* ctx, PredRel& r, u64 need) {
     if (need <= r.cap) return KB_OK;
     u64 cap = std::max<u64>(need, r.cap * 2);
@@ -116,6 +164,16 @@ kb_status grow_rel(kb_ctx* ctx, PredRel& r, u64 need) {
         KB_CUDA(ctx, cudaMemcpyAsync(no.ptr, r.o.ptr, r.n * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
     }
     r.s = ns; r.o = no; r.cap = cap;
+    return KB_OK;
+}
+
+// append n rows (s,o) to a predicate relation
+kb_status append_rows(kb_ctx* ctx, PredRel& r, const u32* s, const u32* o, u64 n) {
+    if (!n) return KB_OK;
+    KB_TRY(grow_rel(ctx, r, r.n + n));
+    KB_CUDA(ctx, cudaMemcpyAsync(r.s.ptr + r.n, s, n * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
+    KB_CUDA(ctx, cudaMemcpyAsync(r.o.ptr + r.n, o, n * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
+    r.n += n;
     return KB_OK;
 }
 
@@ -196,36 +254,11 @@ kb_status enforce_constants(kb_ctx* ctx, const Premise& pr, std::unique_ptr<kb_r
     return KB_OK;
 }
 
-}  // namespace
-
-// `seed` == nullptr: kb_datalog_fixpoint (every fact of the store is the first delta). With a seed (kb_datalog_fixpoint_seed): the store
-// is taken as closed under the rules already, the seed facts the store does not hold yet are accepted into it and form the first delta.
-static kb_status fixpoint_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rules, uint32_t strategy, bool seeded, const kb_rel* seed,
-                               kb_rel** inferred, uint64_t* n_seed_new, kb_fixpoint_stats* stats) {
-    if (!ctx) return KB_E_INVALID;
-    int prev_dev = -1;
-    cudaGetDevice(&prev_dev);
-    cudaSetDevice(ctx->device);
-    struct Restore { int d; ~Restore() { if (d >= 0) cudaSetDevice(d); } } restore{prev_dev};
-    KB_TRY(begin_call(ctx));
-    if ((n_rules && !rules) || !inferred) return fail(ctx, KB_E_INVALID, "NULL argument");
-    if (strategy != KB_SEMI_NAIVE && strategy != KB_NAIVE && strategy != KB_SEMI_NAIVE_PARALLEL && strategy != KB_SEMI_NAIVE_OLD_DELTA)
-        return fail(ctx, KB_E_INVALID, "unknown strategy %u", strategy);
-    if (seeded && !seed) return fail(ctx, KB_E_INVALID, "NULL seed");
-    if (seed && (seed->pair || seed->cols.size() != 3 || seed->col_of(0) != 0 || seed->col_of(1) != 1 || seed->col_of(2) != 2))
-        return fail(ctx, KB_E_INVALID, "the seed must be a 3-column relation with slots 0,1,2 = s,p,o");
-    if (seed && seed->n >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "seed too large");
-    const bool old_delta = strategy == KB_SEMI_NAIVE_OLD_DELTA;
-    const bool strict = strategy == KB_SEMI_NAIVE_PARALLEL;
-    kb_fixpoint_stats st{};
-    ScopedEvent ev0, ev1;
-    cudaEventRecord(ev0, ctx->st);
-
-    // ---- compile the rules (host): variable slots, synthetic variables for constants in s/o (quirk Q6), safety checks
-    std::vector<RulePlan> plans(n_rules);
-    Fix fx;
-    Trace tr;
-    fx.ctx = ctx;
+// compile the rules (host): variable slots, synthetic variables for constants in s/o (quirk Q6), safety checks; every predicate a rule
+// mentions gets an entry in `rels` (is_head: it occurs in a conclusion)
+kb_status compile_rules(kb_ctx* ctx, const kb_rule* rules, u32 n_rules, std::vector<RulePlan>* plans_out, std::map<u32, PredRel>* rels) {
+    std::vector<RulePlan>& plans = *plans_out;
+    plans.assign(n_rules, RulePlan{});
     for (u32 r = 0; r < n_rules; r++) {
         const kb_rule& rule = rules[r];
         if (rule.n_premise > KB_MAX_PREMISES || rule.n_conclusion > KB_MAX_CONCLUSIONS || rule.n_filters > KB_MAX_RULE_FILTERS)
@@ -254,7 +287,7 @@ static kb_status fixpoint_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
             pr.o_is_const = !p.o.is_var; pr.o_const = p.o.value;
             if (pr.s_var == pr.o_var)
                 return fail(ctx, KB_E_UNSUPPORTED, "rule %u premise %u repeats one variable in subject and object", r, i);
-            if (pr.pred_const) { fx.rels[pr.pred].pred = pr.pred; bound.insert((u32)pr.s_var); bound.insert((u32)pr.o_var); }
+            if (pr.pred_const) { (*rels)[pr.pred].pred = pr.pred; bound.insert((u32)pr.s_var); bound.insert((u32)pr.o_var); }
             plans[r].prem.push_back(pr);
         }
         plans[r].n_vars = next;
@@ -265,18 +298,273 @@ static kb_status fixpoint_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
             const kb_term* ts[2] = {&h.s, &h.o};
             for (auto* t : ts) if (t->is_var && !bound.count(t->value))
                 return fail(ctx, KB_E_UNSUPPORTED, "rule %u: head variable (slot %u) is not bound by the premises (quirk Q8: the reference invents ml_output_placeholder terms / id 0)", r, t->value);
-            fx.rels[h.p.value].pred = h.p.value;
-            fx.rels[h.p.value].is_head = true;
+            (*rels)[h.p.value].pred = h.p.value;
+            (*rels)[h.p.value].is_head = true;
         }
         for (u32 f = 0; f < rule.n_filters; f++) {
             if (rule.filters[f].cmp > KB_CMP_NE) return fail(ctx, KB_E_INVALID, "rule %u filter %u: bad comparison", r, f);
         }
     }
+    return KB_OK;
+}
+
+// kb_datalog_maintain's acceptance test in front of the dedup (launch_derive, gated): the candidate must be a member of `must` and must
+// have no positive count in the `veto` table
+struct Gate {
+    const u64* must = nullptr;
+    u32 must_slots = 0;
+    const BaseCount* veto = nullptr;
+};
+
+// ---- one head of one rule over the joined bindings `cur`: filters + instantiate + dedup against the known facts of `fx` + append to
+// fx's pending facts (`rule_p` == nullptr: no rule filters — the seed facts of kb_datalog_fixpoint_seed take the same way in)
+kb_status derive_head(Fix& fx, const kb_rel* cur, const kb_pattern& h, const kb_rule* rule_p, bool strict, const Gate* gate, Trace& tr,
+                      u64* derivations) {
+    kb_ctx* ctx = fx.ctx;
+    DeriveParams D{};
+    for (size_t k = 0; k < cur->cols.size(); k++) D.bcol[k] = cur->cols[k].ptr;
+    D.n = (u32)cur->n;
+    auto term = [&](const kb_term& t) {
+        HeadTerm ht;
+        ht.is_var = t.is_var;
+        ht.value = t.is_var ? (u32)cur->col_of(t.value) : t.value;
+        return ht;
+    };
+    D.head_s = term(h.s);
+    D.head_o = term(h.o);
+    D.n_filt = 0;
+    for (u32 f = 0; f < (strict || !rule_p ? 0u : rule_p->n_filters); f++) {  // the parallel variant never evaluates the rule filters
+        const kb_rule_filter& rf = rule_p->filters[f];
+        const int lc = cur->col_of(rf.lhs_slot);
+        if (lc < 0 || rf.cmp == 0) continue;  // unbound lhs: the reference skips the filter (rules.rs:139)
+        RuleFilterDev d;
+        d.lhs_col = (u32)lc;
+        d.cmp = rf.cmp;
+        d.rhs_value = rf.rhs_value;
+        d.rhs_is_var = 0; d.rhs_col = 0;
+        if (rf.rhs_is_var) {
+            const int rc = cur->col_of(rf.rhs_slot);
+            if (rc >= 0) { d.rhs_is_var = 1; d.rhs_col = (u32)rc; }
+            // rhs names an unbound variable: the reference falls to the numeric branch with value.parse() (rules.rs:148-151)
+        }
+        D.filt[D.n_filt++] = d;
+    }
+    D.nt = numtab(ctx);
+    if (gate) {
+        D.gate_set = gate->must;
+        D.gate_slots = gate->must_slots;
+        if (gate->veto) {
+            D.veto_keys = static_cast<const u64*>(gate->veto->keys->p);
+            D.veto_cnt = static_cast<const u32*>(gate->veto->cnt->p);
+            D.veto_slots = gate->veto->slots;
+        }
+    }
+    PredRel& hr = fx.rels[h.p.value];
+    KB_TRY(ensure_set(fx, hr, cur->n));
+    tr.mark(ctx, "  ensure_set", hr.set_slots);
+    Pending pd;
+    pd.pred = h.p.value;
+    pd.count = 0;
+    KB_TRY(alloc_col(ctx, cur->n, &pd.s));
+    KB_TRY(alloc_col(ctx, cur->n, &pd.o));
+    const u32 coff = ctrl_alloc(ctx, 8);
+    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + coff, 0, 8 * sizeof(u32), ctx->st));
+    D.out_s = pd.s.ptr; D.out_o = pd.o.ptr;
+    D.out_cap = (u32)cur->n;
+    D.out_count = ctx->ctrl + coff;
+    D.overflow = ctx->ctrl + coff + 1;
+    D.n_deriv = reinterpret_cast<unsigned long long*>(ctx->ctrl + coff + 4);
+    const u64 count_before = hr.set_count;
+    for (;;) {
+        D.set = static_cast<u64*>(hr.set->p);
+        D.set_slots = hr.set_slots;
+        // the set may fill up to 3/4 before it has to grow (expected: 1/2)
+        D.budget = (u32)std::min<u64>((u64)hr.set_slots / 4 * 3 - count_before, 0xFFFFFFFFull);
+        // Large candidate sets against a table far beyond L2: radix-partition the candidates by the high bits of their
+        // home slot and probe partition by partition (each slice stays L2-resident) instead of one random DRAM line per
+        // candidate. Partitions: ~32 MB slices, at least ~1 M candidates each (so that the CTAs of the probe pass sit on
+        // one or two slices at a time), at most 1024. (A gated launch always takes the direct path.)
+        u64 n_parts = 0;
+        {
+            const u64 set_bytes = (u64)hr.set_slots * sizeof(u64);
+            u64 want = std::min<u64>(set_bytes / ctx->derive_slice_bytes, std::min<u64>(cur->n / ctx->derive_min_part_rows, 1024));
+            while (want >= 2 && n_parts * 2 <= want) n_parts = n_parts ? n_parts * 2 : 2;  // power of two
+            if (ctx->derive_part == 0 || gate) n_parts = 0;
+        }
+        if (n_parts >= 2) {
+            DerivePartParams Q{};
+            Q.d = D;
+            Q.n_parts = (u32)n_parts;
+            u32 set_bits = 0;
+            while ((1ull << set_bits) < hr.set_slots) set_bits++;
+            u32 part_bits = 0;
+            while ((1ull << part_bits) < n_parts) part_bits++;
+            Q.slice_bits = set_bits - part_bits;
+            Q.bucket_cap = (u32)std::min<u64>(cur->n / n_parts + cur->n / n_parts / 8 + ctx->derive_bucket_slack, 0xFFFFFFF0ull);
+            Buf ctl;
+            const size_t bucket_bytes = n_parts * (u64)Q.bucket_cap * sizeof(u64);
+            if (!fx.buckets || fx.buckets->bytes < bucket_bytes) {
+                fx.buckets.reset();
+                KB_TRY(alloc_buf(ctx, bucket_bytes + bucket_bytes / 4, &fx.buckets));
+            }
+            Buf buckets = fx.buckets;
+            KB_TRY(alloc_buf(ctx, (2 * n_parts + 8) * sizeof(u32), &ctl));
+            KB_CUDA(ctx, cudaMemsetAsync(ctl->p, 0, (2 * n_parts + 8) * sizeof(u32), ctx->st));
+            Q.buckets = static_cast<u64*>(buckets->p);
+            Q.cursors = static_cast<u32*>(ctl->p);
+            Q.tile_start = Q.cursors + n_parts;
+            Q.tickets = Q.tile_start + n_parts + 1 + ((n_parts + 1) & 1u);
+            tr.mark(ctx, "    derive: buckets allocated", n_parts);
+            timer_begin(ctx, F_OTHER, 3);
+            launch_derive_partitioned(Q, ctx->n_sms, ctx->st);
+            timer_end(ctx);
+            ctx->stats.rows_built += cur->n;  // (counted as table traffic: partitioned candidates)
+        } else {
+            timer_begin(ctx, F_OTHER);
+            launch_derive(D, ctx->n_sms, ctx->st);
+            timer_end(ctx);
+        }
+        KB_CUDA(ctx, cudaGetLastError());
+        // counts are read immediately: the control arena may be recycled by later joins of this round
+        KB_TRY(ctrl_read(ctx));
+        pd.count = ctx->h_ctrl[coff];
+        if (ctx->h_ctrl[coff + 1] == 1u) return fail(ctx, KB_E_LIMIT, "known-fact set overflow");
+        if (ctx->h_ctrl[coff + 1] == 0u) break;
+        // budget reached: rebuild the set larger WITH the facts appended so far, then repeat the launch (facts already
+        // inserted are found present and are not appended twice; the derivation count is the last, complete pass's)
+        fx.pend.push_back(pd);
+        const kb_status gs = ensure_set(fx, hr, cur->n, true);
+        fx.pend.pop_back();
+        if (gs != KB_OK) return gs;
+        KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + coff + 1, 0, sizeof(u32), ctx->st));
+        KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + coff + 4, 0, 2 * sizeof(u32), ctx->st));
+    }
+    unsigned long long nd;
+    memcpy(&nd, ctx->h_ctrl + coff + 4, sizeof nd);
+    *derivations += nd;
+    hr.set_count = count_before;
+    hr.set_count += pd.count;
+    if (pd.count) fx.pend.push_back(pd);
+    tr.mark(ctx, "  derive", pd.count);
+    return KB_OK;
+}
+
+// end of a round: the pending facts become visible (appended to their relations); returns how many there were
+kb_status flush_pending(Fix& fx, u64* appended) {
+    *appended = 0;
+    for (auto& pd : fx.pend) {
+        KB_TRY(append_rows(fx.ctx, fx.rels[pd.pred], pd.s.ptr, pd.o.ptr, pd.count));
+        *appended += pd.count;
+    }
+    fx.pend.clear();
+    return KB_OK;
+}
+
+// ---- rounds: from the current delta of every relation ([delta_start, n)) to the fixpoint
+kb_status run_rounds(Fix& fx, const kb_rule* rules, u32 n_rules, const std::vector<RulePlan>& plans, u32 strategy, kb_fixpoint_stats& st,
+                     Trace& tr) {
+    kb_ctx* ctx = fx.ctx;
+    const bool old_delta = strategy == KB_SEMI_NAIVE_OLD_DELTA;
+    const bool strict = strategy == KB_SEMI_NAIVE_PARALLEL;
+    for (u32 round = 0;; round++) {
+        for (auto& kv : fx.rels) kv.second.snapshot = kv.second.n;
+        fx.pend.clear();
+        for (u32 r = 0; r < n_rules; r++) {
+            const kb_rule& rule = rules[r];
+            const RulePlan& pl = plans[r];
+            const u32 np = (u32)pl.prem.size();
+            if (np == 0) continue;
+            bool dead = false;
+            for (auto& pr : pl.prem) if (!pr.pred_const) dead = true;  // a variable predicate never matches (join_algorithm.rs:515-521)
+            if (dead) continue;
+            if (strict && np != 1 && np != 2) continue;  // semi_naive_parallel.rs:149: other arities are skipped
+            const u32 n_start = strategy == KB_NAIVE ? 1 : np;
+            for (u32 i = 0; i < n_start; i++) {
+                // premise i over the delta (semi-naive) or over all facts (naive), then the others over all facts
+                std::unique_ptr<kb_rel> cur;
+                {
+                    const PredRel& pr = fx.rels[pl.prem[i].pred];
+                    const u64 a = strategy == KB_NAIVE ? 0 : pr.delta_start;
+                    const u64 n = pr.snapshot - a;
+                    if (n == 0) continue;
+                    KB_TRY(make_view(ctx, pr, a, n, (u32)pl.prem[i].s_var, (u32)pl.prem[i].o_var, &cur));
+                    if (strict) KB_TRY(enforce_constants(ctx, pl.prem[i], &cur));
+                }
+                for (u32 j = 0; j < np && cur->n; j++) {
+                    if (j == i) continue;
+                    const PredRel& pr = fx.rels[pl.prem[j].pred];
+                    // KB_SEMI_NAIVE_OLD_DELTA: a premise before the delta premise sees only the facts older than its delta
+                    const u64 visible = old_delta && j < i ? pr.delta_start : pr.snapshot;
+                    if (visible == 0) { cur->n = 0; break; }
+                    std::unique_ptr<kb_rel> all, joined;
+                    KB_TRY(make_view(ctx, pr, 0, visible, (u32)pl.prem[j].s_var, (u32)pl.prem[j].o_var, &all));
+                    if (strict) KB_TRY(enforce_constants(ctx, pl.prem[j], &all));
+                    tr.mark(ctx, "  views");
+                    KB_TRY(hash_join_impl(ctx, *cur, *all, nullptr, &joined));
+                    cur = std::move(joined);
+                    tr.mark(ctx, "  join", cur->n);
+                }
+                if (cur->n == 0) continue;
+                // heads: filters + instantiate + dedup against known facts + append
+                for (u32 c = 0; c < rule.n_conclusion; c++) {
+                    KB_TRY(derive_head(fx, cur.get(), rule.conclusion[c], &rule, strict, nullptr, tr, &st.derivations));
+                }
+            }
+        }
+        // ---- end of round: the facts that were new become visible (infer_generic.rs:42-48)
+        for (auto& kv : fx.rels) kv.second.delta_start = kv.second.snapshot;
+        u64 round_new = 0;
+        KB_TRY(flush_pending(fx, &round_new));
+        tr.mark(ctx, "round end: append", round_new);
+        if (round_new == 0) break;
+        if (st.rounds < 64) st.round_new[st.rounds] = round_new;
+        st.rounds++;
+        st.inferred += round_new;
+        if (round > 100000) return fail(ctx, KB_E_LIMIT, "fixpoint did not converge");
+    }
+    return KB_OK;
+}
+
+}  // namespace
+
+// `seed` == nullptr: kb_datalog_fixpoint (every fact of the store is the first delta). With a seed (kb_datalog_fixpoint_seed): the store
+// is taken as closed under the rules already, the seed facts the store does not hold yet are accepted into it and form the first delta.
+static kb_status fixpoint_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rules, uint32_t strategy, bool seeded, const kb_rel* seed,
+                               kb_rel** inferred, uint64_t* n_seed_new, kb_fixpoint_stats* stats) {
+    if (!ctx) return KB_E_INVALID;
+    int prev_dev = -1;
+    cudaGetDevice(&prev_dev);
+    cudaSetDevice(ctx->device);
+    struct Restore { int d; ~Restore() { if (d >= 0) cudaSetDevice(d); } } restore{prev_dev};
+    KB_TRY(begin_call(ctx));
+    if ((n_rules && !rules) || !inferred) return fail(ctx, KB_E_INVALID, "NULL argument");
+    if (strategy != KB_SEMI_NAIVE && strategy != KB_NAIVE && strategy != KB_SEMI_NAIVE_PARALLEL && strategy != KB_SEMI_NAIVE_OLD_DELTA)
+        return fail(ctx, KB_E_INVALID, "unknown strategy %u", strategy);
+    if (seeded && !seed) return fail(ctx, KB_E_INVALID, "NULL seed");
+    if (seed && (seed->pair || seed->cols.size() != 3 || seed->col_of(0) != 0 || seed->col_of(1) != 1 || seed->col_of(2) != 2))
+        return fail(ctx, KB_E_INVALID, "the seed must be a 3-column relation with slots 0,1,2 = s,p,o");
+    if (seed && seed->n >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "seed too large");
+    const bool strict = strategy == KB_SEMI_NAIVE_PARALLEL;
+    kb_fixpoint_stats st{};
+    ScopedEvent ev0, ev1;
+    cudaEventRecord(ev0, ctx->st);
+
+    // ---- compile the rules (host): variable slots, synthetic variables for constants in s/o (quirk Q6), safety checks
+    std::vector<RulePlan> plans;
+    Fix fx;
+    Trace tr;
+    fx.ctx = ctx;
+    KB_TRY(compile_rules(ctx, rules, n_rules, &plans, &fx.rels));
     // a seed fact may belong to any predicate of the rules: each of them needs its known-fact set (to tell the new seed facts from the old)
     if (seed) for (auto& kv : fx.rels) kv.second.is_head = true;
+    // the closed token (kb_datalog_maintain's precondition) is recorded again only by an unseeded hash-join fixpoint over a store that has
+    // no inferred segment yet: then the inferred segment it appends is exactly closure(B) \ B
+    bool had_inferred = false;
+    for (auto& sg : ctx->segs) if (sg.tag == KB_TAG_INFERRED) had_inferred = true;
+    ctx->closed.reset();
 
     // ---- a seeded call may find the state its predecessor left (FixState): then nothing below reads the store
-    const bool state_off = getenv("KOLIBRIE_FIX_STATE") && getenv("KOLIBRIE_FIX_STATE")[0] == '0';  // (read per call: a test flips it)
+    const bool state_off = state_disabled();
     const std::string sig = seed && !state_off ? rules_signature(rules, n_rules) : std::string();
     bool reused = false;
     if (seed && !state_off && ctx->fix_state) {
@@ -337,128 +625,6 @@ static kb_status fixpoint_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
     }
     tr.mark(ctx, "initial known-fact sets");
 
-    // ---- one head of one rule over the joined bindings `cur`: filters + instantiate + dedup against the known facts + append to the
-    // round's pending facts (`rule_p` == nullptr: no rule filters — the seed facts of kb_datalog_fixpoint_seed take the same way in)
-    auto derive_head = [&](const kb_rel* cur, const kb_pattern& h, const kb_rule* rule_p) -> kb_status {
-        DeriveParams D{};
-        for (size_t k = 0; k < cur->cols.size(); k++) D.bcol[k] = cur->cols[k].ptr;
-        D.n = (u32)cur->n;
-        auto term = [&](const kb_term& t) {
-            HeadTerm ht;
-            ht.is_var = t.is_var;
-            ht.value = t.is_var ? (u32)cur->col_of(t.value) : t.value;
-            return ht;
-        };
-        D.head_s = term(h.s);
-        D.head_o = term(h.o);
-        D.n_filt = 0;
-        for (u32 f = 0; f < (strict || !rule_p ? 0u : rule_p->n_filters); f++) {  // the parallel variant never evaluates the rule filters
-            const kb_rule_filter& rf = rule_p->filters[f];
-            const int lc = cur->col_of(rf.lhs_slot);
-            if (lc < 0 || rf.cmp == 0) continue;  // unbound lhs: the reference skips the filter (rules.rs:139)
-            RuleFilterDev d;
-            d.lhs_col = (u32)lc;
-            d.cmp = rf.cmp;
-            d.rhs_value = rf.rhs_value;
-            d.rhs_is_var = 0; d.rhs_col = 0;
-            if (rf.rhs_is_var) {
-                const int rc = cur->col_of(rf.rhs_slot);
-                if (rc >= 0) { d.rhs_is_var = 1; d.rhs_col = (u32)rc; }
-                // rhs names an unbound variable: the reference falls to the numeric branch with value.parse() (rules.rs:148-151)
-            }
-            D.filt[D.n_filt++] = d;
-        }
-        D.nt = numtab(ctx);
-        PredRel& hr = fx.rels[h.p.value];
-        KB_TRY(ensure_set(fx, hr, cur->n));
-        tr.mark(ctx, "  ensure_set", hr.set_slots);
-        Pending pd;
-        pd.pred = h.p.value;
-        pd.count = 0;
-        KB_TRY(alloc_col(ctx, cur->n, &pd.s));
-        KB_TRY(alloc_col(ctx, cur->n, &pd.o));
-        const u32 coff = ctrl_alloc(ctx, 8);
-        KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + coff, 0, 8 * sizeof(u32), ctx->st));
-        D.out_s = pd.s.ptr; D.out_o = pd.o.ptr;
-        D.out_cap = (u32)cur->n;
-        D.out_count = ctx->ctrl + coff;
-        D.overflow = ctx->ctrl + coff + 1;
-        D.n_deriv = reinterpret_cast<unsigned long long*>(ctx->ctrl + coff + 4);
-        const u64 count_before = hr.set_count;
-        for (;;) {
-            D.set = static_cast<u64*>(hr.set->p);
-            D.set_slots = hr.set_slots;
-            // the set may fill up to 3/4 before it has to grow (expected: 1/2)
-            D.budget = (u32)std::min<u64>((u64)hr.set_slots / 4 * 3 - count_before, 0xFFFFFFFFull);
-            // Large candidate sets against a table far beyond L2: radix-partition the candidates by the high bits of their
-            // home slot and probe partition by partition (each slice stays L2-resident) instead of one random DRAM line per
-            // candidate. Partitions: ~32 MB slices, at least ~1 M candidates each (so that the CTAs of the probe pass sit on
-            // one or two slices at a time), at most 1024.
-            u64 n_parts = 0;
-            {
-                const u64 set_bytes = (u64)hr.set_slots * sizeof(u64);
-                u64 want = std::min<u64>(set_bytes / ctx->derive_slice_bytes, std::min<u64>(cur->n / ctx->derive_min_part_rows, 1024));
-                while (want >= 2 && n_parts * 2 <= want) n_parts = n_parts ? n_parts * 2 : 2;  // power of two
-                if (ctx->derive_part == 0) n_parts = 0;
-            }
-            if (n_parts >= 2) {
-                DerivePartParams Q{};
-                Q.d = D;
-                Q.n_parts = (u32)n_parts;
-                u32 set_bits = 0;
-                while ((1ull << set_bits) < hr.set_slots) set_bits++;
-                u32 part_bits = 0;
-                while ((1ull << part_bits) < n_parts) part_bits++;
-                Q.slice_bits = set_bits - part_bits;
-                Q.bucket_cap = (u32)std::min<u64>(cur->n / n_parts + cur->n / n_parts / 8 + ctx->derive_bucket_slack, 0xFFFFFFF0ull);
-                Buf ctl;
-                const size_t bucket_bytes = n_parts * (u64)Q.bucket_cap * sizeof(u64);
-                if (!fx.buckets || fx.buckets->bytes < bucket_bytes) {
-                    fx.buckets.reset();
-                    KB_TRY(alloc_buf(ctx, bucket_bytes + bucket_bytes / 4, &fx.buckets));
-                }
-                Buf buckets = fx.buckets;
-                KB_TRY(alloc_buf(ctx, (2 * n_parts + 8) * sizeof(u32), &ctl));
-                KB_CUDA(ctx, cudaMemsetAsync(ctl->p, 0, (2 * n_parts + 8) * sizeof(u32), ctx->st));
-                Q.buckets = static_cast<u64*>(buckets->p);
-                Q.cursors = static_cast<u32*>(ctl->p);
-                Q.tile_start = Q.cursors + n_parts;
-                Q.tickets = Q.tile_start + n_parts + 1 + ((n_parts + 1) & 1u);
-                tr.mark(ctx, "    derive: buckets allocated", n_parts);
-                timer_begin(ctx, F_OTHER, 3);
-                launch_derive_partitioned(Q, ctx->n_sms, ctx->st);
-                timer_end(ctx);
-                ctx->stats.rows_built += cur->n;  // (counted as table traffic: partitioned candidates)
-            } else {
-                timer_begin(ctx, F_OTHER);
-                launch_derive(D, ctx->n_sms, ctx->st);
-                timer_end(ctx);
-            }
-            KB_CUDA(ctx, cudaGetLastError());
-            // counts are read immediately: the control arena may be recycled by later joins of this round
-            KB_TRY(ctrl_read(ctx));
-            pd.count = ctx->h_ctrl[coff];
-            if (ctx->h_ctrl[coff + 1] == 1u) return fail(ctx, KB_E_LIMIT, "known-fact set overflow");
-            if (ctx->h_ctrl[coff + 1] == 0u) break;
-            // budget reached: rebuild the set larger WITH the facts appended so far, then repeat the launch (facts already
-            // inserted are found present and are not appended twice; the derivation count is the last, complete pass's)
-            fx.pend.push_back(pd);
-            const kb_status gs = ensure_set(fx, hr, cur->n, true);
-            fx.pend.pop_back();
-            if (gs != KB_OK) return gs;
-            KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + coff + 1, 0, sizeof(u32), ctx->st));
-            KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + coff + 4, 0, 2 * sizeof(u32), ctx->st));
-        }
-        unsigned long long nd;
-        memcpy(&nd, ctx->h_ctrl + coff + 4, sizeof nd);
-        st.derivations += nd;
-        hr.set_count = count_before;
-        hr.set_count += pd.count;
-        if (pd.count) fx.pend.push_back(pd);
-        tr.mark(ctx, "  derive", pd.count);
-        return KB_OK;
-    };
-
     // ---- seed: its facts take the way of derived heads (dedup against the known facts); the winners become visible now and are the
     // first delta, everything the store held is OLD
     u64 seed_new = 0;
@@ -475,90 +641,17 @@ static kb_status fixpoint_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
             if (sub->n == 0) continue;
             kb_pattern h{};
             h.s = kb_term{1, 0}; h.p = kb_term{0, kv.first}; h.o = kb_term{1, 2};
-            KB_TRY(derive_head(sub.get(), h, nullptr));
+            KB_TRY(derive_head(fx, sub.get(), h, nullptr, strict, nullptr, tr, &st.derivations));
         }
         for (auto& kv : fx.rels) kv.second.delta_start = kv.second.snapshot;
-        for (auto& pd : fx.pend) {
-            PredRel& r = fx.rels[pd.pred];
-            const u64 cnt = pd.count;
-            KB_TRY(grow_rel(ctx, r, r.n + cnt));
-            KB_CUDA(ctx, cudaMemcpyAsync(r.s.ptr + r.n, pd.s.ptr, cnt * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
-            KB_CUDA(ctx, cudaMemcpyAsync(r.o.ptr + r.n, pd.o.ptr, cnt * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
-            r.n += cnt;
-            seed_new += cnt;
-        }
-        fx.pend.clear();
+        KB_TRY(flush_pending(fx, &seed_new));
         for (auto& kv : fx.rels) kv.second.base_n = kv.second.n;
         st.derivations = 0;  // (the seed's facts are not derivations)
         tr.mark(ctx, "seed accepted", seed_new);
     }
 
     // ---- rounds
-    for (u32 round = 0;; round++) {
-        for (auto& kv : fx.rels) kv.second.snapshot = kv.second.n;
-        fx.pend.clear();
-        for (u32 r = 0; r < n_rules; r++) {
-            const kb_rule& rule = rules[r];
-            const RulePlan& pl = plans[r];
-            const u32 np = (u32)pl.prem.size();
-            if (np == 0) continue;
-            bool dead = false;
-            for (auto& pr : pl.prem) if (!pr.pred_const) dead = true;  // a variable predicate never matches (join_algorithm.rs:515-521)
-            if (dead) continue;
-            if (strict && np != 1 && np != 2) continue;  // semi_naive_parallel.rs:149: other arities are skipped
-            const u32 n_start = strategy == KB_NAIVE ? 1 : np;
-            for (u32 i = 0; i < n_start; i++) {
-                // premise i over the delta (semi-naive) or over all facts (naive), then the others over all facts
-                std::unique_ptr<kb_rel> cur;
-                {
-                    const PredRel& pr = fx.rels[pl.prem[i].pred];
-                    const u64 a = strategy == KB_NAIVE ? 0 : pr.delta_start;
-                    const u64 n = pr.snapshot - a;
-                    if (n == 0) continue;
-                    KB_TRY(make_view(ctx, pr, a, n, (u32)pl.prem[i].s_var, (u32)pl.prem[i].o_var, &cur));
-                    if (strict) KB_TRY(enforce_constants(ctx, pl.prem[i], &cur));
-                }
-                for (u32 j = 0; j < np && cur->n; j++) {
-                    if (j == i) continue;
-                    const PredRel& pr = fx.rels[pl.prem[j].pred];
-                    // KB_SEMI_NAIVE_OLD_DELTA: a premise before the delta premise sees only the facts older than its delta
-                    const u64 visible = old_delta && j < i ? pr.delta_start : pr.snapshot;
-                    if (visible == 0) { cur->n = 0; break; }
-                    std::unique_ptr<kb_rel> all, joined;
-                    KB_TRY(make_view(ctx, pr, 0, visible, (u32)pl.prem[j].s_var, (u32)pl.prem[j].o_var, &all));
-                    if (strict) KB_TRY(enforce_constants(ctx, pl.prem[j], &all));
-                    tr.mark(ctx, "  views");
-                    KB_TRY(hash_join_impl(ctx, *cur, *all, nullptr, &joined));
-                    cur = std::move(joined);
-                    tr.mark(ctx, "  join", cur->n);
-                }
-                if (cur->n == 0) continue;
-                // heads: filters + instantiate + dedup against known facts + append
-                for (u32 c = 0; c < rule.n_conclusion; c++) {
-                    KB_TRY(derive_head(cur.get(), rule.conclusion[c], &rule));
-                }
-            }
-        }
-        // ---- end of round: the facts that were new become visible (infer_generic.rs:42-48)
-        u64 round_new = 0;
-        for (auto& kv : fx.rels) kv.second.delta_start = kv.second.snapshot;
-        for (auto& pd : fx.pend) {
-            PredRel& r = fx.rels[pd.pred];
-            const u64 cnt = pd.count;
-            KB_TRY(grow_rel(ctx, r, r.n + cnt));
-            KB_CUDA(ctx, cudaMemcpyAsync(r.s.ptr + r.n, pd.s.ptr, cnt * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
-            KB_CUDA(ctx, cudaMemcpyAsync(r.o.ptr + r.n, pd.o.ptr, cnt * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
-            r.n += cnt;
-            round_new += cnt;
-        }
-        fx.pend.clear();
-        tr.mark(ctx, "round end: append", round_new);
-        if (round_new == 0) break;
-        if (st.rounds < 64) st.round_new[st.rounds] = round_new;
-        st.rounds++;
-        st.inferred += round_new;
-        if (round > 100000) return fail(ctx, KB_E_LIMIT, "fixpoint did not converge");
-    }
+    KB_TRY(run_rounds(fx, rules, n_rules, plans, strategy, st, tr));
 
     // ---- result: inferred facts as (s,p,o) columns; also appended to the store (infer_generic.rs:46 index_manager.insert)
     auto res = std::make_unique<kb_rel>();
@@ -612,6 +705,14 @@ static kb_status fixpoint_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
         fs->rels = std::move(fx.rels);
         ctx->fix_state = fs;
     }
+    if (!seed && !strict && !had_inferred) {
+        auto cl = std::make_shared<Closed>();
+        cl->sig = rules_signature(rules, n_rules);
+        cl->store_version = ctx->store_version;
+        cl->num_version = ctx->num_version;
+        cl->numeric = rules_read_numbers(rules, n_rules);
+        ctx->closed = cl;
+    }
     if (stats) *stats = st;
     if (n_seed_new) *n_seed_new = seed_new;
     ctx->stats.rows_out = st.inferred;
@@ -629,5 +730,605 @@ extern "C" kb_status kb_datalog_fixpoint(kb_ctx* ctx, const kb_rule* rules, uint
 // again) and by the sharded fixpoint (kolibrie_b200/dist.py: facts derived on another rank arrive as seeds).
 extern "C" kb_status kb_datalog_fixpoint_seed(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rules, uint32_t strategy, const kb_rel* seed,
                                               kb_rel** out, uint64_t* n_seed_new, kb_fixpoint_stats* stats) {
+    // (the seed facts are stored with KB_TAG_INFERRED: base and inferred facts can no longer be told apart, so the closed token goes)
     return fixpoint_impl(ctx, rules, n_rules, strategy, true, seed, out, n_seed_new, stats);
+}
+
+// =====================================================================================================================================
+// kb_datalog_maintain: delete-and-rederive (DRed) of the inferred segment across a window slide
+namespace {
+
+struct Pairs {  // a list of (s,o) facts of one predicate
+    Col s, o;
+    u64 n = 0;
+};
+
+u64 slots_for(u64 n) {
+    u64 s = 1024;
+    while (s < 2 * n) s <<= 1;
+    return s;
+}
+
+kb_status base_alloc(kb_ctx* ctx, BaseCount& b, u64 slots) {
+    if (slots > (1ull << 31)) return fail(ctx, KB_E_LIMIT, "base count table would need more than 2^31 slots");
+    BaseCount nb;
+    nb.slots = (u32)slots;
+    KB_TRY(alloc_buf(ctx, slots * sizeof(u64), &nb.keys));
+    KB_TRY(alloc_buf(ctx, slots * sizeof(u32), &nb.cnt));
+    KB_CUDA(ctx, cudaMemsetAsync(nb.keys->p, 0xFF, slots * sizeof(u64), ctx->st));
+    KB_CUDA(ctx, cudaMemsetAsync(nb.cnt->p, 0, slots * sizeof(u32), ctx->st));
+    b = nb;
+    return KB_OK;
+}
+
+// n rows join (delta +1) or leave (delta -1) the base; *edge (nullable) receives the facts whose count crossed zero: the facts that were
+// not base facts before (+1), the facts that are no base facts any more (-1). Every such fact comes out once.
+kb_status base_update(kb_ctx* ctx, BaseCount& b, const u32* s, const u32* o, u64 n, int delta, Pairs* edge) {
+    if (edge) *edge = Pairs{};
+    // +1 may claim up to n slots. When that could take the table past 3/4, the LIVE keys move to a fresh table sized for them and the
+    // rows (the keys whose count fell to 0 are dropped): the table follows the live facts, not the rows a long-running window has seen
+    // (the reference's firing protocol re-adds the whole window every firing, n ~ the window, most keys already there)
+    if (delta > 0 && (b.occupied + n) * 4 > (u64)b.slots * 3) {
+        BaseCount nb;
+        KB_TRY(base_alloc(ctx, nb, slots_for(b.live + n)));
+        const u32 off = ctrl_alloc(ctx, 2);
+        KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, 2 * sizeof(u32), ctx->st));
+        launch_base_count_rehash(static_cast<const u64*>(b.keys->p), static_cast<const u32*>(b.cnt->p), b.slots, static_cast<u64*>(nb.keys->p),
+                                 static_cast<u32*>(nb.cnt->p), nb.slots, ctx->ctrl + off, ctx->ctrl + off + 1, ctx->n_sms, ctx->st);
+        KB_CUDA(ctx, cudaGetLastError());
+        KB_TRY(ctrl_read(ctx));
+        if (ctx->h_ctrl[off + 1]) return fail(ctx, KB_E_LIMIT, "base count table overflow");
+        if (ctx->h_ctrl[off] != b.live) return fail(ctx, KB_E_INVALID, "base count table: %u live keys moved, %llu expected", ctx->h_ctrl[off], (unsigned long long)b.live);
+        nb.occupied = nb.live = b.live;
+        b = nb;
+    }
+    if (n == 0) return KB_OK;
+    BaseCountParams P{};
+    P.keys = static_cast<u64*>(b.keys->p);
+    P.cnt = static_cast<u32*>(b.cnt->p);
+    P.slots = b.slots;
+    P.s = s; P.o = o;
+    P.n = (u32)n;
+    P.delta = delta;
+    if (edge) {
+        KB_TRY(alloc_col(ctx, n, &edge->s));
+        KB_TRY(alloc_col(ctx, n, &edge->o));
+        P.out_s = edge->s.ptr; P.out_o = edge->o.ptr;
+    }
+    const u32 off = ctrl_alloc(ctx, 4);
+    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, 4 * sizeof(u32), ctx->st));
+    P.out_count = ctx->ctrl + off;
+    P.overflow = ctx->ctrl + off + 1;
+    P.claimed = ctx->ctrl + off + 2;
+    timer_begin(ctx, F_BUILD);
+    launch_base_count(P, ctx->n_sms, ctx->st);
+    timer_end(ctx);
+    KB_CUDA(ctx, cudaGetLastError());
+    KB_TRY(ctrl_read(ctx));
+    if (ctx->h_ctrl[off + 1]) return fail(ctx, KB_E_LIMIT, "base count table overflow");
+    const u64 crossed = ctx->h_ctrl[off];
+    b.occupied += ctx->h_ctrl[off + 2];
+    if (delta > 0) b.live += crossed;
+    else b.live -= std::min<u64>(crossed, b.live);
+    if (edge) edge->n = crossed;
+    return KB_OK;
+}
+
+// the rows (s,o) whose membership in a set (keys/cnt/slots: a count table, cnt == nullptr: a plain 64-bit set; keys == nullptr: the
+// empty set) equals `keep_present`
+kb_status select_pairs(kb_ctx* ctx, const u32* s, const u32* o, u64 n, const u64* keys, const u32* cnt, u32 slots, bool keep_present, Pairs* out) {
+    *out = Pairs{};
+    KB_TRY(alloc_col(ctx, n, &out->s));
+    KB_TRY(alloc_col(ctx, n, &out->o));
+    if (n == 0) return KB_OK;
+    if (!keys) {
+        if (keep_present) return KB_OK;
+        KB_CUDA(ctx, cudaMemcpyAsync(out->s.ptr, s, n * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
+        KB_CUDA(ctx, cudaMemcpyAsync(out->o.ptr, o, n * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
+        out->n = n;
+        return KB_OK;
+    }
+    PairSelectParams P{};
+    P.s = s; P.o = o;
+    P.n = (u32)n;
+    P.keys = keys; P.cnt = cnt; P.slots = slots;
+    P.keep_present = keep_present ? 1u : 0u;
+    P.out_s = out->s.ptr; P.out_o = out->o.ptr;
+    const u32 off = ctrl_alloc(ctx, 1);
+    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, sizeof(u32), ctx->st));
+    P.out_count = ctx->ctrl + off;
+    timer_begin(ctx, F_FILTER);
+    launch_pair_select(P, ctx->n_sms, ctx->st);
+    timer_end(ctx);
+    KB_CUDA(ctx, cudaGetLastError());
+    KB_TRY(ctrl_read(ctx));
+    out->n = ctx->h_ctrl[off];
+    return KB_OK;
+}
+const u64* set_of(const PredRel& r) { return r.set ? static_cast<const u64*>(r.set->p) : nullptr; }
+
+// the rows of the store segments `which` selects, split by predicate: out[p] = (s, o) of every predicate of `preds` (one fused scan per 8
+// predicates over those segments only)
+kb_status split_segments(kb_ctx* ctx, const std::vector<u32>& preds, const std::function<bool(const Segment&)>& which, std::map<u32, Pairs>* out) {
+    std::vector<Segment> part;
+    u64 n = 0;
+    for (auto& sg : ctx->segs) if (which(sg)) { part.push_back(sg); n += sg.n; }
+    for (u32 p : preds) (*out)[p] = Pairs{};
+    if (n == 0 || preds.empty()) return KB_OK;
+    struct Swap {  // the scan reads ctx->segs: it sees the selected segments, and the store is whole again on every return path
+        kb_ctx* c;
+        std::vector<Segment> segs;
+        u64 n;
+        ~Swap() { c->segs.swap(segs); c->n_triples = n; c->in_index_build = false; }
+    } sw{ctx, std::move(part), ctx->n_triples};
+    ctx->segs.swap(sw.segs);
+    ctx->n_triples = n;
+    ctx->in_index_build = true;  // read the segments themselves, not the index
+    for (size_t b = 0; b < preds.size(); b += MAXP) {
+        const u32 k = (u32)std::min<size_t>(MAXP, preds.size() - b);
+        kb_pattern pats[MAXP];
+        for (u32 i = 0; i < k; i++) { pats[i].s = kb_term{1, 0}; pats[i].p = kb_term{0, preds[b + i]}; pats[i].o = kb_term{1, 1}; }
+        std::vector<std::unique_ptr<kb_rel>> res;
+        std::vector<FilterProg> none;
+        KB_TRY(scan_impl(ctx, pats, k, none, false, false, &res));
+        for (u32 i = 0; i < k; i++) {
+            Pairs& p = (*out)[preds[b + i]];
+            p.s = res[i]->cols[0];
+            p.o = res[i]->cols[1];
+            p.n = res[i]->n;
+        }
+    }
+    return KB_OK;
+}
+
+// (s,p,o) relation of per-predicate fact lists
+kb_status assemble(kb_ctx* ctx, const std::vector<std::pair<u32, Pairs>>& parts, std::unique_ptr<kb_rel>* out) {
+    u64 total = 0;
+    for (auto& pp : parts) total += pp.second.n;
+    if (total >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "result exceeds 2^32 - 16 rows");
+    auto res = std::make_unique<kb_rel>();
+    res->slots = {0, 1, 2};
+    res->n = total;
+    Col cs, cp, co;
+    KB_TRY(alloc_col(ctx, total, &cs));
+    KB_TRY(alloc_col(ctx, total, &cp));
+    KB_TRY(alloc_col(ctx, total, &co));
+    u64 off = 0;
+    for (auto& pp : parts) {
+        const u64 cnt = pp.second.n;
+        if (!cnt) continue;
+        KB_CUDA(ctx, cudaMemcpyAsync(cs.ptr + off, pp.second.s.ptr, cnt * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
+        KB_CUDA(ctx, cudaMemcpyAsync(co.ptr + off, pp.second.o.ptr, cnt * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
+        launch_fill_u32(cp.ptr + off, pp.first, cnt, ctx->st);
+        off += cnt;
+    }
+    res->cols = {cs, cp, co};
+    *out = std::move(res);
+    return KB_OK;
+}
+
+// the facts of a head predicate as bindings of the head's variables (a constant of the head binds nothing: every fact derived from
+// these bindings is checked against the facts themselves by the gate); nullptr when the head has no variable
+std::unique_ptr<kb_rel> head_view(const PredRel& D, const kb_pattern& h) {
+    auto v = std::make_unique<kb_rel>();
+    v->n = D.n;
+    if (h.s.is_var) { v->slots.push_back(h.s.value); v->cols.push_back(D.s); }
+    if (h.o.is_var && !(h.s.is_var && h.o.value == h.s.value)) { v->slots.push_back(h.o.value); v->cols.push_back(D.o); }
+    if (v->slots.empty()) return nullptr;
+    return v;
+}
+
+}  // namespace
+
+static kb_status maintain_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rules, uint32_t strategy, const uint64_t* evict_tags, uint32_t n_evict,
+                               const kb_rel* add, uint64_t add_tag, kb_rel** inferred_removed, kb_rel** inferred_added, kb_maintain_stats* stats) {
+    // ---- validation: nothing changes before all of it passed
+    if ((n_rules && !rules) || (n_evict && !evict_tags)) return fail(ctx, KB_E_INVALID, "NULL argument");
+    if (strategy != KB_SEMI_NAIVE && strategy != KB_NAIVE && strategy != KB_SEMI_NAIVE_PARALLEL && strategy != KB_SEMI_NAIVE_OLD_DELTA)
+        return fail(ctx, KB_E_INVALID, "unknown strategy %u", strategy);
+    if (strategy == KB_SEMI_NAIVE_PARALLEL) return fail(ctx, KB_E_UNSUPPORTED, "kb_datalog_maintain: KB_SEMI_NAIVE_PARALLEL has its own closure; not maintained");
+    if (add && (add->pair || add->cols.size() != 3 || add->col_of(0) != 0 || add->col_of(1) != 1 || add->col_of(2) != 2))
+        return fail(ctx, KB_E_INVALID, "`add` must be a 3-column relation with slots 0,1,2 = s,p,o");
+    if (add && add->n >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "`add` too large");
+    if (add && add_tag == KB_TAG_INFERRED) return fail(ctx, KB_E_INVALID, "KB_TAG_INFERRED is not a tag `add` can take");
+    std::set<u64> evict(evict_tags, evict_tags + n_evict);
+    if (evict.count(KB_TAG_INFERRED)) return fail(ctx, KB_E_INVALID, "KB_TAG_INFERRED cannot be evicted by kb_datalog_maintain");
+    std::vector<RulePlan> plans;
+    Fix fx;
+    fx.ctx = ctx;
+    KB_TRY(compile_rules(ctx, rules, n_rules, &plans, &fx.rels));
+    std::map<u32, bool> head;  // predicates that occur in a conclusion (the only ones with inferred facts)
+    for (auto& kv : fx.rels) { head[kv.first] = kv.second.is_head; kv.second.is_head = true; }
+    const std::string sig = rules_signature(rules, n_rules);
+    auto cl = std::static_pointer_cast<Closed>(ctx->closed);
+    if (!cl || cl->sig != sig || cl->store_version != ctx->store_version || (cl->numeric && cl->num_version != ctx->num_version))
+        return fail(ctx, KB_E_INVALID, "store not closed under these rules: run kb_datalog_fixpoint");
+    for (u64 t : evict) {
+        bool found = false;
+        for (auto& sg : ctx->segs) if (sg.tag == t) found = true;
+        if (!found) return fail(ctx, KB_E_NOT_FOUND, "no segment with tag %llu", (unsigned long long)t);
+    }
+    kb_maintain_stats ms{};
+    ScopedEvent ev0, ev1;
+    cudaEventRecord(ev0, ctx->st);
+    Trace tr;
+    std::unique_ptr<kb_rel> out_removed, out_added;
+    if (evict.empty() && !add) {  // nothing moves
+        KB_TRY(assemble(ctx, {}, &out_removed));
+        KB_TRY(assemble(ctx, {}, &out_added));
+        if (stats) *stats = ms;
+        if (inferred_removed) *inferred_removed = out_removed.release();
+        if (inferred_added) *inferred_added = out_added.release();
+        return KB_OK;
+    }
+    std::vector<u32> preds;
+    for (auto& kv : fx.rels) preds.push_back(kv.first);
+
+    // ---- the kept state (the relations of B ∪ I, their known-fact sets, the base multiplicities) or the same rebuilt from the store.
+    // From here until the store is rewritten the store does not change: a failure drops the state (the next call rebuilds it) and keeps
+    // the token, since the store is still closed.
+    const bool state_off = state_disabled();
+    std::map<u32, BaseCount> base;
+    if (cl->has_state && !state_off) {
+        fx.rels = std::move(cl->rels);
+        base = std::move(cl->base);
+    }
+    const bool reused = cl->has_state && !state_off;
+    cl->has_state = false;
+    cl->rels.clear();
+    cl->base.clear();
+    if (!reused) {
+        std::map<u32, Pairs> bsplit, isplit;
+        KB_TRY(split_segments(ctx, preds, [](const Segment& sg) { return sg.tag != KB_TAG_INFERRED; }, &bsplit));
+        KB_TRY(split_segments(ctx, preds, [](const Segment& sg) { return sg.tag == KB_TAG_INFERRED; }, &isplit));
+        for (u32 p : preds) {
+            PredRel& r = fx.rels[p];
+            const Pairs &b = bsplit[p], &i = isplit[p];
+            KB_TRY(grow_rel(ctx, r, std::max<u64>((b.n + i.n) * 2, 1024)));
+            KB_TRY(append_rows(ctx, r, b.s.ptr, b.o.ptr, b.n));
+            KB_TRY(append_rows(ctx, r, i.s.ptr, i.o.ptr, i.n));
+            r.set_count = r.n;
+            KB_TRY(ensure_set(fx, r, 1024));
+            KB_TRY(base_alloc(ctx, base[p], slots_for(b.n + 1024)));
+            KB_TRY(base_update(ctx, base[p], b.s.ptr, b.o.ptr, b.n, +1, nullptr));
+        }
+    }
+    tr.mark(ctx, "maintain: state", reused);
+
+    // ---- 1. base difference from set membership: the rows of `add` join the base, then the rows of the evicted segments leave it.
+    // D0 = facts whose count reached 0 (B \ B'), `fresh` = facts of `add` whose count left 0 (B' \ B). A fact that another live segment
+    // or `add` still holds keeps a positive count and does not move.
+    std::map<u32, Pairs> evicted, d0, fresh;
+    std::map<u32, std::unique_ptr<kb_rel>> add_of;
+    KB_TRY(split_segments(ctx, preds, [&](const Segment& sg) { return evict.count(sg.tag) != 0; }, &evicted));
+    for (u32 p : preds) {
+        if (add && add->n) {
+            FilterProg f;
+            kb_filter_op op{};
+            op.op = KB_F_EQ_ID; op.slot = 1; op.id = p;
+            f.ops.push_back(op);
+            KB_TRY(filter_impl(ctx, *add, f, &add_of[p]));
+            const kb_rel& a = *add_of[p];
+            KB_TRY(base_update(ctx, base[p], a.cols[a.col_of(0)].ptr, a.cols[a.col_of(2)].ptr, a.n, +1, &fresh[p]));
+        }
+        KB_TRY(base_update(ctx, base[p], evicted[p].s.ptr, evicted[p].o.ptr, evicted[p].n, -1, &d0[p]));
+        ms.base_added += fresh[p].n;
+        ms.base_removed += d0[p].n;
+    }
+    // facts of `add` that were inferred: they leave I (they are base facts now), read before the known-fact sets change
+    std::vector<std::pair<u32, Pairs>> removed_parts, added_parts;
+    for (u32 p : preds) {
+        if (!head[p] || fresh[p].n == 0) continue;
+        Pairs moved;
+        const PredRel& r = fx.rels[p];
+        KB_TRY(select_pairs(ctx, fresh[p].s.ptr, fresh[p].o.ptr, fresh[p].n, set_of(r), nullptr, r.set_slots, true, &moved));
+        removed_parts.push_back({p, moved});
+    }
+    tr.mark(ctx, "maintain: base difference", ms.base_removed);
+    if (tr.on) {  // (what a long-running window holds in base count tables: bounded by the live facts)
+        u64 slots = 0;
+        for (auto& kv : base) slots += kv.second.slots;
+        tr.mark(ctx, "maintain: base count slots", slots);
+    }
+
+    // ---- 2. over-delete, semi-naive from D0: the delta of one premise joined against the OLD facts (B ∪ I) of the others; a head that is
+    // known, is no fact of B', and was not marked yet joins the next delta. `del` holds D0 ∪ OD per predicate (list + set).
+    Fix del;
+    del.ctx = ctx;
+    std::map<u32, u64> d0n;
+    for (u32 p : preds) {
+        PredRel& r = del.rels[p];
+        r.pred = p;
+        r.is_head = true;
+        KB_TRY(append_rows(ctx, r, d0[p].s.ptr, d0[p].o.ptr, d0[p].n));
+        d0n[p] = r.n;
+        r.set_count = r.n;
+        KB_TRY(ensure_set(del, r, 1024));
+    }
+    u64 derivations = 0;
+    for (;;) {
+        for (auto& kv : del.rels) kv.second.snapshot = kv.second.n;
+        del.pend.clear();
+        for (u32 r = 0; r < n_rules; r++) {
+            const kb_rule& rule = rules[r];
+            const RulePlan& pl = plans[r];
+            const u32 np = (u32)pl.prem.size();
+            bool dead = np == 0;
+            for (auto& pr : pl.prem) if (!pr.pred_const) dead = true;
+            if (dead) continue;
+            for (u32 i = 0; i < np; i++) {
+                const PredRel& dr = del.rels[pl.prem[i].pred];
+                const u64 n = dr.snapshot - dr.delta_start;
+                if (n == 0) continue;
+                std::unique_ptr<kb_rel> cur;
+                KB_TRY(make_view(ctx, dr, dr.delta_start, n, (u32)pl.prem[i].s_var, (u32)pl.prem[i].o_var, &cur));
+                for (u32 j = 0; j < np && cur->n; j++) {
+                    if (j == i) continue;
+                    const PredRel& pr = fx.rels[pl.prem[j].pred];
+                    if (pr.n == 0) { cur->n = 0; break; }
+                    std::unique_ptr<kb_rel> all, joined;
+                    KB_TRY(make_view(ctx, pr, 0, pr.n, (u32)pl.prem[j].s_var, (u32)pl.prem[j].o_var, &all));
+                    KB_TRY(hash_join_impl(ctx, *cur, *all, nullptr, &joined));
+                    cur = std::move(joined);
+                }
+                if (cur->n == 0) continue;
+                for (u32 c = 0; c < rule.n_conclusion; c++) {
+                    const PredRel& known = fx.rels[rule.conclusion[c].p.value];
+                    Gate g;
+                    g.must = set_of(known);
+                    g.must_slots = known.set_slots;
+                    g.veto = &base[rule.conclusion[c].p.value];
+                    KB_TRY(derive_head(del, cur.get(), rule.conclusion[c], &rule, false, &g, tr, &derivations));
+                }
+            }
+        }
+        for (auto& kv : del.rels) kv.second.delta_start = kv.second.snapshot;
+        u64 marked = 0;
+        KB_TRY(flush_pending(del, &marked));
+        if (marked == 0) break;
+        ms.overdeleted += marked;
+        ms.overdelete_rounds++;
+        if (ms.overdelete_rounds > 100000) return fail(ctx, KB_E_LIMIT, "over-deletion did not converge");
+    }
+    tr.mark(ctx, "maintain: over-delete", ms.overdeleted);
+
+    // ---- 3. remove D0 ∪ OD: the relations are compacted (mark-and-compact against the deletion set), the known-fact sets get
+    // tombstones (they go when the set is next rebuilt from its relation)
+    for (u32 p : preds) {
+        const PredRel& dr = del.rels[p];
+        if (dr.n == 0) continue;
+        PredRel& r = fx.rels[p];
+        Pairs keep;
+        KB_TRY(select_pairs(ctx, r.s.ptr, r.o.ptr, r.n, set_of(dr), nullptr, dr.set_slots, false, &keep));
+        r.s = keep.s; r.o = keep.o; r.n = keep.n; r.cap = keep.n;  // (the next append reallocates)
+        launch_set64_erase(static_cast<u64*>(r.set->p), r.set_slots, dr.s.ptr, dr.o.ptr, (u32)dr.n, ctx->n_sms, ctx->st);
+        KB_CUDA(ctx, cudaGetLastError());
+    }
+    tr.mark(ctx, "maintain: remove");
+
+    // ---- 4. rederive: the removed facts of a head, used as an extra first premise that binds the head's variables, joined against the
+    // remaining facts; a derived head that is one of the removed facts (gate) is still derivable
+    Fix red;
+    red.ctx = ctx;
+    for (u32 p : preds) { red.rels[p].pred = p; red.rels[p].is_head = true; }
+    for (u32 r = 0; r < n_rules; r++) {
+        const kb_rule& rule = rules[r];
+        const RulePlan& pl = plans[r];
+        const u32 np = (u32)pl.prem.size();
+        bool dead = np == 0;
+        for (auto& pr : pl.prem) if (!pr.pred_const) dead = true;
+        if (dead) continue;
+        for (u32 c = 0; c < rule.n_conclusion; c++) {
+            const kb_pattern& h = rule.conclusion[c];
+            const PredRel& dr = del.rels[h.p.value];
+            if (dr.n == 0) continue;
+            std::unique_ptr<kb_rel> cur = head_view(dr, h);
+            std::vector<bool> used(np, false);
+            for (u32 step = 0; step < np && (!cur || cur->n); step++) {
+                u32 j = np;  // next premise: the first one that shares a variable with the bindings so far (no cartesian products)
+                for (u32 k = 0; k < np && j == np; k++)
+                    if (!used[k] && cur && (cur->col_of((u32)pl.prem[k].s_var) >= 0 || cur->col_of((u32)pl.prem[k].o_var) >= 0)) j = k;
+                for (u32 k = 0; k < np && j == np; k++) if (!used[k]) j = k;
+                used[j] = true;
+                const PredRel& pr = fx.rels[pl.prem[j].pred];
+                std::unique_ptr<kb_rel> all, joined;
+                KB_TRY(make_view(ctx, pr, 0, pr.n, (u32)pl.prem[j].s_var, (u32)pl.prem[j].o_var, &all));
+                if (!cur) { cur = std::move(all); continue; }
+                if (pr.n == 0) { cur->n = 0; break; }
+                KB_TRY(hash_join_impl(ctx, *cur, *all, nullptr, &joined));
+                cur = std::move(joined);
+            }
+            if (!cur || cur->n == 0) continue;
+            Gate g;
+            g.must = set_of(dr);
+            g.must_slots = dr.set_slots;
+            KB_TRY(derive_head(red, cur.get(), h, &rule, false, &g, tr, &derivations));
+        }
+    }
+    {
+        u64 n = 0;
+        KB_TRY(flush_pending(red, &n));
+        ms.rederived = n;
+    }
+    tr.mark(ctx, "maintain: rederive", ms.rederived);
+
+    // ---- 5. insert: the seeds (rederived facts, then the facts of `add` the closure does not hold) take the seed path of
+    // kb_datalog_fixpoint_seed, then semi-naive rounds (KB_NAIVE: the same closure, reached from the delta)
+    for (auto& kv : fx.rels) kv.second.snapshot = kv.second.seed_from = kv.second.n;
+    fx.pend.clear();
+    {
+        u64 seed_derivations = 0;  // (seed facts are not derivations)
+        for (u32 p : preds) {
+            kb_pattern h{};
+            h.s = kb_term{1, 0}; h.p = kb_term{0, p}; h.o = kb_term{1, 2};
+            const PredRel& rr = red.rels[p];
+            if (rr.n) {
+                std::unique_ptr<kb_rel> v;
+                KB_TRY(make_view(ctx, rr, 0, rr.n, 0, 2, &v));
+                KB_TRY(derive_head(fx, v.get(), h, nullptr, false, nullptr, tr, &seed_derivations));
+            }
+            auto a = add_of.find(p);
+            if (a != add_of.end() && a->second->n) KB_TRY(derive_head(fx, a->second.get(), h, nullptr, false, nullptr, tr, &seed_derivations));
+        }
+    }
+    for (auto& kv : fx.rels) kv.second.delta_start = kv.second.snapshot;
+    {
+        u64 n = 0;
+        KB_TRY(flush_pending(fx, &n));
+    }
+    for (auto& kv : fx.rels) kv.second.base_n = kv.second.n;
+    kb_fixpoint_stats ist{};
+    KB_TRY(run_rounds(fx, rules, n_rules, plans, strategy == KB_SEMI_NAIVE_OLD_DELTA ? KB_SEMI_NAIVE_OLD_DELTA : KB_SEMI_NAIVE, ist, tr));
+    ms.insert_rounds = ist.rounds;
+    derivations += ist.derivations;
+    ms.derivations = derivations;
+    tr.mark(ctx, "maintain: insert", ist.inferred);
+
+    // ---- the differences: I \ I' = over-deleted facts that did not come back (+ the inferred facts `add` made base facts, above);
+    // I' \ I = removed base facts that are derivable now + the facts the rounds found that were never known
+    for (u32 p : preds) {
+        if (!head[p]) continue;
+        const PredRel &r = fx.rels[p], &dr = del.rels[p];
+        if (dr.n > d0n[p]) {
+            Pairs gone;
+            KB_TRY(select_pairs(ctx, dr.s.ptr + d0n[p], dr.o.ptr + d0n[p], dr.n - d0n[p], set_of(r), nullptr, r.set_slots, false, &gone));
+            removed_parts.push_back({p, gone});
+        }
+        if (d0n[p]) {
+            Pairs back;
+            KB_TRY(select_pairs(ctx, dr.s.ptr, dr.o.ptr, d0n[p], set_of(r), nullptr, r.set_slots, true, &back));
+            added_parts.push_back({p, back});
+        }
+        if (r.n > r.base_n) {
+            Pairs fresh_inf;
+            KB_TRY(select_pairs(ctx, r.s.ptr + r.base_n, r.o.ptr + r.base_n, r.n - r.base_n, set_of(dr), nullptr, dr.set_slots, false, &fresh_inf));
+            added_parts.push_back({p, fresh_inf});
+        }
+    }
+    KB_TRY(assemble(ctx, removed_parts, &out_removed));
+    KB_TRY(assemble(ctx, added_parts, &out_added));
+    ms.inferred_removed = out_removed->n;
+    ms.inferred_added = out_added->n;
+
+    // ---- 6. the new segments are built before the store changes: `add` as kb_store_append_device stores it, I' = the facts of the head
+    // relations with no base count (when I did not change and is one segment, that segment stays)
+    u32 n_inferred_segs = 0;
+    u64 evicted_rows = 0;
+    for (auto& sg : ctx->segs) {
+        if (sg.tag == KB_TAG_INFERRED) n_inferred_segs++;
+        if (evict.count(sg.tag)) evicted_rows += sg.n;
+    }
+    const bool rewrite = ms.inferred_removed || ms.inferred_added || n_inferred_segs > 1;
+    Segment sa, si;
+    if (add) {
+        sa.tag = add_tag;
+        sa.n = add->n;
+        KB_TRY(alloc_col(ctx, sa.n, &sa.s));
+        KB_TRY(alloc_col(ctx, sa.n, &sa.p));
+        KB_TRY(alloc_col(ctx, sa.n, &sa.o));
+        if (sa.n) {
+            KB_CUDA(ctx, cudaMemcpyAsync(sa.s.ptr, add->cols[0].ptr, sa.n * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
+            KB_CUDA(ctx, cudaMemcpyAsync(sa.p.ptr, add->cols[1].ptr, sa.n * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
+            KB_CUDA(ctx, cudaMemcpyAsync(sa.o.ptr, add->cols[2].ptr, sa.n * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
+            KB_TRY(segment_stats(ctx, &sa));
+        }
+    }
+    if (rewrite) {
+        std::vector<std::pair<u32, Pairs>> iparts;
+        for (u32 p : preds) {
+            if (!head[p]) continue;
+            const PredRel& r = fx.rels[p];
+            const BaseCount& b = base[p];
+            Pairs inf;
+            KB_TRY(select_pairs(ctx, r.s.ptr, r.o.ptr, r.n, static_cast<const u64*>(b.keys->p), static_cast<const u32*>(b.cnt->p), b.slots, false, &inf));
+            iparts.push_back({p, inf});
+        }
+        std::unique_ptr<kb_rel> irel;
+        KB_TRY(assemble(ctx, iparts, &irel));
+        si.tag = KB_TAG_INFERRED;
+        si.n = irel->n;
+        si.s = irel->cols[0]; si.p = irel->cols[1]; si.o = irel->cols[2];
+        if (si.n) KB_TRY(segment_stats(ctx, &si));
+    }
+    u64 live = ctx->n_triples - evicted_rows + (add ? add->n : 0);
+    if (rewrite) {
+        for (auto& sg : ctx->segs) if (sg.tag == KB_TAG_INFERRED) live -= sg.n;
+        live += si.n;
+    }
+    if (live >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "store would exceed 2^32-16 triples");
+    tr.mark(ctx, "maintain: segments built", si.n);
+
+    // ---- rewrite the store, the index maintained in place (kb_store_evict / kb_store_append_device do the same). A failure from here on
+    // leaves exactly the B' segments, no inferred segment, no kept state and no token: kb_datalog_fixpoint restores the precondition.
+    auto drop_inferred = [&]() {
+        for (size_t i = 0; i < ctx->segs.size();) {
+            if (ctx->segs[i].tag == KB_TAG_INFERRED) { ctx->n_triples -= ctx->segs[i].n; ctx->segs.erase(ctx->segs.begin() + i); }
+            else i++;
+        }
+        ctx->store_version++;
+        ctx->index.clear();
+        ctx->index_version = ~0ull;
+        ctx->closed.reset();
+    };
+    std::vector<u64> gone(evict.begin(), evict.end());
+    if (rewrite) gone.push_back(KB_TAG_INFERRED);
+    for (u64 t : gone) {
+        for (size_t i = 0; i < ctx->segs.size();) {
+            if (ctx->segs[i].tag == t) { ctx->n_triples -= ctx->segs[i].n; ctx->segs.erase(ctx->segs.begin() + i); }
+            else i++;
+        }
+        const bool maintain = ctx->index_maintain && ctx->index_version == ctx->store_version && !ctx->index.empty();
+        ctx->store_version++;
+        ctx->multi_valued.clear();
+        ctx->single_valued.clear();
+        if (maintain && index_evict_tag(ctx, t) == KB_OK) ctx->index_version = ctx->store_version;
+        else { ctx->index.clear(); ctx->index_version = ~0ull; }
+    }
+    if (add) {
+        const kb_status rc = store_add_device_segment(ctx, sa);
+        if (rc != KB_OK) { drop_inferred(); return rc; }
+    }
+    if (rewrite && si.n) {
+        const kb_status rc = store_add_device_segment(ctx, si);
+        if (rc != KB_OK) { drop_inferred(); return rc; }
+    }
+    ctx->fix_state.reset();
+    cudaEventRecord(ev1, ctx->st);
+    {
+        const cudaError_t e = cudaStreamSynchronize(ctx->st);
+        if (e != cudaSuccess) { drop_inferred(); return fail(ctx, KB_E_CUDA, "kb_datalog_maintain: %s", cudaGetErrorString(e)); }
+    }
+    timers_flush(ctx);
+    float ms_dev = 0.f;
+    cudaEventElapsedTime(&ms_dev, ev0, ev1);
+    ms.device_ms = ms_dev;
+    cl->store_version = ctx->store_version;
+    cl->num_version = ctx->num_version;
+    if (!state_off) {
+        for (auto& kv : fx.rels) { kv.second.base_n = kv.second.seed_from = kv.second.delta_start = kv.second.snapshot = kv.second.n; }
+        cl->rels = std::move(fx.rels);
+        cl->base = std::move(base);
+        cl->has_state = true;
+    }
+    tr.mark(ctx, "maintain: store rewritten");
+    if (stats) *stats = ms;
+    ctx->stats.rows_out = ms.inferred_added;
+    if (inferred_removed) *inferred_removed = out_removed.release();
+    if (inferred_added) *inferred_added = out_added.release();
+    return KB_OK;
+}
+
+// Delete-and-rederive across a window slide (rsp_engine.rs:94-109 + simple_r2r.rs:103-128 without the closure from scratch)
+extern "C" kb_status kb_datalog_maintain(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rules, uint32_t strategy, const uint64_t* evict_tags,
+                                         uint32_t n_evict, const kb_rel* add, uint64_t add_tag, kb_rel** inferred_removed, kb_rel** inferred_added,
+                                         kb_maintain_stats* stats) {
+    if (!ctx) return KB_E_INVALID;
+    int prev_dev = -1;
+    cudaGetDevice(&prev_dev);
+    cudaSetDevice(ctx->device);
+    struct Restore { int d; ~Restore() { if (d >= 0) cudaSetDevice(d); } } restore{prev_dev};
+    KB_TRY(begin_call(ctx));
+    if (inferred_removed) *inferred_removed = nullptr;
+    if (inferred_added) *inferred_added = nullptr;
+    return maintain_impl(ctx, rules, n_rules, strategy, evict_tags, n_evict, add, add_tag, inferred_removed, inferred_added, stats);
 }

@@ -211,6 +211,8 @@ struct kb_ctx {
     std::map<kb::u32, kb::u64> fix_hint;  // head predicate -> facts it held when the last fixpoint ended (sizes the next run's known-fact sets)
     std::shared_ptr<void> fix_state;      // kb_datalog_fixpoint_seed: the per-predicate relations and known-fact sets of the last seeded
                                           // call (kb_datalog.cu: FixState), valid while store_version is the one it was left at
+    std::shared_ptr<void> closed;         // kb_datalog_fixpoint / kb_datalog_maintain: the store is closed under the rules (kb_datalog.cu:
+                                          // Closed), valid while store_version / num_version are the ones recorded; kb_datalog_maintain's kept state
     std::set<std::pair<kb::u32, kb::u32>> multi_valued;
     std::set<std::pair<kb::u32, kb::u32>> single_valued;  // verified duplicate-free by an earlier direct build on this store version
     cudaStream_t st2 = nullptr;                            // second compute stream: independent direct builds run concurrently

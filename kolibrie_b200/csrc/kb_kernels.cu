@@ -2744,6 +2744,47 @@ void launch_set64_insert(u64* set, u32 set_slots, const u32* s, const u32* o, u3
     set64_insert_kernel<<<grid, 256, 0, st>>>(set, set_slots, s, o, n, overflow);
 }
 
+// slot of (s,o) in a 64-bit set, EMPTY32 when absent (the set is not written by the same launch)
+__device__ __forceinline__ u32 set64_find(const u64* set, u32 n_slots, u32 s, u32 o) {
+    const u64 key = ((u64)s << 32) | (u64)o;
+    const u32 mask = n_slots - 1u;
+    u32 slot = mix32(mix32(s) * 0x9E3779B1u ^ mix32(o + 0x632BE5ABu)) & mask;
+    for (u32 probes = 0; probes < n_slots; probes++) {
+        const u64 cur = set[slot];
+        if (cur == key) return slot;
+        if (cur == EMPTY64) return EMPTY32;
+        slot = (slot + 1u) & mask;
+    }
+    return EMPTY32;
+}
+// set64_insert that returns the key's slot (EMPTY32: table full); *claimed = this call took a free slot for the key
+__device__ __forceinline__ u32 set64_insert_slot(u64* set, u32 n_slots, u32 s, u32 o, bool* claimed) {
+    const u64 key = ((u64)s << 32) | (u64)o;
+    const u32 mask = n_slots - 1u;
+    u32 slot = mix32(mix32(s) * 0x9E3779B1u ^ mix32(o + 0x632BE5ABu)) & mask;
+    *claimed = false;
+    for (u32 probes = 0; probes < n_slots; probes++) {
+        const u64 cur = *reinterpret_cast<volatile u64*>(&set[slot]);
+        if (cur == key) return slot;
+        if (cur == EMPTY64) {
+            const u64 old = atomicCAS(reinterpret_cast<unsigned long long*>(&set[slot]), (unsigned long long)EMPTY64, (unsigned long long)key);
+            if (old == EMPTY64) { *claimed = true; return slot; }
+            if (old == key) return slot;
+        }
+        slot = (slot + 1u) & mask;
+    }
+    return EMPTY32;
+}
+// kb_datalog_maintain's acceptance test in front of the dedup: member of the gate set, no positive count in the veto table
+__device__ __forceinline__ bool derive_gate_pass(const DeriveParams& P, u32 s, u32 o) {
+    if (P.gate_set && set64_find(P.gate_set, P.gate_slots, s, o) == EMPTY32) return false;
+    if (P.veto_keys) {
+        const u32 slot = set64_find(P.veto_keys, P.veto_slots, s, o);
+        if (slot != EMPTY32 && P.veto_cnt[slot] > 0u) return false;
+    }
+    return true;
+}
+
 __device__ __forceinline__ bool rule_filters_pass(const DeriveParams& P, u32 i) {
     for (u32 f = 0; f < P.n_filt; f++) {
         const RuleFilterDev fl = P.filt[f];
@@ -2769,6 +2810,7 @@ __device__ __forceinline__ bool rule_filters_pass(const DeriveParams& P, u32 i) 
     return true;
 }
 
+template <bool GATED>
 __global__ void __launch_bounds__(256) derive_kernel(const __grid_constant__ DeriveParams P) {
     const int lane = threadIdx.x & 31;
     const u32 stride = gridDim.x * blockDim.x;
@@ -2786,6 +2828,9 @@ __global__ void __launch_bounds__(256) derive_kernel(const __grid_constant__ Der
         if (pass) {
             s = P.head_s.is_var ? P.bcol[P.head_s.value][i] : P.head_s.value;
             o = P.head_o.is_var ? P.bcol[P.head_o.value][i] : P.head_o.value;
+            if (GATED && !derive_gate_pass(P, s, o)) pass = false;
+        }
+        if (pass) {
             const u32 r = set64_insert(P.set, P.set_slots, s, o);
             if (r == 2u) atomicMax(P.overflow, 1u);
             fresh = r == 1u;
@@ -3023,7 +3068,123 @@ void launch_derive_partitioned(const DerivePartParams& p, int n_sms, cudaStream_
 void launch_derive(const DeriveParams& p, int n_sms, cudaStream_t st) {
     if (p.n == 0) return;
     int grid = (int)umin64((u64)n_sms * 8ull, ((u64)p.n + 255ull) / 256ull);
-    derive_kernel<<<grid, 256, 0, st>>>(p);
+    if (p.gate_set || p.veto_keys) derive_kernel<true><<<grid, 256, 0, st>>>(p);
+    else derive_kernel<false><<<grid, 256, 0, st>>>(p);
+}
+
+// ---- kb_datalog_maintain: base multiplicities, selection by set membership, erasure
+__device__ __forceinline__ void emit_pair(bool take, u32 s, u32 o, u32* out_s, u32* out_o, u32* out_count) {  // warp-aggregated append
+    const int lane = threadIdx.x & 31;
+    const unsigned b = __ballot_sync(0xffffffffu, take);
+    if (!b) return;
+    u32 basepos = 0;
+    if (lane == __ffs(b) - 1) basepos = atomicAdd(out_count, (u32)__popc(b));
+    basepos = __shfl_sync(0xffffffffu, basepos, __ffs(b) - 1);
+    if (take) {
+        const u32 r = basepos + (u32)__popc(b & ((1u << lane) - 1u));
+        out_s[r] = s;
+        out_o[r] = o;
+    }
+}
+
+__global__ void __launch_bounds__(256) base_count_kernel(const __grid_constant__ BaseCountParams P) {
+    const u32 stride = gridDim.x * blockDim.x;
+    const u32 n_round = (P.n + 31u) & ~31u;
+    u32 n_edges = 0, n_claimed = 0;  // (counted here when nothing is emitted)
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += stride) {
+        bool edge = false;  // this row moved the count across zero
+        u32 s = 0, o = 0;
+        if (i < P.n) {
+            s = P.s[i];
+            o = P.o[i];
+            if (P.delta > 0) {
+                bool claimed = false;
+                const u32 slot = set64_insert_slot(P.keys, P.slots, s, o, &claimed);
+                if (slot == EMPTY32) *P.overflow = 1u;
+                else edge = atomicAdd(&P.cnt[slot], 1u) == 0u;
+                n_claimed += claimed ? 1u : 0u;
+            } else {
+                const u32 slot = set64_find(P.keys, P.slots, s, o);
+                if (slot != EMPTY32) edge = atomicSub(&P.cnt[slot], 1u) == 1u;
+            }
+        }
+        if (P.out_s) emit_pair(edge, s, o, P.out_s, P.out_o, P.out_count);
+        else n_edges += edge ? 1u : 0u;
+    }
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+        n_edges += __shfl_xor_sync(0xffffffffu, n_edges, d);
+        n_claimed += __shfl_xor_sync(0xffffffffu, n_claimed, d);
+    }
+    if ((threadIdx.x & 31) == 0) {
+        if (n_edges) atomicAdd(P.out_count, n_edges);
+        if (n_claimed) atomicAdd(P.claimed, n_claimed);
+    }
+}
+void launch_base_count(const BaseCountParams& p, int n_sms, cudaStream_t st) {
+    if (p.n == 0) return;
+    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)p.n + 255ull) / 256ull);
+    base_count_kernel<<<grid, 256, 0, st>>>(p);
+}
+
+__global__ void __launch_bounds__(256) base_count_rehash_kernel(const u64* okeys, const u32* ocnt, u32 oslots, u64* nkeys, u32* ncnt, u32 nslots,
+                                                                u32* n_live, u32* overflow) {
+    const u32 stride = gridDim.x * blockDim.x;
+    u32 moved = 0;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < oslots; i += stride) {
+        const u64 k = okeys[i];
+        const u32 c = ocnt[i];
+        if (k == EMPTY64 || c == 0u) continue;
+        bool claimed = false;
+        const u32 slot = set64_insert_slot(nkeys, nslots, (u32)(k >> 32), (u32)k, &claimed);
+        if (slot == EMPTY32) { *overflow = 1u; continue; }
+        ncnt[slot] = c;  // keys are distinct: one writer per slot
+        moved++;
+    }
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) moved += __shfl_xor_sync(0xffffffffu, moved, d);
+    if ((threadIdx.x & 31) == 0 && moved) atomicAdd(n_live, moved);
+}
+void launch_base_count_rehash(const u64* okeys, const u32* ocnt, u32 oslots, u64* nkeys, u32* ncnt, u32 nslots, u32* n_live, u32* overflow, int n_sms,
+                              cudaStream_t st) {
+    if (oslots == 0) return;
+    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)oslots + 255ull) / 256ull);
+    base_count_rehash_kernel<<<grid, 256, 0, st>>>(okeys, ocnt, oslots, nkeys, ncnt, nslots, n_live, overflow);
+}
+
+__global__ void __launch_bounds__(256) pair_select_kernel(const __grid_constant__ PairSelectParams P) {
+    const u32 stride = gridDim.x * blockDim.x;
+    const u32 n_round = (P.n + 31u) & ~31u;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += stride) {
+        bool take = false;
+        u32 s = 0, o = 0;
+        if (i < P.n) {
+            s = P.s[i];
+            o = P.o[i];
+            const u32 slot = set64_find(P.keys, P.slots, s, o);
+            const bool present = slot != EMPTY32 && (!P.cnt || P.cnt[slot] > 0u);
+            take = present == (P.keep_present != 0u);
+        }
+        emit_pair(take, s, o, P.out_s, P.out_o, P.out_count);
+    }
+}
+void launch_pair_select(const PairSelectParams& p, int n_sms, cudaStream_t st) {
+    if (p.n == 0) return;
+    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)p.n + 255ull) / 256ull);
+    pair_select_kernel<<<grid, 256, 0, st>>>(p);
+}
+
+__global__ void __launch_bounds__(256) set64_erase_kernel(u64* set, u32 set_slots, const u32* s, const u32* o, u32 n) {
+    const u32 stride = gridDim.x * blockDim.x;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        const u32 slot = set64_find(set, set_slots, s[i], o[i]);
+        if (slot != EMPTY32) set[slot] = TOMB64;
+    }
+}
+void launch_set64_erase(u64* set, u32 set_slots, const u32* s, const u32* o, u32 n, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull);
+    set64_erase_kernel<<<grid, 256, 0, st>>>(set, set_slots, s, o, n);
 }
 
 // =================================================================================================================

@@ -426,6 +426,13 @@ struct DeriveParams {
     u32* out_count;               // appended so far (atomic cursor)
     unsigned long long* n_deriv;  // candidates that passed the filters
     u32* overflow;                // 1: set or output full (error); 2: budget reached, the host grows the set and runs the launch again
+    // kb_datalog_maintain (delete-and-rederive): a candidate takes part in the dedup only if it is a member of gate_set (when non-null)
+    // and has no positive count in the veto table (when non-null). Gated launches never take the partitioned path.
+    const u64* gate_set;
+    u32 gate_slots;
+    const u64* veto_keys;
+    const u32* veto_cnt;
+    u32 veto_slots;
 };
 void launch_derive(const DeriveParams& p, int n_sms, cudaStream_t st);
 // RADIX-PARTITIONED candidate dedup (the same work as launch_derive for large candidate sets). The known-fact set is an open-addressing
@@ -447,6 +454,44 @@ void launch_derive_partitioned(const DerivePartParams& p, int n_sms, cudaStream_
 void launch_set64_insert(u64* set, u32 set_slots, const u32* s, const u32* o, u32 n, u32* overflow, int n_sms, cudaStream_t st);
 void launch_set_insert(uint4* set, u32 set_slots, const u32* s, const u32* p /*null: p_const*/, u32 p_const, const u32* o, u32 n, u32* overflow,
                        int n_sms, cudaStream_t st);
+
+// ---- delete-and-rederive maintenance of a closed store (kb_datalog_maintain)
+// An erased key of a 64-bit (s,o) set: lookups walk past it, inserts never reuse it (s = KB_ID_NONE is never a fact). The set is rebuilt
+// from its relation when it fills up, which drops the tombstones.
+constexpr u64 TOMB64 = 0xFFFFFFFFFFFFFFFEull;
+// base multiplicity of a predicate's facts: a 64-bit (s,o) key table and a parallel u32 count per slot (a key whose count is 0 is not a
+// base fact; it keeps its slot until the table is rehashed)
+struct BaseCountParams {
+    u64* keys;
+    u32* cnt;
+    u32 slots;  // power of two
+    const u32 *s, *o;
+    u32 n;
+    int delta;  // +1: the rows join the base (a count that leaves 0 emits the fact), -1: they leave it (a count that reaches 0 emits it)
+    u32 *out_s, *out_o;  // nullable: no emission (the facts that crossed zero are then only counted)
+    u32* out_count;      // facts that crossed zero
+    u32* claimed;        // keys that took a free slot of the table
+    u32* overflow;       // 1: key table full
+};
+void launch_base_count(const BaseCountParams& p, int n_sms, cudaStream_t st);
+// live entries (count > 0) of one count table into an empty larger one; *n_live += entries moved
+void launch_base_count_rehash(const u64* okeys, const u32* ocnt, u32 oslots, u64* nkeys, u32* ncnt, u32 nslots, u32* n_live, u32* overflow, int n_sms,
+                              cudaStream_t st);
+// rows (s,o) whose presence in a 64-bit set equals keep_present go to out (warp-aggregated compaction, order not kept). With `cnt` the
+// set is a count table and a key is present only with a positive count.
+struct PairSelectParams {
+    const u32 *s, *o;
+    u32 n;
+    const u64* keys;
+    const u32* cnt;
+    u32 slots;
+    u32 keep_present;
+    u32 *out_s, *out_o;
+    u32* out_count;
+};
+void launch_pair_select(const PairSelectParams& p, int n_sms, cudaStream_t st);
+// the keys (s,o) of the rows become TOMB64 in the set (keys that are not there are ignored)
+void launch_set64_erase(u64* set, u32 set_slots, const u32* s, const u32* o, u32 n, int n_sms, cudaStream_t st);
 
 // fused partition + transfer of the multi-GPU join-key shuffle: a tile of rows is sorted by destination rank d = shard_of(key, n_parts)
 // in shared memory, one range per (tile, destination) is reserved with an atomicAdd on *cursor_ptrs[d] — the destination's own cursor

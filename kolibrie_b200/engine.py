@@ -653,6 +653,144 @@ class Reasoner:
         return [tuple(int(cols[k][i]) if fixed[k] is None else fixed[k] for k in range(3)) for i in range(n)]
 
 
+class SimpleR2R:
+    """rsp/simple_r2r.rs over the device store, the host-side window a stream engine drives: a firing is remove(previous window) +
+    add(current window) + materialize() + execute_query(op) (rsp_engine.rs:94-109). The adds of one firing become ONE store segment tagged
+    with the firing number; a segment is evicted when all of its triples have left the window (so the store index is maintained, not
+    rebuilt). materialize(): the first time, and whenever the rules changed or the store was changed outside it, the inferred segment is
+    evicted and kb_datalog_fixpoint closes the window; from then on ONE kb_datalog_maintain per firing moves the closure by the slide
+    (delete-and-rederive) instead of recomputing it. Triples are dictionary id tuples (s, p, o) of `item.dictionary`.
+
+    Divergence from the reference (quirk Q11): SimpleR2R::materialize deletes the previous firing's derived triples AFTER the firing's
+    adds (simple_r2r.rs:103-108), so a streamed triple equal to a previously derived one is missing from that firing's store; here it is
+    kept (the relational answer)."""
+
+    def __init__(self, ctx: Optional[c.Context] = None, device: int = 0, strategy: int = c.SEMI_NAIVE):
+        self.item = SparqlDatabase(ctx, device)  # the window's base triples (host set) + dictionary; the device store holds segments
+        self.ctx = self.item.ctx
+        self.rules: List[Rule] = []
+        self.strategy = strategy
+        self.derived: set = set()       # the inferred segment, mirrored on the host
+        self.last_stats = None          # KbFixpointStats or KbMaintainStats of the last materialize()
+        self.last_mode: Optional[str] = None  # "fixpoint" / "maintain"
+        self._pending: List[Tuple[int, int, int]] = []  # adds of the current firing, not on the device yet
+        self._pending_set: set = set()
+        self._evicted: List[int] = []   # segments whose triples all left the window, not evicted on the device yet
+        self._firing = 1
+        self._tag_of: Dict[Tuple[int, int, int], int] = {}
+        self._live: Dict[int, int] = {}  # tag -> triples of that segment still in the window
+        self._closed_sig: Optional[str] = None  # the rules the device store is closed under (None: not closed)
+        self._numeric_ids = -1          # dictionary size of the numeric table on the device
+        self._strings_ids = -1
+
+    def add_reasoning_rules(self, rules: Sequence[Rule]):
+        self.rules.extend(rules)
+
+    def add(self, t: Tuple[int, int, int]):
+        t = tuple(int(x) for x in t)
+        self.item.add_triple(t)
+        if t in self._tag_of or t in self._pending_set:  # already in the window (the reference's store is a set)
+            return
+        self._pending.append(t)
+        self._pending_set.add(t)
+
+    def remove(self, t: Tuple[int, int, int]):
+        t = tuple(int(x) for x in t)
+        self.item.delete_triple(t)
+        if t in self._pending_set:
+            self._pending_set.discard(t)
+            self._pending.remove(t)
+            return
+        tag = self._tag_of.pop(t, None)
+        if tag is None:
+            return
+        self._live[tag] -= 1
+        if self._live[tag] == 0:  # the whole slide left the window
+            del self._live[tag]
+            self._evicted.append(tag)
+
+    def _commit_pending(self):
+        if self._pending:
+            self._live[self._firing] = len(self._pending)
+            for t in self._pending:
+                self._tag_of[t] = self._firing
+        self._pending, self._pending_set = [], set()
+        self._firing += 1
+
+    def _flush(self):
+        """the window's changes as plain segment operations (no rules involved): the store is no longer closed"""
+        for tag in self._evicted:
+            self.ctx.store_evict(tag)
+            self._closed_sig = None
+        self._evicted = []
+        if self._pending:
+            a = np.array(self._pending, dtype=np.uint32).reshape(-1, 3)
+            self.ctx.store_append(a[:, 0], a[:, 1], a[:, 2], self._firing)
+            self._commit_pending()
+            self._closed_sig = None
+
+    def _signature(self) -> str:
+        return repr([(r.premise, r.conclusion, r.filters) for r in self.rules])
+
+    def _load_tables(self):
+        """the dictionary's numeric and string tables on the device when it grew (FILTERs of rules and queries read the first; loading
+        it voids the closed token only when a rule filter compares numbers)"""
+        n = len(self.item.dictionary.id_to_string)
+        if n != self._numeric_ids:
+            num, isn = self.item.dictionary.numeric_table()
+            self.ctx.dict_numeric_load(num, isn)
+            self._numeric_ids = n
+        if n != self._strings_ids:
+            self.ctx.dict_strings_load(self.item.dictionary.id_to_string)
+            self._strings_ids = n
+
+    def materialize(self) -> List[Tuple[int, int, int]]:
+        """the closure of the current window's triples beyond them (simple_r2r.rs:103-128), sorted"""
+        if not self.rules:
+            self._flush()
+            return []
+        self._load_tables()
+        rules = [compile_rule(r) for r in self.rules]
+        sig = self._signature()
+        done = False
+        if self._closed_sig == sig:
+            add = np.array(self._pending, dtype=np.uint32).reshape(-1, 3) if self._pending else None
+            try:
+                gone, new, st = self.ctx.datalog_maintain(rules, list(self._evicted), add, self._firing, self.strategy)
+                done = True
+            except c.KolibrieError as e:
+                if e.status != c.KB_E_INVALID:  # (INVALID: the token is void — a numeric table that a rule filter reads was reloaded)
+                    raise
+                self._closed_sig = None
+        if done:
+            self._evicted = []
+            if self._pending:
+                self._commit_pending()
+            self.derived.difference_update(map(tuple, gone.to_numpy([0, 1, 2]).tolist()))
+            self.derived.update(map(tuple, new.to_numpy([0, 1, 2]).tolist()))
+            self.last_mode = "maintain"
+        else:
+            self._flush()
+            try:
+                self.ctx.store_evict(c.KB_TAG_INFERRED)
+            except c.KolibrieError as e:
+                if e.status != c.KB_E_NOT_FOUND:
+                    raise
+            rel, st = self.ctx.datalog_fixpoint(rules, self.strategy)
+            self.derived = set(map(tuple, rel.to_numpy([0, 1, 2]).tolist()))
+            self._closed_sig = sig
+            self.last_mode = "fixpoint"
+        self.last_stats = st
+        return sorted(self.derived)
+
+    def execute_query(self, op) -> List[Dict[str, str]]:
+        """ExecutionEngine over the window (its base triples and, after materialize(), the inferred ones)"""
+        self._flush()
+        self._load_tables()
+        self.item._uploaded_version = self.item._version  # the device store is maintained segment by segment, never reloaded from the set
+        return ExecutionEngine.execute(op, self.item)
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # The LEGACY executor's BGP + FILTER stage (kolibrie/src/execute_query.rs:151-341 — the path `execute_query` takes: CLI, criterion bench,
 # README): patterns are joined one by one by perform_join_par_simd_with_strict_filter_1 (sparql_database.rs:2056-2213) over rows of

@@ -26,6 +26,9 @@ pub const KB_TAG_INFERRED: u64 = 0xFFFF_FFFF_FFFF_FFF0;
     pub filter_launches: u64, pub group_launches: u64, pub other_launches: u64, pub rows_scanned: u64, pub rows_built: u64, pub rows_probed: u64,
     pub rows_out: u64, pub h2d_bytes: u64, pub d2h_bytes: u64, pub kernel_launches: u64, pub fused_scan_builds: u64, pub index_joins: u64 }
 #[repr(C)] pub struct KbFixpointStats { pub rounds: u32, pub inferred: u64, pub derivations: u64, pub round_new: [u64; 64], pub device_ms: c_double }
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbMaintainStats { pub base_removed: u64, pub base_added: u64, pub overdeleted: u64, pub rederived: u64,
+    pub inferred_removed: u64, pub inferred_added: u64, pub derivations: u64, pub overdelete_rounds: u32, pub insert_rounds: u32, pub device_ms: c_double }
+pub type kb_maintain_stats = KbMaintainStats;  // (the header's name, as the declaration below spells it)
 
 // kb_filter_opcode / kb_cmp / kb_agg_kind / kb_strategy
 pub const KB_F_CMP_NUM: u32 = 1; pub const KB_F_EQ_ID: u32 = 2; pub const KB_F_NE_ID: u32 = 3; pub const KB_F_AND: u32 = 4; pub const KB_F_OR: u32 = 5;
@@ -91,6 +94,9 @@ extern "C" {
     // incremental: the store is closed under the rules already, `seed` (s, p, o) are the triples added since
     pub fn kb_datalog_fixpoint_seed(ctx: *mut KbCtx, rules: *const KbRule, n: u32, strategy: u32, seed: *const KbRel, out: *mut *mut KbRel, n_seed_new: *mut u64,
                                     stats: *mut KbFixpointStats) -> kb_status;
+    // delete-and-rederive across a window slide: the store is closed under the rules (the last fixpoint / maintain with the same rules)
+    pub fn kb_datalog_maintain(ctx: *mut KbCtx, rules: *const KbRule, n: u32, strategy: u32, evict_tags: *const u64, n_evict: u32, add: *const KbRel,
+                               add_tag: u64, inferred_removed: *mut *mut KbRel, inferred_added: *mut *mut KbRel, stats: *mut kb_maintain_stats) -> kb_status;
     // multi-GPU helpers
     pub fn kb_shard_of(key: u32, n_shards: u32) -> u32;
     pub fn kb_set_sharding(ctx: *mut KbCtx, rank: u32, world: u32) -> kb_status;

@@ -29,6 +29,9 @@ pub struct DeviceStore {
     synced_triples: usize,
     synced_dict: usize,
     indexed: bool,
+    /// the store is maintained segment by segment by its owner (GpuR2R: one segment per firing, the inferred segment): `sync` then
+    /// mirrors the dictionary only and never replaces the store with `database.triples`
+    pub segmented: bool,
 }
 unsafe impl Send for DeviceStore {}
 
@@ -39,7 +42,7 @@ impl DeviceStore {
         if rc != KB_OK {
             return Err(unsafe { CStr::from_ptr(kb_last_error(ptr::null())) }.to_string_lossy().into_owned());
         }
-        Ok(Self { ctx, synced_triples: usize::MAX, synced_dict: usize::MAX, indexed: false })
+        Ok(Self { ctx, synced_triples: usize::MAX, synced_dict: usize::MAX, indexed: false, segmented: false })
     }
 
     pub fn last_error(&self) -> String {
@@ -66,7 +69,7 @@ impl DeviceStore {
             if unsafe { kb_dict_strings_load(self.ctx, offs.as_ptr(), bytes.as_ptr(), n as u32) } != KB_OK { return Err(self.last_error()); }
             self.synced_dict = n;
         }
-        if database.triples.len() != self.synced_triples {
+        if !self.segmented && database.triples.len() != self.synced_triples {
             let n = database.triples.len();
             let (mut s, mut p, mut o) = (Vec::with_capacity(n), Vec::with_capacity(n), Vec::with_capacity(n));
             for t in database.triples.iter() { s.push(t.subject); p.push(t.predicate); o.push(t.object); }

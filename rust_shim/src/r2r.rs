@@ -2,36 +2,116 @@
 //! `execute_query(plan)` (rsp_engine.rs:94-109; simple_r2r.rs:95-142). The adds of one firing become ONE store segment tagged with the
 //! firing number, the removes evict the segment of the firing they were added in; the store index is maintained across both (one chunk
 //! per segment), so that the per-slide query keeps the one-kernel index path.
+//!
+//! Rules run on the device. The first firing evicts the inferred segment and runs `kb_datalog_fixpoint` over the window; from then on
+//! the store is closed under the rules and every firing is ONE `kb_datalog_maintain` call (the segments that left the window, the
+//! firing's adds): delete-and-rederive from the slide instead of a closure from scratch per firing (simple_r2r.rs:103-128).
+//!
+//! The device store is this operator's: `DeviceStore::segmented` keeps `execute_query` from replacing it with `inner.item.triples`
+//! (which would drop the firing tags and the inferred segment); the dictionary's tables are still mirrored before every firing and query
+//! (a numeric-table load voids the closed token only when a rule filter compares numbers). The derived triples are mirrored into
+//! `inner.item`, so the host's query path (shapes the device does not take) sees them too.
 use crate::ffi::*;
+use crate::reasoner::compile_rule;
 use crate::{try_execute, DeviceStore};
 use kolibrie::rsp::r2r::{AsAnyMut, R2ROperator};
 use kolibrie::rsp::simple_r2r::SimpleR2R;
 use kolibrie::streamertail_optimizer::PhysicalOperator;
 use shared::triple::Triple;
 use std::any::Any;
-use std::collections::HashMap;
+use std::collections::{HashMap, HashSet};
+use std::ptr;
 
 pub struct GpuR2R {
     pub inner: SimpleR2R,       // parsing, rules, dictionary: unchanged host logic
     pub dev: DeviceStore,
     pending: Vec<Triple>,       // adds of the current firing, not yet on the device
+    evicted: Vec<u64>,          // segments whose triples all left the window since the last firing, not yet evicted on the device
     firing: u64,
     tag_of: HashMap<Triple, u64>,
     live: HashMap<u64, usize>,  // tag -> triples of that segment still in the window
+    closed: bool,               // the device store is closed under the rules (the last materialize succeeded, nothing changed since)
+    derived: HashSet<Triple>,   // the inferred segment, mirrored on the host (what materialize returns)
+}
+
+fn triples_of(dev: &DeviceStore, rel: *mut KbRel) -> Vec<Triple> {
+    let mut n = 0u64;
+    unsafe { kb_rel_info(rel, &mut n, ptr::null_mut(), ptr::null_mut()) };
+    let mut cols = [vec![0u32; n as usize], vec![0u32; n as usize], vec![0u32; n as usize]];
+    for c in 0..3 { unsafe { kb_rel_download(dev.ctx, rel, c as u32, cols[c].as_mut_ptr()) }; }
+    unsafe { kb_rel_free(dev.ctx, rel) };
+    (0..n as usize).map(|i| Triple { subject: cols[0][i], predicate: cols[1][i], object: cols[2][i] }).collect()
 }
 
 impl GpuR2R {
     pub fn new(inner: SimpleR2R, device: i32) -> Result<Self, String> {
-        Ok(Self { inner, dev: DeviceStore::new(device)?, pending: Vec::new(), firing: 1, tag_of: HashMap::new(), live: HashMap::new() })
+        let mut dev = DeviceStore::new(device)?;
+        dev.segmented = true;
+        Ok(Self { inner, dev, pending: Vec::new(), evicted: Vec::new(), firing: 1, tag_of: HashMap::new(), live: HashMap::new(),
+                  closed: false, derived: HashSet::new() })
     }
-    fn flush(&mut self) {
-        if self.pending.is_empty() { return; }
-        let (s, p, o): (Vec<u32>, Vec<u32>, Vec<u32>) = (self.pending.iter().map(|t| t.subject).collect(), self.pending.iter().map(|t| t.predicate).collect(),
-                                                         self.pending.iter().map(|t| t.object).collect());
-        unsafe { kb_store_append(self.dev.ctx, s.as_ptr(), p.as_ptr(), o.as_ptr(), s.len() as u64, self.firing) };
+    /// the derived triples as the device now holds them, mirrored into the host database (a derived triple that is also a live streamed
+    /// triple stays there when it stops being derived: Q11)
+    fn set_derived(&mut self, gone: Vec<Triple>, new: Vec<Triple>) {
+        let pending: HashSet<&Triple> = self.pending.iter().collect();
+        for t in gone {
+            self.derived.remove(&t);
+            if !self.tag_of.contains_key(&t) && !pending.contains(&t) { self.inner.item.delete_triple(&t); }
+        }
+        for t in new { self.inner.item.add_triple(t.clone()); self.derived.insert(t); }
+    }
+    fn columns(&self) -> (Vec<u32>, Vec<u32>, Vec<u32>) {
+        (self.pending.iter().map(|t| t.subject).collect(), self.pending.iter().map(|t| t.predicate).collect(), self.pending.iter().map(|t| t.object).collect())
+    }
+    fn commit_pending(&mut self) {
         self.live.insert(self.firing, self.pending.len());
         for t in self.pending.drain(..) { self.tag_of.insert(t, self.firing); }
         self.firing += 1;
+    }
+    /// the window's changes go to the store as plain segment operations (no rules involved): the store is no longer closed
+    fn flush(&mut self) {
+        for tag in self.evicted.drain(..) { unsafe { kb_store_evict(self.dev.ctx, tag) }; self.closed = false; }
+        if self.pending.is_empty() { return; }
+        let (s, p, o) = self.columns();
+        unsafe { kb_store_append(self.dev.ctx, s.as_ptr(), p.as_ptr(), o.as_ptr(), s.len() as u64, self.firing) };
+        self.commit_pending();
+        self.closed = false;
+    }
+    /// one firing's maintenance: Some(()) when the device did it, None when the rules need the host (quoted-triple terms, unsupported shapes)
+    fn maintain(&mut self, kr: &[KbRule]) -> Option<()> {
+        let ctx = self.dev.ctx;
+        let (s, p, o) = self.columns();
+        let mut add: *mut KbRel = ptr::null_mut();
+        let slots = [0u32, 1, 2];
+        let cols = [s.as_ptr(), p.as_ptr(), o.as_ptr()];
+        if !self.pending.is_empty() && unsafe { kb_rel_from_host(ctx, slots.as_ptr(), 3, cols.as_ptr(), s.len() as u64, &mut add) } != KB_OK { return None; }
+        let (mut gone, mut new): (*mut KbRel, *mut KbRel) = (ptr::null_mut(), ptr::null_mut());
+        let mut st = KbMaintainStats::default();
+        let rc = unsafe { kb_datalog_maintain(ctx, kr.as_ptr(), kr.len() as u32, KB_SEMI_NAIVE, self.evicted.as_ptr(), self.evicted.len() as u32, add, self.firing,
+                                              &mut gone, &mut new, &mut st) };
+        if !add.is_null() { unsafe { kb_rel_free(ctx, add) }; }
+        if rc != KB_OK {
+            // a failure while the store was being rewritten may have stored `add` under this firing's tag already: the fallback's
+            // flush appends the pending triples again, so that segment goes first (KB_E_NOT_FOUND when it was not stored)
+            unsafe { kb_store_evict(ctx, self.firing) };
+            return None;
+        }
+        self.evicted.clear();
+        let (gone, new) = (triples_of(&self.dev, gone), triples_of(&self.dev, new));
+        self.set_derived(gone, new);
+        if !self.pending.is_empty() { self.commit_pending(); }
+        Some(())
+    }
+    fn fixpoint(&mut self, kr: &[KbRule]) -> Option<()> {
+        self.flush();
+        unsafe { kb_store_evict(self.dev.ctx, KB_TAG_INFERRED) };
+        let mut rel: *mut KbRel = ptr::null_mut();
+        let mut st = std::mem::MaybeUninit::<KbFixpointStats>::zeroed();
+        if unsafe { kb_datalog_fixpoint(self.dev.ctx, kr.as_ptr(), kr.len() as u32, KB_SEMI_NAIVE, &mut rel, st.as_mut_ptr()) } != KB_OK { return None; }
+        let gone: Vec<Triple> = self.derived.iter().cloned().collect();
+        let new = triples_of(&self.dev, rel);
+        self.set_derived(gone, new);
+        Some(())
     }
 }
 
@@ -39,21 +119,41 @@ impl AsAnyMut for GpuR2R { fn as_any_mut(&mut self) -> &mut dyn Any { self } }
 
 impl R2ROperator<Triple, Vec<(String, String)>, Vec<(String, String)>> for GpuR2R {
     fn load_triples(&mut self, data: &str, syntax: String) -> Result<(), String> { self.inner.load_triples(data, syntax) }
-    fn load_rules(&mut self, data: &str) -> Result<(), &'static str> { self.inner.load_rules(data) }
+    fn load_rules(&mut self, data: &str) -> Result<(), &'static str> { self.closed = false; self.inner.load_rules(data) }
     fn add(&mut self, data: Triple) { self.inner.add(data.clone()); self.pending.push(data); }
     fn remove(&mut self, data: &Triple) {
         self.inner.remove(data);
         if let Some(tag) = self.tag_of.remove(data) {
             let left = self.live.get_mut(&tag).map(|n| { *n -= 1; *n }).unwrap_or(0);
-            if left == 0 { self.live.remove(&tag); unsafe { kb_store_evict(self.dev.ctx, tag) }; }  // the whole slide left the window
+            if left == 0 { self.live.remove(&tag); self.evicted.push(tag); }  // the whole slide left the window
         }
     }
     fn materialize(&mut self) -> Vec<Triple> {
-        self.flush();
-        // rules on the device: kb_datalog_fixpoint over the live window; the inferred segment is dropped before the next firing
-        // (SimpleR2R re-materialises from scratch, simple_r2r.rs:103-128). Rule compilation: reasoner.rs::compile_rule.
-        unsafe { kb_store_evict(self.dev.ctx, KB_TAG_INFERRED) };
-        self.inner.materialize()
+        if self.inner.rules.is_empty() { self.flush(); return Vec::new(); }
+        if self.dev.sync(&self.inner.item).is_err() { self.closed = false; }  // the dictionary's tables (the store itself is ours)
+        let compiled: Option<Vec<_>> = self.inner.rules.iter().map(compile_rule).collect();
+        let done = compiled.as_ref().and_then(|compiled| {
+            let kr: Vec<KbRule> = compiled.iter().map(|(pr, fl, co)| KbRule { premise: pr.as_ptr(), n_premise: pr.len() as u32, filters: fl.as_ptr(),
+                n_filters: fl.len() as u32, conclusion: co.as_ptr(), n_conclusion: co.len() as u32 }).collect();
+            // the first firing (or the first after a plain store change): evict the inferred segment, closure from scratch; then DRed
+            let r = if self.closed { self.maintain(&kr).or_else(|| self.fixpoint(&kr)) } else { self.fixpoint(&kr) };
+            self.closed = r.is_some();
+            r
+        });
+        if done.is_none() {  // rules the device does not take: the host's SimpleR2R materialises (simple_r2r.rs:103-128)
+            self.flush();
+            unsafe { kb_store_evict(self.dev.ctx, KB_TAG_INFERRED) };
+            let old: Vec<Triple> = self.derived.drain().collect();
+            for t in old { if !self.tag_of.contains_key(&t) { self.inner.item.delete_triple(&t); } }
+            let derived = self.inner.materialize();
+            // the device store holds what the host derived, as its inferred segment, for the device query path
+            let (s, p, o): (Vec<u32>, Vec<u32>, Vec<u32>) = (derived.iter().map(|t| t.subject).collect(), derived.iter().map(|t| t.predicate).collect(),
+                                                             derived.iter().map(|t| t.object).collect());
+            if !derived.is_empty() { unsafe { kb_store_append(self.dev.ctx, s.as_ptr(), p.as_ptr(), o.as_ptr(), s.len() as u64, KB_TAG_INFERRED) }; }
+            self.closed = false;
+            return derived;
+        }
+        self.derived.iter().cloned().collect()
     }
     fn execute_query(&mut self, op: &PhysicalOperator) -> Vec<Vec<(String, String)>> {
         self.flush();

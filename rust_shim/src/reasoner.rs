@@ -16,7 +16,7 @@ impl<'a> GpuSemiNaiveStrategy<'a> {
 }
 
 /// `Rule` -> (patterns, filters) in slot form; FilterCondition semantics of rules.rs:133-165
-fn compile_rule(rule: &Rule) -> Option<(Vec<KbPattern>, Vec<KbRuleFilter>, Vec<KbPattern>)> {
+pub(crate) fn compile_rule(rule: &Rule) -> Option<(Vec<KbPattern>, Vec<KbRuleFilter>, Vec<KbPattern>)> {
     let mut slots = SlotMap::default();
     let prem: Option<Vec<KbPattern>> = rule.premise.iter().map(|p| slots.pattern(p)).collect();
     let conc: Option<Vec<KbPattern>> = rule.conclusion.iter().map(|p| slots.pattern(p)).collect();
