@@ -36,8 +36,6 @@ struct DeviceGuard {
     }
 };
 
-static inline size_t round256(size_t b) { return (b + 255) & ~(size_t)255; }
-
 kb_status alloc_buf(kb_ctx* ctx, size_t bytes, Buf* out) {
     auto b = std::make_shared<DevBuf>();
     b->bytes = round256(bytes) + 256;  // every column can be over-read to the next 16-byte boundary by the TMA tile loads
@@ -265,25 +263,35 @@ std::set<u32> filter_slots(const FilterProg& f) {
     return s;
 }
 
-// append `f` (slots remapped through `remap`) to the device op array, AND-ing it with what is already there
-static bool append_prog(std::vector<FilterOp>* dst, const FilterProg& f, const std::map<u32, u32>& remap) {
-    const bool had = !dst->empty();
+// AND the program `f` into `dst`
+static void and_into(FilterProg* dst, const FilterProg& f) {
+    if (f.ops.empty()) return;
+    const bool had = !dst->ops.empty();
+    dst->ops.insert(dst->ops.end(), f.ops.begin(), f.ops.end());
+    if (had) { kb_filter_op a{}; a.op = KB_F_AND; dst->ops.push_back(a); }
+}
+
+// a program over the variables `slots` as device ops: variable slots[i] is read from column i of the kernel's row, or from position
+// (*pos)[i] (0 s, 1 p, 2 o) of a pattern's triple
+static kb_status compile_prog(kb_ctx* ctx, const FilterProg& f, const std::vector<u32>& slots, std::vector<FilterOp>* ops,
+                              const std::vector<u32>* pos = nullptr) {
+    ops->clear();
     for (auto& op : f.ops) {
         FilterOp d;
         d.op = op.op; d.slot = op.slot; d.cmp = op.cmp; d.id = op.id; d.value = op.value;
         if (op_has_slot(op.op)) {
-            auto it = remap.find(op.slot);
-            if (it == remap.end()) return false;
-            d.slot = it->second;
+            bool bound = false;
+            for (size_t i = 0; i < slots.size(); i++) {
+                if (slots[i] != op.slot) continue;
+                d.slot = pos ? (*pos)[i] : (u32)i;
+                bound = true;
+            }
+            if (!bound) return fail(ctx, KB_E_INVALID, "filter uses a variable that is not bound where it is evaluated");
         }
-        dst->push_back(d);
+        ops->push_back(d);
     }
-    if (had) {
-        FilterOp a{};
-        a.op = KB_F_AND;
-        dst->push_back(a);
-    }
-    return true;
+    if (ops->size() > KB_MAX_FILTER_OPS) return fail(ctx, KB_E_LIMIT, "filter too long");
+    return KB_OK;
 }
 
 void pattern_vars(const kb_pattern& pt, std::vector<u32>* slots, std::vector<u32>* src) {
@@ -352,6 +360,15 @@ kb_status unpair_rel(kb_ctx* ctx, std::unique_ptr<kb_rel>* r) {
     return KB_OK;
 }
 
+// a relation of zero rows over `slots`
+static kb_status empty_rel(kb_ctx* ctx, const std::vector<u32>& slots, std::unique_ptr<kb_rel>* out) {
+    auto r = std::make_unique<kb_rel>();
+    r->slots = slots;
+    for (size_t c = 0; c < slots.size(); c++) { Col col; KB_TRY(alloc_col(ctx, 0, &col)); r->cols.push_back(col); }
+    *out = std::move(r);
+    return KB_OK;
+}
+
 // IndexScan proper (engine.rs:1192-1407, the 8-case lookup of index_manager.rs:253-340 for a constant predicate): with a valid store
 // index a pattern whose predicate is constant is answered from the predicate's slice — (c P ?o) from the subject table / directory,
 // (?s P c) from the object table / directory, (?s P ?o) is the slice itself — without touching the 12-byte/triple store.
@@ -362,13 +379,9 @@ static kb_status index_lookup(kb_ctx* ctx, const kb_pattern& pt, std::unique_ptr
     std::vector<u32> slots, src;
     pattern_vars(pt, &slots, &src);
     auto it = ctx->index.find(pt.p.value);
+    if (it == ctx->index.end() || it->second.n == 0) return empty_rel(ctx, slots, out);  // the predicate does not occur: empty answer
     auto rel = std::make_unique<kb_rel>();
     rel->slots = slots;
-    if (it == ctx->index.end() || it->second.n == 0) {  // the predicate does not occur: empty answer
-        for (size_t c = 0; c < slots.size(); c++) { Col col; KB_TRY(alloc_col(ctx, 0, &col)); rel->cols.push_back(col); }
-        *out = std::move(rel);
-        return KB_OK;
-    }
     const PredSlice& ps = it->second;
     if (pt.s.is_var && pt.o.is_var) {
         if (pt.s.value == pt.o.value) return KB_OK;  // ?x P ?x: the scan enforces the equality
@@ -398,11 +411,7 @@ static kb_status index_lookup(kb_ctx* ctx, const kb_pattern& pt, std::unique_ptr
     const Buf& val = by_y ? ps.yval : ps.xval;
     if (tab) {  // unique column: one table slot
         const u32 cs = by_y ? 0u : ps.tab_cshift;
-        if (cs != 0u && shard_of(key, ctx->shard_world) != ctx->shard_rank) {  // a key of another shard: not in this store
-            Col col; KB_TRY(alloc_col(ctx, 0, &col)); rel->cols.push_back(col);
-            *out = std::move(rel);
-            return KB_OK;
-        }
+        if (cs != 0u && shard_of(key, ctx->shard_world) != ctx->shard_rank) return empty_rel(ctx, slots, out);  // a key of another shard: not in this store
         const u32 o = compact_key(key, cs) - (by_y ? ps.ytab_min : ps.xtab_min);
         u32 v = EMPTY32;
         if (o < (by_y ? ps.ytab_range : ps.xtab_range)) {
@@ -535,12 +544,10 @@ kb_status scan_impl(kb_ctx* ctx, const kb_pattern* pats, u32 K, const std::vecto
         sp.f_begin = (u32)ops.size();
         sp.f_len = 0;
         if (k < pushdown.size() && !pushdown[k].ops.empty()) {
-            std::map<u32, u32> remap;
             std::vector<u32> vs, vsrc;
             pattern_vars(pt, &vs, &vsrc);
-            for (size_t i = 0; i < vs.size(); i++) remap[vs[i]] = vsrc[i];
             std::vector<FilterOp> local;
-            if (!append_prog(&local, pushdown[k], remap)) return fail(ctx, KB_E_INVALID, "pushed-down filter of pattern %u uses a variable the pattern does not bind", k);
+            KB_TRY(compile_prog(ctx, pushdown[k], vs, &local, &vsrc));
             if (ops.size() + local.size() > KB_MAX_FILTER_OPS) return fail(ctx, KB_E_LIMIT, "pushed-down filters exceed %d ops", KB_MAX_FILTER_OPS);
             ops.insert(ops.end(), local.begin(), local.end());
             sp.f_len = (u32)local.size();
@@ -633,6 +640,36 @@ kb_status scan_impl(kb_ctx* ctx, const kb_pattern* pats, u32 K, const std::vecto
 
 // ---------------------------------------------------------------------------------------------------------------
 // filter (= probe kernel with zero tables)
+
+// what every probe launch shares: the output columns (`ocs`, n rows each, appended to res->cols), the FILTER over them, tile state,
+// control words {ticket, total, zero} and a fresh epoch
+template <class Params>
+static kb_status probe_setup(kb_ctx* ctx, Params* P, u64 n, const std::vector<OutCol>& ocs, const std::vector<FilterOp>& fops, u32* ctrl,
+                             const u32* abort_flag, kb_rel* res) {
+    P->n_out = (u32)ocs.size();
+    for (u32 c = 0; c < P->n_out; c++) {
+        Col col;
+        KB_TRY(alloc_col(ctx, n, &col));
+        res->cols.push_back(col);
+        P->oc[c] = ocs[c];
+        P->out[c] = col.ptr;
+    }
+    P->cap = (u32)n;
+    P->n_ops = (u32)fops.size();
+    for (size_t i = 0; i < fops.size(); i++) P->ops[i] = fops[i];
+    P->nt = numtab(ctx);
+    KB_TRY(ensure_tile_state(ctx, P->n_tiles));
+    P->tile_state = static_cast<u64*>(ctx->tile_state->p);
+    P->block_state = static_cast<u64*>(ctx->block_state->p);
+    P->ordered = ctx->ordered;
+    P->ticket = ctrl;
+    P->total = ctrl + 1;
+    P->zero_word = ctrl + 2;
+    P->abort_flag = abort_flag;
+    P->epoch = ctx->epoch++;
+    return KB_OK;
+}
+
 kb_status filter_impl(kb_ctx* ctx, const kb_rel& in, const FilterProg& f, std::unique_ptr<kb_rel>* out) {
     auto rel = std::make_unique<kb_rel>();
     rel->slots = in.slots;
@@ -646,38 +683,18 @@ kb_status filter_impl(kb_ctx* ctx, const kb_rel& in, const FilterProg& f, std::u
     ProbeDParams P{};
     P.n_pcols = (u32)in.cols.size();
     if (P.n_pcols == 0) return fail(ctx, KB_E_UNSUPPORTED, "filter on a relation without columns");
-    P.key_col = 0;
-    P.n = (u32)in.n;
+    P.n = (u32)in.n;  // key_col 0, T = 0 tables
     P.n_tiles = (u32)((in.n + PROBE_TILE - 1) / PROBE_TILE);
-    P.T = 0;
-    P.n_out = P.n_pcols;
-    std::map<u32, u32> remap;
+    std::vector<OutCol> ocs;
     for (u32 c = 0; c < P.n_pcols; c++) {
         P.pcol[c] = in.cols[c].ptr;
-        P.oc[c] = OutCol{OUT_PROBE, c, 0};
-        Col col;
-        KB_TRY(alloc_col(ctx, in.n, &col));
-        rel->cols.push_back(col);
-        P.out[c] = col.ptr;
-        remap[in.slots[c]] = c;
+        ocs.push_back(OutCol{OUT_PROBE, c, 0});
     }
     std::vector<FilterOp> ops;
-    if (!append_prog(&ops, f, remap)) return fail(ctx, KB_E_INVALID, "filter uses a variable that is not a column of the relation");
-    P.n_ops = (u32)ops.size();
-    for (size_t i = 0; i < ops.size(); i++) P.ops[i] = ops[i];
-    P.cap = (u32)in.n;
-    P.nt = numtab(ctx);
-    KB_TRY(ensure_tile_state(ctx, P.n_tiles));
-    P.tile_state = static_cast<u64*>(ctx->tile_state->p);
-    P.block_state = static_cast<u64*>(ctx->block_state->p);
-    P.ordered = ctx->ordered;
+    KB_TRY(compile_prog(ctx, f, in.slots, &ops));
     const u32 off = ctrl_alloc(ctx, 4);
     KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, 4 * sizeof(u32), ctx->st));
-    P.ticket = ctx->ctrl + off;
-    P.total = ctx->ctrl + off + 1;
-    P.zero_word = ctx->ctrl + off + 2;
-    P.epoch = ctx->epoch++;
-    P.abort_flag = nullptr;
+    KB_TRY(probe_setup(ctx, &P, in.n, ocs, ops, ctx->ctrl + off, nullptr, rel.get()));
     timer_begin(ctx, F_FILTER);
     launch_probe_direct(P, ctx->n_sms, ctx->st);
     timer_end(ctx);
@@ -705,12 +722,7 @@ kb_status hash_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_rel& R, const Fi
         else rel->slots.push_back(s);
     }
     if (rel->slots.size() > KB_MAX_COLS) return fail(ctx, KB_E_LIMIT, "join result has more than %d columns", KB_MAX_COLS);
-    if (L.n == 0 || R.n == 0) {  // engine.rs:714-716
-        rel->n = 0;
-        for (size_t c = 0; c < rel->slots.size(); c++) { Col col; KB_TRY(alloc_col(ctx, 0, &col)); rel->cols.push_back(col); }
-        *out = std::move(rel);
-        return KB_OK;
-    }
+    if (L.n == 0 || R.n == 0) return empty_rel(ctx, rel->slots, out);  // engine.rs:714-716
     if (L.n >= 0xFFFFFFF0ull || R.n >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "relation too large");
     if (common.empty()) {  // cartesian product (engine.rs:1054-1071)
         const u64 total = L.n * R.n;
@@ -864,14 +876,10 @@ kb_status hash_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_rel& R, const Fi
         kernel_slots.push_back(B.slots[c]);
     }
     P.n_out = (u32)kernel_slots.size();
-    if (post && !post->ops.empty()) {
-        std::map<u32, u32> remap;
-        for (u32 c = 0; c < P.n_out; c++) remap[kernel_slots[c]] = c;
-        std::vector<FilterOp> ops;
-        if (!append_prog(&ops, *post, remap)) return fail(ctx, KB_E_INVALID, "join filter uses a variable that neither side binds");
-        P.n_ops = (u32)ops.size();
-        for (size_t i = 0; i < ops.size(); i++) P.ops[i] = ops[i];
-    }
+    std::vector<FilterOp> ops;
+    if (post) KB_TRY(compile_prog(ctx, *post, kernel_slots, &ops));
+    P.n_ops = (u32)ops.size();
+    for (size_t i = 0; i < ops.size(); i++) P.ops[i] = ops[i];
     P.nt = numtab(ctx);
     KB_TRY(ensure_tile_state(ctx, P.n_tiles));
     P.tile_state = static_cast<u64*>(ctx->tile_state->p);
@@ -927,622 +935,727 @@ static std::unique_ptr<kb_rel> select_cols(const kb_rel& in, const std::vector<u
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// star join: fused scan -> direct builds -> fused multiway probe; falls back to chained binary joins on 1:N keys
-kb_status star_join_impl(kb_ctx* ctx, u32 join_slot, const kb_pattern* pats, u32 K, const kb_filter_op* filter, u32 n_ops,
-                         std::unique_ptr<kb_rel>* out) {
-    return star_join_impl2(ctx, join_slot, pats, K, filter, n_ops, true, out);
-}
+// star join: five routes, tried in this order by star_join_impl
+//   R1 one-kernel index join   every build side is a persistent table of the store index: one probe_index_kernel (fused GROUP BY)
+//   R2 index join with builds  direct tables built from predicate slices, then the fused multiway probe
+//   R3 fused scan + build      the scan fills the direct tables, then the fused multiway probe
+//   R4 scan, then builds       direct tables in batches of at most MAXT per probe launch
+//   R5 chained joins           natural joins on the multimap operator: 1:N keys, quirk Q3, sparse key ranges
+struct StarQuery {  // a star join, validated once: what every route reads
+    u32 join_slot = 0, K = 0;
+    const kb_pattern* pats = nullptr;
+    std::vector<std::vector<u32>> pv, psrc;  // variables of pattern k in order of appearance, and their positions (0 s, 1 p, 2 o)
+    std::vector<u32> all_slots;              // column order of the result
+    std::vector<FilterProg> pushdown;        // FILTER conjuncts over one pattern's variables, evaluated while that pattern is read
+    FilterProg post;                         // the other conjuncts, evaluated on the joined row
+    std::vector<u32> key_pos;                // position of the join variable in pattern k
+    // fast path shape: every pattern binds exactly two variables in subject and object position (the join variable + one more)
+    bool all_pairs = false;
+    // no variable but the join variable occurs in two patterns (quirk Q3: the reference never checks the others — we must, so such
+    // shapes take the natural-join chain)
+    bool only_join_shared = true;
+};
 
-kb_status star_join_impl2(kb_ctx* ctx, u32 join_slot, const kb_pattern* pats, u32 K, const kb_filter_op* filter, u32 n_ops, bool allow_fused_scan,
-                          std::unique_ptr<kb_rel>* out, AggSpec* agg, IndexPlan* plan_only) {
-    if (K == 0 || K > (u32)MAXP) return fail(ctx, KB_E_LIMIT, "a star join takes 1..%d patterns (got %u)", MAXP, K);
-    KB_TRY(validate_filter(ctx, filter, n_ops));
-    std::vector<std::vector<u32>> pv(K), psrc(K);
-    std::vector<u32> all_slots;
-    for (u32 k = 0; k < K; k++) {
-        KB_TRY(check_pattern(ctx, pats[k]));
-        pattern_vars(pats[k], &pv[k], &psrc[k]);
-        if (std::find(pv[k].begin(), pv[k].end(), join_slot) == pv[k].end())
-            return fail(ctx, KB_E_INVALID, "star join: pattern %u does not contain the join variable (slot %u)", k, join_slot);
-        for (u32 s : pv[k]) if (std::find(all_slots.begin(), all_slots.end(), s) == all_slots.end()) all_slots.push_back(s);
-    }
-    if (all_slots.size() > KB_MAX_COLS) return fail(ctx, KB_E_LIMIT, "more than %d variables", KB_MAX_COLS);
-    // FILTER: conjuncts over one pattern's variables are evaluated while scanning that pattern
-    std::vector<FilterProg> conj, pushdown(K);
-    FilterProg post;
+enum class Route { answered, declined, retry };
+
+// FILTER: a conjunct over one pattern's variables goes to the first pattern that binds them all, every other conjunct to `post`
+static kb_status split_filter(kb_ctx* ctx, const kb_filter_op* filter, u32 n_ops, const std::vector<std::vector<u32>>& pv,
+                              const std::vector<u32>& all_slots, std::vector<FilterProg>* pushdown, FilterProg* post) {
+    std::vector<FilterProg> conj;
     if (!split_conjuncts(filter, n_ops, &conj)) return fail(ctx, KB_E_INVALID, "malformed filter program");
+    pushdown->assign(pv.size(), FilterProg{});
     for (auto& c : conj) {
         std::set<u32> fs = filter_slots(c);
         for (u32 s : fs) if (std::find(all_slots.begin(), all_slots.end(), s) == all_slots.end())
             return fail(ctx, KB_E_UNSUPPORTED, "filter references slot %u which no pattern binds (the reference evaluates it to false, types.rs:149-151)", s);
         int target = -1;
-        for (u32 k = 0; k < K && target < 0; k++) {
+        for (size_t k = 0; k < pv.size() && target < 0; k++) {
             bool all = true;
             for (u32 s : fs) if (std::find(pv[k].begin(), pv[k].end(), s) == pv[k].end()) all = false;
             if (all) target = (int)k;
         }
-        FilterProg* dst = target >= 0 ? &pushdown[target] : &post;
-        const bool had = !dst->ops.empty();
-        dst->ops.insert(dst->ops.end(), c.ops.begin(), c.ops.end());
-        if (had) { kb_filter_op a{}; a.op = KB_F_AND; dst->ops.push_back(a); }
+        and_into(target >= 0 ? &(*pushdown)[target] : post, c);
     }
-    // key range of the join variable from the load-time column statistics of the store (its position is the same in every
-    // pattern that can take the fused path)
-    auto key_pos = [&](u32 k) { for (size_t i = 0; i < pv[k].size(); i++) if (pv[k][i] == join_slot) return psrc[k][i]; return 0u; };
-    // fast path shape: every pattern binds exactly two variables in subject and object position (the join variable + one more)
-    bool all_pairs = K >= 2;
-    for (u32 k = 0; k < K; k++) if (!(pv[k].size() == 2 && psrc[k][0] == 0 && psrc[k][1] == 2)) all_pairs = false;
+    return KB_OK;
+}
 
-    // ---- INDEX path: every pattern is (?s P ?o) over a predicate the store index has a slice for: no store scan at all. Build sides
-    // are inserted from their slices (pushed-down FILTER evaluated in the build kernel), the probe side IS its slice (zero copy).
-    if (allow_fused_scan && ctx->use_index && ctx->index_version == ctx->store_version && all_pairs && K - 1 <= (u32)MAXT) {
-        bool ok = true, empty = false;
-        std::vector<const PredSlice*> sl(K, nullptr);
-        for (u32 k = 0; k < K; k++) {
-            if (pats[k].p.is_var) { ok = false; break; }
-            auto it = ctx->index.find(pats[k].p.value);
-            if (it == ctx->index.end() || it->second.n == 0) { empty = true; continue; }  // predicate absent from the store
-            sl[k] = &it->second;
-        }
-        for (u32 a = 0; a < K && ok; a++)
-            for (u32 b = a + 1; b < K && ok; b++)
-                for (u32 s2 : pv[a]) if (s2 != join_slot && std::find(pv[b].begin(), pv[b].end(), s2) != pv[b].end()) ok = false;
-        if (ok && empty && plan_only) return fail(ctx, KB_E_UNSUPPORTED, "prepared plan: a pattern's predicate does not occur in the store (the answer is empty)");
-        if (ok && empty) {
-            auto r = std::make_unique<kb_rel>();
-            r->slots = all_slots;
-            for (size_t c = 0; c < all_slots.size(); c++) { Col col; KB_TRY(alloc_col(ctx, 0, &col)); r->cols.push_back(col); }
-            *out = std::move(r);
-            return KB_OK;
-        }
-        u32 kmn = 0xFFFFFFFFu, kmx = 0;
-        u32 cshift = 0;
-        if (ok) {
-            bool subj = true;
-            for (u32 k = 0; k < K; k++) {
-                const bool y = key_pos(k) == 2;
-                kmn = std::min(kmn, y ? sl[k]->ymin : sl[k]->xmin);
-                kmx = std::max(kmx, y ? sl[k]->ymax : sl[k]->xmax);
-                if (y) subj = false;
-            }
-            for (auto& sg : ctx->segs) if (sg.n && (!sg.has_stats || sg.stats_world != ctx->shard_world || !sg.sharded_ok)) subj = false;
-            const u32 w = ctx->shard_world;
-            if (subj && w > 1 && (w & (w - 1)) == 0) while ((1u << cshift) < w) cshift++;
-            kmn = compact_key(kmn, cshift);
-            kmx = compact_key(kmx, cshift);
-        }
-        // a pattern whose key column has a persistent table in the index needs no build at all: it is looked up like spo[s][P]
-        auto persistent = [&](u32 k) -> bool {
-            if (!ok) return false;
-            const bool y = key_pos(k) == 2;
-            return y ? (bool)sl[k]->ytab : ((bool)sl[k]->xtab && sl[k]->tab_cshift == cshift);
-        };
-        // probe side: prefer a pattern WITHOUT a persistent table (it would need a build), then the smallest slice (fewest lookups);
-        // when builds remain, the classic choice: the largest unfiltered slice probes, filtered sides build
-        int probe_k = -1;
-        bool all_persistent = ok;
-        for (u32 k = 0; k < K && ok; k++) if (!persistent(k)) all_persistent = false;
-        if (ok && all_persistent) {
-            // no builds at all: the probe side should be the most selective stream — a pattern that carries its own FILTER (evaluated
-            // on the probe row before any lookup), else the smallest slice
-            probe_k = -1;
-            for (u32 k = 0; k < K; k++) if (!pushdown[k].ops.empty() && pushdown[k].ops.size() <= 8 && (probe_k < 0 || sl[k]->n < sl[probe_k]->n)) probe_k = (int)k;
-            if (probe_k < 0) { probe_k = 0; for (u32 k = 1; k < K; k++) if (sl[k]->n < sl[probe_k]->n) probe_k = (int)k; }
+static kb_status star_query(kb_ctx* ctx, u32 join_slot, const kb_pattern* pats, u32 K, const kb_filter_op* filter, u32 n_ops, StarQuery* q) {
+    if (K == 0 || K > (u32)MAXP) return fail(ctx, KB_E_LIMIT, "a star join takes 1..%d patterns (got %u)", MAXP, K);
+    KB_TRY(validate_filter(ctx, filter, n_ops));
+    q->join_slot = join_slot;
+    q->K = K;
+    q->pats = pats;
+    q->pv.resize(K);
+    q->psrc.resize(K);
+    q->key_pos.resize(K);
+    for (u32 k = 0; k < K; k++) {
+        KB_TRY(check_pattern(ctx, pats[k]));
+        pattern_vars(pats[k], &q->pv[k], &q->psrc[k]);
+        const auto j = std::find(q->pv[k].begin(), q->pv[k].end(), join_slot);
+        if (j == q->pv[k].end()) return fail(ctx, KB_E_INVALID, "star join: pattern %u does not contain the join variable (slot %u)", k, join_slot);
+        q->key_pos[k] = q->psrc[k][j - q->pv[k].begin()];
+        for (u32 s : q->pv[k]) if (std::find(q->all_slots.begin(), q->all_slots.end(), s) == q->all_slots.end()) q->all_slots.push_back(s);
+    }
+    if (q->all_slots.size() > KB_MAX_COLS) return fail(ctx, KB_E_LIMIT, "more than %d variables", KB_MAX_COLS);
+    KB_TRY(split_filter(ctx, filter, n_ops, q->pv, q->all_slots, &q->pushdown, &q->post));
+    q->all_pairs = K >= 2;
+    for (u32 k = 0; k < K; k++) if (!(q->pv[k].size() == 2 && q->psrc[k][0] == 0 && q->psrc[k][1] == 2)) q->all_pairs = false;
+    for (u32 a = 0; a < K; a++)
+        for (u32 b = a + 1; b < K; b++)
+            for (u32 s2 : q->pv[a]) if (s2 != join_slot && std::find(q->pv[b].begin(), q->pv[b].end(), s2) != q->pv[b].end()) q->only_join_shared = false;
+    return KB_OK;
+}
+
+// key range of the join variable over the store, from the load-time column statistics of its segments
+static kb_status store_key_range(kb_ctx* ctx, const StarQuery& q, u32* kmin, u32* kmax) {
+    *kmin = 0xFFFFFFFFu;
+    *kmax = 0;
+    for (auto& sg : ctx->segs) {
+        if (sg.n == 0) continue;
+        if (!sg.has_stats) KB_TRY(segment_stats(ctx, &sg));
+        for (u32 k = 0; k < q.K; k++) { const u32 c = q.key_pos[k]; *kmin = std::min(*kmin, sg.cmin[c]); *kmax = std::max(*kmax, sg.cmax[c]); }
+    }
+    return KB_OK;
+}
+
+// a subject-sharded store (kb_set_sharding) owns every world-th block of ids: subject keys are compacted by this shift so that the
+// tables stay dense. 0 unless every key is a subject and no segment may hold a foreign subject (current_stats: the statistics that
+// say so must have been taken under the current sharding)
+static u32 subject_cshift(const kb_ctx* ctx, const StarQuery& q, bool current_stats) {
+    bool subj = true;
+    for (u32 k = 0; k < q.K; k++) if (q.key_pos[k] != 0) subj = false;
+    for (auto& sg : ctx->segs)
+        if (sg.n && (!sg.sharded_ok || (current_stats && (!sg.has_stats || sg.stats_world != ctx->shard_world)))) subj = false;
+    u32 cshift = 0;
+    const u32 w = ctx->shard_world;
+    if (subj && w > 1 && (w & (w - 1)) == 0) while ((1u << cshift) < w) cshift++;
+    return cshift;
+}
+
+// a persistent table of the store index, looked up like spo[s][P] (subject key) or pos[P][o] (object key)
+static DirectTab persistent_tab(const PredSlice& s, bool key_is_y) {
+    DirectTab D{};
+    D.tab = static_cast<const u32*>(key_is_y ? s.ytab->p : s.xtab->p);
+    D.kmin = key_is_y ? s.ytab_min : s.xtab_min;
+    D.range = key_is_y ? s.ytab_range : s.xtab_range;
+    D.cshift = key_is_y ? 0u : s.tab_cshift;
+    return D;
+}
+
+// the fused multiway probe over pair rows (probe_fast_kernel) against T direct tables; P may carry a pre-filter. The output columns
+// (`ocs`, `n` rows each) are appended to res->cols; the row count lands in ctrl[1]
+static kb_status probe_fast(kb_ctx* ctx, ProbeFParams& P, const uint2* pairs, u64 n, u32 key_is_y, const DirectTab* dt, u32 T,
+                            const std::vector<OutCol>& ocs, const std::vector<FilterOp>& fops, u32* ctrl, const u32* abort_flag, kb_rel* res) {
+    P.pairs = pairs;
+    P.key_is_y = key_is_y;
+    P.n = (u32)n;
+    P.n_tiles = (u32)((n + PROBEF_TILE - 1) / PROBEF_TILE);
+    P.T = T;
+    for (u32 q = 0; q < T; q++) P.tab[q] = dt[q];
+    KB_TRY(probe_setup(ctx, &P, n, ocs, fops, ctrl, abort_flag, res));
+    timer_begin(ctx, F_PROBE);
+    launch_probe_fast(P, ctx->n_sms, ctx->st);
+    timer_end(ctx);
+    KB_CUDA(ctx, cudaGetLastError());
+    ctx->stats.rows_probed += n;
+    return KB_OK;
+}
+
+// what the store index says about a star of (?s P ?o) patterns
+struct IndexSlices {
+    bool shape = false;   // valid index, every pattern (?s P ?o), at most MAXT build sides
+    bool empty = false;   // a pattern's predicate does not occur in the store: the answer is empty
+    bool usable = false;  // every predicate constant and present, the patterns share only the join variable
+    std::vector<const PredSlice*> sl;
+    std::vector<bool> persistent;  // the key column of pattern k has a persistent table in the index: it needs no build
+    bool all_persistent = false;
+    u32 kmin = 0xFFFFFFFFu, kmax = 0, cshift = 0;
+    int probe_k = -1;
+};
+
+static IndexSlices index_slices(const kb_ctx* ctx, const StarQuery& q) {
+    IndexSlices ix;
+    ix.shape = ctx->use_index && ctx->index_version == ctx->store_version && q.all_pairs && q.K - 1 <= (u32)MAXT;
+    if (!ix.shape) return ix;
+    const u32 K = q.K;
+    bool ok = q.only_join_shared, empty = false;
+    ix.sl.assign(K, nullptr);
+    for (u32 k = 0; k < K; k++) {
+        if (q.pats[k].p.is_var) { ok = false; break; }
+        auto it = ctx->index.find(q.pats[k].p.value);
+        if (it == ctx->index.end() || it->second.n == 0) { empty = true; continue; }  // predicate absent from the store
+        ix.sl[k] = &it->second;
+    }
+    ix.empty = ok && empty;
+    ix.usable = ok && !empty;
+    if (!ix.usable) return ix;
+    // key range of the join variable from the slices (its position is the same in every pattern that can take this path)
+    for (u32 k = 0; k < K; k++) {
+        const bool y = q.key_pos[k] == 2;
+        ix.kmin = std::min(ix.kmin, y ? ix.sl[k]->ymin : ix.sl[k]->xmin);
+        ix.kmax = std::max(ix.kmax, y ? ix.sl[k]->ymax : ix.sl[k]->xmax);
+    }
+    ix.cshift = subject_cshift(ctx, q, true);
+    ix.kmin = compact_key(ix.kmin, ix.cshift);
+    ix.kmax = compact_key(ix.kmax, ix.cshift);
+    ix.persistent.resize(K);
+    ix.all_persistent = true;
+    for (u32 k = 0; k < K; k++) {
+        ix.persistent[k] = q.key_pos[k] == 2 ? (bool)ix.sl[k]->ytab : ((bool)ix.sl[k]->xtab && ix.sl[k]->tab_cshift == ix.cshift);
+        if (!ix.persistent[k]) ix.all_persistent = false;
+    }
+    // probe side: prefer a pattern WITHOUT a persistent table (it would need a build), then the smallest slice (fewest lookups);
+    // when builds remain, the classic choice: the largest unfiltered slice probes, filtered sides build
+    int& probe_k = ix.probe_k;
+    if (ix.all_persistent) {
+        // no builds at all: the probe side should be the most selective stream — a pattern that carries its own FILTER (evaluated
+        // on the probe row before any lookup), else the smallest slice
+        for (u32 k = 0; k < K; k++)
+            if (!q.pushdown[k].ops.empty() && q.pushdown[k].ops.size() <= 8 && (probe_k < 0 || ix.sl[k]->n < ix.sl[probe_k]->n)) probe_k = (int)k;
+        if (probe_k < 0) { probe_k = 0; for (u32 k = 1; k < K; k++) if (ix.sl[k]->n < ix.sl[probe_k]->n) probe_k = (int)k; }
+    } else {
+        for (u32 k = 0; k < K; k++) if (q.pushdown[k].ops.empty() && (probe_k < 0 || ix.sl[k]->n > ix.sl[probe_k]->n)) probe_k = (int)k;
+        if (probe_k < 0) { probe_k = 0; for (u32 k = 1; k < K; k++) if (ix.sl[k]->n > ix.sl[probe_k]->n) probe_k = (int)k; }
+    }
+    return ix;
+}
+
+kb_status alloc_index_out(kb_ctx* ctx, u64 rows, u32 n_out, std::vector<Col>* cols) {
+    const size_t stride = round256((size_t)rows * sizeof(u32)) + 256;
+    Buf b;
+    KB_TRY(alloc_buf(ctx, stride * n_out, &b));
+    cols->clear();
+    for (u32 c = 0; c < n_out; c++) {
+        Col col;
+        col.buf = b;
+        col.ptr = reinterpret_cast<u32*>(static_cast<char*>(b->p) + stride * c);
+        cols->push_back(col);
+    }
+    return KB_OK;
+}
+
+kb_status launch_index_rows(kb_ctx* ctx, ProbeIParams& P, const std::vector<Col>& cols) {
+    for (size_t c = 0; c < cols.size(); c++) P.out[c] = cols[c].ptr;
+    P.ordered = ctx->ordered;
+    if (P.ordered) {
+        KB_TRY(ensure_tile_state(ctx, P.n_tiles));
+        P.tile_state = static_cast<u64*>(ctx->tile_state->p);
+        P.block_state = static_cast<u64*>(ctx->block_state->p);
+    }
+    timer_begin(ctx, F_PROBE);
+    launch_probe_index(P, nullptr, ctx->n_sms, ctx->st);
+    timer_end(ctx);
+    KB_CUDA(ctx, cudaGetLastError());
+    return KB_OK;
+}
+
+static kb_status resolve_index_plan(kb_ctx* ctx, const StarQuery& q, const IndexSlices& ix, const AggSpec* agg, IndexPlan* ip) {
+    if (!ix.shape) { ip->why = "it needs a valid store index (kb_store_build_index) and (?s P ?o) patterns"; return KB_OK; }
+    if (ix.empty) { ip->why = "a pattern's predicate does not occur in the store (the answer is empty)"; return KB_OK; }
+    if (!ix.usable || !ix.all_persistent || !ctx->fast_index_kernel || ix.sl[ix.probe_k]->chunks.size() > (size_t)PROBEI_MAXSEG) {
+        ip->why = "every pattern (?s P ?o) over a predicate whose key column has a persistent table in the store index";
+        return KB_OK;
+    }
+    const u32 pk = (u32)ix.probe_k, T = q.K - 1;
+    const PredSlice& PS = *ix.sl[pk];
+    ProbeIParams& P = ip->P;
+    ip->out_slots = q.pv[pk];
+    FilterProg postp = q.post;  // filters of patterns that are not built (every one here) run on the joined row
+    u32 t = 0;
+    for (u32 k = 0; k < q.K; k++) {
+        if (k == pk) continue;
+        const bool y = q.key_pos[k] == 2;
+        P.tab[t++] = persistent_tab(*ix.sl[k], y);
+        and_into(&postp, q.pushdown[k]);
+        ip->out_slots.push_back(q.pv[k][y ? 0 : 1]);
+    }
+    const FilterProg& pf = q.pushdown[pk];
+    if (pf.ops.size() > 8) and_into(&postp, pf);
+    else if (!pf.ops.empty()) {
+        std::vector<FilterOp> fo;  // slots of the probe pattern's own filter -> pair halves (x = subject, y = object)
+        KB_TRY(compile_prog(ctx, pf, q.pv[pk], &fo));
+        const bool typed = PS.typed(ctx->num_version) && fo.size() == 1 && fo[0].op == KB_F_CMP_NUM && fo[0].slot == 1u;
+        if (typed) {
+            P.pre_mode = 1; P.pre_cmp = fo[0].cmp; P.pre_val = fo[0].value;
         } else {
-            for (u32 k = 0; k < K && ok; k++) if (pushdown[k].ops.empty() && (probe_k < 0 || sl[k]->n > sl[probe_k]->n)) probe_k = (int)k;
-            if (ok && probe_k < 0) { probe_k = 0; for (u32 k = 1; k < K; k++) if (sl[k]->n > sl[probe_k]->n) probe_k = (int)k; }
-        }
-        const u64 rng = (ok && kmx >= kmn) ? (u64)kmx - kmn + 1 : 0;
-        for (u32 k = 0; k < K && ok; k++) {
-            if ((int)k == probe_k || persistent(k)) continue;
-            if (rng == 0 || rng > std::max<u64>(8 * sl[k]->n, 1ull << 16) || rng > (1ull << 31)) ok = false;
-            if (ctx->multi_valued.count({pats[k].p.value, key_pos(k)})) ok = false;
-        }
-        if (ok && all_persistent && ctx->fast_index_kernel && sl[probe_k]->chunks.size() <= (size_t)PROBEI_MAXSEG) {
-            // every build side is a persistent table: the whole join is one launch of probe_index_kernel
-            const PredSlice& PS = *sl[probe_k];
-            const u32 T = K - 1;
-            ProbeIParams P{};
-            std::vector<u32> out_slots = pv[probe_k];
-            FilterProg postp = post;
-            auto to_post = [&](u32 k) {
-                if (pushdown[k].ops.empty()) return;
-                const bool had = !postp.ops.empty();
-                postp.ops.insert(postp.ops.end(), pushdown[k].ops.begin(), pushdown[k].ops.end());
-                if (had) { kb_filter_op a{}; a.op = KB_F_AND; postp.ops.push_back(a); }
-            };
-            u32 t = 0;
-            for (u32 k = 0; k < K; k++) {
-                if ((int)k == probe_k) continue;
-                const bool y = key_pos(k) == 2;
-                DirectTab& D = P.tab[t++];
-                D.mode = 0; D.n_pay = 0; D.pay[0] = D.pay[1] = nullptr;
-                D.tab = static_cast<const u32*>(y ? sl[k]->ytab->p : sl[k]->xtab->p);
-                D.kmin = y ? sl[k]->ytab_min : sl[k]->xtab_min;
-                D.range = y ? sl[k]->ytab_range : sl[k]->xtab_range;
-                D.cshift = y ? 0u : sl[k]->tab_cshift;
-                to_post(k);
-                out_slots.push_back(pv[k][y ? 0 : 1]);
-            }
-            const FilterProg& pf = pushdown[probe_k];
-            if (!pf.ops.empty()) {
-                if (pf.ops.size() > 8) to_post((u32)probe_k);
-                else {
-                    std::map<u32, u32> remap;  // slots of the probe pattern's own filter -> pair halves (x = subject, y = object)
-                    for (size_t i = 0; i < pv[probe_k].size(); i++) remap[pv[probe_k][i]] = psrc[probe_k][i] == 0 ? 0u : 1u;
-                    std::vector<FilterOp> fo;
-                    if (!append_prog(&fo, pf, remap)) return fail(ctx, KB_E_INVALID, "filter uses an unbound variable");
-                    const bool typed = PS.typed(ctx->num_version) && fo.size() == 1 && fo[0].op == KB_F_CMP_NUM && fo[0].slot == 1u;
-                    if (typed) {
-                        P.pre_mode = 1; P.pre_cmp = fo[0].cmp; P.pre_val = fo[0].value;
-                    } else {
-                        P.pre_mode = 2; P.n_pre = (u32)fo.size();
-                        for (size_t i = 0; i < fo.size(); i++) P.pre_ops[i] = fo[i];
-                    }
-                }
-            }
-            const u32 n_out = 2 + T;
-            if (!postp.ops.empty()) {
-                std::map<u32, u32> remap;
-                for (u32 c = 0; c < n_out; c++) remap[out_slots[c]] = c;
-                std::vector<FilterOp> fops;
-                if (!append_prog(&fops, postp, remap)) return fail(ctx, KB_E_INVALID, "filter uses an unbound variable");
-                if (fops.size() > KB_MAX_FILTER_OPS) return fail(ctx, KB_E_LIMIT, "filter too long");
-                P.n_ops = (u32)fops.size();
-                for (size_t i = 0; i < fops.size(); i++) P.ops[i] = fops[i];
-            }
-            // table mode: the probe pattern's own subject table is the probe stream (keys ascending whatever the store / id order)
-            const bool tab_mode = ctx->probe_table_mode && !ctx->ordered && persistent((u32)probe_k) && key_pos((u32)probe_k) == 0 &&
-                                  (P.pre_mode != 1u || (PS.xnum && PS.xnum_version == ctx->num_version));
-            P.n_seg = 0;
-            P.n_tiles = 0;
-            if (tab_mode) {
-                // walk the slots that can hold a key (smallest to largest live subject), not the table's growth headroom nor the
-                // slots an evicted past has left empty; the first slot stays 128-byte aligned for the bulk loads
-                const u32 lo = ((compact_key(PS.xmin, PS.tab_cshift) - PS.xtab_min) / 32u) * 32u;
-                const u32 hi = std::min<u32>(PS.xtab_range, compact_key(PS.xmax, PS.tab_cshift) - PS.xtab_min + 1u);
-                P.ptab = static_cast<const u32*>(PS.xtab->p) + lo;
-                P.pnum = P.pre_mode == 1u ? static_cast<const double*>(PS.xnum->p) + lo : nullptr;
-                P.ptab_min = PS.xtab_min + lo;
-                P.ptab_range = hi > lo ? hi - lo : 0u;
-                P.ptab_cshift = PS.tab_cshift;
-                P.shard_rank = ctx->shard_rank;
-                P.n_tiles = (u32)(((u64)P.ptab_range + PROBEF_TILE - 1) / PROBEF_TILE);
-            }
-            for (auto& ch : PS.chunks) {  // one chunk per store segment: an RSP window of slides is walked in ONE launch
-                if (tab_mode) break;
-                if (ch.n == 0) continue;
-                ProbeISeg& g = P.seg[P.n_seg++];
-                g.pairs = reinterpret_cast<const uint2*>(ch.pairs.ptr);
-                g.ynum = P.pre_mode == 1u ? static_cast<const double*>(ch.ynum->p) : nullptr;
-                g.n = (u32)ch.n;
-                g.tile0 = P.n_tiles;
-                P.n_tiles += (u32)((ch.n + PROBEF_TILE - 1) / PROBEF_TILE);
-            }
-            P.key_is_y = key_pos((u32)probe_k) == 2 ? 1u : 0u;
-            P.n = (u32)PS.n;
-            P.T = T;
-            P.cap = (u32)PS.n;
-            P.nt = numtab(ctx);
-            P.cb = ctx->fast_cb;
-            P.host_total = ctx->d_fast;
-            if (plan_only) {  // kb_star_join_prepare: keep the resolved launch, run nothing
-                plan_only->P = P;
-                plan_only->out_slots = out_slots;
-                plan_only->all_slots = all_slots;
-                plan_only->n_out = n_out;
-                plan_only->probe_rows = PS.n;
-                if (agg) {
-                    int gsel = -1, asel = -1;
-                    for (u32 c = 0; c < n_out; c++) {
-                        if (out_slots[c] == agg->group_slot) gsel = (int)c;
-                        if (agg->has_agg && out_slots[c] == agg->agg_slot) asel = (int)c;
-                    }
-                    const bool needs_value = agg->has_agg && agg->kind != KB_AGG_COUNT;
-                    if (gsel < 0 || (needs_value && asel < 0))
-                        return fail(ctx, KB_E_UNSUPPORTED, "prepared GROUP BY: the group or aggregate variable is not bound by the join");
-                    plan_only->agg = true;
-                    plan_only->has_agg = agg->has_agg;
-                    plan_only->agg_kind = agg->has_agg ? agg->kind : (u32)KB_AGG_COUNT;
-                    plan_only->agg_slot = agg->agg_slot;
-                    plan_only->group_slot = agg->group_slot;
-                    plan_only->P.gsel = (u32)gsel;
-                    plan_only->P.asel = asel >= 0 ? (u32)asel : 0u;
-                    plan_only->P.akind = plan_only->agg_kind;
-                }
-                plan_only->ok = true;
-                return KB_OK;
-            }
-            if (agg) {
-                // GROUP BY folded into the probe kernel: no joined row is written. One try with a 4096-slot table; more groups than
-                // that (or a group / aggregate variable the join does not bind) leave agg->applied false: the caller groups separately
-                int gsel = -1, asel = -1;
-                for (u32 c = 0; c < n_out; c++) {
-                    if (out_slots[c] == agg->group_slot) gsel = (int)c;
-                    if (agg->has_agg && out_slots[c] == agg->agg_slot) asel = (int)c;
-                }
-                const bool needs_value = agg->has_agg && agg->kind != KB_AGG_COUNT;
-                if (gsel >= 0 && (!needs_value || asel >= 0)) {
-                    GroupParams G{};
-                    G.n_gcols = 1;
-                    G.n_aggs = agg->has_agg ? 1u : 0u;
-                    G.akind[0] = agg->has_agg ? agg->kind : (u32)KB_AGG_COUNT;
-                    G.nt = numtab(ctx);
-                    GroupTable tab;
-                    KB_TRY(group_table_create(ctx, 1u << 12, &G, &tab));
-                    const u32 goff = ctrl_alloc(ctx, 4);
-                    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + goff, 0, 4 * sizeof(u32), ctx->st));
-                    G.overflow = ctx->ctrl + goff;
-                    P.gsel = (u32)gsel;
-                    P.asel = asel >= 0 ? (u32)asel : 0u;
-                    P.akind = G.akind[0];
-                    P.ordered = 0;
-                    P.epoch = ctx->epoch++;
-                    timer_begin(ctx, F_PROBE);
-                    launch_probe_index(P, &G, ctx->n_sms, ctx->st);
-                    timer_end(ctx);
-                    KB_CUDA(ctx, cudaGetLastError());
-                    ctx->stats.rows_probed += PS.n;
-                    ctx->stats.index_joins++;
-                    KB_TRY(ctrl_read(ctx));
-                    if (ctx->h_ctrl[goff] == 0) {
-                        agg->n_rows = *reinterpret_cast<volatile u32*>(ctx->h_fast);
-                        agg->groups = std::make_unique<kb_groups>();
-                        agg->groups->keys.resize(1);
-                        agg->groups->vals.resize(agg->has_agg ? 1 : 0);
-                        kb_agg a1{agg->kind, agg->agg_slot};
-                        KB_TRY(group_table_collect(ctx, tab, 1, &a1, agg->has_agg ? 1u : 0u, agg->groups.get()));
-                        agg->applied = true;
-                        return KB_OK;
-                    }
-                }
-                // fall through: join without the fused GROUP BY (the control block was left clean by the kernel)
-            }
-            auto res = std::make_unique<kb_rel>();
-            res->slots = out_slots;
-            {   // one allocation holds all output columns
-                const size_t stride = round256((size_t)PS.n * sizeof(u32)) + 256;
-                Buf b;
-                KB_TRY(alloc_buf(ctx, stride * n_out, &b));
-                for (u32 c = 0; c < n_out; c++) {
-                    Col col;
-                    col.buf = b;
-                    col.ptr = reinterpret_cast<u32*>(static_cast<char*>(b->p) + stride * c);
-                    res->cols.push_back(col);
-                    P.out[c] = col.ptr;
-                }
-            }
-            P.ordered = ctx->ordered;
-            if (P.ordered) {
-                KB_TRY(ensure_tile_state(ctx, P.n_tiles));
-                P.tile_state = static_cast<u64*>(ctx->tile_state->p);
-                P.block_state = static_cast<u64*>(ctx->block_state->p);
-            }
-            P.epoch = ctx->epoch++;
-            timer_begin(ctx, F_PROBE);
-            launch_probe_index(P, nullptr, ctx->n_sms, ctx->st);
-            timer_end(ctx);
-            KB_CUDA(ctx, cudaGetLastError());
-            ctx->stats.rows_probed += PS.n;
-            ctx->stats.index_joins++;
-            KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
-            timers_flush(ctx);
-            ctx->stats.d2h_bytes += sizeof(u32);
-            res->n = *reinterpret_cast<volatile u32*>(ctx->h_fast);
-            *out = select_cols(*res, all_slots);
-            return KB_OK;
-        }
-        for (u32 k = 0; k < K && ok; k++) if (!sl[k]->single()) ok = false;  // the build-from-slice path reads one contiguous slice per pattern
-        if (plan_only) return fail(ctx, KB_E_UNSUPPORTED, "prepared plans take the one-kernel index path only: every pattern (?s P ?o) over a predicate whose key column has a persistent table in the store index");
-        if (ok) {
-            const u32 range = (u32)rng;
-            const u32 off = ctrl_alloc(ctx, 16 + 2 * MAXT);
-            KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, (16 + 2 * MAXT) * sizeof(u32), ctx->st));
-            std::vector<Buf> tabs;
-            DirectTab dt[MAXT];
-            std::vector<u32> tab_k;
-            std::vector<u32> out_slots = pv[probe_k];
-            std::vector<OutCol> ocs{OutCol{OUT_PROBE, 0, 0}, OutCol{OUT_PROBE, 1, 0}};
-            const u32 T = K - 1;
-            FilterProg postp = post;  // filters of patterns that are not built (probe side, persistent tables) run on the joined row
-            auto to_post = [&](u32 k) {
-                if (pushdown[k].ops.empty()) return;
-                const bool had = !postp.ops.empty();
-                postp.ops.insert(postp.ops.end(), pushdown[k].ops.begin(), pushdown[k].ops.end());
-                if (had) { kb_filter_op a{}; a.op = KB_F_AND; postp.ops.push_back(a); }
-            };
-            const bool pre_filter = !pushdown[probe_k].ops.empty() && pushdown[probe_k].ops.size() <= 8;
-            if (!pre_filter) to_post((u32)probe_k);
-            u32 n_build = 0;
-            for (u32 k = 0; k < K; k++) if ((int)k != probe_k && !persistent(k)) n_build++;
-            if (n_build) timer_begin(ctx, F_BUILD, (int)n_build);
-            for (u32 k = 0; k < K; k++) if ((int)k != probe_k && !persistent(k)) { Buf b; KB_TRY(alloc_buf(ctx, (size_t)range * sizeof(u32), &b)); tabs.push_back(b); }
-            if (n_build > 1) {
-                KB_CUDA(ctx, cudaEventRecord(ctx->ev_fork, ctx->st));
-                KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st2, ctx->ev_fork, 0));
-            }
-            u32 t = 0, bi = 0;
-            for (u32 k = 0; k < K; k++) {
-                if ((int)k == probe_k) continue;
-                DirectTab& D = dt[t];
-                D.mode = 0; D.n_pay = 0; D.pay[0] = D.pay[1] = nullptr;
-                if (persistent(k)) {
-                    const bool y = key_pos(k) == 2;
-                    D.tab = static_cast<const u32*>(y ? sl[k]->ytab->p : sl[k]->xtab->p);
-                    D.kmin = y ? sl[k]->ytab_min : sl[k]->xtab_min;
-                    D.range = y ? sl[k]->ytab_range : sl[k]->xtab_range;
-                    D.cshift = y ? 0u : sl[k]->tab_cshift;
-                    to_post(k);
-                } else {
-                    cudaStream_t bs = (n_build > 1 && (bi & 1)) ? ctx->st2 : ctx->st;
-                    u32* tab = static_cast<u32*>(tabs[bi]->p);
-                    KB_CUDA(ctx, cudaMemsetAsync(tab, 0xFF, (size_t)range * sizeof(u32), bs));
-                    BuildPairsParams B{};
-                    B.kv = reinterpret_cast<const uint2*>(sl[k]->single()->pairs.ptr);
-                    B.n = (u32)sl[k]->n;
-                    B.key_is_y = key_pos(k) == 2 ? 1u : 0u;
-                    B.pred = pats[k].p.value;
-                    B.table = tab; B.kmin = kmn; B.range = range; B.cshift = cshift;
-                    B.dup_flag = ctx->ctrl + off + 16 + t;
-                    B.count = ctx->ctrl + off + 16 + MAXT + t;
-                    B.trusted = ((key_pos(k) == 2 ? sl[k]->y_unique : sl[k]->x_unique) || ctx->single_valued.count({pats[k].p.value, key_pos(k)})) ? 1u : 0u;
-                    B.nt = numtab(ctx);
-                    if (!pushdown[k].ops.empty()) {
-                        std::map<u32, u32> remap;
-                        for (size_t i = 0; i < pv[k].size(); i++) remap[pv[k][i]] = psrc[k][i];
-                        std::vector<FilterOp> fo;
-                        if (!append_prog(&fo, pushdown[k], remap)) return fail(ctx, KB_E_INVALID, "pushed-down filter uses a variable the pattern does not bind");
-                        B.n_ops = (u32)fo.size();
-                        for (size_t i = 0; i < fo.size(); i++) B.ops[i] = fo[i];
-                    }
-                    launch_build_direct_pairs_filtered(B, ctx->n_sms, bs);
-                    D.tab = tab; D.kmin = kmn; D.range = range; D.cshift = cshift;
-                    ctx->stats.rows_built += sl[k]->n;
-                    bi++;
-                }
-                out_slots.push_back(pv[k][key_pos(k) == 0 ? 1 : 0]);
-                ocs.push_back(OutCol{OUT_TABVAL, t, 0});
-                tab_k.push_back(k);
-                t++;
-            }
-            if (n_build > 1) {
-                KB_CUDA(ctx, cudaEventRecord(ctx->ev_join, ctx->st2));
-                KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st, ctx->ev_join, 0));
-            }
-            if (n_build) timer_end(ctx);
-            const PredSlice& PS = *sl[probe_k];
-            auto res = std::make_unique<kb_rel>();
-            res->slots = out_slots;
-            const u32 n_out = (u32)out_slots.size();
-            std::vector<FilterOp> fops;
-            if (!postp.ops.empty()) {
-                std::map<u32, u32> remap;
-                for (u32 c = 0; c < n_out; c++) remap[out_slots[c]] = c;
-                if (!append_prog(&fops, postp, remap)) return fail(ctx, KB_E_INVALID, "filter uses an unbound variable");
-                if (fops.size() > KB_MAX_FILTER_OPS) return fail(ctx, KB_E_LIMIT, "filter too long");
-            }
-            ProbeFParams P{};
-            if (pre_filter) {  // slots of the probe pattern's own filter -> pair halves (x = subject, y = object)
-                std::map<u32, u32> remap;
-                for (size_t i = 0; i < pv[probe_k].size(); i++) remap[pv[probe_k][i]] = psrc[probe_k][i] == 0 ? 0u : 1u;
-                std::vector<FilterOp> fo;
-                if (!append_prog(&fo, pushdown[probe_k], remap)) return fail(ctx, KB_E_INVALID, "filter uses an unbound variable");
-                P.n_pre = (u32)fo.size();
-                for (size_t i = 0; i < fo.size(); i++) P.pre_ops[i] = fo[i];
-                if (sl[probe_k]->typed(ctx->num_version)) P.pre_num = static_cast<const double*>(sl[probe_k]->single()->ynum->p);
-            }
-            P.pairs = reinterpret_cast<const uint2*>(PS.single()->pairs.ptr);
-            P.key_is_y = key_pos((u32)probe_k) == 2 ? 1u : 0u;
-            P.n = (u32)PS.n;
-            P.n_tiles = (u32)((PS.n + PROBEF_TILE - 1) / PROBEF_TILE);
-            P.T = T;
-            for (u32 q = 0; q < T; q++) P.tab[q] = dt[q];
-            P.n_out = n_out;
-            for (u32 c = 0; c < n_out; c++) {
-                Col col;
-                KB_TRY(alloc_col(ctx, PS.n, &col));
-                res->cols.push_back(col);
-                P.oc[c] = ocs[c];
-                P.out[c] = col.ptr;
-            }
-            P.cap = (u32)PS.n;
-            P.n_ops = (u32)fops.size();
-            for (size_t i = 0; i < fops.size(); i++) P.ops[i] = fops[i];
-            P.nt = numtab(ctx);
-            KB_TRY(ensure_tile_state(ctx, P.n_tiles));
-            P.tile_state = static_cast<u64*>(ctx->tile_state->p);
-            P.block_state = static_cast<u64*>(ctx->block_state->p);
-            P.ordered = ctx->ordered;
-            P.ticket = ctx->ctrl + off;
-            P.total = ctx->ctrl + off + 1;
-            P.zero_word = ctx->ctrl + off + 2;
-            P.abort_flag = nullptr;
-            P.epoch = ctx->epoch++;
-            timer_begin(ctx, F_PROBE);
-            launch_probe_fast(P, ctx->n_sms, ctx->st);
-            timer_end(ctx);
-            KB_CUDA(ctx, cudaGetLastError());
-            ctx->stats.rows_probed += PS.n;
-            ctx->stats.index_joins++;
-            KB_TRY(ctrl_read(ctx));
-            bool dup = false;
-            for (u32 q = 0; q < T; q++) if (ctx->h_ctrl[off + 16 + q]) {
-                dup = true;
-                ctx->multi_valued.insert({pats[tab_k[q]].p.value, key_pos(tab_k[q])});
-            }
-            if (dup) return star_join_impl2(ctx, join_slot, pats, K, filter, n_ops, true, out, agg);  // multi-valued is now cached: takes the chained route
-            for (u32 q = 0; q < T; q++)
-                if (!persistent(tab_k[q]) && pushdown[tab_k[q]].ops.empty()) ctx->single_valued.insert({pats[tab_k[q]].p.value, key_pos(tab_k[q])});
-            res->n = ctx->h_ctrl[off + 1];
-            *out = select_cols(*res, all_slots);
-            return KB_OK;
+            P.pre_mode = 2; P.n_pre = (u32)fo.size();
+            for (size_t i = 0; i < fo.size(); i++) P.pre_ops[i] = fo[i];
         }
     }
+    ip->n_out = 2 + T;
+    std::vector<FilterOp> fops;
+    KB_TRY(compile_prog(ctx, postp, ip->out_slots, &fops));
+    P.n_ops = (u32)fops.size();
+    for (size_t i = 0; i < fops.size(); i++) P.ops[i] = fops[i];
+    // table mode: the probe pattern's own subject table is the probe stream (keys ascending whatever the store / id order)
+    const bool tab_mode = ctx->probe_table_mode && !ctx->ordered && ix.persistent[pk] && q.key_pos[pk] == 0 &&
+                          (P.pre_mode != 1u || (PS.xnum && PS.xnum_version == ctx->num_version));
+    if (tab_mode) {
+        // walk the slots that can hold a key (smallest to largest live subject), not the table's growth headroom nor the
+        // slots an evicted past has left empty; the first slot stays 128-byte aligned for the bulk loads
+        const u32 lo = ((compact_key(PS.xmin, PS.tab_cshift) - PS.xtab_min) / 32u) * 32u;
+        const u32 hi = std::min<u32>(PS.xtab_range, compact_key(PS.xmax, PS.tab_cshift) - PS.xtab_min + 1u);
+        P.ptab = static_cast<const u32*>(PS.xtab->p) + lo;
+        P.pnum = P.pre_mode == 1u ? static_cast<const double*>(PS.xnum->p) + lo : nullptr;
+        P.ptab_min = PS.xtab_min + lo;
+        P.ptab_range = hi > lo ? hi - lo : 0u;
+        P.ptab_cshift = PS.tab_cshift;
+        P.shard_rank = ctx->shard_rank;
+        P.n_tiles = (u32)(((u64)P.ptab_range + PROBEF_TILE - 1) / PROBEF_TILE);
+    } else {
+        for (auto& ch : PS.chunks) {  // one chunk per store segment: an RSP window of slides is walked in ONE launch
+            if (ch.n == 0) continue;
+            ProbeISeg& g = P.seg[P.n_seg++];
+            g.pairs = reinterpret_cast<const uint2*>(ch.pairs.ptr);
+            g.ynum = P.pre_mode == 1u ? static_cast<const double*>(ch.ynum->p) : nullptr;
+            g.n = (u32)ch.n;
+            g.tile0 = P.n_tiles;
+            P.n_tiles += (u32)((ch.n + PROBEF_TILE - 1) / PROBEF_TILE);
+        }
+    }
+    P.key_is_y = q.key_pos[pk] == 2 ? 1u : 0u;
+    P.n = (u32)PS.n;
+    P.T = T;
+    P.cap = (u32)PS.n;
+    P.nt = numtab(ctx);
+    P.cb = ctx->fast_cb;
+    P.host_total = ctx->d_fast;
+    ip->all_slots = q.all_slots;
+    ip->probe_rows = PS.n;
+    if (agg) {  // GROUP BY folded into the kernel when the join binds the group variable (and the aggregated one, if any)
+        int gsel = -1, asel = -1;
+        for (u32 c = 0; c < ip->n_out; c++) {
+            if (ip->out_slots[c] == agg->group_slot) gsel = (int)c;
+            if (agg->has_agg && ip->out_slots[c] == agg->agg_slot) asel = (int)c;
+        }
+        const bool needs_value = agg->has_agg && agg->kind != KB_AGG_COUNT;
+        if (gsel >= 0 && (!needs_value || asel >= 0)) {
+            ip->agg = true;
+            ip->has_agg = agg->has_agg;
+            ip->agg_kind = agg->has_agg ? agg->kind : (u32)KB_AGG_COUNT;
+            ip->agg_slot = agg->agg_slot;
+            ip->group_slot = agg->group_slot;
+            P.gsel = (u32)gsel;
+            P.asel = asel >= 0 ? (u32)asel : 0u;
+            P.akind = ip->agg_kind;
+        }
+    }
+    ip->ok = true;
+    return KB_OK;
+}
 
-    if (plan_only) return fail(ctx, KB_E_UNSUPPORTED, "prepared plans need a valid store index (kb_store_build_index) and (?s P ?o) patterns");
-    // ---- scan + build FUSED: the build-side patterns insert straight into their direct tables while the store is scanned; only the
-    // probe-side pattern is materialised. Needs the key range before the scan (load-time statistics) and a probe side chosen without
-    // knowing the counts: the last pattern that carries no pushed-down filter (a filtered side is the smaller build side).
-    if (allow_fused_scan && all_pairs && K - 1 <= (u32)MAXT && ctx->upload_stats_off < 0 && ctx->n_triples > 0) {
-        bool ok = true;
-        u32 kmn = 0xFFFFFFFFu, kmx = 0;
-        for (auto& sg : ctx->segs) {
-            if (sg.n == 0) continue;
-            if (!sg.has_stats) KB_TRY(segment_stats(ctx, &sg));
-            for (u32 k = 0; k < K; k++) { const u32 c = key_pos(k); kmn = std::min(kmn, sg.cmin[c]); kmx = std::max(kmx, sg.cmax[c]); }
+kb_status resolve_index_plan(kb_ctx* ctx, u32 join_slot, const kb_pattern* pats, u32 K, const kb_filter_op* filter, u32 n_ops, const AggSpec* agg,
+                             IndexPlan* plan) {
+    StarQuery q;
+    KB_TRY(star_query(ctx, join_slot, pats, K, filter, n_ops, &q));
+    return resolve_index_plan(ctx, q, index_slices(ctx, q), agg, plan);
+}
+
+// R1: the whole join is one launch of probe_index_kernel
+static kb_status index_join_one_kernel(kb_ctx* ctx, const StarQuery& q, const IndexSlices& ix, AggSpec* agg, std::unique_ptr<kb_rel>* out,
+                                       Route* route) {
+    *route = Route::answered;
+    if (ix.empty) return empty_rel(ctx, q.all_slots, out);
+    IndexPlan ip;
+    KB_TRY(resolve_index_plan(ctx, q, ix, agg, &ip));
+    if (!ip.ok) {
+        *route = Route::declined;
+        return KB_OK;
+    }
+    ProbeIParams& P = ip.P;
+    if (ip.agg) {
+        // GROUP BY folded into the probe kernel: no joined row is written. One try with a 4096-slot table; more groups than that (or
+        // a group / aggregate variable the join does not bind) leave agg->applied false: the caller groups separately
+        GroupParams G{};
+        G.n_gcols = 1;
+        G.n_aggs = ip.has_agg ? 1u : 0u;
+        G.akind[0] = ip.agg_kind;
+        G.nt = numtab(ctx);
+        GroupTable tab;
+        KB_TRY(group_table_create(ctx, 1u << 12, &G, &tab));
+        const u32 goff = ctrl_alloc(ctx, 4);
+        KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + goff, 0, 4 * sizeof(u32), ctx->st));
+        G.overflow = ctx->ctrl + goff;
+        P.ordered = 0;
+        P.epoch = ctx->epoch++;
+        timer_begin(ctx, F_PROBE);
+        launch_probe_index(P, &G, ctx->n_sms, ctx->st);
+        timer_end(ctx);
+        KB_CUDA(ctx, cudaGetLastError());
+        ctx->stats.rows_probed += ip.probe_rows;
+        ctx->stats.index_joins++;
+        KB_TRY(ctrl_read(ctx));
+        if (ctx->h_ctrl[goff] == 0) {
+            agg->n_rows = *reinterpret_cast<volatile u32*>(ctx->h_fast);
+            agg->groups = std::make_unique<kb_groups>();
+            agg->groups->keys.resize(1);
+            agg->groups->vals.resize(agg->has_agg ? 1 : 0);
+            kb_agg a1{agg->kind, agg->agg_slot};
+            KB_TRY(group_table_collect(ctx, tab, 1, &a1, agg->has_agg ? 1u : 0u, agg->groups.get()));
+            agg->applied = true;
+            return KB_OK;
         }
-        // a subject-sharded store (kb_set_sharding) owns every world-th block of ids: compact the key domain so the tables stay dense
-        u32 cshift = 0;
-        {
-            bool subj = true;
-            for (u32 k = 0; k < K; k++) if (key_pos(k) != 0) subj = false;
-            for (auto& sg : ctx->segs) if (sg.n && !sg.sharded_ok) subj = false;
-            const u32 w = ctx->shard_world;
-            if (subj && w > 1 && (w & (w - 1)) == 0) while ((1u << cshift) < w) cshift++;
+        // fall through: join without the fused GROUP BY (the control block was left clean by the kernel)
+    }
+    auto res = std::make_unique<kb_rel>();
+    res->slots = ip.out_slots;
+    KB_TRY(alloc_index_out(ctx, ip.probe_rows, ip.n_out, &res->cols));
+    P.epoch = ctx->epoch++;
+    KB_TRY(launch_index_rows(ctx, P, res->cols));
+    ctx->stats.rows_probed += ip.probe_rows;
+    ctx->stats.index_joins++;
+    KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
+    timers_flush(ctx);
+    ctx->stats.d2h_bytes += sizeof(u32);
+    res->n = *reinterpret_cast<volatile u32*>(ctx->h_fast);
+    *out = select_cols(*res, q.all_slots);
+    return KB_OK;
+}
+
+// R2: build sides are inserted from their slices (pushed-down FILTER evaluated in the build kernel), the probe side IS its slice
+// (zero copy). A duplicate key asks for a retry: the (predicate, position) is then cached as multi-valued, which this route declines
+static kb_status index_join_built(kb_ctx* ctx, const StarQuery& q, const IndexSlices& ix, std::unique_ptr<kb_rel>* out, Route* route) {
+    *route = Route::declined;
+    if (!ix.usable) return KB_OK;
+    const u32 K = q.K, pk = (u32)ix.probe_k, T = K - 1;
+    const u64 rng = ix.kmax >= ix.kmin ? (u64)ix.kmax - ix.kmin + 1 : 0;
+    for (u32 k = 0; k < K; k++) {
+        if (k == pk || ix.persistent[k]) continue;
+        if (rng == 0 || rng > std::max<u64>(8 * ix.sl[k]->n, 1ull << 16) || rng > (1ull << 31)) return KB_OK;
+        if (ctx->multi_valued.count({q.pats[k].p.value, q.key_pos[k]})) return KB_OK;
+    }
+    for (u32 k = 0; k < K; k++) if (!ix.sl[k]->single()) return KB_OK;  // the build kernel reads one contiguous slice per pattern
+    const u32 range = (u32)rng;
+    const u32 off = ctrl_alloc(ctx, 16 + 2 * MAXT);
+    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, (16 + 2 * MAXT) * sizeof(u32), ctx->st));
+    std::vector<Buf> tabs;
+    DirectTab dt[MAXT];
+    std::vector<u32> tab_k;
+    std::vector<u32> out_slots = q.pv[pk];
+    std::vector<OutCol> ocs{OutCol{OUT_PROBE, 0, 0}, OutCol{OUT_PROBE, 1, 0}};
+    FilterProg postp = q.post;  // filters of patterns that are not built (probe side, persistent tables) run on the joined row
+    const bool pre_filter = !q.pushdown[pk].ops.empty() && q.pushdown[pk].ops.size() <= 8;
+    if (!pre_filter) and_into(&postp, q.pushdown[pk]);
+    for (u32 k = 0; k < K; k++) if (k != pk && !ix.persistent[k]) { Buf b; KB_TRY(alloc_buf(ctx, (size_t)range * sizeof(u32), &b)); tabs.push_back(b); }
+    const u32 n_build = (u32)tabs.size();
+    if (n_build) timer_begin(ctx, F_BUILD, (int)n_build);
+    if (n_build > 1) {
+        KB_CUDA(ctx, cudaEventRecord(ctx->ev_fork, ctx->st));
+        KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st2, ctx->ev_fork, 0));
+    }
+    u32 t = 0, bi = 0;
+    for (u32 k = 0; k < K; k++) {
+        if (k == pk) continue;
+        const bool y = q.key_pos[k] == 2;
+        if (ix.persistent[k]) {
+            dt[t] = persistent_tab(*ix.sl[k], y);
+            and_into(&postp, q.pushdown[k]);
+        } else {
+            cudaStream_t bs = (n_build > 1 && (bi & 1)) ? ctx->st2 : ctx->st;
+            u32* tab = static_cast<u32*>(tabs[bi]->p);
+            KB_CUDA(ctx, cudaMemsetAsync(tab, 0xFF, (size_t)range * sizeof(u32), bs));
+            BuildPairsParams B{};
+            B.kv = reinterpret_cast<const uint2*>(ix.sl[k]->single()->pairs.ptr);
+            B.n = (u32)ix.sl[k]->n;
+            B.key_is_y = y ? 1u : 0u;
+            B.pred = q.pats[k].p.value;
+            B.table = tab; B.kmin = ix.kmin; B.range = range; B.cshift = ix.cshift;
+            B.dup_flag = ctx->ctrl + off + 16 + t;
+            B.count = ctx->ctrl + off + 16 + MAXT + t;
+            B.trusted = ((y ? ix.sl[k]->y_unique : ix.sl[k]->x_unique) || ctx->single_valued.count({q.pats[k].p.value, q.key_pos[k]})) ? 1u : 0u;
+            B.nt = numtab(ctx);
+            std::vector<FilterOp> fo;  // the pattern's own filter, over the positions of (s, P, o)
+            KB_TRY(compile_prog(ctx, q.pushdown[k], q.pv[k], &fo, &q.psrc[k]));
+            B.n_ops = (u32)fo.size();
+            for (size_t i = 0; i < fo.size(); i++) B.ops[i] = fo[i];
+            launch_build_direct_pairs_filtered(B, ctx->n_sms, bs);
+            dt[t] = DirectTab{};
+            dt[t].tab = tab; dt[t].kmin = ix.kmin; dt[t].range = range; dt[t].cshift = ix.cshift;
+            ctx->stats.rows_built += ix.sl[k]->n;
+            bi++;
         }
-        if (kmx >= kmn) { kmn = compact_key(kmn, cshift); kmx = compact_key(kmx, cshift); }
-        const u64 rng = kmx >= kmn ? (u64)kmx - kmn + 1 : 0;
-        if (rng == 0 || rng > std::max<u64>(4 * ctx->n_triples, 1ull << 16) || rng > (1ull << 31)) ok = false;
-        for (u32 a = 0; a < K && ok; a++)
-            for (u32 b = a + 1; b < K && ok; b++)
-                for (u32 s2 : pv[a]) if (s2 != join_slot && std::find(pv[b].begin(), pv[b].end(), s2) != pv[b].end()) ok = false;
-        int probe_k = -1;
-        for (u32 k = 0; k < K; k++) if (pushdown[k].ops.empty()) probe_k = (int)k;
-        if (probe_k < 0) probe_k = (int)K - 1;
-        for (u32 k = 0; k < K && ok; k++)
-            if ((int)k != probe_k && !pats[k].p.is_var && ctx->multi_valued.count({pats[k].p.value, key_pos(k)})) ok = false;
-        if (ok) {
-            const u32 range = (u32)rng;
-            const u32 off = ctrl_alloc(ctx, 8 + MAXT);
-            KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, (8 + MAXT) * sizeof(u32), ctx->st));
-            std::vector<ScanTable> st(K);
-            std::vector<Buf> tabs;
-            std::vector<u32> tab_of(K, 0);
-            DirectTab dt[MAXT];
-            std::vector<u32> out_slots = pv[probe_k];
-            std::vector<OutCol> ocs{OutCol{OUT_PROBE, 0, 0}, OutCol{OUT_PROBE, 1, 0}};
-            timer_begin(ctx, F_BUILD, 0);
-            u32 t = 0;
-            for (u32 k = 0; k < K; k++) {
-                if ((int)k == probe_k) continue;
-                Buf b;
-                KB_TRY(alloc_buf(ctx, (size_t)range * sizeof(u32), &b));
-                tabs.push_back(b);
-                st[k].tab = static_cast<u32*>(b->p);
-                st[k].clear = true;  // cleared by the scan (scan_impl)
-                st[k].kmin = kmn; st[k].range = range; st[k].cshift = cshift;
-                st[k].key_is_o = key_pos(k) == 2 ? 1u : 0u;
-                st[k].trusted = (!pats[k].p.is_var && ctx->single_valued.count({pats[k].p.value, key_pos(k)})) ? 1u : 0u;
-                st[k].dup_flag = ctx->ctrl + off + 8 + t;
-                DirectTab& D = dt[t];
-                D.tab = st[k].tab; D.kmin = kmn; D.range = range; D.cshift = cshift; D.mode = 0; D.n_pay = 0; D.pay[0] = D.pay[1] = nullptr;
-                out_slots.push_back(pv[k][key_pos(k) == 0 ? 1 : 0]);
-                ocs.push_back(OutCol{OUT_TABVAL, t, 0});
-                tab_of[k] = t;
-                t++;
+        out_slots.push_back(q.pv[k][y ? 0 : 1]);
+        ocs.push_back(OutCol{OUT_TABVAL, t, 0});
+        tab_k.push_back(k);
+        t++;
+    }
+    if (n_build > 1) {
+        KB_CUDA(ctx, cudaEventRecord(ctx->ev_join, ctx->st2));
+        KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st, ctx->ev_join, 0));
+    }
+    if (n_build) timer_end(ctx);
+    const PredSlice& PS = *ix.sl[pk];
+    auto res = std::make_unique<kb_rel>();
+    res->slots = out_slots;
+    std::vector<FilterOp> fops;
+    KB_TRY(compile_prog(ctx, postp, out_slots, &fops));
+    ProbeFParams P{};
+    if (pre_filter) {  // slots of the probe pattern's own filter -> pair halves (x = subject, y = object)
+        std::vector<FilterOp> fo;
+        KB_TRY(compile_prog(ctx, q.pushdown[pk], q.pv[pk], &fo));
+        P.n_pre = (u32)fo.size();
+        for (size_t i = 0; i < fo.size(); i++) P.pre_ops[i] = fo[i];
+        if (PS.typed(ctx->num_version)) P.pre_num = static_cast<const double*>(PS.single()->ynum->p);
+    }
+    KB_TRY(probe_fast(ctx, P, reinterpret_cast<const uint2*>(PS.single()->pairs.ptr), PS.n, q.key_pos[pk] == 2 ? 1u : 0u, dt, T, ocs, fops,
+                      ctx->ctrl + off, nullptr, res.get()));
+    ctx->stats.index_joins++;
+    KB_TRY(ctrl_read(ctx));
+    for (u32 q2 = 0; q2 < T; q2++) if (ctx->h_ctrl[off + 16 + q2]) {
+        *route = Route::retry;
+        ctx->multi_valued.insert({q.pats[tab_k[q2]].p.value, q.key_pos[tab_k[q2]]});
+    }
+    if (*route == Route::retry) return KB_OK;
+    for (u32 q2 = 0; q2 < T; q2++)
+        if (!ix.persistent[tab_k[q2]] && q.pushdown[tab_k[q2]].ops.empty()) ctx->single_valued.insert({q.pats[tab_k[q2]].p.value, q.key_pos[tab_k[q2]]});
+    res->n = ctx->h_ctrl[off + 1];
+    *out = select_cols(*res, q.all_slots);
+    *route = Route::answered;
+    return KB_OK;
+}
+
+// R3: the build-side patterns insert straight into their direct tables while the store is scanned; only the probe-side pattern is
+// materialised. Needs the key range before the scan (load-time statistics) and a probe side chosen without knowing the counts: the
+// last pattern that carries no pushed-down filter (a filtered side is the smaller build side). A duplicate or out-of-range key asks
+// for a retry without the fusion (the chained operator needs the build rows)
+static kb_status fused_scan_join(kb_ctx* ctx, const StarQuery& q, std::unique_ptr<kb_rel>* out, Route* route) {
+    *route = Route::declined;
+    const u32 K = q.K;
+    if (!q.all_pairs || K - 1 > (u32)MAXT || ctx->upload_stats_off >= 0 || ctx->n_triples == 0) return KB_OK;
+    u32 kmn, kmx;
+    KB_TRY(store_key_range(ctx, q, &kmn, &kmx));
+    const u32 cshift = subject_cshift(ctx, q, false);
+    if (kmx >= kmn) { kmn = compact_key(kmn, cshift); kmx = compact_key(kmx, cshift); }
+    const u64 rng = kmx >= kmn ? (u64)kmx - kmn + 1 : 0;
+    if (rng == 0 || rng > std::max<u64>(4 * ctx->n_triples, 1ull << 16) || rng > (1ull << 31) || !q.only_join_shared) return KB_OK;
+    int probe_k = -1;
+    for (u32 k = 0; k < K; k++) if (q.pushdown[k].ops.empty()) probe_k = (int)k;
+    if (probe_k < 0) probe_k = (int)K - 1;
+    for (u32 k = 0; k < K; k++)
+        if ((int)k != probe_k && !q.pats[k].p.is_var && ctx->multi_valued.count({q.pats[k].p.value, q.key_pos[k]})) return KB_OK;
+    const u32 range = (u32)rng;
+    const u32 off = ctrl_alloc(ctx, 8 + MAXT);
+    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, (8 + MAXT) * sizeof(u32), ctx->st));
+    std::vector<ScanTable> st(K);
+    std::vector<Buf> tabs;
+    std::vector<u32> tab_of(K, 0);
+    DirectTab dt[MAXT];
+    std::vector<u32> out_slots = q.pv[probe_k];
+    std::vector<OutCol> ocs{OutCol{OUT_PROBE, 0, 0}, OutCol{OUT_PROBE, 1, 0}};
+    timer_begin(ctx, F_BUILD, 0);
+    u32 t = 0;
+    for (u32 k = 0; k < K; k++) {
+        if ((int)k == probe_k) continue;
+        Buf b;
+        KB_TRY(alloc_buf(ctx, (size_t)range * sizeof(u32), &b));
+        tabs.push_back(b);
+        st[k].tab = static_cast<u32*>(b->p);
+        st[k].clear = true;  // cleared by the scan (scan_impl)
+        st[k].kmin = kmn; st[k].range = range; st[k].cshift = cshift;
+        st[k].key_is_o = q.key_pos[k] == 2 ? 1u : 0u;
+        st[k].trusted = (!q.pats[k].p.is_var && ctx->single_valued.count({q.pats[k].p.value, q.key_pos[k]})) ? 1u : 0u;
+        st[k].dup_flag = ctx->ctrl + off + 8 + t;
+        dt[t] = DirectTab{};
+        dt[t].tab = st[k].tab; dt[t].kmin = kmn; dt[t].range = range; dt[t].cshift = cshift;
+        out_slots.push_back(q.pv[k][q.key_pos[k] == 0 ? 1 : 0]);
+        ocs.push_back(OutCol{OUT_TABVAL, t, 0});
+        tab_of[k] = t;
+        t++;
+    }
+    timer_end(ctx);
+    std::vector<std::unique_ptr<kb_rel>> rels;
+    KB_TRY(scan_impl(ctx, q.pats, K, q.pushdown, false, true, &rels, &st));
+    ctx->stats.fused_scan_builds++;
+    // duplicate keys: the scan stores without reading back, so a multi-valued key shows up as fewer occupied slots than
+    // inserted rows. Tables of (predicate, position) pairs already verified for this store version are not re-counted.
+    bool counted = false;
+    const u32 offc = ctrl_alloc(ctx, MAXT);
+    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + offc, 0, MAXT * sizeof(u32), ctx->st));
+    for (u32 k = 0; k < K; k++) {
+        if ((int)k == probe_k || st[k].trusted) continue;
+        if (!counted) timer_begin(ctx, F_BUILD, 0);
+        counted = true;
+        ctx->stats.kernel_launches++;
+        launch_count_nonempty(st[k].tab, range, ctx->ctrl + offc + tab_of[k], ctx->n_sms, ctx->st);
+    }
+    if (counted) timer_end(ctx);  // the counts are read together with the probe's result: no extra synchronisation
+    auto check_dups = [&]() -> bool {
+        bool dup = false;
+        for (u32 k = 0; k < K; k++) {
+            if ((int)k == probe_k) continue;
+            const bool fewer = !st[k].trusted && ctx->h_ctrl[offc + tab_of[k]] != rels[k]->n;
+            if (ctx->h_ctrl[off + 8 + tab_of[k]] || fewer) {
+                dup = true;
+                if (!q.pats[k].p.is_var) ctx->multi_valued.insert({q.pats[k].p.value, q.key_pos[k]});
             }
-            timer_end(ctx);
-            const u32 T = t;
-            std::vector<std::unique_ptr<kb_rel>> rels;
-            KB_TRY(scan_impl(ctx, pats, K, pushdown, false, true, &rels, &st));
-            ctx->stats.fused_scan_builds++;
-            // duplicate keys: the scan stores without reading back, so a multi-valued key shows up as fewer occupied slots than
-            // inserted rows. Tables of (predicate, position) pairs already verified for this store version are not re-counted.
-            bool counted = false;
-            const u32 offc = ctrl_alloc(ctx, MAXT);
-            KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + offc, 0, MAXT * sizeof(u32), ctx->st));
-            for (u32 k = 0; k < K; k++) {
-                if ((int)k == probe_k || st[k].trusted) continue;
-                if (!counted) timer_begin(ctx, F_BUILD, 0);
-                counted = true;
-                ctx->stats.kernel_launches++;
-                launch_count_nonempty(st[k].tab, range, ctx->ctrl + offc + tab_of[k], ctx->n_sms, ctx->st);
-            }
-            if (counted) timer_end(ctx);  // the counts are read together with the probe's result: no extra synchronisation
-            auto check_dups = [&]() -> bool {
-                bool dup = false;
-                for (u32 k = 0; k < K; k++) {
-                    if ((int)k == probe_k) continue;
-                    const bool fewer = !st[k].trusted && ctx->h_ctrl[offc + tab_of[k]] != rels[k]->n;
-                    if (ctx->h_ctrl[off + 8 + tab_of[k]] || fewer) {
-                        dup = true;
-                        if (!pats[k].p.is_var) ctx->multi_valued.insert({pats[k].p.value, key_pos(k)});
+        }
+        return dup;
+    };
+    for (u32 k = 0; k < K; k++) if ((int)k != probe_k) ctx->stats.rows_built += rels[k]->n;
+    *route = Route::answered;
+    for (u32 k = 0; k < K; k++) if (rels[k]->n == 0) return empty_rel(ctx, q.all_slots, out);
+    for (u32 k = 0; k < K; k++) if ((int)k != probe_k && ctx->h_ctrl[off + 8 + tab_of[k]]) {  // key outside the table range (cannot happen with store statistics)
+        KB_TRY(ctrl_read(ctx));
+        check_dups();
+        *route = Route::retry;
+        return KB_OK;
+    }
+    const kb_rel& PR = *rels[probe_k];
+    auto res = std::make_unique<kb_rel>();
+    res->slots = out_slots;
+    std::vector<FilterOp> fops;
+    KB_TRY(compile_prog(ctx, q.post, out_slots, &fops));
+    const u32 off2 = ctrl_alloc(ctx, 8);
+    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off2, 0, 8 * sizeof(u32), ctx->st));
+    ProbeFParams P{};
+    KB_TRY(probe_fast(ctx, P, reinterpret_cast<const uint2*>(PR.cols[0].ptr), PR.n, q.key_pos[probe_k] == 2 ? 1u : 0u, dt, t, ocs, fops,
+                      ctx->ctrl + off2, nullptr, res.get()));
+    KB_TRY(ctrl_read(ctx));
+    if (check_dups()) { *route = Route::retry; return KB_OK; }
+    for (u32 k = 0; k < K; k++)
+        if ((int)k != probe_k && !q.pats[k].p.is_var && q.pushdown[k].ops.empty()) ctx->single_valued.insert({q.pats[k].p.value, q.key_pos[k]});
+    res->n = ctx->h_ctrl[off2 + 1];
+    *out = select_cols(*res, q.all_slots);
+    return KB_OK;
+}
+
+// R5: natural joins of `cur` (null: the probe relation) with the relations `rest`, smallest build sides first; the post-filter rides on
+// the last one
+static kb_status chained_join(kb_ctx* ctx, const StarQuery& q, std::vector<std::unique_ptr<kb_rel>>& rels, u32 probe, std::unique_ptr<kb_rel> cur,
+                              std::vector<u32> rest, std::unique_ptr<kb_rel>* out) {
+    for (auto& r : rels) KB_TRY(unpair_rel(ctx, &r));
+    if (!cur) cur = std::move(rels[probe]);
+    std::sort(rest.begin(), rest.end(), [&](u32 a, u32 b) { return rels[a]->n < rels[b]->n; });
+    for (size_t i = 0; i < rest.size(); i++) {
+        std::unique_ptr<kb_rel> j;
+        KB_TRY(hash_join_impl(ctx, *cur, *rels[rest[i]], (i + 1 == rest.size() && !q.post.ops.empty()) ? &q.post : nullptr, &j));
+        cur = std::move(j);
+    }
+    *out = select_cols(*cur, q.all_slots);
+    return KB_OK;
+}
+
+// R4: direct tables over the key range [kmin, kmin + range), built in batches of at most MAXT per probe launch; the first batch over
+// pair relations takes the register-staged fast probe. A build side that meets a duplicate key hands what is left to R5
+static kb_status batched_join(kb_ctx* ctx, const StarQuery& q, std::vector<std::unique_ptr<kb_rel>>& rels, u32 probe, const std::vector<u32>& builds,
+                              u32 kmin, u32 range, std::unique_ptr<kb_rel>* out) {
+    std::unique_ptr<kb_rel> cur;  // result of the batches done so far (columnar); null = still the scan output of `probe`
+    bool dup_seen = false;
+    size_t done = 0;
+    while (done < builds.size() && !dup_seen) {
+        const size_t nb = std::min<size_t>(MAXT, builds.size() - done);
+        const bool last = done + nb == builds.size();
+        const bool fast = q.all_pairs && !cur;  // first batch over pair relations -> register-staged fast probe
+        const kb_rel& PR = cur ? *cur : *rels[probe];
+        const u32 off = ctrl_alloc(ctx, 8 + MAXT);
+        KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, (8 + MAXT) * sizeof(u32), ctx->st));
+        std::vector<Buf> tables(nb);
+        DirectTab dt[MAXT];
+        std::vector<u32> out_slots = PR.slots;
+        std::vector<OutCol> ocs;
+        for (u32 c = 0; c < (u32)PR.slots.size(); c++) ocs.push_back(OutCol{OUT_PROBE, c, 0});
+        timer_begin(ctx, F_BUILD, (int)nb);
+        for (size_t t = 0; t < nb; t++) KB_TRY(alloc_buf(ctx, (size_t)range * sizeof(u32), &tables[t]));  // stream-ordered on st
+        if (nb > 1) {  // independent tables: odd ones are memset + built on the second stream, concurrently with the even ones
+            KB_CUDA(ctx, cudaEventRecord(ctx->ev_fork, ctx->st));
+            KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st2, ctx->ev_fork, 0));
+        }
+        for (size_t t = 0; t < nb; t++) {
+            const u32 k = builds[done + t];
+            const kb_rel& B = *rels[k];
+            cudaStream_t bs = (nb > 1 && (t & 1)) ? ctx->st2 : ctx->st;
+            u32* tab = static_cast<u32*>(tables[t]->p);
+            KB_CUDA(ctx, cudaMemsetAsync(tab, 0xFF, (size_t)range * sizeof(u32), bs));
+            DirectTab& D = dt[t];
+            D = DirectTab{};
+            D.tab = tab; D.kmin = kmin; D.range = range;
+            const int kc = B.col_of(q.join_slot);
+            if (B.pair) {
+                out_slots.push_back(B.slots[kc == 0 ? 1 : 0]);
+                ocs.push_back(OutCol{OUT_TABVAL, (u32)t, 0});
+                const u32 trusted = (!q.pats[k].p.is_var && ctx->single_valued.count({q.pats[k].p.value, q.key_pos[k]})) ? 1u : 0u;
+                launch_build_direct_pairs(reinterpret_cast<const uint2*>(B.cols[0].ptr), kc == 1 ? 1u : 0u, (u32)B.n, tab, kmin, range, 0u,
+                                          ctx->ctrl + off + 8 + (u32)t, trusted, ctx->n_sms, bs);
+            } else {
+                const u32* vals = nullptr;
+                if (B.cols.size() == 1) { D.mode = 2; }
+                else if (B.cols.size() == 2) {
+                    const int vc = kc == 0 ? 1 : 0;
+                    vals = B.cols[vc].ptr;
+                    out_slots.push_back(B.slots[vc]);
+                    ocs.push_back(OutCol{OUT_TABVAL, (u32)t, 0});
+                } else {
+                    D.mode = 1;
+                    for (size_t c = 0; c < B.cols.size(); c++) if ((int)c != kc) {
+                        D.pay[D.n_pay] = B.cols[c].ptr;
+                        out_slots.push_back(B.slots[c]);
+                        ocs.push_back(OutCol{OUT_TABPAY, (u32)t, D.n_pay});
+                        D.n_pay++;
                     }
                 }
-                return dup;
-            };
-            for (u32 k = 0; k < K; k++) if ((int)k != probe_k) ctx->stats.rows_built += rels[k]->n;
-            auto empty_result2 = [&]() -> kb_status {
-                auto r = std::make_unique<kb_rel>();
-                r->slots = all_slots;
-                for (size_t c = 0; c < all_slots.size(); c++) { Col col; KB_TRY(alloc_col(ctx, 0, &col)); r->cols.push_back(col); }
-                *out = std::move(r);
-                return KB_OK;
-            };
-            for (u32 k = 0; k < K; k++) if (rels[k]->n == 0) return empty_result2();
-            for (u32 k = 0; k < K; k++) if ((int)k != probe_k && ctx->h_ctrl[off + 8 + tab_of[k]]) {  // key outside the table range (cannot happen with store statistics)
-                KB_TRY(ctrl_read(ctx));
-                check_dups();
-                return star_join_impl2(ctx, join_slot, pats, K, filter, n_ops, false, out, agg);
+                launch_build_direct(B.cols[kc].ptr, vals, (u32)B.n, tab, kmin, range, 0u, ctx->ctrl + off + 8 + (u32)t, ctx->n_sms, bs);
             }
-            const kb_rel& PR = *rels[probe_k];
-            auto res = std::make_unique<kb_rel>();
-            res->slots = out_slots;
-            const u32 n_out = (u32)out_slots.size();
-            std::vector<FilterOp> fops;
-            if (!post.ops.empty()) {
-                std::map<u32, u32> remap;
-                for (u32 c = 0; c < n_out; c++) remap[out_slots[c]] = c;
-                if (!append_prog(&fops, post, remap)) return fail(ctx, KB_E_INVALID, "filter uses an unbound variable");
-            }
+            ctx->stats.rows_built += B.n;
+        }
+        if (nb > 1) {
+            KB_CUDA(ctx, cudaEventRecord(ctx->ev_join, ctx->st2));
+            KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st, ctx->ev_join, 0));
+        }
+        timer_end(ctx);
+        auto res = std::make_unique<kb_rel>();
+        res->slots = out_slots;
+        std::vector<FilterOp> fops;
+        if (last) KB_TRY(compile_prog(ctx, q.post, out_slots, &fops));
+        if (fast) {
             ProbeFParams P{};
-            P.pairs = reinterpret_cast<const uint2*>(PR.cols[0].ptr);
-            P.key_is_y = key_pos((u32)probe_k) == 2 ? 1u : 0u;
+            KB_TRY(probe_fast(ctx, P, reinterpret_cast<const uint2*>(PR.cols[0].ptr), PR.n, PR.col_of(q.join_slot) == 1 ? 1u : 0u, dt, (u32)nb, ocs, fops,
+                              ctx->ctrl + off, ctx->ctrl + off + 8, res.get()));
+        } else {
+            ProbeDParams P{};  // columnar input: the previous batch's result, or a scan without pair output (not all_pairs)
+            P.n_pcols = (u32)PR.cols.size();
+            for (u32 c = 0; c < P.n_pcols; c++) P.pcol[c] = PR.cols[c].ptr;
+            P.key_col = (u32)PR.col_of(q.join_slot);
             P.n = (u32)PR.n;
-            P.n_tiles = (u32)((PR.n + PROBEF_TILE - 1) / PROBEF_TILE);
-            P.T = T;
-            for (u32 q = 0; q < T; q++) P.tab[q] = dt[q];
-            P.n_out = n_out;
-            for (u32 c = 0; c < n_out; c++) {
-                Col col;
-                KB_TRY(alloc_col(ctx, PR.n, &col));
-                res->cols.push_back(col);
-                P.oc[c] = ocs[c];
-                P.out[c] = col.ptr;
-            }
-            P.cap = (u32)PR.n;
-            P.n_ops = (u32)fops.size();
-            for (size_t i = 0; i < fops.size(); i++) P.ops[i] = fops[i];
-            P.nt = numtab(ctx);
-            KB_TRY(ensure_tile_state(ctx, P.n_tiles));
-            P.tile_state = static_cast<u64*>(ctx->tile_state->p);
-            P.block_state = static_cast<u64*>(ctx->block_state->p);
-            P.ordered = ctx->ordered;
-            const u32 off2 = ctrl_alloc(ctx, 8);
-            KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off2, 0, 8 * sizeof(u32), ctx->st));
-            P.ticket = ctx->ctrl + off2;
-            P.total = ctx->ctrl + off2 + 1;
-            P.zero_word = ctx->ctrl + off2 + 2;
-            P.abort_flag = nullptr;
-            P.epoch = ctx->epoch++;
+            P.n_tiles = (u32)((PR.n + PROBE_TILE - 1) / PROBE_TILE);
+            P.T = (u32)nb;
+            for (size_t t = 0; t < nb; t++) P.tab[t] = dt[t];
+            KB_TRY(probe_setup(ctx, &P, PR.n, ocs, fops, ctx->ctrl + off, ctx->ctrl + off + 8, res.get()));
             timer_begin(ctx, F_PROBE);
-            launch_probe_fast(P, ctx->n_sms, ctx->st);
+            launch_probe_direct(P, ctx->n_sms, ctx->st);
             timer_end(ctx);
             KB_CUDA(ctx, cudaGetLastError());
             ctx->stats.rows_probed += PR.n;
-            KB_TRY(ctrl_read(ctx));
-            if (check_dups())  // a build side is multi-valued: redo without the fusion (the chained operator needs the build rows)
-                return star_join_impl2(ctx, join_slot, pats, K, filter, n_ops, false, out, agg);
-            for (u32 k = 0; k < K; k++)
-                if ((int)k != probe_k && !pats[k].p.is_var && pushdown[k].ops.empty()) ctx->single_valued.insert({pats[k].p.value, key_pos(k)});
-            res->n = ctx->h_ctrl[off2 + 1];
-            *out = select_cols(*res, all_slots);
-            return KB_OK;
         }
+        KB_TRY(ctrl_read(ctx));
+        for (size_t t = 0; t < nb; t++) if (ctx->h_ctrl[off + 8 + t]) {
+            dup_seen = true;
+            const u32 k = builds[done + t];
+            if (!q.pats[k].p.is_var) ctx->multi_valued.insert({q.pats[k].p.value, q.key_pos[k]});
+        }
+        if (dup_seen) break;
+        for (size_t t = 0; t < nb; t++) {  // verified duplicate-free: later builds of the same (predicate, key position) use plain stores
+            const u32 k = builds[done + t];
+            // only when the build side was the WHOLE (?s P ?o) relation: a filtered subset proves nothing about the rest
+            if (!q.pats[k].p.is_var && rels[k]->pair && q.pushdown[k].ops.empty()) ctx->single_valued.insert({q.pats[k].p.value, q.key_pos[k]});
+        }
+        res->n = ctx->h_ctrl[off + 1];
+        cur = std::move(res);
+        done += nb;
+        if (cur->n == 0) return empty_rel(ctx, q.all_slots, out);
     }
+    if (!dup_seen) {
+        *out = select_cols(*cur, q.all_slots);
+        return KB_OK;
+    }
+    // a build side has duplicate keys: join what is left with the chained (multimap) operator
+    return chained_join(ctx, q, rels, probe, std::move(cur), std::vector<u32>(builds.begin() + done, builds.end()), out);
+}
 
+// R4 / R5: every pattern is scanned (or looked up in the index), then joined by direct tables (R4) or chained joins (R5)
+static kb_status scan_join(kb_ctx* ctx, const StarQuery& q, std::unique_ptr<kb_rel>* out) {
+    const u32 K = q.K;
     std::vector<std::unique_ptr<kb_rel>> rels;
-    KB_TRY(scan_impl(ctx, pats, K, pushdown, false, all_pairs, &rels));
+    KB_TRY(scan_impl(ctx, q.pats, K, q.pushdown, false, q.all_pairs, &rels));
     if (ctx->upload_stats_off >= 0) {  // one-shot host call: the copy stream computed the column ranges chunk by chunk
         const u32 o = (u32)ctx->upload_stats_off;
         for (auto& sg : ctx->segs) {
@@ -1551,26 +1664,13 @@ kb_status star_join_impl2(kb_ctx* ctx, u32 join_slot, const kb_pattern* pats, u3
         }
         ctx->upload_stats_off = -1;
     }
-    u32 kmin = 0xFFFFFFFFu, kmax = 0;
-    for (auto& sg : ctx->segs) {
-        if (sg.n == 0) continue;
-        if (!sg.has_stats) KB_TRY(segment_stats(ctx, &sg));
-        for (u32 k = 0; k < K; k++) { const u32 c = key_pos(k); kmin = std::min(kmin, sg.cmin[c]); kmax = std::max(kmax, sg.cmax[c]); }
-    }
-
-    auto empty_result = [&]() -> kb_status {
-        auto r = std::make_unique<kb_rel>();
-        r->slots = all_slots;
-        for (size_t c = 0; c < all_slots.size(); c++) { Col col; KB_TRY(alloc_col(ctx, 0, &col)); r->cols.push_back(col); }
-        *out = std::move(r);
-        return KB_OK;
-    };
-    for (u32 k = 0; k < K; k++) if (rels[k]->n == 0) return empty_result();
-
+    u32 kmin, kmax;
+    KB_TRY(store_key_range(ctx, q, &kmin, &kmax));
+    for (u32 k = 0; k < K; k++) if (rels[k]->n == 0) return empty_rel(ctx, q.all_slots, out);
     if (K == 1) {
         std::unique_ptr<kb_rel> r = std::move(rels[0]);
         KB_TRY(unpair_rel(ctx, &r));
-        if (!post.ops.empty()) { std::unique_ptr<kb_rel> f; KB_TRY(filter_impl(ctx, *r, post, &f)); r = std::move(f); }
+        if (!q.post.ops.empty()) { std::unique_ptr<kb_rel> f; KB_TRY(filter_impl(ctx, *r, q.post, &f)); r = std::move(f); }
         *out = std::move(r);
         return KB_OK;
     }
@@ -1579,216 +1679,33 @@ kb_status star_join_impl2(kb_ctx* ctx, u32 join_slot, const kb_pattern* pats, u3
     for (u32 k = 1; k < K; k++) if (rels[k]->n > rels[probe]->n) probe = k;
     std::vector<u32> builds;
     for (u32 k = 0; k < K; k++) if (k != probe) builds.push_back(k);
-
-    // the fused path needs: patterns share only the join variable (quirk Q3: the reference never checks the others — we must,
-    // so such shapes take the natural-join chain), a dense key range, and single-valued keys
-    bool fused_ok = kmax >= kmin;
-    for (u32 a = 0; a < K && fused_ok; a++)
-        for (u32 b = a + 1; b < K && fused_ok; b++)
-            for (u32 s2 : pv[a]) if (s2 != join_slot && std::find(pv[b].begin(), pv[b].end(), s2) != pv[b].end()) fused_ok = false;
+    // direct tables need: patterns that share only the join variable, a dense key range, and single-valued keys
+    bool fused_ok = kmax >= kmin && q.only_join_shared;
     const u64 range64 = fused_ok ? (u64)kmax - kmin + 1 : 0;
     for (u32 k : builds) {
         if (range64 > std::max<u64>(8 * rels[k]->n, 1ull << 16) || range64 > (1ull << 31)) fused_ok = false;
-        if (!pats[k].p.is_var && ctx->multi_valued.count({pats[k].p.value, key_pos(k)})) fused_ok = false;
-        if (pv[k].size() > 3) fused_ok = false;
+        if (!q.pats[k].p.is_var && ctx->multi_valued.count({q.pats[k].p.value, q.key_pos[k]})) fused_ok = false;
+        if (q.pv[k].size() > 3) fused_ok = false;
     }
-    const u32 range = (u32)range64;
+    if (fused_ok) return batched_join(ctx, q, rels, probe, builds, kmin, (u32)range64, out);
+    return chained_join(ctx, q, rels, probe, nullptr, builds, out);
+}
 
-    auto to_columnar = [&]() -> kb_status {
-        for (u32 k = 0; k < K; k++) KB_TRY(unpair_rel(ctx, &rels[k]));
-        return KB_OK;
-    };
-
-    if (fused_ok) {
-        std::unique_ptr<kb_rel> cur;  // result of the batches done so far (columnar); null = still the scan output of `probe`
-        bool dup_seen = false;
-        size_t done = 0;
-        while (done < builds.size() && !dup_seen) {
-            const size_t nb = std::min<size_t>(MAXT, builds.size() - done);
-            const bool last = done + nb == builds.size();
-            const bool fast = all_pairs && !cur;  // first batch over pair relations -> register-staged fast probe
-            const kb_rel& PR = cur ? *cur : *rels[probe];
-            const u32 off = ctrl_alloc(ctx, 8 + MAXT);
-            KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, (8 + MAXT) * sizeof(u32), ctx->st));
-            std::vector<Buf> tables(nb);
-            DirectTab dt[MAXT];
-            std::vector<u32> out_slots = PR.slots;
-            std::vector<OutCol> ocs;
-            for (u32 c = 0; c < (u32)PR.slots.size(); c++) ocs.push_back(OutCol{OUT_PROBE, c, 0});
-            timer_begin(ctx, F_BUILD, (int)nb);
-            for (size_t t = 0; t < nb; t++) KB_TRY(alloc_buf(ctx, (size_t)range * sizeof(u32), &tables[t]));  // stream-ordered on st
-            if (nb > 1) {  // independent tables: odd ones are memset + built on the second stream, concurrently with the even ones
-                KB_CUDA(ctx, cudaEventRecord(ctx->ev_fork, ctx->st));
-                KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st2, ctx->ev_fork, 0));
-            }
-            for (size_t t = 0; t < nb; t++) {
-                const u32 k = builds[done + t];
-                const kb_rel& B = *rels[k];
-                cudaStream_t bs = (nb > 1 && (t & 1)) ? ctx->st2 : ctx->st;
-                u32* tab = static_cast<u32*>(tables[t]->p);
-                KB_CUDA(ctx, cudaMemsetAsync(tab, 0xFF, (size_t)range * sizeof(u32), bs));
-                DirectTab& D = dt[t];
-                D.tab = tab; D.kmin = kmin; D.range = range; D.cshift = 0; D.n_pay = 0; D.pay[0] = D.pay[1] = nullptr;
-                const int kc = B.col_of(join_slot);
-                if (B.pair) {
-                    D.mode = 0;
-                    out_slots.push_back(B.slots[kc == 0 ? 1 : 0]);
-                    ocs.push_back(OutCol{OUT_TABVAL, (u32)t, 0});
-                    const u32 trusted = (!pats[k].p.is_var && ctx->single_valued.count({pats[k].p.value, key_pos(k)})) ? 1u : 0u;
-                    launch_build_direct_pairs(reinterpret_cast<const uint2*>(B.cols[0].ptr), kc == 1 ? 1u : 0u, (u32)B.n, tab, kmin, range, 0u,
-                                              ctx->ctrl + off + 8 + (u32)t, trusted, ctx->n_sms, bs);
-                } else {
-                    const u32* vals = nullptr;
-                    if (B.cols.size() == 1) { D.mode = 2; }
-                    else if (B.cols.size() == 2) {
-                        D.mode = 0;
-                        const int vc = kc == 0 ? 1 : 0;
-                        vals = B.cols[vc].ptr;
-                        out_slots.push_back(B.slots[vc]);
-                        ocs.push_back(OutCol{OUT_TABVAL, (u32)t, 0});
-                    } else {
-                        D.mode = 1;
-                        for (size_t c = 0; c < B.cols.size(); c++) if ((int)c != kc) {
-                            D.pay[D.n_pay] = B.cols[c].ptr;
-                            out_slots.push_back(B.slots[c]);
-                            ocs.push_back(OutCol{OUT_TABPAY, (u32)t, D.n_pay});
-                            D.n_pay++;
-                        }
-                    }
-                    launch_build_direct(B.cols[kc].ptr, vals, (u32)B.n, tab, kmin, range, 0u, ctx->ctrl + off + 8 + (u32)t, ctx->n_sms, bs);
-                }
-                ctx->stats.rows_built += B.n;
-            }
-            if (nb > 1) {
-                KB_CUDA(ctx, cudaEventRecord(ctx->ev_join, ctx->st2));
-                KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st, ctx->ev_join, 0));
-            }
-            timer_end(ctx);
-            auto res = std::make_unique<kb_rel>();
-            res->slots = out_slots;
-            const u32 n_out = (u32)out_slots.size();
-            std::vector<FilterOp> fops;
-            if (last && !post.ops.empty()) {
-                std::map<u32, u32> remap;
-                for (u32 c = 0; c < n_out; c++) remap[out_slots[c]] = c;
-                if (!append_prog(&fops, post, remap)) return fail(ctx, KB_E_INVALID, "filter uses an unbound variable");
-            }
-            std::vector<u32*> outp(n_out);
-            for (u32 c = 0; c < n_out; c++) {
-                Col col;
-                KB_TRY(alloc_col(ctx, PR.n, &col));
-                res->cols.push_back(col);
-                outp[c] = col.ptr;
-            }
-            if (fast) {
-                ProbeFParams P{};
-                P.pairs = reinterpret_cast<const uint2*>(PR.cols[0].ptr);
-                P.key_is_y = PR.col_of(join_slot) == 1 ? 1u : 0u;
-                P.n = (u32)PR.n;
-                P.n_tiles = (u32)((PR.n + PROBEF_TILE - 1) / PROBEF_TILE);
-                P.T = (u32)nb;
-                for (size_t t = 0; t < nb; t++) P.tab[t] = dt[t];
-                P.n_out = n_out;
-                for (u32 c = 0; c < n_out; c++) { P.oc[c] = ocs[c]; P.out[c] = outp[c]; }
-                P.cap = (u32)PR.n;
-                P.n_ops = (u32)fops.size();
-                for (size_t i = 0; i < fops.size(); i++) P.ops[i] = fops[i];
-                P.nt = numtab(ctx);
-                KB_TRY(ensure_tile_state(ctx, P.n_tiles));
-                P.tile_state = static_cast<u64*>(ctx->tile_state->p);
-                P.block_state = static_cast<u64*>(ctx->block_state->p);
-                P.ordered = ctx->ordered;
-                P.ticket = ctx->ctrl + off;
-                P.total = ctx->ctrl + off + 1;
-                P.zero_word = ctx->ctrl + off + 2;
-                P.abort_flag = ctx->ctrl + off + 8;
-                P.epoch = ctx->epoch++;
-                timer_begin(ctx, F_PROBE);
-                launch_probe_fast(P, ctx->n_sms, ctx->st);
-                timer_end(ctx);
-            } else {
-                std::unique_ptr<kb_rel> tmp;
-                const kb_rel* src = &PR;
-                if (PR.pair) {  // generic probe reads columnar input
-                    tmp = std::make_unique<kb_rel>();
-                    tmp->slots = PR.slots; tmp->cols = PR.cols; tmp->n = PR.n; tmp->pair = true;
-                    KB_TRY(unpair_rel(ctx, &tmp));
-                    src = tmp.get();
-                }
-                ProbeDParams P{};
-                P.n_pcols = (u32)src->cols.size();
-                for (u32 c = 0; c < P.n_pcols; c++) P.pcol[c] = src->cols[c].ptr;
-                P.key_col = (u32)src->col_of(join_slot);
-                P.n = (u32)src->n;
-                P.n_tiles = (u32)((src->n + PROBE_TILE - 1) / PROBE_TILE);
-                P.T = (u32)nb;
-                for (size_t t = 0; t < nb; t++) P.tab[t] = dt[t];
-                P.n_out = n_out;
-                for (u32 c = 0; c < n_out; c++) { P.oc[c] = ocs[c]; P.out[c] = outp[c]; }
-                P.cap = (u32)src->n;
-                P.n_ops = (u32)fops.size();
-                for (size_t i = 0; i < fops.size(); i++) P.ops[i] = fops[i];
-                P.nt = numtab(ctx);
-                KB_TRY(ensure_tile_state(ctx, P.n_tiles));
-                P.tile_state = static_cast<u64*>(ctx->tile_state->p);
-                P.block_state = static_cast<u64*>(ctx->block_state->p);
-                P.ordered = ctx->ordered;
-                P.ticket = ctx->ctrl + off;
-                P.total = ctx->ctrl + off + 1;
-                P.zero_word = ctx->ctrl + off + 2;
-                P.abort_flag = ctx->ctrl + off + 8;
-                P.epoch = ctx->epoch++;
-                timer_begin(ctx, F_PROBE);
-                launch_probe_direct(P, ctx->n_sms, ctx->st);
-                timer_end(ctx);
-            }
-            KB_CUDA(ctx, cudaGetLastError());
-            ctx->stats.rows_probed += PR.n;
-            KB_TRY(ctrl_read(ctx));
-            for (size_t t = 0; t < nb; t++) if (ctx->h_ctrl[off + 8 + t]) {
-                dup_seen = true;
-                const u32 k = builds[done + t];
-                if (!pats[k].p.is_var) ctx->multi_valued.insert({pats[k].p.value, key_pos(k)});
-            }
-            if (dup_seen) break;
-            for (size_t t = 0; t < nb; t++) {  // verified duplicate-free: later builds of the same (predicate, key position) use plain stores
-                const u32 k = builds[done + t];
-                // only when the build side was the WHOLE (?s P ?o) relation: a filtered subset proves nothing about the rest
-                if (!pats[k].p.is_var && rels[k]->pair && pushdown[k].ops.empty()) ctx->single_valued.insert({pats[k].p.value, key_pos(k)});
-            }
-            res->n = ctx->h_ctrl[off + 1];
-            cur = std::move(res);
-            done += nb;
-            if (cur->n == 0) return empty_result();
-        }
-        if (!dup_seen) {
-            *out = select_cols(*cur, all_slots);
-            return KB_OK;
-        }
-        // a build side has duplicate keys: join what is left with the chained (multimap) operator
-        KB_TRY(to_columnar());
-        if (!cur) cur = std::move(rels[probe]);
-        std::vector<u32> rest(builds.begin() + done, builds.end());
-        std::sort(rest.begin(), rest.end(), [&](u32 a, u32 b) { return rels[a]->n < rels[b]->n; });
-        for (size_t i = 0; i < rest.size(); i++) {
-            std::unique_ptr<kb_rel> j;
-            KB_TRY(hash_join_impl(ctx, *cur, *rels[rest[i]], (i + 1 == rest.size() && !post.ops.empty()) ? &post : nullptr, &j));
-            cur = std::move(j);
-        }
-        *out = select_cols(*cur, all_slots);
-        return KB_OK;
-    }
-    // general chain: natural joins, smallest build sides first
-    KB_TRY(to_columnar());
-    std::unique_ptr<kb_rel> cur = std::move(rels[probe]);
-    std::sort(builds.begin(), builds.end(), [&](u32 a, u32 b) { return rels[a]->n < rels[b]->n; });
-    for (size_t i = 0; i < builds.size(); i++) {
-        std::unique_ptr<kb_rel> j;
-        KB_TRY(hash_join_impl(ctx, *cur, *rels[builds[i]], (i + 1 == builds.size() && !post.ops.empty()) ? &post : nullptr, &j));
-        cur = std::move(j);
-    }
-    *out = select_cols(*cur, all_slots);
-    return KB_OK;
+kb_status star_join_impl(kb_ctx* ctx, u32 join_slot, const kb_pattern* pats, u32 K, const kb_filter_op* filter, u32 n_ops,
+                         std::unique_ptr<kb_rel>* out, AggSpec* agg) {
+    StarQuery q;
+    KB_TRY(star_query(ctx, join_slot, pats, K, filter, n_ops, &q));
+    const IndexSlices ix = index_slices(ctx, q);  // R1 and R2 read it; neither changes what it describes
+    Route r;
+    do {  // R2's duplicate key: the pair is now cached as multi-valued — start again from the top, with the index allowed
+        KB_TRY(index_join_one_kernel(ctx, q, ix, agg, out, &r));
+        if (r == Route::declined) KB_TRY(index_join_built(ctx, q, ix, out, &r));
+    } while (r == Route::retry);
+    if (r == Route::answered) return KB_OK;
+    KB_TRY(fused_scan_join(ctx, q, out, &r));
+    if (r == Route::answered) return KB_OK;
+    // declined, or a duplicate / out-of-range key in R3's tables (r == Route::retry): scan again, without the index and the fusion
+    return scan_join(ctx, q, out);
 }
 
 }  // namespace kb
@@ -1809,12 +1726,7 @@ kb_status group_table_create(kb_ctx* ctx, u64 slots, GroupParams* P, GroupTable*
     t->o_state = t->o_keys + slots * 4 * sizeof(u32);
     t->bytes = t->o_state + slots * sizeof(u32);
     KB_TRY(alloc_buf(ctx, t->bytes, &t->buf));
-    char* tb = static_cast<char*>(t->buf->p);
-    P->n_slots = (u32)slots;
-    P->gval = (double*)(tb + t->o_val);
-    P->gcnt = (unsigned long long*)(tb + t->o_cnt);
-    P->gkeys = (u32*)(tb + t->o_keys);
-    P->gstate = (u32*)(tb + t->o_state);
+    t->point(P, static_cast<char*>(t->buf->p));
     launch_group_init(*P, ctx->st);
     return KB_OK;
 }
@@ -2968,24 +2880,9 @@ kb_status kb_bgp_execute(kb_ctx* ctx, const kb_pattern* pats, uint32_t n_pats, c
         KB_TRY(kb::star_join_impl(ctx, (u32)star, pats, n_pats, filter, n_ops, &cur));
     } else {
         // left-deep natural joins in textual order (build_logical_plan, utils.rs:101-191)
-        std::vector<kb::FilterProg> conj, pushdown(n_pats);
+        std::vector<kb::FilterProg> pushdown;
         kb::FilterProg post;
-        if (!kb::split_conjuncts(filter, n_ops, &conj)) return kb::fail(ctx, KB_E_INVALID, "malformed filter program");
-        for (auto& c : conj) {
-            std::set<u32> fs = kb::filter_slots(c);
-            for (u32 s : fs) if (std::find(all_slots.begin(), all_slots.end(), s) == all_slots.end())
-                return kb::fail(ctx, KB_E_UNSUPPORTED, "filter references slot %u which no pattern binds", s);
-            int target = -1;
-            for (u32 k = 0; k < n_pats && target < 0; k++) {
-                bool all = true;
-                for (u32 s : fs) if (std::find(pv[k].begin(), pv[k].end(), s) == pv[k].end()) all = false;
-                if (all) target = (int)k;
-            }
-            kb::FilterProg* dst = target >= 0 ? &pushdown[target] : &post;
-            const bool had = !dst->ops.empty();
-            dst->ops.insert(dst->ops.end(), c.ops.begin(), c.ops.end());
-            if (had) { kb_filter_op a{}; a.op = KB_F_AND; dst->ops.push_back(a); }
-        }
+        KB_TRY(kb::split_filter(ctx, filter, n_ops, pv, all_slots, &pushdown, &post));
         std::vector<std::unique_ptr<kb_rel>> rels;
         KB_TRY(kb::scan_impl(ctx, pats, n_pats, pushdown, false, false, &rels));
         cur = std::move(rels[0]);
@@ -3191,15 +3088,10 @@ kb_status kb_star_join_aggregate(kb_ctx* ctx, uint32_t join_slot, const kb_patte
     if (n_group == 0 || n_group > 4) return kb::fail(ctx, KB_E_LIMIT, "GROUP BY takes 1..4 variables");
     if (n_aggs > 8) return kb::fail(ctx, KB_E_LIMIT, "at most 8 aggregates");
     for (u32 a = 0; a < n_aggs; a++) if (aggs[a].kind > KB_AGG_AVG) return kb::fail(ctx, KB_E_INVALID, "unknown aggregate kind %u", aggs[a].kind);
-    kb::AggSpec spec;
     const bool fusable = n_group == 1 && n_aggs <= 1;
-    if (fusable) {
-        spec.group_slot = group_slots[0];
-        spec.has_agg = n_aggs == 1;
-        if (n_aggs) { spec.kind = aggs[0].kind; spec.agg_slot = aggs[0].slot; }
-    }
+    kb::AggSpec spec(group_slots[0], n_aggs ? aggs : nullptr);
     std::unique_ptr<kb_rel> rel;
-    KB_TRY(kb::star_join_impl2(ctx, join_slot, pats, n_pats, filter, n_ops, true, &rel, fusable ? &spec : nullptr));
+    KB_TRY(kb::star_join_impl(ctx, join_slot, pats, n_pats, filter, n_ops, &rel, fusable ? &spec : nullptr));
     if (spec.applied) {
         if (n_rows) *n_rows = spec.n_rows;
         *out = spec.groups.release();

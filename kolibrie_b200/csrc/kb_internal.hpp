@@ -240,6 +240,7 @@ struct kb_ctx {
 namespace kb {
 
 kb_status fail(kb_ctx* ctx, kb_status code, const char* fmt, ...);
+inline size_t round256(size_t b) { return (b + 255) & ~(size_t)255; }
 #define KB_CUDA(ctx, call)                                                                                             \
     do {                                                                                                               \
         cudaError_t _e = (call);                                                                                       \
@@ -284,6 +285,8 @@ kb_status scan_impl(kb_ctx* ctx, const kb_pattern* pats, u32 n_pats, const std::
                     std::vector<std::unique_ptr<kb_rel>>* out, const std::vector<ScanTable>* tables = nullptr);
 // fused GROUP BY of a star join (kb_star_join_aggregate): in = group / aggregate spec; out = groups when the one-kernel index path took it
 struct AggSpec {
+    AggSpec() = default;
+    AggSpec(u32 group, const kb_agg* a) : group_slot(group), has_agg(a != nullptr), kind(a ? a->kind : 0u), agg_slot(a ? a->slot : 0u) {}
     u32 group_slot = 0;
     bool has_agg = false;
     u32 kind = 0, agg_slot = 0;
@@ -303,15 +306,29 @@ struct IndexPlan {
     bool agg = false;            // GROUP BY folded into the kernel (P.gsel / P.asel / P.akind are set)
     bool has_agg = false;
     u32 agg_kind = 0, agg_slot = 0, group_slot = 0;
+    const char* why = nullptr;   // not ok: what the one-kernel index path needs that the query lacks
 };
-// plan_only != nullptr: resolve the one-kernel index path and return without launching (KB_E_UNSUPPORTED when the query does not take it)
-kb_status star_join_impl2(kb_ctx* ctx, u32 join_slot, const kb_pattern* pats, u32 n_pats, const kb_filter_op* filter, u32 n_ops, bool allow_fused_scan,
-                          std::unique_ptr<kb_rel>* out, AggSpec* agg = nullptr, IndexPlan* plan_only = nullptr);
+// errors only for an invalid query; a query the one-kernel index path does not take leaves plan->ok false. agg: the GROUP BY is folded
+// into the plan (plan->agg) when the join binds its variables
+kb_status resolve_index_plan(kb_ctx* ctx, u32 join_slot, const kb_pattern* pats, u32 n_pats, const kb_filter_op* filter, u32 n_ops,
+                             const AggSpec* agg, IndexPlan* plan);
+// the output of the one-kernel index join: n_out columns of `rows` rows in one allocation
+kb_status alloc_index_out(kb_ctx* ctx, u64 rows, u32 n_out, std::vector<Col>* cols);
+// the row-writing launch of the one-kernel index join into such columns (P.epoch is set by the caller)
+kb_status launch_index_rows(kb_ctx* ctx, ProbeIParams& P, const std::vector<Col>& cols);
 // GROUP BY hash table on the device (kb_group_aggregate and the fused path): one buffer [val | cnt | keys | state]
 struct GroupTable {
     Buf buf;
     u64 slots = 0;
     size_t o_val = 0, o_cnt = 0, o_keys = 0, o_state = 0, bytes = 0;
+    // point P at a table of this layout that starts at `base` (this table's buffer, or a rank's copy in peer scratch)
+    void point(GroupParams* P, char* base) const {
+        P->n_slots = (u32)slots;
+        P->gval = (double*)(base + o_val);
+        P->gcnt = (unsigned long long*)(base + o_cnt);
+        P->gkeys = (u32*)(base + o_keys);
+        P->gstate = (u32*)(base + o_state);
+    }
 };
 kb_status group_table_create(kb_ctx* ctx, u64 slots, GroupParams* P, GroupTable* t);  // allocates, points P at it, runs the init kernel
 // downloads the table and appends its groups to g (AVG divided, COUNT filled in)
@@ -327,8 +344,9 @@ kb_status store_add_device_segment(kb_ctx* ctx, Segment& sg);
 kb_status unpair_rel(kb_ctx* ctx, std::unique_ptr<kb_rel>* r);
 kb_status filter_impl(kb_ctx* ctx, const kb_rel& in, const FilterProg& f, std::unique_ptr<kb_rel>* out);
 kb_status hash_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_rel& R, const FilterProg* post, std::unique_ptr<kb_rel>* out);
+// agg != nullptr (kb_star_join_aggregate): agg->applied when the GROUP BY was folded into the join, else *out is the joined relation
 kb_status star_join_impl(kb_ctx* ctx, u32 join_slot, const kb_pattern* pats, u32 n_pats, const kb_filter_op* filter, u32 n_ops,
-                         std::unique_ptr<kb_rel>* out);
+                         std::unique_ptr<kb_rel>* out, AggSpec* agg = nullptr);
 void pattern_vars(const kb_pattern& pt, std::vector<u32>* slots, std::vector<u32>* src);
 u32 pow2_at_least(u64 x);
 kb_status check_pattern(kb_ctx* ctx, const kb_pattern& pt);

@@ -19,8 +19,7 @@ struct kb_plan {
     IndexPlan ip;
     u32 ring = 0;
     struct Slot {
-        Buf out;                  // one allocation: n_out columns of probe_rows rows (row plans)
-        std::vector<Col> cols;
+        std::vector<Col> cols;    // row plans: n_out columns of probe_rows rows (alloc_index_out)
         GroupTable tab;           // aggregate plans: the device group table of this slot (the overflow word rides behind it) ...
         char* h_rec = nullptr;    // ... and the mapped pinned list its groups are compacted into: {u32 count, u32 overflow, pad} + GroupRecord[cap]
         char* d_rec = nullptr;
@@ -47,8 +46,6 @@ struct kb_plan {
 };
 
 namespace {
-inline size_t round256(size_t b) { return (b + 255) & ~(size_t)255; }
-
 struct DevGuard {
     int prev = -1;
     explicit DevGuard(int dev) {
@@ -85,16 +82,11 @@ kb_status kb_star_join_prepare(kb_ctx* ctx, uint32_t join_slot, const kb_pattern
         return fail(ctx, KB_E_UNSUPPORTED, "a prepared GROUP BY takes one variable and at most one aggregate (other shapes: kb_star_join + kb_group_aggregate)");
     if (!grouped && n_aggs) return fail(ctx, KB_E_INVALID, "aggregates without GROUP BY");
     if (n_aggs && aggs[0].kind > KB_AGG_AVG) return fail(ctx, KB_E_INVALID, "unknown aggregate kind %u", aggs[0].kind);
-    AggSpec spec;
-    if (grouped) {
-        spec.group_slot = group_slots[0];
-        spec.has_agg = n_aggs == 1;
-        if (n_aggs) { spec.kind = aggs[0].kind; spec.agg_slot = aggs[0].slot; }
-    }
+    AggSpec spec(grouped ? group_slots[0] : 0u, n_aggs ? aggs : nullptr);
     auto pl = std::unique_ptr<kb_plan, void (*)(kb_plan*)>(new kb_plan, plan_release);
-    std::unique_ptr<kb_rel> unused;
-    KB_TRY(star_join_impl2(ctx, join_slot, pats, n_pats, filter, n_ops, true, &unused, grouped ? &spec : nullptr, &pl->ip));
-    if (!pl->ip.ok) return fail(ctx, KB_E_UNSUPPORTED, "the query does not take the one-kernel index path");
+    KB_TRY(resolve_index_plan(ctx, join_slot, pats, n_pats, filter, n_ops, grouped ? &spec : nullptr, &pl->ip));
+    if (!pl->ip.ok) return fail(ctx, KB_E_UNSUPPORTED, "prepared plans take the one-kernel index path only: %s", pl->ip.why);
+    if (grouped && !pl->ip.agg) return fail(ctx, KB_E_UNSUPPORTED, "prepared GROUP BY: the group or aggregate variable is not bound by the join");
     pl->ctx = ctx;
     pl->life = ctx->life;
     pl->store_version = ctx->store_version;
@@ -123,14 +115,7 @@ kb_status kb_star_join_prepare(kb_ctx* ctx, uint32_t join_slot, const kb_pattern
             memset(s.h_rec, 0, 16);
             KB_CUDA(ctx, cudaHostGetDevicePointer(reinterpret_cast<void**>(&s.d_rec), s.h_rec, 0));
         } else {
-            const size_t stride = round256((size_t)ip.probe_rows * sizeof(u32)) + 256;
-            KB_TRY(alloc_buf(ctx, stride * ip.n_out, &s.out));
-            for (u32 c = 0; c < ip.n_out; c++) {
-                Col col;
-                col.buf = s.out;
-                col.ptr = reinterpret_cast<u32*>(static_cast<char*>(s.out->p) + stride * c);
-                s.cols.push_back(col);
-            }
+            KB_TRY(alloc_index_out(ctx, ip.probe_rows, ip.n_out, &s.cols));
         }
     }
     if (ip.P.ordered || ctx->ordered) KB_TRY(ensure_tile_state(ctx, ip.P.n_tiles));
@@ -161,11 +146,7 @@ kb_status kb_plan_submit(kb_ctx* ctx, kb_plan* pl, uint64_t* ticket) {
         G.nt = numtab(ctx);
         const u32 si = (u32)(t % pl->ring);
         char* tb = pl->attached ? pl->peer_scratch[pl->rank] + 256 + (size_t)si * pl->table_stride : static_cast<char*>(s.tab.buf->p);
-        G.n_slots = (u32)s.tab.slots;
-        G.gval = (double*)(tb + s.tab.o_val);
-        G.gcnt = (unsigned long long*)(tb + s.tab.o_cnt);
-        G.gkeys = (u32*)(tb + s.tab.o_keys);
-        G.gstate = (u32*)(tb + s.tab.o_state);
+        s.tab.point(&G, tb);
         G.overflow = (u32*)(tb + s.tab.bytes);
         P.ordered = 0;
         timer_begin(ctx, F_GROUP);
@@ -190,11 +171,7 @@ kb_status kb_plan_submit(kb_ctx* ctx, kb_plan* pl, uint64_t* ticket) {
             kb_plan::Merged& M = pl->merged[si];
             GroupParams Gm = G;
             char* mb = static_cast<char*>(M.tab.buf->p);
-            Gm.n_slots = (u32)M.tab.slots;
-            Gm.gval = (double*)(mb + M.tab.o_val);
-            Gm.gcnt = (unsigned long long*)(mb + M.tab.o_cnt);
-            Gm.gkeys = (u32*)(mb + M.tab.o_keys);
-            Gm.gstate = (u32*)(mb + M.tab.o_state);
+            M.tab.point(&Gm, mb);
             Gm.overflow = (u32*)(mb + M.tab.bytes);
             timer_begin(ctx, F_GROUP, 3);
             launch_peer_barrier(T, (u32)t, ctx->st);
@@ -211,16 +188,7 @@ kb_status kb_plan_submit(kb_ctx* ctx, kb_plan* pl, uint64_t* ticket) {
             KB_CUDA(ctx, cudaGetLastError());
         }
     } else {
-        for (u32 c = 0; c < pl->ip.n_out; c++) P.out[c] = s.cols[c].ptr;
-        P.ordered = ctx->ordered;
-        if (P.ordered) {
-            P.tile_state = static_cast<u64*>(ctx->tile_state->p);
-            P.block_state = static_cast<u64*>(ctx->block_state->p);
-        }
-        timer_begin(ctx, F_PROBE);
-        launch_probe_index(P, nullptr, ctx->n_sms, ctx->st);
-        timer_end(ctx);
-        KB_CUDA(ctx, cudaGetLastError());
+        KB_TRY(launch_index_rows(ctx, P, s.cols));
     }
     KB_CUDA(ctx, cudaEventRecord(s.done, ctx->st));
     ctx->stats.rows_probed += pl->ip.probe_rows;
