@@ -372,6 +372,39 @@ KB_API kb_status kb_datalog_maintain(kb_ctx* ctx, const kb_rule* rules, uint32_t
                                      kb_rel** inferred_removed /* nullable */, kb_rel** inferred_added /* nullable */,
                                      kb_maintain_stats* stats /* nullable */);
 
+/* ------------------------------------------------------------------ Relation-to-Stream operators (Relation2StreamOperator,
+ * kolibrie/src/rsp/r2s.rs:24-58), applied to every firing's result (rsp_engine.rs:349-360): the result stays in device memory and only
+ * the rows that changed are emitted.
+ * State. The operator holds `last`: the distinct rows of the previous ISTREAM/DSTREAM evaluation. It starts empty and lives in device
+ *   memory owned by the operator. It holds ids only, so store mutations, index rebuilds and dictionary reloads do not affect it. It must
+ *   be freed before its context is destroyed.
+ * Rows. A row is the tuple of a response's columns, taken in the order of `slots` given at create time. `response` must have exactly
+ *   that slot set, though its columns may come in any order; otherwise the call returns KB_E_INVALID and the state is unchanged.
+ *   - Equality is equality of u32 ids. It equals the reference's equality of `Vec<(String,String)>` sorted by variable name, because the
+ *     dictionary is a bijection.
+ *   - `n_cols` is 1..KB_MAX_COLS.
+ *   - A response with 0 rows is valid.
+ *   - ISTREAM and DSTREAM emit their rows with the columns in the order of `slots`.
+ * RSTREAM. `emitted` is a zero-copy view of `response`, as kb_project gives one. `last` is not touched, as in r2s.rs:39.
+ * ISTREAM. `emitted` holds every row of `response` whose tuple is not in `last`.
+ *   - It follows response order, and duplicates are kept: a bag row that is new is emitted once per occurrence (r2s.rs:41-44).
+ *   - Then `last` becomes the distinct rows of `response`.
+ * DSTREAM. `emitted` holds every row of `last` whose tuple is not in `response`, each row once.
+ *   - Its order is the order of the row's first occurrence in the response that set `last`. The reference leaves this order unspecified
+ *     (HashSet iteration, r2s.rs:50); pinning it makes the device deterministic.
+ *   - Then `last` becomes the distinct rows of `response`.
+ * Errors.
+ *   - More than 2^32-1 response rows: KB_E_LIMIT.
+ *   - A CUDA or out-of-memory error: `last` is exactly what it was before the call (the new state is built in fresh buffers and swapped
+ *     in only on success).
+ * kb_r2s_info: *last_rows = distinct rows held, *stream_op = the operator (either pointer may be NULL). */
+enum kb_stream_op { KB_RSTREAM = 0, KB_ISTREAM = 1, KB_DSTREAM = 2 }; /* r2s.rs:15-17 */
+typedef struct kb_r2s kb_r2s;
+KB_API kb_status kb_r2s_create(kb_ctx* ctx, uint32_t stream_op, const uint32_t* slots, uint32_t n_cols, kb_r2s** out);
+KB_API kb_status kb_r2s_eval(kb_ctx* ctx, kb_r2s* op, const kb_rel* response, kb_rel** emitted);
+KB_API kb_status kb_r2s_info(const kb_r2s* op, uint64_t* last_rows, uint32_t* stream_op);
+KB_API void kb_r2s_free(kb_ctx* ctx, kb_r2s* op);
+
 /* ------------------------------------------------------------------ multi-GPU helpers (one process per GPU; the host layer
  * runs the NCCL all-to-all between kb_partition and kb_rel_from_device) */
 /* Shard function (host and device agree): block-cyclic on the dictionary id, (key >> KB_SHARD_BLOCK_BITS) % n_shards. Dictionary ids

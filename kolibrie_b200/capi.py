@@ -32,6 +32,7 @@ CMP_GT, CMP_GE, CMP_LT, CMP_LE, CMP_EQ, CMP_NE = range(1, 7)
 AGG_COUNT, AGG_SUM, AGG_MIN, AGG_MAX, AGG_AVG = range(5)
 SEMI_NAIVE, NAIVE, SEMI_NAIVE_PARALLEL = 0, 1, 2
 SEMI_NAIVE_OLD_DELTA = 3  # textbook OLD/delta scheme: same facts, rounds and per-round counts, fewer candidates (include/kolibrie_b200.h)
+RSTREAM, ISTREAM, DSTREAM = 0, 1, 2  # kb_stream_op (r2s.rs:15-17)
 
 
 class KbTerm(C.Structure):
@@ -207,6 +208,10 @@ def lib() -> C.CDLL:
         "kb_datalog_fixpoint": (i32, [vp, P(KbRule), u32, u32, P(vp), P(KbFixpointStats)]),
         "kb_datalog_fixpoint_seed": (i32, [vp, P(KbRule), u32, u32, vp, P(vp), P(u64), P(KbFixpointStats)]),
         "kb_datalog_maintain": (i32, [vp, P(KbRule), u32, u32, P(u64), u32, vp, u64, P(vp), P(vp), P(KbMaintainStats)]),
+        "kb_r2s_create": (i32, [vp, u32, P(u32), u32, P(vp)]),
+        "kb_r2s_eval": (i32, [vp, vp, vp, P(vp)]),
+        "kb_r2s_info": (i32, [vp, P(u64), P(u32)]),
+        "kb_r2s_free": (None, [vp, vp]),
         "kb_shard_of": (u32, [u32, u32]),
         "kb_set_sharding": (i32, [vp, u32, u32]),
         "kb_partition": (i32, [vp, vp, u32, u32, P(vp), P(u64)]),
@@ -237,7 +242,7 @@ EXPORTED_SYMBOLS = [
     "kb_rel_from_device", "kb_rel_free", "kb_scan", "kb_filter", "kb_project", "kb_hash_join", "kb_bind_join", "kb_star_join", "kb_bgp_execute",
     "kb_group_aggregate", "kb_groups_info", "kb_groups_keys", "kb_groups_values", "kb_groups_counts", "kb_groups_free", "kb_groups_pack", "kb_groups_merge", "kb_star_join_aggregate",
     "kb_star_join_prepare", "kb_plan_submit", "kb_plan_collect", "kb_plan_info", "kb_plan_free", "kb_plan_peer_scratch_bytes", "kb_plan_attach_peers",
-    "kb_datalog_fixpoint", "kb_datalog_fixpoint_seed", "kb_datalog_maintain", "kb_shard_of", "kb_set_sharding", "kb_partition", "kb_partition_counts", "kb_segment_write", "kb_segment_info", "kb_segment_save", "kb_store_append_file", "kb_shuffle_scatter", "kb_shuffle_push", "kb_rel_wrap_device", "kb_star_join_host", "kb_star_join_host_into", "perform_hash_join_cuda",
+    "kb_datalog_fixpoint", "kb_datalog_fixpoint_seed", "kb_datalog_maintain", "kb_r2s_create", "kb_r2s_eval", "kb_r2s_info", "kb_r2s_free", "kb_shard_of", "kb_set_sharding", "kb_partition", "kb_partition_counts", "kb_segment_write", "kb_segment_info", "kb_segment_save", "kb_store_append_file", "kb_shuffle_scatter", "kb_shuffle_push", "kb_rel_wrap_device", "kb_star_join_host", "kb_star_join_host_into", "perform_hash_join_cuda",
 ]
 
 
@@ -651,6 +656,14 @@ class Context:
                                               C.byref(rem), C.byref(new), C.byref(st)))
         return Relation(self, rem), Relation(self, new), st
 
+    def r2s(self, stream_op: int, slots: Sequence[int]) -> "StreamOperator":
+        """kb_r2s_create: a Relation-to-Stream operator (RSTREAM / ISTREAM / DSTREAM) over rows of the variables `slots` (their order is
+        the column order of what ISTREAM / DSTREAM emit)"""
+        sl = (C.c_uint32 * max(len(slots), 1))(*slots)
+        h = C.c_void_p()
+        self._check(lib().kb_r2s_create(self.h, stream_op, sl, len(slots), C.byref(h)))
+        return StreamOperator(self, h)
+
     def partition(self, rel: Relation, key_slot: int, n_parts: int):
         out = C.c_void_p()
         offs = (C.c_uint64 * (n_parts + 1))()
@@ -777,6 +790,37 @@ class Plan:
     def free(self):
         if self.h:
             lib().kb_plan_free(self.ctx.h, self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+class StreamOperator:
+    """kb_r2s: a Relation-to-Stream operator whose state (the previous evaluation's distinct rows) lives in device memory.
+    eval(rel) returns the emitted rows as a Relation; info() = (distinct rows held, stream operator)."""
+
+    def __init__(self, ctx: Context, handle):
+        self.ctx = ctx
+        self.h = handle
+        ctx._plans.add(self)  # freed with the context's other handles, before the context itself
+
+    def eval(self, rel: Relation) -> Relation:
+        out = C.c_void_p()
+        self.ctx._check(lib().kb_r2s_eval(self.ctx.h, self.h, rel.h, C.byref(out)))
+        return Relation(self.ctx, out)
+
+    def info(self) -> Tuple[int, int]:
+        n, op = C.c_uint64(), C.c_uint32()
+        self.ctx._check(lib().kb_r2s_info(self.h, C.byref(n), C.byref(op)))
+        return n.value, op.value
+
+    def free(self):
+        if self.h:
+            lib().kb_r2s_free(self.ctx.h, self.h)
             self.h = None
 
     def __del__(self):

@@ -24,18 +24,6 @@ kb_status fail(kb_ctx* ctx, kb_status code, const char* fmt, ...) {
     return code;
 }
 
-struct DeviceGuard {
-    int prev = -1;
-    explicit DeviceGuard(int dev) {
-        cudaGetDevice(&prev);
-        if (prev != dev) cudaSetDevice(dev);
-        else prev = -1;
-    }
-    ~DeviceGuard() {
-        if (prev >= 0) cudaSetDevice(prev);
-    }
-};
-
 kb_status alloc_buf(kb_ctx* ctx, size_t bytes, Buf* out) {
     auto b = std::make_shared<DevBuf>();
     b->bytes = round256(bytes) + 256;  // every column can be over-read to the next 16-byte boundary by the TMA tile loads

@@ -240,6 +240,17 @@ struct kb_ctx {
 namespace kb {
 
 kb_status fail(kb_ctx* ctx, kb_status code, const char* fmt, ...);
+struct DeviceGuard {  // the calling thread's current device is restored on return
+    int prev = -1;
+    explicit DeviceGuard(int dev) {
+        cudaGetDevice(&prev);
+        if (prev != dev) cudaSetDevice(dev);
+        else prev = -1;
+    }
+    ~DeviceGuard() {
+        if (prev >= 0) cudaSetDevice(prev);
+    }
+};
 inline size_t round256(size_t b) { return (b + 255) & ~(size_t)255; }
 #define KB_CUDA(ctx, call)                                                                                             \
     do {                                                                                                               \

@@ -522,6 +522,42 @@ void launch_decode_gather(const u32* ids, u32 n, const unsigned long long* dict_
                           unsigned char* out, int n_sms, cudaStream_t st);
 
 // ---------------------------------------------------------------------------------------------------------------
+// Relation-to-Stream operators (kb_r2s_eval; Relation2StreamOperator::eval, r2s.rs:37-58). A set of rows is an open-addressing table
+// of u32 row indices (EMPTY32 = free slot) keyed by a 64-bit mix of the row's columns in the operator's slot order; a hash hit is
+// confirmed by comparing every column.
+struct R2sRows {
+    const u32* col[KB_MAX_COLS];  // columns in the operator's slot order
+    u32 n;
+    u32* tab;                     // table over the rows (unused when n == 0)
+    u32 mask;                     // table slots - 1
+};
+struct R2sParams {
+    R2sRows cur;      // the response: its table is built, then remapped to the new state's columns
+    R2sRows last;     // the previous state (read only)
+    u32 n_cols;
+    u32 probe_last;   // ISTREAM: flag the response rows whose tuple `last` does not hold
+    u32* rep;         // [cur.n] 1 where row i is its tuple's representative (first occurrence); then its exclusive prefix
+    u32* slot_of;     // [cur.n] table slot of row i's tuple
+    u32* emit;        // ISTREAM: [cur.n] emitted response rows; DSTREAM: [last.n] rows of `last` that are gone (flags, then prefix)
+    u32* counts;      // [2] zeroed: representatives, emitted rows
+    u32 n_rep, n_emit;  // write passes: the totals of the two flag arrays
+    u32* out_state[KB_MAX_COLS];
+    u32* out_emit[KB_MAX_COLS];
+};
+// build: every response row goes into cur's table (atomicCAS on a free slot, atomicMin on a slot holding an equal row: the slot ends
+// up holding the tuple's first occurrence, whatever the thread order)
+void launch_r2s_build(const R2sParams& p, int n_sms, cudaStream_t st);
+// mark: rep, slot_of and, with probe_last, emit (+ counts)
+void launch_r2s_mark(const R2sParams& p, int n_sms, cudaStream_t st);
+// DSTREAM mark: emit[j] = row j of `last` has no equal row in the response (+ counts[1]); runs before the remap
+void launch_r2s_gone_mark(const R2sParams& p, int n_sms, cudaStream_t st);
+// write, after the exclusive scans: the representatives into out_state (and cur's table remapped to them), with probe_last the
+// emitted rows into out_emit
+void launch_r2s_write(const R2sParams& p, int n_sms, cudaStream_t st);
+// DSTREAM write: the gone rows of `last` into out_emit, in `last` order
+void launch_r2s_gone_write(const R2sParams& p, int n_sms, cudaStream_t st);
+
+// ---------------------------------------------------------------------------------------------------------------
 // small utilities
 void launch_fill_u32(u32* p, u32 v, u64 n, cudaStream_t st);
 void launch_fill_const_col(u32* p, u32 v, u64 n, cudaStream_t st);

@@ -783,12 +783,53 @@ class SimpleR2R:
         self.last_stats = st
         return sorted(self.derived)
 
-    def execute_query(self, op) -> List[Dict[str, str]]:
-        """ExecutionEngine over the window (its base triples and, after materialize(), the inferred ones)"""
+    def _device_ready(self):
         self._flush()
         self._load_tables()
         self.item._uploaded_version = self.item._version  # the device store is maintained segment by segment, never reloaded from the set
+
+    def execute_query(self, op) -> List[Dict[str, str]]:
+        """ExecutionEngine over the window (its base triples and, after materialize(), the inferred ones)"""
+        self._device_ready()
         return ExecutionEngine.execute(op, self.item)
+
+    def execute_query_rel(self, op) -> c.Relation:
+        """execute_query without the download and the decode: the firing's result as a device relation, what
+        Relation2StreamOperator.eval takes. `slot_names[s]` is the name of the variable in slot s (the same for every firing of op)."""
+        self._device_ready()
+        slots = SlotMap()
+        rel = ExecutionEngine._run(op, self.item, slots)
+        self.slot_names = list(slots.names)
+        return rel
+
+
+_STREAM_OPS = {"RSTREAM": c.RSTREAM, "ISTREAM": c.ISTREAM, "DSTREAM": c.DSTREAM}
+
+
+class Relation2StreamOperator:
+    """rsp/r2s.rs:24-58 on device relations (kb_r2s_eval): eval(response, ts) returns the emitted rows as a device relation. The
+    previous evaluation's distinct rows stay in device memory, so an ISTREAM / DSTREAM firing downloads only what it emits. Rows compare
+    by their ids (the dictionary is a bijection), with the columns in slot order; ISTREAM keeps the response's order and duplicates,
+    DSTREAM emits the rows that left in the order they first appeared (r2s.rs:50 leaves that order to a HashSet)."""
+
+    def __init__(self, ctx: c.Context, stream_operator: Union[int, str] = c.RSTREAM, _start_time: int = 0):
+        self.ctx = ctx
+        self.stream_operator = _STREAM_OPS.get(stream_operator, stream_operator)
+        self._op: Optional[c.StreamOperator] = None  # created at the first response: its variables fix the row shape
+
+    def eval(self, new_response: c.Relation, _ts: int = 0) -> c.Relation:
+        if self._op is None:
+            self._op = self.ctx.r2s(self.stream_operator, sorted(new_response.slots))
+        return self._op.eval(new_response)
+
+    def last_rows(self) -> int:
+        """distinct rows of the previous ISTREAM / DSTREAM evaluation"""
+        return self._op.info()[0] if self._op is not None else 0
+
+    def free(self):
+        if self._op is not None:
+            self._op.free()
+            self._op = None
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -38,7 +38,11 @@ pub const KB_CMP_GT: u32 = 1; pub const KB_CMP_GE: u32 = 2; pub const KB_CMP_LT:
 pub const KB_AGG_COUNT: u32 = 0; pub const KB_AGG_SUM: u32 = 1; pub const KB_AGG_MIN: u32 = 2; pub const KB_AGG_MAX: u32 = 3; pub const KB_AGG_AVG: u32 = 4;
 pub const KB_SEMI_NAIVE: u32 = 0; pub const KB_NAIVE: u32 = 1; pub const KB_SEMI_NAIVE_PARALLEL: u32 = 2; pub const KB_SEMI_NAIVE_OLD_DELTA: u32 = 3;
 
-pub enum KbCtx {} pub enum KbRel {} pub enum KbGroups {} pub enum KbStrings {} pub enum KbPlan {}
+// kb_stream_op (r2s.rs:15-17)
+pub const KB_RSTREAM: u32 = 0; pub const KB_ISTREAM: u32 = 1; pub const KB_DSTREAM: u32 = 2;
+
+pub enum KbCtx {} pub enum KbRel {} pub enum KbGroups {} pub enum KbStrings {} pub enum KbPlan {} pub enum KbR2s {}
+pub type kb_r2s = KbR2s;  // (the header's name, as the declarations below spell it)
 
 extern "C" {
     pub fn kb_version() -> *const c_char;
@@ -97,6 +101,11 @@ extern "C" {
     // delete-and-rederive across a window slide: the store is closed under the rules (the last fixpoint / maintain with the same rules)
     pub fn kb_datalog_maintain(ctx: *mut KbCtx, rules: *const KbRule, n: u32, strategy: u32, evict_tags: *const u64, n_evict: u32, add: *const KbRel,
                                add_tag: u64, inferred_removed: *mut *mut KbRel, inferred_added: *mut *mut KbRel, stats: *mut kb_maintain_stats) -> kb_status;
+    // Relation-to-Stream operators: the previous evaluation's distinct rows stay on the device, an evaluation emits the rows that changed
+    pub fn kb_r2s_create(ctx: *mut KbCtx, stream_op: u32, slots: *const u32, n_cols: u32, out: *mut *mut kb_r2s) -> kb_status;
+    pub fn kb_r2s_eval(ctx: *mut KbCtx, op: *mut kb_r2s, response: *const KbRel, emitted: *mut *mut KbRel) -> kb_status;
+    pub fn kb_r2s_info(op: *const kb_r2s, last_rows: *mut u64, stream_op: *mut u32) -> kb_status;
+    pub fn kb_r2s_free(ctx: *mut KbCtx, op: *mut kb_r2s);
     // multi-GPU helpers
     pub fn kb_shard_of(key: u32, n_shards: u32) -> u32;
     pub fn kb_set_sharding(ctx: *mut KbCtx, rank: u32, world: u32) -> kb_status;

@@ -2,7 +2,8 @@
 //!
 //! * [`try_execute`]            for `ExecutionEngine::execute_with_ids` (kolibrie/src/streamertail_optimizer/execution/engine.rs:54)
 //! * [`GpuSemiNaiveStrategy`]   for `Reasoner::infer_with_strategy`    (datalog/src/reasoning/materialisation/infer_generic.rs:27-53)
-//! * [`GpuR2R`]                 for the RSP engine's `R2ROperator`      (kolibrie/src/rsp/r2r.rs:17-30)
+//! * [`GpuR2R`]                 for the RSP engine's `R2ROperator`      (kolibrie/src/rsp/r2r.rs:17-30), optionally with the
+//!                              Relation-to-Stream operator on the device (`GpuR2R::with_stream_operator`, kolibrie/src/rsp/r2s.rs:37-58)
 //!
 //! plus [`planner`]: the device operators' cost constants for Streamertail's estimator (cost/estimator.rs:17-29).
 //!
@@ -187,7 +188,8 @@ pub fn compile_condition(cond: &Condition, slots: &mut SlotMap, database: &Sparq
     Some(out)
 }
 
-struct Rel(*mut KbRel, *mut KbCtx);
+/// a device relation owned by the shim (freed on drop)
+pub struct Rel(pub *mut KbRel, pub *mut KbCtx);
 impl Drop for Rel { fn drop(&mut self) { unsafe { kb_rel_free(self.1, self.0) } } }
 
 fn run(op: &PhysicalOperator, dev: &DeviceStore, db: &SparqlDatabase, slots: &mut SlotMap) -> Option<Rel> {
@@ -257,18 +259,34 @@ fn run(op: &PhysicalOperator, dev: &DeviceStore, db: &SparqlDatabase, slots: &mu
 /// ```
 /// None means "shape not handled on the device" (KB_E_UNSUPPORTED or an operator outside the hot path): run the CPU path.
 pub fn try_execute(op: &PhysicalOperator, database: &SparqlDatabase, dev: &mut DeviceStore) -> Option<Vec<HashMap<String, u32>>> {
+    let res = try_execute_rel(op, database, dev)?;
+    download_rows(dev, res.rel.0, &res.names)
+}
+
+/// The operator's result on the device, before any download: the relation and the variable name of each of its columns.
+pub struct DeviceResult { pub rel: Rel, pub names: Vec<String> }
+
+/// The device half of [`try_execute`]. None: shape not handled on the device.
+pub fn try_execute_rel(op: &PhysicalOperator, database: &SparqlDatabase, dev: &mut DeviceStore) -> Option<DeviceResult> {
     dev.sync(database).ok()?;
     let mut slots = SlotMap::default();
     let rel = run(op, dev, database, &mut slots)?;
-    let (mut n, mut nc) = (0u64, 0u32);
+    let mut nc = 0u32;
     let mut rs = [0u32; KB_MAX_COLS];
-    if unsafe { kb_rel_info(rel.0, &mut n, &mut nc, rs.as_mut_ptr()) } != KB_OK { return None; }
-    let mut cols: Vec<Vec<u32>> = Vec::with_capacity(nc as usize);
-    for c in 0..nc {
+    if unsafe { kb_rel_info(rel.0, ptr::null_mut(), &mut nc, rs.as_mut_ptr()) } != KB_OK { return None; }
+    let names = (0..nc as usize).map(|c| slots.names[rs[c] as usize].clone()).collect();
+    Some(DeviceResult { rel, names })
+}
+
+/// Every row of a device relation as a (variable -> id) map; `names[c]` is the variable of column c.
+pub fn download_rows(dev: &DeviceStore, rel: *const KbRel, names: &[String]) -> Option<Vec<HashMap<String, u32>>> {
+    let mut n = 0u64;
+    if unsafe { kb_rel_info(rel, &mut n, ptr::null_mut(), ptr::null_mut()) } != KB_OK { return None; }
+    let mut cols: Vec<Vec<u32>> = Vec::with_capacity(names.len());
+    for c in 0..names.len() {
         let mut v = vec![0u32; n as usize];
-        if unsafe { kb_rel_download(dev.ctx, rel.0, c, v.as_mut_ptr()) } != KB_OK { return None; }
+        if unsafe { kb_rel_download(dev.ctx, rel, c as u32, v.as_mut_ptr()) } != KB_OK { return None; }
         cols.push(v);
     }
-    let names: Vec<&String> = (0..nc as usize).map(|c| &slots.names[rs[c] as usize]).collect();
-    Some((0..n as usize).map(|i| names.iter().enumerate().map(|(c, k)| ((*k).clone(), cols[c][i])).collect()).collect())
+    Some((0..n as usize).map(|i| names.iter().enumerate().map(|(c, k)| (k.clone(), cols[c][i])).collect()).collect())
 }

@@ -11,10 +11,15 @@
 //! (which would drop the firing tags and the inferred segment); the dictionary's tables are still mirrored before every firing and query
 //! (a numeric-table load voids the closed token only when a rule filter compares numbers). The derived triples are mirrored into
 //! `inner.item`, so the host's query path (shapes the device does not take) sees them too.
+//!
+//! `with_stream_operator` moves the Relation-to-Stream operator (r2s.rs:37-58) onto the device as well: `execute_query` then runs
+//! `kb_r2s_eval` on the firing's device result and downloads and decodes only the rows it emits. Register such an engine with RSTREAM,
+//! whose operator is a passthrough (r2s.rs:39): the composition is the reference's ISTREAM / DSTREAM.
 use crate::ffi::*;
 use crate::reasoner::compile_rule;
-use crate::{try_execute, DeviceStore};
+use crate::{try_execute, try_execute_rel, DeviceStore};
 use kolibrie::rsp::r2r::{AsAnyMut, R2ROperator};
+use kolibrie::rsp::r2s::StreamOperator;
 use kolibrie::rsp::simple_r2r::SimpleR2R;
 use kolibrie::streamertail_optimizer::PhysicalOperator;
 use shared::triple::Triple;
@@ -32,6 +37,15 @@ pub struct GpuR2R {
     live: HashMap<u64, usize>,  // tag -> triples of that segment still in the window
     closed: bool,               // the device store is closed under the rules (the last materialize succeeded, nothing changed since)
     derived: HashSet<Triple>,   // the inferred segment, mirrored on the host (what materialize returns)
+    stream: Option<DeviceStream>,  // with_stream_operator: the R2S operator runs on the device result
+}
+
+/// The device R2S operator of a `GpuR2R`. Its rows are the query's variables in name order: slot i is `names[i]`, whichever slots the
+/// query's own relation used, so that device results and host fallbacks feed one state.
+struct DeviceStream {
+    kind: u32,
+    op: *mut kb_r2s,      // created at the first firing, when the variables are known
+    names: Vec<String>,
 }
 
 fn triples_of(dev: &DeviceStore, rel: *mut KbRel) -> Vec<Triple> {
@@ -48,7 +62,69 @@ impl GpuR2R {
         let mut dev = DeviceStore::new(device)?;
         dev.segmented = true;
         Ok(Self { inner, dev, pending: Vec::new(), evicted: Vec::new(), firing: 1, tag_of: HashMap::new(), live: HashMap::new(),
-                  closed: false, derived: HashSet::new() })
+                  closed: false, derived: HashSet::new(), stream: None })
+    }
+    /// Opt in to the device R2S operator: `execute_query` returns what `stream_operator` emits for the firing, not the whole result.
+    pub fn with_stream_operator(mut self, stream_operator: StreamOperator) -> Self {
+        let kind = match stream_operator { StreamOperator::RSTREAM => KB_RSTREAM, StreamOperator::ISTREAM => KB_ISTREAM, StreamOperator::DSTREAM => KB_DSTREAM };
+        self.stream = Some(DeviceStream { kind, op: ptr::null_mut(), names: Vec::new() });
+        self
+    }
+    /// `kb_r2s_eval` on a firing's result (`names[c]` = variable of column c), then the emitted rows decoded. None: the result has
+    /// other variables than the operator's, or a device error (the operator's state is then unchanged).
+    fn stream_eval(&mut self, rel: *const KbRel, names: &[String]) -> Option<Vec<Vec<(String, String)>>> {
+        let ctx = self.dev.ctx;
+        let st = self.stream.as_mut()?;
+        if st.op.is_null() {
+            let mut sorted = names.to_vec();
+            sorted.sort();
+            let slots: Vec<u32> = (0..sorted.len() as u32).collect();
+            if unsafe { kb_r2s_create(ctx, st.kind, slots.as_ptr(), slots.len() as u32, &mut st.op) } != KB_OK { return None; }
+            st.names = sorted;
+        }
+        // the same columns under the operator's slots (a view, no copy)
+        let (mut n, mut sl, mut cols) = (0u64, Vec::new(), Vec::new());
+        unsafe { kb_rel_info(rel, &mut n, ptr::null_mut(), ptr::null_mut()) };
+        for (c, k) in names.iter().enumerate() {
+            sl.push(st.names.iter().position(|x| x == k)? as u32);
+            let mut p: *const u32 = ptr::null();
+            unsafe { kb_rel_device_col(rel, c as u32, &mut p) };
+            cols.push(p as *mut u32);
+        }
+        let mut view: *mut KbRel = ptr::null_mut();
+        if unsafe { kb_rel_wrap_device(ctx, sl.as_ptr(), sl.len() as u32, cols.as_ptr(), n, &mut view) } != KB_OK { return None; }
+        let mut emitted: *mut KbRel = ptr::null_mut();
+        let rc = unsafe { kb_r2s_eval(ctx, st.op, view, &mut emitted) };
+        unsafe { kb_rel_free(ctx, view) };
+        if rc != KB_OK { return None; }
+        let out_names = if st.kind == KB_RSTREAM { names.to_vec() } else { st.names.clone() };  // RSTREAM: the response's own columns
+        let rows = crate::download_rows(&self.dev, emitted, &out_names);
+        unsafe { kb_rel_free(ctx, emitted) };
+        let dict = self.inner.item.dictionary.read().unwrap();
+        Some(rows?.into_iter().map(|r| {
+            let mut r: Vec<(String, String)> = r.into_iter().map(|(k, v)| (k, dict.decode(v).unwrap_or("unknown").to_string())).collect();
+            r.sort();
+            r
+        }).collect())
+    }
+    /// a host fallback's rows, encoded back to ids and passed through the same device operator
+    fn stream_eval_host(&mut self, rows: Vec<Vec<(String, String)>>) -> Option<Vec<Vec<(String, String)>>> {
+        let names: Vec<String> = match (rows.first(), self.stream.as_ref()) {
+            (_, Some(st)) if !st.names.is_empty() => st.names.clone(),
+            (Some(r), _) => { let mut v: Vec<String> = r.iter().map(|(k, _)| k.clone()).collect(); v.sort(); v }
+            (None, _) => return Some(Vec::new()),  // no firing yet told the variables, and nothing to emit
+        };
+        let cols: Vec<Vec<u32>> = {
+            let dict = self.inner.item.dictionary.read().unwrap();
+            names.iter().map(|k| rows.iter().map(|r| r.iter().find(|(x, _)| x == k)
+                .and_then(|(_, v)| dict.string_to_id.get(v.as_str()).copied()).unwrap_or(KB_ID_NONE)).collect()).collect()
+        };
+        let slots: Vec<u32> = (0..names.len() as u32).collect();
+        let ptrs: Vec<*const u32> = cols.iter().map(|c| c.as_ptr()).collect();
+        let mut rel: *mut KbRel = ptr::null_mut();
+        if unsafe { kb_rel_from_host(self.dev.ctx, slots.as_ptr(), slots.len() as u32, ptrs.as_ptr(), rows.len() as u64, &mut rel) } != KB_OK { return None; }
+        let rel = crate::Rel(rel, self.dev.ctx);
+        self.stream_eval(rel.0, &names)
     }
     /// the derived triples as the device now holds them, mirrored into the host database (a derived triple that is also a live streamed
     /// triple stays there when it stops being derived: Q11)
@@ -115,6 +191,13 @@ impl GpuR2R {
     }
 }
 
+impl Drop for GpuR2R {
+    // the operator's state lives in the context's memory: it goes before `dev` destroys the context
+    fn drop(&mut self) {
+        if let Some(st) = self.stream.take() { unsafe { kb_r2s_free(self.dev.ctx, st.op) }; }
+    }
+}
+
 impl AsAnyMut for GpuR2R { fn as_any_mut(&mut self) -> &mut dyn Any { self } }
 
 impl R2ROperator<Triple, Vec<(String, String)>, Vec<(String, String)>> for GpuR2R {
@@ -157,6 +240,16 @@ impl R2ROperator<Triple, Vec<(String, String)>, Vec<(String, String)>> for GpuR2
     }
     fn execute_query(&mut self, op: &PhysicalOperator) -> Vec<Vec<(String, String)>> {
         self.flush();
+        if self.stream.is_some() {
+            let emitted = match try_execute_rel(op, &self.inner.item, &mut self.dev) {
+                Some(res) => self.stream_eval(res.rel.0, &res.names),
+                None => { let rows = self.inner.execute_query(op); self.stream_eval_host(rows) }
+            };
+            return emitted.unwrap_or_else(|| {
+                eprintln!("kb_r2s_eval failed: {}", self.dev.last_error());
+                Vec::new()
+            });
+        }
         match try_execute(op, &self.inner.item, &mut self.dev) {
             Some(rows) => {
                 let dict = self.inner.item.dictionary.read().unwrap();
