@@ -55,16 +55,25 @@ typedef struct kb_rel kb_rel;       /* device-resident columnar bag of binding r
 typedef struct kb_groups kb_groups; /* host-resident GROUP BY result */
 
 /* Term of a triple pattern — reference `Term::{Variable,Constant}` (shared/src/terms.rs:14-21).
- * QuotedTriple terms are resolved on the host before reaching the device (engine.rs:59-70). */
+ * `Term::QuotedTriple` is KB_TERM_QUOTED, which only kb_scan_quoted accepts; every other entry point refuses is_var > 1 (KB_E_INVALID). */
 typedef struct kb_term {
-    uint32_t is_var; /* 1: `value` is a variable slot; 0: `value` is a constant term id */
+    uint32_t is_var; /* 1: `value` is a variable slot; 0: `value` is a constant term id; KB_TERM_QUOTED: see kb_quoted_pattern */
     uint32_t value;
 } kb_term;
+#define KB_TERM_QUOTED 2u
 
 /* reference `TriplePattern = (Term, Term, Term)` (shared/src/terms.rs:22) */
 typedef struct kb_pattern {
     kb_term s, p, o;
 } kb_pattern;
+
+/* An RDF-star pattern (engine.rs:1111-1188). In `outer`, a subject (object) whose is_var is KB_TERM_QUOTED is the term
+ * `<< inner_s >>` (`<< inner_o >>`); the inner pattern of a position that is not quoted is ignored. Inside an inner pattern a
+ * KB_TERM_QUOTED term stands for "any quoted-triple id" — all the reference checks for a nested term (engine.rs:1100-1105).
+ * A quoted predicate in `outer` -> KB_E_UNSUPPORTED. */
+typedef struct kb_quoted_pattern {
+    kb_pattern outer, inner_s, inner_o;
+} kb_quoted_pattern;
 
 /* ---- FILTER programs: postfix encoding of `FilterExpression` (shared/src/query.rs:15-22) with the
  *      semantics of `Condition::evaluate_with_ids` (kolibrie/src/streamertail_optimizer/types.rs:110-186) ---- */
@@ -208,7 +217,13 @@ KB_API kb_status kb_dict_legacy_i32_load(kb_ctx* ctx, const int32_t* val, const 
 KB_API kb_status kb_dict_strings_load(kb_ctx* ctx, const uint64_t* offsets /* [n_ids + 1] */, const uint8_t* bytes, uint32_t n_ids);
 typedef struct kb_strings kb_strings; /* device-resident decoded column: offsets [n+1] + bytes */
 /* Decodes column `col` of `r`: row i becomes the string of its id; an id the dictionary does not hold becomes "unknown" (engine.rs:44).
- * Quoted-triple ids (bit 31, shared/src/quoted_triple_store.rs:28-55) -> KB_E_UNSUPPORTED. At most 2^32-1 bytes per call. */
+ * Quoted-triple ids (bit 31, shared/src/quoted_triple_store.rs:28-55): without a quoted-triple table (kb_quoted_load) -> KB_E_UNSUPPORTED.
+ * With one, a quoted id renders as Dictionary::decode_term renders it (shared/src/dictionary.rs:60-72): `<< s p o >>`, components decoded
+ * the same way, recursively. When decode_term gives None at any depth (an id neither table holds), the whole term is "unknown"
+ * (engine.rs:42-43). A walk that reaches a quoted id more than KB_QUOTED_MAX_DEPTH levels deep (the top-level id is level 1) before it
+ * meets such an id -> KB_E_LIMIT: the table comes from the caller and a cycle in it would otherwise never end. At most 2^32-1 bytes per
+ * call. Launches and device time count in kb_stats' `other` family. */
+#define KB_QUOTED_MAX_DEPTH 16
 KB_API kb_status kb_rel_decode(kb_ctx* ctx, const kb_rel* r, uint32_t col, kb_strings** out);
 /* Dictionary::encode (shared/src/dictionary.rs:32-48) for a BATCH of terms — the load-time encode of sparql_database.rs:1000-1013 — on
  * the device: term i = bytes[offsets[i] .. offsets[i+1]) (host memory, offsets[0] = 0). A term the device dictionary already holds
@@ -224,6 +239,16 @@ KB_API kb_status kb_dict_strings_info(kb_ctx* ctx, uint32_t* n_ids, uint64_t* n_
 KB_API kb_status kb_strings_info(const kb_strings* s, uint64_t* n_strings, uint64_t* total_bytes);
 KB_API kb_status kb_strings_download(kb_ctx* ctx, const kb_strings* s, uint64_t* offsets /* [n + 1] */, uint8_t* bytes /* total_bytes */);
 KB_API void kb_strings_free(kb_ctx* ctx, kb_strings* s);
+
+/* Quoted-triple table on the device: QuotedTripleStore::id_to_components (shared/src/quoted_triple_store.rs:28-55), entry i =
+ * (ids[i] -> (s[i], p[i], o[i])). It REPLACES the context's table; n = 0 clears it. The table is indexed by id & 0x7FFFFFFF (the
+ * reference hands ids out sequentially from 0x80000000); ids never given are empty slots. A component may itself be a quoted id
+ * (nesting). Checked before anything changes — a refused call leaves the previous table in place:
+ *   an id without bit 31, an id or a component equal to KB_ID_NONE, a repeated id -> KB_E_INVALID;
+ *   an index id & 0x7FFFFFFF >= KB_QUOTED_MAX_SLOTS -> KB_E_LIMIT (the table takes 12 bytes per slot up to the largest index).
+ * Like the dictionary tables, the quoted table is not tied to the store version: store mutations and index builds keep it. */
+#define KB_QUOTED_MAX_SLOTS (1u << 28)
+KB_API kb_status kb_quoted_load(kb_ctx* ctx, const uint32_t* ids, const uint32_t* s, const uint32_t* p, const uint32_t* o, uint64_t n);
 
 /* ------------------------------------------------------------------ relations */
 KB_API kb_status kb_rel_info(const kb_rel* r, uint64_t* n_rows, uint32_t* n_cols, uint32_t* slots /* [KB_MAX_COLS] or NULL */);
@@ -251,6 +276,17 @@ KB_API kb_status kb_hash_join(kb_ctx* ctx, const kb_rel* left, const kb_rel* rig
  * index, the pattern (?x P ?y) and exactly one of its variables bound by `left` through a unique dense column of the predicate, it is
  * one probe kernel against the index's persistent table (the reference's spo[x][P] / pos[P][y] lookups); otherwise scan + hash join. */
 KB_API kb_status kb_bind_join(kb_ctx* ctx, const kb_rel* left, const kb_pattern* pattern, kb_rel** out);
+/* Quoted-triple scan: the bag resolve_quoted_triple_scan returns (engine.rs:1111-1188). Every table entry that match_term accepts
+ * (engine.rs:1088-1107; constants by id, a variable binds on first use and must be equal afterwards, within and across both inner
+ * patterns) fills the quoted position(s) of `outer`; with subject AND object quoted, ONE entry must satisfy both inner patterns and fills
+ * both positions (engine.rs:1135-1163). The outer pattern is then matched with the bindings merged; rows whose shared variables conflict
+ * are dropped. Columns: one per distinct variable, in order of first appearance when the pattern is read s, p, o with each quoted term
+ * inlined as its own s, p, o. Row order is unspecified (the reference's is HashMap order). No table loaded, or no entry matching ->
+ * 0 rows. `outer` must quote its subject or its object (otherwise KB_E_INVALID: use kb_scan).
+ * Work: ONE streaming pass over the table (the match kernel, counted in kb_stats' `scan` family) yields (entry id, inner variables);
+ * the outer pattern with a fresh variable in the quoted position(s) is then bind-joined to it exactly as kb_bind_join does — with a
+ * valid index, (q P ?o) and a unique, dense subject column of quoted ids, that is one probe launch — and the fresh variable projected away. */
+KB_API kb_status kb_scan_quoted(kb_ctx* ctx, const kb_quoted_pattern* qp, kb_rel** out);
 /* StarJoin (engine.rs:587-691) and bind-join chains on one variable (engine.rs:840-885): fused scan + build + probe.
  * Every pattern must contain join_slot. `filter` (nullable) is applied to the joined rows (engine.rs:73-85);
  * conjuncts that touch one pattern only are pushed into the scan. Result caps of the reference (quirk Q1) are NOT applied. */

@@ -23,6 +23,8 @@ KB_E_INVALID, KB_E_CUDA, KB_E_OOM, KB_E_UNSUPPORTED, KB_E_NOT_FOUND, KB_E_LIMIT 
 KB_ID_NONE = 0xFFFFFFFF
 KB_MAX_COLS = 16
 KB_TAG_INFERRED = 0xFFFFFFFFFFFFFFF0
+KB_TERM_QUOTED = 2  # kb_term.is_var of a `<< s p o >>` term (kb_scan_quoted)
+KB_QUOTED_MAX_DEPTH = 16
 
 # filter opcodes / comparisons / aggregates (mirror the header)
 F_CMP_NUM, F_EQ_ID, F_NE_ID, F_AND, F_OR, F_NOT, F_PUSH_VAR, F_PUSH_CONST, F_ADD, F_SUB, F_MUL, F_DIV, F_TRUTHY, F_IS_TRIPLE, F_CMP_LEGACY = range(1, 16)
@@ -41,6 +43,11 @@ class KbTerm(C.Structure):
 
 class KbPattern(C.Structure):
     _fields_ = [("s", KbTerm), ("p", KbTerm), ("o", KbTerm)]
+
+
+class KbQuotedPattern(C.Structure):
+    """kb_quoted_pattern: `outer` with KB_TERM_QUOTED in its subject and/or object; those terms are `<< inner_s >>` / `<< inner_o >>`"""
+    _fields_ = [("outer", KbPattern), ("inner_s", KbPattern), ("inner_o", KbPattern)]
 
 
 class KbFilterOp(C.Structure):
@@ -176,6 +183,7 @@ def lib() -> C.CDLL:
         "kb_strings_info": (i32, [vp, P(u64), P(u64)]),
         "kb_strings_download": (i32, [vp, vp, vp, vp]),
         "kb_strings_free": (None, [vp, vp]),
+        "kb_quoted_load": (i32, [vp, vp, vp, vp, vp, u64]),
         "kb_rel_info": (i32, [vp, P(u64), P(u32), P(u32)]),
         "kb_rel_download": (i32, [vp, vp, u32, vp]),
         "kb_rel_device_col": (i32, [vp, u32, P(vp)]),
@@ -187,6 +195,7 @@ def lib() -> C.CDLL:
         "kb_project": (i32, [vp, vp, P(u32), u32, P(vp)]),
         "kb_hash_join": (i32, [vp, vp, vp, P(vp)]),
         "kb_bind_join": (i32, [vp, vp, P(KbPattern), P(vp)]),
+        "kb_scan_quoted": (i32, [vp, P(KbQuotedPattern), P(vp)]),
         "kb_star_join": (i32, [vp, u32, P(KbPattern), u32, P(KbFilterOp), u32, P(vp)]),
         "kb_bgp_execute": (i32, [vp, P(KbPattern), u32, P(KbFilterOp), u32, P(u32), u32, P(vp)]),
         "kb_group_aggregate": (i32, [vp, vp, P(u32), u32, P(KbAgg), u32, P(vp)]),
@@ -238,8 +247,8 @@ def lib() -> C.CDLL:
 EXPORTED_SYMBOLS = [
     "kb_version", "kb_ctx_create", "kb_ctx_destroy", "kb_last_error", "kb_set_timing", "kb_get_stats", "kb_synchronize",
     "kb_store_load", "kb_store_load_device", "kb_store_append", "kb_store_append_device", "kb_store_evict", "kb_store_delete", "kb_store_clear", "kb_store_build_index", "kb_set_use_index", "kb_store_size",
-    "kb_store_download", "kb_dict_numeric_load", "kb_dict_legacy_i32_load", "kb_dict_strings_load", "kb_dict_encode", "kb_dict_strings_info", "kb_rel_decode", "kb_strings_info", "kb_strings_download", "kb_strings_free", "kb_rel_info", "kb_rel_download", "kb_rel_device_col", "kb_rel_from_host",
-    "kb_rel_from_device", "kb_rel_free", "kb_scan", "kb_filter", "kb_project", "kb_hash_join", "kb_bind_join", "kb_star_join", "kb_bgp_execute",
+    "kb_store_download", "kb_dict_numeric_load", "kb_dict_legacy_i32_load", "kb_dict_strings_load", "kb_dict_encode", "kb_dict_strings_info", "kb_rel_decode", "kb_strings_info", "kb_strings_download", "kb_strings_free", "kb_quoted_load", "kb_rel_info", "kb_rel_download", "kb_rel_device_col", "kb_rel_from_host",
+    "kb_rel_from_device", "kb_rel_free", "kb_scan", "kb_filter", "kb_project", "kb_hash_join", "kb_bind_join", "kb_scan_quoted", "kb_star_join", "kb_bgp_execute",
     "kb_group_aggregate", "kb_groups_info", "kb_groups_keys", "kb_groups_values", "kb_groups_counts", "kb_groups_free", "kb_groups_pack", "kb_groups_merge", "kb_star_join_aggregate",
     "kb_star_join_prepare", "kb_plan_submit", "kb_plan_collect", "kb_plan_info", "kb_plan_free", "kb_plan_peer_scratch_bytes", "kb_plan_attach_peers",
     "kb_datalog_fixpoint", "kb_datalog_fixpoint_seed", "kb_datalog_maintain", "kb_r2s_create", "kb_r2s_eval", "kb_r2s_info", "kb_r2s_free", "kb_shard_of", "kb_set_sharding", "kb_partition", "kb_partition_counts", "kb_segment_write", "kb_segment_info", "kb_segment_save", "kb_store_append_file", "kb_shuffle_scatter", "kb_shuffle_push", "kb_rel_wrap_device", "kb_star_join_host", "kb_star_join_host_into", "perform_hash_join_cuda",
@@ -460,7 +469,19 @@ class Context:
         self._check(lib().kb_dict_strings_info(self.h, C.byref(n), C.byref(b)))
         return int(n.value), int(b.value)
 
+    def quoted_load(self, ids, s, p, o):
+        """kb_quoted_load: the quoted-triple table (QuotedTripleStore::id_to_components) replaces the context's; empty arrays clear it"""
+        ids, s, p, o = _u32(ids), _u32(s), _u32(p), _u32(o)
+        assert len(ids) == len(s) == len(p) == len(o)
+        self._check(lib().kb_quoted_load(self.h, _ptr(ids), _ptr(s), _ptr(p), _ptr(o), len(ids)))
+
     # ---- operators
+    def scan_quoted(self, qp: KbQuotedPattern) -> Relation:
+        """kb_scan_quoted: the bag of an RDF-star pattern (one match pass over the quoted-triple table, then a bind join)"""
+        out = C.c_void_p()
+        self._check(lib().kb_scan_quoted(self.h, C.byref(qp), C.byref(out)))
+        return Relation(self, out)
+
     def scan(self, pats: Sequence[KbPattern], pushdown: Optional[Sequence[Optional[Sequence[KbFilterOp]]]] = None):
         arr = patterns(pats)
         k = len(pats)

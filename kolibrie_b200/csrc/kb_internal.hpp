@@ -179,6 +179,8 @@ struct kb_ctx {
     kb::Buf dict_index;            // kb_dict_encode: open-addressing index string -> id (hash tag << 32 | id), built lazily
     kb::u64 dict_index_slots = 0;
     kb::u32 dict_indexed = 0;      // ids [0, dict_indexed) are in the index
+    kb::Buf quoted_s, quoted_p, quoted_o;  // kb_quoted_load: the quoted-triple table, indexed by id & 0x7FFFFFFF (EMPTY32: no entry)
+    kb::u32 quoted_slots = 0;
     kb::u32 n_ids = 0;
     kb::u64 num_version = 1;  // bumped by kb_dict_numeric_load: typed literal columns of the index are tied to it
     // tile-state buffer of the look-back prefix (never cleared: words carry the launch epoch)
@@ -358,6 +360,9 @@ kb_status hash_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_rel& R, const Fi
 // agg != nullptr (kb_star_join_aggregate): agg->applied when the GROUP BY was folded into the join, else *out is the joined relation
 kb_status star_join_impl(kb_ctx* ctx, u32 join_slot, const kb_pattern* pats, u32 n_pats, const kb_filter_op* filter, u32 n_ops,
                          std::unique_ptr<kb_rel>* out, AggSpec* agg = nullptr);
+// kb_bind_join behind the entry point (the pattern is checked by the caller)
+kb_status bind_join_impl(kb_ctx* ctx, const kb_rel& left, const kb_pattern& pat, std::unique_ptr<kb_rel>* out);
+QuotedTab quotedtab(const kb_ctx* ctx);
 void pattern_vars(const kb_pattern& pt, std::vector<u32>* slots, std::vector<u32>* src);
 u32 pow2_at_least(u64 x);
 kb_status check_pattern(kb_ctx* ctx, const kb_pattern& pt);

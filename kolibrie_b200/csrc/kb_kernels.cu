@@ -3189,32 +3189,83 @@ void launch_set64_erase(u64* set, u32 set_slots, const u32* s, const u32* o, u32
 
 // =================================================================================================================
 // dictionary decode
+enum { QW_OK = 0, QW_UNKNOWN = 1, QW_DEEP = 2 };
+// Dictionary::decode_term of a quoted id (dictionary.rs:60-72) as an explicit depth-first walk: lit(text, bytes) for "<< ", " ", " >>",
+// word(id) for every dictionary component, in output order. Like the reference's `?`, the walk stops at the first id that neither table
+// holds (QW_UNKNOWN: the whole term is "unknown"); entering a level past KB_QUOTED_MAX_DEPTH gives QW_DEEP. The stack holds one table
+// index per level and a 2-bit component cursor per level.
+template <class Lit, class Word>
+__device__ u32 quoted_walk(u32 id, u32 dict_ids, const QuotedTab& qt, Lit lit, Word word) {
+    u32 ent[KB_QUOTED_MAX_DEPTH];
+    u32 next = 0;  // bits 2d..2d+1: components of level d already emitted
+    int d = 0;
+    u32 cur = id;
+    for (;;) {
+        const u32 x = cur & 0x7FFFFFFFu;
+        if (x >= qt.n || __ldg(qt.p + x) == EMPTY32) return QW_UNKNOWN;
+        if (d == KB_QUOTED_MAX_DEPTH) return QW_DEEP;
+        ent[d] = x;
+        next &= ~(3u << (2 * d));
+        d++;
+        lit("<< ", 3u);
+        for (;;) {
+            const int top = d - 1;
+            const u32 k = (next >> (2 * top)) & 3u;
+            if (k == 3u) {
+                lit(" >>", 3u);
+                if (--d == 0) return QW_OK;
+                continue;
+            }
+            next += 1u << (2 * top);
+            if (k) lit(" ", 1u);
+            const u32 e = ent[top];
+            const u32 c = __ldg((k == 0u ? qt.s : k == 1u ? qt.p : qt.o) + e);
+            if (c & 0x80000000u) { cur = c; break; }
+            if (c >= dict_ids) return QW_UNKNOWN;
+            word(c);
+        }
+    }
+}
+
 __global__ void __launch_bounds__(256) decode_lengths_kernel(const u32* __restrict__ ids, u32 n, const unsigned long long* __restrict__ dict_off, u32 dict_ids,
-                                                             u32* __restrict__ len, unsigned long long* total, u32* quoted) {
+                                                             const QuotedTab qt, u32* __restrict__ len, unsigned long long* total, u32* quoted, u32* deep) {
     const u32 stride = gridDim.x * blockDim.x;
     unsigned long long t = 0;
-    bool q = false;
+    bool q = false, dp = false;
     for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
         const u32 id = ids[i];
-        q = q || (id & 0x80000000u) != 0u;
-        const u32 l = id < dict_ids ? (u32)(__ldg(dict_off + id + 1) - __ldg(dict_off + id)) : 7u;  // "unknown"
-        len[i] = l;
+        unsigned long long l = 7u;  // "unknown"
+        if (id & 0x80000000u) {
+            if (qt.n == 0u) {
+                q = true;
+            } else {
+                unsigned long long acc = 0;
+                const u32 r = quoted_walk(id, dict_ids, qt, [&](const char*, u32 k) { acc += k; },
+                                          [&](u32 c) { acc += __ldg(dict_off + c + 1) - __ldg(dict_off + c); });
+                dp = dp || r == QW_DEEP;
+                if (r == QW_OK) l = acc;
+            }
+        } else if (id < dict_ids) {
+            l = __ldg(dict_off + id + 1) - __ldg(dict_off + id);
+        }
+        len[i] = l > 0xFFFFFFFFull ? 0xFFFFFFFFu : (u32)l;  // (the total then exceeds 2^32-1: the caller refuses the column)
         t += l;
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
     if ((threadIdx.x & 31) == 0 && t) atomicAdd(total, t);
     if (q) *quoted = 1u;
+    if (dp) *deep = 1u;
 }
-void launch_decode_lengths(const u32* ids, u32 n, const unsigned long long* dict_off, u32 dict_ids, u32* len, unsigned long long* total, u32* quoted,
-                           int n_sms, cudaStream_t st) {
+void launch_decode_lengths(const u32* ids, u32 n, const unsigned long long* dict_off, u32 dict_ids, const QuotedTab& qt, u32* len,
+                           unsigned long long* total, u32* quoted, u32* deep, int n_sms, cudaStream_t st) {
     if (n == 0) return;
     const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull);
-    decode_lengths_kernel<<<grid, 256, 0, st>>>(ids, n, dict_off, dict_ids, len, total, quoted);
+    decode_lengths_kernel<<<grid, 256, 0, st>>>(ids, n, dict_off, dict_ids, qt, len, total, quoted, deep);
 }
 __global__ void __launch_bounds__(256) decode_gather_kernel(const u32* __restrict__ ids, u32 n, const unsigned long long* __restrict__ dict_off,
-                                                            const unsigned char* __restrict__ dict_bytes, u32 dict_ids, const u32* __restrict__ off,
-                                                            unsigned char* __restrict__ out) {
+                                                            const unsigned char* __restrict__ dict_bytes, u32 dict_ids, const QuotedTab qt,
+                                                            const u32* __restrict__ off, unsigned char* __restrict__ out) {
     const int lane = threadIdx.x & 31;
     const u32 warps = (gridDim.x * blockDim.x) >> 5;
     const u32 n_chunks = (n + 31u) >> 5;
@@ -3222,29 +3273,112 @@ __global__ void __launch_bounds__(256) decode_gather_kernel(const u32* __restric
         const u32 i = chunk * 32u + (u32)lane;
         u32 id = 0, dst = 0, l = 0;
         unsigned long long src = 0;
-        bool known = false;
+        bool known = false, walk = false;
         if (i < n) {
             id = ids[i];
             dst = off[i];
             l = off[i + 1] - dst;
             known = id < dict_ids;
             if (known) src = __ldg(dict_off + id);
+            walk = (id & 0x80000000u) != 0u && l != 7u;  // a rendered quoted term is at least 8 bytes: 7 is "unknown"
         }
+        const u32 wl = walk ? 0u : l;
         for (int r = 0; r < 32; r++) {  // the warp copies row r of its chunk: consecutive lanes, consecutive bytes
-            const u32 rl = __shfl_sync(0xffffffffu, l, r);
+            const u32 rl = __shfl_sync(0xffffffffu, wl, r);
             if (rl == 0u) continue;
             const u32 rdst = __shfl_sync(0xffffffffu, dst, r);
             const unsigned long long rsrc = __shfl_sync(0xffffffffu, src, r);
             const bool rknown = __shfl_sync(0xffffffffu, known ? 1 : 0, r) != 0;
             for (u32 b = (u32)lane; b < rl; b += 32u) out[rdst + b] = rknown ? __ldg(dict_bytes + rsrc + b) : (unsigned char)"unknown"[b];
         }
+        if (walk) {  // a quoted term: this thread writes it, walking it again
+            unsigned char* w = out + dst;
+            quoted_walk(id, dict_ids, qt, [&](const char* s, u32 k) { for (u32 b = 0; b < k; b++) *w++ = (unsigned char)s[b]; },
+                        [&](u32 c) {
+                            const unsigned long long a = __ldg(dict_off + c), e = __ldg(dict_off + c + 1);
+                            for (unsigned long long b = a; b < e; b++) *w++ = __ldg(dict_bytes + b);
+                        });
+        }
     }
 }
-void launch_decode_gather(const u32* ids, u32 n, const unsigned long long* dict_off, const unsigned char* dict_bytes, u32 dict_ids, const u32* off,
-                          unsigned char* out, int n_sms, cudaStream_t st) {
+void launch_decode_gather(const u32* ids, u32 n, const unsigned long long* dict_off, const unsigned char* dict_bytes, u32 dict_ids, const QuotedTab& qt,
+                          const u32* off, unsigned char* out, int n_sms, cudaStream_t st) {
     if (n == 0) return;
     const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull);
-    decode_gather_kernel<<<grid, 256, 0, st>>>(ids, n, dict_off, dict_bytes, dict_ids, off, out);
+    decode_gather_kernel<<<grid, 256, 0, st>>>(ids, n, dict_off, dict_bytes, dict_ids, qt, off, out);
+}
+
+// =================================================================================================================
+// quoted-triple match (kb_scan_quoted): the table's s, p, o columns stream through two shared stages of QM_TILE entries each; an entry
+// that passes every check is one output row (entry id, inner variables), appended with a warp ballot and one atomic per warp
+__device__ __forceinline__ u32 qm_comp(u32 k, u32 s, u32 p, u32 o) { return k == 0u ? s : k == 1u ? p : o; }
+
+__global__ void __launch_bounds__(QM_THREADS) quoted_match_kernel(const __grid_constant__ QuotedMatchParams P) {
+    __shared__ __align__(128) u32 sbuf[2][3][QM_TILE];
+    __shared__ __align__(8) u64 bars[2];
+    __shared__ u32 s_tile[2];
+    const int tid = threadIdx.x, lane = tid & 31;
+    auto issue = [&](u32 stage) {  // one thread: take the next tile and start its three column copies into `stage`
+        const u32 t = atomicAdd(P.ticket, 1u);
+        s_tile[stage] = t;
+        if (t < P.n_tiles) {
+            const u32 b = t * (u32)QM_TILE;
+            const u32 c = min((u32)QM_TILE, P.t.n - b);
+            const u32 bytes = (c * 4u + 15u) & ~15u;  // columns are padded to 256 B: the rounded-up read stays in bounds
+            mbar_arrive_expect_tx(&bars[stage], bytes * 3u);
+            tma_load_1d(sbuf[stage][0], P.t.s + b, bytes, &bars[stage]);
+            tma_load_1d(sbuf[stage][1], P.t.p + b, bytes, &bars[stage]);
+            tma_load_1d(sbuf[stage][2], P.t.o + b, bytes, &bars[stage]);
+        }
+    };
+    if (tid == 0) {
+        mbar_init(&bars[0], 1);
+        mbar_init(&bars[1], 1);
+        fence_mbar_init();
+        issue(0);
+        issue(1);
+    }
+    __syncthreads();
+    // a CTA's tickets grow with its iterations: once a stage draws a ticket past the end, no copy is in flight in the other one
+    for (u32 it = 0;; it++) {
+        const u32 stage = it & 1u;
+        const u32 tile = s_tile[stage];
+        if (tile >= P.n_tiles) break;
+        mbar_wait(&bars[stage], (it >> 1) & 1u);
+        const u32 base = tile * (u32)QM_TILE;
+        const u32 cnt = min((u32)QM_TILE, P.t.n - base);
+        for (u32 j = (u32)tid; j < (u32)QM_TILE; j += QM_THREADS) {  // the same trip count in every lane: the ballot sees the whole warp
+            u32 s = 0, p = EMPTY32, o = 0;
+            if (j < cnt) { s = sbuf[stage][0][j]; p = sbuf[stage][1][j]; o = sbuf[stage][2][j]; }
+            bool ok = p != EMPTY32;  // (empty slots and the tail of the last tile)
+#pragma unroll
+            for (int k = 0; k < 6; k++) {
+                if ((u32)k >= P.n_chk) break;
+                const u32 v = qm_comp(P.chk_comp[k], s, p, o), a = P.chk_arg[k];
+                const u32 kind = P.chk_kind[k];
+                ok = ok && (kind == QM_CONST ? v == a : kind == QM_EQ ? v == qm_comp(a, s, p, o) : kind == QM_QUOTED ? (v & 0x80000000u) != 0u : true);
+            }
+            const unsigned b = __ballot_sync(0xffffffffu, ok);
+            if (!b) continue;
+            u32 at = 0;
+            if (lane == __ffs(b) - 1) at = atomicAdd(P.count, (u32)__popc(b));
+            at = __shfl_sync(0xffffffffu, at, __ffs(b) - 1);
+            if (ok) {
+                const u32 r = at + (u32)__popc(b & ((1u << lane) - 1u));
+                P.out[0][r] = 0x80000000u | (base + j);
+#pragma unroll
+                for (int c = 1; c < 7; c++)
+                    if ((u32)c < P.n_out) P.out[c][r] = qm_comp(P.out_comp[c], s, p, o);
+            }
+        }
+        __syncthreads();  // every thread is done with the stage: it takes the tile after next
+        if (tid == 0) issue(stage);
+    }
+}
+void launch_quoted_match(const QuotedMatchParams& p, int n_sms, cudaStream_t st) {
+    if (p.n_tiles == 0) return;
+    const int grid = grid_for((const void*)quoted_match_kernel, QM_THREADS, 0, n_sms, p.n_tiles);
+    quoted_match_kernel<<<grid, QM_THREADS, 0, st>>>(p);
 }
 
 // =================================================================================================================

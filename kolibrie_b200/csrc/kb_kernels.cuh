@@ -513,13 +513,40 @@ void launch_shuffle_scatter(const ShuffleParams& p, int n_sms, cudaStream_t st);
 
 // ---------------------------------------------------------------------------------------------------------------
 // id -> string decode of a result column (engine.rs:27-51): lengths, exclusive scan (launch_exclusive_scan_u32), byte gather
-// len[i] = length of the string of ids[i] ("unknown" = 7 bytes when the dictionary does not hold the id); *total += sum; *quoted = 1
-// when an id carries the quoted-triple bit
-void launch_decode_lengths(const u32* ids, u32 n, const unsigned long long* dict_off, u32 dict_ids, u32* len, unsigned long long* total, u32* quoted,
-                           int n_sms, cudaStream_t st);
-// out[off[i] .. off[i+1]) = bytes of the string of ids[i]; one warp per 32 rows, the lanes copy each string together
-void launch_decode_gather(const u32* ids, u32 n, const unsigned long long* dict_off, const unsigned char* dict_bytes, u32 dict_ids, const u32* off,
-                          unsigned char* out, int n_sms, cudaStream_t st);
+// The quoted-triple table (kb_quoted_load): entry id & 0x7FFFFFFF -> (s, p, o); an empty slot holds EMPTY32 in all three columns.
+// n == 0: no table.
+struct QuotedTab {
+    const u32 *s, *p, *o;
+    u32 n;
+};
+// len[i] = length of the string of ids[i] ("unknown" = 7 bytes when the dictionary does not hold the id). A quoted id: without a table
+// *quoted = 1; with one, the length of `<< s p o >>` walked with a bounded stack (dictionary.rs:60-72), "unknown" when any id on the walk
+// is held by neither table, and *deep = 1 when the walk goes past KB_QUOTED_MAX_DEPTH levels first. *total += sum.
+void launch_decode_lengths(const u32* ids, u32 n, const unsigned long long* dict_off, u32 dict_ids, const QuotedTab& qt, u32* len,
+                           unsigned long long* total, u32* quoted, u32* deep, int n_sms, cudaStream_t st);
+// out[off[i] .. off[i+1]) = bytes of the string of ids[i]; one warp per 32 rows, the lanes copy each dictionary string together; a quoted
+// row is written by its own thread, walking the term again
+void launch_decode_gather(const u32* ids, u32 n, const unsigned long long* dict_off, const unsigned char* dict_bytes, u32 dict_ids, const QuotedTab& qt,
+                          const u32* off, unsigned char* out, int n_sms, cudaStream_t st);
+
+// ---------------------------------------------------------------------------------------------------------------
+// Quoted-triple match (kb_scan_quoted; match_term over QuotedTripleStore entries, engine.rs:1088-1107): ONE streaming pass over the
+// table's three columns, QM_TILE-entry tiles TMA-staged into shared memory (two stages), matches compacted with warp ballots (row order
+// unspecified). The inner pattern(s) are compiled into at most 6 checks on the entry's components.
+constexpr int QM_TILE = 1024, QM_THREADS = 256;
+enum QmCheck : u32 { QM_NONE = 0, QM_CONST = 1 /* comp == arg */, QM_EQ = 2 /* comp == component arg */, QM_QUOTED = 3 /* comp has bit 31 */ };
+struct QuotedMatchParams {
+    QuotedTab t;
+    u32 n_tiles;
+    u32 n_chk;
+    u32 chk_kind[6], chk_comp[6], chk_arg[6];  // check k: kind, component (0 s, 1 p, 2 o), argument
+    u32 n_out;                                 // 1 + inner variables
+    u32 out_comp[7];                           // component of output column c >= 1 (column 0 = entry id)
+    u32* out[7];                               // [t.n] each
+    u32* count;                                // zeroed: rows written
+    u32* ticket;                               // zeroed: tile counter
+};
+void launch_quoted_match(const QuotedMatchParams& p, int n_sms, cudaStream_t st);
 
 // ---------------------------------------------------------------------------------------------------------------
 // Relation-to-Stream operators (kb_r2s_eval; Relation2StreamOperator::eval, r2s.rs:37-58). A set of rows is an open-addressing table

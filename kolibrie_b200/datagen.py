@@ -287,6 +287,51 @@ def taxonomy_rules(d: TaxonomyData):
     return [r1, r2]
 
 
+@dataclass
+class AnnotatedSalaries:
+    """The employee shape plus one RDF-star annotation per salary triple: `<< e ds:annual_salary s >> ex:source src_k`."""
+    d: EmployeeData
+    s: np.ndarray            # the store: the employee triples, then the annotation triples
+    p: np.ndarray
+    o: np.ndarray
+    qt_ids: np.ndarray       # quoted-triple table (QuotedTripleStore::id_to_components): id -> (e, ds:annual_salary, s)
+    qt_s: np.ndarray
+    qt_p: np.ndarray
+    qt_o: np.ndarray
+    source: int              # id of ex:source
+    src_of_employee: np.ndarray  # id of the source annotating employee i's salary triple
+    n_ids: int
+    num_or0: np.ndarray
+    is_num: np.ndarray
+
+
+def annotated_salary_dataset(n_employees: int, n_sources: int = 64, seed: int = 42, src_seed: int = 7) -> AnnotatedSalaries:
+    """employee_dataset(n_employees) plus, for employee i, the quoted triple 0x80000000 + i = << e_i ds:annual_salary s_i >> (the ids
+    QuotedTripleStore::encode hands out in that order) and the triple (that id, ex:source, src_k), k = splitmix64(src_seed, i) mod
+    n_sources. ex:source and src_0..src_{n_sources-1} take the next dictionary ids."""
+    d = employee_dataset(n_employees, seed=seed)
+    E = d.n_employees
+    sal = d.o[5::6]
+    subj = d.s[5::6]
+    source = d.n_ids
+    srcs = np.arange(d.n_ids + 1, d.n_ids + 1 + n_sources, dtype=np.uint32)
+    k = (splitmix64_at(src_seed, np.arange(E, dtype=np.uint64)) % np.uint64(n_sources)).astype(np.int64)
+    src_of = srcs[k]
+    qt_ids = (np.uint32(0x80000000) + np.arange(E, dtype=np.uint32)).astype(np.uint32)
+    n_ids = d.n_ids + 1 + n_sources
+    num = np.zeros(n_ids, dtype=np.float64)
+    isn = np.zeros(n_ids, dtype=np.uint8)
+    num[: d.n_ids], isn[: d.n_ids] = d.num_or0, d.is_num
+    return AnnotatedSalaries(d, np.concatenate([d.s, qt_ids]), np.concatenate([d.p, np.full(E, source, np.uint32)]), np.concatenate([d.o, src_of]),
+                             qt_ids, subj.copy(), np.full(E, d.ids["ds:annual_salary"], np.uint32), sal.copy(), source, src_of, n_ids, num, isn)
+
+
+def annotated_salary_answer(a: AnnotatedSalaries, threshold: float = 100000.0) -> np.ndarray:
+    """closed form of `<< ?e ds:annual_salary ?s >> ex:source ?src FILTER(?s > threshold)`: rows (e, s, src)"""
+    keep = a.d.salary_of_employee > threshold
+    return np.stack([a.qt_s[keep], a.qt_o[keep], a.src_of_employee[keep]], axis=1).astype(np.uint32)
+
+
 def canonical_rows(a: np.ndarray) -> np.ndarray:
     """rows sorted lexicographically — the canonical form parity is judged on (the reference's row order is hash order)."""
     a = np.ascontiguousarray(a, dtype=np.uint32)

@@ -176,6 +176,24 @@ class SlotMap:
     def pattern(self, p: TriplePattern) -> c.KbPattern:
         return c.pattern(self.term(p[0]), self.term(p[1]), self.term(p[2]))
 
+    def quoted_pattern(self, p: TriplePattern) -> c.KbQuotedPattern:
+        """kb_quoted_pattern of a pattern with a `<< s p o >>` subject and/or object: inside it, a nested quoted term is KB_TERM_QUOTED
+        ("any quoted-triple id", engine.rs:1100-1105)"""
+        def inner(t) -> c.KbTerm:
+            return c.KbTerm(c.KB_TERM_QUOTED, 0) if isinstance(t, QuotedTriple) else self.term(t)
+
+        def position(t):
+            if isinstance(t, QuotedTriple):
+                return c.KbTerm(c.KB_TERM_QUOTED, 0), c.pattern(inner(t.s), inner(t.p), inner(t.o))
+            return self.term(t), c.KbPattern()
+
+        if isinstance(p[1], QuotedTriple):
+            raise c.KolibrieError(c.KB_E_UNSUPPORTED, "quoted triple in predicate position")
+        s, inner_s = position(p[0])
+        pt = self.term(p[1])
+        o, inner_o = position(p[2])
+        return c.KbQuotedPattern(c.pattern(s, pt, o), inner_s, inner_o)
+
 
 # ---------------------------------------------------------------------------------------------------------------------
 # FILTER expressions (shared/src/query.rs:15-57) and their evaluation contract (types.rs:110-186)
@@ -341,6 +359,7 @@ class SparqlDatabase:
         self.ctx = ctx or c.Context(device)
         self._uploaded_version = -1
         self._version = 0
+        self._uploaded_quoted = -1  # size of the quoted-triple store the context's table was loaded from
 
     def encode_term(self, t) -> int:
         """a term given as a string, or as a nested (s, p, o) tuple for a quoted triple `<< s p o >>` (components encoded first, in
@@ -398,6 +417,7 @@ class SparqlDatabase:
         self.ctx.build_index()
 
     def _sync(self):
+        self._sync_quoted()
         if self._uploaded_version == self._version:
             return
         arr = np.array(sorted(self.triples), dtype=np.uint32).reshape(-1, 3)  # (s,p,o) order: the reference's BTreeSet iteration
@@ -406,6 +426,17 @@ class SparqlDatabase:
         self.ctx.dict_numeric_load(num, isn)
         self.ctx.dict_strings_load(self.dictionary.id_to_string)  # the final id -> string step runs on the device too
         self._uploaded_version = self._version
+
+    def _sync_quoted(self):
+        """the quoted-triple table on the device (kb_quoted_load) whenever the store's size changed (it only grows: encode never
+        removes an entry); an empty store CLEARS the table, so that a context shared with another database never keeps that one's table"""
+        qts = self.quoted_triple_store
+        if len(qts) == self._uploaded_quoted or not hasattr(self.ctx, "quoted_load"):
+            return
+        ids = np.fromiter(qts.id_to_components.keys(), dtype=np.uint32, count=len(qts))
+        comp = np.array(list(qts.id_to_components.values()), dtype=np.uint32).reshape(-1, 3)
+        self.ctx.quoted_load(ids, comp[:, 0], comp[:, 1], comp[:, 2])
+        self._uploaded_quoted = len(qts)
 
 
 class ExecutionEngine:
@@ -416,6 +447,8 @@ class ExecutionEngine:
         ctx = db.ctx
         if isinstance(op, (TableScan, IndexScan)):
             if any(isinstance(t, QuotedTriple) for t in op.pattern):
+                if hasattr(ctx, "scan_quoted"):  # matched, joined and merged on the device (kb_scan_quoted)
+                    return ctx.scan_quoted(slots.quoted_pattern(op.pattern))
                 return ExecutionEngine._scan_quoted(op.pattern, db, slots)
             return ctx.scan([slots.pattern(op.pattern)])[0]
         if isinstance(op, Filter):
@@ -446,12 +479,13 @@ class ExecutionEngine:
 
     @staticmethod
     def _scan_quoted(pattern: TriplePattern, db: SparqlDatabase, slots: SlotMap):
-        """resolve_quoted_triple_scan (engine.rs:1111-1188). The quoted-triple store is a host structure in the reference too: its
-        entries are matched against the `<< s p o >>` term(s) on the host (match_term, engine.rs:1088-1107: constants by id, variables
-        bound on first use and compared afterwards, a nested quoted term only requires a quoted-triple id), which yields one row
-        (quoted id, inner bindings) per matching entry. The reference then runs one index scan per entry with the id substituted and
-        merges the bindings, dropping conflicts; relationally that is the natural join of those rows with ONE scan of the pattern whose
-        quoted position is a fresh variable — which is what runs on the device (kb_scan + kb_rel_from_host + kb_hash_join)."""
+        """resolve_quoted_triple_scan (engine.rs:1111-1188) restated on the host: what kb_scan_quoted does on the device, kept for
+        contexts without it (the oracle) and as the reference the device is tested against. Its entries are matched against the
+        `<< s p o >>` term(s) on the host (match_term, engine.rs:1088-1107: constants by id, variables bound on first use and compared
+        afterwards, a nested quoted term only requires a quoted-triple id), which yields one row (quoted id, inner bindings) per
+        matching entry. The reference then runs one index scan per entry with the id substituted and merges the bindings, dropping
+        conflicts; relationally that is the natural join of those rows with ONE scan of the pattern whose quoted position is a fresh
+        variable (scan + rel_from_host + hash_join)."""
         ctx = db.ctx
         qt_s, qt_o = isinstance(pattern[0], QuotedTriple), isinstance(pattern[2], QuotedTriple)
         if isinstance(pattern[1], QuotedTriple):
@@ -509,8 +543,8 @@ class ExecutionEngine:
         for i in range(len(rslots)):
             try:
                 cols.append(rel.decode_strings(i))
-            except c.KolibrieError as e:  # quoted-triple ids (bit 31) are decoded on the host, recursively (dictionary.rs:58-68)
-                if e.status != c.KB_E_UNSUPPORTED:
+            except c.KolibrieError as e:  # no quoted-triple table, or a term nested too deep: decoded on the host (dictionary.rs:60-72)
+                if e.status not in (c.KB_E_UNSUPPORTED, c.KB_E_LIMIT):
                     raise
                 cols.append([db.decode_term(int(x)) or "unknown" for x in rel.column(i)])
         names = [slots.names[s] for s in rslots]

@@ -13,9 +13,14 @@ pub const KB_E_LIMIT: kb_status = -6;
 pub const KB_ID_NONE: u32 = 0xFFFF_FFFF;
 pub const KB_MAX_COLS: usize = 16;
 pub const KB_TAG_INFERRED: u64 = 0xFFFF_FFFF_FFFF_FFF0;
+pub const KB_TERM_QUOTED: u32 = 2;
+pub const KB_QUOTED_MAX_DEPTH: u32 = 16;
+pub const KB_QUOTED_MAX_SLOTS: u32 = 1 << 28;
 
 #[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbTerm { pub is_var: u32, pub value: u32 }
 #[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbPattern { pub s: KbTerm, pub p: KbTerm, pub o: KbTerm }
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbQuotedPattern { pub outer: KbPattern, pub inner_s: KbPattern, pub inner_o: KbPattern }
+pub type kb_quoted_pattern = KbQuotedPattern;  // (the header's name, as the declaration below spells it)
 #[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbFilterOp { pub op: u32, pub slot: u32, pub cmp: u32, pub id: u32, pub value: c_double }
 #[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbAgg { pub kind: u32, pub slot: u32 }
 #[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbRuleFilter { pub lhs_slot: u32, pub cmp: u32, pub rhs_is_var: u32, pub rhs_slot: u32, pub rhs_value: c_double }
@@ -71,6 +76,8 @@ extern "C" {
     pub fn kb_strings_info(s: *const KbStrings, n_strings: *mut u64, total_bytes: *mut u64) -> kb_status;
     pub fn kb_strings_download(ctx: *mut KbCtx, s: *const KbStrings, offsets: *mut u64, bytes: *mut u8) -> kb_status;
     pub fn kb_strings_free(ctx: *mut KbCtx, s: *mut KbStrings);
+    // the quoted-triple table (QuotedTripleStore::id_to_components); n = 0 clears it
+    pub fn kb_quoted_load(ctx: *mut KbCtx, ids: *const u32, s: *const u32, p: *const u32, o: *const u32, n: u64) -> kb_status;
     pub fn kb_rel_free(ctx: *mut KbCtx, r: *mut KbRel);
     // operators
     pub fn kb_scan(ctx: *mut KbCtx, pats: *const KbPattern, n: u32, pushdown: *const *const KbFilterOp, pushdown_len: *const u32, out: *mut *mut KbRel) -> kb_status;
@@ -78,6 +85,7 @@ extern "C" {
     pub fn kb_project(ctx: *mut KbCtx, r: *const KbRel, slots: *const u32, n: u32, out: *mut *mut KbRel) -> kb_status;
     pub fn kb_hash_join(ctx: *mut KbCtx, l: *const KbRel, r: *const KbRel, out: *mut *mut KbRel) -> kb_status;
     pub fn kb_bind_join(ctx: *mut KbCtx, l: *const KbRel, pattern: *const KbPattern, out: *mut *mut KbRel) -> kb_status;
+    pub fn kb_scan_quoted(ctx: *mut KbCtx, qp: *const kb_quoted_pattern, out: *mut *mut KbRel) -> kb_status;
     pub fn kb_star_join(ctx: *mut KbCtx, join_slot: u32, pats: *const KbPattern, n: u32, f: *const KbFilterOp, nf: u32, out: *mut *mut KbRel) -> kb_status;
     pub fn kb_group_aggregate(ctx: *mut KbCtx, r: *const KbRel, group_slots: *const u32, n_group: u32, aggs: *const KbAgg, n_aggs: u32, out: *mut *mut KbGroups) -> kb_status;
     pub fn kb_star_join_aggregate(ctx: *mut KbCtx, join_slot: u32, pats: *const KbPattern, n: u32, f: *const KbFilterOp, nf: u32, group_slots: *const u32, n_group: u32,

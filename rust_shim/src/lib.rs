@@ -29,6 +29,7 @@ pub struct DeviceStore {
     pub ctx: *mut KbCtx,
     synced_triples: usize,
     synced_dict: usize,
+    synced_quoted: usize,
     indexed: bool,
     /// the store is maintained segment by segment by its owner (GpuR2R: one segment per firing, the inferred segment): `sync` then
     /// mirrors the dictionary only and never replaces the store with `database.triples`
@@ -43,7 +44,7 @@ impl DeviceStore {
         if rc != KB_OK {
             return Err(unsafe { CStr::from_ptr(kb_last_error(ptr::null())) }.to_string_lossy().into_owned());
         }
-        Ok(Self { ctx, synced_triples: usize::MAX, synced_dict: usize::MAX, indexed: false, segmented: false })
+        Ok(Self { ctx, synced_triples: usize::MAX, synced_dict: usize::MAX, synced_quoted: usize::MAX, indexed: false, segmented: false })
     }
 
     pub fn last_error(&self) -> String {
@@ -70,6 +71,16 @@ impl DeviceStore {
             if unsafe { kb_dict_strings_load(self.ctx, offs.as_ptr(), bytes.as_ptr(), n as u32) } != KB_OK { return Err(self.last_error()); }
             self.synced_dict = n;
         }
+        // the quoted-triple table (kb_quoted_load) when the store's size changed; an empty store clears it (n = 0), so that a table
+        // never outlives the database it came from
+        let qt = database.quoted_triple_store.read().unwrap();
+        if qt.id_to_components.len() != self.synced_quoted {
+            let n = qt.id_to_components.len();
+            let (mut ids, mut s, mut p, mut o) = (Vec::with_capacity(n), Vec::with_capacity(n), Vec::with_capacity(n), Vec::with_capacity(n));
+            for (&id, &(a, b, c)) in qt.id_to_components.iter() { ids.push(id); s.push(a); p.push(b); o.push(c); }
+            if unsafe { kb_quoted_load(self.ctx, ids.as_ptr(), s.as_ptr(), p.as_ptr(), o.as_ptr(), n as u64) } != KB_OK { return Err(self.last_error()); }
+            self.synced_quoted = n;
+        }
         if !self.segmented && database.triples.len() != self.synced_triples {
             let n = database.triples.len();
             let (mut s, mut p, mut o) = (Vec::with_capacity(n), Vec::with_capacity(n), Vec::with_capacity(n));
@@ -88,7 +99,7 @@ impl DeviceStore {
         Ok(())
     }
 
-    pub fn invalidate(&mut self) { self.synced_triples = usize::MAX; self.synced_dict = usize::MAX; }
+    pub fn invalidate(&mut self) { self.synced_triples = usize::MAX; self.synced_dict = usize::MAX; self.synced_quoted = usize::MAX; }
 
     /// The per-term `Dictionary::encode` loop of a bulk load (sparql_database.rs:1000-1013) as one device call. Returns the ids of
     /// `terms` (those the sequential loop would hand out, dictionary.rs:32-48) and, for every NEW string in id order, the index of the
@@ -131,11 +142,31 @@ impl SlotMap {
         match t {
             Term::Variable(v) => Some(KbTerm { is_var: 1, value: self.of(v) }),
             Term::Constant(c) => Some(KbTerm { is_var: 0, value: *c }),
-            Term::QuotedTriple(_) => None,  // resolved on the host first (engine.rs:1111-1188); see kolibrie_b200/engine.py::_scan_quoted
+            Term::QuotedTriple(_) => None,  // only a TableScan / IndexScan takes `<< s p o >>` terms: see quoted_pattern
         }
     }
     pub fn pattern(&mut self, p: &TriplePattern) -> Option<KbPattern> {
         Some(KbPattern { s: self.term(&p.0)?, p: self.term(&p.1)?, o: self.term(&p.2)? })
+    }
+    /// kb_quoted_pattern of a scan with a quoted subject and/or object (kb_scan_quoted); inside a quoted term, a nested one is
+    /// KB_TERM_QUOTED: "any quoted-triple id", as match_term checks it (engine.rs:1100-1105). None for a quoted predicate.
+    pub fn quoted_pattern(&mut self, p: &TriplePattern) -> Option<KbQuotedPattern> {
+        const ANY: KbTerm = KbTerm { is_var: KB_TERM_QUOTED, value: 0 };
+        fn inner(m: &mut SlotMap, t: &Term) -> Option<KbTerm> { if t.is_quoted_triple() { Some(ANY) } else { m.term(t) } }
+        fn position(m: &mut SlotMap, t: &Term) -> Option<(KbTerm, KbPattern)> {
+            match t {
+                Term::QuotedTriple(q) => {
+                    let (s, p, o) = &**q;
+                    Some((ANY, KbPattern { s: inner(m, s)?, p: inner(m, p)?, o: inner(m, o)? }))
+                }
+                _ => Some((m.term(t)?, KbPattern::default())),
+            }
+        }
+        if p.1.is_quoted_triple() { return None; }
+        let (s, inner_s) = position(self, &p.0)?;
+        let pt = self.term(&p.1)?;
+        let (o, inner_o) = position(self, &p.2)?;
+        Some(KbQuotedPattern { outer: KbPattern { s, p: pt, o }, inner_s, inner_o })
     }
 }
 
@@ -192,12 +223,18 @@ pub fn compile_condition(cond: &Condition, slots: &mut SlotMap, database: &Sparq
 pub struct Rel(pub *mut KbRel, pub *mut KbCtx);
 impl Drop for Rel { fn drop(&mut self) { unsafe { kb_rel_free(self.1, self.0) } } }
 
+fn is_quoted(p: &TriplePattern) -> bool { p.0.is_quoted_triple() || p.1.is_quoted_triple() || p.2.is_quoted_triple() }
+
 fn run(op: &PhysicalOperator, dev: &DeviceStore, db: &SparqlDatabase, slots: &mut SlotMap) -> Option<Rel> {
     let ctx = dev.ctx;
     let mut out: *mut KbRel = ptr::null_mut();
     let ok = |rc: kb_status, out: *mut KbRel| if rc == KB_OK { Some(Rel(out, ctx)) } else { None };
     match op {
         PhysicalOperator::TableScan { pattern } | PhysicalOperator::IndexScan { pattern } => {
+            if is_quoted(pattern) {  // resolve_quoted_triple_scan (engine.rs:1111-1188) on the device
+                let q = slots.quoted_pattern(pattern)?;
+                return ok(unsafe { kb_scan_quoted(ctx, &q, &mut out) }, out);
+            }
             let p = slots.pattern(pattern)?;
             ok(unsafe { kb_scan(ctx, &p, 1, ptr::null(), ptr::null(), &mut out) }, out)
         }
@@ -225,10 +262,11 @@ fn run(op: &PhysicalOperator, dev: &DeviceStore, db: &SparqlDatabase, slots: &mu
         PhysicalOperator::ParallelJoin { left, right } => {
             let l = run(left, dev, db, slots)?;
             match right.as_ref() {  // a scan on the right is a bind join (engine.rs:935-937): the index's persistent table answers it
-                PhysicalOperator::TableScan { pattern } | PhysicalOperator::IndexScan { pattern } => {
+                PhysicalOperator::TableScan { pattern } | PhysicalOperator::IndexScan { pattern } if !is_quoted(pattern) => {
                     let p = slots.pattern(pattern)?;
                     ok(unsafe { kb_bind_join(ctx, l.0, &p, &mut out) }, out)
                 }
+                // anything else, a quoted scan included (kb_scan_quoted, then the natural join)
                 _ => { let r = run(right, dev, db, slots)?; ok(unsafe { kb_hash_join(ctx, l.0, r.0, &mut out) }, out) }
             }
         }
