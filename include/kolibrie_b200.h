@@ -249,6 +249,67 @@ KB_API void kb_strings_free(kb_ctx* ctx, kb_strings* s);
  * Like the dictionary tables, the quoted table is not tied to the store version: store mutations and index builds keep it. */
 #define KB_QUOTED_MAX_SLOTS (1u << 28)
 KB_API kb_status kb_quoted_load(kb_ctx* ctx, const uint32_t* ids, const uint32_t* s, const uint32_t* p, const uint32_t* o, uint64_t n);
+/* Entries of the quoted-triple table with ids [first_id, first_id + n) (first_id has bit 31): s[k], p[k], o[k] of id first_id + k, all
+ * three KB_ID_NONE for an id the table does not hold. Together with kb_dict_strings_download, what a host QuotedTripleStore and Dictionary
+ * take from kb_bind's kb_bind_info tails to stay equal to the device's. */
+KB_API kb_status kb_quoted_download(kb_ctx* ctx, uint32_t first_id, uint32_t n, uint32_t* s, uint32_t* p, uint32_t* o);
+/* Strings of the device dictionary with ids [first, first + n): offsets[k] .. offsets[k+1] of `bytes` is the string of id first + k,
+ * offsets[0] = 0 (offsets: n + 1 entries). bytes may be NULL (offsets only: offsets[n] is the size `bytes` needs). first + n must not
+ * pass the ids the device dictionary holds (KB_E_INVALID). */
+KB_API kb_status kb_dict_strings_download(kb_ctx* ctx, uint32_t first, uint32_t n, uint64_t* offsets, uint8_t* bytes);
+
+/* ------------------------------------------------------------------ BIND: `PhysicalOperator::Bind` with the built-in functions of
+ * ExecutionEngine::execute_with_ids (kolibrie/src/streamertail_optimizer/execution/engine.rs:144-277) over the rows of `in`, in the order
+ * they lie. *out = `in` with the output column: appended when out_slot is not a column of `in`, else that column replaced (the other
+ * columns are shared with `in`, which is left as it was).
+ *   Unbound (engine.rs:218-273): where the reference inserts nothing into a row, the output column holds KB_ID_NONE —
+ *     or, when out_slot was already a column of `in`, that row's old value (row.insert overwrites, a skipped insert keeps it). An
+ *     argument column holding KB_ID_NONE (an earlier BIND left it unbound) is a missing variable. info.n_unbound = rows whose output
+ *     value is KB_ID_NONE after the call.
+ *   KB_BIND_SUBJECT / _PREDICATE / _OBJECT (engine.rs:218-239): one variable argument; the output is that component of the quoted-triple
+ *     table entry of the argument's id. Unbound when the id is not a quoted id (bit 31), the table does not hold it (a hole, past the end,
+ *     no table) or the argument is missing.
+ *   KB_BIND_IS_TRIPLE (engine.rs:260-273): one variable argument; the output is the dictionary id of "true" (quoted id) or "false".
+ *     Unbound when the argument is missing. The two strings are encoded only when a row needs them, in the order of the first row that
+ *     needs each (the reference calls Dictionary::encode inside its row loop); a string already held keeps its id.
+ *   KB_BIND_TRIPLE (engine.rs:240-259): three arguments, each a variable or a constant id. The reference encodes a constant with
+ *     Dictionary::encode inside the row loop, so constants exist only when `in` has a row: the caller encodes them (in argument order,
+ *     only for a non-empty `in`) and passes their ids. When the three values are bound, QuotedTripleStore::encode(s, p, o)
+ *     (shared/src/quoted_triple_store.rs:45-56): a triple the table holds keeps its id (the smallest, should the table hold it twice);
+ *     every other distinct (s, p, o) gets next_qt_id + the rank of its first row among the first rows of the new triples — the ids the
+ *     sequential loop hands out. The new entries join the table (kb_scan_quoted and kb_rel_decode see them). Unbound when any argument
+ *     is missing.
+ *   KB_BIND_CONCAT (engine.rs:148-182): zero or more arguments. A variable contributes Dictionary::decode(id).unwrap_or("") (dictionary.rs:49-51) — decode,
+ *     not decode_term: a quoted id, an id the dictionary does not hold and a missing variable contribute "" — and a constant contributes
+ *     its bytes as given (the caller passes `arg.trim_matches('"')`: a constant `"a"@en` is `a"@en`). Constant k of the call (is_var 0,
+ *     value k) is const_bytes[const_offsets[k] .. const_offsets[k+1]). The concatenations are encoded as a batch with the ids the
+ *     sequential Dictionary::encode loop gives (kb_dict_encode) and joined to the device dictionary. Every row is bound.
+ * The reference's Bind checks `database.udfs` before SUBJECT..isTRIPLE (engine.rs:183): a caller with a user-defined function of the same name must not
+ * call this. Refused before anything changes: an unknown function (the reference prints "not found" and binds nothing, engine.rs:274-276) or an argument count other than the above, a CONCAT constant index
+ * past n_const, a variable argument that is not a column of `in` (KB_E_INVALID, as are next_qt_id without bit 31 or not above every id
+ * the table holds, for TRIPLE); new quoted ids reaching KB_QUOTED_MAX_SLOTS, more than 2^32-16 concatenated bytes in one call, new
+ * dictionary ids reaching bit 31, a relation of 2^32 rows or more (KB_E_LIMIT).
+ * info: n_rows, n_unbound, the new dictionary ids [dict_first, dict_first + dict_new) and the new quoted ids [quoted_first,
+ * quoted_first + quoted_new), each range in the order the reference creates them (kb_dict_strings_download / kb_quoted_download fetch
+ * them). Launches and device time count in kb_stats' `other` family. */
+enum kb_bind_function { KB_BIND_SUBJECT = 1, KB_BIND_PREDICATE = 2, KB_BIND_OBJECT = 3, KB_BIND_IS_TRIPLE = 4, KB_BIND_TRIPLE = 5, KB_BIND_CONCAT = 6 };
+#define KB_BIND_MAX_ARGS 16
+typedef struct kb_bind_spec {
+    uint32_t function;              /* kb_bind_function */
+    uint32_t n_args;
+    const kb_term* args;            /* is_var 1: variable slot; 0: constant id (TRIPLE) or constant index (CONCAT) */
+    uint32_t n_const;               /* CONCAT constants: const_offsets[n_const + 1] (const_offsets[0] = 0), const_bytes */
+    const uint64_t* const_offsets;
+    const uint8_t* const_bytes;
+    uint32_t out_slot;
+    uint32_t next_qt_id;            /* TRIPLE: QuotedTripleStore::next_qt_id */
+} kb_bind_spec;
+typedef struct kb_bind_info {
+    uint64_t n_rows, n_unbound;
+    uint32_t dict_first, dict_new;
+    uint32_t quoted_first, quoted_new;
+} kb_bind_info;
+KB_API kb_status kb_bind(kb_ctx* ctx, const kb_rel* in, const kb_bind_spec* spec, kb_rel** out, kb_bind_info* info);
 
 /* ------------------------------------------------------------------ relations */
 KB_API kb_status kb_rel_info(const kb_rel* r, uint64_t* n_rows, uint32_t* n_cols, uint32_t* slots /* [KB_MAX_COLS] or NULL */);

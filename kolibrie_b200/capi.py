@@ -35,6 +35,9 @@ AGG_COUNT, AGG_SUM, AGG_MIN, AGG_MAX, AGG_AVG = range(5)
 SEMI_NAIVE, NAIVE, SEMI_NAIVE_PARALLEL = 0, 1, 2
 SEMI_NAIVE_OLD_DELTA = 3  # textbook OLD/delta scheme: same facts, rounds and per-round counts, fewer candidates (include/kolibrie_b200.h)
 RSTREAM, ISTREAM, DSTREAM = 0, 1, 2  # kb_stream_op (r2s.rs:15-17)
+# kb_bind_function (engine.rs:144-277)
+BIND_SUBJECT, BIND_PREDICATE, BIND_OBJECT, BIND_IS_TRIPLE, BIND_TRIPLE, BIND_CONCAT = range(1, 7)
+KB_BIND_MAX_ARGS = 16
 
 
 class KbTerm(C.Structure):
@@ -48,6 +51,21 @@ class KbPattern(C.Structure):
 class KbQuotedPattern(C.Structure):
     """kb_quoted_pattern: `outer` with KB_TERM_QUOTED in its subject and/or object; those terms are `<< inner_s >>` / `<< inner_o >>`"""
     _fields_ = [("outer", KbPattern), ("inner_s", KbPattern), ("inner_o", KbPattern)]
+
+
+class KbBindSpec(C.Structure):
+    """kb_bind_spec: one BIND built-in over a relation"""
+    _fields_ = [("function", C.c_uint32), ("n_args", C.c_uint32), ("args", C.POINTER(KbTerm)), ("n_const", C.c_uint32),
+                ("const_offsets", C.POINTER(C.c_uint64)), ("const_bytes", C.POINTER(C.c_uint8)), ("out_slot", C.c_uint32), ("next_qt_id", C.c_uint32)]
+
+
+class KbBindInfo(C.Structure):
+    """kb_bind_info: rows, rows left unbound, and the new dictionary / quoted-triple ids (first, count)"""
+    _fields_ = [("n_rows", C.c_uint64), ("n_unbound", C.c_uint64), ("dict_first", C.c_uint32), ("dict_new", C.c_uint32),
+                ("quoted_first", C.c_uint32), ("quoted_new", C.c_uint32)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
 
 
 class KbFilterOp(C.Structure):
@@ -184,6 +202,9 @@ def lib() -> C.CDLL:
         "kb_strings_download": (i32, [vp, vp, vp, vp]),
         "kb_strings_free": (None, [vp, vp]),
         "kb_quoted_load": (i32, [vp, vp, vp, vp, vp, u64]),
+        "kb_quoted_download": (i32, [vp, u32, u32, vp, vp, vp]),
+        "kb_dict_strings_download": (i32, [vp, u32, u32, vp, vp]),
+        "kb_bind": (i32, [vp, vp, P(KbBindSpec), P(vp), P(KbBindInfo)]),
         "kb_rel_info": (i32, [vp, P(u64), P(u32), P(u32)]),
         "kb_rel_download": (i32, [vp, vp, u32, vp]),
         "kb_rel_device_col": (i32, [vp, u32, P(vp)]),
@@ -247,7 +268,7 @@ def lib() -> C.CDLL:
 EXPORTED_SYMBOLS = [
     "kb_version", "kb_ctx_create", "kb_ctx_destroy", "kb_last_error", "kb_set_timing", "kb_get_stats", "kb_synchronize",
     "kb_store_load", "kb_store_load_device", "kb_store_append", "kb_store_append_device", "kb_store_evict", "kb_store_delete", "kb_store_clear", "kb_store_build_index", "kb_set_use_index", "kb_store_size",
-    "kb_store_download", "kb_dict_numeric_load", "kb_dict_legacy_i32_load", "kb_dict_strings_load", "kb_dict_encode", "kb_dict_strings_info", "kb_rel_decode", "kb_strings_info", "kb_strings_download", "kb_strings_free", "kb_quoted_load", "kb_rel_info", "kb_rel_download", "kb_rel_device_col", "kb_rel_from_host",
+    "kb_store_download", "kb_dict_numeric_load", "kb_dict_legacy_i32_load", "kb_dict_strings_load", "kb_dict_encode", "kb_dict_strings_info", "kb_rel_decode", "kb_strings_info", "kb_strings_download", "kb_strings_free", "kb_quoted_load", "kb_quoted_download", "kb_dict_strings_download", "kb_bind", "kb_rel_info", "kb_rel_download", "kb_rel_device_col", "kb_rel_from_host",
     "kb_rel_from_device", "kb_rel_free", "kb_scan", "kb_filter", "kb_project", "kb_hash_join", "kb_bind_join", "kb_scan_quoted", "kb_star_join", "kb_bgp_execute",
     "kb_group_aggregate", "kb_groups_info", "kb_groups_keys", "kb_groups_values", "kb_groups_counts", "kb_groups_free", "kb_groups_pack", "kb_groups_merge", "kb_star_join_aggregate",
     "kb_star_join_prepare", "kb_plan_submit", "kb_plan_collect", "kb_plan_info", "kb_plan_free", "kb_plan_peer_scratch_bytes", "kb_plan_attach_peers",
@@ -475,7 +496,37 @@ class Context:
         assert len(ids) == len(s) == len(p) == len(o)
         self._check(lib().kb_quoted_load(self.h, _ptr(ids), _ptr(s), _ptr(p), _ptr(o), len(ids)))
 
+    def quoted_download(self, first_id: int, n: int):
+        """kb_quoted_download: (s, p, o) uint32 arrays of the table entries with ids [first_id, first_id + n) (KB_ID_NONE for a hole)"""
+        s, p, o = (np.empty(n, dtype=np.uint32) for _ in range(3))
+        self._check(lib().kb_quoted_download(self.h, first_id, n, _ptr(s), _ptr(p), _ptr(o)))
+        return s, p, o
+
+    def dict_strings_download(self, first: int, n: int) -> List[str]:
+        """kb_dict_strings_download: the device dictionary's strings with ids [first, first + n)"""
+        off = np.zeros(n + 1, dtype=np.uint64)
+        self._check(lib().kb_dict_strings_download(self.h, first, n, _ptr(off), None))
+        data = np.empty(max(int(off[-1]), 1), dtype=np.uint8)
+        self._check(lib().kb_dict_strings_download(self.h, first, n, _ptr(off), _ptr(data)))
+        raw = data.tobytes()
+        return [raw[int(off[k]):int(off[k + 1])].decode("utf-8") for k in range(n)]
+
     # ---- operators
+    def bind(self, rel: Relation, function: int, args: Sequence[KbTerm], out_slot: int, next_qt_id: int = 0,
+             consts: Sequence[bytes] = ()) -> Tuple[Relation, dict]:
+        """kb_bind: `rel` with the output column of one BIND built-in (appended, or replacing out_slot's column). args: V(slot) for a
+        variable; for TRIPLE K(id) for a constant, for CONCAT K(k) for consts[k] (bytes). Returns (relation, kb_bind_info as a dict)."""
+        terms = (KbTerm * max(len(args), 1))(*args)
+        coff = np.zeros(len(consts) + 1, dtype=np.uint64)
+        if consts:
+            coff[1:] = np.cumsum([len(b) for b in consts], dtype=np.uint64)
+        cdata = np.frombuffer(b"".join(consts) or b"\0", dtype=np.uint8).copy()
+        spec = KbBindSpec(function, len(args), terms, len(consts), coff.ctypes.data_as(C.POINTER(C.c_uint64)),
+                          cdata.ctypes.data_as(C.POINTER(C.c_uint8)), out_slot, next_qt_id)
+        out, info = C.c_void_p(), KbBindInfo()
+        self._check(lib().kb_bind(self.h, rel.h, C.byref(spec), C.byref(out), C.byref(info)))
+        return Relation(self, out), info.as_dict()
+
     def scan_quoted(self, qp: KbQuotedPattern) -> Relation:
         """kb_scan_quoted: the bag of an RDF-star pattern (one match pass over the quoted-triple table, then a bind join)"""
         out = C.c_void_p()

@@ -2859,7 +2859,10 @@ kb_status kb_quoted_load(kb_ctx* ctx, const uint32_t* ids, const uint32_t* s, co
     KB_ENTER(ctx);
     if (n == 0) {
         ctx->quoted_s.reset(); ctx->quoted_p.reset(); ctx->quoted_o.reset();
-        ctx->quoted_slots = 0;
+        ctx->quoted_slots = ctx->quoted_cap = 0;
+        ctx->quoted_rev.reset();
+        ctx->quoted_rev_slots = 0;
+        ctx->quoted_rev_indexed = 0;
         return KB_OK;
     }
     if (!ids || !s || !p || !o) return kb::fail(ctx, KB_E_INVALID, "NULL argument");
@@ -2891,7 +2894,10 @@ kb_status kb_quoted_load(kb_ctx* ctx, const uint32_t* ids, const uint32_t* s, co
     KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
     ctx->stats.h2d_bytes += (u64)slots * 12u;
     ctx->quoted_s = bs; ctx->quoted_p = bp; ctx->quoted_o = bo;
-    ctx->quoted_slots = slots;
+    ctx->quoted_slots = ctx->quoted_cap = slots;
+    ctx->quoted_rev.reset();  // (kb_bind rebuilds it on its next TRIPLE)
+    ctx->quoted_rev_slots = 0;
+    ctx->quoted_rev_indexed = 0;
     return KB_OK;
 }
 

@@ -186,55 +186,24 @@ static kb_status dict_index_ensure(kb_ctx* ctx, u64 extra) {
     return KB_OK;
 }
 
-}  // namespace kb
-
-using namespace kb;
-
-namespace {
-struct DevGuard {  // the calling thread's current device is restored on return
-    int prev = -1;
-    explicit DevGuard(int dev) {
-        cudaGetDevice(&prev);
-        if (prev != dev) cudaSetDevice(dev);
-        else prev = -1;
-    }
-    ~DevGuard() {
-        if (prev >= 0) cudaSetDevice(prev);
-    }
-};
-}  // namespace
-#define KB_ENTER(ctx)                                         \
-    if (!(ctx)) return KB_E_INVALID;                          \
-    DevGuard _guard((ctx)->device);                           \
-    KB_TRY(kb::begin_call(ctx))
-
-extern "C" {
-
-kb_status kb_dict_encode(kb_ctx* ctx, const uint64_t* offsets, const uint8_t* bytes, uint64_t n_terms, uint32_t* out_ids, uint32_t* n_new_out,
-                         uint64_t* new_first_pos) {
-    KB_ENTER(ctx);
-    if (n_new_out) *n_new_out = 0;
+// The body of kb_dict_encode over a batch already in device memory (kb_bind's CONCAT builds its concatenations there): term i =
+// d_bytes[d_off[i] .. d_off[i+1]), d_off[n] = total. The ids go to d_out_ids (device, n entries); *first_pos (nullable) receives a device
+// buffer whose entry k is the batch position of the term that introduced id (ids before the call) + k. Limits are checked before
+// anything changes.
+kb_status dict_encode_device(kb_ctx* ctx, const u64* d_off, const unsigned char* d_bytes, u64 n_terms, u64 total, u32* d_out_ids, u32* n_new_out,
+                             Buf* first_pos) {
+    *n_new_out = 0;
     if (n_terms == 0) return KB_OK;
-    if (!offsets || !out_ids) return fail(ctx, KB_E_INVALID, "NULL argument");
     if (n_terms >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "at most 2^32-16 terms per call");
-    const u64 total = offsets[n_terms];
-    if (offsets[0] != 0 || (total && !bytes)) return fail(ctx, KB_E_INVALID, "offsets must start at 0 and bytes must not be NULL");
     if (total > 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "at most 2^32-16 bytes of terms per call (split the batch)");
     if ((u64)ctx->dict_ids + n_terms >= 0x80000000ull) return fail(ctx, KB_E_LIMIT, "ids would reach bit 31 (reserved for quoted triples, quoted_triple_store.rs:28-55)");
     const u32 n = (u32)n_terms;
-    // the batch on the device
-    Buf d_off, d_bytes, d_hash, d_batch, d_ids, d_slot, d_first, d_flen, d_fpos, d_noff, scratch;
-    KB_TRY(alloc_buf(ctx, ((size_t)n + 1) * sizeof(u64), &d_off));
-    KB_TRY(alloc_buf(ctx, (size_t)total + 16, &d_bytes));
-    KB_CUDA(ctx, cudaMemcpyAsync(d_off->p, offsets, ((size_t)n + 1) * sizeof(u64), cudaMemcpyHostToDevice, ctx->st));
-    if (total) KB_CUDA(ctx, cudaMemcpyAsync(d_bytes->p, bytes, (size_t)total, cudaMemcpyHostToDevice, ctx->st));
-    ctx->stats.h2d_bytes += ((size_t)n + 1) * sizeof(u64) + total;
+    Buf d_hash, d_batch, d_slot, d_first, d_flen, d_fpos, scratch;
     KB_TRY(dict_index_ensure(ctx, n));
     u64 bslots = 1024;
     while (bslots < 2ull * n) bslots <<= 1;
     KB_TRY(alloc_buf(ctx, (size_t)n * sizeof(u64), &d_hash));
     KB_TRY(alloc_buf(ctx, bslots * sizeof(u64), &d_batch));
-    KB_TRY(alloc_buf(ctx, (size_t)n * sizeof(u32), &d_ids));
     KB_TRY(alloc_buf(ctx, (size_t)n * sizeof(u32), &d_slot));
     KB_TRY(alloc_buf(ctx, ((size_t)n + 1) * sizeof(u32), &d_first));
     KB_TRY(alloc_buf(ctx, ((size_t)n + 1) * sizeof(u32), &d_flen));
@@ -244,9 +213,9 @@ kb_status kb_dict_encode(kb_ctx* ctx, const uint64_t* offsets, const uint8_t* by
     KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + c, 0, 4 * sizeof(u32), ctx->st));
     const int grid = grid_1d(n, ctx->n_sms);
     timer_begin(ctx, F_OTHER, 5);
-    dict_hash_kernel<<<grid, 256, 0, ctx->st>>>(static_cast<const u64*>(d_off->p), static_cast<const unsigned char*>(d_bytes->p), n, static_cast<u64*>(d_hash->p));
+    dict_hash_kernel<<<grid, 256, 0, ctx->st>>>(d_off, d_bytes, n, static_cast<u64*>(d_hash->p));
     DictResolveParams P{};
-    P.off = static_cast<const u64*>(d_off->p); P.bytes = static_cast<const unsigned char*>(d_bytes->p); P.n = n;
+    P.off = d_off; P.bytes = d_bytes; P.n = n;
     P.hash = static_cast<const u64*>(d_hash->p);
     P.index = ctx->dict_ids ? static_cast<const u64*>(ctx->dict_index->p) : nullptr;
     P.index_mask = ctx->dict_index_slots - 1;
@@ -254,7 +223,7 @@ kb_status kb_dict_encode(kb_ctx* ctx, const uint64_t* offsets, const uint8_t* by
     P.dict_bytes = ctx->dict_ids ? static_cast<const unsigned char*>(ctx->dict_bytes->p) : nullptr;
     P.dict_ids = ctx->dict_ids;
     P.batch = static_cast<u64*>(d_batch->p); P.batch_mask = bslots - 1;
-    P.out_id = static_cast<u32*>(d_ids->p); P.slot_of = static_cast<u32*>(d_slot->p);
+    P.out_id = d_out_ids; P.slot_of = static_cast<u32*>(d_slot->p);
     P.overflow = ctx->ctrl + c;
     dict_resolve_kernel<<<grid, 256, 0, ctx->st>>>(P);
     dict_mark_kernel<<<grid, 256, 0, ctx->st>>>(P.off, n, P.out_id, P.slot_of, P.batch, static_cast<u32*>(d_first->p), static_cast<u32*>(d_flen->p),
@@ -314,12 +283,66 @@ kb_status kb_dict_encode(kb_ctx* ctx, const uint64_t* offsets, const uint8_t* by
     }
     timer_end(ctx);
     KB_CUDA(ctx, cudaGetLastError());
-    KB_CUDA(ctx, cudaMemcpyAsync(out_ids, d_ids->p, (size_t)n * sizeof(u32), cudaMemcpyDeviceToHost, ctx->st));
-    if (new_first_pos && n_new) KB_CUDA(ctx, cudaMemcpyAsync(new_first_pos, d_fpos->p, (size_t)n_new * sizeof(u64), cudaMemcpyDeviceToHost, ctx->st));
-    KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));  // also: `end` (a stack variable) has been consumed
-    ctx->stats.d2h_bytes += (size_t)n * sizeof(u32) + (new_first_pos ? (size_t)n_new * sizeof(u64) : 0);
+    KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));  // `end` (a stack variable) has been consumed
     ctx->dict_ids = (u32)ids_after;
     if (n_new) KB_TRY(dict_index_ensure(ctx, 0));  // the new ids enter the index
+    *n_new_out = n_new;
+    if (first_pos) *first_pos = d_fpos;
+    return KB_OK;
+}
+
+
+}  // namespace kb
+
+using namespace kb;
+
+namespace {
+struct DevGuard {  // the calling thread's current device is restored on return
+    int prev = -1;
+    explicit DevGuard(int dev) {
+        cudaGetDevice(&prev);
+        if (prev != dev) cudaSetDevice(dev);
+        else prev = -1;
+    }
+    ~DevGuard() {
+        if (prev >= 0) cudaSetDevice(prev);
+    }
+};
+}  // namespace
+#define KB_ENTER(ctx)                                         \
+    if (!(ctx)) return KB_E_INVALID;                          \
+    DevGuard _guard((ctx)->device);                           \
+    KB_TRY(kb::begin_call(ctx))
+
+extern "C" {
+
+kb_status kb_dict_encode(kb_ctx* ctx, const uint64_t* offsets, const uint8_t* bytes, uint64_t n_terms, uint32_t* out_ids, uint32_t* n_new_out,
+                         uint64_t* new_first_pos) {
+    KB_ENTER(ctx);
+    if (n_new_out) *n_new_out = 0;
+    if (n_terms == 0) return KB_OK;
+    if (!offsets || !out_ids) return fail(ctx, KB_E_INVALID, "NULL argument");
+    if (n_terms >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "at most 2^32-16 terms per call");
+    const u64 total = offsets[n_terms];
+    if (offsets[0] != 0 || (total && !bytes)) return fail(ctx, KB_E_INVALID, "offsets must start at 0 and bytes must not be NULL");
+    if (total > 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "at most 2^32-16 bytes of terms per call (split the batch)");
+    if ((u64)ctx->dict_ids + n_terms >= 0x80000000ull) return fail(ctx, KB_E_LIMIT, "ids would reach bit 31 (reserved for quoted triples, quoted_triple_store.rs:28-55)");
+    const u32 n = (u32)n_terms;
+    // the batch on the device
+    Buf d_off, d_bytes, d_ids, d_fpos;
+    KB_TRY(alloc_buf(ctx, ((size_t)n + 1) * sizeof(u64), &d_off));
+    KB_TRY(alloc_buf(ctx, (size_t)total + 16, &d_bytes));
+    KB_TRY(alloc_buf(ctx, (size_t)n * sizeof(u32), &d_ids));
+    KB_CUDA(ctx, cudaMemcpyAsync(d_off->p, offsets, ((size_t)n + 1) * sizeof(u64), cudaMemcpyHostToDevice, ctx->st));
+    if (total) KB_CUDA(ctx, cudaMemcpyAsync(d_bytes->p, bytes, (size_t)total, cudaMemcpyHostToDevice, ctx->st));
+    ctx->stats.h2d_bytes += ((size_t)n + 1) * sizeof(u64) + total;
+    u32 n_new = 0;
+    KB_TRY(dict_encode_device(ctx, static_cast<const u64*>(d_off->p), static_cast<const unsigned char*>(d_bytes->p), n, total, static_cast<u32*>(d_ids->p),
+                              &n_new, &d_fpos));
+    KB_CUDA(ctx, cudaMemcpyAsync(out_ids, d_ids->p, (size_t)n * sizeof(u32), cudaMemcpyDeviceToHost, ctx->st));
+    if (new_first_pos && n_new) KB_CUDA(ctx, cudaMemcpyAsync(new_first_pos, d_fpos->p, (size_t)n_new * sizeof(u64), cudaMemcpyDeviceToHost, ctx->st));
+    KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
+    ctx->stats.d2h_bytes += (size_t)n * sizeof(u32) + (new_first_pos ? (size_t)n_new * sizeof(u64) : 0);
     if (n_new_out) *n_new_out = n_new;
     return KB_OK;
 }

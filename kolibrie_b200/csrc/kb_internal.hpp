@@ -181,6 +181,10 @@ struct kb_ctx {
     kb::u32 dict_indexed = 0;      // ids [0, dict_indexed) are in the index
     kb::Buf quoted_s, quoted_p, quoted_o;  // kb_quoted_load: the quoted-triple table, indexed by id & 0x7FFFFFFF (EMPTY32: no entry)
     kb::u32 quoted_slots = 0;
+    kb::u32 quoted_cap = 0;        // slots the three buffers hold (kb_bind's TRIPLE grows them with headroom; slots past quoted_slots are EMPTY32)
+    kb::Buf quoted_rev;            // kb_bind's TRIPLE: reverse index (s, p, o) -> table index (hash tag << 32 | index), built lazily,
+    kb::u64 quoted_rev_slots = 0;  // dropped by kb_quoted_load
+    kb::u32 quoted_rev_indexed = 0;  // table indices [0, quoted_rev_indexed) are in it
     kb::u32 n_ids = 0;
     kb::u64 num_version = 1;  // bumped by kb_dict_numeric_load: typed literal columns of the index are tied to it
     // tile-state buffer of the look-back prefix (never cleared: words carry the launch epoch)
@@ -363,6 +367,9 @@ kb_status star_join_impl(kb_ctx* ctx, u32 join_slot, const kb_pattern* pats, u32
 // kb_bind_join behind the entry point (the pattern is checked by the caller)
 kb_status bind_join_impl(kb_ctx* ctx, const kb_rel& left, const kb_pattern& pat, std::unique_ptr<kb_rel>* out);
 QuotedTab quotedtab(const kb_ctx* ctx);
+// kb_dict_encode's body over a batch already in device memory (kb_dict.cu)
+kb_status dict_encode_device(kb_ctx* ctx, const u64* d_off, const unsigned char* d_bytes, u64 n_terms, u64 total, u32* d_out_ids, u32* n_new,
+                             Buf* first_pos);
 void pattern_vars(const kb_pattern& pt, std::vector<u32>* slots, std::vector<u32>* src);
 u32 pow2_at_least(u64 x);
 kb_status check_pattern(kb_ctx* ctx, const kb_pattern& pt);

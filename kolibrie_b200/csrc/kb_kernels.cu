@@ -3382,6 +3382,284 @@ void launch_quoted_match(const QuotedMatchParams& p, int n_sms, cudaStream_t st)
 }
 
 // =================================================================================================================
+// BIND built-ins (kb_bind)
+__device__ __forceinline__ void bind_count_unbound(bool unbound, unsigned long long* n_unbound) {
+    const unsigned b = __ballot_sync(0xffffffffu, unbound);
+    if ((threadIdx.x & 31) == 0 && b) atomicAdd(n_unbound, (unsigned long long)__popc(b));
+}
+static int bind_grid(u32 n, int n_sms) { return (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull); }
+
+__global__ void __launch_bounds__(256) bind_component_kernel(const u32* __restrict__ arg, u32 n, const QuotedTab qt, u32 comp, const u32* __restrict__ old,
+                                                             u32* __restrict__ out, unsigned long long* n_unbound) {
+    const u32* __restrict__ tab = comp == 0u ? qt.s : comp == 1u ? qt.p : qt.o;
+    const u32 stride = gridDim.x * blockDim.x;
+    const u32 end = (n + 31u) & ~31u;  // whole warps for the ballot
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < end; i += stride) {
+        u32 v = EMPTY32;
+        if (i < n) {
+            const u32 id = arg[i], x = id & 0x7FFFFFFFu;
+            if ((id & 0x80000000u) && x < qt.n) v = __ldg(tab + x);  // a hole holds EMPTY32; KB_ID_NONE has x = 2^31-1 >= qt.n
+            if (v == EMPTY32 && old) v = old[i];
+            out[i] = v;
+        }
+        bind_count_unbound(i < n && v == EMPTY32, n_unbound);
+    }
+}
+void launch_bind_component(const u32* arg, u32 n, const QuotedTab& qt, u32 comp, const u32* old, u32* out, unsigned long long* n_unbound, int n_sms,
+                           cudaStream_t st) {
+    if (n == 0) return;
+    bind_component_kernel<<<bind_grid(n, n_sms), 256, 0, st>>>(arg, n, qt, comp, old, out, n_unbound);
+}
+
+__global__ void __launch_bounds__(256) bind_istriple_first_kernel(const u32* __restrict__ arg, u32 n, u32* first) {
+    const u32 stride = gridDim.x * blockDim.x;
+    const u32 end = (n + 31u) & ~31u;
+    u32 ft = EMPTY32, ff = EMPTY32;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < end; i += stride) {
+        if (i < n) {
+            const u32 id = arg[i];
+            if (id != EMPTY32) {
+                if (id & 0x80000000u) ft = min(ft, i);
+                else ff = min(ff, i);
+            }
+        }
+    }
+    ft = __reduce_min_sync(0xffffffffu, ft);
+    ff = __reduce_min_sync(0xffffffffu, ff);
+    if ((threadIdx.x & 31) == 0) {
+        if (ft != EMPTY32) atomicMin(first, ft);
+        if (ff != EMPTY32) atomicMin(first + 1, ff);
+    }
+}
+void launch_bind_istriple_first(const u32* arg, u32 n, u32* first, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    bind_istriple_first_kernel<<<bind_grid(n, n_sms), 256, 0, st>>>(arg, n, first);
+}
+__global__ void __launch_bounds__(256) bind_istriple_write_kernel(const u32* __restrict__ arg, u32 n, u32 id_true, u32 id_false, const u32* __restrict__ old,
+                                                                  u32* __restrict__ out, unsigned long long* n_unbound) {
+    const u32 stride = gridDim.x * blockDim.x;
+    const u32 end = (n + 31u) & ~31u;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < end; i += stride) {
+        u32 v = EMPTY32;
+        if (i < n) {
+            const u32 id = arg[i];
+            v = id == EMPTY32 ? (old ? old[i] : EMPTY32) : (id & 0x80000000u) ? id_true : id_false;
+            out[i] = v;
+        }
+        bind_count_unbound(i < n && v == EMPTY32, n_unbound);
+    }
+}
+void launch_bind_istriple_write(const u32* arg, u32 n, u32 id_true, u32 id_false, const u32* old, u32* out, unsigned long long* n_unbound, int n_sms,
+                                cudaStream_t st) {
+    if (n == 0) return;
+    bind_istriple_write_kernel<<<bind_grid(n, n_sms), 256, 0, st>>>(arg, n, id_true, id_false, old, out, n_unbound);
+}
+
+// ---- TRIPLE
+__device__ __forceinline__ u64 triple_hash(u32 s, u32 p, u32 o) {
+    u64 h = ((u64)s << 32 | p) * 0x9E3779B97F4A7C15ull;
+    h ^= (u64)o * 0xC2B2AE3D27D4EB4Full;
+    h ^= h >> 31;  // murmur3 64-bit finaliser
+    h *= 0xff51afd7ed558ccdull;
+    h ^= h >> 33;
+    h *= 0xc4ceb9fe1a85ec53ull;
+    h ^= h >> 33;
+    return h;
+}
+constexpr u64 TEMPTY = 0xFFFFFFFFFFFFFFFFull;
+__device__ __forceinline__ u64 tentry(u64 h, u32 payload) { return (h & 0xFFFFFFFF00000000ull) | payload; }
+__device__ __forceinline__ void bind_triple_row(const BindTripleParams& P, u32 i, u32* s, u32* p, u32* o) {
+    *s = P.col[0] ? P.col[0][i] : P.cval[0];
+    *p = P.col[1] ? P.col[1][i] : P.cval[1];
+    *o = P.col[2] ? P.col[2][i] : P.cval[2];
+}
+
+__global__ void __launch_bounds__(256) bind_triple_resolve_kernel(const __grid_constant__ BindTripleParams P) {
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < P.n; i += gridDim.x * blockDim.x) {
+        u32 s, p, o;
+        bind_triple_row(P, i, &s, &p, &o);
+        u32 hit = EMPTY32, slot_of = EMPTY32;
+        if (s != EMPTY32 && p != EMPTY32 && o != EMPTY32) {
+            const u64 h = triple_hash(s, p, o);
+            if (P.rev) {
+                for (u64 slot = h & P.rev_mask, probes = 0; probes <= P.rev_mask; probes++, slot = (slot + 1) & P.rev_mask) {
+                    const u64 e = P.rev[slot];
+                    if (e == TEMPTY) break;
+                    if ((e >> 32) != (h >> 32)) continue;
+                    const u32 x = (u32)e;
+                    if (__ldg(P.qt.s + x) == s && __ldg(P.qt.p + x) == p && __ldg(P.qt.o + x) == o) { hit = 0x80000000u | x; break; }
+                }
+            }
+            if (hit == EMPTY32) {
+                bool placed = false;
+                for (u64 slot = h & P.batch_mask, probes = 0; probes <= P.batch_mask; probes++, slot = (slot + 1) & P.batch_mask) {
+                    u64 e = *reinterpret_cast<volatile u64*>(&P.batch[slot]);
+                    if (e == TEMPTY) {
+                        e = atomicCAS(reinterpret_cast<unsigned long long*>(&P.batch[slot]), TEMPTY, tentry(h, i));
+                        if (e == TEMPTY) { slot_of = (u32)slot; placed = true; break; }
+                    }
+                    if ((e >> 32) != (h >> 32)) continue;
+                    u32 rs, rp, ro;  // a row holding the slot's triple (the slot's position may be lowered concurrently: always the same triple)
+                    bind_triple_row(P, (u32)e, &rs, &rp, &ro);
+                    if (rs == s && rp == p && ro == o) {
+                        atomicMin(reinterpret_cast<unsigned long long*>(&P.batch[slot]), tentry(h, i));
+                        slot_of = (u32)slot;
+                        placed = true;
+                        break;
+                    }
+                }
+                if (!placed) *P.overflow = 1u;
+            }
+        }
+        P.hit[i] = hit;
+        P.slot_of[i] = slot_of;
+    }
+}
+void launch_bind_triple_resolve(const BindTripleParams& p, int n_sms, cudaStream_t st) {
+    if (p.n == 0) return;
+    bind_triple_resolve_kernel<<<bind_grid(p.n, n_sms), 256, 0, st>>>(p);
+}
+__global__ void __launch_bounds__(256) bind_triple_mark_kernel(const __grid_constant__ BindTripleParams P) {
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < P.n; i += gridDim.x * blockDim.x) {
+        const u32 so = P.slot_of[i];
+        P.first[i] = so != EMPTY32 && (u32)P.batch[so] == i ? 1u : 0u;
+    }
+}
+void launch_bind_triple_mark(const BindTripleParams& p, int n_sms, cudaStream_t st) {
+    if (p.n == 0) return;
+    bind_triple_mark_kernel<<<bind_grid(p.n, n_sms), 256, 0, st>>>(p);
+}
+__global__ void __launch_bounds__(256) bind_triple_assign_kernel(const __grid_constant__ BindTripleParams P) {
+    const u32 stride = gridDim.x * blockDim.x;
+    const u32 end = (P.n + 31u) & ~31u;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < end; i += stride) {
+        u32 v = EMPTY32;
+        if (i < P.n) {
+            const u32 so = P.slot_of[i];
+            if (so != EMPTY32) {
+                const u32 fp = (u32)P.batch[so];
+                const u32 r = P.first[fp];
+                v = P.next_qt_id + r;
+                if (fp == i) {
+                    u32 s, p, o;
+                    bind_triple_row(P, i, &s, &p, &o);
+                    const u32 x = (P.next_qt_id & 0x7FFFFFFFu) + r;
+                    P.ws[x] = s;
+                    P.wp[x] = p;
+                    P.wo[x] = o;
+                }
+            } else {
+                v = P.hit[i];
+                if (v == EMPTY32 && P.old) v = P.old[i];
+            }
+            P.out[i] = v;
+        }
+        bind_count_unbound(i < P.n && v == EMPTY32, P.n_unbound);
+    }
+}
+void launch_bind_triple_assign(const BindTripleParams& p, int n_sms, cudaStream_t st) {
+    if (p.n == 0) return;
+    bind_triple_assign_kernel<<<bind_grid(p.n, n_sms), 256, 0, st>>>(p);
+}
+__global__ void __launch_bounds__(256) quoted_rev_insert_kernel(const QuotedTab qt, u32 first, u32 n, u64* __restrict__ rev, u64 mask, u32* overflow) {
+    for (u32 k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
+        const u32 x = first + k;
+        const u32 s = qt.s[x], p = qt.p[x], o = qt.o[x];
+        if (p == EMPTY32) continue;  // a hole
+        const u64 h = triple_hash(s, p, o);
+        bool placed = false;
+        for (u64 slot = h & mask, probes = 0; probes <= mask; probes++, slot = (slot + 1) & mask) {
+            u64 e = *reinterpret_cast<volatile u64*>(&rev[slot]);
+            if (e == TEMPTY) {
+                e = atomicCAS(reinterpret_cast<unsigned long long*>(&rev[slot]), TEMPTY, tentry(h, x));
+                if (e == TEMPTY) { placed = true; break; }
+            }
+            if ((e >> 32) != (h >> 32)) continue;
+            const u32 y = (u32)e;
+            if (qt.s[y] == s && qt.p[y] == p && qt.o[y] == o) {  // the same triple twice in the table: the smaller index answers
+                atomicMin(reinterpret_cast<unsigned long long*>(&rev[slot]), tentry(h, x));
+                placed = true;
+                break;
+            }
+        }
+        if (!placed) *overflow = 1u;
+    }
+}
+void launch_quoted_rev_insert(const QuotedTab& qt, u32 first, u32 n, u64* rev, u64 mask, u32* overflow, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    quoted_rev_insert_kernel<<<bind_grid(n, n_sms), 256, 0, st>>>(qt, first, n, rev, mask, overflow);
+}
+
+// ---- CONCAT
+__device__ __forceinline__ void concat_piece(const BindConcatParams& P, u32 a, u32 i, const unsigned char** src, u32* len) {
+    if (P.col[a]) {
+        const u32 id = P.col[a][i];
+        if (id < P.dict_ids) {  // Dictionary::decode: quoted ids (>= 2^31 > dict_ids), missing ids and KB_ID_NONE contribute ""
+            const unsigned long long b = __ldg(P.dict_off + id);
+            *src = P.dict_bytes + b;
+            *len = (u32)(__ldg(P.dict_off + id + 1) - b);
+        } else {
+            *src = nullptr;
+            *len = 0u;
+        }
+    } else {
+        *src = P.cbytes + P.coff[a];
+        *len = P.clen[a];
+    }
+}
+__global__ void __launch_bounds__(256) bind_concat_lengths_kernel(const __grid_constant__ BindConcatParams P) {
+    unsigned long long t = 0;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < P.n; i += gridDim.x * blockDim.x) {
+        unsigned long long l = 0;
+        for (u32 a = 0; a < P.n_args; a++) {
+            const unsigned char* src;
+            u32 k;
+            concat_piece(P, a, i, &src, &k);
+            l += k;
+        }
+        P.len[i] = l > 0xFFFFFFFFull ? 0xFFFFFFFFu : (u32)l;  // (the total then exceeds the limit: the caller refuses the call)
+        t += l;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+    if ((threadIdx.x & 31) == 0 && t) atomicAdd(P.total, t);
+}
+void launch_bind_concat_lengths(const BindConcatParams& p, int n_sms, cudaStream_t st) {
+    if (p.n == 0) return;
+    bind_concat_lengths_kernel<<<bind_grid(p.n, n_sms), 256, 0, st>>>(p);
+}
+__global__ void __launch_bounds__(256) bind_concat_gather_kernel(const __grid_constant__ BindConcatParams P) {
+    const int lane = threadIdx.x & 31;
+    const u32 warps = (gridDim.x * blockDim.x) >> 5;
+    const u32 n_chunks = (P.n + 31u) >> 5;
+    for (u32 chunk = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; chunk < n_chunks; chunk += warps) {
+        const u32 i = chunk * 32u + (u32)lane;
+        u32 dst = 0;
+        if (i < P.n) {
+            dst = P.len[i];
+            P.off64[i] = dst;
+            if (i + 1u == P.n) P.off64[P.n] = P.len[P.n];
+        }
+        const u32 rows = min(32u, P.n - chunk * 32u);
+        for (u32 r = 0; r < rows; r++) {  // the warp writes row r of its chunk, piece by piece: consecutive lanes, consecutive bytes
+            const u32 row = chunk * 32u + r;
+            u32 w = __shfl_sync(0xffffffffu, dst, (int)r);
+            for (u32 a = 0; a < P.n_args; a++) {
+                const unsigned char* src;
+                u32 k;
+                concat_piece(P, a, row, &src, &k);  // (the same address in every lane: one broadcast load)
+                for (u32 b = (u32)lane; b < k; b += 32u) P.out[w + b] = __ldg(src + b);
+                w += k;
+            }
+        }
+    }
+}
+void launch_bind_concat_gather(const BindConcatParams& p, int n_sms, cudaStream_t st) {
+    if (p.n == 0) return;
+    bind_concat_gather_kernel<<<bind_grid(p.n, n_sms), 256, 0, st>>>(p);
+}
+
+// =================================================================================================================
 // utilities
 __global__ void fill_kernel(u32* p, u32 v, u64 n) {
     for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) p[i] = v;

@@ -549,6 +549,65 @@ struct QuotedMatchParams {
 void launch_quoted_match(const QuotedMatchParams& p, int n_sms, cudaStream_t st);
 
 // ---------------------------------------------------------------------------------------------------------------
+// BIND built-ins (kb_bind, engine.rs:144-277). Every write pass takes `old` (the replaced column when the output variable was bound
+// already, else null): a row the reference does not insert into keeps old[i], or gets EMPTY32; *n_unbound += rows left EMPTY32.
+// SUBJECT / PREDICATE / OBJECT: out[i] = component `comp` of the table entry of arg[i] (a quoted id the table holds), else unbound
+void launch_bind_component(const u32* arg, u32 n, const QuotedTab& qt, u32 comp, const u32* old, u32* out, unsigned long long* n_unbound,
+                           int n_sms, cudaStream_t st);
+// isTRIPLE, pass 1: first[0] = min row whose argument is a quoted id, first[1] = min row whose argument is bound and not quoted
+// (first[] = EMPTY32 beforehand)
+void launch_bind_istriple_first(const u32* arg, u32 n, u32* first, int n_sms, cudaStream_t st);
+// isTRIPLE, pass 2: out[i] = id_true / id_false, unbound where the argument is
+void launch_bind_istriple_write(const u32* arg, u32 n, u32 id_true, u32 id_false, const u32* old, u32* out, unsigned long long* n_unbound,
+                                int n_sms, cudaStream_t st);
+// TRIPLE: QuotedTripleStore::encode of a batch, the kb_dict_encode scheme on a 96-bit key. The reverse index (s, p, o) -> table index is an
+// open-addressing table of (hash tag << 32 | index) entries, compared against the forward table on a tag match; the batch table keeps
+// (hash tag << 32 | smallest row) per new triple.
+struct BindTripleParams {
+    const u32* col[3];        // argument columns (null: the constant cval[k])
+    u32 cval[3];
+    u32 n;
+    QuotedTab qt;             // forward table: lookups compare against it
+    const u64* rev;           // reverse index (null: empty table)
+    u64 rev_mask;
+    u64* batch;               // all ~0 beforehand
+    u64 batch_mask;
+    u32* hit;                 // [n] id the table holds, else EMPTY32
+    u32* slot_of;             // [n] batch slot of a new triple's row, EMPTY32 for a hit or an unbound row
+    u32* first;               // [n + 1] 1 on the first row of every new triple; then its exclusive prefix (the rank)
+    u32* overflow;
+    u32 next_qt_id;           // the assign pass: ids next_qt_id + rank, entries written into ws / wp / wo at (next_qt_id & 0x7FFFFFFF) + rank
+    u32 *ws, *wp, *wo;
+    const u32* old;
+    u32* out;
+    unsigned long long* n_unbound;
+};
+void launch_bind_triple_resolve(const BindTripleParams& p, int n_sms, cudaStream_t st);
+void launch_bind_triple_mark(const BindTripleParams& p, int n_sms, cudaStream_t st);
+void launch_bind_triple_assign(const BindTripleParams& p, int n_sms, cudaStream_t st);
+// table indices [first, first + n) enter the reverse index (empty slots skipped; of two equal triples the index keeps the smaller)
+void launch_quoted_rev_insert(const QuotedTab& qt, u32 first, u32 n, u64* rev, u64 mask, u32* overflow, int n_sms, cudaStream_t st);
+// CONCAT: the pieces of row i are, per argument a, the dictionary string of col[a][i] ("" when the dictionary does not hold it) or the
+// constant cbytes[coff[a] .. coff[a] + clen[a])
+struct BindConcatParams {
+    u32 n, n_args;
+    const u32* col[KB_BIND_MAX_ARGS];  // null: a constant
+    u64 coff[KB_BIND_MAX_ARGS];
+    u32 clen[KB_BIND_MAX_ARGS];
+    const unsigned char* cbytes;
+    const unsigned long long* dict_off;
+    const unsigned char* dict_bytes;
+    u32 dict_ids;
+    u32* len;                          // lengths pass: [n + 1] (len[n] untouched); then their exclusive prefix
+    unsigned long long* total;         // lengths pass: += bytes of all rows
+    u64* off64;                        // gather pass: [n + 1] the prefix widened (the encode's offsets)
+    unsigned char* out;
+};
+void launch_bind_concat_lengths(const BindConcatParams& p, int n_sms, cudaStream_t st);
+// one warp per 32 rows: the lanes copy each piece of a row together (decode_gather's access pattern)
+void launch_bind_concat_gather(const BindConcatParams& p, int n_sms, cudaStream_t st);
+
+// ---------------------------------------------------------------------------------------------------------------
 // Relation-to-Stream operators (kb_r2s_eval; Relation2StreamOperator::eval, r2s.rs:37-58). A set of rows is an open-addressing table
 // of u32 row indices (EMPTY32 = free slot) keyed by a 64-bit mix of the row's columns in the operator's slot order; a hash hit is
 // confirmed by comparing every column.

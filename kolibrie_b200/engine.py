@@ -160,6 +160,8 @@ class SlotMap:
     def __init__(self):
         self.slot: Dict[str, int] = {}
         self.names: List[str] = []
+        self.bind_out: set = set()   # slots a Bind wrote: a KB_ID_NONE there is an unbound variable (left out of result rows)
+        self.bind_only: set = set()  # Bind outputs no device operator may read (unbound rows, or strings the numeric table lacks)
 
     def of(self, name: str) -> int:
         name = _strip(name)
@@ -234,6 +236,7 @@ class FunctionCall:
 
 
 _CMP = {">": c.CMP_GT, ">=": c.CMP_GE, "<": c.CMP_LT, "<=": c.CMP_LE}
+_SLOT_OPS = {c.F_CMP_NUM, c.F_EQ_ID, c.F_NE_ID, c.F_PUSH_VAR, c.F_IS_TRIPLE, c.F_CMP_LEGACY}  # filter ops that read row[slot]
 
 
 class Condition:
@@ -349,6 +352,20 @@ class InMemoryBuffer:
     content: List[Dict[str, int]]
 
 
+@dataclass
+class Bind:
+    """PhysicalOperator::Bind (operators/physical.rs; engine.rs:144-277): a built-in function of the input's rows into
+    output_variable. Arguments are strings as in the reference: "?x" a variable, anything else a constant."""
+    input: object
+    function_name: str
+    arguments: List[str]
+    output_variable: str
+
+
+_BIND_FUNCTIONS = {"SUBJECT": c.BIND_SUBJECT, "PREDICATE": c.BIND_PREDICATE, "OBJECT": c.BIND_OBJECT, "isTRIPLE": c.BIND_IS_TRIPLE,
+                   "TRIPLE": c.BIND_TRIPLE, "CONCAT": c.BIND_CONCAT}
+
+
 class SparqlDatabase:
     """triples (set semantics, iteration in (s,p,o) order like the reference's BTreeSet) + dictionary + the device store."""
 
@@ -457,25 +474,213 @@ class ExecutionEngine:
                 return ctx.star_join(slots.of(op.input.join_var), [slots.pattern(p) for p in op.input.patterns],
                                      op.condition.compile(slots, db.dictionary))
             rel = ExecutionEngine._run(op.input, db, slots)
-            return ctx.filter(rel, op.condition.compile(slots, db.dictionary))
+            prog = op.condition.compile(slots, db.dictionary)
+            ExecutionEngine._check_reads(slots, {o.slot for o in prog if o.op in _SLOT_OPS}, "a FILTER")
+            return ctx.filter(rel, prog)
         if isinstance(op, Projection):
             rel = ExecutionEngine._run(op.input, db, slots)
             return ctx.project(rel, [slots.of(v) for v in op.variables])
         if isinstance(op, (HashJoin, OptimizedHashJoin, NestedLoopJoin)):
-            return ctx.hash_join(ExecutionEngine._run(op.left, db, slots), ExecutionEngine._run(op.right, db, slots))
+            return ExecutionEngine._join(ctx, slots, ExecutionEngine._run(op.left, db, slots), ExecutionEngine._run(op.right, db, slots))
         if isinstance(op, ParallelJoin):
             # right side a scan -> bind join (engine.rs:935-937) == natural join of left with the pattern's matches: kb_bind_join looks the
             # pattern up in the index's persistent tables when it can, and scans + joins otherwise
             if isinstance(op.right, (TableScan, IndexScan)) and not any(isinstance(t, QuotedTriple) for t in op.right.pattern) and hasattr(ctx, "bind_join"):
-                return ctx.bind_join(ExecutionEngine._run(op.left, db, slots), slots.pattern(op.right.pattern))
-            return ctx.hash_join(ExecutionEngine._run(op.left, db, slots), ExecutionEngine._run(op.right, db, slots))
+                left = ExecutionEngine._run(op.left, db, slots)
+                pat = slots.pattern(op.right.pattern)
+                ExecutionEngine._check_reads(slots, set(left.slots) & {t.value for t in (pat.s, pat.p, pat.o) if t.is_var}, "a join")
+                return ctx.bind_join(left, pat)
+            return ExecutionEngine._join(ctx, slots, ExecutionEngine._run(op.left, db, slots), ExecutionEngine._run(op.right, db, slots))
         if isinstance(op, StarJoin):
             return ctx.star_join(slots.of(op.join_var), [slots.pattern(p) for p in op.patterns])
         if isinstance(op, InMemoryBuffer):
             names = sorted({k for row in op.content for k in row})
             cols = [np.array([row[k] for row in op.content], dtype=np.uint32) for k in names]
             return ctx.rel_from_host([slots.of(k) for k in names], cols)
+        if isinstance(op, Bind):
+            rel = ExecutionEngine._run(op.input, db, slots)
+            if hasattr(ctx, "bind"):  # on the device (kb_bind)
+                return ExecutionEngine._bind_device(op, rel, db, slots)
+            return ExecutionEngine._bind_rel(op, rel, db, slots)
         raise c.KolibrieError(c.KB_E_UNSUPPORTED, f"operator {type(op).__name__} stays on the reference's CPU path")
+
+    @staticmethod
+    def _check_reads(slots: SlotMap, read: set, what: str):
+        """the reference's plan builder puts Bind above every join and filter (utils.rs:101-191); a plan that reads a Bind output
+        with unbound rows, or a CONCAT / isTRIPLE string the device's numeric table does not know, below that is refused"""
+        bad = read & slots.bind_only
+        if bad:
+            raise c.KolibrieError(c.KB_E_UNSUPPORTED, f"{what} reads the BIND output ?{slots.names[min(bad)]}: the reference's CPU path")
+
+    @staticmethod
+    def _join(ctx, slots: SlotMap, left: c.Relation, right: c.Relation) -> c.Relation:
+        ExecutionEngine._check_reads(slots, set(left.slots) & set(right.slots), "a join")
+        return ctx.hash_join(left, right)
+
+    @staticmethod
+    def _bind_host(function_name: str, arguments: Sequence[str], cols: Dict[str, np.ndarray], n: int, old: Optional[np.ndarray],
+                   dictionary: Dictionary, qts: QuotedTripleStore) -> np.ndarray:
+        """Bind (engine.rs:144-277) restated on the host over columns: `cols` maps a variable name (no '?') to its ids, KB_ID_NONE where
+        the row lacks it; `old` is the output variable's column when the input binds it already. Returns the output column (KB_ID_NONE
+        where the reference inserts nothing and `old` has nothing) and makes the encodes the reference makes, in its order, in
+        `dictionary` and `qts`. What kb_bind computes on the device, kept for contexts without it (the oracle) and as the reference
+        the device is tested against."""
+        NONE = c.KB_ID_NONE
+        out = np.full(n, NONE, dtype=np.uint32) if old is None else np.array(old, dtype=np.uint32)
+        if n == 0:
+            return out
+
+        def arg_col(arg: str) -> np.ndarray:  # row.get(arg.strip_prefix('?')): a missing key is KB_ID_NONE
+            col = cols.get(_strip(arg))
+            return np.full(n, NONE, dtype=np.uint32) if col is None else np.asarray(col, dtype=np.uint32)
+
+        if function_name == "CONCAT":  # engine.rs:148-182: Dictionary::decode (not decode_term), "" when it gives None
+            parts = []
+            for arg in arguments:
+                if arg.startswith("?"):
+                    ids = arg_col(arg)
+                    uniq, inv = np.unique(ids, return_inverse=True)
+                    text = np.array([dictionary.decode(int(i)) or "" for i in uniq], dtype=object)
+                    parts.append(text[inv.reshape(-1)])
+                else:
+                    parts.append(np.full(n, arg.strip('"'), dtype=object))  # trim_matches('"'): every leading and trailing quote
+            joined = ["".join(p[i] for p in parts) for i in range(n)] if parts else [""] * n
+            for i, t in enumerate(joined):
+                out[i] = dictionary.encode(t)
+            return out
+        if function_name in ("SUBJECT", "PREDICATE", "OBJECT"):  # engine.rs:218-239
+            if not arguments:
+                return out
+            k = ("SUBJECT", "PREDICATE", "OBJECT").index(function_name)
+            ids = arg_col(arguments[0])
+            q = ((ids & QUOTED_TRIPLE_ID_BIT) != 0) & (ids != NONE)
+            uniq, inv = np.unique(ids[q], return_inverse=True)
+            comp = np.array([(qts.decode(int(i)) or (NONE, NONE, NONE))[k] for i in uniq], dtype=np.uint32)
+            val = comp[inv.reshape(-1)] if len(uniq) else np.empty(0, np.uint32)
+            hit = val != NONE
+            rows = np.nonzero(q)[0][hit]
+            out[rows] = val[hit]
+            return out
+        if function_name == "TRIPLE":  # engine.rs:240-259
+            if len(arguments) != 3:
+                return out
+            vals = []
+            for arg in arguments:  # a constant is encoded inside the row loop: at the first row, in argument order
+                vals.append(arg_col(arg) if arg.startswith("?") else np.full(n, dictionary.encode(arg), dtype=np.uint32))
+            s, p, o = vals
+            bound = np.nonzero((s != NONE) & (p != NONE) & (o != NONE))[0]
+            key = (s[bound].astype(np.uint64) << np.uint64(32) | p[bound].astype(np.uint64), o[bound])
+            order = np.lexsort((bound, key[1], key[0]))  # rows grouped by triple, each group in row order
+            ks, ko = key[0][order], key[1][order]
+            start = np.ones(len(order), dtype=bool)
+            start[1:] = (ks[1:] != ks[:-1]) | (ko[1:] != ko[:-1])
+            firsts = order[start]
+            group = np.cumsum(start) - 1
+            ids = np.empty(len(firsts), dtype=np.uint32)
+            for g in np.argsort(bound[firsts], kind="stable"):  # encode in the order of each triple's first row
+                r = bound[firsts[g]]
+                ids[g] = qts.encode(int(s[r]), int(p[r]), int(o[r]))
+            res = np.empty(len(bound), dtype=np.uint32)
+            res[order] = ids[group]
+            out[bound] = res
+            return out
+        if function_name == "isTRIPLE":  # engine.rs:260-273: "true" / "false" encoded when a row first needs them
+            if not arguments:
+                return out
+            ids = arg_col(arguments[0])
+            bound = ids != NONE
+            quoted = bound & ((ids & QUOTED_TRIPLE_ID_BIT) != 0)
+            plain = bound & ~quoted
+            need = sorted((int(np.argmax(m)), t) for m, t in ((quoted, "true"), (plain, "false")) if m.any())
+            tid = {t: dictionary.encode(t) for _, t in need}
+            if "true" in tid:
+                out[quoted] = tid["true"]
+            if "false" in tid:
+                out[plain] = tid["false"]
+            return out
+        return out  # "Function ... not found": the rows as they were (engine.rs:274-276)
+
+    @staticmethod
+    def _bind_rel(op: "Bind", rel: c.Relation, db: SparqlDatabase, slots: SlotMap) -> c.Relation:
+        """Bind through the host restatement: download, _bind_host, upload"""
+        n, rslots = rel.info()
+        cols = {slots.names[sl]: rel.column(i) for i, sl in enumerate(rslots)}
+        out_name = _strip(op.output_variable)
+        out_slot = slots.of(out_name)
+        n_ids = len(db.dictionary.id_to_string)
+        col = ExecutionEngine._bind_host(op.function_name, op.arguments, cols, n, cols.get(out_name), db.dictionary, db.quoted_triple_store)
+        if len(db.dictionary.id_to_string) != n_ids and hasattr(db.ctx, "dict_strings_load"):
+            db.ctx.dict_strings_load(db.dictionary.id_to_string)  # the final decode reads the new strings on the device
+        db._sync_quoted()
+        cols[out_name] = col
+        ExecutionEngine._mark_bind(slots, out_slot, op.function_name, bool((col == c.KB_ID_NONE).any()))
+        names = list(cols)
+        return db.ctx.rel_from_host([slots.of(k) for k in names], [cols[k] for k in names])
+
+    @staticmethod
+    def _mark_bind(slots: SlotMap, out_slot: int, function_name: str, has_unbound: bool):
+        slots.bind_out.add(out_slot)
+        if has_unbound or function_name in ("CONCAT", "isTRIPLE"):
+            slots.bind_only.add(out_slot)
+        else:
+            slots.bind_only.discard(out_slot)
+
+    @staticmethod
+    def _bind_device(op: "Bind", rel: c.Relation, db: SparqlDatabase, slots: SlotMap) -> c.Relation:
+        """kb_bind, then the host Dictionary and QuotedTripleStore take the new entries in the order the device created them"""
+        ctx = db.ctx
+        fn = _BIND_FUNCTIONS.get(op.function_name)
+        if fn is None:
+            raise c.KolibrieError(c.KB_E_UNSUPPORTED, f"BIND function {op.function_name!r}: the reference's CPU path (UDFs stay there)")
+        n, rslots = rel.info()
+
+        def var(arg: str) -> c.KbTerm:
+            sl = slots.slot.get(_strip(arg))
+            if sl is None or sl not in rslots:
+                raise c.KolibrieError(c.KB_E_UNSUPPORTED, f"BIND argument {arg!r} is not a variable of its input: the reference's CPU path")
+            return c.V(sl)
+
+        args: List[c.KbTerm] = []
+        consts: List[bytes] = []
+        if fn == c.BIND_CONCAT:
+            for arg in op.arguments:
+                sl = slots.slot.get(_strip(arg)) if arg.startswith("?") else None
+                if sl is not None and sl in rslots:
+                    args.append(c.V(sl))
+                else:  # a constant, or a variable the rows lack (it contributes "")
+                    args.append(c.K(len(consts)))
+                    consts.append(b"" if arg.startswith("?") else arg.strip('"').encode("utf-8"))
+        elif fn == c.BIND_TRIPLE:
+            if len(op.arguments) != 3:
+                raise c.KolibrieError(c.KB_E_UNSUPPORTED, "TRIPLE takes 3 arguments")
+            const = [a for a in op.arguments if not a.startswith("?")]
+            ids = iter(db.dictionary.encode_bulk(ctx, const) if (const and n) else [0] * len(const))  # encoded at the first row only
+            args = [var(a) if a.startswith("?") else c.K(int(next(ids))) for a in op.arguments]
+        else:
+            if len(op.arguments) != 1:
+                raise c.KolibrieError(c.KB_E_UNSUPPORTED, f"{op.function_name} takes 1 argument")
+            args = [var(op.arguments[0])]
+        n_dev, _ = ctx.dict_strings_info()
+        if n_dev != len(db.dictionary.id_to_string):
+            ctx.dict_strings_load(db.dictionary.id_to_string)
+        out_slot = slots.of(_strip(op.output_variable))
+        qts = db.quoted_triple_store
+        res, info = ctx.bind(rel, fn, args, out_slot, qts.next_qt_id if fn == c.BIND_TRIPLE else 0, consts)
+        d = db.dictionary
+        for t in ctx.dict_strings_download(info["dict_first"], info["dict_new"]):
+            d.string_to_id[t] = len(d.id_to_string)
+            d.id_to_string.append(t)
+        if info["quoted_new"]:
+            first = info["quoted_first"]
+            qs, qp, qo = ctx.quoted_download(first, info["quoted_new"])
+            for k in range(info["quoted_new"]):
+                key = (int(qs[k]), int(qp[k]), int(qo[k]))
+                qts.id_to_components[first + k] = key
+                qts.components_to_id[key] = first + k
+            qts.next_qt_id = first + info["quoted_new"]
+            db._uploaded_quoted = len(qts)  # the device table holds them already: no reload (it would drop the reverse index)
+        ExecutionEngine._mark_bind(slots, out_slot, op.function_name, info["n_unbound"] > 0)
+        return res
 
     @staticmethod
     def _scan_quoted(pattern: TriplePattern, db: SparqlDatabase, slots: SlotMap):
@@ -530,6 +735,9 @@ class ExecutionEngine:
         n, rslots = rel.info()
         cols = [rel.column(i) for i in range(len(rslots))]
         names = [slots.names[s] for s in rslots]
+        if slots.bind_out:  # a variable a BIND left unbound is not a key of the row (the reference does not insert it)
+            return [{names[j]: int(cols[j][i]) for j in range(len(names)) if not (rslots[j] in slots.bind_out and cols[j][i] == c.KB_ID_NONE)}
+                    for i in range(n)]
         return [{names[j]: int(cols[j][i]) for j in range(len(names))} for i in range(n)]
 
     @staticmethod
@@ -548,6 +756,9 @@ class ExecutionEngine:
                     raise
                 cols.append([db.decode_term(int(x)) or "unknown" for x in rel.column(i)])
         names = [slots.names[s] for s in rslots]
+        unbound = {j: rel.column(j) == c.KB_ID_NONE for j in range(len(rslots)) if rslots[j] in slots.bind_out}
+        if unbound:
+            return [{names[j]: cols[j][i] for j in range(len(names)) if not (j in unbound and unbound[j][i])} for i in range(n)]
         return [{names[j]: cols[j][i] for j in range(len(names))} for i in range(n)]
 
 

@@ -34,6 +34,16 @@ pub type kb_quoted_pattern = KbQuotedPattern;  // (the header's name, as the dec
 #[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbMaintainStats { pub base_removed: u64, pub base_added: u64, pub overdeleted: u64, pub rederived: u64,
     pub inferred_removed: u64, pub inferred_added: u64, pub derivations: u64, pub overdelete_rounds: u32, pub insert_rounds: u32, pub device_ms: c_double }
 pub type kb_maintain_stats = KbMaintainStats;  // (the header's name, as the declaration below spells it)
+#[repr(C)] #[derive(Clone, Copy, Debug)] pub struct KbBindSpec { pub function: u32, pub n_args: u32, pub args: *const KbTerm, pub n_const: u32,
+    pub const_offsets: *const u64, pub const_bytes: *const u8, pub out_slot: u32, pub next_qt_id: u32 }
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbBindInfo { pub n_rows: u64, pub n_unbound: u64, pub dict_first: u32, pub dict_new: u32,
+    pub quoted_first: u32, pub quoted_new: u32 }
+pub type kb_bind_spec = KbBindSpec;  // (the header's names, as the declarations below spell them)
+pub type kb_bind_info = KbBindInfo;
+// kb_bind_function (engine.rs:144-277)
+pub const KB_BIND_SUBJECT: u32 = 1; pub const KB_BIND_PREDICATE: u32 = 2; pub const KB_BIND_OBJECT: u32 = 3; pub const KB_BIND_IS_TRIPLE: u32 = 4;
+pub const KB_BIND_TRIPLE: u32 = 5; pub const KB_BIND_CONCAT: u32 = 6;
+pub const KB_BIND_MAX_ARGS: u32 = 16;
 
 // kb_filter_opcode / kb_cmp / kb_agg_kind / kb_strategy
 pub const KB_F_CMP_NUM: u32 = 1; pub const KB_F_EQ_ID: u32 = 2; pub const KB_F_NE_ID: u32 = 3; pub const KB_F_AND: u32 = 4; pub const KB_F_OR: u32 = 5;
@@ -78,6 +88,9 @@ extern "C" {
     pub fn kb_strings_free(ctx: *mut KbCtx, s: *mut KbStrings);
     // the quoted-triple table (QuotedTripleStore::id_to_components); n = 0 clears it
     pub fn kb_quoted_load(ctx: *mut KbCtx, ids: *const u32, s: *const u32, p: *const u32, o: *const u32, n: u64) -> kb_status;
+    // the tails kb_bind adds: quoted-table entries and dictionary strings by id range
+    pub fn kb_quoted_download(ctx: *mut KbCtx, first_id: u32, n: u32, s: *mut u32, p: *mut u32, o: *mut u32) -> kb_status;
+    pub fn kb_dict_strings_download(ctx: *mut KbCtx, first: u32, n: u32, offsets: *mut u64, bytes: *mut u8) -> kb_status;
     pub fn kb_rel_free(ctx: *mut KbCtx, r: *mut KbRel);
     // operators
     pub fn kb_scan(ctx: *mut KbCtx, pats: *const KbPattern, n: u32, pushdown: *const *const KbFilterOp, pushdown_len: *const u32, out: *mut *mut KbRel) -> kb_status;
@@ -86,6 +99,7 @@ extern "C" {
     pub fn kb_hash_join(ctx: *mut KbCtx, l: *const KbRel, r: *const KbRel, out: *mut *mut KbRel) -> kb_status;
     pub fn kb_bind_join(ctx: *mut KbCtx, l: *const KbRel, pattern: *const KbPattern, out: *mut *mut KbRel) -> kb_status;
     pub fn kb_scan_quoted(ctx: *mut KbCtx, qp: *const kb_quoted_pattern, out: *mut *mut KbRel) -> kb_status;
+    pub fn kb_bind(ctx: *mut KbCtx, r: *const KbRel, spec: *const kb_bind_spec, out: *mut *mut KbRel, info: *mut kb_bind_info) -> kb_status;
     pub fn kb_star_join(ctx: *mut KbCtx, join_slot: u32, pats: *const KbPattern, n: u32, f: *const KbFilterOp, nf: u32, out: *mut *mut KbRel) -> kb_status;
     pub fn kb_group_aggregate(ctx: *mut KbCtx, r: *const KbRel, group_slots: *const u32, n_group: u32, aggs: *const KbAgg, n_aggs: u32, out: *mut *mut KbGroups) -> kb_status;
     pub fn kb_star_join_aggregate(ctx: *mut KbCtx, join_slot: u32, pats: *const KbPattern, n: u32, f: *const KbFilterOp, nf: u32, group_slots: *const u32, n_group: u32,

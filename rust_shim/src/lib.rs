@@ -1,6 +1,8 @@
 //! kolibrie-gpu-b200 — the three seams through which Kolibrie hands its hot path to libkolibrie_b200.so:
 //!
-//! * [`try_execute`]            for `ExecutionEngine::execute_with_ids` (kolibrie/src/streamertail_optimizer/execution/engine.rs:54)
+//! * [`try_execute`]            for `ExecutionEngine::execute_with_ids` (kolibrie/src/streamertail_optimizer/execution/engine.rs:54);
+//!                              [`try_execute_mut`] also runs `Bind` (engine.rs:144-277) and grows the database's dictionary and
+//!                              quoted-triple store as the reference does
 //! * [`GpuSemiNaiveStrategy`]   for `Reasoner::infer_with_strategy`    (datalog/src/reasoning/materialisation/infer_generic.rs:27-53)
 //! * [`GpuR2R`]                 for the RSP engine's `R2ROperator`      (kolibrie/src/rsp/r2r.rs:17-30), optionally with the
 //!                              Relation-to-Stream operator on the device (`GpuR2R::with_stream_operator`, kolibrie/src/rsp/r2s.rs:37-58)
@@ -284,7 +286,105 @@ fn run(op: &PhysicalOperator, dev: &DeviceStore, db: &SparqlDatabase, slots: &mu
             let sl: Vec<u32> = names.iter().map(|k| slots.of(k)).collect();
             ok(unsafe { kb_rel_from_host(ctx, sl.as_ptr(), sl.len() as u32, ptrs.as_ptr(), content.len() as u64, &mut out) }, out)
         }
-        _ => None,  // Bind, Values, MLPredict, Subquery: the reference's CPU path
+        _ => None,  // Bind (see run_mut), Values, MLPredict, Subquery: the reference's CPU path
+    }
+}
+
+/// `run` plus `Bind` with the built-in functions (engine.rs:144-277) through kb_bind. The plan builder puts every Bind above the join and
+/// filter tree (utils.rs:101-191), so only Projection and Bind are looked at here: a Bind anywhere else, or an operator reading a Bind
+/// output, goes through `run`, which returns None. `bind_out` collects the output slots (KB_ID_NONE there = the variable is unbound).
+fn run_mut(op: &PhysicalOperator, dev: &mut DeviceStore, db: &mut SparqlDatabase, slots: &mut SlotMap, bind_out: &mut Vec<u32>) -> Option<Rel> {
+    let ctx = dev.ctx;
+    let mut out: *mut KbRel = ptr::null_mut();
+    match op {
+        PhysicalOperator::Projection { input, variables } => {
+            let r = run_mut(input, dev, db, slots, bind_out)?;
+            let sl: Vec<u32> = variables.iter().map(|v| slots.of(v)).collect();
+            if unsafe { kb_project(ctx, r.0, sl.as_ptr(), sl.len() as u32, &mut out) } != KB_OK { return None; }
+            Some(Rel(out, ctx))
+        }
+        PhysicalOperator::Bind { input, function_name, arguments, output_variable } => {
+            if db.udfs.contains_key(function_name.as_str()) { return None; }  // a UDF shadows the built-ins (engine.rs:183)
+            let function = match function_name.as_str() {
+                "SUBJECT" => KB_BIND_SUBJECT, "PREDICATE" => KB_BIND_PREDICATE, "OBJECT" => KB_BIND_OBJECT,
+                "isTRIPLE" => KB_BIND_IS_TRIPLE, "TRIPLE" => KB_BIND_TRIPLE, "CONCAT" => KB_BIND_CONCAT,
+                _ => return None,
+            };
+            let r = run_mut(input, dev, db, slots, bind_out)?;
+            let (mut n, mut nc, mut rs) = (0u64, 0u32, [0u32; KB_MAX_COLS]);
+            if unsafe { kb_rel_info(r.0, &mut n, &mut nc, rs.as_mut_ptr()) } != KB_OK { return None; }
+            let column = |slots: &SlotMap, a: &str| slots.slot.get(a.strip_prefix('?').unwrap_or(a)).copied().filter(|s| rs[..nc as usize].contains(s));
+            let mut args: Vec<KbTerm> = Vec::new();
+            let mut consts: Vec<u8> = Vec::new();
+            let mut const_offsets: Vec<u64> = vec![0];
+            match function {
+                KB_BIND_CONCAT => for a in arguments {
+                    match column(slots, a).filter(|_| a.starts_with('?')) {
+                        Some(s) => args.push(KbTerm { is_var: 1, value: s }),
+                        None => {  // a constant: arg.trim_matches('"'); a variable the rows lack contributes ""
+                            args.push(KbTerm { is_var: 0, value: (const_offsets.len() - 1) as u32 });
+                            if !a.starts_with('?') { consts.extend_from_slice(a.trim_matches('"').as_bytes()); }
+                            const_offsets.push(consts.len() as u64);
+                        }
+                    }
+                },
+                KB_BIND_TRIPLE => {
+                    if arguments.len() != 3 { return None; }
+                    // constants are encoded inside the reference's row loop: in argument order, and only when there is a row
+                    let constant: Vec<&str> = arguments.iter().filter(|a| !a.starts_with('?')).map(|a| a.as_str()).collect();
+                    let ids = if n > 0 && !constant.is_empty() {
+                        let (ids, first) = dev.encode_bulk(&constant).ok()?;
+                        let mut dict = db.dictionary.write().unwrap();
+                        for &p in &first { dict.encode(constant[p as usize]); }
+                        ids
+                    } else { vec![0; constant.len()] };
+                    let mut k = 0;
+                    for a in arguments {
+                        if a.starts_with('?') { args.push(KbTerm { is_var: 1, value: column(slots, a)? }); }
+                        else { args.push(KbTerm { is_var: 0, value: ids[k] }); k += 1; }
+                    }
+                }
+                _ => {
+                    if arguments.len() != 1 { return None; }
+                    args.push(KbTerm { is_var: 1, value: column(slots, &arguments[0])? });
+                }
+            }
+            let out_slot = slots.of(output_variable);
+            let next_qt_id = db.quoted_triple_store.read().unwrap().next_qt_id;
+            let spec = KbBindSpec { function, n_args: args.len() as u32, args: args.as_ptr(), n_const: (const_offsets.len() - 1) as u32,
+                                    const_offsets: const_offsets.as_ptr(), const_bytes: consts.as_ptr(), out_slot, next_qt_id };
+            let mut info = KbBindInfo::default();
+            if unsafe { kb_bind(ctx, r.0, &spec, &mut out, &mut info) } != KB_OK { return None; }
+            let res = Rel(out, ctx);
+            // the host takes the device's new entries in the order the device created them (no lookup of its own)
+            if info.dict_new > 0 {
+                let mut offs = vec![0u64; info.dict_new as usize + 1];
+                if unsafe { kb_dict_strings_download(ctx, info.dict_first, info.dict_new, offs.as_mut_ptr(), ptr::null_mut()) } != KB_OK { return None; }
+                let mut bytes = vec![0u8; offs[info.dict_new as usize] as usize];
+                if unsafe { kb_dict_strings_download(ctx, info.dict_first, info.dict_new, offs.as_mut_ptr(), bytes.as_mut_ptr()) } != KB_OK { return None; }
+                let mut dict = db.dictionary.write().unwrap();
+                for k in 0..info.dict_new as usize {
+                    dict.encode(std::str::from_utf8(&bytes[offs[k] as usize..offs[k + 1] as usize]).ok()?);
+                }
+                dev.synced_dict = dict.id_to_string.len();
+            }
+            if info.quoted_new > 0 {
+                let m = info.quoted_new as usize;
+                let (mut s, mut p, mut o) = (vec![0u32; m], vec![0u32; m], vec![0u32; m]);
+                if unsafe { kb_quoted_download(ctx, info.quoted_first, info.quoted_new, s.as_mut_ptr(), p.as_mut_ptr(), o.as_mut_ptr()) } != KB_OK { return None; }
+                let mut qt = db.quoted_triple_store.write().unwrap();
+                for k in 0..m {
+                    let id = info.quoted_first + k as u32;
+                    qt.id_to_components.insert(id, (s[k], p[k], o[k]));
+                    qt.components_to_id.insert((s[k], p[k], o[k]), id);
+                }
+                qt.next_qt_id = info.quoted_first + info.quoted_new;
+                dev.synced_quoted = qt.id_to_components.len();  // the device table holds them: no reload (it would drop the reverse index)
+            }
+            bind_out.push(out_slot);
+            Some(res)
+        }
+        _ => run(op, dev, db, slots),
     }
 }
 
@@ -299,6 +399,27 @@ fn run(op: &PhysicalOperator, dev: &DeviceStore, db: &SparqlDatabase, slots: &mu
 pub fn try_execute(op: &PhysicalOperator, database: &SparqlDatabase, dev: &mut DeviceStore) -> Option<Vec<HashMap<String, u32>>> {
     let res = try_execute_rel(op, database, dev)?;
     download_rows(dev, res.rel.0, &res.names)
+}
+
+/// [`try_execute`] for a plan that may hold `Bind` operators with the built-in functions (engine.rs:144-277): they run on the device
+/// (kb_bind) and the dictionary and quoted-triple store of `database` take the strings and quoted triples the device created, in its
+/// order. A variable a Bind left unbound is not a key of the row, as in the reference. [`try_execute`] keeps returning None for a Bind.
+pub fn try_execute_mut(op: &PhysicalOperator, database: &mut SparqlDatabase, dev: &mut DeviceStore) -> Option<Vec<HashMap<String, u32>>> {
+    dev.sync(database).ok()?;
+    let mut slots = SlotMap::default();
+    let mut bind_out = Vec::new();
+    let rel = run_mut(op, dev, database, &mut slots, &mut bind_out)?;
+    let mut nc = 0u32;
+    let mut rs = [0u32; KB_MAX_COLS];
+    if unsafe { kb_rel_info(rel.0, ptr::null_mut(), &mut nc, rs.as_mut_ptr()) } != KB_OK { return None; }
+    let names: Vec<String> = (0..nc as usize).map(|c| slots.names[rs[c] as usize].clone()).collect();
+    let mut rows = download_rows(dev, rel.0, &names)?;
+    for c in 0..nc as usize {
+        if bind_out.contains(&rs[c]) {
+            for row in rows.iter_mut() { if row.get(&names[c]) == Some(&KB_ID_NONE) { row.remove(&names[c]); } }
+        }
+    }
+    Some(rows)
 }
 
 /// The operator's result on the device, before any download: the relation and the variable name of each of its columns.
