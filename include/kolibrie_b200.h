@@ -211,6 +211,30 @@ KB_API kb_status kb_dict_numeric_load(kb_ctx* ctx, const double* num_or0, const 
  * is_i32[id] = whether it parses. ids >= n_ids are not integers. */
 KB_API kb_status kb_dict_legacy_i32_load(kb_ctx* ctx, const int32_t* val, const uint8_t* is_i32, uint32_t n_ids);
 
+/* The same side tables DERIVED ON THE DEVICE from the device dictionary's strings (kb_dict_strings_load, kb_dict_encode, kb_bind's CONCAT
+ * and isTRIPLE), so a host never parses the dictionary or uploads a table:
+ *   KB_NUMERIC_F64: num_or0 / is_num exactly as kb_dict_numeric_load takes them: Rust `str::parse::<f64>()` — optional sign, then
+ *                   inf / infinity / nan in any case, or digits[.digits] / .digits / digits. with an optional e|E[+-]digits, nothing else;
+ *                   the nearest double, ties to even, for input of any length; "-0" is -0.0 and "-nan" has its sign bit set;
+ *   KB_NUMERIC_I32: val / is_i32 exactly as kb_dict_legacy_i32_load takes them: `str::parse::<i32>()`, [+-]?[0-9]+ within range.
+ * n_ids = the ids the device dictionary holds. For each table in `tables`, ids [first_id, n_ids) are parsed; entries below first_id stay as
+ * they were (a load or an earlier derive); afterwards the table covers exactly n_ids ids. first_id = KB_NUMERIC_APPEND: from the first
+ * id the table does not hold yet (per table). Refused with KB_E_INVALID, tables unchanged: tables 0 or with unknown bits; first_id
+ * greater than the ids a selected table holds (a hole); first_id greater than n_ids. The tables grow with headroom, so an append per
+ * window firing does not reallocate each time. KB_NUMERIC_F64 voids what kb_dict_numeric_load voids: num_version (prepared plans go
+ * stale, typed index columns are rebuilt) and hence the closed-store token only when a rule filter compares numbers; KB_NUMERIC_I32
+ * voids nothing, like kb_dict_legacy_i32_load. No host-to-device bytes; launches and device time count in kb_stats' `other` family.
+ * info (may be NULL): n_ids; n_derived = ids parsed (n_ids - the smallest first id); n_numeric / n_i32 = how many of them parse;
+ * n_slow = how many took the exact slow path (the 128-bit Eisel–Lemire step could not decide them). */
+#define KB_NUMERIC_F64 1u             /* the numeric side table of kb_dict_numeric_load */
+#define KB_NUMERIC_I32 2u             /* the legacy view of kb_dict_legacy_i32_load */
+#define KB_NUMERIC_APPEND 0xFFFFFFFFu /* first_id: from the first id the table does not hold yet */
+typedef struct kb_numeric_info { uint32_t n_ids, n_derived, n_numeric, n_i32, n_slow; } kb_numeric_info;
+KB_API kb_status kb_dict_numeric_derive(kb_ctx* ctx, uint32_t tables, uint32_t first_id, kb_numeric_info* info /* nullable */);
+/* Entries [first, first + n) of the side tables: each non-NULL pointer receives its table's entries (num_or0 / is_num: the f64 table;
+ * val / is_i32: the i32 table). first + n past the entries a requested table holds -> KB_E_INVALID. */
+KB_API kb_status kb_dict_numeric_download(kb_ctx* ctx, uint32_t first, uint32_t n, double* num_or0, uint8_t* is_num, int32_t* val, uint8_t* is_i32);
+
 /* Dictionary strings on the device + result decode: the id -> string step that ends ExecutionEngine::execute
  * (kolibrie/src/streamertail_optimizer/execution/engine.rs:27-51) and Dictionary::decode (shared/src/dictionary.rs:50-52).
  * String i is bytes[offsets[i] .. offsets[i+1]) (UTF-8, no terminator). */

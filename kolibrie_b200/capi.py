@@ -25,6 +25,8 @@ KB_MAX_COLS = 16
 KB_TAG_INFERRED = 0xFFFFFFFFFFFFFFF0
 KB_TERM_QUOTED = 2  # kb_term.is_var of a `<< s p o >>` term (kb_scan_quoted)
 KB_QUOTED_MAX_DEPTH = 16
+NUMERIC_F64, NUMERIC_I32 = 1, 2  # kb_dict_numeric_derive's tables
+NUMERIC_APPEND = 0xFFFFFFFF      # first_id: from the first id the table does not hold yet
 
 # filter opcodes / comparisons / aggregates (mirror the header)
 F_CMP_NUM, F_EQ_ID, F_NE_ID, F_AND, F_OR, F_NOT, F_PUSH_VAR, F_PUSH_CONST, F_ADD, F_SUB, F_MUL, F_DIV, F_TRUTHY, F_IS_TRIPLE, F_CMP_LEGACY = range(1, 16)
@@ -63,6 +65,14 @@ class KbBindInfo(C.Structure):
     """kb_bind_info: rows, rows left unbound, and the new dictionary / quoted-triple ids (first, count)"""
     _fields_ = [("n_rows", C.c_uint64), ("n_unbound", C.c_uint64), ("dict_first", C.c_uint32), ("dict_new", C.c_uint32),
                 ("quoted_first", C.c_uint32), ("quoted_new", C.c_uint32)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
+class KbNumericInfo(C.Structure):
+    """kb_numeric_info: ids of the device dictionary, ids parsed, how many of them are numbers / i32, how many took the slow path"""
+    _fields_ = [("n_ids", C.c_uint32), ("n_derived", C.c_uint32), ("n_numeric", C.c_uint32), ("n_i32", C.c_uint32), ("n_slow", C.c_uint32)]
 
     def as_dict(self):
         return {n: getattr(self, n) for n, _ in self._fields_}
@@ -197,6 +207,8 @@ def lib() -> C.CDLL:
         "kb_dict_encode": (i32, [vp, vp, vp, u64, vp, P(u32), vp]),
         "kb_dict_strings_info": (i32, [vp, P(u32), P(u64)]),
         "kb_dict_legacy_i32_load": (i32, [vp, vp, vp, u32]),
+        "kb_dict_numeric_derive": (i32, [vp, u32, u32, P(KbNumericInfo)]),
+        "kb_dict_numeric_download": (i32, [vp, u32, u32, vp, vp, vp, vp]),
         "kb_rel_decode": (i32, [vp, vp, u32, P(vp)]),
         "kb_strings_info": (i32, [vp, P(u64), P(u64)]),
         "kb_strings_download": (i32, [vp, vp, vp, vp]),
@@ -268,7 +280,7 @@ def lib() -> C.CDLL:
 EXPORTED_SYMBOLS = [
     "kb_version", "kb_ctx_create", "kb_ctx_destroy", "kb_last_error", "kb_set_timing", "kb_get_stats", "kb_synchronize",
     "kb_store_load", "kb_store_load_device", "kb_store_append", "kb_store_append_device", "kb_store_evict", "kb_store_delete", "kb_store_clear", "kb_store_build_index", "kb_set_use_index", "kb_store_size",
-    "kb_store_download", "kb_dict_numeric_load", "kb_dict_legacy_i32_load", "kb_dict_strings_load", "kb_dict_encode", "kb_dict_strings_info", "kb_rel_decode", "kb_strings_info", "kb_strings_download", "kb_strings_free", "kb_quoted_load", "kb_quoted_download", "kb_dict_strings_download", "kb_bind", "kb_rel_info", "kb_rel_download", "kb_rel_device_col", "kb_rel_from_host",
+    "kb_store_download", "kb_dict_numeric_load", "kb_dict_legacy_i32_load", "kb_dict_numeric_derive", "kb_dict_numeric_download", "kb_dict_strings_load", "kb_dict_encode", "kb_dict_strings_info", "kb_rel_decode", "kb_strings_info", "kb_strings_download", "kb_strings_free", "kb_quoted_load", "kb_quoted_download", "kb_dict_strings_download", "kb_bind", "kb_rel_info", "kb_rel_download", "kb_rel_device_col", "kb_rel_from_host",
     "kb_rel_from_device", "kb_rel_free", "kb_scan", "kb_filter", "kb_project", "kb_hash_join", "kb_bind_join", "kb_scan_quoted", "kb_star_join", "kb_bgp_execute",
     "kb_group_aggregate", "kb_groups_info", "kb_groups_keys", "kb_groups_values", "kb_groups_counts", "kb_groups_free", "kb_groups_pack", "kb_groups_merge", "kb_star_join_aggregate",
     "kb_star_join_prepare", "kb_plan_submit", "kb_plan_collect", "kb_plan_info", "kb_plan_free", "kb_plan_peer_scratch_bytes", "kb_plan_attach_peers",
@@ -458,6 +470,22 @@ class Context:
         f = np.ascontiguousarray(is_i32, dtype=np.uint8)
         assert len(v) == len(f)
         self._check(lib().kb_dict_legacy_i32_load(self.h, _ptr(v), _ptr(f), len(v)))
+
+    def dict_numeric_derive(self, tables: int = NUMERIC_F64, first_id: int = 0) -> dict:
+        """kb_dict_numeric_derive: the side tables of the ids [first_id, n_ids) the device dictionary holds, parsed from its strings on the
+        device (NUMERIC_F64: the table of dict_numeric_load, NUMERIC_I32: that of dict_legacy_i32_load; first_id NUMERIC_APPEND: from the
+        first id each table lacks). Returns kb_numeric_info as a dict."""
+        info = KbNumericInfo()
+        self._check(lib().kb_dict_numeric_derive(self.h, tables, first_id, C.byref(info)))
+        return info.as_dict()
+
+    def dict_numeric_download(self, first: int, n: int, f64: bool = True, i32: bool = False):
+        """kb_dict_numeric_download: (num_or0 float64, is_num uint8) and/or (val int32, is_i32 uint8) of ids [first, first + n)"""
+        num, isn = (np.empty(n, np.float64), np.empty(n, np.uint8)) if f64 else (None, None)
+        val, isi = (np.empty(n, np.int32), np.empty(n, np.uint8)) if i32 else (None, None)
+        p = lambda a: _ptr(a) if a is not None and len(a) else None
+        self._check(lib().kb_dict_numeric_download(self.h, first, n, p(num), p(isn), p(val), p(isi)))
+        return (num, isn, val, isi) if f64 and i32 else (num, isn) if f64 else (val, isi)
 
     def dict_strings_load(self, strings: Sequence[str]):
         """kb_dict_strings_load: string i = the term with dictionary id i (Dictionary::id_to_string, dictionary.rs:17-21)"""

@@ -1,0 +1,196 @@
+// kb_numeric.cu — the numeric side tables derived on the device from the device dictionary (kb_dict_numeric_derive): num_or0 / is_num
+// (`str::parse::<f64>()`, read by FILTER comparisons, arithmetic, aggregates and rule filters) and the legacy executor's i32 view
+// (`str::parse::<i32>()`). The strings are in HBM already (kb_dict_strings_load, kb_dict_encode, kb_bind's CONCAT / isTRIPLE), so a
+// table costs one pass over the ids it adds and no host-to-device copy.
+//   K1 numeric_derive_kernel  thread per id: kb_numparse.cuh's parse_f64 / parse_i32 of the id's string. Most terms are IRIs and names,
+//                             rejected on their first byte. An id whose value Eisel–Lemire cannot decide is appended to a list.
+//   K2 numeric_slow_kernel    thread per listed id: slow_f64, the exact decimal conversion (its 788-byte decimal lives in local memory)
+#include "kb_internal.hpp"
+#include "kb_numparse.cuh"
+
+namespace kb {
+
+__device__ const kb_np::Tables d_np_tables = {
+    {
+#include "kb_pow5.inc"
+    },
+    KB_NP_POW10_INIT,
+    KB_NP_IPOW10_INIT,
+};
+
+struct NumDeriveParams {
+    const unsigned long long* off; const unsigned char* bytes;  // the device dictionary
+    u32 lo, n;                                                  // ids [lo, n) are parsed
+    double* num; u8* isnum; u32 first_f;                        // f64 table (null: not derived), written for ids >= first_f
+    int* i32v; u8* isi32; u32 first_i;                          // i32 table (null: not derived), written for ids >= first_i
+    u32* slow;                                                  // ids left to numeric_slow_kernel
+    u32* ctr;                                                   // [0] slow ids, [1] numeric ids, [2] i32 ids
+};
+
+__global__ void __launch_bounds__(256) numeric_derive_kernel(const __grid_constant__ NumDeriveParams P) {
+    u32 n_num = 0, n_i32 = 0;
+    for (u32 id = P.lo + blockIdx.x * blockDim.x + threadIdx.x; id < P.n; id += gridDim.x * blockDim.x) {
+        const unsigned long long a = __ldg(P.off + id);
+        const u64 len = __ldg(P.off + id + 1) - a;
+        const u8* s = P.bytes + a;
+        if (P.num && id >= P.first_f) {
+            u64 bits;
+            const u32 route = kb_np::parse_f64(s, len, &d_np_tables, &bits);
+            if (route == kb_np::NUM_SLOW) P.slow[atomicAdd(P.ctr, 1u)] = id;  // (num_or0[id] is written by K2)
+            else P.num[id] = __longlong_as_double((long long)bits);
+            P.isnum[id] = route != kb_np::NUM_REJECT;
+            n_num += route != kb_np::NUM_REJECT;
+        }
+        if (P.i32v && id >= P.first_i) {
+            int v;
+            const bool ok = kb_np::parse_i32(s, len, &v);
+            P.i32v[id] = v;
+            P.isi32[id] = ok;
+            n_i32 += ok;
+        }
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        n_num += __shfl_down_sync(0xffffffffu, n_num, o);
+        n_i32 += __shfl_down_sync(0xffffffffu, n_i32, o);
+    }
+    if ((threadIdx.x & 31) == 0) {
+        if (n_num) atomicAdd(P.ctr + 1, n_num);
+        if (n_i32) atomicAdd(P.ctr + 2, n_i32);
+    }
+}
+
+__global__ void __launch_bounds__(128) numeric_slow_kernel(const unsigned long long* __restrict__ off, const unsigned char* __restrict__ bytes,
+                                                           const u32* __restrict__ slow, u32 n_slow, double* __restrict__ num) {
+    kb_np::Decimal dec;
+    for (u32 k = blockIdx.x * blockDim.x + threadIdx.x; k < n_slow; k += gridDim.x * blockDim.x) {
+        const u32 id = slow[k];
+        const unsigned long long a = off[id];
+        num[id] = __longlong_as_double((long long)kb_np::slow_f64(bytes + a, off[id + 1] - a, &dec));
+    }
+}
+
+// a table of `n` entries of elem_a + elem_b bytes that keeps its first `keep` entries: in place when the buffers hold n, else in new
+// buffers with headroom (an append per window firing must not reallocate and copy each time)
+static kb_status numeric_grow(kb_ctx* ctx, Buf* a, Buf* b, size_t elem_a, u32 keep, u32 n) {
+    if (*a && *b && (*a)->bytes >= (size_t)n * elem_a && (*b)->bytes >= (size_t)n) return KB_OK;
+    const size_t cap = (size_t)n + n / 2 + 1024;
+    Buf na, nb;
+    KB_TRY(alloc_buf(ctx, cap * elem_a, &na));
+    KB_TRY(alloc_buf(ctx, cap, &nb));
+    if (keep) {
+        KB_CUDA(ctx, cudaMemcpyAsync(na->p, (*a)->p, (size_t)keep * elem_a, cudaMemcpyDeviceToDevice, ctx->st));
+        KB_CUDA(ctx, cudaMemcpyAsync(nb->p, (*b)->p, (size_t)keep, cudaMemcpyDeviceToDevice, ctx->st));
+    }
+    *a = na;
+    *b = nb;
+    return KB_OK;
+}
+
+static int grid_for(u64 n, int n_sms, int threads, int per_sm) {
+    const u64 want = (n + threads - 1) / threads;
+    return (int)std::max<u64>(1, std::min<u64>(want, (u64)n_sms * per_sm));
+}
+
+}  // namespace kb
+
+using namespace kb;
+
+namespace {
+struct DevGuard {  // the calling thread's current device is restored on return
+    int prev = -1;
+    explicit DevGuard(int dev) {
+        cudaGetDevice(&prev);
+        if (prev != dev) cudaSetDevice(dev);
+        else prev = -1;
+    }
+    ~DevGuard() {
+        if (prev >= 0) cudaSetDevice(prev);
+    }
+};
+}  // namespace
+#define KB_ENTER(ctx)                                         \
+    if (!(ctx)) return KB_E_INVALID;                          \
+    DevGuard _guard((ctx)->device);                           \
+    KB_TRY(kb::begin_call(ctx))
+
+extern "C" {
+
+kb_status kb_dict_numeric_derive(kb_ctx* ctx, uint32_t tables, uint32_t first_id, kb_numeric_info* info) {
+    KB_ENTER(ctx);
+    if (info) *info = kb_numeric_info{};
+    if (tables == 0 || (tables & ~(KB_NUMERIC_F64 | KB_NUMERIC_I32)))
+        return fail(ctx, KB_E_INVALID, "tables must be a non-empty combination of KB_NUMERIC_F64 and KB_NUMERIC_I32 (got 0x%x)", tables);
+    const bool F = tables & KB_NUMERIC_F64, I = tables & KB_NUMERIC_I32;
+    const u32 n = ctx->dict_ids;
+    const u32 first_f = first_id == KB_NUMERIC_APPEND ? ctx->n_ids : first_id;
+    const u32 first_i = first_id == KB_NUMERIC_APPEND ? ctx->n_i32 : first_id;
+    if (F && first_f > ctx->n_ids) return fail(ctx, KB_E_INVALID, "first_id %u would leave a hole: the f64 table holds %u ids", first_f, ctx->n_ids);
+    if (I && first_i > ctx->n_i32) return fail(ctx, KB_E_INVALID, "first_id %u would leave a hole: the i32 table holds %u ids", first_i, ctx->n_i32);
+    if ((F && first_f > n) || (I && first_i > n)) return fail(ctx, KB_E_INVALID, "first_id is past the %u ids of the device dictionary", n);
+    // checked: nothing changes before this point
+    if (F) KB_TRY(numeric_grow(ctx, &ctx->num, &ctx->isnum, sizeof(double), first_f, n));
+    if (I) KB_TRY(numeric_grow(ctx, &ctx->i32val, &ctx->isi32, sizeof(int32_t), first_i, n));
+    const u32 lo = F && I ? std::min(first_f, first_i) : F ? first_f : first_i;
+    u32 n_slow = 0, n_num = 0, n_i32 = 0;
+    if (lo < n) {
+        Buf slow;
+        KB_TRY(alloc_buf(ctx, (size_t)(F ? n - first_f : 1) * sizeof(u32) + 16, &slow));
+        const u32 c = ctrl_alloc(ctx, 4);
+        KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + c, 0, 4 * sizeof(u32), ctx->st));
+        NumDeriveParams P{};
+        P.off = static_cast<const unsigned long long*>(ctx->dict_off->p);
+        P.bytes = static_cast<const unsigned char*>(ctx->dict_bytes->p);
+        P.lo = lo;
+        P.n = n;
+        if (F) { P.num = static_cast<double*>(ctx->num->p); P.isnum = static_cast<u8*>(ctx->isnum->p); P.first_f = first_f; }
+        if (I) { P.i32v = static_cast<int*>(ctx->i32val->p); P.isi32 = static_cast<u8*>(ctx->isi32->p); P.first_i = first_i; }
+        P.slow = static_cast<u32*>(slow->p);
+        P.ctr = ctx->ctrl + c;
+        timer_begin(ctx, F_OTHER, 1);
+        numeric_derive_kernel<<<grid_for(n - lo, ctx->n_sms, 256, 8), 256, 0, ctx->st>>>(P);
+        timer_end(ctx);
+        KB_CUDA(ctx, cudaGetLastError());
+        KB_TRY(ctrl_read(ctx));
+        n_slow = ctx->h_ctrl[c];
+        n_num = ctx->h_ctrl[c + 1];
+        n_i32 = ctx->h_ctrl[c + 2];
+        if (n_slow) {
+            timer_begin(ctx, F_OTHER, 1);
+            numeric_slow_kernel<<<grid_for(n_slow, ctx->n_sms, 128, 4), 128, 0, ctx->st>>>(P.off, P.bytes, P.slow, n_slow, P.num);
+            timer_end(ctx);
+            KB_CUDA(ctx, cudaGetLastError());
+        }
+        KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));  // (`slow` is released with the stream order anyway; the counts are final here)
+        timers_flush(ctx);
+    }
+    if (F) {
+        ctx->n_ids = n;
+        ctx->num_version++;  // typed index columns and prepared plans read the table: as after kb_dict_numeric_load
+    }
+    if (I) ctx->n_i32 = n;
+    if (info) {
+        info->n_ids = n;
+        info->n_derived = n - lo;
+        info->n_numeric = n_num;
+        info->n_i32 = n_i32;
+        info->n_slow = n_slow;
+    }
+    return KB_OK;
+}
+
+kb_status kb_dict_numeric_download(kb_ctx* ctx, uint32_t first, uint32_t n, double* num_or0, uint8_t* is_num, int32_t* val, uint8_t* is_i32) {
+    KB_ENTER(ctx);
+    if (n == 0) return KB_OK;
+    if ((num_or0 || is_num) && (u64)first + n > ctx->n_ids) return fail(ctx, KB_E_INVALID, "ids [%u, %u + %u) are past the f64 table's %u", first, first, n, ctx->n_ids);
+    if ((val || is_i32) && (u64)first + n > ctx->n_i32) return fail(ctx, KB_E_INVALID, "ids [%u, %u + %u) are past the i32 table's %u", first, first, n, ctx->n_i32);
+    size_t bytes = 0;
+    if (num_or0) { KB_CUDA(ctx, cudaMemcpyAsync(num_or0, static_cast<const double*>(ctx->num->p) + first, (size_t)n * 8, cudaMemcpyDeviceToHost, ctx->st)); bytes += (size_t)n * 8; }
+    if (is_num) { KB_CUDA(ctx, cudaMemcpyAsync(is_num, static_cast<const u8*>(ctx->isnum->p) + first, n, cudaMemcpyDeviceToHost, ctx->st)); bytes += n; }
+    if (val) { KB_CUDA(ctx, cudaMemcpyAsync(val, static_cast<const int32_t*>(ctx->i32val->p) + first, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->st)); bytes += (size_t)n * 4; }
+    if (is_i32) { KB_CUDA(ctx, cudaMemcpyAsync(is_i32, static_cast<const u8*>(ctx->isi32->p) + first, n, cudaMemcpyDeviceToHost, ctx->st)); bytes += n; }
+    KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
+    ctx->stats.d2h_bytes += bytes;
+    return KB_OK;
+}
+
+}  // extern "C"

@@ -85,6 +85,33 @@ class Dictionary:
         return num, isn
 
 
+def _push_new_strings(ctx, dictionary: Dictionary, synced: int) -> bool:
+    """the device dictionary takes the host strings it lacks. When it still holds the `synced` strings this mirror put there, only
+    id_to_string[synced:] go up (kb_dict_encode, which must hand them the ids synced.. in order); otherwise, or when the ids differ, the
+    whole dictionary is reloaded. Returns True when the device kept its earlier strings (a numeric table over them stays valid)."""
+    n = len(dictionary.id_to_string)
+    n_dev, _ = ctx.dict_strings_info()
+    if synced >= 0 and n_dev == synced <= n:
+        if n == synced:
+            return True
+        ids, _ = ctx.dict_encode(dictionary.id_to_string[synced:])
+        if np.array_equal(ids, np.arange(synced, n, dtype=np.uint32)):
+            return True
+    ctx.dict_strings_load(dictionary.id_to_string)
+    return False
+
+
+def _derive_numeric(ctx, first_id: int = c.NUMERIC_APPEND):
+    """kb_dict_numeric_derive of the f64 table from first_id (default: the ids it lacks); a table the call cannot extend (it holds more
+    ids than the device dictionary: another dictionary's) is derived whole"""
+    try:
+        ctx.dict_numeric_derive(c.NUMERIC_F64, first_id)
+    except c.KolibrieError as e:
+        if e.status != c.KB_E_INVALID or first_id == 0:
+            raise
+        ctx.dict_numeric_derive(c.NUMERIC_F64, 0)
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 @dataclass(frozen=True)
 class Variable:
@@ -439,9 +466,13 @@ class SparqlDatabase:
             return
         arr = np.array(sorted(self.triples), dtype=np.uint32).reshape(-1, 3)  # (s,p,o) order: the reference's BTreeSet iteration
         self.ctx.store_load(arr[:, 0], arr[:, 1], arr[:, 2])
-        num, isn = self.dictionary.numeric_table()
-        self.ctx.dict_numeric_load(num, isn)
-        self.ctx.dict_strings_load(self.dictionary.id_to_string)  # the final id -> string step runs on the device too
+        if hasattr(self.ctx, "dict_numeric_derive"):  # the numeric side table parsed on the device from the strings
+            self.ctx.dict_strings_load(self.dictionary.id_to_string)  # the final id -> string step runs on the device too
+            self.ctx.dict_numeric_derive(c.NUMERIC_F64, 0)
+        else:
+            num, isn = self.dictionary.numeric_table()
+            self.ctx.dict_numeric_load(num, isn)
+            self.ctx.dict_strings_load(self.dictionary.id_to_string)
         self._uploaded_version = self._version
 
     def _sync_quoted(self):
@@ -613,14 +644,15 @@ class ExecutionEngine:
             db.ctx.dict_strings_load(db.dictionary.id_to_string)  # the final decode reads the new strings on the device
         db._sync_quoted()
         cols[out_name] = col
-        ExecutionEngine._mark_bind(slots, out_slot, op.function_name, bool((col == c.KB_ID_NONE).any()))
+        ExecutionEngine._mark_bind(slots, out_slot, op.function_name, bool((col == c.KB_ID_NONE).any()), False)
         names = list(cols)
         return db.ctx.rel_from_host([slots.of(k) for k in names], [cols[k] for k in names])
 
     @staticmethod
-    def _mark_bind(slots: SlotMap, out_slot: int, function_name: str, has_unbound: bool):
+    def _mark_bind(slots: SlotMap, out_slot: int, function_name: str, has_unbound: bool, derived: bool):
+        """derived: the numeric side table covers the strings the BIND created (kb_dict_numeric_derive ran after it)"""
         slots.bind_out.add(out_slot)
-        if has_unbound or function_name in ("CONCAT", "isTRIPLE"):
+        if has_unbound or (function_name in ("CONCAT", "isTRIPLE") and not derived):
             slots.bind_only.add(out_slot)
         else:
             slots.bind_only.discard(out_slot)
@@ -661,7 +693,8 @@ class ExecutionEngine:
                 raise c.KolibrieError(c.KB_E_UNSUPPORTED, f"{op.function_name} takes 1 argument")
             args = [var(op.arguments[0])]
         n_dev, _ = ctx.dict_strings_info()
-        if n_dev != len(db.dictionary.id_to_string):
+        reloaded = n_dev != len(db.dictionary.id_to_string)
+        if reloaded:
             ctx.dict_strings_load(db.dictionary.id_to_string)
         out_slot = slots.of(_strip(op.output_variable))
         qts = db.quoted_triple_store
@@ -679,7 +712,10 @@ class ExecutionEngine:
                 qts.components_to_id[key] = first + k
             qts.next_qt_id = first + info["quoted_new"]
             db._uploaded_quoted = len(qts)  # the device table holds them already: no reload (it would drop the reverse index)
-        ExecutionEngine._mark_bind(slots, out_slot, op.function_name, info["n_unbound"] > 0)
+        derived = hasattr(ctx, "dict_numeric_derive")
+        if derived and (info["dict_new"] or reloaded):  # the numeric side table learns the strings CONCAT / isTRIPLE created, on the device
+            _derive_numeric(ctx, 0 if reloaded else c.NUMERIC_APPEND)
+        ExecutionEngine._mark_bind(slots, out_slot, op.function_name, info["n_unbound"] > 0, derived)
         return res
 
     @staticmethod
@@ -812,6 +848,7 @@ class Reasoner:
         self.last_stats = None
         self._n_in_store: Optional[int] = None  # facts of self._facts the device store holds, once a fixpoint has closed it
         self._closed_rules = -1                 # len(self.rules) at that fixpoint
+        self._strings_ids = -1                  # dictionary strings this reasoner put on the device
 
     def add_abox_triple(self, subject: str, predicate: str, obj: str):
         t = (self.dictionary.encode(subject), self.dictionary.encode(predicate), self.dictionary.encode(obj))
@@ -830,8 +867,18 @@ class Reasoner:
             self._dirty = False
             if self._n_in_store is not None and self._n_in_store != len(self._facts):
                 self._n_in_store = None  # the reloaded store holds triples no fixpoint has seen: it is not a closed store plus a seed
-        num, isn = self.dictionary.numeric_table()
-        self.ctx.dict_numeric_load(num, isn)
+        self._load_numeric()
+
+    def _load_numeric(self):
+        """the numeric side table the rule filters read: on the device, the strings added since the last call go up and the table is
+        extended over their ids (kb_dict_numeric_derive); the host loop for contexts without it"""
+        if hasattr(self.ctx, "dict_numeric_derive"):
+            kept = _push_new_strings(self.ctx, self.dictionary, self._strings_ids)
+            self._strings_ids = len(self.dictionary.id_to_string)
+            _derive_numeric(self.ctx, c.NUMERIC_APPEND if kept else 0)
+        else:
+            num, isn = self.dictionary.numeric_table()
+            self.ctx.dict_numeric_load(num, isn)
 
     def _infer(self, strategy: int) -> List[Tuple[int, int, int]]:
         self._sync()
@@ -855,8 +902,7 @@ class Reasoner:
         rules = [compile_rule(r) for r in self.rules]
         rule_preds = {int(x.p.value) for r in rules for x in list(r["premise"]) + list(r["conclusion"]) if not x.p.is_var}
         added = np.array(self._facts[self._n_in_store:], dtype=np.uint32).reshape(-1, 3)
-        num, isn = self.dictionary.numeric_table()
-        self.ctx.dict_numeric_load(num, isn)
+        self._load_numeric()
         in_rules = np.isin(added[:, 1], np.fromiter(rule_preds, np.uint32, len(rule_preds))) if len(added) else np.zeros(0, bool)
         other = added[~in_rules]
         if len(other):  # predicates no rule mentions: plain store rows
@@ -980,14 +1026,25 @@ class SimpleR2R:
     def _load_tables(self):
         """the dictionary's numeric and string tables on the device when it grew (FILTERs of rules and queries read the first; loading
         it voids the closed token only when a rule filter compares numbers)"""
-        n = len(self.item.dictionary.id_to_string)
-        if n != self._numeric_ids:
-            num, isn = self.item.dictionary.numeric_table()
-            self.ctx.dict_numeric_load(num, isn)
-            self._numeric_ids = n
+        d = self.item.dictionary
+        n = len(d.id_to_string)
+        if not hasattr(self.ctx, "dict_numeric_derive"):
+            if n != self._numeric_ids:
+                num, isn = d.numeric_table()
+                self.ctx.dict_numeric_load(num, isn)
+                self._numeric_ids = n
+            if n != self._strings_ids:
+                self.ctx.dict_strings_load(d.id_to_string)
+                self._strings_ids = n
+            return
+        # incremental: a firing uploads the strings it added and the device parses them (host work and bytes ~ the slide, not the dictionary)
+        kept = True
         if n != self._strings_ids:
-            self.ctx.dict_strings_load(self.item.dictionary.id_to_string)
+            kept = _push_new_strings(self.ctx, d, self._strings_ids)
             self._strings_ids = n
+        if n != self._numeric_ids:
+            _derive_numeric(self.ctx, c.NUMERIC_APPEND if kept and self._numeric_ids >= 0 else 0)
+            self._numeric_ids = n
 
     def materialize(self) -> List[Tuple[int, int, int]]:
         """the closure of the current window's triples beyond them (simple_r2r.rs:103-128), sorted"""
@@ -1111,7 +1168,12 @@ class LegacyExecutor:
         db = self.db
         db._sync()
         n = len(db.dictionary.id_to_string)
-        if n != self._i32_loaded and hasattr(db.ctx, "dict_legacy_i32_load"):
+        if n != self._i32_loaded and hasattr(db.ctx, "dict_numeric_derive"):  # parsed on the device from the dictionary's strings
+            if db.ctx.dict_strings_info()[0] != n:
+                db.ctx.dict_strings_load(db.dictionary.id_to_string)
+            db.ctx.dict_numeric_derive(c.NUMERIC_I32, 0)
+            self._i32_loaded = n
+        elif n != self._i32_loaded and hasattr(db.ctx, "dict_legacy_i32_load"):
             val = np.zeros(n, dtype=np.int32)
             isi = np.zeros(n, dtype=np.uint8)
             for i, st in enumerate(db.dictionary.id_to_string):

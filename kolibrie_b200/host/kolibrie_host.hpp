@@ -229,9 +229,17 @@ class Reasoner {
             dev_->check(kb_store_load(dev_->get(), s.data(), p.data(), o.data(), s.size()));
             dirty_ = false;
         }
-        std::vector<double> num; std::vector<uint8_t> isn;
-        dictionary.numeric_table(&num, &isn);
-        dev_->check(kb_dict_numeric_load(dev_->get(), num.data(), isn.data(), (uint32_t)num.size()));
+        // the numeric side table the rule filters read, parsed on the device from the dictionary's strings (uploaded when the device
+        // dictionary does not hold as many)
+        uint32_t n_dev = 0;
+        dev_->check(kb_dict_strings_info(dev_->get(), &n_dev, nullptr));
+        if (n_dev != dictionary.id_to_string.size()) {
+            std::vector<uint64_t> off(dictionary.id_to_string.size() + 1, 0);
+            std::string bytes;
+            for (size_t i = 0; i < dictionary.id_to_string.size(); i++) { bytes += dictionary.id_to_string[i]; off[i + 1] = bytes.size(); }
+            dev_->check(kb_dict_strings_load(dev_->get(), off.data(), reinterpret_cast<const uint8_t*>(bytes.data()), (uint32_t)dictionary.id_to_string.size()));
+        }
+        dev_->check(kb_dict_numeric_derive(dev_->get(), KB_NUMERIC_F64, 0, nullptr));
     }
     std::vector<Triple> infer(uint32_t strategy) {
         sync();
@@ -338,14 +346,10 @@ class SparqlDatabase {
         std::vector<uint32_t> s, p, o;
         for (auto& t : triples) { s.push_back(t.subject); p.push_back(t.predicate); o.push_back(t.object); }
         dev_->check(kb_store_load(dev_->get(), s.data(), p.data(), o.data(), s.size()));
-        std::vector<double> num; std::vector<uint8_t> isn;
-        dictionary.numeric_table(&num, &isn);
-        dev_->check(kb_dict_numeric_load(dev_->get(), num.data(), isn.data(), (uint32_t)num.size()));
-        // the strings themselves: the final id -> string step of execute() runs on the device (kb_rel_decode)
-        std::vector<uint64_t> off(dictionary.id_to_string.size() + 1, 0);
-        std::string bytes;
-        for (size_t i = 0; i < dictionary.id_to_string.size(); i++) { bytes += dictionary.id_to_string[i]; off[i + 1] = bytes.size(); }
-        dev_->check(kb_dict_strings_load(dev_->get(), off.data(), reinterpret_cast<const uint8_t*>(bytes.data()), (uint32_t)dictionary.id_to_string.size()));
+        // the strings themselves: the final id -> string step of execute() runs on the device (kb_rel_decode), and the numeric side
+        // table is parsed from them there (kb_dict_numeric_derive)
+        upload_strings();
+        dev_->check(kb_dict_numeric_derive(dev_->get(), KB_NUMERIC_F64, 0, nullptr));
         uploaded_ = version_;
     }
     const Device& device() const { return *dev_; }

@@ -44,6 +44,10 @@ pub type kb_bind_info = KbBindInfo;
 pub const KB_BIND_SUBJECT: u32 = 1; pub const KB_BIND_PREDICATE: u32 = 2; pub const KB_BIND_OBJECT: u32 = 3; pub const KB_BIND_IS_TRIPLE: u32 = 4;
 pub const KB_BIND_TRIPLE: u32 = 5; pub const KB_BIND_CONCAT: u32 = 6;
 pub const KB_BIND_MAX_ARGS: u32 = 16;
+// kb_dict_numeric_derive: the side tables derived on the device from the device dictionary's strings
+pub const KB_NUMERIC_F64: u32 = 1; pub const KB_NUMERIC_I32: u32 = 2; pub const KB_NUMERIC_APPEND: u32 = 0xFFFF_FFFF;
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbNumericInfo { pub n_ids: u32, pub n_derived: u32, pub n_numeric: u32, pub n_i32: u32, pub n_slow: u32 }
+pub type kb_numeric_info = KbNumericInfo;  // (the header's name, as the declaration below spells it)
 
 // kb_filter_opcode / kb_cmp / kb_agg_kind / kb_strategy
 pub const KB_F_CMP_NUM: u32 = 1; pub const KB_F_EQ_ID: u32 = 2; pub const KB_F_NE_ID: u32 = 3; pub const KB_F_AND: u32 = 4; pub const KB_F_OR: u32 = 5;
@@ -75,6 +79,8 @@ extern "C" {
     pub fn kb_store_size(ctx: *mut KbCtx, n_triples: *mut u64, n_segments: *mut u32) -> kb_status;
     pub fn kb_dict_numeric_load(ctx: *mut KbCtx, num_or0: *const c_double, is_num: *const u8, n_ids: u32) -> kb_status;
     pub fn kb_dict_strings_load(ctx: *mut KbCtx, offsets: *const u64, bytes: *const u8, n_ids: u32) -> kb_status;
+    pub fn kb_dict_numeric_derive(ctx: *mut KbCtx, tables: u32, first_id: u32, info: *mut kb_numeric_info) -> kb_status;
+    pub fn kb_dict_numeric_download(ctx: *mut KbCtx, first: u32, n: u32, num_or0: *mut c_double, is_num: *mut u8, val: *mut i32, is_i32: *mut u8) -> kb_status;
     pub fn kb_dict_encode(ctx: *mut KbCtx, offsets: *const u64, bytes: *const u8, n_terms: u64, out_ids: *mut u32, n_new: *mut u32, new_first_pos: *mut u64) -> kb_status;
     pub fn kb_dict_strings_info(ctx: *mut KbCtx, n_ids: *mut u32, n_bytes: *mut u64) -> kb_status;
     pub fn kb_store_append_device(ctx: *mut KbCtx, d_s: *const u32, d_p: *const u32, d_o: *const u32, n: u64, tag: u64) -> kb_status;

@@ -60,17 +60,13 @@ impl DeviceStore {
         let dict = database.dictionary.read().unwrap();
         if dict.id_to_string.len() != self.synced_dict {
             let n = dict.id_to_string.len();
-            let mut num = vec![0f64; n];
-            let mut isn = vec![0u8; n];
-            for (i, s) in dict.id_to_string.iter().enumerate() {
-                if let Ok(v) = s.parse::<f64>() { num[i] = v; isn[i] = 1; }  // types.rs:133-148 / 163-167
-            }
-            if unsafe { kb_dict_numeric_load(self.ctx, num.as_ptr(), isn.as_ptr(), n as u32) } != KB_OK { return Err(self.last_error()); }
             let mut offs = Vec::with_capacity(n + 1);
             let mut bytes = Vec::new();
             offs.push(0u64);
             for s in dict.id_to_string.iter() { bytes.extend_from_slice(s.as_bytes()); offs.push(bytes.len() as u64); }
             if unsafe { kb_dict_strings_load(self.ctx, offs.as_ptr(), bytes.as_ptr(), n as u32) } != KB_OK { return Err(self.last_error()); }
+            // the numeric side table (`s.parse::<f64>()`, types.rs:133-148 / 163-167) parsed on the device from those strings
+            if unsafe { kb_dict_numeric_derive(self.ctx, KB_NUMERIC_F64, 0, ptr::null_mut()) } != KB_OK { return Err(self.last_error()); }
             self.synced_dict = n;
         }
         // the quoted-triple table (kb_quoted_load) when the store's size changed; an empty store clears it (n = 0), so that a table
