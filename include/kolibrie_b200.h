@@ -357,6 +357,25 @@ KB_API kb_status kb_project(kb_ctx* ctx, const kb_rel* in, const uint32_t* slots
 /* OptimizedHashJoin / HashJoin / merge join / NestedLoopJoin (engine.rs:710-837, 970-1039): natural join on the
  * common slots; no common slot -> cartesian product (engine.rs:1054-1071, limited to 2^28 output rows). */
 KB_API kb_status kb_hash_join(kb_ctx* ctx, const kb_rel* left, const kb_rel* right, kb_rel** out);
+/* The join of SPARQL mappings over rows that may leave variables unbound: natural_join (rsp_engine.rs:684-718), which the RSP engine's
+ * emit step uses to join the latest results of several windows and the static data (rsp_engine.rs:647-681), on ids. The dictionary is
+ * shared by every window and the static store (rsp_engine.rs:215-243), so the reference's string equality is id equality. A cell holding
+ * KB_ID_NONE means "this row does not bind this variable" (what kb_bind leaves unbound).
+ *   Columns. The union of both slot sets: `left`'s slots in order, then the slots of `right` that `left` lacks.
+ *   Rows. A (left, right) row pair is emitted iff every shared slot bound in BOTH rows holds equal ids. The merged cell holds the right
+ *     value when it is bound, else the left one (`merged.insert` overwrites, rsp_engine.rs:708-711; where both are bound they are equal),
+ *     so a slot unbound on both sides stays KB_ID_NONE.
+ *   A bag: every compatible pair once, so duplicates multiply. Row order is unspecified. Either side empty -> 0 rows (:688-690).
+ *   No shared slot -> the cartesian product, limited to 2^28 rows as in kb_hash_join.
+ * Routes. A check pass reads the shared columns of both sides (launch and time in kb_stats' `other` family).
+ *   - No shared column holds KB_ID_NONE: exactly kb_hash_join (its launches, its limits: at most 4 shared slots).
+ *   - Otherwise U = the shared slots holding KB_ID_NONE on at least one side. Each side is partitioned by its rows' bound-masks over U
+ *     (two more `other` launches), and every pair of non-empty mask groups (mL, mR) is joined as kb_hash_join joins, on the key (shared
+ *     slots outside U) ∪ (U ∩ mL ∩ mR) — an empty key is the cartesian product of the two groups, limited to 2^28 rows per pair. The
+ *     output is then written from the pairs' row indices (one coalesce launch per non-empty pair, timed together in `other`).
+ * Refused before any output exists (*out untouched): |U| > 4 (more than 256 mask pairs), a join key of more than 4 slots, more than
+ * KB_MAX_COLS output columns, a relation of 2^32 rows or more, an output of 2^32 rows or more (KB_E_LIMIT). */
+KB_API kb_status kb_natural_join(kb_ctx* ctx, const kb_rel* left, const kb_rel* right, kb_rel** out);
 /* BindJoin of a relation with ONE store pattern (engine.rs:840-885): natural join of `left` with the pattern's matches. With a valid store
  * index, the pattern (?x P ?y) and exactly one of its variables bound by `left` through a unique dense column of the predicate, it is
  * one probe kernel against the index's persistent table (the reference's spo[x][P] / pos[P][y] lookups); otherwise scan + hash join. */

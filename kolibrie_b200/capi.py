@@ -227,6 +227,7 @@ def lib() -> C.CDLL:
         "kb_filter": (i32, [vp, vp, P(KbFilterOp), u32, P(vp)]),
         "kb_project": (i32, [vp, vp, P(u32), u32, P(vp)]),
         "kb_hash_join": (i32, [vp, vp, vp, P(vp)]),
+        "kb_natural_join": (i32, [vp, vp, vp, P(vp)]),
         "kb_bind_join": (i32, [vp, vp, P(KbPattern), P(vp)]),
         "kb_scan_quoted": (i32, [vp, P(KbQuotedPattern), P(vp)]),
         "kb_star_join": (i32, [vp, u32, P(KbPattern), u32, P(KbFilterOp), u32, P(vp)]),
@@ -281,7 +282,7 @@ EXPORTED_SYMBOLS = [
     "kb_version", "kb_ctx_create", "kb_ctx_destroy", "kb_last_error", "kb_set_timing", "kb_get_stats", "kb_synchronize",
     "kb_store_load", "kb_store_load_device", "kb_store_append", "kb_store_append_device", "kb_store_evict", "kb_store_delete", "kb_store_clear", "kb_store_build_index", "kb_set_use_index", "kb_store_size",
     "kb_store_download", "kb_dict_numeric_load", "kb_dict_legacy_i32_load", "kb_dict_numeric_derive", "kb_dict_numeric_download", "kb_dict_strings_load", "kb_dict_encode", "kb_dict_strings_info", "kb_rel_decode", "kb_strings_info", "kb_strings_download", "kb_strings_free", "kb_quoted_load", "kb_quoted_download", "kb_dict_strings_download", "kb_bind", "kb_rel_info", "kb_rel_download", "kb_rel_device_col", "kb_rel_from_host",
-    "kb_rel_from_device", "kb_rel_free", "kb_scan", "kb_filter", "kb_project", "kb_hash_join", "kb_bind_join", "kb_scan_quoted", "kb_star_join", "kb_bgp_execute",
+    "kb_rel_from_device", "kb_rel_free", "kb_scan", "kb_filter", "kb_project", "kb_hash_join", "kb_natural_join", "kb_bind_join", "kb_scan_quoted", "kb_star_join", "kb_bgp_execute",
     "kb_group_aggregate", "kb_groups_info", "kb_groups_keys", "kb_groups_values", "kb_groups_counts", "kb_groups_free", "kb_groups_pack", "kb_groups_merge", "kb_star_join_aggregate",
     "kb_star_join_prepare", "kb_plan_submit", "kb_plan_collect", "kb_plan_info", "kb_plan_free", "kb_plan_peer_scratch_bytes", "kb_plan_attach_peers",
     "kb_datalog_fixpoint", "kb_datalog_fixpoint_seed", "kb_datalog_maintain", "kb_r2s_create", "kb_r2s_eval", "kb_r2s_info", "kb_r2s_free", "kb_shard_of", "kb_set_sharding", "kb_partition", "kb_partition_counts", "kb_segment_write", "kb_segment_info", "kb_segment_save", "kb_store_append_file", "kb_shuffle_scatter", "kb_shuffle_push", "kb_rel_wrap_device", "kb_star_join_host", "kb_star_join_host_into", "perform_hash_join_cuda",
@@ -593,6 +594,13 @@ class Context:
     def hash_join(self, left: Relation, right: Relation) -> Relation:
         out = C.c_void_p()
         self._check(lib().kb_hash_join(self.h, left.h, right.h, C.byref(out)))
+        return Relation(self, out)
+
+    def natural_join(self, left: Relation, right: Relation) -> Relation:
+        """kb_natural_join: the join of mappings (rsp_engine.rs:684-718) — a KB_ID_NONE cell is an unbound variable, compatible with
+        any value; the merged cell is the right value if bound, else the left one"""
+        out = C.c_void_p()
+        self._check(lib().kb_natural_join(self.h, left.h, right.h, C.byref(out)))
         return Relation(self, out)
 
     def bind_join(self, left: Relation, pat: KbPattern) -> Relation:

@@ -102,7 +102,7 @@ kb_status ctrl_read(kb_ctx* ctx) {
 }
 
 kb_status ensure_tile_state(kb_ctx* ctx, u64 tiles) {
-    if (tiles <= ctx->tile_state_tiles) return KB_OK;
+    if (ctx->tile_state && tiles <= ctx->tile_state_tiles) return KB_OK;  // (a scan of a store never loaded asks for 0 tiles: still allocate)
     u64 want = std::max<u64>(tiles, 1024) * 2;
     Buf b, b2;
     KB_TRY(alloc_buf(ctx, want * MAXP * sizeof(u64), &b));

@@ -1095,11 +1095,12 @@ class SimpleR2R:
         self._device_ready()
         return ExecutionEngine.execute(op, self.item)
 
-    def execute_query_rel(self, op) -> c.Relation:
+    def execute_query_rel(self, op, slots: Optional[SlotMap] = None) -> c.Relation:
         """execute_query without the download and the decode: the firing's result as a device relation, what
-        Relation2StreamOperator.eval takes. `slot_names[s]` is the name of the variable in slot s (the same for every firing of op)."""
+        Relation2StreamOperator.eval takes. `slot_names[s]` is the name of the variable in slot s (the same for every firing of op).
+        `slots`: a map shared with other plans (every window plan and the static plan of one WindowJoin), else a fresh one."""
         self._device_ready()
-        slots = SlotMap()
+        slots = slots if slots is not None else SlotMap()
         rel = ExecutionEngine._run(op, self.item, slots)
         self.slot_names = list(slots.names)
         return rel
@@ -1132,6 +1133,166 @@ class Relation2StreamOperator:
         if self._op is not None:
             self._op.free()
             self._op = None
+
+
+class WindowJoin:
+    """The emit step of a query over several windows, or over windows and static data (rsp_engine.rs:647-681), on device relations:
+    the latest result of every window is natural-joined (kb_natural_join) in the order `windows` lists them — the join is commutative and
+    associative on bags, so the order does not change the answer —, then joined with the static plan's result, then passed through
+    Relation2StreamOperator and decoded. Around it, the two emit rules of the reference:
+      * single thread (process_single_thread_window_results, rsp_engine.rs:549-593): put() queues results, process_single_thread()
+        drains them; it emits once every window has a result, then Wait and Timeout clear the results and Steal keeps them;
+      * coordinator (rsp_engine.rs:387-508) without its thread: receive(batch, now) is a result plus those that arrived with it, tick(now)
+        the deadline of Timeout{Steal, Drop} expiring. The clock is the caller's (seconds).
+    policy: "wait", "steal" or ("timeout", seconds, "steal" | "drop").
+
+    Every window plan and the static plan must run through `slots` (one SlotMap), so that a variable has one slot everywhere. The static
+    data lives in its own SparqlDatabase on a second context of the same device, sharing the windows' Dictionary object
+    (rsp_engine.rs:238-243): static triples are invisible to window queries. Its result is copied device to device into the window
+    context and kept while the static store and the dictionary are unchanged (the reference recomputes it per emit; the answer is the same).
+    An emitted row is its bound variables as (name, value) pairs sorted by name; a variable left unbound (KB_ID_NONE) is not in it."""
+
+    def __init__(self, ctx: c.Context, windows: Sequence[str], slots: SlotMap, stream_operator: Union[int, str] = c.RSTREAM, policy="wait",
+                 static_db: Optional[SparqlDatabase] = None, static_plan=None):
+        self.ctx, self.windows, self.slots, self.policy = ctx, list(windows), slots, policy
+        self.r2s = Relation2StreamOperator(ctx, stream_operator)
+        self.static_db, self.static_plan = static_db, static_plan
+        self.last: Dict[str, c.Relation] = {}
+        self._pending: List[Tuple[str, c.Relation, int]] = []
+        self._static: Optional[c.Relation] = None
+        self._static_key = None
+        self._triggered: set = set()
+        self._cycle_start: Optional[float] = None
+        self._max_ts = 0
+
+    def _store(self, window_iri: str, rel: c.Relation):
+        if window_iri not in self.windows:
+            raise ValueError(f"unknown window {window_iri}")
+        old = self.last.get(window_iri)
+        self.last[window_iri] = rel
+        if old is not None and old is not rel:
+            old.free()
+
+    def _clear(self):
+        for r in self.last.values():
+            r.free()
+        self.last = {}
+
+    def put(self, window_iri: str, rel: c.Relation, ts: int):
+        """a window's firing result (single thread): queued until process_single_thread(); it then replaces (and frees) the window's
+        previous result"""
+        self._pending.append((window_iri, rel, ts))
+
+    def process_single_thread(self) -> Optional[List[List[Tuple[str, str]]]]:
+        """rsp_engine.rs:549-593: the emitted rows, or None when nothing was emitted"""
+        if not self._pending:
+            return None
+        max_ts = 0
+        for iri, rel, ts in self._pending:
+            max_ts = max(max_ts, ts)
+            self._store(iri, rel)
+        self._pending = []
+        if len(self.last) != len(self.windows):
+            return None
+        rows = self.emit(max_ts)
+        if self.policy != "steal":  # Wait, and Timeout (no wall clock in a single thread)
+            self._clear()
+        return rows
+
+    def _reset_cycle(self):
+        self._triggered.clear()
+        self._cycle_start = None
+        self._max_ts = 0
+
+    def tick(self, now: float) -> List[List[List[Tuple[str, str]]]]:
+        """Timeout's deadline (rsp_engine.rs:421-440): past it, Steal emits with what it has and Drop discards the cycle"""
+        out = []
+        if not isinstance(self.policy, tuple) or self._cycle_start is None or now - self._cycle_start < self.policy[1]:
+            return out
+        if self._triggered:
+            if self.policy[2] == "steal" and len(self.last) == len(self.windows):
+                out.append(self.emit(self._max_ts))
+            self._reset_cycle()
+        return out
+
+    def receive(self, batch: Sequence[Tuple[str, c.Relation, int]], now: float) -> List[List[List[Tuple[str, str]]]]:
+        """rsp_engine.rs:450-503: batch[0] is the result received, the rest arrived with it; returns the emits (a deadline that passed
+        before `now` fires first)"""
+        out = self.tick(now)
+        for k, (iri, rel, ts) in enumerate(batch):
+            self._max_ts = max(self._max_ts, ts)
+            self._store(iri, rel)
+            if k == 0 and not self._triggered:
+                self._cycle_start = now
+            self._triggered.add(iri)
+        if len(self._triggered) == len(self.windows):
+            out.append(self.emit(self._max_ts))
+            self._reset_cycle()
+        elif self.policy == "steal":
+            if len(self.last) == len(self.windows):
+                out.append(self.emit(self._max_ts))
+            self._reset_cycle()
+        return out
+
+    def static_relation(self) -> Optional[c.Relation]:
+        """the static plan's result in the window context, recomputed when the static store or the dictionary changed"""
+        if self.static_plan is None:
+            return None
+        db = self.static_db
+        key = (db._version, len(db.dictionary.id_to_string))
+        if self._static is None or self._static_key != key:
+            db._sync()
+            rel = ExecutionEngine._run(self.static_plan, db, self.slots)
+            db.ctx.synchronize()  # the copy below runs on the window context's stream
+            n, rslots = rel.info()
+            copy = self.ctx.rel_from_device(rslots, [rel.device_ptr(i) for i in range(len(rslots))], n)
+            self.ctx.synchronize()  # the source's columns go back to the static context's pool: the copy must have read them
+            rel.free()
+            if self._static is not None:
+                self._static.free()
+            self._static, self._static_key = copy, key
+        return self._static
+
+    def join(self) -> c.Relation:
+        """the natural join of every window's latest result and the static result (kb_natural_join), before R2S"""
+        joined = None
+        for iri in self.windows:
+            rel = self.last[iri]
+            nxt = rel if joined is None else self.ctx.natural_join(joined, rel)
+            if joined is not None and joined is not self.last[self.windows[0]]:
+                joined.free()
+            joined = nxt
+        static = self.static_relation()
+        if static is not None:
+            nxt = self.ctx.natural_join(joined, static)
+            if joined is not self.last[self.windows[0]]:
+                joined.free()
+            joined = nxt
+        return joined
+
+    def emit(self, ts: int = 0) -> List[List[Tuple[str, str]]]:
+        """emit_results (rsp_engine.rs:647-681): join, R2S, decode"""
+        joined = self.join()
+        emitted = self.r2s.eval(joined, ts)
+        if joined is not self.last[self.windows[0]]:
+            joined.free()
+        n, rslots = emitted.info()
+        names = [self.slots.names[s] for s in rslots]
+        ids = [emitted.column(j) for j in range(len(rslots))]
+        vals = [emitted.decode_strings(j) if n else [] for j in range(len(rslots))]
+        emitted.free()
+        order = sorted(range(len(rslots)), key=lambda j: names[j])
+        return [[(names[j], vals[j][i]) for j in order if ids[j][i] != c.KB_ID_NONE] for i in range(n)]
+
+    def free(self):
+        self._clear()
+        for _, rel, _ in self._pending:
+            rel.free()
+        self._pending = []
+        if self._static is not None:
+            self._static.free()
+            self._static = None
+        self.r2s.free()
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -103,6 +103,8 @@ extern "C" {
     pub fn kb_filter(ctx: *mut KbCtx, r: *const KbRel, prog: *const KbFilterOp, n: u32, out: *mut *mut KbRel) -> kb_status;
     pub fn kb_project(ctx: *mut KbCtx, r: *const KbRel, slots: *const u32, n: u32, out: *mut *mut KbRel) -> kb_status;
     pub fn kb_hash_join(ctx: *mut KbCtx, l: *const KbRel, r: *const KbRel, out: *mut *mut KbRel) -> kb_status;
+    // natural_join of the RSP emit step: rows may leave shared variables unbound (KB_ID_NONE)
+    pub fn kb_natural_join(ctx: *mut KbCtx, l: *const KbRel, r: *const KbRel, out: *mut *mut KbRel) -> kb_status;
     pub fn kb_bind_join(ctx: *mut KbCtx, l: *const KbRel, pattern: *const KbPattern, out: *mut *mut KbRel) -> kb_status;
     pub fn kb_scan_quoted(ctx: *mut KbCtx, qp: *const kb_quoted_pattern, out: *mut *mut KbRel) -> kb_status;
     pub fn kb_bind(ctx: *mut KbCtx, r: *const KbRel, spec: *const kb_bind_spec, out: *mut *mut KbRel, info: *mut kb_bind_info) -> kb_status;
