@@ -7,6 +7,7 @@
 #include <mutex>
 
 #include "kb_internal.hpp"
+#include "kb_numrank.cuh"
 
 using namespace kb;
 
@@ -1177,14 +1178,19 @@ static kb_status resolve_index_plan(kb_ctx* ctx, const StarQuery& q, const Index
     for (size_t i = 0; i < fops.size(); i++) P.ops[i] = fops[i];
     // table mode: the probe pattern's own subject table is the probe stream (keys ascending whatever the store / id order)
     const bool tab_mode = ctx->probe_table_mode && !ctx->ordered && ix.persistent[pk] && q.key_pos[pk] == 0 &&
-                          (P.pre_mode != 1u || (PS.xnum && PS.xnum_version == ctx->num_version));
+                          (P.pre_mode != 1u || (PS.xkey && PS.xkey_version == ctx->num_version && ctx->numv_version == ctx->num_version));
     if (tab_mode) {
         // walk the slots that can hold a key (smallest to largest live subject), not the table's growth headroom nor the
         // slots an evicted past has left empty; the first slot stays 128-byte aligned for the bulk loads
         const u32 lo = ((compact_key(PS.xmin, PS.tab_cshift) - PS.xtab_min) / 32u) * 32u;
         const u32 hi = std::min<u32>(PS.xtab_range, compact_key(PS.xmax, PS.tab_cshift) - PS.xtab_min + 1u);
         P.ptab = static_cast<const u32*>(PS.xtab->p) + lo;
-        P.pnum = P.pre_mode == 1u ? static_cast<const double*>(PS.xnum->p) + lo : nullptr;
+        if (P.pre_mode == 1u) {  // FILTER(?o <cmp> c) on the value becomes a range of its ranks in the value order
+            P.pkey = static_cast<const u32*>(PS.xkey->p) + lo;
+            const kb_nr::Range r = kb_nr::cmp_range(P.pre_cmp, ctx->h_numv.data(), (u32)ctx->h_numv.size(), P.pre_val);
+            P.key_lo = r.lo;
+            P.key_hi = r.hi;
+        }
         P.ptab_min = PS.xtab_min + lo;
         P.ptab_range = hi > lo ? hi - lo : 0u;
         P.ptab_cshift = PS.tab_cshift;
@@ -1848,6 +1854,7 @@ void kb_ctx_destroy(kb_ctx* ctx) {
     ctx->index.clear();
     ctx->num.reset();
     ctx->isnum.reset();
+    ctx->numv.reset();
     ctx->i32val.reset();
     ctx->isi32.reset();
     ctx->dict_off.reset();
@@ -2023,6 +2030,23 @@ kb_status kb_set_use_index(kb_ctx* ctx, int enabled) {
 
 // ---- store index, one chunk per (predicate, store segment)
 namespace kb {
+// the rank column of a slice's subject table: xkey[compact(subject) - xtab_min] = rank of the object's value in the value order (slots
+// without a key are never read: they stay unset)
+static kb_status build_rank_column(kb_ctx* ctx, PredSlice& ps) {
+    bool ok = false;
+    KB_TRY(ensure_num_order(ctx, &ok));
+    if (!ok) return KB_OK;
+    KB_TRY(alloc_buf(ctx, (size_t)ps.xtab_range * sizeof(u32), &ps.xkey));
+    for (auto& ch : ps.chunks) {
+        if (!ch.n) continue;
+        launch_pair_ranktab(reinterpret_cast<const uint2*>(ch.pairs.ptr), (u32)ch.n, numtab(ctx), static_cast<const double*>(ctx->numv->p),
+                            (u32)ctx->h_numv.size(), static_cast<u32*>(ps.xkey->p), ps.xtab_min, ps.xtab_range, ps.tab_cshift, ctx->n_sms, ctx->st);
+        ctx->stats.kernel_launches++;
+    }
+    ps.xkey_version = ctx->num_version;
+    return KB_OK;
+}
+
 // (re)build or extend the persistent table of one column of a slice after `added` (index into ps.chunks; -1: all chunks) arrived.
 // flag_word: control word the insert kernels raise on a duplicate key. Returns through *touched whether a flag has to be read.
 static kb_status slice_table_update(kb_ctx* ctx, PredSlice& ps, u32 y, int added, u32 cshift, u32 flag_off, bool* touched) {
@@ -2040,7 +2064,7 @@ static kb_status slice_table_update(kb_ctx* ctx, PredSlice& ps, u32 y, int added
     if (!fits) {
         // (re)build over every chunk, with headroom above the largest key: dictionary ids grow, so appended segments bring larger ones
         tab.reset();
-        if (!y) ps.xnum.reset();
+        if (!y) ps.xkey.reset();
         tried = true;
         unique = false;
         if (range > std::max<u64>(4 * ps.n + 65536, 1ull << 16) || range > (1ull << 28)) return KB_OK;  // not dense: keep no table
@@ -2064,17 +2088,8 @@ static kb_status slice_table_update(kb_ctx* ctx, PredSlice& ps, u32 y, int added
         ctx->stats.kernel_launches++;
         *touched = true;
     }
-    // a subject table rebuilt outside the full build takes its typed column along (the table-mode probe filters on it)
-    if (!y && !fits && !ctx->in_full_index_build && ctx->n_ids && ps.typed(ctx->num_version)) {
-        KB_TRY(alloc_buf(ctx, (size_t)tcap * sizeof(double), &ps.xnum));
-        KB_CUDA(ctx, cudaMemsetAsync(ps.xnum->p, 0, (size_t)tcap * sizeof(double), ctx->st));
-        for (auto& ch : ps.chunks) {
-            if (!ch.n) continue;
-            launch_pair_numtab(reinterpret_cast<const uint2*>(ch.pairs.ptr), (u32)ch.n, numtab(ctx), static_cast<double*>(ps.xnum->p), tmin, tcap, cs, ctx->n_sms, ctx->st);
-            ctx->stats.kernel_launches++;
-        }
-        ps.xnum_version = ctx->num_version;
-    }
+    // a subject table rebuilt outside the full build takes its rank column along (the table-mode probe filters on it)
+    if (!y && !fits && !ctx->in_full_index_build && ctx->n_ids && ps.typed(ctx->num_version)) KB_TRY(build_rank_column(ctx, ps));
     return KB_OK;
 }
 
@@ -2109,8 +2124,11 @@ static kb_status index_add_segment_split(kb_ctx* ctx, const Segment& sg, u32 csh
         rebuild[i][0] = ps.xtab ? !xok : !ps.x_tried;
         rebuild[i][1] = !ps.ytab && !ps.y_tried;
         if (xok) { e.xtab = static_cast<u32*>(ps.xtab->p); e.xtab_min = ps.xtab_min; e.xtab_range = ps.xtab_range; e.cshift = cshift; }
-        if (xok && ps.xnum && ps.xnum_version == ctx->num_version && ctx->n_ids) e.xnum = static_cast<double*>(ps.xnum->p);
-        else ps.xnum.reset();
+        if (xok && ps.xkey && ps.xkey_version == ctx->num_version && ctx->numv_version == ctx->num_version && ctx->n_ids) {
+            e.xkey = static_cast<u32*>(ps.xkey->p);
+            P.numv = static_cast<const double*>(ctx->numv->p);
+            P.n_numv = (u32)ctx->h_numv.size();
+        } else ps.xkey.reset();
         if (ps.ytab) { e.ytab = static_cast<u32*>(ps.ytab->p); e.ytab_min = ps.ytab_min; e.ytab_range = ps.ytab_range; }
     }
     timer_begin(ctx, F_OTHER);
@@ -2131,14 +2149,14 @@ static kb_status index_add_segment_split(kb_ctx* ctx, const Segment& sg, u32 csh
                                                   h[SPLIT_CURSOR], (unsigned long long)ch.n);
         ch.xmin = ~h[SPLIT_XMIN]; ch.ymin = ~h[SPLIT_YMIN]; ch.xmax = h[SPLIT_XMAX]; ch.ymax = h[SPLIT_YMAX];
         if (ch.ynum && h[SPLIT_NNUM] > 0) ch.ynum_version = ctx->num_version;
-        else { ch.ynum.reset(); ps.xnum.reset(); }
+        else { ch.ynum.reset(); ps.xkey.reset(); }
         ps.xmin = std::min(ps.xmin, ch.xmin); ps.ymin = std::min(ps.ymin, ch.ymin);
         ps.xmax = std::max(ps.xmax, ch.xmax); ps.ymax = std::max(ps.ymax, ch.ymax);
         chunk_of[i] = (int)ps.chunks.size();
         ps.chunks.push_back(ch);
         ps.n += ch.n;
         if (ps.chunks.size() > 1) { ps.xoff.reset(); ps.xval.reset(); ps.yoff.reset(); ps.yval.reset(); }  // the directories describe one chunk
-        if (h[SPLIT_XDUP]) { ps.x_unique = false; ps.xtab.reset(); ps.xnum.reset(); }  // a subject occurs twice
+        if (h[SPLIT_XDUP]) { ps.x_unique = false; ps.xtab.reset(); ps.xkey.reset(); }  // a subject occurs twice
         if (h[SPLIT_YDUP]) { ps.y_unique = false; ps.ytab.reset(); }
         if (h[SPLIT_XOUT] && ps.xtab) rebuild[i][0] = true;  // a key outside the table: rebuild it over every chunk, with new headroom
         if (h[SPLIT_YOUT] && ps.ytab) rebuild[i][1] = true;
@@ -2246,7 +2264,7 @@ kb_status index_add_segment(kb_ctx* ctx, size_t seg_idx, bool* indexable) {
             ps.chunks.push_back(ch);
             ps.n += ch.n;
             if (ps.chunks.size() > 1) { ps.xoff.reset(); ps.xval.reset(); ps.yoff.reset(); ps.yval.reset(); }  // the directories describe one chunk
-            if (!ctx->in_full_index_build) ps.xnum.reset();  // (kept in table order by the full build only)
+            if (!ctx->in_full_index_build) ps.xkey.reset();  // (kept in table order by the full build only)
         }
         KB_CUDA(ctx, cudaGetLastError());
         KB_TRY(ctrl_read(ctx));
@@ -2323,7 +2341,7 @@ kb_status index_evict_tag(kb_ctx* ctx, u64 tag) {
             ps.n -= ch.n;
             dying.push_back(ch);
             ps.chunks.erase(ps.chunks.begin() + c);
-            ps.xoff.reset(); ps.xval.reset(); ps.yoff.reset(); ps.yval.reset();  // (xnum stays: its slots are only read where xtab holds a key)
+            ps.xoff.reset(); ps.xval.reset(); ps.yoff.reset(); ps.yval.reset();  // (xkey stays: its slots are only read where xtab holds a key)
         }
         if (hit) {  // the slice's id ranges shrink to the surviving chunks': a long-running window does not walk its whole past
             ps.xmin = ps.ymin = 0xFFFFFFFFu;
@@ -2365,18 +2383,11 @@ kb_status kb_store_build_index(kb_ctx* ctx, uint32_t* n_predicates, double* buil
             return KB_OK;  // too many predicates: keep scanning (n_predicates = 0)
         }
     }
-    // typed values in table order for subject tables whose slice is numeric: the table-mode probe reads FILTER operands sequentially
+    // value ranks in table order for subject tables whose slice is numeric: the table-mode probe reads FILTER operands sequentially
     for (auto& kv : ctx->index) {
         kb::PredSlice& ps = kv.second;
         if (!ps.xtab || !ctx->n_ids || !ps.typed(ctx->num_version)) continue;
-        KB_TRY(kb::alloc_buf(ctx, (size_t)ps.xtab_range * sizeof(double), &ps.xnum));
-        KB_CUDA(ctx, cudaMemsetAsync(ps.xnum->p, 0, (size_t)ps.xtab_range * sizeof(double), ctx->st));
-        for (auto& ch : ps.chunks) {
-            kb::launch_pair_numtab(reinterpret_cast<const uint2*>(ch.pairs.ptr), (u32)ch.n, kb::numtab(ctx), static_cast<double*>(ps.xnum->p), ps.xtab_min, ps.xtab_range,
-                                   ps.tab_cshift, ctx->n_sms, ctx->st);
-            ctx->stats.kernel_launches++;
-        }
-        ps.xnum_version = ctx->num_version;
+        KB_TRY(kb::build_rank_column(ctx, ps));
     }
     // key-grouped directories (counting sort by the dense key) for the columns that did not get a direct table
     for (auto& kv : ctx->index) {

@@ -149,8 +149,9 @@ struct PredSlice {  // one predicate's (subject, object) rows of the store — t
     // slice sorted by that column — a counting sort, the ids being dense — as off[key - min .. ] + the other half in key order. What the
     // reference's spo[s][P] -> {o} and pos[P][o] -> {s} sets are (index_manager.rs:18-26, 253-340): a bound subject / object is a range
     // of val, not a scan. Built by kb_store_build_index for single-chunk slices; dropped when the predicate's slice is appended to.
-    Buf xnum;                // typed values in TABLE order: xnum[compact(subject) - xtab_min] = num_or0[object] (built with xtab by kb_store_build_index
-    u64 xnum_version = 0;    // when the slice has numeric objects; the table-mode probe filters on it sequentially)
+    Buf xkey;                // value ranks in TABLE order: xkey[compact(subject) - xtab_min] = rank of num_or0[object] in the context's value
+    u64 xkey_version = 0;    // order (kb_numrank.cuh; built with xtab by kb_store_build_index when the slice has numeric objects; the
+                             // table-mode probe filters on it sequentially, 4 bytes a slot)
     Buf xoff, xval, yoff, yval;
     u32 xcsr_min = 0, xcsr_range = 0, ycsr_min = 0, ycsr_range = 0;
     const SliceChunk* single() const { return chunks.size() == 1 ? &chunks[0] : nullptr; }
@@ -187,6 +188,12 @@ struct kb_ctx {
     kb::u32 quoted_rev_indexed = 0;  // table indices [0, quoted_rev_indexed) are in it
     kb::u32 n_ids = 0;
     kb::u64 num_version = 1;  // bumped by kb_dict_numeric_load: typed literal columns of the index are tied to it
+    // value order of the numeric side table (kb_numrank.cuh: sorted distinct non-NaN values, -0.0 folded, 0.0 included), on the device
+    // and on the host (a FILTER constant becomes a rank range there); built with the index's rank columns, valid while numv_version ==
+    // num_version
+    kb::Buf numv;
+    std::vector<double> h_numv;
+    kb::u64 numv_version = 0;
     // tile-state buffer of the look-back prefix (never cleared: words carry the launch epoch)
     kb::Buf tile_state, block_state;
     size_t tile_state_tiles = 0;
@@ -276,6 +283,9 @@ u32 ctrl_alloc(kb_ctx* ctx, u32 words);                 // returns word offset i
 kb_status ctrl_read(kb_ctx* ctx);                       // D2H of the used part of the arena + stream sync
 kb_status ensure_tile_state(kb_ctx* ctx, u64 tiles);
 NumTab numtab(const kb_ctx* ctx);
+// ctx->numv / h_numv for the current num_version (a device sort of the side table; one read-back). *ok = false: no value order (the
+// table holds 2^31 ids or more), the index keeps no rank columns
+kb_status ensure_num_order(kb_ctx* ctx, bool* ok);
 void timer_begin(kb_ctx* ctx, int fam, int n_kernels = 1);
 void timer_end(kb_ctx* ctx);
 void timers_flush(kb_ctx* ctx);  // after a stream sync

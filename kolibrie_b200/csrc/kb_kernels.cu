@@ -3,6 +3,7 @@
 // mbarrier), matches are compacted with warp ballots, and output positions come from a single-pass decoupled look-back
 // prefix over tiles, so every kernel reads its input exactly once and writes a deterministic, input-ordered output.
 #include "kb_kernels.cuh"
+#include "kb_numrank.cuh"
 
 #include <math_constants.h>
 #include <cmath>
@@ -838,6 +839,13 @@ __global__ void __launch_bounds__(256) segment_split_kernel(const __grid_constan
 #pragma unroll
             for (u32 e = 0; e < MAXP; e++) if (e < P.k && P.e[e].pred == vp && i < P.n) which[j] = e;
         }
+        u32 xk[SPLIT_ITEMS];  // value ranks for the rank columns (xkey): the SPLIT_ITEMS searches in V run side by side
+        if (P.n_numv) {
+            double xv[SPLIT_ITEMS];
+#pragma unroll
+            for (u32 j = 0; j < SPLIT_ITEMS; j++) xv[j] = which[j] != EMPTY32 && P.e[which[j]].xkey ? kb_nr::fold(num_of(P.nt, vo[j])) : 0.0;
+            kb_nr::rank_of_n<SPLIT_ITEMS>(P.numv, P.n_numv, xv, xk);
+        }
 #pragma unroll
         for (u32 j = 0; j < SPLIT_ITEMS; j++) {
             const unsigned act = __ballot_sync(0xffffffffu, which[j] != EMPTY32);
@@ -879,7 +887,7 @@ __global__ void __launch_bounds__(256) segment_split_kernel(const __grid_constan
                 const u32 off = compact_key(vs[j], E.cshift) - E.xtab_min;
                 if (off < E.xtab_range) {
                     if (atomicExch(&E.xtab[off], vo[j]) != EMPTY32) s_flag[w][0] = 1u;
-                    if (E.xnum) E.xnum[off] = num_of(P.nt, vo[j]);
+                    if (E.xkey) E.xkey[off] = xk[j];
                 } else s_flag[w][2] = 1u;
             }
             if (E.ytab) {
@@ -958,18 +966,50 @@ __global__ void __launch_bounds__(256) pair_numcol_kernel(const uint2* __restric
     c = warp_sum(c);
     if ((threadIdx.x & 31) == 0 && c) atomicAdd(n_numeric, c);
 }
-__global__ void __launch_bounds__(256) pair_numtab_kernel(const uint2* __restrict__ kv, u32 n, NumTab nt, double* __restrict__ out, u32 kmin, u32 range, u32 cshift) {
-    const u32 stride = gridDim.x * blockDim.x;
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-        const uint2 v = kv[i];
-        const u32 off = compact_key(v.x, cshift) - kmin;
-        if (off < range) out[off] = num_of(nt, v.y);
+// RANKTAB_ITEMS rows per thread (striped over the CTA's chunk): their searches in V run side by side
+constexpr u32 RANKTAB_ITEMS = 4;
+__global__ void __launch_bounds__(256) pair_ranktab_kernel(const uint2* __restrict__ kv, u32 n, NumTab nt, const double* __restrict__ numv, u32 n_numv,
+                                                          u32* __restrict__ out, u32 kmin, u32 range, u32 cshift) {
+    for (u32 row0 = blockIdx.x * 256u * RANKTAB_ITEMS; row0 < n; row0 += gridDim.x * 256u * RANKTAB_ITEMS) {
+        double x[RANKTAB_ITEMS];
+        u32 off[RANKTAB_ITEMS], r[RANKTAB_ITEMS];
+#pragma unroll
+        for (u32 j = 0; j < RANKTAB_ITEMS; j++) {
+            const u32 i = row0 + j * 256u + threadIdx.x;
+            off[j] = EMPTY32;
+            x[j] = 0.0;
+            if (i < n) {
+                const uint2 v = kv[i];
+                off[j] = compact_key(v.x, cshift) - kmin;
+                x[j] = kb_nr::fold(num_of(nt, v.y));
+            }
+        }
+        kb_nr::rank_of_n<RANKTAB_ITEMS>(numv, n_numv, x, r);
+#pragma unroll
+        for (u32 j = 0; j < RANKTAB_ITEMS; j++) if (off[j] < range) out[off[j]] = r[j];
     }
 }
-void launch_pair_numtab(const uint2* kv, u32 n, NumTab nt, double* out, u32 kmin, u32 range, u32 cshift, int n_sms, cudaStream_t st) {
+void launch_pair_ranktab(const uint2* kv, u32 n, NumTab nt, const double* numv, u32 n_numv, u32* out, u32 kmin, u32 range, u32 cshift, int n_sms,
+                         cudaStream_t st) {
+    if (n == 0) return;
+    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 256ull * RANKTAB_ITEMS - 1ull) / (256ull * RANKTAB_ITEMS));
+    pair_ranktab_kernel<<<grid, 256, 0, st>>>(kv, n, nt, numv, n_numv, out, kmin, range, cshift);
+}
+// the value order's keys (kb_numrank.cuh: order_key / order_value); id n is the extra 0.0
+__global__ void __launch_bounds__(256) numorder_keys_kernel(const double* __restrict__ num, u32 n, unsigned long long* __restrict__ keys) {
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += (u64)gridDim.x * blockDim.x) keys[i] = kb_nr::order_key(i < n ? num[i] : 0.0);
+}
+__global__ void __launch_bounds__(256) numorder_values_kernel(const unsigned long long* __restrict__ keys, u32 n, double* __restrict__ out) {
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = kb_nr::order_value(keys[i]);
+}
+void launch_numorder_keys(const double* num_or0, u32 n, unsigned long long* keys, int n_sms, cudaStream_t st) {
+    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 256ull) / 256ull);
+    numorder_keys_kernel<<<grid, 256, 0, st>>>(num_or0, n, keys);
+}
+void launch_numorder_values(const unsigned long long* keys, u32 n, double* out, int n_sms, cudaStream_t st) {
     if (n == 0) return;
     const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull);
-    pair_numtab_kernel<<<grid, 256, 0, st>>>(kv, n, nt, out, kmin, range, cshift);
+    numorder_values_kernel<<<grid, 256, 0, st>>>(keys, n, out);
 }
 void launch_pair_numcol(const uint2* kv, u32 n, NumTab nt, double* out, u32* n_numeric, int n_sms, cudaStream_t st) {
     if (n == 0) return;
@@ -1271,13 +1311,13 @@ __device__ void atomic_max_f64(double* addr, double v);
 // other half of the triple whose key is (table base + i), EMPTY32 where no triple has that key. The keys then come in ascending order
 // whatever the order of the store and of the dictionary ids, so the lookups into the other patterns' tables are sequential too — a
 // direct table over dense ids IS the slice sorted by that column (with the gaps of the id space). With a FILTER on the other half's
-// numeric value the typed column is read from a second table in the same order.
+// numeric value the 4-byte value ranks are read from a second table in the same order (kb_numrank.cuh: the FILTER is a rank range).
 template <int T, int PRE, bool AGG, bool TAB>
 __global__ void __launch_bounds__(PROBEF_THREADS, KB_PI_MINB) probe_index_kernel(const __grid_constant__ ProbeIParams P, const __grid_constant__ GroupParams G) {
     constexpr int R = 4;  // rows per thread (striped over the warp's 128-row chunk, see below)
     constexpr u32 TILE = PROBEF_THREADS * R;
     extern __shared__ __align__(128) u32 smem_all[];  // per stage: TILE pairs [+ TILE doubles]
-    constexpr u32 STAGE_WORDS = TAB ? (PRE == 1 ? 3u : 1u) * TILE : (PRE == 1 ? 4u : 2u) * TILE;  // TAB: TILE values [+ TILE doubles]
+    constexpr u32 STAGE_WORDS = TAB ? (PRE == 1 ? 2u : 1u) * TILE : (PRE == 1 ? 4u : 2u) * TILE;  // TAB: TILE values [+ TILE ranks]
     __shared__ __align__(8) u64 bars[2];
     __shared__ u32 s_nexts[2];
     __shared__ u32 s_wcnt[PROBEF_THREADS / 32];
@@ -1303,9 +1343,9 @@ __global__ void __launch_bounds__(PROBEF_THREADS, KB_PI_MINB) probe_index_kernel
             const u32 c = min(TILE, P.ptab_range - b);
             const u32 bytes = (c * 4u + 15u) & ~15u;
             s_tcnt[stage] = c;
-            mbar_arrive_expect_tx(&bar, PRE == 1 ? 3u * bytes : bytes);
+            mbar_arrive_expect_tx(&bar, PRE == 1 ? 2u * bytes : bytes);
             tma_load_1d(smem, P.ptab + b, bytes, &bar);
-            if (PRE == 1) tma_load_1d(smem + TILE, P.pnum + b, 2u * bytes, &bar);
+            if (PRE == 1) tma_load_1d(smem + TILE, P.pkey + b, bytes, &bar);
             return;
         }
         u32 g = 0;  // the chunk (store segment) this tile belongs to
@@ -1340,7 +1380,8 @@ __global__ void __launch_bounds__(PROBEF_THREADS, KB_PI_MINB) probe_index_kernel
         mbar_wait(&bars[stage], (it >> 1) & 1u);
         const u32 cnt = s_tcnt[stage];
         u32 rx[R], ry[R];
-        double pa[R];
+        double pa[R];  // PRE == 1: the FILTER operand (slice mode: the f64 value, table mode: its rank in pk)
+        u32 pk[R];
         // striped: row j of this thread is row (warp*128 + j*32 + lane) of the tile, so one warp instruction touches 32 CONSECUTIVE
         // rows: lookups into a table indexed by a sorted key hit 4 sectors instead of 16, and the compacted stores of one j are
         // one contiguous run
@@ -1355,7 +1396,7 @@ __global__ void __launch_bounds__(PROBEF_THREADS, KB_PI_MINB) probe_index_kernel
                 const u32 key = P.ptab_cshift ? (((((ck >> SHARD_B) << P.ptab_cshift) | P.shard_rank) << SHARD_B) | (ck & ((1u << SHARD_B) - 1u))) : ck;
                 rx[j] = P.key_is_y ? v : key;
                 ry[j] = P.key_is_y ? key : v;
-                if (PRE == 1) pa[j] = reinterpret_cast<const double*>(smem + TILE)[idx];
+                if (PRE == 1) pk[j] = smem[TILE + idx];
                 vmask |= ((idx < cnt && v != EMPTY32) ? 1u : 0u) << j;
             }
         } else {
@@ -1372,7 +1413,12 @@ __global__ void __launch_bounds__(PROBEF_THREADS, KB_PI_MINB) probe_index_kernel
         if (PRE == 1) {
             u32 pass = 0;
 #pragma unroll
-            for (int j = 0; j < R; j++) pass |= (cmp_num(P.pre_cmp, pa[j], P.pre_val) ? 1u : 0u) << j;
+            for (int j = 0; j < R; j++) {
+                bool ok;
+                if constexpr (TAB) ok = kb_nr::in_range(pk[j], P.key_lo, P.key_hi);
+                else ok = cmp_num(P.pre_cmp, pa[j], P.pre_val);
+                pass |= (ok ? 1u : 0u) << j;
+            }
             vmask &= pass;
         } else if (P.pre_mode == 2u && vmask != 0u) {
 #pragma unroll
@@ -1553,7 +1599,7 @@ __global__ void __launch_bounds__(PROBEF_THREADS, KB_PI_MINB) probe_index_kernel
 template <int T, int PRE, bool AGG, bool TAB>
 static void launch_probe_index_tp(const ProbeIParams& p, const GroupParams& g, int n_sms, cudaStream_t st) {
     static int per_sm = 0;  // occupancy is a property of the kernel image: asked once per instantiation
-    const size_t smem = TAB ? (size_t)PROBEF_THREADS * 4 * (PRE == 1 ? 12 : 4) * 2 : (size_t)PROBEF_THREADS * 4 * (PRE == 1 ? 16 : 8) * 2;
+    const size_t smem = TAB ? (size_t)PROBEF_THREADS * 4 * (PRE == 1 ? 8 : 4) * 2 : (size_t)PROBEF_THREADS * 4 * (PRE == 1 ? 16 : 8) * 2;
     if (per_sm == 0) {
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, probe_index_kernel<T, PRE, AGG, TAB>, PROBEF_THREADS, smem);
         if (per_sm < 1) per_sm = 1;

@@ -179,10 +179,12 @@ struct ProbeIParams {
     ProbeISeg seg[PROBEI_MAXSEG];
     u32 n_seg;
     // table mode (ptab != nullptr): the probe stream is the probe pattern's own persistent table, slot by slot (keys ascending), and
-    // pnum the numeric value of the slot's other half (pre_mode == 1); keys are rebuilt from the slot number (ptab_min + slot, then
-    // the inverse of the shard compaction)
+    // pkey the rank of the numeric value of the slot's other half in the value order of the numeric side table (pre_mode == 1: the
+    // FILTER is `rank in [key_lo, key_hi)`, kb_numrank.cuh); keys are rebuilt from the slot number (ptab_min + slot, then the inverse
+    // of the shard compaction)
     const u32* ptab;
-    const double* pnum;
+    const u32* pkey;
+    u32 key_lo, key_hi;
     u32 ptab_min, ptab_range, ptab_cshift, shard_rank;
     u32 key_is_y, n, n_tiles, T;  // n = rows over all chunks
     DirectTab tab[MAXT];
@@ -241,7 +243,7 @@ struct SplitEntry {
     uint2* pairs;       // the new chunk
     double* ynum;       // its typed literal column (null: no numeric side table loaded)
     u32* xtab; u32 xtab_min, xtab_range, cshift;   // subject table to insert into (null: none)
-    double* xnum;       // typed values in table order, maintained with xtab (null: none)
+    u32* xkey;          // value ranks in table order, maintained with xtab (null: none)
     u32* ytab; u32 ytab_min, ytab_range;           // object table (null: none)
 };
 // control words per entry (all 0 at launch): cursor, n_numeric, xdup, ydup, xout, yout, pad, pad, ~xmin, ~ymin, xmax, ymax
@@ -253,6 +255,8 @@ struct SplitParams {
     SplitEntry e[MAXP];
     u32* ctrl;  // k * SPLIT_WORDS words
     NumTab nt;
+    const double* numv;  // value order of the numeric side table (kb_numrank.cuh), for the entries' xkey (n_numv = 0: no entry has one)
+    u32 n_numv;
 };
 void launch_segment_split(const SplitParams& p, int n_sms, cudaStream_t st);
 
@@ -267,8 +271,14 @@ void launch_clear_chunks(const ClearParams& p, int n_sms, cudaStream_t st);
 // min/max of both halves of a pair relation: out[0..3] = min x, min y, max x, max y
 // typed literal column of a predicate slice: out[i] = num_or0[kv[i].y]; *n_numeric += rows whose object is numeric
 void launch_pair_numcol(const uint2* kv, u32 n, NumTab nt, double* out, u32* n_numeric, int n_sms, cudaStream_t st);
-// the same values laid out like the subject-keyed direct table: out[compact(subject) - kmin] = num_or0[object]
-void launch_pair_numtab(const uint2* kv, u32 n, NumTab nt, double* out, u32 kmin, u32 range, u32 cshift, int n_sms, cudaStream_t st);
+// the ranks of those values in the value order numv[0 .. n_numv) (kb_numrank.cuh), laid out like the subject-keyed direct table:
+// out[compact(subject) - kmin] = rank_of(num_of(object))
+void launch_pair_ranktab(const uint2* kv, u32 n, NumTab nt, const double* numv, u32 n_numv, u32* out, u32 kmin, u32 range, u32 cshift, int n_sms,
+                         cudaStream_t st);
+// the value order of the numeric side table: keys[i] = order-preserving u64 of fold(num_or0[i]) for i < n, of 0.0 for i == n and for NaN
+void launch_numorder_keys(const double* num_or0, u32 n, unsigned long long* keys, int n_sms, cudaStream_t st);
+// the inverse, over the sorted distinct keys
+void launch_numorder_values(const unsigned long long* keys, u32 n, double* out, int n_sms, cudaStream_t st);
 void launch_pair_minmax(const uint2* kv, u32 n, u32* out4, int n_sms, cudaStream_t st);
 // number of occupied (non-EMPTY32) slots of a direct table: equals the number of inserted rows iff the keys were single-valued
 void launch_count_nonempty(const u32* table, u32 n, u32* out_count, int n_sms, cudaStream_t st);

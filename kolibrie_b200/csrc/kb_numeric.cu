@@ -5,6 +5,13 @@
 //   K1 numeric_derive_kernel  thread per id: kb_numparse.cuh's parse_f64 / parse_i32 of the id's string. Most terms are IRIs and names,
 //                             rejected on their first byte. An id whose value Eisel–Lemire cannot decide is appended to a list.
 //   K2 numeric_slow_kernel    thread per listed id: slow_f64, the exact decimal conversion (its 788-byte decimal lives in local memory)
+// and, for the store index's rank columns, the value order of the f64 table (ensure_num_order, kb_numrank.cuh).
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_select.cuh>
+
+#include <algorithm>
+#include <climits>
+
 #include "kb_internal.hpp"
 #include "kb_numparse.cuh"
 
@@ -89,6 +96,47 @@ static kb_status numeric_grow(kb_ctx* ctx, Buf* a, Buf* b, size_t elem_a, u32 ke
 static int grid_for(u64 n, int n_sms, int threads, int per_sm) {
     const u64 want = (n + threads - 1) / threads;
     return (int)std::max<u64>(1, std::min<u64>(want, (u64)n_sms * per_sm));
+}
+
+// The value order V of the f64 table (kb_numrank.cuh): every value as an order-preserving u64 key (NaN as 0.0, -0.0 as +0.0, one extra
+// 0.0), a radix sort, the distinct keys, back to doubles; then the host copy that FILTER constants are resolved against. Run by the
+// index build for its rank columns, never by a query.
+kb_status ensure_num_order(kb_ctx* ctx, bool* ok) {
+    *ok = true;
+    if (ctx->numv && ctx->numv_version == ctx->num_version) return KB_OK;
+    ctx->numv.reset();
+    ctx->h_numv.clear();
+    const u64 m = (u64)ctx->n_ids + 1;
+    if (m > (u64)INT32_MAX) { *ok = false; return KB_OK; }
+    Buf a, b, cnt, tmp;
+    KB_TRY(alloc_buf(ctx, m * sizeof(unsigned long long), &a));
+    KB_TRY(alloc_buf(ctx, m * sizeof(unsigned long long), &b));
+    KB_TRY(alloc_buf(ctx, sizeof(int), &cnt));
+    unsigned long long* ka = static_cast<unsigned long long*>(a->p);
+    unsigned long long* kb_ = static_cast<unsigned long long*>(b->p);
+    int* d_cnt = static_cast<int*>(cnt->p);
+    size_t t_sort = 0, t_uniq = 0;
+    KB_CUDA(ctx, cub::DeviceRadixSort::SortKeys(nullptr, t_sort, ka, kb_, (int)m, 0, 64, ctx->st));
+    KB_CUDA(ctx, cub::DeviceSelect::Unique(nullptr, t_uniq, kb_, ka, d_cnt, (int)m, ctx->st));
+    KB_TRY(alloc_buf(ctx, std::max<size_t>(std::max(t_sort, t_uniq), 16), &tmp));
+    launch_numorder_keys(ctx->num ? static_cast<const double*>(ctx->num->p) : nullptr, ctx->n_ids, ka, ctx->n_sms, ctx->st);
+    KB_CUDA(ctx, cub::DeviceRadixSort::SortKeys(tmp->p, t_sort, ka, kb_, (int)m, 0, 64, ctx->st));
+    KB_CUDA(ctx, cub::DeviceSelect::Unique(tmp->p, t_uniq, kb_, ka, d_cnt, (int)m, ctx->st));
+    int n_v = 0;
+    KB_CUDA(ctx, cudaMemcpyAsync(&n_v, d_cnt, sizeof(int), cudaMemcpyDeviceToHost, ctx->st));
+    KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
+    Buf v;
+    KB_TRY(alloc_buf(ctx, (size_t)n_v * sizeof(double), &v));
+    launch_numorder_values(ka, (u32)n_v, static_cast<double*>(v->p), ctx->n_sms, ctx->st);
+    KB_CUDA(ctx, cudaGetLastError());
+    ctx->stats.kernel_launches += 2;
+    ctx->h_numv.resize((size_t)n_v);
+    KB_CUDA(ctx, cudaMemcpyAsync(ctx->h_numv.data(), v->p, (size_t)n_v * sizeof(double), cudaMemcpyDeviceToHost, ctx->st));
+    KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
+    ctx->stats.d2h_bytes += sizeof(int) + (size_t)n_v * sizeof(double);
+    ctx->numv = v;
+    ctx->numv_version = ctx->num_version;
+    return KB_OK;
 }
 
 }  // namespace kb
