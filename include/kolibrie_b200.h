@@ -43,7 +43,7 @@ typedef int32_t kb_status;
  * it is never a dictionary id (< 0x8000_0000) and is used here as "no such term" / empty hash slot. */
 #define KB_ID_NONE 0xFFFFFFFFu
 
-#define KB_MAX_PATTERNS 8   /* patterns fused in one scan / one star join */
+#define KB_MAX_PATTERNS 8   /* patterns fused in one scan / one star join (kb_bgp_execute takes up to KB_BGP_MAX_PATTERNS) */
 #define KB_MAX_COLS 16      /* columns (variables) per relation */
 #define KB_MAX_FILTER_OPS 32
 #define KB_MAX_PREMISES 6
@@ -396,11 +396,48 @@ KB_API kb_status kb_scan_quoted(kb_ctx* ctx, const kb_quoted_pattern* qp, kb_rel
  * conjuncts that touch one pattern only are pushed into the scan. Result caps of the reference (quirk Q1) are NOT applied. */
 KB_API kb_status kb_star_join(kb_ctx* ctx, uint32_t join_slot, const kb_pattern* pats, uint32_t n_pats,
                               const kb_filter_op* filter, uint32_t n_filter_ops, kb_rel** out);
-/* whole BGP: patterns joined left-deep in the given order (build_logical_plan, utils.rs:101-191), star-fused when
- * all patterns share one variable (optimizer.rs:84-152); then FILTER, then projection (NULL = all variables). */
+/* Whole BGP: the bag of rows of the patterns' natural join, with one column per distinct variable in order of first appearance
+ * over the patterns; then FILTER (conjuncts over one pattern's variables are applied while that pattern is read, the rest to the
+ * joined rows), then projection (NULL = all variables). Row order is unspecified. Two routes:
+ *   star        at most KB_MAX_PATTERNS patterns and one variable shared by every pattern: kb_star_join (optimizer.rs:84-152).
+ *   components  every other BGP of 1..KB_BGP_MAX_PATTERNS patterns. The patterns are scanned (fused groups of KB_MAX_PATTERNS; index
+ *               lookups with a valid index); an empty pattern ends the call with an empty result. They are split into connected
+ *               components over shared variables (a pattern without variables is a component of its own). A component of three
+ *               or more patterns is first reduced on the device: every variable held by two or more of its patterns keeps a bitmap
+ *               over the store's id range of the values all of them hold, and each round drops the rows that a bitmap rejects
+ *               (ids beyond the bitmap, such as quoted ids, are kept) until no relation shrinks, at most one round per pattern.
+ *               Inside a component only patterns that share a variable are joined: along the GYO join tree when the component is
+ *               acyclic, starting at its smallest relation and adding the smallest tree neighbour; otherwise adding the smallest
+ *               relation that shares a variable with the rows so far. The components are then cross-joined, smallest first.
+ * Limits: more than KB_BGP_MAX_PATTERNS patterns or more than KB_MAX_COLS variables -> KB_E_LIMIT; a cartesian product of more
+ * than 2^28 rows, which only a cross join between components forms -> KB_E_LIMIT. kb_bgp_last_plan describes the call. The
+ * reduction's launches and device time count in kb_stats' `filter` family. */
+#define KB_BGP_MAX_PATTERNS 16
 KB_API kb_status kb_bgp_execute(kb_ctx* ctx, const kb_pattern* pats, uint32_t n_pats,
                                 const kb_filter_op* filter, uint32_t n_filter_ops,
                                 const uint32_t* project_slots, uint32_t n_project, kb_rel** out);
+/* What the context's last successful kb_bgp_execute did. Arrays are indexed by pattern (k < n_patterns), by component
+ * (c < n_components) or by join step. Star route: n_components = 1 and only route / n_patterns / rows_unprojected are set. */
+enum kb_bgp_route { KB_BGP_NONE = 0, KB_BGP_STAR = 1, KB_BGP_COMPONENTS = 2 };
+typedef struct kb_bgp_plan_info {
+    uint32_t route;                                   /* kb_bgp_route */
+    uint32_t n_patterns, n_components;
+    uint32_t component[KB_BGP_MAX_PATTERNS];          /* component of pattern k (components in the order of their first pattern) */
+    uint32_t acyclic[KB_BGP_MAX_PATTERNS];            /* per component: 1 when GYO reduces it (its joins follow the join tree) */
+    uint32_t reduce_rounds[KB_BGP_MAX_PATTERNS];      /* per component: domain-reduction rounds run (0: not reduced) */
+    uint64_t rows_scanned[KB_BGP_MAX_PATTERNS];       /* rows of pattern k after its scan */
+    uint64_t rows_reduced[KB_BGP_MAX_PATTERNS];       /* rows of pattern k after the reduction (= rows_scanned when not reduced) */
+    uint32_t join_order[KB_BGP_MAX_PATTERNS];         /* patterns in the order they were joined, component by component (not set
+                                                         when a pattern's relation is empty: the call returns before any join) */
+    uint64_t component_rows[KB_BGP_MAX_PATTERNS];     /* per component: rows of its join */
+    uint64_t component_max_rows[KB_BGP_MAX_PATTERNS]; /* per component: the largest relation among its joins' outputs */
+    uint32_t cross_order[KB_BGP_MAX_PATTERNS];        /* components in the order they were cross-joined */
+    uint64_t reduce_bytes;                            /* the reduction's modelled HBM bytes: 4 per column and row read, 4 per column and row written */
+    uint64_t reduce_bit_ops;                          /* the reduction's bitmap operations: one probe (filtering rounds) and one atomicOr per row and reduced variable */
+    uint64_t max_intermediate;                        /* the largest join output of the call, cross joins included */
+    uint64_t rows_unprojected;                        /* rows before projection */
+} kb_bgp_plan_info;
+KB_API kb_status kb_bgp_last_plan(kb_ctx* ctx, kb_bgp_plan_info* out);
 /* GROUP BY + aggregates (execute_query.rs:1150-1227) */
 KB_API kb_status kb_group_aggregate(kb_ctx* ctx, const kb_rel* in, const uint32_t* group_slots, uint32_t n_group,
                                     const kb_agg* aggs, uint32_t n_aggs, kb_groups** out);

@@ -108,6 +108,30 @@ class KbMaintainStats(C.Structure):
         ("overdelete_rounds", C.c_uint32), ("insert_rounds", C.c_uint32), ("device_ms", C.c_double)]
 
 
+KB_BGP_MAX_PATTERNS = 16
+BGP_NONE, BGP_STAR, BGP_COMPONENTS = 0, 1, 2  # kb_bgp_route
+
+
+class KbBgpPlanInfo(C.Structure):
+    """kb_bgp_plan_info: what the last kb_bgp_execute did (route, components, reduction, join order, intermediate sizes)"""
+    _M = KB_BGP_MAX_PATTERNS
+    _fields_ = [("route", C.c_uint32), ("n_patterns", C.c_uint32), ("n_components", C.c_uint32), ("component", C.c_uint32 * _M),
+                ("acyclic", C.c_uint32 * _M), ("reduce_rounds", C.c_uint32 * _M), ("rows_scanned", C.c_uint64 * _M), ("rows_reduced", C.c_uint64 * _M),
+                ("join_order", C.c_uint32 * _M), ("component_rows", C.c_uint64 * _M), ("component_max_rows", C.c_uint64 * _M),
+                ("cross_order", C.c_uint32 * _M), ("reduce_bytes", C.c_uint64), ("reduce_bit_ops", C.c_uint64), ("max_intermediate", C.c_uint64), ("rows_unprojected", C.c_uint64)]
+
+    def as_dict(self):
+        """arrays cut to the patterns / components / join steps the call had"""
+        n, m = self.n_patterns, self.n_components
+        cut = {"component": n, "rows_scanned": n, "rows_reduced": n, "join_order": n if self.route == BGP_COMPONENTS else 0, "acyclic": m,
+               "reduce_rounds": m, "component_rows": m, "component_max_rows": m, "cross_order": m}
+        out = {}
+        for name, _ in self._fields_:
+            v = getattr(self, name)
+            out[name] = [int(x) for x in v[: cut[name]]] if name in cut else int(v)
+        return out
+
+
 class KbStats(C.Structure):
     _fields_ = [(n, C.c_double) for n in ("scan_ms", "build_ms", "probe_ms", "filter_ms", "group_ms", "other_ms", "total_ms")] + [
         (n, C.c_uint64)
@@ -232,6 +256,7 @@ def lib() -> C.CDLL:
         "kb_scan_quoted": (i32, [vp, P(KbQuotedPattern), P(vp)]),
         "kb_star_join": (i32, [vp, u32, P(KbPattern), u32, P(KbFilterOp), u32, P(vp)]),
         "kb_bgp_execute": (i32, [vp, P(KbPattern), u32, P(KbFilterOp), u32, P(u32), u32, P(vp)]),
+        "kb_bgp_last_plan": (i32, [vp, P(KbBgpPlanInfo)]),
         "kb_group_aggregate": (i32, [vp, vp, P(u32), u32, P(KbAgg), u32, P(vp)]),
         "kb_groups_info": (i32, [vp, P(u64), P(u32), P(u32)]),
         "kb_groups_keys": (i32, [vp, u32, P(P(u32))]),
@@ -282,7 +307,7 @@ EXPORTED_SYMBOLS = [
     "kb_version", "kb_ctx_create", "kb_ctx_destroy", "kb_last_error", "kb_set_timing", "kb_get_stats", "kb_synchronize",
     "kb_store_load", "kb_store_load_device", "kb_store_append", "kb_store_append_device", "kb_store_evict", "kb_store_delete", "kb_store_clear", "kb_store_build_index", "kb_set_use_index", "kb_store_size",
     "kb_store_download", "kb_dict_numeric_load", "kb_dict_legacy_i32_load", "kb_dict_numeric_derive", "kb_dict_numeric_download", "kb_dict_strings_load", "kb_dict_encode", "kb_dict_strings_info", "kb_rel_decode", "kb_strings_info", "kb_strings_download", "kb_strings_free", "kb_quoted_load", "kb_quoted_download", "kb_dict_strings_download", "kb_bind", "kb_rel_info", "kb_rel_download", "kb_rel_device_col", "kb_rel_from_host",
-    "kb_rel_from_device", "kb_rel_free", "kb_scan", "kb_filter", "kb_project", "kb_hash_join", "kb_natural_join", "kb_bind_join", "kb_scan_quoted", "kb_star_join", "kb_bgp_execute",
+    "kb_rel_from_device", "kb_rel_free", "kb_scan", "kb_filter", "kb_project", "kb_hash_join", "kb_natural_join", "kb_bind_join", "kb_scan_quoted", "kb_star_join", "kb_bgp_execute", "kb_bgp_last_plan",
     "kb_group_aggregate", "kb_groups_info", "kb_groups_keys", "kb_groups_values", "kb_groups_counts", "kb_groups_free", "kb_groups_pack", "kb_groups_merge", "kb_star_join_aggregate",
     "kb_star_join_prepare", "kb_plan_submit", "kb_plan_collect", "kb_plan_info", "kb_plan_free", "kb_plan_peer_scratch_bytes", "kb_plan_attach_peers",
     "kb_datalog_fixpoint", "kb_datalog_fixpoint_seed", "kb_datalog_maintain", "kb_r2s_create", "kb_r2s_eval", "kb_r2s_info", "kb_r2s_free", "kb_shard_of", "kb_set_sharding", "kb_partition", "kb_partition_counts", "kb_segment_write", "kb_segment_info", "kb_segment_save", "kb_store_append_file", "kb_shuffle_scatter", "kb_shuffle_push", "kb_rel_wrap_device", "kb_star_join_host", "kb_star_join_host_into", "perform_hash_join_cuda",
@@ -625,6 +650,13 @@ class Context:
         else:
             self._check(lib().kb_bgp_execute(self.h, patterns(pats), len(pats), a, n, None, 0, C.byref(out)))
         return Relation(self, out)
+
+    def bgp_last_plan(self) -> dict:
+        """kb_bgp_last_plan: the route, components, reduction rounds, rows per pattern, join order and intermediate sizes of the last
+        successful bgp_execute"""
+        info = KbBgpPlanInfo()
+        self._check(lib().kb_bgp_last_plan(self.h, C.byref(info)))
+        return info.as_dict()
 
     def rel_from_host(self, slots: Sequence[int], cols: Sequence[np.ndarray]) -> Relation:
         cols = [_u32(c) for c in cols]

@@ -349,8 +349,7 @@ kb_status unpair_rel(kb_ctx* ctx, std::unique_ptr<kb_rel>* r) {
     return KB_OK;
 }
 
-// a relation of zero rows over `slots`
-static kb_status empty_rel(kb_ctx* ctx, const std::vector<u32>& slots, std::unique_ptr<kb_rel>* out) {
+kb_status empty_rel(kb_ctx* ctx, const std::vector<u32>& slots, std::unique_ptr<kb_rel>* out) {
     auto r = std::make_unique<kb_rel>();
     r->slots = slots;
     for (size_t c = 0; c < slots.size(); c++) { Col col; KB_TRY(alloc_col(ctx, 0, &col)); r->cols.push_back(col); }
@@ -910,8 +909,7 @@ kb_status hash_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_rel& R, const Fi
     return KB_OK;
 }
 
-// reorder / select columns (zero-copy)
-static std::unique_ptr<kb_rel> select_cols(const kb_rel& in, const std::vector<u32>& slots) {
+std::unique_ptr<kb_rel> select_cols(const kb_rel& in, const std::vector<u32>& slots) {
     auto r = std::make_unique<kb_rel>();
     r->n = in.n;
     for (u32 s : slots) {
@@ -947,9 +945,8 @@ struct StarQuery {  // a star join, validated once: what every route reads
 
 enum class Route { answered, declined, retry };
 
-// FILTER: a conjunct over one pattern's variables goes to the first pattern that binds them all, every other conjunct to `post`
-static kb_status split_filter(kb_ctx* ctx, const kb_filter_op* filter, u32 n_ops, const std::vector<std::vector<u32>>& pv,
-                              const std::vector<u32>& all_slots, std::vector<FilterProg>* pushdown, FilterProg* post) {
+kb_status split_filter(kb_ctx* ctx, const kb_filter_op* filter, u32 n_ops, const std::vector<std::vector<u32>>& pv,
+                       const std::vector<u32>& all_slots, std::vector<FilterProg>* pushdown, FilterProg* post) {
     std::vector<FilterProg> conj;
     if (!split_conjuncts(filter, n_ops, &conj)) return fail(ctx, KB_E_INVALID, "malformed filter program");
     pushdown->assign(pv.size(), FilterProg{});
@@ -3029,7 +3026,7 @@ kb_status kb_bgp_execute(kb_ctx* ctx, const kb_pattern* pats, uint32_t n_pats, c
                          const uint32_t* project, uint32_t n_project, kb_rel** out) {
     KB_ENTER(ctx);
     if (!pats || !out || n_pats == 0) return kb::fail(ctx, KB_E_INVALID, "NULL or empty BGP");
-    if (n_pats > (u32)kb::MAXP) return kb::fail(ctx, KB_E_LIMIT, "more than %d patterns", kb::MAXP);
+    if (n_pats > KB_BGP_MAX_PATTERNS) return kb::fail(ctx, KB_E_LIMIT, "more than %d patterns", KB_BGP_MAX_PATTERNS);
     KB_TRY(kb::validate_filter(ctx, filter, n_ops));
     std::vector<std::vector<u32>> pv(n_pats), ps(n_pats);
     std::vector<u32> all_slots;
@@ -3039,7 +3036,7 @@ kb_status kb_bgp_execute(kb_ctx* ctx, const kb_pattern* pats, uint32_t n_pats, c
     }
     // a variable shared by every pattern -> star join (optimizer.rs:84-152); prefer the subject position
     int star = -1;
-    for (size_t i = 0; i < pv[0].size() && star < 0; i++) {
+    for (size_t i = 0; n_pats <= (u32)kb::MAXP && i < pv[0].size() && star < 0; i++) {
         bool all = true;
         for (u32 k = 1; k < n_pats; k++) if (std::find(pv[k].begin(), pv[k].end(), pv[0][i]) == pv[k].end()) all = false;
         if (all) star = (int)pv[0][i];
@@ -3047,21 +3044,13 @@ kb_status kb_bgp_execute(kb_ctx* ctx, const kb_pattern* pats, uint32_t n_pats, c
     std::unique_ptr<kb_rel> cur;
     if (star >= 0) {
         KB_TRY(kb::star_join_impl(ctx, (u32)star, pats, n_pats, filter, n_ops, &cur));
+        ctx->bgp_last = kb_bgp_plan_info{};
+        ctx->bgp_last.route = KB_BGP_STAR;
+        ctx->bgp_last.n_patterns = n_pats;
+        ctx->bgp_last.n_components = 1;
+        ctx->bgp_last.rows_unprojected = cur->n;
     } else {
-        // left-deep natural joins in textual order (build_logical_plan, utils.rs:101-191)
-        std::vector<kb::FilterProg> pushdown;
-        kb::FilterProg post;
-        KB_TRY(kb::split_filter(ctx, filter, n_ops, pv, all_slots, &pushdown, &post));
-        std::vector<std::unique_ptr<kb_rel>> rels;
-        KB_TRY(kb::scan_impl(ctx, pats, n_pats, pushdown, false, false, &rels));
-        cur = std::move(rels[0]);
-        for (u32 k = 1; k < n_pats; k++) {
-            std::unique_ptr<kb_rel> j;
-            KB_TRY(kb::hash_join_impl(ctx, *cur, *rels[k], (k + 1 == n_pats && !post.ops.empty()) ? &post : nullptr, &j));
-            cur = std::move(j);
-        }
-        if (n_pats == 1 && !post.ops.empty()) { std::unique_ptr<kb_rel> f; KB_TRY(kb::filter_impl(ctx, *cur, post, &f)); cur = std::move(f); }
-        cur = kb::select_cols(*cur, all_slots);
+        KB_TRY(kb::bgp_components(ctx, pats, n_pats, filter, n_ops, pv, all_slots, &cur));
     }
     if (project) {
         std::vector<u32> v(project, project + n_project);

@@ -248,6 +248,7 @@ struct kb_ctx {
     bool index_maintain = true;          // KOLIBRIE_INDEX_MAINTAIN=0: append / evict drop the index instead of maintaining it (A/B switch)
     kb::u32 shard_rank = 0, shard_world = 1;  // kb_set_sharding: the store is shard `rank` of `world`, sharded by subject
     int upload_stats_off = -1;  // chunked upload in flight: control words where the copy stream accumulates the column ranges
+    kb_bgp_plan_info bgp_last{};  // kb_bgp_last_plan
 };
 
 namespace kb {
@@ -381,6 +382,15 @@ QuotedTab quotedtab(const kb_ctx* ctx);
 kb_status dict_encode_device(kb_ctx* ctx, const u64* d_off, const unsigned char* d_bytes, u64 n_terms, u64 total, u32* d_out_ids, u32* n_new,
                              Buf* first_pos);
 void pattern_vars(const kb_pattern& pt, std::vector<u32>* slots, std::vector<u32>* src);
+kb_status empty_rel(kb_ctx* ctx, const std::vector<u32>& slots, std::unique_ptr<kb_rel>* out);  // zero rows over `slots`
+std::unique_ptr<kb_rel> select_cols(const kb_rel& in, const std::vector<u32>& slots);          // reorder / select columns (zero-copy)
+// FILTER: a conjunct over one pattern's variables goes to the first pattern that binds them all, every other conjunct to `post`
+kb_status split_filter(kb_ctx* ctx, const kb_filter_op* filter, u32 n_ops, const std::vector<std::vector<u32>>& pv,
+                       const std::vector<u32>& all_slots, std::vector<FilterProg>* pushdown, FilterProg* post);
+// kb_bgp_execute's component route (kb_bgp.cu): pv / all_slots as kb_bgp_execute derived them; *out has the columns of all_slots.
+// Fills ctx->bgp_last.
+kb_status bgp_components(kb_ctx* ctx, const kb_pattern* pats, u32 n_pats, const kb_filter_op* filter, u32 n_ops,
+                         const std::vector<std::vector<u32>>& pv, const std::vector<u32>& all_slots, std::unique_ptr<kb_rel>* out);
 u32 pow2_at_least(u64 x);
 kb_status check_pattern(kb_ctx* ctx, const kb_pattern& pt);
 

@@ -395,3 +395,133 @@ def multivalued_dataset(n_subjects: int, per_subject: int = 3, seed: int = 9):
     num[lit0:] = np.arange(1000, dtype=np.float64)
     isn[lit0:] = 1
     return s.astype(np.uint32), p, o.astype(np.uint32), num, isn, {"subj": subj, "score": score, "tags": tags, "lit0": lit0, "per_subject": per_subject}
+
+
+# ---------------------------------------------------------------------------------------------------------------------------------
+# WatDiv-shaped workload: the entity classes, predicates and named constants of the 20 WatDiv queries of the reference's harness
+# (kolibrie/examples/sparql_syntax/n_triples_data/n_triple_10M.rs:104-570; tests/golden/watdiv/queries.json). It is WatDiv-SHAPED,
+# not WatDiv: its numbers are not comparable with the reference's WatDiv latencies.
+WATDIV_NS = {"wsdbm": "http://db.uwaterloo.ca/~galuc/wsdbm/", "sorg": "http://schema.org/", "dc": "http://purl.org/dc/terms/",
+             "foaf": "http://xmlns.com/foaf/", "gr": "http://purl.org/goodrelations/", "gn": "http://www.geonames.org/ontology#",
+             "mo": "http://purl.org/ontology/mo/", "og": "http://ogp.me/ns#", "rev": "http://purl.org/stuff/rev#",
+             "rdf": "http://www.w3.org/1999/02/22-rdf-syntax-ns#"}
+# entity classes (IRI wsdbm:<Class><i>) and, per scale unit s, how many of each; fixed-size classes hold every named constant
+WATDIV_CLASSES = ("User", "Product", "Review", "Offer", "Retailer", "Purchase", "Website", "City", "Country", "Topic", "SubGenre",
+                  "ProductCategory", "Role", "AgeGroup", "Language", "Genre")
+_WD_LIT = len(WATDIV_CLASSES)  # literal terms: class id _WD_LIT, sub = predicate
+
+
+def watdiv_sizes(n_triples: int) -> Dict[str, int]:
+    s = max(1, n_triples // 462)  # ~462 triples per scale unit
+    return {"User": 10 * s, "Product": 10 * s, "Review": 15 * s, "Offer": 10 * s, "Retailer": 10 + s // 10, "Purchase": 15 * s,
+            "Website": 600 + s, "City": 50 + s // 20, "Country": 25, "Topic": 100, "SubGenre": 150, "ProductCategory": 5, "Role": 3,
+            "AgeGroup": 9, "Language": 25, "Genre": 1}
+
+
+# (predicate, subject class, object: a class name, "lit" (a literal per subject), "lit:<k>" (one of k literals); every subject
+# carries it when `every` == 1, else the subjects i with i % every == 0; `per` objects per subject)
+WATDIV_PREDICATES = (
+    ("wsdbm:likes", "User", "Product", 1, 2), ("wsdbm:friendOf", "User", "User", 1, 2), ("dc:Location", "User", "City", 1, 1),
+    ("foaf:age", "User", "AgeGroup", 1, 1), ("wsdbm:gender", "User", "lit:2", 1, 1), ("foaf:givenName", "User", "lit", 1, 1),
+    ("foaf:familyName", "User", "lit", 1, 1), ("wsdbm:subscribes", "User", "Website", 1, 1), ("sorg:nationality", "User", "Country", 1, 1),
+    ("rdf:type", "User", "Role", 1, 1), ("foaf:homepage", "User", "Website", 2, 1), ("sorg:jobTitle", "User", "lit:50", 3, 1),
+    ("sorg:caption", "Product", "lit", 1, 1), ("sorg:text", "Product", "lit", 1, 1), ("sorg:contentRating", "Product", "lit:10", 1, 1),
+    ("og:tag", "Product", "Topic", 1, 1), ("rdf:type", "Product", "ProductCategory", 1, 1), ("wsdbm:hasGenre", "Product", "SubGenre", 1, 1),
+    ("sorg:keywords", "Product", "lit", 1, 1), ("foaf:homepage", "Product", "Website", 1, 1), ("og:title", "Product", "lit", 1, 1),
+    ("sorg:description", "Product", "lit", 1, 1), ("sorg:contentSize", "Product", "lit:1000", 1, 1), ("sorg:language", "Product", "Language", 1, 1),
+    ("sorg:trailer", "Product", "lit", 4, 1), ("mo:conductor", "Product", "User", 5, 1), ("sorg:actor", "Product", "User", 3, 1),
+    ("mo:artist", "Product", "User", 5, 1), ("sorg:publisher", "Product", "lit:200", 2, 1),
+    ("rev:hasReview", "Review", "Product", 1, 1),  # (stored reversed: product rev:hasReview review)
+    ("rev:title", "Review", "lit", 1, 1), ("rev:reviewer", "Review", "User", 1, 1), ("rev:totalVotes", "Review", "lit:100", 1, 1),
+    ("gr:includes", "Offer", "Product", 1, 1), ("sorg:eligibleRegion", "Offer", "Country", 1, 1), ("gr:price", "Offer", "lit:1000", 1, 1),
+    ("gr:serialNumber", "Offer", "lit", 1, 1), ("gr:validFrom", "Offer", "lit:365", 1, 1), ("gr:validThrough", "Offer", "lit:365", 1, 1),
+    ("sorg:eligibleQuantity", "Offer", "lit:20", 1, 1), ("sorg:priceValidUntil", "Offer", "lit:365", 1, 1),
+    ("gr:offers", "Offer", "Retailer", 1, 1),  # (stored reversed: retailer gr:offers offer)
+    ("sorg:legalName", "Retailer", "lit", 1, 1),
+    ("wsdbm:makesPurchase", "Purchase", "User", 1, 1),  # (stored reversed: user wsdbm:makesPurchase purchase)
+    ("wsdbm:purchaseFor", "Purchase", "Product", 1, 1), ("wsdbm:purchaseDate", "Purchase", "lit:365", 1, 1),
+    ("sorg:url", "Website", "lit", 1, 1), ("wsdbm:hits", "Website", "lit:1000", 1, 1), ("sorg:language", "Website", "Language", 1, 1),
+    ("gn:parentCountry", "City", "Country", 1, 1),
+    ("og:tag", "SubGenre", "Topic", 1, 1), ("rdf:type", "SubGenre", "Genre", 1, 1),
+)
+_WD_REVERSED = {"rev:hasReview", "gr:offers", "wsdbm:makesPurchase"}
+# the constants the queries name, drawn most often (rank 0, 1, ...) by the popularity law below
+WATDIV_POPULAR = {"Country": (1, 5, 6), "Topic": (1, 7, 10), "SubGenre": (1, 5, 26), "Retailer": (0, 1), "Website": (546,), "City": (0,),
+                  "Product": (0,), "User": (7,), "ProductCategory": (2, 4), "Role": (2,), "AgeGroup": (4,), "Language": (0,)}
+
+
+def watdiv_iri(prefixed: str) -> str:
+    pre, local = prefixed.split(":", 1)
+    return "<" + WATDIV_NS[pre] + local + ">"
+
+
+def watdiv_predicate_counts(n_triples: int) -> Dict[str, int]:
+    """closed form: rows per predicate IRI"""
+    sz, out = watdiv_sizes(n_triples), {}
+    for p, cls, _, every, per in WATDIV_PREDICATES:
+        out[watdiv_iri(p)] = out.get(watdiv_iri(p), 0) + ((sz[cls] + every - 1) // every) * per
+    return out
+
+
+@dataclass
+class WatDivData:
+    s: np.ndarray
+    p: np.ndarray
+    o: np.ndarray
+    n_ids: int
+    ids: Dict[str, int]  # IRI (<...>) of every predicate and of every entity a query names -> dictionary id
+    sizes: Dict[str, int]
+
+
+def watdiv(n_triples: int, seed: int = 11) -> WatDivData:
+    """A seeded WatDiv-shaped store of about n_triples triples (splitmix64 draws). Objects of entity-valued predicates follow a
+    Zipf-like popularity law over a rank order whose first ranks are the named constants (rank r of m drawn with probability about
+    1 / (2 sqrt(m r))), so every query has answers at ~100 K triples already while the most popular entity keeps a share of 1/sqrt(m). Dictionary ids are assigned in first-seen order over (s, p, o) per triple."""
+    sz = watdiv_sizes(n_triples)
+    cls_id = {c: i for i, c in enumerate(WATDIV_CLASSES)}
+    preds = []
+    for p, *_ in WATDIV_PREDICATES:
+        if p not in preds:
+            preds.append(p)
+    S, P, O = [], [], []
+    key = lambda c, sub, idx: (np.uint64(c) << np.uint64(56)) | (np.uint64(sub) << np.uint64(32)) | idx.astype(np.uint64)
+    PRED_CLASS = _WD_LIT + 1
+    for j, (p, cls, obj, every, per) in enumerate(WATDIV_PREDICATES):
+        subj = np.arange(0, sz[cls], every, dtype=np.uint64)
+        subj = np.repeat(subj, per)
+        r = splitmix64_at(seed + 1000 * j, np.arange(len(subj), dtype=np.uint64))
+        if obj.startswith("lit"):
+            k = int(obj.split(":")[1]) if ":" in obj else 0
+            val = (r % np.uint64(k)) if k else subj
+            o = key(_WD_LIT, j, val)
+        else:
+            m = sz[obj]
+            u = (r >> np.uint64(11)).astype(np.float64) / float(1 << 53)
+            rank = np.minimum((float(m) * u * u).astype(np.int64), m - 1)  # P(rank r) ~ 1 / (2 sqrt(m r)): rank 0 gets 1/sqrt(m)
+            named = list(WATDIV_POPULAR.get(obj, ()))
+            order = np.concatenate([np.array(named, np.int64), np.setdiff1d(np.arange(m, dtype=np.int64), named)])
+            o = key(cls_id[obj], 0, order[rank].astype(np.uint64))
+        s = key(cls_id[cls], 0, subj)
+        if p in _WD_REVERSED:
+            s, o = o, s
+        S.append(s)
+        P.append(np.full(len(s), (np.uint64(PRED_CLASS) << np.uint64(56)) | np.uint64(preds.index(p)), np.uint64))
+        O.append(o)
+    S, P, O = np.concatenate(S), np.concatenate(P), np.concatenate(O)
+    # interleave the triples' terms -> ids in first-seen order
+    allk = np.stack([S, P, O], axis=1).reshape(-1)
+    uniq, first, inv = np.unique(allk, return_index=True, return_inverse=True)
+    rank_of = np.empty(len(uniq), np.int64)
+    rank_of[np.argsort(first, kind="stable")] = np.arange(len(uniq))
+    ids_all = rank_of[inv].astype(np.uint32).reshape(-1, 3)
+    ids: Dict[str, int] = {}
+    for i, p in enumerate(preds):
+        k = (np.uint64(PRED_CLASS) << np.uint64(56)) | np.uint64(i)
+        ids[watdiv_iri(p)] = int(rank_of[np.searchsorted(uniq, k)])
+    for c, named in WATDIV_POPULAR.items():
+        for x in named:
+            k = key(cls_id[c], 0, np.array([x]))[0]
+            at = np.searchsorted(uniq, k)
+            if at < len(uniq) and uniq[at] == k:
+                ids[watdiv_iri("wsdbm:" + c + str(x))] = int(rank_of[at])
+    return WatDivData(ids_all[:, 0].copy(), ids_all[:, 1].copy(), ids_all[:, 2].copy(), int(len(uniq)), ids, sz)

@@ -48,6 +48,15 @@ pub const KB_BIND_MAX_ARGS: u32 = 16;
 pub const KB_NUMERIC_F64: u32 = 1; pub const KB_NUMERIC_I32: u32 = 2; pub const KB_NUMERIC_APPEND: u32 = 0xFFFF_FFFF;
 #[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbNumericInfo { pub n_ids: u32, pub n_derived: u32, pub n_numeric: u32, pub n_i32: u32, pub n_slow: u32 }
 pub type kb_numeric_info = KbNumericInfo;  // (the header's name, as the declaration below spells it)
+// kb_bgp_execute: up to 16 patterns; kb_bgp_last_plan describes the last call (kb_bgp_route)
+pub const KB_BGP_MAX_PATTERNS: usize = 16;
+pub const KB_BGP_NONE: u32 = 0; pub const KB_BGP_STAR: u32 = 1; pub const KB_BGP_COMPONENTS: u32 = 2;
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbBgpPlanInfo { pub route: u32, pub n_patterns: u32, pub n_components: u32,
+    pub component: [u32; KB_BGP_MAX_PATTERNS], pub acyclic: [u32; KB_BGP_MAX_PATTERNS], pub reduce_rounds: [u32; KB_BGP_MAX_PATTERNS],
+    pub rows_scanned: [u64; KB_BGP_MAX_PATTERNS], pub rows_reduced: [u64; KB_BGP_MAX_PATTERNS], pub join_order: [u32; KB_BGP_MAX_PATTERNS],
+    pub component_rows: [u64; KB_BGP_MAX_PATTERNS], pub component_max_rows: [u64; KB_BGP_MAX_PATTERNS], pub cross_order: [u32; KB_BGP_MAX_PATTERNS],
+    pub reduce_bytes: u64, pub reduce_bit_ops: u64, pub max_intermediate: u64, pub rows_unprojected: u64 }
+pub type kb_bgp_plan_info = KbBgpPlanInfo;  // (the header's name, as the declaration below spells it)
 
 // kb_filter_opcode / kb_cmp / kb_agg_kind / kb_strategy
 pub const KB_F_CMP_NUM: u32 = 1; pub const KB_F_EQ_ID: u32 = 2; pub const KB_F_NE_ID: u32 = 3; pub const KB_F_AND: u32 = 4; pub const KB_F_OR: u32 = 5;
@@ -152,6 +161,7 @@ extern "C" {
     pub fn kb_rel_device_col(r: *const KbRel, col: u32, d_ptr: *mut *const u32) -> kb_status;
     pub fn kb_bgp_execute(ctx: *mut KbCtx, pats: *const KbPattern, n_pats: u32, filter: *const KbFilterOp, n_filter_ops: u32, project_slots: *const u32, n_project: u32,
                           out: *mut *mut KbRel) -> kb_status;
+    pub fn kb_bgp_last_plan(ctx: *mut KbCtx, out: *mut kb_bgp_plan_info) -> kb_status;
     pub fn kb_plan_info(plan: *const KbPlan, ring: *mut u32, capacity_rows: *mut u64, n_cols: *mut u32, slots: *mut u32, grouped: *mut u32) -> kb_status;
     pub fn kb_plan_peer_scratch_bytes(plan: *const KbPlan) -> u64;
     pub fn kb_plan_attach_peers(ctx: *mut KbCtx, plan: *mut KbPlan, rank: u32, world: u32, peer_scratch: *const *mut c_void) -> kb_status;
