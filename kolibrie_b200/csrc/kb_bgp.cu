@@ -270,7 +270,7 @@ kb_status bgp_components(kb_ctx* ctx, const kb_pattern* pats, u32 n_pats, const 
         const u32 m = std::min(n_pats - g, (u32)MAXP);
         std::vector<FilterProg> pd(pushdown.begin() + g, pushdown.begin() + g + m);
         std::vector<std::unique_ptr<kb_rel>> part;
-        KB_TRY(scan_impl(ctx, pats + g, m, pd, false, false, &part));
+        KB_TRY(scan_impl(ctx, ctx->segs, pats + g, m, pd, /*use_index=*/true, false, false, &part));
         for (auto& r : part) rels.push_back(std::move(r));
     }
     const std::vector<std::vector<u32>> comps = kb_bgp::components(pv);

@@ -588,10 +588,7 @@ static kb_status fixpoint_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
             std::vector<FilterProg> none;
             // the predicate relations are append-only buffers with the capacity of a whole-store scan output: take the scan, not the
             // (exactly sized) index slices
-            ctx->in_index_build = true;
-            const kb_status src = scan_impl(ctx, pats, k, none, false, false, &out);
-            ctx->in_index_build = false;
-            KB_TRY(src);
+            KB_TRY(scan_impl(ctx, ctx->segs, pats, k, none, /*use_index=*/false, false, false, &out));
             for (u32 i = 0; i < k; i++) {
                 PredRel& r = fx.rels[preds[b + i]];
                 r.s = out[i]->cols[0];
@@ -684,12 +681,7 @@ static kb_status fixpoint_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
         sg.tag = KB_TAG_INFERRED;
         sg.n = total;
         sg.s = cs; sg.p = cp; sg.o = co;
-        ctx->segs.push_back(sg);
-        ctx->n_triples += total;
-        ctx->store_version++;
-        ctx->multi_valued.clear();
-        ctx->single_valued.clear();
-        ctx->index.clear();
+        KB_TRY(store_add_device_segment(ctx, sg, /*keep_index=*/false));  // (no statistics pass over the closure)
     }
     tr.mark(ctx, "result assembly", total);
     cudaEventRecord(ev1, ctx->st);
@@ -855,22 +847,13 @@ kb_status split_segments(kb_ctx* ctx, const std::vector<u32>& preds, const std::
     for (auto& sg : ctx->segs) if (which(sg)) { part.push_back(sg); n += sg.n; }
     for (u32 p : preds) (*out)[p] = Pairs{};
     if (n == 0 || preds.empty()) return KB_OK;
-    struct Swap {  // the scan reads ctx->segs: it sees the selected segments, and the store is whole again on every return path
-        kb_ctx* c;
-        std::vector<Segment> segs;
-        u64 n;
-        ~Swap() { c->segs.swap(segs); c->n_triples = n; c->in_index_build = false; }
-    } sw{ctx, std::move(part), ctx->n_triples};
-    ctx->segs.swap(sw.segs);
-    ctx->n_triples = n;
-    ctx->in_index_build = true;  // read the segments themselves, not the index
     for (size_t b = 0; b < preds.size(); b += MAXP) {
         const u32 k = (u32)std::min<size_t>(MAXP, preds.size() - b);
         kb_pattern pats[MAXP];
         for (u32 i = 0; i < k; i++) { pats[i].s = kb_term{1, 0}; pats[i].p = kb_term{0, preds[b + i]}; pats[i].o = kb_term{1, 1}; }
         std::vector<std::unique_ptr<kb_rel>> res;
         std::vector<FilterProg> none;
-        KB_TRY(scan_impl(ctx, pats, k, none, false, false, &res));
+        KB_TRY(scan_impl(ctx, part, pats, k, none, /*use_index=*/false, false, false, &res));
         for (u32 i = 0; i < k; i++) {
             Pairs& p = (*out)[preds[b + i]];
             p.s = res[i]->cols[0];
@@ -1261,29 +1244,12 @@ static kb_status maintain_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
     // ---- rewrite the store, the index maintained in place (kb_store_evict / kb_store_append_device do the same). A failure from here on
     // leaves exactly the B' segments, no inferred segment, no kept state and no token: kb_datalog_fixpoint restores the precondition.
     auto drop_inferred = [&]() {
-        for (size_t i = 0; i < ctx->segs.size();) {
-            if (ctx->segs[i].tag == KB_TAG_INFERRED) { ctx->n_triples -= ctx->segs[i].n; ctx->segs.erase(ctx->segs.begin() + i); }
-            else i++;
-        }
-        ctx->store_version++;
-        ctx->index.clear();
-        ctx->index_version = ~0ull;
+        store_evict_tag(ctx, KB_TAG_INFERRED, /*keep_index=*/false);
         ctx->closed.reset();
     };
     std::vector<u64> gone(evict.begin(), evict.end());
     if (rewrite) gone.push_back(KB_TAG_INFERRED);
-    for (u64 t : gone) {
-        for (size_t i = 0; i < ctx->segs.size();) {
-            if (ctx->segs[i].tag == t) { ctx->n_triples -= ctx->segs[i].n; ctx->segs.erase(ctx->segs.begin() + i); }
-            else i++;
-        }
-        const bool maintain = ctx->index_maintain && ctx->index_version == ctx->store_version && !ctx->index.empty();
-        ctx->store_version++;
-        ctx->multi_valued.clear();
-        ctx->single_valued.clear();
-        if (maintain && index_evict_tag(ctx, t) == KB_OK) ctx->index_version = ctx->store_version;
-        else { ctx->index.clear(); ctx->index_version = ~0ull; }
-    }
+    for (u64 t : gone) store_evict_tag(ctx, t, /*keep_index=*/true);
     if (add) {
         const kb_status rc = store_add_device_segment(ctx, sa);
         if (rc != KB_OK) { drop_inferred(); return rc; }

@@ -170,6 +170,8 @@ struct kb_ctx {
     cudaEvent_t ev_copy = nullptr;
     std::string err;
     std::shared_ptr<kb::Life> life = std::make_shared<kb::Life>();
+    // the store: written only by kb_store.cu (store_replace, store_add_device_segment, store_evict_tag), like store_version, the two
+    // hint sets and the index below
     std::vector<kb::Segment> segs;
     kb::u64 n_triples = 0;
     kb::Buf num, isnum;
@@ -242,8 +244,6 @@ struct kb_ctx {
     kb::u64 derive_bucket_slack = 8192;  // KOLIBRIE_DERIVE_SLACK: rows a bucket holds beyond 9/8 of its fair share
     bool fast_index_kernel = true;       // KOLIBRIE_INDEX_KERNEL=0: index joins go through the generic probe kernel (A/B switch)
     bool use_index = true;               // KOLIBRIE_USE_INDEX=0 / kb_set_use_index: force the scanning path
-    bool in_index_build = false;         // scan_impl must read the store itself (index build in progress / remaining patterns of a mixed scan)
-    bool in_full_index_build = false;
     bool probe_table_mode = true;        // KOLIBRIE_PROBE_TABLE=0: the index probe always streams the slice (A/B switch)
     bool index_maintain = true;          // KOLIBRIE_INDEX_MAINTAIN=0: append / evict drop the index instead of maintaining it (A/B switch)
     kb::u32 shard_rank = 0, shard_world = 1;  // kb_set_sharding: the store is shard `rank` of `world`, sharded by subject
@@ -300,7 +300,6 @@ kb_status validate_filter(kb_ctx* ctx, const kb_filter_op* ops, u32 n);
 bool split_conjuncts(const kb_filter_op* ops, u32 n, std::vector<FilterProg>* out);
 std::set<u32> filter_slots(const FilterProg& f);
 
-// pairs=true: 2-variable (?s P ?o)-shaped patterns are emitted as interleaved (s,o) pair relations (internal fast path)
 struct ScanTable {  // scan+build fusion: pattern k inserts its matches into this direct table instead of emitting rows
     u32* tab = nullptr;
     u32 kmin = 0, range = 0;  // compacted key space when cshift != 0
@@ -309,8 +308,13 @@ struct ScanTable {  // scan+build fusion: pattern k inserts its matches into thi
     u32* dup_flag = nullptr;
     bool clear = false;  // the table has not been set to 0xFF yet: scan_impl clears it (inside the scan kernel when it can)
 };
-kb_status scan_impl(kb_ctx* ctx, const kb_pattern* pats, u32 n_pats, const std::vector<FilterProg>& pushdown, bool want_index, bool pairs,
-                    std::vector<std::unique_ptr<kb_rel>>* out, const std::vector<ScanTable>* tables = nullptr);
+// One fused scan of `segs` (the store, ctx->segs, or segments a caller selected or built) for up to MAXP patterns.
+// use_index: patterns the store index answers are looked up instead of scanned; only a scan of ctx->segs itself without row_index,
+// pairs or tables does that. row_index: every pattern emits the row positions of its matches. pairs: 2-variable (?s P ?o)-shaped
+// patterns are emitted as interleaved (s,o) pair relations (internal fast path).
+kb_status scan_impl(kb_ctx* ctx, const std::vector<Segment>& segs, const kb_pattern* pats, u32 n_pats, const std::vector<FilterProg>& pushdown,
+                    bool use_index, bool row_index, bool pairs, std::vector<std::unique_ptr<kb_rel>>* out,
+                    const std::vector<ScanTable>* tables = nullptr);
 // fused GROUP BY of a star join (kb_star_join_aggregate): in = group / aggregate spec; out = groups when the one-kernel index path took it
 struct AggSpec {
     AggSpec() = default;
@@ -366,9 +370,16 @@ void groups_from_host_table(const char* hb, const GroupTable& t, u32 n_group, co
 // the same from a dense record list (launch_group_compact)
 void groups_from_records(const GroupRecord* recs, u64 n, u32 n_group, const kb_agg* aggs, u32 n_aggs, kb_groups* g);
 kb_status segment_stats(kb_ctx* ctx, Segment* sg);
-kb_status index_add_segment(kb_ctx* ctx, size_t seg_idx, bool* indexable);
-kb_status index_evict_tag(kb_ctx* ctx, u64 tag);
-kb_status store_add_device_segment(kb_ctx* ctx, Segment& sg);
+// Changes to the store (kb_store.cu). Each one bumps store_version, which voids what is keyed to it (prepared plans, the seeded
+// fixpoint's state, the closed token), and clears the hint sets.
+// the store becomes `segs`; the index is dropped
+void store_replace(kb_ctx* ctx, std::vector<Segment> segs);
+// a segment whose columns are already in HBM joins the store. keep_index: its statistics are computed (if it has none) and the index is
+// maintained when it describes the store (else dropped); false: the segment joins as it is and the index is dropped
+kb_status store_add_device_segment(kb_ctx* ctx, Segment& sg, bool keep_index = true);
+// the segments tagged `tag` leave the store; keep_index: the index is maintained when it describes the store (else dropped).
+// Returns whether a segment carried the tag.
+bool store_evict_tag(kb_ctx* ctx, u64 tag, bool keep_index);
 kb_status unpair_rel(kb_ctx* ctx, std::unique_ptr<kb_rel>* r);
 kb_status filter_impl(kb_ctx* ctx, const kb_rel& in, const FilterProg& f, std::unique_ptr<kb_rel>* out);
 kb_status hash_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_rel& R, const FilterProg* post, std::unique_ptr<kb_rel>* out);

@@ -16,9 +16,7 @@ static kb_ctx* g_legacy_ctx = nullptr;
 static kb_status legacy_select(kb_ctx* ctx, const u32* h_p, const u32* h_o, u32 n, u32 pred, const u32* literal, u32** out_idx, u32* out_n) {
     KB_TRY(begin_call(ctx));
     ctx->ordered = 1;  // the legacy contract returns ascending indices
-    ctx->segs.clear();
-    ctx->n_triples = 0;
-    Segment sg;
+    Segment sg;  // scanned on its own: the context's store is not involved
     sg.n = n;
     KB_TRY(alloc_col(ctx, n, &sg.p));
     KB_CUDA(ctx, cudaMemcpyAsync(sg.p.ptr, h_p, (size_t)n * sizeof(u32), cudaMemcpyHostToDevice, ctx->st));
@@ -30,15 +28,13 @@ static kb_status legacy_select(kb_ctx* ctx, const u32* h_p, const u32* h_o, u32 
         sg.o = sg.p;
     }
     ctx->stats.h2d_bytes += (literal ? 2ull : 1ull) * n * sizeof(u32);
-    ctx->segs.push_back(sg);
-    ctx->n_triples = n;
     kb_pattern pt;
     pt.s = kb_term{1, 0};
     pt.p = kb_term{0, pred};
     pt.o = literal ? kb_term{0, *literal} : kb_term{1, 1};
     std::vector<std::unique_ptr<kb_rel>> rels;
     std::vector<FilterProg> none;
-    KB_TRY(scan_impl(ctx, &pt, 1, none, /*want_index=*/true, false, &rels));
+    KB_TRY(scan_impl(ctx, {sg}, &pt, 1, none, /*use_index=*/false, /*row_index=*/true, false, &rels));
     const u64 m = rels[0]->n;
     u32* idx = static_cast<u32*>(malloc(std::max<size_t>(m * sizeof(u32), 4)));
     if (!idx) return fail(ctx, KB_E_OOM, "malloc failed");
@@ -49,8 +45,6 @@ static kb_status legacy_select(kb_ctx* ctx, const u32* h_p, const u32* h_o, u32 
     }
     *out_idx = idx;
     *out_n = (u32)m;
-    ctx->segs.clear();
-    ctx->n_triples = 0;
     return KB_OK;
 }
 
