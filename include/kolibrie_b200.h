@@ -350,7 +350,9 @@ KB_API void kb_rel_free(kb_ctx* ctx, kb_rel* r);
  * pushdown[k] (nullable) is a filter program over pattern k's own variables applied while scanning. */
 KB_API kb_status kb_scan(kb_ctx* ctx, const kb_pattern* pats, uint32_t n_pats,
                          const kb_filter_op* const* pushdown, const uint32_t* pushdown_len, kb_rel** out);
-/* Filter (engine.rs:73-85) */
+/* Filter (engine.rs:73-85). A KB_ID_NONE cell is a variable the row leaves unbound (kb_bind, kb_natural_join, a ragged InMemoryBuffer):
+ * as in types.rs:126-183, KB_F_CMP_NUM, KB_F_EQ_ID, KB_F_NE_ID and KB_F_IS_TRIPLE over it are false, KB_F_PUSH_VAR pushes an invalid
+ * operand (so the arithmetic and its KB_F_TRUTHY are false), and KB_F_NOT inverts each of these. */
 KB_API kb_status kb_filter(kb_ctx* ctx, const kb_rel* in, const kb_filter_op* prog, uint32_t n_ops, kb_rel** out);
 /* Projection — bag semantics, duplicates kept (engine.rs:86-106); zero-copy */
 KB_API kb_status kb_project(kb_ctx* ctx, const kb_rel* in, const uint32_t* slots, uint32_t n_slots, kb_rel** out);

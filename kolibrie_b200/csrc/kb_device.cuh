@@ -324,16 +324,18 @@ static __device__ __noinline__ bool eval_filter_general(const FilterOp* ops, u32
     for (u32 i = 0; i < n_ops; i++) {
         const FilterOp op = ops[i];
         switch (op.op) {
-            case KB_F_CMP_NUM: st[sp] = cmp_num(op.cmp, num_of(nt, vals[op.slot]), op.value) ? 1.0 : 0.0; okm |= 1u << sp; sp++; break;
+            // a row that leaves the variable unbound (KB_ID_NONE, written by kb_bind, kb_natural_join or a ragged InMemoryBuffer) fails
+            // every comparison, != included (types.rs:128, :143-145): its NOT is true
+            case KB_F_CMP_NUM: st[sp] = (vals[op.slot] != EMPTY32 && cmp_num(op.cmp, num_of(nt, vals[op.slot]), op.value)) ? 1.0 : 0.0; okm |= 1u << sp; sp++; break;
             case KB_F_EQ_ID: st[sp] = (op.id != EMPTY32 && vals[op.slot] == op.id) ? 1.0 : 0.0; okm |= 1u << sp; sp++; break;
-            case KB_F_NE_ID: st[sp] = (op.id == EMPTY32 || vals[op.slot] != op.id) ? 1.0 : 0.0; okm |= 1u << sp; sp++; break;
+            case KB_F_NE_ID: st[sp] = (vals[op.slot] != EMPTY32 && (op.id == EMPTY32 || vals[op.slot] != op.id)) ? 1.0 : 0.0; okm |= 1u << sp; sp++; break;
             case KB_F_AND: sp--; st[sp - 1] = (st[sp - 1] != 0.0 && st[sp] != 0.0) ? 1.0 : 0.0; break;
             case KB_F_OR: sp--; st[sp - 1] = (st[sp - 1] != 0.0 || st[sp] != 0.0) ? 1.0 : 0.0; break;
             case KB_F_NOT: st[sp - 1] = (st[sp - 1] == 0.0) ? 1.0 : 0.0; break;
             case KB_F_PUSH_VAR: {
                 u32 id = vals[op.slot];
                 st[sp] = num_of(nt, id);
-                if (isnum_of(nt, id)) okm |= 1u << sp; else okm &= ~(1u << sp);
+                if (id != EMPTY32 && isnum_of(nt, id)) okm |= 1u << sp; else okm &= ~(1u << sp);  // unbound: the resolver's `?` (types.rs:161)
                 sp++;
             } break;
             case KB_F_PUSH_CONST: st[sp] = op.value; okm |= 1u << sp; sp++; break;
@@ -349,7 +351,7 @@ static __device__ __noinline__ bool eval_filter_general(const FilterOp* ops, u32
                 if (v) okm |= 1u << (sp - 1); else okm &= ~(1u << (sp - 1));
             } break;
             case KB_F_TRUTHY: st[sp - 1] = (((okm >> (sp - 1)) & 1u) && st[sp - 1] != 0.0) ? 1.0 : 0.0; okm |= 1u << (sp - 1); break;
-            case KB_F_IS_TRIPLE: st[sp] = (vals[op.slot] & 0x80000000u) ? 1.0 : 0.0; okm |= 1u << sp; sp++; break;
+            case KB_F_IS_TRIPLE: st[sp] = (vals[op.slot] != EMPTY32 && (vals[op.slot] & 0x80000000u)) ? 1.0 : 0.0; okm |= 1u << sp; sp++; break;  // types.rs:172-176
             case KB_F_CMP_LEGACY: {  // sparql_database.rs:1420-1620: i32 comparison when both sides are integers, else string equality
                 const u32 id = vals[op.slot];
                 const u32 cmp = op.cmp & 0xFFu;
@@ -377,8 +379,8 @@ static __device__ __noinline__ bool eval_filter_general(const FilterOp* ops, u32
 
 __device__ __forceinline__ bool eval_filter(const FilterOp* ops, u32 n_ops, const u32* vals, const NumTab& nt) {
     if (n_ops == 0) return true;
-    if (n_ops == 1 && ops[0].op == KB_F_CMP_NUM)  // FILTER(?x > c): the common case, no stack machine
-        return cmp_num(ops[0].cmp, num_of(nt, vals[ops[0].slot]), ops[0].value);
+    if (n_ops == 1 && ops[0].op == KB_F_CMP_NUM)  // FILTER(?x > c): the common case, no stack machine; unbound is false
+        return vals[ops[0].slot] != EMPTY32 && cmp_num(ops[0].cmp, num_of(nt, vals[ops[0].slot]), ops[0].value);
     return eval_filter_general(ops, n_ops, vals, nt);
 }
 

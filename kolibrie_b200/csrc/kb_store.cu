@@ -588,12 +588,9 @@ kb_status kb_store_delete(kb_ctx* ctx, const uint32_t* s, const uint32_t* p, con
     KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
     kb_pattern pt{{1, 0}, {1, 1}, {1, 2}};
     kb::FilterProg keep;
-    kb_filter_op tr{};
-    tr.op = KB_F_IS_TRIPLE; tr.slot = 1;  // marked predicates (0xFFFFFFFF) have bit 31 set; real predicate ids never do
-    kb_filter_op nt{};
-    nt.op = KB_F_NOT;
-    keep.ops.push_back(tr);
-    keep.ops.push_back(nt);
+    kb_filter_op ne{};
+    ne.op = KB_F_NE_ID; ne.slot = 1; ne.id = KB_ID_NONE;  // true for every bound predicate; a marked one reads as unbound: false
+    keep.ops.push_back(ne);
     const std::vector<kb::FilterProg> pd{keep};
     // the new segments are built aside: the store changes only when all of them are (a failure leaves it as it was)
     std::vector<kb::Segment> kept;

@@ -128,7 +128,8 @@ bool eval_filter(const kb_filter_op* ops, u32 n_ops, const NumTable& nt, F&& val
         const kb_filter_op& op = ops[i];
         switch (op.op) {
             case KB_F_CMP_NUM: {
-                double a = nt.num(val(op.slot)), b = op.value;
+                const u32 id = val(op.slot);
+                double a = nt.num(id), b = op.value;
                 bool r = false;
                 switch (op.cmp) {  // types.rs:133-148
                     case KB_CMP_GT: r = a > b; break;
@@ -137,14 +138,14 @@ bool eval_filter(const kb_filter_op* ops, u32 n_ops, const NumTable& nt, F&& val
                     case KB_CMP_LE: r = a <= b; break;
                     default: r = false;
                 }
-                st[sp] = r; ok[sp++] = true;
+                st[sp] = r && id != KB_ID_NONE; ok[sp++] = true;  // an unbound variable fails every comparison (types.rs:143-145)
             } break;
             case KB_F_EQ_ID: st[sp] = (op.id != KB_ID_NONE && val(op.slot) == op.id); ok[sp++] = true; break;  // types.rs:131
-            case KB_F_NE_ID: st[sp] = (op.id == KB_ID_NONE || val(op.slot) != op.id); ok[sp++] = true; break;  // types.rs:132
+            case KB_F_NE_ID: st[sp] = val(op.slot) != KB_ID_NONE && (op.id == KB_ID_NONE || val(op.slot) != op.id); ok[sp++] = true; break;  // types.rs:132, :143-145
             case KB_F_AND: sp--; st[sp - 1] = (st[sp - 1] != 0.0 && st[sp] != 0.0); break;
             case KB_F_OR: sp--; st[sp - 1] = (st[sp - 1] != 0.0 || st[sp] != 0.0); break;
             case KB_F_NOT: st[sp - 1] = (st[sp - 1] == 0.0); break;
-            case KB_F_PUSH_VAR: { u32 id = val(op.slot); st[sp] = nt.num(id); ok[sp++] = nt.isnum(id); } break;  // types.rs:163-167
+            case KB_F_PUSH_VAR: { u32 id = val(op.slot); st[sp] = nt.num(id); ok[sp++] = id != KB_ID_NONE && nt.isnum(id); } break;  // types.rs:159-163
             case KB_F_PUSH_CONST: st[sp] = op.value; ok[sp++] = true; break;
             case KB_F_ADD: sp--; st[sp - 1] = st[sp - 1] + st[sp]; ok[sp - 1] = ok[sp - 1] && ok[sp]; break;
             case KB_F_SUB: sp--; st[sp - 1] = st[sp - 1] - st[sp]; ok[sp - 1] = ok[sp - 1] && ok[sp]; break;
@@ -156,7 +157,7 @@ bool eval_filter(const kb_filter_op* ops, u32 n_ops, const NumTable& nt, F&& val
                 ok[sp - 1] = v;
             } break;
             case KB_F_TRUTHY: st[sp - 1] = (ok[sp - 1] && st[sp - 1] != 0.0); ok[sp - 1] = true; break;  // types.rs:168
-            case KB_F_IS_TRIPLE: st[sp] = (val(op.slot) & 0x80000000u) != 0; ok[sp++] = true; break;     // types.rs:170-183
+            case KB_F_IS_TRIPLE: st[sp] = val(op.slot) != KB_ID_NONE && (val(op.slot) & 0x80000000u) != 0; ok[sp++] = true; break;  // types.rs:167-176
             default: return false;
         }
     }

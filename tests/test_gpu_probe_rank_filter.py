@@ -9,6 +9,7 @@ import pytest
 
 from kolibrie_b200 import capi as c
 from kolibrie_b200 import datagen
+from tests import filter_cases as FC
 from tests import oracle_api as O
 
 pytestmark = pytest.mark.gpu
@@ -23,16 +24,8 @@ E = 2000         # employees per segment
 # (range <= 4 rows + 65 536) for the tables to be rebuilt rather than dropped
 REBUILD_GAP = 72_000
 
-INF = np.inf
-DMIN = np.nextafter(0.0, 1.0)
-BASE = [0.0, -0.0, INF, -INF, np.nan, np.copysign(np.nan, -1.0), DMIN, -DMIN, 2 * DMIN, 2.2250738585072014e-308, -2.2250738585072014e-308,
-        np.nextafter(2.2250738585072014e-308, 0.0), 1.7976931348623157e308, -1.7976931348623157e308, 1.0, -1.0, 0.5, 100000.0, 99999.5,
-        -100000.0, 3.0]
-with np.errstate(over="ignore"):  # (the neighbours of +-DBL_MAX are +-inf)
-    VALUES = np.array(BASE + [np.nextafter(x, INF) for x in BASE] + [np.nextafter(x, -INF) for x in BASE], dtype=np.float64)
+VALUES, CONSTS = FC.VALUES, FC.CONSTS
 N_IDS = LIT0 + len(VALUES) + N_PLAIN
-CONSTS = [0.0, -0.0, INF, -INF, np.nan, DMIN, -DMIN, 100000.0, np.nextafter(100000.0, INF), np.nextafter(100000.0, -INF), 99999.75, 2.5,
-          -1.7976931348623157e308, 1.7976931348623157e308, np.nextafter(0.0, -1.0)]
 CMPS = [c.CMP_GT, c.CMP_GE, c.CMP_LT, c.CMP_LE]
 
 
