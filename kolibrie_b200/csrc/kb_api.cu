@@ -252,18 +252,8 @@ std::set<u32> filter_slots(const FilterProg& f) {
     return s;
 }
 
-// AND the program `f` into `dst`
-static void and_into(FilterProg* dst, const FilterProg& f) {
-    if (f.ops.empty()) return;
-    const bool had = !dst->ops.empty();
-    dst->ops.insert(dst->ops.end(), f.ops.begin(), f.ops.end());
-    if (had) { kb_filter_op a{}; a.op = KB_F_AND; dst->ops.push_back(a); }
-}
-
-// a program over the variables `slots` as device ops: variable slots[i] is read from column i of the kernel's row, or from position
-// (*pos)[i] (0 s, 1 p, 2 o) of a pattern's triple
-static kb_status compile_prog(kb_ctx* ctx, const FilterProg& f, const std::vector<u32>& slots, std::vector<FilterOp>* ops,
-                              const std::vector<u32>* pos = nullptr) {
+kb_status compile_prog(kb_ctx* ctx, const FilterProg& f, const std::vector<u32>& slots, std::vector<FilterOp>* ops,
+                       const std::vector<u32>* pos) {
     ops->clear();
     for (auto& op : f.ops) {
         FilterOp d;
@@ -526,10 +516,6 @@ kb_status scan_impl(kb_ctx* ctx, const std::vector<Segment>& segs, const kb_patt
     KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off_ticket, 0, std::max(n_seg, 1u) * sizeof(u32), ctx->st));
     u64 all_tiles = 0;
     for (auto& sg : segs) all_tiles += (sg.n + SCAN_TILE - 1) / SCAN_TILE;
-    KB_TRY(ensure_tile_state(ctx, all_tiles * 4));  // the star-shape kernel may walk the store in smaller tiles than SCAN_TILE
-    P.tile_state = static_cast<u64*>(ctx->tile_state->p);
-    P.block_state = static_cast<u64*>(ctx->block_state->p);
-    P.ordered = ctx->ordered;
     // One launch walks up to SCAN_MAXSEG consecutive segments (an RSP window is ~10 slides). A segment whose upload is still in
     // flight (chunked kb_star_join_host) closes the group before it, so the scan of the chunks that already landed can start.
     u64 index_base = 0;
@@ -567,8 +553,8 @@ kb_status scan_impl(kb_ctx* ctx, const std::vector<Segment>& segs, const kb_patt
             P.totals_in = P.totals_out = ctx->ctrl + off_tot;
         }
         n_launched++;
-        P.epoch = ctx->epoch++;
-        if (ctx->epoch >= (1ull << 30)) ctx->epoch = 1;
+        // (the star-shape kernel may walk the store in smaller tiles than SCAN_TILE)
+        KB_TRY(compact_setup(ctx, all_tiles * 4, nullptr, &P.c));
         P.n_clear = 0;
         if (!pending_clear.empty()) {
             if (pending_clear.size() <= 4 && scan_clears_tables(P)) {
@@ -598,1077 +584,10 @@ kb_status scan_impl(kb_ctx* ctx, const std::vector<Segment>& segs, const kb_patt
     return KB_OK;
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// filter (= probe kernel with zero tables)
-
-// what every probe launch shares: the output columns (`ocs`, n rows each, appended to res->cols), the FILTER over them, tile state,
-// control words {ticket, total, zero} and a fresh epoch
-template <class Params>
-static kb_status probe_setup(kb_ctx* ctx, Params* P, u64 n, const std::vector<OutCol>& ocs, const std::vector<FilterOp>& fops, u32* ctrl,
-                             const u32* abort_flag, kb_rel* res) {
-    P->n_out = (u32)ocs.size();
-    for (u32 c = 0; c < P->n_out; c++) {
-        Col col;
-        KB_TRY(alloc_col(ctx, n, &col));
-        res->cols.push_back(col);
-        P->oc[c] = ocs[c];
-        P->out[c] = col.ptr;
-    }
-    P->cap = (u32)n;
-    P->n_ops = (u32)fops.size();
-    for (size_t i = 0; i < fops.size(); i++) P->ops[i] = fops[i];
-    P->nt = numtab(ctx);
-    KB_TRY(ensure_tile_state(ctx, P->n_tiles));
-    P->tile_state = static_cast<u64*>(ctx->tile_state->p);
-    P->block_state = static_cast<u64*>(ctx->block_state->p);
-    P->ordered = ctx->ordered;
-    P->ticket = ctrl;
-    P->total = ctrl + 1;
-    P->zero_word = ctrl + 2;
-    P->abort_flag = abort_flag;
-    P->epoch = ctx->epoch++;
-    return KB_OK;
-}
-
-kb_status filter_impl(kb_ctx* ctx, const kb_rel& in, const FilterProg& f, std::unique_ptr<kb_rel>* out) {
-    auto rel = std::make_unique<kb_rel>();
-    rel->slots = in.slots;
-    if (in.n == 0 || f.ops.empty()) {
-        rel->cols = in.cols;
-        rel->n = in.n;
-        *out = std::move(rel);
-        return KB_OK;
-    }
-    if (in.n >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "relation too large");
-    ProbeDParams P{};
-    P.n_pcols = (u32)in.cols.size();
-    if (P.n_pcols == 0) return fail(ctx, KB_E_UNSUPPORTED, "filter on a relation without columns");
-    P.n = (u32)in.n;  // key_col 0, T = 0 tables
-    P.n_tiles = (u32)((in.n + PROBE_TILE - 1) / PROBE_TILE);
-    std::vector<OutCol> ocs;
-    for (u32 c = 0; c < P.n_pcols; c++) {
-        P.pcol[c] = in.cols[c].ptr;
-        ocs.push_back(OutCol{OUT_PROBE, c, 0});
-    }
-    std::vector<FilterOp> ops;
-    KB_TRY(compile_prog(ctx, f, in.slots, &ops));
-    const u32 off = ctrl_alloc(ctx, 4);
-    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, 4 * sizeof(u32), ctx->st));
-    KB_TRY(probe_setup(ctx, &P, in.n, ocs, ops, ctx->ctrl + off, nullptr, rel.get()));
-    timer_begin(ctx, F_FILTER);
-    launch_probe_direct(P, ctx->n_sms, ctx->st);
-    timer_end(ctx);
-    KB_CUDA(ctx, cudaGetLastError());
-    KB_TRY(ctrl_read(ctx));
-    rel->n = ctx->h_ctrl[off + 1];
-    *out = std::move(rel);
-    return KB_OK;
-}
-
 u32 pow2_at_least(u64 x) {
     u64 p = 1024;
     while (p < x) p <<= 1;
     return (u32)std::min<u64>(p, 1ull << 31);
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// general natural join (chained multimap)
-kb_status hash_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_rel& R, const FilterProg* post, std::unique_ptr<kb_rel>* out) {
-    auto rel = std::make_unique<kb_rel>();
-    rel->slots = L.slots;
-    std::vector<u32> common;
-    for (u32 s : R.slots) {
-        if (L.col_of(s) >= 0) common.push_back(s);
-        else rel->slots.push_back(s);
-    }
-    if (rel->slots.size() > KB_MAX_COLS) return fail(ctx, KB_E_LIMIT, "join result has more than %d columns", KB_MAX_COLS);
-    if (L.n == 0 || R.n == 0) return empty_rel(ctx, rel->slots, out);  // engine.rs:714-716
-    if (L.n >= 0xFFFFFFF0ull || R.n >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "relation too large");
-    if (common.empty()) {  // cartesian product (engine.rs:1054-1071)
-        const u64 total = L.n * R.n;
-        if (total > (1ull << 28)) return fail(ctx, KB_E_LIMIT, "cartesian product of %llu x %llu rows exceeds 2^28", (unsigned long long)L.n, (unsigned long long)R.n);
-        std::vector<const u32*> lc, rc;
-        std::vector<u32*> oc;
-        for (auto& c : L.cols) lc.push_back(c.ptr);
-        for (auto& c : R.cols) rc.push_back(c.ptr);
-        for (size_t c = 0; c < rel->slots.size(); c++) { Col col; KB_TRY(alloc_col(ctx, total, &col)); rel->cols.push_back(col); oc.push_back(col.ptr); }
-        timer_begin(ctx, F_PROBE);
-        launch_cartesian(lc.data(), (u32)L.n, (u32)lc.size(), rc.data(), (u32)R.n, (u32)rc.size(), oc.data(), ctx->st);
-        timer_end(ctx);
-        KB_CUDA(ctx, cudaGetLastError());
-        rel->n = total;
-        if (post && !post->ops.empty()) {
-            std::unique_ptr<kb_rel> f;
-            KB_TRY(filter_impl(ctx, *rel, *post, &f));
-            rel = std::move(f);
-        }
-        *out = std::move(rel);
-        return KB_OK;
-    }
-    if (common.size() > 4) return fail(ctx, KB_E_LIMIT, "join on more than 4 common variables");
-    const bool build_left = L.n <= R.n;  // engine.rs:729-733: build on the smaller side
-    const kb_rel& B = build_left ? L : R;
-    const kb_rel& Pr = build_left ? R : L;
-
-    // ---- grouped (CSR) join: one key column with a dense id range and no join filter
-    if (ctx->csr_join && common.size() == 1 && (!post || post->ops.empty())) {
-        const u32* bk = B.cols[B.col_of(common[0])].ptr;
-        const u32 off = ctrl_alloc(ctx, 8);  // [0] min, [1] max, [2..3] u64 output rows, [4] ticket, [5] total, [6] zero, [7] heavy tiles
-        KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0xFF, sizeof(u32), ctx->st));
-        KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off + 1, 0, 7 * sizeof(u32), ctx->st));
-        timer_begin(ctx, F_BUILD);
-        launch_col_minmax(bk, (u32)B.n, ctx->ctrl + off, ctx->ctrl + off + 1, ctx->n_sms, ctx->st);
-        timer_end(ctx);
-        KB_TRY(ctrl_read(ctx));
-        const u32 kmin = ctx->h_ctrl[off], kmax = ctx->h_ctrl[off + 1];
-        const u64 range = (u64)kmax - kmin + 1;
-        if (kmax >= kmin && range <= std::max<u64>(16 * B.n, 1ull << 20) && range < (1ull << 31)) {
-            Buf dir, cursor, scratch;
-            KB_TRY(alloc_buf(ctx, (range + 1) * sizeof(u32), &dir));
-            KB_TRY(alloc_buf(ctx, range * sizeof(u32), &cursor));
-            KB_TRY(alloc_buf(ctx, ((range + 1) / 2048 + 4) * sizeof(u32), &scratch));
-            CsrTab tab{};
-            tab.off = static_cast<const u32*>(dir->p);
-            tab.kmin = kmin;
-            tab.range = (u32)range;
-            std::vector<u32> kernel_slots = Pr.slots;  // kernel output order: probe columns, then build payload columns
-            std::vector<const u32*> pay_in;
-            std::vector<u32*> pay_out;
-            std::vector<Col> pay_cols;
-            for (size_t c = 0; c < B.slots.size(); c++) {
-                if (B.slots[c] == common[0]) continue;
-                Col pc;
-                KB_TRY(alloc_col(ctx, B.n, &pc));
-                pay_cols.push_back(pc);
-                pay_in.push_back(B.cols[c].ptr);
-                pay_out.push_back(pc.ptr);
-                tab.pay[tab.n_pay++] = pc.ptr;
-                kernel_slots.push_back(B.slots[c]);
-            }
-            timer_begin(ctx, F_BUILD, 5);
-            KB_CUDA(ctx, cudaMemsetAsync(dir->p, 0, (range + 1) * sizeof(u32), ctx->st));
-            launch_csr_count(bk, (u32)B.n, kmin, static_cast<u32*>(dir->p), ctx->n_sms, ctx->st);
-            launch_exclusive_scan_u32(static_cast<u32*>(dir->p), (u32)range + 1, static_cast<u32*>(scratch->p), ctx->st);
-            KB_CUDA(ctx, cudaMemcpyAsync(cursor->p, dir->p, range * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
-            launch_csr_fill(bk, (u32)B.n, kmin, static_cast<u32*>(cursor->p), pay_in.data(), pay_out.data(), tab.n_pay, ctx->n_sms, ctx->st);
-            timer_end(ctx);
-            ctx->stats.rows_built += B.n;
-            const u32* pk = Pr.cols[Pr.col_of(common[0])].ptr;
-            timer_begin(ctx, F_PROBE);
-            launch_csr_total(pk, (u32)Pr.n, tab, reinterpret_cast<unsigned long long*>(ctx->ctrl + off + 2), ctx->n_sms, ctx->st);
-            timer_end(ctx);
-            KB_CUDA(ctx, cudaGetLastError());
-            KB_TRY(ctrl_read(ctx));
-            unsigned long long total = 0;
-            memcpy(&total, ctx->h_ctrl + off + 2, sizeof total);
-            if (total >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "join result of %llu rows exceeds 2^32", total);
-            ProbeGParams G{};
-            G.n_pcols = (u32)Pr.cols.size();
-            G.n = (u32)Pr.n;
-            G.n_tiles = (u32)((Pr.n + PROBEG_TILE - 1) / PROBEG_TILE);
-            for (u32 c = 0; c < G.n_pcols; c++) G.pcol[c] = Pr.cols[c].ptr;
-            G.pkey = (u32)Pr.col_of(common[0]);
-            G.tab = tab;
-            rel->cols.clear();
-            rel->cols.resize(rel->slots.size());
-            for (size_t c = 0; c < kernel_slots.size(); c++) {
-                Col col;
-                KB_TRY(alloc_col(ctx, total, &col));
-                rel->cols[rel->col_of(kernel_slots[c])] = col;
-                G.out[c] = col.ptr;
-            }
-            G.cap = (u32)total;
-            KB_TRY(ensure_tile_state(ctx, G.n_tiles));
-            G.tile_state = static_cast<u64*>(ctx->tile_state->p);
-            G.block_state = static_cast<u64*>(ctx->block_state->p);
-            G.ordered = ctx->ordered;
-            G.ticket = ctx->ctrl + off + 4;
-            G.total = ctx->ctrl + off + 5;
-            G.zero_word = ctx->ctrl + off + 6;
-            G.epoch = ctx->epoch++;
-            Buf heavy;  // tiles whose expansion is spread over the grid by the second launch (skewed keys)
-            if (total > PROBEG_HEAVY) {
-                KB_TRY(alloc_buf(ctx, (size_t)G.n_tiles * sizeof(ProbeGParams::Heavy), &heavy));
-                G.heavy = static_cast<ProbeGParams::Heavy*>(heavy->p);
-                G.heavy_count = ctx->ctrl + off + 7;
-            }
-            ctx->stats.rows_probed += Pr.n;
-            if (total) {
-                timer_begin(ctx, F_PROBE, G.heavy ? 2 : 1);
-                launch_probe_grouped(G, ctx->n_sms, ctx->st);
-                timer_end(ctx);
-                KB_CUDA(ctx, cudaGetLastError());
-            }
-            rel->n = total;
-            // dir / cursor / payload copies are released stream-ordered (cudaFreeAsync on ctx->st), i.e. after the launch above
-            *out = std::move(rel);
-            return KB_OK;
-        }
-    }
-
-    ChainTab T{};
-    T.n_slots = pow2_at_least(B.n * 2);
-    T.n_keys = (u32)common.size();
-    Buf slots_buf, next_buf;
-    KB_TRY(alloc_buf(ctx, (size_t)T.n_slots * sizeof(u64), &slots_buf));
-    KB_TRY(alloc_buf(ctx, (size_t)B.n * sizeof(u32), &next_buf));
-    T.slots = static_cast<u64*>(slots_buf->p);
-    T.next = static_cast<u32*>(next_buf->p);
-    for (u32 q = 0; q < T.n_keys; q++) T.bkey[q] = B.cols[B.col_of(common[q])].ptr;
-    timer_begin(ctx, F_BUILD);
-    KB_CUDA(ctx, cudaMemsetAsync(T.slots, 0xFF, (size_t)T.n_slots * sizeof(u64), ctx->st));
-    launch_build_chained(T, (u32)B.n, ctx->n_sms, ctx->st);
-    timer_end(ctx);
-    ctx->stats.rows_built += B.n;
-
-    ProbeCParams P{};
-    P.tab = T;
-    P.n_pcols = (u32)Pr.cols.size();
-    P.n = (u32)Pr.n;
-    P.n_tiles = (u32)((Pr.n + PROBEC_TILE - 1) / PROBEC_TILE);
-    for (u32 c = 0; c < P.n_pcols; c++) P.pcol[c] = Pr.cols[c].ptr;
-    for (u32 q = 0; q < T.n_keys; q++) P.pkey[q] = (u32)Pr.col_of(common[q]);
-    std::vector<u32> kernel_slots = Pr.slots;  // kernel output order: probe columns, then build payload columns
-    P.n_bpay = 0;
-    for (size_t c = 0; c < B.slots.size(); c++) {
-        if (std::find(common.begin(), common.end(), B.slots[c]) != common.end()) continue;
-        P.bpay[P.n_bpay++] = B.cols[c].ptr;
-        kernel_slots.push_back(B.slots[c]);
-    }
-    P.n_out = (u32)kernel_slots.size();
-    std::vector<FilterOp> ops;
-    if (post) KB_TRY(compile_prog(ctx, *post, kernel_slots, &ops));
-    P.n_ops = (u32)ops.size();
-    for (size_t i = 0; i < ops.size(); i++) P.ops[i] = ops[i];
-    P.nt = numtab(ctx);
-    KB_TRY(ensure_tile_state(ctx, P.n_tiles));
-    P.tile_state = static_cast<u64*>(ctx->tile_state->p);
-    P.block_state = static_cast<u64*>(ctx->block_state->p);
-    P.ordered = ctx->ordered;
-    const u32 off = ctrl_alloc(ctx, 8);  // [0] ticket, [1] total (32-bit positions), [2] zero, [4..5] exact total in 64 bits
-    P.total = ctx->ctrl + off + 1;
-    P.zero_word = ctx->ctrl + off + 2;
-    P.total64 = reinterpret_cast<unsigned long long*>(ctx->ctrl + off + 4);
-    u64 cap = std::max(Pr.n, B.n);
-    ctx->stats.rows_probed += Pr.n;
-    for (int attempt = 0; attempt < 2; attempt++) {
-        rel->cols.clear();
-        rel->cols.resize(rel->slots.size());
-        for (u32 c = 0; c < P.n_out; c++) {
-            Col col;
-            KB_TRY(alloc_col(ctx, cap, &col));
-            rel->cols[rel->col_of(kernel_slots[c])] = col;
-            P.out[c] = col.ptr;
-        }
-        P.cap = (u32)std::min<u64>(cap, 0xFFFFFFF0ull);
-        KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, 8 * sizeof(u32), ctx->st));
-        P.ticket = ctx->ctrl + off;
-        P.epoch = ctx->epoch++;
-        timer_begin(ctx, F_PROBE);
-        launch_probe_chained(P, ctx->n_sms, ctx->st);
-        timer_end(ctx);
-        KB_CUDA(ctx, cudaGetLastError());
-        KB_TRY(ctrl_read(ctx));
-        unsigned long long total = 0;
-        memcpy(&total, ctx->h_ctrl + off + 4, sizeof total);
-        if (total >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "join result of %llu rows exceeds 2^32", total);
-        rel->n = total;
-        if (total <= cap) break;
-        if (attempt == 1) return fail(ctx, KB_E_LIMIT, "join output did not fit after resizing");
-        cap = total;  // the first pass doubled as the exact count
-    }
-    *out = std::move(rel);
-    return KB_OK;
-}
-
-std::unique_ptr<kb_rel> select_cols(const kb_rel& in, const std::vector<u32>& slots) {
-    auto r = std::make_unique<kb_rel>();
-    r->n = in.n;
-    for (u32 s : slots) {
-        int c = in.col_of(s);
-        if (c < 0) continue;
-        r->slots.push_back(s);
-        r->cols.push_back(in.cols[c]);
-    }
-    return r;
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// star join: five routes, tried in this order by star_join_impl
-//   R1 one-kernel index join   every build side is a persistent table of the store index: one probe_index_kernel (fused GROUP BY)
-//   R2 index join with builds  direct tables built from predicate slices, then the fused multiway probe
-//   R3 fused scan + build      the scan fills the direct tables, then the fused multiway probe
-//   R4 scan, then builds       direct tables in batches of at most MAXT per probe launch
-//   R5 chained joins           natural joins on the multimap operator: 1:N keys, quirk Q3, sparse key ranges
-struct StarQuery {  // a star join, validated once: what every route reads
-    u32 join_slot = 0, K = 0;
-    const kb_pattern* pats = nullptr;
-    std::vector<std::vector<u32>> pv, psrc;  // variables of pattern k in order of appearance, and their positions (0 s, 1 p, 2 o)
-    std::vector<u32> all_slots;              // column order of the result
-    std::vector<FilterProg> pushdown;        // FILTER conjuncts over one pattern's variables, evaluated while that pattern is read
-    FilterProg post;                         // the other conjuncts, evaluated on the joined row
-    std::vector<u32> key_pos;                // position of the join variable in pattern k
-    // fast path shape: every pattern binds exactly two variables in subject and object position (the join variable + one more)
-    bool all_pairs = false;
-    // no variable but the join variable occurs in two patterns (quirk Q3: the reference never checks the others — we must, so such
-    // shapes take the natural-join chain)
-    bool only_join_shared = true;
-};
-
-enum class Route { answered, declined, retry };
-
-kb_status split_filter(kb_ctx* ctx, const kb_filter_op* filter, u32 n_ops, const std::vector<std::vector<u32>>& pv,
-                       const std::vector<u32>& all_slots, std::vector<FilterProg>* pushdown, FilterProg* post) {
-    std::vector<FilterProg> conj;
-    if (!split_conjuncts(filter, n_ops, &conj)) return fail(ctx, KB_E_INVALID, "malformed filter program");
-    pushdown->assign(pv.size(), FilterProg{});
-    for (auto& c : conj) {
-        std::set<u32> fs = filter_slots(c);
-        for (u32 s : fs) if (std::find(all_slots.begin(), all_slots.end(), s) == all_slots.end())
-            return fail(ctx, KB_E_UNSUPPORTED, "filter references slot %u which no pattern binds (the reference evaluates it to false, types.rs:149-151)", s);
-        int target = -1;
-        for (size_t k = 0; k < pv.size() && target < 0; k++) {
-            bool all = true;
-            for (u32 s : fs) if (std::find(pv[k].begin(), pv[k].end(), s) == pv[k].end()) all = false;
-            if (all) target = (int)k;
-        }
-        and_into(target >= 0 ? &(*pushdown)[target] : post, c);
-    }
-    return KB_OK;
-}
-
-static kb_status star_query(kb_ctx* ctx, u32 join_slot, const kb_pattern* pats, u32 K, const kb_filter_op* filter, u32 n_ops, StarQuery* q) {
-    if (K == 0 || K > (u32)MAXP) return fail(ctx, KB_E_LIMIT, "a star join takes 1..%d patterns (got %u)", MAXP, K);
-    KB_TRY(validate_filter(ctx, filter, n_ops));
-    q->join_slot = join_slot;
-    q->K = K;
-    q->pats = pats;
-    q->pv.resize(K);
-    q->psrc.resize(K);
-    q->key_pos.resize(K);
-    for (u32 k = 0; k < K; k++) {
-        KB_TRY(check_pattern(ctx, pats[k]));
-        pattern_vars(pats[k], &q->pv[k], &q->psrc[k]);
-        const auto j = std::find(q->pv[k].begin(), q->pv[k].end(), join_slot);
-        if (j == q->pv[k].end()) return fail(ctx, KB_E_INVALID, "star join: pattern %u does not contain the join variable (slot %u)", k, join_slot);
-        q->key_pos[k] = q->psrc[k][j - q->pv[k].begin()];
-        for (u32 s : q->pv[k]) if (std::find(q->all_slots.begin(), q->all_slots.end(), s) == q->all_slots.end()) q->all_slots.push_back(s);
-    }
-    if (q->all_slots.size() > KB_MAX_COLS) return fail(ctx, KB_E_LIMIT, "more than %d variables", KB_MAX_COLS);
-    KB_TRY(split_filter(ctx, filter, n_ops, q->pv, q->all_slots, &q->pushdown, &q->post));
-    q->all_pairs = K >= 2;
-    for (u32 k = 0; k < K; k++) if (!(q->pv[k].size() == 2 && q->psrc[k][0] == 0 && q->psrc[k][1] == 2)) q->all_pairs = false;
-    for (u32 a = 0; a < K; a++)
-        for (u32 b = a + 1; b < K; b++)
-            for (u32 s2 : q->pv[a]) if (s2 != join_slot && std::find(q->pv[b].begin(), q->pv[b].end(), s2) != q->pv[b].end()) q->only_join_shared = false;
-    return KB_OK;
-}
-
-// key range of the join variable over the store, from the load-time column statistics of its segments
-static kb_status store_key_range(kb_ctx* ctx, const StarQuery& q, u32* kmin, u32* kmax) {
-    *kmin = 0xFFFFFFFFu;
-    *kmax = 0;
-    for (auto& sg : ctx->segs) {
-        if (sg.n == 0) continue;
-        if (!sg.has_stats) KB_TRY(segment_stats(ctx, &sg));
-        for (u32 k = 0; k < q.K; k++) { const u32 c = q.key_pos[k]; *kmin = std::min(*kmin, sg.cmin[c]); *kmax = std::max(*kmax, sg.cmax[c]); }
-    }
-    return KB_OK;
-}
-
-// a subject-sharded store (kb_set_sharding) owns every world-th block of ids: subject keys are compacted by this shift so that the
-// tables stay dense. 0 unless every key is a subject and no segment may hold a foreign subject (current_stats: the statistics that
-// say so must have been taken under the current sharding)
-static u32 subject_cshift(const kb_ctx* ctx, const StarQuery& q, bool current_stats) {
-    bool subj = true;
-    for (u32 k = 0; k < q.K; k++) if (q.key_pos[k] != 0) subj = false;
-    for (auto& sg : ctx->segs)
-        if (sg.n && (!sg.sharded_ok || (current_stats && (!sg.has_stats || sg.stats_world != ctx->shard_world)))) subj = false;
-    u32 cshift = 0;
-    const u32 w = ctx->shard_world;
-    if (subj && w > 1 && (w & (w - 1)) == 0) while ((1u << cshift) < w) cshift++;
-    return cshift;
-}
-
-// a persistent table of the store index, looked up like spo[s][P] (subject key) or pos[P][o] (object key)
-static DirectTab persistent_tab(const PredSlice& s, bool key_is_y) {
-    DirectTab D{};
-    D.tab = static_cast<const u32*>(key_is_y ? s.ytab->p : s.xtab->p);
-    D.kmin = key_is_y ? s.ytab_min : s.xtab_min;
-    D.range = key_is_y ? s.ytab_range : s.xtab_range;
-    D.cshift = key_is_y ? 0u : s.tab_cshift;
-    return D;
-}
-
-// the fused multiway probe over pair rows (probe_fast_kernel) against T direct tables; P may carry a pre-filter. The output columns
-// (`ocs`, `n` rows each) are appended to res->cols; the row count lands in ctrl[1]
-static kb_status probe_fast(kb_ctx* ctx, ProbeFParams& P, const uint2* pairs, u64 n, u32 key_is_y, const DirectTab* dt, u32 T,
-                            const std::vector<OutCol>& ocs, const std::vector<FilterOp>& fops, u32* ctrl, const u32* abort_flag, kb_rel* res) {
-    P.pairs = pairs;
-    P.key_is_y = key_is_y;
-    P.n = (u32)n;
-    P.n_tiles = (u32)((n + PROBEF_TILE - 1) / PROBEF_TILE);
-    P.T = T;
-    for (u32 q = 0; q < T; q++) P.tab[q] = dt[q];
-    KB_TRY(probe_setup(ctx, &P, n, ocs, fops, ctrl, abort_flag, res));
-    timer_begin(ctx, F_PROBE);
-    launch_probe_fast(P, ctx->n_sms, ctx->st);
-    timer_end(ctx);
-    KB_CUDA(ctx, cudaGetLastError());
-    ctx->stats.rows_probed += n;
-    return KB_OK;
-}
-
-// what the store index says about a star of (?s P ?o) patterns
-struct IndexSlices {
-    bool shape = false;   // valid index, every pattern (?s P ?o), at most MAXT build sides
-    bool empty = false;   // a pattern's predicate does not occur in the store: the answer is empty
-    bool usable = false;  // every predicate constant and present, the patterns share only the join variable
-    std::vector<const PredSlice*> sl;
-    std::vector<bool> persistent;  // the key column of pattern k has a persistent table in the index: it needs no build
-    bool all_persistent = false;
-    u32 kmin = 0xFFFFFFFFu, kmax = 0, cshift = 0;
-    int probe_k = -1;
-};
-
-static IndexSlices index_slices(const kb_ctx* ctx, const StarQuery& q) {
-    IndexSlices ix;
-    ix.shape = ctx->use_index && ctx->index_version == ctx->store_version && q.all_pairs && q.K - 1 <= (u32)MAXT;
-    if (!ix.shape) return ix;
-    const u32 K = q.K;
-    bool ok = q.only_join_shared, empty = false;
-    ix.sl.assign(K, nullptr);
-    for (u32 k = 0; k < K; k++) {
-        if (q.pats[k].p.is_var) { ok = false; break; }
-        auto it = ctx->index.find(q.pats[k].p.value);
-        if (it == ctx->index.end() || it->second.n == 0) { empty = true; continue; }  // predicate absent from the store
-        ix.sl[k] = &it->second;
-    }
-    ix.empty = ok && empty;
-    ix.usable = ok && !empty;
-    if (!ix.usable) return ix;
-    // key range of the join variable from the slices (its position is the same in every pattern that can take this path)
-    for (u32 k = 0; k < K; k++) {
-        const bool y = q.key_pos[k] == 2;
-        ix.kmin = std::min(ix.kmin, y ? ix.sl[k]->ymin : ix.sl[k]->xmin);
-        ix.kmax = std::max(ix.kmax, y ? ix.sl[k]->ymax : ix.sl[k]->xmax);
-    }
-    ix.cshift = subject_cshift(ctx, q, true);
-    ix.kmin = compact_key(ix.kmin, ix.cshift);
-    ix.kmax = compact_key(ix.kmax, ix.cshift);
-    ix.persistent.resize(K);
-    ix.all_persistent = true;
-    for (u32 k = 0; k < K; k++) {
-        ix.persistent[k] = q.key_pos[k] == 2 ? (bool)ix.sl[k]->ytab : ((bool)ix.sl[k]->xtab && ix.sl[k]->tab_cshift == ix.cshift);
-        if (!ix.persistent[k]) ix.all_persistent = false;
-    }
-    // probe side: prefer a pattern WITHOUT a persistent table (it would need a build), then the smallest slice (fewest lookups);
-    // when builds remain, the classic choice: the largest unfiltered slice probes, filtered sides build
-    int& probe_k = ix.probe_k;
-    if (ix.all_persistent) {
-        // no builds at all: the probe side should be the most selective stream — a pattern that carries its own FILTER (evaluated
-        // on the probe row before any lookup), else the smallest slice
-        for (u32 k = 0; k < K; k++)
-            if (!q.pushdown[k].ops.empty() && q.pushdown[k].ops.size() <= 8 && (probe_k < 0 || ix.sl[k]->n < ix.sl[probe_k]->n)) probe_k = (int)k;
-        if (probe_k < 0) { probe_k = 0; for (u32 k = 1; k < K; k++) if (ix.sl[k]->n < ix.sl[probe_k]->n) probe_k = (int)k; }
-    } else {
-        for (u32 k = 0; k < K; k++) if (q.pushdown[k].ops.empty() && (probe_k < 0 || ix.sl[k]->n > ix.sl[probe_k]->n)) probe_k = (int)k;
-        if (probe_k < 0) { probe_k = 0; for (u32 k = 1; k < K; k++) if (ix.sl[k]->n > ix.sl[probe_k]->n) probe_k = (int)k; }
-    }
-    return ix;
-}
-
-kb_status alloc_index_out(kb_ctx* ctx, u64 rows, u32 n_out, std::vector<Col>* cols) {
-    const size_t stride = round256((size_t)rows * sizeof(u32)) + 256;
-    Buf b;
-    KB_TRY(alloc_buf(ctx, stride * n_out, &b));
-    cols->clear();
-    for (u32 c = 0; c < n_out; c++) {
-        Col col;
-        col.buf = b;
-        col.ptr = reinterpret_cast<u32*>(static_cast<char*>(b->p) + stride * c);
-        cols->push_back(col);
-    }
-    return KB_OK;
-}
-
-kb_status launch_index_rows(kb_ctx* ctx, ProbeIParams& P, const std::vector<Col>& cols) {
-    for (size_t c = 0; c < cols.size(); c++) P.out[c] = cols[c].ptr;
-    P.ordered = ctx->ordered;
-    if (P.ordered) {
-        KB_TRY(ensure_tile_state(ctx, P.n_tiles));
-        P.tile_state = static_cast<u64*>(ctx->tile_state->p);
-        P.block_state = static_cast<u64*>(ctx->block_state->p);
-    }
-    timer_begin(ctx, F_PROBE);
-    launch_probe_index(P, nullptr, ctx->n_sms, ctx->st);
-    timer_end(ctx);
-    KB_CUDA(ctx, cudaGetLastError());
-    return KB_OK;
-}
-
-static kb_status resolve_index_plan(kb_ctx* ctx, const StarQuery& q, const IndexSlices& ix, const AggSpec* agg, IndexPlan* ip) {
-    if (!ix.shape) { ip->why = "it needs a valid store index (kb_store_build_index) and (?s P ?o) patterns"; return KB_OK; }
-    if (ix.empty) { ip->why = "a pattern's predicate does not occur in the store (the answer is empty)"; return KB_OK; }
-    if (!ix.usable || !ix.all_persistent || !ctx->fast_index_kernel || ix.sl[ix.probe_k]->chunks.size() > (size_t)PROBEI_MAXSEG) {
-        ip->why = "every pattern (?s P ?o) over a predicate whose key column has a persistent table in the store index";
-        return KB_OK;
-    }
-    const u32 pk = (u32)ix.probe_k, T = q.K - 1;
-    const PredSlice& PS = *ix.sl[pk];
-    ProbeIParams& P = ip->P;
-    ip->out_slots = q.pv[pk];
-    FilterProg postp = q.post;  // filters of patterns that are not built (every one here) run on the joined row
-    u32 t = 0;
-    for (u32 k = 0; k < q.K; k++) {
-        if (k == pk) continue;
-        const bool y = q.key_pos[k] == 2;
-        P.tab[t++] = persistent_tab(*ix.sl[k], y);
-        and_into(&postp, q.pushdown[k]);
-        ip->out_slots.push_back(q.pv[k][y ? 0 : 1]);
-    }
-    const FilterProg& pf = q.pushdown[pk];
-    if (pf.ops.size() > 8) and_into(&postp, pf);
-    else if (!pf.ops.empty()) {
-        std::vector<FilterOp> fo;  // slots of the probe pattern's own filter -> pair halves (x = subject, y = object)
-        KB_TRY(compile_prog(ctx, pf, q.pv[pk], &fo));
-        const bool typed = PS.typed(ctx->num_version) && fo.size() == 1 && fo[0].op == KB_F_CMP_NUM && fo[0].slot == 1u;
-        if (typed) {
-            P.pre_mode = 1; P.pre_cmp = fo[0].cmp; P.pre_val = fo[0].value;
-        } else {
-            P.pre_mode = 2; P.n_pre = (u32)fo.size();
-            for (size_t i = 0; i < fo.size(); i++) P.pre_ops[i] = fo[i];
-        }
-    }
-    ip->n_out = 2 + T;
-    std::vector<FilterOp> fops;
-    KB_TRY(compile_prog(ctx, postp, ip->out_slots, &fops));
-    P.n_ops = (u32)fops.size();
-    for (size_t i = 0; i < fops.size(); i++) P.ops[i] = fops[i];
-    // table mode: the probe pattern's own subject table is the probe stream (keys ascending whatever the store / id order)
-    const bool tab_mode = ctx->probe_table_mode && !ctx->ordered && ix.persistent[pk] && q.key_pos[pk] == 0 &&
-                          (P.pre_mode != 1u || (PS.xkey && PS.xkey_version == ctx->num_version && ctx->numv_version == ctx->num_version));
-    if (tab_mode) {
-        // walk the slots that can hold a key (smallest to largest live subject), not the table's growth headroom nor the
-        // slots an evicted past has left empty; the first slot stays 128-byte aligned for the bulk loads
-        const u32 lo = ((compact_key(PS.xmin, PS.tab_cshift) - PS.xtab_min) / 32u) * 32u;
-        const u32 hi = std::min<u32>(PS.xtab_range, compact_key(PS.xmax, PS.tab_cshift) - PS.xtab_min + 1u);
-        P.ptab = static_cast<const u32*>(PS.xtab->p) + lo;
-        if (P.pre_mode == 1u) {  // FILTER(?o <cmp> c) on the value becomes a range of its ranks in the value order
-            P.pkey = static_cast<const u32*>(PS.xkey->p) + lo;
-            const kb_nr::Range r = kb_nr::cmp_range(P.pre_cmp, ctx->h_numv.data(), (u32)ctx->h_numv.size(), P.pre_val);
-            P.key_lo = r.lo;
-            P.key_hi = r.hi;
-        }
-        P.ptab_min = PS.xtab_min + lo;
-        P.ptab_range = hi > lo ? hi - lo : 0u;
-        P.ptab_cshift = PS.tab_cshift;
-        P.shard_rank = ctx->shard_rank;
-        P.n_tiles = (u32)(((u64)P.ptab_range + PROBEF_TILE - 1) / PROBEF_TILE);
-    } else {
-        for (auto& ch : PS.chunks) {  // one chunk per store segment: an RSP window of slides is walked in ONE launch
-            if (ch.n == 0) continue;
-            ProbeISeg& g = P.seg[P.n_seg++];
-            g.pairs = reinterpret_cast<const uint2*>(ch.pairs.ptr);
-            g.ynum = P.pre_mode == 1u ? static_cast<const double*>(ch.ynum->p) : nullptr;
-            g.n = (u32)ch.n;
-            g.tile0 = P.n_tiles;
-            P.n_tiles += (u32)((ch.n + PROBEF_TILE - 1) / PROBEF_TILE);
-        }
-    }
-    P.key_is_y = q.key_pos[pk] == 2 ? 1u : 0u;
-    P.n = (u32)PS.n;
-    P.T = T;
-    P.cap = (u32)PS.n;
-    P.nt = numtab(ctx);
-    P.cb = ctx->fast_cb;
-    P.host_total = ctx->d_fast;
-    ip->all_slots = q.all_slots;
-    ip->probe_rows = PS.n;
-    if (agg) {  // GROUP BY folded into the kernel when the join binds the group variable (and the aggregated one, if any)
-        int gsel = -1, asel = -1;
-        for (u32 c = 0; c < ip->n_out; c++) {
-            if (ip->out_slots[c] == agg->group_slot) gsel = (int)c;
-            if (agg->has_agg && ip->out_slots[c] == agg->agg_slot) asel = (int)c;
-        }
-        const bool needs_value = agg->has_agg && agg->kind != KB_AGG_COUNT;
-        if (gsel >= 0 && (!needs_value || asel >= 0)) {
-            ip->agg = true;
-            ip->has_agg = agg->has_agg;
-            ip->agg_kind = agg->has_agg ? agg->kind : (u32)KB_AGG_COUNT;
-            ip->agg_slot = agg->agg_slot;
-            ip->group_slot = agg->group_slot;
-            P.gsel = (u32)gsel;
-            P.asel = asel >= 0 ? (u32)asel : 0u;
-            P.akind = ip->agg_kind;
-        }
-    }
-    ip->ok = true;
-    return KB_OK;
-}
-
-kb_status resolve_index_plan(kb_ctx* ctx, u32 join_slot, const kb_pattern* pats, u32 K, const kb_filter_op* filter, u32 n_ops, const AggSpec* agg,
-                             IndexPlan* plan) {
-    StarQuery q;
-    KB_TRY(star_query(ctx, join_slot, pats, K, filter, n_ops, &q));
-    return resolve_index_plan(ctx, q, index_slices(ctx, q), agg, plan);
-}
-
-// R1: the whole join is one launch of probe_index_kernel
-static kb_status index_join_one_kernel(kb_ctx* ctx, const StarQuery& q, const IndexSlices& ix, AggSpec* agg, std::unique_ptr<kb_rel>* out,
-                                       Route* route) {
-    *route = Route::answered;
-    if (ix.empty) return empty_rel(ctx, q.all_slots, out);
-    IndexPlan ip;
-    KB_TRY(resolve_index_plan(ctx, q, ix, agg, &ip));
-    if (!ip.ok) {
-        *route = Route::declined;
-        return KB_OK;
-    }
-    ProbeIParams& P = ip.P;
-    if (ip.agg) {
-        // GROUP BY folded into the probe kernel: no joined row is written. One try with a 4096-slot table; more groups than that (or
-        // a group / aggregate variable the join does not bind) leave agg->applied false: the caller groups separately
-        GroupParams G{};
-        G.n_gcols = 1;
-        G.n_aggs = ip.has_agg ? 1u : 0u;
-        G.akind[0] = ip.agg_kind;
-        G.nt = numtab(ctx);
-        GroupTable tab;
-        KB_TRY(group_table_create(ctx, 1u << 12, &G, &tab));
-        const u32 goff = ctrl_alloc(ctx, 4);
-        KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + goff, 0, 4 * sizeof(u32), ctx->st));
-        G.overflow = ctx->ctrl + goff;
-        P.ordered = 0;
-        P.epoch = ctx->epoch++;
-        timer_begin(ctx, F_PROBE);
-        launch_probe_index(P, &G, ctx->n_sms, ctx->st);
-        timer_end(ctx);
-        KB_CUDA(ctx, cudaGetLastError());
-        ctx->stats.rows_probed += ip.probe_rows;
-        ctx->stats.index_joins++;
-        KB_TRY(ctrl_read(ctx));
-        if (ctx->h_ctrl[goff] == 0) {
-            agg->n_rows = *reinterpret_cast<volatile u32*>(ctx->h_fast);
-            agg->groups = std::make_unique<kb_groups>();
-            agg->groups->keys.resize(1);
-            agg->groups->vals.resize(agg->has_agg ? 1 : 0);
-            kb_agg a1{agg->kind, agg->agg_slot};
-            KB_TRY(group_table_collect(ctx, tab, 1, &a1, agg->has_agg ? 1u : 0u, agg->groups.get()));
-            agg->applied = true;
-            return KB_OK;
-        }
-        // fall through: join without the fused GROUP BY (the control block was left clean by the kernel)
-    }
-    auto res = std::make_unique<kb_rel>();
-    res->slots = ip.out_slots;
-    KB_TRY(alloc_index_out(ctx, ip.probe_rows, ip.n_out, &res->cols));
-    P.epoch = ctx->epoch++;
-    KB_TRY(launch_index_rows(ctx, P, res->cols));
-    ctx->stats.rows_probed += ip.probe_rows;
-    ctx->stats.index_joins++;
-    KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
-    timers_flush(ctx);
-    ctx->stats.d2h_bytes += sizeof(u32);
-    res->n = *reinterpret_cast<volatile u32*>(ctx->h_fast);
-    *out = select_cols(*res, q.all_slots);
-    return KB_OK;
-}
-
-// R2: build sides are inserted from their slices (pushed-down FILTER evaluated in the build kernel), the probe side IS its slice
-// (zero copy). A duplicate key asks for a retry: the (predicate, position) is then cached as multi-valued, which this route declines
-static kb_status index_join_built(kb_ctx* ctx, const StarQuery& q, const IndexSlices& ix, std::unique_ptr<kb_rel>* out, Route* route) {
-    *route = Route::declined;
-    if (!ix.usable) return KB_OK;
-    const u32 K = q.K, pk = (u32)ix.probe_k, T = K - 1;
-    const u64 rng = ix.kmax >= ix.kmin ? (u64)ix.kmax - ix.kmin + 1 : 0;
-    for (u32 k = 0; k < K; k++) {
-        if (k == pk || ix.persistent[k]) continue;
-        if (rng == 0 || rng > std::max<u64>(8 * ix.sl[k]->n, 1ull << 16) || rng > (1ull << 31)) return KB_OK;
-        if (ctx->multi_valued.count({q.pats[k].p.value, q.key_pos[k]})) return KB_OK;
-    }
-    for (u32 k = 0; k < K; k++) if (!ix.sl[k]->single()) return KB_OK;  // the build kernel reads one contiguous slice per pattern
-    const u32 range = (u32)rng;
-    const u32 off = ctrl_alloc(ctx, 16 + 2 * MAXT);
-    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, (16 + 2 * MAXT) * sizeof(u32), ctx->st));
-    std::vector<Buf> tabs;
-    DirectTab dt[MAXT];
-    std::vector<u32> tab_k;
-    std::vector<u32> out_slots = q.pv[pk];
-    std::vector<OutCol> ocs{OutCol{OUT_PROBE, 0, 0}, OutCol{OUT_PROBE, 1, 0}};
-    FilterProg postp = q.post;  // filters of patterns that are not built (probe side, persistent tables) run on the joined row
-    const bool pre_filter = !q.pushdown[pk].ops.empty() && q.pushdown[pk].ops.size() <= 8;
-    if (!pre_filter) and_into(&postp, q.pushdown[pk]);
-    for (u32 k = 0; k < K; k++) if (k != pk && !ix.persistent[k]) { Buf b; KB_TRY(alloc_buf(ctx, (size_t)range * sizeof(u32), &b)); tabs.push_back(b); }
-    const u32 n_build = (u32)tabs.size();
-    if (n_build) timer_begin(ctx, F_BUILD, (int)n_build);
-    if (n_build > 1) {
-        KB_CUDA(ctx, cudaEventRecord(ctx->ev_fork, ctx->st));
-        KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st2, ctx->ev_fork, 0));
-    }
-    u32 t = 0, bi = 0;
-    for (u32 k = 0; k < K; k++) {
-        if (k == pk) continue;
-        const bool y = q.key_pos[k] == 2;
-        if (ix.persistent[k]) {
-            dt[t] = persistent_tab(*ix.sl[k], y);
-            and_into(&postp, q.pushdown[k]);
-        } else {
-            cudaStream_t bs = (n_build > 1 && (bi & 1)) ? ctx->st2 : ctx->st;
-            u32* tab = static_cast<u32*>(tabs[bi]->p);
-            KB_CUDA(ctx, cudaMemsetAsync(tab, 0xFF, (size_t)range * sizeof(u32), bs));
-            BuildPairsParams B{};
-            B.kv = reinterpret_cast<const uint2*>(ix.sl[k]->single()->pairs.ptr);
-            B.n = (u32)ix.sl[k]->n;
-            B.key_is_y = y ? 1u : 0u;
-            B.pred = q.pats[k].p.value;
-            B.table = tab; B.kmin = ix.kmin; B.range = range; B.cshift = ix.cshift;
-            B.dup_flag = ctx->ctrl + off + 16 + t;
-            B.count = ctx->ctrl + off + 16 + MAXT + t;
-            B.trusted = ((y ? ix.sl[k]->y_unique : ix.sl[k]->x_unique) || ctx->single_valued.count({q.pats[k].p.value, q.key_pos[k]})) ? 1u : 0u;
-            B.nt = numtab(ctx);
-            std::vector<FilterOp> fo;  // the pattern's own filter, over the positions of (s, P, o)
-            KB_TRY(compile_prog(ctx, q.pushdown[k], q.pv[k], &fo, &q.psrc[k]));
-            B.n_ops = (u32)fo.size();
-            for (size_t i = 0; i < fo.size(); i++) B.ops[i] = fo[i];
-            launch_build_direct_pairs_filtered(B, ctx->n_sms, bs);
-            dt[t] = DirectTab{};
-            dt[t].tab = tab; dt[t].kmin = ix.kmin; dt[t].range = range; dt[t].cshift = ix.cshift;
-            ctx->stats.rows_built += ix.sl[k]->n;
-            bi++;
-        }
-        out_slots.push_back(q.pv[k][y ? 0 : 1]);
-        ocs.push_back(OutCol{OUT_TABVAL, t, 0});
-        tab_k.push_back(k);
-        t++;
-    }
-    if (n_build > 1) {
-        KB_CUDA(ctx, cudaEventRecord(ctx->ev_join, ctx->st2));
-        KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st, ctx->ev_join, 0));
-    }
-    if (n_build) timer_end(ctx);
-    const PredSlice& PS = *ix.sl[pk];
-    auto res = std::make_unique<kb_rel>();
-    res->slots = out_slots;
-    std::vector<FilterOp> fops;
-    KB_TRY(compile_prog(ctx, postp, out_slots, &fops));
-    ProbeFParams P{};
-    if (pre_filter) {  // slots of the probe pattern's own filter -> pair halves (x = subject, y = object)
-        std::vector<FilterOp> fo;
-        KB_TRY(compile_prog(ctx, q.pushdown[pk], q.pv[pk], &fo));
-        P.n_pre = (u32)fo.size();
-        for (size_t i = 0; i < fo.size(); i++) P.pre_ops[i] = fo[i];
-        if (PS.typed(ctx->num_version)) P.pre_num = static_cast<const double*>(PS.single()->ynum->p);
-    }
-    KB_TRY(probe_fast(ctx, P, reinterpret_cast<const uint2*>(PS.single()->pairs.ptr), PS.n, q.key_pos[pk] == 2 ? 1u : 0u, dt, T, ocs, fops,
-                      ctx->ctrl + off, nullptr, res.get()));
-    ctx->stats.index_joins++;
-    KB_TRY(ctrl_read(ctx));
-    for (u32 q2 = 0; q2 < T; q2++) if (ctx->h_ctrl[off + 16 + q2]) {
-        *route = Route::retry;
-        ctx->multi_valued.insert({q.pats[tab_k[q2]].p.value, q.key_pos[tab_k[q2]]});
-    }
-    if (*route == Route::retry) return KB_OK;
-    for (u32 q2 = 0; q2 < T; q2++)
-        if (!ix.persistent[tab_k[q2]] && q.pushdown[tab_k[q2]].ops.empty()) ctx->single_valued.insert({q.pats[tab_k[q2]].p.value, q.key_pos[tab_k[q2]]});
-    res->n = ctx->h_ctrl[off + 1];
-    *out = select_cols(*res, q.all_slots);
-    *route = Route::answered;
-    return KB_OK;
-}
-
-// R3: the build-side patterns insert straight into their direct tables while the store is scanned; only the probe-side pattern is
-// materialised. Needs the key range before the scan (load-time statistics) and a probe side chosen without knowing the counts: the
-// last pattern that carries no pushed-down filter (a filtered side is the smaller build side). A duplicate or out-of-range key asks
-// for a retry without the fusion (the chained operator needs the build rows)
-static kb_status fused_scan_join(kb_ctx* ctx, const StarQuery& q, std::unique_ptr<kb_rel>* out, Route* route) {
-    *route = Route::declined;
-    const u32 K = q.K;
-    if (!q.all_pairs || K - 1 > (u32)MAXT || ctx->upload_stats_off >= 0 || ctx->n_triples == 0) return KB_OK;
-    u32 kmn, kmx;
-    KB_TRY(store_key_range(ctx, q, &kmn, &kmx));
-    const u32 cshift = subject_cshift(ctx, q, false);
-    if (kmx >= kmn) { kmn = compact_key(kmn, cshift); kmx = compact_key(kmx, cshift); }
-    const u64 rng = kmx >= kmn ? (u64)kmx - kmn + 1 : 0;
-    if (rng == 0 || rng > std::max<u64>(4 * ctx->n_triples, 1ull << 16) || rng > (1ull << 31) || !q.only_join_shared) return KB_OK;
-    int probe_k = -1;
-    for (u32 k = 0; k < K; k++) if (q.pushdown[k].ops.empty()) probe_k = (int)k;
-    if (probe_k < 0) probe_k = (int)K - 1;
-    for (u32 k = 0; k < K; k++)
-        if ((int)k != probe_k && !q.pats[k].p.is_var && ctx->multi_valued.count({q.pats[k].p.value, q.key_pos[k]})) return KB_OK;
-    const u32 range = (u32)rng;
-    const u32 off = ctrl_alloc(ctx, 8 + MAXT);
-    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, (8 + MAXT) * sizeof(u32), ctx->st));
-    std::vector<ScanTable> st(K);
-    std::vector<Buf> tabs;
-    std::vector<u32> tab_of(K, 0);
-    DirectTab dt[MAXT];
-    std::vector<u32> out_slots = q.pv[probe_k];
-    std::vector<OutCol> ocs{OutCol{OUT_PROBE, 0, 0}, OutCol{OUT_PROBE, 1, 0}};
-    timer_begin(ctx, F_BUILD, 0);
-    u32 t = 0;
-    for (u32 k = 0; k < K; k++) {
-        if ((int)k == probe_k) continue;
-        Buf b;
-        KB_TRY(alloc_buf(ctx, (size_t)range * sizeof(u32), &b));
-        tabs.push_back(b);
-        st[k].tab = static_cast<u32*>(b->p);
-        st[k].clear = true;  // cleared by the scan (scan_impl)
-        st[k].kmin = kmn; st[k].range = range; st[k].cshift = cshift;
-        st[k].key_is_o = q.key_pos[k] == 2 ? 1u : 0u;
-        st[k].trusted = (!q.pats[k].p.is_var && ctx->single_valued.count({q.pats[k].p.value, q.key_pos[k]})) ? 1u : 0u;
-        st[k].dup_flag = ctx->ctrl + off + 8 + t;
-        dt[t] = DirectTab{};
-        dt[t].tab = st[k].tab; dt[t].kmin = kmn; dt[t].range = range; dt[t].cshift = cshift;
-        out_slots.push_back(q.pv[k][q.key_pos[k] == 0 ? 1 : 0]);
-        ocs.push_back(OutCol{OUT_TABVAL, t, 0});
-        tab_of[k] = t;
-        t++;
-    }
-    timer_end(ctx);
-    std::vector<std::unique_ptr<kb_rel>> rels;
-    KB_TRY(scan_impl(ctx, ctx->segs, q.pats, K, q.pushdown, /*use_index=*/false, false, true, &rels, &st));
-    ctx->stats.fused_scan_builds++;
-    // duplicate keys: the scan stores without reading back, so a multi-valued key shows up as fewer occupied slots than
-    // inserted rows. Tables of (predicate, position) pairs already verified for this store version are not re-counted.
-    bool counted = false;
-    const u32 offc = ctrl_alloc(ctx, MAXT);
-    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + offc, 0, MAXT * sizeof(u32), ctx->st));
-    for (u32 k = 0; k < K; k++) {
-        if ((int)k == probe_k || st[k].trusted) continue;
-        if (!counted) timer_begin(ctx, F_BUILD, 0);
-        counted = true;
-        ctx->stats.kernel_launches++;
-        launch_count_nonempty(st[k].tab, range, ctx->ctrl + offc + tab_of[k], ctx->n_sms, ctx->st);
-    }
-    if (counted) timer_end(ctx);  // the counts are read together with the probe's result: no extra synchronisation
-    auto check_dups = [&]() -> bool {
-        bool dup = false;
-        for (u32 k = 0; k < K; k++) {
-            if ((int)k == probe_k) continue;
-            const bool fewer = !st[k].trusted && ctx->h_ctrl[offc + tab_of[k]] != rels[k]->n;
-            if (ctx->h_ctrl[off + 8 + tab_of[k]] || fewer) {
-                dup = true;
-                if (!q.pats[k].p.is_var) ctx->multi_valued.insert({q.pats[k].p.value, q.key_pos[k]});
-            }
-        }
-        return dup;
-    };
-    for (u32 k = 0; k < K; k++) if ((int)k != probe_k) ctx->stats.rows_built += rels[k]->n;
-    *route = Route::answered;
-    for (u32 k = 0; k < K; k++) if (rels[k]->n == 0) return empty_rel(ctx, q.all_slots, out);
-    for (u32 k = 0; k < K; k++) if ((int)k != probe_k && ctx->h_ctrl[off + 8 + tab_of[k]]) {  // key outside the table range (cannot happen with store statistics)
-        KB_TRY(ctrl_read(ctx));
-        check_dups();
-        *route = Route::retry;
-        return KB_OK;
-    }
-    const kb_rel& PR = *rels[probe_k];
-    auto res = std::make_unique<kb_rel>();
-    res->slots = out_slots;
-    std::vector<FilterOp> fops;
-    KB_TRY(compile_prog(ctx, q.post, out_slots, &fops));
-    const u32 off2 = ctrl_alloc(ctx, 8);
-    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off2, 0, 8 * sizeof(u32), ctx->st));
-    ProbeFParams P{};
-    KB_TRY(probe_fast(ctx, P, reinterpret_cast<const uint2*>(PR.cols[0].ptr), PR.n, q.key_pos[probe_k] == 2 ? 1u : 0u, dt, t, ocs, fops,
-                      ctx->ctrl + off2, nullptr, res.get()));
-    KB_TRY(ctrl_read(ctx));
-    if (check_dups()) { *route = Route::retry; return KB_OK; }
-    for (u32 k = 0; k < K; k++)
-        if ((int)k != probe_k && !q.pats[k].p.is_var && q.pushdown[k].ops.empty()) ctx->single_valued.insert({q.pats[k].p.value, q.key_pos[k]});
-    res->n = ctx->h_ctrl[off2 + 1];
-    *out = select_cols(*res, q.all_slots);
-    return KB_OK;
-}
-
-// R5: natural joins of `cur` (null: the probe relation) with the relations `rest`, smallest build sides first; the post-filter rides on
-// the last one
-static kb_status chained_join(kb_ctx* ctx, const StarQuery& q, std::vector<std::unique_ptr<kb_rel>>& rels, u32 probe, std::unique_ptr<kb_rel> cur,
-                              std::vector<u32> rest, std::unique_ptr<kb_rel>* out) {
-    for (auto& r : rels) KB_TRY(unpair_rel(ctx, &r));
-    if (!cur) cur = std::move(rels[probe]);
-    std::sort(rest.begin(), rest.end(), [&](u32 a, u32 b) { return rels[a]->n < rels[b]->n; });
-    for (size_t i = 0; i < rest.size(); i++) {
-        std::unique_ptr<kb_rel> j;
-        KB_TRY(hash_join_impl(ctx, *cur, *rels[rest[i]], (i + 1 == rest.size() && !q.post.ops.empty()) ? &q.post : nullptr, &j));
-        cur = std::move(j);
-    }
-    *out = select_cols(*cur, q.all_slots);
-    return KB_OK;
-}
-
-// R4: direct tables over the key range [kmin, kmin + range), built in batches of at most MAXT per probe launch; the first batch over
-// pair relations takes the register-staged fast probe. A build side that meets a duplicate key hands what is left to R5
-static kb_status batched_join(kb_ctx* ctx, const StarQuery& q, std::vector<std::unique_ptr<kb_rel>>& rels, u32 probe, const std::vector<u32>& builds,
-                              u32 kmin, u32 range, std::unique_ptr<kb_rel>* out) {
-    std::unique_ptr<kb_rel> cur;  // result of the batches done so far (columnar); null = still the scan output of `probe`
-    bool dup_seen = false;
-    size_t done = 0;
-    while (done < builds.size() && !dup_seen) {
-        const size_t nb = std::min<size_t>(MAXT, builds.size() - done);
-        const bool last = done + nb == builds.size();
-        const bool fast = q.all_pairs && !cur;  // first batch over pair relations -> register-staged fast probe
-        const kb_rel& PR = cur ? *cur : *rels[probe];
-        const u32 off = ctrl_alloc(ctx, 8 + MAXT);
-        KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, (8 + MAXT) * sizeof(u32), ctx->st));
-        std::vector<Buf> tables(nb);
-        DirectTab dt[MAXT];
-        std::vector<u32> out_slots = PR.slots;
-        std::vector<OutCol> ocs;
-        for (u32 c = 0; c < (u32)PR.slots.size(); c++) ocs.push_back(OutCol{OUT_PROBE, c, 0});
-        timer_begin(ctx, F_BUILD, (int)nb);
-        for (size_t t = 0; t < nb; t++) KB_TRY(alloc_buf(ctx, (size_t)range * sizeof(u32), &tables[t]));  // stream-ordered on st
-        if (nb > 1) {  // independent tables: odd ones are memset + built on the second stream, concurrently with the even ones
-            KB_CUDA(ctx, cudaEventRecord(ctx->ev_fork, ctx->st));
-            KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st2, ctx->ev_fork, 0));
-        }
-        for (size_t t = 0; t < nb; t++) {
-            const u32 k = builds[done + t];
-            const kb_rel& B = *rels[k];
-            cudaStream_t bs = (nb > 1 && (t & 1)) ? ctx->st2 : ctx->st;
-            u32* tab = static_cast<u32*>(tables[t]->p);
-            KB_CUDA(ctx, cudaMemsetAsync(tab, 0xFF, (size_t)range * sizeof(u32), bs));
-            DirectTab& D = dt[t];
-            D = DirectTab{};
-            D.tab = tab; D.kmin = kmin; D.range = range;
-            const int kc = B.col_of(q.join_slot);
-            if (B.pair) {
-                out_slots.push_back(B.slots[kc == 0 ? 1 : 0]);
-                ocs.push_back(OutCol{OUT_TABVAL, (u32)t, 0});
-                const u32 trusted = (!q.pats[k].p.is_var && ctx->single_valued.count({q.pats[k].p.value, q.key_pos[k]})) ? 1u : 0u;
-                launch_build_direct_pairs(reinterpret_cast<const uint2*>(B.cols[0].ptr), kc == 1 ? 1u : 0u, (u32)B.n, tab, kmin, range, 0u,
-                                          ctx->ctrl + off + 8 + (u32)t, trusted, ctx->n_sms, bs);
-            } else {
-                const u32* vals = nullptr;
-                if (B.cols.size() == 1) { D.mode = 2; }
-                else if (B.cols.size() == 2) {
-                    const int vc = kc == 0 ? 1 : 0;
-                    vals = B.cols[vc].ptr;
-                    out_slots.push_back(B.slots[vc]);
-                    ocs.push_back(OutCol{OUT_TABVAL, (u32)t, 0});
-                } else {
-                    D.mode = 1;
-                    for (size_t c = 0; c < B.cols.size(); c++) if ((int)c != kc) {
-                        D.pay[D.n_pay] = B.cols[c].ptr;
-                        out_slots.push_back(B.slots[c]);
-                        ocs.push_back(OutCol{OUT_TABPAY, (u32)t, D.n_pay});
-                        D.n_pay++;
-                    }
-                }
-                launch_build_direct(B.cols[kc].ptr, vals, (u32)B.n, tab, kmin, range, 0u, ctx->ctrl + off + 8 + (u32)t, ctx->n_sms, bs);
-            }
-            ctx->stats.rows_built += B.n;
-        }
-        if (nb > 1) {
-            KB_CUDA(ctx, cudaEventRecord(ctx->ev_join, ctx->st2));
-            KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st, ctx->ev_join, 0));
-        }
-        timer_end(ctx);
-        auto res = std::make_unique<kb_rel>();
-        res->slots = out_slots;
-        std::vector<FilterOp> fops;
-        if (last) KB_TRY(compile_prog(ctx, q.post, out_slots, &fops));
-        if (fast) {
-            ProbeFParams P{};
-            KB_TRY(probe_fast(ctx, P, reinterpret_cast<const uint2*>(PR.cols[0].ptr), PR.n, PR.col_of(q.join_slot) == 1 ? 1u : 0u, dt, (u32)nb, ocs, fops,
-                              ctx->ctrl + off, ctx->ctrl + off + 8, res.get()));
-        } else {
-            ProbeDParams P{};  // columnar input: the previous batch's result, or a scan without pair output (not all_pairs)
-            P.n_pcols = (u32)PR.cols.size();
-            for (u32 c = 0; c < P.n_pcols; c++) P.pcol[c] = PR.cols[c].ptr;
-            P.key_col = (u32)PR.col_of(q.join_slot);
-            P.n = (u32)PR.n;
-            P.n_tiles = (u32)((PR.n + PROBE_TILE - 1) / PROBE_TILE);
-            P.T = (u32)nb;
-            for (size_t t = 0; t < nb; t++) P.tab[t] = dt[t];
-            KB_TRY(probe_setup(ctx, &P, PR.n, ocs, fops, ctx->ctrl + off, ctx->ctrl + off + 8, res.get()));
-            timer_begin(ctx, F_PROBE);
-            launch_probe_direct(P, ctx->n_sms, ctx->st);
-            timer_end(ctx);
-            KB_CUDA(ctx, cudaGetLastError());
-            ctx->stats.rows_probed += PR.n;
-        }
-        KB_TRY(ctrl_read(ctx));
-        for (size_t t = 0; t < nb; t++) if (ctx->h_ctrl[off + 8 + t]) {
-            dup_seen = true;
-            const u32 k = builds[done + t];
-            if (!q.pats[k].p.is_var) ctx->multi_valued.insert({q.pats[k].p.value, q.key_pos[k]});
-        }
-        if (dup_seen) break;
-        for (size_t t = 0; t < nb; t++) {  // verified duplicate-free: later builds of the same (predicate, key position) use plain stores
-            const u32 k = builds[done + t];
-            // only when the build side was the WHOLE (?s P ?o) relation: a filtered subset proves nothing about the rest
-            if (!q.pats[k].p.is_var && rels[k]->pair && q.pushdown[k].ops.empty()) ctx->single_valued.insert({q.pats[k].p.value, q.key_pos[k]});
-        }
-        res->n = ctx->h_ctrl[off + 1];
-        cur = std::move(res);
-        done += nb;
-        if (cur->n == 0) return empty_rel(ctx, q.all_slots, out);
-    }
-    if (!dup_seen) {
-        *out = select_cols(*cur, q.all_slots);
-        return KB_OK;
-    }
-    // a build side has duplicate keys: join what is left with the chained (multimap) operator
-    return chained_join(ctx, q, rels, probe, std::move(cur), std::vector<u32>(builds.begin() + done, builds.end()), out);
-}
-
-// R4 / R5: every pattern is scanned (or looked up in the index), then joined by direct tables (R4) or chained joins (R5)
-static kb_status scan_join(kb_ctx* ctx, const StarQuery& q, std::unique_ptr<kb_rel>* out) {
-    const u32 K = q.K;
-    std::vector<std::unique_ptr<kb_rel>> rels;
-    KB_TRY(scan_impl(ctx, ctx->segs, q.pats, K, q.pushdown, /*use_index=*/true, false, q.all_pairs, &rels));
-    if (ctx->upload_stats_off >= 0) {  // one-shot host call: the copy stream computed the column ranges chunk by chunk
-        const u32 o = (u32)ctx->upload_stats_off;
-        for (auto& sg : ctx->segs) {
-            for (int c = 0; c < 3; c++) { sg.cmin[c] = ctx->h_ctrl[o + c]; sg.cmax[c] = ctx->h_ctrl[o + 4 + c]; }
-            sg.has_stats = true;
-        }
-        ctx->upload_stats_off = -1;
-    }
-    u32 kmin, kmax;
-    KB_TRY(store_key_range(ctx, q, &kmin, &kmax));
-    for (u32 k = 0; k < K; k++) if (rels[k]->n == 0) return empty_rel(ctx, q.all_slots, out);
-    if (K == 1) {
-        std::unique_ptr<kb_rel> r = std::move(rels[0]);
-        KB_TRY(unpair_rel(ctx, &r));
-        if (!q.post.ops.empty()) { std::unique_ptr<kb_rel> f; KB_TRY(filter_impl(ctx, *r, q.post, &f)); r = std::move(f); }
-        *out = std::move(r);
-        return KB_OK;
-    }
-    // probe side = largest relation (ties: first)
-    u32 probe = 0;
-    for (u32 k = 1; k < K; k++) if (rels[k]->n > rels[probe]->n) probe = k;
-    std::vector<u32> builds;
-    for (u32 k = 0; k < K; k++) if (k != probe) builds.push_back(k);
-    // direct tables need: patterns that share only the join variable, a dense key range, and single-valued keys
-    bool fused_ok = kmax >= kmin && q.only_join_shared;
-    const u64 range64 = fused_ok ? (u64)kmax - kmin + 1 : 0;
-    for (u32 k : builds) {
-        if (range64 > std::max<u64>(8 * rels[k]->n, 1ull << 16) || range64 > (1ull << 31)) fused_ok = false;
-        if (!q.pats[k].p.is_var && ctx->multi_valued.count({q.pats[k].p.value, q.key_pos[k]})) fused_ok = false;
-        if (q.pv[k].size() > 3) fused_ok = false;
-    }
-    if (fused_ok) return batched_join(ctx, q, rels, probe, builds, kmin, (u32)range64, out);
-    return chained_join(ctx, q, rels, probe, nullptr, builds, out);
-}
-
-kb_status star_join_impl(kb_ctx* ctx, u32 join_slot, const kb_pattern* pats, u32 K, const kb_filter_op* filter, u32 n_ops,
-                         std::unique_ptr<kb_rel>* out, AggSpec* agg) {
-    StarQuery q;
-    KB_TRY(star_query(ctx, join_slot, pats, K, filter, n_ops, &q));
-    const IndexSlices ix = index_slices(ctx, q);  // R1 and R2 read it; neither changes what it describes
-    Route r;
-    do {  // R2's duplicate key: the pair is now cached as multi-valued — start again from the top, with the index allowed
-        KB_TRY(index_join_one_kernel(ctx, q, ix, agg, out, &r));
-        if (r == Route::declined) KB_TRY(index_join_built(ctx, q, ix, out, &r));
-    } while (r == Route::retry);
-    if (r == Route::answered) return KB_OK;
-    KB_TRY(fused_scan_join(ctx, q, out, &r));
-    if (r == Route::answered) return KB_OK;
-    // declined, or a duplicate / out-of-range key in R3's tables (r == Route::retry): scan again, without the index and the fusion
-    return scan_join(ctx, q, out);
 }
 
 }  // namespace kb
@@ -2123,95 +1042,6 @@ kb_status kb_bind_join(kb_ctx* ctx, const kb_rel* left, const kb_pattern* pat, k
 }
 }  // extern "C"
 
-kb_status kb::bind_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_pattern& pt, std::unique_ptr<kb_rel>* out) {
-    const kb_rel* left = &L;
-    const kb_pattern* pat = &pt;
-    std::vector<u32> pv, psrc;
-    kb::pattern_vars(*pat, &pv, &psrc);
-    const bool pair_shape = pv.size() == 2 && psrc[0] == 0 && psrc[1] == 2 && !pat->p.is_var;
-    if (pair_shape && ctx->use_index && ctx->index_version == ctx->store_version && left->n > 0 && left->n < 0xFFFFFFF0ull && !left->pair &&
-        left->cols.size() < KB_MAX_COLS) {
-        const int cx = left->col_of(pv[0]), cy = left->col_of(pv[1]);
-        auto it = ctx->index.find(pat->p.value);
-        if ((cx >= 0) != (cy >= 0) && it != ctx->index.end() && it->second.n > 0) {
-            const kb::PredSlice& ps = it->second;
-            const bool by_y = cy >= 0;  // the bound variable is the pattern's object: look up pos[P][y]
-            const kb::Buf& tab = by_y ? ps.ytab : ps.xtab;
-            // the persistent tables of a subject-sharded store are keyed by the COMPACTED subject: a relation that went through a
-            // shuffle holds exactly the keys this shard owns, so the compaction applies to its rows too
-            bool usable = (bool)tab;
-            if (usable && !by_y && ps.tab_cshift != 0u) {
-                // compacted keys alias across shards: the lookup is only sound when every key of `left` belongs to this shard
-                const u32 foff = kb::ctrl_alloc(ctx, 4);
-                KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + foff, 0, 4 * sizeof(u32), ctx->st));
-                kb::timer_begin(ctx, kb::F_OTHER);
-                kb::launch_count_foreign(left->cols[cx].ptr, (u32)left->n, ctx->shard_rank, ctx->shard_world, ctx->ctrl + foff, ctx->n_sms, ctx->st);
-                kb::timer_end(ctx);
-                KB_CUDA(ctx, cudaGetLastError());
-                KB_TRY(kb::ctrl_read(ctx));
-                usable = ctx->h_ctrl[foff] == 0;
-            }
-            if (usable) {
-                kb::ProbeDParams P{};
-                P.n_pcols = (u32)left->cols.size();
-                P.key_col = (u32)(by_y ? cy : cx);
-                P.n = (u32)left->n;
-                P.n_tiles = (u32)((left->n + kb::PROBE_TILE - 1) / kb::PROBE_TILE);
-                P.T = 1;
-                kb::DirectTab& D = P.tab[0];
-                D.tab = static_cast<const u32*>(tab->p);
-                D.kmin = by_y ? ps.ytab_min : ps.xtab_min;
-                D.range = by_y ? ps.ytab_range : ps.xtab_range;
-                D.cshift = by_y ? 0u : ps.tab_cshift;
-                D.mode = 0; D.n_pay = 0; D.pay[0] = D.pay[1] = nullptr;
-                auto rel = std::make_unique<kb_rel>();
-                rel->slots = left->slots;
-                rel->slots.push_back(by_y ? pv[0] : pv[1]);
-                P.n_out = (u32)rel->slots.size();
-                const size_t stride = round256((size_t)left->n * sizeof(u32)) + 256;
-                kb::Buf b;
-                KB_TRY(kb::alloc_buf(ctx, stride * P.n_out, &b));
-                for (u32 c2 = 0; c2 < P.n_out; c2++) {
-                    kb::Col col;
-                    col.buf = b;
-                    col.ptr = reinterpret_cast<u32*>(static_cast<char*>(b->p) + stride * c2);
-                    rel->cols.push_back(col);
-                    P.out[c2] = col.ptr;
-                    P.oc[c2] = c2 + 1 < P.n_out ? kb::OutCol{kb::OUT_PROBE, c2, 0} : kb::OutCol{kb::OUT_TABVAL, 0, 0};
-                    if (c2 + 1 < P.n_out) P.pcol[c2] = left->cols[c2].ptr;
-                }
-                P.cap = (u32)left->n;
-                P.nt = kb::numtab(ctx);
-                KB_TRY(kb::ensure_tile_state(ctx, P.n_tiles));
-                P.tile_state = static_cast<u64*>(ctx->tile_state->p);
-                P.block_state = static_cast<u64*>(ctx->block_state->p);
-                P.ordered = ctx->ordered;
-                const u32 off = kb::ctrl_alloc(ctx, 4);
-                KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, 4 * sizeof(u32), ctx->st));
-                P.ticket = ctx->ctrl + off;
-                P.total = ctx->ctrl + off + 1;
-                P.zero_word = ctx->ctrl + off + 2;
-                P.epoch = ctx->epoch++;
-                P.abort_flag = nullptr;
-                kb::timer_begin(ctx, kb::F_PROBE);
-                kb::launch_probe_direct(P, ctx->n_sms, ctx->st);
-                kb::timer_end(ctx);
-                KB_CUDA(ctx, cudaGetLastError());
-                ctx->stats.rows_probed += left->n;
-                ctx->stats.index_joins++;
-                KB_TRY(kb::ctrl_read(ctx));
-                rel->n = ctx->h_ctrl[off + 1];
-                *out = std::move(rel);
-                return KB_OK;
-            }
-        }
-    }
-    std::vector<std::unique_ptr<kb_rel>> rels;
-    std::vector<kb::FilterProg> none;
-    KB_TRY(kb::scan_impl(ctx, ctx->segs, pat, 1, none, /*use_index=*/true, false, false, &rels));
-    return kb::hash_join_impl(ctx, *left, *rels[0], nullptr, out);
-}
-
 // ------------------------------------------------------------------ quoted triples
 kb::QuotedTab kb::quotedtab(const kb_ctx* ctx) {
     kb::QuotedTab t{};
@@ -2337,16 +1167,8 @@ kb_status kb_scan_quoted(kb_ctx* ctx, const kb_quoted_pattern* qp, kb_rel** out)
     }
     auto m = std::make_unique<kb_rel>();
     m->slots = mslots;
-    const size_t stride = kb::round256((size_t)P.t.n * sizeof(u32)) + 256;
-    kb::Buf b;
-    KB_TRY(kb::alloc_buf(ctx, stride * P.n_out, &b));
-    for (u32 c = 0; c < P.n_out; c++) {
-        kb::Col col;
-        col.buf = b;
-        col.ptr = reinterpret_cast<u32*>(static_cast<char*>(b->p) + stride * c);
-        m->cols.push_back(col);
-        P.out[c] = col.ptr;
-    }
+    KB_TRY(kb::alloc_strided_cols(ctx, P.t.n, P.n_out, &m->cols));
+    for (u32 c = 0; c < P.n_out; c++) P.out[c] = m->cols[c].ptr;
     const u32 off = kb::ctrl_alloc(ctx, 4);
     KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, 4 * sizeof(u32), ctx->st));
     P.count = ctx->ctrl + off;

@@ -78,11 +78,12 @@ __device__ __forceinline__ u32 warp_sum(u32 v) {
 }
 
 // Single-pass ordered prefix across tiles ("decoupled look-back"). One state word per (tile, counter):
-//   [63:34] launch epoch (so the buffer never needs clearing)  [33:32] status 1=A(ggregate) 2=P(refix)  [31:0] value.
+//   [63:34] launch epoch (so the buffer is cleared only when the epoch wraps)  [33:32] status 1=A(ggregate) 2=P(refix)  [31:0] value.
 // Tiles take tickets from an atomic counter, so a tile only ever waits on tiles that are already running.
 // Called by ALL 32 lanes of one warp once counts[0..K) (shared memory) are final; writes the exclusive prefix of this tile
 // to excl[0..K). base[k] (global, may be null) is added to tile 0: the running total of earlier launches (store segments).
 constexpr u64 TS_A = 1ull << 32, TS_P = 2ull << 32;
+constexpr int TS_EPOCH_BITS = 30;  // the epoch field: launches take epochs 1 .. 2^30 - 1 (next_epoch, kb_join.cu)
 __device__ __forceinline__ void tile_prefix_warp(u64* __restrict__ state, u32 tile, u32 K, u64 epoch, const u32* counts, u32* excl,
                                                  const u32* base, int lane) {
     const u64 tag = epoch << 34;

@@ -196,7 +196,7 @@ struct kb_ctx {
     kb::Buf numv;
     std::vector<double> h_numv;
     kb::u64 numv_version = 0;
-    // tile-state buffer of the look-back prefix (never cleared: words carry the launch epoch)
+    // tile-state buffer of the look-back prefix (words carry the launch epoch; cleared only when it wraps: compact_setup, kb_join.cu)
     kb::Buf tile_state, block_state;
     size_t tile_state_tiles = 0;
     // 0 (default): compaction in tile-completion order (one atomic per tile; row order of results is unspecified, as in the
@@ -282,7 +282,7 @@ kb_status alloc_col(kb_ctx* ctx, u64 rows, Col* out);
 kb_status begin_call(kb_ctx* ctx);                      // zero the control arena
 u32 ctrl_alloc(kb_ctx* ctx, u32 words);                 // returns word offset into ctx->ctrl
 kb_status ctrl_read(kb_ctx* ctx);                       // D2H of the used part of the arena + stream sync
-kb_status ensure_tile_state(kb_ctx* ctx, u64 tiles);
+kb_status ensure_tile_state(kb_ctx* ctx, u64 tiles);  // (compact_setup calls it; kb_star_join_prepare, so that a submit allocates nothing)
 NumTab numtab(const kb_ctx* ctx);
 // ctx->numv / h_numv for the current num_version (a device sort of the side table; one read-back). *ok = false: no value order (the
 // table holds 2^31 ids or more), the index keeps no rank columns
@@ -299,6 +299,10 @@ kb_status validate_filter(kb_ctx* ctx, const kb_filter_op* ops, u32 n);
 // split a postfix program into its top-level AND conjuncts
 bool split_conjuncts(const kb_filter_op* ops, u32 n, std::vector<FilterProg>* out);
 std::set<u32> filter_slots(const FilterProg& f);
+// a program over the variables `slots` as device ops: variable slots[i] is read from column i of the kernel's row, or from position
+// (*pos)[i] (0 s, 1 p, 2 o) of a pattern's triple
+kb_status compile_prog(kb_ctx* ctx, const FilterProg& f, const std::vector<u32>& slots, std::vector<FilterOp>* ops,
+                       const std::vector<u32>* pos = nullptr);
 
 struct ScanTable {  // scan+build fusion: pattern k inserts its matches into this direct table instead of emitting rows
     u32* tab = nullptr;
@@ -344,9 +348,12 @@ struct IndexPlan {
 // into the plan (plan->agg) when the join binds its variables
 kb_status resolve_index_plan(kb_ctx* ctx, u32 join_slot, const kb_pattern* pats, u32 n_pats, const kb_filter_op* filter, u32 n_ops,
                              const AggSpec* agg, IndexPlan* plan);
-// the output of the one-kernel index join: n_out columns of `rows` rows in one allocation
-kb_status alloc_index_out(kb_ctx* ctx, u64 rows, u32 n_out, std::vector<Col>* cols);
-// the row-writing launch of the one-kernel index join into such columns (P.epoch is set by the caller)
+// n_cols columns of `rows` rows in one allocation
+kb_status alloc_strided_cols(kb_ctx* ctx, u64 rows, u32 n_cols, std::vector<Col>* cols);
+// the compaction block of one launch over n_tiles tiles: the tile state (allocated whether or not the output is ordered), the order
+// mode, a fresh epoch and the control words ctrl = {ticket, total, zero} (null: the launch brings its own, as the scan does)
+kb_status compact_setup(kb_ctx* ctx, u64 n_tiles, u32* ctrl, Compact* c);
+// the row-writing launch of the one-kernel index join into n_out columns of probe_rows rows
 kb_status launch_index_rows(kb_ctx* ctx, ProbeIParams& P, const std::vector<Col>& cols);
 // GROUP BY hash table on the device (kb_group_aggregate and the fused path): one buffer [val | cnt | keys | state]
 struct GroupTable {

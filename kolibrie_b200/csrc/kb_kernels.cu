@@ -174,7 +174,7 @@ __global__ void __launch_bounds__(SCAN_THREADS, (K <= 4 ? 1024 / SCAN_THREADS : 
             }
             const u32 total = __shfl_sync(0xffffffffu, incl, SCAN_THREADS / 32 - 1);
             if (lane < SCAN_THREADS / 32) s_wcnt[lane][warp] = incl - c;
-            const u32 ex = tile_prefix_2level(P.tile_state, P.block_state, tile, P.n_tiles, (u32)warp, P.epoch, total, P.totals_in, P.totals_out, P.ordered, lane);
+            const u32 ex = tile_prefix_2level(P.c.tile_state, P.c.block_state, tile, P.n_tiles, (u32)warp, P.c.epoch, total, P.totals_in, P.totals_out, P.c.ordered, lane);
             if (lane == 0) s_excl[warp] = ex;
         }
         __syncthreads();
@@ -407,7 +407,7 @@ __global__ void __launch_bounds__(STAR_THREADS, 1024 / STAR_THREADS) scan_star_k
             }
             const u32 total = __shfl_sync(0xffffffffu, incl, STAR_THREADS / 32 - 1);
             if (lane < STAR_THREADS / 32) s_wcnt[lane][warp] = incl - c;
-            const u32 ex = tile_prefix_2level(P.tile_state, P.block_state, tile, P.n_tiles, (u32)warp, P.epoch, total, P.totals_in, P.totals_out, P.ordered, lane);
+            const u32 ex = tile_prefix_2level(P.c.tile_state, P.c.block_state, tile, P.n_tiles, (u32)warp, P.c.epoch, total, P.totals_in, P.totals_out, P.c.ordered, lane);
             if (lane == 0) s_excl[warp] = ex;
         }
         __syncthreads();
@@ -459,7 +459,7 @@ __global__ void __launch_bounds__(STAR_THREADS, 1024 / STAR_THREADS) scan_star_k
 
 // does the star-shape kernel apply?
 static bool scan_is_star(const ScanParams& p) {
-    if (p.K > 4 || p.ordered) return false;  // store-order output (KOLIBRIE_ORDERED, legacy FFI): the general kernel
+    if (p.K > 4 || p.c.ordered) return false;  // store-order output (KOLIBRIE_ORDERED, legacy FFI): the general kernel
     for (u32 k = 0; k < p.K; k++) {
         const ScanPat& sp = p.pat[k];
         const u32 shape = sp.flags & ~(SP_TABLE | SP_TKEY_O | SP_TTRUSTED | SP_PAIR);
@@ -1056,20 +1056,6 @@ __global__ void __launch_bounds__(256) count_nonempty_kernel(const uint4* __rest
     c = warp_sum(c);
     if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, c);
 }
-__global__ void __launch_bounds__(256) clear_direct_pairs_kernel(const uint2* __restrict__ kv, u32 key_is_y, u32 n, u32* __restrict__ table, u32 kmin, u32 range,
-                                                                 u32 cshift) {
-    const u32 stride = gridDim.x * blockDim.x;
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-        const uint2 v = kv[i];
-        const u32 off = compact_key(key_is_y ? v.y : v.x, cshift) - kmin;
-        if (off < range) table[off] = EMPTY32;
-    }
-}
-void launch_clear_direct_pairs(const uint2* kv, u32 key_is_y, u32 n, u32* table, u32 kmin, u32 range, u32 cshift, int n_sms, cudaStream_t st) {
-    if (n == 0) return;
-    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull);
-    clear_direct_pairs_kernel<<<grid, 256, 0, st>>>(kv, key_is_y, n, table, kmin, range, cshift);
-}
 void launch_count_nonempty(const u32* table, u32 n, u32* out_count, int n_sms, cudaStream_t st) {
     if (n == 0) return;
     const u32 n4 = n / 4;
@@ -1109,7 +1095,7 @@ __global__ void __launch_bounds__(PROBEF_THREADS, (PROBEF_ITEMS <= 4 ? 4 : 3)) p
     }
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     auto issue_next = [&](u32 stage) {
-        const u32 t = atomicAdd(P.ticket, 1u);
+        const u32 t = atomicAdd(P.c.ticket, 1u);
         s_nexts[stage] = t;
         if (t < P.n_tiles) {
             const u32 b = t * (u32)PROBEF_TILE;
@@ -1249,7 +1235,7 @@ __global__ void __launch_bounds__(PROBEF_THREADS, (PROBEF_ITEMS <= 4 ? 4 : 3)) p
             }
             const u32 total = __shfl_sync(0xffffffffu, wi, PROBEF_THREADS / 32 - 1);
             if (lane < PROBEF_THREADS / 32) s_wcnt[lane] = wi - wc;
-            const u32 ex = tile_prefix_2level(P.tile_state, P.block_state, tile, P.n_tiles, 0u, P.epoch, total, P.zero_word, P.total, P.ordered, lane);
+            const u32 ex = tile_prefix_2level(P.c.tile_state, P.c.block_state, tile, P.n_tiles, 0u, P.c.epoch, total, P.c.zero_word, P.c.total, P.c.ordered, lane);
             if (lane == 0) s_excl1 = ex;
         }
         __syncthreads();
@@ -1546,7 +1532,7 @@ __global__ void __launch_bounds__(PROBEF_THREADS, KB_PI_MINB) probe_index_kernel
             }
             const u32 total = __shfl_sync(0xffffffffu, wi, PROBEF_THREADS / 32 - 1);
             if (lane < PROBEF_THREADS / 32) s_wcnt[lane] = wi - wc;
-            const u32 ex = tile_prefix_2level(P.tile_state, P.block_state, tile, P.n_tiles, 0u, P.epoch, total, P.cb + 2, P.cb + 1, P.ordered, lane);
+            const u32 ex = tile_prefix_2level(P.c.tile_state, P.c.block_state, tile, P.n_tiles, 0u, P.c.epoch, total, P.c.zero_word, P.c.total, P.c.ordered, lane);
             if (lane == 0) s_excl1 = ex;
         }
         __syncthreads();
@@ -1661,7 +1647,7 @@ __global__ void __launch_bounds__(PROBE_THREADS) probe_direct_kernel(const __gri
     const u32* sKey = smem + P.key_col * PROBE_TILE;
 
     for (;;) {
-        if (tid == 0) s_tile = atomicAdd(P.ticket, 1u);
+        if (tid == 0) s_tile = atomicAdd(P.c.ticket, 1u);
         __syncthreads();
         const u32 tile = s_tile;
         if (tile >= P.n_tiles) break;
@@ -1732,7 +1718,7 @@ __global__ void __launch_bounds__(PROBE_THREADS) probe_direct_kernel(const __gri
             }
             __syncwarp();
             const u32 total = __shfl_sync(0xffffffffu, s_cnt[0], 0);
-            const u32 ex = tile_prefix_2level(P.tile_state, P.block_state, tile, P.n_tiles, 0u, P.epoch, total, P.zero_word, P.total, P.ordered, lane);
+            const u32 ex = tile_prefix_2level(P.c.tile_state, P.c.block_state, tile, P.n_tiles, 0u, P.c.epoch, total, P.c.zero_word, P.c.total, P.c.ordered, lane);
             if (lane == 0) {
                 s_excl[0] = ex;
             }
@@ -1850,7 +1836,7 @@ __global__ void __launch_bounds__(PROBEC_THREADS) probe_chained_kernel(const __g
     }
     u32 parity = 0;
     for (;;) {
-        if (tid == 0) s_tile = atomicAdd(P.ticket, 1u);
+        if (tid == 0) s_tile = atomicAdd(P.c.ticket, 1u);
         __syncthreads();
         const u32 tile = s_tile;
         if (tile >= P.n_tiles) break;
@@ -1892,7 +1878,7 @@ __global__ void __launch_bounds__(PROBEC_THREADS) probe_chained_kernel(const __g
             }
             __syncwarp();
             const u32 total = __shfl_sync(0xffffffffu, s_cnt[0], 0);
-            const u32 ex = tile_prefix_2level(P.tile_state, P.block_state, tile, P.n_tiles, 0u, P.epoch, total, P.zero_word, P.total, P.ordered, lane);
+            const u32 ex = tile_prefix_2level(P.c.tile_state, P.c.block_state, tile, P.n_tiles, 0u, P.c.epoch, total, P.c.zero_word, P.c.total, P.c.ordered, lane);
             if (lane == 0) {
                 s_excl[0] = ex;
                 if (total) atomicAdd(P.total64, (unsigned long long)total);
@@ -2219,7 +2205,7 @@ __global__ void __launch_bounds__(PROBEG_THREADS) probe_grouped_kernel(const __g
                 if (blockIdx.x < pieces) { t = e.tile; h_gbase = e.gbase; h_total = e.total; break; }
             }
             if (tid == 0) s_tile = t;
-        } else if (tid == 0) s_tile = atomicAdd(P.ticket, 1u);
+        } else if (tid == 0) s_tile = atomicAdd(P.c.ticket, 1u);
         __syncthreads();
         const u32 tile = s_tile;
         if (tile >= P.n_tiles) break;
@@ -2272,7 +2258,7 @@ __global__ void __launch_bounds__(PROBEG_THREADS) probe_grouped_kernel(const __g
             if (lane < PROBEG_THREADS / 32) s_w[lane] = wi - w;
             if (lane == 0) s_w[PROBEG_THREADS / 32] = total;
             if (!HEAVY) {
-                const u32 ex = tile_prefix_2level(P.tile_state, P.block_state, tile, P.n_tiles, 0u, P.epoch, total, P.zero_word, P.total, P.ordered, lane);
+                const u32 ex = tile_prefix_2level(P.c.tile_state, P.c.block_state, tile, P.n_tiles, 0u, P.c.epoch, total, P.c.zero_word, P.c.total, P.c.ordered, lane);
                 if (lane == 0) {
                     s_base = ex;
                     if (P.heavy && total > PROBEG_HEAVY) {  // recorded for the second launch
@@ -3715,7 +3701,6 @@ void launch_fill_u32(u32* p, u32 v, u64 n, cudaStream_t st) {
     int grid = (int)umin64(H100_SMS * 8, (n + 255) / 256);
     fill_kernel<<<grid, 256, 0, st>>>(p, v, n);
 }
-void launch_fill_const_col(u32* p, u32 v, u64 n, cudaStream_t st) { launch_fill_u32(p, v, n, st); }
 
 __global__ void __launch_bounds__(256) part_count_kernel(const u32* key, u32 n, u32 n_parts, u32* counts) {
     __shared__ u32 sc[64];

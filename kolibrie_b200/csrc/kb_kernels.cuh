@@ -40,6 +40,17 @@ struct ScanSeg {
     u32 tile0;       // first tile of this segment in the launch's tile numbering
     u32 index_base;  // global index of the segment's first triple
 };
+// what a compacting launch hands tile_prefix_2level (kb_device.cuh): the look-back state, the order mode, the launch's epoch, and the
+// control words {ticket, total, zero} (set by compact_setup, kb_join.cu)
+struct Compact {
+    u64* tile_state;   // level 1: [n_tiles][MAXP]
+    u64* block_state;  // level 2: [ceil(n_tiles/32)][MAXP]
+    u32 ordered;       // 1: output in input order (two-level prefix)  0: tile completion order (atomic cursor)
+    u64 epoch;
+    u32* ticket;
+    u32* total;            // result row count; must be zero at launch
+    const u32* zero_word;  // a word that stays zero (ordered mode reads its base from here)
+};
 struct ScanParams {
     ScanSeg seg[SCAN_MAXSEG];
     u32 n_seg;
@@ -55,11 +66,8 @@ struct ScanParams {
     u32 clear_words[4];
     u32 n_clear;
     u32* clear_barrier;
-    u64* tile_state;   // level 1: [n_tiles][MAXP]
-    u64* block_state;  // level 2: [ceil(n_tiles/32)][MAXP]
-    u32 ordered;       // 1: output in store order (two-level prefix)  0: tile completion order (atomic cursor)
+    Compact c;         // total / zero_word unused: the scan counts per pattern in totals_in / totals_out
     u32* ticket;
-    u64 epoch;
     const u32* totals_in;  // [MAXP] rows written by earlier segments
     u32* totals_out;       // [MAXP] rows written so far (ordered: a different array than totals_in; unordered: the same, used as atomic cursor)
 };
@@ -117,13 +125,7 @@ struct ProbeDParams {
     FilterOp ops[KB_MAX_FILTER_OPS];  // slots = output column indices
     u32 n_ops;
     NumTab nt;
-    u64* tile_state;
-    u64* block_state;
-    u32 ordered;
-    u32* ticket;
-    u64 epoch;
-    u32* total;            // result row count; must be zero at launch
-    const u32* zero_word;  // a word that stays zero (ordered mode reads its base from here)
+    Compact c;
     const u32* abort_flag;  // non-null: exit immediately if *abort_flag != 0 (a direct build met duplicate keys)
 };
 void launch_probe_direct(const ProbeDParams& p, int n_sms, cudaStream_t st);
@@ -152,13 +154,7 @@ struct ProbeFParams {
     const double* pre_num;  // non-null: numeric value of pair.y per probe row (typed literal column of the index): a coalesced read
                             // replaces the random gather num_or0[pair.y] when the pre-filter is FILTER(?y <cmp> c)
     NumTab nt;
-    u64* tile_state;
-    u64* block_state;
-    u32 ordered;
-    u32* ticket;
-    u64 epoch;
-    u32* total;
-    const u32* zero_word;
+    Compact c;
     const u32* abort_flag;
 };
 void launch_probe_fast(const ProbeFParams& p, int n_sms, cudaStream_t st);
@@ -198,10 +194,7 @@ struct ProbeIParams {
     FilterOp ops[KB_MAX_FILTER_OPS];  // conjuncts that need a looked-up value: evaluated over the output row
     u32 n_ops;
     NumTab nt;
-    u64* tile_state;
-    u64* block_state;
-    u32 ordered;
-    u64 epoch;
+    Compact c;  // {ticket, total, zero} = cb[0..2]
     u32 gsel, asel, akind;  // fused GROUP BY (launch_probe_index with `agg`): output column of the key / of the aggregated value, kb_agg kind
     u32* cb;          // device control block: [0] ticket, [1] total, [2] always 0, [3] CTAs done
     u32* host_total;  // mapped pinned host word
@@ -282,8 +275,6 @@ void launch_numorder_values(const unsigned long long* keys, u32 n, double* out, 
 void launch_pair_minmax(const uint2* kv, u32 n, u32* out4, int n_sms, cudaStream_t st);
 // number of occupied (non-EMPTY32) slots of a direct table: equals the number of inserted rows iff the keys were single-valued
 void launch_count_nonempty(const u32* table, u32 n, u32* out_count, int n_sms, cudaStream_t st);
-// eviction of a chunk: the table entries of its keys go back to EMPTY32 (keys are unique while a persistent table exists)
-void launch_clear_direct_pairs(const uint2* kv, u32 key_is_y, u32 n, u32* table, u32 kmin, u32 range, u32 cshift, int n_sms, cudaStream_t st);
 // number of keys that do NOT belong to shard `rank` of `world` (kb_shard_of): 0 for a correctly sharded column
 void launch_count_foreign(const u32* col, u32 n, u32 rank, u32 world, u32* out, int n_sms, cudaStream_t st);
 void launch_col_minmax(const u32* col, u32 n, u32* out_min, u32* out_max, int n_sms, cudaStream_t st);
@@ -307,13 +298,7 @@ struct ProbeCParams {
     FilterOp ops[KB_MAX_FILTER_OPS];
     u32 n_ops;
     NumTab nt;
-    u64* tile_state;
-    u64* block_state;
-    u32 ordered;
-    u32* ticket;
-    u64 epoch;
-    u32* total;
-    const u32* zero_word;
+    Compact c;
     unsigned long long* total64;  // exact output size in 64 bits (the 32-bit positions wrap past 2^32 rows: the host checks this one)
 };
 void launch_probe_chained(const ProbeCParams& p, int n_sms, cudaStream_t st);
@@ -348,13 +333,7 @@ struct ProbeGParams {
     CsrTab tab;
     u32* out[KB_MAX_COLS];  // n_pcols probe columns, then tab.n_pay payload columns
     u32 cap;
-    u64* tile_state;
-    u64* block_state;
-    u32 ordered;
-    u32* ticket;
-    u64 epoch;
-    u32* total;
-    const u32* zero_word;
+    Compact c;
     // tiles whose expansion exceeds PROBEG_HEAVY output rows are not expanded by the CTA that scanned them: it appends them here
     // (heavy_count[0] entries) and a second launch spreads each one's output range over the whole grid in PROBEG_CHUNK-row pieces
     struct Heavy { u32 tile, gbase, total, pad; };
@@ -656,7 +635,6 @@ void launch_r2s_gone_write(const R2sParams& p, int n_sms, cudaStream_t st);
 // ---------------------------------------------------------------------------------------------------------------
 // small utilities
 void launch_fill_u32(u32* p, u32 v, u64 n, cudaStream_t st);
-void launch_fill_const_col(u32* p, u32 v, u64 n, cudaStream_t st);
 // partition rows by mix32(key) % n_parts (multi-GPU shuffle): count then scatter
 void launch_part_count(const u32* key, u32 n, u32 n_parts, u32* counts, int n_sms, cudaStream_t st);
 void launch_part_scatter(const u32* key, u32 n, u32 n_parts, u32* cursors, const u32* const* in_cols, u32* const* out_cols, u32 n_cols,

@@ -19,7 +19,7 @@ struct kb_plan {
     IndexPlan ip;
     u32 ring = 0;
     struct Slot {
-        std::vector<Col> cols;    // row plans: n_out columns of probe_rows rows (alloc_index_out)
+        std::vector<Col> cols;    // row plans: n_out columns of probe_rows rows (alloc_strided_cols)
         GroupTable tab;           // aggregate plans: the device group table of this slot (the overflow word rides behind it) ...
         char* h_rec = nullptr;    // ... and the mapped pinned list its groups are compacted into: {u32 count, u32 overflow, pad} + GroupRecord[cap]
         char* d_rec = nullptr;
@@ -115,10 +115,10 @@ kb_status kb_star_join_prepare(kb_ctx* ctx, uint32_t join_slot, const kb_pattern
             memset(s.h_rec, 0, 16);
             KB_CUDA(ctx, cudaHostGetDevicePointer(reinterpret_cast<void**>(&s.d_rec), s.h_rec, 0));
         } else {
-            KB_TRY(alloc_index_out(ctx, ip.probe_rows, ip.n_out, &s.cols));
+            KB_TRY(alloc_strided_cols(ctx, ip.probe_rows, ip.n_out, &s.cols));
         }
     }
-    if (ip.P.ordered || ctx->ordered) KB_TRY(ensure_tile_state(ctx, ip.P.n_tiles));
+    KB_TRY(ensure_tile_state(ctx, ip.P.n_tiles));  // a submit allocates nothing
     KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
     *out = pl.release();
     return KB_OK;
@@ -136,8 +136,6 @@ kb_status kb_plan_submit(kb_ctx* ctx, kb_plan* pl, uint64_t* ticket) {
     ProbeIParams P = pl->ip.P;
     P.cb = ctx->fast_cb;  // launches of one context are serialised on its stream: they share the self-cleaning control block
     P.host_total = pl->d_totals + (t % pl->ring) * 16;
-    P.epoch = ctx->epoch++;
-    if (ctx->epoch >= (1ull << 30)) ctx->epoch = 1;
     if (pl->ip.agg) {
         GroupParams G{};
         G.n_gcols = 1;
@@ -148,7 +146,8 @@ kb_status kb_plan_submit(kb_ctx* ctx, kb_plan* pl, uint64_t* ticket) {
         char* tb = pl->attached ? pl->peer_scratch[pl->rank] + 256 + (size_t)si * pl->table_stride : static_cast<char*>(s.tab.buf->p);
         s.tab.point(&G, tb);
         G.overflow = (u32*)(tb + s.tab.bytes);
-        P.ordered = 0;
+        KB_TRY(compact_setup(ctx, P.n_tiles, ctx->fast_cb, &P.c));
+        P.c.ordered = 0;  // the rows are folded into groups: no output order to keep
         timer_begin(ctx, F_GROUP);
         launch_group_init(G, ctx->st);
         timer_end(ctx);
