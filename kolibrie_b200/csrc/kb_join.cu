@@ -613,8 +613,10 @@ static kb_status resolve_index_plan(kb_ctx* ctx, const StarQuery& q, const Index
         const u32 hi = std::min<u32>(PS.xtab_range, compact_key(PS.xmax, PS.tab_cshift) - PS.xtab_min + 1u);
         P.ptab = static_cast<const u32*>(PS.xtab->p) + lo;
         if (P.pre_mode == 1u) {  // FILTER(?o <cmp> c) on the value becomes a range of its ranks in the value order
-            P.pkey = static_cast<const u32*>(PS.xkey->p) + lo;
-            const kb_nr::Range r = kb_nr::cmp_range(P.pre_cmp, ctx->h_numv.data(), (u32)ctx->h_numv.size(), P.pre_val);
+            P.pkey = static_cast<const u16*>(PS.xkey->p) + lo;
+            const u32 n_v = (u32)ctx->h_numv.size();
+            P.key_shift = kb_nr::rank_shift(n_v);
+            const kb_nr::Range16 r = kb_nr::range16(kb_nr::cmp_range(P.pre_cmp, ctx->h_numv.data(), n_v, P.pre_val), P.key_shift);
             P.key_lo = r.lo;
             P.key_hi = r.hi;
         }

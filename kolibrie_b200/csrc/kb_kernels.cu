@@ -887,7 +887,7 @@ __global__ void __launch_bounds__(256) segment_split_kernel(const __grid_constan
                 const u32 off = compact_key(vs[j], E.cshift) - E.xtab_min;
                 if (off < E.xtab_range) {
                     if (atomicExch(&E.xtab[off], vo[j]) != EMPTY32) s_flag[w][0] = 1u;
-                    if (E.xkey) E.xkey[off] = xk[j];
+                    if (E.xkey) E.xkey[off] = kb_nr::rank16(xk[j], kb_nr::rank_shift(P.n_numv));
                 } else s_flag[w][2] = 1u;
             }
             if (E.ytab) {
@@ -969,7 +969,7 @@ __global__ void __launch_bounds__(256) pair_numcol_kernel(const uint2* __restric
 // RANKTAB_ITEMS rows per thread (striped over the CTA's chunk): their searches in V run side by side
 constexpr u32 RANKTAB_ITEMS = 4;
 __global__ void __launch_bounds__(256) pair_ranktab_kernel(const uint2* __restrict__ kv, u32 n, NumTab nt, const double* __restrict__ numv, u32 n_numv,
-                                                          u32* __restrict__ out, u32 kmin, u32 range, u32 cshift) {
+                                                          u16* __restrict__ out, u32 kmin, u32 range, u32 cshift) {
     for (u32 row0 = blockIdx.x * 256u * RANKTAB_ITEMS; row0 < n; row0 += gridDim.x * 256u * RANKTAB_ITEMS) {
         double x[RANKTAB_ITEMS];
         u32 off[RANKTAB_ITEMS], r[RANKTAB_ITEMS];
@@ -985,11 +985,12 @@ __global__ void __launch_bounds__(256) pair_ranktab_kernel(const uint2* __restri
             }
         }
         kb_nr::rank_of_n<RANKTAB_ITEMS>(numv, n_numv, x, r);
+        const u32 shift = kb_nr::rank_shift(n_numv);
 #pragma unroll
-        for (u32 j = 0; j < RANKTAB_ITEMS; j++) if (off[j] < range) out[off[j]] = r[j];
+        for (u32 j = 0; j < RANKTAB_ITEMS; j++) if (off[j] < range) out[off[j]] = kb_nr::rank16(r[j], shift);
     }
 }
-void launch_pair_ranktab(const uint2* kv, u32 n, NumTab nt, const double* numv, u32 n_numv, u32* out, u32 kmin, u32 range, u32 cshift, int n_sms,
+void launch_pair_ranktab(const uint2* kv, u32 n, NumTab nt, const double* numv, u32 n_numv, u16* out, u32 kmin, u32 range, u32 cshift, int n_sms,
                          cudaStream_t st) {
     if (n == 0) return;
     const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 256ull * RANKTAB_ITEMS - 1ull) / (256ull * RANKTAB_ITEMS));
@@ -1297,13 +1298,14 @@ __device__ void atomic_max_f64(double* addr, double v);
 // other half of the triple whose key is (table base + i), EMPTY32 where no triple has that key. The keys then come in ascending order
 // whatever the order of the store and of the dictionary ids, so the lookups into the other patterns' tables are sequential too — a
 // direct table over dense ids IS the slice sorted by that column (with the gaps of the id space). With a FILTER on the other half's
-// numeric value the 4-byte value ranks are read from a second table in the same order (kb_numrank.cuh: the FILTER is a rank range).
+// numeric value the 2-byte value ranks are read from a second table in the same order (kb_numrank.cuh: the FILTER is a range of
+// stored ranks; a slot whose stored rank is at an end of that range is decided on its value, num_of(object)).
 template <int T, int PRE, bool AGG, bool TAB>
 __global__ void __launch_bounds__(PROBEF_THREADS, KB_PI_MINB) probe_index_kernel(const __grid_constant__ ProbeIParams P, const __grid_constant__ GroupParams G) {
     constexpr int R = 4;  // rows per thread (striped over the warp's 128-row chunk, see below)
     constexpr u32 TILE = PROBEF_THREADS * R;
     extern __shared__ __align__(128) u32 smem_all[];  // per stage: TILE pairs [+ TILE doubles]
-    constexpr u32 STAGE_WORDS = TAB ? (PRE == 1 ? 2u : 1u) * TILE : (PRE == 1 ? 4u : 2u) * TILE;  // TAB: TILE values [+ TILE ranks]
+    constexpr u32 STAGE_WORDS = TAB ? (PRE == 1 ? 3u * TILE / 2u : TILE) : (PRE == 1 ? 4u : 2u) * TILE;  // TAB: TILE values [+ TILE u16 ranks]
     __shared__ __align__(8) u64 bars[2];
     __shared__ u32 s_nexts[2];
     __shared__ u32 s_wcnt[PROBEF_THREADS / 32];
@@ -1328,10 +1330,11 @@ __global__ void __launch_bounds__(PROBEF_THREADS, KB_PI_MINB) probe_index_kernel
             const u32 b = t * TILE;
             const u32 c = min(TILE, P.ptab_range - b);
             const u32 bytes = (c * 4u + 15u) & ~15u;
+            const u32 kbytes = (c * 2u + 15u) & ~15u;
             s_tcnt[stage] = c;
-            mbar_arrive_expect_tx(&bar, PRE == 1 ? 2u * bytes : bytes);
+            mbar_arrive_expect_tx(&bar, PRE == 1 ? bytes + kbytes : bytes);
             tma_load_1d(smem, P.ptab + b, bytes, &bar);
-            if (PRE == 1) tma_load_1d(smem + TILE, P.pkey + b, bytes, &bar);
+            if (PRE == 1) tma_load_1d(smem + TILE, P.pkey + b, kbytes, &bar);
             return;
         }
         u32 g = 0;  // the chunk (store segment) this tile belongs to
@@ -1382,7 +1385,7 @@ __global__ void __launch_bounds__(PROBEF_THREADS, KB_PI_MINB) probe_index_kernel
                 const u32 key = P.ptab_cshift ? (((((ck >> SHARD_B) << P.ptab_cshift) | P.shard_rank) << SHARD_B) | (ck & ((1u << SHARD_B) - 1u))) : ck;
                 rx[j] = P.key_is_y ? v : key;
                 ry[j] = P.key_is_y ? key : v;
-                if (PRE == 1) pk[j] = smem[TILE + idx];
+                if (PRE == 1) pk[j] = reinterpret_cast<const u16*>(smem + TILE)[idx];
                 vmask |= ((idx < cnt && v != EMPTY32) ? 1u : 0u) << j;
             }
         } else {
@@ -1397,15 +1400,25 @@ __global__ void __launch_bounds__(PROBEF_THREADS, KB_PI_MINB) probe_index_kernel
             for (int j = 0; j < R; j++) vmask |= (((u32)warp * (32u * R) + (u32)j * 32u + (u32)lane) < cnt ? 1u : 0u) << j;
         }
         if (PRE == 1) {
-            u32 pass = 0;
+            u32 pass = 0, edge = 0;
 #pragma unroll
             for (int j = 0; j < R; j++) {
                 bool ok;
-                if constexpr (TAB) ok = kb_nr::in_range(pk[j], P.key_lo, P.key_hi);
-                else ok = cmp_num(P.pre_cmp, pa[j], P.pre_val);
+                if constexpr (TAB) {
+                    ok = pk[j] >= P.key_lo && pk[j] <= P.key_hi;
+                    edge |= ((ok && (pk[j] == P.key_lo || pk[j] == P.key_hi)) ? 1u : 0u) << j;
+                } else ok = cmp_num(P.pre_cmp, pa[j], P.pre_val);
                 pass |= (ok ? 1u : 0u) << j;
             }
             vmask &= pass;
+            if (TAB && P.key_shift != 0u && (edge & vmask) != 0u) {  // a stored rank at an end of the range: its values straddle the constant
+#pragma unroll
+                for (int j = 0; j < R; j++) {
+                    if (((edge & vmask) >> j) & 1u) {
+                        if (!cmp_num(P.pre_cmp, num_of(P.nt, P.key_is_y ? rx[j] : ry[j]), P.pre_val)) vmask &= ~(1u << j);
+                    }
+                }
+            }
         } else if (P.pre_mode == 2u && vmask != 0u) {
 #pragma unroll
             for (int j = 0; j < R; j++) {
@@ -1585,7 +1598,7 @@ __global__ void __launch_bounds__(PROBEF_THREADS, KB_PI_MINB) probe_index_kernel
 template <int T, int PRE, bool AGG, bool TAB>
 static void launch_probe_index_tp(const ProbeIParams& p, const GroupParams& g, int n_sms, cudaStream_t st) {
     static int per_sm = 0;  // occupancy is a property of the kernel image: asked once per instantiation
-    const size_t smem = TAB ? (size_t)PROBEF_THREADS * 4 * (PRE == 1 ? 8 : 4) * 2 : (size_t)PROBEF_THREADS * 4 * (PRE == 1 ? 16 : 8) * 2;
+    const size_t smem = TAB ? (size_t)PROBEF_THREADS * 4 * (PRE == 1 ? 6 : 4) * 2 : (size_t)PROBEF_THREADS * 4 * (PRE == 1 ? 16 : 8) * 2;
     if (per_sm == 0) {
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, probe_index_kernel<T, PRE, AGG, TAB>, PROBEF_THREADS, smem);
         if (per_sm < 1) per_sm = 1;

@@ -179,8 +179,8 @@ struct ProbeIParams {
     // FILTER is `rank in [key_lo, key_hi)`, kb_numrank.cuh); keys are rebuilt from the slot number (ptab_min + slot, then the inverse
     // of the shard compaction)
     const u32* ptab;
-    const u32* pkey;
-    u32 key_lo, key_hi;
+    const u16* pkey;
+    u32 key_lo, key_hi, key_shift;  // stored ranks [key_lo, key_hi] pass; key_shift != 0: the two ends are decided on the value
     u32 ptab_min, ptab_range, ptab_cshift, shard_rank;
     u32 key_is_y, n, n_tiles, T;  // n = rows over all chunks
     DirectTab tab[MAXT];
@@ -236,7 +236,7 @@ struct SplitEntry {
     uint2* pairs;       // the new chunk
     double* ynum;       // its typed literal column (null: no numeric side table loaded)
     u32* xtab; u32 xtab_min, xtab_range, cshift;   // subject table to insert into (null: none)
-    u32* xkey;          // value ranks in table order, maintained with xtab (null: none)
+    u16* xkey;          // value ranks in table order (kb_numrank.cuh: rank16), maintained with xtab (null: none)
     u32* ytab; u32 ytab_min, ytab_range;           // object table (null: none)
 };
 // control words per entry (all 0 at launch): cursor, n_numeric, xdup, ydup, xout, yout, pad, pad, ~xmin, ~ymin, xmax, ymax
@@ -266,7 +266,7 @@ void launch_clear_chunks(const ClearParams& p, int n_sms, cudaStream_t st);
 void launch_pair_numcol(const uint2* kv, u32 n, NumTab nt, double* out, u32* n_numeric, int n_sms, cudaStream_t st);
 // the ranks of those values in the value order numv[0 .. n_numv) (kb_numrank.cuh), laid out like the subject-keyed direct table:
 // out[compact(subject) - kmin] = rank_of(num_of(object))
-void launch_pair_ranktab(const uint2* kv, u32 n, NumTab nt, const double* numv, u32 n_numv, u32* out, u32 kmin, u32 range, u32 cshift, int n_sms,
+void launch_pair_ranktab(const uint2* kv, u32 n, NumTab nt, const double* numv, u32 n_numv, u16* out, u32 kmin, u32 range, u32 cshift, int n_sms,
                          cudaStream_t st);
 // the value order of the numeric side table: keys[i] = order-preserving u64 of fold(num_or0[i]) for i < n, of 0.0 for i == n and for NaN
 void launch_numorder_keys(const double* num_or0, u32 n, unsigned long long* keys, int n_sms, cudaStream_t st);

@@ -106,4 +106,23 @@ KB_NR_HD Range cmp_range(uint32_t cmp, const double* v, uint32_t n, double c) {
 // unsigned: one compare, and NAN_RANK is outside every range
 KB_NR_HD bool in_range(uint32_t rank, uint32_t lo, uint32_t hi) { return rank - lo < hi - lo; }
 
+// The 16-bit rank columns of the store index: a rank r of a V of n values is stored as r >> rank_shift(n), the smallest shift that
+// keeps every rank below NAN_RANK16 (0 while n <= 65535: the stored rank is exact). A rank range [lo, hi) then covers the stored
+// ranks [lo >> s, (hi - 1) >> s]; every stored rank strictly inside is wholly in the range, and only the two at its ends can hold
+// values on both sides of the constant, which the reader decides from the value itself.
+constexpr uint32_t NAN_RANK16 = 0xFFFFu;
+KB_NR_HD uint32_t rank_shift(uint32_t n) {
+    uint32_t s = 0;
+    while (n > 0 && ((n - 1) >> s) >= NAN_RANK16) s++;
+    return s;
+}
+KB_NR_HD uint16_t rank16(uint32_t rank, uint32_t shift) { return (uint16_t)(rank == NAN_RANK ? NAN_RANK16 : rank >> shift); }
+struct Range16 {
+    uint32_t lo, hi;  // stored ranks [lo, hi], inclusive (lo > hi: empty)
+};
+KB_NR_HD Range16 range16(Range r, uint32_t shift) {
+    if (r.lo >= r.hi) return Range16{1u, 0u};
+    return Range16{r.lo >> shift, (r.hi - 1u) >> shift};
+}
+
 }  // namespace kb_nr

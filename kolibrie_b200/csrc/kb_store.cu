@@ -50,11 +50,11 @@ static kb_status build_rank_column(kb_ctx* ctx, PredSlice& ps) {
     bool ok = false;
     KB_TRY(ensure_num_order(ctx, &ok));
     if (!ok) return KB_OK;
-    KB_TRY(alloc_buf(ctx, (size_t)ps.xtab_range * sizeof(u32), &ps.xkey));
+    KB_TRY(alloc_buf(ctx, (size_t)ps.xtab_range * sizeof(u16), &ps.xkey));
     for (auto& ch : ps.chunks) {
         if (!ch.n) continue;
         launch_pair_ranktab(reinterpret_cast<const uint2*>(ch.pairs.ptr), (u32)ch.n, numtab(ctx), static_cast<const double*>(ctx->numv->p),
-                            (u32)ctx->h_numv.size(), static_cast<u32*>(ps.xkey->p), ps.xtab_min, ps.xtab_range, ps.tab_cshift, ctx->n_sms, ctx->st);
+                            (u32)ctx->h_numv.size(), static_cast<u16*>(ps.xkey->p), ps.xtab_min, ps.xtab_range, ps.tab_cshift, ctx->n_sms, ctx->st);
         ctx->stats.kernel_launches++;
     }
     ps.xkey_version = ctx->num_version;
@@ -140,7 +140,7 @@ static kb_status index_add_segment_split(kb_ctx* ctx, const Segment& sg, u32 csh
         rebuild[i][1] = !ps.ytab && !ps.y_tried;
         if (xok) { e.xtab = static_cast<u32*>(ps.xtab->p); e.xtab_min = ps.xtab_min; e.xtab_range = ps.xtab_range; e.cshift = cshift; }
         if (xok && ps.xkey && ps.xkey_version == ctx->num_version && ctx->numv_version == ctx->num_version && ctx->n_ids) {
-            e.xkey = static_cast<u32*>(ps.xkey->p);
+            e.xkey = static_cast<u16*>(ps.xkey->p);
             P.numv = static_cast<const double*>(ctx->numv->p);
             P.n_numv = (u32)ctx->h_numv.size();
         } else ps.xkey.reset();
