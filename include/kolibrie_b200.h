@@ -440,6 +440,40 @@ typedef struct kb_bgp_plan_info {
     uint64_t rows_unprojected;                        /* rows before projection */
 } kb_bgp_plan_info;
 KB_API kb_status kb_bgp_last_plan(kb_ctx* ctx, kb_bgp_plan_info* out);
+/* ORDER BY + LIMIT (apply_order_by and the LIMIT cut, execute_query.rs:113-149, 693-699). The value of a row for a key is its rendered
+ * result string (what kb_rel_decode gives: the dictionary string, `<< s p o >>`, "unknown"), or "" when the row lacks the variable
+ * (a KB_ID_NONE cell, or a slot that is not a column of `in`). Two values compare as f64 when both parse (is_num of the numeric side
+ * table; NaN equal to everything), else byte by byte, a proper prefix first; DESC reverses a key; the first key that is not equal decides.
+ * That comparison is not an order when a key column is MIXED: it holds a number and a non-empty string that is not a number, or NaN and
+ * a number that is not NaN (then the reference's result depends on its sort's internals). On every other column it is: "" first, numbers
+ * by value (-0.0 == 0.0, NaNs equal), strings in byte order.
+ *   *out has `in`'s slots in `in`'s order and `in`'s rows sorted STABLY by the keys (ties keep `in`'s row order, also under DESC),
+ *     then the first `limit` rows when limit > 0 (limit 0: no cut). n_keys = 0, or keys whose values all compare equal: the first
+ *     `limit` rows, as a view of `in`. `in` is not changed.
+ *   Refused before any output exists (*out untouched):
+ *     KB_E_UNSUPPORTED (run the reference's CPU sort): a mixed key column; a string key without device dictionary strings; a numeric
+ *       side table that covers fewer ids than the device dictionary holds; quoted-triple ids without a quoted-triple table;
+ *     KB_E_INVALID: a NULL argument, n_keys > KB_MAX_COLS;  KB_E_LIMIT: 2^32 rows or more.
+ * info (nullable): route = KB_ORDER_VIEW (nothing to sort), KB_ORDER_SORT (stable radix sort of the whole relation) or KB_ORDER_TOPK
+ * (limit > 0, at most 2 keys that order anything, limit * 16 <= rows: a radix select of the limit-th packed key, then only the rows
+ * below it are sorted); per key k: its kind (KB_ORDER_NUMERIC / _STRING / _CONST: every value compares equal, or the slot is not a
+ * column), its distinct ids (0: not a column) and the refinement rounds of its string sort (7 bytes a round). Launches and device time
+ * count in kb_stats' `other` family. */
+enum kb_order_route { KB_ORDER_VIEW = 0, KB_ORDER_SORT = 1, KB_ORDER_TOPK = 2 };
+enum kb_order_kind { KB_ORDER_CONST = 0, KB_ORDER_NUMERIC = 1, KB_ORDER_STRING = 2 };
+typedef struct kb_order_key {
+    uint32_t slot;
+    uint32_t descending; /* 0: ASC, else DESC */
+} kb_order_key;
+typedef struct kb_order_info {
+    uint64_t n_rows_in, n_rows_out;
+    uint32_t route;                      /* kb_order_route */
+    uint32_t key_kind[KB_MAX_COLS];      /* kb_order_kind per key */
+    uint32_t n_distinct[KB_MAX_COLS];    /* distinct ids in the key column */
+    uint32_t string_rounds[KB_MAX_COLS]; /* refinement rounds of the string sort (0 for a numeric key) */
+} kb_order_info;
+KB_API kb_status kb_order_by(kb_ctx* ctx, const kb_rel* in, const kb_order_key* keys, uint32_t n_keys, uint64_t limit, kb_rel** out,
+                             kb_order_info* info /* nullable */);
 /* GROUP BY + aggregates (execute_query.rs:1150-1227) */
 KB_API kb_status kb_group_aggregate(kb_ctx* ctx, const kb_rel* in, const uint32_t* group_slots, uint32_t n_group,
                                     const kb_agg* aggs, uint32_t n_aggs, kb_groups** out);

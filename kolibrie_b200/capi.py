@@ -108,6 +108,25 @@ class KbMaintainStats(C.Structure):
         ("overdelete_rounds", C.c_uint32), ("insert_rounds", C.c_uint32), ("device_ms", C.c_double)]
 
 
+ORDER_VIEW, ORDER_SORT, ORDER_TOPK = 0, 1, 2          # kb_order_route
+ORDER_CONST, ORDER_NUMERIC, ORDER_STRING = 0, 1, 2    # kb_order_kind
+
+
+class KbOrderKey(C.Structure):
+    _fields_ = [("slot", C.c_uint32), ("descending", C.c_uint32)]
+
+
+class KbOrderInfo(C.Structure):
+    """kb_order_info: rows in / out, the route, and per key its kind, distinct ids and string refinement rounds"""
+    _fields_ = [("n_rows_in", C.c_uint64), ("n_rows_out", C.c_uint64), ("route", C.c_uint32), ("key_kind", C.c_uint32 * KB_MAX_COLS),
+                ("n_distinct", C.c_uint32 * KB_MAX_COLS), ("string_rounds", C.c_uint32 * KB_MAX_COLS)]
+
+    def as_dict(self, n_keys: int):
+        """per-key arrays cut to the call's n_keys"""
+        return {"n_rows_in": self.n_rows_in, "n_rows_out": self.n_rows_out, "route": self.route,
+                **{n: list(getattr(self, n))[:n_keys] for n in ("key_kind", "n_distinct", "string_rounds")}}
+
+
 KB_BGP_MAX_PATTERNS = 16
 BGP_NONE, BGP_STAR, BGP_COMPONENTS = 0, 1, 2  # kb_bgp_route
 
@@ -257,6 +276,7 @@ def lib() -> C.CDLL:
         "kb_star_join": (i32, [vp, u32, P(KbPattern), u32, P(KbFilterOp), u32, P(vp)]),
         "kb_bgp_execute": (i32, [vp, P(KbPattern), u32, P(KbFilterOp), u32, P(u32), u32, P(vp)]),
         "kb_bgp_last_plan": (i32, [vp, P(KbBgpPlanInfo)]),
+        "kb_order_by": (i32, [vp, vp, P(KbOrderKey), u32, u64, P(vp), P(KbOrderInfo)]),
         "kb_group_aggregate": (i32, [vp, vp, P(u32), u32, P(KbAgg), u32, P(vp)]),
         "kb_groups_info": (i32, [vp, P(u64), P(u32), P(u32)]),
         "kb_groups_keys": (i32, [vp, u32, P(P(u32))]),
@@ -308,7 +328,7 @@ EXPORTED_SYMBOLS = [
     "kb_store_load", "kb_store_load_device", "kb_store_append", "kb_store_append_device", "kb_store_evict", "kb_store_delete", "kb_store_clear", "kb_store_build_index", "kb_set_use_index", "kb_store_size",
     "kb_store_download", "kb_dict_numeric_load", "kb_dict_legacy_i32_load", "kb_dict_numeric_derive", "kb_dict_numeric_download", "kb_dict_strings_load", "kb_dict_encode", "kb_dict_strings_info", "kb_rel_decode", "kb_strings_info", "kb_strings_download", "kb_strings_free", "kb_quoted_load", "kb_quoted_download", "kb_dict_strings_download", "kb_bind", "kb_rel_info", "kb_rel_download", "kb_rel_device_col", "kb_rel_from_host",
     "kb_rel_from_device", "kb_rel_free", "kb_scan", "kb_filter", "kb_project", "kb_hash_join", "kb_natural_join", "kb_bind_join", "kb_scan_quoted", "kb_star_join", "kb_bgp_execute", "kb_bgp_last_plan",
-    "kb_group_aggregate", "kb_groups_info", "kb_groups_keys", "kb_groups_values", "kb_groups_counts", "kb_groups_free", "kb_groups_pack", "kb_groups_merge", "kb_star_join_aggregate",
+    "kb_order_by", "kb_group_aggregate", "kb_groups_info", "kb_groups_keys", "kb_groups_values", "kb_groups_counts", "kb_groups_free", "kb_groups_pack", "kb_groups_merge", "kb_star_join_aggregate",
     "kb_star_join_prepare", "kb_plan_submit", "kb_plan_collect", "kb_plan_info", "kb_plan_free", "kb_plan_peer_scratch_bytes", "kb_plan_attach_peers",
     "kb_datalog_fixpoint", "kb_datalog_fixpoint_seed", "kb_datalog_maintain", "kb_r2s_create", "kb_r2s_eval", "kb_r2s_info", "kb_r2s_free", "kb_shard_of", "kb_set_sharding", "kb_partition", "kb_partition_counts", "kb_segment_write", "kb_segment_info", "kb_segment_save", "kb_store_append_file", "kb_shuffle_scatter", "kb_shuffle_push", "kb_rel_wrap_device", "kb_star_join_host", "kb_star_join_host_into", "perform_hash_join_cuda",
 ]
@@ -673,6 +693,14 @@ class Context:
         out = C.c_void_p()
         self._check(lib().kb_rel_from_device(self.h, sl, len(slots), ptrs, n, C.byref(out)))
         return Relation(self, out)
+
+    def order_by(self, rel: Relation, keys: Sequence[Tuple[int, bool]] = (), limit: int = 0) -> Tuple[Relation, dict]:
+        """kb_order_by: `rel`'s rows sorted stably by keys = [(slot, descending)], then cut to `limit` rows when limit > 0.
+        Returns (relation, kb_order_info as a dict). KB_E_UNSUPPORTED (a mixed key column, ...) raises: sort on the host."""
+        arr = (KbOrderKey * max(len(keys), 1))(*[KbOrderKey(int(s_), 1 if d else 0) for s_, d in keys])
+        out, info = C.c_void_p(), KbOrderInfo()
+        self._check(lib().kb_order_by(self.h, rel.h, arr, len(keys), int(limit), C.byref(out), C.byref(info)))
+        return Relation(self, out), info.as_dict(len(keys))
 
     def group_aggregate(self, rel: Relation, group_slots: Sequence[int], aggs: Sequence[tuple]):
         """aggs: [(kind, slot)] -> dict(keys=[cols], values=[cols], counts=array)"""

@@ -38,6 +38,15 @@ KB_NR_HD uint64_t order_key(double x) {
     memcpy(&b, &x, sizeof b);
     return (b >> 63) ? ~b : (b | (1ull << 63));
 }
+// ORDER BY's order of numbers (kb_order.cu): as order_key, except that every NaN takes one key of its own above +inf (a key column that
+// holds NaN and another number is refused, so where NaN sits never matters), and 0, which no number takes, is left for ""
+KB_NR_HD uint64_t order_key_total(double x) {
+    if (x != x) return ~0ull;
+    x = fold(x);
+    uint64_t b;
+    memcpy(&b, &x, sizeof b);
+    return (b >> 63) ? ~b : (b | (1ull << 63));
+}
 KB_NR_HD double order_value(uint64_t k) {
     const uint64_t b = (k >> 63) ? (k & ~(1ull << 63)) : ~k;
     double x;

@@ -777,11 +777,31 @@ class ExecutionEngine:
         return [{names[j]: int(cols[j][i]) for j in range(len(names))} for i in range(n)]
 
     @staticmethod
-    def execute(op, db: SparqlDatabase) -> List[Dict[str, str]]:
-        # engine.rs:33-49: ids are turned into strings only at the very end — here by kb_rel_decode, column by column, on the device
+    def execute(op, db: SparqlDatabase, order_by: Sequence["OrderCondition"] = (), limit: int = 0) -> List[Dict[str, str]]:
+        # engine.rs:33-49: ids are turned into strings only at the very end — here by kb_rel_decode, column by column, on the device.
+        # order_by / limit: apply_order_by and the LIMIT cut that follow it (execute_query.rs:693-699), run by kb_order_by before the
+        # decode so that only the rows kept are decoded; a key column the device refuses (KB_E_UNSUPPORTED) is sorted here after the decode
         db._sync()
         slots = SlotMap()
         rel = ExecutionEngine._run(op, db, slots)
+        host_order = False
+        if order_by or limit > 0:
+            keys = [(slots.slot[_strip(o.variable)], o.direction == SortDirection.DESC) for o in order_by if _strip(o.variable) in slots.slot]
+            try:
+                rel, _ = db.ctx.order_by(rel, keys, limit)
+            except c.KolibrieError as e:
+                if e.status != c.KB_E_UNSUPPORTED:
+                    raise
+                host_order = True
+        rows = ExecutionEngine._decode_rows(rel, db, slots)
+        if host_order:
+            rows = apply_order_by(rows, order_by)
+            if limit > 0:
+                rows = rows[:limit]
+        return rows
+
+    @staticmethod
+    def _decode_rows(rel: c.Relation, db: SparqlDatabase, slots: SlotMap) -> List[Dict[str, str]]:
         n, rslots = rel.info()
         cols = []
         for i in range(len(rslots)):
@@ -796,6 +816,46 @@ class ExecutionEngine:
         if unbound:
             return [{names[j]: cols[j][i] for j in range(len(names)) if not (j in unbound and unbound[j][i])} for i in range(n)]
         return [{names[j]: cols[j][i] for j in range(len(names))} for i in range(n)]
+
+
+class SortDirection:  # shared/src/query.rs:234-237
+    ASC = "ASC"
+    DESC = "DESC"
+
+
+@dataclass(frozen=True)
+class OrderCondition:  # shared/src/query.rs:240-243
+    variable: str
+    direction: str = SortDirection.ASC
+
+
+def _order_cmp(a: str, b: str) -> int:
+    x, y = rust_parse_f64(a), rust_parse_f64(b)
+    if x is not None and y is not None:  # partial_cmp, NaN -> Equal
+        return -1 if x < y else 1 if x > y else 0
+    ab, bb = a.encode("utf-8"), b.encode("utf-8")  # str::cmp: byte order, a proper prefix first
+    return -1 if ab < bb else 1 if ab > bb else 0
+
+
+def apply_order_by(rows: List[Dict[str, str]], conditions: Sequence[OrderCondition]) -> List[Dict[str, str]]:
+    """apply_order_by (execute_query.rs:113-149) on decoded rows: a stable sort (`sort_by`) where a missing variable is "". Where the
+    comparison is not an order (a mixed column) the result depends on the sort algorithm, as the reference's does."""
+    import functools
+
+    if not conditions:
+        return rows
+
+    def cmp(ra, rb):
+        for o in conditions:
+            v = _strip(o.variable)
+            r = _order_cmp(ra.get(v, ""), rb.get(v, ""))
+            if o.direction == SortDirection.DESC:
+                r = -r
+            if r:
+                return r
+        return 0
+
+    return sorted(rows, key=functools.cmp_to_key(cmp))
 
 
 # ---------------------------------------------------------------------------------------------------------------------

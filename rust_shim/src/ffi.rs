@@ -57,6 +57,14 @@ pub const KB_BGP_NONE: u32 = 0; pub const KB_BGP_STAR: u32 = 1; pub const KB_BGP
     pub component_rows: [u64; KB_BGP_MAX_PATTERNS], pub component_max_rows: [u64; KB_BGP_MAX_PATTERNS], pub cross_order: [u32; KB_BGP_MAX_PATTERNS],
     pub reduce_bytes: u64, pub reduce_bit_ops: u64, pub max_intermediate: u64, pub rows_unprojected: u64 }
 pub type kb_bgp_plan_info = KbBgpPlanInfo;  // (the header's name, as the declaration below spells it)
+// kb_order_by: ORDER BY + LIMIT over a device relation (kb_order_route, kb_order_kind)
+pub const KB_ORDER_VIEW: u32 = 0; pub const KB_ORDER_SORT: u32 = 1; pub const KB_ORDER_TOPK: u32 = 2;
+pub const KB_ORDER_CONST: u32 = 0; pub const KB_ORDER_NUMERIC: u32 = 1; pub const KB_ORDER_STRING: u32 = 2;
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbOrderKey { pub slot: u32, pub descending: u32 }
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbOrderInfo { pub n_rows_in: u64, pub n_rows_out: u64, pub route: u32,
+    pub key_kind: [u32; KB_MAX_COLS], pub n_distinct: [u32; KB_MAX_COLS], pub string_rounds: [u32; KB_MAX_COLS] }
+pub type kb_order_key = KbOrderKey;  // (the header's names, as the declaration below spells them)
+pub type kb_order_info = KbOrderInfo;
 
 // kb_filter_opcode / kb_cmp / kb_agg_kind / kb_strategy
 pub const KB_F_CMP_NUM: u32 = 1; pub const KB_F_EQ_ID: u32 = 2; pub const KB_F_NE_ID: u32 = 3; pub const KB_F_AND: u32 = 4; pub const KB_F_OR: u32 = 5;
@@ -118,6 +126,8 @@ extern "C" {
     pub fn kb_scan_quoted(ctx: *mut KbCtx, qp: *const kb_quoted_pattern, out: *mut *mut KbRel) -> kb_status;
     pub fn kb_bind(ctx: *mut KbCtx, r: *const KbRel, spec: *const kb_bind_spec, out: *mut *mut KbRel, info: *mut kb_bind_info) -> kb_status;
     pub fn kb_star_join(ctx: *mut KbCtx, join_slot: u32, pats: *const KbPattern, n: u32, f: *const KbFilterOp, nf: u32, out: *mut *mut KbRel) -> kb_status;
+    pub fn kb_order_by(ctx: *mut KbCtx, r: *const KbRel, keys: *const kb_order_key, n_keys: u32, limit: u64, out: *mut *mut KbRel,
+                       info: *mut kb_order_info) -> kb_status;
     pub fn kb_group_aggregate(ctx: *mut KbCtx, r: *const KbRel, group_slots: *const u32, n_group: u32, aggs: *const KbAgg, n_aggs: u32, out: *mut *mut KbGroups) -> kb_status;
     pub fn kb_star_join_aggregate(ctx: *mut KbCtx, join_slot: u32, pats: *const KbPattern, n: u32, f: *const KbFilterOp, nf: u32, group_slots: *const u32, n_group: u32,
                                   aggs: *const KbAgg, n_aggs: u32, out: *mut *mut KbGroups, n_rows: *mut u64) -> kb_status;
