@@ -594,83 +594,6 @@ u32 pow2_at_least(u64 x) {
 
 // =================================================================================================================
 // C ABI
-#define KB_ENTER(ctx)                                         \
-    if (!(ctx)) return KB_E_INVALID;                          \
-    kb::DeviceGuard _guard((ctx)->device);                    \
-    KB_TRY(kb::begin_call(ctx))
-
-namespace kb {
-kb_status group_table_create(kb_ctx* ctx, u64 slots, GroupParams* P, GroupTable* t) {
-    t->slots = slots;
-    t->o_val = 0;
-    t->o_cnt = t->o_val + slots * 8 * sizeof(double);
-    t->o_keys = t->o_cnt + slots * sizeof(unsigned long long);
-    t->o_state = t->o_keys + slots * 4 * sizeof(u32);
-    t->bytes = t->o_state + slots * sizeof(u32);
-    KB_TRY(alloc_buf(ctx, t->bytes, &t->buf));
-    t->point(P, static_cast<char*>(t->buf->p));
-    launch_group_init(*P, ctx->st);
-    return KB_OK;
-}
-void groups_from_host_table(const char* hb, const GroupTable& t, u32 n_group, const kb_agg* aggs, u32 n_aggs, kb_groups* g) {
-    const double* hval = (const double*)(hb + t.o_val);
-    const unsigned long long* hcnt = (const unsigned long long*)(hb + t.o_cnt);
-    const u32* hkeys = (const u32*)(hb + t.o_keys);
-    const u32* hstate = (const u32*)(hb + t.o_state);
-    if (g->kinds.empty()) for (u32 a = 0; a < n_aggs; a++) g->kinds.push_back(aggs[a].kind);
-    g->raw.resize(n_aggs);
-    for (u64 i = 0; i < t.slots; i++) {
-        if (hstate[i] != 2u) continue;
-        for (u32 c = 0; c < n_group; c++) g->keys[c].push_back(hkeys[i * 4 + c]);
-        g->counts.push_back(hcnt[i]);
-        for (u32 a = 0; a < n_aggs; a++) {
-            double v = hval[i * 8 + a];
-            g->raw[a].push_back(v);
-            if (aggs[a].kind == KB_AGG_AVG) v = v / (double)hcnt[i];   // execute_query.rs:1216
-            if (aggs[a].kind == KB_AGG_COUNT) v = (double)hcnt[i];
-            g->vals[a].push_back(v);
-        }
-    }
-}
-void groups_from_records(const GroupRecord* recs, u64 n, u32 n_group, const kb_agg* aggs, u32 n_aggs, kb_groups* g) {
-    if (g->kinds.empty()) for (u32 a = 0; a < n_aggs; a++) g->kinds.push_back(aggs[a].kind);
-    g->raw.resize(n_aggs);
-    for (u64 i = 0; i < n; i++) {
-        const GroupRecord& r = recs[i];
-        for (u32 c = 0; c < n_group; c++) g->keys[c].push_back(r.keys[c]);
-        g->counts.push_back(r.count);
-        for (u32 a = 0; a < n_aggs; a++) {
-            double v = r.raw[a];
-            g->raw[a].push_back(v);
-            if (aggs[a].kind == KB_AGG_AVG) v = v / (double)r.count;   // execute_query.rs:1216
-            if (aggs[a].kind == KB_AGG_COUNT) v = (double)r.count;
-            g->vals[a].push_back(v);
-        }
-    }
-}
-kb_status group_table_collect(kb_ctx* ctx, const GroupTable& t, u32 n_group, const kb_agg* aggs, u32 n_aggs, kb_groups* g) {
-    std::vector<char> big;  // tables past 32 MB (hundreds of thousands of groups) are not worth pinning
-    void* dst = nullptr;
-    if (t.bytes <= (32u << 20)) {
-        if (ctx->pinned_bytes < t.bytes) {
-            if (ctx->pinned) cudaFreeHost(ctx->pinned);
-            ctx->pinned = nullptr; ctx->pinned_bytes = 0;
-            KB_CUDA(ctx, cudaMallocHost(&ctx->pinned, t.bytes));
-            ctx->pinned_bytes = t.bytes;
-        }
-        dst = ctx->pinned;
-    } else {
-        big.resize(t.bytes);
-        dst = big.data();
-    }
-    KB_CUDA(ctx, cudaMemcpyAsync(dst, t.buf->p, t.bytes, cudaMemcpyDeviceToHost, ctx->st));
-    KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
-    ctx->stats.d2h_bytes += t.bytes;
-    groups_from_host_table(static_cast<const char*>(dst), t, n_group, aggs, n_aggs, g);
-    return KB_OK;
-}
-}  // namespace kb
-
 extern "C" {
 
 const char* kb_version(void) { return "kolibrie_b200 0.1.0 (sm_90a)"; }
@@ -1243,204 +1166,6 @@ kb_status kb_bgp_execute(kb_ctx* ctx, const kb_pattern* pats, uint32_t n_pats, c
     ctx->stats.rows_out = cur->n;
     *out = cur.release();
     return KB_OK;
-}
-
-// ------------------------------------------------------------------ GROUP BY
-kb_status kb_group_aggregate(kb_ctx* ctx, const kb_rel* in, const uint32_t* group_slots, uint32_t n_group, const kb_agg* aggs, uint32_t n_aggs, kb_groups** out) {
-    KB_ENTER(ctx);
-    if (!in || !out || (n_group && !group_slots) || (n_aggs && !aggs)) return kb::fail(ctx, KB_E_INVALID, "NULL argument");
-    if (n_group == 0 || n_group > 4) return kb::fail(ctx, KB_E_LIMIT, "GROUP BY takes 1..4 variables");
-    if (n_aggs > 8) return kb::fail(ctx, KB_E_LIMIT, "at most 8 aggregates");
-    if (in->n >= 0xFFFFFFF0ull) return kb::fail(ctx, KB_E_LIMIT, "relation too large");
-    kb::GroupParams P{};
-    P.n_gcols = n_group;
-    for (u32 c = 0; c < n_group; c++) {
-        int ci = in->col_of(group_slots[c]);
-        if (ci < 0) return kb::fail(ctx, KB_E_INVALID, "GROUP BY slot %u is not a column", group_slots[c]);
-        P.gcol[c] = in->cols[ci].ptr;
-    }
-    P.n_aggs = n_aggs;
-    for (u32 a = 0; a < n_aggs; a++) {
-        P.akind[a] = aggs[a].kind;
-        P.acol[a] = nullptr;
-        if (aggs[a].kind > KB_AGG_AVG) return kb::fail(ctx, KB_E_INVALID, "unknown aggregate kind %u", aggs[a].kind);
-        if (aggs[a].kind != KB_AGG_COUNT) {
-            int ci = in->col_of(aggs[a].slot);
-            if (ci < 0) return kb::fail(ctx, KB_E_INVALID, "aggregate slot %u is not a column", aggs[a].slot);
-            P.acol[a] = in->cols[ci].ptr;
-        }
-    }
-    P.n = (u32)in->n;
-    P.nt = kb::numtab(ctx);
-    auto g = std::make_unique<kb_groups>();
-    g->keys.resize(n_group);
-    g->vals.resize(n_aggs);
-    if (in->n == 0) { *out = g.release(); return KB_OK; }
-    u64 slots = 1u << 12;  // small first try: the table is downloaded whole; overflow -> 16x larger and rerun
-    for (;;) {
-        kb::GroupTable tab;
-        KB_TRY(kb::group_table_create(ctx, slots, &P, &tab));
-        const u32 off = kb::ctrl_alloc(ctx, 4);
-        KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, 4 * sizeof(u32), ctx->st));
-        P.overflow = ctx->ctrl + off;
-        kb::timer_begin(ctx, kb::F_GROUP, 2);
-        kb::launch_group(P, ctx->n_sms, ctx->st);
-        kb::timer_end(ctx);
-        KB_CUDA(ctx, cudaGetLastError());
-        KB_TRY(kb::ctrl_read(ctx));
-        if (ctx->h_ctrl[off] == 0) {
-            KB_TRY(kb::group_table_collect(ctx, tab, n_group, aggs, n_aggs, g.get()));
-            break;
-        }
-        if (slots >= 2 * in->n && slots >= (1u << 20)) return kb::fail(ctx, KB_E_LIMIT, "group table overflow");
-        slots *= 16;
-        if (slots > (1ull << 30)) slots = 1ull << 30;
-    }
-    *out = g.release();
-    return KB_OK;
-}
-kb_status kb_groups_info(const kb_groups* g, uint64_t* n_groups, uint32_t* n_group_cols, uint32_t* n_aggs) {
-    if (!g) return KB_E_INVALID;
-    if (n_groups) *n_groups = g->counts.size();
-    if (n_group_cols) *n_group_cols = (uint32_t)g->keys.size();
-    if (n_aggs) *n_aggs = (uint32_t)g->vals.size();
-    return KB_OK;
-}
-kb_status kb_groups_keys(const kb_groups* g, uint32_t col, const uint32_t** keys) {
-    if (!g || !keys || col >= g->keys.size()) return KB_E_INVALID;
-    *keys = g->keys[col].data();
-    return KB_OK;
-}
-kb_status kb_groups_values(const kb_groups* g, uint32_t agg, const double** values) {
-    if (!g || !values || agg >= g->vals.size()) return KB_E_INVALID;
-    *values = g->vals[agg].data();
-    return KB_OK;
-}
-kb_status kb_groups_counts(const kb_groups* g, const uint64_t** counts) {
-    if (!g || !counts) return KB_E_INVALID;
-    *counts = g->counts.data();
-    return KB_OK;
-}
-void kb_groups_free(kb_groups* g) { delete g; }
-
-// ---- partial GROUP BY results across ranks (SURVEY.md 8e): pack on every rank, gather, merge on the device
-namespace {
-struct GroupsHeader {
-    uint64_t magic, n_groups;
-    uint32_t n_group_cols, n_aggs;
-    uint32_t kinds[8];
-};
-static_assert(sizeof(GroupsHeader) == 56, "layout");
-constexpr uint64_t GROUPS_MAGIC = 0x4B4247524F555031ull;  // "KBGROUP1"
-}  // namespace
-
-kb_status kb_groups_pack(const kb_groups* g, void* dst, uint64_t capacity_bytes, uint64_t* bytes) {
-    if (!g || !bytes) return KB_E_INVALID;
-    const uint64_t n = g->counts.size();
-    const uint64_t need = sizeof(GroupsHeader) + n * sizeof(kb::GroupRecord);
-    *bytes = need;
-    if (!dst) return KB_OK;  // size query
-    if (capacity_bytes < need) return KB_E_LIMIT;
-    if (g->keys.size() > 4 || g->vals.size() > 8 || g->raw.size() != g->vals.size() || g->kinds.size() != g->vals.size()) return KB_E_INVALID;
-    GroupsHeader h{};
-    h.magic = GROUPS_MAGIC;
-    h.n_groups = n;
-    h.n_group_cols = (uint32_t)g->keys.size();
-    h.n_aggs = (uint32_t)g->vals.size();
-    for (size_t a = 0; a < g->kinds.size(); a++) h.kinds[a] = g->kinds[a];
-    memcpy(dst, &h, sizeof h);
-    auto* rec = reinterpret_cast<kb::GroupRecord*>(static_cast<char*>(dst) + sizeof h);
-    for (uint64_t i = 0; i < n; i++) {
-        kb::GroupRecord r{};
-        for (size_t c = 0; c < g->keys.size(); c++) r.keys[c] = g->keys[c][i];
-        r.count = g->counts[i];
-        for (size_t a = 0; a < g->raw.size(); a++) r.raw[a] = g->raw[a][i];
-        memcpy(rec + i, &r, sizeof r);
-    }
-    return KB_OK;
-}
-
-kb_status kb_groups_merge(kb_ctx* ctx, const void* const* parts, const uint64_t* part_bytes, uint32_t n_parts, kb_groups** out) {
-    KB_ENTER(ctx);
-    if (!parts || !part_bytes || !out || n_parts == 0) return kb::fail(ctx, KB_E_INVALID, "NULL or empty argument");
-    GroupsHeader h0{};
-    uint64_t total = 0;
-    for (u32 i = 0; i < n_parts; i++) {
-        if (!parts[i] || part_bytes[i] < sizeof(GroupsHeader)) return kb::fail(ctx, KB_E_INVALID, "partial %u is truncated", i);
-        GroupsHeader h;
-        memcpy(&h, parts[i], sizeof h);
-        if (h.magic != GROUPS_MAGIC) return kb::fail(ctx, KB_E_INVALID, "partial %u is not a kb_groups_pack buffer", i);
-        if (part_bytes[i] < sizeof h + h.n_groups * sizeof(kb::GroupRecord)) return kb::fail(ctx, KB_E_INVALID, "partial %u is truncated", i);
-        if (i == 0) h0 = h;
-        else if (h.n_group_cols != h0.n_group_cols || h.n_aggs != h0.n_aggs || memcmp(h.kinds, h0.kinds, sizeof h.kinds) != 0)
-            return kb::fail(ctx, KB_E_INVALID, "partial %u was produced by a different GROUP BY (columns / aggregates differ)", i);
-        total += h.n_groups;
-    }
-    if (h0.n_group_cols == 0 || h0.n_group_cols > 4 || h0.n_aggs > 8) return kb::fail(ctx, KB_E_INVALID, "bad header");
-    if (total >= (1ull << 30)) return kb::fail(ctx, KB_E_LIMIT, "too many partial groups");
-    auto g = std::make_unique<kb_groups>();
-    g->keys.resize(h0.n_group_cols);
-    g->vals.resize(h0.n_aggs);
-    std::vector<kb_agg> aggs(h0.n_aggs);
-    for (u32 a = 0; a < h0.n_aggs; a++) { aggs[a].kind = h0.kinds[a]; aggs[a].slot = 0; }
-    if (total == 0) {
-        for (u32 a = 0; a < h0.n_aggs; a++) g->kinds.push_back(h0.kinds[a]);
-        g->raw.resize(h0.n_aggs);
-        *out = g.release();
-        return KB_OK;
-    }
-    // partial records -> device, merged by find-or-insert into a group table sized for the worst case (every partial group distinct)
-    kb::Buf recs;
-    KB_TRY(kb::alloc_buf(ctx, total * sizeof(kb::GroupRecord), &recs));
-    uint64_t at = 0;
-    for (u32 i = 0; i < n_parts; i++) {
-        GroupsHeader h;
-        memcpy(&h, parts[i], sizeof h);
-        if (h.n_groups == 0) continue;
-        KB_CUDA(ctx, cudaMemcpyAsync(static_cast<kb::GroupRecord*>(recs->p) + at, static_cast<const char*>(parts[i]) + sizeof h, h.n_groups * sizeof(kb::GroupRecord),
-                                     cudaMemcpyHostToDevice, ctx->st));
-        at += h.n_groups;
-    }
-    ctx->stats.h2d_bytes += total * sizeof(kb::GroupRecord);
-    kb::GroupParams P{};
-    P.n_gcols = h0.n_group_cols;
-    P.n_aggs = h0.n_aggs;
-    for (u32 a = 0; a < h0.n_aggs; a++) P.akind[a] = h0.kinds[a];
-    P.nt = kb::numtab(ctx);
-    kb::GroupTable tab;
-    KB_TRY(kb::group_table_create(ctx, kb::pow2_at_least(std::max<u64>(2 * total, 1024)), &P, &tab));
-    const u32 off = kb::ctrl_alloc(ctx, 4);
-    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, 4 * sizeof(u32), ctx->st));
-    P.overflow = ctx->ctrl + off;
-    kb::timer_begin(ctx, kb::F_GROUP);
-    kb::launch_group_merge(P, static_cast<const kb::GroupRecord*>(recs->p), (u32)total, ctx->n_sms, ctx->st);
-    kb::timer_end(ctx);
-    KB_CUDA(ctx, cudaGetLastError());
-    KB_TRY(kb::ctrl_read(ctx));
-    if (ctx->h_ctrl[off]) return kb::fail(ctx, KB_E_LIMIT, "group table overflow while merging partials");
-    KB_TRY(kb::group_table_collect(ctx, tab, h0.n_group_cols, aggs.data(), h0.n_aggs, g.get()));
-    *out = g.release();
-    return KB_OK;
-}
-
-kb_status kb_star_join_aggregate(kb_ctx* ctx, uint32_t join_slot, const kb_pattern* pats, uint32_t n_pats, const kb_filter_op* filter, uint32_t n_ops,
-                                 const uint32_t* group_slots, uint32_t n_group, const kb_agg* aggs, uint32_t n_aggs, kb_groups** out, uint64_t* n_rows) {
-    KB_ENTER(ctx);
-    if (!pats || !out || (n_group && !group_slots) || (n_aggs && !aggs)) return kb::fail(ctx, KB_E_INVALID, "NULL argument");
-    if (n_group == 0 || n_group > 4) return kb::fail(ctx, KB_E_LIMIT, "GROUP BY takes 1..4 variables");
-    if (n_aggs > 8) return kb::fail(ctx, KB_E_LIMIT, "at most 8 aggregates");
-    for (u32 a = 0; a < n_aggs; a++) if (aggs[a].kind > KB_AGG_AVG) return kb::fail(ctx, KB_E_INVALID, "unknown aggregate kind %u", aggs[a].kind);
-    const bool fusable = n_group == 1 && n_aggs <= 1;
-    kb::AggSpec spec(group_slots[0], n_aggs ? aggs : nullptr);
-    std::unique_ptr<kb_rel> rel;
-    KB_TRY(kb::star_join_impl(ctx, join_slot, pats, n_pats, filter, n_ops, &rel, fusable ? &spec : nullptr));
-    if (spec.applied) {
-        if (n_rows) *n_rows = spec.n_rows;
-        *out = spec.groups.release();
-        return KB_OK;
-    }
-    if (n_rows) *n_rows = rel->n;
-    return kb_group_aggregate(ctx, rel.get(), group_slots, n_group, aggs, n_aggs, out);
 }
 
 // ------------------------------------------------------------------ multi-GPU helpers

@@ -15,18 +15,6 @@ using namespace kb;
 
 namespace {
 
-struct DevGuard {  // the calling thread's current device is restored on return
-    int prev = -1;
-    explicit DevGuard(int dev) {
-        cudaGetDevice(&prev);
-        if (prev != dev) cudaSetDevice(dev);
-        else prev = -1;
-    }
-    ~DevGuard() {
-        if (prev >= 0) cudaSetDevice(prev);
-    }
-};
-
 // the reverse index holds every entry of the table and stays below load 1/2 with `extra` more entries (rebuilt larger otherwise)
 kb_status quoted_rev_ensure(kb_ctx* ctx, u64 extra) {
     const u64 need = ((u64)ctx->quoted_slots + extra) * 2 + 64;
@@ -242,11 +230,6 @@ kb_status bind_concat(kb_ctx* ctx, const kb_bind_spec& spec, const u32* const* c
 }
 
 }  // namespace
-
-#define KB_ENTER(ctx)                                         \
-    if (!(ctx)) return KB_E_INVALID;                          \
-    DevGuard _guard((ctx)->device);                           \
-    KB_TRY(kb::begin_call(ctx))
 
 extern "C" {
 

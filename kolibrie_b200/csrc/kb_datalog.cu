@@ -531,12 +531,7 @@ kb_status run_rounds(Fix& fx, const kb_rule* rules, u32 n_rules, const std::vect
 // is taken as closed under the rules already, the seed facts the store does not hold yet are accepted into it and form the first delta.
 static kb_status fixpoint_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rules, uint32_t strategy, bool seeded, const kb_rel* seed,
                                kb_rel** inferred, uint64_t* n_seed_new, kb_fixpoint_stats* stats) {
-    if (!ctx) return KB_E_INVALID;
-    int prev_dev = -1;
-    cudaGetDevice(&prev_dev);
-    cudaSetDevice(ctx->device);
-    struct Restore { int d; ~Restore() { if (d >= 0) cudaSetDevice(d); } } restore{prev_dev};
-    KB_TRY(begin_call(ctx));
+    KB_ENTER(ctx);
     if ((n_rules && !rules) || !inferred) return fail(ctx, KB_E_INVALID, "NULL argument");
     if (strategy != KB_SEMI_NAIVE && strategy != KB_NAIVE && strategy != KB_SEMI_NAIVE_PARALLEL && strategy != KB_SEMI_NAIVE_OLD_DELTA)
         return fail(ctx, KB_E_INVALID, "unknown strategy %u", strategy);
@@ -1288,12 +1283,7 @@ static kb_status maintain_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
 extern "C" kb_status kb_datalog_maintain(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rules, uint32_t strategy, const uint64_t* evict_tags,
                                          uint32_t n_evict, const kb_rel* add, uint64_t add_tag, kb_rel** inferred_removed, kb_rel** inferred_added,
                                          kb_maintain_stats* stats) {
-    if (!ctx) return KB_E_INVALID;
-    int prev_dev = -1;
-    cudaGetDevice(&prev_dev);
-    cudaSetDevice(ctx->device);
-    struct Restore { int d; ~Restore() { if (d >= 0) cudaSetDevice(d); } } restore{prev_dev};
-    KB_TRY(begin_call(ctx));
+    KB_ENTER(ctx);
     if (inferred_removed) *inferred_removed = nullptr;
     if (inferred_added) *inferred_added = nullptr;
     return maintain_impl(ctx, rules, n_rules, strategy, evict_tags, n_evict, add, add_tag, inferred_removed, inferred_added, stats);

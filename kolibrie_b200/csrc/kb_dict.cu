@@ -296,24 +296,6 @@ kb_status dict_encode_device(kb_ctx* ctx, const u64* d_off, const unsigned char*
 
 using namespace kb;
 
-namespace {
-struct DevGuard {  // the calling thread's current device is restored on return
-    int prev = -1;
-    explicit DevGuard(int dev) {
-        cudaGetDevice(&prev);
-        if (prev != dev) cudaSetDevice(dev);
-        else prev = -1;
-    }
-    ~DevGuard() {
-        if (prev >= 0) cudaSetDevice(prev);
-    }
-};
-}  // namespace
-#define KB_ENTER(ctx)                                         \
-    if (!(ctx)) return KB_E_INVALID;                          \
-    DevGuard _guard((ctx)->device);                           \
-    KB_TRY(kb::begin_call(ctx))
-
 extern "C" {
 
 kb_status kb_dict_encode(kb_ctx* ctx, const uint64_t* offsets, const uint8_t* bytes, uint64_t n_terms, uint32_t* out_ids, uint32_t* n_new_out,

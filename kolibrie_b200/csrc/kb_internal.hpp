@@ -94,7 +94,10 @@ struct kb_strings {
     kb::u64 n = 0, total = 0;
 };
 
-struct kb_groups {
+struct kb_groups {  // (kb_group.cu)
+    kb_groups(kb::u32 n_group, const kb_agg* aggs, kb::u32 n_aggs);  // no group yet: n_group key columns, the kinds of `aggs`
+    // appends one group: its key, its row count and the accumulators as the device left them
+    void add(const kb::u32* key, uint64_t count, const double* acc);
     std::vector<std::vector<kb::u32>> keys;
     std::vector<std::vector<double>> vals;
     std::vector<uint64_t> counts;
@@ -276,6 +279,11 @@ inline size_t round256(size_t b) { return (b + 255) & ~(size_t)255; }
         kb_status _s = (expr);           \
         if (_s != KB_OK) return _s;      \
     } while (0)
+// the preamble of an entry point that takes a context: the context's device is current until it returns, its control arena is zeroed
+#define KB_ENTER(ctx)                      \
+    if (!(ctx)) return KB_E_INVALID;       \
+    kb::DeviceGuard _guard((ctx)->device); \
+    KB_TRY(kb::begin_call(ctx))
 
 kb_status alloc_buf(kb_ctx* ctx, size_t bytes, Buf* out);
 kb_status alloc_col(kb_ctx* ctx, u64 rows, Col* out);
@@ -355,27 +363,34 @@ kb_status alloc_strided_cols(kb_ctx* ctx, u64 rows, u32 n_cols, std::vector<Col>
 kb_status compact_setup(kb_ctx* ctx, u64 n_tiles, u32* ctrl, Compact* c);
 // the row-writing launch of the one-kernel index join into n_out columns of probe_rows rows
 kb_status launch_index_rows(kb_ctx* ctx, ProbeIParams& P, const std::vector<Col>& cols);
-// GROUP BY hash table on the device (kb_group_aggregate and the fused path): one buffer [val | cnt | keys | state]
+// GROUP BY (kb_group.cu). The spec every entry point takes: group slots and aggregates present, 1..4 variables and at most 8
+// aggregates (KB_E_LIMIT), of known kinds (KB_E_INVALID). Each entry point adds its own restrictions.
+kb_status check_group_spec(kb_ctx* ctx, const uint32_t* group_slots, u32 n_group, const kb_agg* aggs, u32 n_aggs);
+// the GroupParams of n_group key columns and these aggregates, without input columns and table
+GroupParams group_params(const kb_ctx* ctx, u32 n_group, const kb_agg* aggs, u32 n_aggs);
+// the device hash table: one buffer [val | cnt | keys | state], and the overflow word, which is either a control-arena word (the
+// synchronous calls read it with the arena) or the 16 bytes behind the table (prepared plans: the word travels with the table)
 struct GroupTable {
     Buf buf;
     u64 slots = 0;
     size_t o_val = 0, o_cnt = 0, o_keys = 0, o_state = 0, bytes = 0;
+    u32* ctrl = nullptr;  // the control-arena word (ctrl_off), or null: the word is behind the table
+    u32 ctrl_off = 0;
     // point P at a table of this layout that starts at `base` (this table's buffer, or a rank's copy in peer scratch)
-    void point(GroupParams* P, char* base) const {
-        P->n_slots = (u32)slots;
-        P->gval = (double*)(base + o_val);
-        P->gcnt = (unsigned long long*)(base + o_cnt);
-        P->gkeys = (u32*)(base + o_keys);
-        P->gstate = (u32*)(base + o_state);
-    }
+    void point(GroupParams* P, char* base) const;
 };
-kb_status group_table_create(kb_ctx* ctx, u64 slots, GroupParams* P, GroupTable* t);  // allocates, points P at it, runs the init kernel
-// downloads the table and appends its groups to g (AVG divided, COUNT filled in)
-kb_status group_table_collect(kb_ctx* ctx, const GroupTable& t, u32 n_group, const kb_agg* aggs, u32 n_aggs, kb_groups* g);
-// the host half of it: `hb` = a host copy of the table's buffer
-void groups_from_host_table(const char* hb, const GroupTable& t, u32 n_group, const kb_agg* aggs, u32 n_aggs, kb_groups* g);
-// the same from a dense record list (launch_group_compact)
-void groups_from_records(const GroupRecord* recs, u64 n, u32 n_group, const kb_agg* aggs, u32 n_aggs, kb_groups* g);
+// allocates a table of `slots` slots, points P at it and runs the init kernel (which zeroes the overflow word); in_ctrl: the word
+// is a control-arena word, else it is behind the table
+kb_status group_table_create(kb_ctx* ctx, u64 slots, bool in_ctrl, GroupParams* P, GroupTable* t);
+// after a launch into a table whose word is in the control arena: reads the arena back, and unless *overflowed downloads the table
+// and appends its groups to g
+kb_status group_table_collect(kb_ctx* ctx, const GroupTable& t, kb_groups* g, bool* overflowed);
+// a grouped plan's partial tables in peer scratch: 64 flag words (256 bytes), then per ring slot one table laid out like t with its
+// overflow word behind it
+u64 group_peer_scratch_bytes(const GroupTable& t, u32 ring);
+char* group_peer_table(char* scratch, const GroupTable& t, u32 ring_slot);
+// what the peer merge of ring slot `ring_slot` reads: every rank's flags and partial table
+PeerTables group_peer_tables(const GroupTable& t, const std::vector<char*>& scratch, u32 rank, u32 ring_slot);
 kb_status segment_stats(kb_ctx* ctx, Segment* sg);
 // Changes to the store (kb_store.cu). Each one bumps store_version, which voids what is keyed to it (prepared plans, the seeded
 // fixpoint's state, the closed token), and clears the hint sets.

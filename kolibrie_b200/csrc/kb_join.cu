@@ -689,16 +689,11 @@ static kb_status index_join_one_kernel(kb_ctx* ctx, const StarQuery& q, const In
     if (ip.agg) {
         // GROUP BY folded into the probe kernel: no joined row is written. One try with a 4096-slot table; more groups than that (or
         // a group / aggregate variable the join does not bind) leave agg->applied false: the caller groups separately
-        GroupParams G{};
-        G.n_gcols = 1;
-        G.n_aggs = ip.has_agg ? 1u : 0u;
-        G.akind[0] = ip.agg_kind;
-        G.nt = numtab(ctx);
+        const kb_agg a1{agg->kind, agg->agg_slot};
+        const u32 n_aggs = agg->has_agg ? 1u : 0u;
+        GroupParams G = group_params(ctx, 1, &a1, n_aggs);
         GroupTable tab;
-        KB_TRY(group_table_create(ctx, 1u << 12, &G, &tab));
-        const u32 goff = ctrl_alloc(ctx, 4);
-        KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + goff, 0, 4 * sizeof(u32), ctx->st));
-        G.overflow = ctx->ctrl + goff;
+        KB_TRY(group_table_create(ctx, 1u << 12, true, &G, &tab));
         KB_TRY(compact_setup(ctx, P.n_tiles, ctx->fast_cb, &P.c));
         P.c.ordered = 0;  // the rows are folded into groups: no output order to keep
         timer_begin(ctx, F_PROBE);
@@ -707,14 +702,12 @@ static kb_status index_join_one_kernel(kb_ctx* ctx, const StarQuery& q, const In
         KB_CUDA(ctx, cudaGetLastError());
         ctx->stats.rows_probed += ip.probe_rows;
         ctx->stats.index_joins++;
-        KB_TRY(ctrl_read(ctx));
-        if (ctx->h_ctrl[goff] == 0) {
+        auto g = std::make_unique<kb_groups>(1, &a1, n_aggs);
+        bool overflowed;
+        KB_TRY(group_table_collect(ctx, tab, g.get(), &overflowed));
+        if (!overflowed) {
             agg->n_rows = *reinterpret_cast<volatile u32*>(ctx->h_fast);
-            agg->groups = std::make_unique<kb_groups>();
-            agg->groups->keys.resize(1);
-            agg->groups->vals.resize(agg->has_agg ? 1 : 0);
-            kb_agg a1{agg->kind, agg->agg_slot};
-            KB_TRY(group_table_collect(ctx, tab, 1, &a1, agg->has_agg ? 1u : 0u, agg->groups.get()));
+            agg->groups = std::move(g);
             agg->applied = true;
             return KB_OK;
         }

@@ -2,6 +2,7 @@
 // All of them are HBM-bound integer kernels: column tiles are staged global->shared with TMA bulk copies (cp.async.bulk +
 // mbarrier), matches are compacted with warp ballots, and output positions come from a single-pass decoupled look-back
 // prefix over tiles, so every kernel reads its input exactly once and writes a deterministic, input-ordered output.
+#include "kb_group.cuh"
 #include "kb_kernels.cuh"
 #include "kb_numrank.cuh"
 
@@ -12,10 +13,6 @@
 #include <type_traits>
 
 namespace kb {
-
-static inline u64 umin64(u64 a, u64 b) { return a < b ? a : b; }
-// grid-stride utility kernels are capped at a few CTAs per SM of an H100; the persistent kernels size their grids from the device's count
-constexpr u64 H100_SMS = 132;
 
 static inline int grid_for(const void* kernel, int threads, size_t smem, int n_sms, u32 n_tiles) {
     int per_sm = 1;
@@ -1291,9 +1288,6 @@ void launch_probe_fast(const ProbeFParams& p, int n_sms, cudaStream_t st) {
 // (execute_query.rs:1150-1227 over the rows of engine.rs:587-691): per warp __match_any_sync on the key, a 64-entry CTA table in shared
 // memory, flushed to the global group table when the CTA is done. Only the row count and the groups leave the kernel.
 constexpr int PI_GROUP_SMEM = 64;
-__device__ void group_update_global(const GroupParams& P, const u32* k, unsigned long long cnt, const double* val);
-__device__ void atomic_min_f64(double* addr, double v);
-__device__ void atomic_max_f64(double* addr, double v);
 // TAB = true: the probe stream is not the slice but the probe pattern's own persistent TABLE, walked slot by slot: slot i holds the
 // other half of the triple whose key is (table base + i), EMPTY32 where no triple has that key. The keys then come in ascending order
 // whatever the order of the store and of the dictionary ids, so the lookups into the other patterns' tables are sequential too — a
@@ -2356,369 +2350,6 @@ void launch_cartesian(const u32* const* lcols, u32 nl, u32 n_lcols, const u32* c
     if (total == 0) return;
     int grid = (int)umin64(H100_SMS * 8, (total + 255) / 256);
     cartesian_kernel<<<grid, 256, 0, st>>>(P);
-}
-
-// =================================================================================================================
-// K_group
-__device__ void atomic_min_f64(double* addr, double v) {
-    unsigned long long* a = reinterpret_cast<unsigned long long*>(addr);
-    unsigned long long old = *a;
-    while (v < __longlong_as_double((long long)old) || __longlong_as_double((long long)old) != __longlong_as_double((long long)old)) {
-        const unsigned long long assumed = old;
-        old = atomicCAS(a, assumed, (unsigned long long)__double_as_longlong(v));
-        if (old == assumed) break;
-    }
-}
-__device__ void atomic_max_f64(double* addr, double v) {
-    unsigned long long* a = reinterpret_cast<unsigned long long*>(addr);
-    unsigned long long old = *a;
-    while (v > __longlong_as_double((long long)old) || __longlong_as_double((long long)old) != __longlong_as_double((long long)old)) {
-        const unsigned long long assumed = old;
-        old = atomicCAS(a, assumed, (unsigned long long)__double_as_longlong(v));
-        if (old == assumed) break;
-    }
-}
-
-
-__global__ void group_init_kernel(const GroupParams P) {
-    const u32 stride = gridDim.x * blockDim.x;
-    if (P.overflow != nullptr && blockIdx.x == 0 && threadIdx.x == 0) *P.overflow = 0u;  // prepared plans: the flag lives behind the table
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < P.n_slots; i += stride) {
-        P.gstate[i] = 0u;
-        P.gcnt[i] = 0ull;
-        for (u32 a = 0; a < P.n_aggs; a++) P.gval[(u64)i * 8 + a] = agg_identity(P.akind[a]);
-    }
-}
-void launch_group_init(const GroupParams& p, cudaStream_t st) {
-    int grid = (int)umin64(H100_SMS * 4, ((u64)p.n_slots + 255) / 256);
-    group_init_kernel<<<grid, 256, 0, st>>>(p);
-}
-
-// find-or-insert the group of key k[] in the global table; returns slot or EMPTY32 on overflow
-__device__ __forceinline__ u32 group_slot(const GroupParams& P, const u32* k) {
-    u32 h = 0x9E3779B9u;
-    for (u32 c = 0; c < P.n_gcols; c++) h = mix32(h ^ k[c]) * 0x85EBCA77u + c;
-    const u32 mask = P.n_slots - 1u;
-    u32 slot = mix32(h) & mask;
-    for (u32 probes = 0; probes < P.n_slots; probes++) {
-        u32 st = *reinterpret_cast<volatile u32*>(&P.gstate[slot]);  // read first: a ready slot must not cost an atomic
-        if (st == 0u) st = atomicCAS(&P.gstate[slot], 0u, 1u);
-        else if (st == 2u) st = 3u;  // ready, skip the claim path
-        if (st == 0u) {
-            for (u32 c = 0; c < P.n_gcols; c++) P.gkeys[(u64)slot * 4 + c] = k[c];
-            __threadfence();
-            atomicExch(&P.gstate[slot], 2u);
-            return slot;
-        }
-        while (st == 1u) st = *reinterpret_cast<volatile u32*>(&P.gstate[slot]);
-        __threadfence();
-        bool eq = true;
-        for (u32 c = 0; c < P.n_gcols; c++) eq = eq && (*reinterpret_cast<volatile u32*>(&P.gkeys[(u64)slot * 4 + c]) == k[c]);
-        if (eq) return slot;
-        slot = (slot + 1u) & mask;
-    }
-    return EMPTY32;
-}
-
-// Two levels of pre-aggregation keep a GROUP BY with a handful of groups from serialising on a handful of addresses:
-// (1) a warp folds its 32 rows per distinct group (__match_any_sync), (2) leaders accumulate into a 64-entry shared-memory
-// table of the CTA, flushed to the global table once per CTA. Rows whose group does not fit the CTA table go straight to global.
-constexpr int GROUP_SMEM = 64;
-__device__ void group_update_global(const GroupParams& P, const u32* k, unsigned long long cnt, const double* val) {
-    const u32 slot = group_slot(P, k);
-    if (slot == EMPTY32) { *P.overflow = 1u; return; }
-    atomicAdd(&P.gcnt[slot], cnt);
-    for (u32 a = 0; a < P.n_aggs; a++) {
-        double* dst = &P.gval[(u64)slot * 8 + a];
-        if (P.akind[a] == KB_AGG_MIN) atomic_min_f64(dst, val[a]);
-        else if (P.akind[a] == KB_AGG_MAX) atomic_max_f64(dst, val[a]);
-        else if (P.akind[a] != KB_AGG_COUNT) atomicAdd(dst, val[a]);
-    }
-}
-
-__global__ void __launch_bounds__(256) group_merge_kernel(const __grid_constant__ GroupParams P, const GroupRecord* __restrict__ recs, u32 n) {
-    const u32 stride = gridDim.x * blockDim.x;
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-        const GroupRecord r = recs[i];
-        if (r.count == 0ull) continue;
-        group_update_global(P, r.keys, r.count, r.raw);
-    }
-}
-void launch_group_merge(const GroupParams& p, const GroupRecord* recs, u32 n, int n_sms, cudaStream_t st) {
-    if (n == 0) return;
-    const int grid = (int)umin64((u64)n_sms * 4ull, ((u64)n + 255ull) / 256ull);
-    group_merge_kernel<<<grid, 256, 0, st>>>(p, recs, n);
-}
-
-__global__ void __launch_bounds__(1024) group_compact_kernel(const __grid_constant__ GroupParams P, GroupRecord* __restrict__ out, u32* header, u32 cap) {
-    __shared__ u32 s_n;
-    if (threadIdx.x == 0) s_n = 0u;
-    __syncthreads();
-    for (u32 i = threadIdx.x; i < P.n_slots; i += blockDim.x) {
-        if (P.gstate[i] != 2u) continue;
-        const u32 at = atomicAdd(&s_n, 1u);
-        if (at >= cap) continue;
-        GroupRecord r;
-#pragma unroll
-        for (int c = 0; c < 4; c++) r.keys[c] = (u32)c < P.n_gcols ? P.gkeys[(u64)i * 4 + c] : 0u;
-        r.count = P.gcnt[i];
-#pragma unroll
-        for (int a = 0; a < 8; a++) r.raw[a] = (u32)a < P.n_aggs ? P.gval[(u64)i * 8 + a] : 0.0;
-        out[at] = r;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        header[1] = (P.overflow ? *P.overflow : 0u) | (s_n > cap ? 1u : 0u);
-        header[0] = min(s_n, cap);
-        __threadfence_system();
-    }
-}
-void launch_group_compact(const GroupParams& p, GroupRecord* out, u32* header, u32 cap, cudaStream_t st) {
-    group_compact_kernel<<<1, 1024, 0, st>>>(p, out, header, cap);
-}
-
-// ---- cross-rank GROUP BY over peer memory
-__device__ __forceinline__ void st_release_sys(u32* p, u32 v) { asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
-__device__ __forceinline__ u32 ld_acquire_sys(const u32* p) {
-    u32 v;
-    asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-template <class T>
-__device__ __forceinline__ T ld_sys(const T* p) { return *reinterpret_cast<const volatile T*>(p); }
-
-__global__ void __launch_bounds__(64) peer_barrier_kernel(const __grid_constant__ PeerTables T, u32 epoch) {
-    const u32 r = threadIdx.x;
-    __threadfence_system();
-    if (r < T.world) {
-        st_release_sys(T.flags[r] + T.rank, epoch);                                  // "I have arrived" in r's array
-        const u32* mine = T.flags[T.rank] + r;
-        unsigned long long t0, now;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-        while ((int)(ld_acquire_sys(mine) - epoch) < 0) {                            // r has arrived (epochs only grow; wrap-safe compare)
-            __nanosleep(100);
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
-            if (now - t0 > 5000000000ull) {  // 5 s: a rank never submitted this query — give up loudly instead of hanging the GPU
-                atomicExch(T.flags[T.rank] + 63, 1u);
-                break;
-            }
-        }
-    }
-    __syncthreads();
-    __threadfence_system();
-}
-void launch_peer_barrier(const PeerTables& t, u32 epoch, cudaStream_t st) { peer_barrier_kernel<<<1, 64, 0, st>>>(t, epoch); }
-
-__global__ void __launch_bounds__(256) group_merge_peers_kernel(const __grid_constant__ GroupParams P, const __grid_constant__ PeerTables T) {
-    const u32 total = T.world * T.n_slots;
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-        const u32 r = i / T.n_slots, s = i - r * T.n_slots;
-        const char* tb = T.table[r];
-        if (s == 0u && ld_sys(reinterpret_cast<const u32*>(tb + T.o_overflow)) != 0u) *P.overflow = 1u;  // a partial overflowed: so does the merge
-        if (i == 0u && ld_sys(T.flags[T.rank] + 63) != 0u) *P.overflow = 2u;                               // the barrier before this kernel timed out
-        if (ld_sys(reinterpret_cast<const u32*>(tb + T.o_state) + s) != 2u) continue;
-        u32 k[4];
-        double v[8];
-#pragma unroll
-        for (int c = 0; c < 4; c++) k[c] = ld_sys(reinterpret_cast<const u32*>(tb + T.o_keys) + (u64)s * 4 + c);
-        const unsigned long long cnt = ld_sys(reinterpret_cast<const unsigned long long*>(tb + T.o_cnt) + s);
-#pragma unroll
-        for (int a = 0; a < 8; a++) v[a] = (u32)a < P.n_aggs ? ld_sys(reinterpret_cast<const double*>(tb + T.o_val) + (u64)s * 8 + a) : 0.0;
-        group_update_global(P, k, cnt, v);
-    }
-}
-void launch_group_merge_peers(const GroupParams& p, const PeerTables& t, int n_sms, cudaStream_t st) {
-    const u64 total = (u64)t.world * t.n_slots;
-    const int grid = (int)umin64((u64)n_sms * 2ull, (total + 255ull) / 256ull);
-    group_merge_peers_kernel<<<grid, 256, 0, st>>>(p, t);
-}
-
-__global__ void __launch_bounds__(256) group_kernel(const __grid_constant__ GroupParams P) {
-    __shared__ u32 sk[GROUP_SMEM][4];
-    __shared__ u32 sstate[GROUP_SMEM];  // 0 free, 1 being written, 2 ready
-    __shared__ unsigned long long scnt[GROUP_SMEM];
-    __shared__ double sval[GROUP_SMEM][8];
-    for (int i = threadIdx.x; i < GROUP_SMEM; i += blockDim.x) {
-        sstate[i] = 0u;
-        scnt[i] = 0ull;
-        for (u32 a = 0; a < 8; a++) sval[i][a] = agg_identity(a < P.n_aggs ? P.akind[a] : (u32)KB_AGG_COUNT);
-    }
-    __syncthreads();
-    const int lane = threadIdx.x & 31;
-    const u32 stride = gridDim.x * blockDim.x;
-    const u32 n_round = (P.n + 31u) & ~31u;
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += stride) {
-        const bool valid = i < P.n;
-        u32 k[4] = {0, 0, 0, 0};
-        u32 h = 0;
-        if (valid) for (u32 c = 0; c < P.n_gcols; c++) { k[c] = P.gcol[c][i]; h = mix32(h ^ k[c]) + c; }
-        const unsigned act = __ballot_sync(0xffffffffu, valid);
-        if (!valid) continue;
-        // lanes with the same full key form a group: match on the hash, then confirm equality with the leader
-        unsigned peers = __match_any_sync(act, h);
-        int leader = __ffs(peers) - 1;
-        bool same = true;
-        for (u32 c = 0; c < P.n_gcols; c++) {  // every lane of `peers` must reach every shuffle: no short-circuit around it
-            const u32 lk = __shfl_sync(peers, k[c], leader);
-            same = same && lk == k[c];
-        }
-        const unsigned agree = __ballot_sync(act, same);
-        peers = same ? (peers & agree) : (1u << lane);  // rare hash collision inside a warp: the odd lanes go alone
-        leader = __ffs(peers) - 1;
-        double val[8];
-        for (u32 a = 0; a < P.n_aggs; a++) val[a] = P.acol[a] ? num_of(P.nt, P.acol[a][i]) : 0.0;
-        const unsigned long long cnt = (unsigned long long)__popc(peers);
-        for (u32 a = 0; a < P.n_aggs; a++) {
-            if (P.akind[a] == KB_AGG_COUNT) continue;  // COUNT needs no values: popc(peers) is the fold
-            double acc = val[a];
-            unsigned rest = peers & ~(1u << leader);
-            while (rest) {  // every lane of the group runs the same shuffles
-                const int src = __ffs(rest) - 1;
-                rest &= rest - 1u;
-                const double o = __shfl_sync(peers, val[a], src);
-                if (P.akind[a] == KB_AGG_MIN) acc = fmin(acc, o);
-                else if (P.akind[a] == KB_AGG_MAX) acc = fmax(acc, o);
-                else acc += o;
-            }
-            val[a] = acc;
-        }
-        if (lane != leader) continue;
-        // CTA table: find or claim
-        u32 slot = mix32(h) & (GROUP_SMEM - 1);
-        bool done = false;
-        for (int probes = 0; probes < GROUP_SMEM && !done; probes++) {
-            u32 st = *reinterpret_cast<volatile u32*>(&sstate[slot]);
-            if (st == 0u) st = atomicCAS(&sstate[slot], 0u, 1u);
-            else if (st == 2u) st = 3u;
-            if (st == 0u) {
-                for (u32 c = 0; c < 4; c++) sk[slot][c] = k[c];
-                __threadfence_block();
-                atomicExch(&sstate[slot], 2u);
-                st = 3u;
-            }
-            while (st == 1u) st = *reinterpret_cast<volatile u32*>(&sstate[slot]);
-            __threadfence_block();
-            bool eq = true;
-            for (u32 c = 0; c < P.n_gcols; c++) eq = eq && (*reinterpret_cast<volatile u32*>(&sk[slot][c]) == k[c]);
-            if (eq) {
-                atomicAdd(&scnt[slot], cnt);
-                for (u32 a = 0; a < P.n_aggs; a++) {
-                    if (P.akind[a] == KB_AGG_MIN) atomic_min_f64(&sval[slot][a], val[a]);
-                    else if (P.akind[a] == KB_AGG_MAX) atomic_max_f64(&sval[slot][a], val[a]);
-                    else if (P.akind[a] != KB_AGG_COUNT) atomicAdd(&sval[slot][a], val[a]);
-                }
-                done = true;
-            } else slot = (slot + 1u) & (GROUP_SMEM - 1);
-        }
-        if (!done) group_update_global(P, k, cnt, val);  // more than 64 distinct groups in this CTA
-    }
-    __syncthreads();
-    for (int i = threadIdx.x; i < GROUP_SMEM; i += blockDim.x) {
-        if (sstate[i] != 2u) continue;
-        u32 k[4] = {sk[i][0], sk[i][1], sk[i][2], sk[i][3]};
-        double v[8];
-        for (u32 a = 0; a < 8; a++) v[a] = sval[i][a];
-        group_update_global(P, k, scnt[i], v);
-    }
-}
-// GROUP BY one variable with at most one aggregate (GROUP BY ?t COUNT, SUM/AVG/MIN/MAX(?x) GROUP BY ?t — execute_query.rs:1150-1227):
-// the key itself is the match value, four rows per thread are loaded before any is folded (the loop is load-latency bound), the CTA
-// table is keyed by a CAS on the key word and counts are 32-bit shared atomics.
-template <int AGG>  // 0: COUNT only, else the kb_agg kind of the single value aggregate
-__global__ void __launch_bounds__(256) group1_kernel(const __grid_constant__ GroupParams P) {
-    constexpr int IT = 4;
-    __shared__ u32 sk[GROUP_SMEM];
-    __shared__ u32 scnt[GROUP_SMEM];
-    __shared__ double sval[GROUP_SMEM];
-    for (int i = threadIdx.x; i < GROUP_SMEM; i += blockDim.x) {
-        sk[i] = EMPTY32;
-        scnt[i] = 0u;
-        sval[i] = agg_identity((u32)AGG);
-    }
-    __syncthreads();
-    const int lane = threadIdx.x & 31;
-    const u32 stride = gridDim.x * blockDim.x;
-    const u32 n_round = (P.n + 31u) & ~31u;
-    const u32* __restrict__ kc = P.gcol[0];
-    const u32* __restrict__ ac = P.acol[0];
-    for (u32 i0 = blockIdx.x * blockDim.x + threadIdx.x; i0 < n_round; i0 += IT * stride) {
-        u32 key[IT];
-        double val[IT];
-#pragma unroll
-        for (int j = 0; j < IT; j++) {
-            const u32 i = i0 + (u32)j * stride;
-            key[j] = i < P.n ? __ldg(kc + i) : EMPTY32;
-            if (AGG != 0) val[j] = i < P.n ? num_of(P.nt, __ldg(ac + i)) : 0.0;
-        }
-#pragma unroll
-        for (int j = 0; j < IT; j++) {
-            const u32 i = i0 + (u32)j * stride;
-            if (i - (u32)lane >= P.n) continue;  // the whole warp is past the end (warp-uniform)
-            const bool valid = i < P.n;
-            const unsigned act = __ballot_sync(0xffffffffu, valid);
-            if (!valid) continue;
-            const unsigned peers = __match_any_sync(act, key[j]);
-            const int leader = __ffs(peers) - 1;
-            double acc = 0.0;
-            if (AGG != 0) {
-                acc = val[j];
-                unsigned rest = peers & ~(1u << leader);
-                while (rest) {
-                    const int src = __ffs(rest) - 1;
-                    rest &= rest - 1u;
-                    const double o = __shfl_sync(peers, val[j], src);
-                    if (AGG == KB_AGG_MIN) acc = fmin(acc, o);
-                    else if (AGG == KB_AGG_MAX) acc = fmax(acc, o);
-                    else acc += o;
-                }
-            }
-            if (lane != leader) continue;
-            const u32 cnt = (u32)__popc(peers);
-            u32 slot = mix32(key[j]) & (GROUP_SMEM - 1);
-            bool done = false;
-            for (int probes = 0; probes < GROUP_SMEM && !done && key[j] != EMPTY32; probes++) {  // EMPTY32 marks a free entry
-                u32 cur = *reinterpret_cast<volatile u32*>(&sk[slot]);
-                if (cur == EMPTY32) cur = atomicCAS(&sk[slot], EMPTY32, key[j]);
-                if (cur == EMPTY32 || cur == key[j]) {
-                    atomicAdd(&scnt[slot], cnt);
-                    if (AGG == KB_AGG_MIN) atomic_min_f64(&sval[slot], acc);
-                    else if (AGG == KB_AGG_MAX) atomic_max_f64(&sval[slot], acc);
-                    else if (AGG != 0) atomicAdd(&sval[slot], acc);
-                    done = true;
-                } else slot = (slot + 1u) & (GROUP_SMEM - 1);
-            }
-            if (!done) {  // more than 64 distinct groups in this CTA
-                u32 k[4] = {key[j], 0u, 0u, 0u};
-                double v[8] = {acc, 0, 0, 0, 0, 0, 0, 0};
-                group_update_global(P, k, (unsigned long long)cnt, v);
-            }
-        }
-    }
-    __syncthreads();
-    for (int i = threadIdx.x; i < GROUP_SMEM; i += blockDim.x) {
-        if (sk[i] == EMPTY32) continue;
-        u32 k[4] = {sk[i], 0u, 0u, 0u};
-        double v[8] = {sval[i], 0, 0, 0, 0, 0, 0, 0};
-        group_update_global(P, k, (unsigned long long)scnt[i], v);
-    }
-}
-void launch_group(const GroupParams& p, int n_sms, cudaStream_t st) {
-    if (p.n == 0) return;
-    if (p.n_gcols == 1 && p.n_aggs <= 1) {
-        // a CTA's 32-bit shared counters see at most n / grid * ... rows: far below 2^32
-        int grid = (int)umin64((u64)n_sms * 8ull, ((u64)p.n + 1023ull) / 1024ull);
-        const u32 kind = (p.n_aggs == 0 || p.akind[0] == KB_AGG_COUNT) ? 0u : p.akind[0];
-        switch (kind) {
-            case 0: group1_kernel<0><<<grid, 256, 0, st>>>(p); break;
-            case KB_AGG_SUM: group1_kernel<KB_AGG_SUM><<<grid, 256, 0, st>>>(p); break;
-            case KB_AGG_AVG: group1_kernel<KB_AGG_AVG><<<grid, 256, 0, st>>>(p); break;
-            case KB_AGG_MIN: group1_kernel<KB_AGG_MIN><<<grid, 256, 0, st>>>(p); break;
-            default: group1_kernel<KB_AGG_MAX><<<grid, 256, 0, st>>>(p); break;
-        }
-        return;
-    }
-    int grid = (int)umin64((u64)n_sms * 8ull, ((u64)p.n + 255ull) / 256ull);
-    group_kernel<<<grid, 256, 0, st>>>(p);
 }
 
 // =================================================================================================================

@@ -4,6 +4,10 @@
 
 namespace kb {
 
+static inline u64 umin64(u64 a, u64 b) { return a < b ? a : b; }
+// grid-stride utility kernels are capped at a few CTAs per SM of an H100; the persistent kernels size their grids from the device's count
+constexpr u64 H100_SMS = 132;
+
 // ---------------------------------------------------------------------------------------------------------------
 // K_scan: fused multi-pattern triple scan + constant filter + pushed-down FILTER + ordered compaction.
 // Replaces execute_table_scan_with_ids (engine.rs:510-584), the index scans (engine.rs:1192-1407), QueryBuilder's

@@ -143,24 +143,6 @@ kb_status ensure_num_order(kb_ctx* ctx, bool* ok) {
 
 using namespace kb;
 
-namespace {
-struct DevGuard {  // the calling thread's current device is restored on return
-    int prev = -1;
-    explicit DevGuard(int dev) {
-        cudaGetDevice(&prev);
-        if (prev != dev) cudaSetDevice(dev);
-        else prev = -1;
-    }
-    ~DevGuard() {
-        if (prev >= 0) cudaSetDevice(prev);
-    }
-};
-}  // namespace
-#define KB_ENTER(ctx)                                         \
-    if (!(ctx)) return KB_E_INVALID;                          \
-    DevGuard _guard((ctx)->device);                           \
-    KB_TRY(kb::begin_call(ctx))
-
 extern "C" {
 
 kb_status kb_dict_numeric_derive(kb_ctx* ctx, uint32_t tables, uint32_t first_id, kb_numeric_info* info) {

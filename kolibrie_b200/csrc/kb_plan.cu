@@ -33,29 +33,15 @@ struct kb_plan {
     u32* d_totals = nullptr;
     u64 next_ticket = 1;
     kb_agg agg1{};
-    // kb_plan_attach_peers: the partial group tables live in peer-mapped scratch [flags: 64 words][ring x table_stride]; after a
-    // device-side barrier a merge kernel reads every rank's partial table over NVLink into the slot's local merged table
+    // kb_plan_attach_peers: the partial group tables live in peer-mapped scratch (group_peer_table); after a device-side barrier a
+    // merge kernel reads every rank's partial table over NVLink into the slot's local merged table
     bool attached = false;
-    u32 world = 1, rank = 0;
-    size_t table_stride = 0;
+    u32 rank = 0;
     std::vector<char*> peer_scratch;
-    struct Merged {
-        GroupTable tab;
-    };
-    std::vector<Merged> merged;
+    std::vector<GroupTable> merged;
 };
 
 namespace {
-struct DevGuard {
-    int prev = -1;
-    explicit DevGuard(int dev) {
-        cudaGetDevice(&prev);
-        if (prev != dev) cudaSetDevice(dev);
-        else prev = -1;
-    }
-    ~DevGuard() { if (prev >= 0) cudaSetDevice(prev); }
-};
-
 void plan_release(kb_plan* pl) {
     for (auto& s : pl->slots) {
         if (s.done) cudaEventDestroy(s.done);
@@ -71,9 +57,7 @@ extern "C" {
 
 kb_status kb_star_join_prepare(kb_ctx* ctx, uint32_t join_slot, const kb_pattern* pats, uint32_t n_pats, const kb_filter_op* filter, uint32_t n_ops,
                                const uint32_t* group_slots, uint32_t n_group, const kb_agg* aggs, uint32_t n_aggs, uint32_t ring, kb_plan** out) {
-    if (!ctx) return KB_E_INVALID;
-    DevGuard guard(ctx->device);
-    KB_TRY(begin_call(ctx));
+    KB_ENTER(ctx);
     if (!pats || !out) return fail(ctx, KB_E_INVALID, "NULL argument");
     if (ring == 0 || ring > 64) return fail(ctx, KB_E_LIMIT, "ring depth must be 1..64 (got %u)", ring);
     if ((n_group && !group_slots) || (n_aggs && !aggs)) return fail(ctx, KB_E_INVALID, "NULL argument");
@@ -81,7 +65,7 @@ kb_status kb_star_join_prepare(kb_ctx* ctx, uint32_t join_slot, const kb_pattern
     if (grouped && (n_group != 1 || n_aggs > 1))
         return fail(ctx, KB_E_UNSUPPORTED, "a prepared GROUP BY takes one variable and at most one aggregate (other shapes: kb_star_join + kb_group_aggregate)");
     if (!grouped && n_aggs) return fail(ctx, KB_E_INVALID, "aggregates without GROUP BY");
-    if (n_aggs && aggs[0].kind > KB_AGG_AVG) return fail(ctx, KB_E_INVALID, "unknown aggregate kind %u", aggs[0].kind);
+    if (grouped) KB_TRY(check_group_spec(ctx, group_slots, n_group, aggs, n_aggs));
     AggSpec spec(grouped ? group_slots[0] : 0u, n_aggs ? aggs : nullptr);
     auto pl = std::unique_ptr<kb_plan, void (*)(kb_plan*)>(new kb_plan, plan_release);
     KB_TRY(resolve_index_plan(ctx, join_slot, pats, n_pats, filter, n_ops, grouped ? &spec : nullptr, &pl->ip));
@@ -105,11 +89,7 @@ kb_status kb_star_join_prepare(kb_ctx* ctx, uint32_t join_slot, const kb_pattern
         KB_CUDA(ctx, cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
         if (ip.agg) {
             GroupParams G{};
-            KB_TRY(group_table_create(ctx, 1u << 12, &G, &s.tab));  // the same 4096-slot table the synchronous fused path tries first
-            // the overflow word rides behind the table so that ONE copy brings both to the host
-            Buf b;
-            KB_TRY(alloc_buf(ctx, s.tab.bytes + 16, &b));
-            s.tab.buf = b;
+            KB_TRY(group_table_create(ctx, 1u << 12, false, &G, &s.tab));  // the same 4096-slot table the synchronous fused path tries first
             s.rec_cap = (u32)s.tab.slots;
             KB_CUDA(ctx, cudaHostAlloc(reinterpret_cast<void**>(&s.h_rec), 16 + (size_t)s.rec_cap * sizeof(GroupRecord), cudaHostAllocMapped));
             memset(s.h_rec, 0, 16);
@@ -126,7 +106,7 @@ kb_status kb_star_join_prepare(kb_ctx* ctx, uint32_t join_slot, const kb_pattern
 
 kb_status kb_plan_submit(kb_ctx* ctx, kb_plan* pl, uint64_t* ticket) {
     if (!ctx || !pl || pl->ctx != ctx) return KB_E_INVALID;
-    DevGuard guard(ctx->device);
+    DeviceGuard guard(ctx->device);
     if (pl->store_version != ctx->store_version || pl->index_version != ctx->index_version || ctx->index_version != ctx->store_version ||
         pl->num_version != ctx->num_version || pl->shard_world != ctx->shard_world)
         return fail(ctx, KB_E_INVALID, "stale plan: the store, its index or the numeric table changed since kb_star_join_prepare");
@@ -137,15 +117,9 @@ kb_status kb_plan_submit(kb_ctx* ctx, kb_plan* pl, uint64_t* ticket) {
     P.cb = ctx->fast_cb;  // launches of one context are serialised on its stream: they share the self-cleaning control block
     P.host_total = pl->d_totals + (t % pl->ring) * 16;
     if (pl->ip.agg) {
-        GroupParams G{};
-        G.n_gcols = 1;
-        G.n_aggs = pl->ip.has_agg ? 1u : 0u;
-        G.akind[0] = pl->ip.agg_kind;
-        G.nt = numtab(ctx);
+        GroupParams G = group_params(ctx, 1, &pl->agg1, pl->ip.has_agg ? 1u : 0u);
         const u32 si = (u32)(t % pl->ring);
-        char* tb = pl->attached ? pl->peer_scratch[pl->rank] + 256 + (size_t)si * pl->table_stride : static_cast<char*>(s.tab.buf->p);
-        s.tab.point(&G, tb);
-        G.overflow = (u32*)(tb + s.tab.bytes);
+        s.tab.point(&G, pl->attached ? group_peer_table(pl->peer_scratch[pl->rank], s.tab, si) : static_cast<char*>(s.tab.buf->p));
         KB_TRY(compact_setup(ctx, P.n_tiles, ctx->fast_cb, &P.c));
         P.c.ordered = 0;  // the rows are folded into groups: no output order to keep
         timer_begin(ctx, F_GROUP);
@@ -158,20 +132,9 @@ kb_status kb_plan_submit(kb_ctx* ctx, kb_plan* pl, uint64_t* ticket) {
         if (pl->attached) {
             // device-side barrier (every rank's partial table of this ticket is complete and visible), then ONE kernel folds all the
             // partial tables, read from the peers' memory, into this slot's merged table
-            PeerTables T{};
-            T.world = pl->world; T.rank = pl->rank;
-            T.n_slots = (u32)s.tab.slots;
-            T.o_val = (u32)s.tab.o_val; T.o_cnt = (u32)s.tab.o_cnt; T.o_keys = (u32)s.tab.o_keys; T.o_state = (u32)s.tab.o_state;
-            T.o_overflow = (u32)s.tab.bytes;
-            for (u32 r = 0; r < pl->world; r++) {
-                T.flags[r] = reinterpret_cast<u32*>(pl->peer_scratch[r]);
-                T.table[r] = pl->peer_scratch[r] + 256 + (size_t)si * pl->table_stride;
-            }
-            kb_plan::Merged& M = pl->merged[si];
+            const PeerTables T = group_peer_tables(s.tab, pl->peer_scratch, pl->rank, si);
             GroupParams Gm = G;
-            char* mb = static_cast<char*>(M.tab.buf->p);
-            M.tab.point(&Gm, mb);
-            Gm.overflow = (u32*)(mb + M.tab.bytes);
+            pl->merged[si].point(&Gm, static_cast<char*>(pl->merged[si].buf->p));
             timer_begin(ctx, F_GROUP, 3);
             launch_peer_barrier(T, (u32)t, ctx->st);
             launch_group_init(Gm, ctx->st);
@@ -201,7 +164,7 @@ kb_status kb_plan_submit(kb_ctx* ctx, kb_plan* pl, uint64_t* ticket) {
 
 kb_status kb_plan_collect(kb_ctx* ctx, kb_plan* pl, uint64_t ticket, uint64_t* n_rows, kb_rel** rows, kb_groups** groups) {
     if (!ctx || !pl || pl->ctx != ctx) return KB_E_INVALID;
-    DevGuard guard(ctx->device);
+    DeviceGuard guard(ctx->device);
     kb_plan::Slot& s = pl->slots[ticket % pl->ring];
     if (!s.busy || s.ticket != ticket)
         return fail(ctx, KB_E_NOT_FOUND, "ticket %llu is not in flight (already collected, or its ring slot was never submitted)", (unsigned long long)ticket);
@@ -224,10 +187,9 @@ kb_status kb_plan_collect(kb_ctx* ctx, kb_plan* pl, uint64_t ticket, uint64_t* n
             return fail(ctx, KB_E_LIMIT, "more than %llu groups%s: the prepared GROUP BY holds fixed tables (use kb_star_join + kb_group_aggregate)",
                         (unsigned long long)s.tab.slots, pl->attached ? " on some rank or in the merge" : "");
         if (groups) {
-            auto g = std::make_unique<kb_groups>();
-            g->keys.resize(1);
-            g->vals.resize(pl->ip.has_agg ? 1 : 0);
-            groups_from_records(reinterpret_cast<const GroupRecord*>(s.h_rec + 16), n_groups, 1, &pl->agg1, pl->ip.has_agg ? 1u : 0u, g.get());
+            auto g = std::make_unique<kb_groups>(1, &pl->agg1, pl->ip.has_agg ? 1u : 0u);
+            const GroupRecord* rec = reinterpret_cast<const GroupRecord*>(s.h_rec + 16);
+            for (u32 i = 0; i < n_groups; i++) g->add(rec[i].keys, rec[i].count, rec[i].raw);
             *groups = g.release();
         }
         return KB_OK;
@@ -251,21 +213,18 @@ kb_status kb_plan_collect(kb_ctx* ctx, kb_plan* pl, uint64_t ticket, uint64_t* n
 
 uint64_t kb_plan_peer_scratch_bytes(const kb_plan* pl) {
     if (!pl || !pl->ip.agg) return 0;
-    const size_t stride = round256(pl->slots[0].tab.bytes + 16);
-    return 256 + (uint64_t)pl->ring * stride;
+    return group_peer_scratch_bytes(pl->slots[0].tab, pl->ring);
 }
 
 kb_status kb_plan_attach_peers(kb_ctx* ctx, kb_plan* pl, uint32_t rank, uint32_t world, void* const* peer_scratch) {
     if (!ctx || !pl || pl->ctx != ctx) return KB_E_INVALID;
-    DevGuard guard(ctx->device);
+    DeviceGuard guard(ctx->device);
     if (!pl->ip.agg) return fail(ctx, KB_E_UNSUPPORTED, "only grouped plans merge across ranks (row plans need no exchange for subject stars)");
     if (!peer_scratch || world == 0 || world > 64 || rank >= world) return fail(ctx, KB_E_INVALID, "rank %u / world %u (1..64 ranks)", rank, world);
     if (pl->ring < 2) return fail(ctx, KB_E_INVALID, "a plan that merges across ranks needs a ring of at least 2 (a slot must not be refilled while a peer still reads it)");
     if (pl->next_ticket != 1) return fail(ctx, KB_E_INVALID, "attach the peers before the first submit");
     for (u32 r = 0; r < world; r++) if (!peer_scratch[r]) return fail(ctx, KB_E_INVALID, "peer scratch %u is NULL", r);
-    pl->world = world;
     pl->rank = rank;
-    pl->table_stride = round256(pl->slots[0].tab.bytes + 16);
     pl->peer_scratch.assign(world, nullptr);
     for (u32 r = 0; r < world; r++) pl->peer_scratch[r] = static_cast<char*>(peer_scratch[r]);
     pl->merged.resize(pl->ring);
@@ -273,10 +232,7 @@ kb_status kb_plan_attach_peers(kb_ctx* ctx, kb_plan* pl, uint32_t rank, uint32_t
         GroupParams G{};
         // the GLOBAL result is bounded like a rank's: at most `slots` groups (the record list's capacity); the merged table holds
         // them at load <= 1/2, more distinct groups than that are reported as overflow by the compaction
-        KB_TRY(group_table_create(ctx, 2 * pl->slots[0].tab.slots, &G, &pl->merged[i].tab));
-        Buf b;
-        KB_TRY(alloc_buf(ctx, pl->merged[i].tab.bytes + 16, &b));
-        pl->merged[i].tab.buf = b;
+        KB_TRY(group_table_create(ctx, 2 * pl->slots[0].tab.slots, false, &G, &pl->merged[i]));
     }
     KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
     pl->attached = true;
@@ -296,7 +252,7 @@ kb_status kb_plan_info(const kb_plan* pl, uint32_t* ring, uint64_t* capacity_row
 void kb_plan_free(kb_ctx* ctx, kb_plan* pl) {
     if (!pl) return;
     if (pl->life && pl->life->alive && pl->ctx) {
-        DevGuard guard(pl->ctx->device);
+        DeviceGuard guard(pl->ctx->device);
         cudaStreamSynchronize(pl->ctx->st);  // launches still reading the ring
         plan_release(pl);
     } else {

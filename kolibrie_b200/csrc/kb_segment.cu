@@ -38,11 +38,6 @@ struct File {
     FILE* f = nullptr;
     ~File() { if (f) fclose(f); }
 };
-struct DevGuard {
-    int prev = -1;
-    explicit DevGuard(int dev) { cudaGetDevice(&prev); if (prev != dev) cudaSetDevice(dev); else prev = -1; }
-    ~DevGuard() { if (prev >= 0) cudaSetDevice(prev); }
-};
 }  // namespace
 
 extern "C" {
@@ -91,7 +86,7 @@ kb_status kb_segment_info(const char* path, uint64_t* n_triples, uint64_t* tag, 
 
 kb_status kb_segment_save(kb_ctx* ctx, uint64_t tag, int whole_store, const char* path) {
     if (!ctx || !path) return KB_E_INVALID;
-    DevGuard guard(ctx->device);
+    DeviceGuard guard(ctx->device);
     KB_TRY(begin_call(ctx));
     uint64_t n = 0;
     for (auto& sg : ctx->segs) if (whole_store || sg.tag == tag) n += sg.n;
@@ -119,7 +114,7 @@ kb_status kb_segment_save(kb_ctx* ctx, uint64_t tag, int whole_store, const char
 
 extern "C" kb_status kb_store_append_file(kb_ctx* ctx, const char* path, uint64_t tag, int verify) {
     if (!ctx || !path) return KB_E_INVALID;
-    DevGuard guard(ctx->device);
+    DeviceGuard guard(ctx->device);
     KB_TRY(begin_call(ctx));
     File fh;
     fh.f = fopen(path, "rb");

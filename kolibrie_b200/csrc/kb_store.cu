@@ -10,11 +10,6 @@
 
 using namespace kb;
 
-#define KB_ENTER(ctx)                                         \
-    if (!(ctx)) return KB_E_INVALID;                          \
-    kb::DeviceGuard _guard((ctx)->device);                    \
-    KB_TRY(kb::begin_call(ctx))
-
 namespace kb {
 
 kb_status segment_stats(kb_ctx* ctx, Segment* sg) {
