@@ -335,6 +335,28 @@ typedef struct kb_bind_info {
 } kb_bind_info;
 KB_API kb_status kb_bind(kb_ctx* ctx, const kb_rel* in, const kb_bind_spec* spec, kb_rel** out, kb_bind_info* info);
 
+/* ------------------------------------------------------------------ VALUES: `PhysicalOperator::Values` (engine.rs:279-308) as a device
+ * relation. The block has n_vars header variables (slots[v]; a slot may repeat) and n_rows rows; cell (r, v) is row-major index
+ * i = r * n_vars + v, its bytes are bytes[offsets[i] .. offsets[i+1]) and undef[i] != 0 marks it UNDEF (an UNDEF cell must be empty;
+ * a row shorter than the header has UNDEF trailing cells, as `value_row.get(i)` gives None).
+ *   Encode. Every defined cell is Dictionary::encode'd VERBATIM (no prefix resolution, no bracket stripping), rows in order, cells in
+ *     header order: the ids are those of that sequential loop, and new strings join the device dictionary in first-seen order as ids
+ *     [info.dict_first, info.dict_first + info.dict_new) (kb_dict_strings_download fetches them). When the f64 numeric side table
+ *     covers exactly the ids the dictionary held, it is extended over the new ids (kb_dict_numeric_derive, KB_NUMERIC_APPEND: one
+ *     parse of the new strings); a table that is shorter or longer is left as it is, for the caller to derive.
+ *   *out. One column per distinct slot, in order of first appearance in the header. Row r's cell of slot s is the id of its LAST
+ *     defined cell of s (row.insert overwrites), else KB_ID_NONE (the row does not bind s). A row without a defined cell is dropped
+ *     (`if !row.is_empty()`), the others keep their order; info.rows_dropped counts the dropped rows.
+ *   Refused before the dictionary changes: a NULL argument, offsets not starting at 0 or decreasing, a non-empty UNDEF cell
+ *     (KB_E_INVALID); more than KB_MAX_COLS distinct slots, 2^32-16 rows or cells or bytes or more, new ids reaching bit 31 (KB_E_LIMIT).
+ * Launches and device time count in kb_stats' `other` family (flags, two scans, compaction, kb_dict_encode's launches, scatter). */
+typedef struct kb_values_info {
+    uint32_t dict_first, dict_new;
+    uint64_t rows_dropped;
+} kb_values_info;
+KB_API kb_status kb_values(kb_ctx* ctx, const uint32_t* slots, uint32_t n_vars, uint64_t n_rows, const uint8_t* undef, const uint64_t* offsets,
+                           const uint8_t* bytes, kb_rel** out, kb_values_info* info /* nullable */);
+
 /* ------------------------------------------------------------------ relations */
 KB_API kb_status kb_rel_info(const kb_rel* r, uint64_t* n_rows, uint32_t* n_cols, uint32_t* slots /* [KB_MAX_COLS] or NULL */);
 KB_API kb_status kb_rel_download(kb_ctx* ctx, const kb_rel* r, uint32_t col, uint32_t* host_dst /* n_rows */);
@@ -378,6 +400,28 @@ KB_API kb_status kb_hash_join(kb_ctx* ctx, const kb_rel* left, const kb_rel* rig
  * Refused before any output exists (*out untouched): |U| > 4 (more than 256 mask pairs), a join key of more than 4 slots, more than
  * KB_MAX_COLS output columns, a relation of 2^32 rows or more, an output of 2^32 rows or more (KB_E_LIMIT). */
 KB_API kb_status kb_natural_join(kb_ctx* ctx, const kb_rel* left, const kb_rel* right, kb_rel** out);
+/* The hash joins of the Streamertail engine over rows that may leave variables unbound (a VALUES block with UNDEF cells, kb_values):
+ * HashJoin, OptimizedHashJoin, the merge join and their cartesian product (engine.rs:710-811, 970-1071). Their key is NOT the shared
+ * slots: it is the variables bound in row 0 of both sides, which the caller reads and passes as key_slots (n_key = 0: the cartesian
+ * product, limited to 2^28 rows as in kb_hash_join). Row 0 is the reference's row 0 only where the caller's relation lies in the
+ * reference's order (kb_values' output, a scan); the output of a join lies in device order, so above one the key the caller reads
+ * may differ from the reference's, whose row 0 is hash-iteration order there.
+ *   Columns. As kb_natural_join: `left`'s slots in order, then the slots of `right` that `left` lacks.
+ *   Rows. A (left, right) row pair is emitted iff its key cells are equal; no other slot is compared. Every other slot both sides hold
+ *     is coalesced by `merge`: KB_MERGE_LEFT_FIRST keeps the left cell when it is bound, else the right one (HashJoin and the merge join
+ *     insert only the keys the left row lacks; OptimizedHashJoin when the right side is its build side); KB_MERGE_RIGHT_FIRST the other
+ *     way round (OptimizedHashJoin with the left side as build side — the smaller side, left on ties — and the cartesian product, whose
+ *     `extend` overwrites). A bag; row order is unspecified; either side empty -> 0 rows (engine.rs:714, 770, 974).
+ *   Refused before any output exists (*out untouched): a key cell holding KB_ID_NONE on either side, when both sides have rows
+ *     (KB_E_UNSUPPORTED: there the reference panics on `tuple[var]`, or its merge join compares keys of different shapes); a NULL argument,
+ *     an unknown policy, a key slot that is not a column of both sides or is repeated (KB_E_INVALID); more than 4 key slots (checked
+ *     first, before any launch), more than KB_MAX_COLS output columns, a relation or output of 2^32 rows or more (KB_E_LIMIT).
+ * Launches: the check pass (when n_key > 0 and both sides have rows), one row-index launch per non-empty side, kb_hash_join's launches
+ * for the (key, row index) views, and one coalesce launch when the output has rows; the check, index and coalesce launches count in
+ * kb_stats' `other` family. */
+enum kb_merge_policy { KB_MERGE_LEFT_FIRST = 0, KB_MERGE_RIGHT_FIRST = 1 };
+KB_API kb_status kb_hash_join_keyed(kb_ctx* ctx, const kb_rel* left, const kb_rel* right, const uint32_t* key_slots, uint32_t n_key,
+                                    uint32_t merge, kb_rel** out);
 /* BindJoin of a relation with ONE store pattern (engine.rs:840-885): natural join of `left` with the pattern's matches. With a valid store
  * index, the pattern (?x P ?y) and exactly one of its variables bound by `left` through a unique dense column of the predicate, it is
  * one probe kernel against the index's persistent table (the reference's spo[x][P] / pos[P][y] lookups); otherwise scan + hash join. */

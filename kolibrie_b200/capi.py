@@ -70,6 +70,17 @@ class KbBindInfo(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+class KbValuesInfo(C.Structure):
+    """kb_values_info: the new dictionary ids (first, count) and the rows dropped for having no defined cell"""
+    _fields_ = [("dict_first", C.c_uint32), ("dict_new", C.c_uint32), ("rows_dropped", C.c_uint64)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
+MERGE_LEFT_FIRST, MERGE_RIGHT_FIRST = 0, 1  # kb_merge_policy
+
+
 class KbNumericInfo(C.Structure):
     """kb_numeric_info: ids of the device dictionary, ids parsed, how many of them are numbers / i32, how many took the slow path"""
     _fields_ = [("n_ids", C.c_uint32), ("n_derived", C.c_uint32), ("n_numeric", C.c_uint32), ("n_i32", C.c_uint32), ("n_slow", C.c_uint32)]
@@ -271,6 +282,8 @@ def lib() -> C.CDLL:
         "kb_project": (i32, [vp, vp, P(u32), u32, P(vp)]),
         "kb_hash_join": (i32, [vp, vp, vp, P(vp)]),
         "kb_natural_join": (i32, [vp, vp, vp, P(vp)]),
+        "kb_hash_join_keyed": (i32, [vp, vp, vp, P(u32), u32, u32, P(vp)]),
+        "kb_values": (i32, [vp, P(u32), u32, u64, vp, vp, vp, P(vp), P(KbValuesInfo)]),
         "kb_bind_join": (i32, [vp, vp, P(KbPattern), P(vp)]),
         "kb_scan_quoted": (i32, [vp, P(KbQuotedPattern), P(vp)]),
         "kb_star_join": (i32, [vp, u32, P(KbPattern), u32, P(KbFilterOp), u32, P(vp)]),
@@ -327,7 +340,7 @@ EXPORTED_SYMBOLS = [
     "kb_version", "kb_ctx_create", "kb_ctx_destroy", "kb_last_error", "kb_set_timing", "kb_get_stats", "kb_synchronize",
     "kb_store_load", "kb_store_load_device", "kb_store_append", "kb_store_append_device", "kb_store_evict", "kb_store_delete", "kb_store_clear", "kb_store_build_index", "kb_set_use_index", "kb_store_size",
     "kb_store_download", "kb_dict_numeric_load", "kb_dict_legacy_i32_load", "kb_dict_numeric_derive", "kb_dict_numeric_download", "kb_dict_strings_load", "kb_dict_encode", "kb_dict_strings_info", "kb_rel_decode", "kb_strings_info", "kb_strings_download", "kb_strings_free", "kb_quoted_load", "kb_quoted_download", "kb_dict_strings_download", "kb_bind", "kb_rel_info", "kb_rel_download", "kb_rel_device_col", "kb_rel_from_host",
-    "kb_rel_from_device", "kb_rel_free", "kb_scan", "kb_filter", "kb_project", "kb_hash_join", "kb_natural_join", "kb_bind_join", "kb_scan_quoted", "kb_star_join", "kb_bgp_execute", "kb_bgp_last_plan",
+    "kb_rel_from_device", "kb_rel_free", "kb_scan", "kb_filter", "kb_project", "kb_hash_join", "kb_natural_join", "kb_hash_join_keyed", "kb_values", "kb_bind_join", "kb_scan_quoted", "kb_star_join", "kb_bgp_execute", "kb_bgp_last_plan",
     "kb_order_by", "kb_group_aggregate", "kb_groups_info", "kb_groups_keys", "kb_groups_values", "kb_groups_counts", "kb_groups_free", "kb_groups_pack", "kb_groups_merge", "kb_star_join_aggregate",
     "kb_star_join_prepare", "kb_plan_submit", "kb_plan_collect", "kb_plan_info", "kb_plan_free", "kb_plan_peer_scratch_bytes", "kb_plan_attach_peers",
     "kb_datalog_fixpoint", "kb_datalog_fixpoint_seed", "kb_datalog_maintain", "kb_r2s_create", "kb_r2s_eval", "kb_r2s_info", "kb_r2s_free", "kb_shard_of", "kb_set_sharding", "kb_partition", "kb_partition_counts", "kb_segment_write", "kb_segment_info", "kb_segment_save", "kb_store_append_file", "kb_shuffle_scatter", "kb_shuffle_push", "kb_rel_wrap_device", "kb_star_join_host", "kb_star_join_host_into", "perform_hash_join_cuda",
@@ -647,6 +660,36 @@ class Context:
         out = C.c_void_p()
         self._check(lib().kb_natural_join(self.h, left.h, right.h, C.byref(out)))
         return Relation(self, out)
+
+    def hash_join_keyed(self, left: Relation, right: Relation, key_slots: Sequence[int], merge: int) -> Relation:
+        """kb_hash_join_keyed: rows paired on key_slots only, every other shared slot coalesced MERGE_LEFT_FIRST or MERGE_RIGHT_FIRST;
+        a key cell holding KB_ID_NONE raises KB_E_UNSUPPORTED"""
+        keys = (C.c_uint32 * max(len(key_slots), 1))(*key_slots)
+        out = C.c_void_p()
+        self._check(lib().kb_hash_join_keyed(self.h, left.h, right.h, keys, len(key_slots), merge, C.byref(out)))
+        return Relation(self, out)
+
+    def values(self, slots: Sequence[int], rows: Sequence[Sequence[Optional[Union[str, bytes]]]]) -> Tuple[Relation, dict]:
+        """kb_values: a VALUES block as a device relation. rows[r][v] is the term of header variable slots[v], None for UNDEF; a row
+        shorter than the header is UNDEF in its missing cells. Returns (relation, kb_values_info as a dict)."""
+        nv, nr = len(slots), len(rows)
+        undef = np.ones(nr * nv, dtype=np.uint8)
+        lens = np.zeros(nr * nv, dtype=np.uint64)
+        parts = []
+        for r, row in enumerate(rows):
+            for v, t in enumerate(row[:nv]):
+                if t is not None:
+                    b = t.encode("utf-8") if isinstance(t, str) else bytes(t)
+                    undef[r * nv + v] = 0
+                    lens[r * nv + v] = len(b)
+                    parts.append(b)
+        off = np.zeros(nr * nv + 1, dtype=np.uint64)
+        off[1:] = np.cumsum(lens, dtype=np.uint64)
+        data = np.frombuffer(b"".join(parts) or b"\0", dtype=np.uint8).copy()
+        sl = (C.c_uint32 * max(nv, 1))(*slots)
+        out, info = C.c_void_p(), KbValuesInfo()
+        self._check(lib().kb_values(self.h, sl, nv, nr, _ptr(undef) if len(undef) else None, _ptr(off), _ptr(data), C.byref(out), C.byref(info)))
+        return Relation(self, out), info.as_dict()
 
     def bind_join(self, left: Relation, pat: KbPattern) -> Relation:
         """kb_bind_join: `left` joined with one store pattern (index lookup kernel when the index has a table for it)"""

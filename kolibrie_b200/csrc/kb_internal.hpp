@@ -414,6 +414,8 @@ QuotedTab quotedtab(const kb_ctx* ctx);
 // kb_dict_encode's body over a batch already in device memory (kb_dict.cu)
 kb_status dict_encode_device(kb_ctx* ctx, const u64* d_off, const unsigned char* d_bytes, u64 n_terms, u64 total, u32* d_out_ids, u32* n_new,
                              Buf* first_pos);
+// kb_dict_numeric_derive behind the entry point (kb_numeric.cu)
+kb_status numeric_derive(kb_ctx* ctx, uint32_t tables, uint32_t first_id, kb_numeric_info* info);
 void pattern_vars(const kb_pattern& pt, std::vector<u32>* slots, std::vector<u32>* src);
 kb_status empty_rel(kb_ctx* ctx, const std::vector<u32>& slots, std::unique_ptr<kb_rel>* out);  // zero rows over `slots`
 std::unique_ptr<kb_rel> select_cols(const kb_rel& in, const std::vector<u32>& slots);          // reorder / select columns (zero-copy)

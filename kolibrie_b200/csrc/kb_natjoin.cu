@@ -9,6 +9,11 @@
 //     sub-joins                    for every pair of non-empty groups (mL, mR): hash_join_impl on the key (S \ U) ∪ (U ∩ mL ∩ mR),
 //                                  carrying the two row indices (an empty key is the groups' cartesian product)
 //     K3 natjoin_coalesce_kernel   the output rows from the sub-joins' row-index pairs: the right cell if bound, else the left one
+// and kb_hash_join_keyed, the hash joins of the Streamertail engine over rows that may leave variables unbound (engine.rs:710-811, 970-1071):
+//   check pass                   natjoin_check_kernel over the key columns: a KB_ID_NONE there is refused
+//   K4 keyed_index_kernel        every side's row index
+//   sub-join                     hash_join_impl of the (key columns, row index) views: the row-index pairs
+//   K3                           the output rows, every non-key shared slot coalesced by the call's merge policy
 #include <algorithm>
 
 #include "kb_internal.hpp"
@@ -45,6 +50,7 @@ struct NjCoalesceParams {
     const u32* r[KB_MAX_COLS];
     u32* out[KB_MAX_COLS];
     u32 n_out;
+    u32 right_first;          // a slot both sides hold: the preferred side's cell if bound, else the other side's
 };
 
 __global__ void __launch_bounds__(256) natjoin_check_kernel(const __grid_constant__ NjCheckParams P) {
@@ -104,11 +110,14 @@ __global__ void __launch_bounds__(256) natjoin_coalesce_kernel(const __grid_cons
     for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < P.n; i += gridDim.x * blockDim.x) {
         const u32 li = __ldg(P.li + i), ri = __ldg(P.ri + i);
         for (u32 c = 0; c < P.n_out; c++) {
-            u32 v = P.r[c] ? __ldg(P.r[c] + ri) : KB_ID_NONE;  // merged.insert: the right value overwrites (rsp_engine.rs:708-711)
-            if (v == KB_ID_NONE && P.l[c]) v = __ldg(P.l[c] + li);
-            P.out[c][P.base + i] = v;
+            const u32 lv = P.l[c] ? __ldg(P.l[c] + li) : KB_ID_NONE, rv = P.r[c] ? __ldg(P.r[c] + ri) : KB_ID_NONE;
+            P.out[c][P.base + i] = P.right_first ? (rv != KB_ID_NONE ? rv : lv) : (lv != KB_ID_NONE ? lv : rv);
         }
     }
+}
+
+__global__ void __launch_bounds__(256) keyed_index_kernel(u32* idx, u32 n) {
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) idx[i] = i;
 }
 
 int nj_grid(u64 n, int n_sms) { return (int)std::max<u64>(1, std::min<u64>((n + 255) / 256, (u64)n_sms * 8)); }
@@ -125,6 +134,15 @@ std::unique_ptr<kb_rel> group_view(const std::vector<u32>& shared, const std::ve
     v->slots.push_back(idx_slot);
     v->cols.push_back(Col{perm, static_cast<u32*>(perm->p) + start});
     return v;
+}
+
+// the two slots that name no variable of either side and carry the row indices through a sub-join
+void index_slots(const kb_rel& L, const kb_rel& R, u32 idx_slot[2]) {
+    u32 cand = 0xFFFFFFFEu;
+    for (int k = 0; k < 2; k++) {
+        while (L.col_of(cand) >= 0 || R.col_of(cand) >= 0) cand--;
+        idx_slot[k] = cand--;
+    }
 }
 
 kb_status natural_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_rel& R, std::unique_ptr<kb_rel>* out) {
@@ -212,12 +230,8 @@ kb_status natural_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_rel& R, std::
     timer_end(ctx);
     KB_CUDA(ctx, cudaGetLastError());
 
-    // row-index slots that name no variable of either side
-    u32 idx_slot[2], cand = 0xFFFFFFFEu;
-    for (int k = 0; k < 2; k++) {
-        while (L.col_of(cand) >= 0 || R.col_of(cand) >= 0) cand--;
-        idx_slot[k] = cand--;
-    }
+    u32 idx_slot[2];
+    index_slots(L, R, idx_slot);
     struct Sub { std::unique_ptr<kb_rel> rel; u64 base; };
     std::vector<Sub> subs;
     u64 total = 0;
@@ -245,6 +259,7 @@ kb_status natural_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_rel& R, std::
     rel->n = total;
     NjCoalesceParams Q{};
     Q.n_out = (u32)out_slots.size();
+    Q.right_first = 1;  // merged.insert: the right value overwrites (rsp_engine.rs:708-711)
     for (u32 c = 0; c < Q.n_out; c++) {
         Col col;
         KB_TRY(alloc_col(ctx, total, &col));
@@ -270,6 +285,90 @@ kb_status natural_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_rel& R, std::
     return KB_OK;
 }
 
+kb_status keyed_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_rel& R, const u32* key, u32 n_key, u32 merge, std::unique_ptr<kb_rel>* out) {
+    std::vector<u32> out_slots = L.slots;
+    for (u32 s : R.slots)
+        if (L.col_of(s) < 0) out_slots.push_back(s);
+    if (out_slots.size() > KB_MAX_COLS) return fail(ctx, KB_E_LIMIT, "join result has more than %d columns", KB_MAX_COLS);
+    if (L.n >= 0xFFFFFFF0ull || R.n >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "relation too large");
+    const kb_rel* side[2] = {&L, &R};
+    // a key cell without a value: the reference's hash joins panic on `tuple[var]`, its merge join compares keys of another shape
+    if (n_key && L.n && R.n) {
+        NjCheckParams C{};
+        C.n_cols = n_key;
+        for (int s = 0; s < 2; s++) {
+            C.side[s].n = (u32)side[s]->n;
+            for (u32 k = 0; k < n_key; k++) C.side[s].col[k] = side[s]->cols[side[s]->col_of(key[k])].ptr;
+        }
+        const u32 cw = ctrl_alloc(ctx, 2);
+        KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + cw, 0, 2 * sizeof(u32), ctx->st));
+        C.flags = ctx->ctrl + cw;
+        timer_begin(ctx, F_OTHER);
+        natjoin_check_kernel<<<dim3(nj_grid(std::max(L.n, R.n), ctx->n_sms), 2), 256, 0, ctx->st>>>(C);
+        timer_end(ctx);
+        KB_CUDA(ctx, cudaGetLastError());
+        KB_TRY(ctrl_read(ctx));
+        const u32 f = ctx->h_ctrl[cw] | ctx->h_ctrl[cw + 1];
+        if (f) {
+            u32 k = 0;
+            while (!(f >> k & 1u)) k++;
+            return fail(ctx, KB_E_UNSUPPORTED, "kb_hash_join_keyed: key slot %u is unbound in a %s row (the reference panics there)", key[k],
+                        ctx->h_ctrl[cw] >> k & 1u ? "left" : "right");
+        }
+    }
+    u32 idx_slot[2];
+    index_slots(L, R, idx_slot);
+    Buf idx[2];
+    std::unique_ptr<kb_rel> view[2];
+    for (int s = 0; s < 2; s++) {
+        KB_TRY(alloc_buf(ctx, std::max<u64>(side[s]->n, 1) * sizeof(u32), &idx[s]));
+        if (side[s]->n) {
+            timer_begin(ctx, F_OTHER);
+            keyed_index_kernel<<<nj_grid(side[s]->n, ctx->n_sms), 256, 0, ctx->st>>>(static_cast<u32*>(idx[s]->p), (u32)side[s]->n);
+            timer_end(ctx);
+            KB_CUDA(ctx, cudaGetLastError());
+        }
+        view[s] = std::make_unique<kb_rel>();
+        view[s]->n = side[s]->n;
+        for (u32 k = 0; k < n_key; k++) {
+            view[s]->slots.push_back(key[k]);
+            view[s]->cols.push_back(side[s]->cols[side[s]->col_of(key[k])]);
+        }
+        view[s]->slots.push_back(idx_slot[s]);
+        view[s]->cols.push_back(Col{idx[s], static_cast<u32*>(idx[s]->p)});
+    }
+    std::unique_ptr<kb_rel> j;
+    KB_TRY(hash_join_impl(ctx, *view[0], *view[1], nullptr, &j));
+    if (j->n >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "join result of more than 2^32 rows");
+
+    auto rel = std::make_unique<kb_rel>();
+    rel->slots = out_slots;
+    rel->n = j->n;
+    NjCoalesceParams Q{};
+    Q.n_out = (u32)out_slots.size();
+    Q.right_first = merge == KB_MERGE_RIGHT_FIRST;
+    for (u32 c = 0; c < Q.n_out; c++) {
+        Col col;
+        KB_TRY(alloc_col(ctx, j->n, &col));
+        rel->cols.push_back(col);
+        Q.out[c] = col.ptr;
+        const int lc = L.col_of(out_slots[c]), rc = R.col_of(out_slots[c]);
+        Q.l[c] = lc >= 0 ? L.cols[lc].ptr : nullptr;
+        Q.r[c] = rc >= 0 ? R.cols[rc].ptr : nullptr;
+    }
+    if (j->n) {
+        Q.li = j->cols[j->col_of(idx_slot[0])].ptr;
+        Q.ri = j->cols[j->col_of(idx_slot[1])].ptr;
+        Q.n = (u32)j->n;
+        timer_begin(ctx, F_OTHER);
+        natjoin_coalesce_kernel<<<nj_grid(j->n, ctx->n_sms), 256, 0, ctx->st>>>(Q);
+        timer_end(ctx);
+        KB_CUDA(ctx, cudaGetLastError());
+    }
+    *out = std::move(rel);
+    return KB_OK;
+}
+
 }  // namespace
 }  // namespace kb
 
@@ -283,6 +382,30 @@ kb_status kb_natural_join(kb_ctx* ctx, const kb_rel* left, const kb_rel* right, 
     if (left->pair || right->pair) return kb::fail(ctx, KB_E_INVALID, "internal pair relation");
     std::unique_ptr<kb_rel> r;
     KB_TRY(kb::natural_join_impl(ctx, *left, *right, &r));
+    ctx->stats.rows_out = r->n;
+    *out = r.release();
+    return KB_OK;
+}
+
+}  // extern "C"
+
+extern "C" {
+
+kb_status kb_hash_join_keyed(kb_ctx* ctx, const kb_rel* left, const kb_rel* right, const uint32_t* key_slots, uint32_t n_key, uint32_t merge,
+                             kb_rel** out) {
+    KB_ENTER(ctx);
+    if (!left || !right || !out || (n_key && !key_slots)) return kb::fail(ctx, KB_E_INVALID, "NULL argument");
+    if (left->pair || right->pair) return kb::fail(ctx, KB_E_INVALID, "internal pair relation");
+    if (merge != KB_MERGE_LEFT_FIRST && merge != KB_MERGE_RIGHT_FIRST) return kb::fail(ctx, KB_E_INVALID, "kb_hash_join_keyed: unknown merge policy %u", merge);
+    if (n_key > 4) return kb::fail(ctx, KB_E_LIMIT, "kb_hash_join_keyed: %u key slots (a hash join key holds at most 4)", n_key);
+    for (uint32_t k = 0; k < n_key; k++) {
+        if (left->col_of(key_slots[k]) < 0 || right->col_of(key_slots[k]) < 0)
+            return kb::fail(ctx, KB_E_INVALID, "kb_hash_join_keyed: key slot %u is not a column of both sides", key_slots[k]);
+        for (uint32_t m = 0; m < k; m++)
+            if (key_slots[m] == key_slots[k]) return kb::fail(ctx, KB_E_INVALID, "kb_hash_join_keyed: key slot %u repeated", key_slots[k]);
+    }
+    std::unique_ptr<kb_rel> r;
+    KB_TRY(kb::keyed_join_impl(ctx, *left, *right, key_slots, n_key, merge, &r));
     ctx->stats.rows_out = r->n;
     *out = r.release();
     return KB_OK;

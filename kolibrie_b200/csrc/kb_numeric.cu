@@ -139,14 +139,7 @@ kb_status ensure_num_order(kb_ctx* ctx, bool* ok) {
     return KB_OK;
 }
 
-}  // namespace kb
-
-using namespace kb;
-
-extern "C" {
-
-kb_status kb_dict_numeric_derive(kb_ctx* ctx, uint32_t tables, uint32_t first_id, kb_numeric_info* info) {
-    KB_ENTER(ctx);
+kb_status numeric_derive(kb_ctx* ctx, uint32_t tables, uint32_t first_id, kb_numeric_info* info) {
     if (info) *info = kb_numeric_info{};
     if (tables == 0 || (tables & ~(KB_NUMERIC_F64 | KB_NUMERIC_I32)))
         return fail(ctx, KB_E_INVALID, "tables must be a non-empty combination of KB_NUMERIC_F64 and KB_NUMERIC_I32 (got 0x%x)", tables);
@@ -206,6 +199,17 @@ kb_status kb_dict_numeric_derive(kb_ctx* ctx, uint32_t tables, uint32_t first_id
         info->n_slow = n_slow;
     }
     return KB_OK;
+}
+
+}  // namespace kb
+
+using namespace kb;
+
+extern "C" {
+
+kb_status kb_dict_numeric_derive(kb_ctx* ctx, uint32_t tables, uint32_t first_id, kb_numeric_info* info) {
+    KB_ENTER(ctx);
+    return numeric_derive(ctx, tables, first_id, info);
 }
 
 kb_status kb_dict_numeric_download(kb_ctx* ctx, uint32_t first, uint32_t n, double* num_or0, uint8_t* is_num, int32_t* val, uint8_t* is_i32) {

@@ -4,7 +4,7 @@ Same names, argument meaning and error behaviour as the reference (paths relativ
 
 * `Dictionary`            — shared/src/dictionary.rs:17-51 (ids dense from 0 in first-seen order)
 * `Term`/`TriplePattern`  — shared/src/terms.rs:13-23
-* `PhysicalOperator`      — kolibrie/src/streamertail_optimizer/operators/physical.rs:16-76 (the operators on the hot path)
+* `PhysicalOperator`      — kolibrie/src/streamertail_optimizer/operators/physical.rs:16-76 (the operators on the hot path, and Values)
 * `ExecutionEngine`       — kolibrie/src/streamertail_optimizer/execution/engine.rs:27,54 (`execute`, `execute_with_ids`)
 * `Condition`             — kolibrie/src/streamertail_optimizer/types.rs:110-186 (FILTER expressions)
 * `SparqlDatabase`        — kolibrie/src/sparql_database.rs:49-60,215-258,3364-3394 (triples + dictionary + build_all_indexes)
@@ -189,6 +189,7 @@ class SlotMap:
         self.names: List[str] = []
         self.bind_out: set = set()   # slots a Bind wrote: a KB_ID_NONE there is an unbound variable (left out of result rows)
         self.bind_only: set = set()  # Bind outputs no device operator may read (unbound rows, or strings the numeric table lacks)
+        self.ragged: set = set()     # slots a VALUES block binds: a KB_ID_NONE there is an UNDEF cell, which each join treats its own way
 
     def of(self, name: str) -> int:
         name = _strip(name)
@@ -389,6 +390,14 @@ class Bind:
     output_variable: str
 
 
+@dataclass
+class Values:
+    """PhysicalOperator::Values (operators/physical.rs; engine.rs:279-308): the rows of a VALUES block, each a list of terms in header
+    order, None for UNDEF (a row may be shorter than the header)"""
+    variables: List[str]
+    values: List[List[Optional[str]]]
+
+
 _BIND_FUNCTIONS = {"SUBJECT": c.BIND_SUBJECT, "PREDICATE": c.BIND_PREDICATE, "OBJECT": c.BIND_OBJECT, "isTRIPLE": c.BIND_IS_TRIPLE,
                    "TRIPLE": c.BIND_TRIPLE, "CONCAT": c.BIND_CONCAT}
 
@@ -512,22 +521,27 @@ class ExecutionEngine:
             rel = ExecutionEngine._run(op.input, db, slots)
             return ctx.project(rel, [slots.of(v) for v in op.variables])
         if isinstance(op, (HashJoin, OptimizedHashJoin, NestedLoopJoin)):
-            return ExecutionEngine._join(ctx, slots, ExecutionEngine._run(op.left, db, slots), ExecutionEngine._run(op.right, db, slots))
+            return ExecutionEngine._join(ctx, slots, ExecutionEngine._run(op.left, db, slots), ExecutionEngine._run(op.right, db, slots), type(op).__name__)
         if isinstance(op, ParallelJoin):
             # right side a scan -> bind join (engine.rs:935-937) == natural join of left with the pattern's matches: kb_bind_join looks the
             # pattern up in the index's persistent tables when it can, and scans + joins otherwise
             if isinstance(op.right, (TableScan, IndexScan)) and not any(isinstance(t, QuotedTriple) for t in op.right.pattern) and hasattr(ctx, "bind_join"):
                 left = ExecutionEngine._run(op.left, db, slots)
                 pat = slots.pattern(op.right.pattern)
-                ExecutionEngine._check_reads(slots, set(left.slots) & {t.value for t in (pat.s, pat.p, pat.o) if t.is_var}, "a join")
+                shared = set(left.slots) & {t.value for t in (pat.s, pat.p, pat.o) if t.is_var}
+                ExecutionEngine._check_reads(slots, shared, "a join")
+                if shared & slots.ragged:  # bind_pattern leaves a variable the row lacks free: the join of mappings
+                    return ctx.natural_join(left, ctx.scan([pat])[0])
                 return ctx.bind_join(left, pat)
-            return ExecutionEngine._join(ctx, slots, ExecutionEngine._run(op.left, db, slots), ExecutionEngine._run(op.right, db, slots))
+            return ExecutionEngine._join(ctx, slots, ExecutionEngine._run(op.left, db, slots), ExecutionEngine._run(op.right, db, slots), "ParallelJoin")
         if isinstance(op, StarJoin):
             return ctx.star_join(slots.of(op.join_var), [slots.pattern(p) for p in op.patterns])
         if isinstance(op, InMemoryBuffer):
             names = sorted({k for row in op.content for k in row})
             cols = [np.array([row[k] for row in op.content], dtype=np.uint32) for k in names]
             return ctx.rel_from_host([slots.of(k) for k in names], cols)
+        if isinstance(op, Values):
+            return ExecutionEngine._values(op, db, slots)
         if isinstance(op, Bind):
             rel = ExecutionEngine._run(op.input, db, slots)
             if hasattr(ctx, "bind"):  # on the device (kb_bind)
@@ -544,9 +558,49 @@ class ExecutionEngine:
             raise c.KolibrieError(c.KB_E_UNSUPPORTED, f"{what} reads the BIND output ?{slots.names[min(bad)]}: the reference's CPU path")
 
     @staticmethod
-    def _join(ctx, slots: SlotMap, left: c.Relation, right: c.Relation) -> c.Relation:
-        ExecutionEngine._check_reads(slots, set(left.slots) & set(right.slots), "a join")
-        return ctx.hash_join(left, right)
+    def _join(ctx, slots: SlotMap, left: c.Relation, right: c.Relation, kind: str = "HashJoin") -> c.Relation:
+        """the join operator `kind` over device relations. Without an UNDEF cell in a shared column every operator is the natural join
+        (kb_hash_join). Over VALUES rows they differ (engine.rs:710-1071): NestedLoopJoin is the join of mappings (kb_natural_join); the
+        hash joins and the merge join pair rows on the shared variables bound in row 0 of both sides and coalesce the other shared
+        variables left-first, except OptimizedHashJoin whose probe side (the larger, right on ties) wins and the cartesian product,
+        whose right side wins (kb_hash_join_keyed; a key cell a row lacks raises KB_E_UNSUPPORTED where the reference panics).
+        Row 0 is the device relation's row 0. That is the reference's row 0 where the relation lies in the reference's order (a VALUES
+        block, a scan); above a join it lies in device order, while the reference's row 0 there is hash-iteration order (after its merge
+        join's unstable sort, not even fixed). So above a join the key can differ from the reference's: the device may refuse where
+        the reference answers, or answer where it panics, depending on the row order. Where both answer, the answers agree."""
+        shared = set(left.slots) & set(right.slots)
+        ExecutionEngine._check_reads(slots, shared, "a join")
+        if not shared & slots.ragged:
+            return ctx.hash_join(left, right)
+        if kind == "NestedLoopJoin":
+            return ctx.natural_join(left, right)
+        (nl, lslots), (nr, rslots) = left.info(), right.info()
+        key = []
+        if nl and nr:  # row 0 of each side: a one-row view, 4 bytes a shared column
+            l0, r0 = ctx.order_by(left, [], 1)[0], ctx.order_by(right, [], 1)[0]
+            key = [s_ for s_ in sorted(shared) if l0.column(lslots.index(s_))[0] != c.KB_ID_NONE and r0.column(rslots.index(s_))[0] != c.KB_ID_NONE]
+        right_first = not key or (kind == "OptimizedHashJoin" and nl <= nr)
+        return ctx.hash_join_keyed(left, right, key, c.MERGE_RIGHT_FIRST if right_first else c.MERGE_LEFT_FIRST)
+
+    @staticmethod
+    def _values(op: "Values", db: SparqlDatabase, slots: SlotMap) -> c.Relation:
+        """kb_values, then the host Dictionary takes the new strings in the order the device created them"""
+        ctx = db.ctx
+        n_dev, _ = ctx.dict_strings_info()
+        reloaded = n_dev != len(db.dictionary.id_to_string)
+        if reloaded:
+            ctx.dict_strings_load(db.dictionary.id_to_string)
+        sl = [slots.of(v) for v in op.variables]
+        rel, info = ctx.values(sl, op.values)
+        d = db.dictionary
+        for t in ctx.dict_strings_download(info["dict_first"], info["dict_new"]):
+            d.string_to_id[t] = len(d.id_to_string)
+            d.id_to_string.append(t)
+        if reloaded:  # kb_values extended the numeric table of the strings the device held before the reload
+            _derive_numeric(ctx, 0)
+        slots.ragged.update(sl)
+        slots.bind_out.update(sl)  # an UNDEF cell is a variable the row does not bind
+        return rel
 
     @staticmethod
     def _bind_host(function_name: str, arguments: Sequence[str], cols: Dict[str, np.ndarray], n: int, old: Optional[np.ndarray],

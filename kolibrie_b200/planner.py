@@ -3,7 +3,7 @@ the hot path and extended by the device operators, so that the optimizer *choose
 CPU plans after the fact (SURVEY.md §8 (f)3).
 
 Mirrored (paths relative to kolibrie/src/streamertail_optimizer of the Kolibrie checkout):
-* `LogicalOperator::{Scan, Selection, Projection, Join}`        operators/logical.rs
+* `LogicalOperator::{Scan, Selection, Projection, Join, Values}` operators/logical.rs
 * `DatabaseStats` (predicate / subject / object cardinalities)  stats.rs, consumed by cost/estimator.rs:193-255
 * `CostConstants`, `CostEstimator::estimate_cost`               cost/estimator.rs:17-29, 43-191 (the hot-path variants)
 * `Streamertail::find_best_plan`                                optimizer.rs:60-62, 84-152 (star detection), 192-300 (candidates),
@@ -51,10 +51,19 @@ class Join:
     right: object
 
 
-def build_logical_plan(patterns: Sequence[E.TriplePattern], condition: Optional[E.Condition] = None, variables: Optional[List[str]] = None):
-    """build_logical_plan (utils.rs:101-191): left-deep joins in textual order, then the selection, then the projection"""
-    plan = Scan(patterns[0])
-    for p in patterns[1:]:
+@dataclass
+class LValues:
+    """LogicalOperator::Values: a VALUES block, rows of terms in header order, None for UNDEF"""
+    variables: List[str]
+    values: List[List[Optional[str]]]
+
+
+def build_logical_plan(patterns: Sequence[E.TriplePattern], condition: Optional[E.Condition] = None, variables: Optional[List[str]] = None,
+                       values: Optional[LValues] = None):
+    """build_logical_plan (utils.rs:101-191): left-deep joins in textual order, then the selection, then the projection. A VALUES
+    block is the base of the chain and every pattern is joined onto it (utils.rs:110-171)."""
+    plan = values if values is not None else Scan(patterns[0])
+    for p in patterns[0 if values is not None else 1:]:
         plan = Join(plan, Scan(p))
     if condition is not None:
         plan = Selection(plan, condition)
@@ -212,6 +221,8 @@ class CostEstimator:
             return max(self.estimate_output_cardinality(plan.left), self.estimate_output_cardinality(plan.right))
         if isinstance(plan, E.InMemoryBuffer):
             return len(plan.content)
+        if isinstance(plan, E.Values):  # estimator.rs:399-402
+            return len(plan.values)
         return 1
 
     # ---- costs (estimator.rs:43-191) + the device operators
@@ -262,6 +273,8 @@ class CostEstimator:
                     + (self.estimate_output_cardinality(plan.left) + self.estimate_output_cardinality(plan.right)) // G.ROWS_PER_UNIT_JOIN)
         if isinstance(plan, E.InMemoryBuffer):
             return 0
+        if isinstance(plan, E.Values):  # estimator.rs:169-173
+            return len(plan.values) * C.TUPLE_COST
         raise TypeError(plan)
 
 
@@ -359,7 +372,56 @@ class Streamertail:
             return int(self._logical_card(plan.predicate) * self.cost.estimate_selectivity(plan.condition))
         if isinstance(plan, LProjection):
             return self._logical_card(plan.predicate)
+        if isinstance(plan, LValues):  # optimizer.rs:762-764
+            return len(plan.values)
         return 1
+
+    # ---- the logical estimates of optimizer.rs:643-757, used to order and gate the joins of a plan with a VALUES block: over UNDEF
+    # cells the join operators answer differently, so the side order and the operator must be the reference's
+    def _join_selectivity(self, l, r) -> float:  # estimate_join_selectivity (optimizer.rs:698-709), database_stats.rs:129-152
+        def pred(plan):  # extract_predicate_from_plan (optimizer.rs:712-730)
+            if isinstance(plan, Scan):
+                return plan.pattern[1].id if _is_const(plan.pattern[1]) else None
+            if isinstance(plan, Join):
+                return pred(plan.left)
+            if isinstance(plan, (Selection, LProjection)):
+                return pred(plan.predicate)
+            return None
+        p = pred(l)
+        if p is None:
+            p = pred(r)
+        if p is None or self.stats.total_triples <= 0:
+            return 0.1
+        return self.stats.get_predicate_cardinality(p) / self.stats.total_triples
+
+    def _ref_logical_card(self, plan) -> int:  # estimate_output_cardinality_from_logical (optimizer.rs:733-768)
+        if isinstance(plan, Scan):
+            return self.cost.estimate_cardinality(plan.pattern)
+        if isinstance(plan, Selection):
+            return max(int(self._ref_logical_card(plan.predicate) * self.cost.estimate_selectivity(plan.condition)), 1)
+        if isinstance(plan, LProjection):
+            return self._ref_logical_card(plan.predicate)
+        if isinstance(plan, Join):
+            lc, rc = self._ref_logical_card(plan.left), self._ref_logical_card(plan.right)
+            return max(int(min(lc, rc) * self._join_selectivity(plan.left, plan.right)), 1)
+        if isinstance(plan, LValues):
+            return len(plan.values)
+        raise TypeError(plan)
+
+    def _ref_logical_cost(self, plan) -> int:  # estimate_logical_cost (optimizer.rs:643-695)
+        if isinstance(plan, Scan):
+            return self.cost.estimate_cardinality(plan.pattern)
+        if isinstance(plan, Join):
+            lcard, rcard = self._ref_logical_card(plan.left), self._ref_logical_card(plan.right)
+            return (self._ref_logical_cost(plan.left) + self._ref_logical_cost(plan.right)
+                    + int(lcard * rcard * self._join_selectivity(plan.left, plan.right)))
+        if isinstance(plan, Selection):
+            return int(self._ref_logical_cost(plan.predicate) * self.cost.estimate_selectivity(plan.condition))
+        if isinstance(plan, LProjection):
+            return self._ref_logical_cost(plan.predicate)
+        if isinstance(plan, LValues):
+            return len(plan.values)
+        raise TypeError(plan)
 
     def find_best_plan(self, plan):
         # star shapes first (optimizer.rs:200-232)
@@ -378,25 +440,38 @@ class Streamertail:
         cands = []
         if isinstance(plan, Scan):
             cands.append(self.choose_best_scan(plan.pattern))
+        elif isinstance(plan, LValues):  # a leaf (optimizer.rs:325-330)
+            cands.append(E.Values(plan.variables, plan.values))
         elif isinstance(plan, Selection):
             cands.append(E.Filter(self.find_best_plan(plan.predicate), plan.condition))
         elif isinstance(plan, LProjection):
             cands.append(E.Projection(self.find_best_plan(plan.predicate), plan.variables))
         elif isinstance(plan, Join):
             l, r = plan.left, plan.right
-            if self._logical_card(l) > self._logical_card(r):  # cheaper side first (optimizer.rs:254-262)
+            values = _has_values(l) or _has_values(r)
+            cost = self._ref_logical_cost if values else self._logical_card
+            card = self._ref_logical_card if values else self._logical_card
+            if cost(l) > cost(r):  # cheaper side first (optimizer.rs:254-262)
                 l, r = r, l
             bl, br = self.find_best_plan(l), self.find_best_plan(r)
             cands += [E.OptimizedHashJoin(bl, br), E.HashJoin(bl, br), E.ParallelJoin(bl, br)]
-            if self._logical_card(l) < 1000 and self._logical_card(r) < 1000:
+            if card(l) < 1000 and card(r) < 1000:  # optimizer.rs:276-285
                 cands.append(E.NestedLoopJoin(bl, br))
-            if self.gpu:
+            # over a VALUES block the join operators differ in what they do with UNDEF cells (ExecutionEngine._join): only the
+            # reference's own candidates, so that the mirror picks the operator the reference picks
+            if self.gpu and not values:
                 cands.append(GpuHashJoin(bl, br))
                 if isinstance(r, Scan) and not any(isinstance(t, E.QuotedTriple) for t in r.pattern):
                     cands.append(GpuBindJoin(bl, r.pattern))
         else:
             raise TypeError(plan)
         return min(cands, key=self.cost.estimate_cost)
+
+
+def _has_values(plan) -> bool:
+    if isinstance(plan, LValues):
+        return True
+    return any(_has_values(getattr(plan, a)) for a in ("left", "right", "predicate") if hasattr(plan, a))
 
 
 def uses_device(plan) -> bool:

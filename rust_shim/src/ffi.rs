@@ -48,6 +48,10 @@ pub const KB_BIND_MAX_ARGS: u32 = 16;
 pub const KB_NUMERIC_F64: u32 = 1; pub const KB_NUMERIC_I32: u32 = 2; pub const KB_NUMERIC_APPEND: u32 = 0xFFFF_FFFF;
 #[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbNumericInfo { pub n_ids: u32, pub n_derived: u32, pub n_numeric: u32, pub n_i32: u32, pub n_slow: u32 }
 pub type kb_numeric_info = KbNumericInfo;  // (the header's name, as the declaration below spells it)
+// kb_values (engine.rs:279-308) and kb_hash_join_keyed's merge policy
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbValuesInfo { pub dict_first: u32, pub dict_new: u32, pub rows_dropped: u64 }
+pub type kb_values_info = KbValuesInfo;  // (the header's name, as the declaration below spells it)
+pub const KB_MERGE_LEFT_FIRST: u32 = 0; pub const KB_MERGE_RIGHT_FIRST: u32 = 1;
 // kb_bgp_execute: up to 16 patterns; kb_bgp_last_plan describes the last call (kb_bgp_route)
 pub const KB_BGP_MAX_PATTERNS: usize = 16;
 pub const KB_BGP_NONE: u32 = 0; pub const KB_BGP_STAR: u32 = 1; pub const KB_BGP_COMPONENTS: u32 = 2;
@@ -122,6 +126,11 @@ extern "C" {
     pub fn kb_hash_join(ctx: *mut KbCtx, l: *const KbRel, r: *const KbRel, out: *mut *mut KbRel) -> kb_status;
     // natural_join of the RSP emit step: rows may leave shared variables unbound (KB_ID_NONE)
     pub fn kb_natural_join(ctx: *mut KbCtx, l: *const KbRel, r: *const KbRel, out: *mut *mut KbRel) -> kb_status;
+    // the Streamertail hash joins over VALUES rows: pairs on key_slots (row 0's shared variables), the other shared slots by `merge`
+    pub fn kb_hash_join_keyed(ctx: *mut KbCtx, l: *const KbRel, r: *const KbRel, key_slots: *const u32, n_key: u32, merge: u32,
+                              out: *mut *mut KbRel) -> kb_status;
+    pub fn kb_values(ctx: *mut KbCtx, slots: *const u32, n_vars: u32, n_rows: u64, undef: *const u8, offsets: *const u64, bytes: *const u8,
+                     out: *mut *mut KbRel, info: *mut kb_values_info) -> kb_status;
     pub fn kb_bind_join(ctx: *mut KbCtx, l: *const KbRel, pattern: *const KbPattern, out: *mut *mut KbRel) -> kb_status;
     pub fn kb_scan_quoted(ctx: *mut KbCtx, qp: *const kb_quoted_pattern, out: *mut *mut KbRel) -> kb_status;
     pub fn kb_bind(ctx: *mut KbCtx, r: *const KbRel, spec: *const kb_bind_spec, out: *mut *mut KbRel, info: *mut kb_bind_info) -> kb_status;

@@ -1,8 +1,8 @@
 //! kolibrie-gpu-b200 — the three seams through which Kolibrie hands its hot path to libkolibrie_b200.so:
 //!
 //! * [`try_execute`]            for `ExecutionEngine::execute_with_ids` (kolibrie/src/streamertail_optimizer/execution/engine.rs:54);
-//!                              [`try_execute_mut`] also runs `Bind` (engine.rs:144-277) and grows the database's dictionary and
-//!                              quoted-triple store as the reference does
+//!                              [`try_execute_mut`] also runs `Bind` (engine.rs:144-277) and `Values` (engine.rs:279-308) and
+//!                              grows the database's dictionary and quoted-triple store as the reference does
 //! * [`GpuSemiNaiveStrategy`]   for `Reasoner::infer_with_strategy`    (datalog/src/reasoning/materialisation/infer_generic.rs:27-53)
 //! * [`GpuR2R`]                 for the RSP engine's `R2ROperator`      (kolibrie/src/rsp/r2r.rs:17-30), optionally with the
 //!                              Relation-to-Stream operator on the device (`GpuR2R::with_stream_operator`, kolibrie/src/rsp/r2s.rs:37-58)
@@ -282,8 +282,85 @@ fn run(op: &PhysicalOperator, dev: &DeviceStore, db: &SparqlDatabase, slots: &mu
             let sl: Vec<u32> = names.iter().map(|k| slots.of(k)).collect();
             ok(unsafe { kb_rel_from_host(ctx, sl.as_ptr(), sl.len() as u32, ptrs.as_ptr(), content.len() as u64, &mut out) }, out)
         }
-        _ => None,  // Bind (see run_mut), Values, MLPredict, Subquery: the reference's CPU path
+        _ => None,  // Bind and Values (see run_mut), MLPredict, Subquery: the reference's CPU path
     }
+}
+
+/// The device dictionary's ids [first, first + n) join the host dictionary, in the order the device created them (no lookup of its own).
+fn take_new_strings(dev: &mut DeviceStore, db: &mut SparqlDatabase, first: u32, n: u32) -> Option<()> {
+    if n == 0 { return Some(()); }
+    let ctx = dev.ctx;
+    let mut offs = vec![0u64; n as usize + 1];
+    if unsafe { kb_dict_strings_download(ctx, first, n, offs.as_mut_ptr(), ptr::null_mut()) } != KB_OK { return None; }
+    let mut bytes = vec![0u8; offs[n as usize] as usize];
+    if unsafe { kb_dict_strings_download(ctx, first, n, offs.as_mut_ptr(), bytes.as_mut_ptr()) } != KB_OK { return None; }
+    let mut dict = db.dictionary.write().unwrap();
+    for k in 0..n as usize {
+        dict.encode(std::str::from_utf8(&bytes[offs[k] as usize..offs[k + 1] as usize]).ok()?);
+    }
+    dev.synced_dict = dict.id_to_string.len();
+    Some(())
+}
+
+fn has_values(op: &PhysicalOperator) -> bool {
+    match op {
+        PhysicalOperator::Values { .. } => true,
+        PhysicalOperator::Filter { input, .. } | PhysicalOperator::Projection { input, .. } => has_values(input),
+        PhysicalOperator::HashJoin { left, right } | PhysicalOperator::OptimizedHashJoin { left, right }
+        | PhysicalOperator::NestedLoopJoin { left, right } | PhysicalOperator::ParallelJoin { left, right } => has_values(left) || has_values(right),
+        _ => false,
+    }
+}
+
+fn rel_slots(r: &Rel) -> Option<(u64, Vec<u32>)> {
+    let (mut n, mut nc, mut rs) = (0u64, 0u32, [0u32; KB_MAX_COLS]);
+    if unsafe { kb_rel_info(r.0, &mut n, &mut nc, rs.as_mut_ptr()) } != KB_OK { return None; }
+    Some((n, rs[..nc as usize].to_vec()))
+}
+
+#[derive(Clone, Copy, PartialEq)]
+enum JoinKind { Hash, OptimizedHash, NestedLoop, Parallel }
+
+/// One join operator of the reference over device relations whose `ragged` slots may hold KB_ID_NONE (a VALUES block's UNDEF cells),
+/// as engine.py's ExecutionEngine._join: without KB_ID_NONE in a shared slot every operator is kb_hash_join; NestedLoopJoin is the join
+/// of mappings (kb_natural_join, engine.rs:814-837); the hash joins and the merge join pair rows on the shared variables bound in row 0
+/// of both sides (kb_hash_join_keyed, engine.rs:710-811, 970-1039), the other shared variables left-first, except the probe side of
+/// OptimizedHashJoin (the right side when the left is the smaller or equal one) and the cartesian product (engine.rs:1054-1071), which
+/// are right-first. A key cell a row leaves unbound is refused (None: the CPU path, where the reference panics). Row 0 is the device
+/// relation's: below a join that is the join's device order, not the reference's hash order.
+fn join_ragged(ctx: *mut KbCtx, kind: JoinKind, l: &Rel, r: &Rel, ragged: &[u32]) -> Option<Rel> {
+    let mut out: *mut KbRel = ptr::null_mut();
+    let (nl, ls) = rel_slots(l)?;
+    let (nr, rs) = rel_slots(r)?;
+    let shared: Vec<u32> = ls.iter().copied().filter(|s| rs.contains(s)).collect();
+    let rc = if !shared.iter().any(|s| ragged.contains(s)) {
+        unsafe { kb_hash_join(ctx, l.0, r.0, &mut out) }
+    } else if kind == JoinKind::NestedLoop {
+        unsafe { kb_natural_join(ctx, l.0, r.0, &mut out) }
+    } else {
+        let mut key = Vec::new();
+        if nl > 0 && nr > 0 {
+            let row0 = |rel: &Rel, slots: &[u32]| -> Option<Vec<u32>> {
+                let mut v: *mut KbRel = ptr::null_mut();
+                if unsafe { kb_order_by(ctx, rel.0, ptr::null(), 0, 1, &mut v, ptr::null_mut()) } != KB_OK { return None; }
+                let v = Rel(v, ctx);
+                let mut row = vec![KB_ID_NONE; slots.len()];
+                for c in 0..slots.len() {
+                    if unsafe { kb_rel_download(ctx, v.0, c as u32, &mut row[c]) } != KB_OK { return None; }
+                }
+                Some(row)
+            };
+            let (l0, r0) = (row0(l, &ls)?, row0(r, &rs)?);
+            for &s in &shared {
+                let (i, j) = (ls.iter().position(|&x| x == s)?, rs.iter().position(|&x| x == s)?);
+                if l0[i] != KB_ID_NONE && r0[j] != KB_ID_NONE { key.push(s); }
+            }
+        }
+        let right_first = key.is_empty() || (kind == JoinKind::OptimizedHash && nl <= nr);
+        let merge = if right_first { KB_MERGE_RIGHT_FIRST } else { KB_MERGE_LEFT_FIRST };
+        unsafe { kb_hash_join_keyed(ctx, l.0, r.0, key.as_ptr(), key.len() as u32, merge, &mut out) }
+    };
+    if rc == KB_OK { Some(Rel(out, ctx)) } else { None }
 }
 
 /// `run` plus `Bind` with the built-in functions (engine.rs:144-277) through kb_bind. The plan builder puts every Bind above the join and
@@ -298,6 +375,72 @@ fn run_mut(op: &PhysicalOperator, dev: &mut DeviceStore, db: &mut SparqlDatabase
             let sl: Vec<u32> = variables.iter().map(|v| slots.of(v)).collect();
             if unsafe { kb_project(ctx, r.0, sl.as_ptr(), sl.len() as u32, &mut out) } != KB_OK { return None; }
             Some(Rel(out, ctx))
+        }
+        // VALUES (engine.rs:279-308) through kb_values: every defined cell encoded verbatim, in row-major order, into the device
+        // dictionary, which the host dictionary then follows; an UNDEF cell is KB_ID_NONE, so its slots join `bind_out`
+        PhysicalOperator::Values { variables, values } => {
+            let sl: Vec<u32> = variables.iter().map(|v| slots.of(v)).collect();
+            let nv = sl.len();
+            let mut undef = vec![1u8; values.len() * nv];
+            let mut offs = vec![0u64; values.len() * nv + 1];
+            let mut bytes: Vec<u8> = Vec::new();
+            for (r, row) in values.iter().enumerate() {
+                for v in 0..nv {
+                    let i = r * nv + v;
+                    if let Some(Some(t)) = row.get(v) {  // value_row.get(i): a missing trailing cell is UNDEF
+                        undef[i] = 0;
+                        bytes.extend_from_slice(t.as_bytes());
+                    }
+                    offs[i + 1] = bytes.len() as u64;
+                }
+            }
+            let mut info = KbValuesInfo::default();
+            if unsafe { kb_values(ctx, sl.as_ptr(), nv as u32, values.len() as u64, undef.as_ptr(), offs.as_ptr(), bytes.as_ptr(), &mut out, &mut info) } != KB_OK {
+                return None;
+            }
+            let res = Rel(out, ctx);
+            take_new_strings(dev, db, info.dict_first, info.dict_new)?;
+            for s in sl { if !bind_out.contains(&s) { bind_out.push(s); } }
+            Some(res)
+        }
+        // the plan builder puts a VALUES block at the base of the join chain (utils.rs:110-171): the operators above it come here
+        PhysicalOperator::Filter { input, condition } if has_values(input) => {
+            let r = run_mut(input, dev, db, slots, bind_out)?;
+            let prog = compile_condition(condition, slots, db)?;
+            if unsafe { kb_filter(ctx, r.0, prog.as_ptr(), prog.len() as u32, &mut out) } != KB_OK { return None; }
+            Some(Rel(out, ctx))
+        }
+        PhysicalOperator::HashJoin { left, right } | PhysicalOperator::OptimizedHashJoin { left, right }
+        | PhysicalOperator::NestedLoopJoin { left, right } if has_values(left) || has_values(right) => {
+            let kind = match op {
+                PhysicalOperator::HashJoin { .. } => JoinKind::Hash,
+                PhysicalOperator::OptimizedHashJoin { .. } => JoinKind::OptimizedHash,
+                _ => JoinKind::NestedLoop,
+            };
+            let l = run_mut(left, dev, db, slots, bind_out)?;
+            let r = run_mut(right, dev, db, slots, bind_out)?;
+            join_ragged(ctx, kind, &l, &r, bind_out)
+        }
+        PhysicalOperator::ParallelJoin { left, right } if has_values(left) || has_values(right) => {
+            let l = run_mut(left, dev, db, slots, bind_out)?;
+            match right.as_ref() {
+                // a bind join (engine.rs:840-923): bind_pattern leaves a variable the row lacks free, which is the join of mappings
+                PhysicalOperator::TableScan { pattern } | PhysicalOperator::IndexScan { pattern } if !is_quoted(pattern) => {
+                    let p = slots.pattern(pattern)?;
+                    let (_, ls) = rel_slots(&l)?;
+                    let ragged = [p.s, p.p, p.o].iter().any(|t| t.is_var == 1 && ls.contains(&t.value) && bind_out.contains(&t.value));
+                    if !ragged {
+                        if unsafe { kb_bind_join(ctx, l.0, &p, &mut out) } != KB_OK { return None; }
+                        return Some(Rel(out, ctx));
+                    }
+                    if unsafe { kb_scan(ctx, &p, 1, ptr::null(), ptr::null(), &mut out) } != KB_OK { return None; }
+                    let m = Rel(out, ctx);
+                    let mut j: *mut KbRel = ptr::null_mut();
+                    if unsafe { kb_natural_join(ctx, l.0, m.0, &mut j) } != KB_OK { return None; }
+                    Some(Rel(j, ctx))
+                }
+                _ => { let r = run_mut(right, dev, db, slots, bind_out)?; join_ragged(ctx, JoinKind::Parallel, &l, &r, bind_out) }
+            }
         }
         PhysicalOperator::Bind { input, function_name, arguments, output_variable } => {
             if db.udfs.contains_key(function_name.as_str()) { return None; }  // a UDF shadows the built-ins (engine.rs:183)
@@ -353,17 +496,7 @@ fn run_mut(op: &PhysicalOperator, dev: &mut DeviceStore, db: &mut SparqlDatabase
             if unsafe { kb_bind(ctx, r.0, &spec, &mut out, &mut info) } != KB_OK { return None; }
             let res = Rel(out, ctx);
             // the host takes the device's new entries in the order the device created them (no lookup of its own)
-            if info.dict_new > 0 {
-                let mut offs = vec![0u64; info.dict_new as usize + 1];
-                if unsafe { kb_dict_strings_download(ctx, info.dict_first, info.dict_new, offs.as_mut_ptr(), ptr::null_mut()) } != KB_OK { return None; }
-                let mut bytes = vec![0u8; offs[info.dict_new as usize] as usize];
-                if unsafe { kb_dict_strings_download(ctx, info.dict_first, info.dict_new, offs.as_mut_ptr(), bytes.as_mut_ptr()) } != KB_OK { return None; }
-                let mut dict = db.dictionary.write().unwrap();
-                for k in 0..info.dict_new as usize {
-                    dict.encode(std::str::from_utf8(&bytes[offs[k] as usize..offs[k + 1] as usize]).ok()?);
-                }
-                dev.synced_dict = dict.id_to_string.len();
-            }
+            take_new_strings(dev, db, info.dict_first, info.dict_new)?;
             if info.quoted_new > 0 {
                 let m = info.quoted_new as usize;
                 let (mut s, mut p, mut o) = (vec![0u32; m], vec![0u32; m], vec![0u32; m]);
