@@ -185,6 +185,11 @@ KB_API kb_status kb_synchronize(kb_ctx* ctx);
 
 /* ------------------------------------------------------------------ triple store (device cache of `SparqlDatabase.triples`,
  * kolibrie/src/sparql_database.rs:50; segments = RSP window slides, kolibrie/src/rsp_engine.rs:94-104) */
+/* A triple holding KB_ID_NONE (0xFFFFFFFF, reserved: the direct tables use it as their empty slot) in any position is refused by
+ * kb_store_load, kb_store_load_device, kb_store_append, kb_store_append_device, kb_store_append_file and the one-shot
+ * kb_star_join_host[_into] -> KB_E_INVALID, the message naming the position. A load (and a one-shot call) empties the store first,
+ * so a refused one leaves it empty (at a new version: the closed token of
+ * kb_datalog_fixpoint / kb_datalog_maintain is void); a refused append leaves the store as it was. */
 KB_API kb_status kb_store_load(kb_ctx* ctx, const uint32_t* s, const uint32_t* p, const uint32_t* o, uint64_t n);
 /* same, columns already in device memory of ctx's device (copied device-to-device) */
 KB_API kb_status kb_store_load_device(kb_ctx* ctx, const uint32_t* d_s, const uint32_t* d_p, const uint32_t* d_o, uint64_t n);

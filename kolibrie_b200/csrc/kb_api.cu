@@ -1405,6 +1405,19 @@ static kb_status star_join_host_common(kb_ctx* ctx, const uint32_t* s, const uin
     std::unique_ptr<kb_rel> r;
     kb_status rc = kb::star_join_impl(ctx, join_slot, pats, n_pats, filter, n_ops, &r);
     if (rc != KB_OK) return finish(rc);
+    if (n) {  // a column holding KB_ID_NONE (reserved) is refused like kb_store_load refuses it: the store is left empty, nothing returned
+        // the scan stage took the upload's column ranges into the segments; a join that ended before it reads them from the
+        // control words the copy stream filled
+        u32 mx[3];
+        if (!ctx->segs.empty() && ctx->segs[0].has_stats) {
+            for (int c = 0; c < 3; c++) mx[c] = ctx->segs[0].cmax[c];
+        } else {
+            KB_HOST_CUDA(cudaStreamSynchronize(ctx->st_copy));
+            KB_HOST_CUDA(cudaMemcpy(mx, ctx->ctrl + soff + 4, sizeof mx, cudaMemcpyDeviceToHost));
+        }
+        rc = kb::refuse_reserved_id(ctx, mx);
+        if (rc != KB_OK) return finish(rc);
+    }
     *n_cols = (u32)r->slots.size();
     *n_rows = r->n;
     for (size_t c = 0; c < r->slots.size(); c++) slots[c] = r->slots[c];

@@ -392,6 +392,9 @@ char* group_peer_table(char* scratch, const GroupTable& t, u32 ring_slot);
 // what the peer merge of ring slot `ring_slot` reads: every rank's flags and partial table
 PeerTables group_peer_tables(const GroupTable& t, const std::vector<char*>& scratch, u32 rank, u32 ring_slot);
 kb_status segment_stats(kb_ctx* ctx, Segment* sg);
+// KB_ID_NONE is reserved: the direct tables use it as their empty slot, so a stored triple holding it would drop out of a join.
+// cmax: a new segment's largest id per column (its profile pass, or a segment file's header) -> KB_E_INVALID naming the position
+kb_status refuse_reserved_id(kb_ctx* ctx, const u32 cmax[3]);
 // Changes to the store (kb_store.cu). Each one bumps store_version, which voids what is keyed to it (prepared plans, the seeded
 // fixpoint's state, the closed token), and clears the hint sets.
 // the store becomes `segs`; the index is dropped

@@ -122,6 +122,7 @@ extern "C" kb_status kb_store_append_file(kb_ctx* ctx, const char* path, uint64_
     SegHeader h{};
     if (fread(&h, 1, sizeof h, fh.f) != sizeof h || h.magic != SEG_MAGIC || h.version != 1) return fail(ctx, KB_E_INVALID, "%s is not a segment file", path);
     const uint64_t n = h.n_triples;
+    if (n) KB_TRY(refuse_reserved_id(ctx, h.cmax));
     if (ctx->n_triples + n >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "store would exceed 2^32-16 triples");
     Segment sg;
     sg.tag = tag;

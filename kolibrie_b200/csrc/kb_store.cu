@@ -38,6 +38,13 @@ kb_status segment_stats(kb_ctx* ctx, Segment* sg) {
     return KB_OK;
 }
 
+kb_status refuse_reserved_id(kb_ctx* ctx, const u32 cmax[3]) {
+    static const char* const pos[3] = {"subject", "predicate", "object"};
+    for (int c = 0; c < 3; c++)
+        if (cmax[c] == KB_ID_NONE) return fail(ctx, KB_E_INVALID, "a triple's %s is 0xFFFFFFFF, which is reserved (KB_ID_NONE)", pos[c]);
+    return KB_OK;
+}
+
 // ---- store index, one chunk per (predicate, store segment)
 // the rank column of a slice's subject table: xkey[compact(subject) - xtab_min] = rank of the object's value in the value order (slots
 // without a key are never read: they stay unset)
@@ -449,6 +456,7 @@ static kb_status store_add_segment(kb_ctx* ctx, const u32* s, const u32* p, cons
         // the statistics pass ends with a read-back on the same stream: when it returns the copies are done too (the caller's
         // buffers are borrowed for this call only)
         KB_TRY(kb::segment_stats(ctx, &sg));
+        KB_TRY(kb::refuse_reserved_id(ctx, sg.cmax));
         if (trace)
             fprintf(stderr, "[kb trace] segment of %llu triples: copies %.3f ms, statistics %.3f ms\n", (unsigned long long)n,
                     std::chrono::duration<double, std::milli>(t1 - t0).count(),
@@ -462,7 +470,8 @@ kb_status kb_store_clear(kb_ctx* ctx) {
     kb::store_replace(ctx, {});
     return KB_OK;
 }
-// a load empties the store first: a rejected load leaves it empty, at a new version
+// a load empties the store first: a rejected load (a NULL column, a triple holding KB_ID_NONE) leaves it empty, at a new version;
+// a rejected append leaves the store as it was
 kb_status kb_store_load(kb_ctx* ctx, const uint32_t* s, const uint32_t* p, const uint32_t* o, uint64_t n) {
     KB_ENTER(ctx);
     kb::store_replace(ctx, {});
