@@ -287,6 +287,45 @@ KB_API kb_status kb_quoted_download(kb_ctx* ctx, uint32_t first_id, uint32_t n, 
  * pass the ids the device dictionary holds (KB_E_INVALID). */
 KB_API kb_status kb_dict_strings_download(kb_ctx* ctx, uint32_t first, uint32_t n, uint64_t* offsets, uint8_t* bytes);
 
+/* ------------------------------------------------------------------ the store as RDF text: SparqlDatabase::generate_ntriples and
+ * generate_turtle (kolibrie/src/sparql_database.rs:301-382), byte for byte.
+ *   The triples are the store's SET, in ascending (s, p, o) id order (the reference's BTreeSet<Triple>, shared/src/triple.rs:13-18): a
+ *   triple held twice (two segments, an append) is written once. A term's text is decode_any(id).unwrap_or_default()
+ *   (sparql_database.rs:111-121): the dictionary string, `<< s p o >>` for a quoted id (recursively), and "" when the id, or any component
+ *   of a quoted id, is held by neither table (unlike kb_rel_decode's "unknown"). Nothing is escaped.
+ *   KB_SER_NTRIPLES: one line "S <P> O .\n" per triple. KB_SER_TURTLE: one "@prefix name: <uri> .\n" line per prefix pair in the given
+ *   order and a "\n" after them when there is one; then the triples grouped by subject TEXT, then predicate TEXT, both in byte order,
+ *   objects in id order within a group ("S <P1> O1 , O2 ;\n    <P2> O3 .\n"). S is the text when it starts with "<<", else <text>;
+ *   O the text when it starts with "<<", <text> when it starts with "http://" or "https://", else "text".
+ * kb_serialize_begin sorts, deduplicates, renders every distinct term once and lays the text out as UNITS (one N-Triples line; one
+ * triple's share of the Turtle text with its separators; the Turtle header); it keeps O(triples) device state and no text.
+ * prefix_offsets[2 * n_prefixes + 1] / prefix_bytes: string 2k is prefix k's name, 2k + 1 its URI (ignored for N-Triples).
+ * kb_serialize_next renders the next whole units that fit in `capacity` bytes (through a device staging buffer of at most
+ * KB_SER_STAGING_BYTES) into host_dst; *bytes_written = 0 once the text is complete. The pieces concatenated are the text for every
+ * capacity >= info.max_unit_bytes.
+ * Refused, nothing written and the store unchanged: an unknown format, a NULL argument (KB_E_INVALID); quoted ids in the store without a
+ * quoted-triple table, a non-empty store without device dictionary strings (KB_E_UNSUPPORTED); a walk deeper than KB_QUOTED_MAX_DEPTH
+ * (KB_E_LIMIT: the reference recurses without bound), more than 2^32-1 bytes of distinct rendered terms, a unit larger than
+ * KB_SER_STAGING_BYTES, 2^32 / 3 stored triples or more (KB_E_LIMIT). kb_serialize_next: capacity < max_unit_bytes (KB_E_LIMIT, nothing
+ * consumed); the store changed since begin, or a serializer of another context (KB_E_INVALID). Launches and device time count in
+ * kb_stats' `other` family. */
+enum kb_serialize_format { KB_SER_NTRIPLES = 0, KB_SER_TURTLE = 1 };
+#define KB_SER_STAGING_BYTES (256ull << 20)
+typedef struct kb_serializer kb_serializer;
+typedef struct kb_serialize_info {
+    uint64_t n_triples;        /* distinct triples */
+    uint64_t total_bytes;      /* bytes of the whole text, Turtle header included */
+    uint64_t max_unit_bytes;   /* the largest unit */
+    uint64_t n_subject_groups; /* Turtle: subject groups (0 for N-Triples) */
+    uint32_t n_terms;          /* distinct ids rendered */
+    uint32_t rank_rounds;      /* Turtle: refinement rounds of the text ranks (7 bytes a round) */
+    double phase_ms[4];        /* device time of begin's phases: sort + dedup, render, ranks, unit lengths + scan */
+} kb_serialize_info;
+KB_API kb_status kb_serialize_begin(kb_ctx* ctx, uint32_t format, const uint64_t* prefix_offsets, const uint8_t* prefix_bytes, uint32_t n_prefixes,
+                                    kb_serializer** out, kb_serialize_info* info /* nullable */);
+KB_API kb_status kb_serialize_next(kb_ctx* ctx, kb_serializer* ser, uint8_t* host_dst, uint64_t capacity, uint64_t* bytes_written);
+KB_API void kb_serialize_free(kb_serializer* ser);
+
 /* ------------------------------------------------------------------ BIND: `PhysicalOperator::Bind` with the built-in functions of
  * ExecutionEngine::execute_with_ids (kolibrie/src/streamertail_optimizer/execution/engine.rs:144-277) over the rows of `in`, in the order
  * they lie. *out = `in` with the output column: appended when out_slot is not a column of `in`, else that column replaced (the other

@@ -138,6 +138,19 @@ class KbOrderInfo(C.Structure):
                 **{n: list(getattr(self, n))[:n_keys] for n in ("key_kind", "n_distinct", "string_rounds")}}
 
 
+SER_NTRIPLES, SER_TURTLE = 0, 1  # kb_serialize_format
+
+
+class KbSerializeInfo(C.Structure):
+    """kb_serialize_info: distinct triples, text bytes, the largest unit, Turtle subject groups, rendered terms, rank rounds, and the
+    device time of kb_serialize_begin's phases (sort + dedup, render, ranks, unit lengths + scan)"""
+    _fields_ = [("n_triples", C.c_uint64), ("total_bytes", C.c_uint64), ("max_unit_bytes", C.c_uint64), ("n_subject_groups", C.c_uint64),
+                ("n_terms", C.c_uint32), ("rank_rounds", C.c_uint32), ("phase_ms", C.c_double * 4)]
+
+    def as_dict(self):
+        return {n: (list(getattr(self, n)) if n == "phase_ms" else int(getattr(self, n))) for n, _ in self._fields_}
+
+
 KB_BGP_MAX_PATTERNS = 16
 BGP_NONE, BGP_STAR, BGP_COMPONENTS = 0, 1, 2  # kb_bgp_route
 
@@ -270,6 +283,9 @@ def lib() -> C.CDLL:
         "kb_quoted_load": (i32, [vp, vp, vp, vp, vp, u64]),
         "kb_quoted_download": (i32, [vp, u32, u32, vp, vp, vp]),
         "kb_dict_strings_download": (i32, [vp, u32, u32, vp, vp]),
+        "kb_serialize_begin": (i32, [vp, u32, vp, vp, u32, P(vp), P(KbSerializeInfo)]),
+        "kb_serialize_next": (i32, [vp, vp, vp, u64, P(u64)]),
+        "kb_serialize_free": (None, [vp]),
         "kb_bind": (i32, [vp, vp, P(KbBindSpec), P(vp), P(KbBindInfo)]),
         "kb_rel_info": (i32, [vp, P(u64), P(u32), P(u32)]),
         "kb_rel_download": (i32, [vp, vp, u32, vp]),
@@ -339,7 +355,7 @@ def lib() -> C.CDLL:
 EXPORTED_SYMBOLS = [
     "kb_version", "kb_ctx_create", "kb_ctx_destroy", "kb_last_error", "kb_set_timing", "kb_get_stats", "kb_synchronize",
     "kb_store_load", "kb_store_load_device", "kb_store_append", "kb_store_append_device", "kb_store_evict", "kb_store_delete", "kb_store_clear", "kb_store_build_index", "kb_set_use_index", "kb_store_size",
-    "kb_store_download", "kb_dict_numeric_load", "kb_dict_legacy_i32_load", "kb_dict_numeric_derive", "kb_dict_numeric_download", "kb_dict_strings_load", "kb_dict_encode", "kb_dict_strings_info", "kb_rel_decode", "kb_strings_info", "kb_strings_download", "kb_strings_free", "kb_quoted_load", "kb_quoted_download", "kb_dict_strings_download", "kb_bind", "kb_rel_info", "kb_rel_download", "kb_rel_device_col", "kb_rel_from_host",
+    "kb_store_download", "kb_dict_numeric_load", "kb_dict_legacy_i32_load", "kb_dict_numeric_derive", "kb_dict_numeric_download", "kb_dict_strings_load", "kb_dict_encode", "kb_dict_strings_info", "kb_rel_decode", "kb_strings_info", "kb_strings_download", "kb_strings_free", "kb_quoted_load", "kb_quoted_download", "kb_dict_strings_download", "kb_serialize_begin", "kb_serialize_next", "kb_serialize_free", "kb_bind", "kb_rel_info", "kb_rel_download", "kb_rel_device_col", "kb_rel_from_host",
     "kb_rel_from_device", "kb_rel_free", "kb_scan", "kb_filter", "kb_project", "kb_hash_join", "kb_natural_join", "kb_hash_join_keyed", "kb_values", "kb_bind_join", "kb_scan_quoted", "kb_star_join", "kb_bgp_execute", "kb_bgp_last_plan",
     "kb_order_by", "kb_group_aggregate", "kb_groups_info", "kb_groups_keys", "kb_groups_values", "kb_groups_counts", "kb_groups_free", "kb_groups_pack", "kb_groups_merge", "kb_star_join_aggregate",
     "kb_star_join_prepare", "kb_plan_submit", "kb_plan_collect", "kb_plan_info", "kb_plan_free", "kb_plan_peer_scratch_bytes", "kb_plan_attach_peers",
@@ -597,6 +613,31 @@ class Context:
         self._check(lib().kb_dict_strings_download(self.h, first, n, _ptr(off), _ptr(data)))
         raw = data.tobytes()
         return [raw[int(off[k]):int(off[k + 1])].decode("utf-8") for k in range(n)]
+
+    def serialize(self, fmt: int, prefixes: Sequence[Tuple[str, str]] = (), capacity: int = 64 << 20, info: Optional[dict] = None):
+        """kb_serialize_begin / _next: the store as N-Triples-star (SER_NTRIPLES) or Turtle-star (SER_TURTLE) text, yielded as bytes
+        pieces of at most `capacity` bytes (whole units each; capacity must hold the largest unit). prefixes: (name, uri) pairs, in the
+        order the Turtle header lists them. `info`, when given, receives kb_serialize_info as a dict before the first piece."""
+        enc = [x.encode("utf-8") for pr in prefixes for x in pr]
+        off = np.zeros(len(enc) + 1, dtype=np.uint64)
+        if enc:
+            off[1:] = np.cumsum([len(b) for b in enc], dtype=np.uint64)
+        data = np.frombuffer(b"".join(enc), dtype=np.uint8) if off[-1] else np.empty(0, np.uint8)
+        h, inf = C.c_void_p(), KbSerializeInfo()
+        self._check(lib().kb_serialize_begin(self.h, fmt, _ptr(off), _ptr(data) if len(data) else None, len(prefixes), C.byref(h), C.byref(inf)))
+        try:
+            if info is not None:
+                info.update(inf.as_dict())
+            cap = min(capacity, inf.total_bytes)  # (a capacity below the largest unit is refused by the library)
+            buf = np.empty(max(cap, 1), dtype=np.uint8)
+            got = C.c_uint64()
+            while True:
+                self._check(lib().kb_serialize_next(self.h, h, _ptr(buf), cap, C.byref(got)))
+                if got.value == 0:
+                    return
+                yield buf[: got.value].tobytes()
+        finally:
+            lib().kb_serialize_free(h)
 
     # ---- operators
     def bind(self, rel: Relation, function: int, args: Sequence[KbTerm], out_slot: int, next_qt_id: int = 0,

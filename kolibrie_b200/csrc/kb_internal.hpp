@@ -414,6 +414,10 @@ kb_status star_join_impl(kb_ctx* ctx, u32 join_slot, const kb_pattern* pats, u32
 // kb_bind_join behind the entry point (the pattern is checked by the caller)
 kb_status bind_join_impl(kb_ctx* ctx, const kb_rel& left, const kb_pattern& pat, std::unique_ptr<kb_rel>* out);
 QuotedTab quotedtab(const kb_ctx* ctx);
+// Dense ranks of d >= 1 values (kb_order.cu), given by an order key per value (nkey, numeric) or by their rendered strings (str_off[d + 1]
+// u32 offsets into bytes, compared byte by byte, a proper prefix first): afterwards rank_of[v] is the rank of value v, *n_values the
+// number of distinct values and *rounds the refinement rounds taken (7 bytes of string a round).
+kb_status rank_values(kb_ctx* ctx, u32 d, const unsigned long long* nkey, const u32* str_off, const u8* bytes, u32* rank_of, u32* n_values, u32* rounds);
 // kb_dict_encode's body over a batch already in device memory (kb_dict.cu)
 kb_status dict_encode_device(kb_ctx* ctx, const u64* d_off, const unsigned char* d_bytes, u64 n_terms, u64 total, u32* d_out_ids, u32* n_new,
                              Buf* first_pos);

@@ -2904,13 +2904,14 @@ __device__ u32 quoted_walk(u32 id, u32 dict_ids, const QuotedTab& qt, Lit lit, W
 }
 
 __global__ void __launch_bounds__(256) decode_lengths_kernel(const u32* __restrict__ ids, u32 n, const unsigned long long* __restrict__ dict_off, u32 dict_ids,
-                                                             const QuotedTab qt, u32* __restrict__ len, unsigned long long* total, u32* quoted, u32* deep) {
+                                                             const QuotedTab qt, u32* __restrict__ len, unsigned long long* total, u32* quoted, u32* deep,
+                                                             u32 missing_len) {
     const u32 stride = gridDim.x * blockDim.x;
     unsigned long long t = 0;
     bool q = false, dp = false;
     for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
         const u32 id = ids[i];
-        unsigned long long l = 7u;  // "unknown"
+        unsigned long long l = missing_len;  // "unknown" or ""
         if (id & 0x80000000u) {
             if (qt.n == 0u) {
                 q = true;
@@ -2934,10 +2935,10 @@ __global__ void __launch_bounds__(256) decode_lengths_kernel(const u32* __restri
     if (dp) *deep = 1u;
 }
 void launch_decode_lengths(const u32* ids, u32 n, const unsigned long long* dict_off, u32 dict_ids, const QuotedTab& qt, u32* len,
-                           unsigned long long* total, u32* quoted, u32* deep, int n_sms, cudaStream_t st) {
+                           unsigned long long* total, u32* quoted, u32* deep, int n_sms, cudaStream_t st, bool missing_empty) {
     if (n == 0) return;
     const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull);
-    decode_lengths_kernel<<<grid, 256, 0, st>>>(ids, n, dict_off, dict_ids, qt, len, total, quoted, deep);
+    decode_lengths_kernel<<<grid, 256, 0, st>>>(ids, n, dict_off, dict_ids, qt, len, total, quoted, deep, missing_empty ? 0u : 7u);
 }
 __global__ void __launch_bounds__(256) decode_gather_kernel(const u32* __restrict__ ids, u32 n, const unsigned long long* __restrict__ dict_off,
                                                             const unsigned char* __restrict__ dict_bytes, u32 dict_ids, const QuotedTab qt,
@@ -2956,7 +2957,7 @@ __global__ void __launch_bounds__(256) decode_gather_kernel(const u32* __restric
             l = off[i + 1] - dst;
             known = id < dict_ids;
             if (known) src = __ldg(dict_off + id);
-            walk = (id & 0x80000000u) != 0u && l != 7u;  // a rendered quoted term is at least 8 bytes: 7 is "unknown"
+            walk = (id & 0x80000000u) != 0u && l >= 8u;  // a rendered quoted term is at least 8 bytes: 7 is "unknown", 0 is ""
         }
         const u32 wl = walk ? 0u : l;
         for (int r = 0; r < 32; r++) {  // the warp copies row r of its chunk: consecutive lanes, consecutive bytes

@@ -515,10 +515,13 @@ struct QuotedTab {
 // len[i] = length of the string of ids[i] ("unknown" = 7 bytes when the dictionary does not hold the id). A quoted id: without a table
 // *quoted = 1; with one, the length of `<< s p o >>` walked with a bounded stack (dictionary.rs:60-72), "unknown" when any id on the walk
 // is held by neither table, and *deep = 1 when the walk goes past KB_QUOTED_MAX_DEPTH levels first. *total += sum.
+// missing_empty: a term the tables do not hold renders as "" instead of "unknown" (decode_any(..).unwrap_or_default(), the serializers'
+// rule, sparql_database.rs:301-322).
 void launch_decode_lengths(const u32* ids, u32 n, const unsigned long long* dict_off, u32 dict_ids, const QuotedTab& qt, u32* len,
-                           unsigned long long* total, u32* quoted, u32* deep, int n_sms, cudaStream_t st);
+                           unsigned long long* total, u32* quoted, u32* deep, int n_sms, cudaStream_t st, bool missing_empty = false);
 // out[off[i] .. off[i+1]) = bytes of the string of ids[i]; one warp per 32 rows, the lanes copy each dictionary string together; a quoted
-// row is written by its own thread, walking the term again
+// row is written by its own thread, walking the term again (a missing term is 7 bytes, "unknown", or 0: either way shorter than the
+// 8 bytes of the shortest rendered quoted term)
 void launch_decode_gather(const u32* ids, u32 n, const unsigned long long* dict_off, const unsigned char* dict_bytes, u32 dict_ids, const QuotedTab& qt,
                           const u32* off, unsigned char* out, int n_sms, cudaStream_t st);
 

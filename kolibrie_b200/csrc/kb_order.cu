@@ -232,8 +232,9 @@ struct KeyRank {
     u32 kind = KB_ORDER_CONST, distinct = 0, rounds = 0;
 };
 
-// Ranks D values, given by an order key per value (numeric) or by their rendered strings (str_off != null): afterwards rank_of[v] is
-// the dense rank of value v and *n_values the number of distinct values.
+}  // namespace
+
+// (declared in kb_internal.hpp: kb_serialize.cu ranks rendered terms with it)
 kb_status rank_values(kb_ctx* ctx, u32 d, const unsigned long long* nkey, const u32* str_off, const u8* bytes, u32* rank_of, u32* n_values, u32* rounds) {
     Buf ord, grp, act, act2, key, key2, gkey, gs, gs2, s_of, idx, idx2, idx3, head, hp, more;
     const size_t n4 = (size_t)d * sizeof(u32);
@@ -290,6 +291,8 @@ kb_status rank_values(kb_ctx* ctx, u32 d, const unsigned long long* nkey, const 
     ctx->stats.d2h_bytes += sizeof(u32);
     return KB_OK;
 }
+
+namespace {
 
 // the rank column of one key; refusals (KB_E_UNSUPPORTED) before any output exists
 kb_status rank_key(kb_ctx* ctx, const kb_rel& in, u32 col, bool desc, KeyRank* kr) {

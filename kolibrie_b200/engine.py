@@ -413,6 +413,7 @@ class SparqlDatabase:
         self._uploaded_version = -1
         self._version = 0
         self._uploaded_quoted = -1  # size of the quoted-triple store the context's table was loaded from
+        self.prefixes: List[Tuple[str, str]] = []  # sparql_database.rs:54, ordered: the Turtle header lists them in this order
 
     def encode_term(self, t) -> int:
         """a term given as a string, or as a nested (s, p, o) tuple for a quoted triple `<< s p o >>` (components encoded first, in
@@ -433,6 +434,39 @@ class SparqlDatabase:
                 return None
             return "<< " + " ".join(parts) + " >>"
         return self.dictionary.decode(i)
+
+    def set_prefixes(self, prefixes):
+        """SparqlDatabase::set_prefixes (sparql_database.rs:193-195) with an ORDER: (name, uri) pairs, or a dict in its iteration order.
+        The reference keeps a HashMap, so the order of its Turtle header is unspecified; here it is this order."""
+        self.prefixes = [(str(k), str(v)) for k, v in (prefixes.items() if isinstance(prefixes, dict) else prefixes)]
+
+    def generate_ntriples(self) -> str:
+        """SparqlDatabase::generate_ntriples (sparql_database.rs:301-322): the store as N-Triples-star, rendered on the device"""
+        return self._serialize(c.SER_NTRIPLES)
+
+    def generate_turtle(self) -> str:
+        """SparqlDatabase::generate_turtle (sparql_database.rs:324-382): the store as Turtle-star with this database's prefixes"""
+        return self._serialize(c.SER_TURTLE)
+
+    def _serialize(self, fmt: int) -> str:
+        if hasattr(self.ctx, "serialize"):  # sorted, grouped and written on the device (kb_serialize_begin / _next)
+            self._sync()
+            return b"".join(self.ctx.serialize(fmt, self.prefixes)).decode("utf-8")
+        # contexts without it (the oracle): the reference's loops over the triple set, decode_any(..).unwrap_or_default()
+        text = lambda i: self.decode_term(i) or ""
+        subj = lambda t: t if t.startswith("<<") else f"<{t}>"
+        obj = lambda t: t if t.startswith("<<") else f"<{t}>" if t.startswith(("http://", "https://")) else f'"{t}"'
+        rows = [tuple(text(x) for x in t) for t in sorted(self.triples)]
+        if fmt == c.SER_NTRIPLES:
+            return "".join(f"{subj(s)} <{p}> {obj(o)} .\n" for s, p, o in rows)
+        out = [f"@prefix {k}: <{v}> .\n" for k, v in self.prefixes] + (["\n"] if self.prefixes else [])
+        groups: Dict[str, Dict[str, List[str]]] = {}
+        for s, p, o in rows:
+            groups.setdefault(s, {}).setdefault(p, []).append(o)
+        for s in sorted(groups):  # str order = UTF-8 byte order (Rust String)
+            preds = groups[s]
+            out.append(subj(s) + " ;\n    ".join(f" <{p}>"[i > 0:] + " ,".join(" " + obj(o) for o in preds[p]) for i, p in enumerate(sorted(preds))) + " .\n")
+        return "".join(out)
 
     def add_statement(self, s, p, o):
         """add one triple whose terms are strings or nested tuples (quoted triples)"""

@@ -69,6 +69,14 @@ pub const KB_ORDER_CONST: u32 = 0; pub const KB_ORDER_NUMERIC: u32 = 1; pub cons
     pub key_kind: [u32; KB_MAX_COLS], pub n_distinct: [u32; KB_MAX_COLS], pub string_rounds: [u32; KB_MAX_COLS] }
 pub type kb_order_key = KbOrderKey;  // (the header's names, as the declaration below spells them)
 pub type kb_order_info = KbOrderInfo;
+// kb_serialize_begin / _next / _free: the store as N-Triples-star or Turtle-star text (kb_serialize_format)
+pub const KB_SER_NTRIPLES: u32 = 0; pub const KB_SER_TURTLE: u32 = 1;
+pub const KB_SER_STAGING_BYTES: u64 = 256 << 20;
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbSerializeInfo { pub n_triples: u64, pub total_bytes: u64, pub max_unit_bytes: u64,
+    pub n_subject_groups: u64, pub n_terms: u32, pub rank_rounds: u32, pub phase_ms: [c_double; 4] }
+pub type kb_serialize_info = KbSerializeInfo;  // (the header's name, as the declaration below spells it)
+pub enum KbSerializer {}
+pub type kb_serializer = KbSerializer;  // (the header's name, as the declarations below spell it)
 
 // kb_filter_opcode / kb_cmp / kb_agg_kind / kb_strategy
 pub const KB_F_CMP_NUM: u32 = 1; pub const KB_F_EQ_ID: u32 = 2; pub const KB_F_NE_ID: u32 = 3; pub const KB_F_AND: u32 = 4; pub const KB_F_OR: u32 = 5;
@@ -119,6 +127,11 @@ extern "C" {
     pub fn kb_quoted_download(ctx: *mut KbCtx, first_id: u32, n: u32, s: *mut u32, p: *mut u32, o: *mut u32) -> kb_status;
     pub fn kb_dict_strings_download(ctx: *mut KbCtx, first: u32, n: u32, offsets: *mut u64, bytes: *mut u8) -> kb_status;
     pub fn kb_rel_free(ctx: *mut KbCtx, r: *mut KbRel);
+    // the store as RDF text, in pieces of whole units (sparql_database.rs:301-382)
+    pub fn kb_serialize_begin(ctx: *mut KbCtx, format: u32, prefix_offsets: *const u64, prefix_bytes: *const u8, n_prefixes: u32,
+                              out: *mut *mut kb_serializer, info: *mut kb_serialize_info) -> kb_status;
+    pub fn kb_serialize_next(ctx: *mut KbCtx, ser: *mut kb_serializer, host_dst: *mut u8, capacity: u64, bytes_written: *mut u64) -> kb_status;
+    pub fn kb_serialize_free(ser: *mut kb_serializer);
     // operators
     pub fn kb_scan(ctx: *mut KbCtx, pats: *const KbPattern, n: u32, pushdown: *const *const KbFilterOp, pushdown_len: *const u32, out: *mut *mut KbRel) -> kb_status;
     pub fn kb_filter(ctx: *mut KbCtx, r: *const KbRel, prog: *const KbFilterOp, n: u32, out: *mut *mut KbRel) -> kb_status;

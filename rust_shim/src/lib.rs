@@ -118,6 +118,33 @@ impl DeviceStore {
         if self.synced_dict != usize::MAX { self.synced_dict += n_new as usize; }
         Ok((ids, first))
     }
+
+    /// `SparqlDatabase::generate_ntriples` (`turtle` false) or `generate_turtle` (sparql_database.rs:301-382) of the device store
+    /// (`sync` first), written on the device: `sink` receives the text in pieces of whole lines / triples, each at most `capacity`
+    /// bytes (at least the largest unit, `kb_serialize_info.max_unit_bytes`). `prefixes` are the Turtle header's (name, uri) pairs
+    /// in the order given.
+    pub fn serialize(&mut self, turtle: bool, prefixes: &[(&str, &str)], capacity: usize, mut sink: impl FnMut(&[u8])) -> Result<kb_serialize_info, String> {
+        let mut offs = vec![0u64];
+        let mut bytes = Vec::new();
+        for (name, uri) in prefixes {
+            for x in [name, uri] { bytes.extend_from_slice(x.as_bytes()); offs.push(bytes.len() as u64); }
+        }
+        let mut ser: *mut kb_serializer = ptr::null_mut();
+        let mut info = KbSerializeInfo::default();
+        let fmt = if turtle { KB_SER_TURTLE } else { KB_SER_NTRIPLES };
+        if unsafe { kb_serialize_begin(self.ctx, fmt, offs.as_ptr(), bytes.as_ptr(), prefixes.len() as u32, &mut ser, &mut info) } != KB_OK {
+            return Err(self.last_error());
+        }
+        let mut buf = vec![0u8; capacity.min(info.total_bytes as usize).max(1)];
+        let result = loop {
+            let mut got = 0u64;
+            if unsafe { kb_serialize_next(self.ctx, ser, buf.as_mut_ptr(), buf.len() as u64, &mut got) } != KB_OK { break Err(self.last_error()); }
+            if got == 0 { break Ok(info); }
+            sink(&buf[..got as usize]);
+        };
+        unsafe { kb_serialize_free(ser) };
+        result
+    }
 }
 
 impl Drop for DeviceStore {
