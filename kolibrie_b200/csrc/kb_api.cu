@@ -64,6 +64,15 @@ kb_status alloc_buf(kb_ctx* ctx, size_t bytes, Buf* out) {
     return KB_OK;
 }
 
+kb_status tag_batch_table(kb_ctx* ctx, u64 n, Buf* tab, u64* slots) {
+    u64 s = 1024;
+    while (s < 2 * n) s <<= 1;
+    KB_TRY(alloc_buf(ctx, s * sizeof(u64), tab));
+    KB_CUDA(ctx, cudaMemsetAsync((*tab)->p, 0xFF, s * sizeof(u64), ctx->st));
+    *slots = s;
+    return KB_OK;
+}
+
 kb_status alloc_col(kb_ctx* ctx, u64 rows, Col* out) {
     Buf b;
     KB_TRY(alloc_buf(ctx, (size_t)rows * sizeof(u32), &b));
@@ -752,96 +761,6 @@ kb_status kb_dict_legacy_i32_load(kb_ctx* ctx, const int32_t* val, const uint8_t
     return KB_OK;
 }
 
-kb_status kb_dict_strings_load(kb_ctx* ctx, const uint64_t* offsets, const uint8_t* bytes, uint32_t n_ids) {
-    KB_ENTER(ctx);
-    ctx->dict_off.reset();
-    ctx->dict_bytes.reset();
-    ctx->dict_ids = 0;
-    ctx->dict_index.reset();  // (kb_dict_encode rebuilds its string -> id index lazily)
-    ctx->dict_index_slots = 0;
-    ctx->dict_indexed = 0;
-    if (n_ids == 0) return KB_OK;
-    if (!offsets) return kb::fail(ctx, KB_E_INVALID, "NULL offsets");
-    const uint64_t total = offsets[n_ids];
-    if (offsets[0] != 0 || (total && !bytes)) return kb::fail(ctx, KB_E_INVALID, "offsets must start at 0 and bytes must not be NULL");
-    for (uint32_t i = 0; i < n_ids; i++) if (offsets[i + 1] < offsets[i]) return kb::fail(ctx, KB_E_INVALID, "offsets decrease at id %u", i);
-    KB_TRY(kb::alloc_buf(ctx, ((size_t)n_ids + 1) * sizeof(uint64_t), &ctx->dict_off));
-    KB_TRY(kb::alloc_buf(ctx, (size_t)total + 16, &ctx->dict_bytes));
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->dict_off->p, offsets, ((size_t)n_ids + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->st));
-    if (total) KB_CUDA(ctx, cudaMemcpyAsync(ctx->dict_bytes->p, bytes, (size_t)total, cudaMemcpyHostToDevice, ctx->st));
-    KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
-    ctx->stats.h2d_bytes += ((size_t)n_ids + 1) * sizeof(uint64_t) + total;
-    ctx->dict_ids = n_ids;
-    return KB_OK;
-}
-
-kb_status kb_rel_decode(kb_ctx* ctx, const kb_rel* r, uint32_t col, kb_strings** out) {
-    KB_ENTER(ctx);
-    if (!r || !out) return kb::fail(ctx, KB_E_INVALID, "NULL argument");
-    if (col >= r->cols.size()) return kb::fail(ctx, KB_E_INVALID, "column %u out of range", col);
-    if (r->n >= 0xFFFFFFF0ull) return kb::fail(ctx, KB_E_LIMIT, "relation too large");
-    auto res = std::make_unique<kb_strings>();
-    res->n = r->n;
-    const u32 n = (u32)r->n;
-    KB_TRY(kb::alloc_buf(ctx, ((size_t)n + 1) * sizeof(u32), &res->off));
-    u32* off = static_cast<u32*>(res->off->p);
-    const u32 c = kb::ctrl_alloc(ctx, 4);  // [0..1] u64 total bytes, [2] quoted-triple id seen without a table, [3] walk too deep
-    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + c, 0, 4 * sizeof(u32), ctx->st));
-    KB_CUDA(ctx, cudaMemsetAsync(off + n, 0, sizeof(u32), ctx->st));  // the scan runs over n + 1 entries: off[n] becomes the total
-    const auto* doff = ctx->dict_ids ? static_cast<const unsigned long long*>(ctx->dict_off->p) : nullptr;
-    const auto* dbytes = ctx->dict_ids ? static_cast<const unsigned char*>(ctx->dict_bytes->p) : nullptr;
-    const kb::QuotedTab qt = kb::quotedtab(ctx);
-    kb::Buf scratch;
-    KB_TRY(kb::alloc_buf(ctx, (((size_t)n + 1) / 2048 + 4) * sizeof(u32), &scratch));
-    kb::timer_begin(ctx, kb::F_OTHER, 4);
-    kb::launch_decode_lengths(r->cols[col].ptr, n, doff, ctx->dict_ids, qt, off, reinterpret_cast<unsigned long long*>(ctx->ctrl + c), ctx->ctrl + c + 2,
-                              ctx->ctrl + c + 3, ctx->n_sms, ctx->st);
-    kb::launch_exclusive_scan_u32(off, n + 1, static_cast<u32*>(scratch->p), ctx->st);
-    kb::timer_end(ctx);
-    KB_CUDA(ctx, cudaGetLastError());
-    KB_TRY(kb::ctrl_read(ctx));
-    unsigned long long total = 0;
-    memcpy(&total, ctx->h_ctrl + c, sizeof total);
-    if (ctx->h_ctrl[c + 2]) return kb::fail(ctx, KB_E_UNSUPPORTED, "the column holds quoted-triple ids (bit 31) and no quoted-triple table is loaded (kb_quoted_load)");
-    if (ctx->h_ctrl[c + 3]) return kb::fail(ctx, KB_E_LIMIT, "a quoted-triple term nests deeper than %d levels", KB_QUOTED_MAX_DEPTH);
-    if (total > 0xFFFFFFFFull) return kb::fail(ctx, KB_E_LIMIT, "decoded column would take %llu bytes (limit 2^32-1 per call)", total);
-    res->total = total;
-    KB_TRY(kb::alloc_buf(ctx, (size_t)total + 16, &res->bytes));
-    kb::timer_begin(ctx, kb::F_OTHER);
-    kb::launch_decode_gather(r->cols[col].ptr, n, doff, dbytes, ctx->dict_ids, qt, off, static_cast<unsigned char*>(res->bytes->p), ctx->n_sms, ctx->st);
-    kb::timer_end(ctx);
-    KB_CUDA(ctx, cudaGetLastError());
-    *out = res.release();
-    return KB_OK;
-}
-kb_status kb_strings_info(const kb_strings* s, uint64_t* n_strings, uint64_t* total_bytes) {
-    if (!s) return KB_E_INVALID;
-    if (n_strings) *n_strings = s->n;
-    if (total_bytes) *total_bytes = s->total;
-    return KB_OK;
-}
-kb_status kb_strings_download(kb_ctx* ctx, const kb_strings* s, uint64_t* offsets, uint8_t* bytes) {
-    if (!ctx || !s) return KB_E_INVALID;
-    kb::DeviceGuard guard(ctx->device);
-    if (offsets) {
-        std::vector<u32> h((size_t)s->n + 1);
-        KB_CUDA(ctx, cudaMemcpyAsync(h.data(), s->off->p, h.size() * sizeof(u32), cudaMemcpyDeviceToHost, ctx->st));
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
-        for (size_t i = 0; i < h.size(); i++) offsets[i] = h[i];
-    }
-    if (bytes && s->total) {
-        KB_CUDA(ctx, cudaMemcpyAsync(bytes, s->bytes->p, (size_t)s->total, cudaMemcpyDeviceToHost, ctx->st));
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
-    }
-    ctx->stats.d2h_bytes += ((size_t)s->n + 1) * sizeof(u32) + s->total;
-    return KB_OK;
-}
-void kb_strings_free(kb_ctx* ctx, kb_strings* s) {
-    if (!s) return;
-    if (ctx) { kb::DeviceGuard guard(ctx->device); delete s; }
-    else delete s;
-}
-
 // ------------------------------------------------------------------ relations
 kb_status kb_rel_info(const kb_rel* r, uint64_t* n_rows, uint32_t* n_cols, uint32_t* slots) {
     if (!r) return KB_E_INVALID;
@@ -961,161 +880,6 @@ kb_status kb_bind_join(kb_ctx* ctx, const kb_rel* left, const kb_pattern* pat, k
     KB_TRY(kb::bind_join_impl(ctx, *left, *pat, &r));
     ctx->stats.rows_out = r->n;
     *out = r.release();
-    return KB_OK;
-}
-}  // extern "C"
-
-// ------------------------------------------------------------------ quoted triples
-kb::QuotedTab kb::quotedtab(const kb_ctx* ctx) {
-    kb::QuotedTab t{};
-    if (ctx->quoted_slots) {
-        t.s = static_cast<const u32*>(ctx->quoted_s->p);
-        t.p = static_cast<const u32*>(ctx->quoted_p->p);
-        t.o = static_cast<const u32*>(ctx->quoted_o->p);
-        t.n = ctx->quoted_slots;
-    }
-    return t;
-}
-
-extern "C" {
-kb_status kb_quoted_load(kb_ctx* ctx, const uint32_t* ids, const uint32_t* s, const uint32_t* p, const uint32_t* o, uint64_t n) {
-    KB_ENTER(ctx);
-    if (n == 0) {
-        ctx->quoted_s.reset(); ctx->quoted_p.reset(); ctx->quoted_o.reset();
-        ctx->quoted_slots = ctx->quoted_cap = 0;
-        ctx->quoted_rev.reset();
-        ctx->quoted_rev_slots = 0;
-        ctx->quoted_rev_indexed = 0;
-        return KB_OK;
-    }
-    if (!ids || !s || !p || !o) return kb::fail(ctx, KB_E_INVALID, "NULL argument");
-    u32 slots = 0;
-    for (uint64_t i = 0; i < n; i++) {
-        if (!(ids[i] & 0x80000000u) || ids[i] == KB_ID_NONE)
-            return kb::fail(ctx, KB_E_INVALID, "entry %llu: id 0x%08x is not a quoted-triple id (bit 31, not KB_ID_NONE)", (unsigned long long)i, ids[i]);
-        if (s[i] == KB_ID_NONE || p[i] == KB_ID_NONE || o[i] == KB_ID_NONE)
-            return kb::fail(ctx, KB_E_INVALID, "entry %llu: component KB_ID_NONE (reserved)", (unsigned long long)i);
-        const u32 x = ids[i] & 0x7FFFFFFFu;
-        if (x >= KB_QUOTED_MAX_SLOTS) return kb::fail(ctx, KB_E_LIMIT, "quoted-triple id 0x%08x: index beyond the table's %u slots", ids[i], KB_QUOTED_MAX_SLOTS);
-        slots = std::max(slots, x + 1u);
-    }
-    std::vector<u32> h((size_t)slots * 3, kb::EMPTY32);  // s | p | o
-    for (uint64_t i = 0; i < n; i++) {
-        const u32 x = ids[i] & 0x7FFFFFFFu;
-        if (h[(size_t)slots + x] != kb::EMPTY32) return kb::fail(ctx, KB_E_INVALID, "quoted-triple id 0x%08x given twice", ids[i]);
-        h[x] = s[i];
-        h[(size_t)slots + x] = p[i];
-        h[2 * (size_t)slots + x] = o[i];
-    }
-    kb::Buf bs, bp, bo;  // the new table is complete before it replaces the old one
-    KB_TRY(kb::alloc_buf(ctx, (size_t)slots * sizeof(u32), &bs));
-    KB_TRY(kb::alloc_buf(ctx, (size_t)slots * sizeof(u32), &bp));
-    KB_TRY(kb::alloc_buf(ctx, (size_t)slots * sizeof(u32), &bo));
-    KB_CUDA(ctx, cudaMemcpyAsync(bs->p, h.data(), (size_t)slots * sizeof(u32), cudaMemcpyHostToDevice, ctx->st));
-    KB_CUDA(ctx, cudaMemcpyAsync(bp->p, h.data() + slots, (size_t)slots * sizeof(u32), cudaMemcpyHostToDevice, ctx->st));
-    KB_CUDA(ctx, cudaMemcpyAsync(bo->p, h.data() + 2 * (size_t)slots, (size_t)slots * sizeof(u32), cudaMemcpyHostToDevice, ctx->st));
-    KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
-    ctx->stats.h2d_bytes += (u64)slots * 12u;
-    ctx->quoted_s = bs; ctx->quoted_p = bp; ctx->quoted_o = bo;
-    ctx->quoted_slots = ctx->quoted_cap = slots;
-    ctx->quoted_rev.reset();  // (kb_bind rebuilds it on its next TRIPLE)
-    ctx->quoted_rev_slots = 0;
-    ctx->quoted_rev_indexed = 0;
-    return KB_OK;
-}
-
-// resolve_quoted_triple_scan (engine.rs:1111-1188): the match kernel gives one row (entry id in a fresh slot F, inner variables) per
-// accepted entry; the outer pattern with F in the quoted position(s) is bind-joined to those rows, which merges the bindings and drops
-// the rows whose shared variables conflict; F is projected away.
-kb_status kb_scan_quoted(kb_ctx* ctx, const kb_quoted_pattern* qp, kb_rel** out) {
-    KB_ENTER(ctx);
-    if (!qp || !out) return kb::fail(ctx, KB_E_INVALID, "NULL argument");
-    const kb_pattern& op = qp->outer;
-    if (op.p.is_var == KB_TERM_QUOTED) return kb::fail(ctx, KB_E_UNSUPPORTED, "quoted triple in predicate position");
-    const bool qs = op.s.is_var == KB_TERM_QUOTED, qo = op.o.is_var == KB_TERM_QUOTED;
-    if (!qs && !qo) return kb::fail(ctx, KB_E_INVALID, "kb_scan_quoted: neither subject nor object is quoted (use kb_scan)");
-    // the terms in reading order: s, p, o with each quoted term inlined as its own s, p, o; inner terms carry their component
-    struct T { const kb_term* t; int comp; };  // comp -1: a term of the outer pattern
-    std::vector<T> terms;
-    auto inline_pos = [&](const kb_term& t, const kb_pattern& in) {
-        if (t.is_var == KB_TERM_QUOTED) { terms.push_back({&in.s, 0}); terms.push_back({&in.p, 1}); terms.push_back({&in.o, 2}); }
-        else terms.push_back({&t, -1});
-    };
-    inline_pos(op.s, qp->inner_s);
-    terms.push_back({&op.p, -1});
-    inline_pos(op.o, qp->inner_o);
-    std::vector<u32> used, order;  // every variable; the result's columns
-    for (const T& x : terms) {
-        if (x.t->is_var > KB_TERM_QUOTED || (x.comp < 0 && x.t->is_var == KB_TERM_QUOTED))
-            return kb::fail(ctx, KB_E_INVALID, "kb_term.is_var must be 0 or 1 (or KB_TERM_QUOTED in a quoted position / inside an inner pattern)");
-        if (x.t->is_var == 0 && x.t->value == KB_ID_NONE) return kb::fail(ctx, KB_E_INVALID, "constant id 0xFFFFFFFF is reserved (KB_ID_NONE)");
-        if (x.t->is_var == 1) {
-            if (x.t->value >= 4096) return kb::fail(ctx, KB_E_LIMIT, "variable slot %u too large (max 4095)", x.t->value);
-            if (std::find(order.begin(), order.end(), x.t->value) == order.end()) order.push_back(x.t->value);
-        }
-    }
-    u32 F = 0;  // a slot no variable of the pattern uses
-    while (std::find(order.begin(), order.end(), F) != order.end()) F++;
-    // the match: checks on the entry's components, output columns (entry id, inner variables in order of first appearance)
-    kb::QuotedMatchParams P{};
-    P.t = kb::quotedtab(ctx);
-    std::vector<u32> mslots{F};
-    std::vector<std::pair<u32, u32>> first;  // inner variable -> component of its first occurrence
-    for (const T& x : terms) {
-        if (x.comp < 0) continue;
-        if (x.t->is_var != 1u) {
-            P.chk_kind[P.n_chk] = x.t->is_var == KB_TERM_QUOTED ? kb::QM_QUOTED : kb::QM_CONST;
-            P.chk_comp[P.n_chk] = (u32)x.comp;
-            P.chk_arg[P.n_chk++] = x.t->value;
-        } else {
-            auto it = std::find_if(first.begin(), first.end(), [&](const std::pair<u32, u32>& f) { return f.first == x.t->value; });
-            if (it == first.end()) {
-                first.push_back({x.t->value, (u32)x.comp});
-                P.out_comp[mslots.size()] = (u32)x.comp;
-                mslots.push_back(x.t->value);
-            } else if (it->second != (u32)x.comp) {  // a repeated variable: equal components (the same entry fills both quoted positions)
-                P.chk_kind[P.n_chk] = kb::QM_EQ;
-                P.chk_comp[P.n_chk] = (u32)x.comp;
-                P.chk_arg[P.n_chk++] = it->second;
-            }
-        }
-    }
-    P.n_out = (u32)mslots.size();
-    std::unique_ptr<kb_rel> res;
-    if (P.t.n == 0) {
-        KB_TRY(kb::empty_rel(ctx, order, &res));
-        ctx->stats.rows_out = 0;
-        *out = res.release();
-        return KB_OK;
-    }
-    auto m = std::make_unique<kb_rel>();
-    m->slots = mslots;
-    KB_TRY(kb::alloc_strided_cols(ctx, P.t.n, P.n_out, &m->cols));
-    for (u32 c = 0; c < P.n_out; c++) P.out[c] = m->cols[c].ptr;
-    const u32 off = kb::ctrl_alloc(ctx, 4);
-    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, 4 * sizeof(u32), ctx->st));
-    P.count = ctx->ctrl + off;
-    P.ticket = ctx->ctrl + off + 1;
-    P.n_tiles = (P.t.n + kb::QM_TILE - 1) / kb::QM_TILE;
-    kb::timer_begin(ctx, kb::F_SCAN);
-    kb::launch_quoted_match(P, ctx->n_sms, ctx->st);
-    kb::timer_end(ctx);
-    KB_CUDA(ctx, cudaGetLastError());
-    KB_TRY(kb::ctrl_read(ctx));
-    m->n = ctx->h_ctrl[off];
-    ctx->stats.rows_scanned += P.t.n;
-    if (m->n == 0) {
-        KB_TRY(kb::empty_rel(ctx, order, &res));
-    } else {
-        kb_pattern po = op;
-        if (qs) po.s = kb_term{1, F};
-        if (qo) po.o = kb_term{1, F};
-        std::unique_ptr<kb_rel> j;
-        KB_TRY(kb::bind_join_impl(ctx, *m, po, &j));
-        res = kb::select_cols(*j, order);
-    }
-    ctx->stats.rows_out = res->n;
-    *out = res.release();
     return KB_OK;
 }
 

@@ -3,138 +3,160 @@
 // send the scans, joins and filters beneath it back to the CPU. The semantics are in include/kolibrie_b200.h; here:
 //   SUBJECT / PREDICATE / OBJECT  one gather pass over the quoted-triple table
 //   isTRIPLE                      a pass for the first row that needs "true" / "false", the encode of those strings, a write pass
-//   TRIPLE                        QuotedTripleStore::encode of the batch: reverse-index probe, batch table of the misses (smallest row
-//                                 wins), first-occurrence scan, ids next_qt_id + rank; the new entries join the table and the index
+//   TRIPLE                        QuotedTripleStore::encode of the batch (quoted_encode, kb_quoted.cu)
 //   CONCAT                        lengths, scan, byte gather, then kb_dict_encode's body on the concatenations (dict_encode_device)
 #include <algorithm>
 #include <cstring>
 
 #include "kb_internal.hpp"
 
+namespace kb {
+
+// BIND built-ins (kb_bind, engine.rs:144-277). Every write pass takes `old` (the replaced column when the output variable was bound
+// already, else null): a row the reference does not insert into keeps old[i], or gets EMPTY32; *n_unbound += rows left EMPTY32.
+// SUBJECT / PREDICATE / OBJECT: out[i] = component `comp` of the table entry of arg[i] (a quoted id the table holds), else unbound
+__global__ void __launch_bounds__(256) bind_component_kernel(const u32* __restrict__ arg, u32 n, const QuotedTab qt, u32 comp, const u32* __restrict__ old,
+                                                             u32* __restrict__ out, unsigned long long* n_unbound) {
+    const u32* __restrict__ tab = comp == 0u ? qt.s : comp == 1u ? qt.p : qt.o;
+    const u32 stride = gridDim.x * blockDim.x;
+    const u32 end = (n + 31u) & ~31u;  // whole warps for the ballot
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < end; i += stride) {
+        u32 v = EMPTY32;
+        if (i < n) {
+            const u32 id = arg[i], x = id & 0x7FFFFFFFu;
+            if ((id & 0x80000000u) && x < qt.n) v = __ldg(tab + x);  // a hole holds EMPTY32; KB_ID_NONE has x = 2^31-1 >= qt.n
+            if (v == EMPTY32 && old) v = old[i];
+            out[i] = v;
+        }
+        bind_count_unbound(i < n && v == EMPTY32, n_unbound);
+    }
+}
+
+// isTRIPLE, pass 1: first[0] = min row whose argument is a quoted id, first[1] = min row whose argument is bound and not quoted
+// (first[] = EMPTY32 beforehand)
+__global__ void __launch_bounds__(256) bind_istriple_first_kernel(const u32* __restrict__ arg, u32 n, u32* first) {
+    const u32 stride = gridDim.x * blockDim.x;
+    const u32 end = (n + 31u) & ~31u;
+    u32 ft = EMPTY32, ff = EMPTY32;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < end; i += stride) {
+        if (i < n) {
+            const u32 id = arg[i];
+            if (id != EMPTY32) {
+                if (id & 0x80000000u) ft = min(ft, i);
+                else ff = min(ff, i);
+            }
+        }
+    }
+    ft = __reduce_min_sync(0xffffffffu, ft);
+    ff = __reduce_min_sync(0xffffffffu, ff);
+    if ((threadIdx.x & 31) == 0) {
+        if (ft != EMPTY32) atomicMin(first, ft);
+        if (ff != EMPTY32) atomicMin(first + 1, ff);
+    }
+}
+// isTRIPLE, pass 2: out[i] = id_true / id_false, unbound where the argument is
+__global__ void __launch_bounds__(256) bind_istriple_write_kernel(const u32* __restrict__ arg, u32 n, u32 id_true, u32 id_false, const u32* __restrict__ old,
+                                                                  u32* __restrict__ out, unsigned long long* n_unbound) {
+    const u32 stride = gridDim.x * blockDim.x;
+    const u32 end = (n + 31u) & ~31u;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < end; i += stride) {
+        u32 v = EMPTY32;
+        if (i < n) {
+            const u32 id = arg[i];
+            v = id == EMPTY32 ? (old ? old[i] : EMPTY32) : (id & 0x80000000u) ? id_true : id_false;
+            out[i] = v;
+        }
+        bind_count_unbound(i < n && v == EMPTY32, n_unbound);
+    }
+}
+
+// CONCAT: the pieces of row i are, per argument a, the dictionary string of col[a][i] ("" when the dictionary does not hold it) or the
+// constant cbytes[coff[a] .. coff[a] + clen[a])
+struct BindConcatParams {
+    u32 n, n_args;
+    const u32* col[KB_BIND_MAX_ARGS];  // null: a constant
+    u64 coff[KB_BIND_MAX_ARGS];
+    u32 clen[KB_BIND_MAX_ARGS];
+    const unsigned char* cbytes;
+    DictTab dict;
+    u32* len;                          // lengths pass: [n + 1] (len[n] untouched); then their exclusive prefix
+    unsigned long long* total;         // lengths pass: += bytes of all rows
+    u64* off64;                        // gather pass: [n + 1] the prefix widened (the encode's offsets)
+    unsigned char* out;
+};
+__device__ __forceinline__ void concat_piece(const BindConcatParams& P, u32 a, u32 i, const unsigned char** src, u32* len) {
+    if (P.col[a]) {
+        const u32 id = P.col[a][i];
+        if (id < P.dict.ids) {  // Dictionary::decode: quoted ids (>= 2^31 > dict.ids), missing ids and KB_ID_NONE contribute ""
+            const unsigned long long b = __ldg(P.dict.off + id);
+            *src = P.dict.bytes + b;
+            *len = (u32)(__ldg(P.dict.off + id + 1) - b);
+        } else {
+            *src = nullptr;
+            *len = 0u;
+        }
+    } else {
+        *src = P.cbytes + P.coff[a];
+        *len = P.clen[a];
+    }
+}
+__global__ void __launch_bounds__(256) bind_concat_lengths_kernel(const __grid_constant__ BindConcatParams P) {
+    unsigned long long t = 0;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < P.n; i += gridDim.x * blockDim.x) {
+        unsigned long long l = 0;
+        for (u32 a = 0; a < P.n_args; a++) {
+            const unsigned char* src;
+            u32 k;
+            concat_piece(P, a, i, &src, &k);
+            l += k;
+        }
+        P.len[i] = l > 0xFFFFFFFFull ? 0xFFFFFFFFu : (u32)l;  // (the total then exceeds the limit: the caller refuses the call)
+        t += l;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+    if ((threadIdx.x & 31) == 0 && t) atomicAdd(P.total, t);
+}
+// one warp per 32 rows: the lanes copy each piece of a row together (decode_gather's access pattern)
+__global__ void __launch_bounds__(256) bind_concat_gather_kernel(const __grid_constant__ BindConcatParams P) {
+    const int lane = threadIdx.x & 31;
+    const u32 warps = (gridDim.x * blockDim.x) >> 5;
+    const u32 n_chunks = (P.n + 31u) >> 5;
+    for (u32 chunk = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; chunk < n_chunks; chunk += warps) {
+        const u32 i = chunk * 32u + (u32)lane;
+        u32 dst = 0;
+        if (i < P.n) {
+            dst = P.len[i];
+            P.off64[i] = dst;
+            if (i + 1u == P.n) P.off64[P.n] = P.len[P.n];
+        }
+        const u32 rows = min(32u, P.n - chunk * 32u);
+        for (u32 r = 0; r < rows; r++) {  // the warp writes row r of its chunk, piece by piece: consecutive lanes, consecutive bytes
+            const u32 row = chunk * 32u + r;
+            u32 w = __shfl_sync(0xffffffffu, dst, (int)r);
+            for (u32 a = 0; a < P.n_args; a++) {
+                const unsigned char* src;
+                u32 k;
+                concat_piece(P, a, row, &src, &k);  // (the same address in every lane: one broadcast load)
+                for (u32 b = (u32)lane; b < k; b += 32u) P.out[w + b] = __ldg(src + b);
+                w += k;
+            }
+        }
+    }
+}
+
+}  // namespace kb
+
 using namespace kb;
 
 namespace {
-
-// the reverse index holds every entry of the table and stays below load 1/2 with `extra` more entries (rebuilt larger otherwise)
-kb_status quoted_rev_ensure(kb_ctx* ctx, u64 extra) {
-    const u64 need = ((u64)ctx->quoted_slots + extra) * 2 + 64;
-    if (!ctx->quoted_rev || ctx->quoted_rev_slots < need) {
-        u64 slots = 1024;
-        while (slots < need + need / 2) slots <<= 1;  // headroom: the next batches insert in place
-        ctx->quoted_rev.reset();
-        KB_TRY(alloc_buf(ctx, slots * sizeof(u64), &ctx->quoted_rev));
-        KB_CUDA(ctx, cudaMemsetAsync(ctx->quoted_rev->p, 0xFF, slots * sizeof(u64), ctx->st));
-        ctx->quoted_rev_slots = slots;
-        ctx->quoted_rev_indexed = 0;
-    }
-    if (ctx->quoted_rev_indexed < ctx->quoted_slots) {
-        const u32 c = ctrl_alloc(ctx, 1);
-        KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + c, 0, sizeof(u32), ctx->st));
-        const u32 n = ctx->quoted_slots - ctx->quoted_rev_indexed;
-        timer_begin(ctx, F_OTHER);
-        launch_quoted_rev_insert(quotedtab(ctx), ctx->quoted_rev_indexed, n, static_cast<u64*>(ctx->quoted_rev->p), ctx->quoted_rev_slots - 1, ctx->ctrl + c,
-                                 ctx->n_sms, ctx->st);
-        timer_end(ctx);
-        ctx->stats.kernel_launches++;
-        KB_CUDA(ctx, cudaGetLastError());
-        KB_TRY(ctrl_read(ctx));
-        if (ctx->h_ctrl[c]) return fail(ctx, KB_E_LIMIT, "quoted-triple reverse index overflow");
-        ctx->quoted_rev_indexed = ctx->quoted_slots;
-    }
-    return KB_OK;
-}
-
-// the table's buffers hold at least `slots` entries; new slots are EMPTY32. The buffers keep alloc_buf's padding past their capacity,
-// which the match kernel's rounded-up TMA reads of the last tile rely on.
-kb_status quoted_grow(kb_ctx* ctx, u32 slots) {
-    if (slots <= ctx->quoted_cap) return KB_OK;
-    const u32 cap = (u32)std::min<u64>(KB_QUOTED_MAX_SLOTS, std::max<u64>((u64)slots + slots / 2, 1024));
-    Buf* cols[3] = {&ctx->quoted_s, &ctx->quoted_p, &ctx->quoted_o};
-    Buf nb[3];
-    for (int k = 0; k < 3; k++) {
-        KB_TRY(alloc_buf(ctx, (size_t)cap * sizeof(u32), &nb[k]));
-        launch_fill_u32(static_cast<u32*>(nb[k]->p), EMPTY32, cap, ctx->st);
-        if (ctx->quoted_slots)
-            KB_CUDA(ctx, cudaMemcpyAsync(nb[k]->p, (*cols[k])->p, (size_t)ctx->quoted_slots * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
-    }
-    ctx->stats.kernel_launches += 3;
-    KB_CUDA(ctx, cudaGetLastError());
-    for (int k = 0; k < 3; k++) *cols[k] = nb[k];
-    ctx->quoted_cap = cap;
-    return KB_OK;
-}
-
-kb_status bind_triple(kb_ctx* ctx, const u32* const* col, const u32* cval, u32 n, u32 next_qt_id, const u32* old, u32* out, unsigned long long* n_unbound,
-                      kb_bind_info* info) {
-    KB_TRY(quoted_rev_ensure(ctx, n));
-    u64 bslots = 1024;
-    while (bslots < 2ull * n) bslots <<= 1;
-    Buf batch, hit, slot_of, first, scratch;
-    KB_TRY(alloc_buf(ctx, bslots * sizeof(u64), &batch));
-    KB_TRY(alloc_buf(ctx, (size_t)n * sizeof(u32), &hit));
-    KB_TRY(alloc_buf(ctx, (size_t)n * sizeof(u32), &slot_of));
-    KB_TRY(alloc_buf(ctx, ((size_t)n + 1) * sizeof(u32), &first));
-    KB_TRY(alloc_buf(ctx, (((size_t)n + 1) / 2048 + 4) * sizeof(u32), &scratch));
-    KB_CUDA(ctx, cudaMemsetAsync(batch->p, 0xFF, bslots * sizeof(u64), ctx->st));
-    KB_CUDA(ctx, cudaMemsetAsync(static_cast<u32*>(first->p) + n, 0, sizeof(u32), ctx->st));
-    BindTripleParams P{};
-    for (int k = 0; k < 3; k++) { P.col[k] = col[k]; P.cval[k] = cval[k]; }
-    P.n = n;
-    P.qt = quotedtab(ctx);
-    P.rev = static_cast<const u64*>(ctx->quoted_rev->p);
-    P.rev_mask = ctx->quoted_rev_slots - 1;
-    P.batch = static_cast<u64*>(batch->p);
-    P.batch_mask = bslots - 1;
-    P.hit = static_cast<u32*>(hit->p);
-    P.slot_of = static_cast<u32*>(slot_of->p);
-    P.first = static_cast<u32*>(first->p);
-    const u32 c = ctrl_alloc(ctx, 2);  // [0] overflow, [1] new triples (first[n] after the scan)
-    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + c, 0, 2 * sizeof(u32), ctx->st));
-    P.overflow = ctx->ctrl + c;
-    timer_begin(ctx, F_OTHER, 3);
-    launch_bind_triple_resolve(P, ctx->n_sms, ctx->st);
-    launch_bind_triple_mark(P, ctx->n_sms, ctx->st);
-    launch_exclusive_scan_u32(P.first, n + 1, static_cast<u32*>(scratch->p), ctx->st);
-    timer_end(ctx);
-    ctx->stats.kernel_launches += 3;
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->ctrl + c + 1, P.first + n, sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
-    KB_CUDA(ctx, cudaGetLastError());
-    KB_TRY(ctrl_read(ctx));
-    if (ctx->h_ctrl[c]) return fail(ctx, KB_E_LIMIT, "TRIPLE batch table overflow");
-    const u32 n_new = ctx->h_ctrl[c + 1];
-    const u32 base = next_qt_id & 0x7FFFFFFFu;
-    if (n_new && (u64)base + n_new > KB_QUOTED_MAX_SLOTS)
-        return fail(ctx, KB_E_LIMIT, "TRIPLE: %u new quoted triples from id 0x%08x would pass the table's %u slots", n_new, next_qt_id, KB_QUOTED_MAX_SLOTS);
-    // nothing has changed so far (the reverse index is a cache of the table); from here on the table grows
-    if (n_new) KB_TRY(quoted_grow(ctx, base + n_new));
-    P.next_qt_id = next_qt_id;
-    P.ws = n_new ? static_cast<u32*>(ctx->quoted_s->p) : nullptr;
-    P.wp = n_new ? static_cast<u32*>(ctx->quoted_p->p) : nullptr;
-    P.wo = n_new ? static_cast<u32*>(ctx->quoted_o->p) : nullptr;
-    P.old = old;
-    P.out = out;
-    P.n_unbound = n_unbound;
-    timer_begin(ctx, F_OTHER);
-    launch_bind_triple_assign(P, ctx->n_sms, ctx->st);
-    timer_end(ctx);
-    ctx->stats.kernel_launches++;
-    KB_CUDA(ctx, cudaGetLastError());
-    if (n_new) {
-        ctx->quoted_slots = base + n_new;
-        KB_TRY(quoted_rev_ensure(ctx, 0));  // the new entries enter the reverse index
-    }
-    info->quoted_first = n_new ? next_qt_id : 0;
-    info->quoted_new = n_new;
-    return KB_OK;
-}
 
 kb_status bind_is_triple(kb_ctx* ctx, const u32* arg, u32 n, const u32* old, u32* out, unsigned long long* n_unbound, kb_bind_info* info) {
     const u32 c = ctrl_alloc(ctx, 2);  // first row needing "true", first row needing "false"
     KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + c, 0xFF, 2 * sizeof(u32), ctx->st));
     timer_begin(ctx, F_OTHER);
-    launch_bind_istriple_first(arg, n, ctx->ctrl + c, ctx->n_sms, ctx->st);
+    bind_istriple_first_kernel<<<grid_1d(n, ctx->n_sms), 256, 0, ctx->st>>>(arg, n, ctx->ctrl + c);
     timer_end(ctx);
-    ctx->stats.kernel_launches++;
     KB_CUDA(ctx, cudaGetLastError());
     KB_TRY(ctrl_read(ctx));
     // the strings the rows need, in the order of the first row needing each (the reference encodes inside its row loop)
@@ -165,9 +187,8 @@ kb_status bind_is_triple(kb_ctx* ctx, const u32* arg, u32 n, const u32* old, u32
     u32 id_true = EMPTY32, id_false = EMPTY32;
     for (size_t k = 0; k < need.size(); k++) (need[k].second[0] == 't' ? id_true : id_false) = ids[k];
     timer_begin(ctx, F_OTHER);
-    launch_bind_istriple_write(arg, n, id_true, id_false, old, out, n_unbound, ctx->n_sms, ctx->st);
+    bind_istriple_write_kernel<<<grid_1d(n, ctx->n_sms), 256, 0, ctx->st>>>(arg, n, id_true, id_false, old, out, n_unbound);
     timer_end(ctx);
-    ctx->stats.kernel_launches++;
     KB_CUDA(ctx, cudaGetLastError());
     return KB_OK;
 }
@@ -192,9 +213,7 @@ kb_status bind_concat(kb_ctx* ctx, const kb_bind_spec& spec, const u32* const* c
             P.clen[a] = (u32)(spec.const_offsets[k + 1] - spec.const_offsets[k]);
         }
     }
-    P.dict_off = ctx->dict_ids ? static_cast<const unsigned long long*>(ctx->dict_off->p) : nullptr;
-    P.dict_bytes = ctx->dict_ids ? static_cast<const unsigned char*>(ctx->dict_bytes->p) : nullptr;
-    P.dict_ids = ctx->dict_ids;
+    P.dict = dicttab(ctx);
     KB_TRY(alloc_buf(ctx, ((size_t)n + 1) * sizeof(u32), &len));
     KB_TRY(alloc_buf(ctx, (((size_t)n + 1) / 2048 + 4) * sizeof(u32), &scratch));
     P.len = static_cast<u32*>(len->p);
@@ -202,11 +221,10 @@ kb_status bind_concat(kb_ctx* ctx, const kb_bind_spec& spec, const u32* const* c
     P.total = reinterpret_cast<unsigned long long*>(ctx->ctrl + c);
     KB_CUDA(ctx, cudaMemsetAsync(P.total, 0, sizeof(unsigned long long), ctx->st));
     KB_CUDA(ctx, cudaMemsetAsync(P.len + n, 0, sizeof(u32), ctx->st));
-    timer_begin(ctx, F_OTHER, 2);
-    launch_bind_concat_lengths(P, ctx->n_sms, ctx->st);
+    timer_begin(ctx, F_OTHER, 4);
+    bind_concat_lengths_kernel<<<grid_1d(n, ctx->n_sms), 256, 0, ctx->st>>>(P);
     launch_exclusive_scan_u32(P.len, n + 1, static_cast<u32*>(scratch->p), ctx->st);
     timer_end(ctx);
-    ctx->stats.kernel_launches += 2;
     KB_CUDA(ctx, cudaGetLastError());
     KB_TRY(ctrl_read(ctx));
     unsigned long long total = 0;
@@ -218,9 +236,8 @@ kb_status bind_concat(kb_ctx* ctx, const kb_bind_spec& spec, const u32* const* c
     P.off64 = static_cast<u64*>(off64->p);
     P.out = static_cast<unsigned char*>(bytes->p);
     timer_begin(ctx, F_OTHER);
-    launch_bind_concat_gather(P, ctx->n_sms, ctx->st);
+    bind_concat_gather_kernel<<<grid_1d(n, ctx->n_sms), 256, 0, ctx->st>>>(P);
     timer_end(ctx);
-    ctx->stats.kernel_launches++;
     KB_CUDA(ctx, cudaGetLastError());
     info->dict_first = ctx->dict_ids;
     u32 n_new = 0;
@@ -289,13 +306,12 @@ kb_status kb_bind(kb_ctx* ctx, const kb_rel* in, const kb_bind_spec* spec, kb_re
         case KB_BIND_PREDICATE:
         case KB_BIND_OBJECT:
             timer_begin(ctx, F_OTHER);
-            launch_bind_component(col[0], n, quotedtab(ctx), fn - KB_BIND_SUBJECT, old, res.ptr, n_unbound, ctx->n_sms, ctx->st);
+            bind_component_kernel<<<grid_1d(n, ctx->n_sms), 256, 0, ctx->st>>>(col[0], n, quotedtab(ctx), fn - KB_BIND_SUBJECT, old, res.ptr, n_unbound);
             timer_end(ctx);
-            ctx->stats.kernel_launches++;
             KB_CUDA(ctx, cudaGetLastError());
             break;
         case KB_BIND_IS_TRIPLE: KB_TRY(bind_is_triple(ctx, col[0], n, old, res.ptr, n_unbound, &inf)); break;
-        case KB_BIND_TRIPLE: KB_TRY(bind_triple(ctx, col, cval, n, spec->next_qt_id, old, res.ptr, n_unbound, &inf)); break;
+        case KB_BIND_TRIPLE: KB_TRY(quoted_encode(ctx, col, cval, n, spec->next_qt_id, old, res.ptr, n_unbound, &inf)); break;
         default: KB_TRY(bind_concat(ctx, *spec, col, n, res.ptr, &inf)); break;
         }
         KB_TRY(ctrl_read(ctx));
@@ -310,43 +326,6 @@ kb_status kb_bind(kb_ctx* ctx, const kb_rel* in, const kb_bind_spec* spec, kb_re
     ctx->stats.rows_out = r->n;
     if (info) *info = inf;
     *out = r.release();
-    return KB_OK;
-}
-
-kb_status kb_quoted_download(kb_ctx* ctx, uint32_t first_id, uint32_t n, uint32_t* s, uint32_t* p, uint32_t* o) {
-    KB_ENTER(ctx);
-    if (n == 0) return KB_OK;
-    if (!s || !p || !o) return fail(ctx, KB_E_INVALID, "NULL argument");
-    if (!(first_id & 0x80000000u)) return fail(ctx, KB_E_INVALID, "0x%08x is not a quoted-triple id", first_id);
-    const u64 x = first_id & 0x7FFFFFFFu;
-    if (x + n > 0x7FFFFFFFull) return fail(ctx, KB_E_INVALID, "id range past 0xFFFFFFFE");
-    const u64 held = x < ctx->quoted_slots ? std::min<u64>(n, ctx->quoted_slots - x) : 0;
-    uint32_t* dst[3] = {s, p, o};
-    const Buf* src[3] = {&ctx->quoted_s, &ctx->quoted_p, &ctx->quoted_o};
-    for (int k = 0; k < 3; k++) {
-        if (held) KB_CUDA(ctx, cudaMemcpyAsync(dst[k], static_cast<const u32*>((*src[k])->p) + x, held * sizeof(u32), cudaMemcpyDeviceToHost, ctx->st));
-        std::fill(dst[k] + held, dst[k] + n, KB_ID_NONE);
-    }
-    KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
-    ctx->stats.d2h_bytes += held * 12u;
-    return KB_OK;
-}
-
-kb_status kb_dict_strings_download(kb_ctx* ctx, uint32_t first, uint32_t n, uint64_t* offsets, uint8_t* bytes) {
-    KB_ENTER(ctx);
-    if (!offsets) return fail(ctx, KB_E_INVALID, "NULL offsets");
-    if ((u64)first + n > ctx->dict_ids) return fail(ctx, KB_E_INVALID, "ids [%u, %llu) past the %u the device dictionary holds", first, (unsigned long long)first + n, ctx->dict_ids);
-    offsets[0] = 0;
-    if (n == 0) return KB_OK;
-    KB_CUDA(ctx, cudaMemcpyAsync(offsets, static_cast<const unsigned long long*>(ctx->dict_off->p) + first, ((size_t)n + 1) * sizeof(u64), cudaMemcpyDeviceToHost, ctx->st));
-    KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
-    const u64 base = offsets[0];
-    for (u32 k = 0; k <= n; k++) offsets[k] -= base;
-    if (bytes && offsets[n]) {
-        KB_CUDA(ctx, cudaMemcpyAsync(bytes, static_cast<const unsigned char*>(ctx->dict_bytes->p) + base, (size_t)offsets[n], cudaMemcpyDeviceToHost, ctx->st));
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
-    }
-    ctx->stats.d2h_bytes += ((size_t)n + 1) * sizeof(u64) + (bytes ? offsets[n] : 0);
     return KB_OK;
 }
 

@@ -18,6 +18,17 @@ constexpr u32 EMPTY32 = 0xFFFFFFFFu;  // == KB_ID_NONE: reserved id, never a dic
 constexpr u64 EMPTY64 = ~0ull;
 constexpr int MAXP = KB_MAX_PATTERNS;
 
+// the grid of a persistent tile kernel: as many CTAs as are resident on every SM at once, at most one per tile
+static inline int grid_for(const void* kernel, int threads, size_t smem, int n_sms, u32 n_tiles) {
+    int per_sm = 1;
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem);
+    if (per_sm < 1) per_sm = 1;
+    long long g = (long long)per_sm * n_sms;  // persistent: a whole number of resident CTAs per SM, on every SM
+    if (g > (long long)n_tiles) g = n_tiles;
+    if (g < 1) g = 1;
+    return (int)g;
+}
+
 __host__ __device__ __forceinline__ u32 mix32(u32 x) {  // murmur3 finaliser; also the shard function (kb_shard_of)
     x ^= x >> 16; x *= 0x85ebca6bu; x ^= x >> 13; x *= 0xc2b2ae35u; x ^= x >> 16;
     return x;

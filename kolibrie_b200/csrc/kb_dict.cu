@@ -13,8 +13,10 @@
 //   K4 dict_assign_kernel      ids of the new terms = base + rank[first position]; first_pos[rank] = i; offsets of the new strings
 //   K5 dict_append_kernel      the new strings' bytes appended to the device dictionary (warp per string)
 //   K6 dict_index_insert_kernel  the new ids enter the persistent index (rebuilt larger beyond load 1/2)
+// Both tables are tag-indexed (kb_tagtab.cuh). This file owns the device dictionary: its loads, its growth, the decode of ids into text
+// (decode_ids: kb_rel_decode, string ORDER BY keys, the serializers) and its downloads.
 #include "kb_internal.hpp"
-#include "kb_kernels.cuh"
+#include "kb_tagtab.cuh"
 
 #include <cstring>
 
@@ -32,9 +34,7 @@ __device__ __forceinline__ bool bytes_equal(const unsigned char* __restrict__ a,
     for (u64 i = 0; i < len; i++) if (__ldg(a + i) != __ldg(b + i)) return false;
     return true;
 }
-constexpr u64 DEMPTY = 0xFFFFFFFFFFFFFFFFull;
-// an entry = (hash tag in the high 32 bits, payload in the low 32): payload = id (persistent index) or position in the batch (batch table)
-__device__ __forceinline__ u64 dentry(u64 h, u32 payload) { return (h & 0xFFFFFFFF00000000ull) | payload; }
+// the payload of an entry: the id (persistent index) or a position in the batch (batch table)
 
 __global__ void __launch_bounds__(256) dict_hash_kernel(const u64* __restrict__ off, const unsigned char* __restrict__ bytes, u32 n, u64* __restrict__ hash) {
     for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -47,8 +47,8 @@ struct DictResolveParams {
     const u64* off; const unsigned char* bytes; u32 n;           // the batch
     const u64* hash;
     const u64* index; u64 index_mask;                             // persistent index (null: empty dictionary)
-    const unsigned long long* dict_off; const unsigned char* dict_bytes; u32 dict_ids;
-    u64* batch; u64 batch_mask;                                   // batch table, all DEMPTY
+    DictTab dict;
+    u64* batch; u64 batch_mask;                                   // batch table, all empty
     u32* out_id;                                                  // id, or EMPTY32 for a term that is new
     u32* slot_of;                                                 // slot of the term's string in the batch table (new terms)
     u32* overflow;
@@ -59,36 +59,19 @@ __global__ void __launch_bounds__(256) dict_resolve_kernel(const __grid_constant
         const unsigned char* s = P.bytes + a;
         const u64 h = P.hash[i];
         u32 id = EMPTY32;
-        if (P.index) {
-            for (u64 slot = h & P.index_mask, probes = 0; probes <= P.index_mask; probes++, slot = (slot + 1) & P.index_mask) {
-                const u64 e = P.index[slot];
-                if (e == DEMPTY) break;
-                if ((e >> 32) != (h >> 32)) continue;
-                const u32 cand = (u32)e;
-                const unsigned long long ca = P.dict_off[cand];
-                if (P.dict_off[cand + 1] - ca == len && bytes_equal(P.dict_bytes + ca, s, len)) { id = cand; break; }
-            }
-        }
+        if (P.index)
+            id = tag_find(P.index, P.index_mask, h, [&](u32 cand) {
+                const unsigned long long ca = P.dict.off[cand];
+                return P.dict.off[cand + 1] - ca == len && bytes_equal(P.dict.bytes + ca, s, len);
+            });
         P.out_id[i] = id;
         if (id != EMPTY32) continue;
-        bool placed = false;
-        for (u64 slot = h & P.batch_mask, probes = 0; probes <= P.batch_mask; probes++, slot = (slot + 1) & P.batch_mask) {
-            u64 e = *reinterpret_cast<volatile u64*>(&P.batch[slot]);
-            if (e == DEMPTY) {
-                e = atomicCAS(reinterpret_cast<unsigned long long*>(&P.batch[slot]), DEMPTY, dentry(h, i));
-                if (e == DEMPTY) { P.slot_of[i] = (u32)slot; placed = true; break; }
-            }
-            if ((e >> 32) != (h >> 32)) continue;
-            const u32 rep = (u32)e;  // some position of the slot's string (it may be lowered concurrently: always the same string)
-            const u64 ra = P.off[rep];
-            if (P.off[rep + 1] - ra == len && bytes_equal(P.bytes + ra, s, len)) {
-                atomicMin(reinterpret_cast<unsigned long long*>(&P.batch[slot]), dentry(h, i));  // same tag: the minimum is over the position
-                P.slot_of[i] = (u32)slot;
-                placed = true;
-                break;
-            }
-        }
-        if (!placed) *P.overflow = 1u;
+        // `rep`: some position of the slot's string (it may be lowered concurrently: always the same string)
+        if (!tag_claim_min(P.batch, P.batch_mask, h, i, [&](u32 rep) {
+                const u64 ra = P.off[rep];
+                return P.off[rep + 1] - ra == len && bytes_equal(P.bytes + ra, s, len);
+            }, &P.slot_of[i]))
+            *P.overflow = 1u;
     }
 }
 
@@ -136,61 +119,161 @@ __global__ void __launch_bounds__(256) dict_append_kernel(const u64* __restrict_
 }
 
 // ids [first, first + n) of the device dictionary enter the persistent index
-__global__ void __launch_bounds__(256) dict_index_insert_kernel(const unsigned long long* __restrict__ dict_off, const unsigned char* __restrict__ dict_bytes, u32 first, u32 n,
-                                                                u64* __restrict__ index, u64 mask, u32* overflow) {
+__global__ void __launch_bounds__(256) dict_index_insert_kernel(const DictTab dict, u32 first, u32 n, u64* __restrict__ index, u64 mask, u32* overflow) {
     for (u32 k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
         const u32 id = first + k;
-        const unsigned long long a = dict_off[id];
-        const u64 h = fnv1a64(dict_bytes + a, dict_off[id + 1] - a);
-        bool placed = false;
-        for (u64 slot = h & mask, probes = 0; probes <= mask; probes++, slot = (slot + 1) & mask) {
-            if (*reinterpret_cast<volatile u64*>(&index[slot]) != DEMPTY) continue;  // ids are distinct strings: nothing to compare
-            if (atomicCAS(reinterpret_cast<unsigned long long*>(&index[slot]), DEMPTY, dentry(h, id)) == DEMPTY) { placed = true; break; }
+        const unsigned long long a = dict.off[id];
+        u32 slot;  // ids are distinct strings: nothing to compare
+        if (!tag_claim_min(index, mask, fnv1a64(dict.bytes + a, dict.off[id + 1] - a), id, [](u32) { return false; }, &slot)) *overflow = 1u;
+    }
+}
+
+enum { QW_OK = 0, QW_UNKNOWN = 1, QW_DEEP = 2 };
+// Dictionary::decode_term of a quoted id (dictionary.rs:60-72) as an explicit depth-first walk: lit(text, bytes) for "<< ", " ", " >>",
+// word(id) for every dictionary component, in output order. Like the reference's `?`, the walk stops at the first id that neither table
+// holds (QW_UNKNOWN: the whole term is "unknown"); entering a level past KB_QUOTED_MAX_DEPTH gives QW_DEEP. The stack holds one table
+// index per level and a 2-bit component cursor per level.
+template <class Lit, class Word>
+__device__ u32 quoted_walk(u32 id, u32 dict_ids, const QuotedTab& qt, Lit lit, Word word) {
+    u32 ent[KB_QUOTED_MAX_DEPTH];
+    u32 next = 0;  // bits 2d..2d+1: components of level d already emitted
+    int d = 0;
+    u32 cur = id;
+    for (;;) {
+        const u32 x = cur & 0x7FFFFFFFu;
+        if (x >= qt.n || __ldg(qt.p + x) == EMPTY32) return QW_UNKNOWN;
+        if (d == KB_QUOTED_MAX_DEPTH) return QW_DEEP;
+        ent[d] = x;
+        next &= ~(3u << (2 * d));
+        d++;
+        lit("<< ", 3u);
+        for (;;) {
+            const int top = d - 1;
+            const u32 k = (next >> (2 * top)) & 3u;
+            if (k == 3u) {
+                lit(" >>", 3u);
+                if (--d == 0) return QW_OK;
+                continue;
+            }
+            next += 1u << (2 * top);
+            if (k) lit(" ", 1u);
+            const u32 e = ent[top];
+            const u32 c = __ldg((k == 0u ? qt.s : k == 1u ? qt.p : qt.o) + e);
+            if (c & 0x80000000u) { cur = c; break; }
+            if (c >= dict_ids) return QW_UNKNOWN;
+            word(c);
         }
-        if (!placed) *overflow = 1u;
     }
 }
 
-static int grid_1d(u64 n, int n_sms, int per_sm = 8) {
-    const u64 want = (n + 255) / 256;
-    const u64 cap = (u64)n_sms * per_sm;
-    return (int)std::max<u64>(1, std::min(want, cap));
+// decode_lengths_kernel: len[i] = length of the string of ids[i] ("unknown" = 7 bytes when the dictionary does not hold the id). A quoted id: without a table
+// *quoted = 1; with one, the length of `<< s p o >>` walked with a bounded stack (dictionary.rs:60-72), "unknown" when any id on the walk
+// is held by neither table, and *deep = 1 when the walk goes past KB_QUOTED_MAX_DEPTH levels first. *total += sum.
+// missing_len: 7, or 0 when a term the tables do not hold renders as "" instead of "unknown" (decode_any(..).unwrap_or_default(), the serializers'
+// rule, sparql_database.rs:301-322).
+__global__ void __launch_bounds__(256) decode_lengths_kernel(const u32* __restrict__ ids, u32 n, const DictTab dict, const QuotedTab qt, u32* __restrict__ len, unsigned long long* total, u32* quoted, u32* deep,
+                                                             u32 missing_len) {
+    const u32 stride = gridDim.x * blockDim.x;
+    unsigned long long t = 0;
+    bool q = false, dp = false;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        const u32 id = ids[i];
+        unsigned long long l = missing_len;  // "unknown" or ""
+        if (id & 0x80000000u) {
+            if (qt.n == 0u) {
+                q = true;
+            } else {
+                unsigned long long acc = 0;
+                const u32 r = quoted_walk(id, dict.ids, qt, [&](const char*, u32 k) { acc += k; },
+                                          [&](u32 c) { acc += __ldg(dict.off + c + 1) - __ldg(dict.off + c); });
+                dp = dp || r == QW_DEEP;
+                if (r == QW_OK) l = acc;
+            }
+        } else if (id < dict.ids) {
+            l = __ldg(dict.off + id + 1) - __ldg(dict.off + id);
+        }
+        len[i] = l > 0xFFFFFFFFull ? 0xFFFFFFFFu : (u32)l;  // (the total then exceeds 2^32-1: the caller refuses the column)
+        t += l;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+    if ((threadIdx.x & 31) == 0 && t) atomicAdd(total, t);
+    if (q) *quoted = 1u;
+    if (dp) *deep = 1u;
+}
+// out[off[i] .. off[i+1]) = bytes of the string of ids[i]; one warp per 32 rows, the lanes copy each dictionary string together; a quoted
+// row is written by its own thread, walking the term again (a missing term is 7 bytes, "unknown", or 0: either way shorter than the
+// 8 bytes of the shortest rendered quoted term)
+__global__ void __launch_bounds__(256) decode_gather_kernel(const u32* __restrict__ ids, u32 n, const DictTab dict, const QuotedTab qt,
+                                                            const u32* __restrict__ off, unsigned char* __restrict__ out) {
+    const int lane = threadIdx.x & 31;
+    const u32 warps = (gridDim.x * blockDim.x) >> 5;
+    const u32 n_chunks = (n + 31u) >> 5;
+    for (u32 chunk = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; chunk < n_chunks; chunk += warps) {
+        const u32 i = chunk * 32u + (u32)lane;
+        u32 id = 0, dst = 0, l = 0;
+        unsigned long long src = 0;
+        bool known = false, walk = false;
+        if (i < n) {
+            id = ids[i];
+            dst = off[i];
+            l = off[i + 1] - dst;
+            known = id < dict.ids;
+            if (known) src = __ldg(dict.off + id);
+            walk = (id & 0x80000000u) != 0u && l >= 8u;  // a rendered quoted term is at least 8 bytes: 7 is "unknown", 0 is ""
+        }
+        const u32 wl = walk ? 0u : l;
+        for (int r = 0; r < 32; r++) {  // the warp copies row r of its chunk: consecutive lanes, consecutive bytes
+            const u32 rl = __shfl_sync(0xffffffffu, wl, r);
+            if (rl == 0u) continue;
+            const u32 rdst = __shfl_sync(0xffffffffu, dst, r);
+            const unsigned long long rsrc = __shfl_sync(0xffffffffu, src, r);
+            const bool rknown = __shfl_sync(0xffffffffu, known ? 1 : 0, r) != 0;
+            for (u32 b = (u32)lane; b < rl; b += 32u) out[rdst + b] = rknown ? __ldg(dict.bytes + rsrc + b) : (unsigned char)"unknown"[b];
+        }
+        if (walk) {  // a quoted term: this thread writes it, walking it again
+            unsigned char* w = out + dst;
+            quoted_walk(id, dict.ids, qt, [&](const char* s, u32 k) { for (u32 b = 0; b < k; b++) *w++ = (unsigned char)s[b]; },
+                        [&](u32 c) {
+                            const unsigned long long a = __ldg(dict.off + c), e = __ldg(dict.off + c + 1);
+                            for (unsigned long long b = a; b < e; b++) *w++ = __ldg(dict.bytes + b);
+                        });
+        }
+    }
 }
 
-// (re)build the persistent index so that it holds every id and stays below load 1/2 with `extra` more
-static kb_status dict_index_ensure(kb_ctx* ctx, u64 extra) {
-    const u64 need = ((u64)ctx->dict_ids + extra) * 2 + 64;
-    if (ctx->dict_index && ctx->dict_index_slots >= need && ctx->dict_indexed == ctx->dict_ids) return KB_OK;
-    if (!ctx->dict_index || ctx->dict_index_slots < need) {
-        u64 slots = 1024;
-        while (slots < need + need / 2) slots <<= 1;  // headroom: the next batches extend it in place
-        ctx->dict_index.reset();
-        KB_TRY(alloc_buf(ctx, slots * sizeof(u64), &ctx->dict_index));
-        KB_CUDA(ctx, cudaMemsetAsync(ctx->dict_index->p, 0xFF, slots * sizeof(u64), ctx->st));
-        ctx->dict_index_slots = slots;
-        ctx->dict_indexed = 0;
+
+}  // namespace kb
+
+using namespace kb;
+
+DictTab kb::dicttab(const kb_ctx* ctx) {
+    DictTab t{};
+    if (ctx->dict_ids) {
+        t.off = static_cast<const unsigned long long*>(ctx->dict_off->p);
+        t.bytes = static_cast<const unsigned char*>(ctx->dict_bytes->p);
+        t.ids = ctx->dict_ids;
     }
-    if (ctx->dict_indexed < ctx->dict_ids) {
-        const u32 c = ctrl_alloc(ctx, 4);
-        KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + c, 0, 4 * sizeof(u32), ctx->st));
-        const u32 n = ctx->dict_ids - ctx->dict_indexed;
-        dict_index_insert_kernel<<<grid_1d(n, ctx->n_sms), 256, 0, ctx->st>>>(static_cast<const unsigned long long*>(ctx->dict_off->p),
-                                                                                static_cast<const unsigned char*>(ctx->dict_bytes->p), ctx->dict_indexed, n,
-                                                                                static_cast<u64*>(ctx->dict_index->p), ctx->dict_index_slots - 1, ctx->ctrl + c);
-        ctx->stats.kernel_launches++;
-        KB_CUDA(ctx, cudaGetLastError());
-        KB_TRY(ctrl_read(ctx));
-        if (ctx->h_ctrl[c]) return fail(ctx, KB_E_LIMIT, "dictionary index overflow");
-        ctx->dict_indexed = ctx->dict_ids;
-    }
-    return KB_OK;
+    return t;
 }
+
+namespace {
+
+// the persistent index holds every id and stays below load 1/2 with `extra` more
+kb_status dict_index_ensure(kb_ctx* ctx, u64 extra) {
+    const DictTab dict = dicttab(ctx);
+    return tag_index_ensure(ctx, &ctx->dict_index, ctx->dict_ids, extra, "dictionary index", [&](u32 first, u32 n, u64* tab, u64 mask, u32* overflow) {
+        dict_index_insert_kernel<<<grid_1d(n, ctx->n_sms), 256, 0, ctx->st>>>(dict, first, n, tab, mask, overflow);
+    });
+}
+
+}  // namespace
 
 // The body of kb_dict_encode over a batch already in device memory (kb_bind's CONCAT builds its concatenations there): term i =
 // d_bytes[d_off[i] .. d_off[i+1]), d_off[n] = total. The ids go to d_out_ids (device, n entries); *first_pos (nullable) receives a device
 // buffer whose entry k is the batch position of the term that introduced id (ids before the call) + k. Limits are checked before
 // anything changes.
-kb_status dict_encode_device(kb_ctx* ctx, const u64* d_off, const unsigned char* d_bytes, u64 n_terms, u64 total, u32* d_out_ids, u32* n_new_out,
+kb_status kb::dict_encode_device(kb_ctx* ctx, const u64* d_off, const unsigned char* d_bytes, u64 n_terms, u64 total, u32* d_out_ids, u32* n_new_out,
                              Buf* first_pos) {
     *n_new_out = 0;
     if (n_terms == 0) return KB_OK;
@@ -200,28 +283,24 @@ kb_status dict_encode_device(kb_ctx* ctx, const u64* d_off, const unsigned char*
     const u32 n = (u32)n_terms;
     Buf d_hash, d_batch, d_slot, d_first, d_flen, d_fpos, scratch;
     KB_TRY(dict_index_ensure(ctx, n));
-    u64 bslots = 1024;
-    while (bslots < 2ull * n) bslots <<= 1;
+    u64 bslots = 0;
     KB_TRY(alloc_buf(ctx, (size_t)n * sizeof(u64), &d_hash));
-    KB_TRY(alloc_buf(ctx, bslots * sizeof(u64), &d_batch));
+    KB_TRY(tag_batch_table(ctx, n, &d_batch, &bslots));
     KB_TRY(alloc_buf(ctx, (size_t)n * sizeof(u32), &d_slot));
     KB_TRY(alloc_buf(ctx, ((size_t)n + 1) * sizeof(u32), &d_first));
     KB_TRY(alloc_buf(ctx, ((size_t)n + 1) * sizeof(u32), &d_flen));
     KB_TRY(alloc_buf(ctx, (((size_t)n + 1) / 2048 + 4) * sizeof(u32), &scratch));
-    KB_CUDA(ctx, cudaMemsetAsync(d_batch->p, 0xFF, bslots * sizeof(u64), ctx->st));
     const u32 c = ctrl_alloc(ctx, 4);  // [0] overflow, [2..3] u64 bytes of the new strings
     KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + c, 0, 4 * sizeof(u32), ctx->st));
     const int grid = grid_1d(n, ctx->n_sms);
-    timer_begin(ctx, F_OTHER, 5);
+    timer_begin(ctx, F_OTHER, 9);
     dict_hash_kernel<<<grid, 256, 0, ctx->st>>>(d_off, d_bytes, n, static_cast<u64*>(d_hash->p));
     DictResolveParams P{};
     P.off = d_off; P.bytes = d_bytes; P.n = n;
     P.hash = static_cast<const u64*>(d_hash->p);
-    P.index = ctx->dict_ids ? static_cast<const u64*>(ctx->dict_index->p) : nullptr;
-    P.index_mask = ctx->dict_index_slots - 1;
-    P.dict_off = ctx->dict_ids ? static_cast<const unsigned long long*>(ctx->dict_off->p) : nullptr;
-    P.dict_bytes = ctx->dict_ids ? static_cast<const unsigned char*>(ctx->dict_bytes->p) : nullptr;
-    P.dict_ids = ctx->dict_ids;
+    P.index = ctx->dict_ids ? static_cast<const u64*>(ctx->dict_index.tab->p) : nullptr;
+    P.index_mask = ctx->dict_index.slots - 1;
+    P.dict = dicttab(ctx);
     P.batch = static_cast<u64*>(d_batch->p); P.batch_mask = bslots - 1;
     P.out_id = d_out_ids; P.slot_of = static_cast<u32*>(d_slot->p);
     P.overflow = ctx->ctrl + c;
@@ -233,7 +312,6 @@ kb_status dict_encode_device(kb_ctx* ctx, const u64* d_off, const unsigned char*
     launch_exclusive_scan_u32(static_cast<u32*>(d_first->p), n + 1, static_cast<u32*>(scratch->p), ctx->st);
     launch_exclusive_scan_u32(static_cast<u32*>(d_flen->p), n + 1, static_cast<u32*>(scratch->p), ctx->st);
     timer_end(ctx);
-    ctx->stats.kernel_launches += 3;
     // the number of new strings (= first[n] after the scan) and their bytes
     const u32 c2 = ctrl_alloc(ctx, 4);
     KB_CUDA(ctx, cudaMemcpyAsync(ctx->ctrl + c2, static_cast<u32*>(d_first->p) + n, sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
@@ -268,18 +346,16 @@ kb_status dict_encode_device(kb_ctx* ctx, const u64* d_off, const unsigned char*
             ctx->dict_bytes = nbytes;
         }
     }
-    timer_begin(ctx, F_OTHER, 2);
+    timer_begin(ctx, F_OTHER, n_new ? 2 : 1);
     dict_assign_kernel<<<grid, 256, 0, ctx->st>>>(P.off, n, base_id, base_bytes, P.out_id, P.slot_of, P.batch, static_cast<const u32*>(d_first->p),
                                                   static_cast<const u32*>(d_flen->p), static_cast<u64*>(d_fpos->p),
                                                   n_new ? static_cast<unsigned long long*>(ctx->dict_off->p) + base_id : nullptr);
-    ctx->stats.kernel_launches++;
     if (n_new) {
         const unsigned long long end = base_bytes + new_bytes;
         KB_CUDA(ctx, cudaMemcpyAsync(static_cast<unsigned long long*>(ctx->dict_off->p) + ids_after, &end, sizeof end, cudaMemcpyHostToDevice, ctx->st));
         dict_append_kernel<<<grid_1d((u64)n_new * 32, ctx->n_sms), 256, 0, ctx->st>>>(P.off, P.bytes, static_cast<const u64*>(d_fpos->p),
                                                                                      static_cast<const unsigned long long*>(ctx->dict_off->p) + base_id, n_new,
                                                                                      static_cast<unsigned char*>(ctx->dict_bytes->p));
-        ctx->stats.kernel_launches++;
     }
     timer_end(ctx);
     KB_CUDA(ctx, cudaGetLastError());
@@ -292,9 +368,42 @@ kb_status dict_encode_device(kb_ctx* ctx, const u64* d_off, const unsigned char*
 }
 
 
-}  // namespace kb
-
-using namespace kb;
+kb_status kb::decode_ids(kb_ctx* ctx, const u32* ids, u32 n, u32 n_empty, bool missing_empty, const char* what, Buf* off_out, Buf* bytes_out,
+                         u64* total_out) {
+    const size_t m = (size_t)n + n_empty;
+    Buf off, scratch, bytes;
+    KB_TRY(alloc_buf(ctx, (m + 1) * sizeof(u32), &off));
+    KB_TRY(alloc_buf(ctx, ((m + 1) / 2048 + 4) * sizeof(u32), &scratch));
+    u32* d_off = static_cast<u32*>(off->p);
+    KB_CUDA(ctx, cudaMemsetAsync(d_off + n, 0, ((size_t)n_empty + 1) * sizeof(u32), ctx->st));  // the scan runs over m + 1 entries: off[m] = total
+    const u32 c = ctrl_alloc(ctx, 4);  // [0..1] u64 total bytes, [2] quoted-triple id seen without a table, [3] walk too deep
+    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + c, 0, 4 * sizeof(u32), ctx->st));
+    const DictTab dict = dicttab(ctx);
+    const QuotedTab qt = quotedtab(ctx);
+    const int grid = grid_1d(n, ctx->n_sms);
+    timer_begin(ctx, F_OTHER, 4);
+    if (n)
+        decode_lengths_kernel<<<grid, 256, 0, ctx->st>>>(ids, n, dict, qt, d_off, reinterpret_cast<unsigned long long*>(ctx->ctrl + c), ctx->ctrl + c + 2,
+                                                         ctx->ctrl + c + 3, missing_empty ? 0u : 7u);
+    launch_exclusive_scan_u32(d_off, (u32)m + 1, static_cast<u32*>(scratch->p), ctx->st);
+    timer_end(ctx);
+    KB_CUDA(ctx, cudaGetLastError());
+    KB_TRY(ctrl_read(ctx));
+    unsigned long long total = 0;
+    memcpy(&total, ctx->h_ctrl + c, sizeof total);
+    if (ctx->h_ctrl[c + 2]) return fail(ctx, KB_E_UNSUPPORTED, "%s holds quoted-triple ids (bit 31) and no quoted-triple table is loaded (kb_quoted_load)", what);
+    if (ctx->h_ctrl[c + 3]) return fail(ctx, KB_E_LIMIT, "a quoted-triple term nests deeper than %d levels", KB_QUOTED_MAX_DEPTH);
+    if (total > 0xFFFFFFFFull) return fail(ctx, KB_E_LIMIT, "the text of %s would take %llu bytes (limit 2^32-1 per call)", what, total);
+    KB_TRY(alloc_buf(ctx, (size_t)total + 16, &bytes));
+    timer_begin(ctx, F_OTHER);
+    if (n) decode_gather_kernel<<<grid, 256, 0, ctx->st>>>(ids, n, dict, qt, d_off, static_cast<unsigned char*>(bytes->p));
+    timer_end(ctx);
+    KB_CUDA(ctx, cudaGetLastError());
+    *off_out = off;
+    *bytes_out = bytes;
+    if (total_out) *total_out = total;
+    return KB_OK;
+}
 
 extern "C" {
 
@@ -340,6 +449,84 @@ kb_status kb_dict_strings_info(kb_ctx* ctx, uint32_t* n_ids, uint64_t* n_bytes) 
         }
         *n_bytes = b;
     }
+    return KB_OK;
+}
+
+kb_status kb_dict_strings_load(kb_ctx* ctx, const uint64_t* offsets, const uint8_t* bytes, uint32_t n_ids) {
+    KB_ENTER(ctx);
+    ctx->dict_off.reset();
+    ctx->dict_bytes.reset();
+    ctx->dict_ids = 0;
+    ctx->dict_index = TagIndex{};  // (kb_dict_encode rebuilds its string -> id index lazily)
+    if (n_ids == 0) return KB_OK;
+    if (!offsets) return fail(ctx, KB_E_INVALID, "NULL offsets");
+    const uint64_t total = offsets[n_ids];
+    if (offsets[0] != 0 || (total && !bytes)) return fail(ctx, KB_E_INVALID, "offsets must start at 0 and bytes must not be NULL");
+    for (uint32_t i = 0; i < n_ids; i++) if (offsets[i + 1] < offsets[i]) return fail(ctx, KB_E_INVALID, "offsets decrease at id %u", i);
+    KB_TRY(alloc_buf(ctx, ((size_t)n_ids + 1) * sizeof(uint64_t), &ctx->dict_off));
+    KB_TRY(alloc_buf(ctx, (size_t)total + 16, &ctx->dict_bytes));
+    KB_CUDA(ctx, cudaMemcpyAsync(ctx->dict_off->p, offsets, ((size_t)n_ids + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->st));
+    if (total) KB_CUDA(ctx, cudaMemcpyAsync(ctx->dict_bytes->p, bytes, (size_t)total, cudaMemcpyHostToDevice, ctx->st));
+    KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
+    ctx->stats.h2d_bytes += ((size_t)n_ids + 1) * sizeof(uint64_t) + total;
+    ctx->dict_ids = n_ids;
+    return KB_OK;
+}
+
+kb_status kb_rel_decode(kb_ctx* ctx, const kb_rel* r, uint32_t col, kb_strings** out) {
+    KB_ENTER(ctx);
+    if (!r || !out) return fail(ctx, KB_E_INVALID, "NULL argument");
+    if (col >= r->cols.size()) return fail(ctx, KB_E_INVALID, "column %u out of range", col);
+    if (r->n >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "relation too large");
+    auto res = std::make_unique<kb_strings>();
+    res->n = r->n;
+    KB_TRY(decode_ids(ctx, r->cols[col].ptr, (u32)r->n, 0, false, "the column", &res->off, &res->bytes, &res->total));
+    *out = res.release();
+    return KB_OK;
+}
+kb_status kb_strings_info(const kb_strings* s, uint64_t* n_strings, uint64_t* total_bytes) {
+    if (!s) return KB_E_INVALID;
+    if (n_strings) *n_strings = s->n;
+    if (total_bytes) *total_bytes = s->total;
+    return KB_OK;
+}
+kb_status kb_strings_download(kb_ctx* ctx, const kb_strings* s, uint64_t* offsets, uint8_t* bytes) {
+    if (!ctx || !s) return KB_E_INVALID;
+    DeviceGuard guard(ctx->device);
+    if (offsets) {
+        std::vector<u32> h((size_t)s->n + 1);
+        KB_CUDA(ctx, cudaMemcpyAsync(h.data(), s->off->p, h.size() * sizeof(u32), cudaMemcpyDeviceToHost, ctx->st));
+        KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
+        for (size_t i = 0; i < h.size(); i++) offsets[i] = h[i];
+    }
+    if (bytes && s->total) {
+        KB_CUDA(ctx, cudaMemcpyAsync(bytes, s->bytes->p, (size_t)s->total, cudaMemcpyDeviceToHost, ctx->st));
+        KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
+    }
+    ctx->stats.d2h_bytes += ((size_t)s->n + 1) * sizeof(u32) + s->total;
+    return KB_OK;
+}
+void kb_strings_free(kb_ctx* ctx, kb_strings* s) {
+    if (!s) return;
+    if (ctx) { DeviceGuard guard(ctx->device); delete s; }
+    else delete s;
+}
+
+kb_status kb_dict_strings_download(kb_ctx* ctx, uint32_t first, uint32_t n, uint64_t* offsets, uint8_t* bytes) {
+    KB_ENTER(ctx);
+    if (!offsets) return fail(ctx, KB_E_INVALID, "NULL offsets");
+    if ((u64)first + n > ctx->dict_ids) return fail(ctx, KB_E_INVALID, "ids [%u, %llu) past the %u the device dictionary holds", first, (unsigned long long)first + n, ctx->dict_ids);
+    offsets[0] = 0;
+    if (n == 0) return KB_OK;
+    KB_CUDA(ctx, cudaMemcpyAsync(offsets, static_cast<const unsigned long long*>(ctx->dict_off->p) + first, ((size_t)n + 1) * sizeof(u64), cudaMemcpyDeviceToHost, ctx->st));
+    KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
+    const u64 base = offsets[0];
+    for (u32 k = 0; k <= n; k++) offsets[k] -= base;
+    if (bytes && offsets[n]) {
+        KB_CUDA(ctx, cudaMemcpyAsync(bytes, static_cast<const unsigned char*>(ctx->dict_bytes->p) + base, (size_t)offsets[n], cudaMemcpyDeviceToHost, ctx->st));
+        KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
+    }
+    ctx->stats.d2h_bytes += ((size_t)n + 1) * sizeof(u64) + (bytes ? offsets[n] : 0);
     return KB_OK;
 }
 

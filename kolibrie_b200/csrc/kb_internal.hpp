@@ -75,6 +75,20 @@ struct PendingTimer {
     int fam;
 };
 
+// A persistent tag-indexed table (kb_tagtab.cuh) over keys 0, 1, ... of a growing set: keys [0, indexed) are in it.
+struct TagIndex {
+    Buf tab;
+    u64 slots = 0;
+    u32 indexed = 0;
+};
+
+// the grid of a 1-D grid-stride kernel over n items
+inline int grid_1d(u64 n, int n_sms, int threads = 256, int per_sm = 8) {
+    const u64 want = (n + threads - 1) / threads, cap = (u64)n_sms * per_sm;
+    return (int)(want < 1 ? 1 : want < cap ? want : cap);
+}
+inline u32 bits_of(u64 x) { return x ? 64u - (u32)__builtin_clzll(x) : 0u; }
+
 }  // namespace kb
 
 struct kb_rel {
@@ -180,17 +194,15 @@ struct kb_ctx {
     kb::Buf num, isnum;
     kb::Buf i32val, isi32;  // kb_dict_legacy_i32_load: the legacy executor's integer view of the terms
     kb::u32 n_i32 = 0;
-    kb::Buf dict_off, dict_bytes;  // kb_dict_strings_load / kb_dict_encode: u64 offsets [dict_ids + 1] + UTF-8 bytes
+    // the device dictionary: written only by kb_dict.cu (kb_dict_strings_load, dict_encode_device), and released by kb_ctx_destroy
+    kb::Buf dict_off, dict_bytes;  // u64 offsets [dict_ids + 1] + UTF-8 bytes
     kb::u32 dict_ids = 0;
-    kb::Buf dict_index;            // kb_dict_encode: open-addressing index string -> id (hash tag << 32 | id), built lazily
-    kb::u64 dict_index_slots = 0;
-    kb::u32 dict_indexed = 0;      // ids [0, dict_indexed) are in the index
-    kb::Buf quoted_s, quoted_p, quoted_o;  // kb_quoted_load: the quoted-triple table, indexed by id & 0x7FFFFFFF (EMPTY32: no entry)
+    kb::TagIndex dict_index;       // kb_dict_encode: string -> id (payload: the id), built lazily
+    // the quoted-triple table: written only by kb_quoted.cu (kb_quoted_load, quoted_encode)
+    kb::Buf quoted_s, quoted_p, quoted_o;  // indexed by id & 0x7FFFFFFF (EMPTY32: no entry)
     kb::u32 quoted_slots = 0;
-    kb::u32 quoted_cap = 0;        // slots the three buffers hold (kb_bind's TRIPLE grows them with headroom; slots past quoted_slots are EMPTY32)
-    kb::Buf quoted_rev;            // kb_bind's TRIPLE: reverse index (s, p, o) -> table index (hash tag << 32 | index), built lazily,
-    kb::u64 quoted_rev_slots = 0;  // dropped by kb_quoted_load
-    kb::u32 quoted_rev_indexed = 0;  // table indices [0, quoted_rev_indexed) are in it
+    kb::u32 quoted_cap = 0;        // slots the three buffers hold (TRIPLE grows them with headroom; slots past quoted_slots are EMPTY32)
+    kb::TagIndex quoted_rev;       // TRIPLE: (s, p, o) -> table index (payload: the index), built lazily, dropped by kb_quoted_load
     kb::u32 n_ids = 0;
     kb::u64 num_version = 1;  // bumped by kb_dict_numeric_load: typed literal columns of the index are tied to it
     // value order of the numeric side table (kb_numrank.cuh: sorted distinct non-NaN values, -0.0 folded, 0.0 included), on the device
@@ -286,6 +298,16 @@ inline size_t round256(size_t b) { return (b + 255) & ~(size_t)255; }
     KB_TRY(kb::begin_call(ctx))
 
 kb_status alloc_buf(kb_ctx* ctx, size_t bytes, Buf* out);
+// one CUB device call: size query, scratch, call
+template <class F>
+kb_status cub_run(kb_ctx* ctx, F f) {
+    size_t t = 0;
+    KB_CUDA(ctx, f(nullptr, t));
+    Buf b;
+    KB_TRY(alloc_buf(ctx, t > 16 ? t : 16, &b));
+    KB_CUDA(ctx, f(b->p, t));
+    return KB_OK;
+}
 kb_status alloc_col(kb_ctx* ctx, u64 rows, Col* out);
 kb_status begin_call(kb_ctx* ctx);                      // zero the control arena
 u32 ctrl_alloc(kb_ctx* ctx, u32 words);                 // returns word offset into ctx->ctrl
@@ -413,7 +435,25 @@ kb_status star_join_impl(kb_ctx* ctx, u32 join_slot, const kb_pattern* pats, u32
                          std::unique_ptr<kb_rel>* out, AggSpec* agg = nullptr);
 // kb_bind_join behind the entry point (the pattern is checked by the caller)
 kb_status bind_join_impl(kb_ctx* ctx, const kb_rel& left, const kb_pattern& pat, std::unique_ptr<kb_rel>* out);
+// the device dictionary and the quoted-triple table as the kernels read them (null / n = 0 while empty)
+DictTab dicttab(const kb_ctx* ctx);
 QuotedTab quotedtab(const kb_ctx* ctx);
+// The text of n ids (kb_dict.cu), rendered as kb_rel_decode renders them (missing_empty: a term the tables do not hold is "" instead of
+// "unknown"), followed by n_empty more "": *off = u32 offsets [n + n_empty + 1], *bytes the text, *total (nullable) its bytes. One control-arena read. A quoted id
+// without a table is KB_E_UNSUPPORTED, a walk past KB_QUOTED_MAX_DEPTH or more than 2^32-1 bytes KB_E_LIMIT; `what` names the ids.
+kb_status decode_ids(kb_ctx* ctx, const u32* ids, u32 n, u32 n_empty, bool missing_empty, const char* what, Buf* off, Buf* bytes, u64* total);
+// ensure the persistent index holds keys [0, n_keys) and stays below load 1/2 with `extra` more (kb_api.cu): rebuilt larger (1024 slots
+// at least, 1.5x headroom) when too small, then insert(first, n, tab, mask, overflow word) launches the insert of the keys it lacks
+// (one kernel). KB_E_LIMIT names `what` when the insert overflows.
+template <class Insert>
+kb_status tag_index_ensure(kb_ctx* ctx, TagIndex* ix, u32 n_keys, u64 extra, const char* what, Insert insert);
+// a batch table for n keys (kb_tagtab.cuh): a power of two >= 2n, 1024 slots at least, every slot empty
+kb_status tag_batch_table(kb_ctx* ctx, u64 n, Buf* tab, u64* slots);
+// TRIPLE of kb_bind: QuotedTripleStore::encode of n rows (kb_quoted.cu). col[k] (null: the constant cval[k]) are the components; a new
+// triple gets id next_qt_id + rank of its first row and joins the table. out[i] = the id, or old[i] (null: EMPTY32) where a component is
+// unbound; *n_unbound += rows left EMPTY32.
+kb_status quoted_encode(kb_ctx* ctx, const u32* const* col, const u32* cval, u32 n, u32 next_qt_id, const u32* old, u32* out,
+                        unsigned long long* n_unbound, kb_bind_info* info);
 // Dense ranks of d >= 1 values (kb_order.cu), given by an order key per value (nkey, numeric) or by their rendered strings (str_off[d + 1]
 // u32 offsets into bytes, compared byte by byte, a proper prefix first): afterwards rank_of[v] is the rank of value v, *n_values the
 // number of distinct values and *rounds the refinement rounds taken (7 bytes of string a round).
@@ -435,5 +475,30 @@ kb_status bgp_components(kb_ctx* ctx, const kb_pattern* pats, u32 n_pats, const 
                          const std::vector<std::vector<u32>>& pv, const std::vector<u32>& all_slots, std::unique_ptr<kb_rel>* out);
 u32 pow2_at_least(u64 x);
 kb_status check_pattern(kb_ctx* ctx, const kb_pattern& pt);
+
+template <class Insert>
+kb_status tag_index_ensure(kb_ctx* ctx, TagIndex* ix, u32 n_keys, u64 extra, const char* what, Insert insert) {
+    const u64 need = ((u64)n_keys + extra) * 2 + 64;
+    if (!ix->tab || ix->slots < need) {
+        u64 slots = 1024;
+        while (slots < need + need / 2) slots <<= 1;  // headroom: the next batches insert in place
+        ix->tab.reset();
+        KB_TRY(alloc_buf(ctx, slots * sizeof(u64), &ix->tab));
+        KB_CUDA(ctx, cudaMemsetAsync(ix->tab->p, 0xFF, slots * sizeof(u64), ctx->st));
+        ix->slots = slots;
+        ix->indexed = 0;
+    }
+    if (ix->indexed < n_keys) {
+        const u32 c = ctrl_alloc(ctx, 1);
+        KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + c, 0, sizeof(u32), ctx->st));
+        insert(ix->indexed, n_keys - ix->indexed, static_cast<u64*>(ix->tab->p), ix->slots - 1, ctx->ctrl + c);
+        ctx->stats.kernel_launches++;
+        KB_CUDA(ctx, cudaGetLastError());
+        KB_TRY(ctrl_read(ctx));
+        if (ctx->h_ctrl[c]) return fail(ctx, KB_E_LIMIT, "%s overflow", what);
+        ix->indexed = n_keys;
+    }
+    return KB_OK;
+}
 
 }  // namespace kb

@@ -3,7 +3,7 @@
 // mbarrier), matches are compacted with warp ballots, and output positions come from a single-pass decoupled look-back
 // prefix over tiles, so every kernel reads its input exactly once and writes a deterministic, input-ordered output.
 #include "kb_group.cuh"
-#include "kb_kernels.cuh"
+#include "kb_internal.hpp"
 #include "kb_numrank.cuh"
 
 #include <math_constants.h>
@@ -13,16 +13,6 @@
 #include <type_traits>
 
 namespace kb {
-
-static inline int grid_for(const void* kernel, int threads, size_t smem, int n_sms, u32 n_tiles) {
-    int per_sm = 1;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem);
-    if (per_sm < 1) per_sm = 1;
-    long long g = (long long)per_sm * n_sms;  // persistent: a whole number of resident CTAs per SM, on every SM
-    if (g > (long long)n_tiles) g = n_tiles;
-    if (g < 1) g = 1;
-    return (int)g;
-}
 
 // =================================================================================================================
 // K_scan
@@ -2864,479 +2854,6 @@ void launch_set64_erase(u64* set, u32 set_slots, const u32* s, const u32* o, u32
 }
 
 // =================================================================================================================
-// dictionary decode
-enum { QW_OK = 0, QW_UNKNOWN = 1, QW_DEEP = 2 };
-// Dictionary::decode_term of a quoted id (dictionary.rs:60-72) as an explicit depth-first walk: lit(text, bytes) for "<< ", " ", " >>",
-// word(id) for every dictionary component, in output order. Like the reference's `?`, the walk stops at the first id that neither table
-// holds (QW_UNKNOWN: the whole term is "unknown"); entering a level past KB_QUOTED_MAX_DEPTH gives QW_DEEP. The stack holds one table
-// index per level and a 2-bit component cursor per level.
-template <class Lit, class Word>
-__device__ u32 quoted_walk(u32 id, u32 dict_ids, const QuotedTab& qt, Lit lit, Word word) {
-    u32 ent[KB_QUOTED_MAX_DEPTH];
-    u32 next = 0;  // bits 2d..2d+1: components of level d already emitted
-    int d = 0;
-    u32 cur = id;
-    for (;;) {
-        const u32 x = cur & 0x7FFFFFFFu;
-        if (x >= qt.n || __ldg(qt.p + x) == EMPTY32) return QW_UNKNOWN;
-        if (d == KB_QUOTED_MAX_DEPTH) return QW_DEEP;
-        ent[d] = x;
-        next &= ~(3u << (2 * d));
-        d++;
-        lit("<< ", 3u);
-        for (;;) {
-            const int top = d - 1;
-            const u32 k = (next >> (2 * top)) & 3u;
-            if (k == 3u) {
-                lit(" >>", 3u);
-                if (--d == 0) return QW_OK;
-                continue;
-            }
-            next += 1u << (2 * top);
-            if (k) lit(" ", 1u);
-            const u32 e = ent[top];
-            const u32 c = __ldg((k == 0u ? qt.s : k == 1u ? qt.p : qt.o) + e);
-            if (c & 0x80000000u) { cur = c; break; }
-            if (c >= dict_ids) return QW_UNKNOWN;
-            word(c);
-        }
-    }
-}
-
-__global__ void __launch_bounds__(256) decode_lengths_kernel(const u32* __restrict__ ids, u32 n, const unsigned long long* __restrict__ dict_off, u32 dict_ids,
-                                                             const QuotedTab qt, u32* __restrict__ len, unsigned long long* total, u32* quoted, u32* deep,
-                                                             u32 missing_len) {
-    const u32 stride = gridDim.x * blockDim.x;
-    unsigned long long t = 0;
-    bool q = false, dp = false;
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-        const u32 id = ids[i];
-        unsigned long long l = missing_len;  // "unknown" or ""
-        if (id & 0x80000000u) {
-            if (qt.n == 0u) {
-                q = true;
-            } else {
-                unsigned long long acc = 0;
-                const u32 r = quoted_walk(id, dict_ids, qt, [&](const char*, u32 k) { acc += k; },
-                                          [&](u32 c) { acc += __ldg(dict_off + c + 1) - __ldg(dict_off + c); });
-                dp = dp || r == QW_DEEP;
-                if (r == QW_OK) l = acc;
-            }
-        } else if (id < dict_ids) {
-            l = __ldg(dict_off + id + 1) - __ldg(dict_off + id);
-        }
-        len[i] = l > 0xFFFFFFFFull ? 0xFFFFFFFFu : (u32)l;  // (the total then exceeds 2^32-1: the caller refuses the column)
-        t += l;
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-    if ((threadIdx.x & 31) == 0 && t) atomicAdd(total, t);
-    if (q) *quoted = 1u;
-    if (dp) *deep = 1u;
-}
-void launch_decode_lengths(const u32* ids, u32 n, const unsigned long long* dict_off, u32 dict_ids, const QuotedTab& qt, u32* len,
-                           unsigned long long* total, u32* quoted, u32* deep, int n_sms, cudaStream_t st, bool missing_empty) {
-    if (n == 0) return;
-    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull);
-    decode_lengths_kernel<<<grid, 256, 0, st>>>(ids, n, dict_off, dict_ids, qt, len, total, quoted, deep, missing_empty ? 0u : 7u);
-}
-__global__ void __launch_bounds__(256) decode_gather_kernel(const u32* __restrict__ ids, u32 n, const unsigned long long* __restrict__ dict_off,
-                                                            const unsigned char* __restrict__ dict_bytes, u32 dict_ids, const QuotedTab qt,
-                                                            const u32* __restrict__ off, unsigned char* __restrict__ out) {
-    const int lane = threadIdx.x & 31;
-    const u32 warps = (gridDim.x * blockDim.x) >> 5;
-    const u32 n_chunks = (n + 31u) >> 5;
-    for (u32 chunk = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; chunk < n_chunks; chunk += warps) {
-        const u32 i = chunk * 32u + (u32)lane;
-        u32 id = 0, dst = 0, l = 0;
-        unsigned long long src = 0;
-        bool known = false, walk = false;
-        if (i < n) {
-            id = ids[i];
-            dst = off[i];
-            l = off[i + 1] - dst;
-            known = id < dict_ids;
-            if (known) src = __ldg(dict_off + id);
-            walk = (id & 0x80000000u) != 0u && l >= 8u;  // a rendered quoted term is at least 8 bytes: 7 is "unknown", 0 is ""
-        }
-        const u32 wl = walk ? 0u : l;
-        for (int r = 0; r < 32; r++) {  // the warp copies row r of its chunk: consecutive lanes, consecutive bytes
-            const u32 rl = __shfl_sync(0xffffffffu, wl, r);
-            if (rl == 0u) continue;
-            const u32 rdst = __shfl_sync(0xffffffffu, dst, r);
-            const unsigned long long rsrc = __shfl_sync(0xffffffffu, src, r);
-            const bool rknown = __shfl_sync(0xffffffffu, known ? 1 : 0, r) != 0;
-            for (u32 b = (u32)lane; b < rl; b += 32u) out[rdst + b] = rknown ? __ldg(dict_bytes + rsrc + b) : (unsigned char)"unknown"[b];
-        }
-        if (walk) {  // a quoted term: this thread writes it, walking it again
-            unsigned char* w = out + dst;
-            quoted_walk(id, dict_ids, qt, [&](const char* s, u32 k) { for (u32 b = 0; b < k; b++) *w++ = (unsigned char)s[b]; },
-                        [&](u32 c) {
-                            const unsigned long long a = __ldg(dict_off + c), e = __ldg(dict_off + c + 1);
-                            for (unsigned long long b = a; b < e; b++) *w++ = __ldg(dict_bytes + b);
-                        });
-        }
-    }
-}
-void launch_decode_gather(const u32* ids, u32 n, const unsigned long long* dict_off, const unsigned char* dict_bytes, u32 dict_ids, const QuotedTab& qt,
-                          const u32* off, unsigned char* out, int n_sms, cudaStream_t st) {
-    if (n == 0) return;
-    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull);
-    decode_gather_kernel<<<grid, 256, 0, st>>>(ids, n, dict_off, dict_bytes, dict_ids, qt, off, out);
-}
-
-// =================================================================================================================
-// quoted-triple match (kb_scan_quoted): the table's s, p, o columns stream through two shared stages of QM_TILE entries each; an entry
-// that passes every check is one output row (entry id, inner variables), appended with a warp ballot and one atomic per warp
-__device__ __forceinline__ u32 qm_comp(u32 k, u32 s, u32 p, u32 o) { return k == 0u ? s : k == 1u ? p : o; }
-
-__global__ void __launch_bounds__(QM_THREADS) quoted_match_kernel(const __grid_constant__ QuotedMatchParams P) {
-    __shared__ __align__(128) u32 sbuf[2][3][QM_TILE];
-    __shared__ __align__(8) u64 bars[2];
-    __shared__ u32 s_tile[2];
-    const int tid = threadIdx.x, lane = tid & 31;
-    auto issue = [&](u32 stage) {  // one thread: take the next tile and start its three column copies into `stage`
-        const u32 t = atomicAdd(P.ticket, 1u);
-        s_tile[stage] = t;
-        if (t < P.n_tiles) {
-            const u32 b = t * (u32)QM_TILE;
-            const u32 c = min((u32)QM_TILE, P.t.n - b);
-            const u32 bytes = (c * 4u + 15u) & ~15u;  // columns are padded to 256 B: the rounded-up read stays in bounds
-            mbar_arrive_expect_tx(&bars[stage], bytes * 3u);
-            tma_load_1d(sbuf[stage][0], P.t.s + b, bytes, &bars[stage]);
-            tma_load_1d(sbuf[stage][1], P.t.p + b, bytes, &bars[stage]);
-            tma_load_1d(sbuf[stage][2], P.t.o + b, bytes, &bars[stage]);
-        }
-    };
-    if (tid == 0) {
-        mbar_init(&bars[0], 1);
-        mbar_init(&bars[1], 1);
-        fence_mbar_init();
-        issue(0);
-        issue(1);
-    }
-    __syncthreads();
-    // a CTA's tickets grow with its iterations: once a stage draws a ticket past the end, no copy is in flight in the other one
-    for (u32 it = 0;; it++) {
-        const u32 stage = it & 1u;
-        const u32 tile = s_tile[stage];
-        if (tile >= P.n_tiles) break;
-        mbar_wait(&bars[stage], (it >> 1) & 1u);
-        const u32 base = tile * (u32)QM_TILE;
-        const u32 cnt = min((u32)QM_TILE, P.t.n - base);
-        for (u32 j = (u32)tid; j < (u32)QM_TILE; j += QM_THREADS) {  // the same trip count in every lane: the ballot sees the whole warp
-            u32 s = 0, p = EMPTY32, o = 0;
-            if (j < cnt) { s = sbuf[stage][0][j]; p = sbuf[stage][1][j]; o = sbuf[stage][2][j]; }
-            bool ok = p != EMPTY32;  // (empty slots and the tail of the last tile)
-#pragma unroll
-            for (int k = 0; k < 6; k++) {
-                if ((u32)k >= P.n_chk) break;
-                const u32 v = qm_comp(P.chk_comp[k], s, p, o), a = P.chk_arg[k];
-                const u32 kind = P.chk_kind[k];
-                ok = ok && (kind == QM_CONST ? v == a : kind == QM_EQ ? v == qm_comp(a, s, p, o) : kind == QM_QUOTED ? (v & 0x80000000u) != 0u : true);
-            }
-            const unsigned b = __ballot_sync(0xffffffffu, ok);
-            if (!b) continue;
-            u32 at = 0;
-            if (lane == __ffs(b) - 1) at = atomicAdd(P.count, (u32)__popc(b));
-            at = __shfl_sync(0xffffffffu, at, __ffs(b) - 1);
-            if (ok) {
-                const u32 r = at + (u32)__popc(b & ((1u << lane) - 1u));
-                P.out[0][r] = 0x80000000u | (base + j);
-#pragma unroll
-                for (int c = 1; c < 7; c++)
-                    if ((u32)c < P.n_out) P.out[c][r] = qm_comp(P.out_comp[c], s, p, o);
-            }
-        }
-        __syncthreads();  // every thread is done with the stage: it takes the tile after next
-        if (tid == 0) issue(stage);
-    }
-}
-void launch_quoted_match(const QuotedMatchParams& p, int n_sms, cudaStream_t st) {
-    if (p.n_tiles == 0) return;
-    const int grid = grid_for((const void*)quoted_match_kernel, QM_THREADS, 0, n_sms, p.n_tiles);
-    quoted_match_kernel<<<grid, QM_THREADS, 0, st>>>(p);
-}
-
-// =================================================================================================================
-// BIND built-ins (kb_bind)
-__device__ __forceinline__ void bind_count_unbound(bool unbound, unsigned long long* n_unbound) {
-    const unsigned b = __ballot_sync(0xffffffffu, unbound);
-    if ((threadIdx.x & 31) == 0 && b) atomicAdd(n_unbound, (unsigned long long)__popc(b));
-}
-static int bind_grid(u32 n, int n_sms) { return (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull); }
-
-__global__ void __launch_bounds__(256) bind_component_kernel(const u32* __restrict__ arg, u32 n, const QuotedTab qt, u32 comp, const u32* __restrict__ old,
-                                                             u32* __restrict__ out, unsigned long long* n_unbound) {
-    const u32* __restrict__ tab = comp == 0u ? qt.s : comp == 1u ? qt.p : qt.o;
-    const u32 stride = gridDim.x * blockDim.x;
-    const u32 end = (n + 31u) & ~31u;  // whole warps for the ballot
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < end; i += stride) {
-        u32 v = EMPTY32;
-        if (i < n) {
-            const u32 id = arg[i], x = id & 0x7FFFFFFFu;
-            if ((id & 0x80000000u) && x < qt.n) v = __ldg(tab + x);  // a hole holds EMPTY32; KB_ID_NONE has x = 2^31-1 >= qt.n
-            if (v == EMPTY32 && old) v = old[i];
-            out[i] = v;
-        }
-        bind_count_unbound(i < n && v == EMPTY32, n_unbound);
-    }
-}
-void launch_bind_component(const u32* arg, u32 n, const QuotedTab& qt, u32 comp, const u32* old, u32* out, unsigned long long* n_unbound, int n_sms,
-                           cudaStream_t st) {
-    if (n == 0) return;
-    bind_component_kernel<<<bind_grid(n, n_sms), 256, 0, st>>>(arg, n, qt, comp, old, out, n_unbound);
-}
-
-__global__ void __launch_bounds__(256) bind_istriple_first_kernel(const u32* __restrict__ arg, u32 n, u32* first) {
-    const u32 stride = gridDim.x * blockDim.x;
-    const u32 end = (n + 31u) & ~31u;
-    u32 ft = EMPTY32, ff = EMPTY32;
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < end; i += stride) {
-        if (i < n) {
-            const u32 id = arg[i];
-            if (id != EMPTY32) {
-                if (id & 0x80000000u) ft = min(ft, i);
-                else ff = min(ff, i);
-            }
-        }
-    }
-    ft = __reduce_min_sync(0xffffffffu, ft);
-    ff = __reduce_min_sync(0xffffffffu, ff);
-    if ((threadIdx.x & 31) == 0) {
-        if (ft != EMPTY32) atomicMin(first, ft);
-        if (ff != EMPTY32) atomicMin(first + 1, ff);
-    }
-}
-void launch_bind_istriple_first(const u32* arg, u32 n, u32* first, int n_sms, cudaStream_t st) {
-    if (n == 0) return;
-    bind_istriple_first_kernel<<<bind_grid(n, n_sms), 256, 0, st>>>(arg, n, first);
-}
-__global__ void __launch_bounds__(256) bind_istriple_write_kernel(const u32* __restrict__ arg, u32 n, u32 id_true, u32 id_false, const u32* __restrict__ old,
-                                                                  u32* __restrict__ out, unsigned long long* n_unbound) {
-    const u32 stride = gridDim.x * blockDim.x;
-    const u32 end = (n + 31u) & ~31u;
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < end; i += stride) {
-        u32 v = EMPTY32;
-        if (i < n) {
-            const u32 id = arg[i];
-            v = id == EMPTY32 ? (old ? old[i] : EMPTY32) : (id & 0x80000000u) ? id_true : id_false;
-            out[i] = v;
-        }
-        bind_count_unbound(i < n && v == EMPTY32, n_unbound);
-    }
-}
-void launch_bind_istriple_write(const u32* arg, u32 n, u32 id_true, u32 id_false, const u32* old, u32* out, unsigned long long* n_unbound, int n_sms,
-                                cudaStream_t st) {
-    if (n == 0) return;
-    bind_istriple_write_kernel<<<bind_grid(n, n_sms), 256, 0, st>>>(arg, n, id_true, id_false, old, out, n_unbound);
-}
-
-// ---- TRIPLE
-__device__ __forceinline__ u64 triple_hash(u32 s, u32 p, u32 o) {
-    u64 h = ((u64)s << 32 | p) * 0x9E3779B97F4A7C15ull;
-    h ^= (u64)o * 0xC2B2AE3D27D4EB4Full;
-    h ^= h >> 31;  // murmur3 64-bit finaliser
-    h *= 0xff51afd7ed558ccdull;
-    h ^= h >> 33;
-    h *= 0xc4ceb9fe1a85ec53ull;
-    h ^= h >> 33;
-    return h;
-}
-constexpr u64 TEMPTY = 0xFFFFFFFFFFFFFFFFull;
-__device__ __forceinline__ u64 tentry(u64 h, u32 payload) { return (h & 0xFFFFFFFF00000000ull) | payload; }
-__device__ __forceinline__ void bind_triple_row(const BindTripleParams& P, u32 i, u32* s, u32* p, u32* o) {
-    *s = P.col[0] ? P.col[0][i] : P.cval[0];
-    *p = P.col[1] ? P.col[1][i] : P.cval[1];
-    *o = P.col[2] ? P.col[2][i] : P.cval[2];
-}
-
-__global__ void __launch_bounds__(256) bind_triple_resolve_kernel(const __grid_constant__ BindTripleParams P) {
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < P.n; i += gridDim.x * blockDim.x) {
-        u32 s, p, o;
-        bind_triple_row(P, i, &s, &p, &o);
-        u32 hit = EMPTY32, slot_of = EMPTY32;
-        if (s != EMPTY32 && p != EMPTY32 && o != EMPTY32) {
-            const u64 h = triple_hash(s, p, o);
-            if (P.rev) {
-                for (u64 slot = h & P.rev_mask, probes = 0; probes <= P.rev_mask; probes++, slot = (slot + 1) & P.rev_mask) {
-                    const u64 e = P.rev[slot];
-                    if (e == TEMPTY) break;
-                    if ((e >> 32) != (h >> 32)) continue;
-                    const u32 x = (u32)e;
-                    if (__ldg(P.qt.s + x) == s && __ldg(P.qt.p + x) == p && __ldg(P.qt.o + x) == o) { hit = 0x80000000u | x; break; }
-                }
-            }
-            if (hit == EMPTY32) {
-                bool placed = false;
-                for (u64 slot = h & P.batch_mask, probes = 0; probes <= P.batch_mask; probes++, slot = (slot + 1) & P.batch_mask) {
-                    u64 e = *reinterpret_cast<volatile u64*>(&P.batch[slot]);
-                    if (e == TEMPTY) {
-                        e = atomicCAS(reinterpret_cast<unsigned long long*>(&P.batch[slot]), TEMPTY, tentry(h, i));
-                        if (e == TEMPTY) { slot_of = (u32)slot; placed = true; break; }
-                    }
-                    if ((e >> 32) != (h >> 32)) continue;
-                    u32 rs, rp, ro;  // a row holding the slot's triple (the slot's position may be lowered concurrently: always the same triple)
-                    bind_triple_row(P, (u32)e, &rs, &rp, &ro);
-                    if (rs == s && rp == p && ro == o) {
-                        atomicMin(reinterpret_cast<unsigned long long*>(&P.batch[slot]), tentry(h, i));
-                        slot_of = (u32)slot;
-                        placed = true;
-                        break;
-                    }
-                }
-                if (!placed) *P.overflow = 1u;
-            }
-        }
-        P.hit[i] = hit;
-        P.slot_of[i] = slot_of;
-    }
-}
-void launch_bind_triple_resolve(const BindTripleParams& p, int n_sms, cudaStream_t st) {
-    if (p.n == 0) return;
-    bind_triple_resolve_kernel<<<bind_grid(p.n, n_sms), 256, 0, st>>>(p);
-}
-__global__ void __launch_bounds__(256) bind_triple_mark_kernel(const __grid_constant__ BindTripleParams P) {
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < P.n; i += gridDim.x * blockDim.x) {
-        const u32 so = P.slot_of[i];
-        P.first[i] = so != EMPTY32 && (u32)P.batch[so] == i ? 1u : 0u;
-    }
-}
-void launch_bind_triple_mark(const BindTripleParams& p, int n_sms, cudaStream_t st) {
-    if (p.n == 0) return;
-    bind_triple_mark_kernel<<<bind_grid(p.n, n_sms), 256, 0, st>>>(p);
-}
-__global__ void __launch_bounds__(256) bind_triple_assign_kernel(const __grid_constant__ BindTripleParams P) {
-    const u32 stride = gridDim.x * blockDim.x;
-    const u32 end = (P.n + 31u) & ~31u;
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < end; i += stride) {
-        u32 v = EMPTY32;
-        if (i < P.n) {
-            const u32 so = P.slot_of[i];
-            if (so != EMPTY32) {
-                const u32 fp = (u32)P.batch[so];
-                const u32 r = P.first[fp];
-                v = P.next_qt_id + r;
-                if (fp == i) {
-                    u32 s, p, o;
-                    bind_triple_row(P, i, &s, &p, &o);
-                    const u32 x = (P.next_qt_id & 0x7FFFFFFFu) + r;
-                    P.ws[x] = s;
-                    P.wp[x] = p;
-                    P.wo[x] = o;
-                }
-            } else {
-                v = P.hit[i];
-                if (v == EMPTY32 && P.old) v = P.old[i];
-            }
-            P.out[i] = v;
-        }
-        bind_count_unbound(i < P.n && v == EMPTY32, P.n_unbound);
-    }
-}
-void launch_bind_triple_assign(const BindTripleParams& p, int n_sms, cudaStream_t st) {
-    if (p.n == 0) return;
-    bind_triple_assign_kernel<<<bind_grid(p.n, n_sms), 256, 0, st>>>(p);
-}
-__global__ void __launch_bounds__(256) quoted_rev_insert_kernel(const QuotedTab qt, u32 first, u32 n, u64* __restrict__ rev, u64 mask, u32* overflow) {
-    for (u32 k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
-        const u32 x = first + k;
-        const u32 s = qt.s[x], p = qt.p[x], o = qt.o[x];
-        if (p == EMPTY32) continue;  // a hole
-        const u64 h = triple_hash(s, p, o);
-        bool placed = false;
-        for (u64 slot = h & mask, probes = 0; probes <= mask; probes++, slot = (slot + 1) & mask) {
-            u64 e = *reinterpret_cast<volatile u64*>(&rev[slot]);
-            if (e == TEMPTY) {
-                e = atomicCAS(reinterpret_cast<unsigned long long*>(&rev[slot]), TEMPTY, tentry(h, x));
-                if (e == TEMPTY) { placed = true; break; }
-            }
-            if ((e >> 32) != (h >> 32)) continue;
-            const u32 y = (u32)e;
-            if (qt.s[y] == s && qt.p[y] == p && qt.o[y] == o) {  // the same triple twice in the table: the smaller index answers
-                atomicMin(reinterpret_cast<unsigned long long*>(&rev[slot]), tentry(h, x));
-                placed = true;
-                break;
-            }
-        }
-        if (!placed) *overflow = 1u;
-    }
-}
-void launch_quoted_rev_insert(const QuotedTab& qt, u32 first, u32 n, u64* rev, u64 mask, u32* overflow, int n_sms, cudaStream_t st) {
-    if (n == 0) return;
-    quoted_rev_insert_kernel<<<bind_grid(n, n_sms), 256, 0, st>>>(qt, first, n, rev, mask, overflow);
-}
-
-// ---- CONCAT
-__device__ __forceinline__ void concat_piece(const BindConcatParams& P, u32 a, u32 i, const unsigned char** src, u32* len) {
-    if (P.col[a]) {
-        const u32 id = P.col[a][i];
-        if (id < P.dict_ids) {  // Dictionary::decode: quoted ids (>= 2^31 > dict_ids), missing ids and KB_ID_NONE contribute ""
-            const unsigned long long b = __ldg(P.dict_off + id);
-            *src = P.dict_bytes + b;
-            *len = (u32)(__ldg(P.dict_off + id + 1) - b);
-        } else {
-            *src = nullptr;
-            *len = 0u;
-        }
-    } else {
-        *src = P.cbytes + P.coff[a];
-        *len = P.clen[a];
-    }
-}
-__global__ void __launch_bounds__(256) bind_concat_lengths_kernel(const __grid_constant__ BindConcatParams P) {
-    unsigned long long t = 0;
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < P.n; i += gridDim.x * blockDim.x) {
-        unsigned long long l = 0;
-        for (u32 a = 0; a < P.n_args; a++) {
-            const unsigned char* src;
-            u32 k;
-            concat_piece(P, a, i, &src, &k);
-            l += k;
-        }
-        P.len[i] = l > 0xFFFFFFFFull ? 0xFFFFFFFFu : (u32)l;  // (the total then exceeds the limit: the caller refuses the call)
-        t += l;
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-    if ((threadIdx.x & 31) == 0 && t) atomicAdd(P.total, t);
-}
-void launch_bind_concat_lengths(const BindConcatParams& p, int n_sms, cudaStream_t st) {
-    if (p.n == 0) return;
-    bind_concat_lengths_kernel<<<bind_grid(p.n, n_sms), 256, 0, st>>>(p);
-}
-__global__ void __launch_bounds__(256) bind_concat_gather_kernel(const __grid_constant__ BindConcatParams P) {
-    const int lane = threadIdx.x & 31;
-    const u32 warps = (gridDim.x * blockDim.x) >> 5;
-    const u32 n_chunks = (P.n + 31u) >> 5;
-    for (u32 chunk = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; chunk < n_chunks; chunk += warps) {
-        const u32 i = chunk * 32u + (u32)lane;
-        u32 dst = 0;
-        if (i < P.n) {
-            dst = P.len[i];
-            P.off64[i] = dst;
-            if (i + 1u == P.n) P.off64[P.n] = P.len[P.n];
-        }
-        const u32 rows = min(32u, P.n - chunk * 32u);
-        for (u32 r = 0; r < rows; r++) {  // the warp writes row r of its chunk, piece by piece: consecutive lanes, consecutive bytes
-            const u32 row = chunk * 32u + r;
-            u32 w = __shfl_sync(0xffffffffu, dst, (int)r);
-            for (u32 a = 0; a < P.n_args; a++) {
-                const unsigned char* src;
-                u32 k;
-                concat_piece(P, a, row, &src, &k);  // (the same address in every lane: one broadcast load)
-                for (u32 b = (u32)lane; b < k; b += 32u) P.out[w + b] = __ldg(src + b);
-                w += k;
-            }
-        }
-    }
-}
-void launch_bind_concat_gather(const BindConcatParams& p, int n_sms, cudaStream_t st) {
-    if (p.n == 0) return;
-    bind_concat_gather_kernel<<<bind_grid(p.n, n_sms), 256, 0, st>>>(p);
-}
-
-// =================================================================================================================
 // utilities
 __global__ void fill_kernel(u32* p, u32 v, u64 n) {
     for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) p[i] = v;
@@ -3725,21 +3242,20 @@ __global__ void __launch_bounds__(256) r2s_gone_write_kernel(const __grid_consta
             for (u32 c = 0; c < P.n_cols; c++) P.out_emit[c][at] = P.last.col[c][(u32)k];
     }
 }
-static int r2s_grid(u64 n, int n_sms) { return (int)umin64((u64)n_sms * 8ull, (n + 255ull) / 256ull); }
 void launch_r2s_build(const R2sParams& p, int n_sms, cudaStream_t st) {
-    if (p.cur.n) r2s_build_kernel<<<r2s_grid(p.cur.n, n_sms), 256, 0, st>>>(p);
+    if (p.cur.n) r2s_build_kernel<<<grid_1d(p.cur.n, n_sms), 256, 0, st>>>(p);
 }
 void launch_r2s_mark(const R2sParams& p, int n_sms, cudaStream_t st) {
-    if (p.cur.n) r2s_mark_kernel<<<r2s_grid(p.cur.n, n_sms), 256, 0, st>>>(p);
+    if (p.cur.n) r2s_mark_kernel<<<grid_1d(p.cur.n, n_sms), 256, 0, st>>>(p);
 }
 void launch_r2s_gone_mark(const R2sParams& p, int n_sms, cudaStream_t st) {
-    if (p.last.n) r2s_gone_mark_kernel<<<r2s_grid(p.last.n, n_sms), 256, 0, st>>>(p);
+    if (p.last.n) r2s_gone_mark_kernel<<<grid_1d(p.last.n, n_sms), 256, 0, st>>>(p);
 }
 void launch_r2s_write(const R2sParams& p, int n_sms, cudaStream_t st) {
-    if (p.cur.n) r2s_write_kernel<<<r2s_grid(p.cur.n, n_sms), 256, 0, st>>>(p);
+    if (p.cur.n) r2s_write_kernel<<<grid_1d(p.cur.n, n_sms), 256, 0, st>>>(p);
 }
 void launch_r2s_gone_write(const R2sParams& p, int n_sms, cudaStream_t st) {
-    if (p.last.n) r2s_gone_write_kernel<<<r2s_grid(p.last.n, n_sms), 256, 0, st>>>(p);
+    if (p.last.n) r2s_gone_write_kernel<<<grid_1d(p.last.n, n_sms), 256, 0, st>>>(p);
 }
 
 }  // namespace kb

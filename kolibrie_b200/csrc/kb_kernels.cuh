@@ -505,103 +505,23 @@ struct ShuffleParams {
 void launch_shuffle_scatter(const ShuffleParams& p, int n_sms, cudaStream_t st);
 
 // ---------------------------------------------------------------------------------------------------------------
-// id -> string decode of a result column (engine.rs:27-51): lengths, exclusive scan (launch_exclusive_scan_u32), byte gather
-// The quoted-triple table (kb_quoted_load): entry id & 0x7FFFFFFF -> (s, p, o); an empty slot holds EMPTY32 in all three columns.
+// The quoted-triple table (kb_quoted.cu): entry id & 0x7FFFFFFF -> (s, p, o); an empty slot holds EMPTY32 in all three columns.
 // n == 0: no table.
 struct QuotedTab {
     const u32 *s, *p, *o;
     u32 n;
 };
-// len[i] = length of the string of ids[i] ("unknown" = 7 bytes when the dictionary does not hold the id). A quoted id: without a table
-// *quoted = 1; with one, the length of `<< s p o >>` walked with a bounded stack (dictionary.rs:60-72), "unknown" when any id on the walk
-// is held by neither table, and *deep = 1 when the walk goes past KB_QUOTED_MAX_DEPTH levels first. *total += sum.
-// missing_empty: a term the tables do not hold renders as "" instead of "unknown" (decode_any(..).unwrap_or_default(), the serializers'
-// rule, sparql_database.rs:301-322).
-void launch_decode_lengths(const u32* ids, u32 n, const unsigned long long* dict_off, u32 dict_ids, const QuotedTab& qt, u32* len,
-                           unsigned long long* total, u32* quoted, u32* deep, int n_sms, cudaStream_t st, bool missing_empty = false);
-// out[off[i] .. off[i+1]) = bytes of the string of ids[i]; one warp per 32 rows, the lanes copy each dictionary string together; a quoted
-// row is written by its own thread, walking the term again (a missing term is 7 bytes, "unknown", or 0: either way shorter than the
-// 8 bytes of the shortest rendered quoted term)
-void launch_decode_gather(const u32* ids, u32 n, const unsigned long long* dict_off, const unsigned char* dict_bytes, u32 dict_ids, const QuotedTab& qt,
-                          const u32* off, unsigned char* out, int n_sms, cudaStream_t st);
-
-// ---------------------------------------------------------------------------------------------------------------
-// Quoted-triple match (kb_scan_quoted; match_term over QuotedTripleStore entries, engine.rs:1088-1107): ONE streaming pass over the
-// table's three columns, QM_TILE-entry tiles TMA-staged into shared memory (two stages), matches compacted with warp ballots (row order
-// unspecified). The inner pattern(s) are compiled into at most 6 checks on the entry's components.
-constexpr int QM_TILE = 1024, QM_THREADS = 256;
-enum QmCheck : u32 { QM_NONE = 0, QM_CONST = 1 /* comp == arg */, QM_EQ = 2 /* comp == component arg */, QM_QUOTED = 3 /* comp has bit 31 */ };
-struct QuotedMatchParams {
-    QuotedTab t;
-    u32 n_tiles;
-    u32 n_chk;
-    u32 chk_kind[6], chk_comp[6], chk_arg[6];  // check k: kind, component (0 s, 1 p, 2 o), argument
-    u32 n_out;                                 // 1 + inner variables
-    u32 out_comp[7];                           // component of output column c >= 1 (column 0 = entry id)
-    u32* out[7];                               // [t.n] each
-    u32* count;                                // zeroed: rows written
-    u32* ticket;                               // zeroed: tile counter
+// The device dictionary (kb_dict.cu): string of id i = bytes[off[i] .. off[i + 1]) for i < ids. ids == 0: no dictionary (null pointers).
+struct DictTab {
+    const unsigned long long* off;
+    const unsigned char* bytes;
+    u32 ids;
 };
-void launch_quoted_match(const QuotedMatchParams& p, int n_sms, cudaStream_t st);
-
-// ---------------------------------------------------------------------------------------------------------------
-// BIND built-ins (kb_bind, engine.rs:144-277). Every write pass takes `old` (the replaced column when the output variable was bound
-// already, else null): a row the reference does not insert into keeps old[i], or gets EMPTY32; *n_unbound += rows left EMPTY32.
-// SUBJECT / PREDICATE / OBJECT: out[i] = component `comp` of the table entry of arg[i] (a quoted id the table holds), else unbound
-void launch_bind_component(const u32* arg, u32 n, const QuotedTab& qt, u32 comp, const u32* old, u32* out, unsigned long long* n_unbound,
-                           int n_sms, cudaStream_t st);
-// isTRIPLE, pass 1: first[0] = min row whose argument is a quoted id, first[1] = min row whose argument is bound and not quoted
-// (first[] = EMPTY32 beforehand)
-void launch_bind_istriple_first(const u32* arg, u32 n, u32* first, int n_sms, cudaStream_t st);
-// isTRIPLE, pass 2: out[i] = id_true / id_false, unbound where the argument is
-void launch_bind_istriple_write(const u32* arg, u32 n, u32 id_true, u32 id_false, const u32* old, u32* out, unsigned long long* n_unbound,
-                                int n_sms, cudaStream_t st);
-// TRIPLE: QuotedTripleStore::encode of a batch, the kb_dict_encode scheme on a 96-bit key. The reverse index (s, p, o) -> table index is an
-// open-addressing table of (hash tag << 32 | index) entries, compared against the forward table on a tag match; the batch table keeps
-// (hash tag << 32 | smallest row) per new triple.
-struct BindTripleParams {
-    const u32* col[3];        // argument columns (null: the constant cval[k])
-    u32 cval[3];
-    u32 n;
-    QuotedTab qt;             // forward table: lookups compare against it
-    const u64* rev;           // reverse index (null: empty table)
-    u64 rev_mask;
-    u64* batch;               // all ~0 beforehand
-    u64 batch_mask;
-    u32* hit;                 // [n] id the table holds, else EMPTY32
-    u32* slot_of;             // [n] batch slot of a new triple's row, EMPTY32 for a hit or an unbound row
-    u32* first;               // [n + 1] 1 on the first row of every new triple; then its exclusive prefix (the rank)
-    u32* overflow;
-    u32 next_qt_id;           // the assign pass: ids next_qt_id + rank, entries written into ws / wp / wo at (next_qt_id & 0x7FFFFFFF) + rank
-    u32 *ws, *wp, *wo;
-    const u32* old;
-    u32* out;
-    unsigned long long* n_unbound;
-};
-void launch_bind_triple_resolve(const BindTripleParams& p, int n_sms, cudaStream_t st);
-void launch_bind_triple_mark(const BindTripleParams& p, int n_sms, cudaStream_t st);
-void launch_bind_triple_assign(const BindTripleParams& p, int n_sms, cudaStream_t st);
-// table indices [first, first + n) enter the reverse index (empty slots skipped; of two equal triples the index keeps the smaller)
-void launch_quoted_rev_insert(const QuotedTab& qt, u32 first, u32 n, u64* rev, u64 mask, u32* overflow, int n_sms, cudaStream_t st);
-// CONCAT: the pieces of row i are, per argument a, the dictionary string of col[a][i] ("" when the dictionary does not hold it) or the
-// constant cbytes[coff[a] .. coff[a] + clen[a])
-struct BindConcatParams {
-    u32 n, n_args;
-    const u32* col[KB_BIND_MAX_ARGS];  // null: a constant
-    u64 coff[KB_BIND_MAX_ARGS];
-    u32 clen[KB_BIND_MAX_ARGS];
-    const unsigned char* cbytes;
-    const unsigned long long* dict_off;
-    const unsigned char* dict_bytes;
-    u32 dict_ids;
-    u32* len;                          // lengths pass: [n + 1] (len[n] untouched); then their exclusive prefix
-    unsigned long long* total;         // lengths pass: += bytes of all rows
-    u64* off64;                        // gather pass: [n + 1] the prefix widened (the encode's offsets)
-    unsigned char* out;
-};
-void launch_bind_concat_lengths(const BindConcatParams& p, int n_sms, cudaStream_t st);
-// one warp per 32 rows: the lanes copy each piece of a row together (decode_gather's access pattern)
-void launch_bind_concat_gather(const BindConcatParams& p, int n_sms, cudaStream_t st);
+// a BIND write pass (kb_bind.cu, kb_quoted.cu): *n_unbound += the rows of the warp left unbound (every lane of the warp calls it)
+__device__ __forceinline__ void bind_count_unbound(bool unbound, unsigned long long* n_unbound) {
+    const unsigned b = __ballot_sync(0xffffffffu, unbound);
+    if ((threadIdx.x & 31) == 0 && b) atomicAdd(n_unbound, (unsigned long long)__popc(b));
+}
 
 // ---------------------------------------------------------------------------------------------------------------
 // Relation-to-Stream operators (kb_r2s_eval; Relation2StreamOperator::eval, r2s.rs:37-58). A set of rows is an open-addressing table

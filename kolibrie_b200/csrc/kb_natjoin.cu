@@ -120,7 +120,6 @@ __global__ void __launch_bounds__(256) keyed_index_kernel(u32* idx, u32 n) {
     for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) idx[i] = i;
 }
 
-int nj_grid(u64 n, int n_sms) { return (int)std::max<u64>(1, std::min<u64>((n + 255) / 256, (u64)n_sms * 8)); }
 
 // a view of rows [start, start + n) of the sorted side: the key columns of `key` (positions into the shared slots) plus the row index
 std::unique_ptr<kb_rel> group_view(const std::vector<u32>& shared, const std::vector<u32>& key, const std::vector<Buf>& keycols, const Buf& perm, u32 idx_slot,
@@ -169,7 +168,7 @@ kb_status natural_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_rel& R, std::
     KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + cw, 0, (2 + 4 * NJ_MASKS) * sizeof(u32), ctx->st));
     C.flags = ctx->ctrl + cw;
     timer_begin(ctx, F_OTHER);
-    natjoin_check_kernel<<<dim3(nj_grid(std::max(L.n, R.n), ctx->n_sms), 2), 256, 0, ctx->st>>>(C);
+    natjoin_check_kernel<<<dim3(grid_1d(std::max(L.n, R.n), ctx->n_sms), 2), 256, 0, ctx->st>>>(C);
     timer_end(ctx);
     KB_CUDA(ctx, cudaGetLastError());
     KB_TRY(ctrl_read(ctx));
@@ -193,7 +192,7 @@ kb_status natural_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_rel& R, std::
         for (u32 j = 0; j < M.n_u; j++) M.side[s].col[j] = C.side[s].col[U[j]];
     }
     timer_begin(ctx, F_OTHER);
-    natjoin_mask_kernel<<<dim3(nj_grid(std::max(L.n, R.n), ctx->n_sms), 2), 256, 0, ctx->st>>>(M);
+    natjoin_mask_kernel<<<dim3(grid_1d(std::max(L.n, R.n), ctx->n_sms), 2), 256, 0, ctx->st>>>(M);
     timer_end(ctx);
     KB_CUDA(ctx, cudaGetLastError());
     KB_TRY(ctrl_read(ctx));
@@ -226,7 +225,7 @@ kb_status natural_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_rel& R, std::
         S.n = (u32)side[s]->n;
     }
     timer_begin(ctx, F_OTHER);
-    natjoin_partition_kernel<<<dim3(nj_grid(std::max(L.n, R.n), ctx->n_sms), 2), 256, 0, ctx->st>>>(Pp);
+    natjoin_partition_kernel<<<dim3(grid_1d(std::max(L.n, R.n), ctx->n_sms), 2), 256, 0, ctx->st>>>(Pp);
     timer_end(ctx);
     KB_CUDA(ctx, cudaGetLastError());
 
@@ -276,7 +275,7 @@ kb_status natural_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_rel& R, std::
             Q.ri = s.rel->cols[s.rel->col_of(idx_slot[1])].ptr;
             Q.n = (u32)s.rel->n;
             Q.base = s.base;
-            natjoin_coalesce_kernel<<<nj_grid(s.rel->n, ctx->n_sms), 256, 0, ctx->st>>>(Q);
+            natjoin_coalesce_kernel<<<grid_1d(s.rel->n, ctx->n_sms), 256, 0, ctx->st>>>(Q);
         }
         timer_end(ctx);
         KB_CUDA(ctx, cudaGetLastError());
@@ -304,7 +303,7 @@ kb_status keyed_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_rel& R, const u
         KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + cw, 0, 2 * sizeof(u32), ctx->st));
         C.flags = ctx->ctrl + cw;
         timer_begin(ctx, F_OTHER);
-        natjoin_check_kernel<<<dim3(nj_grid(std::max(L.n, R.n), ctx->n_sms), 2), 256, 0, ctx->st>>>(C);
+        natjoin_check_kernel<<<dim3(grid_1d(std::max(L.n, R.n), ctx->n_sms), 2), 256, 0, ctx->st>>>(C);
         timer_end(ctx);
         KB_CUDA(ctx, cudaGetLastError());
         KB_TRY(ctrl_read(ctx));
@@ -324,7 +323,7 @@ kb_status keyed_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_rel& R, const u
         KB_TRY(alloc_buf(ctx, std::max<u64>(side[s]->n, 1) * sizeof(u32), &idx[s]));
         if (side[s]->n) {
             timer_begin(ctx, F_OTHER);
-            keyed_index_kernel<<<nj_grid(side[s]->n, ctx->n_sms), 256, 0, ctx->st>>>(static_cast<u32*>(idx[s]->p), (u32)side[s]->n);
+            keyed_index_kernel<<<grid_1d(side[s]->n, ctx->n_sms), 256, 0, ctx->st>>>(static_cast<u32*>(idx[s]->p), (u32)side[s]->n);
             timer_end(ctx);
             KB_CUDA(ctx, cudaGetLastError());
         }
@@ -361,7 +360,7 @@ kb_status keyed_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_rel& R, const u
         Q.ri = j->cols[j->col_of(idx_slot[1])].ptr;
         Q.n = (u32)j->n;
         timer_begin(ctx, F_OTHER);
-        natjoin_coalesce_kernel<<<nj_grid(j->n, ctx->n_sms), 256, 0, ctx->st>>>(Q);
+        natjoin_coalesce_kernel<<<grid_1d(j->n, ctx->n_sms), 256, 0, ctx->st>>>(Q);
         timer_end(ctx);
         KB_CUDA(ctx, cudaGetLastError());
     }

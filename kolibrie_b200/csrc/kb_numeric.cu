@@ -93,11 +93,6 @@ static kb_status numeric_grow(kb_ctx* ctx, Buf* a, Buf* b, size_t elem_a, u32 ke
     return KB_OK;
 }
 
-static int grid_for(u64 n, int n_sms, int threads, int per_sm) {
-    const u64 want = (n + threads - 1) / threads;
-    return (int)std::max<u64>(1, std::min<u64>(want, (u64)n_sms * per_sm));
-}
-
 // The value order V of the f64 table (kb_numrank.cuh): every value as an order-preserving u64 key (NaN as 0.0, -0.0 as +0.0, one extra
 // 0.0), a radix sort, the distinct keys, back to doubles; then the host copy that FILTER constants are resolved against. Run by the
 // index build for its rank columns, never by a query.
@@ -161,8 +156,9 @@ kb_status numeric_derive(kb_ctx* ctx, uint32_t tables, uint32_t first_id, kb_num
         const u32 c = ctrl_alloc(ctx, 4);
         KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + c, 0, 4 * sizeof(u32), ctx->st));
         NumDeriveParams P{};
-        P.off = static_cast<const unsigned long long*>(ctx->dict_off->p);
-        P.bytes = static_cast<const unsigned char*>(ctx->dict_bytes->p);
+        const DictTab dict = dicttab(ctx);
+        P.off = dict.off;
+        P.bytes = dict.bytes;
         P.lo = lo;
         P.n = n;
         if (F) { P.num = static_cast<double*>(ctx->num->p); P.isnum = static_cast<u8*>(ctx->isnum->p); P.first_f = first_f; }
@@ -170,7 +166,7 @@ kb_status numeric_derive(kb_ctx* ctx, uint32_t tables, uint32_t first_id, kb_num
         P.slow = static_cast<u32*>(slow->p);
         P.ctr = ctx->ctrl + c;
         timer_begin(ctx, F_OTHER, 1);
-        numeric_derive_kernel<<<grid_for(n - lo, ctx->n_sms, 256, 8), 256, 0, ctx->st>>>(P);
+        numeric_derive_kernel<<<grid_1d(n - lo, ctx->n_sms), 256, 0, ctx->st>>>(P);
         timer_end(ctx);
         KB_CUDA(ctx, cudaGetLastError());
         KB_TRY(ctrl_read(ctx));
@@ -179,7 +175,7 @@ kb_status numeric_derive(kb_ctx* ctx, uint32_t tables, uint32_t first_id, kb_num
         n_i32 = ctx->h_ctrl[c + 2];
         if (n_slow) {
             timer_begin(ctx, F_OTHER, 1);
-            numeric_slow_kernel<<<grid_for(n_slow, ctx->n_sms, 128, 4), 128, 0, ctx->st>>>(P.off, P.bytes, P.slow, n_slow, P.num);
+            numeric_slow_kernel<<<grid_1d(n_slow, ctx->n_sms, 128, 4), 128, 0, ctx->st>>>(P.off, P.bytes, P.slow, n_slow, P.num);
             timer_end(ctx);
             KB_CUDA(ctx, cudaGetLastError());
         }

@@ -208,19 +208,6 @@ __global__ void __launch_bounds__(OT) order_gather_kernel(const __grid_constant_
     }
 }
 
-int grid_of(u64 n, int n_sms) { return (int)std::max<u64>(1, std::min<u64>((n + OT - 1) / OT, (u64)n_sms * 8)); }
-u32 bits_of(u64 x) { return x ? 64u - (u32)__builtin_clzll(x) : 0u; }
-
-// one CUB device call: size query, scratch, call
-template <class F>
-kb_status cub_run(kb_ctx* ctx, F f) {
-    size_t t = 0;
-    KB_CUDA(ctx, f(nullptr, t));
-    Buf b;
-    KB_TRY(alloc_buf(ctx, std::max<size_t>(t, 16), &b));
-    KB_CUDA(ctx, f(b->p, t));
-    return KB_OK;
-}
 
 struct MaxOp {
     __device__ __forceinline__ u32 operator()(u32 a, u32 b) const { return a > b ? a : b; }
@@ -242,7 +229,7 @@ kb_status rank_values(kb_ctx* ctx, u32 d, const unsigned long long* nkey, const 
     KB_TRY(alloc_buf(ctx, (size_t)d * 8, &key));
     KB_TRY(alloc_buf(ctx, (size_t)d * 8, &key2));
     KB_TRY(alloc_buf(ctx, d, &more));
-    const int g = grid_of(d, ctx->n_sms);
+    const int g = grid_1d(d, ctx->n_sms);
     auto U = [](Buf& b) { return static_cast<u32*>(b->p); };
     timer_begin(ctx, F_OTHER, 2);
     iota_kernel<<<g, OT, 0, ctx->st>>>(U(ord), d);
@@ -257,7 +244,7 @@ kb_status rank_values(kb_ctx* ctx, u32 d, const unsigned long long* nkey, const 
         P.str_off = str_off; P.bytes = bytes; P.nkey = nkey; P.round = r;
         P.key = static_cast<unsigned long long*>(key->p); P.gkey = U(gkey); P.s_of = U(s_of); P.idx = U(idx);
         unsigned long long* k2 = static_cast<unsigned long long*>(key2->p);
-        const int gm = grid_of(m, ctx->n_sms);
+        const int gm = grid_1d(m, ctx->n_sms);
         timer_begin(ctx, F_OTHER, 4);
         refine_prep_kernel<<<gm, OT, 0, ctx->st>>>(P);
         KB_TRY(cub_run(ctx, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, P.key, k2, P.idx, U(idx2), m, 0, 64, ctx->st); }));
@@ -319,13 +306,14 @@ kb_status rank_key(kb_ctx* ctx, const kb_rel& in, u32 col, bool desc, KeyRank* k
     P.num = ctx->num ? static_cast<const double*>(ctx->num->p) : nullptr;
     P.isnum = ctx->isnum ? static_cast<const u8*>(ctx->isnum->p) : nullptr;
     P.n_ids = P.num ? ctx->n_ids : 0u;
-    P.dict_off = ctx->dict_ids ? static_cast<const unsigned long long*>(ctx->dict_off->p) : nullptr;
-    P.dict_ids = ctx->dict_ids;
+    const DictTab dict = dicttab(ctx);
+    P.dict_off = dict.off;
+    P.dict_ids = dict.ids;
     P.quoted_slots = ctx->quoted_slots;
     P.key = static_cast<unsigned long long*>(nkey->p);
     P.ctr = ctx->ctrl + c + 4;
     timer_begin(ctx, F_OTHER, 1);
-    order_classify_kernel<<<grid_of(d, ctx->n_sms), OT, 0, ctx->st>>>(P);
+    order_classify_kernel<<<grid_1d(d, ctx->n_sms, OT), OT, 0, ctx->st>>>(P);
     timer_end(ctx);
     KB_CUDA(ctx, cudaGetLastError());
     KB_TRY(ctrl_read(ctx));
@@ -343,32 +331,10 @@ kb_status rank_key(kb_ctx* ctx, const kb_rel& in, u32 col, bool desc, KeyRank* k
         KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
         ctx->stats.d2h_bytes += sizeof(u32);
         const u32 dr = none == EMPTY32 ? d - 1 : d;
-        Buf off, scratch, bytes;
-        KB_TRY(alloc_buf(ctx, ((size_t)d + 1) * 4, &off));
-        KB_TRY(alloc_buf(ctx, (((size_t)d + 1) / 2048 + 4) * 4, &scratch));
-        u32* d_off = static_cast<u32*>(off->p);
-        KB_CUDA(ctx, cudaMemsetAsync(d_off + dr, 0, ((size_t)d - dr + 1) * 4, ctx->st));
-        const u32 cd = ctrl_alloc(ctx, 4);  // [0..1] u64 total bytes, [2] quoted id without a table, [3] walk too deep
-        KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + cd, 0, 4 * sizeof(u32), ctx->st));
-        const QuotedTab qt = quotedtab(ctx);
-        const auto* dbytes = static_cast<const unsigned char*>(ctx->dict_bytes->p);
-        timer_begin(ctx, F_OTHER, 4);
-        launch_decode_lengths(d_uniq, dr, P.dict_off, ctx->dict_ids, qt, d_off, reinterpret_cast<unsigned long long*>(ctx->ctrl + cd), ctx->ctrl + cd + 2,
-                              ctx->ctrl + cd + 3, ctx->n_sms, ctx->st);
-        launch_exclusive_scan_u32(d_off, d + 1, static_cast<u32*>(scratch->p), ctx->st);
-        timer_end(ctx);
-        KB_CUDA(ctx, cudaGetLastError());
-        KB_TRY(ctrl_read(ctx));
-        unsigned long long total = 0;
-        memcpy(&total, ctx->h_ctrl + cd, sizeof total);
-        if (ctx->h_ctrl[cd + 3]) return fail(ctx, KB_E_LIMIT, "a quoted-triple term nests deeper than %d levels", KB_QUOTED_MAX_DEPTH);
-        if (total > 0xFFFFFFFFull) return fail(ctx, KB_E_LIMIT, "the distinct values of an ORDER BY key take %llu bytes (limit 2^32-1)", total);
-        KB_TRY(alloc_buf(ctx, (size_t)total + 16, &bytes));
-        timer_begin(ctx, F_OTHER, 1);
-        launch_decode_gather(d_uniq, dr, P.dict_off, dbytes, ctx->dict_ids, qt, d_off, static_cast<unsigned char*>(bytes->p), ctx->n_sms, ctx->st);
-        timer_end(ctx);
-        KB_CUDA(ctx, cudaGetLastError());
-        KB_TRY(rank_values(ctx, d, nullptr, d_off, static_cast<const u8*>(bytes->p), static_cast<u32*>(rank_of->p), &kr->n_values, &kr->rounds));
+        Buf off, bytes;
+        KB_TRY(decode_ids(ctx, d_uniq, dr, d - dr, false, "the ORDER BY column", &off, &bytes, nullptr));
+        KB_TRY(rank_values(ctx, d, nullptr, static_cast<const u32*>(off->p), static_cast<const u8*>(bytes->p), static_cast<u32*>(rank_of->p), &kr->n_values,
+                           &kr->rounds));
         kr->kind = KB_ORDER_STRING;
     } else {
         u32 rounds = 0;
@@ -378,7 +344,7 @@ kb_status rank_key(kb_ctx* ctx, const kb_rel& in, u32 col, bool desc, KeyRank* k
     if (kr->n_values <= 1) kr->kind = KB_ORDER_CONST;
     KB_TRY(alloc_buf(ctx, (size_t)n * 4, &kr->rank));
     timer_begin(ctx, F_OTHER, 1);
-    row_rank_kernel<<<grid_of(n, ctx->n_sms), OT, 0, ctx->st>>>(ids, n, d_uniq, d, static_cast<const u32*>(rank_of->p), desc ? kr->n_values - 1u : 0u,
+    row_rank_kernel<<<grid_1d(n, ctx->n_sms, OT), OT, 0, ctx->st>>>(ids, n, d_uniq, d, static_cast<const u32*>(rank_of->p), desc ? kr->n_values - 1u : 0u,
                                                                  static_cast<u32*>(kr->rank->p));
     timer_end(ctx);
     KB_CUDA(ctx, cudaGetLastError());
@@ -423,7 +389,7 @@ static kb_status order_by_impl(kb_ctx* ctx, const kb_rel& in, const kb_order_key
     auto U = [](const Buf& b) { return static_cast<u32*>(b->p); };
     Buf order;  // row indices in sorted order, n_out of them
     const u32 nk = (u32)sort_keys.size();
-    const int g = grid_of(n, ctx->n_sms);
+    const int g = grid_1d(n, ctx->n_sms);
     if (limit > 0 && nk <= 2 && (u64)limit * ORDER_TOPK_RATIO <= n) {
         // top-k: T = the k-th smallest packed key; rows below T sorted, then the first rows equal to T in input order
         info->route = KB_ORDER_TOPK;
@@ -509,7 +475,7 @@ static kb_status order_by_impl(kb_ctx* ctx, const kb_rel& in, const kb_order_key
     for (u32 c = 0; c < G.n_cols; c++) { G.in[c] = in.cols[c].ptr; G.out[c] = r->cols[c].ptr; }
     if (n_out) {
         timer_begin(ctx, F_OTHER, 1);
-        order_gather_kernel<<<grid_of(n_out, ctx->n_sms), OT, 0, ctx->st>>>(G);
+        order_gather_kernel<<<grid_1d(n_out, ctx->n_sms, OT), OT, 0, ctx->st>>>(G);
         timer_end(ctx);
     }
     KB_CUDA(ctx, cudaGetLastError());

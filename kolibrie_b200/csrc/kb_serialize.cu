@@ -48,18 +48,6 @@ constexpr int ST = 256;  // threads per block of every kernel here
 enum : u8 { TC_QUOTED = 1, TC_IRI = 2 };                   // term class: text starts with "<<"; with "http://" or "https://"
 enum : u8 { SF_SUBJ = 1, SF_PRED = 2, SF_SUBJ_END = 4 };  // unit flags: first of its subject group, of its predicate group; last of its subject group
 
-int grid_of(u64 n, int n_sms) { return (int)std::max<u64>(1, std::min<u64>((n + ST - 1) / ST, (u64)n_sms * 8)); }
-u32 bits_of(u64 x) { return x ? 64u - (u32)__builtin_clzll(x) : 0u; }
-
-template <class F>
-kb_status cub_run(kb_ctx* ctx, F f) {
-    size_t t = 0;
-    KB_CUDA(ctx, f(nullptr, t));
-    Buf b;
-    KB_TRY(alloc_buf(ctx, std::max<size_t>(t, 16), &b));
-    KB_CUDA(ctx, f(b->p, t));
-    return KB_OK;
-}
 
 __global__ void __launch_bounds__(ST) ser_load_kernel(const u32* __restrict__ s, const u32* __restrict__ p, const u32* __restrict__ o, u64 n,
                                                       u32* __restrict__ S, unsigned long long* __restrict__ PO) {
@@ -303,7 +291,7 @@ kb_status serialize_begin(kb_ctx* ctx, u32 format, const u64* poff, const u8* pb
             if (!sg.n) continue;
             if (sg.ready) KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st, sg.ready, 0));
             timer_begin(ctx, F_OTHER, 1);
-            ser_load_kernel<<<grid_of(sg.n, ctx->n_sms), ST, 0, ctx->st>>>(sg.s.ptr, sg.p.ptr, sg.o.ptr, sg.n, U(S) + at, U64(PO) + at);
+            ser_load_kernel<<<grid_1d(sg.n, ctx->n_sms, ST), ST, 0, ctx->st>>>(sg.s.ptr, sg.p.ptr, sg.o.ptr, sg.n, U(S) + at, U64(PO) + at);
             timer_end(ctx);
             at += sg.n;
         }
@@ -317,7 +305,7 @@ kb_status serialize_begin(kb_ctx* ctx, u32 format, const u64* poff, const u8* pb
     KB_TRY(alloc_buf(ctx, n_raw, &keep));
     const u32 c = ctrl_alloc(ctx, 4);  // [0] distinct triples, [1] distinct terms
     timer_begin(ctx, F_OTHER, 3);
-    ser_distinct_flags_kernel<<<grid_of(nr, ctx->n_sms), ST, 0, ctx->st>>>(U(S), U64(PO), nr, static_cast<u8*>(keep->p));
+    ser_distinct_flags_kernel<<<grid_1d(nr, ctx->n_sms, ST), ST, 0, ctx->st>>>(U(S), U64(PO), nr, static_cast<u8*>(keep->p));
     KB_TRY(cub_run(ctx, [&](void* t, size_t& b) {
         return cub::DeviceSelect::Flagged(t, b, U(S), static_cast<const u8*>(keep->p), U(S2), ctx->ctrl + c, nr, ctx->st);
     }));
@@ -339,7 +327,7 @@ kb_status serialize_begin(kb_ctx* ctx, u32 format, const u64* poff, const u8* pb
     KB_TRY(alloc_buf(ctx, n3 * 4, &sorted_ids));
     KB_TRY(alloc_buf(ctx, n3 * 4, &terms));
     timer_begin(ctx, F_OTHER, 3);
-    ser_ids_kernel<<<grid_of(n, ctx->n_sms), ST, 0, ctx->st>>>(U(S2), U64(PO2), n, U(ids));
+    ser_ids_kernel<<<grid_1d(n, ctx->n_sms, ST), ST, 0, ctx->st>>>(U(S2), U64(PO2), n, U(ids));
     KB_TRY(cub_run(ctx, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortKeys(t, b, U(ids), U(sorted_ids), (u32)n3, 0, 32, ctx->st); }));
     KB_TRY(cub_run(ctx, [&](void* t, size_t& b) { return cub::DeviceSelect::Unique(t, b, U(sorted_ids), U(terms), ctx->ctrl + c + 1, (u32)n3, ctx->st); }));
     timer_end(ctx);
@@ -348,34 +336,13 @@ kb_status serialize_begin(kb_ctx* ctx, u32 format, const u64* poff, const u8* pb
     KB_TRY(ctrl_read(ctx));
     const u32 nu = ctx->h_ctrl[c + 1];
     info->n_terms = nu;
-    KB_TRY(alloc_buf(ctx, ((size_t)nu + 1) * 4, &ser->toff));
-    Buf scratch;
-    KB_TRY(alloc_buf(ctx, (((size_t)nu + 1) / 2048 + 4) * 4, &scratch));
-    KB_CUDA(ctx, cudaMemsetAsync(U(ser->toff) + nu, 0, 4, ctx->st));
-    const u32 cd = ctrl_alloc(ctx, 4);  // [0..1] u64 total bytes, [2] quoted id without a table, [3] walk too deep
-    const auto* dict_off = static_cast<const unsigned long long*>(ctx->dict_off->p);
-    const QuotedTab qt = quotedtab(ctx);
-    timer_begin(ctx, F_OTHER, 2);
-    launch_decode_lengths(U(terms), nu, dict_off, ctx->dict_ids, qt, U(ser->toff), reinterpret_cast<unsigned long long*>(ctx->ctrl + cd), ctx->ctrl + cd + 2,
-                          ctx->ctrl + cd + 3, ctx->n_sms, ctx->st, true);
-    launch_exclusive_scan_u32(U(ser->toff), nu + 1, U(scratch), ctx->st);
-    timer_end(ctx);
-    KB_CUDA(ctx, cudaGetLastError());
-    KB_TRY(ctrl_read(ctx));
-    unsigned long long total = 0;
-    memcpy(&total, ctx->h_ctrl + cd, sizeof total);
-    if (ctx->h_ctrl[cd + 2]) return fail(ctx, KB_E_UNSUPPORTED, "the store holds quoted-triple ids (bit 31) and no quoted-triple table is loaded (kb_quoted_load)");
-    if (ctx->h_ctrl[cd + 3]) return fail(ctx, KB_E_LIMIT, "a quoted-triple term nests deeper than %d levels", KB_QUOTED_MAX_DEPTH);
-    if (total > 0xFFFFFFFFull) return fail(ctx, KB_E_LIMIT, "the distinct terms of the store render to %llu bytes (limit 2^32-1)", total);
-    KB_TRY(alloc_buf(ctx, (size_t)total + 16, &ser->tbytes));
+    KB_TRY(decode_ids(ctx, U(terms), nu, 0, true, "the store", &ser->toff, &ser->tbytes, nullptr));
     KB_TRY(alloc_buf(ctx, (size_t)nu + 16, &ser->tcls));
     u8* tbytes = static_cast<u8*>(ser->tbytes->p);
     u8* tcls = static_cast<u8*>(ser->tcls->p);
-    timer_begin(ctx, F_OTHER, 3);
-    launch_decode_gather(U(terms), nu, dict_off, static_cast<const unsigned char*>(ctx->dict_bytes->p), ctx->dict_ids, qt, U(ser->toff), tbytes, ctx->n_sms,
-                         ctx->st);
-    ser_class_kernel<<<grid_of(nu, ctx->n_sms), ST, 0, ctx->st>>>(U(ser->toff), tbytes, nu, tcls);
-    ser_term_index_kernel<<<grid_of(n3, ctx->n_sms), ST, 0, ctx->st>>>(U(ids), n3, U(terms), nu);
+    timer_begin(ctx, F_OTHER, 2);
+    ser_class_kernel<<<grid_1d(nu, ctx->n_sms, ST), ST, 0, ctx->st>>>(U(ser->toff), tbytes, nu, tcls);
+    ser_term_index_kernel<<<grid_1d(n3, ctx->n_sms, ST), ST, 0, ctx->st>>>(U(ids), n3, U(terms), nu);
     timer_end(ctx);
     KB_CUDA(ctx, cudaGetLastError());
     terms.reset();
@@ -398,11 +365,11 @@ kb_status serialize_begin(kb_ctx* ctx, u32 format, const u64* poff, const u8* pb
         KB_TRY(alloc_buf(ctx, n3 * 4, &placed));
         KB_TRY(alloc_buf(ctx, (size_t)n + 16, &ser->flags));
         timer_begin(ctx, F_OTHER, 3);
-        ser_group_key_kernel<<<grid_of(n, ctx->n_sms), ST, 0, ctx->st>>>(ts, tp, n, U(rank_of), rb, U64(key), U(idx));
+        ser_group_key_kernel<<<grid_1d(n, ctx->n_sms, ST), ST, 0, ctx->st>>>(ts, tp, n, U(rank_of), rb, U64(key), U(idx));
         KB_TRY(cub_run(ctx, [&](void* t, size_t& b) {
             return cub::DeviceRadixSort::SortPairs(t, b, U64(key), U64(key2), U(idx), U(idx2), n, 0, (int)(2 * rb), ctx->st);
         }));
-        ser_group_place_kernel<<<grid_of(n, ctx->n_sms), ST, 0, ctx->st>>>(U64(key2), U(idx2), n, rb, ts, tp, to, U(placed), U(placed) + n,
+        ser_group_place_kernel<<<grid_1d(n, ctx->n_sms, ST), ST, 0, ctx->st>>>(U64(key2), U(idx2), n, rb, ts, tp, to, U(placed), U(placed) + n,
                                                                            U(placed) + 2ull * n, static_cast<u8*>(ser->flags->p));
         timer_end(ctx);
         KB_CUDA(ctx, cudaGetLastError());
@@ -420,7 +387,7 @@ kb_status serialize_begin(kb_ctx* ctx, u32 format, const u64* poff, const u8* pb
     UnitParams P{ts, tp, to, turtle ? static_cast<const u8*>(ser->flags->p) : nullptr, U(ser->toff), tcls, n};
     KB_CUDA(ctx, cudaMemsetAsync(U64(ser->uoff) + n, 0, 8, ctx->st));
     timer_begin(ctx, F_OTHER, 2);
-    ser_unit_len_kernel<<<grid_of(n, ctx->n_sms), ST, 0, ctx->st>>>(P, U64(ser->uoff), reinterpret_cast<unsigned long long*>(ctx->ctrl + cu), ctx->ctrl + cu + 2);
+    ser_unit_len_kernel<<<grid_1d(n, ctx->n_sms, ST), ST, 0, ctx->st>>>(P, U64(ser->uoff), reinterpret_cast<unsigned long long*>(ctx->ctrl + cu), ctx->ctrl + cu + 2);
     KB_TRY(cub_run(ctx, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, U64(ser->uoff), U64(ser->uoff), n + 1, ctx->st); }));
     timer_end(ctx);
     pt.mark(ctx->st);
@@ -478,7 +445,7 @@ kb_status serialize_next(kb_ctx* ctx, kb_serializer* ser, u8* dst, u64 capacity,
             if (u1 == ser->cursor) break;  // the next unit does not fit what is left of `capacity`
             const u32 m = (u32)(u1 - ser->cursor);
             timer_begin(ctx, F_OTHER, 1);
-            ser_write_kernel<<<grid_of((u64)m * 32, ctx->n_sms), ST, 0, ctx->st>>>(P, static_cast<const u8*>(ser->tbytes->p), uoff, ser->cursor, m,
+            ser_write_kernel<<<grid_1d((u64)m * 32, ctx->n_sms, ST), ST, 0, ctx->st>>>(P, static_cast<const u8*>(ser->tbytes->p), uoff, ser->cursor, m,
                                                                                   static_cast<u8*>(staging->p));
             timer_end(ctx);
             KB_CUDA(ctx, cudaGetLastError());

@@ -62,8 +62,6 @@ __global__ void __launch_bounds__(256) values_scatter_kernel(const __grid_consta
     }
 }
 
-int values_grid(u64 n, int n_sms) { return (int)std::max<u64>(1, std::min<u64>((n + 255) / 256, (u64)n_sms * 8)); }
-
 }  // namespace
 }  // namespace kb
 
@@ -135,7 +133,7 @@ kb_status kb_values(kb_ctx* ctx, const uint32_t* slots, uint32_t n_vars, uint64_
     KB_CUDA(ctx, cudaMemsetAsync(P.cell_rank + n_cells, 0, sizeof(u32), ctx->st));
     KB_CUDA(ctx, cudaMemsetAsync(P.row_rank + nr, 0, sizeof(u32), ctx->st));
     timer_begin(ctx, F_OTHER, 3);
-    values_flag_kernel<<<values_grid(nr, ctx->n_sms), 256, 0, ctx->st>>>(P);
+    values_flag_kernel<<<grid_1d(nr, ctx->n_sms), 256, 0, ctx->st>>>(P);
     launch_exclusive_scan_u32(P.cell_rank, (u32)n_cells + 1, static_cast<u32*>(scratch->p), ctx->st);
     launch_exclusive_scan_u32(P.row_rank, nr + 1, static_cast<u32*>(scratch->p), ctx->st);
     timer_end(ctx);
@@ -153,7 +151,7 @@ kb_status kb_values(kb_ctx* ctx, const uint32_t* slots, uint32_t n_vars, uint64_
     P.enc_off = static_cast<u64*>(enc_off->p);
     P.ids = static_cast<const u32*>(ids->p);
     timer_begin(ctx, F_OTHER);
-    values_compact_kernel<<<values_grid(n_cells + 1, ctx->n_sms), 256, 0, ctx->st>>>(P);
+    values_compact_kernel<<<grid_1d(n_cells + 1, ctx->n_sms), 256, 0, ctx->st>>>(P);
     timer_end(ctx);
     KB_CUDA(ctx, cudaGetLastError());
     u32 n_new = 0;
@@ -171,7 +169,7 @@ kb_status kb_values(kb_ctx* ctx, const uint32_t* slots, uint32_t n_vars, uint64_
     }
     if (n_kept) {
         timer_begin(ctx, F_OTHER);
-        values_scatter_kernel<<<values_grid(nr, ctx->n_sms), 256, 0, ctx->st>>>(P);
+        values_scatter_kernel<<<grid_1d(nr, ctx->n_sms), 256, 0, ctx->st>>>(P);
         timer_end(ctx);
         KB_CUDA(ctx, cudaGetLastError());
     }
