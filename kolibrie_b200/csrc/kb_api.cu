@@ -303,293 +303,11 @@ kb_status check_pattern(kb_ctx* ctx, const kb_pattern& pt) {
     return KB_OK;
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// scan
-kb_status unpair_rel(kb_ctx* ctx, std::unique_ptr<kb_rel>* r) {
-    if (!(*r)->pair) return KB_OK;
-    auto c = std::make_unique<kb_rel>();
-    c->slots = (*r)->slots;
-    c->n = (*r)->n;
-    Col x, y;
-    KB_TRY(alloc_col(ctx, c->n, &x));
-    KB_TRY(alloc_col(ctx, c->n, &y));
-    timer_begin(ctx, F_OTHER);
-    launch_unpair(reinterpret_cast<const uint2*>((*r)->cols[0].ptr), (u32)c->n, x.ptr, y.ptr, ctx->st);
-    timer_end(ctx);
-    KB_CUDA(ctx, cudaGetLastError());
-    c->cols = {x, y};
-    *r = std::move(c);
-    return KB_OK;
-}
-
 kb_status empty_rel(kb_ctx* ctx, const std::vector<u32>& slots, std::unique_ptr<kb_rel>* out) {
     auto r = std::make_unique<kb_rel>();
     r->slots = slots;
     for (size_t c = 0; c < slots.size(); c++) { Col col; KB_TRY(alloc_col(ctx, 0, &col)); r->cols.push_back(col); }
     *out = std::move(r);
-    return KB_OK;
-}
-
-// IndexScan proper (engine.rs:1192-1407, the 8-case lookup of index_manager.rs:253-340 for a constant predicate): with a valid store
-// index a pattern whose predicate is constant is answered from the predicate's slice — (c P ?o) from the subject table / directory,
-// (?s P c) from the object table / directory, (?s P ?o) is the slice itself — without touching the 12-byte/triple store.
-// *out stays null when the index cannot answer the pattern (the caller scans).
-static kb_status index_lookup(kb_ctx* ctx, const kb_pattern& pt, std::unique_ptr<kb_rel>* out) {
-    out->reset();
-    if (!ctx->use_index || ctx->index_version != ctx->store_version || pt.p.is_var) return KB_OK;
-    std::vector<u32> slots, src;
-    pattern_vars(pt, &slots, &src);
-    auto it = ctx->index.find(pt.p.value);
-    if (it == ctx->index.end() || it->second.n == 0) return empty_rel(ctx, slots, out);  // the predicate does not occur: empty answer
-    auto rel = std::make_unique<kb_rel>();
-    rel->slots = slots;
-    const PredSlice& ps = it->second;
-    if (pt.s.is_var && pt.o.is_var) {
-        if (pt.s.value == pt.o.value) return KB_OK;  // ?x P ?x: the scan enforces the equality
-        Col x, y;  // the slice itself, de-interleaved (all chunks)
-        KB_TRY(alloc_col(ctx, ps.n, &x));
-        KB_TRY(alloc_col(ctx, ps.n, &y));
-        u64 at = 0;
-        timer_begin(ctx, F_SCAN, (int)ps.chunks.size());
-        for (auto& ch : ps.chunks) {
-            // (chunk boundaries keep 16-byte alignment only by luck: unpair writes element-wise, no TMA on the output side)
-            launch_unpair(reinterpret_cast<const uint2*>(ch.pairs.ptr), (u32)ch.n, x.ptr + at, y.ptr + at, ctx->st);
-            at += ch.n;
-        }
-        timer_end(ctx);
-        KB_CUDA(ctx, cudaGetLastError());
-        rel->cols = {x, y};
-        rel->n = ps.n;
-        ctx->stats.index_joins++;
-        *out = std::move(rel);
-        return KB_OK;
-    }
-    if (pt.s.is_var == pt.o.is_var) return KB_OK;  // both constant: left to the scan
-    const bool by_y = !pt.o.is_var;                // the bound position is the object
-    const u32 key = by_y ? pt.o.value : pt.s.value;
-    const Buf& tab = by_y ? ps.ytab : ps.xtab;
-    const Buf& off = by_y ? ps.yoff : ps.xoff;
-    const Buf& val = by_y ? ps.yval : ps.xval;
-    if (tab) {  // unique column: one table slot
-        const u32 cs = by_y ? 0u : ps.tab_cshift;
-        if (cs != 0u && shard_of(key, ctx->shard_world) != ctx->shard_rank) return empty_rel(ctx, slots, out);  // a key of another shard: not in this store
-        const u32 o = compact_key(key, cs) - (by_y ? ps.ytab_min : ps.xtab_min);
-        u32 v = EMPTY32;
-        if (o < (by_y ? ps.ytab_range : ps.xtab_range)) {
-            KB_CUDA(ctx, cudaMemcpyAsync(&v, static_cast<const u32*>(tab->p) + o, sizeof(u32), cudaMemcpyDeviceToHost, ctx->st));
-            KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
-            ctx->stats.d2h_bytes += 4;
-        }
-        Col col;
-        KB_TRY(alloc_col(ctx, v == EMPTY32 ? 0 : 1, &col));
-        if (v != EMPTY32) KB_CUDA(ctx, cudaMemcpyAsync(col.ptr, &v, sizeof(u32), cudaMemcpyHostToDevice, ctx->st));
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
-        rel->cols.push_back(col);
-        rel->n = v == EMPTY32 ? 0 : 1;
-        ctx->stats.index_joins++;
-        *out = std::move(rel);
-        return KB_OK;
-    }
-    if (off && val) {  // multi-valued column: the key's run in the directory
-        const u32 kmin = by_y ? ps.ycsr_min : ps.xcsr_min, range = by_y ? ps.ycsr_range : ps.xcsr_range;
-        u32 be[2] = {0, 0};
-        if (key >= kmin && key - kmin < range) {
-            KB_CUDA(ctx, cudaMemcpyAsync(be, static_cast<const u32*>(off->p) + (key - kmin), 2 * sizeof(u32), cudaMemcpyDeviceToHost, ctx->st));
-            KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
-            ctx->stats.d2h_bytes += 8;
-        }
-        const u64 n = be[1] - be[0];
-        Col col;
-        if ((be[0] & 3u) == 0 && n) {  // 16-byte aligned run: a view of the directory's values, no copy
-            col.buf = val;
-            col.ptr = static_cast<u32*>(val->p) + be[0];
-        } else {
-            KB_TRY(alloc_col(ctx, n, &col));
-            if (n) KB_CUDA(ctx, cudaMemcpyAsync(col.ptr, static_cast<const u32*>(val->p) + be[0], n * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
-        }
-        rel->cols.push_back(col);
-        rel->n = n;
-        ctx->stats.index_joins++;
-        *out = std::move(rel);
-        return KB_OK;
-    }
-    return KB_OK;
-}
-
-kb_status scan_impl(kb_ctx* ctx, const std::vector<Segment>& segs, const kb_pattern* pats, u32 K, const std::vector<FilterProg>& pushdown,
-                    bool use_index, bool row_index, bool pairs, std::vector<std::unique_ptr<kb_rel>>* out, const std::vector<ScanTable>* tables) {
-    if (K == 0 || K > (u32)MAXP) return fail(ctx, KB_E_LIMIT, "a fused scan takes 1..%d patterns (got %u)", MAXP, K);
-    if (use_index && &segs == &ctx->segs && !row_index && !pairs && !tables && ctx->use_index && ctx->index_version == ctx->store_version) {
-        // patterns the index answers are not scanned; the rest (if any) go through one fused scan
-        std::vector<std::unique_ptr<kb_rel>> got(K);
-        std::vector<u32> rest;
-        for (u32 k = 0; k < K; k++) {
-            KB_TRY(check_pattern(ctx, pats[k]));
-            KB_TRY(index_lookup(ctx, pats[k], &got[k]));
-            if (!got[k]) { rest.push_back(k); continue; }
-            if (k < pushdown.size() && !pushdown[k].ops.empty()) {  // the pattern's own FILTER, applied to the looked-up rows
-                std::unique_ptr<kb_rel> f;
-                KB_TRY(filter_impl(ctx, *got[k], pushdown[k], &f));
-                got[k] = std::move(f);
-            }
-        }
-        if (rest.size() < K) {
-            if (!rest.empty()) {
-                std::vector<kb_pattern> rp;
-                std::vector<FilterProg> rf;
-                for (u32 k : rest) { rp.push_back(pats[k]); rf.push_back(k < pushdown.size() ? pushdown[k] : FilterProg{}); }
-                std::vector<std::unique_ptr<kb_rel>> sub;
-                KB_TRY(scan_impl(ctx, segs, rp.data(), (u32)rp.size(), rf, /*use_index=*/false, false, false, &sub));
-                for (size_t i = 0; i < rest.size(); i++) got[rest[i]] = std::move(sub[i]);
-            }
-            out->clear();
-            for (u32 k = 0; k < K; k++) out->push_back(std::move(got[k]));
-            return KB_OK;
-        }
-    }
-    u64 N = 0;
-    for (auto& sg : segs) N += sg.n;
-    if (N >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "store holds %llu triples; row positions are 32-bit", (unsigned long long)N);
-    ScanParams P{};
-    P.K = K;
-    P.nt = numtab(ctx);
-    std::vector<FilterOp> ops;
-    out->clear();
-    for (u32 k = 0; k < K; k++) {
-        KB_TRY(check_pattern(ctx, pats[k]));
-        const kb_pattern& pt = pats[k];
-        ScanPat& sp = P.pat[k];
-        sp.flags = 0;
-        if (!pt.s.is_var) { sp.flags |= SP_HAS_S; sp.cs = pt.s.value; }
-        if (!pt.p.is_var) { sp.flags |= SP_HAS_P; sp.cp = pt.p.value; }
-        if (!pt.o.is_var) { sp.flags |= SP_HAS_O; sp.co = pt.o.value; }
-        if (pt.s.is_var && pt.p.is_var && pt.s.value == pt.p.value) sp.flags |= SP_EQ_SP;
-        if (pt.s.is_var && pt.o.is_var && pt.s.value == pt.o.value) sp.flags |= SP_EQ_SO;
-        if (pt.p.is_var && pt.o.is_var && pt.p.value == pt.o.value) sp.flags |= SP_EQ_PO;
-        std::vector<u32> slots, src;
-        pattern_vars(pt, &slots, &src);
-        auto rel = std::make_unique<kb_rel>();
-        if (row_index) {
-            slots.assign(1, 0u);
-            src.assign(1, 3u);
-        }
-        rel->slots = slots;
-        for (int q = 0; q < 4; q++) sp.outp[q] = nullptr;
-        if (tables && k < tables->size() && (*tables)[k].tab) {  // fused build: no output relation, the table is the output
-            const ScanTable& tb = (*tables)[k];
-            rel->pair = true;
-            sp.outp[0] = tb.tab;
-            sp.outp[1] = tb.dup_flag;
-            sp.cs = tb.kmin;
-            sp.co = tb.range;
-            sp.flags |= SP_TABLE | (tb.key_is_o ? SP_TKEY_O : 0u) | (tb.trusted ? SP_TTRUSTED : 0u);
-            P.cshift = tb.cshift;
-        } else if (pairs && !row_index && slots.size() == 2 && src[0] == 0 && src[1] == 2) {
-            Col col;  // interleaved (subject, object) rows: one 8-byte store per match
-            KB_TRY(alloc_col(ctx, 2 * N, &col));
-            rel->cols.push_back(col);
-            rel->pair = true;
-            sp.outp[0] = col.ptr;
-            sp.flags |= SP_PAIR;
-        } else {
-            for (size_t c = 0; c < slots.size(); c++) {  // columns come out in s,p,o order = order of first appearance
-                Col col;
-                KB_TRY(alloc_col(ctx, N, &col));
-                rel->cols.push_back(col);
-                sp.outp[src[c]] = col.ptr;
-                sp.flags |= src[c] == 0 ? SP_EMIT_S : src[c] == 1 ? SP_EMIT_P : src[c] == 2 ? SP_EMIT_O : SP_EMIT_IDX;
-            }
-        }
-        sp.f_begin = (u32)ops.size();
-        sp.f_len = 0;
-        if (k < pushdown.size() && !pushdown[k].ops.empty()) {
-            std::vector<u32> vs, vsrc;
-            pattern_vars(pt, &vs, &vsrc);
-            std::vector<FilterOp> local;
-            KB_TRY(compile_prog(ctx, pushdown[k], vs, &local, &vsrc));
-            if (ops.size() + local.size() > KB_MAX_FILTER_OPS) return fail(ctx, KB_E_LIMIT, "pushed-down filters exceed %d ops", KB_MAX_FILTER_OPS);
-            ops.insert(ops.end(), local.begin(), local.end());
-            sp.f_len = (u32)local.size();
-        }
-        out->push_back(std::move(rel));
-    }
-    for (size_t i = 0; i < ops.size(); i++) P.ops[i] = ops[i];
-
-    const u32 n_seg = (u32)segs.size();
-    // the guard depends on the segment count alone: where the arena cursor stands is irrelevant, ctrl_alloc wraps (an index build
-    // over hundreds of predicates hands out ~76 words per 8-predicate batch and every consumer clears its own words)
-    if (std::max(n_seg, 1u) + 2u * MAXP > kb_ctx::CTRL_WORDS - 64u) return fail(ctx, KB_E_LIMIT, "too many store segments (%u)", n_seg);
-    const u32 off_tot = ctrl_alloc(ctx, 2 * MAXP);
-    const u32 off_ticket = ctrl_alloc(ctx, std::max(n_seg, 1u));
-    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off_tot, 0, 2 * MAXP * sizeof(u32), ctx->st));
-    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off_ticket, 0, std::max(n_seg, 1u) * sizeof(u32), ctx->st));
-    u64 all_tiles = 0;
-    for (auto& sg : segs) all_tiles += (sg.n + SCAN_TILE - 1) / SCAN_TILE;
-    // One launch walks up to SCAN_MAXSEG consecutive segments (an RSP window is ~10 slides). A segment whose upload is still in
-    // flight (chunked kb_star_join_host) closes the group before it, so the scan of the chunks that already landed can start.
-    u64 index_base = 0;
-    u32 n_launched = 0;
-    u32 g = 0;
-    // tables that still have to be set to 0xFF: by the first launch itself when it is the star-shape kernel, else by memsets here
-    std::vector<std::pair<u32*, u32>> pending_clear;
-    if (tables) for (auto& tb : *tables) if (tb.tab && tb.clear) pending_clear.push_back({tb.tab, tb.range});
-    u32 off_clear = 0;
-    bool clear_folded = false;
-    while (g < n_seg) {
-        P.n_seg = 0;
-        P.n_tiles = 0;
-        cudaEvent_t wait_ev = nullptr;
-        while (g < n_seg && P.n_seg < (u32)SCAN_MAXSEG) {
-            const Segment& sg = segs[g];
-            if (sg.n == 0) { g++; continue; }
-            if (sg.ready && P.n_seg > 0) break;  // starts its own group
-            ScanSeg& d = P.seg[P.n_seg++];
-            d.s = sg.s.ptr; d.p = sg.p.ptr; d.o = sg.o.ptr;
-            d.n = (u32)sg.n;
-            d.tile0 = P.n_tiles;
-            d.index_base = (u32)index_base;
-            P.n_tiles += (u32)((sg.n + SCAN_TILE - 1) / SCAN_TILE);
-            index_base += sg.n;
-            g++;
-            if (sg.ready) { wait_ev = sg.ready; break; }
-        }
-        if (P.n_seg == 0) break;
-        P.ticket = ctx->ctrl + off_ticket + n_launched;
-        if (ctx->ordered) {  // ping-pong: a launch never writes the word its tiles read their base from
-            P.totals_in = ctx->ctrl + off_tot + (n_launched & 1u) * MAXP;
-            P.totals_out = ctx->ctrl + off_tot + ((n_launched + 1u) & 1u) * MAXP;
-        } else {
-            P.totals_in = P.totals_out = ctx->ctrl + off_tot;
-        }
-        n_launched++;
-        // (the star-shape kernel may walk the store in smaller tiles than SCAN_TILE)
-        KB_TRY(compact_setup(ctx, all_tiles * 4, nullptr, &P.c));
-        P.n_clear = 0;
-        if (!pending_clear.empty()) {
-            if (pending_clear.size() <= 4 && scan_clears_tables(P)) {
-                off_clear = ctrl_alloc(ctx, 4);
-                KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off_clear, 0, 4 * sizeof(u32), ctx->st));
-                for (auto& pc : pending_clear) { P.clear_tab[P.n_clear] = pc.first; P.clear_words[P.n_clear] = pc.second; P.n_clear++; }
-                P.clear_barrier = ctx->ctrl + off_clear;
-                clear_folded = true;
-            } else {
-                timer_begin(ctx, F_BUILD, 0);
-                for (auto& pc : pending_clear) KB_CUDA(ctx, cudaMemsetAsync(pc.first, 0xFF, (size_t)pc.second * sizeof(u32), ctx->st));
-                timer_end(ctx);
-            }
-            pending_clear.clear();
-        }
-        if (wait_ev) KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st, wait_ev, 0));  // chunked upload: start as soon as this chunk landed
-        timer_begin(ctx, F_SCAN);
-        launch_scan(P, ctx->n_sms, ctx->st);
-        timer_end(ctx);
-    }
-    for (auto& pc : pending_clear) KB_CUDA(ctx, cudaMemsetAsync(pc.first, 0xFF, (size_t)pc.second * sizeof(u32), ctx->st));  // (nothing was launched)
-    KB_CUDA(ctx, cudaGetLastError());
-    ctx->stats.rows_scanned += N;
-    KB_TRY(ctrl_read(ctx));
-    if (clear_folded && ctx->h_ctrl[off_clear + 1]) return fail(ctx, KB_E_CUDA, "scan: the grid did not meet at the table-clear barrier (another kernel holds SMs?)");
-    for (u32 k = 0; k < K; k++) (*out)[k]->n = ctx->h_ctrl[off_tot + (ctx->ordered ? (n_launched & 1u) * MAXP : 0u) + k];
     return KB_OK;
 }
 
@@ -821,22 +539,6 @@ void kb_rel_free(kb_ctx* ctx, kb_rel* r) {
 }
 
 // ------------------------------------------------------------------ operators
-kb_status kb_scan(kb_ctx* ctx, const kb_pattern* pats, uint32_t n_pats, const kb_filter_op* const* pushdown, const uint32_t* pushdown_len, kb_rel** out) {
-    KB_ENTER(ctx);
-    if (!pats || !out) return kb::fail(ctx, KB_E_INVALID, "NULL argument");
-    std::vector<kb::FilterProg> pd(n_pats);
-    if (pushdown && pushdown_len)
-        for (u32 k = 0; k < n_pats; k++) if (pushdown[k] && pushdown_len[k]) {
-            KB_TRY(kb::validate_filter(ctx, pushdown[k], pushdown_len[k]));
-            pd[k].ops.assign(pushdown[k], pushdown[k] + pushdown_len[k]);
-        }
-    std::vector<std::unique_ptr<kb_rel>> rels;
-    KB_TRY(kb::scan_impl(ctx, ctx->segs, pats, n_pats, pd, /*use_index=*/true, false, false, &rels));
-    for (u32 k = 0; k < n_pats; k++) out[k] = rels[k].release();
-    if (n_pats) ctx->stats.rows_out = out[n_pats - 1]->n;
-    return KB_OK;
-}
-
 kb_status kb_filter(kb_ctx* ctx, const kb_rel* in, const kb_filter_op* prog, uint32_t n_ops, kb_rel** out) {
     KB_ENTER(ctx);
     if (!in || !out) return kb::fail(ctx, KB_E_INVALID, "NULL argument");
@@ -1091,6 +793,7 @@ kb_status kb_partition(kb_ctx* ctx, const kb_rel* in, uint32_t key_slot, uint32_
 }
 
 // ------------------------------------------------------------------ one-shot host-buffer star join
+static constexpr u64 HOST_UPLOAD_CHUNK = 8ull << 20;  // triples per upload chunk (one store segment each): 32 MiB per column
 static kb_status star_join_host_common(kb_ctx* ctx, const uint32_t* s, const uint32_t* p, const uint32_t* o, uint64_t n, uint32_t join_slot,
                                        const kb_pattern* pats, uint32_t n_pats, const kb_filter_op* filter, uint32_t n_ops, uint32_t* n_cols,
                                        uint32_t* slots, uint32_t** cols, uint64_t* n_rows, bool caller_bufs, uint64_t caller_cap) {
@@ -1119,7 +822,7 @@ static kb_status star_join_host_common(kb_ctx* ctx, const uint32_t* s, const uin
     KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + soff, 0xFF, 4 * sizeof(u32), ctx->st));
     KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + soff + 4, 0, 4 * sizeof(u32), ctx->st));
     KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));  // allocations are stream-ordered on st; the copy stream must see them
-    const u64 chunk = (u64)kb::SCAN_TILE * 4096;   // 8 Mi triples = 32 MiB per column
+    const u64 chunk = HOST_UPLOAD_CHUNK;
     std::vector<cudaEvent_t> evs;
     std::vector<kb::Segment> segs;
     // whatever happens from here on, the caller's buffers are not read after this function returns and a failed call leaves an
@@ -1165,7 +868,7 @@ static kb_status star_join_host_common(kb_ctx* ctx, const uint32_t* s, const uin
     kb::store_replace(ctx, std::move(segs));
     ctx->stats.h2d_bytes += 3 * n * sizeof(u32);
     ctx->upload_stats_off = (int)soff;
-    // scan_impl makes st wait on each segment's `ready` event right before that segment's scan kernel: copy i+1 overlaps scan i
+    // scan_segments makes st wait on each segment's `ready` event right before that segment's scan kernel: copy i+1 overlaps scan i
     std::unique_ptr<kb_rel> r;
     kb_status rc = kb::star_join_impl(ctx, join_slot, pats, n_pats, filter, n_ops, &r);
     if (rc != KB_OK) return finish(rc);

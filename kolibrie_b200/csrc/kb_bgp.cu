@@ -1,6 +1,6 @@
 // kb_bgp.cu — kb_bgp_execute's component route: every BGP that is not a star of at most KB_MAX_PATTERNS patterns. The semantics are
 // in include/kolibrie_b200.h; here:
-//   scans              scan_impl in fused groups of at most MAXP patterns (index lookups with a valid index)
+//   scans              scan_store in fused groups of at most MAXP patterns (index lookups with a valid index)
 //   plan               components, GYO and the join order: kb_bgp_plan.hpp (host C++, shared with a CPU test driver)
 //   domain reduction   components of three or more patterns. For every variable v that two or more of the component's patterns hold,
 //                      D(v) is a bitmap over v's id range (the intersection of the segment profiles' ranges of the positions v
@@ -270,7 +270,7 @@ kb_status bgp_components(kb_ctx* ctx, const kb_pattern* pats, u32 n_pats, const 
         const u32 m = std::min(n_pats - g, (u32)MAXP);
         std::vector<FilterProg> pd(pushdown.begin() + g, pushdown.begin() + g + m);
         std::vector<std::unique_ptr<kb_rel>> part;
-        KB_TRY(scan_impl(ctx, ctx->segs, pats + g, m, pd, /*use_index=*/true, false, false, &part));
+        KB_TRY(scan_store(ctx, pats + g, m, pd, &part));
         for (auto& r : part) rels.push_back(std::move(r));
     }
     const std::vector<std::vector<u32>> comps = kb_bgp::components(pv);

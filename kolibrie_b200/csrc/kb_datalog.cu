@@ -577,13 +577,10 @@ static kb_status fixpoint_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
         for (auto& kv : fx.rels) preds.push_back(kv.first);
         for (size_t b = 0; b < preds.size(); b += MAXP) {
             const u32 k = (u32)std::min<size_t>(MAXP, preds.size() - b);
-            kb_pattern pats[MAXP];
-            for (u32 i = 0; i < k; i++) { pats[i].s = kb_term{1, 0}; pats[i].p = kb_term{0, preds[b + i]}; pats[i].o = kb_term{1, 1}; }
             std::vector<std::unique_ptr<kb_rel>> out;
-            std::vector<FilterProg> none;
             // the predicate relations are append-only buffers with the capacity of a whole-store scan output: take the scan, not the
             // (exactly sized) index slices
-            KB_TRY(scan_impl(ctx, ctx->segs, pats, k, none, /*use_index=*/false, false, false, &out));
+            KB_TRY(scan_predicates(ctx, ctx->segs, preds.data() + b, k, ScanOut::Cols, &out));
             for (u32 i = 0; i < k; i++) {
                 PredRel& r = fx.rels[preds[b + i]];
                 r.s = out[i]->cols[0];
@@ -844,11 +841,8 @@ kb_status split_segments(kb_ctx* ctx, const std::vector<u32>& preds, const std::
     if (n == 0 || preds.empty()) return KB_OK;
     for (size_t b = 0; b < preds.size(); b += MAXP) {
         const u32 k = (u32)std::min<size_t>(MAXP, preds.size() - b);
-        kb_pattern pats[MAXP];
-        for (u32 i = 0; i < k; i++) { pats[i].s = kb_term{1, 0}; pats[i].p = kb_term{0, preds[b + i]}; pats[i].o = kb_term{1, 1}; }
         std::vector<std::unique_ptr<kb_rel>> res;
-        std::vector<FilterProg> none;
-        KB_TRY(scan_impl(ctx, part, pats, k, none, /*use_index=*/false, false, false, &res));
+        KB_TRY(scan_predicates(ctx, part, preds.data() + b, k, ScanOut::Cols, &res));
         for (u32 i = 0; i < k; i++) {
             Pairs& p = (*out)[preds[b + i]];
             p.s = res[i]->cols[0];

@@ -340,15 +340,22 @@ struct ScanTable {  // scan+build fusion: pattern k inserts its matches into thi
     u32 cshift = 0;
     u32 key_is_o = 0, trusted = 0;
     u32* dup_flag = nullptr;
-    bool clear = false;  // the table has not been set to 0xFF yet: scan_impl clears it (inside the scan kernel when it can)
+    bool clear = false;  // the table has not been set to 0xFF yet: scan_segments clears it (inside the scan kernel when it can)
 };
-// One fused scan of `segs` (the store, ctx->segs, or segments a caller selected or built) for up to MAXP patterns.
-// use_index: patterns the store index answers are looked up instead of scanned; only a scan of ctx->segs itself without row_index,
-// pairs or tables does that. row_index: every pattern emits the row positions of its matches. pairs: 2-variable (?s P ?o)-shaped
-// patterns are emitted as interleaved (s,o) pair relations (internal fast path).
-kb_status scan_impl(kb_ctx* ctx, const std::vector<Segment>& segs, const kb_pattern* pats, u32 n_pats, const std::vector<FilterProg>& pushdown,
-                    bool use_index, bool row_index, bool pairs, std::vector<std::unique_ptr<kb_rel>>* out,
-                    const std::vector<ScanTable>* tables = nullptr);
+// The triple scan (kb_scan.cu). What a scan emits per pattern: its variables as columns (s,p,o order); a 2-variable (?s P ?o)-shaped
+// pattern as one interleaved (s,o) pair relation (internal fast path; other shapes still get columns); or the row positions of its
+// matches.
+enum class ScanOut { Cols, Pairs, RowIndex };
+// One fused scan of `segs` (the store, ctx->segs, or segments a caller selected or built) for 1..MAXP patterns. tables: per pattern,
+// a direct table that takes its matches instead of an output relation.
+kb_status scan_segments(kb_ctx* ctx, const std::vector<Segment>& segs, const kb_pattern* pats, u32 n_pats, const std::vector<FilterProg>& pushdown,
+                        ScanOut mode, std::vector<std::unique_ptr<kb_rel>>* out, const std::vector<ScanTable>* tables = nullptr);
+// The patterns over the store, as columns: with a valid index (and ctx->use_index) the patterns it answers are looked up, and one fused
+// scan of ctx->segs handles the rest.
+kb_status scan_store(kb_ctx* ctx, const kb_pattern* pats, u32 n_pats, const std::vector<FilterProg>& pushdown, std::vector<std::unique_ptr<kb_rel>>* out);
+// (?0 P ?1) for each of the k <= MAXP predicates `preds`, in one fused scan of `segs` without pushdown
+kb_status scan_predicates(kb_ctx* ctx, const std::vector<Segment>& segs, const u32* preds, u32 k, ScanOut mode,
+                          std::vector<std::unique_ptr<kb_rel>>* out);
 // fused GROUP BY of a star join (kb_star_join_aggregate): in = group / aggregate spec; out = groups when the one-kernel index path took it
 struct AggSpec {
     AggSpec() = default;

@@ -864,7 +864,7 @@ static kb_status fused_scan_join(kb_ctx* ctx, const StarQuery& q, std::unique_pt
         KB_TRY(alloc_buf(ctx, (size_t)range * sizeof(u32), &b));
         tabs.push_back(b);
         st[k].tab = static_cast<u32*>(b->p);
-        st[k].clear = true;  // cleared by the scan (scan_impl)
+        st[k].clear = true;  // cleared by the scan (scan_segments)
         st[k].kmin = kmn; st[k].range = range; st[k].cshift = cshift;
         st[k].key_is_o = q.key_pos[k] == 2 ? 1u : 0u;
         st[k].trusted = build_keys(ctx, q, k) == Keys::single ? 1u : 0u;
@@ -878,7 +878,7 @@ static kb_status fused_scan_join(kb_ctx* ctx, const StarQuery& q, std::unique_pt
     }
     timer_end(ctx);
     std::vector<std::unique_ptr<kb_rel>> rels;
-    KB_TRY(scan_impl(ctx, ctx->segs, q.pats, K, q.pushdown, /*use_index=*/false, false, true, &rels, &st));
+    KB_TRY(scan_segments(ctx, ctx->segs, q.pats, K, q.pushdown, ScanOut::Pairs, &rels, &st));
     ctx->stats.fused_scan_builds++;
     // duplicate keys: the scan stores without reading back, so a multi-valued key shows up as fewer occupied slots than
     // inserted rows. Tables of (predicate, position) pairs already verified for this store version are not re-counted.
@@ -1063,7 +1063,7 @@ static kb_status batched_join(kb_ctx* ctx, const StarQuery& q, std::vector<std::
 static kb_status scan_join(kb_ctx* ctx, const StarQuery& q, std::unique_ptr<kb_rel>* out) {
     const u32 K = q.K;
     std::vector<std::unique_ptr<kb_rel>> rels;
-    KB_TRY(scan_impl(ctx, ctx->segs, q.pats, K, q.pushdown, /*use_index=*/true, false, q.all_pairs, &rels));
+    KB_TRY(q.all_pairs ? scan_segments(ctx, ctx->segs, q.pats, K, q.pushdown, ScanOut::Pairs, &rels) : scan_store(ctx, q.pats, K, q.pushdown, &rels));
     if (ctx->upload_stats_off >= 0) {  // one-shot host call: the copy stream computed the column ranges chunk by chunk
         const u32 o = (u32)ctx->upload_stats_off;
         for (auto& sg : ctx->segs) {
@@ -1177,7 +1177,7 @@ kb_status bind_join_impl(kb_ctx* ctx, const kb_rel& L, const kb_pattern& pt, std
     }
     std::vector<std::unique_ptr<kb_rel>> rels;
     std::vector<FilterProg> none;
-    KB_TRY(scan_impl(ctx, ctx->segs, pat, 1, none, /*use_index=*/true, false, false, &rels));
+    KB_TRY(scan_store(ctx, pat, 1, none, &rels));
     return hash_join_impl(ctx, *left, *rels[0], nullptr, out);
 }
 

@@ -10,521 +10,8 @@
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
-#include <type_traits>
 
 namespace kb {
-
-// =================================================================================================================
-// K_scan
-// Thread t owns the 8 consecutive triples [8t, 8t+8) of a 2048-triple tile. The tile is TMA-staged into shared memory, pulled
-// into registers with six LDS.128, and the shared buffer is immediately handed back to TMA for the NEXT tile (single buffer,
-// register-staged double buffering). K is a template parameter so every pattern field is a constant-bank operand.
-__device__ __forceinline__ u32 eq8(const uint4& a, const uint4& b, u32 c) {
-    return (a.x == c ? 1u : 0u) | (a.y == c ? 2u : 0u) | (a.z == c ? 4u : 0u) | (a.w == c ? 8u : 0u) | (b.x == c ? 16u : 0u) | (b.y == c ? 32u : 0u) |
-           (b.z == c ? 64u : 0u) | (b.w == c ? 128u : 0u);
-}
-__device__ __forceinline__ u32 eqv8(const uint4& a0, const uint4& a1, const uint4& b0, const uint4& b1) {
-    return (a0.x == b0.x ? 1u : 0u) | (a0.y == b0.y ? 2u : 0u) | (a0.z == b0.z ? 4u : 0u) | (a0.w == b0.w ? 8u : 0u) | (a1.x == b1.x ? 16u : 0u) |
-           (a1.y == b1.y ? 32u : 0u) | (a1.z == b1.z ? 64u : 0u) | (a1.w == b1.w ? 128u : 0u);
-}
-#define KB_ELEM(v0, v1, j) ((j) == 0 ? v0.x : (j) == 1 ? v0.y : (j) == 2 ? v0.z : (j) == 3 ? v0.w : (j) == 4 ? v1.x : (j) == 5 ? v1.y : (j) == 6 ? v1.z : v1.w)
-
-template <int K>
-__global__ void __launch_bounds__(SCAN_THREADS, (K <= 4 ? 1024 / SCAN_THREADS : 512 / SCAN_THREADS)) scan_kernel(const __grid_constant__ ScanParams P) {
-    // two shared stages of three column tiles each: tile i+1 is in flight while tile i is processed; the stage of tile i is handed
-    // back to TMA (for tile i+2) right after the first compaction barrier — every thread has its triples in registers by then, so
-    // the hand-over costs no barrier of its own
-    extern __shared__ __align__(128) u32 smem_all[];
-    constexpr u32 STAGE_WORDS = 3u * SCAN_TILE;
-    __shared__ __align__(8) u64 bars[2];
-    __shared__ u32 s_nexts[2];
-    __shared__ u32 s_wcnt[SCAN_THREADS / 32][MAXP];
-    __shared__ u32 s_excl[MAXP];
-    constexpr int NW = (K + 2) / 3;  // packed count words: three 10-bit fields each (a warp holds at most 256 matches per pattern)
-    __shared__ u32 s_tcnt[2], s_tindex[2];  // triples in the staged tile, global index of its first triple
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    // one thread: take the next tile, find its segment, start the three column copies into `stage`
-    auto issue_next = [&](u32 stage) {
-        const u32 t = atomicAdd(P.ticket, 1u);
-        s_nexts[stage] = t;
-        if (t < P.n_tiles) {
-            u32 g = 0;
-            while (g + 1u < P.n_seg && t >= P.seg[g + 1u].tile0) g++;
-            const ScanSeg& sg = P.seg[g];
-            const u32 b = (t - sg.tile0) * (u32)SCAN_TILE;
-            const u32 c = min((u32)SCAN_TILE, sg.n - b);
-            const u32 bytes = (c * 4u + 15u) & ~15u;  // columns are padded to 256 B: the rounded-up read stays in bounds
-            s_tcnt[stage] = c;
-            s_tindex[stage] = sg.index_base + b;
-            u32* dst = smem_all + stage * STAGE_WORDS;
-            mbar_arrive_expect_tx(&bars[stage], bytes * 3u);
-            tma_load_1d(dst, sg.s + b, bytes, &bars[stage]);
-            tma_load_1d(dst + SCAN_TILE, sg.p + b, bytes, &bars[stage]);
-            tma_load_1d(dst + 2 * SCAN_TILE, sg.o + b, bytes, &bars[stage]);
-        }
-    };
-    if (tid == 0) {
-        mbar_init(&bars[0], 1);
-        mbar_init(&bars[1], 1);
-        fence_mbar_init();
-        issue_next(0);
-        issue_next(1);
-    }
-    __syncthreads();
-    u32 tile = s_nexts[0];
-    u32 it = 0;
-
-    while (tile < P.n_tiles) {
-        const u32 stage = it & 1u;
-        mbar_wait(&bars[stage], (it >> 1) & 1u);
-        const uint4* sS4 = reinterpret_cast<const uint4*>(smem_all + stage * STAGE_WORDS);
-        const uint4* sP4 = sS4 + SCAN_TILE / 4;
-        const uint4* sO4 = sS4 + 2 * (SCAN_TILE / 4);
-        const uint4 s0 = sS4[2 * tid], s1 = sS4[2 * tid + 1];
-        const uint4 p0 = sP4[2 * tid], p1 = sP4[2 * tid + 1];
-        const uint4 o0 = sO4[2 * tid], o1 = sO4[2 * tid + 1];
-        const u32 cnt = s_tcnt[stage], tindex = s_tindex[stage];
-        // ---- match: bit j of mk[k] = triple 8*tid+j matches pattern k
-        const u32 first = (u32)tid * 8u;
-        const u32 vmask = first >= cnt ? 0u : (cnt - first >= 8u ? 0xFFu : ((1u << (cnt - first)) - 1u));
-        u32 mk[K];
-#pragma unroll
-        for (int k = 0; k < K; k++) {
-            const u32 f = P.pat[k].flags;
-            u32 m = vmask;
-            if (f & SP_HAS_P) m &= eq8(p0, p1, P.pat[k].cp);
-            if (f & SP_HAS_S) m &= eq8(s0, s1, P.pat[k].cs);
-            if (f & SP_HAS_O) m &= eq8(o0, o1, P.pat[k].co);
-            if (f & (SP_EQ_SP | SP_EQ_SO | SP_EQ_PO)) {
-                if (f & SP_EQ_SP) m &= eqv8(s0, s1, p0, p1);
-                if (f & SP_EQ_SO) m &= eqv8(s0, s1, o0, o1);
-                if (f & SP_EQ_PO) m &= eqv8(p0, p1, o0, o1);
-            }
-            if (P.pat[k].f_len != 0u && m != 0u) {
-                const FilterOp* fo = P.ops + P.pat[k].f_begin;
-                if (P.pat[k].f_len == 1u && fo[0].op == KB_F_CMP_NUM) {  // FILTER(?x <cmp> c): gather the 8 numeric values, then compare
-                    const u32 slot = fo[0].slot, cmp = fo[0].cmp;
-                    const double cv = fo[0].value;
-                    // the column is chosen once (two vector selects), not once per element
-                    const uint4 x0 = slot == 0u ? s0 : (slot == 1u ? p0 : o0);
-                    const uint4 x1 = slot == 0u ? s1 : (slot == 1u ? p1 : o1);
-                    double a[8];
-#pragma unroll
-                    for (int j = 0; j < 8; j++) a[j] = ((m >> j) & 1u) ? num_of(P.nt, KB_ELEM(x0, x1, j)) : 0.0;
-                    u32 pass = 0;
-#pragma unroll
-                    for (int j = 0; j < 8; j++) pass |= (cmp_num(cmp, a[j], cv) ? 1u : 0u) << j;
-                    m &= pass;
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 8; j++) {
-                        if ((m >> j) & 1u) {
-                            u32 vals[3] = {KB_ELEM(s0, s1, j), KB_ELEM(p0, p1, j), KB_ELEM(o0, o1, j)};
-                            if (!eval_filter(fo, P.pat[k].f_len, vals, P.nt)) m &= ~(1u << j);
-                        }
-                    }
-                }
-            }
-            mk[k] = m;
-        }
-        // ---- ranks: one packed warp scan per three patterns
-        u32 wex[K];
-#pragma unroll
-        for (int w = 0; w < NW; w++) {
-            u32 packed = 0;
-#pragma unroll
-            for (int q = 0; q < 3; q++) if (w * 3 + q < K) packed |= (u32)__popc(mk[w * 3 + q]) << (10 * q);
-            u32 incl = packed;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const u32 y = __shfl_up_sync(0xffffffffu, incl, o);
-                if (lane >= o) incl += y;
-            }
-            const u32 excl = incl - packed;
-            const u32 tot = __shfl_sync(0xffffffffu, incl, 31);
-#pragma unroll
-            for (int q = 0; q < 3; q++) if (w * 3 + q < K) {
-                wex[w * 3 + q] = (excl >> (10 * q)) & 1023u;
-                if (lane == 0) s_wcnt[warp][w * 3 + q] = (tot >> (10 * q)) & 1023u;
-            }
-        }
-        __syncthreads();
-        const u32 following = s_nexts[stage ^ 1u];  // the next iteration's tile (its copies are already in flight)
-        if (tid == SCAN_THREADS - 1) issue_next(stage);
-        if (warp < K) {  // warp k owns counter k: cross-warp prefix of its per-warp totals, then the look-back across tiles
-            const u32 c = lane < SCAN_THREADS / 32 ? s_wcnt[lane][warp] : 0u;
-            u32 incl = c;
-#pragma unroll
-            for (int o = 1; o < SCAN_THREADS / 32; o <<= 1) {
-                const u32 y = __shfl_up_sync(0xffffffffu, incl, o);
-                if (lane >= o) incl += y;
-            }
-            const u32 total = __shfl_sync(0xffffffffu, incl, SCAN_THREADS / 32 - 1);
-            if (lane < SCAN_THREADS / 32) s_wcnt[lane][warp] = incl - c;
-            const u32 ex = tile_prefix_2level(P.c.tile_state, P.c.block_state, tile, P.n_tiles, (u32)warp, P.c.epoch, total, P.totals_in, P.totals_out, P.c.ordered, lane);
-            if (lane == 0) s_excl[warp] = ex;
-        }
-        __syncthreads();
-        // ---- write: rank = tile prefix + warp prefix + thread prefix, then a running rank over this thread's 8 triples
-#pragma unroll
-        for (int k = 0; k < K; k++) {
-            const u32 m = mk[k];
-            if (m == 0u) continue;
-            const u32 f = P.pat[k].flags;
-            if (f & SP_TABLE) {  // fused build: insert into the direct table of this pattern
-                u32* tab = P.pat[k].outp[0];
-                const u32 kbase = P.pat[k].cs, krange = P.pat[k].co;
-                // key / value columns chosen once; offsets computed for all eight triples, stores predicated (no branch per triple).
-                // Plain fire-and-forget stores: a returning atomic here stalls the tile loop (slower than a separate
-                // scan + build); duplicate keys are detected afterwards by counting the occupied slots
-                const bool key_o = (f & SP_TKEY_O) != 0u;
-                const uint4 k0 = key_o ? o0 : s0, k1 = key_o ? o1 : s1;
-                const uint4 v0 = key_o ? s0 : o0, v1 = key_o ? s1 : o1;
-                u32 bad = 0;
-                if (P.cshift == 0u) {
-#pragma unroll
-                    for (int j = 0; j < 8; j++) {
-                        const u32 off = KB_ELEM(k0, k1, j) - kbase;
-                        const bool on = (m >> j) & 1u;
-                        if (on && off < krange) tab[off] = KB_ELEM(v0, v1, j);
-                        bad |= (on && off >= krange) ? 1u : 0u;
-                    }
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 8; j++) {
-                        const u32 off = compact_key(KB_ELEM(k0, k1, j), P.cshift) - kbase;
-                        const bool on = (m >> j) & 1u;
-                        if (on && off < krange) tab[off] = KB_ELEM(v0, v1, j);
-                        bad |= (on && off >= krange) ? 1u : 0u;
-                    }
-                }
-                const bool dup = bad != 0u;
-                if (dup) *P.pat[k].outp[1] = 1u;
-                continue;
-            }
-            const u32 pos = s_excl[k] + s_wcnt[warp][k] + wex[k];
-            if (f & SP_PAIR) {
-                uint2* out = reinterpret_cast<uint2*>(P.pat[k].outp[0]) + pos;
-#pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    if ((m >> j) & 1u) *out = make_uint2(KB_ELEM(s0, s1, j), KB_ELEM(o0, o1, j));
-                    out += (m >> j) & 1u;
-                }
-                continue;
-            }
-            if (f & SP_EMIT_S) {
-                u32* out = P.pat[k].outp[0] + pos;
-#pragma unroll
-                for (int j = 0; j < 8; j++) { if ((m >> j) & 1u) *out = KB_ELEM(s0, s1, j); out += (m >> j) & 1u; }
-            }
-            if (f & SP_EMIT_P) {
-                u32* out = P.pat[k].outp[1] + pos;
-#pragma unroll
-                for (int j = 0; j < 8; j++) { if ((m >> j) & 1u) *out = KB_ELEM(p0, p1, j); out += (m >> j) & 1u; }
-            }
-            if (f & SP_EMIT_O) {
-                u32* out = P.pat[k].outp[2] + pos;
-#pragma unroll
-                for (int j = 0; j < 8; j++) { if ((m >> j) & 1u) *out = KB_ELEM(o0, o1, j); out += (m >> j) & 1u; }
-            }
-            if (f & SP_EMIT_IDX) {
-                u32* out = P.pat[k].outp[3] + pos;
-#pragma unroll
-                for (int j = 0; j < 8; j++) { if ((m >> j) & 1u) *out = tindex + first + (u32)j; out += (m >> j) & 1u; }
-            }
-        }
-        tile = following;
-        it++;
-    }
-}
-
-// K_scan, STAR shape: every pattern is (?s P ?o) with a constant predicate and distinct variables, its output goes to a direct join
-// table (fused build) or to an interleaved (s,o) pair relation, and its pushed-down FILTER — if any — is one numeric comparison on the
-// subject or the object. That is what a star join's scan looks like (engine.rs:587-691 over engine.rs:1364-1378), and knowing it at
-// compile time removes what made the general kernel issue-bound (2.8 warp instructions per triple): no per-tile flag tests, no
-// comparison switch per element (a < c is evaluated as -a > -c, so every operator is one DSETP), no divergent branches — every store is
-// predicated — and no rank computation for patterns whose matches go to a table.
-#ifndef KB_STAR_THREADS
-#define KB_STAR_THREADS 256
-#endif
-constexpr int STAR_THREADS = KB_STAR_THREADS;  // K <= 4 patterns need 4 prefix warps: 128 threads suffice (smaller CTAs, cheaper barriers)
-constexpr int STAR_TILE = STAR_THREADS * SCAN_ITEMS;
-template <int K>
-__global__ void __launch_bounds__(STAR_THREADS, 1024 / STAR_THREADS) scan_star_kernel(const __grid_constant__ ScanParams P) {
-    extern __shared__ __align__(128) u32 smem_all[];
-    constexpr u32 STAGE_WORDS = 3u * STAR_TILE;
-    __shared__ __align__(8) u64 bars[2];
-    __shared__ u32 s_nexts[2];
-    __shared__ u32 s_wcnt[STAR_THREADS / 32][MAXP];
-    __shared__ u32 s_excl[MAXP];
-    __shared__ u32 s_tcnt[2];
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    auto issue_next = [&](u32 stage) {
-        const u32 t = atomicAdd(P.ticket, 1u);
-        s_nexts[stage] = t;
-        if (t < P.n_tiles) {
-            u32 g = 0;
-            while (g + 1u < P.n_seg && t >= P.seg[g + 1u].tile0) g++;
-            const ScanSeg& sg = P.seg[g];
-            const u32 b = (t - sg.tile0) * (u32)STAR_TILE;
-            const u32 c = min((u32)STAR_TILE, sg.n - b);
-            const u32 bytes = (c * 4u + 15u) & ~15u;
-            s_tcnt[stage] = c;
-            u32* dst = smem_all + stage * STAGE_WORDS;
-            mbar_arrive_expect_tx(&bars[stage], bytes * 3u);
-            tma_load_1d(dst, sg.s + b, bytes, &bars[stage]);
-            tma_load_1d(dst + STAR_TILE, sg.p + b, bytes, &bars[stage]);
-            tma_load_1d(dst + 2 * STAR_TILE, sg.o + b, bytes, &bars[stage]);
-        }
-    };
-    if (tid == 0) {
-        mbar_init(&bars[0], 1);
-        mbar_init(&bars[1], 1);
-        fence_mbar_init();
-        issue_next(0);
-        issue_next(1);
-    }
-    if (P.n_clear) {
-        // the tables this scan inserts into are cleared by the grid itself while the first tiles are in flight, then every CTA waits
-        // until all have finished (the grid is sized to residency, so all of them are running)
-        const uint4 ones = make_uint4(EMPTY32, EMPTY32, EMPTY32, EMPTY32);
-        for (u32 t = 0; t < P.n_clear; t++) {
-            uint4* t4 = reinterpret_cast<uint4*>(P.clear_tab[t]);
-            const u32 n4 = P.clear_words[t] >> 2;
-            for (u32 i = blockIdx.x * STAR_THREADS + (u32)tid; i < n4; i += gridDim.x * STAR_THREADS) t4[i] = ones;
-            if (blockIdx.x == 0) for (u32 i = (n4 << 2) + (u32)tid; i < P.clear_words[t]; i += STAR_THREADS) P.clear_tab[t][i] = EMPTY32;
-        }
-        __threadfence();
-        __syncthreads();
-        if (tid == 0) {
-            atomicAdd(P.clear_barrier, 1u);
-            u32 spins = 0;
-            while (*reinterpret_cast<volatile u32*>(P.clear_barrier) < gridDim.x) {
-                __nanosleep(100);
-                if (++spins > (1u << 24)) { P.clear_barrier[1] = 1u; break; }  // ~2 s: reported by the host as an error
-            }
-            __threadfence();
-        }
-    }
-    __syncthreads();
-    u32 tile = s_nexts[0];
-    u32 it = 0;
-    u32 bad_any = 0;
-    while (tile < P.n_tiles) {
-        const u32 stage = it & 1u;
-        mbar_wait(&bars[stage], (it >> 1) & 1u);
-        const uint4* sS4 = reinterpret_cast<const uint4*>(smem_all + stage * STAGE_WORDS);
-        const uint4* sP4 = sS4 + STAR_TILE / 4;
-        const uint4* sO4 = sS4 + 2 * (STAR_TILE / 4);
-        // thread t owns triples [4t, 4t+4) of EACH half of the tile: consecutive threads read consecutive 16-byte words (LDS.128 without
-        // bank conflicts; 8 consecutive triples per thread put two threads of a quarter-warp on the same banks). The rows of a tile
-        // therefore come out in a fixed permutation of store order — fine for tables and for completion-order results; ordered
-        // contexts take the general kernel.
-        constexpr u32 HALF4 = STAR_TILE / 8;  // uint4 words per half column
-        const uint4 s0 = sS4[tid], s1 = sS4[HALF4 + tid];
-        const uint4 p0 = sP4[tid], p1 = sP4[HALF4 + tid];
-        const uint4 o0 = sO4[tid], o1 = sO4[HALF4 + tid];
-        const u32 cnt = s_tcnt[stage];
-        const u32 first = (u32)tid * 4u;
-        const u32 lo = first >= cnt ? 0u : (cnt - first >= 4u ? 0xFu : ((1u << (cnt - first)) - 1u));
-        const u32 first2 = (u32)STAR_TILE / 2u + first;
-        const u32 hi = first2 >= cnt ? 0u : (cnt - first2 >= 4u ? 0xFu : ((1u << (cnt - first2)) - 1u));
-        const u32 vmask = lo | (hi << 4);
-        u32 mk[K];
-#pragma unroll
-        for (int k = 0; k < K; k++) {
-            u32 m = eq8(p0, p1, P.pat[k].cp) & vmask;
-            if (P.pat[k].f_len != 0u) {  // uniform per pattern: FILTER(?x <cmp> c) on the subject (slot 0) or the object (slot 2)
-                // the launcher canonicalised the comparison to >= or <= (a > c is a >= nextup(c)): one DSETP per triple, no operator switch
-                const FilterOp fo = P.ops[P.pat[k].f_begin];
-                const bool on_s = fo.slot == 0u;
-                const double cv = fo.value;
-                const uint4 x0 = on_s ? s0 : o0, x1 = on_s ? s1 : o1;
-                double a[8];
-#pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    const u32 id = KB_ELEM(x0, x1, j);
-                    a[j] = 0.0;
-                    if (((m >> j) & 1u) && id < P.nt.n_ids) a[j] = __ldg(P.nt.num_or0 + id);
-                }
-                u32 pass = 0;
-                if (fo.cmp == KB_CMP_GE) {
-#pragma unroll
-                    for (int j = 0; j < 8; j++) pass |= (a[j] >= cv ? 1u : 0u) << j;
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 8; j++) pass |= (a[j] <= cv ? 1u : 0u) << j;
-                }
-                m &= pass;
-            }
-            mk[k] = m;
-        }
-        // ---- counts: a packed warp scan per three patterns (ranks are only consumed by pair outputs; totals by every pattern)
-        constexpr int NW = (K + 2) / 3;
-        u32 wex[K];
-#pragma unroll
-        for (int w = 0; w < NW; w++) {
-            u32 packed = 0;
-#pragma unroll
-            for (int q = 0; q < 3; q++) if (w * 3 + q < K) packed |= (u32)__popc(mk[w * 3 + q]) << (10 * q);
-            u32 incl = packed;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const u32 y = __shfl_up_sync(0xffffffffu, incl, o);
-                if (lane >= o) incl += y;
-            }
-            const u32 excl = incl - packed;
-            const u32 tot = __shfl_sync(0xffffffffu, incl, 31);
-#pragma unroll
-            for (int q = 0; q < 3; q++) if (w * 3 + q < K) {
-                wex[w * 3 + q] = (excl >> (10 * q)) & 1023u;
-                if (lane == 0) s_wcnt[warp][w * 3 + q] = (tot >> (10 * q)) & 1023u;
-            }
-        }
-        __syncthreads();
-        const u32 following = s_nexts[stage ^ 1u];
-        if (tid == STAR_THREADS - 1) issue_next(stage);  // every thread holds its triples in registers: the stage takes the tile after next
-        if (warp < K) {
-            const u32 c = lane < STAR_THREADS / 32 ? s_wcnt[lane][warp] : 0u;
-            u32 incl = c;
-#pragma unroll
-            for (int o = 1; o < STAR_THREADS / 32; o <<= 1) {
-                const u32 y = __shfl_up_sync(0xffffffffu, incl, o);
-                if (lane >= o) incl += y;
-            }
-            const u32 total = __shfl_sync(0xffffffffu, incl, STAR_THREADS / 32 - 1);
-            if (lane < STAR_THREADS / 32) s_wcnt[lane][warp] = incl - c;
-            const u32 ex = tile_prefix_2level(P.c.tile_state, P.c.block_state, tile, P.n_tiles, (u32)warp, P.c.epoch, total, P.totals_in, P.totals_out, P.c.ordered, lane);
-            if (lane == 0) s_excl[warp] = ex;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int k = 0; k < K; k++) {
-            const u32 m = mk[k];
-            if (P.pat[k].flags & SP_TABLE) {  // uniform: the matches go straight into this pattern's direct table
-                u32* tab = P.pat[k].outp[0];
-                const u32 kbase = P.pat[k].cs, krange = P.pat[k].co;
-                auto stores = [&](const uint4& k0, const uint4& k1, const uint4& v0, const uint4& v1, auto with_cshift) {
-                    u32 worst = 0;  // largest offset of a matching triple: one range test per pattern and tile instead of one flag update per triple
-#pragma unroll
-                    for (int j = 0; j < 8; j++) {
-                        const u32 key = KB_ELEM(k0, k1, j);
-                        const u32 off = (with_cshift.value ? compact_key(key, P.cshift) : key) - kbase;
-                        const bool on = (m >> j) & 1u;  // (the compiler folds this with the predicate comparison the bit came from)
-                        if (on && off < krange) tab[off] = KB_ELEM(v0, v1, j);
-                        worst = max(worst, on ? off : 0u);
-                    }
-                    bad_any |= worst >= krange ? (1u << k) : 0u;
-                };
-                const bool key_o = (P.pat[k].flags & SP_TKEY_O) != 0u;
-                if (P.cshift == 0u) {
-                    if (key_o) stores(o0, o1, s0, s1, std::false_type{});
-                    else stores(s0, s1, o0, o1, std::false_type{});
-                } else {
-                    if (key_o) stores(o0, o1, s0, s1, std::true_type{});
-                    else stores(s0, s1, o0, o1, std::true_type{});
-                }
-            } else {
-                u32 pos = s_excl[k] + s_wcnt[warp][k] + wex[k];
-                uint2* out = reinterpret_cast<uint2*>(P.pat[k].outp[0]);
-#pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    const bool on = (m >> j) & 1u;
-                    if (on) out[pos] = make_uint2(KB_ELEM(s0, s1, j), KB_ELEM(o0, o1, j));
-                    pos += on ? 1u : 0u;
-                }
-            }
-        }
-        tile = following;
-        it++;
-    }
-    if (bad_any) {  // a key outside the table range (cannot happen with load-time statistics): reported like a duplicate
-#pragma unroll
-        for (int k = 0; k < K; k++) if ((bad_any >> k) & 1u) *P.pat[k].outp[1] = 1u;
-    }
-}
-
-// does the star-shape kernel apply?
-static bool scan_is_star(const ScanParams& p) {
-    if (p.K > 4 || p.c.ordered) return false;  // store-order output (KOLIBRIE_ORDERED, legacy FFI): the general kernel
-    for (u32 k = 0; k < p.K; k++) {
-        const ScanPat& sp = p.pat[k];
-        const u32 shape = sp.flags & ~(SP_TABLE | SP_TKEY_O | SP_TTRUSTED | SP_PAIR);
-        if (shape != SP_HAS_P) return false;                       // constant predicate only, nothing emitted column-wise
-        if (!(sp.flags & (SP_TABLE | SP_PAIR))) return false;
-        if ((sp.flags & SP_TABLE) && (sp.flags & SP_PAIR)) return false;
-        if (sp.f_len > 1u) return false;
-        if (sp.f_len == 1u) {
-            const FilterOp& fo = p.ops[sp.f_begin];
-            if (fo.op != KB_F_CMP_NUM || (fo.slot != 0u && fo.slot != 2u) || fo.cmp < KB_CMP_GT || fo.cmp > KB_CMP_LE) return false;
-        }
-    }
-    return true;
-}
-template <int K>
-static void launch_scan_star_k(const ScanParams& p_in, int n_sms, cudaStream_t st) {
-    ScanParams p = p_in;
-    for (u32 k = 0; k < (u32)K; k++) {
-        if (p.pat[k].f_len != 1u) continue;
-        // strict comparisons become non-strict ones against the neighbouring double: a > c <=> a >= nextup(c) (c = +inf: never true -> NaN)
-        FilterOp& fo = p.ops[p.pat[k].f_begin];
-        if (fo.cmp == KB_CMP_GT) { fo.value = fo.value == HUGE_VAL ? NAN : nextafter(fo.value, HUGE_VAL); fo.cmp = KB_CMP_GE; }
-        else if (fo.cmp == KB_CMP_LT) { fo.value = fo.value == -HUGE_VAL ? NAN : nextafter(fo.value, -HUGE_VAL); fo.cmp = KB_CMP_LE; }
-    }
-    // the kernel walks the store in STAR_TILE-triple tiles: renumber the segments' first tiles
-    p.n_tiles = 0;
-    for (u32 g = 0; g < p.n_seg; g++) {
-        p.seg[g].tile0 = p.n_tiles;
-        p.n_tiles += (p.seg[g].n + (u32)STAR_TILE - 1u) / (u32)STAR_TILE;
-    }
-    const size_t smem = 2 * 3 * STAR_TILE * sizeof(u32);
-    static int grid_max = 0;
-    if (grid_max == 0) {
-        cudaFuncSetAttribute(scan_star_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        int per_sm = 1;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, scan_star_kernel<K>, STAR_THREADS, smem);
-        grid_max = (per_sm < 1 ? 1 : per_sm) * n_sms;
-    }
-    const int grid = (int)umin64((u64)grid_max, (u64)p.n_tiles);
-    scan_star_kernel<K><<<grid, STAR_THREADS, smem, st>>>(p);
-}
-
-template <int K>
-static void launch_scan_k(const ScanParams& p, int n_sms, cudaStream_t st) {
-    const size_t smem = 2 * 3 * SCAN_TILE * sizeof(u32);  // two stages: 48 KB, above the default dynamic limit
-    cudaFuncSetAttribute(scan_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    const int grid = grid_for((const void*)scan_kernel<K>, SCAN_THREADS, smem, n_sms, p.n_tiles);
-    scan_kernel<K><<<grid, SCAN_THREADS, smem, st>>>(p);
-}
-static bool scan_star_enabled() {
-    static const bool star_off = getenv("KOLIBRIE_SCAN_STAR") && getenv("KOLIBRIE_SCAN_STAR")[0] == '0';  // A/B switch
-    return !star_off;
-}
-bool scan_clears_tables(const ScanParams& p) {
-    static const bool fold_off = getenv("KOLIBRIE_SCAN_CLEAR_FOLD") && getenv("KOLIBRIE_SCAN_CLEAR_FOLD")[0] == '0';  // A/B switch
-    return !fold_off && p.n_tiles != 0 && scan_star_enabled() && scan_is_star(p);
-}
-void launch_scan(const ScanParams& p, int n_sms, cudaStream_t st) {
-    if (p.n_tiles == 0) return;
-    if (scan_star_enabled() && scan_is_star(p)) {
-        switch (p.K) {
-            case 1: launch_scan_star_k<1>(p, n_sms, st); return;
-            case 2: launch_scan_star_k<2>(p, n_sms, st); return;
-            case 3: launch_scan_star_k<3>(p, n_sms, st); return;
-            default: launch_scan_star_k<4>(p, n_sms, st); return;
-        }
-    }
-    switch (p.K) {
-        case 1: launch_scan_k<1>(p, n_sms, st); break;
-        case 2: launch_scan_k<2>(p, n_sms, st); break;
-        case 3: launch_scan_k<3>(p, n_sms, st); break;
-        case 4: launch_scan_k<4>(p, n_sms, st); break;
-        case 5: launch_scan_k<5>(p, n_sms, st); break;
-        case 6: launch_scan_k<6>(p, n_sms, st); break;
-        case 7: launch_scan_k<7>(p, n_sms, st); break;
-        default: launch_scan_k<8>(p, n_sms, st); break;
-    }
-}
 
 // =================================================================================================================
 // K_build
@@ -1008,19 +495,6 @@ void launch_pair_minmax(const uint2* kv, u32 n, u32* out4, int n_sms, cudaStream
     if (n == 0) return;
     int grid = (int)umin64((u64)n_sms * 4ull, ((u64)n + 255ull) / 256ull);
     pair_minmax_kernel<<<grid, 256, 0, st>>>(kv, n, out4);
-}
-
-__global__ void unpair_kernel(const uint2* __restrict__ kv, u32 n, u32* __restrict__ x, u32* __restrict__ y) {
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const uint2 e = kv[i];
-        x[i] = e.x;
-        y[i] = e.y;
-    }
-}
-void launch_unpair(const uint2* kv, u32 n, u32* x, u32* y, cudaStream_t st) {
-    if (n == 0) return;
-    int grid = (int)umin64(H100_SMS * 8, ((u64)n + 255) / 256);
-    unpair_kernel<<<grid, 256, 0, st>>>(kv, n, x, y);
 }
 
 __global__ void __launch_bounds__(256) col_minmax_kernel(const u32* __restrict__ col, u32 n, u32* out_min, u32* out_max) {

@@ -8,42 +8,6 @@ static inline u64 umin64(u64 a, u64 b) { return a < b ? a : b; }
 // grid-stride utility kernels are capped at a few CTAs per SM of an H100; the persistent kernels size their grids from the device's count
 constexpr u64 H100_SMS = 132;
 
-// ---------------------------------------------------------------------------------------------------------------
-// K_scan: fused multi-pattern triple scan + constant filter + pushed-down FILTER + ordered compaction.
-// Replaces execute_table_scan_with_ids (engine.rs:510-584), the index scans (engine.rs:1192-1407), QueryBuilder's
-// Exact filter scan (query_builder.rs:486-531) and the reference's hash_join_kernel (cuda_join.cu:26-45).
-#ifndef KB_SCAN_THREADS
-#define KB_SCAN_THREADS 256
-#endif
-constexpr int SCAN_THREADS = KB_SCAN_THREADS;
-constexpr int SCAN_ITEMS = 8;
-constexpr int SCAN_TILE = SCAN_THREADS * SCAN_ITEMS;  // 2048 triples = 24 KB of shared memory per CTA
-
-enum : u32 {
-    SP_HAS_S = 1, SP_HAS_P = 2, SP_HAS_O = 4,      // constant in that position
-    SP_EQ_SP = 8, SP_EQ_SO = 16, SP_EQ_PO = 32,    // same variable twice in one pattern (quirk Q4: enforced)
-    SP_EMIT_S = 64, SP_EMIT_P = 128, SP_EMIT_O = 256,  // positions written to the output (columns come out in s,p,o order)
-    SP_EMIT_IDX = 512,                              // global triple index (legacy FFI)
-    SP_PAIR = 1024,  // emit (subject, object) interleaved as uint2 into outp[0]: one 8-byte store per match (2-variable patterns)
-    // scan + build fused: the match goes straight into a direct join table, table[key - cs] = other half (cs = key base, co = key
-    // range, outp[0] = table, outp[1] = duplicate flag); no intermediate relation is written or re-read
-    SP_TABLE = 2048,
-    SP_TKEY_O = 4096,    // the join key is the object (default: the subject)
-    SP_TTRUSTED = 8192   // (kept for the A/B switch) atomicExch-with-return duplicate detection inside the scan when NOT set and KB_FUSED_ATOMIC
-};
-struct ScanPat {
-    u32 cs, cp, co;
-    u32 flags;
-    u32* outp[4];        // output column of position s / p / o / index (null when not emitted)
-    u32 f_begin, f_len;  // pushed-down FILTER program (slots = positions 0/1/2)
-};
-constexpr int SCAN_MAXSEG = 16;  // store segments one launch can walk (an RSP window of slides is scanned in ONE launch)
-struct ScanSeg {
-    const u32 *s, *p, *o;
-    u32 n;           // triples
-    u32 tile0;       // first tile of this segment in the launch's tile numbering
-    u32 index_base;  // global index of the segment's first triple
-};
 // what a compacting launch hands tile_prefix_2level (kb_device.cuh): the look-back state, the order mode, the launch's epoch, and the
 // control words {ticket, total, zero} (set by compact_setup, kb_join.cu)
 struct Compact {
@@ -55,28 +19,6 @@ struct Compact {
     u32* total;            // result row count; must be zero at launch
     const u32* zero_word;  // a word that stays zero (ordered mode reads its base from here)
 };
-struct ScanParams {
-    ScanSeg seg[SCAN_MAXSEG];
-    u32 n_seg;
-    u32 n_tiles, K;  // n_tiles: over all segments of the launch
-    u32 cshift;      // SP_TABLE patterns: log2(world) key compaction of a subject-sharded store (0 = none)
-    ScanPat pat[MAXP];
-    FilterOp ops[KB_MAX_FILTER_OPS];
-    NumTab nt;
-    // direct tables the FIRST launch of a scan clears itself (scan_star_kernel: every CTA fills a slice with 0xFF, then the grid meets
-    // at clear_barrier[0] before any insert; clear_barrier[1] is raised when the meeting timed out) — two 67 MB cudaMemsetAsync calls
-    // in front of the kernel cost two launch gaps and more time than the same bytes written by the resident grid
-    u32* clear_tab[4];
-    u32 clear_words[4];
-    u32 n_clear;
-    u32* clear_barrier;
-    Compact c;         // total / zero_word unused: the scan counts per pattern in totals_in / totals_out
-    u32* ticket;
-    const u32* totals_in;  // [MAXP] rows written by earlier segments
-    u32* totals_out;       // [MAXP] rows written so far (ordered: a different array than totals_in; unordered: the same, used as atomic cursor)
-};
-void launch_scan(const ScanParams& p, int n_sms, cudaStream_t st);
-bool scan_clears_tables(const ScanParams& p);  // true when launch_scan(p) runs the kernel that honours clear_tab / n_clear
 
 // ---------------------------------------------------------------------------------------------------------------
 // K_build
@@ -206,7 +148,6 @@ struct ProbeIParams {
 struct GroupParams;
 // agg == nullptr: the joined rows are written to p.out; else they are folded into the group table *agg (GROUP BY column p.gsel)
 void launch_probe_index(const ProbeIParams& p, const GroupParams* agg, int n_sms, cudaStream_t st);
-void launch_unpair(const uint2* kv, u32 n, u32* x, u32* y, cudaStream_t st);
 // direct build from a predicate slice of the store index, with the pattern's pushed-down FILTER evaluated on (s, P, o)
 struct BuildPairsParams {
     const uint2* kv;

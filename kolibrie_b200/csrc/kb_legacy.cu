@@ -34,7 +34,7 @@ static kb_status legacy_select(kb_ctx* ctx, const u32* h_p, const u32* h_o, u32 
     pt.o = literal ? kb_term{0, *literal} : kb_term{1, 1};
     std::vector<std::unique_ptr<kb_rel>> rels;
     std::vector<FilterProg> none;
-    KB_TRY(scan_impl(ctx, {sg}, &pt, 1, none, /*use_index=*/false, /*row_index=*/true, false, &rels));
+    KB_TRY(scan_segments(ctx, {sg}, &pt, 1, none, ScanOut::RowIndex, &rels));
     const u64 m = rels[0]->n;
     u32* idx = static_cast<u32*>(malloc(std::max<size_t>(m * sizeof(u32), 4)));
     if (!idx) return fail(ctx, KB_E_OOM, "malloc failed");

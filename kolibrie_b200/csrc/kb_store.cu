@@ -253,11 +253,8 @@ static kb_status index_add_segment(kb_ctx* ctx, size_t seg_idx, bool full_build,
     const std::vector<Segment> one{sg};
     for (size_t b = 0; b < preds.size(); b += MAXP) {
         const u32 k = (u32)std::min<size_t>(MAXP, preds.size() - b);
-        kb_pattern pats[MAXP];
-        for (u32 i = 0; i < k; i++) { pats[i].s = kb_term{1, 0}; pats[i].p = kb_term{0, preds[b + i]}; pats[i].o = kb_term{1, 1}; }
         std::vector<std::unique_ptr<kb_rel>> rels;
-        std::vector<FilterProg> none;
-        KB_TRY(scan_impl(ctx, one, pats, k, none, /*use_index=*/false, false, true, &rels));
+        KB_TRY(scan_predicates(ctx, one, preds.data() + b, k, ScanOut::Pairs, &rels));
         const u32 soff = ctrl_alloc(ctx, 4 * MAXP);
         KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + soff, 0, 4 * MAXP * sizeof(u32), ctx->st));
         for (u32 i = 0; i < k; i++) KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + soff + 4 * i, 0xFF, 2 * sizeof(u32), ctx->st));
@@ -607,7 +604,7 @@ kb_status kb_store_delete(kb_ctx* ctx, const uint32_t* s, const uint32_t* p, con
         }
         // rescan this one segment
         std::vector<std::unique_ptr<kb_rel>> rels;
-        KB_TRY(kb::scan_impl(ctx, {marked}, &pt, 1, pd, /*use_index=*/false, false, false, &rels));
+        KB_TRY(kb::scan_segments(ctx, {marked}, &pt, 1, pd, kb::ScanOut::Cols, &rels));
         kb::Segment ns;
         ns.tag = sg.tag;
         ns.n = rels[0]->n;

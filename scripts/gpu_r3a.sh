@@ -1,8 +1,2 @@
 #!/bin/bash
 timeout 1200 python -m pytest tests -m gpu -x -q 2>&1 | tail -4
-for f in 1 0; do
-KOLIBRIE_SCAN_CLEAR_FOLD=$f python bench.py --no-cpu --no-e2e --no-adversarial --no-configs 2>/dev/null | python -c "
-import json,sys
-l=json.loads(sys.stdin.read().strip().splitlines()[-1]); s=l['scan_path']
-print('fold $f: scan_path', s['value'], s['ms_per_step'], 'scan+build frac', s['roofline']['frac'], {k:(v.get('ms'), v.get('frac')) for k,v in s['roofline'].get('families',{}).items()})"
-done
