@@ -200,6 +200,30 @@ KB_API kb_status kb_store_append_device(kb_ctx* ctx, const uint32_t* d_s, const 
 KB_API kb_status kb_store_evict(kb_ctx* ctx, uint64_t segment_tag);
 /* set-difference by value (SparqlDatabase::delete_triple, sparql_database.rs:229-242) */
 KB_API kb_status kb_store_delete(kb_ctx* ctx, const uint32_t* s, const uint32_t* p, const uint32_t* o, uint64_t n);
+/* Set-semantic writes: the store as the reference's BTreeSet (SparqlDatabase::add_triple / delete_triple, sparql_database.rs:215-226),
+ * changed in place. A call that changes the store bumps its version exactly as any other mutation does; a call that changes nothing
+ * (every triple already there, none there to remove) does not. An indexed store stays indexed: the segments a call replaces leave the
+ * predicate slices and the persistent tables as an evicted one does, the segments it adds come in as a window slide's do; a slice that
+ * cannot be maintained drops the index, as the appends do. Refused with the store unchanged: NULL columns with n > 0 or a triple
+ * holding KB_ID_NONE (KB_E_INVALID, the message naming the position, as the appends do); a batch of more than 2^30 triples (for the
+ * template: relation rows x patterns) or a store reaching 2^32-16 triples (KB_E_LIMIT). */
+/* BTreeSet::insert for each triple, in batch order. inserted[i] = 1 iff triple i was in neither the store nor an earlier entry of this
+ * batch (inserted may be NULL). The new triples, in batch order, go into a segment tagged segment_tag; it absorbs the latest segments
+ * of that tag while each holds at most twice the triples gathered so far, so that many small inserts leave O(log n) segments. */
+KB_API kb_status kb_store_insert(kb_ctx* ctx, const uint32_t* s, const uint32_t* p, const uint32_t* o, uint64_t n, uint64_t segment_tag,
+                                 uint8_t* inserted, uint64_t* n_inserted);
+/* BTreeSet::remove for each triple, in batch order. removed[i] = 1 iff triple i was in the store and no earlier entry of the batch
+ * removed it (removed may be NULL). Every stored copy goes, whatever segment or tag holds it; segments without one stay as they are. */
+KB_API kb_status kb_store_remove(kb_ctx* ctx, const uint32_t* s, const uint32_t* p, const uint32_t* o, uint64_t n, uint8_t* removed,
+                                 uint64_t* n_removed);
+/* DELETE { template } WHERE { ... } (kolibrie/src/execute_query.rs:354-413): each of the n_tmpl (at most 16) template patterns is
+ * filled from every row of rel — constants as given, variables from rel's columns — row by row, and the triples are removed as one
+ * kb_store_remove batch; *n_removed counts the triples that were in the store. Refused with KB_E_UNSUPPORTED, store unchanged: a
+ * template variable that is not a column of rel; a variable cell that is unbound (the reference deletes the variable's name as a
+ * term), or whose term the reference, which decodes each binding and encodes it again with encode_term_star, would turn into another
+ * id: a quoted id, an id without a string in the device dictionary, a string with surrounding whitespace, one that starts with '<' and
+ * ends with '>' (so also "<< s p o >>"), one that starts with '"'. */
+KB_API kb_status kb_store_remove_template(kb_ctx* ctx, const kb_rel* rel, const kb_pattern* tmpl, uint32_t n_tmpl, uint64_t* n_removed);
 KB_API kb_status kb_store_clear(kb_ctx* ctx);
 /* SparqlDatabase::build_all_indexes (kolibrie/src/sparql_database.rs:3364-3394) on the device: partitions the store by predicate into
  * interleaved (subject, object) slices — what the reference's pos/pso indexes give an index scan of `?s P ?o` (engine.rs:1364-1378).

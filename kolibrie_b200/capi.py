@@ -264,6 +264,9 @@ def lib() -> C.CDLL:
         "kb_store_append": (i32, [vp, vp, vp, vp, u64, u64]),
         "kb_store_evict": (i32, [vp, u64]),
         "kb_store_delete": (i32, [vp, vp, vp, vp, u64]),
+        "kb_store_insert": (i32, [vp, vp, vp, vp, u64, u64, vp, P(u64)]),
+        "kb_store_remove": (i32, [vp, vp, vp, vp, u64, vp, P(u64)]),
+        "kb_store_remove_template": (i32, [vp, vp, P(KbPattern), u32, P(u64)]),
         "kb_store_clear": (i32, [vp]),
         "kb_store_build_index": (i32, [vp, P(u32), P(C.c_double)]),
         "kb_set_use_index": (i32, [vp, C.c_int]),
@@ -354,7 +357,7 @@ def lib() -> C.CDLL:
 
 EXPORTED_SYMBOLS = [
     "kb_version", "kb_ctx_create", "kb_ctx_destroy", "kb_last_error", "kb_set_timing", "kb_get_stats", "kb_synchronize",
-    "kb_store_load", "kb_store_load_device", "kb_store_append", "kb_store_append_device", "kb_store_evict", "kb_store_delete", "kb_store_clear", "kb_store_build_index", "kb_set_use_index", "kb_store_size",
+    "kb_store_load", "kb_store_load_device", "kb_store_append", "kb_store_append_device", "kb_store_evict", "kb_store_delete", "kb_store_insert", "kb_store_remove", "kb_store_remove_template", "kb_store_clear", "kb_store_build_index", "kb_set_use_index", "kb_store_size",
     "kb_store_download", "kb_dict_numeric_load", "kb_dict_legacy_i32_load", "kb_dict_numeric_derive", "kb_dict_numeric_download", "kb_dict_strings_load", "kb_dict_encode", "kb_dict_strings_info", "kb_rel_decode", "kb_strings_info", "kb_strings_download", "kb_strings_free", "kb_quoted_load", "kb_quoted_download", "kb_dict_strings_download", "kb_serialize_begin", "kb_serialize_next", "kb_serialize_free", "kb_bind", "kb_rel_info", "kb_rel_download", "kb_rel_device_col", "kb_rel_from_host",
     "kb_rel_from_device", "kb_rel_free", "kb_scan", "kb_filter", "kb_project", "kb_hash_join", "kb_natural_join", "kb_hash_join_keyed", "kb_values", "kb_bind_join", "kb_scan_quoted", "kb_star_join", "kb_bgp_execute", "kb_bgp_last_plan",
     "kb_order_by", "kb_group_aggregate", "kb_groups_info", "kb_groups_keys", "kb_groups_values", "kb_groups_counts", "kb_groups_free", "kb_groups_pack", "kb_groups_merge", "kb_star_join_aggregate",
@@ -500,6 +503,31 @@ class Context:
     def store_delete(self, s, p, o):
         s, p, o = _u32(s), _u32(p), _u32(o)
         self._check(lib().kb_store_delete(self.h, _ptr(s), _ptr(p), _ptr(o), len(s)))
+
+    def store_insert(self, s, p, o, tag: int = 0) -> np.ndarray:
+        """kb_store_insert: BTreeSet::insert of each triple in batch order. Returns inserted[i] (bool): triple i was in neither the
+        store nor an earlier entry of the batch. The new triples go into a segment tagged `tag`."""
+        s, p, o = _u32(s), _u32(p), _u32(o)
+        flags = np.zeros(len(s), dtype=np.uint8)
+        n = C.c_uint64()
+        self._check(lib().kb_store_insert(self.h, _ptr(s), _ptr(p), _ptr(o), len(s), tag, _ptr(flags), C.byref(n)))
+        return flags.astype(bool)
+
+    def store_remove(self, s, p, o) -> np.ndarray:
+        """kb_store_remove: BTreeSet::remove of each triple in batch order. Returns removed[i] (bool): triple i was in the store and
+        no earlier entry of the batch removed it."""
+        s, p, o = _u32(s), _u32(p), _u32(o)
+        flags = np.zeros(len(s), dtype=np.uint8)
+        n = C.c_uint64()
+        self._check(lib().kb_store_remove(self.h, _ptr(s), _ptr(p), _ptr(o), len(s), _ptr(flags), C.byref(n)))
+        return flags.astype(bool)
+
+    def store_remove_template(self, rel: Relation, tmpl: Sequence[KbPattern]) -> int:
+        """kb_store_remove_template: DELETE { tmpl } WHERE { ... } with the WHERE's bindings in `rel`. Returns the triples removed."""
+        arr = patterns(tmpl)
+        n = C.c_uint64()
+        self._check(lib().kb_store_remove_template(self.h, rel.h, arr, len(tmpl), C.byref(n)))
+        return n.value
 
     def store_clear(self):
         self._check(lib().kb_store_clear(self.h))

@@ -123,6 +123,7 @@ struct kb_groups {  // (kb_group.cu)
 namespace kb {
 struct Segment {
     u64 tag = 0;
+    u64 id = 0;  // unique within the context, given when the segment joins the store: the index chunks built from it carry it
     Col s, p, o;
     u64 n = 0;
     cudaEvent_t ready = nullptr;  // set while a chunked upload is in flight: the scan waits on it
@@ -141,6 +142,7 @@ struct Segment {
 namespace kb {
 struct SliceChunk {  // the rows of ONE store segment that carry the predicate: interleaved (subject, object)
     u64 tag = 0;           // the segment's tag (kb_store_append): evicting the segment drops the chunk
+    u64 seg = 0;           // the segment's id: a set-semantic write that compacts or merges the segment replaces the chunk
     Col pairs;
     u64 n = 0;
     Buf ynum;              // typed literal column: f64 value of every object (num_or0), kept when the chunk has numeric objects
@@ -191,6 +193,7 @@ struct kb_ctx {
     // hint sets and the index below
     std::vector<kb::Segment> segs;
     kb::u64 n_triples = 0;
+    kb::u64 seg_ids = 0;  // the last Segment::id given
     kb::Buf num, isnum;
     kb::Buf i32val, isi32;  // kb_dict_legacy_i32_load: the legacy executor's integer view of the terms
     kb::u32 n_i32 = 0;

@@ -2598,6 +2598,158 @@ void launch_delete_mark(const u32* s, const u32* p, const u32* o, u32 n, const u
     delete_mark_kernel<<<grid, 256, 0, st>>>(s, p, o, n, set, set_slots, p_out);
 }
 
+// ---- kb_store_insert / kb_store_remove: the batch as a key set (the layout of set_insert, so that delete_mark reads it too), the
+// batch index of each key's first occurrence, and a found bit per key set by one pass over the store
+// set_insert that returns the key's slot, whether it was inserted now or found (EMPTY32: the set is full)
+__device__ __forceinline__ u32 set_insert_slot(uint4* set, u32 n_slots, u32 s, u32 p, u32 o) {
+    const u32 mask = n_slots - 1u;
+    u32 slot = set_hash(s, p, o) & mask;
+    for (u32 probes = 0; probes < n_slots; probes++) {
+        u32* st_ptr = &reinterpret_cast<u32*>(&set[slot])[3];
+        u32 st = atomicCAS(st_ptr, 0u, 1u);
+        if (st == 0u) {
+            u32* w = reinterpret_cast<u32*>(&set[slot]);
+            w[0] = s; w[1] = p; w[2] = o;
+            __threadfence();
+            atomicExch(st_ptr, 2u);
+            return slot;
+        }
+        while (st == 1u) st = *reinterpret_cast<volatile u32*>(st_ptr);
+        __threadfence();
+        const volatile u32* w = reinterpret_cast<const volatile u32*>(&set[slot]);
+        if (w[0] == s && w[1] == p && w[2] == o) return slot;
+        slot = (slot + 1u) & mask;
+    }
+    return EMPTY32;
+}
+__global__ void __launch_bounds__(256) batch_set_kernel(uint4* set, u32 set_slots, const u32* s, const u32* p, const u32* o, u32 n, u32* first,
+                                                        u32* slot_of, u32* overflow) {
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const u32 slot = set_insert_slot(set, set_slots, s[i], p[i], o[i]);
+        slot_of[i] = slot;
+        if (slot == EMPTY32) *overflow = 1u;
+        else atomicMin(&first[slot], i);
+    }
+}
+void launch_batch_set(uint4* set, u32 set_slots, const u32* s, const u32* p, const u32* o, u32 n, u32* first, u32* slot_of, u32* overflow,
+                      int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull);
+    batch_set_kernel<<<grid, 256, 0, st>>>(set, set_slots, s, p, o, n, first, slot_of, overflow);
+}
+
+__global__ void __launch_bounds__(256) batch_mark_kernel(const u32* __restrict__ s, const u32* __restrict__ p, const u32* __restrict__ o, u32 n,
+                                                         const uint4* __restrict__ set, u32 set_slots, u32* found, u32* hits) {
+    const u32 mask = set_slots - 1u;
+    u32 mine = 0;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const u32 vs = s[i], vp = p[i], vo = o[i];
+        u32 slot = set_hash(vs, vp, vo) & mask;
+        for (u32 probes = 0; probes < set_slots; probes++) {
+            const uint4 e = set[slot];
+            if (e.w == 0u) break;
+            if (e.x == vs && e.y == vp && e.z == vo) { found[slot] = 1u; mine++; break; }
+            slot = (slot + 1u) & mask;
+        }
+    }
+    if (mine) atomicAdd(hits, mine);
+}
+void launch_batch_mark(const u32* s, const u32* p, const u32* o, u32 n, const uint4* set, u32 set_slots, u32* found, u32* hits, int n_sms,
+                       cudaStream_t st) {
+    if (n == 0) return;
+    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull);
+    batch_mark_kernel<<<grid, 256, 0, st>>>(s, p, o, n, set, set_slots, found, hits);
+}
+
+__global__ void __launch_bounds__(256) batch_flags_kernel(u32 n, const u32* slot_of, const u32* first, const u32* found, u32 want_found, u8* flag8,
+                                                          u32* flag32, u32* count) {
+    u32 mine = 0;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const u32 slot = slot_of[i];
+        const bool f = slot != EMPTY32 && first[slot] == i && (found[slot] != 0u) == (want_found != 0u);
+        flag8[i] = f ? 1 : 0;
+        flag32[i] = f ? 1u : 0u;
+        mine += f ? 1u : 0u;
+    }
+    if (mine) atomicAdd(count, mine);
+}
+void launch_batch_flags(u32 n, const u32* slot_of, const u32* first, const u32* found, bool want_found, u8* flag8, u32* flag32, u32* count, int n_sms,
+                        cudaStream_t st) {
+    if (n == 0) return;
+    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull);
+    batch_flags_kernel<<<grid, 256, 0, st>>>(n, slot_of, first, found, want_found ? 1u : 0u, flag8, flag32, count);
+}
+
+__global__ void __launch_bounds__(256) batch_gather_kernel(const u32* s, const u32* p, const u32* o, u32 n, const u8* flag8, const u32* pos, u32* out_s,
+                                                           u32* out_p, u32* out_o) {
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        if (!flag8[i]) continue;
+        const u32 k = pos[i];
+        out_s[k] = s[i]; out_p[k] = p[i]; out_o[k] = o[i];
+    }
+}
+void launch_batch_gather(const u32* s, const u32* p, const u32* o, u32 n, const u8* flag8, const u32* pos, u32* out_s, u32* out_p, u32* out_o, int n_sms,
+                         cudaStream_t st) {
+    if (n == 0) return;
+    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull);
+    batch_gather_kernel<<<grid, 256, 0, st>>>(s, p, o, n, flag8, pos, out_s, out_p, out_o);
+}
+
+// kb_store_remove_template: triple (row r, template pattern t) at r * n_tmpl + t. bad[0] counts unbound cells; bad[1] the cells whose
+// term the reference would not re-encode to the same id (execute_query.rs:398-403 decodes every binding and encodes it again with
+// encode_term_star): a quoted id (its rendering is re-parsed), an id the device dictionary does not hold, or a string that
+// encode_term_star changes: surrounding whitespace, '<' ... '>' (and so "<< ... >>"), a leading '"'
+__device__ __forceinline__ bool reencodes_to_itself(u32 id, const DictTab& d) {
+    if ((id & 0x80000000u) || id >= d.ids) return false;
+    const unsigned long long a = d.off[id], b = d.off[id + 1];
+    if (a == b) return true;
+    const unsigned char c0 = d.bytes[a], c1 = d.bytes[b - 1];
+    // Rust's str::trim: char::is_whitespace (U+0009..U+000D, U+0020, U+0085, U+00A0, U+1680, U+2000..U+200A, U+2028, U+2029, U+202F,
+    // U+205F, U+3000) at either end
+    const auto ws_cp = [](u32 cp) {
+        return (cp >= 0x09 && cp <= 0x0D) || cp == 0x20 || cp == 0x85 || cp == 0xA0 || cp == 0x1680 || (cp >= 0x2000 && cp <= 0x200A) ||
+               cp == 0x2028 || cp == 0x2029 || cp == 0x202F || cp == 0x205F || cp == 0x3000;
+    };
+    const auto cp_at = [&](unsigned long long i, u32 len) {  // the code point of the len-byte UTF-8 sequence at i (EMPTY32: not one)
+        if (i + len > b) return EMPTY32;
+        const unsigned char x = d.bytes[i];
+        u32 cp = len == 1 ? x : len == 2 ? (x & 0x1Fu) : (x & 0x0Fu);
+        for (u32 k = 1; k < len; k++) cp = (cp << 6) | (d.bytes[i + k] & 0x3Fu);
+        return cp;
+    };
+    const u32 lead = c0 < 0x80 ? 1u : (c0 & 0xE0) == 0xC0 ? 2u : (c0 & 0xF0) == 0xE0 ? 3u : 4u;
+    if (lead <= 3 && ws_cp(cp_at(a, lead))) return false;
+    u32 tail = 1;  // the last character starts at the last byte that is not a continuation byte
+    while (tail < 4 && tail < b - a && (d.bytes[b - tail] & 0xC0) == 0x80) tail++;
+    if (tail <= 3 && ws_cp(cp_at(b - tail, tail))) return false;
+    if (c0 == '<' && c1 == '>') return false;
+    return c0 != '"';
+}
+__global__ void __launch_bounds__(256) template_fill_kernel(const __grid_constant__ TemplateFillParams P) {
+    const u64 total = (u64)P.rows * P.n_tmpl;
+    u32 unbound = 0, changes = 0;
+    for (u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x; k < total; k += (u64)gridDim.x * blockDim.x) {
+        const u32 r = (u32)(k / P.n_tmpl), t = (u32)(k % P.n_tmpl);
+        u32 v[3];
+        for (int c = 0; c < 3; c++) {
+            const u32* col = P.col[t][c];
+            v[c] = col ? col[r] : P.cval[t][c];
+            if (!col) continue;
+            if (v[c] == EMPTY32) unbound++;
+            else if (!reencodes_to_itself(v[c], P.dict)) changes++;
+        }
+        P.s[k] = v[0]; P.p[k] = v[1]; P.o[k] = v[2];
+    }
+    if (unbound) atomicAdd(&P.bad[0], unbound);
+    if (changes) atomicAdd(&P.bad[1], changes);
+}
+void launch_template_fill(const TemplateFillParams& P, int n_sms, cudaStream_t st) {
+    const u64 total = (u64)P.rows * P.n_tmpl;
+    if (total == 0) return;
+    const int grid = (int)umin64((u64)n_sms * 8ull, (total + 255ull) / 256ull);
+    template_fill_kernel<<<grid, 256, 0, st>>>(P);
+}
+
 // =================================================================================================================
 // Relation-to-Stream operators (kb_r2s_eval). Row indices are 64-bit in the loops: a response may hold up to 2^32-1 rows.
 __device__ __forceinline__ u64 r2s_mix64(u64 x) {  // murmur3 64-bit finaliser

@@ -510,5 +510,32 @@ void launch_part_scatter(const u32* key, u32 n, u32 n_parts, u32* cursors, const
 // mark rows of a segment that equal any triple of a (small) delete set held in a 96-bit set; then compaction is a scan with flags
 void launch_delete_mark(const u32* s, const u32* p, const u32* o, u32 n, const uint4* set, u32 set_slots, u32* p_out /*p with EMPTY32 where deleted*/,
                         int n_sms, cudaStream_t st);
+// kb_store_insert / kb_store_remove (kb_store.cu). The batch's keys go into a set laid out as launch_set_insert's (set_slots a power of
+// two, zeroed); slot_of[i] = the slot of triple i, first[slot] (set to EMPTY32 before) = the smallest batch index holding that key;
+// *overflow = 1 when the set is full
+void launch_batch_set(uint4* set, u32 set_slots, const u32* s, const u32* p, const u32* o, u32 n, u32* first, u32* slot_of, u32* overflow,
+                      int n_sms, cudaStream_t st);
+// one stored segment against the batch set: found[slot] = 1 for every key the segment holds, *hits += its triples that match a key
+void launch_batch_mark(const u32* s, const u32* p, const u32* o, u32 n, const uint4* set, u32 set_slots, u32* found, u32* hits, int n_sms,
+                       cudaStream_t st);
+// flag[i] = 1 iff triple i is the first of its key in the batch and found[its slot] equals want_found; *count += the flags set.
+// flag8 is what the caller reads back, flag32 what an exclusive scan turns into output positions
+void launch_batch_flags(u32 n, const u32* slot_of, const u32* first, const u32* found, bool want_found, u8* flag8, u32* flag32, u32* count, int n_sms,
+                        cudaStream_t st);
+// out[pos[i]] = triple i for every flagged i (batch order is kept: pos is the exclusive scan of the flags)
+void launch_batch_gather(const u32* s, const u32* p, const u32* o, u32 n, const u8* flag8, const u32* pos, u32* out_s, u32* out_p, u32* out_o, int n_sms,
+                         cudaStream_t st);
+// kb_store_remove_template: one triple per (relation row, template pattern); col[t][c] null: position c of pattern t is the constant
+// cval[t][c]. bad[0] += the variable cells that are unbound, bad[1] += those whose term would not re-encode to the same id
+constexpr u32 TEMPLATE_MAX = 16;
+struct TemplateFillParams {
+    const u32* col[TEMPLATE_MAX][3];
+    u32 cval[TEMPLATE_MAX][3];
+    u32 n_tmpl, rows;
+    u32 *s, *p, *o;
+    DictTab dict;
+    u32* bad;
+};
+void launch_template_fill(const TemplateFillParams& P, int n_sms, cudaStream_t st);
 
 }  // namespace kb

@@ -1,7 +1,7 @@
 // kb_store.cu — the device triple store: its segments, the version that everything derived from it is keyed to (prepared plans, the
 // seeded fixpoint's state, kb_datalog_maintain's closed token), the per-version hints of the star-join builds and the
 // predicate-partitioned index. This file is the only writer of that state: every change to the store goes through store_replace,
-// store_add_device_segment or store_evict_tag, which bump the version, drop the hints and maintain or drop the index.
+// store_add_device_segment, store_evict_tag or store_swap, which bump the version, drop the hints and maintain or drop the index.
 #include <algorithm>
 #include <chrono>
 #include <cstdlib>
@@ -129,6 +129,7 @@ static kb_status index_add_segment_split(kb_ctx* ctx, const Segment& sg, u32 csh
         PredSlice& ps = ctx->index[sg.pred_rows[i].first];
         SliceChunk& ch = chs[i];
         ch.tag = sg.tag;
+        ch.seg = sg.id;
         ch.n = sg.pred_rows[i].second;
         KB_TRY(alloc_col(ctx, 2 * ch.n, &ch.pairs));
         if (ctx->n_ids) KB_TRY(alloc_buf(ctx, ch.n * sizeof(double), &ch.ynum));
@@ -264,6 +265,7 @@ static kb_status index_add_segment(kb_ctx* ctx, size_t seg_idx, bool full_build,
             PredSlice& ps = ctx->index[preds[b + i]];
             SliceChunk ch;
             ch.tag = sg.tag;
+            ch.seg = sg.id;
             ch.n = rels[i]->n;
             KB_TRY(alloc_col(ctx, 2 * ch.n, &ch.pairs));
             KB_CUDA(ctx, cudaMemcpyAsync(ch.pairs.ptr, rels[i]->cols[0].ptr, ch.n * sizeof(uint2), cudaMemcpyDeviceToDevice, ctx->st));
@@ -323,8 +325,10 @@ static kb_status index_add_segment(kb_ctx* ctx, size_t seg_idx, bool full_build,
     return KB_OK;
 }
 
-// eviction of the segment(s) tagged `tag`: their chunks leave the slices, their keys leave the persistent tables
-static kb_status index_evict_tag(kb_ctx* ctx, u64 tag) {
+// eviction of the chunks `dies` selects (those of the segments tagged `tag`, or of given segments): they leave the slices, their keys
+// leave the persistent tables
+template <class Dies>
+static kb_status index_evict(kb_ctx* ctx, Dies dies) {
     ClearParams C{};
     std::vector<SliceChunk> dying;  // kept until the clears are queued: their buffers are released stream-ordered behind them
     auto flush = [&]() {
@@ -336,7 +340,7 @@ static kb_status index_evict_tag(kb_ctx* ctx, u64 tag) {
         bool hit = false;
         for (size_t c = 0; c < ps.chunks.size();) {
             SliceChunk& ch = ps.chunks[c];
-            if (ch.tag != tag) { c++; continue; }
+            if (!dies(ch)) { c++; continue; }
             hit = true;
             if ((ps.xtab || ps.ytab) && ch.n) {
                 ClearEntry& e = C.e[C.k++];
@@ -385,6 +389,7 @@ static void drop_index(kb_ctx* ctx) {
 
 void store_replace(kb_ctx* ctx, std::vector<Segment> segs) {
     ctx->segs = std::move(segs);
+    for (auto& sg : ctx->segs) sg.id = ++ctx->seg_ids;
     ctx->n_triples = 0;
     for (auto& sg : ctx->segs) ctx->n_triples += sg.n;
     bump_version(ctx);
@@ -394,6 +399,7 @@ void store_replace(kb_ctx* ctx, std::vector<Segment> segs) {
 kb_status store_add_device_segment(kb_ctx* ctx, Segment& sg, bool keep_index) {
     if (keep_index && sg.n && !sg.has_stats) KB_TRY(segment_stats(ctx, &sg));
     const bool maintain = keep_index && index_maintainable(ctx);
+    sg.id = ++ctx->seg_ids;
     ctx->segs.push_back(sg);
     ctx->n_triples += sg.n;
     bump_version(ctx);
@@ -421,9 +427,208 @@ bool store_evict_tag(kb_ctx* ctx, u64 tag, bool keep_index) {
     }
     const bool maintain = keep_index && index_maintainable(ctx);
     bump_version(ctx);
-    if (maintain && index_evict_tag(ctx, tag) == KB_OK) ctx->index_version = ctx->store_version;
+    if (maintain && index_evict(ctx, [tag](const SliceChunk& ch) { return ch.tag == tag; }) == KB_OK) ctx->index_version = ctx->store_version;
     else drop_index(ctx);
     return found;
+}
+
+// one new store version in which the segments at `out` (indices into ctx->segs) are replaced by `in` (empty ones are left out). The
+// index is maintained when it describes the store: the chunks of the replaced segments leave it as an eviction's do and every new
+// segment comes in as a slide's does; a slice it cannot maintain drops the whole index.
+static kb_status store_swap(kb_ctx* ctx, std::vector<size_t> out, std::vector<Segment> in) {
+    for (auto& sg : in) if (sg.n && !sg.has_stats) KB_TRY(segment_stats(ctx, &sg));
+    bool maintain = index_maintainable(ctx);
+    std::set<u64> gone;
+    std::sort(out.rbegin(), out.rend());
+    for (size_t i : out) {
+        gone.insert(ctx->segs[i].id);
+        ctx->n_triples -= ctx->segs[i].n;
+        ctx->segs.erase(ctx->segs.begin() + i);
+    }
+    bump_version(ctx);
+    kb_status rc = KB_OK;
+    if (maintain && !gone.empty()) maintain = index_evict(ctx, [&gone](const SliceChunk& ch) { return gone.count(ch.seg) != 0; }) == KB_OK;
+    for (auto& sg : in) {
+        if (!sg.n) continue;
+        sg.id = ++ctx->seg_ids;
+        ctx->segs.push_back(sg);
+        ctx->n_triples += sg.n;
+        if (!maintain) continue;
+        bool indexable = true;
+        rc = index_add_segment(ctx, ctx->segs.size() - 1, /*full_build=*/false, &indexable);
+        maintain = rc == KB_OK && indexable;
+    }
+    if (maintain) ctx->index_version = ctx->store_version;
+    else drop_index(ctx);
+    return rc;
+}
+
+// the triples of `sg` that are not in the 96-bit set (kb_store_delete's compaction): a copy of the predicate column with KB_ID_NONE
+// where a triple is in the set, then a rescan with (?s ?p ?o) — a row whose predicate is KB_ID_NONE can never equal a real constant,
+// and the pattern's pushed-down filter NE_ID drops it
+static kb_status segment_without(kb_ctx* ctx, const Segment& sg, const Buf& set, u32 set_slots, Segment* out) {
+    static const kb_pattern pt{{1, 0}, {1, 1}, {1, 2}};
+    FilterProg keep;
+    kb_filter_op ne{};
+    ne.op = KB_F_NE_ID; ne.slot = 1; ne.id = KB_ID_NONE;  // true for every bound predicate; a marked one reads as unbound: false
+    keep.ops.push_back(ne);
+    const std::vector<FilterProg> pd{keep};
+    Segment marked = sg;
+    if (sg.n) {
+        KB_TRY(alloc_col(ctx, sg.n, &marked.p));
+        launch_delete_mark(sg.s.ptr, sg.p.ptr, sg.o.ptr, (u32)sg.n, static_cast<const uint4*>(set->p), set_slots, marked.p.ptr, ctx->n_sms, ctx->st);
+    }
+    std::vector<std::unique_ptr<kb_rel>> rels;
+    KB_TRY(scan_segments(ctx, {marked}, &pt, 1, pd, ScanOut::Cols, &rels));
+    *out = Segment{};
+    out->tag = sg.tag;
+    out->n = rels[0]->n;
+    out->s = rels[0]->cols[0]; out->p = rels[0]->cols[1]; out->o = rels[0]->cols[2];
+    return KB_OK;
+}
+
+// ---- set-semantic writes (kb_store_insert, kb_store_remove, kb_store_remove_template) over a batch in device memory
+// the batch's key set has a power of two >= 2n slots and pow2_at_least stops at 2^31: larger batches are refused up front
+constexpr u64 BATCH_MAX = 1ull << 30;
+struct BatchMark {
+    Buf set, first, slot_of, found, flag8, flag32;
+    u32 slots = 0, n = 0;
+    u32 n_flagged = 0;                // triples of the batch the call acts on
+    std::vector<u32> seg_hits;        // per segment of ctx->segs: its triples that equal a key of the batch
+};
+
+// The batch's key set, one mark pass over every segment, and the per-triple flags: want_found = false flags each triple that is in
+// neither the store nor an earlier entry of the batch (BTreeSet::insert), true each that is in the store and not earlier in the batch
+// (BTreeSet::remove).
+static kb_status batch_mark(kb_ctx* ctx, const u32* s, const u32* p, const u32* o, u32 n, bool want_found, BatchMark* b) {
+    b->n = n;
+    b->slots = pow2_at_least((u64)n * 2);
+    KB_TRY(alloc_buf(ctx, (size_t)b->slots * sizeof(uint4), &b->set));
+    KB_TRY(alloc_buf(ctx, (size_t)b->slots * sizeof(u32), &b->first));
+    KB_TRY(alloc_buf(ctx, (size_t)b->slots * sizeof(u32), &b->found));
+    KB_TRY(alloc_buf(ctx, (size_t)n * sizeof(u32), &b->slot_of));
+    KB_TRY(alloc_buf(ctx, (size_t)n, &b->flag8));
+    KB_TRY(alloc_buf(ctx, ((size_t)n + 1) * sizeof(u32), &b->flag32));
+    KB_CUDA(ctx, cudaMemsetAsync(b->set->p, 0, (size_t)b->slots * sizeof(uint4), ctx->st));
+    KB_CUDA(ctx, cudaMemsetAsync(b->first->p, 0xFF, (size_t)b->slots * sizeof(u32), ctx->st));
+    KB_CUDA(ctx, cudaMemsetAsync(b->found->p, 0, (size_t)b->slots * sizeof(u32), ctx->st));
+    KB_CUDA(ctx, cudaMemsetAsync(static_cast<u32*>(b->flag32->p) + n, 0, sizeof(u32), ctx->st));
+    const size_t nseg = ctx->segs.size();
+    Buf hits;
+    KB_TRY(alloc_buf(ctx, (nseg + 1) * sizeof(u32), &hits));
+    KB_CUDA(ctx, cudaMemsetAsync(hits->p, 0, (nseg + 1) * sizeof(u32), ctx->st));
+    const u32 c = ctrl_alloc(ctx, 2);  // [0] set overflow, [1] flagged triples
+    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + c, 0, 2 * sizeof(u32), ctx->st));
+    int launches = 2;  // the set and the flags, and one mark pass per non-empty segment
+    for (auto& sg : ctx->segs) launches += sg.n ? 1 : 0;
+    timer_begin(ctx, F_OTHER, launches);
+    launch_batch_set(static_cast<uint4*>(b->set->p), b->slots, s, p, o, n, static_cast<u32*>(b->first->p), static_cast<u32*>(b->slot_of->p), ctx->ctrl + c,
+                     ctx->n_sms, ctx->st);
+    for (size_t g = 0; g < nseg; g++) {
+        const Segment& sg = ctx->segs[g];
+        if (sg.ready) KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st, sg.ready, 0));
+        launch_batch_mark(sg.s.ptr, sg.p.ptr, sg.o.ptr, (u32)sg.n, static_cast<const uint4*>(b->set->p), b->slots, static_cast<u32*>(b->found->p),
+                          static_cast<u32*>(hits->p) + g, ctx->n_sms, ctx->st);
+    }
+    launch_batch_flags(n, static_cast<const u32*>(b->slot_of->p), static_cast<const u32*>(b->first->p), static_cast<const u32*>(b->found->p), want_found,
+                       static_cast<u8*>(b->flag8->p), static_cast<u32*>(b->flag32->p), ctx->ctrl + c + 1, ctx->n_sms, ctx->st);
+    timer_end(ctx);
+    KB_CUDA(ctx, cudaGetLastError());
+    b->seg_hits.assign(nseg, 0);
+    if (nseg) KB_CUDA(ctx, cudaMemcpyAsync(b->seg_hits.data(), hits->p, nseg * sizeof(u32), cudaMemcpyDeviceToHost, ctx->st));
+    KB_TRY(ctrl_read(ctx));  // (synchronises the stream: seg_hits has arrived too)
+    if (ctx->h_ctrl[c]) return fail(ctx, KB_E_CUDA, "update batch set overflow");
+    b->n_flagged = ctx->h_ctrl[c + 1];
+    return KB_OK;
+}
+
+static kb_status batch_flags_out(kb_ctx* ctx, const BatchMark& b, uint8_t* flags) {
+    if (!flags || !b.n) return KB_OK;
+    KB_CUDA(ctx, cudaMemcpyAsync(flags, b.flag8->p, b.n, cudaMemcpyDeviceToHost, ctx->st));
+    KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
+    ctx->stats.d2h_bytes += b.n;
+    return KB_OK;
+}
+
+// kb_store_insert over a batch in device memory
+static kb_status store_insert_device(kb_ctx* ctx, const u32* s, const u32* p, const u32* o, u32 n, u64 tag, uint8_t* inserted, uint64_t* n_inserted) {
+    BatchMark b;
+    KB_TRY(batch_mark(ctx, s, p, o, n, /*want_found=*/false, &b));
+    const u32 n_new = b.n_flagged;
+    if (ctx->n_triples + n_new >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "store would exceed 2^32-16 triples");
+    KB_TRY(batch_flags_out(ctx, b, inserted));
+    if (n_inserted) *n_inserted = n_new;
+    if (n_new == 0) return KB_OK;  // nothing changes: no new version
+    // geometric merge: the new triples absorb the latest segments of the same tag while each holds at most twice what is gathered so
+    // far, so that a run of small inserts leaves O(log n) segments and every triple is copied O(log n) times
+    std::vector<size_t> absorbed;
+    u64 total = n_new;
+    for (size_t g = ctx->segs.size(); g-- > 0;) {
+        const Segment& sg = ctx->segs[g];
+        if (sg.tag != tag || sg.ready) continue;
+        if (sg.n > 2 * total) break;
+        absorbed.push_back(g);
+        total += sg.n;
+    }
+    Segment ns;
+    ns.tag = tag;
+    ns.n = total;
+    KB_TRY(alloc_col(ctx, total, &ns.s));
+    KB_TRY(alloc_col(ctx, total, &ns.p));
+    KB_TRY(alloc_col(ctx, total, &ns.o));
+    u64 at = 0;
+    for (size_t k = absorbed.size(); k-- > 0;) {  // the absorbed segments in store order, then the new triples in batch order
+        const Segment& sg = ctx->segs[absorbed[k]];
+        KB_CUDA(ctx, cudaMemcpyAsync(ns.s.ptr + at, sg.s.ptr, sg.n * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
+        KB_CUDA(ctx, cudaMemcpyAsync(ns.p.ptr + at, sg.p.ptr, sg.n * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
+        KB_CUDA(ctx, cudaMemcpyAsync(ns.o.ptr + at, sg.o.ptr, sg.n * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
+        at += sg.n;
+    }
+    Buf scratch;
+    KB_TRY(alloc_buf(ctx, (((size_t)n + 1) / 2048 + 4) * sizeof(u32), &scratch));
+    u32* pos = static_cast<u32*>(b.flag32->p);
+    timer_begin(ctx, F_OTHER, 4);  // the scan's three kernels and the gather
+    launch_exclusive_scan_u32(pos, n + 1, static_cast<u32*>(scratch->p), ctx->st);
+    launch_batch_gather(s, p, o, n, static_cast<const u8*>(b.flag8->p), pos, ns.s.ptr + at, ns.p.ptr + at, ns.o.ptr + at, ctx->n_sms, ctx->st);
+    timer_end(ctx);
+    KB_CUDA(ctx, cudaGetLastError());
+    return store_swap(ctx, std::move(absorbed), {ns});
+}
+
+// kb_store_remove over a batch in device memory
+static kb_status store_remove_device(kb_ctx* ctx, const u32* s, const u32* p, const u32* o, u32 n, uint8_t* removed, uint64_t* n_removed) {
+    BatchMark b;
+    KB_TRY(batch_mark(ctx, s, p, o, n, /*want_found=*/true, &b));
+    KB_TRY(batch_flags_out(ctx, b, removed));
+    if (n_removed) *n_removed = b.n_flagged;
+    if (b.n_flagged == 0) return KB_OK;  // nothing stored matches: no new version
+    // segments without a hit stay as they are (their buffers and index chunks); the others are compacted
+    std::vector<size_t> hit;
+    std::vector<Segment> kept;
+    for (size_t g = 0; g < ctx->segs.size(); g++) {
+        if (!b.seg_hits[g]) continue;
+        Segment ns;
+        KB_TRY(segment_without(ctx, ctx->segs[g], b.set, b.slots, &ns));
+        hit.push_back(g);
+        kept.push_back(ns);
+    }
+    return store_swap(ctx, std::move(hit), std::move(kept));
+}
+
+// a host batch checked as the appends check theirs (NULL columns, KB_ID_NONE) and copied to the device
+static kb_status upload_batch(kb_ctx* ctx, const u32* s, const u32* p, const u32* o, u64 n, Buf* d) {
+    if (!s || !p || !o) return fail(ctx, KB_E_INVALID, "NULL column pointer");
+    if (n > BATCH_MAX) return fail(ctx, KB_E_LIMIT, "a batch of %llu triples: at most 2^30", (unsigned long long)n);
+    u32 cmax[3] = {0, 0, 0};
+    const u32* col[3] = {s, p, o};
+    for (int c = 0; c < 3; c++)
+        for (u64 i = 0; i < n; i++) if (col[c][i] == KB_ID_NONE) { cmax[c] = KB_ID_NONE; break; }
+    KB_TRY(refuse_reserved_id(ctx, cmax));
+    KB_TRY(alloc_buf(ctx, 3 * n * sizeof(u32), d));
+    u32* dst = static_cast<u32*>((*d)->p);
+    for (int c = 0; c < 3; c++) KB_CUDA(ctx, cudaMemcpyAsync(dst + c * n, col[c], n * sizeof(u32), cudaMemcpyHostToDevice, ctx->st));
+    ctx->stats.h2d_bytes += 3 * n * sizeof(u32);
+    return KB_OK;
 }
 }  // namespace kb
 
@@ -570,9 +775,7 @@ kb_status kb_store_delete(kb_ctx* ctx, const uint32_t* s, const uint32_t* p, con
     KB_ENTER(ctx);
     if (n == 0 || ctx->n_triples == 0) return KB_OK;
     if (!s || !p || !o) return kb::fail(ctx, KB_E_INVALID, "NULL column pointer");
-    // 1. the delete set (96-bit keys), 2. mark matching triples by overwriting a copy of the predicate column with KB_ID_NONE,
-    // 3. rescan every segment with (?s ?p ?o) — a row whose predicate is KB_ID_NONE can never equal a real constant, and the
-    //    pattern's pushed-down filter NE_ID drops it.
+    // the delete set (96-bit keys), then every segment without its triples (segment_without)
     const u32 set_slots = kb::pow2_at_least(n * 2);
     kb::Buf set, ds, dp, dob;
     KB_TRY(kb::alloc_buf(ctx, (size_t)set_slots * sizeof(uint4), &set));
@@ -587,32 +790,86 @@ kb_status kb_store_delete(kb_ctx* ctx, const uint32_t* s, const uint32_t* p, con
     kb::launch_set_insert(static_cast<uint4*>(set->p), set_slots, (const u32*)ds->p, (const u32*)dp->p, 0u, (const u32*)dob->p, (u32)n,
                           ctx->ctrl + off, ctx->n_sms, ctx->st);
     KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
-    kb_pattern pt{{1, 0}, {1, 1}, {1, 2}};
-    kb::FilterProg keep;
-    kb_filter_op ne{};
-    ne.op = KB_F_NE_ID; ne.slot = 1; ne.id = KB_ID_NONE;  // true for every bound predicate; a marked one reads as unbound: false
-    keep.ops.push_back(ne);
-    const std::vector<kb::FilterProg> pd{keep};
     // the new segments are built aside: the store changes only when all of them are (a failure leaves it as it was)
     std::vector<kb::Segment> kept;
     for (auto& sg : ctx->segs) {
-        kb::Segment marked = sg;
-        if (sg.n) {
-            KB_TRY(kb::alloc_col(ctx, sg.n, &marked.p));
-            kb::launch_delete_mark(sg.s.ptr, sg.p.ptr, sg.o.ptr, (u32)sg.n, static_cast<const uint4*>(set->p), set_slots, marked.p.ptr,
-                                   ctx->n_sms, ctx->st);
-        }
-        // rescan this one segment
-        std::vector<std::unique_ptr<kb_rel>> rels;
-        KB_TRY(kb::scan_segments(ctx, {marked}, &pt, 1, pd, kb::ScanOut::Cols, &rels));
         kb::Segment ns;
-        ns.tag = sg.tag;
-        ns.n = rels[0]->n;
-        ns.s = rels[0]->cols[0]; ns.p = rels[0]->cols[1]; ns.o = rels[0]->cols[2];
+        KB_TRY(kb::segment_without(ctx, sg, set, set_slots, &ns));
         kept.push_back(ns);
     }
     kb::store_replace(ctx, std::move(kept));
     return KB_OK;
+}
+
+kb_status kb_store_insert(kb_ctx* ctx, const uint32_t* s, const uint32_t* p, const uint32_t* o, uint64_t n, uint64_t segment_tag, uint8_t* inserted,
+                          uint64_t* n_inserted) {
+    KB_ENTER(ctx);
+    if (n_inserted) *n_inserted = 0;
+    if (n == 0) return KB_OK;
+    kb::Buf d;
+    KB_TRY(kb::upload_batch(ctx, s, p, o, n, &d));
+    const u32* b = static_cast<const u32*>(d->p);
+    return kb::store_insert_device(ctx, b, b + n, b + 2 * n, (u32)n, segment_tag, inserted, n_inserted);
+}
+
+kb_status kb_store_remove(kb_ctx* ctx, const uint32_t* s, const uint32_t* p, const uint32_t* o, uint64_t n, uint8_t* removed, uint64_t* n_removed) {
+    KB_ENTER(ctx);
+    if (n_removed) *n_removed = 0;
+    if (n == 0) return KB_OK;
+    kb::Buf d;
+    KB_TRY(kb::upload_batch(ctx, s, p, o, n, &d));
+    const u32* b = static_cast<const u32*>(d->p);
+    return kb::store_remove_device(ctx, b, b + n, b + 2 * n, (u32)n, removed, n_removed);
+}
+
+kb_status kb_store_remove_template(kb_ctx* ctx, const kb_rel* rel, const kb_pattern* tmpl, uint32_t n_tmpl, uint64_t* n_removed) {
+    KB_ENTER(ctx);
+    if (n_removed) *n_removed = 0;
+    if (!rel || (n_tmpl && !tmpl)) return kb::fail(ctx, KB_E_INVALID, "NULL relation or template");
+    if (rel->pair) return kb::fail(ctx, KB_E_INVALID, "an internal pair relation");
+    if (n_tmpl > kb::TEMPLATE_MAX) return kb::fail(ctx, KB_E_LIMIT, "%u template patterns: at most %u", n_tmpl, kb::TEMPLATE_MAX);
+    static const char* const pos[3] = {"subject", "predicate", "object"};
+    kb::TemplateFillParams P{};
+    for (u32 t = 0; t < n_tmpl; t++) {
+        const kb_term* term[3] = {&tmpl[t].s, &tmpl[t].p, &tmpl[t].o};
+        for (int c = 0; c < 3; c++) {
+            if (term[c]->is_var > 1) return kb::fail(ctx, KB_E_INVALID, "template pattern %u: the %s is not a variable or a constant", t, pos[c]);
+            if (!term[c]->is_var) {
+                if (term[c]->value == KB_ID_NONE)
+                    return kb::fail(ctx, KB_E_INVALID, "template pattern %u: the %s is 0xFFFFFFFF, which is reserved (KB_ID_NONE)", t, pos[c]);
+                P.cval[t][c] = term[c]->value;
+                continue;
+            }
+            const int col = rel->col_of(term[c]->value);
+            if (col < 0) return kb::fail(ctx, KB_E_UNSUPPORTED, "template pattern %u: the %s variable %u is not a column of the relation", t, pos[c], term[c]->value);
+            P.col[t][c] = rel->cols[col].ptr;
+        }
+    }
+    const u64 total = rel->n * n_tmpl;
+    if (total == 0) return KB_OK;
+    if (total > kb::BATCH_MAX) return kb::fail(ctx, KB_E_LIMIT, "%llu template triples (rows x patterns): at most 2^30", (unsigned long long)total);
+    kb::Buf d;
+    KB_TRY(kb::alloc_buf(ctx, 3 * total * sizeof(u32), &d));
+    u32* b = static_cast<u32*>(d->p);
+    P.n_tmpl = n_tmpl;
+    P.rows = (u32)rel->n;
+    P.s = b; P.p = b + total; P.o = b + 2 * total;
+    P.dict = kb::dicttab(ctx);
+    const u32 c = kb::ctrl_alloc(ctx, 2);
+    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + c, 0, 2 * sizeof(u32), ctx->st));
+    P.bad = ctx->ctrl + c;
+    kb::timer_begin(ctx, kb::F_OTHER);
+    kb::launch_template_fill(P, ctx->n_sms, ctx->st);
+    kb::timer_end(ctx);
+    KB_CUDA(ctx, cudaGetLastError());
+    KB_TRY(kb::ctrl_read(ctx));
+    if (ctx->h_ctrl[c])
+        return kb::fail(ctx, KB_E_UNSUPPORTED, "%u template cells are unbound: the reference would delete the variable's name as a term", ctx->h_ctrl[c]);
+    if (ctx->h_ctrl[c + 1])
+        return kb::fail(ctx, KB_E_UNSUPPORTED,
+                        "%u template cells hold a term that encode_term_star would not re-encode to the same id (a quoted id, an id without a "
+                        "device dictionary string, or a string it strips or parses)", ctx->h_ctrl[c + 1]);
+    return kb::store_remove_device(ctx, P.s, P.p, P.o, (u32)total, nullptr, n_removed);
 }
 
 kb_status kb_store_download(kb_ctx* ctx, uint32_t* s, uint32_t* p, uint32_t* o, uint64_t cap, uint64_t* n) {

@@ -177,6 +177,59 @@ class QuotedTripleStore:
         self.next_qt_id = max(self.next_qt_id, other.next_qt_id)
 
 
+def _clean_term(t: str) -> str:
+    """the plain-term branch of encode_term_star (sparql_database.rs:96-106) on a trimmed term"""
+    if t.startswith("<") and t.endswith(">"):
+        return t[1:-1]
+    if t.startswith('"'):
+        close = t[1:].find('"')
+        return t[1:close + 1] if close >= 0 else t.strip('"')
+    return t
+
+
+def _split_quoted_content(content: str) -> Tuple[str, str, str]:
+    """split_quoted_triple_content (sparql_database.rs:125-190): `s p o` split at top-level whitespace, outside IRIs, literals and
+    nested `<< >>`; parts past the third are joined into the object, missing ones are empty"""
+    parts: List[str] = []
+    cur = ""
+    depth = 0
+    in_uri = in_lit = esc = False
+    for ch in content:
+        if esc:
+            cur += ch
+            esc = False
+        elif ch == "\\" and in_lit:
+            cur += ch
+            esc = True
+        elif ch == '"' and not in_uri:
+            in_lit = not in_lit
+            cur += ch
+        elif ch == "<" and not in_lit:
+            cur += ch
+            if cur.endswith("<<"):
+                depth += 1
+            elif depth == 0:
+                in_uri = True
+        elif ch == ">" and not in_lit:
+            cur += ch
+            if in_uri:
+                in_uri = False
+            elif cur.endswith(">>") and depth > 0:
+                depth -= 1
+        elif ch in " \t\n\r" and depth == 0 and not in_uri and not in_lit:
+            if cur.strip():
+                parts.append(cur.strip())
+                cur = ""
+        else:
+            cur += ch
+    if cur.strip():
+        parts.append(cur.strip())
+    if len(parts) >= 3:
+        return parts[0], parts[1], " ".join(parts[2:])
+    parts += [""] * (3 - len(parts))
+    return parts[0], parts[1], parts[2]
+
+
 def _strip(v: str) -> str:
     return v[1:] if v.startswith("?") else v  # engine.rs strips '?' from variable names everywhere
 
@@ -496,6 +549,167 @@ class SparqlDatabase:
             self._version += 1
             return True
         return False
+
+    def insert_triples(self, ids) -> List[bool]:
+        """add_triple of each (s, p, o) id triple in order, applied to this set and to the device store together (kb_store_insert):
+        result[i] is whether triple i was new. The device store is left current, so the next query uploads nothing; it keeps the new
+        triples in a segment of their own, in batch order, rather than in the set's order."""
+        return self._write(ids, insert=True)
+
+    def delete_triples(self, ids) -> List[bool]:
+        """delete_triple of each (s, p, o) id triple in order, on this set and on the device store together (kb_store_remove):
+        result[i] is whether triple i was there to remove"""
+        return self._write(ids, insert=False)
+
+    def _write(self, ids, insert: bool) -> List[bool]:
+        arr = np.asarray(ids, dtype=np.uint32).reshape(-1, 3)
+        if len(arr) == 0:
+            return []
+        self._sync()  # the device store holds this set before the batch applies to both
+        if insert:
+            dev = self.ctx.store_insert(arr[:, 0], arr[:, 1], arr[:, 2])
+        else:
+            dev = self.ctx.store_remove(arr[:, 0], arr[:, 1], arr[:, 2])
+        flags = []
+        for row in arr:
+            t = (int(row[0]), int(row[1]), int(row[2]))
+            flags.append(t not in self.triples if insert else t in self.triples)
+            if insert:
+                self.triples.add(t)
+            else:
+                self.triples.discard(t)
+        if flags != [bool(f) for f in dev]:
+            raise RuntimeError("the device store and the host set disagree on a batch write")
+        if any(flags):
+            self._version += 1
+            self._uploaded_version = self._version
+        # the device dictionary and its numeric side table take the strings the batch's terms added (encode_bulk has put them in the
+        # device dictionary already; terms encoded on the host have not)
+        n_dev, _ = self.ctx.dict_strings_info()
+        kept = n_dev == len(self.dictionary.id_to_string) or _push_new_strings(self.ctx, self.dictionary, n_dev)
+        _derive_numeric(self.ctx, c.NUMERIC_APPEND if kept else 0)
+        self._sync_quoted()
+        return flags
+
+    def encode_terms_star(self, terms: Sequence[str]) -> List[int]:
+        """encode_term_star (sparql_database.rs:82-109) of each term in order: a `<< s p o >>` term is split
+        (split_quoted_triple_content, :125-190), its components encoded first and the triple then; a plain term is trimmed and
+        cleaned (<iri> loses its brackets, a literal keeps what lies between its first two quotes). All plain terms go through one
+        device encode (Dictionary.encode_bulk) in the order the reference's recursion meets them, so they get the same ids."""
+        self._sync()  # the device dictionary mirrors this one before the batch encode (a shared context may hold another's)
+        plain: List[str] = []
+
+        def walk(term: str):  # -> a plan: ("d", position in plain) or ("q", plan_s, plan_p, plan_o)
+            t = term.strip()
+            if t.startswith("<<") and t.endswith(">>"):
+                return ("q",) + tuple(walk(x) for x in _split_quoted_content(t[2:-2].strip()))
+            plain.append(_clean_term(t))
+            return ("d", len(plain) - 1)
+
+        plans = [walk(t) for t in terms]
+        ids = self.dictionary.encode_bulk(self.ctx, plain) if plain else np.empty(0, np.uint32)
+
+        def resolve(plan) -> int:
+            if plan[0] == "d":
+                return int(ids[plan[1]])
+            return self.quoted_triple_store.encode(resolve(plan[1]), resolve(plan[2]), resolve(plan[3]))
+
+        return [resolve(pl) for pl in plans]
+
+    def handle_update(self, kind: str, triples: Sequence[Tuple[str, str, str]]) -> str:
+        """SparqlDatabase::handle_update (sparql_database.rs:3091-3117) given what parse_insert / parse_delete yield: the kind
+        ("INSERT" or "DELETE") and the term strings of each triple. Every term is encoded with encode_term_star, then the triples are
+        inserted or removed as one batch on the host set and the device store. Returns the reference's strings."""
+        if kind not in ("INSERT", "DELETE"):
+            return "Update Failed"
+        ids = self.encode_terms_star([x for t in triples for x in t])
+        if kind == "INSERT":
+            self.insert_triples(ids)
+        else:
+            self.delete_triples(ids)
+        return "Update Successful"
+
+    def execute_delete_where(self, delete_template: Sequence[Tuple[str, str, str]], where_patterns: Sequence[Tuple[str, str, str]],
+                             insert_template: Optional[Sequence[Tuple[str, str, str]]] = None) -> int:
+        """DELETE { delete_template } WHERE { where_patterns } [INSERT { insert_template }] as execute_query_rayon_parallel2_volcano runs
+        it (execute_query.rs:354-413). Terms are the parser's strings ("?x", "<iri>", "\\"literal\\"", "<< s p o >>" in a template).
+        The WHERE runs on the device (kb_bgp_execute); kb_store_remove_template then fills the template from its rows and removes the
+        result from the device store, and the host set loses the same triples. Where the device refuses a binding (one that
+        encode_term_star would not map back to its own id, or a template variable the WHERE leaves unbound) the reference's loop runs
+        instead: every row decoded, every filled term encoded with encode_term_star, the triples removed as one batch. Returns the
+        triples removed. The reference's quirks are kept:
+          - the WHERE is its patterns only: the reference rebuilds the query from them, so a FILTER in it has no effect;
+          - the INSERT template is inserted as written (process_insert_clause, execute_query.rs:758-773), so "?x" in it is a term;
+          - the template's constants are encoded for the first WHERE row, so a DELETE of unknown terms adds them to the dictionary.
+        A WHERE constant is looked up in the dictionary (one it lacks matches nothing); a quoted term in the WHERE is refused
+        (ValueError)."""
+        self._sync()
+        slots = SlotMap()
+        pats, matches = [], True
+        for tp in where_patterns:
+            terms = []
+            for x in tp:
+                if x.startswith("?"):
+                    terms.append(c.V(slots.of(x)))
+                    continue
+                t = x.strip()
+                if t.startswith("<<") and t.endswith(">>"):
+                    raise ValueError("a quoted term in the WHERE of a DELETE WHERE is not supported")
+                i = self.dictionary.lookup(_clean_term(t))
+                matches = matches and i is not None
+                terms.append(c.K(0 if i is None else i))
+            pats.append(c.pattern(*terms))
+        removed = 0
+        rel = self.ctx.bgp_execute(pats) if pats and matches else None
+        try:
+            if rel is not None and rel.n_rows:
+                removed = self._remove_template(rel, slots, delete_template)
+        finally:
+            if rel is not None:
+                rel.free()
+        if insert_template:
+            self.handle_update("INSERT", insert_template)
+        return removed
+
+    def _remove_template(self, rel: c.Relation, slots: SlotMap, template: Sequence[Tuple[str, str, str]]) -> int:
+        consts = [x for tp in template for x in tp if not x.startswith("?")]
+        ids = iter(self.encode_terms_star(consts))  # what the first row's encode_term_star calls add, in their order
+        _derive_numeric(self.ctx)
+        tmpl = [c.pattern(*[c.V(slots.of(x)) if x.startswith("?") else c.K(next(ids)) for x in tp]) for tp in template]
+        self._sync_quoted()
+        rel_slots = rel.slots
+        rows = rel.to_numpy(rel_slots)
+        try:
+            n = self.ctx.store_remove_template(rel, tmpl)
+        except c.KolibrieError as e:
+            if e.status != c.KB_E_UNSUPPORTED:
+                raise
+            # the reference's loop: each row's bindings as text, the filled terms encoded with encode_term_star, one remove batch
+            col = {name: rel_slots.index(s) for name, s in slots.slot.items() if s in rel_slots}
+            terms = []
+            for row in rows:
+                for tp in template:
+                    for x in tp:
+                        j = col.get(_strip(x)) if x.startswith("?") else None
+                        v = self.decode_term(int(row[j])) if j is not None and int(row[j]) != c.KB_ID_NONE else None
+                        terms.append(x if v is None else v)
+            return sum(self.delete_triples(self.encode_terms_star(terms)))
+        # the device removed the filled triples; the host set loses the same ones
+        col = [[rel_slots.index(t.value) if t.is_var else None for t in (p.s, p.p, p.o)] for p in tmpl]
+        const = [[t.value for t in (p.s, p.p, p.o)] for p in tmpl]
+        gone = 0
+        for row in rows:
+            for cj, cv in zip(col, const):
+                t = tuple(int(row[j]) if j is not None else v for j, v in zip(cj, cv))
+                if t in self.triples:
+                    self.triples.remove(t)
+                    gone += 1
+        if gone != n:
+            raise RuntimeError("the device store and the host set disagree on a DELETE WHERE")
+        if n:
+            self._version += 1
+            self._uploaded_version = self._version
+        return n
 
     def build_all_indexes(self):
         """The reference builds its six hash indexes here (sparql_database.rs:3364-3394); the device store is (re)uploaded and

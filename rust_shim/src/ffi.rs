@@ -103,6 +103,10 @@ extern "C" {
     pub fn kb_store_append(ctx: *mut KbCtx, s: *const u32, p: *const u32, o: *const u32, n: u64, tag: u64) -> kb_status;
     pub fn kb_store_evict(ctx: *mut KbCtx, tag: u64) -> kb_status;
     pub fn kb_store_delete(ctx: *mut KbCtx, s: *const u32, p: *const u32, o: *const u32, n: u64) -> kb_status;
+    pub fn kb_store_insert(ctx: *mut KbCtx, s: *const u32, p: *const u32, o: *const u32, n: u64, segment_tag: u64, inserted: *mut u8,
+                           n_inserted: *mut u64) -> kb_status;
+    pub fn kb_store_remove(ctx: *mut KbCtx, s: *const u32, p: *const u32, o: *const u32, n: u64, removed: *mut u8, n_removed: *mut u64) -> kb_status;
+    pub fn kb_store_remove_template(ctx: *mut KbCtx, rel: *const KbRel, tmpl: *const KbPattern, n_tmpl: u32, n_removed: *mut u64) -> kb_status;
     pub fn kb_store_clear(ctx: *mut KbCtx) -> kb_status;
     pub fn kb_store_build_index(ctx: *mut KbCtx, n_predicates: *mut u32, build_ms: *mut c_double) -> kb_status;
     pub fn kb_store_size(ctx: *mut KbCtx, n_triples: *mut u64, n_segments: *mut u32) -> kb_status;

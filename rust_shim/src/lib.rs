@@ -22,6 +22,7 @@ use kolibrie::sparql_database::SparqlDatabase;
 use kolibrie::streamertail_optimizer::{Condition, PhysicalOperator};
 use shared::query::{ArithmeticExpression, FilterExpression};
 use shared::terms::{Term, TriplePattern};
+use shared::triple::Triple;
 use std::collections::HashMap;
 use std::ffi::CStr;
 use std::ptr;
@@ -117,6 +118,101 @@ impl DeviceStore {
         first.truncate(n_new as usize);
         if self.synced_dict != usize::MAX { self.synced_dict += n_new as usize; }
         Ok((ids, first))
+    }
+
+    /// `add_triple` of each triple in order (sparql_database.rs:215-218) on `database` and on the device store together
+    /// (kb_store_insert, into a segment tagged `tag`): returns whether each triple was new. `sync` first, so that the device holds the
+    /// set the batch applies to; the sync counter then moves with the set, so the next `sync` uploads no triples.
+    pub fn insert(&mut self, database: &mut SparqlDatabase, triples: &[Triple], tag: u64) -> Result<Vec<bool>, String> {
+        self.write(database, triples, Some(tag))
+    }
+
+    /// `delete_triple` of each triple in order (sparql_database.rs:220-226) on `database` and on the device store together
+    /// (kb_store_remove): returns what each `delete_triple` returns
+    pub fn remove(&mut self, database: &mut SparqlDatabase, triples: &[Triple]) -> Result<Vec<bool>, String> {
+        self.write(database, triples, None)
+    }
+
+    fn write(&mut self, database: &mut SparqlDatabase, triples: &[Triple], insert_tag: Option<u64>) -> Result<Vec<bool>, String> {
+        if triples.is_empty() { return Ok(Vec::new()); }
+        if self.segmented { return Err("the store is maintained segment by segment by its owner".into()); }
+        self.sync(database)?;
+        let s: Vec<u32> = triples.iter().map(|t| t.subject).collect();
+        let p: Vec<u32> = triples.iter().map(|t| t.predicate).collect();
+        let o: Vec<u32> = triples.iter().map(|t| t.object).collect();
+        let mut flags = vec![0u8; triples.len()];
+        let mut n = 0u64;
+        let rc = unsafe {
+            match insert_tag {
+                Some(tag) => kb_store_insert(self.ctx, s.as_ptr(), p.as_ptr(), o.as_ptr(), s.len() as u64, tag, flags.as_mut_ptr(), &mut n),
+                None => kb_store_remove(self.ctx, s.as_ptr(), p.as_ptr(), o.as_ptr(), s.len() as u64, flags.as_mut_ptr(), &mut n),
+            }
+        };
+        if rc != KB_OK { return Err(self.last_error()); }
+        let mut host = Vec::with_capacity(triples.len());
+        for t in triples {
+            host.push(match insert_tag {
+                Some(_) => { let new = !database.triples.contains(t); database.add_triple(t.clone()); new }
+                None => database.delete_triple(t),
+            });
+        }
+        if host.iter().zip(flags.iter()).any(|(h, &d)| *h != (d != 0)) {
+            self.invalidate();  // the next sync uploads the host set again
+            return Err("the device store and the host set disagree on a batch write".into());
+        }
+        self.synced_triples = database.triples.len();
+        Ok(host)
+    }
+
+    /// DELETE { template } WHERE { ... } (execute_query.rs:354-413) once the WHERE's rows are `rel` on the device (`try_execute_rel`):
+    /// kb_store_remove_template fills `template` from every row and removes the triples from the device store, and `database` loses
+    /// the same triples. Returns the triples removed, or None where the device refuses a binding (KB_E_UNSUPPORTED: one that
+    /// `encode_term_star` would not map back to its own id, or a template variable the WHERE leaves unbound): the caller then runs the
+    /// reference's loop, and both stores are as they were.
+    pub fn remove_template(&mut self, database: &mut SparqlDatabase, rel: &Rel, names: &[String], template: &[KbPattern]) -> Result<Option<u64>, String> {
+        let mut n = 0u64;
+        let rc = unsafe { kb_store_remove_template(self.ctx, rel.0, template.as_ptr(), template.len() as u32, &mut n) };
+        if rc == KB_E_UNSUPPORTED { return Ok(None); }
+        if rc != KB_OK { return Err(self.last_error()); }
+        let rows = download_rows(self, rel.0, names).ok_or_else(|| self.last_error())?;
+        let (_, slots) = rel_slots(rel).ok_or_else(|| self.last_error())?;  // names[c] is the variable of column c, slots[c] its slot
+        let value = |t: &KbTerm, row: &HashMap<String, u32>| if t.is_var == 1 {
+            slots.iter().position(|&s| s == t.value).and_then(|c| names.get(c)).and_then(|k| row.get(k)).copied()
+        } else { Some(t.value) };
+        let mut gone = 0u64;
+        for row in &rows {
+            for pt in template {
+                if let (Some(s), Some(p), Some(o)) = (value(&pt.s, row), value(&pt.p, row), value(&pt.o, row)) {
+                    if database.delete_triple(&Triple { subject: s, predicate: p, object: o }) { gone += 1; }
+                }
+            }
+        }
+        if gone != n {
+            self.invalidate();
+            return Err("the device store and the host set disagree on a DELETE WHERE".into());
+        }
+        self.synced_triples = database.triples.len();
+        Ok(Some(n))
+    }
+
+    /// `SparqlDatabase::handle_update` (sparql_database.rs:3091-3117) with the store written as one batch: the reference's loop
+    /// encodes every term with `encode_term_star` in its order, then the triples are inserted or removed on `database` and on the
+    /// device together. Returns the reference's strings.
+    pub fn handle_update(&mut self, database: &mut SparqlDatabase, update: &str) -> Result<String, String> {
+        use kolibrie::parser::{parse_delete, parse_insert};
+        let trimmed = update.trim();
+        let (insert, terms) = if trimmed.starts_with("INSERT") {
+            match parse_insert(trimmed) { Ok((_, c)) => (true, c.triples), Err(_) => return Ok("Update Failed".into()) }
+        } else if trimmed.starts_with("DELETE") {
+            match parse_delete(trimmed) { Ok((_, c)) => (false, c.triples), Err(_) => return Ok("Update Failed".into()) }
+        } else {
+            return Ok("Update Failed".into());
+        };
+        let triples: Vec<Triple> = terms.iter().map(|(s, p, o)| Triple {
+            subject: database.encode_term_star(s), predicate: database.encode_term_star(p), object: database.encode_term_star(o),
+        }).collect();
+        if insert { self.insert(database, &triples, 0)?; } else { self.remove(database, &triples)?; }
+        Ok("Update Successful".into())
     }
 
     /// `SparqlDatabase::generate_ntriples` (`turtle` false) or `generate_turtle` (sparql_database.rs:301-382) of the device store
