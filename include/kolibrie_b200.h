@@ -657,6 +657,41 @@ KB_API kb_status kb_datalog_fixpoint(kb_ctx* ctx, const kb_rule* rules, uint32_t
 KB_API kb_status kb_datalog_fixpoint_seed(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rules, uint32_t strategy, const kb_rel* seed,
                                           kb_rel** out, uint64_t* n_seed_new, kb_fixpoint_stats* stats);
 
+/* Backward chaining (Reasoner::backward_chaining, datalog/src/reasoning/backward_chaining.rs:165-259): the distinct bindings of the
+ * variables of `query` over T^max_depth, where T^0 = the store and T^k = T^(k-1) plus the heads of every rule whose premises match
+ * facts of T^(k-1). Premise constants are enforced and rule filters are ignored, as the reference's SLD resolution does; with
+ * max_depth = KB_BC_MAX_DEPTH this is what it answers (its MAX_DEPTH, :197-198). The reference returns one map per derivation, with
+ * the renamed rule variables in it; here each distinct binding of the query's own variables comes once (quirk Q12, DESIGN §4).
+ * Evaluation: at most max_depth semi-naive rounds over the facts the query can use: demand patterns are compiled from the query and the
+ * rules on the host, only the rules whose head unifies with one run, and only facts that match a demand pattern of their predicate are
+ * read or kept. A query whose constants bind nothing (such as (?x P C) under a transitive rule) demands every fact of the predicates
+ * involved and costs a bounded closure. A ground query stops after the first round in which a derive launch finds the queried triple in its
+ * predicate's known-fact set (a probe read back with the launch's own counts).
+ * The store is read only: it, its index, prepared plans and the state the forward calls keep (kb_datalog_maintain's precondition, the
+ * seeded fixpoint's state) stay as they were.
+ * `*out` has one column per distinct query variable, in s, p, o first-appearance order (kb_scan's convention); its rows are distinct and
+ * in no particular order. A ground query gives a relation without columns and 0 or 1 rows.
+ * Refused, with nothing changed: max_depth > KB_BC_DEPTH_LIMIT (KB_E_LIMIT); a quoted term in the query or a rule, a rule without
+ * premises, a variable predicate in a premise (KB_E_UNSUPPORTED); a constant KB_ID_NONE (KB_E_INVALID); and the rule shapes
+ * kb_datalog_fixpoint refuses. */
+#define KB_BC_MAX_DEPTH 10u
+#define KB_BC_DEPTH_LIMIT 64u
+typedef struct kb_bc_stats {
+    uint32_t rounds;                /* semi-naive rounds run (<= max_depth) */
+    uint32_t reached_fixpoint;      /* 1: a round derived nothing new before the depth bound */
+    uint32_t stopped_early;         /* 1: a ground query found its triple before the depth bound */
+    uint32_t relevant_rules;        /* rules with a head that unifies with a demand pattern: the ones that ran */
+    uint32_t demand_patterns;       /* demand patterns over all predicates */
+    uint32_t restricted_predicates; /* predicates whose facts were restricted to their demand patterns */
+    uint64_t base_facts;            /* store facts of the rule and query predicates read after the restriction */
+    uint64_t derived;               /* new facts the rounds derived */
+    uint64_t derivations;           /* candidate head instances before dedup */
+    uint64_t answers;               /* rows of *out */
+    double device_ms;               /* CUDA-event time of the whole call */
+} kb_bc_stats;
+KB_API kb_status kb_datalog_query(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rules, const kb_pattern* query, uint32_t max_depth,
+                                  kb_rel** out, kb_bc_stats* stats /* nullable */);
+
 /* Sliding-window maintenance of the closure by delete-and-rederive: what a window firing with rules reaches by evicting the previous
  * window, adding the current one and materialising from scratch (rsp_engine.rs:94-109, simple_r2r.rs:103-128), reached from the slide.
  *   B  = the distinct triples of every segment whose tag is not KB_TAG_INFERRED, I = the triples of the KB_TAG_INFERRED segments,

@@ -75,6 +75,11 @@ struct Fix {
     std::vector<Pending> pend;
     Buf buckets;  // candidate buckets of the radix-partitioned dedup, kept across the derive calls of one fixpoint (a 3 GB allocation
                   // from the stream-ordered pool can cost milliseconds when the pool has to remap)
+    const BcDemandDev* demand = nullptr;  // kb_datalog_query: a derived fact of a restricted predicate must match one of its demand patterns
+    // kb_datalog_query, ground query whose predicate is a rule head: every derive launch of that predicate probes its known-fact set for
+    // the queried fact, read back with the launch's own counts
+    struct Probe { u32 pred = 0, s = 0, o = 0; bool found = false; };
+    Probe* probe = nullptr;
 };
 
 // What a seeded call leaves in the context for the next one: the store split by predicate and a known-fact set per rule predicate. While
@@ -359,6 +364,10 @@ kb_status derive_head(Fix& fx, const kb_rel* cur, const kb_pattern& h, const kb_
             D.veto_slots = gate->veto->slots;
         }
     }
+    if (fx.demand) {
+        auto it = fx.demand->of.find(h.p.value);
+        if (it != fx.demand->of.end()) { D.demand = it->second.first; D.n_demand = it->second.second; }
+    }
     PredRel& hr = fx.rels[h.p.value];
     KB_TRY(ensure_set(fx, hr, cur->n));
     tr.mark(ctx, "  ensure_set", hr.set_slots);
@@ -374,6 +383,8 @@ kb_status derive_head(Fix& fx, const kb_rel* cur, const kb_pattern& h, const kb_
     D.out_count = ctx->ctrl + coff;
     D.overflow = ctx->ctrl + coff + 1;
     D.n_deriv = reinterpret_cast<unsigned long long*>(ctx->ctrl + coff + 4);
+    const bool probe = fx.probe && fx.probe->pred == h.p.value;
+    const u32 poff = probe ? ctrl_alloc(ctx, 1) : 0u;
     const u64 count_before = hr.set_count;
     for (;;) {
         D.set = static_cast<u64*>(hr.set->p);
@@ -424,6 +435,7 @@ kb_status derive_head(Fix& fx, const kb_rel* cur, const kb_pattern& h, const kb_
             launch_derive(D, ctx->n_sms, ctx->st);
             timer_end(ctx);
         }
+        if (probe) launch_bc_probe(D.set, D.set_slots, fx.probe->s, fx.probe->o, ctx->ctrl + poff, ctx->st);
         KB_CUDA(ctx, cudaGetLastError());
         // counts are read immediately: the control arena may be recycled by later joins of this round
         KB_TRY(ctrl_read(ctx));
@@ -439,6 +451,7 @@ kb_status derive_head(Fix& fx, const kb_rel* cur, const kb_pattern& h, const kb_
         KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + coff + 1, 0, sizeof(u32), ctx->st));
         KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + coff + 4, 0, 2 * sizeof(u32), ctx->st));
     }
+    if (probe && ctx->h_ctrl[poff]) fx.probe->found = true;
     unsigned long long nd;
     memcpy(&nd, ctx->h_ctrl + coff + 4, sizeof nd);
     *derivations += nd;
@@ -460,13 +473,79 @@ kb_status flush_pending(Fix& fx, u64* appended) {
     return KB_OK;
 }
 
-// ---- rounds: from the current delta of every relation ([delta_start, n)) to the fixpoint
+// the store split by predicate: every relation of fx.rels gets its predicate's facts (one fused scan per 8 predicates). demand
+// (kb_datalog_query): a restricted predicate keeps only the facts that match one of its demand patterns.
+kb_status split_store(Fix& fx) {
+    kb_ctx* ctx = fx.ctx;
+    std::vector<u32> preds;
+    for (auto& kv : fx.rels) preds.push_back(kv.first);
+    for (size_t b = 0; b < preds.size(); b += MAXP) {
+        const u32 k = (u32)std::min<size_t>(MAXP, preds.size() - b);
+        std::vector<std::unique_ptr<kb_rel>> out;
+        // the predicate relations are append-only buffers with the capacity of a whole-store scan output: take the scan, not the
+        // (exactly sized) index slices
+        KB_TRY(scan_predicates(ctx, ctx->segs, preds.data() + b, k, ScanOut::Cols, &out));
+        // a restricted predicate's rows are selected into new columns of the scanned row count, which is then their capacity; the
+        // selections of a batch are read back together
+        std::vector<int> selected(k, -1);
+        for (u32 i = 0; i < k; i++) {
+            PredRel& r = fx.rels[preds[b + i]];
+            r.s = out[i]->cols[0];
+            r.o = out[i]->cols[1];
+            r.n = out[i]->n;
+            r.cap = ctx->n_triples;
+            if (!fx.demand) continue;
+            auto it = fx.demand->of.find(r.pred);
+            if (it == fx.demand->of.end()) continue;
+            selected[i] = (int)ctrl_alloc(ctx, 1);
+            Col ns, no;
+            KB_TRY(bc_demand_select(ctx, it->second.first, it->second.second, r.s, r.o, r.n, &ns, &no, (u32)selected[i]));
+            r.s = ns;
+            r.o = no;
+            r.cap = r.n;
+        }
+        if (std::any_of(selected.begin(), selected.end(), [](int w) { return w >= 0; })) KB_TRY(ctrl_read(ctx));
+        for (u32 i = 0; i < k; i++) {
+            PredRel& r = fx.rels[preds[b + i]];
+            if (selected[i] >= 0) r.n = ctx->h_ctrl[selected[i]];
+            r.base_n = r.n;
+            if (r.n * 4 < r.cap) {  // shrink: the scan allocates for the worst case
+                r.cap = 0;
+                Col os = r.s, oo = r.o;
+                u64 n = r.n;
+                r.n = 0;
+                KB_TRY(grow_rel(ctx, r, std::max<u64>(n * 2, 1024)));
+                if (n) {
+                    KB_CUDA(ctx, cudaMemcpyAsync(r.s.ptr, os.ptr, n * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
+                    KB_CUDA(ctx, cudaMemcpyAsync(r.o.ptr, oo.ptr, n * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
+                }
+                r.n = n;
+            }
+        }
+    }
+    return KB_OK;
+}
+
+// kb_datalog_query's rounds: premise constants enforced at every arity, no rule filters (derive_head's strict mode), at most max_rounds
+// rounds, and a ground query stops at the end of the first round in which a derive launch found the queried fact in its known-fact set
+// (fx.probe)
+struct QueryMode {
+    u32 max_rounds = 0;
+    u32 rounds = 0;                  // rounds run
+    bool fixpoint = false, stopped_early = false;
+};
+
+// ---- rounds: from the current delta of every relation ([delta_start, n)) to the fixpoint (qm: a query's rounds)
 kb_status run_rounds(Fix& fx, const kb_rule* rules, u32 n_rules, const std::vector<RulePlan>& plans, u32 strategy, kb_fixpoint_stats& st,
-                     Trace& tr) {
+                     Trace& tr, QueryMode* qm = nullptr) {
     kb_ctx* ctx = fx.ctx;
     const bool old_delta = strategy == KB_SEMI_NAIVE_OLD_DELTA;
-    const bool strict = strategy == KB_SEMI_NAIVE_PARALLEL;
+    const bool strict = strategy == KB_SEMI_NAIVE_PARALLEL || qm;
     for (u32 round = 0;; round++) {
+        if (qm) {
+            if (round >= qm->max_rounds) break;
+            qm->rounds++;
+        }
         for (auto& kv : fx.rels) kv.second.snapshot = kv.second.n;
         fx.pend.clear();
         for (u32 r = 0; r < n_rules; r++) {
@@ -477,7 +556,7 @@ kb_status run_rounds(Fix& fx, const kb_rule* rules, u32 n_rules, const std::vect
             bool dead = false;
             for (auto& pr : pl.prem) if (!pr.pred_const) dead = true;  // a variable predicate never matches (join_algorithm.rs:515-521)
             if (dead) continue;
-            if (strict && np != 1 && np != 2) continue;  // semi_naive_parallel.rs:149: other arities are skipped
+            if (strategy == KB_SEMI_NAIVE_PARALLEL && np != 1 && np != 2) continue;  // semi_naive_parallel.rs:149: other arities are skipped
             const u32 n_start = strategy == KB_NAIVE ? 1 : np;
             for (u32 i = 0; i < n_start; i++) {
                 // premise i over the delta (semi-naive) or over all facts (naive), then the others over all facts
@@ -516,10 +595,20 @@ kb_status run_rounds(Fix& fx, const kb_rule* rules, u32 n_rules, const std::vect
         u64 round_new = 0;
         KB_TRY(flush_pending(fx, &round_new));
         tr.mark(ctx, "round end: append", round_new);
-        if (round_new == 0) break;
-        if (st.rounds < 64) st.round_new[st.rounds] = round_new;
-        st.rounds++;
-        st.inferred += round_new;
+        const bool found = qm && fx.probe && fx.probe->found;
+        if (round_new == 0 && !found) {
+            if (qm) qm->fixpoint = true;
+            break;
+        }
+        if (round_new) {
+            if (st.rounds < 64) st.round_new[st.rounds] = round_new;
+            st.rounds++;
+            st.inferred += round_new;
+        }
+        if (found) {
+            qm->stopped_early = true;
+            break;
+        }
         if (round > 100000) return fail(ctx, KB_E_LIMIT, "fixpoint did not converge");
     }
     return KB_OK;
@@ -571,37 +660,8 @@ static kb_status fixpoint_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
     }
     ctx->fix_state.reset();  // taken, stale, or about to be (an unseeded run appends to the store)
 
-    // ---- split the store by predicate: one fused scan per 8 predicates
-    if (!reused) {
-        std::vector<u32> preds;
-        for (auto& kv : fx.rels) preds.push_back(kv.first);
-        for (size_t b = 0; b < preds.size(); b += MAXP) {
-            const u32 k = (u32)std::min<size_t>(MAXP, preds.size() - b);
-            std::vector<std::unique_ptr<kb_rel>> out;
-            // the predicate relations are append-only buffers with the capacity of a whole-store scan output: take the scan, not the
-            // (exactly sized) index slices
-            KB_TRY(scan_predicates(ctx, ctx->segs, preds.data() + b, k, ScanOut::Cols, &out));
-            for (u32 i = 0; i < k; i++) {
-                PredRel& r = fx.rels[preds[b + i]];
-                r.s = out[i]->cols[0];
-                r.o = out[i]->cols[1];
-                r.n = r.base_n = out[i]->n;
-                r.cap = ctx->n_triples;
-                if (r.n * 4 < r.cap) {  // shrink: the scan allocates for the worst case
-                    r.cap = 0;
-                    Col os = r.s, oo = r.o;
-                    u64 n = r.n;
-                    r.n = 0;
-                    KB_TRY(grow_rel(ctx, r, std::max<u64>(n * 2, 1024)));
-                    if (n) {
-                        KB_CUDA(ctx, cudaMemcpyAsync(r.s.ptr, os.ptr, n * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
-                        KB_CUDA(ctx, cudaMemcpyAsync(r.o.ptr, oo.ptr, n * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
-                    }
-                    r.n = n;
-                }
-            }
-        }
-    }
+    // ---- split the store by predicate
+    if (!reused) KB_TRY(split_store(fx));
     tr.mark(ctx, "split store by predicate");
     if (!reused) for (auto& kv : fx.rels) if (kv.second.is_head) {
         kv.second.set_count = kv.second.n;
@@ -716,6 +776,126 @@ extern "C" kb_status kb_datalog_fixpoint_seed(kb_ctx* ctx, const kb_rule* rules,
                                               kb_rel** out, uint64_t* n_seed_new, kb_fixpoint_stats* stats) {
     // (the seed facts are stored with KB_TAG_INFERRED: base and inferred facts can no longer be told apart, so the closed token goes)
     return fixpoint_impl(ctx, rules, n_rules, strategy, true, seed, out, n_seed_new, stats);
+}
+
+// Reasoner::backward_chaining (backward_chaining.rs:165-259): the distinct bindings of the query's variables over T^max_depth, the facts
+// with a proof of height <= max_depth, computed by at most max_depth semi-naive rounds over the demanded facts (kb_backward.cu). Reads
+// the store and leaves it, its index and every state kept for the forward calls as they were.
+extern "C" kb_status kb_datalog_query(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rules, const kb_pattern* query, uint32_t max_depth,
+                                      kb_rel** out, kb_bc_stats* stats) {
+    KB_ENTER(ctx);
+    if ((n_rules && !rules) || !query || !out) return fail(ctx, KB_E_INVALID, "NULL argument");
+    if (max_depth > KB_BC_DEPTH_LIMIT) return fail(ctx, KB_E_LIMIT, "max_depth %u exceeds %u", max_depth, KB_BC_DEPTH_LIMIT);
+    auto term_ok = [&](const kb_term& t, const char* what, u32 r) -> kb_status {
+        if (t.is_var == KB_TERM_QUOTED) return fail(ctx, KB_E_UNSUPPORTED, "%s %u: a quoted-triple term (quoted-triple unification is not supported)", what, r);
+        if (t.is_var > 1) return fail(ctx, KB_E_INVALID, "%s %u: bad term kind %u", what, r, t.is_var);
+        if (!t.is_var && t.value == KB_ID_NONE) return fail(ctx, KB_E_INVALID, "%s %u: KB_ID_NONE is reserved", what, r);
+        return KB_OK;
+    };
+    for (const kb_term* t : {&query->s, &query->p, &query->o}) KB_TRY(term_ok(*t, "query", 0));
+    for (u32 r = 0; r < n_rules; r++) {
+        const kb_rule& rule = rules[r];
+        if (rule.n_premise == 0) return fail(ctx, KB_E_UNSUPPORTED, "rule %u has no premise", r);
+        for (u32 i = 0; i < rule.n_premise; i++) {
+            for (const kb_term* t : {&rule.premise[i].s, &rule.premise[i].p, &rule.premise[i].o}) KB_TRY(term_ok(*t, "rule", r));
+            // the forward rounds never match a variable predicate, SLD resolution would match every fact: refused rather than answered differently
+            if (rule.premise[i].p.is_var) return fail(ctx, KB_E_UNSUPPORTED, "rule %u premise %u: variable predicate", r, i);
+        }
+        for (u32 c = 0; c < rule.n_conclusion; c++)
+            for (const kb_term* t : {&rule.conclusion[c].s, &rule.conclusion[c].p, &rule.conclusion[c].o}) KB_TRY(term_ok(*t, "rule", r));
+    }
+    {  // the shapes the forward driver refuses (unsafe head, variable head predicate, one variable as subject and object of a premise)
+        std::vector<RulePlan> pl;
+        std::map<u32, PredRel> scratch;
+        KB_TRY(compile_rules(ctx, rules, n_rules, &pl, &scratch));
+    }
+    ScopedEvent ev0, ev1;
+    cudaEventRecord(ev0, ctx->st);
+    kb_bc_stats bs{};
+
+    // ---- demand (host): the relevant rules and, per predicate, the patterns its useful facts match
+    BcDemand dem;
+    bc_demand_compile(rules, n_rules, *query, &dem);
+    std::vector<kb_rule> relevant;
+    for (u32 r = 0; r < n_rules; r++) if (dem.relevant[r]) relevant.push_back(rules[r]);
+    Fix fx;
+    Trace tr;
+    fx.ctx = ctx;
+    std::vector<RulePlan> plans;
+    KB_TRY(compile_rules(ctx, relevant.data(), (u32)relevant.size(), &plans, &fx.rels));
+    if (!query->p.is_var) fx.rels[query->p.value].pred = query->p.value;
+    std::vector<u32> preds;
+    for (auto& kv : fx.rels) preds.push_back(kv.first);
+    BcDemandDev dd;
+    KB_TRY(bc_demand_upload(ctx, dem, preds, &dd));
+    fx.demand = &dd;
+
+    // ---- the demanded facts of every predicate the relevant rules and the query mention, and the known-fact sets of the heads
+    KB_TRY(split_store(fx));
+    for (auto& kv : fx.rels) {
+        bs.base_facts += kv.second.n;
+        if (!kv.second.is_head) continue;
+        kv.second.set_count = kv.second.n;
+        KB_TRY(ensure_set(fx, kv.second, 1024));
+    }
+    tr.mark(ctx, "query: demanded facts", bs.base_facts);
+
+    // ---- rounds
+    QueryMode qm;
+    qm.max_rounds = max_depth;
+    Fix::Probe probe;
+    if (!query->s.is_var && !query->p.is_var && !query->o.is_var && fx.rels[query->p.value].is_head) {
+        probe.pred = query->p.value;
+        probe.s = query->s.value;
+        probe.o = query->o.value;
+        fx.probe = &probe;
+    }
+    kb_fixpoint_stats st{};
+    KB_TRY(run_rounds(fx, relevant.data(), (u32)relevant.size(), plans, KB_SEMI_NAIVE, st, tr, &qm));
+
+    // ---- answers: the query's predicate relation; a variable predicate reads every store segment and every derived fact
+    std::vector<BcSource> src;
+    auto rel_source = [&](const PredRel& r, u64 from) {
+        BcSource b;
+        b.in[0] = r.s.ptr + from;
+        b.cval[1] = r.pred;
+        b.in[2] = r.o.ptr + from;
+        b.n = r.n - from;
+        if (b.n) src.push_back(b);
+    };
+    if (!query->p.is_var) rel_source(fx.rels[query->p.value], 0);
+    else {
+        for (auto& sg : ctx->segs) {
+            if (sg.ready) KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st, sg.ready, 0));
+            BcSource b;
+            b.in[0] = sg.s.ptr; b.in[1] = sg.p.ptr; b.in[2] = sg.o.ptr;
+            b.n = sg.n;
+            if (b.n) src.push_back(b);
+        }
+        for (auto& kv : fx.rels) rel_source(kv.second, kv.second.base_n);
+    }
+    std::unique_ptr<kb_rel> res;
+    KB_TRY(bc_answer(ctx, *query, src, &res));
+    tr.mark(ctx, "query: answers", res->n);
+    cudaEventRecord(ev1, ctx->st);
+    KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
+    timers_flush(ctx);
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, ev0, ev1);
+    bs.rounds = qm.rounds;
+    bs.reached_fixpoint = qm.fixpoint;
+    bs.stopped_early = qm.stopped_early;
+    bs.relevant_rules = (u32)relevant.size();
+    bs.demand_patterns = dem.n_patterns;
+    bs.restricted_predicates = (u32)dd.of.size();
+    bs.derived = st.inferred;
+    bs.derivations = st.derivations;
+    bs.answers = res->n;
+    bs.device_ms = ms;
+    if (stats) *stats = bs;
+    ctx->stats.rows_out = res->n;
+    *out = res.release();
+    return KB_OK;
 }
 
 // =====================================================================================================================================

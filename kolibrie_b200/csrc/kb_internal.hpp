@@ -486,6 +486,34 @@ kb_status bgp_components(kb_ctx* ctx, const kb_pattern* pats, u32 n_pats, const 
 u32 pow2_at_least(u64 x);
 kb_status check_pattern(kb_ctx* ctx, const kb_pattern& pt);
 
+// Backward-chaining queries (kb_backward.cu). Demand patterns of a query: per predicate, (x = subject, y = object) with KB_ID_NONE for
+// "any"; a predicate whose list is {(any, any)} is demanded in full, one without a list not at all.
+constexpr u32 BC_MAX_DEMAND = 64;  // patterns per predicate on the host, and in the device table of one call
+struct BcDemand {
+    std::vector<bool> relevant;  // per rule: a conclusion unifies with a demand pattern
+    std::map<u32, std::vector<uint2>> pats;
+    u32 n_patterns = 0;
+};
+// the query's demand patterns: the query's own, then for every rule head that unifies with a demand pattern each premise, with its own
+// constants and the head variables the demand binds, until no new pattern appears (rules as kb_datalog_query has checked them)
+void bc_demand_compile(const kb_rule* rules, u32 n_rules, const kb_pattern& q, BcDemand* d);
+struct BcDemandDev {
+    Buf tab;                                              // the device table
+    std::map<u32, std::pair<const uint2*, u32>> of;       // restricted predicates of `preds`: their patterns in tab (the others: every fact)
+};
+kb_status bc_demand_upload(kb_ctx* ctx, const BcDemand& d, const std::vector<u32>& preds, BcDemandDev* out);
+// launches the selection of the rows of (s, o) [0, n) that match one of the n_dem patterns into new columns of n rows (*out_s, *out_o);
+// their count is control-arena word `count_word` after the caller's next ctrl_read
+kb_status bc_demand_select(kb_ctx* ctx, const uint2* dem, u32 n_dem, const Col& s, const Col& o, u64 n, Col* out_s, Col* out_o, u32 count_word);
+struct BcSource {  // n rows of (s, p, o); in[k] null: every row holds cval[k]
+    const u32* in[3] = {nullptr, nullptr, nullptr};
+    u32 cval[3] = {0, 0, 0};
+    u64 n = 0;
+};
+// the distinct bindings of the query's variables over the facts of `src` that match it: one column per distinct variable in s, p, o
+// first-appearance order; a ground query gives no column and 0 or 1 rows
+kb_status bc_answer(kb_ctx* ctx, const kb_pattern& q, const std::vector<BcSource>& src, std::unique_ptr<kb_rel>* out);
+
 template <class Insert>
 kb_status tag_index_ensure(kb_ctx* ctx, TagIndex* ix, u32 n_keys, u64 extra, const char* what, Insert insert) {
     const u64 need = ((u64)n_keys + extra) * 2 + 64;

@@ -1817,32 +1817,7 @@ void launch_cartesian(const u32* const* lcols, u32 nl, u32 n_lcols, const u32* c
 }
 
 // =================================================================================================================
-// Datalog: known-fact set with 96-bit keys in 16-byte slots {s,p,o,state}
-__device__ __forceinline__ u32 set_hash(u32 s, u32 p, u32 o) { return mix32(mix32(s) * 0x9E3779B1u ^ mix32(o + 0x632BE5ABu) ^ (p * 0x85EBCA77u)); }
-
-// returns 1 if (s,p,o) was inserted now, 0 if it was already there, 2 on overflow
-__device__ __forceinline__ u32 set_insert(uint4* set, u32 n_slots, u32 s, u32 p, u32 o) {
-    const u32 mask = n_slots - 1u;
-    u32 slot = set_hash(s, p, o) & mask;
-    for (u32 probes = 0; probes < n_slots; probes++) {
-        u32* st_ptr = &reinterpret_cast<u32*>(&set[slot])[3];
-        u32 st = atomicCAS(st_ptr, 0u, 1u);
-        if (st == 0u) {
-            u32* w = reinterpret_cast<u32*>(&set[slot]);
-            w[0] = s; w[1] = p; w[2] = o;
-            __threadfence();
-            atomicExch(st_ptr, 2u);
-            return 1u;
-        }
-        while (st == 1u) st = *reinterpret_cast<volatile u32*>(st_ptr);
-        __threadfence();
-        const volatile u32* w = reinterpret_cast<const volatile u32*>(&set[slot]);
-        if (w[0] == s && w[1] == p && w[2] == o) return 0u;
-        slot = (slot + 1u) & mask;
-    }
-    return 2u;
-}
-
+// Datalog: known-fact sets (kb_kernels.cuh)
 __global__ void __launch_bounds__(256) set_insert_kernel(uint4* set, u32 set_slots, const u32* s, const u32* p, u32 p_const, const u32* o,
                                                          u32 n, u32* overflow) {
     const u32 stride = gridDim.x * blockDim.x;
@@ -1856,23 +1831,6 @@ void launch_set_insert(uint4* set, u32 set_slots, const u32* s, const u32* p, u3
     set_insert_kernel<<<grid, 256, 0, st>>>(set, set_slots, s, p, p_const, o, n, overflow);
 }
 
-// 64-bit (s,o) set of one predicate: returns 1 inserted now, 0 already present, 2 table full
-__device__ __forceinline__ u32 set64_insert(u64* set, u32 n_slots, u32 s, u32 o) {
-    const u64 key = ((u64)s << 32) | (u64)o;
-    const u32 mask = n_slots - 1u;
-    u32 slot = mix32(mix32(s) * 0x9E3779B1u ^ mix32(o + 0x632BE5ABu)) & mask;
-    for (u32 probes = 0; probes < n_slots; probes++) {
-        const u64 cur = *reinterpret_cast<volatile u64*>(&set[slot]);
-        if (cur == key) return 0u;
-        if (cur == EMPTY64) {
-            const u64 old = atomicCAS(reinterpret_cast<unsigned long long*>(&set[slot]), (unsigned long long)EMPTY64, (unsigned long long)key);
-            if (old == EMPTY64) return 1u;
-            if (old == key) return 0u;
-        }
-        slot = (slot + 1u) & mask;
-    }
-    return 2u;
-}
 __global__ void __launch_bounds__(256) set64_insert_kernel(u64* set, u32 set_slots, const u32* s, const u32* o, u32 n, u32* overflow) {
     const u32 stride = gridDim.x * blockDim.x;
     for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
@@ -1884,19 +1842,6 @@ void launch_set64_insert(u64* set, u32 set_slots, const u32* s, const u32* o, u3
     set64_insert_kernel<<<grid, 256, 0, st>>>(set, set_slots, s, o, n, overflow);
 }
 
-// slot of (s,o) in a 64-bit set, EMPTY32 when absent (the set is not written by the same launch)
-__device__ __forceinline__ u32 set64_find(const u64* set, u32 n_slots, u32 s, u32 o) {
-    const u64 key = ((u64)s << 32) | (u64)o;
-    const u32 mask = n_slots - 1u;
-    u32 slot = mix32(mix32(s) * 0x9E3779B1u ^ mix32(o + 0x632BE5ABu)) & mask;
-    for (u32 probes = 0; probes < n_slots; probes++) {
-        const u64 cur = set[slot];
-        if (cur == key) return slot;
-        if (cur == EMPTY64) return EMPTY32;
-        slot = (slot + 1u) & mask;
-    }
-    return EMPTY32;
-}
 // set64_insert that returns the key's slot (EMPTY32: table full); *claimed = this call took a free slot for the key
 __device__ __forceinline__ u32 set64_insert_slot(u64* set, u32 n_slots, u32 s, u32 o, bool* claimed) {
     const u64 key = ((u64)s << 32) | (u64)o;
@@ -1915,8 +1860,10 @@ __device__ __forceinline__ u32 set64_insert_slot(u64* set, u32 n_slots, u32 s, u
     }
     return EMPTY32;
 }
-// kb_datalog_maintain's acceptance test in front of the dedup: member of the gate set, no positive count in the veto table
+// the acceptance test in front of the dedup: demanded (kb_datalog_query), member of the gate set and no positive count in the veto table
+// (kb_datalog_maintain)
 __device__ __forceinline__ bool derive_gate_pass(const DeriveParams& P, u32 s, u32 o) {
+    if (P.demand && !bc_demanded(P.demand, P.n_demand, s, o)) return false;
     if (P.gate_set && set64_find(P.gate_set, P.gate_slots, s, o) == EMPTY32) return false;
     if (P.veto_keys) {
         const u32 slot = set64_find(P.veto_keys, P.veto_slots, s, o);
@@ -2043,6 +1990,7 @@ __global__ void __launch_bounds__(DPART_THREADS) derive_partition_kernel(const _
                 nd++;
                 s = P.head_s.is_var ? __ldg(P.bcol[P.head_s.value] + i) : P.head_s.value;
                 o = P.head_o.is_var ? __ldg(P.bcol[P.head_o.value] + i) : P.head_o.value;
+                if (P.demand && !bc_demanded(P.demand, P.n_demand, s, o)) pass = false;
             }
             key[j] = ((u64)s << 32) | (u64)o;
             part[j] = pass ? (set64_home(P.set_slots, s, o) >> Q.slice_bits) : 0xFFFFu;
@@ -2208,7 +2156,7 @@ void launch_derive_partitioned(const DerivePartParams& p, int n_sms, cudaStream_
 void launch_derive(const DeriveParams& p, int n_sms, cudaStream_t st) {
     if (p.n == 0) return;
     int grid = (int)umin64((u64)n_sms * 8ull, ((u64)p.n + 255ull) / 256ull);
-    if (p.gate_set || p.veto_keys) derive_kernel<true><<<grid, 256, 0, st>>>(p);
+    if (p.gate_set || p.veto_keys || p.demand) derive_kernel<true><<<grid, 256, 0, st>>>(p);
     else derive_kernel<false><<<grid, 256, 0, st>>>(p);
 }
 

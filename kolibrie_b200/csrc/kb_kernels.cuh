@@ -367,6 +367,10 @@ struct DeriveParams {
     const u64* veto_keys;
     const u32* veto_cnt;
     u32 veto_slots;
+    // kb_datalog_query: a candidate takes part in the dedup only if it matches one of the head predicate's n_demand demand patterns
+    // (x = subject, y = object, KB_ID_NONE = any; null: every fact is demanded). Applied on both dedup routes.
+    const uint2* demand;
+    u32 n_demand;
 };
 void launch_derive(const DeriveParams& p, int n_sms, cudaStream_t st);
 // RADIX-PARTITIONED candidate dedup (the same work as launch_derive for large candidate sets). The known-fact set is an open-addressing
@@ -386,6 +390,97 @@ struct DerivePartParams {
 };
 void launch_derive_partitioned(const DerivePartParams& p, int n_sms, cudaStream_t st);
 void launch_set64_insert(u64* set, u32 set_slots, const u32* s, const u32* o, u32 n, u32* overflow, int n_sms, cudaStream_t st);
+// ---- the known-fact sets (device side, shared with kb_backward.cu)
+// Datalog: known-fact set with 96-bit keys in 16-byte slots {s,p,o,state}
+__device__ __forceinline__ u32 set_hash(u32 s, u32 p, u32 o) { return mix32(mix32(s) * 0x9E3779B1u ^ mix32(o + 0x632BE5ABu) ^ (p * 0x85EBCA77u)); }
+
+// returns 1 if (s,p,o) was inserted now, 0 if it was already there, 2 on overflow
+__device__ __forceinline__ u32 set_insert(uint4* set, u32 n_slots, u32 s, u32 p, u32 o) {
+    const u32 mask = n_slots - 1u;
+    u32 slot = set_hash(s, p, o) & mask;
+    for (u32 probes = 0; probes < n_slots; probes++) {
+        u32* st_ptr = &reinterpret_cast<u32*>(&set[slot])[3];
+        u32 st = atomicCAS(st_ptr, 0u, 1u);
+        if (st == 0u) {
+            u32* w = reinterpret_cast<u32*>(&set[slot]);
+            w[0] = s; w[1] = p; w[2] = o;
+            __threadfence();
+            atomicExch(st_ptr, 2u);
+            return 1u;
+        }
+        while (st == 1u) st = *reinterpret_cast<volatile u32*>(st_ptr);
+        __threadfence();
+        const volatile u32* w = reinterpret_cast<const volatile u32*>(&set[slot]);
+        if (w[0] == s && w[1] == p && w[2] == o) return 0u;
+        slot = (slot + 1u) & mask;
+    }
+    return 2u;
+}
+
+// 64-bit (s,o) set of one predicate: returns 1 inserted now, 0 already present, 2 table full
+__device__ __forceinline__ u32 set64_insert(u64* set, u32 n_slots, u32 s, u32 o) {
+    const u64 key = ((u64)s << 32) | (u64)o;
+    const u32 mask = n_slots - 1u;
+    u32 slot = mix32(mix32(s) * 0x9E3779B1u ^ mix32(o + 0x632BE5ABu)) & mask;
+    for (u32 probes = 0; probes < n_slots; probes++) {
+        const u64 cur = *reinterpret_cast<volatile u64*>(&set[slot]);
+        if (cur == key) return 0u;
+        if (cur == EMPTY64) {
+            const u64 old = atomicCAS(reinterpret_cast<unsigned long long*>(&set[slot]), (unsigned long long)EMPTY64, (unsigned long long)key);
+            if (old == EMPTY64) return 1u;
+            if (old == key) return 0u;
+        }
+        slot = (slot + 1u) & mask;
+    }
+    return 2u;
+}
+
+// slot of (s,o) in a 64-bit set, EMPTY32 when absent (the set is not written by the same launch)
+__device__ __forceinline__ u32 set64_find(const u64* set, u32 n_slots, u32 s, u32 o) {
+    const u64 key = ((u64)s << 32) | (u64)o;
+    const u32 mask = n_slots - 1u;
+    u32 slot = mix32(mix32(s) * 0x9E3779B1u ^ mix32(o + 0x632BE5ABu)) & mask;
+    for (u32 probes = 0; probes < n_slots; probes++) {
+        const u64 cur = set[slot];
+        if (cur == key) return slot;
+        if (cur == EMPTY64) return EMPTY32;
+        slot = (slot + 1u) & mask;
+    }
+    return EMPTY32;
+}
+// ---- backward-chaining queries (kb_backward.cu)
+// whether (s,o) matches one of n demand patterns (x = subject, y = object, KB_ID_NONE = any)
+__device__ __forceinline__ bool bc_demanded(const uint2* dem, u32 n, u32 s, u32 o) {
+    for (u32 k = 0; k < n; k++) {
+        const uint2 d = dem[k];
+        if ((d.x == 0xFFFFFFFFu || d.x == s) && (d.y == 0xFFFFFFFFu || d.y == o)) return true;
+    }
+    return false;
+}
+// out = the rows (s,o) that match one of the n_dem demand patterns, in no particular order; *out_count = their number (zeroed)
+void launch_bc_demand_select(const u32* s, const u32* o, u32 n, const uint2* dem, u32 n_dem, u32* out_s, u32* out_o, u32* out_count,
+                             int n_sms, cudaStream_t st);
+// The answer pass of kb_datalog_query over n rows of (s, p, o) (in[k] null: every row holds cval[k] there): a row matches the query when
+// every constant position holds q_val and every repeated variable holds the value of its first position; the projection onto the
+// query's n_vars distinct variables (out column j = the value at position var_pos[j]) enters a key set (64-bit keys up to 2 variables,
+// 96-bit keys for 3) and is appended to out[] when it was new.
+struct BcAnswerParams {
+    const u32* in[3];
+    u32 cval[3];
+    u32 n;
+    u32 q_is_var[3], q_val[3];  // per position: a variable (q_val = the position of its first appearance) or the constant q_val
+    u32 n_vars, var_pos[3];
+    u64* set64;                 // n_vars <= 2
+    uint4* set96;               // n_vars == 3
+    u32 set_slots;              // power of two
+    u32* out[3];
+    u32 out_cap;
+    u32* out_count;
+    u32* overflow;              // set or output full
+};
+void launch_bc_answer(const BcAnswerParams& p, int n_sms, cudaStream_t st);
+// *found = 1 when (s,o) is a member of the 64-bit set (a one-thread probe)
+void launch_bc_probe(const u64* set, u32 set_slots, u32 s, u32 o, u32* found, cudaStream_t st);
 void launch_set_insert(uint4* set, u32 set_slots, const u32* s, const u32* p /*null: p_const*/, u32 p_const, const u32* o, u32 n, u32* overflow,
                        int n_sms, cudaStream_t st);
 

@@ -1293,6 +1293,22 @@ class Reasoner:
     def infer_new_facts(self):
         return self.infer_new_facts_naive()  # my_naive.rs:78-80 "for backward compatibility"
 
+    def backward_chaining(self, query: TriplePattern, max_depth: int = c.BC_MAX_DEPTH) -> List[Dict[str, Term]]:
+        """backward_chaining.rs:165-171 on the device (kb_datalog_query): the bindings of the query's variables over the facts with a
+        proof of height <= max_depth. Each distinct binding of the query's own variables comes once, without the renamed rule variables
+        the reference's per-derivation maps carry (quirk Q12). A ground query gives [{}] when it holds and [] when it does not. The
+        store is only read."""
+        self._sync()
+        slots = SlotMap()
+        q = slots.pattern(query)
+        rel, st = self.ctx.datalog_query([compile_rule(r) for r in self.rules], q, max_depth)
+        self.last_stats = st
+        n, sl = rel.info()
+        if not sl:
+            return [{}] if n else []
+        cols = [rel.column(i) for i in range(len(sl))]
+        return [{slots.names[s]: Constant(int(cols[j][i])) for j, s in enumerate(sl)} for i in range(n)]
+
     def query_abox(self, subject: Optional[str], predicate: Optional[str], obj: Optional[str]):
         """reasoning.rs:79-93 — note: like the reference, querying ENCODES unknown strings (they simply match nothing)."""
         self._sync()

@@ -212,6 +212,28 @@ class Reasoner {
         return out;
     }
 
+    // backward_chaining.rs:165-171 on the device (kb_datalog_query): the distinct bindings of the query's variables over the facts with a
+    // proof of height <= max_depth, each once, without the reference's renamed rule variables (quirk Q12); a ground query gives one empty
+    // map when it holds, none when it does not. The store is only read.
+    std::vector<std::map<std::string, Term>> backward_chaining(const TriplePattern& query, uint32_t max_depth = KB_BC_MAX_DEPTH) {
+        sync();
+        CompiledRules cr = compile_rules();
+        SlotMap sm;
+        const kb_pattern q = sm.pattern(query);
+        kb_rel* out = nullptr;
+        dev_->check(kb_datalog_query(dev_->get(), cr.kr.data(), (uint32_t)cr.kr.size(), &q, max_depth, &out, &last_bc_stats));
+        RelHandle h(dev_.get(), out);
+        std::vector<uint32_t> slots;
+        auto cols = download(*dev_, out, &slots);
+        uint64_t n = 0;
+        dev_->check(kb_rel_info(out, &n, nullptr, nullptr));
+        std::vector<std::map<std::string, Term>> res(n);
+        for (uint64_t i = 0; i < n; i++)
+            for (size_t c = 0; c < slots.size(); c++) res[i][sm.names[slots[c]]] = Term::Constant(cols[c][i]);
+        return res;
+    }
+    kb_bc_stats last_bc_stats{};
+
   private:
     static uint32_t cmp_of(const std::string& op) {
         if (op == ">") return KB_CMP_GT;
@@ -241,11 +263,15 @@ class Reasoner {
         }
         dev_->check(kb_dict_numeric_derive(dev_->get(), KB_NUMERIC_F64, 0, nullptr));
     }
-    std::vector<Triple> infer(uint32_t strategy) {
-        sync();
-        std::vector<std::vector<kb_pattern>> prem(rules.size()), conc(rules.size());
-        std::vector<std::vector<kb_rule_filter>> fl(rules.size());
-        std::vector<kb_rule> kr(rules.size());
+    struct CompiledRules {  // kb_rule views over their own pattern and filter arrays
+        std::vector<std::vector<kb_pattern>> prem, conc;
+        std::vector<std::vector<kb_rule_filter>> fl;
+        std::vector<kb_rule> kr;
+    };
+    CompiledRules compile_rules() const {
+        CompiledRules c;
+        auto& prem = c.prem; auto& conc = c.conc; auto& fl = c.fl; auto& kr = c.kr;
+        prem.resize(rules.size()); conc.resize(rules.size()); fl.resize(rules.size()); kr.resize(rules.size());
         for (size_t r = 0; r < rules.size(); r++) {
             SlotMap sm;
             for (auto& p : rules[r].premise) prem[r].push_back(sm.pattern(p));
@@ -259,8 +285,13 @@ class Reasoner {
             }
             kr[r] = kb_rule{prem[r].data(), (uint32_t)prem[r].size(), fl[r].data(), (uint32_t)fl[r].size(), conc[r].data(), (uint32_t)conc[r].size()};
         }
+        return c;
+    }
+    std::vector<Triple> infer(uint32_t strategy) {
+        sync();
+        CompiledRules cr = compile_rules();
         kb_rel* out = nullptr;
-        dev_->check(kb_datalog_fixpoint(dev_->get(), kr.data(), (uint32_t)kr.size(), strategy, &out, &last_stats));
+        dev_->check(kb_datalog_fixpoint(dev_->get(), cr.kr.data(), (uint32_t)cr.kr.size(), strategy, &out, &last_stats));
         RelHandle h(dev_.get(), out);
         std::vector<uint32_t> slots;
         auto cols = download(*dev_, out, &slots);

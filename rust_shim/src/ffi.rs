@@ -34,6 +34,11 @@ pub type kb_quoted_pattern = KbQuotedPattern;  // (the header's name, as the dec
 #[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbMaintainStats { pub base_removed: u64, pub base_added: u64, pub overdeleted: u64, pub rederived: u64,
     pub inferred_removed: u64, pub inferred_added: u64, pub derivations: u64, pub overdelete_rounds: u32, pub insert_rounds: u32, pub device_ms: c_double }
 pub type kb_maintain_stats = KbMaintainStats;  // (the header's name, as the declaration below spells it)
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbBcStats { pub rounds: u32, pub reached_fixpoint: u32, pub stopped_early: u32,
+    pub relevant_rules: u32, pub demand_patterns: u32, pub restricted_predicates: u32, pub base_facts: u64, pub derived: u64, pub derivations: u64,
+    pub answers: u64, pub device_ms: c_double }
+pub type kb_bc_stats = KbBcStats;  // (the header's name, as the declaration below spells it)
+pub const KB_BC_MAX_DEPTH: u32 = 10; pub const KB_BC_DEPTH_LIMIT: u32 = 64;
 #[repr(C)] #[derive(Clone, Copy, Debug)] pub struct KbBindSpec { pub function: u32, pub n_args: u32, pub args: *const KbTerm, pub n_const: u32,
     pub const_offsets: *const u64, pub const_bytes: *const u8, pub out_slot: u32, pub next_qt_id: u32 }
 #[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbBindInfo { pub n_rows: u64, pub n_unbound: u64, pub dict_first: u32, pub dict_new: u32,
@@ -176,6 +181,9 @@ extern "C" {
     // delete-and-rederive across a window slide: the store is closed under the rules (the last fixpoint / maintain with the same rules)
     pub fn kb_datalog_maintain(ctx: *mut KbCtx, rules: *const KbRule, n: u32, strategy: u32, evict_tags: *const u64, n_evict: u32, add: *const KbRel,
                                add_tag: u64, inferred_removed: *mut *mut KbRel, inferred_added: *mut *mut KbRel, stats: *mut kb_maintain_stats) -> kb_status;
+    // backward chaining: the distinct bindings of the query's variables over the facts with a proof of height <= max_depth; the store is only read
+    pub fn kb_datalog_query(ctx: *mut KbCtx, rules: *const KbRule, n_rules: u32, query: *const KbPattern, max_depth: u32, out: *mut *mut KbRel,
+                            stats: *mut kb_bc_stats) -> kb_status;
     // Relation-to-Stream operators: the previous evaluation's distinct rows stay on the device, an evaluation emits the rows that changed
     pub fn kb_r2s_create(ctx: *mut KbCtx, stream_op: u32, slots: *const u32, n_cols: u32, out: *mut *mut kb_r2s) -> kb_status;
     pub fn kb_r2s_eval(ctx: *mut KbCtx, op: *mut kb_r2s, response: *const KbRel, emitted: *mut *mut KbRel) -> kb_status;

@@ -65,3 +65,34 @@ impl<'a> InferenceStrategy for GpuSemiNaiveStrategy<'a> {
         (0..nrows as usize).map(|i| Triple { subject: cols[0][i], predicate: cols[1][i], object: cols[2][i] }).collect()
     }
 }
+
+/// `Reasoner::backward_chaining` (backward_chaining.rs:165-171) on the device: `all_facts` become the store and kb_datalog_query answers
+/// `query` over the facts with a proof of height <= `max_depth` (KB_BC_MAX_DEPTH = the reference's MAX_DEPTH). Each distinct binding of
+/// the query's own variables comes once, without the renamed rule variables (quirk Q12); a ground query gives one empty map when it
+/// holds. None: the device refuses the shape (a quoted term, a rule without premises, a variable premise predicate): the caller runs
+/// the reference's own method.
+pub fn backward_chaining(dev: &mut DeviceStore, all_facts: &[Triple], rules: &[Rule], query: &shared::terms::TriplePattern, max_depth: u32)
+                         -> Option<Vec<std::collections::HashMap<String, shared::terms::Term>>> {
+    let ctx = dev.ctx;
+    let n = all_facts.len();
+    let (mut s, mut p, mut o) = (Vec::with_capacity(n), Vec::with_capacity(n), Vec::with_capacity(n));
+    for t in all_facts { s.push(t.subject); p.push(t.predicate); o.push(t.object); }
+    if unsafe { kb_store_load(ctx, s.as_ptr(), p.as_ptr(), o.as_ptr(), n as u64) } != KB_OK { return None; }
+    dev.invalidate();
+    let compiled: Option<Vec<_>> = rules.iter().map(compile_rule).collect();
+    let compiled = compiled?;
+    let kr: Vec<KbRule> = compiled.iter().map(|(pr, fl, co)| KbRule { premise: pr.as_ptr(), n_premise: pr.len() as u32, filters: fl.as_ptr(),
+        n_filters: fl.len() as u32, conclusion: co.as_ptr(), n_conclusion: co.len() as u32 }).collect();
+    let mut slots = SlotMap::default();
+    let q = slots.pattern(query)?;
+    let mut rel: *mut KbRel = ptr::null_mut();
+    let mut st = std::mem::MaybeUninit::<KbBcStats>::zeroed();
+    if unsafe { kb_datalog_query(ctx, kr.as_ptr(), kr.len() as u32, &q, max_depth, &mut rel, st.as_mut_ptr()) } != KB_OK { return None; }
+    let (mut nrows, mut ncols) = (0u64, 0u32);
+    let mut sl = [0u32; KB_MAX_COLS as usize];
+    unsafe { kb_rel_info(rel, &mut nrows, &mut ncols, sl.as_mut_ptr()) };
+    let mut cols = vec![vec![0u32; nrows as usize]; ncols as usize];
+    for c in 0..ncols as usize { unsafe { kb_rel_download(ctx, rel, c as u32, cols[c].as_mut_ptr()) }; }
+    unsafe { kb_rel_free(ctx, rel) };
+    Some((0..nrows as usize).map(|i| (0..ncols as usize).map(|c| (slots.names[sl[c] as usize].clone(), shared::terms::Term::Constant(cols[c][i]))).collect()).collect())
+}
