@@ -692,6 +692,44 @@ typedef struct kb_bc_stats {
 KB_API kb_status kb_datalog_query(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rules, const kb_pattern* query, uint32_t max_depth,
                                   kb_rel** out, kb_bc_stats* stats /* nullable */);
 
+/* Inconsistency-tolerant querying (Reasoner::add_constraint / query_with_repairs, datalog/src/reasoning.rs:95-150 and
+ * datalog/src/reasoning/repairs.rs:10-43) under IAR semantics: the matches of `query` over the store minus every fact that lies in some
+ * minimal conflict of the constraints. A set of facts violates a constraint iff the constraint's premises all match facts of the set
+ * (constants enforced in every position, a repeated variable equal, the constraint's filters and conclusion ignored); a constraint
+ * without premises never fires. A conflict is the set of distinct facts one match of a constraint's premises instantiates, and it is
+ * minimal iff no other conflict is a strict subset of it. A fact lies in every maximal consistent subset of the store iff it lies in no
+ * minimal conflict, so this is the intersection of the maximal repairs. The reference keeps all maximal repairs and, depending on its
+ * hash order, some non-maximal ones, so its answer can be a strict subset of this one (quirk Q13, DESIGN §4); on a consistent store
+ * both are the query's matches.
+ * Evaluation, recomputed on every call: each constraint's premises run through kb_bgp_execute (its scans, index lookups, reduction,
+ * join order and limits). One kernel instantiates the premises of every match, enters each fact into a fact set whose slot is the
+ * fact's id, and enters the sorted ids of the match's distinct facts into a conflict set. When every conflict has the same size none
+ * can contain another and all are minimal; otherwise one launch probes each conflict's proper subsets (of at least the smallest
+ * conflict size) in the conflict set. The query is then matched by kb_scan's one-pattern path and its matches projected as
+ * kb_datalog_query projects them, dropping every match whose fact is in a minimal conflict.
+ * The store is read only: it, its index, prepared plans and the state the forward calls keep stay as they were.
+ * `*out` has one column per distinct query variable, in s, p, o first-appearance order; its rows are distinct and in no particular
+ * order. A ground query gives a relation without columns and 0 or 1 rows.
+ * Refused before any launch, with nothing changed: a quoted term in the query or a premise, a sharded context (KB_E_UNSUPPORTED); a
+ * constant KB_ID_NONE or a NULL premise array (KB_E_INVALID); more than KB_MAX_PREMISES premises or more than KB_MAX_COLS variables in
+ * a constraint (KB_E_LIMIT). Later, KB_E_LIMIT: kb_bgp_execute's limits, more than 2^32 - 16 matches of one constraint, or a fact
+ * set or conflict set of more than 2^31 slots. */
+typedef struct kb_repair_stats {
+    uint32_t constraints;       /* constraints with at least one premise */
+    uint32_t subsets_probed;    /* 1: conflict sizes differed and the subset probe ran */
+    uint64_t matches;           /* rows of the constraint bodies */
+    uint64_t conflicts;         /* distinct conflict sets */
+    uint64_t minimal_conflicts;
+    uint64_t conflicted_facts;  /* distinct facts in some minimal conflict */
+    uint64_t answers;           /* rows of *out */
+    double device_ms;           /* CUDA-event time of the whole call */
+    double match_ms;            /* of which: the constraint bodies (kb_bgp_execute) */
+    double conflict_ms;         /* the conflict and minimality kernels, with their set allocation and read-backs */
+    double answer_ms;           /* the query's scan and the answer pass */
+} kb_repair_stats;
+KB_API kb_status kb_datalog_query_repairs(kb_ctx* ctx, const kb_rule* constraints, uint32_t n_constraints, const kb_pattern* query,
+                                          kb_rel** out, kb_repair_stats* stats /* nullable */);
+
 /* Sliding-window maintenance of the closure by delete-and-rederive: what a window firing with rules reaches by evicting the previous
  * window, adding the current one and materialising from scratch (rsp_engine.rs:94-109, simple_r2r.rs:103-128), reached from the slide.
  *   B  = the distinct triples of every segment whose tag is not KB_TAG_INFERRED, I = the triples of the KB_TAG_INFERRED segments,

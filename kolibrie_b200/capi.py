@@ -131,6 +131,16 @@ class KbBcStats(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+class KbRepairStats(C.Structure):
+    """kb_repair_stats: what one kb_datalog_query_repairs call matched, found and answered"""
+    _fields_ = [(n, C.c_uint32) for n in ("constraints", "subsets_probed")] + [
+        (n, C.c_uint64) for n in ("matches", "conflicts", "minimal_conflicts", "conflicted_facts", "answers")] + [
+        (n, C.c_double) for n in ("device_ms", "match_ms", "conflict_ms", "answer_ms")]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
 ORDER_VIEW, ORDER_SORT, ORDER_TOPK = 0, 1, 2          # kb_order_route
 ORDER_CONST, ORDER_NUMERIC, ORDER_STRING = 0, 1, 2    # kb_order_kind
 
@@ -341,6 +351,7 @@ def lib() -> C.CDLL:
         "kb_datalog_fixpoint_seed": (i32, [vp, P(KbRule), u32, u32, vp, P(vp), P(u64), P(KbFixpointStats)]),
         "kb_datalog_maintain": (i32, [vp, P(KbRule), u32, u32, P(u64), u32, vp, u64, P(vp), P(vp), P(KbMaintainStats)]),
         "kb_datalog_query": (i32, [vp, P(KbRule), u32, P(KbPattern), u32, P(vp), P(KbBcStats)]),
+        "kb_datalog_query_repairs": (i32, [vp, P(KbRule), u32, P(KbPattern), P(vp), P(KbRepairStats)]),
         "kb_r2s_create": (i32, [vp, u32, P(u32), u32, P(vp)]),
         "kb_r2s_eval": (i32, [vp, vp, vp, P(vp)]),
         "kb_r2s_info": (i32, [vp, P(u64), P(u32)]),
@@ -375,7 +386,7 @@ EXPORTED_SYMBOLS = [
     "kb_rel_from_device", "kb_rel_free", "kb_scan", "kb_filter", "kb_project", "kb_hash_join", "kb_natural_join", "kb_hash_join_keyed", "kb_values", "kb_bind_join", "kb_scan_quoted", "kb_star_join", "kb_bgp_execute", "kb_bgp_last_plan",
     "kb_order_by", "kb_group_aggregate", "kb_groups_info", "kb_groups_keys", "kb_groups_values", "kb_groups_counts", "kb_groups_free", "kb_groups_pack", "kb_groups_merge", "kb_star_join_aggregate",
     "kb_star_join_prepare", "kb_plan_submit", "kb_plan_collect", "kb_plan_info", "kb_plan_free", "kb_plan_peer_scratch_bytes", "kb_plan_attach_peers",
-    "kb_datalog_fixpoint", "kb_datalog_fixpoint_seed", "kb_datalog_maintain", "kb_datalog_query", "kb_r2s_create", "kb_r2s_eval", "kb_r2s_info", "kb_r2s_free", "kb_shard_of", "kb_set_sharding", "kb_partition", "kb_partition_counts", "kb_segment_write", "kb_segment_info", "kb_segment_save", "kb_store_append_file", "kb_shuffle_scatter", "kb_shuffle_push", "kb_rel_wrap_device", "kb_star_join_host", "kb_star_join_host_into", "perform_hash_join_cuda",
+    "kb_datalog_fixpoint", "kb_datalog_fixpoint_seed", "kb_datalog_maintain", "kb_datalog_query", "kb_datalog_query_repairs", "kb_r2s_create", "kb_r2s_eval", "kb_r2s_info", "kb_r2s_free", "kb_shard_of", "kb_set_sharding", "kb_partition", "kb_partition_counts", "kb_segment_write", "kb_segment_info", "kb_segment_save", "kb_store_append_file", "kb_shuffle_scatter", "kb_shuffle_push", "kb_rel_wrap_device", "kb_star_join_host", "kb_star_join_host_into", "perform_hash_join_cuda",
 ]
 
 
@@ -958,6 +969,19 @@ class Context:
         st = KbBcStats()
         q = KbPattern(query.s, query.p, query.o)
         self._check(lib().kb_datalog_query(self.h, arr, len(rules), C.byref(q), max_depth, C.byref(out), C.byref(st)))
+        return Relation(self, out), st
+
+    def datalog_query_repairs(self, constraints: Sequence[dict], query: KbPattern):
+        """kb_datalog_query_repairs: Reasoner::query_with_repairs on the device, under IAR semantics. `constraints` are rule dicts whose
+        "premise" is read ("conclusion" and "filters" may be absent and are ignored). Returns (relation, stats): one column per distinct
+        variable of `query` (s, p, o first-appearance order), each distinct binding of its matches over the store minus the facts of
+        every minimal conflict once; a ground query gives no column and 0 or 1 rows. The store is left as it was."""
+        arr, keep = make_rules([{"premise": r["premise"], "conclusion": r.get("conclusion", []), "filters": r.get("filters", [])}
+                                for r in constraints])
+        out = C.c_void_p()
+        st = KbRepairStats()
+        q = KbPattern(query.s, query.p, query.o)
+        self._check(lib().kb_datalog_query_repairs(self.h, arr, len(constraints), C.byref(q), C.byref(out), C.byref(st)))
         return Relation(self, out), st
 
     def r2s(self, stream_op: int, slots: Sequence[int]) -> "StreamOperator":

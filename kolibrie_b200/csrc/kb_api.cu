@@ -598,7 +598,19 @@ kb_status kb_star_join(kb_ctx* ctx, uint32_t join_slot, const kb_pattern* pats, 
 kb_status kb_bgp_execute(kb_ctx* ctx, const kb_pattern* pats, uint32_t n_pats, const kb_filter_op* filter, uint32_t n_ops,
                          const uint32_t* project, uint32_t n_project, kb_rel** out) {
     KB_ENTER(ctx);
-    if (!pats || !out || n_pats == 0) return kb::fail(ctx, KB_E_INVALID, "NULL or empty BGP");
+    if (!out) return kb::fail(ctx, KB_E_INVALID, "NULL or empty BGP");
+    std::unique_ptr<kb_rel> cur;
+    KB_TRY(kb::bgp_execute_impl(ctx, pats, n_pats, filter, n_ops, project, n_project, &cur));
+    ctx->stats.rows_out = cur->n;
+    *out = cur.release();
+    return KB_OK;
+}
+
+}  // extern "C"
+
+kb_status kb::bgp_execute_impl(kb_ctx* ctx, const kb_pattern* pats, u32 n_pats, const kb_filter_op* filter, u32 n_ops, const u32* project,
+                               u32 n_project, std::unique_ptr<kb_rel>* out) {
+    if (!pats || n_pats == 0) return kb::fail(ctx, KB_E_INVALID, "NULL or empty BGP");
     if (n_pats > KB_BGP_MAX_PATTERNS) return kb::fail(ctx, KB_E_LIMIT, "more than %d patterns", KB_BGP_MAX_PATTERNS);
     KB_TRY(kb::validate_filter(ctx, filter, n_ops));
     std::vector<std::vector<u32>> pv(n_pats), ps(n_pats);
@@ -629,10 +641,11 @@ kb_status kb_bgp_execute(kb_ctx* ctx, const kb_pattern* pats, uint32_t n_pats, c
         std::vector<u32> v(project, project + n_project);
         cur = kb::select_cols(*cur, v);
     }
-    ctx->stats.rows_out = cur->n;
-    *out = cur.release();
+    *out = std::move(cur);
     return KB_OK;
 }
+
+extern "C" {
 
 // ------------------------------------------------------------------ multi-GPU helpers
 uint32_t kb_shard_of(uint32_t key, uint32_t n_shards) { return n_shards ? kb::shard_of(key, n_shards) : 0; }

@@ -149,6 +149,10 @@ __global__ void __launch_bounds__(256) bc_answer_kernel(const __grid_constant__ 
             for (int k = 0; k < 3; k++) v[k] = P.in[k] ? P.in[k][i] : P.cval[k];
 #pragma unroll
             for (int k = 0; k < 3; k++) ok = ok && (P.q_is_var[k] ? v[k] == v[P.q_val[k]] : v[k] == P.q_val[k]);
+            if (ok && P.excl) {
+                const u32 slot = set_find(P.excl, P.excl_slots, v[0], v[1], v[2]);
+                ok = slot == EMPTY32 || P.excl_flag[slot] == 0;
+            }
             if (ok) {
 #pragma unroll
                 for (int j = 0; j < 3; j++) key[j] = j < (int)P.n_vars ? v[P.var_pos[j]] : 0u;
@@ -195,9 +199,14 @@ kb_status bc_demand_select(kb_ctx* ctx, const uint2* dem, u32 n_dem, const Col& 
     return KB_OK;
 }
 
-kb_status bc_answer(kb_ctx* ctx, const kb_pattern& q, const std::vector<BcSource>& src, std::unique_ptr<kb_rel>* out) {
+kb_status bc_answer(kb_ctx* ctx, const kb_pattern& q, const std::vector<BcSource>& src, std::unique_ptr<kb_rel>* out, const BcExclude* excl) {
     // the query's distinct variables in s, p, o first-appearance order (kb_scan's column order)
     BcAnswerParams P{};
+    if (excl) {
+        P.excl = excl->set;
+        P.excl_slots = excl->slots;
+        P.excl_flag = excl->flag;
+    }
     const kb_term* qt[3] = {&q.s, &q.p, &q.o};
     std::vector<u32> slots;
     for (u32 k = 0; k < 3; k++) {

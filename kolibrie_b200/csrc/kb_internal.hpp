@@ -510,9 +510,18 @@ struct BcSource {  // n rows of (s, p, o); in[k] null: every row holds cval[k]
     u32 cval[3] = {0, 0, 0};
     u64 n = 0;
 };
-// the distinct bindings of the query's variables over the facts of `src` that match it: one column per distinct variable in s, p, o
-// first-appearance order; a ground query gives no column and 0 or 1 rows
-kb_status bc_answer(kb_ctx* ctx, const kb_pattern& q, const std::vector<BcSource>& src, std::unique_ptr<kb_rel>* out);
+struct BcExclude {  // facts left out of an answer: those of the 96-bit fact set `set` whose slot has a non-zero byte in `flag`
+    const uint4* set = nullptr;
+    u32 slots = 0;
+    const u8* flag = nullptr;
+};
+// the distinct bindings of the query's variables over the facts of `src` that match it (and that `excl`, when given, does not exclude):
+// one column per distinct variable in s, p, o first-appearance order; a ground query gives no column and 0 or 1 rows
+kb_status bc_answer(kb_ctx* ctx, const kb_pattern& q, const std::vector<BcSource>& src, std::unique_ptr<kb_rel>* out,
+                    const BcExclude* excl = nullptr);
+// kb_bgp_execute without the entry preamble, for calls that run a BGP inside their own (kb_datalog_query_repairs)
+kb_status bgp_execute_impl(kb_ctx* ctx, const kb_pattern* pats, u32 n_pats, const kb_filter_op* filter, u32 n_ops, const u32* project,
+                           u32 n_project, std::unique_ptr<kb_rel>* out);
 
 template <class Insert>
 kb_status tag_index_ensure(kb_ctx* ctx, TagIndex* ix, u32 n_keys, u64 extra, const char* what, Insert insert) {

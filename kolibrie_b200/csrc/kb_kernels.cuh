@@ -394,8 +394,8 @@ void launch_set64_insert(u64* set, u32 set_slots, const u32* s, const u32* o, u3
 // Datalog: known-fact set with 96-bit keys in 16-byte slots {s,p,o,state}
 __device__ __forceinline__ u32 set_hash(u32 s, u32 p, u32 o) { return mix32(mix32(s) * 0x9E3779B1u ^ mix32(o + 0x632BE5ABu) ^ (p * 0x85EBCA77u)); }
 
-// returns 1 if (s,p,o) was inserted now, 0 if it was already there, 2 on overflow
-__device__ __forceinline__ u32 set_insert(uint4* set, u32 n_slots, u32 s, u32 p, u32 o) {
+// returns 1 if (s,p,o) was inserted now, 0 if it was already there, 2 on overflow; *at = the key's slot (1 and 0)
+__device__ __forceinline__ u32 set_insert_at(uint4* set, u32 n_slots, u32 s, u32 p, u32 o, u32* at) {
     const u32 mask = n_slots - 1u;
     u32 slot = set_hash(s, p, o) & mask;
     for (u32 probes = 0; probes < n_slots; probes++) {
@@ -406,15 +406,32 @@ __device__ __forceinline__ u32 set_insert(uint4* set, u32 n_slots, u32 s, u32 p,
             w[0] = s; w[1] = p; w[2] = o;
             __threadfence();
             atomicExch(st_ptr, 2u);
+            *at = slot;
             return 1u;
         }
         while (st == 1u) st = *reinterpret_cast<volatile u32*>(st_ptr);
         __threadfence();
         const volatile u32* w = reinterpret_cast<const volatile u32*>(&set[slot]);
-        if (w[0] == s && w[1] == p && w[2] == o) return 0u;
+        if (w[0] == s && w[1] == p && w[2] == o) { *at = slot; return 0u; }
         slot = (slot + 1u) & mask;
     }
     return 2u;
+}
+__device__ __forceinline__ u32 set_insert(uint4* set, u32 n_slots, u32 s, u32 p, u32 o) {
+    u32 at;
+    return set_insert_at(set, n_slots, s, p, o, &at);
+}
+// slot of (s,p,o) in a 96-bit set, EMPTY32 when absent (the set is not written by the same launch)
+__device__ __forceinline__ u32 set_find(const uint4* set, u32 n_slots, u32 s, u32 p, u32 o) {
+    const u32 mask = n_slots - 1u;
+    u32 slot = set_hash(s, p, o) & mask;
+    for (u32 probes = 0; probes < n_slots; probes++) {
+        const uint4 w = set[slot];
+        if (w.w == 0u) return EMPTY32;
+        if (w.x == s && w.y == p && w.z == o) return slot;
+        slot = (slot + 1u) & mask;
+    }
+    return EMPTY32;
 }
 
 // 64-bit (s,o) set of one predicate: returns 1 inserted now, 0 already present, 2 table full
@@ -477,6 +494,11 @@ struct BcAnswerParams {
     u32 out_cap;
     u32* out_count;
     u32* overflow;              // set or output full
+    // kb_datalog_query_repairs (null for kb_datalog_query): a row whose fact (s, p, o) is in the fact set `excl` at a slot whose byte
+    // excl_flag[slot] is non-zero is dropped
+    const uint4* excl;
+    u32 excl_slots;
+    const u8* excl_flag;
 };
 void launch_bc_answer(const BcAnswerParams& p, int n_sms, cudaStream_t st);
 // *found = 1 when (s,o) is a member of the 64-bit set (a one-thread probe)

@@ -287,6 +287,26 @@ def taxonomy_rules(d: TaxonomyData):
     return [r1, r2]
 
 
+def taxonomy_conflicts(d: TaxonomyData, fanout: int = 10, depth: int = 6, frac: float = 0.01, seed: int = 47):
+    """Inconsistency for the taxonomy shape: a second, seeded leaf type for `frac` of the instances, and `disjointWith` (id d.n_ids)
+    between every ordered pair of the `fanout` level-1 classes. Returns (s, p, o) of the added facts, the disjointWith id and the
+    level-1 class ids. An instance whose two leaves lie under different level-1 classes violates
+    (?x type ?a), (?x type ?b), (?a disjointWith ?b) once the types are closed under subClassOf."""
+    g = np.random.default_rng(seed)
+    X0 = 2 + d.n_classes
+    n_leaves = fanout ** depth
+    xs = np.unique(g.integers(0, d.n_instances, max(1, int(d.n_instances * frac)))) + X0
+    leaves = 2 + d.n_classes - n_leaves + g.integers(0, n_leaves, len(xs))
+    dw = d.n_ids
+    level1 = np.arange(3, 3 + fanout, dtype=np.int64)
+    a, b = np.meshgrid(level1, level1, indexing="ij")
+    keep = a != b
+    s = np.concatenate([xs, a[keep]]).astype(np.uint32)
+    p = np.concatenate([np.full(len(xs), d.ids["rdf:type"]), np.full(int(keep.sum()), dw)]).astype(np.uint32)
+    o = np.concatenate([leaves, b[keep]]).astype(np.uint32)
+    return (s, p, o), dw, level1.astype(np.uint32)
+
+
 @dataclass
 class AnnotatedSalaries:
     """The employee shape plus one RDF-star annotation per salary triple: `<< e ds:annual_salary s >> ex:source src_k`."""

@@ -1203,6 +1203,7 @@ class Reasoner:
     def __init__(self, ctx: Optional[c.Context] = None, device: int = 0):
         self.dictionary = Dictionary()
         self.rules: List[Rule] = []
+        self.constraints: List[Rule] = []
         self.ctx = ctx or c.Context(device)
         self._facts: List[Tuple[int, int, int]] = []
         self._fact_set: set = set()
@@ -1221,6 +1222,10 @@ class Reasoner:
 
     def add_rule(self, rule: Rule):
         self.rules.append(rule)
+
+    def add_constraint(self, constraint: Rule):
+        """reasoning.rs:95-98: a denial constraint; only its premises are read (its filters and conclusion are ignored)"""
+        self.constraints.append(constraint)
 
     def _sync(self):
         if self._dirty:
@@ -1308,6 +1313,22 @@ class Reasoner:
             return [{}] if n else []
         cols = [rel.column(i) for i in range(len(sl))]
         return [{slots.names[s]: Constant(int(cols[j][i])) for j, s in enumerate(sl)} for i in range(n)]
+
+    def query_with_repairs(self, query: TriplePattern) -> List[Dict[str, int]]:
+        """repairs.rs:10-43 on the device (kb_datalog_query_repairs), under IAR semantics: the query's bindings over the facts that lie
+        in no minimal conflict of the constraints. Each distinct binding comes once, as ids (the reference's u32 values). The
+        reference's answer can be a strict subset of this one when its search keeps a non-maximal repair (quirk Q13). A ground query
+        gives [{}] when it holds and [] when it does not. The store is only read."""
+        self._sync()
+        slots = SlotMap()
+        q = slots.pattern(query)
+        rel, st = self.ctx.datalog_query_repairs([compile_rule(r) for r in self.constraints], q)
+        self.last_stats = st
+        n, sl = rel.info()
+        if not sl:
+            return [{}] if n else []
+        cols = [rel.column(i) for i in range(len(sl))]
+        return [{slots.names[s]: int(cols[j][i]) for j, s in enumerate(sl)} for i in range(n)]
 
     def query_abox(self, subject: Optional[str], predicate: Optional[str], obj: Optional[str]):
         """reasoning.rs:79-93 — note: like the reference, querying ENCODES unknown strings (they simply match nothing)."""

@@ -173,6 +173,7 @@ class Reasoner {
   public:
     Dictionary dictionary;
     std::vector<Rule> rules;
+    std::vector<Rule> constraints;
     kb_fixpoint_stats last_stats{};
     explicit Reasoner(std::shared_ptr<Device> dev = std::make_shared<Device>(0)) : dev_(std::move(dev)) {}
 
@@ -181,6 +182,8 @@ class Reasoner {
         if (fact_set_.insert(t).second) { facts_.push_back(t); dirty_ = true; }  // index_manager.insert dedups (index_manager.rs:41-57)
     }
     void add_rule(const Rule& r) { rules.push_back(r); }
+    // reasoning.rs:95-98: a denial constraint; only its premises are read (its filters and conclusion are ignored)
+    void add_constraint(const Rule& r) { constraints.push_back(r); }
     std::vector<Triple> infer_new_facts_semi_naive() { return infer(KB_SEMI_NAIVE); }
     std::vector<Triple> infer_new_facts_naive() { return infer(KB_NAIVE); }
     std::vector<Triple> infer_new_facts() { return infer_new_facts_naive(); }  // my_naive.rs:78-80
@@ -217,7 +220,7 @@ class Reasoner {
     // map when it holds, none when it does not. The store is only read.
     std::vector<std::map<std::string, Term>> backward_chaining(const TriplePattern& query, uint32_t max_depth = KB_BC_MAX_DEPTH) {
         sync();
-        CompiledRules cr = compile_rules();
+        CompiledRules cr = compile_rules(rules);
         SlotMap sm;
         const kb_pattern q = sm.pattern(query);
         kb_rel* out = nullptr;
@@ -233,6 +236,28 @@ class Reasoner {
         return res;
     }
     kb_bc_stats last_bc_stats{};
+
+    // repairs.rs:10-43 on the device (kb_datalog_query_repairs), under IAR semantics: the distinct bindings of the query's variables, as
+    // ids, over the facts that lie in no minimal conflict of the constraints. The reference's answer can be a strict subset when its
+    // search keeps a non-maximal repair (quirk Q13). A ground query gives one empty map when it holds. The store is only read.
+    std::vector<std::map<std::string, uint32_t>> query_with_repairs(const TriplePattern& query) {
+        sync();
+        CompiledRules cr = compile_rules(constraints);
+        SlotMap sm;
+        const kb_pattern q = sm.pattern(query);
+        kb_rel* out = nullptr;
+        dev_->check(kb_datalog_query_repairs(dev_->get(), cr.kr.data(), (uint32_t)cr.kr.size(), &q, &out, &last_repair_stats));
+        RelHandle h(dev_.get(), out);
+        std::vector<uint32_t> slots;
+        auto cols = download(*dev_, out, &slots);
+        uint64_t n = 0;
+        dev_->check(kb_rel_info(out, &n, nullptr, nullptr));
+        std::vector<std::map<std::string, uint32_t>> res(n);
+        for (uint64_t i = 0; i < n; i++)
+            for (size_t c = 0; c < slots.size(); c++) res[i][sm.names[slots[c]]] = cols[c][i];
+        return res;
+    }
+    kb_repair_stats last_repair_stats{};
 
   private:
     static uint32_t cmp_of(const std::string& op) {
@@ -268,15 +293,15 @@ class Reasoner {
         std::vector<std::vector<kb_rule_filter>> fl;
         std::vector<kb_rule> kr;
     };
-    CompiledRules compile_rules() const {
+    CompiledRules compile_rules(const std::vector<Rule>& rs) const {
         CompiledRules c;
         auto& prem = c.prem; auto& conc = c.conc; auto& fl = c.fl; auto& kr = c.kr;
-        prem.resize(rules.size()); conc.resize(rules.size()); fl.resize(rules.size()); kr.resize(rules.size());
-        for (size_t r = 0; r < rules.size(); r++) {
+        prem.resize(rs.size()); conc.resize(rs.size()); fl.resize(rs.size()); kr.resize(rs.size());
+        for (size_t r = 0; r < rs.size(); r++) {
             SlotMap sm;
-            for (auto& p : rules[r].premise) prem[r].push_back(sm.pattern(p));
-            for (auto& p : rules[r].conclusion) conc[r].push_back(sm.pattern(p));
-            for (auto& f : rules[r].filters) {
+            for (auto& p : rs[r].premise) prem[r].push_back(sm.pattern(p));
+            for (auto& p : rs[r].conclusion) conc[r].push_back(sm.pattern(p));
+            for (auto& f : rs[r].filters) {
                 if (!sm.has(f.variable)) continue;  // unbound lhs: the reference skips the filter (rules.rs:139)
                 kb_rule_filter k{sm.of(f.variable), cmp_of(f.op), 0, 0, 0.0};
                 if (sm.has(f.value)) { k.rhs_is_var = 1; k.rhs_slot = sm.of(f.value); }
@@ -289,7 +314,7 @@ class Reasoner {
     }
     std::vector<Triple> infer(uint32_t strategy) {
         sync();
-        CompiledRules cr = compile_rules();
+        CompiledRules cr = compile_rules(rules);
         kb_rel* out = nullptr;
         dev_->check(kb_datalog_fixpoint(dev_->get(), cr.kr.data(), (uint32_t)cr.kr.size(), strategy, &out, &last_stats));
         RelHandle h(dev_.get(), out);

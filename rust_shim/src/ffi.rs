@@ -39,6 +39,10 @@ pub type kb_maintain_stats = KbMaintainStats;  // (the header's name, as the dec
     pub answers: u64, pub device_ms: c_double }
 pub type kb_bc_stats = KbBcStats;  // (the header's name, as the declaration below spells it)
 pub const KB_BC_MAX_DEPTH: u32 = 10; pub const KB_BC_DEPTH_LIMIT: u32 = 64;
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbRepairStats { pub constraints: u32, pub subsets_probed: u32, pub matches: u64,
+    pub conflicts: u64, pub minimal_conflicts: u64, pub conflicted_facts: u64, pub answers: u64, pub device_ms: c_double, pub match_ms: c_double,
+    pub conflict_ms: c_double, pub answer_ms: c_double }
+pub type kb_repair_stats = KbRepairStats;  // (the header's name, as the declaration below spells it)
 #[repr(C)] #[derive(Clone, Copy, Debug)] pub struct KbBindSpec { pub function: u32, pub n_args: u32, pub args: *const KbTerm, pub n_const: u32,
     pub const_offsets: *const u64, pub const_bytes: *const u8, pub out_slot: u32, pub next_qt_id: u32 }
 #[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbBindInfo { pub n_rows: u64, pub n_unbound: u64, pub dict_first: u32, pub dict_new: u32,
@@ -184,6 +188,8 @@ extern "C" {
     // backward chaining: the distinct bindings of the query's variables over the facts with a proof of height <= max_depth; the store is only read
     pub fn kb_datalog_query(ctx: *mut KbCtx, rules: *const KbRule, n_rules: u32, query: *const KbPattern, max_depth: u32, out: *mut *mut KbRel,
                             stats: *mut kb_bc_stats) -> kb_status;
+    pub fn kb_datalog_query_repairs(ctx: *mut KbCtx, constraints: *const KbRule, n_constraints: u32, query: *const KbPattern, out: *mut *mut KbRel,
+                                    stats: *mut kb_repair_stats) -> kb_status;
     // Relation-to-Stream operators: the previous evaluation's distinct rows stay on the device, an evaluation emits the rows that changed
     pub fn kb_r2s_create(ctx: *mut KbCtx, stream_op: u32, slots: *const u32, n_cols: u32, out: *mut *mut kb_r2s) -> kb_status;
     pub fn kb_r2s_eval(ctx: *mut KbCtx, op: *mut kb_r2s, response: *const KbRel, emitted: *mut *mut KbRel) -> kb_status;

@@ -96,3 +96,34 @@ pub fn backward_chaining(dev: &mut DeviceStore, all_facts: &[Triple], rules: &[R
     unsafe { kb_rel_free(ctx, rel) };
     Some((0..nrows as usize).map(|i| (0..ncols as usize).map(|c| (slots.names[sl[c] as usize].clone(), shared::terms::Term::Constant(cols[c][i]))).collect()).collect())
 }
+
+/// `Reasoner::query_with_repairs` (repairs.rs:10-43) on the device, under IAR semantics: `all_facts` become the store and
+/// kb_datalog_query_repairs answers `query` over the facts that lie in no minimal conflict of `constraints` (their premises are read,
+/// their filters and conclusions are not). Each distinct binding comes once, as ids; the reference's answer can be a strict subset of it
+/// when its search keeps a non-maximal repair (quirk Q13). A ground query gives one empty map when it holds. None: the device refuses
+/// the shape (a quoted term, more than KB_MAX_PREMISES premises): the caller runs the reference's own method.
+pub fn query_with_repairs(dev: &mut DeviceStore, all_facts: &[Triple], constraints: &[Rule], query: &shared::terms::TriplePattern)
+                          -> Option<Vec<std::collections::HashMap<String, u32>>> {
+    let ctx = dev.ctx;
+    let n = all_facts.len();
+    let (mut s, mut p, mut o) = (Vec::with_capacity(n), Vec::with_capacity(n), Vec::with_capacity(n));
+    for t in all_facts { s.push(t.subject); p.push(t.predicate); o.push(t.object); }
+    if unsafe { kb_store_load(ctx, s.as_ptr(), p.as_ptr(), o.as_ptr(), n as u64) } != KB_OK { return None; }
+    dev.invalidate();
+    let compiled: Option<Vec<_>> = constraints.iter().map(compile_rule).collect();
+    let compiled = compiled?;
+    let kr: Vec<KbRule> = compiled.iter().map(|(pr, fl, co)| KbRule { premise: pr.as_ptr(), n_premise: pr.len() as u32, filters: fl.as_ptr(),
+        n_filters: fl.len() as u32, conclusion: co.as_ptr(), n_conclusion: co.len() as u32 }).collect();
+    let mut slots = SlotMap::default();
+    let q = slots.pattern(query)?;
+    let mut rel: *mut KbRel = ptr::null_mut();
+    let mut st = std::mem::MaybeUninit::<KbRepairStats>::zeroed();
+    if unsafe { kb_datalog_query_repairs(ctx, kr.as_ptr(), kr.len() as u32, &q, &mut rel, st.as_mut_ptr()) } != KB_OK { return None; }
+    let (mut nrows, mut ncols) = (0u64, 0u32);
+    let mut sl = [0u32; KB_MAX_COLS as usize];
+    unsafe { kb_rel_info(rel, &mut nrows, &mut ncols, sl.as_mut_ptr()) };
+    let mut cols = vec![vec![0u32; nrows as usize]; ncols as usize];
+    for c in 0..ncols as usize { unsafe { kb_rel_download(ctx, rel, c as u32, cols[c].as_mut_ptr()) }; }
+    unsafe { kb_rel_free(ctx, rel) };
+    Some((0..nrows as usize).map(|i| (0..ncols as usize).map(|c| (slots.names[sl[c] as usize].clone(), cols[c][i])).collect()).collect())
+}
