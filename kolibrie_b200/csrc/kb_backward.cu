@@ -104,10 +104,10 @@ kb_status bc_demand_upload(kb_ctx* ctx, const BcDemand& d, const std::vector<u32
     return KB_OK;
 }
 
-// ---- kernels
-__global__ void __launch_bounds__(256) bc_demand_select_kernel(const u32* __restrict__ s, const u32* __restrict__ o, u32 n, const uint2* dem,
-                                                               u32 n_dem, u32* out_s, u32* out_o, u32* out_count) {
-    const int lane = threadIdx.x & 31;
+// ---- kernels and their launch formats (private to this file)
+// out = the rows (s,o) that match one of the n_dem demand patterns, in no particular order; *out_count = their number (zeroed)
+static __global__ void __launch_bounds__(256) bc_demand_select_kernel(const u32* __restrict__ s, const u32* __restrict__ o, u32 n, const uint2* dem,
+                                                                      u32 n_dem, u32* out_s, u32* out_o, u32* out_count) {
     const u32 stride = gridDim.x * blockDim.x;
     const u32 n_round = (n + 31u) & ~31u;
     for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += stride) {
@@ -118,25 +118,39 @@ __global__ void __launch_bounds__(256) bc_demand_select_kernel(const u32* __rest
             b = o[i];
             take = bc_demanded(dem, n_dem, a, b);
         }
-        const unsigned m = __ballot_sync(0xffffffffu, take);  // warp-aggregated compaction
-        if (!m) continue;
-        u32 base = 0;
-        if (lane == __ffs(m) - 1) base = atomicAdd(out_count, (u32)__popc(m));
-        base = __shfl_sync(0xffffffffu, base, __ffs(m) - 1);
-        if (take) {
-            const u32 r = base + (u32)__popc(m & ((1u << lane) - 1u));
-            out_s[r] = a;
-            out_o[r] = b;
-        }
+        emit_pair(take, a, b, out_s, out_o, out_count);
     }
 }
-void launch_bc_demand_select(const u32* s, const u32* o, u32 n, const uint2* dem, u32 n_dem, u32* out_s, u32* out_o, u32* out_count,
-                             int n_sms, cudaStream_t st) {
+static void launch_bc_demand_select(const u32* s, const u32* o, u32 n, const uint2* dem, u32 n_dem, u32* out_s, u32* out_o, u32* out_count,
+                                    int n_sms, cudaStream_t st) {
     if (n == 0) return;
     bc_demand_select_kernel<<<grid_1d(n, n_sms), 256, 0, st>>>(s, o, n, dem, n_dem, out_s, out_o, out_count);
 }
 
-__global__ void __launch_bounds__(256) bc_answer_kernel(const __grid_constant__ BcAnswerParams P) {
+// The answer pass of kb_datalog_query over n rows of (s, p, o) (in[k] null: every row holds cval[k] there): a row matches the query when
+// every constant position holds q_val and every repeated variable holds the value of its first position; the projection onto the
+// query's n_vars distinct variables (out column j = the value at position var_pos[j]) enters a key set (64-bit keys up to 2 variables,
+// 96-bit keys for 3) and is appended to out[] when it was new.
+struct BcAnswerParams {
+    const u32* in[3];
+    u32 cval[3];
+    u32 n;
+    u32 q_is_var[3], q_val[3];  // per position: a variable (q_val = the position of its first appearance) or the constant q_val
+    u32 n_vars, var_pos[3];
+    u64* set64;                 // n_vars <= 2
+    uint4* set96;               // n_vars == 3
+    u32 set_slots;              // power of two
+    u32* out[3];
+    u32 out_cap;
+    u32* out_count;
+    u32* overflow;              // set or output full
+    // kb_datalog_query_repairs (null for kb_datalog_query): a row whose fact (s, p, o) is in the fact set `excl` at a slot whose byte
+    // excl_flag[slot] is non-zero is dropped
+    const uint4* excl;
+    u32 excl_slots;
+    const u8* excl_flag;
+};
+static __global__ void __launch_bounds__(256) bc_answer_kernel(const __grid_constant__ BcAnswerParams P) {
     const int lane = threadIdx.x & 31;
     const u32 stride = gridDim.x * blockDim.x;
     const u32 n_round = (P.n + 31u) & ~31u;
@@ -175,16 +189,9 @@ __global__ void __launch_bounds__(256) bc_answer_kernel(const __grid_constant__ 
         }
     }
 }
-void launch_bc_answer(const BcAnswerParams& p, int n_sms, cudaStream_t st) {
+static void launch_bc_answer(const BcAnswerParams& p, int n_sms, cudaStream_t st) {
     if (p.n == 0) return;
     bc_answer_kernel<<<grid_1d(p.n, n_sms), 256, 0, st>>>(p);
-}
-
-__global__ void bc_probe_kernel(const u64* set, u32 set_slots, u32 s, u32 o, u32* found) {
-    *found = set64_find(set, set_slots, s, o) != EMPTY32 ? 1u : 0u;
-}
-void launch_bc_probe(const u64* set, u32 set_slots, u32 s, u32 o, u32* found, cudaStream_t st) {
-    bc_probe_kernel<<<1, 1, 0, st>>>(set, set_slots, s, o, found);
 }
 
 // ---- host side of the two passes

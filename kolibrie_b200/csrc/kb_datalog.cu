@@ -1,4 +1,7 @@
-// kb_datalog.cu — semi-naive / naive Datalog materialisation on the device.
+// kb_datalog.cu — Datalog on the device: semi-naive / naive materialisation (kb_datalog_fixpoint, kb_datalog_fixpoint_seed),
+// backward-chaining queries (kb_datalog_query; demand patterns and the answer pass in kb_backward.cu) and delete-and-rederive
+// maintenance (kb_datalog_maintain). The file owns the Datalog kernels (known-fact sets, derive and its radix-partitioned variant, the
+// maintenance kernels), their launch formats, and the host driver that launches them.
 // Replaces Reasoner::infer_with_strategy (datalog/src/reasoning/materialisation/infer_generic.rs:27-53) driving
 // SemiNaiveStrategy (semi_naive.rs:17-85) or NaiveStrategy (my_naive.rs:18-69), whose join is
 // perform_hash_join_for_rules (shared/src/join_algorithm.rs:499-677).
@@ -6,8 +9,8 @@
 // Layout: one (s,o) column pair per predicate that occurs in a rule, append-only, exactly like the reference's
 // `all_facts: Vec<Triple>` with its delta suffix (semi_naive.rs:57-59) but partitioned by predicate once instead of
 // re-filtered by predicate for every premise of every rule of every round (join_algorithm.rs:528-534).
-// known_facts (infer_generic.rs:30) is a device hash set of 96-bit (s,p,o) keys; a derived fact is new iff its insert wins.
-// Round structure is the reference's: every rule of a round sees the same snapshot; new facts become visible (and become the
+// known_facts (infer_generic.rs:30) is a device hash set of 64-bit (s,o) keys per head predicate; a derived fact is new iff its insert
+// wins. Round structure is the reference's: every rule of a round sees the same snapshot; new facts become visible (and become the
 // next delta) only after the round (infer_generic.rs:42-48) — so round counts and per-round fact counts match the oracle.
 //
 // kb_datalog_maintain keeps a closed store closed across a window slide by delete-and-rederive (DRed) over the same per-predicate
@@ -16,12 +19,539 @@
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
-#include <functional>
 
 #include "kb_internal.hpp"
 
 using namespace kb;
 
+namespace kb {
+
+// =====================================================================================================================================
+// Device side. The launch formats below and everything behind them are private to this file; what kb_backward.cu reads too (set64_insert,
+// set64_find, bc_demanded, emit_pair) is in kb_kernels.cuh.
+
+// ---- known-fact sets: 64-bit (s,o) keys of one predicate
+static __global__ void __launch_bounds__(256) set64_insert_kernel(u64* set, u32 set_slots, const u32* s, const u32* o, u32 n, u32* overflow) {
+    const u32 stride = gridDim.x * blockDim.x;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+        if (set64_insert(set, set_slots, s[i], o[i]) == 2u) *overflow = 1u;
+}
+static void launch_set64_insert(u64* set, u32 set_slots, const u32* s, const u32* o, u32 n, u32* overflow, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull);
+    set64_insert_kernel<<<grid, 256, 0, st>>>(set, set_slots, s, o, n, overflow);
+}
+
+// ---- derive
+// instantiate rule heads from binding columns, apply rule filters (rules.rs:133-165), insert into the head predicate's known-fact set
+// and append the facts that were new (infer_generic.rs:42-48)
+struct HeadTerm { u32 is_var, value; };  // value = binding column index or constant id
+struct RuleFilterDev { u32 lhs_col, cmp, rhs_is_var, rhs_col; double rhs_value; };
+struct DeriveParams {
+    const u32* bcol[KB_MAX_COLS];
+    u32 n;
+    HeadTerm head_s, head_o;  // the head predicate is a constant: one known-fact set per predicate, keyed by (s << 32) | o
+    RuleFilterDev filt[KB_MAX_RULE_FILTERS];
+    u32 n_filt;
+    NumTab nt;
+    u64* set;       // open addressing, EMPTY64 = free; a fact is new iff its atomicCAS wins
+    u32 set_slots;  // power of two
+    u32 *out_s, *out_o;
+    u32 out_cap;
+    u32 budget;                   // stop inserting once this many facts were appended (keeps the set's load bounded): overflow = 2
+    u32* out_count;               // appended so far (atomic cursor)
+    unsigned long long* n_deriv;  // candidates that passed the filters
+    u32* overflow;                // 1: set or output full (error); 2: budget reached, the host grows the set and runs the launch again
+    // kb_datalog_maintain (delete-and-rederive): a candidate takes part in the dedup only if it is a member of gate_set (when non-null)
+    // and has no positive count in the veto table (when non-null). Gated launches never take the partitioned path.
+    const u64* gate_set;
+    u32 gate_slots;
+    const u64* veto_keys;
+    const u32* veto_cnt;
+    u32 veto_slots;
+    // kb_datalog_query: a candidate takes part in the dedup only if it matches one of the head predicate's n_demand demand patterns
+    // (x = subject, y = object, KB_ID_NONE = any; null: every fact is demanded). Applied on both dedup routes.
+    const uint2* demand;
+    u32 n_demand;
+};
+// RADIX-PARTITIONED candidate dedup (the same work as launch_derive for large candidate sets). The known-fact set is an open-addressing
+// table far larger than L2 (config 4: 8 GB), so a direct probe per candidate is one random DRAM line per candidate. Here the
+// candidates are first partitioned by the HIGH bits of their home slot (tile sorted by partition in shared memory, one range
+// reservation per tile and partition, coalesced runs), so that partition p only touches slice p of the table; the probe pass then walks
+// the partitions in order, every CTA on (nearly) the same slice, which is sized to stay resident in L2.
+struct DerivePartParams {
+    DeriveParams d;            // candidates, head, filters, set, outputs, counters (as for launch_derive)
+    u32 slice_bits;            // log2(slots per slice); partition = home slot >> slice_bits
+    u32 n_parts;               // set_slots >> slice_bits, <= 1024
+    u64* buckets;              // [n_parts][bucket_cap] candidate keys (s << 32 | o)
+    u32 bucket_cap;
+    u32* cursors;              // [n_parts] keys in each bucket (zeroed)
+    u32* tile_start;           // [n_parts + 1] first probe tile of each partition (written by the launch)
+    u32* tickets;              // [2] zeroed: tile counters of the two passes
+};
+
+// set64_insert that returns the key's slot (EMPTY32: table full); *claimed = this call took a free slot for the key
+static __device__ __forceinline__ u32 set64_insert_slot(u64* set, u32 n_slots, u32 s, u32 o, bool* claimed) {
+    const u64 key = ((u64)s << 32) | (u64)o;
+    const u32 mask = n_slots - 1u;
+    u32 slot = mix32(mix32(s) * 0x9E3779B1u ^ mix32(o + 0x632BE5ABu)) & mask;
+    *claimed = false;
+    for (u32 probes = 0; probes < n_slots; probes++) {
+        const u64 cur = *reinterpret_cast<volatile u64*>(&set[slot]);
+        if (cur == key) return slot;
+        if (cur == EMPTY64) {
+            const u64 old = atomicCAS(reinterpret_cast<unsigned long long*>(&set[slot]), (unsigned long long)EMPTY64, (unsigned long long)key);
+            if (old == EMPTY64) { *claimed = true; return slot; }
+            if (old == key) return slot;
+        }
+        slot = (slot + 1u) & mask;
+    }
+    return EMPTY32;
+}
+// the acceptance test in front of the dedup: demanded (kb_datalog_query), member of the gate set and no positive count in the veto table
+// (kb_datalog_maintain)
+static __device__ __forceinline__ bool derive_gate_pass(const DeriveParams& P, u32 s, u32 o) {
+    if (P.demand && !bc_demanded(P.demand, P.n_demand, s, o)) return false;
+    if (P.gate_set && set64_find(P.gate_set, P.gate_slots, s, o) == EMPTY32) return false;
+    if (P.veto_keys) {
+        const u32 slot = set64_find(P.veto_keys, P.veto_slots, s, o);
+        if (slot != EMPTY32 && P.veto_cnt[slot] > 0u) return false;
+    }
+    return true;
+}
+
+static __device__ __forceinline__ bool rule_filters_pass(const DeriveParams& P, u32 i) {
+    for (u32 f = 0; f < P.n_filt; f++) {
+        const RuleFilterDev fl = P.filt[f];
+        const u32 lhs = P.bcol[fl.lhs_col][i];
+        if (fl.rhs_is_var) {  // rules.rs:141-146 — ids of two bound variables; only = / != act
+            const u32 rhs = P.bcol[fl.rhs_col][i];
+            if (fl.cmp == KB_CMP_NE && lhs == rhs) return false;
+            if (fl.cmp == KB_CMP_EQ && lhs != rhs) return false;
+        } else {  // rules.rs:148-160
+            const double a = num_of(P.nt, lhs), c = fl.rhs_value;
+            const double eps = 2.220446049250313e-16;
+            switch (fl.cmp) {
+                case KB_CMP_GT: if (a <= c) return false; break;
+                case KB_CMP_LT: if (a >= c) return false; break;
+                case KB_CMP_GE: if (a < c) return false; break;
+                case KB_CMP_LE: if (a > c) return false; break;
+                case KB_CMP_EQ: if (fabs(a - c) > eps) return false; break;
+                case KB_CMP_NE: if (fabs(a - c) <= eps) return false; break;
+                default: break;
+            }
+        }
+    }
+    return true;
+}
+
+template <bool GATED>
+static __global__ void __launch_bounds__(256) derive_kernel(const __grid_constant__ DeriveParams P) {
+    const int lane = threadIdx.x & 31;
+    const u32 stride = gridDim.x * blockDim.x;
+    const u32 n_round = (P.n + 31u) & ~31u;
+    unsigned long long nd = 0;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += stride) {
+        bool pass = i < P.n && rule_filters_pass(P, i);
+        bool fresh = false;
+        u32 s = 0, o = 0;
+        if (pass) nd++;
+        if (pass && *reinterpret_cast<volatile u32*>(P.out_count) >= P.budget) {  // the set must grow first; this launch is run again
+            *P.overflow = 2u;
+            pass = false;
+        }
+        if (pass) {
+            s = P.head_s.is_var ? P.bcol[P.head_s.value][i] : P.head_s.value;
+            o = P.head_o.is_var ? P.bcol[P.head_o.value][i] : P.head_o.value;
+            if (GATED && !derive_gate_pass(P, s, o)) pass = false;
+        }
+        if (pass) {
+            const u32 r = set64_insert(P.set, P.set_slots, s, o);
+            if (r == 2u) atomicMax(P.overflow, 1u);
+            fresh = r == 1u;
+        }
+        const unsigned b = __ballot_sync(0xffffffffu, fresh);  // warp-aggregated append of the facts that were new
+        if (b) {
+            u32 basepos = 0;
+            if (lane == __ffs(b) - 1) basepos = atomicAdd(P.out_count, (u32)__popc(b));
+            basepos = __shfl_sync(0xffffffffu, basepos, __ffs(b) - 1);
+            if (fresh) {
+                const u32 r = basepos + (u32)__popc(b & ((1u << lane) - 1u));
+                if (r < P.out_cap) { P.out_s[r] = s; P.out_o[r] = o; }
+                else *P.overflow = 1u;
+            }
+        }
+    }
+    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 16);
+    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 8);
+    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 4);
+    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 2);
+    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 1);
+    if (lane == 0 && nd) atomicAdd(P.n_deriv, nd);
+}
+// ---- radix-partitioned variant
+constexpr int DPART_THREADS = 256;
+constexpr int DPART_ITEMS = 16;
+constexpr int DPART_TILE = DPART_THREADS * DPART_ITEMS;  // 4096 candidates: 32 KB of keys + 8 KB of partition ids in shared memory
+constexpr int DPART_MAXP = 1024;
+static __device__ __forceinline__ u32 set64_home(u32 n_slots, u32 s, u32 o) { return mix32(mix32(s) * 0x9E3779B1u ^ mix32(o + 0x632BE5ABu)) & (n_slots - 1u); }
+
+// insert + append of ONE candidate outside any warp-cooperative section (bucket overflow path of the partition pass)
+static __device__ __noinline__ void derive_one(const DeriveParams& P, u32 s, u32 o) {
+    if (*reinterpret_cast<volatile u32*>(P.out_count) >= P.budget) { *P.overflow = 2u; return; }
+    const u32 r = set64_insert(P.set, P.set_slots, s, o);
+    if (r == 2u) *P.overflow = 2u;
+    if (r == 1u) {
+        const u32 at = atomicAdd(P.out_count, 1u);
+        if (at < P.out_cap) { P.out_s[at] = s; P.out_o[at] = o; }
+        else *P.overflow = 1u;
+    }
+}
+
+static __global__ void __launch_bounds__(DPART_THREADS) derive_partition_kernel(const __grid_constant__ DerivePartParams Q) {
+    extern __shared__ __align__(128) u64 sh_keys[];  // [DPART_TILE] keys sorted by partition, then u16 partition ids
+    __shared__ u32 s_cnt[DPART_MAXP], s_off[DPART_MAXP], s_gbase[DPART_MAXP];
+    __shared__ u32 s_tile;
+    const DeriveParams& P = Q.d;
+    unsigned short* s_dest = reinterpret_cast<unsigned short*>(sh_keys + DPART_TILE);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const u32 n_tiles = (P.n + DPART_TILE - 1u) / DPART_TILE;
+    unsigned long long nd = 0;
+    for (;;) {
+        if (tid == 0) s_tile = atomicAdd(&Q.tickets[0], 1u);
+        for (u32 d = (u32)tid; d < Q.n_parts; d += DPART_THREADS) s_cnt[d] = 0u;
+        __syncthreads();
+        const u32 tile = s_tile;
+        if (tile >= n_tiles) break;
+        const u32 row0 = tile * (u32)DPART_TILE;
+        const u32 cnt = min((u32)DPART_TILE, P.n - row0);
+        // ---- 1. head instantiation + rule filters; partition = high bits of the key's home slot; histogram
+        u64 key[DPART_ITEMS];
+        u32 part[DPART_ITEMS], rank[DPART_ITEMS];
+#pragma unroll
+        for (int j = 0; j < DPART_ITEMS; j++) {
+            const u32 r = (u32)j * DPART_THREADS + (u32)tid;
+            const u32 i = row0 + r;
+            bool pass = r < cnt && rule_filters_pass(P, i);
+            u32 s = 0, o = 0;
+            if (pass) {
+                nd++;
+                s = P.head_s.is_var ? __ldg(P.bcol[P.head_s.value] + i) : P.head_s.value;
+                o = P.head_o.is_var ? __ldg(P.bcol[P.head_o.value] + i) : P.head_o.value;
+                if (P.demand && !bc_demanded(P.demand, P.n_demand, s, o)) pass = false;
+            }
+            key[j] = ((u64)s << 32) | (u64)o;
+            part[j] = pass ? (set64_home(P.set_slots, s, o) >> Q.slice_bits) : 0xFFFFu;
+            rank[j] = pass ? atomicAdd(&s_cnt[part[j]], 1u) : 0u;  // the key's place among the tile's keys of its partition (kept for step 3)
+        }
+        __syncthreads();
+        // ---- 2. offsets inside the tile (one warp scans the histogram), one range reservation per partition
+        if (warp == 0) {
+            u32 run = 0;
+            for (u32 d0 = 0; d0 < Q.n_parts; d0 += 32u) {
+                const u32 d = d0 + (u32)lane;
+                const u32 c = d < Q.n_parts ? s_cnt[d] : 0u;
+                u32 incl = c;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) {
+                    const u32 y = __shfl_up_sync(0xffffffffu, incl, o);
+                    if (lane >= o) incl += y;
+                }
+                if (d < Q.n_parts) {
+                    s_off[d] = run + incl - c;
+                    s_gbase[d] = c ? atomicAdd(&Q.cursors[d], c) : 0u;
+                }
+                run += __shfl_sync(0xffffffffu, incl, 31);
+            }
+        }
+        __syncthreads();
+        // ---- 3. keys staged in partition order
+#pragma unroll
+        for (int j = 0; j < DPART_ITEMS; j++) {
+            if (part[j] == 0xFFFFu) continue;
+            const u32 pos = s_off[part[j]] + rank[j];
+            sh_keys[pos] = key[j];
+            s_dest[pos] = (unsigned short)part[j];
+        }
+        __syncthreads();
+        // ---- 4. flush: staged position q belongs to partition s_dest[q]; consecutive q of one partition are consecutive in its bucket
+        const u32 staged = s_off[Q.n_parts - 1u] + s_cnt[Q.n_parts - 1u];
+        for (u32 q = (u32)tid; q < staged; q += DPART_THREADS) {
+            const u32 d = s_dest[q];
+            const u32 at = s_gbase[d] + (q - s_off[d]);
+            const u64 k = sh_keys[q];
+            if (at < Q.bucket_cap) Q.buckets[(u64)d * Q.bucket_cap + at] = k;
+            else derive_one(P, (u32)(k >> 32), (u32)k);  // the bucket is full (skewed hash): probe directly
+        }
+        __syncthreads();
+    }
+    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 16);
+    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 8);
+    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 4);
+    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 2);
+    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 1);
+    if (lane == 0 && nd) atomicAdd(P.n_deriv, nd);
+}
+
+constexpr int DPROBE_TILE = 2048;
+static __global__ void __launch_bounds__(1024) derive_tile_starts_kernel(const __grid_constant__ DerivePartParams Q) {
+    __shared__ u32 s_tiles[DPART_MAXP];
+    const int tid = threadIdx.x;
+    if ((u32)tid < Q.n_parts) s_tiles[tid] = (min(Q.cursors[tid], Q.bucket_cap) + DPROBE_TILE - 1u) / DPROBE_TILE;
+    __syncthreads();
+    if (tid == 0) {
+        u32 run = 0;
+        for (u32 d = 0; d < Q.n_parts; d++) { Q.tile_start[d] = run; run += s_tiles[d]; }
+        Q.tile_start[Q.n_parts] = run;
+    }
+}
+
+static __global__ void __launch_bounds__(256) derive_probe_kernel(const __grid_constant__ DerivePartParams Q) {
+    __shared__ u32 s_tile, s_base;
+    __shared__ u32 s_wcnt[8];
+    const DeriveParams& P = Q.d;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const u32 n_tiles = Q.tile_start[Q.n_parts];
+    constexpr int R = DPROBE_TILE / 256;
+    for (;;) {
+        __syncthreads();
+        if (tid == 0) s_tile = atomicAdd(&Q.tickets[1], 1u);  // tickets are handed out in partition order: the CTAs walk the slices together
+        __syncthreads();
+        const u32 tile = s_tile;
+        if (tile >= n_tiles) break;
+        u32 lo = 0, hi = Q.n_parts;  // partition of this tile: last d with tile_start[d] <= tile
+        while (hi - lo > 1u) {
+            const u32 mid = (lo + hi) >> 1;
+            if (Q.tile_start[mid] <= tile) lo = mid; else hi = mid;
+        }
+        const u32 d = lo;
+        const u32 n_keys = min(Q.cursors[d], Q.bucket_cap);
+        const u32 first = (tile - Q.tile_start[d]) * (u32)DPROBE_TILE;
+        const u64* keys = Q.buckets + (u64)d * Q.bucket_cap;
+        // the set must not fill past its budget: checked once per tile (a tile adds at most DPROBE_TILE facts: the budget leaves that room)
+        const bool room = *reinterpret_cast<volatile u32*>(P.out_count) < P.budget;
+        if (!room && tid == 0) *P.overflow = 2u;
+        u64 k[R];
+        u32 fresh = 0;
+#pragma unroll
+        for (int j = 0; j < R; j++) {
+            const u32 q = first + (u32)j * 256u + (u32)tid;
+            k[j] = (room && q < n_keys) ? __ldg(keys + q) : EMPTY64;
+        }
+#pragma unroll
+        for (int j = 0; j < R; j++) {
+            if (k[j] == EMPTY64) continue;  // (s = o = 0xFFFFFFFF is the reserved id: never a fact)
+            const u32 r = set64_insert(P.set, P.set_slots, (u32)(k[j] >> 32), (u32)k[j]);
+            if (r == 2u) *P.overflow = 2u;  // table full (the per-tile budget check lets a small table overshoot): grow and run again
+            fresh |= (r == 1u ? 1u : 0u) << j;
+        }
+        // ONE reservation per tile for the facts that were new (a single global cursor serialises: per-warp reservations
+        // dominated the pass on 1.4e8 new facts), then ranked writes
+        const u32 c = (u32)__popc(fresh);
+        u32 incl = c;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const u32 y = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += y;
+        }
+        if (lane == 31) s_wcnt[warp] = incl;
+        __syncthreads();
+        if (tid == 0) {
+            u32 run = 0;
+#pragma unroll
+            for (int w = 0; w < 8; w++) { const u32 x = s_wcnt[w]; s_wcnt[w] = run; run += x; }
+            s_base = run ? atomicAdd(P.out_count, run) : 0u;
+        }
+        __syncthreads();
+        u32 pos = s_base + s_wcnt[warp] + incl - c;
+#pragma unroll
+        for (int j = 0; j < R; j++) {
+            if ((fresh >> j) & 1u) {
+                if (pos < P.out_cap) { P.out_s[pos] = (u32)(k[j] >> 32); P.out_o[pos] = (u32)k[j]; }
+                else *P.overflow = 1u;
+                pos++;
+            }
+        }
+    }
+}
+
+static void launch_derive_partitioned(const DerivePartParams& p, int n_sms, cudaStream_t st) {
+    if (p.d.n == 0) return;
+    const size_t smem = (size_t)DPART_TILE * (sizeof(u64) + sizeof(unsigned short));
+    static bool attr = false;
+    if (!attr) { cudaFuncSetAttribute(derive_partition_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); attr = true; }
+    const u32 n_tiles = (p.d.n + DPART_TILE - 1u) / DPART_TILE;
+    const int grid1 = grid_for((const void*)derive_partition_kernel, DPART_THREADS, smem, n_sms, n_tiles);
+    static const bool trace = getenv("KOLIBRIE_TRACE") != nullptr;
+    cudaEvent_t e0 = nullptr, e1 = nullptr, e2 = nullptr;
+    if (trace) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventCreate(&e2); cudaEventRecord(e0, st); }
+    derive_partition_kernel<<<grid1, DPART_THREADS, smem, st>>>(p);
+    if (trace) cudaEventRecord(e1, st);
+    derive_tile_starts_kernel<<<1, 1024, 0, st>>>(p);
+    const int grid2 = grid_for((const void*)derive_probe_kernel, 256, 0, n_sms, (p.d.n + DPROBE_TILE - 1u) / DPROBE_TILE + p.n_parts);
+    derive_probe_kernel<<<grid2, 256, 0, st>>>(p);
+    if (trace) {
+        cudaEventRecord(e2, st);
+        cudaEventSynchronize(e2);
+        float a = 0.f, b = 0.f;
+        cudaEventElapsedTime(&a, e0, e1);
+        cudaEventElapsedTime(&b, e1, e2);
+        fprintf(stderr, "[kb trace]     derive partitioned: %u candidates, %u partitions: partition pass %.3f ms, probe pass %.3f ms\n", p.d.n, p.n_parts, a, b);
+        cudaEventDestroy(e0); cudaEventDestroy(e1); cudaEventDestroy(e2);
+    }
+}
+
+static void launch_derive(const DeriveParams& p, int n_sms, cudaStream_t st) {
+    if (p.n == 0) return;
+    int grid = (int)umin64((u64)n_sms * 8ull, ((u64)p.n + 255ull) / 256ull);
+    if (p.gate_set || p.veto_keys || p.demand) derive_kernel<true><<<grid, 256, 0, st>>>(p);
+    else derive_kernel<false><<<grid, 256, 0, st>>>(p);
+}
+
+// *found = 1 when (s,o) is a member of the 64-bit set (a one-thread probe: kb_datalog_query's ground query)
+static __global__ void bc_probe_kernel(const u64* set, u32 set_slots, u32 s, u32 o, u32* found) {
+    *found = set64_find(set, set_slots, s, o) != EMPTY32 ? 1u : 0u;
+}
+static void launch_bc_probe(const u64* set, u32 set_slots, u32 s, u32 o, u32* found, cudaStream_t st) {
+    bc_probe_kernel<<<1, 1, 0, st>>>(set, set_slots, s, o, found);
+}
+
+// ---- kb_datalog_maintain: base multiplicities, selection by set membership, erasure
+// An erased key of a 64-bit (s,o) set: lookups walk past it, inserts never reuse it (s = KB_ID_NONE is never a fact). The set is rebuilt
+// from its relation when it fills up, which drops the tombstones.
+constexpr u64 TOMB64 = 0xFFFFFFFFFFFFFFFEull;
+// base multiplicity of a predicate's facts: a 64-bit (s,o) key table and a parallel u32 count per slot (a key whose count is 0 is not a
+// base fact; it keeps its slot until the table is rehashed)
+struct BaseCountParams {
+    u64* keys;
+    u32* cnt;
+    u32 slots;  // power of two
+    const u32 *s, *o;
+    u32 n;
+    int delta;  // +1: the rows join the base (a count that leaves 0 emits the fact), -1: they leave it (a count that reaches 0 emits it)
+    u32 *out_s, *out_o;  // nullable: no emission (the facts that crossed zero are then only counted)
+    u32* out_count;      // facts that crossed zero
+    u32* claimed;        // keys that took a free slot of the table
+    u32* overflow;       // 1: key table full
+};
+static __global__ void __launch_bounds__(256) base_count_kernel(const __grid_constant__ BaseCountParams P) {
+    const u32 stride = gridDim.x * blockDim.x;
+    const u32 n_round = (P.n + 31u) & ~31u;
+    u32 n_edges = 0, n_claimed = 0;  // (counted here when nothing is emitted)
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += stride) {
+        bool edge = false;  // this row moved the count across zero
+        u32 s = 0, o = 0;
+        if (i < P.n) {
+            s = P.s[i];
+            o = P.o[i];
+            if (P.delta > 0) {
+                bool claimed = false;
+                const u32 slot = set64_insert_slot(P.keys, P.slots, s, o, &claimed);
+                if (slot == EMPTY32) *P.overflow = 1u;
+                else edge = atomicAdd(&P.cnt[slot], 1u) == 0u;
+                n_claimed += claimed ? 1u : 0u;
+            } else {
+                const u32 slot = set64_find(P.keys, P.slots, s, o);
+                if (slot != EMPTY32) edge = atomicSub(&P.cnt[slot], 1u) == 1u;
+            }
+        }
+        if (P.out_s) emit_pair(edge, s, o, P.out_s, P.out_o, P.out_count);
+        else n_edges += edge ? 1u : 0u;
+    }
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+        n_edges += __shfl_xor_sync(0xffffffffu, n_edges, d);
+        n_claimed += __shfl_xor_sync(0xffffffffu, n_claimed, d);
+    }
+    if ((threadIdx.x & 31) == 0) {
+        if (n_edges) atomicAdd(P.out_count, n_edges);
+        if (n_claimed) atomicAdd(P.claimed, n_claimed);
+    }
+}
+static void launch_base_count(const BaseCountParams& p, int n_sms, cudaStream_t st) {
+    if (p.n == 0) return;
+    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)p.n + 255ull) / 256ull);
+    base_count_kernel<<<grid, 256, 0, st>>>(p);
+}
+
+// live entries (count > 0) of one count table into an empty larger one; *n_live += entries moved
+static __global__ void __launch_bounds__(256) base_count_rehash_kernel(const u64* okeys, const u32* ocnt, u32 oslots, u64* nkeys, u32* ncnt, u32 nslots,
+                                                                u32* n_live, u32* overflow) {
+    const u32 stride = gridDim.x * blockDim.x;
+    u32 moved = 0;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < oslots; i += stride) {
+        const u64 k = okeys[i];
+        const u32 c = ocnt[i];
+        if (k == EMPTY64 || c == 0u) continue;
+        bool claimed = false;
+        const u32 slot = set64_insert_slot(nkeys, nslots, (u32)(k >> 32), (u32)k, &claimed);
+        if (slot == EMPTY32) { *overflow = 1u; continue; }
+        ncnt[slot] = c;  // keys are distinct: one writer per slot
+        moved++;
+    }
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) moved += __shfl_xor_sync(0xffffffffu, moved, d);
+    if ((threadIdx.x & 31) == 0 && moved) atomicAdd(n_live, moved);
+}
+static void launch_base_count_rehash(const u64* okeys, const u32* ocnt, u32 oslots, u64* nkeys, u32* ncnt, u32 nslots, u32* n_live, u32* overflow, int n_sms,
+                              cudaStream_t st) {
+    if (oslots == 0) return;
+    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)oslots + 255ull) / 256ull);
+    base_count_rehash_kernel<<<grid, 256, 0, st>>>(okeys, ocnt, oslots, nkeys, ncnt, nslots, n_live, overflow);
+}
+
+// rows (s,o) whose presence in a 64-bit set equals keep_present go to out (warp-aggregated compaction, order not kept). With `cnt` the
+// set is a count table and a key is present only with a positive count.
+struct PairSelectParams {
+    const u32 *s, *o;
+    u32 n;
+    const u64* keys;
+    const u32* cnt;
+    u32 slots;
+    u32 keep_present;
+    u32 *out_s, *out_o;
+    u32* out_count;
+};
+static __global__ void __launch_bounds__(256) pair_select_kernel(const __grid_constant__ PairSelectParams P) {
+    const u32 stride = gridDim.x * blockDim.x;
+    const u32 n_round = (P.n + 31u) & ~31u;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += stride) {
+        bool take = false;
+        u32 s = 0, o = 0;
+        if (i < P.n) {
+            s = P.s[i];
+            o = P.o[i];
+            const u32 slot = set64_find(P.keys, P.slots, s, o);
+            const bool present = slot != EMPTY32 && (!P.cnt || P.cnt[slot] > 0u);
+            take = present == (P.keep_present != 0u);
+        }
+        emit_pair(take, s, o, P.out_s, P.out_o, P.out_count);
+    }
+}
+static void launch_pair_select(const PairSelectParams& p, int n_sms, cudaStream_t st) {
+    if (p.n == 0) return;
+    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)p.n + 255ull) / 256ull);
+    pair_select_kernel<<<grid, 256, 0, st>>>(p);
+}
+
+// the keys (s,o) of the rows become TOMB64 in the set (keys that are not there are ignored)
+static __global__ void __launch_bounds__(256) set64_erase_kernel(u64* set, u32 set_slots, const u32* s, const u32* o, u32 n) {
+    const u32 stride = gridDim.x * blockDim.x;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        const u32 slot = set64_find(set, set_slots, s[i], o[i]);
+        if (slot != EMPTY32) set[slot] = TOMB64;
+    }
+}
+static void launch_set64_erase(u64* set, u32 set_slots, const u32* s, const u32* o, u32 n, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull);
+    set64_erase_kernel<<<grid, 256, 0, st>>>(set, set_slots, s, o, n);
+}
+
+}  // namespace kb
+
+// =====================================================================================================================================
+// Host side: the driver
 namespace {
 
 struct PredRel {
@@ -48,6 +578,12 @@ struct Premise {
 struct RulePlan {
     std::vector<Premise> prem;
     u32 n_vars = 0;
+    bool fires = false;  // it has premises and every premise predicate is a constant (a variable one never matches: join_algorithm.rs:515-521)
+};
+
+struct Pairs {  // a list of (s,o) facts of one predicate
+    Col s, o;
+    u64 n = 0;
 };
 
 struct Pending {  // facts derived in the current round, not yet visible to the joins
@@ -296,6 +832,7 @@ kb_status compile_rules(kb_ctx* ctx, const kb_rule* rules, u32 n_rules, std::vec
             plans[r].prem.push_back(pr);
         }
         plans[r].n_vars = next;
+        plans[r].fires = rule.n_premise > 0 && std::all_of(plans[r].prem.begin(), plans[r].prem.end(), [](const Premise& p) { return p.pred_const; });
         if (next > KB_MAX_COLS) return fail(ctx, KB_E_LIMIT, "rule %u uses more than %d variables", r, KB_MAX_COLS);
         for (u32 c = 0; c < rule.n_conclusion; c++) {
             const kb_pattern& h = rule.conclusion[c];
@@ -473,53 +1010,157 @@ kb_status flush_pending(Fix& fx, u64* appended) {
     return KB_OK;
 }
 
-// the store split by predicate: every relation of fx.rels gets its predicate's facts (one fused scan per 8 predicates). demand
+kb_status check_strategy(kb_ctx* ctx, u32 strategy) {
+    if (strategy != KB_SEMI_NAIVE && strategy != KB_NAIVE && strategy != KB_SEMI_NAIVE_PARALLEL && strategy != KB_SEMI_NAIVE_OLD_DELTA)
+        return fail(ctx, KB_E_INVALID, "unknown strategy %u", strategy);
+    return KB_OK;
+}
+
+// the rows of an (s,p,o) relation (slots 0,1,2) whose predicate is p
+kb_status rows_of_predicate(kb_ctx* ctx, const kb_rel& spo, u32 p, std::unique_ptr<kb_rel>* out) {
+    FilterProg f;
+    kb_filter_op op{};
+    op.op = KB_F_EQ_ID; op.slot = 1; op.id = p;
+    f.ops.push_back(op);
+    return filter_impl(ctx, spo, f, out);
+}
+
+// seed facts take the way of rule-less derived heads: the ones the known facts lack become visible now as the first delta, all else is
+// old. The seeds: `seeds` (predicate, relation with s and o in slots 0 and 2), then the rows of `spo` (nullable; slots 0,1,2 = s,p,o)
+// of each predicate of fx.rels, split off one predicate at a time so that only one predicate's rows are held at once. *accepted = the
+// facts that were new (seed facts are no derivations).
+kb_status accept_seeds(Fix& fx, const std::vector<std::pair<u32, const kb_rel*>>& seeds, const kb_rel* spo, Trace& tr, u64* accepted) {
+    for (auto& kv : fx.rels) kv.second.snapshot = kv.second.seed_from = kv.second.n;
+    u64 derivations = 0;
+    auto seed = [&](u32 p, const kb_rel* rel) -> kb_status {
+        if (rel->n == 0) return KB_OK;
+        kb_pattern h{};
+        h.s = kb_term{1, 0}; h.p = kb_term{0, p}; h.o = kb_term{1, 2};
+        return derive_head(fx, rel, h, nullptr, false, nullptr, tr, &derivations);
+    };
+    for (auto& sd : seeds) KB_TRY(seed(sd.first, sd.second));
+    if (spo && spo->n)
+        for (auto& kv : fx.rels) {
+            std::unique_ptr<kb_rel> sub;
+            KB_TRY(rows_of_predicate(fx.ctx, *spo, kv.first, &sub));
+            KB_TRY(seed(kv.first, sub.get()));
+        }
+    for (auto& kv : fx.rels) kv.second.delta_start = kv.second.snapshot;
+    KB_TRY(flush_pending(fx, accepted));
+    for (auto& kv : fx.rels) kv.second.base_n = kv.second.n;
+    return KB_OK;
+}
+
+// joins premise `pr` over rows [0, visible) of its relation into the bindings `cur` (null: they become the premise's rows); strict:
+// the premise's constants are enforced
+kb_status join_premise(kb_ctx* ctx, std::unique_ptr<kb_rel>& cur, const Premise& pr, const PredRel& r, u64 visible, bool strict, Trace& tr) {
+    if (cur && visible == 0) { cur->n = 0; return KB_OK; }
+    std::unique_ptr<kb_rel> all, joined;
+    KB_TRY(make_view(ctx, r, 0, visible, (u32)pr.s_var, (u32)pr.o_var, &all));
+    if (strict) KB_TRY(enforce_constants(ctx, pr, &all));
+    if (!cur) { cur = std::move(all); return KB_OK; }
+    tr.mark(ctx, "  views");
+    KB_TRY(hash_join_impl(ctx, *cur, *all, nullptr, &joined));
+    cur = std::move(joined);
+    tr.mark(ctx, "  join", cur->n);
+    return KB_OK;
+}
+
+// rows [from, to) of a predicate relation
+Pairs rows_of(const PredRel& r, u64 from, u64 to) {
+    Pairs p;
+    p.s = Col{r.s.buf, r.s.ptr + from};
+    p.o = Col{r.o.buf, r.o.ptr + from};
+    p.n = to - from;
+    return p;
+}
+
+// (s,p,o) relation of per-predicate fact lists
+kb_status assemble(kb_ctx* ctx, const std::vector<std::pair<u32, Pairs>>& parts, std::unique_ptr<kb_rel>* out) {
+    u64 total = 0;
+    for (auto& pp : parts) total += pp.second.n;
+    if (total >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "result exceeds 2^32 - 16 rows");
+    auto res = std::make_unique<kb_rel>();
+    res->slots = {0, 1, 2};
+    res->n = total;
+    Col cs, cp, co;
+    KB_TRY(alloc_col(ctx, total, &cs));
+    KB_TRY(alloc_col(ctx, total, &cp));
+    KB_TRY(alloc_col(ctx, total, &co));
+    u64 off = 0;
+    for (auto& pp : parts) {
+        const u64 cnt = pp.second.n;
+        if (!cnt) continue;
+        KB_CUDA(ctx, cudaMemcpyAsync(cs.ptr + off, pp.second.s.ptr, cnt * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
+        KB_CUDA(ctx, cudaMemcpyAsync(co.ptr + off, pp.second.o.ptr, cnt * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
+        launch_fill_u32(cp.ptr + off, pp.first, cnt, ctx->st);
+        off += cnt;
+    }
+    res->cols = {cs, cp, co};
+    *out = std::move(res);
+    return KB_OK;
+}
+
+// the rows of the segments `segs` split by predicate: out[p] = (s, o) of every predicate of `preds` (one fused scan per MAXP predicates;
+// none when the segments hold no row)
+kb_status split_segments(kb_ctx* ctx, const std::vector<Segment>& segs, const std::vector<u32>& preds, std::map<u32, Pairs>* out) {
+    u64 n = 0;
+    for (auto& sg : segs) n += sg.n;
+    for (u32 p : preds) (*out)[p] = Pairs{};
+    if (n == 0 || preds.empty()) return KB_OK;
+    for (size_t b = 0; b < preds.size(); b += MAXP) {
+        const u32 k = (u32)std::min<size_t>(MAXP, preds.size() - b);
+        std::vector<std::unique_ptr<kb_rel>> res;
+        KB_TRY(scan_predicates(ctx, segs, preds.data() + b, k, ScanOut::Cols, &res));
+        for (u32 i = 0; i < k; i++) {
+            Pairs& p = (*out)[preds[b + i]];
+            p.s = res[i]->cols[0];
+            p.o = res[i]->cols[1];
+            p.n = res[i]->n;
+        }
+    }
+    return KB_OK;
+}
+
+// the store split by predicate: every relation of fx.rels gets its predicate's facts, MAXP predicates at a time. demand
 // (kb_datalog_query): a restricted predicate keeps only the facts that match one of its demand patterns.
 kb_status split_store(Fix& fx) {
     kb_ctx* ctx = fx.ctx;
     std::vector<u32> preds;
     for (auto& kv : fx.rels) preds.push_back(kv.first);
     for (size_t b = 0; b < preds.size(); b += MAXP) {
-        const u32 k = (u32)std::min<size_t>(MAXP, preds.size() - b);
-        std::vector<std::unique_ptr<kb_rel>> out;
+        const std::vector<u32> batch(preds.begin() + b, preds.begin() + std::min<size_t>(b + MAXP, preds.size()));
+        std::map<u32, Pairs> split;
         // the predicate relations are append-only buffers with the capacity of a whole-store scan output: take the scan, not the
         // (exactly sized) index slices
-        KB_TRY(scan_predicates(ctx, ctx->segs, preds.data() + b, k, ScanOut::Cols, &out));
+        KB_TRY(split_segments(ctx, ctx->segs, batch, &split));
         // a restricted predicate's rows are selected into new columns of the scanned row count, which is then their capacity; the
         // selections of a batch are read back together
-        std::vector<int> selected(k, -1);
-        for (u32 i = 0; i < k; i++) {
-            PredRel& r = fx.rels[preds[b + i]];
-            r.s = out[i]->cols[0];
-            r.o = out[i]->cols[1];
-            r.n = out[i]->n;
+        std::map<u32, u32> selected;  // predicate -> control word of its selected row count
+        for (u32 p : batch) {
+            PredRel& r = fx.rels[p];
+            r.s = split[p].s;
+            r.o = split[p].o;
+            r.n = split[p].n;
             r.cap = ctx->n_triples;
             if (!fx.demand) continue;
-            auto it = fx.demand->of.find(r.pred);
+            auto it = fx.demand->of.find(p);
             if (it == fx.demand->of.end()) continue;
-            selected[i] = (int)ctrl_alloc(ctx, 1);
+            selected[p] = ctrl_alloc(ctx, 1);
             Col ns, no;
-            KB_TRY(bc_demand_select(ctx, it->second.first, it->second.second, r.s, r.o, r.n, &ns, &no, (u32)selected[i]));
+            KB_TRY(bc_demand_select(ctx, it->second.first, it->second.second, r.s, r.o, r.n, &ns, &no, selected[p]));
             r.s = ns;
             r.o = no;
             r.cap = r.n;
         }
-        if (std::any_of(selected.begin(), selected.end(), [](int w) { return w >= 0; })) KB_TRY(ctrl_read(ctx));
-        for (u32 i = 0; i < k; i++) {
-            PredRel& r = fx.rels[preds[b + i]];
-            if (selected[i] >= 0) r.n = ctx->h_ctrl[selected[i]];
+        if (!selected.empty()) KB_TRY(ctrl_read(ctx));
+        for (u32 p : batch) {
+            PredRel& r = fx.rels[p];
+            if (selected.count(p)) r.n = ctx->h_ctrl[selected[p]];
             r.base_n = r.n;
-            if (r.n * 4 < r.cap) {  // shrink: the scan allocates for the worst case
+            if (r.n * 4 < r.cap) {  // shrink: the scan allocates for the worst case (grow_rel from no capacity copies the rows over)
                 r.cap = 0;
-                Col os = r.s, oo = r.o;
-                u64 n = r.n;
-                r.n = 0;
-                KB_TRY(grow_rel(ctx, r, std::max<u64>(n * 2, 1024)));
-                if (n) {
-                    KB_CUDA(ctx, cudaMemcpyAsync(r.s.ptr, os.ptr, n * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
-                    KB_CUDA(ctx, cudaMemcpyAsync(r.o.ptr, oo.ptr, n * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
-                }
-                r.n = n;
+                KB_TRY(grow_rel(ctx, r, std::max<u64>(r.n * 2, 1024)));
             }
         }
     }
@@ -552,10 +1193,7 @@ kb_status run_rounds(Fix& fx, const kb_rule* rules, u32 n_rules, const std::vect
             const kb_rule& rule = rules[r];
             const RulePlan& pl = plans[r];
             const u32 np = (u32)pl.prem.size();
-            if (np == 0) continue;
-            bool dead = false;
-            for (auto& pr : pl.prem) if (!pr.pred_const) dead = true;  // a variable predicate never matches (join_algorithm.rs:515-521)
-            if (dead) continue;
+            if (!pl.fires) continue;
             if (strategy == KB_SEMI_NAIVE_PARALLEL && np != 1 && np != 2) continue;  // semi_naive_parallel.rs:149: other arities are skipped
             const u32 n_start = strategy == KB_NAIVE ? 1 : np;
             for (u32 i = 0; i < n_start; i++) {
@@ -573,15 +1211,7 @@ kb_status run_rounds(Fix& fx, const kb_rule* rules, u32 n_rules, const std::vect
                     if (j == i) continue;
                     const PredRel& pr = fx.rels[pl.prem[j].pred];
                     // KB_SEMI_NAIVE_OLD_DELTA: a premise before the delta premise sees only the facts older than its delta
-                    const u64 visible = old_delta && j < i ? pr.delta_start : pr.snapshot;
-                    if (visible == 0) { cur->n = 0; break; }
-                    std::unique_ptr<kb_rel> all, joined;
-                    KB_TRY(make_view(ctx, pr, 0, visible, (u32)pl.prem[j].s_var, (u32)pl.prem[j].o_var, &all));
-                    if (strict) KB_TRY(enforce_constants(ctx, pl.prem[j], &all));
-                    tr.mark(ctx, "  views");
-                    KB_TRY(hash_join_impl(ctx, *cur, *all, nullptr, &joined));
-                    cur = std::move(joined);
-                    tr.mark(ctx, "  join", cur->n);
+                    KB_TRY(join_premise(ctx, cur, pl.prem[j], pr, old_delta && j < i ? pr.delta_start : pr.snapshot, strict, tr));
                 }
                 if (cur->n == 0) continue;
                 // heads: filters + instantiate + dedup against known facts + append
@@ -622,8 +1252,7 @@ static kb_status fixpoint_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
                                kb_rel** inferred, uint64_t* n_seed_new, kb_fixpoint_stats* stats) {
     KB_ENTER(ctx);
     if ((n_rules && !rules) || !inferred) return fail(ctx, KB_E_INVALID, "NULL argument");
-    if (strategy != KB_SEMI_NAIVE && strategy != KB_NAIVE && strategy != KB_SEMI_NAIVE_PARALLEL && strategy != KB_SEMI_NAIVE_OLD_DELTA)
-        return fail(ctx, KB_E_INVALID, "unknown strategy %u", strategy);
+    KB_TRY(check_strategy(ctx, strategy));
     if (seeded && !seed) return fail(ctx, KB_E_INVALID, "NULL seed");
     if (seed && (seed->pair || seed->cols.size() != 3 || seed->col_of(0) != 0 || seed->col_of(1) != 1 || seed->col_of(2) != 2))
         return fail(ctx, KB_E_INVALID, "the seed must be a 3-column relation with slots 0,1,2 = s,p,o");
@@ -674,65 +1303,31 @@ static kb_status fixpoint_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
     }
     tr.mark(ctx, "initial known-fact sets");
 
-    // ---- seed: its facts take the way of derived heads (dedup against the known facts); the winners become visible now and are the
-    // first delta, everything the store held is OLD
+    // ---- seed: the facts the store does not hold yet
     u64 seed_new = 0;
     if (seed) {
-        for (auto& kv : fx.rels) kv.second.snapshot = kv.second.seed_from = kv.second.n;
-        for (auto& kv : fx.rels) {
-            if (seed->n == 0) break;
-            FilterProg f;
-            kb_filter_op op{};
-            op.op = KB_F_EQ_ID; op.slot = 1; op.id = kv.first;
-            f.ops.push_back(op);
-            std::unique_ptr<kb_rel> sub;
-            KB_TRY(filter_impl(ctx, *seed, f, &sub));
-            if (sub->n == 0) continue;
-            kb_pattern h{};
-            h.s = kb_term{1, 0}; h.p = kb_term{0, kv.first}; h.o = kb_term{1, 2};
-            KB_TRY(derive_head(fx, sub.get(), h, nullptr, strict, nullptr, tr, &st.derivations));
-        }
-        for (auto& kv : fx.rels) kv.second.delta_start = kv.second.snapshot;
-        KB_TRY(flush_pending(fx, &seed_new));
-        for (auto& kv : fx.rels) kv.second.base_n = kv.second.n;
-        st.derivations = 0;  // (the seed's facts are not derivations)
+        KB_TRY(accept_seeds(fx, {}, seed, tr, &seed_new));
         tr.mark(ctx, "seed accepted", seed_new);
     }
 
     // ---- rounds
     KB_TRY(run_rounds(fx, rules, n_rules, plans, strategy, st, tr));
 
-    // ---- result: inferred facts as (s,p,o) columns; also appended to the store (infer_generic.rs:46 index_manager.insert)
-    auto res = std::make_unique<kb_rel>();
-    res->slots = {0, 1, 2};
-    // (with a seed: the accepted seed facts first, then the inferred ones)
+    // ---- result: inferred facts as (s,p,o) columns; also appended to the store (infer_generic.rs:46 index_manager.insert). With a seed:
+    // the accepted seed facts first, then the inferred ones, predicate by predicate.
     const u64 total = seed_new + st.inferred;
     if (total >= 0xFFFFFFF0ull || ctx->n_triples + total >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "the closure exceeds 2^32 - 16 triples");
-    res->n = total;
-    Col cs, cp, co;
-    KB_TRY(alloc_col(ctx, total, &cs));
-    KB_TRY(alloc_col(ctx, total, &cp));
-    KB_TRY(alloc_col(ctx, total, &co));
-    u64 off = 0;
-    for (int pass = seed ? 0 : 1; pass < 2; pass++) {
-        for (auto& kv : fx.rels) {
-            PredRel& r = kv.second;
-            const u64 from = pass == 0 ? r.seed_from : r.base_n, to = pass == 0 ? r.base_n : r.n;
-            const u64 cnt = to - from;
-            if (!cnt) continue;
-            KB_CUDA(ctx, cudaMemcpyAsync(cs.ptr + off, r.s.ptr + from, cnt * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
-            KB_CUDA(ctx, cudaMemcpyAsync(co.ptr + off, r.o.ptr + from, cnt * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
-            launch_fill_u32(cp.ptr + off, r.pred, cnt, ctx->st);
-            off += cnt;
-        }
-    }
-    res->cols = {cs, cp, co};
+    std::vector<std::pair<u32, Pairs>> parts;
+    if (seed) for (auto& kv : fx.rels) parts.push_back({kv.first, rows_of(kv.second, kv.second.seed_from, kv.second.base_n)});
+    for (auto& kv : fx.rels) parts.push_back({kv.first, rows_of(kv.second, kv.second.base_n, kv.second.n)});
+    std::unique_ptr<kb_rel> res;
+    KB_TRY(assemble(ctx, parts, &res));
     for (auto& kv : fx.rels) if (kv.second.is_head) ctx->fix_hint[kv.first] = kv.second.n;
     if (total) {
         Segment sg;
         sg.tag = KB_TAG_INFERRED;
         sg.n = total;
-        sg.s = cs; sg.p = cp; sg.o = co;
+        sg.s = res->cols[0]; sg.p = res->cols[1]; sg.o = res->cols[2];
         KB_TRY(store_add_device_segment(ctx, sg, /*keep_index=*/false));  // (no statistics pass over the closure)
     }
     tr.mark(ctx, "result assembly", total);
@@ -902,11 +1497,6 @@ extern "C" kb_status kb_datalog_query(kb_ctx* ctx, const kb_rule* rules, uint32_
 // kb_datalog_maintain: delete-and-rederive (DRed) of the inferred segment across a window slide
 namespace {
 
-struct Pairs {  // a list of (s,o) facts of one predicate
-    Col s, o;
-    u64 n = 0;
-};
-
 u64 slots_for(u64 n) {
     u64 s = 1024;
     while (s < 2 * n) s <<= 1;
@@ -1011,54 +1601,6 @@ kb_status select_pairs(kb_ctx* ctx, const u32* s, const u32* o, u64 n, const u64
 }
 const u64* set_of(const PredRel& r) { return r.set ? static_cast<const u64*>(r.set->p) : nullptr; }
 
-// the rows of the store segments `which` selects, split by predicate: out[p] = (s, o) of every predicate of `preds` (one fused scan per 8
-// predicates over those segments only)
-kb_status split_segments(kb_ctx* ctx, const std::vector<u32>& preds, const std::function<bool(const Segment&)>& which, std::map<u32, Pairs>* out) {
-    std::vector<Segment> part;
-    u64 n = 0;
-    for (auto& sg : ctx->segs) if (which(sg)) { part.push_back(sg); n += sg.n; }
-    for (u32 p : preds) (*out)[p] = Pairs{};
-    if (n == 0 || preds.empty()) return KB_OK;
-    for (size_t b = 0; b < preds.size(); b += MAXP) {
-        const u32 k = (u32)std::min<size_t>(MAXP, preds.size() - b);
-        std::vector<std::unique_ptr<kb_rel>> res;
-        KB_TRY(scan_predicates(ctx, part, preds.data() + b, k, ScanOut::Cols, &res));
-        for (u32 i = 0; i < k; i++) {
-            Pairs& p = (*out)[preds[b + i]];
-            p.s = res[i]->cols[0];
-            p.o = res[i]->cols[1];
-            p.n = res[i]->n;
-        }
-    }
-    return KB_OK;
-}
-
-// (s,p,o) relation of per-predicate fact lists
-kb_status assemble(kb_ctx* ctx, const std::vector<std::pair<u32, Pairs>>& parts, std::unique_ptr<kb_rel>* out) {
-    u64 total = 0;
-    for (auto& pp : parts) total += pp.second.n;
-    if (total >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "result exceeds 2^32 - 16 rows");
-    auto res = std::make_unique<kb_rel>();
-    res->slots = {0, 1, 2};
-    res->n = total;
-    Col cs, cp, co;
-    KB_TRY(alloc_col(ctx, total, &cs));
-    KB_TRY(alloc_col(ctx, total, &cp));
-    KB_TRY(alloc_col(ctx, total, &co));
-    u64 off = 0;
-    for (auto& pp : parts) {
-        const u64 cnt = pp.second.n;
-        if (!cnt) continue;
-        KB_CUDA(ctx, cudaMemcpyAsync(cs.ptr + off, pp.second.s.ptr, cnt * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
-        KB_CUDA(ctx, cudaMemcpyAsync(co.ptr + off, pp.second.o.ptr, cnt * sizeof(u32), cudaMemcpyDeviceToDevice, ctx->st));
-        launch_fill_u32(cp.ptr + off, pp.first, cnt, ctx->st);
-        off += cnt;
-    }
-    res->cols = {cs, cp, co};
-    *out = std::move(res);
-    return KB_OK;
-}
-
 // the facts of a head predicate as bindings of the head's variables (a constant of the head binds nothing: every fact derived from
 // these bindings is checked against the facts themselves by the gate); nullptr when the head has no variable
 std::unique_ptr<kb_rel> head_view(const PredRel& D, const kb_pattern& h) {
@@ -1076,8 +1618,7 @@ static kb_status maintain_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
                                const kb_rel* add, uint64_t add_tag, kb_rel** inferred_removed, kb_rel** inferred_added, kb_maintain_stats* stats) {
     // ---- validation: nothing changes before all of it passed
     if ((n_rules && !rules) || (n_evict && !evict_tags)) return fail(ctx, KB_E_INVALID, "NULL argument");
-    if (strategy != KB_SEMI_NAIVE && strategy != KB_NAIVE && strategy != KB_SEMI_NAIVE_PARALLEL && strategy != KB_SEMI_NAIVE_OLD_DELTA)
-        return fail(ctx, KB_E_INVALID, "unknown strategy %u", strategy);
+    KB_TRY(check_strategy(ctx, strategy));
     if (strategy == KB_SEMI_NAIVE_PARALLEL) return fail(ctx, KB_E_UNSUPPORTED, "kb_datalog_maintain: KB_SEMI_NAIVE_PARALLEL has its own closure; not maintained");
     if (add && (add->pair || add->cols.size() != 3 || add->col_of(0) != 0 || add->col_of(1) != 1 || add->col_of(2) != 2))
         return fail(ctx, KB_E_INVALID, "`add` must be a 3-column relation with slots 0,1,2 = s,p,o");
@@ -1129,10 +1670,15 @@ static kb_status maintain_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
     cl->has_state = false;
     cl->rels.clear();
     cl->base.clear();
+    std::vector<Segment> base_segs, inferred_segs, evicted_segs;
+    for (auto& sg : ctx->segs) {
+        (sg.tag == KB_TAG_INFERRED ? inferred_segs : base_segs).push_back(sg);
+        if (evict.count(sg.tag)) evicted_segs.push_back(sg);
+    }
     if (!reused) {
         std::map<u32, Pairs> bsplit, isplit;
-        KB_TRY(split_segments(ctx, preds, [](const Segment& sg) { return sg.tag != KB_TAG_INFERRED; }, &bsplit));
-        KB_TRY(split_segments(ctx, preds, [](const Segment& sg) { return sg.tag == KB_TAG_INFERRED; }, &isplit));
+        KB_TRY(split_segments(ctx, base_segs, preds, &bsplit));
+        KB_TRY(split_segments(ctx, inferred_segs, preds, &isplit));
         for (u32 p : preds) {
             PredRel& r = fx.rels[p];
             const Pairs &b = bsplit[p], &i = isplit[p];
@@ -1152,14 +1698,10 @@ static kb_status maintain_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
     // or `add` still holds keeps a positive count and does not move.
     std::map<u32, Pairs> evicted, d0, fresh;
     std::map<u32, std::unique_ptr<kb_rel>> add_of;
-    KB_TRY(split_segments(ctx, preds, [&](const Segment& sg) { return evict.count(sg.tag) != 0; }, &evicted));
+    KB_TRY(split_segments(ctx, evicted_segs, preds, &evicted));
     for (u32 p : preds) {
         if (add && add->n) {
-            FilterProg f;
-            kb_filter_op op{};
-            op.op = KB_F_EQ_ID; op.slot = 1; op.id = p;
-            f.ops.push_back(op);
-            KB_TRY(filter_impl(ctx, *add, f, &add_of[p]));
+            KB_TRY(rows_of_predicate(ctx, *add, p, &add_of[p]));
             const kb_rel& a = *add_of[p];
             KB_TRY(base_update(ctx, base[p], a.cols[a.col_of(0)].ptr, a.cols[a.col_of(2)].ptr, a.n, +1, &fresh[p]));
         }
@@ -1205,9 +1747,7 @@ static kb_status maintain_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
             const kb_rule& rule = rules[r];
             const RulePlan& pl = plans[r];
             const u32 np = (u32)pl.prem.size();
-            bool dead = np == 0;
-            for (auto& pr : pl.prem) if (!pr.pred_const) dead = true;
-            if (dead) continue;
+            if (!pl.fires) continue;
             for (u32 i = 0; i < np; i++) {
                 const PredRel& dr = del.rels[pl.prem[i].pred];
                 const u64 n = dr.snapshot - dr.delta_start;
@@ -1217,11 +1757,7 @@ static kb_status maintain_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
                 for (u32 j = 0; j < np && cur->n; j++) {
                     if (j == i) continue;
                     const PredRel& pr = fx.rels[pl.prem[j].pred];
-                    if (pr.n == 0) { cur->n = 0; break; }
-                    std::unique_ptr<kb_rel> all, joined;
-                    KB_TRY(make_view(ctx, pr, 0, pr.n, (u32)pl.prem[j].s_var, (u32)pl.prem[j].o_var, &all));
-                    KB_TRY(hash_join_impl(ctx, *cur, *all, nullptr, &joined));
-                    cur = std::move(joined);
+                    KB_TRY(join_premise(ctx, cur, pl.prem[j], pr, pr.n, false, tr));
                 }
                 if (cur->n == 0) continue;
                 for (u32 c = 0; c < rule.n_conclusion; c++) {
@@ -1267,9 +1803,7 @@ static kb_status maintain_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
         const kb_rule& rule = rules[r];
         const RulePlan& pl = plans[r];
         const u32 np = (u32)pl.prem.size();
-        bool dead = np == 0;
-        for (auto& pr : pl.prem) if (!pr.pred_const) dead = true;
-        if (dead) continue;
+        if (!pl.fires) continue;
         for (u32 c = 0; c < rule.n_conclusion; c++) {
             const kb_pattern& h = rule.conclusion[c];
             const PredRel& dr = del.rels[h.p.value];
@@ -1283,12 +1817,7 @@ static kb_status maintain_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
                 for (u32 k = 0; k < np && j == np; k++) if (!used[k]) j = k;
                 used[j] = true;
                 const PredRel& pr = fx.rels[pl.prem[j].pred];
-                std::unique_ptr<kb_rel> all, joined;
-                KB_TRY(make_view(ctx, pr, 0, pr.n, (u32)pl.prem[j].s_var, (u32)pl.prem[j].o_var, &all));
-                if (!cur) { cur = std::move(all); continue; }
-                if (pr.n == 0) { cur->n = 0; break; }
-                KB_TRY(hash_join_impl(ctx, *cur, *all, nullptr, &joined));
-                cur = std::move(joined);
+                KB_TRY(join_premise(ctx, cur, pl.prem[j], pr, pr.n, false, tr));
             }
             if (!cur || cur->n == 0) continue;
             Gate g;
@@ -1306,29 +1835,22 @@ static kb_status maintain_impl(kb_ctx* ctx, const kb_rule* rules, uint32_t n_rul
 
     // ---- 5. insert: the seeds (rederived facts, then the facts of `add` the closure does not hold) take the seed path of
     // kb_datalog_fixpoint_seed, then semi-naive rounds (KB_NAIVE: the same closure, reached from the delta)
-    for (auto& kv : fx.rels) kv.second.snapshot = kv.second.seed_from = kv.second.n;
-    fx.pend.clear();
     {
-        u64 seed_derivations = 0;  // (seed facts are not derivations)
+        std::vector<std::unique_ptr<kb_rel>> views;
+        std::vector<std::pair<u32, const kb_rel*>> seeds;
         for (u32 p : preds) {
-            kb_pattern h{};
-            h.s = kb_term{1, 0}; h.p = kb_term{0, p}; h.o = kb_term{1, 2};
             const PredRel& rr = red.rels[p];
             if (rr.n) {
-                std::unique_ptr<kb_rel> v;
-                KB_TRY(make_view(ctx, rr, 0, rr.n, 0, 2, &v));
-                KB_TRY(derive_head(fx, v.get(), h, nullptr, false, nullptr, tr, &seed_derivations));
+                views.emplace_back();
+                KB_TRY(make_view(ctx, rr, 0, rr.n, 0, 2, &views.back()));
+                seeds.push_back({p, views.back().get()});
             }
             auto a = add_of.find(p);
-            if (a != add_of.end() && a->second->n) KB_TRY(derive_head(fx, a->second.get(), h, nullptr, false, nullptr, tr, &seed_derivations));
+            if (a != add_of.end()) seeds.push_back({p, a->second.get()});
         }
-    }
-    for (auto& kv : fx.rels) kv.second.delta_start = kv.second.snapshot;
-    {
         u64 n = 0;
-        KB_TRY(flush_pending(fx, &n));
+        KB_TRY(accept_seeds(fx, seeds, nullptr, tr, &n));
     }
-    for (auto& kv : fx.rels) kv.second.base_n = kv.second.n;
     kb_fixpoint_stats ist{};
     KB_TRY(run_rounds(fx, rules, n_rules, plans, strategy == KB_SEMI_NAIVE_OLD_DELTA ? KB_SEMI_NAIVE_OLD_DELTA : KB_SEMI_NAIVE, ist, tr));
     ms.insert_rounds = ist.rounds;

@@ -1817,7 +1817,7 @@ void launch_cartesian(const u32* const* lcols, u32 nl, u32 n_lcols, const u32* c
 }
 
 // =================================================================================================================
-// Datalog: known-fact sets (kb_kernels.cuh)
+// the store's 96-bit (s,p,o) key set (kb_store.cu)
 __global__ void __launch_bounds__(256) set_insert_kernel(uint4* set, u32 set_slots, const u32* s, const u32* p, u32 p_const, const u32* o,
                                                          u32 n, u32* overflow) {
     const u32 stride = gridDim.x * blockDim.x;
@@ -1829,450 +1829,6 @@ void launch_set_insert(uint4* set, u32 set_slots, const u32* s, const u32* p, u3
     if (n == 0) return;
     int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull);
     set_insert_kernel<<<grid, 256, 0, st>>>(set, set_slots, s, p, p_const, o, n, overflow);
-}
-
-__global__ void __launch_bounds__(256) set64_insert_kernel(u64* set, u32 set_slots, const u32* s, const u32* o, u32 n, u32* overflow) {
-    const u32 stride = gridDim.x * blockDim.x;
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
-        if (set64_insert(set, set_slots, s[i], o[i]) == 2u) *overflow = 1u;
-}
-void launch_set64_insert(u64* set, u32 set_slots, const u32* s, const u32* o, u32 n, u32* overflow, int n_sms, cudaStream_t st) {
-    if (n == 0) return;
-    int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull);
-    set64_insert_kernel<<<grid, 256, 0, st>>>(set, set_slots, s, o, n, overflow);
-}
-
-// set64_insert that returns the key's slot (EMPTY32: table full); *claimed = this call took a free slot for the key
-__device__ __forceinline__ u32 set64_insert_slot(u64* set, u32 n_slots, u32 s, u32 o, bool* claimed) {
-    const u64 key = ((u64)s << 32) | (u64)o;
-    const u32 mask = n_slots - 1u;
-    u32 slot = mix32(mix32(s) * 0x9E3779B1u ^ mix32(o + 0x632BE5ABu)) & mask;
-    *claimed = false;
-    for (u32 probes = 0; probes < n_slots; probes++) {
-        const u64 cur = *reinterpret_cast<volatile u64*>(&set[slot]);
-        if (cur == key) return slot;
-        if (cur == EMPTY64) {
-            const u64 old = atomicCAS(reinterpret_cast<unsigned long long*>(&set[slot]), (unsigned long long)EMPTY64, (unsigned long long)key);
-            if (old == EMPTY64) { *claimed = true; return slot; }
-            if (old == key) return slot;
-        }
-        slot = (slot + 1u) & mask;
-    }
-    return EMPTY32;
-}
-// the acceptance test in front of the dedup: demanded (kb_datalog_query), member of the gate set and no positive count in the veto table
-// (kb_datalog_maintain)
-__device__ __forceinline__ bool derive_gate_pass(const DeriveParams& P, u32 s, u32 o) {
-    if (P.demand && !bc_demanded(P.demand, P.n_demand, s, o)) return false;
-    if (P.gate_set && set64_find(P.gate_set, P.gate_slots, s, o) == EMPTY32) return false;
-    if (P.veto_keys) {
-        const u32 slot = set64_find(P.veto_keys, P.veto_slots, s, o);
-        if (slot != EMPTY32 && P.veto_cnt[slot] > 0u) return false;
-    }
-    return true;
-}
-
-__device__ __forceinline__ bool rule_filters_pass(const DeriveParams& P, u32 i) {
-    for (u32 f = 0; f < P.n_filt; f++) {
-        const RuleFilterDev fl = P.filt[f];
-        const u32 lhs = P.bcol[fl.lhs_col][i];
-        if (fl.rhs_is_var) {  // rules.rs:141-146 — ids of two bound variables; only = / != act
-            const u32 rhs = P.bcol[fl.rhs_col][i];
-            if (fl.cmp == KB_CMP_NE && lhs == rhs) return false;
-            if (fl.cmp == KB_CMP_EQ && lhs != rhs) return false;
-        } else {  // rules.rs:148-160
-            const double a = num_of(P.nt, lhs), c = fl.rhs_value;
-            const double eps = 2.220446049250313e-16;
-            switch (fl.cmp) {
-                case KB_CMP_GT: if (a <= c) return false; break;
-                case KB_CMP_LT: if (a >= c) return false; break;
-                case KB_CMP_GE: if (a < c) return false; break;
-                case KB_CMP_LE: if (a > c) return false; break;
-                case KB_CMP_EQ: if (fabs(a - c) > eps) return false; break;
-                case KB_CMP_NE: if (fabs(a - c) <= eps) return false; break;
-                default: break;
-            }
-        }
-    }
-    return true;
-}
-
-template <bool GATED>
-__global__ void __launch_bounds__(256) derive_kernel(const __grid_constant__ DeriveParams P) {
-    const int lane = threadIdx.x & 31;
-    const u32 stride = gridDim.x * blockDim.x;
-    const u32 n_round = (P.n + 31u) & ~31u;
-    unsigned long long nd = 0;
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += stride) {
-        bool pass = i < P.n && rule_filters_pass(P, i);
-        bool fresh = false;
-        u32 s = 0, o = 0;
-        if (pass) nd++;
-        if (pass && *reinterpret_cast<volatile u32*>(P.out_count) >= P.budget) {  // the set must grow first; this launch is run again
-            *P.overflow = 2u;
-            pass = false;
-        }
-        if (pass) {
-            s = P.head_s.is_var ? P.bcol[P.head_s.value][i] : P.head_s.value;
-            o = P.head_o.is_var ? P.bcol[P.head_o.value][i] : P.head_o.value;
-            if (GATED && !derive_gate_pass(P, s, o)) pass = false;
-        }
-        if (pass) {
-            const u32 r = set64_insert(P.set, P.set_slots, s, o);
-            if (r == 2u) atomicMax(P.overflow, 1u);
-            fresh = r == 1u;
-        }
-        const unsigned b = __ballot_sync(0xffffffffu, fresh);  // warp-aggregated append of the facts that were new
-        if (b) {
-            u32 basepos = 0;
-            if (lane == __ffs(b) - 1) basepos = atomicAdd(P.out_count, (u32)__popc(b));
-            basepos = __shfl_sync(0xffffffffu, basepos, __ffs(b) - 1);
-            if (fresh) {
-                const u32 r = basepos + (u32)__popc(b & ((1u << lane) - 1u));
-                if (r < P.out_cap) { P.out_s[r] = s; P.out_o[r] = o; }
-                else *P.overflow = 1u;
-            }
-        }
-    }
-    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 16);
-    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 8);
-    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 4);
-    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 2);
-    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 1);
-    if (lane == 0 && nd) atomicAdd(P.n_deriv, nd);
-}
-// ---- radix-partitioned variant
-constexpr int DPART_THREADS = 256;
-constexpr int DPART_ITEMS = 16;
-constexpr int DPART_TILE = DPART_THREADS * DPART_ITEMS;  // 4096 candidates: 32 KB of keys + 8 KB of partition ids in shared memory
-constexpr int DPART_MAXP = 1024;
-__device__ __forceinline__ u32 set64_home(u32 n_slots, u32 s, u32 o) { return mix32(mix32(s) * 0x9E3779B1u ^ mix32(o + 0x632BE5ABu)) & (n_slots - 1u); }
-
-// insert + append of ONE candidate outside any warp-cooperative section (bucket overflow path of the partition pass)
-__device__ __noinline__ void derive_one(const DeriveParams& P, u32 s, u32 o) {
-    if (*reinterpret_cast<volatile u32*>(P.out_count) >= P.budget) { *P.overflow = 2u; return; }
-    const u32 r = set64_insert(P.set, P.set_slots, s, o);
-    if (r == 2u) *P.overflow = 2u;
-    if (r == 1u) {
-        const u32 at = atomicAdd(P.out_count, 1u);
-        if (at < P.out_cap) { P.out_s[at] = s; P.out_o[at] = o; }
-        else *P.overflow = 1u;
-    }
-}
-
-__global__ void __launch_bounds__(DPART_THREADS) derive_partition_kernel(const __grid_constant__ DerivePartParams Q) {
-    extern __shared__ __align__(16) u64 sh_keys[];  // [DPART_TILE] keys sorted by partition, then u16 partition ids
-    __shared__ u32 s_cnt[DPART_MAXP], s_off[DPART_MAXP], s_gbase[DPART_MAXP];
-    __shared__ u32 s_tile;
-    const DeriveParams& P = Q.d;
-    unsigned short* s_dest = reinterpret_cast<unsigned short*>(sh_keys + DPART_TILE);
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const u32 n_tiles = (P.n + DPART_TILE - 1u) / DPART_TILE;
-    unsigned long long nd = 0;
-    for (;;) {
-        if (tid == 0) s_tile = atomicAdd(&Q.tickets[0], 1u);
-        for (u32 d = (u32)tid; d < Q.n_parts; d += DPART_THREADS) s_cnt[d] = 0u;
-        __syncthreads();
-        const u32 tile = s_tile;
-        if (tile >= n_tiles) break;
-        const u32 row0 = tile * (u32)DPART_TILE;
-        const u32 cnt = min((u32)DPART_TILE, P.n - row0);
-        // ---- 1. head instantiation + rule filters; partition = high bits of the key's home slot; histogram
-        u64 key[DPART_ITEMS];
-        u32 part[DPART_ITEMS], rank[DPART_ITEMS];
-#pragma unroll
-        for (int j = 0; j < DPART_ITEMS; j++) {
-            const u32 r = (u32)j * DPART_THREADS + (u32)tid;
-            const u32 i = row0 + r;
-            bool pass = r < cnt && rule_filters_pass(P, i);
-            u32 s = 0, o = 0;
-            if (pass) {
-                nd++;
-                s = P.head_s.is_var ? __ldg(P.bcol[P.head_s.value] + i) : P.head_s.value;
-                o = P.head_o.is_var ? __ldg(P.bcol[P.head_o.value] + i) : P.head_o.value;
-                if (P.demand && !bc_demanded(P.demand, P.n_demand, s, o)) pass = false;
-            }
-            key[j] = ((u64)s << 32) | (u64)o;
-            part[j] = pass ? (set64_home(P.set_slots, s, o) >> Q.slice_bits) : 0xFFFFu;
-            rank[j] = pass ? atomicAdd(&s_cnt[part[j]], 1u) : 0u;  // the key's place among the tile's keys of its partition (kept for step 3)
-        }
-        __syncthreads();
-        // ---- 2. offsets inside the tile (one warp scans the histogram), one range reservation per partition
-        if (warp == 0) {
-            u32 run = 0;
-            for (u32 d0 = 0; d0 < Q.n_parts; d0 += 32u) {
-                const u32 d = d0 + (u32)lane;
-                const u32 c = d < Q.n_parts ? s_cnt[d] : 0u;
-                u32 incl = c;
-#pragma unroll
-                for (int o = 1; o < 32; o <<= 1) {
-                    const u32 y = __shfl_up_sync(0xffffffffu, incl, o);
-                    if (lane >= o) incl += y;
-                }
-                if (d < Q.n_parts) {
-                    s_off[d] = run + incl - c;
-                    s_gbase[d] = c ? atomicAdd(&Q.cursors[d], c) : 0u;
-                }
-                run += __shfl_sync(0xffffffffu, incl, 31);
-            }
-        }
-        __syncthreads();
-        // ---- 3. keys staged in partition order
-#pragma unroll
-        for (int j = 0; j < DPART_ITEMS; j++) {
-            if (part[j] == 0xFFFFu) continue;
-            const u32 pos = s_off[part[j]] + rank[j];
-            sh_keys[pos] = key[j];
-            s_dest[pos] = (unsigned short)part[j];
-        }
-        __syncthreads();
-        // ---- 4. flush: staged position q belongs to partition s_dest[q]; consecutive q of one partition are consecutive in its bucket
-        const u32 staged = s_off[Q.n_parts - 1u] + s_cnt[Q.n_parts - 1u];
-        for (u32 q = (u32)tid; q < staged; q += DPART_THREADS) {
-            const u32 d = s_dest[q];
-            const u32 at = s_gbase[d] + (q - s_off[d]);
-            const u64 k = sh_keys[q];
-            if (at < Q.bucket_cap) Q.buckets[(u64)d * Q.bucket_cap + at] = k;
-            else derive_one(P, (u32)(k >> 32), (u32)k);  // the bucket is full (skewed hash): probe directly
-        }
-        __syncthreads();
-    }
-    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 16);
-    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 8);
-    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 4);
-    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 2);
-    nd = nd + __shfl_xor_sync(0xffffffffu, nd, 1);
-    if (lane == 0 && nd) atomicAdd(P.n_deriv, nd);
-}
-
-constexpr int DPROBE_TILE = 2048;
-__global__ void __launch_bounds__(1024) derive_tile_starts_kernel(const __grid_constant__ DerivePartParams Q) {
-    __shared__ u32 s_tiles[DPART_MAXP];
-    const int tid = threadIdx.x;
-    if ((u32)tid < Q.n_parts) s_tiles[tid] = (min(Q.cursors[tid], Q.bucket_cap) + DPROBE_TILE - 1u) / DPROBE_TILE;
-    __syncthreads();
-    if (tid == 0) {
-        u32 run = 0;
-        for (u32 d = 0; d < Q.n_parts; d++) { Q.tile_start[d] = run; run += s_tiles[d]; }
-        Q.tile_start[Q.n_parts] = run;
-    }
-}
-
-__global__ void __launch_bounds__(256) derive_probe_kernel(const __grid_constant__ DerivePartParams Q) {
-    __shared__ u32 s_tile, s_base;
-    __shared__ u32 s_wcnt[8];
-    const DeriveParams& P = Q.d;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const u32 n_tiles = Q.tile_start[Q.n_parts];
-    constexpr int R = DPROBE_TILE / 256;
-    for (;;) {
-        __syncthreads();
-        if (tid == 0) s_tile = atomicAdd(&Q.tickets[1], 1u);  // tickets are handed out in partition order: the CTAs walk the slices together
-        __syncthreads();
-        const u32 tile = s_tile;
-        if (tile >= n_tiles) break;
-        u32 lo = 0, hi = Q.n_parts;  // partition of this tile: last d with tile_start[d] <= tile
-        while (hi - lo > 1u) {
-            const u32 mid = (lo + hi) >> 1;
-            if (Q.tile_start[mid] <= tile) lo = mid; else hi = mid;
-        }
-        const u32 d = lo;
-        const u32 n_keys = min(Q.cursors[d], Q.bucket_cap);
-        const u32 first = (tile - Q.tile_start[d]) * (u32)DPROBE_TILE;
-        const u64* keys = Q.buckets + (u64)d * Q.bucket_cap;
-        // the set must not fill past its budget: checked once per tile (a tile adds at most DPROBE_TILE facts: the budget leaves that room)
-        const bool room = *reinterpret_cast<volatile u32*>(P.out_count) < P.budget;
-        if (!room && tid == 0) *P.overflow = 2u;
-        u64 k[R];
-        u32 fresh = 0;
-#pragma unroll
-        for (int j = 0; j < R; j++) {
-            const u32 q = first + (u32)j * 256u + (u32)tid;
-            k[j] = (room && q < n_keys) ? __ldg(keys + q) : EMPTY64;
-        }
-#pragma unroll
-        for (int j = 0; j < R; j++) {
-            if (k[j] == EMPTY64) continue;  // (s = o = 0xFFFFFFFF is the reserved id: never a fact)
-            const u32 r = set64_insert(P.set, P.set_slots, (u32)(k[j] >> 32), (u32)k[j]);
-            if (r == 2u) *P.overflow = 2u;  // table full (the per-tile budget check lets a small table overshoot): grow and run again
-            fresh |= (r == 1u ? 1u : 0u) << j;
-        }
-        // ONE reservation per tile for the facts that were new (a single global cursor serialises: per-warp reservations
-        // dominated the pass on 1.4e8 new facts), then ranked writes
-        const u32 c = (u32)__popc(fresh);
-        u32 incl = c;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const u32 y = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= o) incl += y;
-        }
-        if (lane == 31) s_wcnt[warp] = incl;
-        __syncthreads();
-        if (tid == 0) {
-            u32 run = 0;
-#pragma unroll
-            for (int w = 0; w < 8; w++) { const u32 x = s_wcnt[w]; s_wcnt[w] = run; run += x; }
-            s_base = run ? atomicAdd(P.out_count, run) : 0u;
-        }
-        __syncthreads();
-        u32 pos = s_base + s_wcnt[warp] + incl - c;
-#pragma unroll
-        for (int j = 0; j < R; j++) {
-            if ((fresh >> j) & 1u) {
-                if (pos < P.out_cap) { P.out_s[pos] = (u32)(k[j] >> 32); P.out_o[pos] = (u32)k[j]; }
-                else *P.overflow = 1u;
-                pos++;
-            }
-        }
-    }
-}
-
-void launch_derive_partitioned(const DerivePartParams& p, int n_sms, cudaStream_t st) {
-    if (p.d.n == 0) return;
-    const size_t smem = (size_t)DPART_TILE * (sizeof(u64) + sizeof(unsigned short));
-    static bool attr = false;
-    if (!attr) { cudaFuncSetAttribute(derive_partition_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); attr = true; }
-    const u32 n_tiles = (p.d.n + DPART_TILE - 1u) / DPART_TILE;
-    const int grid1 = grid_for((const void*)derive_partition_kernel, DPART_THREADS, smem, n_sms, n_tiles);
-    static const bool trace = getenv("KOLIBRIE_TRACE") != nullptr;
-    cudaEvent_t e0 = nullptr, e1 = nullptr, e2 = nullptr;
-    if (trace) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventCreate(&e2); cudaEventRecord(e0, st); }
-    derive_partition_kernel<<<grid1, DPART_THREADS, smem, st>>>(p);
-    if (trace) cudaEventRecord(e1, st);
-    derive_tile_starts_kernel<<<1, 1024, 0, st>>>(p);
-    const int grid2 = grid_for((const void*)derive_probe_kernel, 256, 0, n_sms, (p.d.n + DPROBE_TILE - 1u) / DPROBE_TILE + p.n_parts);
-    derive_probe_kernel<<<grid2, 256, 0, st>>>(p);
-    if (trace) {
-        cudaEventRecord(e2, st);
-        cudaEventSynchronize(e2);
-        float a = 0.f, b = 0.f;
-        cudaEventElapsedTime(&a, e0, e1);
-        cudaEventElapsedTime(&b, e1, e2);
-        fprintf(stderr, "[kb trace]     derive partitioned: %u candidates, %u partitions: partition pass %.3f ms, probe pass %.3f ms\n", p.d.n, p.n_parts, a, b);
-        cudaEventDestroy(e0); cudaEventDestroy(e1); cudaEventDestroy(e2);
-    }
-}
-
-void launch_derive(const DeriveParams& p, int n_sms, cudaStream_t st) {
-    if (p.n == 0) return;
-    int grid = (int)umin64((u64)n_sms * 8ull, ((u64)p.n + 255ull) / 256ull);
-    if (p.gate_set || p.veto_keys || p.demand) derive_kernel<true><<<grid, 256, 0, st>>>(p);
-    else derive_kernel<false><<<grid, 256, 0, st>>>(p);
-}
-
-// ---- kb_datalog_maintain: base multiplicities, selection by set membership, erasure
-__device__ __forceinline__ void emit_pair(bool take, u32 s, u32 o, u32* out_s, u32* out_o, u32* out_count) {  // warp-aggregated append
-    const int lane = threadIdx.x & 31;
-    const unsigned b = __ballot_sync(0xffffffffu, take);
-    if (!b) return;
-    u32 basepos = 0;
-    if (lane == __ffs(b) - 1) basepos = atomicAdd(out_count, (u32)__popc(b));
-    basepos = __shfl_sync(0xffffffffu, basepos, __ffs(b) - 1);
-    if (take) {
-        const u32 r = basepos + (u32)__popc(b & ((1u << lane) - 1u));
-        out_s[r] = s;
-        out_o[r] = o;
-    }
-}
-
-__global__ void __launch_bounds__(256) base_count_kernel(const __grid_constant__ BaseCountParams P) {
-    const u32 stride = gridDim.x * blockDim.x;
-    const u32 n_round = (P.n + 31u) & ~31u;
-    u32 n_edges = 0, n_claimed = 0;  // (counted here when nothing is emitted)
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += stride) {
-        bool edge = false;  // this row moved the count across zero
-        u32 s = 0, o = 0;
-        if (i < P.n) {
-            s = P.s[i];
-            o = P.o[i];
-            if (P.delta > 0) {
-                bool claimed = false;
-                const u32 slot = set64_insert_slot(P.keys, P.slots, s, o, &claimed);
-                if (slot == EMPTY32) *P.overflow = 1u;
-                else edge = atomicAdd(&P.cnt[slot], 1u) == 0u;
-                n_claimed += claimed ? 1u : 0u;
-            } else {
-                const u32 slot = set64_find(P.keys, P.slots, s, o);
-                if (slot != EMPTY32) edge = atomicSub(&P.cnt[slot], 1u) == 1u;
-            }
-        }
-        if (P.out_s) emit_pair(edge, s, o, P.out_s, P.out_o, P.out_count);
-        else n_edges += edge ? 1u : 0u;
-    }
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) {
-        n_edges += __shfl_xor_sync(0xffffffffu, n_edges, d);
-        n_claimed += __shfl_xor_sync(0xffffffffu, n_claimed, d);
-    }
-    if ((threadIdx.x & 31) == 0) {
-        if (n_edges) atomicAdd(P.out_count, n_edges);
-        if (n_claimed) atomicAdd(P.claimed, n_claimed);
-    }
-}
-void launch_base_count(const BaseCountParams& p, int n_sms, cudaStream_t st) {
-    if (p.n == 0) return;
-    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)p.n + 255ull) / 256ull);
-    base_count_kernel<<<grid, 256, 0, st>>>(p);
-}
-
-__global__ void __launch_bounds__(256) base_count_rehash_kernel(const u64* okeys, const u32* ocnt, u32 oslots, u64* nkeys, u32* ncnt, u32 nslots,
-                                                                u32* n_live, u32* overflow) {
-    const u32 stride = gridDim.x * blockDim.x;
-    u32 moved = 0;
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < oslots; i += stride) {
-        const u64 k = okeys[i];
-        const u32 c = ocnt[i];
-        if (k == EMPTY64 || c == 0u) continue;
-        bool claimed = false;
-        const u32 slot = set64_insert_slot(nkeys, nslots, (u32)(k >> 32), (u32)k, &claimed);
-        if (slot == EMPTY32) { *overflow = 1u; continue; }
-        ncnt[slot] = c;  // keys are distinct: one writer per slot
-        moved++;
-    }
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) moved += __shfl_xor_sync(0xffffffffu, moved, d);
-    if ((threadIdx.x & 31) == 0 && moved) atomicAdd(n_live, moved);
-}
-void launch_base_count_rehash(const u64* okeys, const u32* ocnt, u32 oslots, u64* nkeys, u32* ncnt, u32 nslots, u32* n_live, u32* overflow, int n_sms,
-                              cudaStream_t st) {
-    if (oslots == 0) return;
-    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)oslots + 255ull) / 256ull);
-    base_count_rehash_kernel<<<grid, 256, 0, st>>>(okeys, ocnt, oslots, nkeys, ncnt, nslots, n_live, overflow);
-}
-
-__global__ void __launch_bounds__(256) pair_select_kernel(const __grid_constant__ PairSelectParams P) {
-    const u32 stride = gridDim.x * blockDim.x;
-    const u32 n_round = (P.n + 31u) & ~31u;
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += stride) {
-        bool take = false;
-        u32 s = 0, o = 0;
-        if (i < P.n) {
-            s = P.s[i];
-            o = P.o[i];
-            const u32 slot = set64_find(P.keys, P.slots, s, o);
-            const bool present = slot != EMPTY32 && (!P.cnt || P.cnt[slot] > 0u);
-            take = present == (P.keep_present != 0u);
-        }
-        emit_pair(take, s, o, P.out_s, P.out_o, P.out_count);
-    }
-}
-void launch_pair_select(const PairSelectParams& p, int n_sms, cudaStream_t st) {
-    if (p.n == 0) return;
-    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)p.n + 255ull) / 256ull);
-    pair_select_kernel<<<grid, 256, 0, st>>>(p);
-}
-
-__global__ void __launch_bounds__(256) set64_erase_kernel(u64* set, u32 set_slots, const u32* s, const u32* o, u32 n) {
-    const u32 stride = gridDim.x * blockDim.x;
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-        const u32 slot = set64_find(set, set_slots, s[i], o[i]);
-        if (slot != EMPTY32) set[slot] = TOMB64;
-    }
-}
-void launch_set64_erase(u64* set, u32 set_slots, const u32* s, const u32* o, u32 n, int n_sms, cudaStream_t st) {
-    if (n == 0) return;
-    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull);
-    set64_erase_kernel<<<grid, 256, 0, st>>>(set, set_slots, s, o, n);
 }
 
 // =================================================================================================================

@@ -1,4 +1,6 @@
-// kb_kernels.cuh — parameter blocks and launch wrappers of the sm_90a kernels (definitions in kb_kernels.cu).
+// kb_kernels.cuh — parameter blocks and launch wrappers of the shared sm_90a kernels (definitions in kb_kernels.cu), and the device
+// functions more than one file's kernels read (the key sets, demand patterns, emit_pair). Kernels with a single owner keep their launch
+// formats in that file: the Datalog ones in kb_datalog.cu, the backward-chaining ones in kb_backward.cu.
 #pragma once
 #include "kb_device.cuh"
 
@@ -340,58 +342,9 @@ void launch_group_compact(const GroupParams& p, GroupRecord* out, u32* header, u
 void launch_peer_barrier(const PeerTables& t, u32 epoch, cudaStream_t st);
 void launch_group_merge_peers(const GroupParams& p, const PeerTables& t, int n_sms, cudaStream_t st);
 
-// ---------------------------------------------------------------------------------------------------------------
-// Datalog: instantiate rule heads from binding columns, apply rule filters (rules.rs:133-165), insert into the
-// known-facts set (96-bit keys) and append the facts that were new (infer_generic.rs:42-48).
-struct HeadTerm { u32 is_var, value; };  // value = binding column index or constant id
-struct RuleFilterDev { u32 lhs_col, cmp, rhs_is_var, rhs_col; double rhs_value; };
-struct DeriveParams {
-    const u32* bcol[KB_MAX_COLS];
-    u32 n;
-    HeadTerm head_s, head_o;  // the head predicate is a constant: one known-fact set per predicate, keyed by (s << 32) | o
-    RuleFilterDev filt[KB_MAX_RULE_FILTERS];
-    u32 n_filt;
-    NumTab nt;
-    u64* set;       // open addressing, EMPTY64 = free; a fact is new iff its atomicCAS wins
-    u32 set_slots;  // power of two
-    u32 *out_s, *out_o;
-    u32 out_cap;
-    u32 budget;                   // stop inserting once this many facts were appended (keeps the set's load bounded): overflow = 2
-    u32* out_count;               // appended so far (atomic cursor)
-    unsigned long long* n_deriv;  // candidates that passed the filters
-    u32* overflow;                // 1: set or output full (error); 2: budget reached, the host grows the set and runs the launch again
-    // kb_datalog_maintain (delete-and-rederive): a candidate takes part in the dedup only if it is a member of gate_set (when non-null)
-    // and has no positive count in the veto table (when non-null). Gated launches never take the partitioned path.
-    const u64* gate_set;
-    u32 gate_slots;
-    const u64* veto_keys;
-    const u32* veto_cnt;
-    u32 veto_slots;
-    // kb_datalog_query: a candidate takes part in the dedup only if it matches one of the head predicate's n_demand demand patterns
-    // (x = subject, y = object, KB_ID_NONE = any; null: every fact is demanded). Applied on both dedup routes.
-    const uint2* demand;
-    u32 n_demand;
-};
-void launch_derive(const DeriveParams& p, int n_sms, cudaStream_t st);
-// RADIX-PARTITIONED candidate dedup (the same work as launch_derive for large candidate sets). The known-fact set is an open-addressing
-// table far larger than L2 (config 4: 8 GB), so a direct probe per candidate is one random DRAM line per candidate. Here the
-// candidates are first partitioned by the HIGH bits of their home slot (tile sorted by partition in shared memory, one range
-// reservation per tile and partition, coalesced runs), so that partition p only touches slice p of the table; the probe pass then walks
-// the partitions in order, every CTA on (nearly) the same slice, which is sized to stay resident in L2.
-struct DerivePartParams {
-    DeriveParams d;            // candidates, head, filters, set, outputs, counters (as for launch_derive)
-    u32 slice_bits;            // log2(slots per slice); partition = home slot >> slice_bits
-    u32 n_parts;               // set_slots >> slice_bits, <= 1024
-    u64* buckets;              // [n_parts][bucket_cap] candidate keys (s << 32 | o)
-    u32 bucket_cap;
-    u32* cursors;              // [n_parts] keys in each bucket (zeroed)
-    u32* tile_start;           // [n_parts + 1] first probe tile of each partition (written by the launch)
-    u32* tickets;              // [2] zeroed: tile counters of the two passes
-};
-void launch_derive_partitioned(const DerivePartParams& p, int n_sms, cudaStream_t st);
-void launch_set64_insert(u64* set, u32 set_slots, const u32* s, const u32* o, u32 n, u32* overflow, int n_sms, cudaStream_t st);
-// ---- the known-fact sets (device side, shared with kb_backward.cu)
-// Datalog: known-fact set with 96-bit keys in 16-byte slots {s,p,o,state}
+// ---- key sets (device side): the Datalog launches (kb_datalog.cu), the answer pass of kb_backward.cu, the store (kb_store.cu) and
+// kb_repairs.cu read them
+// 96-bit (s,p,o) keys in 16-byte slots {s,p,o,state}
 __device__ __forceinline__ u32 set_hash(u32 s, u32 p, u32 o) { return mix32(mix32(s) * 0x9E3779B1u ^ mix32(o + 0x632BE5ABu) ^ (p * 0x85EBCA77u)); }
 
 // returns 1 if (s,p,o) was inserted now, 0 if it was already there, 2 on overflow; *at = the key's slot (1 and 0)
@@ -465,7 +418,11 @@ __device__ __forceinline__ u32 set64_find(const u64* set, u32 n_slots, u32 s, u3
     }
     return EMPTY32;
 }
-// ---- backward-chaining queries (kb_backward.cu)
+// the store's batch insert into a 96-bit set (kb_store.cu)
+void launch_set_insert(uint4* set, u32 set_slots, const u32* s, const u32* p /*null: p_const*/, u32 p_const, const u32* o, u32 n, u32* overflow,
+                       int n_sms, cudaStream_t st);
+
+// ---- demand patterns and compaction, shared by kb_datalog.cu and kb_backward.cu
 // whether (s,o) matches one of n demand patterns (x = subject, y = object, KB_ID_NONE = any)
 __device__ __forceinline__ bool bc_demanded(const uint2* dem, u32 n, u32 s, u32 o) {
     for (u32 k = 0; k < n; k++) {
@@ -474,75 +431,20 @@ __device__ __forceinline__ bool bc_demanded(const uint2* dem, u32 n, u32 s, u32 
     }
     return false;
 }
-// out = the rows (s,o) that match one of the n_dem demand patterns, in no particular order; *out_count = their number (zeroed)
-void launch_bc_demand_select(const u32* s, const u32* o, u32 n, const uint2* dem, u32 n_dem, u32* out_s, u32* out_o, u32* out_count,
-                             int n_sms, cudaStream_t st);
-// The answer pass of kb_datalog_query over n rows of (s, p, o) (in[k] null: every row holds cval[k] there): a row matches the query when
-// every constant position holds q_val and every repeated variable holds the value of its first position; the projection onto the
-// query's n_vars distinct variables (out column j = the value at position var_pos[j]) enters a key set (64-bit keys up to 2 variables,
-// 96-bit keys for 3) and is appended to out[] when it was new.
-struct BcAnswerParams {
-    const u32* in[3];
-    u32 cval[3];
-    u32 n;
-    u32 q_is_var[3], q_val[3];  // per position: a variable (q_val = the position of its first appearance) or the constant q_val
-    u32 n_vars, var_pos[3];
-    u64* set64;                 // n_vars <= 2
-    uint4* set96;               // n_vars == 3
-    u32 set_slots;              // power of two
-    u32* out[3];
-    u32 out_cap;
-    u32* out_count;
-    u32* overflow;              // set or output full
-    // kb_datalog_query_repairs (null for kb_datalog_query): a row whose fact (s, p, o) is in the fact set `excl` at a slot whose byte
-    // excl_flag[slot] is non-zero is dropped
-    const uint4* excl;
-    u32 excl_slots;
-    const u8* excl_flag;
-};
-void launch_bc_answer(const BcAnswerParams& p, int n_sms, cudaStream_t st);
-// *found = 1 when (s,o) is a member of the 64-bit set (a one-thread probe)
-void launch_bc_probe(const u64* set, u32 set_slots, u32 s, u32 o, u32* found, cudaStream_t st);
-void launch_set_insert(uint4* set, u32 set_slots, const u32* s, const u32* p /*null: p_const*/, u32 p_const, const u32* o, u32 n, u32* overflow,
-                       int n_sms, cudaStream_t st);
-
-// ---- delete-and-rederive maintenance of a closed store (kb_datalog_maintain)
-// An erased key of a 64-bit (s,o) set: lookups walk past it, inserts never reuse it (s = KB_ID_NONE is never a fact). The set is rebuilt
-// from its relation when it fills up, which drops the tombstones.
-constexpr u64 TOMB64 = 0xFFFFFFFFFFFFFFFEull;
-// base multiplicity of a predicate's facts: a 64-bit (s,o) key table and a parallel u32 count per slot (a key whose count is 0 is not a
-// base fact; it keeps its slot until the table is rehashed)
-struct BaseCountParams {
-    u64* keys;
-    u32* cnt;
-    u32 slots;  // power of two
-    const u32 *s, *o;
-    u32 n;
-    int delta;  // +1: the rows join the base (a count that leaves 0 emits the fact), -1: they leave it (a count that reaches 0 emits it)
-    u32 *out_s, *out_o;  // nullable: no emission (the facts that crossed zero are then only counted)
-    u32* out_count;      // facts that crossed zero
-    u32* claimed;        // keys that took a free slot of the table
-    u32* overflow;       // 1: key table full
-};
-void launch_base_count(const BaseCountParams& p, int n_sms, cudaStream_t st);
-// live entries (count > 0) of one count table into an empty larger one; *n_live += entries moved
-void launch_base_count_rehash(const u64* okeys, const u32* ocnt, u32 oslots, u64* nkeys, u32* ncnt, u32 nslots, u32* n_live, u32* overflow, int n_sms,
-                              cudaStream_t st);
-// rows (s,o) whose presence in a 64-bit set equals keep_present go to out (warp-aggregated compaction, order not kept). With `cnt` the
-// set is a count table and a key is present only with a positive count.
-struct PairSelectParams {
-    const u32 *s, *o;
-    u32 n;
-    const u64* keys;
-    const u32* cnt;
-    u32 slots;
-    u32 keep_present;
-    u32 *out_s, *out_o;
-    u32* out_count;
-};
-void launch_pair_select(const PairSelectParams& p, int n_sms, cudaStream_t st);
-// the keys (s,o) of the rows become TOMB64 in the set (keys that are not there are ignored)
-void launch_set64_erase(u64* set, u32 set_slots, const u32* s, const u32* o, u32 n, int n_sms, cudaStream_t st);
+// warp-aggregated append of (s,o) for the lanes that `take` it, at *out_count (every lane of the warp calls it)
+__device__ __forceinline__ void emit_pair(bool take, u32 s, u32 o, u32* out_s, u32* out_o, u32* out_count) {
+    const int lane = threadIdx.x & 31;
+    const unsigned b = __ballot_sync(0xffffffffu, take);
+    if (!b) return;
+    u32 basepos = 0;
+    if (lane == __ffs(b) - 1) basepos = atomicAdd(out_count, (u32)__popc(b));
+    basepos = __shfl_sync(0xffffffffu, basepos, __ffs(b) - 1);
+    if (take) {
+        const u32 r = basepos + (u32)__popc(b & ((1u << lane) - 1u));
+        out_s[r] = s;
+        out_o[r] = o;
+    }
+}
 
 // fused partition + transfer of the multi-GPU join-key shuffle: a tile of rows is sorted by destination rank d = shard_of(key, n_parts)
 // in shared memory, one range per (tile, destination) is reserved with an atomicAdd on *cursor_ptrs[d] — the destination's own cursor
