@@ -171,6 +171,11 @@ struct PredSlice {  // one predicate's (subject, object) rows of the store — t
     Buf xkey;                // value ranks in TABLE order: xkey[compact(subject) - xtab_min] = rank of num_or0[object] in the context's value
     u64 xkey_version = 0;    // order (kb_numrank.cuh; built with xtab by kb_store_build_index when the slice has numeric objects; the
                              // table-mode probe filters on it sequentially, 4 bytes a slot)
+    // one-byte codes in TABLE order when the subject table holds at most CODE_MAX distinct objects: xcode[slot] = index of xtab[slot]
+    // in xdict (the objects, ascending), 0xFF where xtab holds EMPTY32. Built by kb_store_build_index only and dropped by every store
+    // mutation (bump_version): xtab stays what the maintenance writes and every other reader reads; the index probe reads xcode.
+    Buf xcode, xdict;
+    u32 n_xdict = 0;
     Buf xoff, xval, yoff, yval;
     u32 xcsr_min = 0, xcsr_range = 0, ycsr_min = 0, ycsr_range = 0;
     const SliceChunk* single() const { return chunks.size() == 1 ? &chunks[0] : nullptr; }

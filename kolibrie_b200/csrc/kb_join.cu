@@ -474,6 +474,11 @@ static DirectTab persistent_tab(const PredSlice& s, bool key_is_y) {
     D.kmin = key_is_y ? s.ytab_min : s.xtab_min;
     D.range = key_is_y ? s.ytab_range : s.xtab_range;
     D.cshift = key_is_y ? 0u : s.tab_cshift;
+    if (!key_is_y && s.xcode) {
+        D.code = static_cast<const u8*>(s.xcode->p);
+        D.dict = static_cast<const u32*>(s.xdict->p);
+        D.n_dict = s.n_xdict;
+    }
     return D;
 }
 

@@ -164,36 +164,80 @@ void launch_build_direct_pairs_filtered(const BuildPairsParams& p, int n_sms, cu
     else build_pairs_filtered_kernel<false><<<grid, 256, 0, st>>>(p);
 }
 
-__global__ void __launch_bounds__(256) distinct_kernel(const u32* __restrict__ col, u32 n, u32* set, u32 set_slots, u32* overflow) {
+// ctrl = {overflow, values inserted}. A value already in the set costs a plain load, never an atomic: a column of a few values
+// repeated millions of times does not serialise on their slots. Every warp stops at its next row once the overflow word is set.
+__global__ void __launch_bounds__(256) distinct_kernel(const u32* __restrict__ col, u32 n, u32* set, u32 set_slots, u32 limit, u32* ctrl) {
     const int lane = threadIdx.x & 31;
     const u32 mask = set_slots - 1u;
     const u32 n_round = (n + 31u) & ~31u;
     u32 last = EMPTY32;  // values come in long runs in real stores: skip what this lane just inserted
     for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += gridDim.x * blockDim.x) {
+        u32 stop = lane == 0 ? *reinterpret_cast<volatile u32*>(&ctrl[0]) : 0u;
+        if (__shfl_sync(0xffffffffu, stop, 0)) break;
         const bool valid = i < n;
         const u32 v = valid ? col[i] : EMPTY32;
-        const unsigned act = __ballot_sync(0xffffffffu, valid && v != last);
-        if (!(valid && v != last)) continue;
+        const bool fresh = valid && v != EMPTY32 && v != last;
+        const unsigned act = __ballot_sync(0xffffffffu, fresh);
+        if (!fresh) continue;
         const unsigned peers = __match_any_sync(act, v);
         last = v;
         if (lane != __ffs(peers) - 1) continue;
         u32 slot = mix32(v) & mask;
         for (u32 probes = 0;; probes++) {
-            if (probes >= set_slots) { *overflow = 1u; break; }
+            if (probes >= set_slots) { ctrl[0] = 1u; break; }
             const u32 cur = *reinterpret_cast<volatile u32*>(&set[slot]);
             if (cur == v) break;
             if (cur == EMPTY32) {
                 const u32 old = atomicCAS(&set[slot], EMPTY32, v);
-                if (old == EMPTY32 || old == v) break;
+                if (old == EMPTY32) {
+                    if (atomicAdd(&ctrl[1], 1u) >= limit) ctrl[0] = 1u;
+                    break;
+                }
+                if (old == v) break;
             }
             slot = (slot + 1u) & mask;
         }
     }
 }
-void launch_distinct(const u32* col, u32 n, u32* set, u32 set_slots, u32* overflow, int n_sms, cudaStream_t st) {
+void launch_distinct(const u32* col, u32 n, u32* set, u32 set_slots, u32 limit, u32* ctrl, int n_sms, cudaStream_t st) {
     if (n == 0) return;
     int grid = (int)umin64((u64)n_sms * 4ull, ((u64)n + 255ull) / 256ull);
-    distinct_kernel<<<grid, 256, 0, st>>>(col, n, set, set_slots, overflow);
+    distinct_kernel<<<grid, 256, 0, st>>>(col, n, set, set_slots, limit, ctrl);
+}
+
+// one-byte codes of a subject table (PredSlice::xcode): code[i] = index of tab[i] in the ascending dictionary, 0xFF where tab[i] is
+// EMPTY32; four slots per thread, one 16-byte load and one 4-byte store
+__global__ void __launch_bounds__(256) tab_code_kernel(const u32* __restrict__ tab, u32 range, const u32* __restrict__ dict, u32 n_dict,
+                                                       u8* __restrict__ code) {
+    __shared__ u32 s_dict[CODE_MAX];
+    for (u32 i = threadIdx.x; i < n_dict; i += blockDim.x) s_dict[i] = dict[i];
+    __syncthreads();
+    const u32 quads = (range + 3u) / 4u;
+    for (u32 q = blockIdx.x * blockDim.x + threadIdx.x; q < quads; q += gridDim.x * blockDim.x) {
+        const uint4 v4 = __ldg(reinterpret_cast<const uint4*>(tab) + q);  // (the buffer is padded past the table's last slot)
+        const u32 v[4] = {v4.x, v4.y, v4.z, v4.w};
+        u32 packed = 0;
+#pragma unroll
+        for (u32 k = 0; k < 4; k++) {
+            u32 c = 0xFFu;
+            if (4u * q + k < range && v[k] != EMPTY32) {
+                u32 lo = 0, hi = n_dict;  // the first entry >= v: v is in the dictionary
+                while (lo < hi) {
+                    const u32 mid = (lo + hi) / 2u;
+                    if (s_dict[mid] < v[k]) lo = mid + 1u;
+                    else hi = mid;
+                }
+                c = lo;
+            }
+            packed |= c << (8u * k);
+        }
+        reinterpret_cast<u32*>(code)[q] = packed;
+    }
+}
+void launch_tab_code(const u32* tab, u32 range, const u32* dict, u32 n_dict, u8* code, int n_sms, cudaStream_t st) {
+    if (range == 0) return;
+    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)range + 1023ull) / 1024ull);
+    tab_code_kernel<<<grid, 256, 0, st>>>(tab, range, dict, n_dict, code);
 }
 
 // One pass over a new segment: id range of the three columns, subjects that belong to another shard, and the segment's distinct
@@ -781,6 +825,13 @@ __global__ void __launch_bounds__(PROBEF_THREADS, KB_PI_MINB) probe_index_kernel
         }
     }
     __shared__ u32 s_tcnt[2];  // rows in the staged tile
+    // dictionaries of the coded tables (DirectTab::code): entry 0xFF is EMPTY32, so a code decodes with one shared load (the barrier
+    // after the stage set-up below publishes them)
+    __shared__ u32 s_dict[T][256];
+#pragma unroll
+    for (int t = 0; t < T; t++)
+        if (P.tab[t].code) s_dict[t][tid] = (u32)tid < P.tab[t].n_dict ? P.tab[t].dict[tid] : EMPTY32;
+    static_assert(PROBEF_THREADS == 256, "one dictionary entry per thread");
     auto issue = [&](u32 t, u32 stage) {
         u32* smem = smem_all + stage * STAGE_WORDS;
         u64& bar = bars[stage];
@@ -886,16 +937,32 @@ __global__ void __launch_bounds__(PROBEF_THREADS, KB_PI_MINB) probe_index_kernel
                 }
             }
         }
+        // a coded table (warp-uniform) is read one byte a slot: a warp's 32 consecutive keys are one sector instead of four. Every
+        // load is issued before the first code is decoded
         u32 tv[R][T];
 #pragma unroll
-        for (int j = 0; j < R; j++) {
-            const u32 key = P.key_is_y ? ry[j] : rx[j];
+        for (int t = 0; t < T; t++) {
+            const DirectTab& D = P.tab[t];
+            if (D.code) {
 #pragma unroll
-            for (int t = 0; t < T; t++) {
-                const u32 off = compact_key(key, P.tab[t].cshift) - P.tab[t].kmin;
-                tv[j][t] = (((vmask >> j) & 1u) && off < P.tab[t].range) ? __ldg(P.tab[t].tab + off) : EMPTY32;
+                for (int j = 0; j < R; j++) {
+                    const u32 off = compact_key(P.key_is_y ? ry[j] : rx[j], D.cshift) - D.kmin;
+                    tv[j][t] = (((vmask >> j) & 1u) && off < D.range) ? (u32)__ldg(D.code + off) : 0xFFu;
+                }
+            } else {
+#pragma unroll
+                for (int j = 0; j < R; j++) {
+                    const u32 off = compact_key(P.key_is_y ? ry[j] : rx[j], D.cshift) - D.kmin;
+                    tv[j][t] = (((vmask >> j) & 1u) && off < D.range) ? __ldg(D.tab + off) : EMPTY32;
+                }
             }
         }
+#pragma unroll
+        for (int t = 0; t < T; t++)
+            if (P.tab[t].code) {
+#pragma unroll
+                for (int j = 0; j < R; j++) tv[j][t] = s_dict[t][tv[j][t]];
+            }
         u32 m = 0;
 #pragma unroll
         for (int j = 0; j < R; j++) {

@@ -50,6 +50,7 @@ constexpr int PROBE_ITEMS = 4;
 constexpr int PROBE_TILE = PROBE_THREADS * PROBE_ITEMS;  // 1024 rows
 constexpr int MAXT = 4;
 
+constexpr u32 CODE_MAX = 255;  // objects a subject table may hold to be coded in one byte per slot (code 0xFF: no object)
 struct DirectTab {
     const u32* tab;
     u32 kmin, range;  // in compacted key space when cshift != 0
@@ -57,6 +58,11 @@ struct DirectTab {
     u32 mode;  // 0: payload is a value column  1: payload is a build-row index (gather pay[])  2: existence only
     u32 n_pay;
     const u32* pay[2];
+    // non-null: the table's one-byte codes (PredSlice::xcode), which probe_index_kernel reads instead of tab: code[slot] indexes dict
+    // (n_dict <= CODE_MAX object ids), 0xFF where tab holds EMPTY32. The other kernels read tab.
+    const u8* code;
+    const u32* dict;
+    u32 n_dict;
 };
 enum : u32 { OUT_PROBE = 0, OUT_TABVAL = 1, OUT_TABPAY = 2 };
 struct OutCol {
@@ -164,8 +170,12 @@ struct BuildPairsParams {
     u32* count;  // rows inserted (after the filter)
 };
 void launch_build_direct_pairs_filtered(const BuildPairsParams& p, int n_sms, cudaStream_t st);
-// distinct values of a column into a small open-addressing set (EMPTY32 = free); *overflow set when it fills up
-void launch_distinct(const u32* col, u32 n, u32* set, u32 set_slots, u32* overflow, int n_sms, cudaStream_t st);
+// distinct values of a column other than EMPTY32 into a small open-addressing set (EMPTY32 = free). ctrl = {overflow, count}, both 0
+// at launch: the overflow word is set when the set fills up or when a value past the first `limit` arrives, and ends the pass
+void launch_distinct(const u32* col, u32 n, u32* set, u32 set_slots, u32 limit, u32* ctrl, int n_sms, cudaStream_t st);
+// code[i] = index of tab[i] in dict (ascending, every value of tab but EMPTY32, n_dict <= CODE_MAX), 0xFF where tab[i] is EMPTY32, for
+// i < range; tab and code start 16-byte aligned and may be read / written up to the next multiple of 4 slots
+void launch_tab_code(const u32* tab, u32 range, const u32* dict, u32 n_dict, u8* code, int n_sms, cudaStream_t st);
 
 // ---- window-slide maintenance of the store index: ONE pass profiles a new segment (column ranges, foreign subjects, its distinct
 // predicates with their row counts), ONE pass splits it into the predicate slices' new chunks — pairs, id ranges, typed literal

@@ -63,6 +63,50 @@ static kb_status build_rank_column(kb_ctx* ctx, PredSlice& ps) {
     return KB_OK;
 }
 
+// the one-byte codes of every subject table that holds at most CODE_MAX distinct objects (PredSlice::xcode): one distinct pass per
+// table, which ends early past CODE_MAX values, one read-back for all of them, the dictionaries sorted here (codes ascend with the
+// object ids), one code pass per coded table
+static kb_status build_subject_codes(kb_ctx* ctx) {
+    constexpr u32 SLOTS = 512;  // the distinct set: at most half full below the limit
+    std::vector<PredSlice*> tabs;
+    for (auto& kv : ctx->index) if (kv.second.xtab) tabs.push_back(&kv.second);
+    if (tabs.empty()) return KB_OK;
+    const size_t n = tabs.size();  // <= 4096 slices: 2 control words each fit the arena
+    Buf sets;
+    KB_TRY(alloc_buf(ctx, n * SLOTS * sizeof(u32), &sets));
+    KB_CUDA(ctx, cudaMemsetAsync(sets->p, 0xFF, n * SLOTS * sizeof(u32), ctx->st));
+    const u32 off = ctrl_alloc(ctx, 2 * (u32)n);
+    KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, 2 * n * sizeof(u32), ctx->st));
+    for (size_t i = 0; i < n; i++) {
+        launch_distinct(static_cast<const u32*>(tabs[i]->xtab->p), tabs[i]->xtab_range, static_cast<u32*>(sets->p) + i * SLOTS, SLOTS, CODE_MAX,
+                        ctx->ctrl + off + 2 * i, ctx->n_sms, ctx->st);
+        ctx->stats.kernel_launches++;
+    }
+    KB_CUDA(ctx, cudaGetLastError());
+    std::vector<u32> h(n * SLOTS);
+    KB_CUDA(ctx, cudaMemcpyAsync(h.data(), sets->p, n * SLOTS * sizeof(u32), cudaMemcpyDeviceToHost, ctx->st));
+    ctx->stats.d2h_bytes += n * SLOTS * sizeof(u32);
+    KB_TRY(ctrl_read(ctx));
+    for (size_t i = 0; i < n; i++) {
+        if (ctx->h_ctrl[off + 2 * i]) continue;  // more than CODE_MAX objects
+        std::vector<u32> dict;
+        for (u32 k = 0; k < SLOTS; k++) if (h[i * SLOTS + k] != EMPTY32) dict.push_back(h[i * SLOTS + k]);
+        if (dict.empty()) continue;
+        std::sort(dict.begin(), dict.end());
+        PredSlice& ps = *tabs[i];
+        KB_TRY(alloc_buf(ctx, dict.size() * sizeof(u32), &ps.xdict));
+        KB_CUDA(ctx, cudaMemcpyAsync(ps.xdict->p, dict.data(), dict.size() * sizeof(u32), cudaMemcpyHostToDevice, ctx->st));
+        ctx->stats.h2d_bytes += dict.size() * sizeof(u32);
+        KB_TRY(alloc_buf(ctx, ps.xtab_range, &ps.xcode));
+        launch_tab_code(static_cast<const u32*>(ps.xtab->p), ps.xtab_range, static_cast<const u32*>(ps.xdict->p), (u32)dict.size(),
+                        static_cast<u8*>(ps.xcode->p), ctx->n_sms, ctx->st);
+        ctx->stats.kernel_launches++;
+        ps.n_xdict = (u32)dict.size();
+    }
+    KB_CUDA(ctx, cudaGetLastError());
+    return KB_OK;
+}
+
 // (re)build or extend the persistent table of one column of a slice after `added` (index into ps.chunks; -1: all chunks) arrived.
 // flag_word: control word the insert kernels raise on a duplicate key. Returns through *touched whether a flag has to be read.
 // full_build: called by kb_store_build_index, which builds the rank columns itself once every chunk is in.
@@ -230,7 +274,7 @@ static kb_status index_add_segment(kb_ctx* ctx, size_t seg_idx, bool full_build,
     const u32 off = ctrl_alloc(ctx, 4);
     KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + off, 0, 4 * sizeof(u32), ctx->st));
     timer_begin(ctx, F_OTHER);
-    launch_distinct(sg.p.ptr, (u32)sg.n, static_cast<u32*>(set->p), set_slots, ctx->ctrl + off, ctx->n_sms, ctx->st);
+    launch_distinct(sg.p.ptr, (u32)sg.n, static_cast<u32*>(set->p), set_slots, set_slots, ctx->ctrl + off, ctx->n_sms, ctx->st);
     timer_end(ctx);
     std::vector<u32> hset(set_slots);
     KB_CUDA(ctx, cudaMemcpyAsync(hset.data(), set->p, set_slots * sizeof(u32), cudaMemcpyDeviceToHost, ctx->st));
@@ -376,11 +420,17 @@ static kb_status index_evict(kb_ctx* ctx, Dies dies) {
 static bool index_maintainable(const kb_ctx* ctx) {
     return ctx->index_maintain && ctx->index_version == ctx->store_version && !ctx->index.empty();
 }
-// a new store version: everything keyed to the old one is void, and what the star-join builds learnt about its predicates is forgotten
+// a new store version: everything keyed to the old one is void, and what the star-join builds learnt about its predicates is forgotten.
+// The subject codes go too: they are built by kb_store_build_index only, never maintained.
 static void bump_version(kb_ctx* ctx) {
     ctx->store_version++;
     ctx->multi_valued.clear();
     ctx->single_valued.clear();
+    for (auto& kv : ctx->index) {
+        kv.second.xcode.reset();
+        kv.second.xdict.reset();
+        kv.second.n_xdict = 0;
+    }
 }
 static void drop_index(kb_ctx* ctx) {
     ctx->index.clear();
@@ -727,6 +777,8 @@ kb_status kb_store_build_index(kb_ctx* ctx, uint32_t* n_predicates, double* buil
         if (!ps.xtab || !ctx->n_ids || !ps.typed(ctx->num_version)) continue;
         KB_TRY(kb::build_rank_column(ctx, ps));
     }
+    // one-byte codes for the subject tables of few distinct objects: the index probe looks them up 1 byte a slot instead of 4
+    KB_TRY(kb::build_subject_codes(ctx));
     // key-grouped directories (counting sort by the dense key) for the columns that did not get a direct table
     for (auto& kv : ctx->index) {
         kb::PredSlice& ps = kv.second;
