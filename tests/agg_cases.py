@@ -10,6 +10,8 @@ from __future__ import annotations
 
 import numpy as np
 
+from tests import hash_mirror as M
+
 NAN, INF = float("nan"), float("inf")
 DBL_MAX = float(np.finfo(np.float64).max)
 DBL_MIN = float(np.finfo(np.float64).tiny)
@@ -123,23 +125,7 @@ def group_keys(rng, n_groups: int, edge_keys=(0, 0x7FFFFFFF, 0x80000000, 0xFFFFF
     return np.array(keys, dtype=np.uint32)
 
 
-def mix32(x: np.ndarray) -> np.ndarray:
-    """the murmur3 finaliser of kb_device.cuh, on u32 arrays"""
-    x = np.asarray(x, dtype=np.uint32).copy()
-    x ^= x >> np.uint32(16)
-    x *= np.uint32(0x85EBCA6B)
-    x ^= x >> np.uint32(13)
-    x *= np.uint32(0xC2B2AE35)
-    x ^= x >> np.uint32(16)
-    return x
-
-
-def warp_hash(cols) -> np.ndarray:
-    """group_kernel's in-warp match value of a multi-column key: h = 0; h = mix32(h ^ k[c]) + c"""
-    h = np.zeros(len(cols[0]), dtype=np.uint32)
-    for c, k in enumerate(cols):
-        h = mix32(h ^ np.asarray(k, dtype=np.uint32)) + np.uint32(c)
-    return h
+warp_hash = M.group_kernel_hash  # group_kernel's in-warp match value of a multi-column key
 
 
 def colliding_pair(seed: int = 7):
