@@ -350,6 +350,32 @@ KB_API kb_status kb_serialize_begin(kb_ctx* ctx, uint32_t format, const uint64_t
 KB_API kb_status kb_serialize_next(kb_ctx* ctx, kb_serializer* ser, uint8_t* host_dst, uint64_t capacity, uint64_t* bytes_written);
 KB_API void kb_serialize_free(kb_serializer* ser);
 
+/* ------------------------------------------------------------------ the optimizer's store statistics: DatabaseStats::gather_stats_fast
+ * (kolibrie/src/streamertail_optimizer/stats/database_stats.rs:43-105), what Streamertail's cost estimator reads for every pattern.
+ *   T = the distinct triples of the store's live segments, ascending by (s, p, o) (the BTreeSet<Triple> order kb_serialize_begin writes).
+ *   max_sample > 0: take = min(T, max_sample), step = T / take when T > max_sample, else 1; the sample is the triples at positions
+ *   0, step, ..., (take - 1) * step, and every count is multiplied by step. The triples past (take - 1) * step are never sampled: for
+ *   max_sample < T < 2 * max_sample, step is 1 and only the first max_sample triples are counted. gather_stats_fast is max_sample = 100000.
+ *   max_sample = 0: every triple, step 1 (exact counts).
+ *   The three maps (subjects, predicates, objects) are (id ascending, count) arrays; every u32 id counts, quoted ids included.
+ *   quoted_triple_count = the entries of the quoted-triple table (kb_quoted_load, kb_bind's TRIPLE): QuotedTripleStore::len().
+ * The result is host-resident (kb_db_stats_counts reads it, kb_db_stats_free releases it). The store, its version and its index are left
+ * as they were. The statistics are those of this context's store (on a sharded context: its shard). An empty store needs no dictionary.
+ * Refused: a NULL `out` (KB_E_INVALID); a store of 2^32 - 16 triples or more (KB_E_LIMIT). kb_db_stats_counts: a NULL argument or a
+ * position other than 0 (subject), 1 (predicate), 2 (object) (KB_E_INVALID). Launches and device time count in kb_stats' `other` family. */
+typedef struct kb_db_stats kb_db_stats;
+typedef struct kb_db_stats_info {
+    uint64_t total_triples;       /* T */
+    uint64_t quoted_triple_count; /* entries of the quoted-triple table */
+    uint64_t take;                /* triples sampled */
+    uint64_t step;                /* sampling stride, the factor every count carries */
+    uint64_t n_ids[3];            /* distinct ids in the subject / predicate / object map */
+    double phase_ms[3];           /* device time: sort + dedup, gather, counts */
+} kb_db_stats_info;
+KB_API kb_status kb_store_gather_stats(kb_ctx* ctx, uint64_t max_sample, kb_db_stats** out, kb_db_stats_info* info /* nullable */);
+KB_API kb_status kb_db_stats_counts(const kb_db_stats* st, uint32_t position, const uint32_t** ids, const uint64_t** counts, uint64_t* n);
+KB_API void kb_db_stats_free(kb_db_stats* st);
+
 /* ------------------------------------------------------------------ BIND: `PhysicalOperator::Bind` with the built-in functions of
  * ExecutionEngine::execute_with_ids (kolibrie/src/streamertail_optimizer/execution/engine.rs:144-277) over the rows of `in`, in the order
  * they lie. *out = `in` with the output column: appended when out_slot is not a column of `in`, else that column replaced (the other

@@ -173,6 +173,20 @@ class KbSerializeInfo(C.Structure):
         return {n: (list(getattr(self, n)) if n == "phase_ms" else int(getattr(self, n))) for n, _ in self._fields_}
 
 
+class KbDbStatsInfo(C.Structure):
+    """kb_db_stats_info: distinct triples T, quoted-triple entries, the sample (take rows every step-th), distinct ids per position
+    (subject, predicate, object) and the device time of the phases (sort + dedup, gather, counts)"""
+    _fields_ = [("total_triples", C.c_uint64), ("quoted_triple_count", C.c_uint64), ("take", C.c_uint64), ("step", C.c_uint64),
+                ("n_ids", C.c_uint64 * 3), ("phase_ms", C.c_double * 3)]
+
+    def as_dict(self):
+        return {n: ([int(x) for x in getattr(self, n)] if n == "n_ids" else list(getattr(self, n)) if n == "phase_ms" else int(getattr(self, n)))
+                for n, _ in self._fields_}
+
+
+GATHER_STATS_FAST = 100000  # gather_stats_fast's sample size (database_stats.rs:50)
+
+
 KB_BGP_MAX_PATTERNS = 16
 BGP_NONE, BGP_STAR, BGP_COMPONENTS = 0, 1, 2  # kb_bgp_route
 
@@ -311,6 +325,9 @@ def lib() -> C.CDLL:
         "kb_serialize_begin": (i32, [vp, u32, vp, vp, u32, P(vp), P(KbSerializeInfo)]),
         "kb_serialize_next": (i32, [vp, vp, vp, u64, P(u64)]),
         "kb_serialize_free": (None, [vp]),
+        "kb_store_gather_stats": (i32, [vp, u64, P(vp), P(KbDbStatsInfo)]),
+        "kb_db_stats_counts": (i32, [vp, u32, P(P(u32)), P(P(u64)), P(u64)]),
+        "kb_db_stats_free": (None, [vp]),
         "kb_bind": (i32, [vp, vp, P(KbBindSpec), P(vp), P(KbBindInfo)]),
         "kb_rel_info": (i32, [vp, P(u64), P(u32), P(u32)]),
         "kb_rel_download": (i32, [vp, vp, u32, vp]),
@@ -382,7 +399,7 @@ def lib() -> C.CDLL:
 EXPORTED_SYMBOLS = [
     "kb_version", "kb_ctx_create", "kb_ctx_destroy", "kb_last_error", "kb_set_timing", "kb_get_stats", "kb_synchronize",
     "kb_store_load", "kb_store_load_device", "kb_store_append", "kb_store_append_device", "kb_store_evict", "kb_store_delete", "kb_store_insert", "kb_store_remove", "kb_store_remove_template", "kb_store_clear", "kb_store_build_index", "kb_set_use_index", "kb_store_size",
-    "kb_store_download", "kb_dict_numeric_load", "kb_dict_legacy_i32_load", "kb_dict_numeric_derive", "kb_dict_numeric_download", "kb_dict_strings_load", "kb_dict_encode", "kb_dict_strings_info", "kb_rel_decode", "kb_strings_info", "kb_strings_download", "kb_strings_free", "kb_quoted_load", "kb_quoted_download", "kb_dict_strings_download", "kb_serialize_begin", "kb_serialize_next", "kb_serialize_free", "kb_bind", "kb_rel_info", "kb_rel_download", "kb_rel_device_col", "kb_rel_from_host",
+    "kb_store_download", "kb_dict_numeric_load", "kb_dict_legacy_i32_load", "kb_dict_numeric_derive", "kb_dict_numeric_download", "kb_dict_strings_load", "kb_dict_encode", "kb_dict_strings_info", "kb_rel_decode", "kb_strings_info", "kb_strings_download", "kb_strings_free", "kb_quoted_load", "kb_quoted_download", "kb_dict_strings_download", "kb_serialize_begin", "kb_serialize_next", "kb_serialize_free", "kb_store_gather_stats", "kb_db_stats_counts", "kb_db_stats_free", "kb_bind", "kb_rel_info", "kb_rel_download", "kb_rel_device_col", "kb_rel_from_host",
     "kb_rel_from_device", "kb_rel_free", "kb_scan", "kb_filter", "kb_project", "kb_hash_join", "kb_natural_join", "kb_hash_join_keyed", "kb_values", "kb_bind_join", "kb_scan_quoted", "kb_star_join", "kb_bgp_execute", "kb_bgp_last_plan",
     "kb_order_by", "kb_group_aggregate", "kb_groups_info", "kb_groups_keys", "kb_groups_values", "kb_groups_counts", "kb_groups_free", "kb_groups_pack", "kb_groups_merge", "kb_star_join_aggregate",
     "kb_star_join_prepare", "kb_plan_submit", "kb_plan_collect", "kb_plan_info", "kb_plan_free", "kb_plan_peer_scratch_bytes", "kb_plan_attach_peers",
@@ -690,6 +707,24 @@ class Context:
                 yield buf[: got.value].tobytes()
         finally:
             lib().kb_serialize_free(h)
+
+    def store_gather_stats(self, max_sample: int = GATHER_STATS_FAST) -> dict:
+        """kb_store_gather_stats: DatabaseStats::gather_stats_fast over the store's distinct triples, sampling at most max_sample of
+        them (0: every triple). Returns kb_db_stats_info as a dict plus "subject", "predicate" and "object": (ids uint32, counts uint64),
+        ids ascending, counts already multiplied by the sampling step."""
+        h, inf = C.c_void_p(), KbDbStatsInfo()
+        self._check(lib().kb_store_gather_stats(self.h, max_sample, C.byref(h), C.byref(inf)))
+        try:
+            out = inf.as_dict()
+            for pos, name in enumerate(("subject", "predicate", "object")):
+                ids, counts, n = C.POINTER(C.c_uint32)(), C.POINTER(C.c_uint64)(), C.c_uint64()
+                self._check(lib().kb_db_stats_counts(h, pos, C.byref(ids), C.byref(counts), C.byref(n)))
+                k = n.value
+                out[name] = (np.ctypeslib.as_array(ids, (k,)).copy() if k else np.empty(0, np.uint32),
+                             np.ctypeslib.as_array(counts, (k,)).copy() if k else np.empty(0, np.uint64))
+            return out
+        finally:
+            lib().kb_db_stats_free(h)
 
     # ---- operators
     def bind(self, rel: Relation, function: int, args: Sequence[KbTerm], out_slot: int, next_qt_id: int = 0,

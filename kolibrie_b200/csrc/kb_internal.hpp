@@ -473,6 +473,10 @@ kb_status quoted_encode(kb_ctx* ctx, const u32* const* col, const u32* cval, u32
 // u32 offsets into bytes, compared byte by byte, a proper prefix first): afterwards rank_of[v] is the rank of value v, *n_values the
 // number of distinct values and *rounds the refinement rounds taken (7 bytes of string a round).
 kb_status rank_values(kb_ctx* ctx, u32 d, const unsigned long long* nkey, const u32* str_off, const u8* bytes, u32* rank_of, u32* n_values, u32* rounds);
+// The distinct triples of the store's live segments in ascending (s, p, o) order, the reference's BTreeSet<Triple> order (kb_serialize.cu):
+// *S their subjects, *PO their (p << 32 | o), *n how many. n_raw = the segments' rows, 0 < n_raw < 2^32 - 16 (the caller checks). The
+// buffers hold n_raw entries. One control-arena read; launches count in the `other` family. The store is not changed.
+kb_status store_distinct(kb_ctx* ctx, u64 n_raw, Buf* S, Buf* PO, u32* n);
 // kb_dict_encode's body over a batch already in device memory (kb_dict.cu)
 kb_status dict_encode_device(kb_ctx* ctx, const u64* d_off, const unsigned char* d_bytes, u64 n_terms, u64 total, u32* d_out_ids, u32* n_new,
                              Buf* first_pos);

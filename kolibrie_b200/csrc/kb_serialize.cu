@@ -5,6 +5,7 @@
 // or one triple's share of the Turtle text with its separators):
 //   sort      the live segments' s / p / o gathered into (s, packed p|o) and sorted by two stable LSD radix sorts (p|o first, then s):
 //             ascending (s, p, o), the reference's BTreeSet<Triple> order (triple.rs:13-18); equal neighbours are dropped
+//             (store_distinct, which kb_store_gather_stats shares)
 //   render    every distinct id of the triples rendered once by the decode kernels of kb_rel_decode in their "missing -> empty" mode
 //             (decode_any(..).unwrap_or_default()), with a class byte per term taken from its rendered bytes (starts with "<<", with
 //             "http://" / "https://"); a triple holds the index of its three terms in the sorted distinct ids
@@ -279,45 +280,12 @@ kb_status serialize_begin(kb_ctx* ctx, u32 format, const u64* poff, const u8* pb
     PhaseTimer pt;
     pt.mark(ctx->st);
 
-    // ---- sort + dedup: (s, p|o) sorted by p|o, then stably by s; equal neighbours dropped
-    Buf S, S2, PO, PO2;
-    KB_TRY(alloc_buf(ctx, n_raw * 4, &S));
-    KB_TRY(alloc_buf(ctx, n_raw * 4, &S2));
-    KB_TRY(alloc_buf(ctx, n_raw * 8, &PO));
-    KB_TRY(alloc_buf(ctx, n_raw * 8, &PO2));
-    {
-        u64 at = 0;
-        for (const Segment& sg : ctx->segs) {
-            if (!sg.n) continue;
-            if (sg.ready) KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st, sg.ready, 0));
-            timer_begin(ctx, F_OTHER, 1);
-            ser_load_kernel<<<grid_1d(sg.n, ctx->n_sms, ST), ST, 0, ctx->st>>>(sg.s.ptr, sg.p.ptr, sg.o.ptr, sg.n, U(S) + at, U64(PO) + at);
-            timer_end(ctx);
-            at += sg.n;
-        }
-    }
-    const u32 nr = (u32)n_raw;
-    timer_begin(ctx, F_OTHER, 2);
-    KB_TRY(cub_run(ctx, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, U64(PO), U64(PO2), U(S), U(S2), nr, 0, 64, ctx->st); }));
-    KB_TRY(cub_run(ctx, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, U(S2), U(S), U64(PO2), U64(PO), nr, 0, 32, ctx->st); }));
-    timer_end(ctx);
-    Buf keep;
-    KB_TRY(alloc_buf(ctx, n_raw, &keep));
-    const u32 c = ctrl_alloc(ctx, 4);  // [0] distinct triples, [1] distinct terms
-    timer_begin(ctx, F_OTHER, 3);
-    ser_distinct_flags_kernel<<<grid_1d(nr, ctx->n_sms, ST), ST, 0, ctx->st>>>(U(S), U64(PO), nr, static_cast<u8*>(keep->p));
-    KB_TRY(cub_run(ctx, [&](void* t, size_t& b) {
-        return cub::DeviceSelect::Flagged(t, b, U(S), static_cast<const u8*>(keep->p), U(S2), ctx->ctrl + c, nr, ctx->st);
-    }));
-    KB_TRY(cub_run(ctx, [&](void* t, size_t& b) {
-        return cub::DeviceSelect::Flagged(t, b, U64(PO), static_cast<const u8*>(keep->p), U64(PO2), ctx->ctrl + c, nr, ctx->st);
-    }));
-    timer_end(ctx);
-    KB_CUDA(ctx, cudaGetLastError());
-    KB_TRY(ctrl_read(ctx));
-    const u32 n = ctx->h_ctrl[c];
+    // ---- sort + dedup
+    Buf S2, PO2;
+    u32 n = 0;
+    KB_TRY(store_distinct(ctx, n_raw, &S2, &PO2, &n));
     ser->n = n;
-    S.reset(); PO.reset(); keep.reset();
+    const u32 c = ctrl_alloc(ctx, 1);  // distinct terms
     pt.mark(ctx->st);
 
     // ---- render: the distinct ids of the three columns, each rendered once
@@ -329,12 +297,12 @@ kb_status serialize_begin(kb_ctx* ctx, u32 format, const u64* poff, const u8* pb
     timer_begin(ctx, F_OTHER, 3);
     ser_ids_kernel<<<grid_1d(n, ctx->n_sms, ST), ST, 0, ctx->st>>>(U(S2), U64(PO2), n, U(ids));
     KB_TRY(cub_run(ctx, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortKeys(t, b, U(ids), U(sorted_ids), (u32)n3, 0, 32, ctx->st); }));
-    KB_TRY(cub_run(ctx, [&](void* t, size_t& b) { return cub::DeviceSelect::Unique(t, b, U(sorted_ids), U(terms), ctx->ctrl + c + 1, (u32)n3, ctx->st); }));
+    KB_TRY(cub_run(ctx, [&](void* t, size_t& b) { return cub::DeviceSelect::Unique(t, b, U(sorted_ids), U(terms), ctx->ctrl + c, (u32)n3, ctx->st); }));
     timer_end(ctx);
     S2.reset(); PO2.reset(); sorted_ids.reset();
     KB_CUDA(ctx, cudaGetLastError());
     KB_TRY(ctrl_read(ctx));
-    const u32 nu = ctx->h_ctrl[c + 1];
+    const u32 nu = ctx->h_ctrl[c];
     info->n_terms = nu;
     KB_TRY(decode_ids(ctx, U(terms), nu, 0, true, "the store", &ser->toff, &ser->tbytes, nullptr));
     KB_TRY(alloc_buf(ctx, (size_t)nu + 16, &ser->tcls));
@@ -462,6 +430,52 @@ kb_status serialize_next(kb_ctx* ctx, kb_serializer* ser, u8* dst, u64 capacity,
 }
 
 }  // namespace
+
+kb_status store_distinct(kb_ctx* ctx, u64 n_raw, Buf* S_out, Buf* PO_out, u32* n_out) {
+    auto U = [](const Buf& b) { return static_cast<u32*>(b->p); };
+    auto U64 = [](const Buf& b) { return static_cast<unsigned long long*>(b->p); };
+    // (s, p|o) sorted by p|o, then stably by s; equal neighbours dropped
+    Buf S, S2, PO, PO2;
+    KB_TRY(alloc_buf(ctx, n_raw * 4, &S));
+    KB_TRY(alloc_buf(ctx, n_raw * 4, &S2));
+    KB_TRY(alloc_buf(ctx, n_raw * 8, &PO));
+    KB_TRY(alloc_buf(ctx, n_raw * 8, &PO2));
+    {
+        u64 at = 0;
+        for (const Segment& sg : ctx->segs) {
+            if (!sg.n) continue;
+            if (sg.ready) KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st, sg.ready, 0));
+            timer_begin(ctx, F_OTHER, 1);
+            ser_load_kernel<<<grid_1d(sg.n, ctx->n_sms, ST), ST, 0, ctx->st>>>(sg.s.ptr, sg.p.ptr, sg.o.ptr, sg.n, U(S) + at, U64(PO) + at);
+            timer_end(ctx);
+            at += sg.n;
+        }
+    }
+    const u32 nr = (u32)n_raw;
+    timer_begin(ctx, F_OTHER, 2);
+    KB_TRY(cub_run(ctx, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, U64(PO), U64(PO2), U(S), U(S2), nr, 0, 64, ctx->st); }));
+    KB_TRY(cub_run(ctx, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, U(S2), U(S), U64(PO2), U64(PO), nr, 0, 32, ctx->st); }));
+    timer_end(ctx);
+    Buf keep;
+    KB_TRY(alloc_buf(ctx, n_raw, &keep));
+    const u32 c = ctrl_alloc(ctx, 1);  // distinct triples
+    timer_begin(ctx, F_OTHER, 3);
+    ser_distinct_flags_kernel<<<grid_1d(nr, ctx->n_sms, ST), ST, 0, ctx->st>>>(U(S), U64(PO), nr, static_cast<u8*>(keep->p));
+    KB_TRY(cub_run(ctx, [&](void* t, size_t& b) {
+        return cub::DeviceSelect::Flagged(t, b, U(S), static_cast<const u8*>(keep->p), U(S2), ctx->ctrl + c, nr, ctx->st);
+    }));
+    KB_TRY(cub_run(ctx, [&](void* t, size_t& b) {
+        return cub::DeviceSelect::Flagged(t, b, U64(PO), static_cast<const u8*>(keep->p), U64(PO2), ctx->ctrl + c, nr, ctx->st);
+    }));
+    timer_end(ctx);
+    KB_CUDA(ctx, cudaGetLastError());
+    KB_TRY(ctrl_read(ctx));
+    *n_out = ctx->h_ctrl[c];
+    *S_out = S2;
+    *PO_out = PO2;
+    return KB_OK;
+}
+
 }  // namespace kb
 
 extern "C" {

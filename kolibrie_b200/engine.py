@@ -467,6 +467,7 @@ class SparqlDatabase:
         self._version = 0
         self._uploaded_quoted = -1  # size of the quoted-triple store the context's table was loaded from
         self.prefixes: List[Tuple[str, str]] = []  # sparql_database.rs:54, ordered: the Turtle header lists them in this order
+        self.cached_stats = None  # sparql_database.rs:58: get_or_build_stats fills it, invalidate_stats_cache empties it
 
     def encode_term(self, t) -> int:
         """a term given as a string, or as a nested (s, p, o) tuple for a quoted triple `<< s p o >>` (components encoded first, in
@@ -520,6 +521,28 @@ class SparqlDatabase:
             preds = groups[s]
             out.append(subj(s) + " ;\n    ".join(f" <{p}>"[i > 0:] + " ,".join(" " + obj(o) for o in preds[p]) for i, p in enumerate(sorted(preds))) + " .\n")
         return "".join(out)
+
+    def get_or_build_stats(self):
+        """SparqlDatabase::get_or_build_stats (sparql_database.rs:197-205): the cached planner.DatabaseStats, or a new one from
+        DatabaseStats::gather_stats_fast, gathered on the device (kb_store_gather_stats) and cached. As in the reference, a later change
+        to the triples does not refresh the cache: call invalidate_stats_cache() after one, as the reference's INSERT / DELETE do."""
+        if self.cached_stats is None:
+            from . import planner
+
+            if hasattr(self.ctx, "store_gather_stats"):
+                self._sync()
+                g = self.ctx.store_gather_stats(c.GATHER_STATS_FAST)
+                maps = [dict(zip(g[k][0].tolist(), g[k][1].tolist())) for k in ("subject", "predicate", "object")]
+                total, quoted = g["total_triples"], g["quoted_triple_count"]
+            else:  # contexts without it (the oracle): gather_stats_fast over the host set
+                total, quoted = len(self.triples), len(self.quoted_triple_store)
+                maps = _gather_stats_fast(sorted(self.triples), c.GATHER_STATS_FAST)
+            self.cached_stats = planner.DatabaseStats.from_counts(total, maps[1], maps[0], maps[2], quoted_triple_count=quoted)
+        return self.cached_stats
+
+    def invalidate_stats_cache(self):
+        """SparqlDatabase::invalidate_stats_cache (sparql_database.rs:207-209): the next get_or_build_stats gathers again"""
+        self.cached_stats = None
 
     def add_statement(self, s, p, o):
         """add one triple whose terms are strings or nested tuples (quoted triples)"""
@@ -742,6 +765,19 @@ class SparqlDatabase:
         comp = np.array(list(qts.id_to_components.values()), dtype=np.uint32).reshape(-1, 3)
         self.ctx.quoted_load(ids, comp[:, 0], comp[:, 1], comp[:, 2])
         self._uploaded_quoted = len(qts)
+
+
+def _gather_stats_fast(triples, max_sample: int):
+    """DatabaseStats::gather_stats_fast's counts (database_stats.rs:43-92) over `triples` in (s, p, o) order: every step-th of the first
+    take * step triples, each counted `step` times; max_sample 0 counts every triple. Returns the subject, predicate and object maps."""
+    total = len(triples)
+    take = min(total, max_sample) if max_sample else total
+    step = total // take if max_sample and total > max_sample else 1
+    maps = ({}, {}, {})
+    for t in triples[: take * step: step]:
+        for m, x in zip(maps, t):
+            m[x] = m.get(x, 0) + step
+    return maps
 
 
 class ExecutionEngine:

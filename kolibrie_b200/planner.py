@@ -113,12 +113,13 @@ class DatabaseStats:
             self.object_card[o] = self.object_card.get(o, 0) + 1
 
     @classmethod
-    def from_counts(cls, total: int, predicate_card: Dict[int, int], subject_card=None, object_card=None):
+    def from_counts(cls, total: int, predicate_card: Dict[int, int], subject_card=None, object_card=None, quoted_triple_count: int = 0):
         st = cls(())
         st.total_triples = total
         st.predicate_card = dict(predicate_card)
         st.subject_card = dict(subject_card or {})
         st.object_card = dict(object_card or {})
+        st.quoted_triple_count = quoted_triple_count
         return st
 
     def get_predicate_cardinality(self, p):

@@ -86,6 +86,12 @@ pub const KB_SER_STAGING_BYTES: u64 = 256 << 20;
 pub type kb_serialize_info = KbSerializeInfo;  // (the header's name, as the declaration below spells it)
 pub enum KbSerializer {}
 pub type kb_serializer = KbSerializer;  // (the header's name, as the declarations below spell it)
+// kb_store_gather_stats / kb_db_stats_counts / kb_db_stats_free: DatabaseStats::gather_stats_fast on the device store
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbDbStatsInfo { pub total_triples: u64, pub quoted_triple_count: u64, pub take: u64,
+    pub step: u64, pub n_ids: [u64; 3], pub phase_ms: [c_double; 3] }
+pub type kb_db_stats_info = KbDbStatsInfo;  // (the header's name, as the declaration below spells it)
+pub enum KbDbStats {}
+pub type kb_db_stats = KbDbStats;  // (the header's name, as the declarations below spell it)
 
 // kb_filter_opcode / kb_cmp / kb_agg_kind / kb_strategy
 pub const KB_F_CMP_NUM: u32 = 1; pub const KB_F_EQ_ID: u32 = 2; pub const KB_F_NE_ID: u32 = 3; pub const KB_F_AND: u32 = 4; pub const KB_F_OR: u32 = 5;
@@ -145,6 +151,9 @@ extern "C" {
                               out: *mut *mut kb_serializer, info: *mut kb_serialize_info) -> kb_status;
     pub fn kb_serialize_next(ctx: *mut KbCtx, ser: *mut kb_serializer, host_dst: *mut u8, capacity: u64, bytes_written: *mut u64) -> kb_status;
     pub fn kb_serialize_free(ser: *mut kb_serializer);
+    pub fn kb_store_gather_stats(ctx: *mut KbCtx, max_sample: u64, out: *mut *mut kb_db_stats, info: *mut kb_db_stats_info) -> kb_status;
+    pub fn kb_db_stats_counts(st: *const kb_db_stats, position: u32, ids: *mut *const u32, counts: *mut *const u64, n: *mut u64) -> kb_status;
+    pub fn kb_db_stats_free(st: *mut kb_db_stats);
     // operators
     pub fn kb_scan(ctx: *mut KbCtx, pats: *const KbPattern, n: u32, pushdown: *const *const KbFilterOp, pushdown_len: *const u32, out: *mut *mut KbRel) -> kb_status;
     pub fn kb_filter(ctx: *mut KbCtx, r: *const KbRel, prog: *const KbFilterOp, n: u32, out: *mut *mut KbRel) -> kb_status;

@@ -241,6 +241,39 @@ impl DeviceStore {
         unsafe { kb_serialize_free(ser) };
         result
     }
+
+    /// `DatabaseStats::gather_stats_fast` (database_stats.rs:43-105) of the device store (`sync` first): `max_sample` 100 000 is the
+    /// reference's sampling, 0 counts every triple. The maps carry the sampling step already; INTEGRATION.md shows how they fill the
+    /// reference's `DatabaseStats` for `Streamertail::with_cached_stats`.
+    pub fn gather_stats(&mut self, max_sample: u64) -> Result<StoreStats, String> {
+        let mut st: *mut kb_db_stats = ptr::null_mut();
+        let mut info = KbDbStatsInfo::default();
+        if unsafe { kb_store_gather_stats(self.ctx, max_sample, &mut st, &mut info) } != KB_OK { return Err(self.last_error()); }
+        let mut maps: [HashMap<u32, u64>; 3] = Default::default();
+        for (pos, map) in maps.iter_mut().enumerate() {
+            let (mut ids, mut counts, mut n): (*const u32, *const u64, u64) = (ptr::null(), ptr::null(), 0);
+            if unsafe { kb_db_stats_counts(st, pos as u32, &mut ids, &mut counts, &mut n) } != KB_OK {
+                unsafe { kb_db_stats_free(st) };
+                return Err("kb_db_stats_counts refused a position".into());
+            }
+            if n > 0 {
+                let (ids, counts) = unsafe { (std::slice::from_raw_parts(ids, n as usize), std::slice::from_raw_parts(counts, n as usize)) };
+                map.extend(ids.iter().copied().zip(counts.iter().copied()));
+            }
+        }
+        unsafe { kb_db_stats_free(st) };
+        let [subject, predicate, object] = maps;
+        Ok(StoreStats { info, subject, predicate, object })
+    }
+}
+
+/// What `DeviceStore::gather_stats` returns: the totals (`info.total_triples`, `info.quoted_triple_count`) and the three cardinality maps
+/// of `DatabaseStats` (database_stats.rs:17-26), counts already scaled by the sampling step.
+pub struct StoreStats {
+    pub info: KbDbStatsInfo,
+    pub subject: HashMap<u32, u64>,
+    pub predicate: HashMap<u32, u64>,
+    pub object: HashMap<u32, u64>,
 }
 
 impl Drop for DeviceStore {
