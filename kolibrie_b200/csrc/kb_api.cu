@@ -1,5 +1,6 @@
 // kb_api.cu — C ABI of libkolibrie_b200.so: context, device triple store, relations and the operator entry points.
-// Host code only orchestrates: every data-touching step is one of the sm_90a kernels in kb_kernels.cu.
+// Host code only orchestrates: every data-touching step is an sm_90a kernel. The ones this file launches, the multi-GPU shuffle's
+// partition, count and fused scatter, are defined here with their launch format.
 #include <cstdarg>
 #include <cstdlib>
 #include <algorithm>
@@ -12,6 +13,259 @@
 using namespace kb;
 
 namespace kb {
+
+// fused partition + transfer of the multi-GPU join-key shuffle: a tile of rows is sorted by destination rank d = shard_of(key, n_parts)
+// in shared memory, one range per (tile, destination) is reserved with an atomicAdd on *cursor_ptrs[d] — the destination's own cursor
+// in peer memory (push mode, base = 0) or a local cursor behind a precomputed base[d] — and the runs are streamed into d's receive
+// buffer (peer memory over NVLink) as 128-byte-aligned warp stores
+struct ShuffleParams {
+    const u32* key;
+    u32 n, n_parts, n_cols;
+    const u32* in[KB_MAX_COLS];
+    u32* const* peer_cols;     // device array [n_parts * n_cols]
+    u32* const* cursor_ptrs;   // device array [n_parts]: word the range of destination d is reserved on
+    const u32* base;           // device array [n_parts]
+    u32 capacity;
+    u32* overflow;
+    u32* ticket;               // zeroed tile counter
+    u32 tile, n_tiles, stride, pow2_mask;  // set by the launcher
+};
+
+// partition rows by mix32(key) % n_parts (multi-GPU shuffle): count then scatter
+
+__global__ void __launch_bounds__(256) part_count_kernel(const u32* key, u32 n, u32 n_parts, u32* counts) {
+    __shared__ u32 sc[64];
+    if (threadIdx.x < 64) sc[threadIdx.x] = 0;
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    const u32 n_round = (n + 31u) & ~31u;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += gridDim.x * blockDim.x) {
+        const bool valid = i < n;
+        const u32 part = valid ? shard_of(key[i], n_parts) : 0xFFFFu;
+        const unsigned act = __ballot_sync(0xffffffffu, valid);
+        if (!valid) continue;
+        // one shared atomic per (warp, destination) instead of one per row: with a handful of destinations the rows of a warp
+        // pile up on a handful of addresses
+        const unsigned peers = __match_any_sync(act, part);
+        if (lane == __ffs(peers) - 1) atomicAdd(&sc[part], (u32)__popc(peers));
+    }
+    __syncthreads();
+    if (threadIdx.x < n_parts && sc[threadIdx.x]) atomicAdd(&counts[threadIdx.x], sc[threadIdx.x]);
+}
+static void launch_part_count(const u32* key, u32 n, u32 n_parts, u32* counts, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    int grid = grid_1d(n, n_sms, 256, 4);
+    part_count_kernel<<<grid, 256, 0, st>>>(key, n, n_parts, counts);
+}
+struct PartScatterParams {
+    const u32* in[KB_MAX_COLS];
+    u32* out[KB_MAX_COLS];
+    u32 n_cols;
+};
+__global__ void __launch_bounds__(256) part_scatter_kernel(const u32* key, u32 n, u32 n_parts, u32* cursors, const PartScatterParams P) {
+    const int lane = threadIdx.x & 31;
+    const u32 n_round = (n + 31u) & ~31u;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += gridDim.x * blockDim.x) {
+        const bool valid = i < n;
+        const u32 part = valid ? shard_of(key[i], n_parts) : 0xFFFFu;
+        const unsigned act = __ballot_sync(0xffffffffu, valid);
+        if (!valid) continue;
+        const unsigned peers = __match_any_sync(act, part);
+        const int leader = __ffs(peers) - 1;
+        u32 basepos = 0;
+        if (lane == leader) basepos = atomicAdd(&cursors[part], (u32)__popc(peers));
+        basepos = __shfl_sync(peers, basepos, leader);
+        const u32 r = basepos + (u32)__popc(peers & ((1u << lane) - 1u));
+        for (u32 c = 0; c < P.n_cols; c++) P.out[c][r] = P.in[c][i];
+    }
+}
+static void launch_part_scatter(const u32* key, u32 n, u32 n_parts, u32* cursors, const u32* const* in_cols, u32* const* out_cols, u32 n_cols,
+                                int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    PartScatterParams P;
+    P.n_cols = n_cols;
+    for (u32 c = 0; c < n_cols; c++) { P.in[c] = in_cols[c]; P.out[c] = out_cols[c]; }
+    int grid = grid_1d(n, n_sms, 256, 4);
+    part_scatter_kernel<<<grid, 256, 0, st>>>(key, n, n_parts, cursors, P);
+}
+
+// Join-key shuffle FUSED with its transfer (SURVEY.md 8e). A CTA takes a tile of rows, sorts it by destination rank in shared memory
+// (histogram -> offsets -> staged columns), reserves ONE range per (tile, destination) in the destination's receive buffer — an
+// atomicAdd on the cursor the destination owns (peer memory: no count pass and no count exchange before the transfer), or on a local
+// cursor when the caller fixed the ranges beforehand — and then streams every (destination, column) run out of shared memory with
+// warp stores whose 32-lane windows are aligned to 128-byte lines of the REMOTE address: NVLink carries full lines, not the 4-byte
+// scatter a row-at-a-time kernel produces.
+// Rows per thread and tile are fixed (8): the keys, the rows' values (NC <= 2 columns: kept in registers from ONE round of independent
+// loads; more columns: re-read when the row is staged), their destination and their rank inside the tile stay in registers from the
+// histogram pass to the staging pass — the first version re-read the inputs and took the ranks with a second round of shared atomics
+// (5.6 warp instructions per row, most stalls on the dependent global loads: far above the HBM floor with all eight destinations
+// LOCAL, i.e. the SM side alone). DIRECT (8 or more destinations): the rank is the
+// return value of a plain shared atomic per row (a warp's 32 rows spread over >= 8 counters: a few passes) instead of match.any +
+// leader election + shuffle (52 instructions per row slot and warp). Flush: the staged run of a destination starts at a shared-memory
+// offset congruent to its place in the receive buffer modulo 16 bytes, so its body goes out as 16-byte vector stores on 128-byte
+// boundaries (512 contiguous bytes per warp instruction: whole NVLink lines), head and tail as one predicated scalar store each.
+constexpr u32 SHUF_ITEMS = 8;
+template <int NC, int THREADS, bool DIRECT>
+__global__ void __launch_bounds__(THREADS) shuffle_scatter_kernel(const __grid_constant__ ShuffleParams P) {
+    extern __shared__ __align__(16) u32 sh_stage[];  // [n_cols][stride] columns sorted by destination
+    __shared__ u32 s_cnt[64], s_off[64], s_gbase[64];
+    __shared__ u32 s_tile;
+    constexpr u32 TILE = SHUF_ITEMS * THREADS;
+    constexpr int NV = NC > 0 ? NC : 1;
+    const u32 STRIDE = P.stride;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const u32 pm = P.pow2_mask;
+    for (;;) {
+        if (tid == 0) s_tile = atomicAdd(P.ticket, 1u);
+        if (tid < 64) s_cnt[tid] = 0u;
+        __syncthreads();
+        const u32 tile = s_tile;
+        if (tile >= P.n_tiles) break;
+        const u32 row0 = tile * TILE;
+        const u32 cnt = min(TILE, P.n - row0);
+        // ---- 0. every load of the tile in flight at once
+        u32 key[SHUF_ITEMS], val[SHUF_ITEMS][NV];
+#pragma unroll
+        for (u32 j = 0; j < SHUF_ITEMS; j++) {
+            const u32 r = j * THREADS + (u32)tid;
+            key[j] = r < cnt ? __ldg(P.key + row0 + r) : 0u;
+        }
+        if (NC > 0) {
+#pragma unroll
+            for (int c = 0; c < NV; c++) {
+                if (P.in[c] == P.key) {
+#pragma unroll
+                    for (u32 j = 0; j < SHUF_ITEMS; j++) val[j][c] = key[j];
+                } else {
+#pragma unroll
+                    for (u32 j = 0; j < SHUF_ITEMS; j++) {
+                        const u32 r = j * THREADS + (u32)tid;
+                        val[j][c] = r < cnt ? __ldg(P.in[c] + row0 + r) : 0u;
+                    }
+                }
+            }
+        }
+        // ---- 1. destinations, histogram, rank of the row among the tile's rows for its destination
+        u32 dest[SHUF_ITEMS], rank[SHUF_ITEMS];
+#pragma unroll
+        for (u32 j = 0; j < SHUF_ITEMS; j++) {
+            const u32 r = j * THREADS + (u32)tid;
+            const bool valid = r < cnt;
+            const u32 blk = key[j] >> SHARD_B;
+            dest[j] = pm ? (blk & pm) : (blk % P.n_parts);  // == shard_of(key, n_parts)
+            rank[j] = 0u;
+            if (DIRECT) {
+                if (valid) rank[j] = atomicAdd(&s_cnt[dest[j]], 1u);
+            } else {
+                const unsigned act = __ballot_sync(0xffffffffu, valid);
+                if (valid) {
+                    const unsigned peers = __match_any_sync(act, dest[j]);
+                    const int leader = __ffs(peers) - 1;
+                    u32 b = 0;
+                    if (lane == leader) b = atomicAdd(&s_cnt[dest[j]], (u32)__popc(peers));
+                    b = __shfl_sync(peers, b, leader);
+                    rank[j] = b + (u32)__popc(peers & ((1u << lane) - 1u));
+                }
+            }
+        }
+        __syncthreads();
+        // ---- 2. one range reservation per destination (remote cursor: the receiver's own word); offsets inside the tile: every
+        // destination gets a 16-byte aligned slot of its count + 8 elements and starts in it at (its place in the receive buffer mod 4)
+        if (warp == 0) {
+            u32 run = 0;
+            for (u32 d0 = 0; d0 < P.n_parts; d0 += 32u) {
+                const u32 d = d0 + (u32)lane;
+                const u32 c = d < P.n_parts ? s_cnt[d] : 0u;
+                const u32 padded = d < P.n_parts ? ((c + 3u + 3u + 3u) & ~3u) : 0u;
+                u32 incl = padded;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) {
+                    const u32 y = __shfl_up_sync(0xffffffffu, incl, o);
+                    if (lane >= o) incl += y;
+                }
+                if (d < P.n_parts) {
+                    u32 g = 0u;
+                    if (c) g = P.base[d] + atomicAdd_system(P.cursor_ptrs[d], c);
+                    if (c && (u64)g + c > (u64)P.capacity) { *P.overflow = 1u; g = EMPTY32; }
+                    s_gbase[d] = g;
+                    s_off[d] = run + incl - padded + (g & 3u);
+                }
+                run += __shfl_sync(0xffffffffu, incl, 31);
+            }
+        }
+        __syncthreads();
+        // ---- 3. stage the columns sorted by destination: position = the destination's offset in the tile + the rank of step 1
+#pragma unroll
+        for (u32 j = 0; j < SHUF_ITEMS; j++) {
+            const u32 r = j * THREADS + (u32)tid;
+            if (r >= cnt) continue;
+            const u32 pos = s_off[dest[j]] + rank[j];
+            if (NC > 0) {
+#pragma unroll
+                for (int c = 0; c < NV; c++) sh_stage[c * STRIDE + pos] = val[j][c];
+            } else {
+                for (u32 c = 0; c < P.n_cols; c++) sh_stage[c * STRIDE + pos] = __ldg(P.in[c] + row0 + r);
+            }
+        }
+        __syncthreads();
+        // ---- 4. flush every (destination, column) run
+        const u32 n_runs = P.n_parts * P.n_cols;
+        for (u32 q = (u32)warp; q < n_runs; q += THREADS / 32) {
+            const u32 d = q / P.n_cols, c = q - d * P.n_cols;
+            const u32 m = s_cnt[d];
+            const u32 g = s_gbase[d];
+            if (m == 0u || g == EMPTY32) continue;
+            u32* dst = P.peer_cols[q] + g;
+            const u32* src = sh_stage + c * STRIDE + s_off[d];
+            const u32 mis = (u32)((reinterpret_cast<uintptr_t>(dst) >> 2) & 31u);  // elements past the previous 128-byte boundary
+            if ((reinterpret_cast<uintptr_t>(P.peer_cols[q]) & 15u) == 0u) {
+                const u32 head = min(m, (32u - mis) & 31u);
+                if ((u32)lane < head) dst[lane] = src[lane];
+                const u32 body = (m - head) >> 2;  // 16-byte vectors, the first one on a 128-byte boundary of the receive buffer
+                const uint4* s4 = reinterpret_cast<const uint4*>(src + head);
+                uint4* d4 = reinterpret_cast<uint4*>(dst + head);
+                for (u32 e = (u32)lane; e < body; e += 32u) d4[e] = s4[e];
+                const u32 t0 = head + (body << 2);
+                if (t0 + (u32)lane < m) dst[t0 + lane] = src[t0 + lane];
+            } else {
+                for (int e0 = -(int)mis; e0 < (int)m; e0 += 32) {
+                    const int e = e0 + lane;
+                    if (e >= 0 && e < (int)m) dst[e] = src[e];
+                }
+            }
+        }
+        __syncthreads();
+    }
+    __threadfence_system();  // the stores must be visible to the peers before the barrier that follows the launch
+}
+template <int NC, int THREADS>
+static void launch_shuffle_t(ShuffleParams p, int n_sms, cudaStream_t st) {
+    p.tile = SHUF_ITEMS * THREADS;
+    p.n_tiles = (p.n + p.tile - 1u) / p.tile;
+    p.stride = (p.tile + 12u * p.n_parts + 3u) & ~3u;
+    p.pow2_mask = (p.n_parts & (p.n_parts - 1u)) == 0u ? p.n_parts - 1u : 0u;
+    if (p.n_parts == 1u) p.pow2_mask = 0u;  // (x % 1 == 0; a zero mask selects the modulo path)
+    const size_t smem = (size_t)p.n_cols * p.stride * sizeof(u32);
+    static const bool direct_env = !(getenv("KOLIBRIE_SHUFFLE_DIRECT") && getenv("KOLIBRIE_SHUFFLE_DIRECT")[0] == '0');
+    if (p.n_parts >= 8u && direct_env) {
+        cudaFuncSetAttribute(shuffle_scatter_kernel<NC, THREADS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
+        const int grid = grid_for((const void*)shuffle_scatter_kernel<NC, THREADS, true>, THREADS, smem, n_sms, p.n_tiles);
+        shuffle_scatter_kernel<NC, THREADS, true><<<grid, THREADS, smem, st>>>(p);
+    } else {
+        cudaFuncSetAttribute(shuffle_scatter_kernel<NC, THREADS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
+        const int grid = grid_for((const void*)shuffle_scatter_kernel<NC, THREADS, false>, THREADS, smem, n_sms, p.n_tiles);
+        shuffle_scatter_kernel<NC, THREADS, false><<<grid, THREADS, smem, st>>>(p);
+    }
+}
+static void launch_shuffle_scatter(const ShuffleParams& p, int n_sms, cudaStream_t st) {
+    if (p.n == 0) return;
+    static const int threads_env = getenv("KOLIBRIE_SHUFFLE_THREADS") ? atoi(getenv("KOLIBRIE_SHUFFLE_THREADS")) : 0;
+    const bool wide = threads_env ? threads_env >= 512 : true;  // 4096-row tiles (512 threads) for the register-resident cases
+    if (p.n_cols == 1) { if (wide) launch_shuffle_t<1, 512>(p, n_sms, st); else launch_shuffle_t<1, 256>(p, n_sms, st); }
+    else if (p.n_cols == 2) { if (wide) launch_shuffle_t<2, 512>(p, n_sms, st); else launch_shuffle_t<2, 256>(p, n_sms, st); }
+    else if (p.n_cols <= 6) launch_shuffle_t<0, 512>(p, n_sms, st);  // <= 6 x (4096 + 768) x 4 B = 114 KB of staging
+    else launch_shuffle_t<0, 128>(p, n_sms, st);                    // 16 columns x (1024 + 768) x 4 B = 112 KB
+}
 
 static std::string g_create_err;
 

@@ -38,7 +38,7 @@ static __global__ void __launch_bounds__(256) set64_insert_kernel(u64* set, u32 
 }
 static void launch_set64_insert(u64* set, u32 set_slots, const u32* s, const u32* o, u32 n, u32* overflow, int n_sms, cudaStream_t st) {
     if (n == 0) return;
-    int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull);
+    int grid = grid_1d(n, n_sms);
     set64_insert_kernel<<<grid, 256, 0, st>>>(set, set_slots, s, o, n, overflow);
 }
 
@@ -403,7 +403,7 @@ static void launch_derive_partitioned(const DerivePartParams& p, int n_sms, cuda
 
 static void launch_derive(const DeriveParams& p, int n_sms, cudaStream_t st) {
     if (p.n == 0) return;
-    int grid = (int)umin64((u64)n_sms * 8ull, ((u64)p.n + 255ull) / 256ull);
+    int grid = grid_1d(p.n, n_sms);
     if (p.gate_set || p.veto_keys || p.demand) derive_kernel<true><<<grid, 256, 0, st>>>(p);
     else derive_kernel<false><<<grid, 256, 0, st>>>(p);
 }
@@ -470,7 +470,7 @@ static __global__ void __launch_bounds__(256) base_count_kernel(const __grid_con
 }
 static void launch_base_count(const BaseCountParams& p, int n_sms, cudaStream_t st) {
     if (p.n == 0) return;
-    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)p.n + 255ull) / 256ull);
+    const int grid = grid_1d(p.n, n_sms);
     base_count_kernel<<<grid, 256, 0, st>>>(p);
 }
 
@@ -496,7 +496,7 @@ static __global__ void __launch_bounds__(256) base_count_rehash_kernel(const u64
 static void launch_base_count_rehash(const u64* okeys, const u32* ocnt, u32 oslots, u64* nkeys, u32* ncnt, u32 nslots, u32* n_live, u32* overflow, int n_sms,
                               cudaStream_t st) {
     if (oslots == 0) return;
-    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)oslots + 255ull) / 256ull);
+    const int grid = grid_1d(oslots, n_sms);
     base_count_rehash_kernel<<<grid, 256, 0, st>>>(okeys, ocnt, oslots, nkeys, ncnt, nslots, n_live, overflow);
 }
 
@@ -530,7 +530,7 @@ static __global__ void __launch_bounds__(256) pair_select_kernel(const __grid_co
 }
 static void launch_pair_select(const PairSelectParams& p, int n_sms, cudaStream_t st) {
     if (p.n == 0) return;
-    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)p.n + 255ull) / 256ull);
+    const int grid = grid_1d(p.n, n_sms);
     pair_select_kernel<<<grid, 256, 0, st>>>(p);
 }
 
@@ -544,7 +544,7 @@ static __global__ void __launch_bounds__(256) set64_erase_kernel(u64* set, u32 s
 }
 static void launch_set64_erase(u64* set, u32 set_slots, const u32* s, const u32* o, u32 n, int n_sms, cudaStream_t st) {
     if (n == 0) return;
-    const int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n + 255ull) / 256ull);
+    const int grid = grid_1d(n, n_sms);
     set64_erase_kernel<<<grid, 256, 0, st>>>(set, set_slots, s, o, n);
 }
 

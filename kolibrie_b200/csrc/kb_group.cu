@@ -37,7 +37,7 @@ __global__ void __launch_bounds__(256) group_merge_kernel(const __grid_constant_
 }
 void launch_group_merge(const GroupParams& p, const GroupRecord* recs, u32 n, int n_sms, cudaStream_t st) {
     if (n == 0) return;
-    const int grid = (int)umin64((u64)n_sms * 4ull, ((u64)n + 255ull) / 256ull);
+    const int grid = grid_1d(n, n_sms, 256, 4);
     group_merge_kernel<<<grid, 256, 0, st>>>(p, recs, n);
 }
 
@@ -297,7 +297,7 @@ void launch_group(const GroupParams& p, int n_sms, cudaStream_t st) {
     if (p.n == 0) return;
     if (p.n_gcols == 1 && p.n_aggs <= 1) {
         // a CTA's 32-bit shared counters see at most n / grid * ... rows: far below 2^32
-        int grid = (int)umin64((u64)n_sms * 8ull, ((u64)p.n + 1023ull) / 1024ull);
+        int grid = grid_1d(p.n, n_sms, 1024);
         const u32 kind = (p.n_aggs == 0 || p.akind[0] == KB_AGG_COUNT) ? 0u : p.akind[0];
         switch (kind) {
             case 0: group1_kernel<0><<<grid, 256, 0, st>>>(p); break;
@@ -308,7 +308,7 @@ void launch_group(const GroupParams& p, int n_sms, cudaStream_t st) {
         }
         return;
     }
-    int grid = (int)umin64((u64)n_sms * 8ull, ((u64)p.n + 255ull) / 256ull);
+    int grid = grid_1d(p.n, n_sms);
     group_kernel<<<grid, 256, 0, st>>>(p);
 }
 

@@ -1,5 +1,5 @@
 // kb_group.cuh — the device side of the GROUP BY hash table that the group kernels (kb_group.cu) and the index probe's fused GROUP BY
-// (probe_index_kernel, kb_kernels.cu) both insert into.
+// (probe_index_kernel, kb_join.cu) both insert into.
 #pragma once
 #include "kb_kernels.cuh"
 

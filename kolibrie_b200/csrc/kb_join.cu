@@ -1,11 +1,1467 @@
 // kb_join.cu — the join operators: FILTER, the natural join (cartesian, grouped, chained), the star join's routes R1-R5, the
-// one-kernel index plan and the bind join; and what every compacting launch shares (tile state, epoch, control words).
+// one-kernel index plan and the bind join; and what every compacting launch shares (tile state, epoch, control words). The file owns
+// the join's kernels (the direct, chained and filtered builds, the CSR directory, the direct, fast, index, chained and grouped probes,
+// the cartesian product) and their launch formats. The index probe's launch format and launcher are declared in kb_kernels.cuh
+// because a prepared plan (kb_plan.cu) holds and launches one; the direct-table build from a pair relation is in kb_kernels.cu because
+// the store index builds the same tables.
 #include <algorithm>
 
+#include "kb_group.cuh"
 #include "kb_internal.hpp"
 #include "kb_numrank.cuh"
 
 namespace kb {
+
+// =================================================================================================================
+// K_build
+__global__ void __launch_bounds__(256) build_direct_kernel(const u32* __restrict__ keys, const u32* __restrict__ vals, u32 n,
+                                                           u32* __restrict__ table, u32 kmin, u32 range, u32 cshift, u32* dup_flag) {
+    const u32 stride = gridDim.x * blockDim.x;
+    bool dup = false;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        const u32 off = compact_key(keys[i], cshift) - kmin;
+        const u32 v = vals ? vals[i] : i;
+        if (off < range) {
+            const u32 old = atomicExch(&table[off], v);
+            dup = dup || (old != EMPTY32);
+        } else {
+            dup = true;  // cannot happen when kmin/range come from the scan statistics; treated like a duplicate -> rebuild chained
+        }
+    }
+    if (__any_sync(0xffffffffu, dup) && (threadIdx.x & 31) == 0) *dup_flag = 1u;
+}
+static void launch_build_direct(const u32* keys, const u32* vals, u32 n, u32* table, u32 kmin, u32 range, u32 cshift, u32* dup_flag, int n_sms,
+                                cudaStream_t st) {
+    if (n == 0) return;
+    int grid = grid_1d(n, n_sms);
+    build_direct_kernel<<<grid, 256, 0, st>>>(keys, vals, n, table, kmin, range, cshift, dup_flag);
+}
+
+// CHAINED multimap: open-addressing slots {key tag, head row} + next[] chains. Insert cost is O(1) whatever the key
+// multiplicity (1:N joins and heavy hitters of the Datalog joins).
+struct ChainTab {
+    u64* slots;   // lo 32: key tag (EMPTY32 free), hi 32: head row index (EMPTY32 = end)
+    u32 n_slots;  // power of two
+    u32* next;    // [n_build]
+    u32 n_keys;   // 1..4 key columns; tag = key itself when n_keys==1 else a 32-bit mix of all
+    const u32* bkey[4];
+};
+__device__ __forceinline__ u32 key_tag(u32 n_keys, u32 k0, u32 k1, u32 k2, u32 k3) {
+    if (n_keys == 1u) return k0;  // ids are never EMPTY32
+    u32 h = mix32(k0) * 0x9E3779B1u ^ mix32(k1 + 0x7F4A7C15u);
+    if (n_keys > 2u) h = mix32(h ^ k2) * 0x85EBCA77u;
+    if (n_keys > 3u) h = mix32(h ^ k3) * 0xC2B2AE3Du;
+    return h == EMPTY32 ? 0x7FFFFFFEu : h;
+}
+
+__global__ void __launch_bounds__(256) build_chained_kernel(const ChainTab T, u32 n) {
+    const u32 stride = gridDim.x * blockDim.x;
+    const u32 mask = T.n_slots - 1u;
+    u32* words = reinterpret_cast<u32*>(T.slots);  // little-endian: word 2*slot = key tag, 2*slot+1 = head row
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        const u32 k0 = T.bkey[0][i];
+        const u32 k1 = T.n_keys > 1u ? T.bkey[1][i] : 0u;
+        const u32 k2 = T.n_keys > 2u ? T.bkey[2][i] : 0u;
+        const u32 k3 = T.n_keys > 3u ? T.bkey[3][i] : 0u;
+        const u32 tag = key_tag(T.n_keys, k0, k1, k2, k3);
+        u32 slot = mix32(tag) & mask;
+        for (;;) {
+            u32 cur = *reinterpret_cast<volatile u32*>(&words[2u * slot]);
+            if (cur == tag) break;
+            if (cur == EMPTY32) {
+                const u32 old = atomicCAS(&words[2u * slot], EMPTY32, tag);
+                if (old == EMPTY32 || old == tag) break;
+            }
+            slot = (slot + 1u) & mask;
+        }
+        T.next[i] = atomicExch(&words[2u * slot + 1u], i);
+    }
+}
+static void launch_build_chained(const ChainTab& t, u32 n, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    int grid = grid_1d(n, n_sms);
+    build_chained_kernel<<<grid, 256, 0, st>>>(t, n);
+}
+
+// direct build from a predicate slice of the store index, with the pattern's pushed-down FILTER evaluated on (s, P, o)
+struct BuildPairsParams {
+    const uint2* kv;
+    u32 n, key_is_y, pred;
+    u32* table;
+    u32 kmin, range, cshift;
+    u32* dup_flag;
+    u32 trusted;
+    FilterOp ops[KB_MAX_FILTER_OPS];  // slots = positions 0/1/2
+    u32 n_ops;
+    NumTab nt;
+    u32* count;  // rows inserted (after the filter)
+};
+// 4 rows per thread and iteration: the slice loads, the FILTER's numeric gathers and the table stores of the four rows are all
+// independent, so each thread keeps 4 memory operations in flight at every stage (the 1-row version was latency-bound on
+// two 16.7 M-row builds that move 0.5 GB).
+template <bool TRUSTED>
+__global__ void __launch_bounds__(256) build_pairs_filtered_kernel(const __grid_constant__ BuildPairsParams P) {
+    constexpr int U = 4;
+    const u32 stride = gridDim.x * blockDim.x;
+    bool dup = false;
+    u32 cnt = 0;
+    const bool fast = P.n_ops == 1u && P.ops[0].op == KB_F_CMP_NUM;
+    for (u32 i0 = blockIdx.x * blockDim.x + threadIdx.x; i0 < P.n; i0 += stride * U) {
+        uint2 e[U];
+        bool ok[U];
+#pragma unroll
+        for (int u = 0; u < U; u++) {
+            const u32 i = i0 + (u32)u * stride;
+            ok[u] = i < P.n;
+            e[u] = ok[u] ? P.kv[i] : make_uint2(0u, 0u);
+        }
+        if (P.n_ops) {
+            if (fast) {
+                const u32 slot = P.ops[0].slot, cmp = P.ops[0].cmp;
+                const double cv = P.ops[0].value;
+                double a[U];
+#pragma unroll
+                for (int u = 0; u < U; u++) a[u] = ok[u] ? num_of(P.nt, slot == 0u ? e[u].x : (slot == 1u ? P.pred : e[u].y)) : 0.0;
+#pragma unroll
+                for (int u = 0; u < U; u++) ok[u] = ok[u] && cmp_num(cmp, a[u], cv);
+            } else {
+#pragma unroll
+                for (int u = 0; u < U; u++) {
+                    if (ok[u]) {
+                        u32 vals[3] = {e[u].x, P.pred, e[u].y};
+                        ok[u] = eval_filter(P.ops, P.n_ops, vals, P.nt);
+                    }
+                }
+            }
+        }
+        u32 old[U];
+#pragma unroll
+        for (int u = 0; u < U; u++) {
+            old[u] = EMPTY32;
+            if (!ok[u]) continue;
+            cnt++;
+            const u32 off = compact_key(P.key_is_y ? e[u].y : e[u].x, P.cshift) - P.kmin;
+            const u32 v = P.key_is_y ? e[u].x : e[u].y;
+            if (off < P.range) {
+                if (TRUSTED) P.table[off] = v;
+                else old[u] = atomicExch(&P.table[off], v);
+            } else dup = true;
+        }
+#pragma unroll
+        for (int u = 0; u < U; u++) dup = dup || (old[u] != EMPTY32);
+    }
+    if (__any_sync(0xffffffffu, dup) && (threadIdx.x & 31) == 0) *P.dup_flag = 1u;
+    cnt = warp_sum(cnt);
+    if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(P.count, cnt);
+}
+static void launch_build_direct_pairs_filtered(const BuildPairsParams& p, int n_sms, cudaStream_t st) {
+    if (p.n == 0) return;
+    int grid = grid_1d(p.n, n_sms, 1024);
+    if (p.trusted) build_pairs_filtered_kernel<true><<<grid, 256, 0, st>>>(p);
+    else build_pairs_filtered_kernel<false><<<grid, 256, 0, st>>>(p);
+}
+
+__global__ void __launch_bounds__(256) count_nonempty_kernel(const uint4* __restrict__ t4, u32 n4, const u32* __restrict__ tail, u32 n_tail, u32* out) {
+    u32 c = 0;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += gridDim.x * blockDim.x) {
+        const uint4 v = t4[i];
+        c += (v.x != EMPTY32) + (v.y != EMPTY32) + (v.z != EMPTY32) + (v.w != EMPTY32);
+    }
+    if (blockIdx.x == 0 && threadIdx.x < n_tail) c += tail[threadIdx.x] != EMPTY32;
+    c = warp_sum(c);
+    if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, c);
+}
+// number of occupied (non-EMPTY32) slots of a direct table: equals the number of inserted rows iff the keys were single-valued
+static void launch_count_nonempty(const u32* table, u32 n, u32* out_count, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    const u32 n4 = n / 4;
+    // one CTA more than the vectors need: n4 may be 0, and block 0 also counts the n % 4 tail slots
+    int grid = (int)umin64((u64)n_sms * 8ull, ((u64)n4 + 255ull) / 256ull + 1ull);
+    count_nonempty_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<const uint4*>(table), n4, table + (u64)n4 * 4, n - n4 * 4, out_count);
+}
+__global__ void __launch_bounds__(256) count_foreign_kernel(const u32* __restrict__ col, u32 n, u32 rank, u32 world, u32* out) {
+    u32 c = 0;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) c += shard_of(col[i], world) != rank;
+    c = warp_sum(c);
+    if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, c);
+}
+// number of keys that do NOT belong to shard `rank` of `world` (kb_shard_of): 0 for a correctly sharded column
+static void launch_count_foreign(const u32* col, u32 n, u32 rank, u32 world, u32* out, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    int grid = grid_1d(n, n_sms, 256, 4);
+    count_foreign_kernel<<<grid, 256, 0, st>>>(col, n, rank, world, out);
+}
+
+// =================================================================================================================
+// K_probe (direct, fused multiway): one probe stream against T<=4 direct tables + FILTER + ordered compaction.
+// Replaces execute_star_join_with_ids (engine.rs:587-691) / bind-join chains (engine.rs:840-885) on unique keys.
+constexpr int PROBE_THREADS = 256;
+constexpr int PROBE_ITEMS = 4;
+constexpr int PROBE_TILE = PROBE_THREADS * PROBE_ITEMS;  // 1024 rows
+enum : u32 { OUT_PROBE = 0, OUT_TABVAL = 1, OUT_TABPAY = 2 };
+struct OutCol {
+    u32 kind, a, b;  // OUT_PROBE: a = probe column; OUT_TABVAL: a = table; OUT_TABPAY: a = table, b = payload column
+};
+struct ProbeDParams {
+    const u32* pcol[KB_MAX_COLS];
+    u32 n_pcols, key_col, n, n_tiles, T;
+    DirectTab tab[MAXT];
+    u32 n_out;
+    OutCol oc[KB_MAX_COLS];
+    u32* out[KB_MAX_COLS];
+    u32 cap;
+    FilterOp ops[KB_MAX_FILTER_OPS];  // slots = output column indices
+    u32 n_ops;
+    NumTab nt;
+    Compact c;
+    const u32* abort_flag;  // non-null: exit immediately if *abort_flag != 0 (a direct build met duplicate keys)
+};
+
+// K_probe (direct, FAST): the probe side is a pair relation; each thread owns 4 consecutive rows held in registers, so the shared
+// tile is refilled by TMA while the rows are probed (same register-staged double buffering as K_scan).
+constexpr int PROBEF_THREADS = 256;
+#ifndef KB_PROBEF_ITEMS
+#define KB_PROBEF_ITEMS 4
+#endif
+constexpr int PROBEF_ITEMS = KB_PROBEF_ITEMS;  // rows per thread: 8 keeps twice the lookups in flight per thread (the kernel is latency-bound)
+constexpr int PROBEF_TILE = PROBEF_THREADS * PROBEF_ITEMS;
+struct ProbeFParams {
+    const uint2* pairs;
+    u32 key_is_y;  // which half of the pair is the join key
+    u32 n, n_tiles, T;
+    DirectTab tab[MAXT];  // mode 0 (value payload) or 2 (existence) only
+    u32 n_out;
+    OutCol oc[KB_MAX_COLS];  // OUT_PROBE: a = 0 (pair.x) / 1 (pair.y); OUT_TABVAL: a = table
+    u32* out[KB_MAX_COLS];
+    u32 cap;
+    FilterOp ops[KB_MAX_FILTER_OPS];
+    u32 n_ops;
+    FilterOp pre_ops[8];  // conjuncts over the probe row alone (slot 0 = pair.x, 1 = pair.y): evaluated BEFORE any table lookup
+    u32 n_pre;
+    const double* pre_num;  // non-null: numeric value of pair.y per probe row (typed literal column of the index): a coalesced read
+                            // replaces the random gather num_or0[pair.y] when the pre-filter is FILTER(?y <cmp> c)
+    NumTab nt;
+    Compact c;
+    const u32* abort_flag;
+};
+template <int T>
+__global__ void __launch_bounds__(PROBEF_THREADS, (PROBEF_ITEMS <= 4 ? 4 : 3)) probe_fast_kernel(const __grid_constant__ ProbeFParams P) {
+    constexpr int R = PROBEF_ITEMS;  // rows per thread, consecutive
+    extern __shared__ __align__(128) u32 smem_all[];  // two stages of PROBEF_TILE pairs (see probe_index_kernel)
+    constexpr u32 STAGE_WORDS = 2u * PROBEF_TILE;
+    __shared__ __align__(8) u64 bars[2];
+    __shared__ u32 s_nexts[2];
+    __shared__ u32 s_wcnt[PROBEF_THREADS / 32];
+    __shared__ u32 s_excl1;
+    if (P.abort_flag != nullptr) {
+        for (int t = 0; t < T; t++) if (reinterpret_cast<const volatile u32*>(P.abort_flag)[t] != 0u) return;
+    }
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    auto issue_next = [&](u32 stage) {
+        const u32 t = atomicAdd(P.c.ticket, 1u);
+        s_nexts[stage] = t;
+        if (t < P.n_tiles) {
+            const u32 b = t * (u32)PROBEF_TILE;
+            const u32 c = min((u32)PROBEF_TILE, P.n - b);
+            const u32 bytes = (c * 8u + 15u) & ~15u;
+            mbar_arrive_expect_tx(&bars[stage], bytes);
+            tma_load_1d(smem_all + stage * STAGE_WORDS, P.pairs + b, bytes, &bars[stage]);
+        }
+    };
+    if (tid == 0) {
+        mbar_init(&bars[0], 1);
+        mbar_init(&bars[1], 1);
+        fence_mbar_init();
+        issue_next(0);
+        issue_next(1);
+    }
+    __syncthreads();
+    u32 tile = s_nexts[0];
+    u32 it = 0;
+    while (tile < P.n_tiles) {
+        const u32 stage = it & 1u;
+        const u32* smem = smem_all + stage * STAGE_WORDS;
+        const u32 base = tile * (u32)PROBEF_TILE;
+        const u32 cnt = min((u32)PROBEF_TILE, P.n - base);
+        mbar_wait(&bars[stage], (it >> 1) & 1u);
+        // striped: row j of this thread is row (warp*32*R + j*32 + lane) of the tile — one warp instruction touches 32 consecutive rows, so
+        // lookups by a sorted key hit 4 sectors instead of 16 and the compacted stores of one j form one contiguous run
+        u32 rx[R], ry[R];
+#pragma unroll
+        for (int j = 0; j < R; j++) {
+            const uint2 v = reinterpret_cast<const uint2*>(smem)[(u32)warp * (32u * R) + (u32)j * 32u + (u32)lane];
+            rx[j] = v.x; ry[j] = v.y;
+        }
+        const u32 row0 = (u32)warp * (32u * R) + (u32)lane;  // row j = row0 + 32*j
+        u32 vmask = 0;
+#pragma unroll
+        for (int j = 0; j < R; j++) vmask |= (row0 + 32u * (u32)j < cnt ? 1u : 0u) << j;
+        // FILTER conjuncts over the probe row alone. The common shape FILTER(?x <cmp> c) needs one numeric gather per row: it is issued
+        // together with the table lookups (independent loads, one memory round trip) and resolved afterwards — gating the lookups on
+        // it would put two dependent round trips on the critical path of a latency-bound kernel.
+        const bool pre_fast = P.n_pre == 1u && P.pre_ops[0].op == KB_F_CMP_NUM;
+        double pa[R];
+        if (pre_fast) {
+            const u32 slot = P.pre_ops[0].slot;
+#pragma unroll
+            for (int j = 0; j < R; j++) {
+                if (P.pre_num != nullptr && slot == 1u) pa[j] = ((vmask >> j) & 1u) ? __ldg(P.pre_num + base + row0 + 32u * (u32)j) : 0.0;
+                else pa[j] = ((vmask >> j) & 1u) ? num_of(P.nt, slot == 0u ? rx[j] : ry[j]) : 0.0;
+            }
+        } else if (P.n_pre != 0u && vmask != 0u) {
+#pragma unroll
+            for (int j = 0; j < R; j++) {
+                if ((vmask >> j) & 1u) {
+                    u32 vals[2] = {rx[j], ry[j]};
+                    if (!eval_filter(P.pre_ops, P.n_pre, vals, P.nt)) vmask &= ~(1u << j);
+                }
+            }
+        }
+        u32 tv[R][T > 0 ? T : 1];
+#pragma unroll
+        for (int j = 0; j < R; j++) {
+            const u32 key = P.key_is_y ? ry[j] : rx[j];
+#pragma unroll
+            for (int t = 0; t < T; t++) {
+                const u32 off = compact_key(key, P.tab[t].cshift) - P.tab[t].kmin;
+                tv[j][t] = (((vmask >> j) & 1u) && off < P.tab[t].range) ? __ldg(P.tab[t].tab + off) : EMPTY32;
+            }
+        }
+        if (pre_fast) {
+            const u32 cmp = P.pre_ops[0].cmp;
+            const double cv = P.pre_ops[0].value;
+            u32 pass = 0;
+#pragma unroll
+            for (int j = 0; j < R; j++) pass |= (cmp_num(cmp, pa[j], cv) ? 1u : 0u) << j;
+            vmask &= pass;
+        }
+        u32 m = 0;
+#pragma unroll
+        for (int j = 0; j < R; j++) {
+            bool hit = (vmask >> j) & 1u;
+#pragma unroll
+            for (int t = 0; t < T; t++) hit = hit && (tv[j][t] != EMPTY32);
+            m |= (hit ? 1u : 0u) << j;
+        }
+        if (P.n_ops != 0u && m != 0u) {
+            if (P.n_ops == 1u && P.ops[0].op == KB_F_CMP_NUM) {
+                const OutCol oc = P.oc[P.ops[0].slot];
+                const u32 cmp = P.ops[0].cmp;
+                const double cv = P.ops[0].value;
+                double a[R];
+#pragma unroll
+                for (int j = 0; j < R; j++) {
+                    u32 id = oc.kind == OUT_PROBE ? (oc.a == 0u ? rx[j] : ry[j]) : 0u;
+#pragma unroll
+                    for (int t = 0; t < T; t++) if (oc.kind == OUT_TABVAL && oc.a == (u32)t) id = tv[j][t];
+                    a[j] = ((m >> j) & 1u) ? num_of(P.nt, id) : 0.0;
+                }
+                u32 pass = 0;
+#pragma unroll
+                for (int j = 0; j < R; j++) pass |= (cmp_num(cmp, a[j], cv) ? 1u : 0u) << j;
+                m &= pass;
+            } else {
+#pragma unroll
+                for (int j = 0; j < R; j++) {
+                    if ((m >> j) & 1u) {
+                        u32 vals[KB_MAX_COLS];
+                        for (u32 c = 0; c < P.n_out; c++) {
+                            const OutCol oc = P.oc[c];
+                            u32 x = oc.kind == OUT_PROBE ? (oc.a == 0u ? rx[j] : ry[j]) : 0u;
+#pragma unroll
+                            for (int t = 0; t < T; t++) if (oc.kind == OUT_TABVAL && oc.a == (u32)t) x = tv[j][t];
+                            vals[c] = x;
+                        }
+                        if (!eval_filter(P.ops, P.n_ops, vals, P.nt)) m &= ~(1u << j);
+                    }
+                }
+            }
+        }
+        u32 bal[R];
+        u32 wtot = 0;
+#pragma unroll
+        for (int j = 0; j < R; j++) {
+            bal[j] = __ballot_sync(0xffffffffu, (m >> j) & 1u);
+            wtot += (u32)__popc(bal[j]);
+        }
+        if (lane == 0) s_wcnt[warp] = wtot;
+        __syncthreads();
+        const u32 following = s_nexts[stage ^ 1u];
+        if (tid == 32) issue_next(stage);  // every thread holds its rows in registers: refill this stage with the tile after next
+        if (warp == 0) {
+            const u32 wc = lane < PROBEF_THREADS / 32 ? s_wcnt[lane] : 0u;
+            u32 wi = wc;
+#pragma unroll
+            for (int o = 1; o < PROBEF_THREADS / 32; o <<= 1) {
+                const u32 y = __shfl_up_sync(0xffffffffu, wi, o);
+                if (lane >= o) wi += y;
+            }
+            const u32 total = __shfl_sync(0xffffffffu, wi, PROBEF_THREADS / 32 - 1);
+            if (lane < PROBEF_THREADS / 32) s_wcnt[lane] = wi - wc;
+            const u32 ex = tile_prefix_2level(P.c.tile_state, P.c.block_state, tile, P.n_tiles, 0u, P.c.epoch, total, P.c.zero_word, P.c.total, P.c.ordered, lane);
+            if (lane == 0) s_excl1 = ex;
+        }
+        __syncthreads();
+        {
+            const u32 lt = (1u << lane) - 1u;
+            const u32 wbase = s_excl1 + s_wcnt[warp];
+            for (u32 cidx = 0; cidx < P.n_out; cidx++) {
+                const OutCol oc = P.oc[cidx];
+                u32* out = P.out[cidx];
+                u32 run = wbase;
+#pragma unroll
+                for (int j = 0; j < R; j++) {
+                    u32 x = oc.kind == OUT_PROBE ? (oc.a == 0u ? rx[j] : ry[j]) : 0u;
+#pragma unroll
+                    for (int t = 0; t < T; t++) if (oc.kind == OUT_TABVAL && oc.a == (u32)t) x = tv[j][t];
+                    const u32 pos = run + (u32)__popc(bal[j] & lt);
+                    if (((m >> j) & 1u) && pos < P.cap) out[pos] = x;
+                    run += (u32)__popc(bal[j]);
+                }
+            }
+        }
+        tile = following;
+        it++;
+    }
+}
+
+static void launch_probe_fast(const ProbeFParams& p, int n_sms, cudaStream_t st) {
+    if (p.n == 0) return;
+    const size_t smem = 2 * (size_t)PROBEF_TILE * sizeof(uint2);
+    const void* fn = nullptr;
+    switch (p.T) {
+        case 1: fn = (const void*)probe_fast_kernel<1>; break;
+        case 2: fn = (const void*)probe_fast_kernel<2>; break;
+        case 3: fn = (const void*)probe_fast_kernel<3>; break;
+        default: fn = (const void*)probe_fast_kernel<4>; break;
+    }
+    const int grid = grid_for(fn, PROBEF_THREADS, smem, n_sms, p.n_tiles);
+    switch (p.T) {
+        case 1: probe_fast_kernel<1><<<grid, PROBEF_THREADS, smem, st>>>(p); break;
+        case 2: probe_fast_kernel<2><<<grid, PROBEF_THREADS, smem, st>>>(p); break;
+        case 3: probe_fast_kernel<3><<<grid, PROBEF_THREADS, smem, st>>>(p); break;
+        default: probe_fast_kernel<4><<<grid, PROBEF_THREADS, smem, st>>>(p); break;
+    }
+}
+
+// =================================================================================================================
+// K_probe (INDEX)
+#ifndef KB_PI_MINB
+#define KB_PI_MINB 4
+#endif
+// AGG = true: the joined rows are not written; GROUP BY one output column with at most one aggregate is folded in the kernel
+// (execute_query.rs:1150-1227 over the rows of engine.rs:587-691): per warp __match_any_sync on the key, a 64-entry CTA table in shared
+// memory, flushed to the global group table when the CTA is done. Only the row count and the groups leave the kernel.
+constexpr int PI_GROUP_SMEM = 64;
+// TAB = true: the probe stream is not the slice but the probe pattern's own persistent TABLE, walked slot by slot: slot i holds the
+// other half of the triple whose key is (table base + i), EMPTY32 where no triple has that key. The keys then come in ascending order
+// whatever the order of the store and of the dictionary ids, so the lookups into the other patterns' tables are sequential too — a
+// direct table over dense ids IS the slice sorted by that column (with the gaps of the id space). With a FILTER on the other half's
+// numeric value the 2-byte value ranks are read from a second table in the same order (kb_numrank.cuh: the FILTER is a range of
+// stored ranks; a slot whose stored rank is at an end of that range is decided on its value, num_of(object)).
+template <int T, int PRE, bool AGG, bool TAB>
+__global__ void __launch_bounds__(PROBEF_THREADS, KB_PI_MINB) probe_index_kernel(const __grid_constant__ ProbeIParams P, const __grid_constant__ GroupParams G) {
+    constexpr int R = 4;  // rows per thread (striped over the warp's 128-row chunk, see below)
+    constexpr u32 TILE = PROBEF_THREADS * R;
+    extern __shared__ __align__(128) u32 smem_all[];  // per stage: TILE pairs [+ TILE doubles]
+    constexpr u32 STAGE_WORDS = TAB ? (PRE == 1 ? 3u * TILE / 2u : TILE) : (PRE == 1 ? 4u : 2u) * TILE;  // TAB: TILE values [+ TILE u16 ranks]
+    __shared__ __align__(8) u64 bars[2];
+    __shared__ u32 s_nexts[2];
+    __shared__ u32 s_wcnt[PROBEF_THREADS / 32];
+    __shared__ u32 s_excl1;
+    __shared__ u32 a_key[AGG ? PI_GROUP_SMEM : 1];
+    __shared__ u32 a_cnt[AGG ? PI_GROUP_SMEM : 1];
+    __shared__ double a_val[AGG ? PI_GROUP_SMEM : 1];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    u32 my_rows = 0;  // AGG: joined rows seen by this thread
+    if (AGG) {
+        for (int i = tid; i < PI_GROUP_SMEM; i += PROBEF_THREADS) {
+            a_key[i] = EMPTY32;
+            a_cnt[i] = 0u;
+            a_val[i] = agg_identity(P.akind);
+        }
+    }
+    __shared__ u32 s_tcnt[2];  // rows in the staged tile
+    // dictionaries of the coded tables (DirectTab::code): entry 0xFF is EMPTY32, so a code decodes with one shared load (the barrier
+    // after the stage set-up below publishes them)
+    __shared__ u32 s_dict[T][256];
+#pragma unroll
+    for (int t = 0; t < T; t++)
+        if (P.tab[t].code) s_dict[t][tid] = (u32)tid < P.tab[t].n_dict ? P.tab[t].dict[tid] : EMPTY32;
+    static_assert(PROBEF_THREADS == 256, "one dictionary entry per thread");
+    auto issue = [&](u32 t, u32 stage) {
+        u32* smem = smem_all + stage * STAGE_WORDS;
+        u64& bar = bars[stage];
+        if constexpr (TAB) {
+            const u32 b = t * TILE;
+            const u32 c = min(TILE, P.ptab_range - b);
+            const u32 bytes = (c * 4u + 15u) & ~15u;
+            const u32 kbytes = (c * 2u + 15u) & ~15u;
+            s_tcnt[stage] = c;
+            mbar_arrive_expect_tx(&bar, PRE == 1 ? bytes + kbytes : bytes);
+            tma_load_1d(smem, P.ptab + b, bytes, &bar);
+            if (PRE == 1) tma_load_1d(smem + TILE, P.pkey + b, kbytes, &bar);
+            return;
+        }
+        u32 g = 0;  // the chunk (store segment) this tile belongs to
+        while (g + 1u < P.n_seg && t >= P.seg[g + 1u].tile0) g++;
+        const ProbeISeg& sg = P.seg[g];
+        const u32 b = (t - sg.tile0) * TILE;
+        const u32 c = min(TILE, sg.n - b);
+        const u32 bytes = (c * 8u + 15u) & ~15u;
+        s_tcnt[stage] = c;
+        mbar_arrive_expect_tx(&bar, PRE == 1 ? 2u * bytes : bytes);
+        tma_load_1d(smem, sg.pairs + b, bytes, &bar);
+        if (PRE == 1) tma_load_1d(smem + 2 * TILE, sg.ynum + b, bytes, &bar);
+    };
+    // two shared stages: tile i+1 is in flight while tile i is processed, and the stage of tile i is refilled (tile i+2) right after
+    // the first compaction barrier — by then every thread has its rows in registers, so no barrier is spent on the hand-over
+    if (tid == 0) {
+        mbar_init(&bars[0], 1);
+        mbar_init(&bars[1], 1);
+        fence_mbar_init();
+        for (u32 st = 0; st < 2; st++) {
+            const u32 t0 = atomicAdd(&P.cb[0], 1u);
+            s_nexts[st] = t0;
+            if (t0 < P.n_tiles) issue(t0, st);
+        }
+    }
+    __syncthreads();
+    u32 tile = s_nexts[0];
+    u32 it = 0;
+    while (tile < P.n_tiles) {
+        const u32 stage = it & 1u;
+        const u32* smem = smem_all + stage * STAGE_WORDS;
+        mbar_wait(&bars[stage], (it >> 1) & 1u);
+        const u32 cnt = s_tcnt[stage];
+        u32 rx[R], ry[R];
+        double pa[R];  // PRE == 1: the FILTER operand (slice mode: the f64 value, table mode: its rank in pk)
+        u32 pk[R];
+        // striped: row j of this thread is row (warp*128 + j*32 + lane) of the tile, so one warp instruction touches 32 CONSECUTIVE
+        // rows: lookups into a table indexed by a sorted key hit 4 sectors instead of 16, and the compacted stores of one j are
+        // one contiguous run
+        u32 vmask = 0;
+        if constexpr (TAB) {
+#pragma unroll
+            for (int j = 0; j < R; j++) {
+                const u32 idx = (u32)warp * (32u * R) + (u32)j * 32u + (u32)lane;
+                const u32 v = smem[idx];
+                // the key of slot (tile base + idx): the inverse of compact_key for this shard's keys
+                const u32 ck = P.ptab_min + tile * TILE + idx;
+                const u32 key = P.ptab_cshift ? (((((ck >> SHARD_B) << P.ptab_cshift) | P.shard_rank) << SHARD_B) | (ck & ((1u << SHARD_B) - 1u))) : ck;
+                rx[j] = P.key_is_y ? v : key;
+                ry[j] = P.key_is_y ? key : v;
+                if (PRE == 1) pk[j] = reinterpret_cast<const u16*>(smem + TILE)[idx];
+                vmask |= ((idx < cnt && v != EMPTY32) ? 1u : 0u) << j;
+            }
+        } else {
+#pragma unroll
+            for (int j = 0; j < R; j++) {
+                const u32 idx = (u32)warp * (32u * R) + (u32)j * 32u + (u32)lane;
+                const uint2 v = reinterpret_cast<const uint2*>(smem)[idx];
+                rx[j] = v.x; ry[j] = v.y;
+                if (PRE == 1) pa[j] = reinterpret_cast<const double*>(smem + 2 * TILE)[idx];
+            }
+#pragma unroll
+            for (int j = 0; j < R; j++) vmask |= (((u32)warp * (32u * R) + (u32)j * 32u + (u32)lane) < cnt ? 1u : 0u) << j;
+        }
+        if (PRE == 1) {
+            u32 pass = 0, edge = 0;
+#pragma unroll
+            for (int j = 0; j < R; j++) {
+                bool ok;
+                if constexpr (TAB) {
+                    ok = pk[j] >= P.key_lo && pk[j] <= P.key_hi;
+                    edge |= ((ok && (pk[j] == P.key_lo || pk[j] == P.key_hi)) ? 1u : 0u) << j;
+                } else ok = cmp_num(P.pre_cmp, pa[j], P.pre_val);
+                pass |= (ok ? 1u : 0u) << j;
+            }
+            vmask &= pass;
+            if (TAB && P.key_shift != 0u && (edge & vmask) != 0u) {  // a stored rank at an end of the range: its values straddle the constant
+#pragma unroll
+                for (int j = 0; j < R; j++) {
+                    if (((edge & vmask) >> j) & 1u) {
+                        if (!cmp_num(P.pre_cmp, num_of(P.nt, P.key_is_y ? rx[j] : ry[j]), P.pre_val)) vmask &= ~(1u << j);
+                    }
+                }
+            }
+        } else if (P.pre_mode == 2u && vmask != 0u) {
+#pragma unroll
+            for (int j = 0; j < R; j++) {
+                if ((vmask >> j) & 1u) {
+                    u32 vals[2] = {rx[j], ry[j]};
+                    if (!eval_filter(P.pre_ops, P.n_pre, vals, P.nt)) vmask &= ~(1u << j);
+                }
+            }
+        }
+        // a coded table (warp-uniform) is read one byte a slot: a warp's 32 consecutive keys are one sector instead of four. Every
+        // load is issued before the first code is decoded
+        u32 tv[R][T];
+#pragma unroll
+        for (int t = 0; t < T; t++) {
+            const DirectTab& D = P.tab[t];
+            if (D.code) {
+#pragma unroll
+                for (int j = 0; j < R; j++) {
+                    const u32 off = compact_key(P.key_is_y ? ry[j] : rx[j], D.cshift) - D.kmin;
+                    tv[j][t] = (((vmask >> j) & 1u) && off < D.range) ? (u32)__ldg(D.code + off) : 0xFFu;
+                }
+            } else {
+#pragma unroll
+                for (int j = 0; j < R; j++) {
+                    const u32 off = compact_key(P.key_is_y ? ry[j] : rx[j], D.cshift) - D.kmin;
+                    tv[j][t] = (((vmask >> j) & 1u) && off < D.range) ? __ldg(D.tab + off) : EMPTY32;
+                }
+            }
+        }
+#pragma unroll
+        for (int t = 0; t < T; t++)
+            if (P.tab[t].code) {
+#pragma unroll
+                for (int j = 0; j < R; j++) tv[j][t] = s_dict[t][tv[j][t]];
+            }
+        u32 m = 0;
+#pragma unroll
+        for (int j = 0; j < R; j++) {
+            bool hit = (vmask >> j) & 1u;
+#pragma unroll
+            for (int t = 0; t < T; t++) hit = hit && (tv[j][t] != EMPTY32);
+            m |= (hit ? 1u : 0u) << j;
+        }
+        if (P.n_ops != 0u && m != 0u) {
+#pragma unroll
+            for (int j = 0; j < R; j++) {
+                if ((m >> j) & 1u) {
+                    u32 vals[KB_MAX_COLS];
+                    vals[0] = rx[j]; vals[1] = ry[j];
+#pragma unroll
+                    for (int t = 0; t < T; t++) vals[2 + t] = tv[j][t];
+                    if (!eval_filter(P.ops, P.n_ops, vals, P.nt)) m &= ~(1u << j);
+                }
+            }
+        }
+        if constexpr (AGG) {
+            __syncthreads();  // every thread holds its rows in registers: the stage can take the tile after next
+            const u32 following_a = s_nexts[stage ^ 1u];
+            if (tid == 32) {
+                const u32 nt = atomicAdd(&P.cb[0], 1u);
+                s_nexts[stage] = nt;
+                if (nt < P.n_tiles) issue(nt, stage);
+            }
+            my_rows += (u32)__popc(m);
+#pragma unroll
+            for (int j = 0; j < R; j++) {
+                const bool on = (m >> j) & 1u;
+                const unsigned act = __ballot_sync(0xffffffffu, on);
+                if (act == 0u || !on) continue;
+                u32 key = P.gsel == 0u ? rx[j] : ry[j];
+                u32 vid = P.asel == 0u ? rx[j] : ry[j];
+#pragma unroll
+                for (int t = 0; t < T; t++) {
+                    if (P.gsel == 2u + (u32)t) key = tv[j][t];
+                    if (P.asel == 2u + (u32)t) vid = tv[j][t];
+                }
+                const unsigned peers = __match_any_sync(act, key);
+                const int leader = __ffs(peers) - 1;
+                double acc = 0.0;
+                if (P.akind != KB_AGG_COUNT) {
+                    const double mine = num_of(P.nt, vid);
+                    acc = mine;
+                    unsigned rest = peers & ~(1u << leader);
+                    while (rest) {  // every lane of the group runs the same shuffles
+                        const int src = __ffs(rest) - 1;
+                        rest &= rest - 1u;
+                        const double o = __shfl_sync(peers, mine, src);
+                        if (P.akind == KB_AGG_MIN) acc = fmin(acc, o);
+                        else if (P.akind == KB_AGG_MAX) acc = fmax(acc, o);
+                        else acc += o;
+                    }
+                }
+                if (lane != leader) continue;
+                const u32 cnt_g = (u32)__popc(peers);
+                u32 slot = mix32(key) & (PI_GROUP_SMEM - 1);
+                bool done = false;
+                for (int probes = 0; probes < PI_GROUP_SMEM && !done && key != EMPTY32; probes++) {  // EMPTY32 marks a free entry
+                    u32 cur = *reinterpret_cast<volatile u32*>(&a_key[slot]);
+                    if (cur == EMPTY32) cur = atomicCAS(&a_key[slot], EMPTY32, key);
+                    if (cur == EMPTY32 || cur == key) {
+                        atomicAdd(&a_cnt[slot], cnt_g);
+                        if (P.akind == KB_AGG_MIN) atomic_min_f64(&a_val[slot], acc);
+                        else if (P.akind == KB_AGG_MAX) atomic_max_f64(&a_val[slot], acc);
+                        else if (P.akind != KB_AGG_COUNT) atomicAdd(&a_val[slot], acc);
+                        done = true;
+                    } else slot = (slot + 1u) & (PI_GROUP_SMEM - 1);
+                }
+                if (!done) {  // more than 64 distinct groups in this CTA
+                    u32 kk[4] = {key, 0u, 0u, 0u};
+                    double vv[8] = {acc, 0, 0, 0, 0, 0, 0, 0};
+                    group_update_global(G, kk, (unsigned long long)cnt_g, vv);
+                }
+            }
+            tile = following_a;
+            it++;
+            continue;
+        }
+        u32 bal[R];
+        u32 wtot = 0;
+#pragma unroll
+        for (int j = 0; j < R; j++) {
+            bal[j] = __ballot_sync(0xffffffffu, (m >> j) & 1u);
+            wtot += (u32)__popc(bal[j]);
+        }
+        if (lane == 0) s_wcnt[warp] = wtot;
+        __syncthreads();
+        const u32 following = s_nexts[stage ^ 1u];  // tile of the next iteration (its copy is in flight)
+        if (tid == 32) {  // a lane outside the prefix warp refills this stage with the tile after that one
+            const u32 nt = atomicAdd(&P.cb[0], 1u);
+            s_nexts[stage] = nt;
+            if (nt < P.n_tiles) issue(nt, stage);
+        }
+        if (warp == 0) {
+            const u32 wc = lane < PROBEF_THREADS / 32 ? s_wcnt[lane] : 0u;
+            u32 wi = wc;
+#pragma unroll
+            for (int o = 1; o < PROBEF_THREADS / 32; o <<= 1) {
+                const u32 y = __shfl_up_sync(0xffffffffu, wi, o);
+                if (lane >= o) wi += y;
+            }
+            const u32 total = __shfl_sync(0xffffffffu, wi, PROBEF_THREADS / 32 - 1);
+            if (lane < PROBEF_THREADS / 32) s_wcnt[lane] = wi - wc;
+            const u32 ex = tile_prefix_2level(P.c.tile_state, P.c.block_state, tile, P.n_tiles, 0u, P.c.epoch, total, P.c.zero_word, P.c.total, P.c.ordered, lane);
+            if (lane == 0) s_excl1 = ex;
+        }
+        __syncthreads();
+        {
+            u32 run = s_excl1 + s_wcnt[warp];
+            const u32 lt = (1u << lane) - 1u;
+#pragma unroll
+            for (int j = 0; j < R; j++) {
+                const u32 pos = run + (u32)__popc(bal[j] & lt);
+                if (((m >> j) & 1u) && pos < P.cap) {
+                    P.out[0][pos] = rx[j];
+                    P.out[1][pos] = ry[j];
+#pragma unroll
+                    for (int t = 0; t < T; t++) P.out[2 + t][pos] = tv[j][t];
+                }
+                run += (u32)__popc(bal[j]);
+            }
+        }
+        tile = following;
+        it++;
+    }
+    if constexpr (AGG) {
+        __syncthreads();
+        for (int i = tid; i < PI_GROUP_SMEM; i += PROBEF_THREADS) {
+            if (a_key[i] == EMPTY32) continue;
+            u32 kk[4] = {a_key[i], 0u, 0u, 0u};
+            double vv[8] = {a_val[i], 0, 0, 0, 0, 0, 0, 0};
+            group_update_global(G, kk, (unsigned long long)a_cnt[i], vv);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) my_rows += __shfl_xor_sync(0xffffffffu, my_rows, o);
+        if (lane == 0 && my_rows) atomicAdd(&P.cb[1], my_rows);
+    }
+    // the last CTA to get here publishes the row count and leaves the control block zeroed for the next launch
+    __syncthreads();
+    if (tid == 0) {
+        __threadfence();
+        const u32 prev = atomicAdd(&P.cb[3], 1u);
+        if (prev == gridDim.x - 1u) {
+            __threadfence();
+            const u32 total = atomicExch(&P.cb[1], 0u);
+            *reinterpret_cast<volatile u32*>(P.host_total) = total;
+            P.cb[0] = 0u;
+            P.cb[3] = 0u;
+            __threadfence_system();
+        }
+    }
+}
+
+template <int T, int PRE, bool AGG, bool TAB>
+static void launch_probe_index_tp(const ProbeIParams& p, const GroupParams& g, int n_sms, cudaStream_t st) {
+    static int per_sm = 0;  // occupancy is a property of the kernel image: asked once per instantiation
+    const size_t smem = TAB ? (size_t)PROBEF_THREADS * 4 * (PRE == 1 ? 6 : 4) * 2 : (size_t)PROBEF_THREADS * 4 * (PRE == 1 ? 16 : 8) * 2;
+    if (per_sm == 0) {
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, probe_index_kernel<T, PRE, AGG, TAB>, PROBEF_THREADS, smem);
+        if (per_sm < 1) per_sm = 1;
+    }
+    long long grid = (long long)per_sm * n_sms;
+    if (grid > (long long)p.n_tiles) grid = p.n_tiles;
+    probe_index_kernel<T, PRE, AGG, TAB><<<(int)grid, PROBEF_THREADS, smem, st>>>(p, g);
+}
+template <int T, bool TAB>
+static void launch_probe_index_t(const ProbeIParams& p, const GroupParams* g, int n_sms, cudaStream_t st) {
+    static const GroupParams none{};
+    if (g) {
+        if (p.pre_mode == 1u) launch_probe_index_tp<T, 1, true, TAB>(p, *g, n_sms, st);
+        else launch_probe_index_tp<T, 0, true, TAB>(p, *g, n_sms, st);
+    } else {
+        if (p.pre_mode == 1u) launch_probe_index_tp<T, 1, false, TAB>(p, none, n_sms, st);
+        else launch_probe_index_tp<T, 0, false, TAB>(p, none, n_sms, st);
+    }
+}
+void launch_probe_index(const ProbeIParams& p, const GroupParams* agg, int n_sms, cudaStream_t st) {
+    if (p.n == 0) return;
+    if (p.ptab) {
+        switch (p.T) {
+            case 1: launch_probe_index_t<1, true>(p, agg, n_sms, st); break;
+            case 2: launch_probe_index_t<2, true>(p, agg, n_sms, st); break;
+            case 3: launch_probe_index_t<3, true>(p, agg, n_sms, st); break;
+            default: launch_probe_index_t<4, true>(p, agg, n_sms, st); break;
+        }
+        return;
+    }
+    switch (p.T) {
+        case 1: launch_probe_index_t<1, false>(p, agg, n_sms, st); break;
+        case 2: launch_probe_index_t<2, false>(p, agg, n_sms, st); break;
+        case 3: launch_probe_index_t<3, false>(p, agg, n_sms, st); break;
+        default: launch_probe_index_t<4, false>(p, agg, n_sms, st); break;
+    }
+}
+
+// =================================================================================================================
+// K_probe (direct, fused multiway)
+template <int T>
+__global__ void __launch_bounds__(PROBE_THREADS) probe_direct_kernel(const __grid_constant__ ProbeDParams P) {
+    extern __shared__ __align__(128) u32 smem[];  // n_pcols tiles of PROBE_TILE
+    __shared__ __align__(8) u64 bar;
+    __shared__ u32 s_tile;
+    __shared__ u32 s_wcnt[PROBE_THREADS / 32];
+    __shared__ u32 s_cnt[MAXP], s_excl[MAXP];
+    if (P.abort_flag != nullptr) {  // a direct build met duplicate keys: the host will redo this join with the chained operator
+        for (int t = 0; t < T; t++) if (reinterpret_cast<const volatile u32*>(P.abort_flag)[t] != 0u) return;
+    }
+
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) {
+        mbar_init(&bar, 1);
+        fence_mbar_init();
+    }
+    u32 parity = 0;
+    const unsigned lt_mask = (1u << lane) - 1u;
+    const u32* sKey = smem + P.key_col * PROBE_TILE;
+
+    for (;;) {
+        if (tid == 0) s_tile = atomicAdd(P.c.ticket, 1u);
+        __syncthreads();
+        const u32 tile = s_tile;
+        if (tile >= P.n_tiles) break;
+        const u32 base = tile * (u32)PROBE_TILE;
+        const u32 cnt = min((u32)PROBE_TILE, P.n - base);
+        if (tid == 0) {
+            const u32 bytes = (cnt * 4u + 15u) & ~15u;
+            mbar_arrive_expect_tx(&bar, bytes * P.n_pcols);
+            for (u32 c = 0; c < P.n_pcols; c++) tma_load_1d(smem + c * PROBE_TILE, P.pcol[c] + base, bytes, &bar);
+        }
+        mbar_wait(&bar, parity);
+        parity ^= 1u;
+
+        // all table loads of this thread's rows are issued before any is consumed (ITEMS*T independent loads in flight)
+        u32 v[PROBE_ITEMS][T > 0 ? T : 1];
+#pragma unroll
+        for (int j = 0; j < PROBE_ITEMS; j++) {
+            const u32 idx = (u32)warp * (32u * PROBE_ITEMS) + (u32)j * 32u + (u32)lane;
+            const bool valid = idx < cnt;
+            const u32 key = sKey[idx];
+#pragma unroll
+            for (int t = 0; t < T; t++) {
+                const u32 off = compact_key(key, P.tab[t].cshift) - P.tab[t].kmin;
+                v[j][t] = (valid && off < P.tab[t].range) ? __ldg(P.tab[t].tab + off) : EMPTY32;
+            }
+            if (T == 0) v[j][0] = valid ? 0u : EMPTY32;
+        }
+        u32 mbits = 0;
+#pragma unroll
+        for (int j = 0; j < PROBE_ITEMS; j++) {
+            const u32 idx = (u32)warp * (32u * PROBE_ITEMS) + (u32)j * 32u + (u32)lane;
+            bool hit = true;
+#pragma unroll
+            for (int t = 0; t < (T > 0 ? T : 1); t++) hit = hit && (v[j][t] != EMPTY32);
+            if (hit && P.n_ops != 0u) {
+                u32 vals[KB_MAX_COLS];
+                for (u32 c = 0; c < P.n_out; c++) {
+                    const OutCol oc = P.oc[c];
+                    u32 x;
+                    if (oc.kind == OUT_PROBE) x = smem[oc.a * PROBE_TILE + idx];
+                    else {
+                        u32 tv = 0;
+#pragma unroll
+                        for (int t = 0; t < T; t++) if ((u32)t == oc.a) tv = v[j][t];
+                        x = oc.kind == OUT_TABVAL ? tv : __ldg(P.tab[oc.a].pay[oc.b] + tv);
+                    }
+                    vals[c] = x;
+                }
+                hit = eval_filter(P.ops, P.n_ops, vals, P.nt);
+            }
+            mbits |= (hit ? 1u : 0u) << j;
+        }
+        {
+            const u32 c = warp_sum((u32)__popc(mbits));
+            if (lane == 0) s_wcnt[warp] = c;
+        }
+        __syncthreads();
+        if (warp == 0) {
+            if (lane == 0) {
+                u32 run = 0;
+#pragma unroll
+                for (int w = 0; w < PROBE_THREADS / 32; w++) {
+                    const u32 c = s_wcnt[w];
+                    s_wcnt[w] = run;
+                    run += c;
+                }
+                s_cnt[0] = run;
+            }
+            __syncwarp();
+            const u32 total = __shfl_sync(0xffffffffu, s_cnt[0], 0);
+            const u32 ex = tile_prefix_2level(P.c.tile_state, P.c.block_state, tile, P.n_tiles, 0u, P.c.epoch, total, P.c.zero_word, P.c.total, P.c.ordered, lane);
+            if (lane == 0) {
+                s_excl[0] = ex;
+            }
+        }
+        __syncthreads();
+        if (__ballot_sync(0xffffffffu, mbits != 0u) != 0u) {
+            u32 pos = s_excl[0] + s_wcnt[warp];
+#pragma unroll
+            for (int j = 0; j < PROBE_ITEMS; j++) {
+                const bool m = (mbits >> j) & 1u;
+                const unsigned b = __ballot_sync(0xffffffffu, m);
+                if (b == 0u) continue;
+                const u32 r = pos + (u32)__popc(b & lt_mask);
+                if (m && r < P.cap) {
+                    const u32 idx = (u32)warp * (32u * PROBE_ITEMS) + (u32)j * 32u + (u32)lane;
+                    for (u32 c = 0; c < P.n_out; c++) {
+                        const OutCol oc = P.oc[c];
+                        u32 x;
+                        if (oc.kind == OUT_PROBE) x = smem[oc.a * PROBE_TILE + idx];
+                        else {
+                            u32 tv = 0;
+#pragma unroll
+                            for (int t = 0; t < T; t++) if ((u32)t == oc.a) tv = v[j][t];
+                            x = oc.kind == OUT_TABVAL ? tv : __ldg(P.tab[oc.a].pay[oc.b] + tv);
+                        }
+                        P.out[c][r] = x;
+                    }
+                }
+                pos += (u32)__popc(b);
+            }
+        }
+    }
+}
+
+static void launch_probe_direct(const ProbeDParams& p, int n_sms, cudaStream_t st) {
+    if (p.n == 0) return;
+    const size_t smem = (size_t)p.n_pcols * PROBE_TILE * sizeof(u32);
+    const void* fn = nullptr;
+    switch (p.T) {
+        case 0: fn = (const void*)probe_direct_kernel<0>; break;
+        case 1: fn = (const void*)probe_direct_kernel<1>; break;
+        case 2: fn = (const void*)probe_direct_kernel<2>; break;
+        case 3: fn = (const void*)probe_direct_kernel<3>; break;
+        default: fn = (const void*)probe_direct_kernel<4>; break;
+    }
+    if (smem > 48 * 1024) cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const int grid = grid_for(fn, PROBE_THREADS, smem, n_sms, p.n_tiles);
+    switch (p.T) {
+        case 0: probe_direct_kernel<0><<<grid, PROBE_THREADS, smem, st>>>(p); break;
+        case 1: probe_direct_kernel<1><<<grid, PROBE_THREADS, smem, st>>>(p); break;
+        case 2: probe_direct_kernel<2><<<grid, PROBE_THREADS, smem, st>>>(p); break;
+        case 3: probe_direct_kernel<3><<<grid, PROBE_THREADS, smem, st>>>(p); break;
+        default: probe_direct_kernel<4><<<grid, PROBE_THREADS, smem, st>>>(p); break;
+    }
+}
+
+// =================================================================================================================
+// K_probe (chained, binary): general natural join with 1:N matches, multi-column keys, FILTER, ordered compaction.
+// Replaces execute_optimized_hash_join_with_ids / execute_hash_join_with_ids / merge join (engine.rs:710-811, 970-1039) and
+// perform_hash_join_for_rules (shared/src/join_algorithm.rs:499-677).
+constexpr int PROBEC_THREADS = 256;
+constexpr int PROBEC_ITEMS = 2;
+constexpr int PROBEC_TILE = PROBEC_THREADS * PROBEC_ITEMS;
+struct ProbeCParams {
+    const u32* pcol[KB_MAX_COLS];
+    u32 n_pcols, n, n_tiles;
+    u32 pkey[4];  // probe columns matching tab.bkey[]
+    ChainTab tab;
+    u32 n_bpay;
+    const u32* bpay[KB_MAX_COLS];  // build columns appended to the output
+    u32 n_out;                      // = n_pcols + n_bpay
+    u32* out[KB_MAX_COLS];
+    u32 cap;
+    FilterOp ops[KB_MAX_FILTER_OPS];
+    u32 n_ops;
+    NumTab nt;
+    Compact c;
+    unsigned long long* total64;  // exact output size in 64 bits (the 32-bit positions wrap past 2^32 rows: the host checks this one)
+};
+__device__ __forceinline__ u32 warp_excl_scan(u32 v, int lane, u32* total) {
+    u32 x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const u32 y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= o) x += y;
+    }
+    *total = __shfl_sync(0xffffffffu, x, 31);
+    return x - v;
+}
+
+// Walks the chain of probe row `idx` (tile-local) and calls emit(build_row) for every build row whose key columns equal the
+// probe row's and whose joined row passes the FILTER.
+template <class Emit>
+__device__ __forceinline__ void chain_walk(const ProbeCParams& P, const u32* smem, u32 idx, Emit&& emit) {
+    const ChainTab& T = P.tab;
+    u32 pk[4];
+#pragma unroll
+    for (int q = 0; q < 4; q++) pk[q] = (u32)q < T.n_keys ? smem[P.pkey[q] * PROBEC_TILE + idx] : 0u;
+    const u32 tag = key_tag(T.n_keys, pk[0], pk[1], pk[2], pk[3]);
+    const u32 mask = T.n_slots - 1u;
+    u32 slot = mix32(tag) & mask;
+    u32 head = EMPTY32;
+    for (;;) {
+        const u64 w = __ldg(reinterpret_cast<const unsigned long long*>(T.slots) + slot);
+        const u32 key = (u32)w;
+        if (key == tag) { head = (u32)(w >> 32); break; }
+        if (key == EMPTY32) break;
+        slot = (slot + 1u) & mask;
+    }
+    for (u32 r = head; r != EMPTY32; r = __ldg(T.next + r)) {
+        bool ok = true;
+        if (T.n_keys > 1u) {
+#pragma unroll
+            for (int q = 0; q < 4; q++) if ((u32)q < T.n_keys) ok = ok && (__ldg(T.bkey[q] + r) == pk[q]);
+        }
+        if (ok && P.n_ops != 0u) {
+            u32 vals[KB_MAX_COLS];
+            for (u32 c = 0; c < P.n_pcols; c++) vals[c] = smem[c * PROBEC_TILE + idx];
+            for (u32 c = 0; c < P.n_bpay; c++) vals[P.n_pcols + c] = __ldg(P.bpay[c] + r);
+            ok = eval_filter(P.ops, P.n_ops, vals, P.nt);
+        }
+        if (ok) emit(r);
+    }
+}
+
+__global__ void __launch_bounds__(PROBEC_THREADS) probe_chained_kernel(const __grid_constant__ ProbeCParams P) {
+    extern __shared__ __align__(128) u32 smem[];
+    __shared__ __align__(8) u64 bar;
+    __shared__ u32 s_tile;
+    __shared__ u32 s_wcnt[PROBEC_THREADS / 32];
+    __shared__ u32 s_cnt[MAXP], s_excl[MAXP];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) {
+        mbar_init(&bar, 1);
+        fence_mbar_init();
+    }
+    u32 parity = 0;
+    for (;;) {
+        if (tid == 0) s_tile = atomicAdd(P.c.ticket, 1u);
+        __syncthreads();
+        const u32 tile = s_tile;
+        if (tile >= P.n_tiles) break;
+        const u32 base = tile * (u32)PROBEC_TILE;
+        const u32 cnt = min((u32)PROBEC_TILE, P.n - base);
+        if (tid == 0) {
+            const u32 bytes = (cnt * 4u + 15u) & ~15u;
+            mbar_arrive_expect_tx(&bar, bytes * P.n_pcols);
+            for (u32 c = 0; c < P.n_pcols; c++) tma_load_1d(smem + c * PROBEC_TILE, P.pcol[c] + base, bytes, &bar);
+        }
+        mbar_wait(&bar, parity);
+        parity ^= 1u;
+
+        u32 mc[PROBEC_ITEMS];
+        u32 tsum = 0;
+#pragma unroll
+        for (int j = 0; j < PROBEC_ITEMS; j++) {
+            const u32 idx = (u32)warp * (32u * PROBEC_ITEMS) + (u32)j * 32u + (u32)lane;
+            u32 c = 0;
+            if (idx < cnt) chain_walk(P, smem, idx, [&](u32) { c++; });
+            mc[j] = c;
+            tsum += c;
+        }
+        {
+            const u32 c = warp_sum(tsum);
+            if (lane == 0) s_wcnt[warp] = c;
+        }
+        __syncthreads();
+        if (warp == 0) {
+            if (lane == 0) {
+                u32 run = 0;
+#pragma unroll
+                for (int w = 0; w < PROBEC_THREADS / 32; w++) {
+                    const u32 c = s_wcnt[w];
+                    s_wcnt[w] = run;
+                    run += c;
+                }
+                s_cnt[0] = run;
+            }
+            __syncwarp();
+            const u32 total = __shfl_sync(0xffffffffu, s_cnt[0], 0);
+            const u32 ex = tile_prefix_2level(P.c.tile_state, P.c.block_state, tile, P.n_tiles, 0u, P.c.epoch, total, P.c.zero_word, P.c.total, P.c.ordered, lane);
+            if (lane == 0) {
+                s_excl[0] = ex;
+                if (total) atomicAdd(P.total64, (unsigned long long)total);
+            }
+        }
+        __syncthreads();
+        u32 pos = s_excl[0] + s_wcnt[warp];
+#pragma unroll
+        for (int j = 0; j < PROBEC_ITEMS; j++) {
+            u32 tot;
+            const u32 ex = warp_excl_scan(mc[j], lane, &tot);
+            if (mc[j] != 0u) {
+                const u32 idx = (u32)warp * (32u * PROBEC_ITEMS) + (u32)j * 32u + (u32)lane;
+                u32 r = pos + ex;
+                chain_walk(P, smem, idx, [&](u32 br) {
+                    if (r < P.cap) {
+                        for (u32 c = 0; c < P.n_pcols; c++) P.out[c][r] = smem[c * PROBEC_TILE + idx];
+                        for (u32 c = 0; c < P.n_bpay; c++) P.out[P.n_pcols + c][r] = __ldg(P.bpay[c] + br);
+                    }
+                    r++;
+                });
+            }
+            pos += tot;
+        }
+    }
+}
+
+static void launch_probe_chained(const ProbeCParams& p, int n_sms, cudaStream_t st) {
+    if (p.n == 0) return;
+    const size_t smem = (size_t)p.n_pcols * PROBEC_TILE * sizeof(u32);
+    const int grid = grid_for((const void*)probe_chained_kernel, PROBEC_THREADS, smem, n_sms, p.n_tiles);
+    probe_chained_kernel<<<grid, PROBEC_THREADS, smem, st>>>(p);
+}
+
+// =================================================================================================================
+// K_build / K_probe (grouped): 1:N equi-join on ONE key column whose ids are dense. The build side is grouped by key into a CSR
+// directory — off[key - kmin] .. off[key - kmin + 1] delimit the key's rows in payload columns permuted into key order — so a probe
+// is two directory reads and a contiguous run of payload, and the expansion can hand consecutive OUTPUT rows to consecutive threads
+// (coalesced stores). Replaces the (tag, head) + next[] chains wherever the key range allows; same bag of rows as
+// perform_hash_join_for_rules (join_algorithm.rs:499-677) / execute_hash_join_with_ids (engine.rs:710-811).
+struct CsrTab {
+    const u32* off;  // [range + 1]
+    u32 kmin, range;
+    u32 n_pay;
+    const u32* pay[KB_MAX_COLS];  // payload columns in key order
+};
+// Directory builds (count, then fill) go tile by tile through a shared-memory hash of the tile's keys: the rows of a tile that carry the
+// same key are counted / ranked with SHARED atomics and the global counter of a key is touched once per (tile, key). A Datalog
+// closure's subClassOf facts name the root class a million times, in no particular order: one global atomic per row (and per warp-level
+// group of equal keys, which random order leaves at size one) made the 2 M-row build of the transitive rule's join take
+// longer than the 331 M-row join next to it.
+constexpr u32 CSR_ITEMS = 8, CSR_TILE = 256 * CSR_ITEMS, CSR_HASH = 4096;
+struct CsrTileHash {
+    u32 key[CSR_HASH], cnt[CSR_HASH], base[CSR_HASH];
+};
+// slot of k in the tile's table (claimed when absent); the table is at most half full (2048 rows, 4096 slots)
+__device__ __forceinline__ u32 csr_slot(CsrTileHash& H, u32 k) {
+    u32 slot = mix32(k) & (CSR_HASH - 1u);
+    for (;;) {
+        u32 cur = *reinterpret_cast<volatile u32*>(&H.key[slot]);
+        if (cur == EMPTY32) cur = atomicCAS(&H.key[slot], EMPTY32, k);
+        if (cur == EMPTY32 || cur == k) return slot;
+        slot = (slot + 1u) & (CSR_HASH - 1u);
+    }
+}
+__global__ void __launch_bounds__(256) csr_count_kernel(const u32* __restrict__ keys, u32 n, u32 kmin, u32* __restrict__ counts) {
+    __shared__ CsrTileHash H;
+    for (u32 i = threadIdx.x; i < CSR_HASH; i += 256u) { H.key[i] = EMPTY32; H.cnt[i] = 0u; }
+    __syncthreads();
+    const u32 n_tiles = (n + CSR_TILE - 1u) / CSR_TILE;
+    for (u32 tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const u32 row0 = tile * CSR_TILE;
+        u32 k[CSR_ITEMS], slot[CSR_ITEMS];
+        bool lead[CSR_ITEMS];
+#pragma unroll
+        for (u32 j = 0; j < CSR_ITEMS; j++) {
+            const u32 i = row0 + j * 256u + threadIdx.x;
+            k[j] = i < n ? keys[i] - kmin : EMPTY32;
+        }
+#pragma unroll
+        for (u32 j = 0; j < CSR_ITEMS; j++) {
+            lead[j] = false;
+            if (k[j] == EMPTY32) continue;
+            slot[j] = csr_slot(H, k[j]);
+            lead[j] = atomicAdd(&H.cnt[slot[j]], 1u) == 0u;  // the first row of the key in this tile speaks for it
+        }
+        __syncthreads();
+#pragma unroll
+        for (u32 j = 0; j < CSR_ITEMS; j++) if (lead[j]) atomicAdd(&counts[k[j]], H.cnt[slot[j]]);
+        __syncthreads();
+#pragma unroll
+        for (u32 j = 0; j < CSR_ITEMS; j++) if (lead[j]) { H.key[slot[j]] = EMPTY32; H.cnt[slot[j]] = 0u; }
+        __syncthreads();
+    }
+}
+static void launch_csr_count(const u32* keys, u32 n, u32 kmin, u32* counts, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    const int grid = grid_1d(n, n_sms, CSR_TILE, 4);
+    csr_count_kernel<<<grid, 256, 0, st>>>(keys, n, kmin, counts);
+}
+
+struct CsrFillParams {
+    const u32* keys;
+    u32 n, kmin, n_pay;
+    u32* cursor;
+    const u32* pay_in[KB_MAX_COLS];
+    u32* pay_out[KB_MAX_COLS];
+};
+__global__ void __launch_bounds__(256) csr_fill_kernel(const __grid_constant__ CsrFillParams P) {
+    __shared__ CsrTileHash H;
+    for (u32 i = threadIdx.x; i < CSR_HASH; i += 256u) { H.key[i] = EMPTY32; H.cnt[i] = 0u; }
+    __syncthreads();
+    const u32 n_tiles = (P.n + CSR_TILE - 1u) / CSR_TILE;
+    for (u32 tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const u32 row0 = tile * CSR_TILE;
+        u32 k[CSR_ITEMS], slot[CSR_ITEMS], rank[CSR_ITEMS];
+#pragma unroll
+        for (u32 j = 0; j < CSR_ITEMS; j++) {
+            const u32 i = row0 + j * 256u + threadIdx.x;
+            k[j] = i < P.n ? P.keys[i] - P.kmin : EMPTY32;
+        }
+#pragma unroll
+        for (u32 j = 0; j < CSR_ITEMS; j++) {
+            rank[j] = EMPTY32;
+            if (k[j] == EMPTY32) continue;
+            slot[j] = csr_slot(H, k[j]);
+            rank[j] = atomicAdd(&H.cnt[slot[j]], 1u);
+        }
+        __syncthreads();
+#pragma unroll
+        for (u32 j = 0; j < CSR_ITEMS; j++)  // one range of the key's run per (tile, key)
+            if (rank[j] == 0u) H.base[slot[j]] = atomicAdd(&P.cursor[k[j]], H.cnt[slot[j]]);
+        __syncthreads();
+#pragma unroll
+        for (u32 j = 0; j < CSR_ITEMS; j++) {
+            if (rank[j] == EMPTY32) continue;
+            const u32 i = row0 + j * 256u + threadIdx.x;
+            const u32 pos = H.base[slot[j]] + rank[j];
+            for (u32 c = 0; c < P.n_pay; c++) P.pay_out[c][pos] = P.pay_in[c][i];
+        }
+        __syncthreads();
+#pragma unroll
+        for (u32 j = 0; j < CSR_ITEMS; j++) if (rank[j] == 0u) { H.key[slot[j]] = EMPTY32; H.cnt[slot[j]] = 0u; }
+        __syncthreads();
+    }
+}
+static void launch_csr_fill(const u32* keys, u32 n, u32 kmin, u32* cursor, const u32* const* pay_in, u32* const* pay_out, u32 n_pay, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    CsrFillParams P{};
+    P.keys = keys; P.n = n; P.kmin = kmin; P.n_pay = n_pay; P.cursor = cursor;
+    for (u32 c = 0; c < n_pay; c++) { P.pay_in[c] = pay_in[c]; P.pay_out[c] = pay_out[c]; }
+    const int grid = grid_1d(n, n_sms, CSR_TILE, 4);
+    csr_fill_kernel<<<grid, 256, 0, st>>>(P);
+}
+
+__global__ void __launch_bounds__(256) csr_total_kernel(const u32* __restrict__ pk, u32 n, const u32* __restrict__ off, u32 kmin, u32 range,
+                                                        unsigned long long* total) {
+    const u32 stride = gridDim.x * blockDim.x;
+    unsigned long long t = 0;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        const u32 o = pk[i] - kmin;
+        if (o < range) t += (unsigned long long)(__ldg(off + o + 1) - __ldg(off + o));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+    if ((threadIdx.x & 31) == 0 && t) atomicAdd(total, t);
+}
+static void launch_csr_total(const u32* pkeys, u32 n, const CsrTab& tab, unsigned long long* total, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    const int grid = grid_1d(n, n_sms);
+    csr_total_kernel<<<grid, 256, 0, st>>>(pkeys, n, tab.off, tab.kmin, tab.range, total);
+}
+
+constexpr int PROBEG_THREADS = 256;
+constexpr int PROBEG_ITEMS = 4;
+constexpr int PROBEG_TILE = PROBEG_THREADS * PROBEG_ITEMS;
+struct ProbeGParams {
+    const u32* pcol[KB_MAX_COLS];
+    u32 n_pcols, n, n_tiles;
+    u32 pkey;  // probe column holding the key
+    CsrTab tab;
+    u32* out[KB_MAX_COLS];  // n_pcols probe columns, then tab.n_pay payload columns
+    u32 cap;
+    Compact c;
+    // tiles whose expansion exceeds PROBEG_HEAVY output rows are not expanded by the CTA that scanned them: it appends them here
+    // (heavy_count[0] entries) and a second launch spreads each one's output range over the whole grid in PROBEG_CHUNK-row pieces
+    struct Heavy { u32 tile, gbase, total, pad; };
+    Heavy* heavy;        // room for n_tiles entries (null: no splitting)
+    u32* heavy_count;    // zeroed control word
+};
+constexpr u32 PROBEG_HEAVY = 32768, PROBEG_CHUNK = 4096;
+// One tile = 1024 probe rows staged by TMA. Pass 1: every row reads its directory entry (begin, count); the counts are scanned over the
+// tile. Pass 2: output row r of the tile belongs to the probe row whose prefix range holds r (binary search in shared memory), so
+// consecutive threads write consecutive output rows and read consecutive payload rows.
+// Skew: a probe row may match 10^5 build rows (the closure of a class tree joined on the ancestor), and a tile of such rows used to be
+// expanded by the ONE CTA that scanned it — the 2 M x 5 M-row join of the transitive rule ran on a handful of SMs. A tile whose
+// expansion exceeds PROBEG_HEAVY rows is now only recorded by the first launch (HEAVY = false); the second launch (HEAVY = true) walks
+// the recorded tiles, every CTA re-stages the tile and expands its share of PROBEG_CHUNK-row pieces.
+template <bool HEAVY>
+__global__ void __launch_bounds__(PROBEG_THREADS) probe_grouped_kernel(const __grid_constant__ ProbeGParams P) {
+    extern __shared__ __align__(128) u32 smem[];  // n_pcols tiles, then begin[TILE], pref[TILE]
+    u32* s_begin = smem + P.n_pcols * PROBEG_TILE;
+    u32* s_pref = s_begin + PROBEG_TILE;
+    __shared__ __align__(8) u64 bar;
+    __shared__ u32 s_tile;
+    __shared__ u32 s_w[PROBEG_THREADS / 32 + 1];
+    __shared__ u32 s_base;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) {
+        mbar_init(&bar, 1);
+        fence_mbar_init();
+    }
+    u32 parity = 0;
+    const u32* sKey = smem + P.pkey * PROBEG_TILE;
+    const u32 n_heavy = HEAVY ? *reinterpret_cast<volatile u32*>(P.heavy_count) : 0u;
+    u32 h_next = 0;  // HEAVY: next recorded tile to look at
+    for (;;) {
+        __syncthreads();  // the previous tile's expansion has finished reading shared memory
+        u32 h_gbase = 0, h_total = 0;
+        if constexpr (HEAVY) {
+            // the recorded tiles in list order; a CTA takes part in a tile when it has at least one piece of it
+            u32 t = EMPTY32;
+            while (h_next < n_heavy) {
+                const ProbeGParams::Heavy e = P.heavy[h_next++];
+                const u32 pieces = (e.total + PROBEG_CHUNK - 1u) / PROBEG_CHUNK;
+                if (blockIdx.x < pieces) { t = e.tile; h_gbase = e.gbase; h_total = e.total; break; }
+            }
+            if (tid == 0) s_tile = t;
+        } else if (tid == 0) s_tile = atomicAdd(P.c.ticket, 1u);
+        __syncthreads();
+        const u32 tile = s_tile;
+        if (tile >= P.n_tiles) break;
+        if (tid == 0) {
+            const u32 b = tile * (u32)PROBEG_TILE;
+            const u32 c = min((u32)PROBEG_TILE, P.n - b);
+            const u32 bytes = (c * 4u + 15u) & ~15u;
+            mbar_arrive_expect_tx(&bar, bytes * P.n_pcols);
+            for (u32 q = 0; q < P.n_pcols; q++) tma_load_1d(smem + q * PROBEG_TILE, P.pcol[q] + b, bytes, &bar);
+        }
+        const u32 cnt = min((u32)PROBEG_TILE, P.n - tile * (u32)PROBEG_TILE);
+        mbar_wait(&bar, parity);
+        parity ^= 1u;
+        // pass 1: directory reads (all of a thread's rows in flight together), warp-local exclusive scan in row order
+        u32 b[PROBEG_ITEMS], c[PROBEG_ITEMS];
+#pragma unroll
+        for (int j = 0; j < PROBEG_ITEMS; j++) {
+            const u32 idx = (u32)warp * (32u * PROBEG_ITEMS) + (u32)j * 32u + (u32)lane;
+            const u32 o = sKey[idx] - P.tab.kmin;
+            const bool ok = idx < cnt && o < P.tab.range;
+            b[j] = ok ? __ldg(P.tab.off + o) : 0u;
+            c[j] = ok ? __ldg(P.tab.off + o + 1) : 0u;
+        }
+        u32 run = 0;
+#pragma unroll
+        for (int j = 0; j < PROBEG_ITEMS; j++) {
+            const u32 idx = (u32)warp * (32u * PROBEG_ITEMS) + (u32)j * 32u + (u32)lane;
+            const u32 n_match = c[j] - b[j];
+            u32 incl = n_match;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const u32 y = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl += y;
+            }
+            s_begin[idx] = b[j];
+            s_pref[idx] = run + incl - n_match;  // exclusive within the warp's 128 rows; the warp base is added below
+            run += __shfl_sync(0xffffffffu, incl, 31);
+        }
+        if (lane == 0) s_w[warp] = run;
+        __syncthreads();
+        if (warp == 0) {
+            const u32 w = lane < PROBEG_THREADS / 32 ? s_w[lane] : 0u;
+            u32 wi = w;
+#pragma unroll
+            for (int o = 1; o < PROBEG_THREADS / 32; o <<= 1) {
+                const u32 y = __shfl_up_sync(0xffffffffu, wi, o);
+                if (lane >= o) wi += y;
+            }
+            const u32 total = __shfl_sync(0xffffffffu, wi, PROBEG_THREADS / 32 - 1);
+            if (lane < PROBEG_THREADS / 32) s_w[lane] = wi - w;
+            if (lane == 0) s_w[PROBEG_THREADS / 32] = total;
+            if (!HEAVY) {
+                const u32 ex = tile_prefix_2level(P.c.tile_state, P.c.block_state, tile, P.n_tiles, 0u, P.c.epoch, total, P.c.zero_word, P.c.total, P.c.ordered, lane);
+                if (lane == 0) {
+                    s_base = ex;
+                    if (P.heavy && total > PROBEG_HEAVY) {  // recorded for the second launch
+                        ProbeGParams::Heavy e;
+                        e.tile = tile; e.gbase = ex; e.total = total; e.pad = 0u;
+                        P.heavy[atomicAdd(P.heavy_count, 1u)] = e;
+                    }
+                }
+            }
+        }
+        __syncthreads();
+        {
+            const u32 wb = s_w[warp];
+#pragma unroll
+            for (int j = 0; j < PROBEG_ITEMS; j++) s_pref[(u32)warp * (32u * PROBEG_ITEMS) + (u32)j * 32u + (u32)lane] += wb;
+        }
+        __syncthreads();
+        // pass 2: load-balanced expansion
+        const u32 total = s_w[PROBEG_THREADS / 32];
+        const u32 gbase = HEAVY ? h_gbase : s_base;
+        if (!HEAVY && P.heavy && total > PROBEG_HEAVY) continue;
+        const u32 pieces = HEAVY ? (h_total + PROBEG_CHUNK - 1u) / PROBEG_CHUNK : 1u;
+        for (u32 piece = HEAVY ? blockIdx.x : 0u; piece < pieces; piece += gridDim.x) {
+            const u32 r0 = HEAVY ? piece * PROBEG_CHUNK : 0u;
+            const u32 r1 = HEAVY ? min(total, r0 + PROBEG_CHUNK) : total;
+            for (u32 r = r0 + (u32)tid; r < r1; r += PROBEG_THREADS) {
+                u32 lo = 0, hi = PROBEG_TILE - 1;  // largest idx with pref[idx] <= r
+#pragma unroll
+                for (int step = 0; step < 10; step++) {
+                    const u32 mid = (lo + hi + 1u) >> 1;
+                    if (s_pref[mid] <= r) lo = mid; else hi = mid - 1u;
+                }
+                const u32 src = lo;
+                const u32 brow = s_begin[src] + (r - s_pref[src]);
+                const u32 pos = gbase + r;
+                if (pos < P.cap) {
+                    for (u32 q = 0; q < P.n_pcols; q++) P.out[q][pos] = smem[q * PROBEG_TILE + src];
+                    for (u32 q = 0; q < P.tab.n_pay; q++) P.out[P.n_pcols + q][pos] = __ldg(P.tab.pay[q] + brow);
+                }
+            }
+        }
+    }
+}
+static void launch_probe_grouped(const ProbeGParams& p, int n_sms, cudaStream_t st) {
+    if (p.n == 0) return;
+    const size_t smem = (size_t)(p.n_pcols + 2) * PROBEG_TILE * sizeof(u32);
+    if (smem > 48 * 1024) {
+        cudaFuncSetAttribute(probe_grouped_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaFuncSetAttribute(probe_grouped_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    }
+    const int grid = grid_for((const void*)probe_grouped_kernel<false>, PROBEG_THREADS, smem, n_sms, p.n_tiles);
+    probe_grouped_kernel<false><<<grid, PROBEG_THREADS, smem, st>>>(p);
+    if (p.heavy) {  // the recorded heavy tiles (usually none: the launch then finds an empty list and ends)
+        const int grid2 = grid_for((const void*)probe_grouped_kernel<true>, PROBEG_THREADS, smem, n_sms, 1u << 20);
+        probe_grouped_kernel<true><<<grid2, PROBEG_THREADS, smem, st>>>(p);
+    }
+}
+
+// cartesian product: output row (i*nr + j) = left row i ++ right row j (engine.rs:1054-1071)
+struct CartParams {
+    const u32* l[KB_MAX_COLS];
+    const u32* r[KB_MAX_COLS];
+    u32* out[KB_MAX_COLS];
+    u32 nl, nr, n_l, n_r;
+};
+__global__ void cartesian_kernel(const CartParams P) {
+    const u64 total = (u64)P.nl * P.nr;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (u64)gridDim.x * blockDim.x) {
+        const u32 li = (u32)(i / P.nr), ri = (u32)(i % P.nr);
+        for (u32 c = 0; c < P.n_l; c++) P.out[c][i] = P.l[c][li];
+        for (u32 c = 0; c < P.n_r; c++) P.out[P.n_l + c][i] = P.r[c][ri];
+    }
+}
+static void launch_cartesian(const u32* const* lcols, u32 nl, u32 n_lcols, const u32* const* rcols, u32 nr, u32 n_rcols, u32* const* out,
+                             cudaStream_t st) {
+    CartParams P;
+    P.nl = nl; P.nr = nr; P.n_l = n_lcols; P.n_r = n_rcols;
+    for (u32 c = 0; c < n_lcols; c++) P.l[c] = lcols[c];
+    for (u32 c = 0; c < n_rcols; c++) P.r[c] = rcols[c];
+    for (u32 c = 0; c < n_lcols + n_rcols; c++) P.out[c] = out[c];
+    const u64 total = (u64)nl * nr;
+    if (total == 0) return;
+    int grid = grid_1d(total, (int)H100_SMS);
+    cartesian_kernel<<<grid, 256, 0, st>>>(P);
+}
 
 // AND the program `f` into `dst`
 static void and_into(FilterProg* dst, const FilterProg& f) {

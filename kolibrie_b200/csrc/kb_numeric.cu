@@ -14,6 +14,7 @@
 
 #include "kb_internal.hpp"
 #include "kb_numparse.cuh"
+#include "kb_numrank.cuh"
 
 namespace kb {
 
@@ -91,6 +92,25 @@ static kb_status numeric_grow(kb_ctx* ctx, Buf* a, Buf* b, size_t elem_a, u32 ke
     *a = na;
     *b = nb;
     return KB_OK;
+}
+
+// the value order's keys (kb_numrank.cuh: order_key / order_value); id n is the extra 0.0
+__global__ void __launch_bounds__(256) numorder_keys_kernel(const double* __restrict__ num, u32 n, unsigned long long* __restrict__ keys) {
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += (u64)gridDim.x * blockDim.x) keys[i] = kb_nr::order_key(i < n ? num[i] : 0.0);
+}
+__global__ void __launch_bounds__(256) numorder_values_kernel(const unsigned long long* __restrict__ keys, u32 n, double* __restrict__ out) {
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = kb_nr::order_value(keys[i]);
+}
+// the value order of the numeric side table: keys[i] = order-preserving u64 of fold(num_or0[i]) for i < n, of 0.0 for i == n and for NaN
+static void launch_numorder_keys(const double* num_or0, u32 n, unsigned long long* keys, int n_sms, cudaStream_t st) {
+    const int grid = grid_1d((u64)n + 1, n_sms);
+    numorder_keys_kernel<<<grid, 256, 0, st>>>(num_or0, n, keys);
+}
+// the inverse, over the sorted distinct keys
+static void launch_numorder_values(const unsigned long long* keys, u32 n, double* out, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    const int grid = grid_1d(n, n_sms);
+    numorder_values_kernel<<<grid, 256, 0, st>>>(keys, n, out);
 }
 
 // The value order V of the f64 table (kb_numrank.cuh): every value as an order-preserving u64 key (NaN as 0.0, -0.0 as +0.0, one extra

@@ -1,5 +1,5 @@
 // kb_numrank.cuh — the value order of the numeric side table, as __host__ __device__ code: the device (the rank fills of the store
-// index, kb_kernels.cu), the host (a FILTER resolved to a rank range, kb_api.cu) and a host build of the same lines
+// index, kb_store.cu), the host (a FILTER resolved to a rank range, kb_api.cu) and a host build of the same lines
 // (tests/test_numrank_cpu.py, g++) run exactly these lines.
 //
 // V = the sorted distinct non-NaN values of num_or0 over all ids, -0.0 folded into +0.0, 0.0 always included (num_of answers 0.0 for

@@ -10,6 +10,175 @@
 
 using namespace kb;
 
+namespace kb {
+
+// ---------------------------------------------------------------------------------------------------------------
+// Relation-to-Stream operators (kb_r2s_eval; Relation2StreamOperator::eval, r2s.rs:37-58). A set of rows is an open-addressing table
+// of u32 row indices (EMPTY32 = free slot) keyed by a 64-bit mix of the row's columns in the operator's slot order; a hash hit is
+// confirmed by comparing every column.
+struct R2sRows {
+    const u32* col[KB_MAX_COLS];  // columns in the operator's slot order
+    u32 n;
+    u32* tab;                     // table over the rows (unused when n == 0)
+    u32 mask;                     // table slots - 1
+};
+struct R2sParams {
+    R2sRows cur;      // the response: its table is built, then remapped to the new state's columns
+    R2sRows last;     // the previous state (read only)
+    u32 n_cols;
+    u32 probe_last;   // ISTREAM: flag the response rows whose tuple `last` does not hold
+    u32* rep;         // [cur.n] 1 where row i is its tuple's representative (first occurrence); then its exclusive prefix
+    u32* slot_of;     // [cur.n] table slot of row i's tuple
+    u32* emit;        // ISTREAM: [cur.n] emitted response rows; DSTREAM: [last.n] rows of `last` that are gone (flags, then prefix)
+    u32* counts;      // [2] zeroed: representatives, emitted rows
+    u32 n_rep, n_emit;  // write passes: the totals of the two flag arrays
+    u32* out_state[KB_MAX_COLS];
+    u32* out_emit[KB_MAX_COLS];
+};
+
+// =================================================================================================================
+// Relation-to-Stream operators (kb_r2s_eval). Row indices are 64-bit in the loops: a response may hold up to 2^32-1 rows.
+__device__ __forceinline__ u64 r2s_mix64(u64 x) {  // murmur3 64-bit finaliser
+    x ^= x >> 33; x *= 0xff51afd7ed558ccdull; x ^= x >> 33; x *= 0xc4ceb9fe1a85ec53ull; x ^= x >> 33;
+    return x;
+}
+// home slot of row i: the columns are mixed in order, so rows that differ only by swapping two columns' values hash apart
+__device__ __forceinline__ u32 r2s_home(const u32* const* col, u32 n_cols, u32 i, u32 mask) {
+    u64 h = 0x9E3779B97F4A7C15ull;
+    for (u32 c = 0; c < n_cols; c++) h = r2s_mix64(h ^ (u64)col[c][i]);
+    return (u32)h & mask;
+}
+__device__ __forceinline__ bool r2s_equal(const u32* const* a, u32 ia, const u32* const* b, u32 ib, u32 n_cols) {
+    for (u32 c = 0; c < n_cols; c++)
+        if (a[c][ia] != b[c][ib]) return false;
+    return true;
+}
+// does the set T hold the tuple of row i of `col`?
+__device__ __forceinline__ bool r2s_contains(const R2sRows& T, const u32* const* col, u32 i, u32 n_cols) {
+    if (T.n == 0u) return false;
+    u32 slot = r2s_home(col, n_cols, i, T.mask);
+    while (true) {
+        const u32 held = T.tab[slot];
+        if (held == EMPTY32) return false;
+        if (r2s_equal(T.col, held, col, i, n_cols)) return true;
+        slot = (slot + 1u) & T.mask;
+    }
+}
+// warp-aggregated count of the lanes whose flag is set (every lane of the warp calls it)
+__device__ __forceinline__ void r2s_count(bool flag, u32* counter) {
+    const u32 b = __ballot_sync(0xffffffffu, flag);
+    if ((threadIdx.x & 31u) == 0u && b) atomicAdd(counter, (u32)__popc(b));
+}
+
+__global__ void __launch_bounds__(256) r2s_build_kernel(const __grid_constant__ R2sParams P) {
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x; k < P.cur.n; k += stride) {
+        const u32 i = (u32)k;
+        u32 slot = r2s_home(P.cur.col, P.n_cols, i, P.cur.mask);
+        while (true) {
+            u32 held = *(volatile u32*)&P.cur.tab[slot];
+            if (held == EMPTY32) {
+                held = atomicCAS(&P.cur.tab[slot], EMPTY32, i);
+                if (held == EMPTY32) break;
+            }
+            // a slot only ever moves to a smaller index of the same tuple: the comparison with `held` stays valid
+            if (r2s_equal(P.cur.col, held, P.cur.col, i, P.n_cols)) {
+                if (held > i) atomicMin(&P.cur.tab[slot], i);
+                break;
+            }
+            slot = (slot + 1u) & P.cur.mask;
+        }
+    }
+}
+__global__ void __launch_bounds__(256) r2s_mark_kernel(const __grid_constant__ R2sParams P) {
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    const u64 n_round = ((u64)P.cur.n + 31ull) & ~31ull;
+    for (u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x; k < n_round; k += stride) {
+        bool rep = false, emit = false;
+        if (k < P.cur.n) {
+            const u32 i = (u32)k;
+            u32 slot = r2s_home(P.cur.col, P.n_cols, i, P.cur.mask);
+            u32 held;
+            while (true) {  // the tuple was inserted: it is found before any free slot
+                held = P.cur.tab[slot];
+                if (held != EMPTY32 && r2s_equal(P.cur.col, held, P.cur.col, i, P.n_cols)) break;
+                slot = (slot + 1u) & P.cur.mask;
+            }
+            rep = held == i;
+            P.rep[i] = rep ? 1u : 0u;
+            P.slot_of[i] = slot;
+            if (P.probe_last) {
+                emit = !r2s_contains(P.last, P.cur.col, i, P.n_cols);
+                P.emit[i] = emit ? 1u : 0u;
+            }
+        }
+        r2s_count(rep, &P.counts[0]);
+        r2s_count(emit, &P.counts[1]);
+    }
+}
+__global__ void __launch_bounds__(256) r2s_gone_mark_kernel(const __grid_constant__ R2sParams P) {
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    const u64 n_round = ((u64)P.last.n + 31ull) & ~31ull;
+    for (u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x; k < n_round; k += stride) {
+        bool gone = false;
+        if (k < P.last.n) {
+            gone = !r2s_contains(P.cur, P.last.col, (u32)k, P.n_cols);
+            P.emit[k] = gone ? 1u : 0u;
+        }
+        r2s_count(gone, &P.counts[1]);
+    }
+}
+// a row is taken iff its exclusive prefix differs from the next row's (the last row: from the total)
+__device__ __forceinline__ bool r2s_taken(const u32* off, u64 k, u64 n, u32 total, u32* at) {
+    *at = off[k];
+    return (k + 1ull < n ? off[k + 1] : total) != *at;
+}
+__global__ void __launch_bounds__(256) r2s_write_kernel(const __grid_constant__ R2sParams P) {
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x; k < P.cur.n; k += stride) {
+        const u32 i = (u32)k;
+        u32 at;
+        if (r2s_taken(P.rep, k, P.cur.n, P.n_rep, &at)) {
+            for (u32 c = 0; c < P.n_cols; c++) P.out_state[c][at] = P.cur.col[c][i];
+            P.cur.tab[P.slot_of[i]] = at;  // the table now indexes the new state's columns
+        }
+        if (P.probe_last && r2s_taken(P.emit, k, P.cur.n, P.n_emit, &at))
+            for (u32 c = 0; c < P.n_cols; c++) P.out_emit[c][at] = P.cur.col[c][i];
+    }
+}
+__global__ void __launch_bounds__(256) r2s_gone_write_kernel(const __grid_constant__ R2sParams P) {
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x; k < P.last.n; k += stride) {
+        u32 at;
+        if (r2s_taken(P.emit, k, P.last.n, P.n_emit, &at))
+            for (u32 c = 0; c < P.n_cols; c++) P.out_emit[c][at] = P.last.col[c][(u32)k];
+    }
+}
+// build: every response row goes into cur's table (atomicCAS on a free slot, atomicMin on a slot holding an equal row: the slot ends
+// up holding the tuple's first occurrence, whatever the thread order)
+static void launch_r2s_build(const R2sParams& p, int n_sms, cudaStream_t st) {
+    if (p.cur.n) r2s_build_kernel<<<grid_1d(p.cur.n, n_sms), 256, 0, st>>>(p);
+}
+// mark: rep, slot_of and, with probe_last, emit (+ counts)
+static void launch_r2s_mark(const R2sParams& p, int n_sms, cudaStream_t st) {
+    if (p.cur.n) r2s_mark_kernel<<<grid_1d(p.cur.n, n_sms), 256, 0, st>>>(p);
+}
+// DSTREAM mark: emit[j] = row j of `last` has no equal row in the response (+ counts[1]); runs before the remap
+static void launch_r2s_gone_mark(const R2sParams& p, int n_sms, cudaStream_t st) {
+    if (p.last.n) r2s_gone_mark_kernel<<<grid_1d(p.last.n, n_sms), 256, 0, st>>>(p);
+}
+// write, after the exclusive scans: the representatives into out_state (and cur's table remapped to them), with probe_last the
+// emitted rows into out_emit
+static void launch_r2s_write(const R2sParams& p, int n_sms, cudaStream_t st) {
+    if (p.cur.n) r2s_write_kernel<<<grid_1d(p.cur.n, n_sms), 256, 0, st>>>(p);
+}
+// DSTREAM write: the gone rows of `last` into out_emit, in `last` order
+static void launch_r2s_gone_write(const R2sParams& p, int n_sms, cudaStream_t st) {
+    if (p.last.n) r2s_gone_write_kernel<<<grid_1d(p.last.n, n_sms), 256, 0, st>>>(p);
+}
+
+}  // namespace kb
+
 struct kb_r2s {
     u32 op = KB_RSTREAM;
     std::vector<u32> slots;  // column order of every row the operator compares, stores and emits

@@ -2,15 +2,646 @@
 // seeded fixpoint's state, kb_datalog_maintain's closed token), the per-version hints of the star-join builds and the
 // predicate-partitioned index. This file is the only writer of that state: every change to the store goes through store_replace,
 // store_add_device_segment, store_evict_tag or store_swap, which bump the version, drop the hints and maintain or drop the index.
+// The kernels behind those changes (the index's profile, split, clear, table, code and rank passes, the key sets of INSERT and DELETE,
+// the DELETE-template fill) and their launch formats are in this file too.
 #include <algorithm>
 #include <chrono>
 #include <cstdlib>
 
 #include "kb_internal.hpp"
+#include "kb_numrank.cuh"
 
 using namespace kb;
 
 namespace kb {
+
+// ctrl = {overflow, values inserted}. A value already in the set costs a plain load, never an atomic: a column of a few values
+// repeated millions of times does not serialise on their slots. Every warp stops at its next row once the overflow word is set.
+__global__ void __launch_bounds__(256) distinct_kernel(const u32* __restrict__ col, u32 n, u32* set, u32 set_slots, u32 limit, u32* ctrl) {
+    const int lane = threadIdx.x & 31;
+    const u32 mask = set_slots - 1u;
+    const u32 n_round = (n + 31u) & ~31u;
+    u32 last = EMPTY32;  // values come in long runs in real stores: skip what this lane just inserted
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += gridDim.x * blockDim.x) {
+        u32 stop = lane == 0 ? *reinterpret_cast<volatile u32*>(&ctrl[0]) : 0u;
+        if (__shfl_sync(0xffffffffu, stop, 0)) break;
+        const bool valid = i < n;
+        const u32 v = valid ? col[i] : EMPTY32;
+        const bool fresh = valid && v != EMPTY32 && v != last;
+        const unsigned act = __ballot_sync(0xffffffffu, fresh);
+        if (!fresh) continue;
+        const unsigned peers = __match_any_sync(act, v);
+        last = v;
+        if (lane != __ffs(peers) - 1) continue;
+        u32 slot = mix32(v) & mask;
+        for (u32 probes = 0;; probes++) {
+            if (probes >= set_slots) { ctrl[0] = 1u; break; }
+            const u32 cur = *reinterpret_cast<volatile u32*>(&set[slot]);
+            if (cur == v) break;
+            if (cur == EMPTY32) {
+                const u32 old = atomicCAS(&set[slot], EMPTY32, v);
+                if (old == EMPTY32) {
+                    if (atomicAdd(&ctrl[1], 1u) >= limit) ctrl[0] = 1u;
+                    break;
+                }
+                if (old == v) break;
+            }
+            slot = (slot + 1u) & mask;
+        }
+    }
+}
+// distinct values of a column other than EMPTY32 into a small open-addressing set (EMPTY32 = free). ctrl = {overflow, count}, both 0
+// at launch: the overflow word is set when the set fills up or when a value past the first `limit` arrives, and ends the pass
+static void launch_distinct(const u32* col, u32 n, u32* set, u32 set_slots, u32 limit, u32* ctrl, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    int grid = grid_1d(n, n_sms, 256, 4);
+    distinct_kernel<<<grid, 256, 0, st>>>(col, n, set, set_slots, limit, ctrl);
+}
+
+// one-byte codes of a subject table (PredSlice::xcode): code[i] = index of tab[i] in the ascending dictionary, 0xFF where tab[i] is
+// EMPTY32; four slots per thread, one 16-byte load and one 4-byte store
+__global__ void __launch_bounds__(256) tab_code_kernel(const u32* __restrict__ tab, u32 range, const u32* __restrict__ dict, u32 n_dict,
+                                                       u8* __restrict__ code) {
+    __shared__ u32 s_dict[CODE_MAX];
+    for (u32 i = threadIdx.x; i < n_dict; i += blockDim.x) s_dict[i] = dict[i];
+    __syncthreads();
+    const u32 quads = (range + 3u) / 4u;
+    for (u32 q = blockIdx.x * blockDim.x + threadIdx.x; q < quads; q += gridDim.x * blockDim.x) {
+        const uint4 v4 = __ldg(reinterpret_cast<const uint4*>(tab) + q);  // (the buffer is padded past the table's last slot)
+        const u32 v[4] = {v4.x, v4.y, v4.z, v4.w};
+        u32 packed = 0;
+#pragma unroll
+        for (u32 k = 0; k < 4; k++) {
+            u32 c = 0xFFu;
+            if (4u * q + k < range && v[k] != EMPTY32) {
+                u32 lo = 0, hi = n_dict;  // the first entry >= v: v is in the dictionary
+                while (lo < hi) {
+                    const u32 mid = (lo + hi) / 2u;
+                    if (s_dict[mid] < v[k]) lo = mid + 1u;
+                    else hi = mid;
+                }
+                c = lo;
+            }
+            packed |= c << (8u * k);
+        }
+        reinterpret_cast<u32*>(code)[q] = packed;
+    }
+}
+// code[i] = index of tab[i] in dict (ascending, every value of tab but EMPTY32, n_dict <= CODE_MAX), 0xFF where tab[i] is EMPTY32, for
+// i < range; tab and code start 16-byte aligned and may be read / written up to the next multiple of 4 slots
+static void launch_tab_code(const u32* tab, u32 range, const u32* dict, u32 n_dict, u8* code, int n_sms, cudaStream_t st) {
+    if (range == 0) return;
+    const int grid = grid_1d(range, n_sms, 1024);
+    tab_code_kernel<<<grid, 256, 0, st>>>(tab, range, dict, n_dict, code);
+}
+
+// ---- window-slide maintenance of the store index: ONE pass profiles a new segment (column ranges, foreign subjects, its distinct
+// predicates with their row counts), ONE pass splits it into the predicate slices' new chunks — pairs, id ranges, typed literal
+// column, in-place inserts into the persistent tables — and ONE pass clears an evicted segment's keys from all of its slices' tables.
+constexpr u32 SEGP_SLOTS = 32;  // open-addressing slots for a segment's distinct predicates (more than that: the batched scan path)
+// control words of segment_profile: [0..2] min s/p/o, [3] unused, [4 .. 4+SLOTS) predicate slots (all 0xFF at launch);
+// then (all 0 at launch) [P_MAX .. +3) max s/p/o, P_FOREIGN, P_OVERFLOW, [P_COUNT .. +SLOTS) rows per slot
+constexpr u32 SEGP_MIN = 0, SEGP_SLOT = 4, SEGP_MAX = 4 + SEGP_SLOTS, SEGP_FOREIGN = SEGP_MAX + 3, SEGP_OVERFLOW = SEGP_MAX + 4, SEGP_COUNT = SEGP_MAX + 8,
+              SEGP_WORDS = SEGP_COUNT + SEGP_SLOTS;
+// One pass over a new segment: id range of the three columns, subjects that belong to another shard, and the segment's distinct
+// predicates with their row counts (32 open-addressing slots in the control words; a 33rd predicate raises the overflow word and the
+// caller takes the batched scan path). Predicates come in short runs (one employee = six consecutive triples), so a warp holds a
+// handful of distinct values: one probe sequence and one count atomic per (warp, value).
+__global__ void __launch_bounds__(256) segment_profile_kernel(const u32* __restrict__ s, const u32* __restrict__ p, const u32* __restrict__ o, u32 n, u32 rank,
+                                                              u32 world, u32* ctrl) {
+    // per CTA: its own 32-slot table (value, rows) in shared memory, merged into the control words once at the end — the global table
+    // sees one probe sequence and one add per (CTA, predicate) instead of one per (warp, predicate) and iteration
+    __shared__ u32 s_key[SEGP_SLOTS], s_cnt[SEGP_SLOTS];
+    __shared__ u32 s_over, s_foreign, s_mn[3], s_mx[3];
+    const int lane = threadIdx.x & 31;
+    if (threadIdx.x < SEGP_SLOTS) { s_key[threadIdx.x] = EMPTY32; s_cnt[threadIdx.x] = 0u; }
+    if (threadIdx.x < 3) { s_mn[threadIdx.x] = EMPTY32; s_mx[threadIdx.x] = 0u; }
+    if (threadIdx.x == 0) { s_over = 0u; s_foreign = 0u; }
+    __syncthreads();
+    u32 mn[3] = {EMPTY32, EMPTY32, EMPTY32}, mx[3] = {0u, 0u, 0u}, foreign = 0u;
+    constexpr u32 U = 4;  // independent loads in flight per thread
+    const u32 stride = gridDim.x * blockDim.x;
+    const u32 n_round = (n + 31u) & ~31u;
+    for (u32 i0 = blockIdx.x * blockDim.x + threadIdx.x; i0 < n_round; i0 += stride * U) {
+        u32 vs[U], vp[U], vo[U];
+        bool valid[U];
+#pragma unroll
+        for (u32 u = 0; u < U; u++) {
+            const u32 i = i0 + u * stride;
+            valid[u] = i < n;
+            vs[u] = valid[u] ? s[i] : 0u; vp[u] = valid[u] ? p[i] : 0u; vo[u] = valid[u] ? o[i] : 0u;
+        }
+#pragma unroll
+        for (u32 u = 0; u < U; u++) {
+            const unsigned act = __ballot_sync(0xffffffffu, valid[u]);  // (i0 + u * stride is warp-uniform in being below n_round or not)
+            if (!valid[u]) continue;
+            mn[0] = min(mn[0], vs[u]); mx[0] = max(mx[0], vs[u]);
+            mn[1] = min(mn[1], vp[u]); mx[1] = max(mx[1], vp[u]);
+            mn[2] = min(mn[2], vo[u]); mx[2] = max(mx[2], vo[u]);
+            if (world > 1u) foreign += shard_of(vs[u], world) != rank;
+            const unsigned peers = __match_any_sync(act, vp[u]);
+            if (lane != __ffs(peers) - 1) continue;
+            u32 slot = mix32(vp[u]) & (SEGP_SLOTS - 1u);
+            for (u32 probes = 0;; probes++) {
+                if (probes >= SEGP_SLOTS) { s_over = 1u; break; }
+                u32 cur = *reinterpret_cast<volatile u32*>(&s_key[slot]);
+                if (cur == EMPTY32) cur = atomicCAS(&s_key[slot], EMPTY32, vp[u]);
+                if (cur == EMPTY32 || cur == vp[u]) { atomicAdd(&s_cnt[slot], (u32)__popc(peers)); break; }
+                slot = (slot + 1u) & (SEGP_SLOTS - 1u);
+            }
+        }
+    }
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        mn[c] = __reduce_min_sync(0xffffffffu, mn[c]);
+        mx[c] = __reduce_max_sync(0xffffffffu, mx[c]);
+    }
+    foreign = warp_sum(foreign);
+    if (lane == 0) {  // CTA-level reduction in shared memory first: 6 global atomics per CTA, not per warp
+#pragma unroll
+        for (int c = 0; c < 3; c++) { atomicMin(&s_mn[c], mn[c]); atomicMax(&s_mx[c], mx[c]); }
+        if (foreign) atomicAdd(&s_foreign, foreign);
+    }
+    __syncthreads();
+    if (threadIdx.x < SEGP_SLOTS && s_key[threadIdx.x] != EMPTY32) {
+        const u32 vp = s_key[threadIdx.x];
+        u32 slot = mix32(vp) & (SEGP_SLOTS - 1u);
+        for (u32 probes = 0;; probes++) {
+            if (probes >= SEGP_SLOTS) { ctrl[SEGP_OVERFLOW] = 1u; break; }
+            u32 cur = *reinterpret_cast<volatile u32*>(&ctrl[SEGP_SLOT + slot]);
+            if (cur == EMPTY32) cur = atomicCAS(&ctrl[SEGP_SLOT + slot], EMPTY32, vp);
+            if (cur == EMPTY32 || cur == vp) { atomicAdd(&ctrl[SEGP_COUNT + slot], s_cnt[threadIdx.x]); break; }
+            slot = (slot + 1u) & (SEGP_SLOTS - 1u);
+        }
+    }
+    if (threadIdx.x == 0 && s_over) ctrl[SEGP_OVERFLOW] = 1u;
+    if (threadIdx.x < 3) { atomicMin(&ctrl[SEGP_MIN + threadIdx.x], s_mn[threadIdx.x]); atomicMax(&ctrl[SEGP_MAX + threadIdx.x], s_mx[threadIdx.x]); }
+    if (threadIdx.x == 0 && s_foreign) atomicAdd(&ctrl[SEGP_FOREIGN], s_foreign);
+}
+static void launch_segment_profile(const u32* s, const u32* p, const u32* o, u32 n, u32 rank, u32 world, u32* ctrl, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    const int grid = grid_1d(n, n_sms, 256, 4);
+    segment_profile_kernel<<<grid, 256, 0, st>>>(s, p, o, n, rank, world, ctrl);
+}
+
+struct SplitEntry {
+    u32 pred;
+    u32 n;              // rows of the predicate in the segment (capacity of pairs / ynum)
+    uint2* pairs;       // the new chunk
+    double* ynum;       // its typed literal column (null: no numeric side table loaded)
+    u32* xtab; u32 xtab_min, xtab_range, cshift;   // subject table to insert into (null: none)
+    u16* xkey;          // value ranks in table order (kb_numrank.cuh: rank16), maintained with xtab (null: none)
+    u32* ytab; u32 ytab_min, ytab_range;           // object table (null: none)
+};
+// control words per entry (all 0 at launch): cursor, n_numeric, xdup, ydup, xout, yout, pad, pad, ~xmin, ~ymin, xmax, ymax
+constexpr u32 SPLIT_CURSOR = 0, SPLIT_NNUM = 1, SPLIT_XDUP = 2, SPLIT_YDUP = 3, SPLIT_XOUT = 4, SPLIT_YOUT = 5, SPLIT_XMIN = 8, SPLIT_YMIN = 9, SPLIT_XMAX = 10,
+              SPLIT_YMAX = 11, SPLIT_WORDS = 12;
+struct SplitParams {
+    const u32 *s, *p, *o;
+    u32 n, k;
+    SplitEntry e[MAXP];
+    u32* ctrl;  // k * SPLIT_WORDS words
+    NumTab nt;
+    const double* numv;  // value order of the numeric side table (kb_numrank.cuh), for the entries' xkey (n_numv = 0: no entry has one)
+    u32 n_numv;
+};
+
+// One pass over a new segment that files every triple under its predicate's slice: the (subject, object) pair goes to the slice's new
+// chunk (one cursor reservation per warp and predicate), the object's f64 value to the chunk's typed column, both ids into the slice's
+// persistent tables (atomicExch: a previous occupant = the column is not unique; a key outside the table = the table has to be
+// rebuilt; both reported through control words), id ranges reduced per CTA in shared memory. Replaces, per slide, a scan + copy + range
+// pass + two table builds + a typed column pass PER PREDICATE (~30 launches and 4 host round trips for six predicates).
+constexpr u32 SPLIT_ITEMS = 4, SPLIT_TILE = 256 * SPLIT_ITEMS;
+__global__ void __launch_bounds__(256) segment_split_kernel(const __grid_constant__ SplitParams P) {
+    // Tile of 1024 triples per CTA and iteration. Positions: rank inside the tile from warp-aggregated SHARED atomics, then ONE global
+    // cursor reservation per (tile, predicate) — with one global atomic per (warp, predicate) the six cursors of the employee shape
+    // took 31 K same-address atomics each for 1 M triples.
+    __shared__ u32 s_mm[MAXP][4];
+    __shared__ u32 s_flag[MAXP][4];
+    __shared__ u32 s_nnum[MAXP];
+    __shared__ u32 s_cnt[MAXP], s_base[MAXP];
+    const int lane = threadIdx.x & 31;
+    if (threadIdx.x < MAXP) {
+        s_mm[threadIdx.x][0] = EMPTY32; s_mm[threadIdx.x][1] = EMPTY32; s_mm[threadIdx.x][2] = 0u; s_mm[threadIdx.x][3] = 0u;
+        s_flag[threadIdx.x][0] = 0u; s_flag[threadIdx.x][1] = 0u; s_flag[threadIdx.x][2] = 0u; s_flag[threadIdx.x][3] = 0u;
+        s_nnum[threadIdx.x] = 0u;
+        s_cnt[threadIdx.x] = 0u;
+    }
+    __syncthreads();
+    const u32 n_tiles = (P.n + SPLIT_TILE - 1u) / SPLIT_TILE;
+    for (u32 tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const u32 row0 = tile * SPLIT_TILE;
+        u32 vs[SPLIT_ITEMS], vo[SPLIT_ITEMS], which[SPLIT_ITEMS], rank[SPLIT_ITEMS];
+#pragma unroll
+        for (u32 j = 0; j < SPLIT_ITEMS; j++) {  // independent loads first
+            const u32 i = row0 + j * 256u + threadIdx.x;
+            u32 vp = EMPTY32;
+            vs[j] = 0u; vo[j] = 0u;
+            if (i < P.n) { vp = P.p[i]; vs[j] = P.s[i]; vo[j] = P.o[i]; }
+            which[j] = EMPTY32;
+#pragma unroll
+            for (u32 e = 0; e < MAXP; e++) if (e < P.k && P.e[e].pred == vp && i < P.n) which[j] = e;
+        }
+        u32 xk[SPLIT_ITEMS];  // value ranks for the rank columns (xkey): the SPLIT_ITEMS searches in V run side by side
+        if (P.n_numv) {
+            double xv[SPLIT_ITEMS];
+#pragma unroll
+            for (u32 j = 0; j < SPLIT_ITEMS; j++) xv[j] = which[j] != EMPTY32 && P.e[which[j]].xkey ? kb_nr::fold(num_of(P.nt, vo[j])) : 0.0;
+            kb_nr::rank_of_n<SPLIT_ITEMS>(P.numv, P.n_numv, xv, xk);
+        }
+#pragma unroll
+        for (u32 j = 0; j < SPLIT_ITEMS; j++) {
+            const unsigned act = __ballot_sync(0xffffffffu, which[j] != EMPTY32);
+            rank[j] = 0u;
+            if (which[j] == EMPTY32) continue;
+            const u32 w = which[j];
+            const unsigned peers = __match_any_sync(act, w);
+            const int leader = __ffs(peers) - 1;
+            u32 b = 0;
+            const u32 xlo = __reduce_min_sync(peers, vs[j]), ylo = __reduce_min_sync(peers, vo[j]);
+            const u32 xhi = __reduce_max_sync(peers, vs[j]), yhi = __reduce_max_sync(peers, vo[j]);
+            const unsigned nm = __ballot_sync(peers, P.e[w].ynum != nullptr && isnum_of(P.nt, vo[j]));
+            if (lane == leader) {
+                b = atomicAdd(&s_cnt[w], (u32)__popc(peers));
+                atomicMin(&s_mm[w][0], xlo); atomicMin(&s_mm[w][1], ylo); atomicMax(&s_mm[w][2], xhi); atomicMax(&s_mm[w][3], yhi);
+                if (nm) atomicAdd(&s_nnum[w], (u32)__popc(nm));
+            }
+            b = __shfl_sync(peers, b, leader);
+            rank[j] = b + (u32)__popc(peers & ((1u << lane) - 1u));
+        }
+        __syncthreads();
+        if (threadIdx.x < P.k) {
+            const u32 c = s_cnt[threadIdx.x];
+            s_base[threadIdx.x] = c ? atomicAdd(&P.ctrl[threadIdx.x * SPLIT_WORDS + SPLIT_CURSOR], c) : 0u;
+            s_cnt[threadIdx.x] = 0u;
+        }
+        __syncthreads();
+#pragma unroll
+        for (u32 j = 0; j < SPLIT_ITEMS; j++) {
+            if (which[j] == EMPTY32) continue;
+            const u32 w = which[j];
+            const SplitEntry& E = P.e[w];
+            const u32 pos = s_base[w] + rank[j];
+            if (pos < E.n) {  // (always: the capacities are the profile pass's exact counts)
+                E.pairs[pos] = make_uint2(vs[j], vo[j]);
+                if (E.ynum) E.ynum[pos] = num_of(P.nt, vo[j]);
+            }
+            if (E.xtab) {
+                const u32 off = compact_key(vs[j], E.cshift) - E.xtab_min;
+                if (off < E.xtab_range) {
+                    if (atomicExch(&E.xtab[off], vo[j]) != EMPTY32) s_flag[w][0] = 1u;
+                    if (E.xkey) E.xkey[off] = kb_nr::rank16(xk[j], kb_nr::rank_shift(P.n_numv));
+                } else s_flag[w][2] = 1u;
+            }
+            if (E.ytab) {
+                const u32 off = vo[j] - E.ytab_min;
+                if (off < E.ytab_range) {
+                    if (atomicExch(&E.ytab[off], vs[j]) != EMPTY32) s_flag[w][1] = 1u;
+                } else s_flag[w][3] = 1u;
+            }
+        }
+        // (s_base is rewritten only after the next tile's first barrier, which every thread reaches after these reads)
+    }
+    __syncthreads();
+    if (threadIdx.x < P.k) {
+        const u32 j = threadIdx.x;
+        u32* c = P.ctrl + j * SPLIT_WORDS;
+        if (s_mm[j][0] != EMPTY32 || s_mm[j][2] != 0u) {  // minima are kept complemented so that every control word starts at 0
+            atomicMax(&c[SPLIT_XMIN], ~s_mm[j][0]); atomicMax(&c[SPLIT_YMIN], ~s_mm[j][1]);
+            atomicMax(&c[SPLIT_XMAX], s_mm[j][2]); atomicMax(&c[SPLIT_YMAX], s_mm[j][3]);
+        }
+        if (s_nnum[j]) atomicAdd(&c[SPLIT_NNUM], s_nnum[j]);
+        if (s_flag[j][0]) c[SPLIT_XDUP] = 1u;
+        if (s_flag[j][1]) c[SPLIT_YDUP] = 1u;
+        if (s_flag[j][2]) c[SPLIT_XOUT] = 1u;
+        if (s_flag[j][3]) c[SPLIT_YOUT] = 1u;
+    }
+}
+static void launch_segment_split(const SplitParams& p, int n_sms, cudaStream_t st) {
+    if (p.n == 0 || p.k == 0) return;
+    const int grid = grid_1d(p.n, n_sms, SPLIT_TILE, 6);
+    segment_split_kernel<<<grid, 256, 0, st>>>(p);
+}
+
+constexpr u32 CLEAR_MAX = 16;
+struct ClearEntry {
+    const uint2* pairs; u32 n;
+    u32* xtab; u32 xtab_min, xtab_range, cshift;
+    u32* ytab; u32 ytab_min, ytab_range;
+};
+struct ClearParams { ClearEntry e[CLEAR_MAX]; u32 k; };
+// the keys of up to CLEAR_MAX evicted chunks leave their slices' persistent tables in one launch (blockIdx.y = chunk)
+__global__ void __launch_bounds__(256) clear_chunks_kernel(const __grid_constant__ ClearParams P) {
+    const ClearEntry& E = P.e[blockIdx.y];
+    const u32 stride = gridDim.x * blockDim.x;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < E.n; i += stride) {
+        const uint2 v = E.pairs[i];
+        if (E.xtab) {
+            const u32 off = compact_key(v.x, E.cshift) - E.xtab_min;
+            if (off < E.xtab_range) E.xtab[off] = EMPTY32;
+        }
+        if (E.ytab) {
+            const u32 off = v.y - E.ytab_min;
+            if (off < E.ytab_range) E.ytab[off] = EMPTY32;
+        }
+    }
+}
+static void launch_clear_chunks(const ClearParams& p, int n_sms, cudaStream_t st) {
+    if (p.k == 0) return;
+    u32 n_max = 0;
+    for (u32 j = 0; j < p.k; j++) n_max = p.e[j].n > n_max ? p.e[j].n : n_max;
+    if (n_max == 0) return;
+    const u32 gx = (u32)umin64((u64)n_sms * 8ull / p.k + 1ull, ((u64)n_max + 255ull) / 256ull);
+    clear_chunks_kernel<<<dim3(gx, p.k), 256, 0, st>>>(p);
+}
+
+__global__ void __launch_bounds__(256) pair_minmax_kernel(const uint2* __restrict__ kv, u32 n, u32* out4) {
+    u32 mnx = EMPTY32, mny = EMPTY32, mxx = 0u, mxy = 0u;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const uint2 e = kv[i];
+        mnx = min(mnx, e.x); mxx = max(mxx, e.x);
+        mny = min(mny, e.y); mxy = max(mxy, e.y);
+    }
+    mnx = __reduce_min_sync(0xffffffffu, mnx); mny = __reduce_min_sync(0xffffffffu, mny);
+    mxx = __reduce_max_sync(0xffffffffu, mxx); mxy = __reduce_max_sync(0xffffffffu, mxy);
+    if ((threadIdx.x & 31) == 0) { atomicMin(&out4[0], mnx); atomicMin(&out4[1], mny); atomicMax(&out4[2], mxx); atomicMax(&out4[3], mxy); }
+}
+__global__ void __launch_bounds__(256) pair_numcol_kernel(const uint2* __restrict__ kv, u32 n, NumTab nt, double* __restrict__ out, u32* n_numeric) {
+    u32 c = 0;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const u32 id = kv[i].y;
+        out[i] = num_of(nt, id);
+        c += isnum_of(nt, id) ? 1u : 0u;
+    }
+    c = warp_sum(c);
+    if ((threadIdx.x & 31) == 0 && c) atomicAdd(n_numeric, c);
+}
+// RANKTAB_ITEMS rows per thread (striped over the CTA's chunk): their searches in V run side by side
+constexpr u32 RANKTAB_ITEMS = 4;
+__global__ void __launch_bounds__(256) pair_ranktab_kernel(const uint2* __restrict__ kv, u32 n, NumTab nt, const double* __restrict__ numv, u32 n_numv,
+                                                          u16* __restrict__ out, u32 kmin, u32 range, u32 cshift) {
+    for (u32 row0 = blockIdx.x * 256u * RANKTAB_ITEMS; row0 < n; row0 += gridDim.x * 256u * RANKTAB_ITEMS) {
+        double x[RANKTAB_ITEMS];
+        u32 off[RANKTAB_ITEMS], r[RANKTAB_ITEMS];
+#pragma unroll
+        for (u32 j = 0; j < RANKTAB_ITEMS; j++) {
+            const u32 i = row0 + j * 256u + threadIdx.x;
+            off[j] = EMPTY32;
+            x[j] = 0.0;
+            if (i < n) {
+                const uint2 v = kv[i];
+                off[j] = compact_key(v.x, cshift) - kmin;
+                x[j] = kb_nr::fold(num_of(nt, v.y));
+            }
+        }
+        kb_nr::rank_of_n<RANKTAB_ITEMS>(numv, n_numv, x, r);
+        const u32 shift = kb_nr::rank_shift(n_numv);
+#pragma unroll
+        for (u32 j = 0; j < RANKTAB_ITEMS; j++) if (off[j] < range) out[off[j]] = kb_nr::rank16(r[j], shift);
+    }
+}
+// the ranks of those values in the value order numv[0 .. n_numv) (kb_numrank.cuh), laid out like the subject-keyed direct table:
+// out[compact(subject) - kmin] = rank_of(num_of(object))
+static void launch_pair_ranktab(const uint2* kv, u32 n, NumTab nt, const double* numv, u32 n_numv, u16* out, u32 kmin, u32 range, u32 cshift, int n_sms,
+                                cudaStream_t st) {
+    if (n == 0) return;
+    const int grid = grid_1d(n, n_sms, 256 * RANKTAB_ITEMS);
+    pair_ranktab_kernel<<<grid, 256, 0, st>>>(kv, n, nt, numv, n_numv, out, kmin, range, cshift);
+}
+// typed literal column of a predicate slice: out[i] = num_or0[kv[i].y]; *n_numeric += rows whose object is numeric
+static void launch_pair_numcol(const uint2* kv, u32 n, NumTab nt, double* out, u32* n_numeric, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    int grid = grid_1d(n, n_sms);
+    pair_numcol_kernel<<<grid, 256, 0, st>>>(kv, n, nt, out, n_numeric);
+}
+// min/max of both halves of a pair relation: out[0..3] = min x, min y, max x, max y
+static void launch_pair_minmax(const uint2* kv, u32 n, u32* out4, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    int grid = grid_1d(n, n_sms, 256, 4);
+    pair_minmax_kernel<<<grid, 256, 0, st>>>(kv, n, out4);
+}
+
+// the CSR directory of a grouped join (CsrTab, kb_join.cu) built from an interleaved (subject, object) slice of the store index: key = one
+// half, payload = the other half.
+// Directory builds over a predicate slice. The key column may hold a handful of distinct values repeated millions of times (the objects
+// of foaf:title, of ds:full_or_part_time ...): one global atomic per row serialises on three addresses. The lanes of a
+// warp that carry the same key are therefore aggregated (__match_any_sync): one atomic per (warp, distinct key), ranks inside the group
+// from the lane mask.
+__global__ void __launch_bounds__(256) csr_count_pairs_kernel(const uint2* __restrict__ kv, u32 key_is_y, u32 n, u32 kmin, u32* __restrict__ counts) {
+    const u32 stride = gridDim.x * blockDim.x;
+    const int lane = threadIdx.x & 31;
+    const u32 n_round = (n + 31u) & ~31u;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += stride) {
+        const bool valid = i < n;
+        const unsigned act = __ballot_sync(0xffffffffu, valid);
+        if (!valid) continue;
+        const uint2 v = kv[i];
+        const u32 key = (key_is_y ? v.y : v.x) - kmin;
+        const unsigned peers = __match_any_sync(act, key);
+        if (lane == __ffs(peers) - 1) atomicAdd(&counts[key], (u32)__popc(peers));
+    }
+}
+static void launch_csr_count_pairs(const uint2* kv, u32 key_is_y, u32 n, u32 kmin, u32* counts, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    const int grid = grid_1d(n, n_sms);
+    csr_count_pairs_kernel<<<grid, 256, 0, st>>>(kv, key_is_y, n, kmin, counts);
+}
+__global__ void __launch_bounds__(256) csr_fill_pairs_kernel(const uint2* __restrict__ kv, u32 key_is_y, u32 n, u32 kmin, u32* __restrict__ cursor,
+                                                             u32* __restrict__ val_out) {
+    const u32 stride = gridDim.x * blockDim.x;
+    const int lane = threadIdx.x & 31;
+    const u32 n_round = (n + 31u) & ~31u;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += stride) {
+        const bool valid = i < n;
+        const unsigned act = __ballot_sync(0xffffffffu, valid);
+        if (!valid) continue;
+        const uint2 v = kv[i];
+        const u32 key = (key_is_y ? v.y : v.x) - kmin;
+        const unsigned peers = __match_any_sync(act, key);
+        const int leader = __ffs(peers) - 1;
+        u32 base = 0;
+        if (lane == leader) base = atomicAdd(&cursor[key], (u32)__popc(peers));
+        base = __shfl_sync(peers, base, leader);
+        val_out[base + (u32)__popc(peers & ((1u << lane) - 1u))] = key_is_y ? v.x : v.y;
+    }
+}
+static void launch_csr_fill_pairs(const uint2* kv, u32 key_is_y, u32 n, u32 kmin, u32* cursor, u32* val_out, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    const int grid = grid_1d(n, n_sms);
+    csr_fill_pairs_kernel<<<grid, 256, 0, st>>>(kv, key_is_y, n, kmin, cursor, val_out);
+}
+
+// the store's 96-bit (s,p,o) key set
+__global__ void __launch_bounds__(256) set_insert_kernel(uint4* set, u32 set_slots, const u32* s, const u32* p, const u32* o, u32 n,
+                                                         u32* overflow) {
+    const u32 stride = gridDim.x * blockDim.x;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+        if (set_insert(set, set_slots, s[i], p[i], o[i]) == 2u) *overflow = 1u;
+}
+static void launch_set_insert(uint4* set, u32 set_slots, const u32* s, const u32* p, const u32* o, u32 n, u32* overflow, int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    set_insert_kernel<<<grid_1d(n, n_sms), 256, 0, st>>>(set, set_slots, s, p, o, n, overflow);
+}
+
+// kb_store_delete: p_out[i] = p[i], or EMPTY32 when (s,p,o)[i] is in the delete set; a scan with a variable predicate and
+// NE_ID(EMPTY32)... is not needed: the store compaction simply rescans with pattern (?s ?p ?o) over (s, p_out, o) and drops
+// rows whose predicate became EMPTY32 (KB_ID_NONE is never a real predicate).
+__global__ void __launch_bounds__(256) delete_mark_kernel(const u32* s, const u32* p, const u32* o, u32 n, const uint4* set, u32 set_slots,
+                                                          u32* p_out) {
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const u32 vp = p[i];
+        p_out[i] = set_find(set, set_slots, s[i], vp, o[i]) != EMPTY32 ? EMPTY32 : vp;
+    }
+}
+// mark rows of a segment that equal any triple of a (small) delete set held in a 96-bit set; then compaction is a scan with flags
+static void launch_delete_mark(const u32* s, const u32* p, const u32* o, u32 n, const uint4* set, u32 set_slots, u32* p_out, int n_sms,
+                               cudaStream_t st) {
+    if (n == 0) return;
+    int grid = grid_1d(n, n_sms);
+    delete_mark_kernel<<<grid, 256, 0, st>>>(s, p, o, n, set, set_slots, p_out);
+}
+
+// ---- kb_store_insert / kb_store_remove: the batch as a key set (the layout of set_insert, so that delete_mark reads it too), the
+// batch index of each key's first occurrence, and a found bit per key set by one pass over the store
+__global__ void __launch_bounds__(256) batch_set_kernel(uint4* set, u32 set_slots, const u32* s, const u32* p, const u32* o, u32 n, u32* first,
+                                                        u32* slot_of, u32* overflow) {
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        u32 slot = EMPTY32;  // stays EMPTY32 when the set is full
+        set_insert_at(set, set_slots, s[i], p[i], o[i], &slot);
+        slot_of[i] = slot;
+        if (slot == EMPTY32) *overflow = 1u;
+        else atomicMin(&first[slot], i);
+    }
+}
+// kb_store_insert / kb_store_remove (kb_store.cu). The batch's keys go into a set laid out as launch_set_insert's (set_slots a power of
+// two, zeroed); slot_of[i] = the slot of triple i, first[slot] (set to EMPTY32 before) = the smallest batch index holding that key;
+// *overflow = 1 when the set is full
+static void launch_batch_set(uint4* set, u32 set_slots, const u32* s, const u32* p, const u32* o, u32 n, u32* first, u32* slot_of, u32* overflow,
+                             int n_sms, cudaStream_t st) {
+    if (n == 0) return;
+    const int grid = grid_1d(n, n_sms);
+    batch_set_kernel<<<grid, 256, 0, st>>>(set, set_slots, s, p, o, n, first, slot_of, overflow);
+}
+
+__global__ void __launch_bounds__(256) batch_mark_kernel(const u32* __restrict__ s, const u32* __restrict__ p, const u32* __restrict__ o, u32 n,
+                                                         const uint4* __restrict__ set, u32 set_slots, u32* found, u32* hits) {
+    u32 mine = 0;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const u32 slot = set_find(set, set_slots, s[i], p[i], o[i]);
+        if (slot != EMPTY32) { found[slot] = 1u; mine++; }
+    }
+    if (mine) atomicAdd(hits, mine);
+}
+// one stored segment against the batch set: found[slot] = 1 for every key the segment holds, *hits += its triples that match a key
+static void launch_batch_mark(const u32* s, const u32* p, const u32* o, u32 n, const uint4* set, u32 set_slots, u32* found, u32* hits, int n_sms,
+                              cudaStream_t st) {
+    if (n == 0) return;
+    const int grid = grid_1d(n, n_sms);
+    batch_mark_kernel<<<grid, 256, 0, st>>>(s, p, o, n, set, set_slots, found, hits);
+}
+
+__global__ void __launch_bounds__(256) batch_flags_kernel(u32 n, const u32* slot_of, const u32* first, const u32* found, u32 want_found, u8* flag8,
+                                                          u32* flag32, u32* count) {
+    u32 mine = 0;
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const u32 slot = slot_of[i];
+        const bool f = slot != EMPTY32 && first[slot] == i && (found[slot] != 0u) == (want_found != 0u);
+        flag8[i] = f ? 1 : 0;
+        flag32[i] = f ? 1u : 0u;
+        mine += f ? 1u : 0u;
+    }
+    if (mine) atomicAdd(count, mine);
+}
+// flag[i] = 1 iff triple i is the first of its key in the batch and found[its slot] equals want_found; *count += the flags set.
+// flag8 is what the caller reads back, flag32 what an exclusive scan turns into output positions
+static void launch_batch_flags(u32 n, const u32* slot_of, const u32* first, const u32* found, bool want_found, u8* flag8, u32* flag32, u32* count, int n_sms,
+                               cudaStream_t st) {
+    if (n == 0) return;
+    const int grid = grid_1d(n, n_sms);
+    batch_flags_kernel<<<grid, 256, 0, st>>>(n, slot_of, first, found, want_found ? 1u : 0u, flag8, flag32, count);
+}
+
+__global__ void __launch_bounds__(256) batch_gather_kernel(const u32* s, const u32* p, const u32* o, u32 n, const u8* flag8, const u32* pos, u32* out_s,
+                                                           u32* out_p, u32* out_o) {
+    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        if (!flag8[i]) continue;
+        const u32 k = pos[i];
+        out_s[k] = s[i]; out_p[k] = p[i]; out_o[k] = o[i];
+    }
+}
+// out[pos[i]] = triple i for every flagged i (batch order is kept: pos is the exclusive scan of the flags)
+static void launch_batch_gather(const u32* s, const u32* p, const u32* o, u32 n, const u8* flag8, const u32* pos, u32* out_s, u32* out_p, u32* out_o, int n_sms,
+                                cudaStream_t st) {
+    if (n == 0) return;
+    const int grid = grid_1d(n, n_sms);
+    batch_gather_kernel<<<grid, 256, 0, st>>>(s, p, o, n, flag8, pos, out_s, out_p, out_o);
+}
+
+// kb_store_remove_template: one triple per (relation row, template pattern); col[t][c] null: position c of pattern t is the constant
+// cval[t][c]. bad[0] += the variable cells that are unbound, bad[1] += those whose term would not re-encode to the same id
+constexpr u32 TEMPLATE_MAX = 16;
+struct TemplateFillParams {
+    const u32* col[TEMPLATE_MAX][3];
+    u32 cval[TEMPLATE_MAX][3];
+    u32 n_tmpl, rows;
+    u32 *s, *p, *o;
+    DictTab dict;
+    u32* bad;
+};
+// kb_store_remove_template: triple (row r, template pattern t) at r * n_tmpl + t. bad[0] counts unbound cells; bad[1] the cells whose
+// term the reference would not re-encode to the same id (execute_query.rs:398-403 decodes every binding and encodes it again with
+// encode_term_star): a quoted id (its rendering is re-parsed), an id the device dictionary does not hold, or a string that
+// encode_term_star changes: surrounding whitespace, '<' ... '>' (and so "<< ... >>"), a leading '"'
+__device__ __forceinline__ bool reencodes_to_itself(u32 id, const DictTab& d) {
+    if ((id & 0x80000000u) || id >= d.ids) return false;
+    const unsigned long long a = d.off[id], b = d.off[id + 1];
+    if (a == b) return true;
+    const unsigned char c0 = d.bytes[a], c1 = d.bytes[b - 1];
+    // Rust's str::trim: char::is_whitespace (U+0009..U+000D, U+0020, U+0085, U+00A0, U+1680, U+2000..U+200A, U+2028, U+2029, U+202F,
+    // U+205F, U+3000) at either end
+    const auto ws_cp = [](u32 cp) {
+        return (cp >= 0x09 && cp <= 0x0D) || cp == 0x20 || cp == 0x85 || cp == 0xA0 || cp == 0x1680 || (cp >= 0x2000 && cp <= 0x200A) ||
+               cp == 0x2028 || cp == 0x2029 || cp == 0x202F || cp == 0x205F || cp == 0x3000;
+    };
+    const auto cp_at = [&](unsigned long long i, u32 len) {  // the code point of the len-byte UTF-8 sequence at i (EMPTY32: not one)
+        if (i + len > b) return EMPTY32;
+        const unsigned char x = d.bytes[i];
+        u32 cp = len == 1 ? x : len == 2 ? (x & 0x1Fu) : (x & 0x0Fu);
+        for (u32 k = 1; k < len; k++) cp = (cp << 6) | (d.bytes[i + k] & 0x3Fu);
+        return cp;
+    };
+    const u32 lead = c0 < 0x80 ? 1u : (c0 & 0xE0) == 0xC0 ? 2u : (c0 & 0xF0) == 0xE0 ? 3u : 4u;
+    if (lead <= 3 && ws_cp(cp_at(a, lead))) return false;
+    u32 tail = 1;  // the last character starts at the last byte that is not a continuation byte
+    while (tail < 4 && tail < b - a && (d.bytes[b - tail] & 0xC0) == 0x80) tail++;
+    if (tail <= 3 && ws_cp(cp_at(b - tail, tail))) return false;
+    if (c0 == '<' && c1 == '>') return false;
+    return c0 != '"';
+}
+__global__ void __launch_bounds__(256) template_fill_kernel(const __grid_constant__ TemplateFillParams P) {
+    const u64 total = (u64)P.rows * P.n_tmpl;
+    u32 unbound = 0, changes = 0;
+    for (u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x; k < total; k += (u64)gridDim.x * blockDim.x) {
+        const u32 r = (u32)(k / P.n_tmpl), t = (u32)(k % P.n_tmpl);
+        u32 v[3];
+        for (int c = 0; c < 3; c++) {
+            const u32* col = P.col[t][c];
+            v[c] = col ? col[r] : P.cval[t][c];
+            if (!col) continue;
+            if (v[c] == EMPTY32) unbound++;
+            else if (!reencodes_to_itself(v[c], P.dict)) changes++;
+        }
+        P.s[k] = v[0]; P.p[k] = v[1]; P.o[k] = v[2];
+    }
+    if (unbound) atomicAdd(&P.bad[0], unbound);
+    if (changes) atomicAdd(&P.bad[1], changes);
+}
+static void launch_template_fill(const TemplateFillParams& P, int n_sms, cudaStream_t st) {
+    const u64 total = (u64)P.rows * P.n_tmpl;
+    if (total == 0) return;
+    const int grid = grid_1d(total, n_sms);
+    template_fill_kernel<<<grid, 256, 0, st>>>(P);
+}
 
 kb_status segment_stats(kb_ctx* ctx, Segment* sg) {
     if ((sg->has_stats && sg->stats_world == ctx->shard_world) || sg->n == 0) { sg->has_stats = true; sg->stats_world = ctx->shard_world; return KB_OK; }
@@ -839,7 +1470,7 @@ kb_status kb_store_delete(kb_ctx* ctx, const uint32_t* s, const uint32_t* p, con
     KB_CUDA(ctx, cudaMemcpyAsync(dp->p, p, n * sizeof(u32), cudaMemcpyHostToDevice, ctx->st));
     KB_CUDA(ctx, cudaMemcpyAsync(dob->p, o, n * sizeof(u32), cudaMemcpyHostToDevice, ctx->st));
     const u32 off = kb::ctrl_alloc(ctx, 4);
-    kb::launch_set_insert(static_cast<uint4*>(set->p), set_slots, (const u32*)ds->p, (const u32*)dp->p, 0u, (const u32*)dob->p, (u32)n,
+    kb::launch_set_insert(static_cast<uint4*>(set->p), set_slots, (const u32*)ds->p, (const u32*)dp->p, (const u32*)dob->p, (u32)n,
                           ctx->ctrl + off, ctx->n_sms, ctx->st);
     KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));
     // the new segments are built aside: the store changes only when all of them are (a failure leaves it as it was)

@@ -127,11 +127,11 @@ def tag_home(h, slots: int):
     return _u64(h) & U64(slots - 1)
 
 
-GROUP_SMEM = 64  # kb_group.cu:28, and PI_GROUP_SMEM (kb_kernels.cu:798)
+GROUP_SMEM = 64  # kb_group.cu:28, and PI_GROUP_SMEM (kb_join.cu:455)
 
 
 def group1_cta_home(key):
-    """group1_kernel's CTA-table home (kb_group.cu:268); the index probe's fused GROUP BY uses the same (kb_kernels.cu:1025)"""
+    """group1_kernel's CTA-table home (kb_group.cu:268); the index probe's fused GROUP BY uses the same (kb_join.cu:682)"""
     return mix32(key) & U32(GROUP_SMEM - 1)
 
 
@@ -167,7 +167,7 @@ def group_slot_home(cols, n_slots: int):
 
 
 def distinct_home(v, n_slots: int):
-    """distinct_kernel's home slot (kb_kernels.cu:185)"""
+    """distinct_kernel's home slot (kb_store.cu:36)"""
     return mix32(v) & U32(n_slots - 1)
 
 
@@ -176,13 +176,13 @@ SET_S, SET_O, SET_P = 0x9E3779B1, 0x632BE5AB, 0x85EBCA77
 
 @_wraps
 def set_hash(s, p, o):
-    """the 96-bit key set's hash (kb_kernels.cuh:358): the store's INSERT / DELETE batch sets"""
+    """the 96-bit key set's hash (kb_kernels.cuh:149): the store's INSERT / DELETE batch sets"""
     return mix32(mix32(s) * U32(SET_S) ^ mix32(_u32(o) + U32(SET_O)) ^ (_u32(p) * U32(SET_P)))
 
 
 @_wraps
 def set64_hash(s, o):
-    """the 64-bit (s, o) set's hash before the mask (kb_kernels.cuh:404, 422)"""
+    """the 64-bit (s, o) set's hash before the mask (kb_kernels.cuh:195, 213)"""
     return mix32(mix32(s) * U32(SET_S) ^ mix32(_u32(o) + U32(SET_O)))
 
 

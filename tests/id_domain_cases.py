@@ -201,7 +201,7 @@ def grouped_pair(hi, past, n_build=1000, n_probe=5000, seed=0):
     return left, right, "chained" if past else "grouped"
 
 
-PROBEG_HEAVY = 32768  # kb_kernels.cuh: a grouped join whose output passes it spreads its heavy probe tiles over the grid (a 2nd launch)
+PROBEG_HEAVY = 32768  # kb_join.cu: a grouped join whose output passes it spreads its heavy probe tiles over the grid (a 2nd launch)
 
 
 def heavy_pair(heavy, n_heavy=40, n_probe=3000, n_build=140, seed=3):
