@@ -626,6 +626,10 @@ kb_status kb_ctx_create(int device, kb_ctx** out) {
     if (const char* ds = getenv("KOLIBRIE_DERIVE_SLICE")) ctx->derive_slice_bytes = std::max<u64>(64, strtoull(ds, nullptr, 10));
     if (const char* dk = getenv("KOLIBRIE_DERIVE_SLACK")) ctx->derive_bucket_slack = strtoull(dk, nullptr, 10);
     if (const char* dr = getenv("KOLIBRIE_DERIVE_MIN_ROWS")) ctx->derive_min_part_rows = std::max<u64>(1, strtoull(dr, nullptr, 10));
+    if (const char* sm = getenv("KOLIBRIE_SMS")) {  // grid cap for tests: every persistent CTA then runs many tiles
+        const long n = strtol(sm, nullptr, 10);
+        if (n > 0) ctx->n_sms = (int)std::min<long>(n, prop.multiProcessorCount);
+    }
     if ((e = cudaMalloc(&ctx->ctrl, kb_ctx::CTRL_WORDS * sizeof(u32))) != cudaSuccess) return bail("cudaMalloc(ctrl)", e);
     if ((e = cudaMallocHost(&ctx->h_ctrl, kb_ctx::CTRL_WORDS * sizeof(u32))) != cudaSuccess) return bail("cudaMallocHost(ctrl)", e);
     if ((e = cudaMalloc(&ctx->fast_cb, 64)) != cudaSuccess) return bail("cudaMalloc(fast_cb)", e);

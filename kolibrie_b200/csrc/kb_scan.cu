@@ -529,14 +529,14 @@ static void launch_scan_star_k(const ScanParams& p_in, int n_sms, cudaStream_t s
         p.n_tiles += (p.seg[g].n + (u32)STAR_TILE - 1u) / (u32)STAR_TILE;
     }
     const size_t smem = 2 * 3 * STAR_TILE * sizeof(u32);
-    static int grid_max = 0;
-    if (grid_max == 0) {
+    static int per_sm = 0;  // occupancy is a property of the kernel image; the grid follows each caller's n_sms
+    if (per_sm == 0) {
         cudaFuncSetAttribute(scan_star_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        int per_sm = 1;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, scan_star_kernel<K>, STAR_THREADS, smem);
-        grid_max = (per_sm < 1 ? 1 : per_sm) * n_sms;
+        int occ = 1;
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, scan_star_kernel<K>, STAR_THREADS, smem);
+        per_sm = occ < 1 ? 1 : occ;
     }
-    const int grid = (int)umin64((u64)grid_max, (u64)p.n_tiles);
+    const int grid = (int)umin64((u64)per_sm * (u64)n_sms, (u64)p.n_tiles);
     scan_star_kernel<K><<<grid, STAR_THREADS, smem, st>>>(p);
 }
 
