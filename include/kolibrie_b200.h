@@ -376,6 +376,64 @@ KB_API kb_status kb_store_gather_stats(kb_ctx* ctx, uint64_t max_sample, kb_db_s
 KB_API kb_status kb_db_stats_counts(const kb_db_stats* st, uint32_t position, const uint32_t** ids, const uint64_t** counts, uint64_t* n);
 KB_API void kb_db_stats_free(kb_db_stats* st);
 
+/* ------------------------------------------------------------------ QueryBuilder triple queries: db.query() ... get_triples() / count()
+ * / get_decoded_triples() / get_subjects() / get_predicates() / get_objects() (kolibrie/src/query_builder.rs:355-643) over the device store.
+ * kb_qb_triples: the rows of `spec` as the reference's apply_filters computes them:
+ *   the input is the store as a SET (a triple held by several segments counts once), in ascending (s, p, o) id order;
+ *   pos[0..2] filter the subject / predicate / object (ANDed; KB_QB_ANY: no filter). KB_QB_EXACT: the id equals `id` (the caller resolves
+ *     the string through its dictionary; an id with bit 31, KB_ID_NONE for a string the dictionary lacks, matches nothing).
+ *     KB_QB_CONTAINS / _STARTS / _ENDS: the id's dictionary string contains / starts with / ends with the `len` pattern bytes, compared
+ *     byte by byte (str::contains / starts_with / ends_with). An id the dictionary does not map (a quoted id, an id past the device
+ *     dictionary) fails every text filter; an empty pattern matches every other id. Each text filter is one pass over the device
+ *     dictionary into a bitmap of 1 bit per id, then one pass over the store tests every row;
+ *   join != 0 and right != NULL: the union over the KB_QB_ON_* bits of (l.s, l.p, r.o) for l.s == r.s (ON_SUBJECT), (l.s, l.p, r.o) for
+ *     l.p == r.p (ON_PREDICATE), (l.s, r.p, r.o) for l.o == r.o (ON_OBJECT), l over the filtered set and r over the whole store of `right`
+ *     (unfiltered, a set too), ids compared raw; the filtered set itself is not part of the result. `right` is read, never written, needs
+ *     no dictionary, may be ctx itself and must be on ctx's device (else KB_E_INVALID);
+ *   offset / limit: rows [offset, min(offset + limit, n)) of that order (limit KB_QB_NO_LIMIT: to the end; offset + limit saturates).
+ *   order_by / asc / desc have no effect in the reference (the sorted Vec is collected back into a BTreeSet) and have no field here.
+ * *out (NULL: count only) is a relation of info.n_rows rows with columns slots[0..2] = subject, predicate, object. The store, its version,
+ * its index and the numeric tables are left as they were.
+ * Refused, nothing changed: a NULL spec or slots, an unknown mode or join bit, a NULL pattern with len > 0, offset > n (the reference
+ * panics), right on another device (KB_E_INVALID); a text filter without device dictionary strings, a sharded ctx or right
+ * (KB_E_UNSUPPORTED: the caller runs its host path); a pattern longer than KB_QB_PATTERN_MAX bytes, a store (ctx or right) of 2^32 - 16
+ * rows or more, a join whose result before the union would reach 2^32 - 16 rows (counted exactly before anything is allocated) (KB_E_LIMIT).
+ * kb_qb_terms: the strings of column `col` of `rows` (a kb_qb_triples result, or any relation) as Dictionary::decode(id).unwrap_or("")
+ * renders them (a quoted id is not walked: it does not decode, like an id past the dictionary):
+ *   KB_QB_TERMS_EMPTY     one string per row, "" where the id does not decode (get_decoded_triples);
+ *   KB_QB_TERMS_DROP      the rows whose id decodes, in row order, duplicates kept (get_subjects / get_predicates / get_objects);
+ *   KB_QB_TERMS_DISTINCT  the distinct strings of those rows sorted by their bytes (the same with distinct()).
+ * Refused: a NULL argument, a column out of range, an unknown mode (KB_E_INVALID); a non-empty relation without device dictionary strings
+ * (KB_E_UNSUPPORTED); more than 2^32 - 16 rows or 2^32 - 1 bytes of text (KB_E_LIMIT). Launches of both count in kb_stats' `other` family. */
+enum kb_qb_mode { KB_QB_ANY = 0, KB_QB_EXACT = 1, KB_QB_CONTAINS = 2, KB_QB_STARTS = 3, KB_QB_ENDS = 4 };
+enum kb_qb_join { KB_QB_ON_SUBJECT = 1, KB_QB_ON_PREDICATE = 2, KB_QB_ON_OBJECT = 4 };
+enum kb_qb_terms_mode { KB_QB_TERMS_EMPTY = 0, KB_QB_TERMS_DROP = 1, KB_QB_TERMS_DISTINCT = 2 };
+#define KB_QB_PATTERN_MAX 4096u
+#define KB_QB_NO_LIMIT 0xFFFFFFFFFFFFFFFFull
+typedef struct kb_qb_filter {
+    uint32_t mode;          /* kb_qb_mode */
+    uint32_t id;            /* KB_QB_EXACT */
+    const uint8_t* pattern; /* KB_QB_CONTAINS / _STARTS / _ENDS: UTF-8 bytes */
+    uint64_t len;
+} kb_qb_filter;
+typedef struct kb_qb_spec {
+    kb_qb_filter pos[3];    /* subject, predicate, object */
+    uint32_t join;          /* KB_QB_ON_* bits */
+    uint32_t reserved;      /* 0 */
+    uint64_t offset;
+    uint64_t limit;         /* KB_QB_NO_LIMIT: none */
+} kb_qb_spec;
+typedef struct kb_qb_info {
+    uint64_t n_raw;         /* store rows read */
+    uint64_t n_selected;    /* distinct triples that pass the filters */
+    uint64_t n_joined;      /* distinct triples of the join (n_selected without one) */
+    uint64_t n_rows;        /* rows after OFFSET / LIMIT */
+    double phase_ms[4];     /* device time: match, selection, sort + dedup, join */
+} kb_qb_info;
+KB_API kb_status kb_qb_triples(kb_ctx* ctx, const kb_qb_spec* spec, const kb_ctx* right /* nullable */, const uint32_t* slots,
+                               kb_rel** out /* nullable: count only */, kb_qb_info* info /* nullable */);
+KB_API kb_status kb_qb_terms(kb_ctx* ctx, const kb_rel* rows, uint32_t col, uint32_t mode, kb_strings** out);
+
 /* ------------------------------------------------------------------ BIND: `PhysicalOperator::Bind` with the built-in functions of
  * ExecutionEngine::execute_with_ids (kolibrie/src/streamertail_optimizer/execution/engine.rs:144-277) over the rows of `in`, in the order
  * they lie. *out = `in` with the output column: appended when out_slot is not a column of `in`, else that column replaced (the other

@@ -186,6 +186,31 @@ class KbDbStatsInfo(C.Structure):
 
 GATHER_STATS_FAST = 100000  # gather_stats_fast's sample size (database_stats.rs:50)
 
+QB_ANY, QB_EXACT, QB_CONTAINS, QB_STARTS, QB_ENDS = 0, 1, 2, 3, 4  # kb_qb_mode
+QB_ON_SUBJECT, QB_ON_PREDICATE, QB_ON_OBJECT = 1, 2, 4  # kb_qb_join
+QB_TERMS_EMPTY, QB_TERMS_DROP, QB_TERMS_DISTINCT = 0, 1, 2  # kb_qb_terms_mode
+QB_PATTERN_MAX = 4096
+QB_NO_LIMIT = 0xFFFFFFFFFFFFFFFF
+
+
+class KbQbFilter(C.Structure):
+    """kb_qb_filter: one position's filter (mode, the id of KB_QB_EXACT, the pattern bytes of the text modes)"""
+    _fields_ = [("mode", C.c_uint32), ("id", C.c_uint32), ("pattern", C.c_void_p), ("len", C.c_uint64)]
+
+
+class KbQbSpec(C.Structure):
+    """kb_qb_spec: subject / predicate / object filters, KB_QB_ON_* join bits, offset and limit (QB_NO_LIMIT: none)"""
+    _fields_ = [("pos", KbQbFilter * 3), ("join", C.c_uint32), ("reserved", C.c_uint32), ("offset", C.c_uint64), ("limit", C.c_uint64)]
+
+
+class KbQbInfo(C.Structure):
+    """kb_qb_info: store rows read, distinct filtered triples, distinct joined triples, rows returned, and the device time of the phases
+    (match, selection, sort + dedup, join)"""
+    _fields_ = [("n_raw", C.c_uint64), ("n_selected", C.c_uint64), ("n_joined", C.c_uint64), ("n_rows", C.c_uint64), ("phase_ms", C.c_double * 4)]
+
+    def as_dict(self):
+        return {n: (list(getattr(self, n)) if n == "phase_ms" else int(getattr(self, n))) for n, _ in self._fields_}
+
 
 KB_BGP_MAX_PATTERNS = 16
 BGP_NONE, BGP_STAR, BGP_COMPONENTS = 0, 1, 2  # kb_bgp_route
@@ -328,6 +353,8 @@ def lib() -> C.CDLL:
         "kb_store_gather_stats": (i32, [vp, u64, P(vp), P(KbDbStatsInfo)]),
         "kb_db_stats_counts": (i32, [vp, u32, P(P(u32)), P(P(u64)), P(u64)]),
         "kb_db_stats_free": (None, [vp]),
+        "kb_qb_triples": (i32, [vp, P(KbQbSpec), vp, P(u32), P(vp), P(KbQbInfo)]),
+        "kb_qb_terms": (i32, [vp, vp, u32, u32, P(vp)]),
         "kb_bind": (i32, [vp, vp, P(KbBindSpec), P(vp), P(KbBindInfo)]),
         "kb_rel_info": (i32, [vp, P(u64), P(u32), P(u32)]),
         "kb_rel_download": (i32, [vp, vp, u32, vp]),
@@ -399,7 +426,7 @@ def lib() -> C.CDLL:
 EXPORTED_SYMBOLS = [
     "kb_version", "kb_ctx_create", "kb_ctx_destroy", "kb_last_error", "kb_set_timing", "kb_get_stats", "kb_synchronize",
     "kb_store_load", "kb_store_load_device", "kb_store_append", "kb_store_append_device", "kb_store_evict", "kb_store_delete", "kb_store_insert", "kb_store_remove", "kb_store_remove_template", "kb_store_clear", "kb_store_build_index", "kb_set_use_index", "kb_store_size",
-    "kb_store_download", "kb_dict_numeric_load", "kb_dict_legacy_i32_load", "kb_dict_numeric_derive", "kb_dict_numeric_download", "kb_dict_strings_load", "kb_dict_encode", "kb_dict_strings_info", "kb_rel_decode", "kb_strings_info", "kb_strings_download", "kb_strings_free", "kb_quoted_load", "kb_quoted_download", "kb_dict_strings_download", "kb_serialize_begin", "kb_serialize_next", "kb_serialize_free", "kb_store_gather_stats", "kb_db_stats_counts", "kb_db_stats_free", "kb_bind", "kb_rel_info", "kb_rel_download", "kb_rel_device_col", "kb_rel_from_host",
+    "kb_store_download", "kb_dict_numeric_load", "kb_dict_legacy_i32_load", "kb_dict_numeric_derive", "kb_dict_numeric_download", "kb_dict_strings_load", "kb_dict_encode", "kb_dict_strings_info", "kb_rel_decode", "kb_strings_info", "kb_strings_download", "kb_strings_free", "kb_quoted_load", "kb_quoted_download", "kb_dict_strings_download", "kb_serialize_begin", "kb_serialize_next", "kb_serialize_free", "kb_store_gather_stats", "kb_db_stats_counts", "kb_db_stats_free", "kb_qb_triples", "kb_qb_terms", "kb_bind", "kb_rel_info", "kb_rel_download", "kb_rel_device_col", "kb_rel_from_host",
     "kb_rel_from_device", "kb_rel_free", "kb_scan", "kb_filter", "kb_project", "kb_hash_join", "kb_natural_join", "kb_hash_join_keyed", "kb_values", "kb_bind_join", "kb_scan_quoted", "kb_star_join", "kb_bgp_execute", "kb_bgp_last_plan",
     "kb_order_by", "kb_group_aggregate", "kb_groups_info", "kb_groups_keys", "kb_groups_values", "kb_groups_counts", "kb_groups_free", "kb_groups_pack", "kb_groups_merge", "kb_star_join_aggregate",
     "kb_star_join_prepare", "kb_plan_submit", "kb_plan_collect", "kb_plan_info", "kb_plan_free", "kb_plan_peer_scratch_bytes", "kb_plan_attach_peers",
@@ -725,6 +752,52 @@ class Context:
             return out
         finally:
             lib().kb_db_stats_free(h)
+
+    def qb_triples(self, filters: Sequence[Optional[Tuple[int, Union[int, bytes, str]]]] = (None, None, None), join: int = 0,
+                   right: Optional["Context"] = None, offset: int = 0, limit: Optional[int] = None, slots: Sequence[int] = (0, 1, 2),
+                   count_only: bool = False) -> Tuple[Optional[Relation], dict]:
+        """kb_qb_triples: QueryBuilder's get_triples over the store. filters: per position None, (QB_EXACT, id) or (QB_CONTAINS /
+        QB_STARTS / QB_ENDS, pattern as str or bytes); join: QB_ON_* bits against `right`'s whole store; rows [offset, offset + limit)
+        of the (s, p, o) set order. Returns (relation with columns `slots` = s, p, o, or None when count_only; kb_qb_info as a dict)."""
+        spec = KbQbSpec()
+        keep = []
+        for k, f in enumerate(filters):
+            if f is None:
+                continue
+            mode, arg = f
+            spec.pos[k].mode = mode
+            if mode == QB_EXACT:
+                spec.pos[k].id = int(arg)
+            else:
+                b = arg.encode("utf-8") if isinstance(arg, str) else bytes(arg)
+                buf = C.create_string_buffer(b, max(len(b), 1))
+                keep.append(buf)
+                spec.pos[k].pattern = C.cast(buf, C.c_void_p)
+                spec.pos[k].len = len(b)
+        spec.join = join
+        spec.offset = offset
+        spec.limit = QB_NO_LIMIT if limit is None else limit
+        sl = (C.c_uint32 * 3)(*slots)
+        h, inf = C.c_void_p(), KbQbInfo()
+        self._check(lib().kb_qb_triples(self.h, C.byref(spec), right.h if right is not None else None, sl, None if count_only else C.byref(h),
+                                        C.byref(inf)))
+        return (None if count_only else Relation(self, h)), inf.as_dict()
+
+    def qb_terms(self, rel: Relation, col: int, mode: int) -> List[str]:
+        """kb_qb_terms: column `col` of `rel` as Dictionary::decode(id).unwrap_or("") renders it: every row (QB_TERMS_EMPTY), the rows
+        whose id decodes (QB_TERMS_DROP) or their distinct strings in byte order (QB_TERMS_DISTINCT)"""
+        h = C.c_void_p()
+        self._check(lib().kb_qb_terms(self.h, rel.h, col, mode, C.byref(h)))
+        try:
+            n, total = C.c_uint64(), C.c_uint64()
+            self._check(lib().kb_strings_info(h, C.byref(n), C.byref(total)))
+            off = np.empty(n.value + 1, dtype=np.uint64)
+            data = np.empty(max(total.value, 1), dtype=np.uint8)
+            self._check(lib().kb_strings_download(self.h, h, _ptr(off), _ptr(data)))
+        finally:
+            lib().kb_strings_free(self.h, h)
+        raw = data.tobytes()
+        return [raw[int(off[i]):int(off[i + 1])].decode("utf-8") for i in range(n.value)]
 
     # ---- operators
     def bind(self, rel: Relation, function: int, args: Sequence[KbTerm], out_slot: int, next_qt_id: int = 0,

@@ -80,7 +80,7 @@ __global__ void __launch_bounds__(DT) dbs_quoted_count_kernel(const u32* __restr
 
 kb_status gather_stats(kb_ctx* ctx, u64 max_sample, kb_db_stats* out, kb_db_stats_info* info) {
     u64 n_raw = 0;
-    for (const Segment& sg : ctx->segs) n_raw += sg.n;
+    const std::vector<ColSpan> spans = store_spans(ctx, &n_raw);
     if (n_raw >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "a store of %llu triples (statistics: limit 2^32 - 16)", (unsigned long long)n_raw);
     auto U = [](const Buf& b) { return static_cast<u32*>(b->p); };
     const u32 cq = ctrl_alloc(ctx, 4);  // [0..2] runs per column, [3] quoted-triple entries
@@ -100,7 +100,7 @@ kb_status gather_stats(kb_ctx* ctx, u64 max_sample, kb_db_stats* out, kb_db_stat
     KB_CUDA(ctx, cudaEventRecord(ev[0], ctx->st));
     Buf S, PO;
     u32 T = 0;
-    KB_TRY(store_distinct(ctx, n_raw, &S, &PO, &T));
+    KB_TRY(store_distinct(ctx, spans, &S, &PO, &T));
     KB_CUDA(ctx, cudaEventRecord(ev[1], ctx->st));
 
     const u64 take = max_sample ? std::min<u64>(T, max_sample) : T;

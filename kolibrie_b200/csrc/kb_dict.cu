@@ -14,7 +14,7 @@
 //   K5 dict_append_kernel      the new strings' bytes appended to the device dictionary (warp per string)
 //   K6 dict_index_insert_kernel  the new ids enter the persistent index (rebuilt larger beyond load 1/2)
 // Both tables are tag-indexed (kb_tagtab.cuh). This file owns the device dictionary: its loads, its growth, the decode of ids into text
-// (decode_ids: kb_rel_decode, string ORDER BY keys, the serializers) and its downloads.
+// (decode_ids: kb_rel_decode, string ORDER BY keys, the serializers, the QueryBuilder term lists) and its downloads.
 #include "kb_internal.hpp"
 #include "kb_tagtab.cuh"
 
@@ -171,15 +171,16 @@ __device__ u32 quoted_walk(u32 id, u32 dict_ids, const QuotedTab& qt, Lit lit, W
 // is held by neither table, and *deep = 1 when the walk goes past KB_QUOTED_MAX_DEPTH levels first. *total += sum.
 // missing_len: 7, or 0 when a term the tables do not hold renders as "" instead of "unknown" (decode_any(..).unwrap_or_default(), the serializers'
 // rule, sparql_database.rs:301-322).
+// plain: Dictionary::decode's rule, a quoted id is "none" (missing_len bytes) without a walk
 __global__ void __launch_bounds__(256) decode_lengths_kernel(const u32* __restrict__ ids, u32 n, const DictTab dict, const QuotedTab qt, u32* __restrict__ len, unsigned long long* total, u32* quoted, u32* deep,
-                                                             u32 missing_len) {
+                                                             u32 missing_len, u32 plain) {
     const u32 stride = gridDim.x * blockDim.x;
     unsigned long long t = 0;
     bool q = false, dp = false;
     for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
         const u32 id = ids[i];
         unsigned long long l = missing_len;  // "unknown" or ""
-        if (id & 0x80000000u) {
+        if ((id & 0x80000000u) && !plain) {
             if (qt.n == 0u) {
                 q = true;
             } else {
@@ -368,7 +369,7 @@ kb_status kb::dict_encode_device(kb_ctx* ctx, const u64* d_off, const unsigned c
 }
 
 
-kb_status kb::decode_ids(kb_ctx* ctx, const u32* ids, u32 n, u32 n_empty, bool missing_empty, const char* what, Buf* off_out, Buf* bytes_out,
+kb_status kb::decode_ids(kb_ctx* ctx, const u32* ids, u32 n, u32 n_empty, Decode mode, const char* what, Buf* off_out, Buf* bytes_out,
                          u64* total_out) {
     const size_t m = (size_t)n + n_empty;
     Buf off, scratch, bytes;
@@ -383,8 +384,9 @@ kb_status kb::decode_ids(kb_ctx* ctx, const u32* ids, u32 n, u32 n_empty, bool m
     const int grid = grid_1d(n, ctx->n_sms);
     timer_begin(ctx, F_OTHER, 4);
     if (n)
-        decode_lengths_kernel<<<grid, 256, 0, ctx->st>>>(ids, n, dict, qt, d_off, reinterpret_cast<unsigned long long*>(ctx->ctrl + c), ctx->ctrl + c + 2,
-                                                         ctx->ctrl + c + 3, missing_empty ? 0u : 7u);
+        decode_lengths_kernel<<<grid, 256, 0, ctx->st>>>(ids, n, dict, mode == Decode::Plain ? QuotedTab{} : qt, d_off,
+                                                         reinterpret_cast<unsigned long long*>(ctx->ctrl + c), ctx->ctrl + c + 2, ctx->ctrl + c + 3,
+                                                         mode == Decode::Unknown ? 7u : 0u, mode == Decode::Plain ? 1u : 0u);
     launch_exclusive_scan_u32(d_off, (u32)m + 1, static_cast<u32*>(scratch->p), ctx->st);
     timer_end(ctx);
     KB_CUDA(ctx, cudaGetLastError());
@@ -396,7 +398,7 @@ kb_status kb::decode_ids(kb_ctx* ctx, const u32* ids, u32 n, u32 n_empty, bool m
     if (total > 0xFFFFFFFFull) return fail(ctx, KB_E_LIMIT, "the text of %s would take %llu bytes (limit 2^32-1 per call)", what, total);
     KB_TRY(alloc_buf(ctx, (size_t)total + 16, &bytes));
     timer_begin(ctx, F_OTHER);
-    if (n) decode_gather_kernel<<<grid, 256, 0, ctx->st>>>(ids, n, dict, qt, d_off, static_cast<unsigned char*>(bytes->p));
+    if (n) decode_gather_kernel<<<grid, 256, 0, ctx->st>>>(ids, n, dict, mode == Decode::Plain ? QuotedTab{} : qt, d_off, static_cast<unsigned char*>(bytes->p));
     timer_end(ctx);
     KB_CUDA(ctx, cudaGetLastError());
     *off_out = off;
@@ -480,7 +482,7 @@ kb_status kb_rel_decode(kb_ctx* ctx, const kb_rel* r, uint32_t col, kb_strings**
     if (r->n >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "relation too large");
     auto res = std::make_unique<kb_strings>();
     res->n = r->n;
-    KB_TRY(decode_ids(ctx, r->cols[col].ptr, (u32)r->n, 0, false, "the column", &res->off, &res->bytes, &res->total));
+    KB_TRY(decode_ids(ctx, r->cols[col].ptr, (u32)r->n, 0, Decode::Unknown, "the column", &res->off, &res->bytes, &res->total));
     *out = res.release();
     return KB_OK;
 }

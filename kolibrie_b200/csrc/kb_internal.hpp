@@ -453,10 +453,14 @@ kb_status bind_join_impl(kb_ctx* ctx, const kb_rel& left, const kb_pattern& pat,
 // the device dictionary and the quoted-triple table as the kernels read them (null / n = 0 while empty)
 DictTab dicttab(const kb_ctx* ctx);
 QuotedTab quotedtab(const kb_ctx* ctx);
-// The text of n ids (kb_dict.cu), rendered as kb_rel_decode renders them (missing_empty: a term the tables do not hold is "" instead of
-// "unknown"), followed by n_empty more "": *off = u32 offsets [n + n_empty + 1], *bytes the text, *total (nullable) its bytes. One control-arena read. A quoted id
-// without a table is KB_E_UNSUPPORTED, a walk past KB_QUOTED_MAX_DEPTH or more than 2^32-1 bytes KB_E_LIMIT; `what` names the ids.
-kb_status decode_ids(kb_ctx* ctx, const u32* ids, u32 n, u32 n_empty, bool missing_empty, const char* what, Buf* off, Buf* bytes, u64* total);
+// How decode_ids renders an id: Unknown as kb_rel_decode does (a term the tables do not hold is "unknown"); Empty as decode_any(..)
+// .unwrap_or_default() does (such a term is ""); Plain as Dictionary::decode(..).unwrap_or("") does (a quoted id is not walked: it is ""
+// like any id past the dictionary).
+enum class Decode { Unknown, Empty, Plain };
+// The text of n ids (kb_dict.cu) rendered by `mode`, followed by n_empty more "": *off = u32 offsets [n + n_empty + 1], *bytes the text,
+// *total (nullable) its bytes. One control-arena read. A quoted id without a table (Unknown / Empty) is KB_E_UNSUPPORTED, a walk past
+// KB_QUOTED_MAX_DEPTH or more than 2^32-1 bytes KB_E_LIMIT; `what` names the ids.
+kb_status decode_ids(kb_ctx* ctx, const u32* ids, u32 n, u32 n_empty, Decode mode, const char* what, Buf* off, Buf* bytes, u64* total);
 // ensure the persistent index holds keys [0, n_keys) and stays below load 1/2 with `extra` more (kb_api.cu): rebuilt larger (1024 slots
 // at least, 1.5x headroom) when too small, then insert(first, n, tab, mask, overflow word) launches the insert of the keys it lacks
 // (one kernel). KB_E_LIMIT names `what` when the insert overflows.
@@ -473,10 +477,18 @@ kb_status quoted_encode(kb_ctx* ctx, const u32* const* col, const u32* cval, u32
 // u32 offsets into bytes, compared byte by byte, a proper prefix first): afterwards rank_of[v] is the rank of value v, *n_values the
 // number of distinct values and *rounds the refinement rounds taken (7 bytes of string a round).
 kb_status rank_values(kb_ctx* ctx, u32 d, const unsigned long long* nkey, const u32* str_off, const u8* bytes, u32* rank_of, u32* n_values, u32* rounds);
-// The distinct triples of the store's live segments in ascending (s, p, o) order, the reference's BTreeSet<Triple> order (kb_serialize.cu):
-// *S their subjects, *PO their (p << 32 | o), *n how many. n_raw = the segments' rows, 0 < n_raw < 2^32 - 16 (the caller checks). The
-// buffers hold n_raw entries. One control-arena read; launches count in the `other` family. The store is not changed.
-kb_status store_distinct(kb_ctx* ctx, u64 n_raw, Buf* S, Buf* PO, u32* n);
+// n rows of three id columns in device memory; ready (nullable): an event the rows wait for (a segment's chunked upload)
+struct ColSpan {
+    const u32 *s = nullptr, *p = nullptr, *o = nullptr;
+    u64 n = 0;
+    cudaEvent_t ready = nullptr;
+};
+// the live segments of a store as spans, and their rows
+std::vector<ColSpan> store_spans(const kb_ctx* ctx, u64* n_raw);
+// The distinct triples of the spans' rows in ascending (s, p, o) order, the reference's BTreeSet<Triple> order (kb_serialize.cu):
+// *S their subjects, *PO their (p << 32 | o), *n how many. The spans hold 0 < n_raw < 2^32 - 16 rows (the caller checks); the buffers
+// hold n_raw entries. One control-arena read; launches count in the `other` family. The spans are not changed.
+kb_status store_distinct(kb_ctx* ctx, const std::vector<ColSpan>& spans, Buf* S, Buf* PO, u32* n);
 // kb_dict_encode's body over a batch already in device memory (kb_dict.cu)
 kb_status dict_encode_device(kb_ctx* ctx, const u64* d_off, const unsigned char* d_bytes, u64 n_terms, u64 total, u32* d_out_ids, u32* n_new,
                              Buf* first_pos);

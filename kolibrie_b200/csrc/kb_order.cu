@@ -332,7 +332,7 @@ kb_status rank_key(kb_ctx* ctx, const kb_rel& in, u32 col, bool desc, KeyRank* k
         ctx->stats.d2h_bytes += sizeof(u32);
         const u32 dr = none == EMPTY32 ? d - 1 : d;
         Buf off, bytes;
-        KB_TRY(decode_ids(ctx, d_uniq, dr, d - dr, false, "the ORDER BY column", &off, &bytes, nullptr));
+        KB_TRY(decode_ids(ctx, d_uniq, dr, d - dr, Decode::Unknown, "the ORDER BY column", &off, &bytes, nullptr));
         KB_TRY(rank_values(ctx, d, nullptr, static_cast<const u32*>(off->p), static_cast<const u8*>(bytes->p), static_cast<u32*>(rank_of->p), &kr->n_values,
                            &kr->rounds));
         kr->kind = KB_ORDER_STRING;

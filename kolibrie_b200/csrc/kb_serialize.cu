@@ -5,7 +5,7 @@
 // or one triple's share of the Turtle text with its separators):
 //   sort      the live segments' s / p / o gathered into (s, packed p|o) and sorted by two stable LSD radix sorts (p|o first, then s):
 //             ascending (s, p, o), the reference's BTreeSet<Triple> order (triple.rs:13-18); equal neighbours are dropped
-//             (store_distinct, which kb_store_gather_stats shares)
+//             (store_distinct, which kb_store_gather_stats and kb_qb_triples share)
 //   render    every distinct id of the triples rendered once by the decode kernels of kb_rel_decode in their "missing -> empty" mode
 //             (decode_any(..).unwrap_or_default()), with a class byte per term taken from its rendered bytes (starts with "<<", with
 //             "http://" / "https://"); a triple holds the index of its three terms in the sorted distinct ids
@@ -268,7 +268,7 @@ kb_status serialize_begin(kb_ctx* ctx, u32 format, const u64* poff, const u8* pb
     ser->max_unit = ser->header.size();
     info->total_bytes = ser->header.size();
     u64 n_raw = 0;
-    for (const Segment& sg : ctx->segs) n_raw += sg.n;
+    const std::vector<ColSpan> spans = store_spans(ctx, &n_raw);
     if (n_raw == 0) {
         *out = std::move(ser);
         return KB_OK;
@@ -283,7 +283,7 @@ kb_status serialize_begin(kb_ctx* ctx, u32 format, const u64* poff, const u8* pb
     // ---- sort + dedup
     Buf S2, PO2;
     u32 n = 0;
-    KB_TRY(store_distinct(ctx, n_raw, &S2, &PO2, &n));
+    KB_TRY(store_distinct(ctx, spans, &S2, &PO2, &n));
     ser->n = n;
     const u32 c = ctrl_alloc(ctx, 1);  // distinct terms
     pt.mark(ctx->st);
@@ -304,7 +304,7 @@ kb_status serialize_begin(kb_ctx* ctx, u32 format, const u64* poff, const u8* pb
     KB_TRY(ctrl_read(ctx));
     const u32 nu = ctx->h_ctrl[c];
     info->n_terms = nu;
-    KB_TRY(decode_ids(ctx, U(terms), nu, 0, true, "the store", &ser->toff, &ser->tbytes, nullptr));
+    KB_TRY(decode_ids(ctx, U(terms), nu, 0, Decode::Empty, "the store", &ser->toff, &ser->tbytes, nullptr));
     KB_TRY(alloc_buf(ctx, (size_t)nu + 16, &ser->tcls));
     u8* tbytes = static_cast<u8*>(ser->tbytes->p);
     u8* tcls = static_cast<u8*>(ser->tcls->p);
@@ -431,7 +431,20 @@ kb_status serialize_next(kb_ctx* ctx, kb_serializer* ser, u8* dst, u64 capacity,
 
 }  // namespace
 
-kb_status store_distinct(kb_ctx* ctx, u64 n_raw, Buf* S_out, Buf* PO_out, u32* n_out) {
+std::vector<ColSpan> store_spans(const kb_ctx* ctx, u64* n_raw) {
+    std::vector<ColSpan> spans;
+    *n_raw = 0;
+    for (const Segment& sg : ctx->segs) {
+        if (!sg.n) continue;
+        spans.push_back({sg.s.ptr, sg.p.ptr, sg.o.ptr, sg.n, sg.ready});
+        *n_raw += sg.n;
+    }
+    return spans;
+}
+
+kb_status store_distinct(kb_ctx* ctx, const std::vector<ColSpan>& spans, Buf* S_out, Buf* PO_out, u32* n_out) {
+    u64 n_raw = 0;
+    for (const ColSpan& sp : spans) n_raw += sp.n;
     auto U = [](const Buf& b) { return static_cast<u32*>(b->p); };
     auto U64 = [](const Buf& b) { return static_cast<unsigned long long*>(b->p); };
     // (s, p|o) sorted by p|o, then stably by s; equal neighbours dropped
@@ -442,13 +455,13 @@ kb_status store_distinct(kb_ctx* ctx, u64 n_raw, Buf* S_out, Buf* PO_out, u32* n
     KB_TRY(alloc_buf(ctx, n_raw * 8, &PO2));
     {
         u64 at = 0;
-        for (const Segment& sg : ctx->segs) {
-            if (!sg.n) continue;
-            if (sg.ready) KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st, sg.ready, 0));
+        for (const ColSpan& sp : spans) {
+            if (!sp.n) continue;
+            if (sp.ready) KB_CUDA(ctx, cudaStreamWaitEvent(ctx->st, sp.ready, 0));
             timer_begin(ctx, F_OTHER, 1);
-            ser_load_kernel<<<grid_1d(sg.n, ctx->n_sms, ST), ST, 0, ctx->st>>>(sg.s.ptr, sg.p.ptr, sg.o.ptr, sg.n, U(S) + at, U64(PO) + at);
+            ser_load_kernel<<<grid_1d(sp.n, ctx->n_sms, ST), ST, 0, ctx->st>>>(sp.s, sp.p, sp.o, sp.n, U(S) + at, U64(PO) + at);
             timer_end(ctx);
-            at += sg.n;
+            at += sp.n;
         }
     }
     const u32 nr = (u32)n_raw;

@@ -203,6 +203,19 @@ def employee_subject_ids(d: EmployeeData, index: np.ndarray) -> np.ndarray:
     return out
 
 
+def employee_strings(d: EmployeeData) -> list:
+    """a dictionary text for every id of `d`: "http://example.org/employee<k>" for employee k's subject, the named constants by their
+    names (predicates, titles, "F", "SALARY", ...), the numeric literals as their integer text, "http://example.org/term<id>" otherwise"""
+    out = np.array(["http://example.org/term%d" % i for i in range(d.n_ids)], dtype=object)
+    for name, i in d.ids.items():
+        out[i] = name
+    k = np.arange(d.n_employees)
+    out[employee_subject_ids(d, k)] = ["http://example.org/employee%d" % i for i in k.tolist()]
+    num = np.nonzero(d.is_num)[0]
+    out[num] = [str(int(v)) for v in d.num_or0[num]]
+    return out.tolist()
+
+
 def employee_title_ids(d: EmployeeData, index: np.ndarray) -> np.ndarray:
     """dictionary id of the foaf:title object of global employee number `index` (closed form: first draw of the employee's pair)"""
     r = splitmix64_at(d.seed, 2 * np.asarray(index, dtype=np.uint64))

@@ -8,6 +8,8 @@ Same names, argument meaning and error behaviour as the reference (paths relativ
 * `ExecutionEngine`       — kolibrie/src/streamertail_optimizer/execution/engine.rs:27,54 (`execute`, `execute_with_ids`)
 * `Condition`             — kolibrie/src/streamertail_optimizer/types.rs:110-186 (FILTER expressions)
 * `SparqlDatabase`        — kolibrie/src/sparql_database.rs:49-60,215-258,3364-3394 (triples + dictionary + build_all_indexes)
+* `QueryBuilder`          — kolibrie/src/query_builder.rs:39-643 without its streaming half (a host restatement runs only for Python
+                            callables, which cannot cross the C ABI, and for contexts without the device query)
 * `Rule`/`FilterCondition`/`Reasoner` — shared/src/rule.rs:14-25, datalog/src/reasoning.rs:31-38,60-100,
                             datalog/src/reasoning/materialisation/semi_naive.rs:89, my_naive.rs:74
 
@@ -544,6 +546,10 @@ class SparqlDatabase:
         """SparqlDatabase::invalidate_stats_cache (sparql_database.rs:207-209): the next get_or_build_stats gathers again"""
         self.cached_stats = None
 
+    def query(self) -> "QueryBuilder":
+        """SparqlDatabase::query (sparql_database.rs): the fluent QueryBuilder over this database"""
+        return QueryBuilder(self)
+
     def add_statement(self, s, p, o):
         """add one triple whose terms are strings or nested tuples (quoted triples)"""
         self.add_triple((self.encode_term(s), self.encode_term(p), self.encode_term(o)))
@@ -765,6 +771,233 @@ class SparqlDatabase:
         comp = np.array(list(qts.id_to_components.values()), dtype=np.uint32).reshape(-1, 3)
         self.ctx.quoted_load(ids, comp[:, 0], comp[:, 1], comp[:, 2])
         self._uploaded_quoted = len(qts)
+
+
+_QB_TEXT = {"Contains": c.QB_CONTAINS, "StartsWith": c.QB_STARTS, "EndsWith": c.QB_ENDS}
+_QB_JOIN = {"OnSubject": c.QB_ON_SUBJECT, "OnPredicate": c.QB_ON_PREDICATE, "OnObject": c.QB_ON_OBJECT}
+
+
+class QueryBuilder:
+    """QueryBuilder (query_builder.rs:39-643) without its streaming half: the same builder methods and results, answered on the device
+    (kb_qb_triples / kb_qb_terms) whenever no Python callable is involved. A position filter is a TripleFilter as a tuple: ("Exact" |
+    "Contains" | "StartsWith" | "EndsWith", text) or ("Custom", callable on the decoded string); the with_* methods set them, and
+    subject_filter / predicate_filter / object_filter may be set to a ("Custom", fn) directly, as the reference's enum allows. Results:
+    get_triples() a set of (s, p, o) id tuples (sorted() gives the BTreeSet order), get_decoded_triples() a list of string triples,
+    get_subjects() / get_predicates() / get_objects() lists of strings, count() an int, group_by() a dict in key order.
+    The host restatement runs instead for filter(fn), a ("Custom", fn) position filter or join_with(fn) (a Python callable cannot cross
+    the C ABI), for contexts without the device query or without device dictionary strings, and for a join with another database that
+    shares this one's context. `last_path` records which ran ("device" or "host"). order_by / asc / desc have no effect, as in the
+    reference: it collects the sorted rows back into a BTreeSet. An offset past the rows raises IndexError, where the reference panics."""
+
+    def __init__(self, db: SparqlDatabase):
+        self.db = db
+        self.subject_filter = self.predicate_filter = self.object_filter = None
+        self.custom_filter = None
+        self.join_conditions: List = []
+        self.join_db: Optional[SparqlDatabase] = None
+        self.distinct_results = False
+        self.sort_key = None
+        self.descending = False
+        self._limit: Optional[int] = None
+        self._offset: Optional[int] = None
+        self.last_path: Optional[str] = None
+
+    def _set(self, attr, kind, text):
+        setattr(self, attr, (kind, text))
+        return self
+
+    def with_subject(self, v): return self._set("subject_filter", "Exact", v)
+    def with_subject_like(self, v): return self._set("subject_filter", "Contains", v)
+    def with_subject_starting(self, v): return self._set("subject_filter", "StartsWith", v)
+    def with_subject_ending(self, v): return self._set("subject_filter", "EndsWith", v)
+    def with_predicate(self, v): return self._set("predicate_filter", "Exact", v)
+    def with_predicate_like(self, v): return self._set("predicate_filter", "Contains", v)
+    def with_predicate_starting(self, v): return self._set("predicate_filter", "StartsWith", v)
+    def with_predicate_ending(self, v): return self._set("predicate_filter", "EndsWith", v)
+    def with_object(self, v): return self._set("object_filter", "Exact", v)
+    def with_object_like(self, v): return self._set("object_filter", "Contains", v)
+    def with_object_starting(self, v): return self._set("object_filter", "StartsWith", v)
+    def with_object_ending(self, v): return self._set("object_filter", "EndsWith", v)
+
+    def filter(self, fn):
+        self.custom_filter = fn
+        return self
+
+    def join(self, other: SparqlDatabase):
+        self.join_db = other
+        return self
+
+    def join_on_subject(self):
+        self.join_conditions.append("OnSubject")
+        return self
+
+    def join_on_predicate(self):
+        self.join_conditions.append("OnPredicate")
+        return self
+
+    def join_on_object(self):
+        self.join_conditions.append("OnObject")
+        return self
+
+    def join_with(self, fn):
+        self.join_conditions.append(fn)
+        return self
+
+    def distinct(self):
+        self.distinct_results = True
+        return self
+
+    def order_by(self, key):
+        self.sort_key = key
+        return self
+
+    def desc(self):
+        self.descending = True
+        return self
+
+    def asc(self):
+        self.descending = False
+        return self
+
+    def limit(self, n: int):
+        self._limit = n
+        return self
+
+    def offset(self, n: int):
+        self._offset = n
+        return self
+
+    # ---- results
+    def get_triples(self) -> set:
+        return set(self._rows())
+
+    def count(self) -> int:
+        n = self._device(count_only=True)
+        return len(self._host_rows()) if n is None else n
+
+    def get_decoded_triples(self) -> List[Tuple[str, str, str]]:
+        rel = self._device()
+        if rel is not None:
+            try:
+                cols = [self.db.ctx.qb_terms(rel, k, c.QB_TERMS_EMPTY) for k in range(3)]
+            finally:
+                rel.free()
+            return list(zip(*cols))
+        d = self.db.dictionary.decode
+        return [tuple(d(x) or "" for x in t) for t in self._host_rows()]
+
+    def get_subjects(self) -> List[str]:
+        return self._terms(0)
+
+    def get_predicates(self) -> List[str]:
+        return self._terms(1)
+
+    def get_objects(self) -> List[str]:
+        return self._terms(2)
+
+    def group_by(self, key_fn) -> dict:
+        """get_triples, then the key function on the host in set order; the groups in key order (a BTreeMap)"""
+        groups: dict = {}
+        for t in sorted(self.get_triples()):
+            groups.setdefault(key_fn(t), []).append(t)
+        return {k: groups[k] for k in sorted(groups)}
+
+    def _terms(self, col: int) -> List[str]:
+        rel = self._device()
+        if rel is not None:
+            try:
+                return self.db.ctx.qb_terms(rel, col, c.QB_TERMS_DISTINCT if self.distinct_results else c.QB_TERMS_DROP)
+            finally:
+                rel.free()
+        d = self.db.dictionary.decode
+        out = [d(t[col]) for t in self._host_rows()]
+        out = [x for x in out if x is not None]
+        return sorted(set(out), key=lambda x: x.encode("utf-8")) if self.distinct_results else out
+
+    def _joins(self) -> bool:
+        return self.join_db is not None and bool(self.join_conditions)
+
+    def _device(self, count_only: bool = False):
+        """the relation of the rows (or their count), or None when the host restatement must run"""
+        db, right = self.db, self.join_db if self._joins() else None
+        filters = (self.subject_filter, self.predicate_filter, self.object_filter)
+        if (self.custom_filter is not None or any(f is not None and f[0] == "Custom" for f in filters)
+                or any(callable(j) for j in self.join_conditions) or not hasattr(db.ctx, "qb_triples")
+                or (right is not None and right is not db and right.ctx is db.ctx)):
+            self.last_path = "host"
+            return None
+        spec = []
+        for f in filters:
+            if f is None:
+                spec.append(None)
+            elif f[0] == "Exact":
+                i = db.dictionary.lookup(f[1])
+                spec.append((c.QB_EXACT, c.KB_ID_NONE if i is None else i))
+            else:
+                spec.append((_QB_TEXT[f[0]], f[1]))
+        join = 0
+        for j in self.join_conditions:
+            join |= _QB_JOIN[j]
+        db._sync()
+        if right is not None:
+            right._sync()
+        try:
+            rel, info = db.ctx.qb_triples(spec, join if right is not None else 0, right.ctx if right is not None else None, self._offset or 0,
+                                       self._limit, count_only=count_only)
+        except c.KolibrieError as e:
+            if e.status == c.KB_E_UNSUPPORTED:
+                self.last_path = "host"
+                return None
+            if e.status == c.KB_E_INVALID and self._offset:
+                raise IndexError(str(e)) from e
+            raise
+        self.last_path = "device"
+        return info["n_rows"] if count_only else rel
+
+    def _rows(self) -> List[Tuple[int, int, int]]:
+        """apply_filters (query_builder.rs:486-568): the rows in set order, on the device or by the host restatement"""
+        rel = self._device()
+        if rel is not None:
+            try:
+                return [tuple(int(x) for x in r) for r in rel.to_numpy()]
+            finally:
+                rel.free()
+        return self._host_rows()
+
+    def _host_rows(self) -> List[Tuple[int, int, int]]:
+        """the host restatement of apply_filters and apply_join"""
+        d = self.db.dictionary.decode
+
+        def ok(f, tid):
+            if f is None:
+                return True
+            v = d(tid)
+            if v is None:
+                return False
+            kind, arg = f
+            return (v == arg if kind == "Exact" else arg in v if kind == "Contains" else v.startswith(arg) if kind == "StartsWith"
+                    else v.endswith(arg) if kind == "EndsWith" else bool(arg(v)))
+
+        filters = (self.subject_filter, self.predicate_filter, self.object_filter)
+        rows = sorted(t for t in self.db.triples if all(ok(f, x) for f, x in zip(filters, t))
+                      and (self.custom_filter is None or self.custom_filter(t)))
+        if self._joins():
+            out = set()
+            right = self.join_db.triples
+            for j in self.join_conditions:
+                for l in rows:
+                    for r in right:
+                        if j == "OnSubject" and l[0] == r[0] or j == "OnPredicate" and l[1] == r[1]:
+                            out.add((l[0], l[1], r[2]))
+                        elif (j == "OnObject" and l[2] == r[2]) or (callable(j) and j(l, r)):
+                            out.add((l[0], r[1], r[2]))
+            rows = sorted(out)
+        if self._offset is not None or self._limit is not None:
+            off = self._offset or 0
+            if off > len(rows):
+                raise IndexError(f"offset {off} past the {len(rows)} rows")
+            rows = rows[off:] if self._limit is None else rows[off:off + self._limit]
+        return rows
 
 
 def _gather_stats_fast(triples, max_sample: int):

@@ -92,6 +92,20 @@ pub type kb_serializer = KbSerializer;  // (the header's name, as the declaratio
 pub type kb_db_stats_info = KbDbStatsInfo;  // (the header's name, as the declaration below spells it)
 pub enum KbDbStats {}
 pub type kb_db_stats = KbDbStats;  // (the header's name, as the declarations below spell it)
+// kb_qb_triples / kb_qb_terms: QueryBuilder triple queries on the device store
+pub const KB_QB_ANY: u32 = 0; pub const KB_QB_EXACT: u32 = 1; pub const KB_QB_CONTAINS: u32 = 2; pub const KB_QB_STARTS: u32 = 3; pub const KB_QB_ENDS: u32 = 4;
+pub const KB_QB_ON_SUBJECT: u32 = 1; pub const KB_QB_ON_PREDICATE: u32 = 2; pub const KB_QB_ON_OBJECT: u32 = 4;
+pub const KB_QB_TERMS_EMPTY: u32 = 0; pub const KB_QB_TERMS_DROP: u32 = 1; pub const KB_QB_TERMS_DISTINCT: u32 = 2;
+pub const KB_QB_PATTERN_MAX: u32 = 4096;
+pub const KB_QB_NO_LIMIT: u64 = u64::MAX;
+#[repr(C)] #[derive(Clone, Copy, Debug)] pub struct KbQbFilter { pub mode: u32, pub id: u32, pub pattern: *const u8, pub len: u64 }
+impl Default for KbQbFilter { fn default() -> Self { Self { mode: KB_QB_ANY, id: 0, pattern: std::ptr::null(), len: 0 } } }
+#[repr(C)] #[derive(Clone, Copy, Debug)] pub struct KbQbSpec { pub pos: [KbQbFilter; 3], pub join: u32, pub reserved: u32, pub offset: u64, pub limit: u64 }
+impl Default for KbQbSpec { fn default() -> Self { Self { pos: [KbQbFilter::default(); 3], join: 0, reserved: 0, offset: 0, limit: KB_QB_NO_LIMIT } } }
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbQbInfo { pub n_raw: u64, pub n_selected: u64, pub n_joined: u64, pub n_rows: u64,
+    pub phase_ms: [c_double; 4] }
+pub type kb_qb_spec = KbQbSpec;  // (the header's names, as the declarations below spell them)
+pub type kb_qb_info = KbQbInfo;
 
 // kb_filter_opcode / kb_cmp / kb_agg_kind / kb_strategy
 pub const KB_F_CMP_NUM: u32 = 1; pub const KB_F_EQ_ID: u32 = 2; pub const KB_F_NE_ID: u32 = 3; pub const KB_F_AND: u32 = 4; pub const KB_F_OR: u32 = 5;
@@ -154,6 +168,9 @@ extern "C" {
     pub fn kb_store_gather_stats(ctx: *mut KbCtx, max_sample: u64, out: *mut *mut kb_db_stats, info: *mut kb_db_stats_info) -> kb_status;
     pub fn kb_db_stats_counts(st: *const kb_db_stats, position: u32, ids: *mut *const u32, counts: *mut *const u64, n: *mut u64) -> kb_status;
     pub fn kb_db_stats_free(st: *mut kb_db_stats);
+    pub fn kb_qb_triples(ctx: *mut KbCtx, spec: *const kb_qb_spec, right: *const KbCtx, slots: *const u32, out: *mut *mut KbRel,
+                         info: *mut kb_qb_info) -> kb_status;
+    pub fn kb_qb_terms(ctx: *mut KbCtx, rows: *const KbRel, col: u32, mode: u32, out: *mut *mut KbStrings) -> kb_status;
     // operators
     pub fn kb_scan(ctx: *mut KbCtx, pats: *const KbPattern, n: u32, pushdown: *const *const KbFilterOp, pushdown_len: *const u32, out: *mut *mut KbRel) -> kb_status;
     pub fn kb_filter(ctx: *mut KbCtx, r: *const KbRel, prog: *const KbFilterOp, n: u32, out: *mut *mut KbRel) -> kb_status;

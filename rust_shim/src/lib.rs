@@ -267,6 +267,74 @@ impl DeviceStore {
     }
 }
 
+/// One position filter of a device QueryBuilder query (`TripleFilter` without `Custom`): `Exact` takes the id the caller's dictionary
+/// gives the string (`KB_ID_NONE` when it lacks it), the others the pattern's text.
+pub enum QbFilter<'a> { Exact(u32), Contains(&'a str), StartsWith(&'a str), EndsWith(&'a str) }
+
+/// A device QueryBuilder result: the rows in `BTreeSet<Triple>` order (`kb_qb_triples`), owned until dropped.
+pub struct QbRows { ctx: *mut KbCtx, rel: *mut KbRel, pub info: KbQbInfo }
+impl Drop for QbRows {
+    fn drop(&mut self) { unsafe { kb_rel_free(self.ctx, self.rel) } }
+}
+
+impl DeviceStore {
+    /// `QueryBuilder::apply_filters` (query_builder.rs:486-568) on the device store (`sync` first), for a query without closures:
+    /// `filters` per position, `join` the `KB_QB_ON_*` bits against `right`'s store (a context on the same device, `self` for a
+    /// self-join; `None`: no join), rows [offset, offset + limit) of the set order. `count_only` gives no rows, only `info.n_rows`
+    /// (`count()`). `get_triples` reads the rows with `QbRows::triples`; `get_decoded_triples` / `get_subjects` & co. with `query_terms`.
+    /// Err(KB_E_UNSUPPORTED's message) means: run the reference's loop.
+    pub fn query_triples(&mut self, filters: [Option<QbFilter>; 3], join: u32, right: Option<&DeviceStore>, offset: u64, limit: Option<u64>,
+                         count_only: bool) -> Result<Option<QbRows>, String> {
+        let mut spec = KbQbSpec { join, offset, limit: limit.unwrap_or(KB_QB_NO_LIMIT), ..Default::default() };
+        for (k, f) in filters.iter().enumerate() {
+            spec.pos[k] = match f {
+                None => KbQbFilter::default(),
+                Some(QbFilter::Exact(id)) => KbQbFilter { mode: KB_QB_EXACT, id: *id, ..Default::default() },
+                Some(QbFilter::Contains(t)) => KbQbFilter { mode: KB_QB_CONTAINS, pattern: t.as_ptr(), len: t.len() as u64, id: 0 },
+                Some(QbFilter::StartsWith(t)) => KbQbFilter { mode: KB_QB_STARTS, pattern: t.as_ptr(), len: t.len() as u64, id: 0 },
+                Some(QbFilter::EndsWith(t)) => KbQbFilter { mode: KB_QB_ENDS, pattern: t.as_ptr(), len: t.len() as u64, id: 0 },
+            };
+        }
+        let slots = [0u32, 1, 2];
+        let mut rel: *mut KbRel = ptr::null_mut();
+        let mut info = KbQbInfo::default();
+        let r = right.map_or(ptr::null(), |d| d.ctx as *const KbCtx);
+        let out = if count_only { ptr::null_mut() } else { &mut rel as *mut *mut KbRel };
+        if unsafe { kb_qb_triples(self.ctx, &spec, r, slots.as_ptr(), out, &mut info) } != KB_OK { return Err(self.last_error()); }
+        Ok(if count_only { None } else { Some(QbRows { ctx: self.ctx, rel, info }) })
+    }
+
+    /// column `col` (0 subject, 1 predicate, 2 object) of a `query_triples` result as `Dictionary::decode(id).unwrap_or("")` renders it:
+    /// `KB_QB_TERMS_EMPTY` every row (`get_decoded_triples`), `KB_QB_TERMS_DROP` the rows that decode (`get_subjects` & co.),
+    /// `KB_QB_TERMS_DISTINCT` their distinct strings in byte order (the same with `distinct()`)
+    pub fn query_terms(&mut self, rows: &QbRows, col: u32, mode: u32) -> Result<Vec<String>, String> {
+        let mut s: *mut KbStrings = ptr::null_mut();
+        if unsafe { kb_qb_terms(self.ctx, rows.rel, col, mode, &mut s) } != KB_OK { return Err(self.last_error()); }
+        let (mut n, mut total) = (0u64, 0u64);
+        unsafe { kb_strings_info(s, &mut n, &mut total) };
+        let mut offs = vec![0u64; n as usize + 1];
+        let mut bytes = vec![0u8; total as usize + 1];
+        let rc = unsafe { kb_strings_download(self.ctx, s, offs.as_mut_ptr(), bytes.as_mut_ptr()) };
+        unsafe { kb_strings_free(self.ctx, s) };
+        if rc != KB_OK { return Err(self.last_error()); }
+        Ok((0..n as usize).map(|i| String::from_utf8_lossy(&bytes[offs[i] as usize..offs[i + 1] as usize]).into_owned()).collect())
+    }
+}
+
+impl QbRows {
+    /// the rows as `Triple`s, in set order (collect them into the `BTreeSet` `get_triples` returns)
+    pub fn triples(&self) -> Result<Vec<Triple>, String> {
+        let n = self.info.n_rows as usize;
+        let mut cols = [vec![0u32; n], vec![0u32; n], vec![0u32; n]];
+        for (c, v) in cols.iter_mut().enumerate() {
+            if n > 0 && unsafe { kb_rel_download(self.ctx, self.rel, c as u32, v.as_mut_ptr()) } != KB_OK {
+                return Err("kb_rel_download refused the result".into());
+            }
+        }
+        Ok((0..n).map(|i| Triple { subject: cols[0][i], predicate: cols[1][i], object: cols[2][i] }).collect())
+    }
+}
+
 /// What `DeviceStore::gather_stats` returns: the totals (`info.total_triples`, `info.quoted_triple_count`) and the three cardinality maps
 /// of `DatabaseStats` (database_stats.rs:17-26), counts already scaled by the sampling step.
 pub struct StoreStats {
