@@ -434,6 +434,50 @@ KB_API kb_status kb_qb_triples(kb_ctx* ctx, const kb_qb_spec* spec, const kb_ctx
                                kb_rel** out /* nullable: count only */, kb_qb_info* info /* nullable */);
 KB_API kb_status kb_qb_terms(kb_ctx* ctx, const kb_rel* rows, uint32_t col, uint32_t mode, kb_strings** out);
 
+/* ------------------------------------------------------------------ two stores combined into a third context: SparqlDatabase::union and
+ * SparqlDatabase::par_join (kolibrie/src/sparql_database.rs:1874-2005). a, b and dst are contexts of one device, none sharded; dst differs
+ * from a and from b; a == b is allowed (both are only read: their stores, versions, indexes and tables are left as they were).
+ * kb_store_union: the database union(a, b) returns.
+ *   Its dictionary is a's (ids and strings) followed by the strings of b's terms a lacks, in the order the reference's loop meets them:
+ *   b's triples as a set in ascending (s, p, o) order of b's ids, s, p, o of each, encode(decode(id)) — a string a holds keeps a's id,
+ *   every other one takes the next id. Its store is a's set together with b's set re-encoded that way, as a set.
+ * kb_store_par_join: the database par_join(a, b, predicate) returns, for a predicate id the caller has encoded in a's dictionary (the
+ *   reference's `dict.encode(predicate)`, which adds the string when a lacks it).
+ *   With A = a's triples with that predicate id and B = b's (ids compared raw, as the reference compares them, whatever b's dictionary
+ *   says): {(s, p, y) : (s,p,o) in A, (o,p,y) in B} together with {(s, p, o) : (s,p,o) in A, o the object of a triple of B}, as a set. Its
+ *   dictionary is a copy of a's.
+ * Both: on success dst's store is replaced by one segment holding the result in ascending (s, p, o) order and dst's index is dropped (the
+ * reference's new index is empty: kb_store_build_index builds one); dst's device dictionary strings become the result's; dst's
+ * quoted-triple table becomes a copy of a's (the result shares a's QuotedTripleStore); dst's numeric side tables are left as they were,
+ * for the caller to derive (kb_dict_numeric_derive), as after kb_dict_strings_load. The timestamped stream log (`streams`) is not kept on
+ * the device and is not combined.
+ * Refused, dst left exactly as it was: NULL contexts, dst == a or dst == b, contexts on different devices, for the union an id of b's
+ * store that b's dictionary does not map (a quoted-triple id, an id past its strings: the reference's decode(..).unwrap() panics), a
+ * predicate of KB_ID_NONE (KB_E_INVALID); a sharded context, for the union a non-empty store of a or b without device dictionary strings,
+ * for par_join a without them (KB_E_UNSUPPORTED); a store of 2^32 - 16 triples or more, 3 x b's distinct triples reaching 2^32 - 16, a
+ * result of 2^32 - 16 rows or more before the dedup (counted exactly before anything is allocated), a's strings plus b's distinct terms
+ * reaching 2^31 ids (KB_E_LIMIT). Launches and device time count in kb_stats' `other` family. */
+typedef struct kb_union_info {
+    uint64_t n_a;          /* distinct triples of a */
+    uint64_t n_b;          /* distinct triples of b */
+    uint64_t n_rows;       /* distinct triples of the result */
+    uint32_t n_terms;      /* distinct ids of b's triples */
+    uint32_t dict_first;   /* strings of a's dictionary: the id the first new string takes */
+    uint32_t dict_new;     /* strings the union added: ids [dict_first, dict_first + dict_new) (kb_dict_strings_download) */
+    uint32_t reserved;
+    double phase_ms[5];    /* device time: the two sets, b's terms, dictionary, remap, union */
+} kb_union_info;
+typedef struct kb_par_join_info {
+    uint64_t n_a;          /* distinct triples of a with the predicate */
+    uint64_t n_b;          /* distinct triples of b with the predicate */
+    uint64_t n_join;       /* rows of the join a.o = b.s */
+    uint64_t n_semi;       /* rows of a whose object is an object of B */
+    uint64_t n_rows;       /* distinct triples of the result */
+    double phase_ms[4];    /* device time: selection, distinct pairs + counts, joins, sort + dedup */
+} kb_par_join_info;
+KB_API kb_status kb_store_union(kb_ctx* dst, const kb_ctx* a, const kb_ctx* b, kb_union_info* info /* nullable */);
+KB_API kb_status kb_store_par_join(kb_ctx* dst, const kb_ctx* a, const kb_ctx* b, uint32_t predicate, kb_par_join_info* info /* nullable */);
+
 /* ------------------------------------------------------------------ BIND: `PhysicalOperator::Bind` with the built-in functions of
  * ExecutionEngine::execute_with_ids (kolibrie/src/streamertail_optimizer/execution/engine.rs:144-277) over the rows of `in`, in the order
  * they lie. *out = `in` with the output column: appended when out_slot is not a column of `in`, else that column replaced (the other

@@ -212,6 +212,26 @@ class KbQbInfo(C.Structure):
         return {n: (list(getattr(self, n)) if n == "phase_ms" else int(getattr(self, n))) for n, _ in self._fields_}
 
 
+class KbUnionInfo(C.Structure):
+    """kb_union_info: distinct triples of a, of b and of the result, b's distinct ids, the first id and the number of the strings the
+    union added, and the device time of the phases (the two sets, b's terms, dictionary, remap, union)"""
+    _fields_ = [("n_a", C.c_uint64), ("n_b", C.c_uint64), ("n_rows", C.c_uint64), ("n_terms", C.c_uint32), ("dict_first", C.c_uint32),
+                ("dict_new", C.c_uint32), ("reserved", C.c_uint32), ("phase_ms", C.c_double * 5)]
+
+    def as_dict(self):
+        return {n: (list(getattr(self, n)) if n == "phase_ms" else int(getattr(self, n))) for n, _ in self._fields_ if n != "reserved"}
+
+
+class KbParJoinInfo(C.Structure):
+    """kb_par_join_info: distinct triples of a and of b with the predicate, rows of the join and of the semi-join, distinct triples of
+    the result, and the device time of the phases (selection, distinct pairs + counts, joins, sort + dedup)"""
+    _fields_ = [("n_a", C.c_uint64), ("n_b", C.c_uint64), ("n_join", C.c_uint64), ("n_semi", C.c_uint64), ("n_rows", C.c_uint64),
+                ("phase_ms", C.c_double * 4)]
+
+    def as_dict(self):
+        return {n: (list(getattr(self, n)) if n == "phase_ms" else int(getattr(self, n))) for n, _ in self._fields_}
+
+
 KB_BGP_MAX_PATTERNS = 16
 BGP_NONE, BGP_STAR, BGP_COMPONENTS = 0, 1, 2  # kb_bgp_route
 
@@ -355,6 +375,8 @@ def lib() -> C.CDLL:
         "kb_db_stats_free": (None, [vp]),
         "kb_qb_triples": (i32, [vp, P(KbQbSpec), vp, P(u32), P(vp), P(KbQbInfo)]),
         "kb_qb_terms": (i32, [vp, vp, u32, u32, P(vp)]),
+        "kb_store_union": (i32, [vp, vp, vp, P(KbUnionInfo)]),
+        "kb_store_par_join": (i32, [vp, vp, vp, u32, P(KbParJoinInfo)]),
         "kb_bind": (i32, [vp, vp, P(KbBindSpec), P(vp), P(KbBindInfo)]),
         "kb_rel_info": (i32, [vp, P(u64), P(u32), P(u32)]),
         "kb_rel_download": (i32, [vp, vp, u32, vp]),
@@ -426,7 +448,7 @@ def lib() -> C.CDLL:
 EXPORTED_SYMBOLS = [
     "kb_version", "kb_ctx_create", "kb_ctx_destroy", "kb_last_error", "kb_set_timing", "kb_get_stats", "kb_synchronize",
     "kb_store_load", "kb_store_load_device", "kb_store_append", "kb_store_append_device", "kb_store_evict", "kb_store_delete", "kb_store_insert", "kb_store_remove", "kb_store_remove_template", "kb_store_clear", "kb_store_build_index", "kb_set_use_index", "kb_store_size",
-    "kb_store_download", "kb_dict_numeric_load", "kb_dict_legacy_i32_load", "kb_dict_numeric_derive", "kb_dict_numeric_download", "kb_dict_strings_load", "kb_dict_encode", "kb_dict_strings_info", "kb_rel_decode", "kb_strings_info", "kb_strings_download", "kb_strings_free", "kb_quoted_load", "kb_quoted_download", "kb_dict_strings_download", "kb_serialize_begin", "kb_serialize_next", "kb_serialize_free", "kb_store_gather_stats", "kb_db_stats_counts", "kb_db_stats_free", "kb_qb_triples", "kb_qb_terms", "kb_bind", "kb_rel_info", "kb_rel_download", "kb_rel_device_col", "kb_rel_from_host",
+    "kb_store_download", "kb_dict_numeric_load", "kb_dict_legacy_i32_load", "kb_dict_numeric_derive", "kb_dict_numeric_download", "kb_dict_strings_load", "kb_dict_encode", "kb_dict_strings_info", "kb_rel_decode", "kb_strings_info", "kb_strings_download", "kb_strings_free", "kb_quoted_load", "kb_quoted_download", "kb_dict_strings_download", "kb_serialize_begin", "kb_serialize_next", "kb_serialize_free", "kb_store_gather_stats", "kb_db_stats_counts", "kb_db_stats_free", "kb_qb_triples", "kb_qb_terms", "kb_store_union", "kb_store_par_join", "kb_bind", "kb_rel_info", "kb_rel_download", "kb_rel_device_col", "kb_rel_from_host",
     "kb_rel_from_device", "kb_rel_free", "kb_scan", "kb_filter", "kb_project", "kb_hash_join", "kb_natural_join", "kb_hash_join_keyed", "kb_values", "kb_bind_join", "kb_scan_quoted", "kb_star_join", "kb_bgp_execute", "kb_bgp_last_plan",
     "kb_order_by", "kb_group_aggregate", "kb_groups_info", "kb_groups_keys", "kb_groups_values", "kb_groups_counts", "kb_groups_free", "kb_groups_pack", "kb_groups_merge", "kb_star_join_aggregate",
     "kb_star_join_prepare", "kb_plan_submit", "kb_plan_collect", "kb_plan_info", "kb_plan_free", "kb_plan_peer_scratch_bytes", "kb_plan_attach_peers",
@@ -782,6 +804,21 @@ class Context:
         self._check(lib().kb_qb_triples(self.h, C.byref(spec), right.h if right is not None else None, sl, None if count_only else C.byref(h),
                                         C.byref(inf)))
         return (None if count_only else Relation(self, h)), inf.as_dict()
+
+    def store_union(self, a: "Context", b: "Context") -> dict:
+        """kb_store_union: this context's store, device dictionary and quoted-triple table become those of SparqlDatabase::union(a, b)
+        (a and b are only read; both must be other contexts on this device). The index is dropped and the numeric side tables are left
+        for dict_numeric_derive. Returns kb_union_info as a dict: the new strings are ids [dict_first, dict_first + dict_new)."""
+        inf = KbUnionInfo()
+        self._check(lib().kb_store_union(self.h, a.h, b.h, C.byref(inf)))
+        return inf.as_dict()
+
+    def store_par_join(self, a: "Context", b: "Context", predicate: int) -> dict:
+        """kb_store_par_join: this context's store becomes SparqlDatabase::par_join(a, b, predicate) for a predicate id of a's
+        dictionary, and its device dictionary and quoted-triple table copies of a's. Returns kb_par_join_info as a dict."""
+        inf = KbParJoinInfo()
+        self._check(lib().kb_store_par_join(self.h, a.h, b.h, predicate, C.byref(inf)))
+        return inf.as_dict()
 
     def qb_terms(self, rel: Relation, col: int, mode: int) -> List[str]:
         """kb_qb_terms: column `col` of `rel` as Dictionary::decode(id).unwrap_or("") renders it: every row (QB_TERMS_EMPTY), the rows

@@ -370,7 +370,7 @@ kb_status kb::dict_encode_device(kb_ctx* ctx, const u64* d_off, const unsigned c
 
 
 kb_status kb::decode_ids(kb_ctx* ctx, const u32* ids, u32 n, u32 n_empty, Decode mode, const char* what, Buf* off_out, Buf* bytes_out,
-                         u64* total_out) {
+                         u64* total_out, const DictTab* from) {
     const size_t m = (size_t)n + n_empty;
     Buf off, scratch, bytes;
     KB_TRY(alloc_buf(ctx, (m + 1) * sizeof(u32), &off));
@@ -379,7 +379,7 @@ kb_status kb::decode_ids(kb_ctx* ctx, const u32* ids, u32 n, u32 n_empty, Decode
     KB_CUDA(ctx, cudaMemsetAsync(d_off + n, 0, ((size_t)n_empty + 1) * sizeof(u32), ctx->st));  // the scan runs over m + 1 entries: off[m] = total
     const u32 c = ctrl_alloc(ctx, 4);  // [0..1] u64 total bytes, [2] quoted-triple id seen without a table, [3] walk too deep
     KB_CUDA(ctx, cudaMemsetAsync(ctx->ctrl + c, 0, 4 * sizeof(u32), ctx->st));
-    const DictTab dict = dicttab(ctx);
+    const DictTab dict = from ? *from : dicttab(ctx);
     const QuotedTab qt = quotedtab(ctx);
     const int grid = grid_1d(n, ctx->n_sms);
     timer_begin(ctx, F_OTHER, 4);
@@ -405,6 +405,33 @@ kb_status kb::decode_ids(kb_ctx* ctx, const u32* ids, u32 n, u32 n_empty, Decode
     *bytes_out = bytes;
     if (total_out) *total_out = total;
     return KB_OK;
+}
+
+kb_status kb::dict_copy(kb_ctx* dst, const kb_ctx* src, DictState* prev) {
+    DictState next;
+    next.ids = src->dict_ids;
+    if (src->dict_ids) {
+        unsigned long long total = 0;
+        KB_CUDA(dst, cudaMemcpyAsync(&total, static_cast<const unsigned long long*>(src->dict_off->p) + src->dict_ids, sizeof total, cudaMemcpyDeviceToHost, dst->st));
+        KB_CUDA(dst, cudaStreamSynchronize(dst->st));
+        KB_TRY(alloc_buf(dst, ((size_t)src->dict_ids + 1) * sizeof(u64), &next.off));
+        KB_TRY(alloc_buf(dst, (size_t)total + 16, &next.bytes));
+        KB_CUDA(dst, cudaMemcpyAsync(next.off->p, src->dict_off->p, ((size_t)src->dict_ids + 1) * sizeof(u64), cudaMemcpyDeviceToDevice, dst->st));
+        if (total) KB_CUDA(dst, cudaMemcpyAsync(next.bytes->p, src->dict_bytes->p, (size_t)total, cudaMemcpyDeviceToDevice, dst->st));
+    }
+    prev->off = dst->dict_off;
+    prev->bytes = dst->dict_bytes;
+    prev->ids = dst->dict_ids;
+    prev->index = dst->dict_index;
+    dict_restore(dst, std::move(next));
+    return KB_OK;
+}
+
+void kb::dict_restore(kb_ctx* dst, DictState&& prev) {
+    dst->dict_off = std::move(prev.off);
+    dst->dict_bytes = std::move(prev.bytes);
+    dst->dict_ids = prev.ids;
+    dst->dict_index = std::move(prev.index);
 }
 
 extern "C" {

@@ -68,6 +68,19 @@ struct ScopedEvent {
     operator cudaEvent_t() const { return e; }
 };
 
+// device time between marks on a stream (an info struct's phase_ms): N marks bound N - 1 phases; ms(k) after a sync
+template <int N>
+struct PhaseTimer {
+    ScopedEvent e[N];
+    int at = 0;
+    void mark(cudaStream_t st) { cudaEventRecord(e[at++], st); }
+    double ms(int k) const {
+        float v = 0.f;
+        cudaEventElapsedTime(&v, e[k], e[k + 1]);
+        return v;
+    }
+};
+
 enum Family { F_SCAN = 0, F_BUILD, F_PROBE, F_FILTER, F_GROUP, F_OTHER, F_COUNT };
 
 struct PendingTimer {
@@ -460,7 +473,22 @@ enum class Decode { Unknown, Empty, Plain };
 // The text of n ids (kb_dict.cu) rendered by `mode`, followed by n_empty more "": *off = u32 offsets [n + n_empty + 1], *bytes the text,
 // *total (nullable) its bytes. One control-arena read. A quoted id without a table (Unknown / Empty) is KB_E_UNSUPPORTED, a walk past
 // KB_QUOTED_MAX_DEPTH or more than 2^32-1 bytes KB_E_LIMIT; `what` names the ids.
-kb_status decode_ids(kb_ctx* ctx, const u32* ids, u32 n, u32 n_empty, Decode mode, const char* what, Buf* off, Buf* bytes, u64* total);
+// from (nullable): the dictionary to read instead of ctx's (another context's on the same device, whose last writes are done).
+kb_status decode_ids(kb_ctx* ctx, const u32* ids, u32 n, u32 n_empty, Decode mode, const char* what, Buf* off, Buf* bytes, u64* total,
+                     const DictTab* from = nullptr);
+// A context's device dictionary as kb_dict.cu keeps it. dict_copy: dst's dictionary becomes a copy of src's strings (device to device on
+// dst's stream; src's last writes are done; the string -> id index is rebuilt by dst's next encode), and *prev receives the one dst held;
+// dict_restore puts that back when a later step of the caller fails. Refused (KB_E_OOM, KB_E_CUDA) with dst unchanged.
+struct DictState {
+    Buf off, bytes;
+    u32 ids = 0;
+    TagIndex index;
+};
+kb_status dict_copy(kb_ctx* dst, const kb_ctx* src, DictState* prev);
+void dict_restore(kb_ctx* dst, DictState&& prev);
+// dst's quoted-triple table becomes a copy of src's (kb_quoted.cu; device to device, src's last writes are done; dst's reverse index is
+// rebuilt by its next TRIPLE). Refused (KB_E_OOM, KB_E_CUDA) with dst's table unchanged.
+kb_status quoted_copy(kb_ctx* dst, const kb_ctx* src);
 // ensure the persistent index holds keys [0, n_keys) and stays below load 1/2 with `extra` more (kb_api.cu): rebuilt larger (1024 slots
 // at least, 1.5x headroom) when too small, then insert(first, n, tab, mask, overflow word) launches the insert of the keys it lacks
 // (one kernel). KB_E_LIMIT names `what` when the insert overflows.
@@ -489,6 +517,14 @@ std::vector<ColSpan> store_spans(const kb_ctx* ctx, u64* n_raw);
 // *S their subjects, *PO their (p << 32 | o), *n how many. The spans hold 0 < n_raw < 2^32 - 16 rows (the caller checks); the buffers
 // hold n_raw entries. One control-arena read; launches count in the `other` family. The spans are not changed.
 kb_status store_distinct(kb_ctx* ctx, const std::vector<ColSpan>& spans, Buf* S, Buf* PO, u32* n);
+// Pair relations (kb_qbuilder.cu). distinct_pairs: the distinct (key << 32 | carried) pairs of the rows (cols[k].first, cols[k].second)
+// over rows[k] rows each, sorted: *out, *n_out of them. pair_rel: n sorted distinct pairs as a two-column relation over (key slot, carried
+// slot). pair_join_count: *cnt = sum over the nl left pairs of the nr right pairs with the same key (both sorted), the exact size of
+// their join. split_sorted: rows [lo, lo + n) of a store_distinct result (S, PO) as three columns.
+kb_status distinct_pairs(kb_ctx* ctx, const std::vector<std::pair<const u32*, const u32*>>& cols, const std::vector<u64>& rows, Buf* out, u32* n_out);
+kb_status pair_rel(kb_ctx* ctx, const Buf& pairs, u32 n, u32 key_slot, u32 car_slot, std::unique_ptr<kb_rel>* out);
+kb_status pair_join_count(kb_ctx* ctx, const Buf& lp, u32 nl, const Buf& rp, u32 nr, u64* cnt);
+kb_status split_sorted(kb_ctx* ctx, const Buf& S, const Buf& PO, u64 lo, u64 n, u32* s, u32* p, u32* o);
 // kb_dict_encode's body over a batch already in device memory (kb_dict.cu)
 kb_status dict_encode_device(kb_ctx* ctx, const u64* d_off, const unsigned char* d_bytes, u64 n_terms, u64 total, u32* d_out_ids, u32* n_new,
                              Buf* first_pos);

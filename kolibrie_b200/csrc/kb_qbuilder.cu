@@ -194,14 +194,10 @@ __global__ void __launch_bounds__(QT) qb_scatter_kernel(const u32* __restrict__ 
     for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[rank_of[i]] = ids[i];
 }
 
-struct PhaseTimer {  // device time between marks on the context's stream
-    ScopedEvent e[5];
-    int at = 0;
-    void mark(cudaStream_t st) { cudaEventRecord(e[at++], st); }
-};
-
 auto U = [](const Buf& b) { return static_cast<u32*>(b->p); };
 auto U64 = [](const Buf& b) { return static_cast<unsigned long long*>(b->p); };
+
+}  // namespace
 
 // the distinct (key << 32 | carried) pairs of the n rows (key[i], car[i]), sorted: *out, *n_out of them
 kb_status distinct_pairs(kb_ctx* ctx, const std::vector<std::pair<const u32*, const u32*>>& cols, const std::vector<u64>& rows, Buf* out, u32* n_out) {
@@ -246,6 +242,32 @@ kb_status pair_rel(kb_ctx* ctx, const Buf& pairs, u32 n, u32 key_slot, u32 car_s
     return KB_OK;
 }
 
+kb_status pair_join_count(kb_ctx* ctx, const Buf& lp, u32 nl, const Buf& rp, u32 nr, u64* cnt) {
+    *cnt = 0;
+    if (!nl || !nr) return KB_OK;
+    const u32 c = ctrl_alloc(ctx, 2);
+    timer_begin(ctx, F_OTHER, 1);
+    qb_join_count_kernel<<<grid_1d(nl, ctx->n_sms, QT), QT, 0, ctx->st>>>(U64(lp), nl, U64(rp), nr, reinterpret_cast<unsigned long long*>(ctx->ctrl + c));
+    timer_end(ctx);
+    KB_CUDA(ctx, cudaGetLastError());
+    KB_TRY(ctrl_read(ctx));
+    unsigned long long v = 0;
+    memcpy(&v, ctx->h_ctrl + c, sizeof v);
+    *cnt = v;
+    return KB_OK;
+}
+
+kb_status split_sorted(kb_ctx* ctx, const Buf& S, const Buf& PO, u64 lo, u64 n, u32* s, u32* p, u32* o) {
+    if (!n) return KB_OK;
+    timer_begin(ctx, F_OTHER, 1);
+    qb_split_kernel<<<grid_1d(n, ctx->n_sms, QT), QT, 0, ctx->st>>>(U(S), U64(PO), lo, n, s, p, o);
+    timer_end(ctx);
+    KB_CUDA(ctx, cudaGetLastError());
+    return KB_OK;
+}
+
+namespace {
+
 struct JoinCond {
     u32 bit;
     int lkey, lcar;  // left position (0 s, 1 p, 2 o) of the key and of the carried id
@@ -283,7 +305,7 @@ kb_status qb_triples(kb_ctx* ctx, const kb_qb_spec& spec, const kb_ctx* right, c
         if (n_right >= 0xFFFFFFF0ull) return fail(ctx, KB_E_LIMIT, "a right store of %llu triples (limit 2^32 - 16)", (unsigned long long)n_right);
     }
     info->n_raw = n_raw;
-    PhaseTimer pt;
+    PhaseTimer<5> pt;
     pt.mark(ctx->st);
 
     // ---- match: a bitmap over the ids per text filter
@@ -355,12 +377,7 @@ kb_status qb_triples(kb_ctx* ctx, const kb_qb_spec& spec, const kb_ctx* right, c
     if (join) {
         Col lc[3];
         for (Col& c : lc) KB_TRY(alloc_col(ctx, n, &c));
-        if (n) {
-            timer_begin(ctx, F_OTHER, 1);
-            qb_split_kernel<<<grid_1d(n, ctx->n_sms, QT), QT, 0, ctx->st>>>(U(S), U64(PO), 0, n, lc[0].ptr, lc[1].ptr, lc[2].ptr);
-            timer_end(ctx);
-            KB_CUDA(ctx, cudaGetLastError());
-        }
+        KB_TRY(split_sorted(ctx, S, PO, 0, n, lc[0].ptr, lc[1].ptr, lc[2].ptr));
         S.reset(); PO.reset();
         if (n_right) KB_CUDA(ctx, cudaStreamSynchronize(right->st));  // the right store's last writes are done
         std::vector<std::unique_ptr<kb_rel>> parts;
@@ -381,14 +398,8 @@ kb_status qb_triples(kb_ctx* ctx, const kb_qb_spec& spec, const kb_ctx* right, c
             }
             KB_TRY(distinct_pairs(ctx, rc, rrows, &rp, &nr));
             if (!nl || !nr) continue;
-            const u32 c = ctrl_alloc(ctx, 2);
-            timer_begin(ctx, F_OTHER, 1);
-            qb_join_count_kernel<<<grid_1d(nl, ctx->n_sms, QT), QT, 0, ctx->st>>>(U64(lp), nl, U64(rp), nr, reinterpret_cast<unsigned long long*>(ctx->ctrl + c));
-            timer_end(ctx);
-            KB_CUDA(ctx, cudaGetLastError());
-            KB_TRY(ctrl_read(ctx));
-            unsigned long long cnt = 0;
-            memcpy(&cnt, ctx->h_ctrl + c, sizeof cnt);
+            u64 cnt = 0;
+            KB_TRY(pair_join_count(ctx, lp, nl, rp, nr, &cnt));
             total += cnt;
             if (total >= 0xFFFFFFF0ull)
                 return fail(ctx, KB_E_LIMIT, "the join gives %llu rows or more before the union (limit 2^32 - 16)", (unsigned long long)total);
@@ -419,12 +430,7 @@ kb_status qb_triples(kb_ctx* ctx, const kb_qb_spec& spec, const kb_ctx* right, c
         r->slots.assign(slots, slots + 3);
         r->n = hi - lo;
         KB_TRY(alloc_strided_cols(ctx, r->n, 3, &r->cols));
-        if (r->n) {
-            timer_begin(ctx, F_OTHER, 1);
-            qb_split_kernel<<<grid_1d(r->n, ctx->n_sms, QT), QT, 0, ctx->st>>>(U(S), U64(PO), lo, r->n, r->cols[0].ptr, r->cols[1].ptr, r->cols[2].ptr);
-            timer_end(ctx);
-            KB_CUDA(ctx, cudaGetLastError());
-        }
+        KB_TRY(split_sorted(ctx, S, PO, lo, r->n, r->cols[0].ptr, r->cols[1].ptr, r->cols[2].ptr));
         *out = r.release();
     }
     KB_CUDA(ctx, cudaStreamSynchronize(ctx->st));

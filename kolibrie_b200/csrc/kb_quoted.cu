@@ -319,6 +319,24 @@ kb_status kb::quoted_encode(kb_ctx* ctx, const u32* const* col, const u32* cval,
     return KB_OK;
 }
 
+kb_status kb::quoted_copy(kb_ctx* dst, const kb_ctx* src) {
+    const u32 slots = src->quoted_slots;
+    if (!slots) {
+        quoted_reset(dst);
+        return KB_OK;
+    }
+    const Buf* from[3] = {&src->quoted_s, &src->quoted_p, &src->quoted_o};
+    Buf nb[3];  // the copy is complete before it replaces dst's table
+    for (int k = 0; k < 3; k++) {
+        KB_TRY(alloc_buf(dst, (size_t)slots * sizeof(u32), &nb[k]));
+        KB_CUDA(dst, cudaMemcpyAsync(nb[k]->p, (*from[k])->p, (size_t)slots * sizeof(u32), cudaMemcpyDeviceToDevice, dst->st));
+    }
+    quoted_reset(dst);
+    dst->quoted_s = nb[0]; dst->quoted_p = nb[1]; dst->quoted_o = nb[2];
+    dst->quoted_slots = dst->quoted_cap = slots;
+    return KB_OK;
+}
+
 extern "C" {
 
 kb_status kb_quoted_load(kb_ctx* ctx, const uint32_t* ids, const uint32_t* s, const uint32_t* p, const uint32_t* o, uint64_t n) {

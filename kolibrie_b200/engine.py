@@ -740,6 +740,118 @@ class SparqlDatabase:
             self._uploaded_version = self._version
         return n
 
+    def union(self, other: "SparqlDatabase") -> "SparqlDatabase":
+        """SparqlDatabase::union (sparql_database.rs:1874-1933): a new database on a new context on this one's device. Its dictionary is
+        a clone of this one's extended with other's strings in the order the reference re-encodes other's triples (ascending (s, p, o)
+        of other's ids, s, p, o of each); its triples are this set together with other's re-encoded set; it shares this database's
+        quoted-triple store and prefixes, and has no index, cached statistics or stream log. On the device (kb_store_union) the new
+        context's store, dictionary strings and quoted table are built there and the triple set and new strings are downloaded; the host
+        restatement runs for contexts without the entry point and for an `other` that shares this context (one context holds one store).
+        An id of other's triples that other's dictionary does not map (a quoted id, an id past it: the reference's decode(..).unwrap()
+        panics) raises ValueError and changes nothing."""
+        if self._device_pair(other, "store_union"):
+            self._sync_strings()
+            other._sync_strings()
+            out = SparqlDatabase(ctx=c.Context(self.ctx.device))
+            try:
+                info = out.ctx.store_union(self.ctx, other.ctx)
+            except c.KolibrieError as e:
+                out.ctx.close()
+                if e.status == c.KB_E_INVALID:
+                    raise ValueError(str(e)) from e
+                if e.status != c.KB_E_UNSUPPORTED:
+                    raise
+            else:
+                out.dictionary = self._clone_dictionary()
+                for t in out.ctx.dict_strings_download(info["dict_first"], info["dict_new"]):
+                    out.dictionary.encode(t)
+                self.last_union_info = info
+                return self._device_result(out)
+        merged = self._clone_dictionary()
+        re_encoded = set()
+        for t in sorted(other.triples):
+            ids = []
+            for x in t:
+                v = other.dictionary.decode(x)
+                if v is None:
+                    raise ValueError(f"id {x} of other's triple {t} has no string in other's dictionary (the reference's decode(..).unwrap() panics)")
+                ids.append(merged.encode(v))
+            re_encoded.add(tuple(ids))
+        out = SparqlDatabase(ctx=self._new_context())
+        out.dictionary = merged
+        for t in sorted(self.triples | re_encoded):
+            out.add_triple(t)
+        return self._host_result(out)
+
+    def par_join(self, other: "SparqlDatabase", predicate: str) -> "SparqlDatabase":
+        """SparqlDatabase::par_join (sparql_database.rs:1935-2005): `predicate` is encoded in this dictionary (which may add it); with A
+        this set's triples with that id and B other's (ids compared raw), the new database holds (s, p, y) for (s,p,o) in A and (o,p,y)
+        in B, and (s, p, o) for (s,p,o) in A whose o is the object of a triple of B. It shares this database's dictionary and
+        quoted-triple store, on a new context on this one's device (kb_store_par_join; the host restatement as for union)."""
+        pid = self.dictionary.encode(predicate)
+        if self._device_pair(other, "store_par_join"):
+            self._sync_strings()
+            other._sync()
+            out = SparqlDatabase(ctx=c.Context(self.ctx.device))
+            try:
+                info = out.ctx.store_par_join(self.ctx, other.ctx, pid)
+            except c.KolibrieError as e:
+                out.ctx.close()
+                if e.status != c.KB_E_UNSUPPORTED:
+                    raise
+            else:
+                out.dictionary = self.dictionary
+                self.last_par_join_info = info
+                return self._device_result(out)
+        keyed: Dict[int, List[Tuple[int, int, int]]] = {}
+        for t in other.triples:
+            if t[1] == pid:
+                keyed.setdefault(t[0], []).append(t)
+                keyed.setdefault(t[2], []).append(t)
+        out = SparqlDatabase(ctx=self._new_context())
+        out.dictionary = self.dictionary
+        for t in sorted({(s, q[1], q[2]) for s, p, o in self.triples if p == pid for q in keyed.get(o, ())}):
+            out.add_triple(t)
+        return self._host_result(out)
+
+    def _device_pair(self, other: "SparqlDatabase", entry: str) -> bool:
+        """whether union / par_join run on the device: the context has the entry point and `other` is this database or has a context
+        of its own on the same device"""
+        return hasattr(self.ctx, entry) and (other is self or (other.ctx is not self.ctx and getattr(other.ctx, "device", None) == self.ctx.device))
+
+    def _new_context(self):
+        return c.Context(self.ctx.device) if isinstance(self.ctx, c.Context) else type(self.ctx)()
+
+    def _clone_dictionary(self) -> Dictionary:
+        d = Dictionary()
+        d.string_to_id = dict(self.dictionary.string_to_id)
+        d.id_to_string = list(self.dictionary.id_to_string)
+        return d
+
+    def _host_result(self, out: "SparqlDatabase") -> "SparqlDatabase":
+        out.quoted_triple_store = self.quoted_triple_store  # Arc::clone(&self.quoted_triple_store)
+        out.prefixes = list(self.prefixes)
+        return out
+
+    def _device_result(self, out: "SparqlDatabase") -> "SparqlDatabase":
+        """the new context holds the result: its triple set is downloaded and marked uploaded, its numeric side table derived"""
+        s, p, o = out.ctx.store_download()
+        out.triples = set(zip(s.tolist(), p.tolist(), o.tolist()))
+        out._uploaded_version = out._version
+        out.quoted_triple_store = self.quoted_triple_store
+        out._uploaded_quoted = len(out.quoted_triple_store)  # the new context's table is a copy of this one's
+        out.prefixes = list(self.prefixes)
+        out.ctx.dict_numeric_derive(c.NUMERIC_F64, 0)
+        return out
+
+    def _sync_strings(self):
+        """the store, and the device dictionary holding every string of this dictionary (strings encoded since the last upload go up)"""
+        self._sync()
+        n_dev, _ = self.ctx.dict_strings_info()
+        if n_dev != len(self.dictionary.id_to_string):
+            kept = _push_new_strings(self.ctx, self.dictionary, n_dev)
+            _derive_numeric(self.ctx, c.NUMERIC_APPEND if kept else 0)
+
     def build_all_indexes(self):
         """The reference builds its six hash indexes here (sparql_database.rs:3364-3394); the device store is (re)uploaded and
         partitioned by predicate (kb_store_build_index)."""

@@ -107,6 +107,14 @@ impl Default for KbQbSpec { fn default() -> Self { Self { pos: [KbQbFilter::defa
 pub type kb_qb_spec = KbQbSpec;  // (the header's names, as the declarations below spell them)
 pub type kb_qb_info = KbQbInfo;
 
+// kb_store_union / kb_store_par_join: SparqlDatabase::union and par_join into a third context
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbUnionInfo { pub n_a: u64, pub n_b: u64, pub n_rows: u64, pub n_terms: u32, pub dict_first: u32,
+    pub dict_new: u32, pub reserved: u32, pub phase_ms: [c_double; 5] }
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)] pub struct KbParJoinInfo { pub n_a: u64, pub n_b: u64, pub n_join: u64, pub n_semi: u64, pub n_rows: u64,
+    pub phase_ms: [c_double; 4] }
+pub type kb_union_info = KbUnionInfo;
+pub type kb_par_join_info = KbParJoinInfo;
+
 // kb_filter_opcode / kb_cmp / kb_agg_kind / kb_strategy
 pub const KB_F_CMP_NUM: u32 = 1; pub const KB_F_EQ_ID: u32 = 2; pub const KB_F_NE_ID: u32 = 3; pub const KB_F_AND: u32 = 4; pub const KB_F_OR: u32 = 5;
 pub const KB_F_NOT: u32 = 6; pub const KB_F_PUSH_VAR: u32 = 7; pub const KB_F_PUSH_CONST: u32 = 8; pub const KB_F_ADD: u32 = 9; pub const KB_F_SUB: u32 = 10;
@@ -171,6 +179,8 @@ extern "C" {
     pub fn kb_qb_triples(ctx: *mut KbCtx, spec: *const kb_qb_spec, right: *const KbCtx, slots: *const u32, out: *mut *mut KbRel,
                          info: *mut kb_qb_info) -> kb_status;
     pub fn kb_qb_terms(ctx: *mut KbCtx, rows: *const KbRel, col: u32, mode: u32, out: *mut *mut KbStrings) -> kb_status;
+    pub fn kb_store_union(dst: *mut KbCtx, a: *const KbCtx, b: *const KbCtx, info: *mut kb_union_info) -> kb_status;
+    pub fn kb_store_par_join(dst: *mut KbCtx, a: *const KbCtx, b: *const KbCtx, predicate: u32, info: *mut kb_par_join_info) -> kb_status;
     // operators
     pub fn kb_scan(ctx: *mut KbCtx, pats: *const KbPattern, n: u32, pushdown: *const *const KbFilterOp, pushdown_len: *const u32, out: *mut *mut KbRel) -> kb_status;
     pub fn kb_filter(ctx: *mut KbCtx, r: *const KbRel, prog: *const KbFilterOp, n: u32, out: *mut *mut KbRel) -> kb_status;

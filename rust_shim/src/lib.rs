@@ -321,6 +321,36 @@ impl DeviceStore {
     }
 }
 
+impl DeviceStore {
+    /// `SparqlDatabase::union(self, other)` (sparql_database.rs:1874-1933) on the device: both stores `sync`ed first, the result in a new
+    /// context on `device` (the same as both). Its store, device dictionary and quoted-triple table are the union's: the new database's
+    /// dictionary is a clone of `database`'s extended with the `info.dict_new` strings from id `info.dict_first` on
+    /// (`kb_dict_strings_download`), its triples the set `kb_store_download` reads. An id of `other`'s triples that its dictionary does
+    /// not map (the reference panics) is an Err.
+    pub fn union(&mut self, database: &SparqlDatabase, other: &mut DeviceStore, other_db: &SparqlDatabase, device: i32)
+                 -> Result<(DeviceStore, KbUnionInfo), String> {
+        self.sync(database)?;
+        other.sync(other_db)?;
+        let mut out = DeviceStore::new(device)?;
+        let mut info = KbUnionInfo::default();
+        if unsafe { kb_store_union(out.ctx, self.ctx, other.ctx, &mut info) } != KB_OK { return Err(out.last_error()); }
+        Ok((out, info))
+    }
+
+    /// `SparqlDatabase::par_join(self, other, predicate)` (sparql_database.rs:1935-2005) for `predicate_id`, the predicate as `database`'s
+    /// dictionary encodes it (the caller encodes it first, as the reference does): the result in a new context on `device`, whose
+    /// dictionary and quoted-triple table are copies of this one's, as the result shares `database`'s.
+    pub fn par_join(&mut self, database: &SparqlDatabase, other: &mut DeviceStore, other_db: &SparqlDatabase, predicate_id: u32, device: i32)
+                    -> Result<(DeviceStore, KbParJoinInfo), String> {
+        self.sync(database)?;
+        other.sync(other_db)?;
+        let mut out = DeviceStore::new(device)?;
+        let mut info = KbParJoinInfo::default();
+        if unsafe { kb_store_par_join(out.ctx, self.ctx, other.ctx, predicate_id, &mut info) } != KB_OK { return Err(out.last_error()); }
+        Ok((out, info))
+    }
+}
+
 impl QbRows {
     /// the rows as `Triple`s, in set order (collect them into the `BTreeSet` `get_triples` returns)
     pub fn triples(&self) -> Result<Vec<Triple>, String> {
